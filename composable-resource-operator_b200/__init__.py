@@ -1,4 +1,4 @@
-"""composable-resource-operator_b200 — B200-native post-attach probe + spec path.
+"""composable-resource-operator_b200 — H100-native post-attach probe + spec path.
 
 Thin ctypes binding of ``libcroprobe.so`` (the C ABI in ``include/croprobe.h``),
 the same entry points a Go host binds with cgo (INTEGRATION.md).  The package
@@ -398,7 +398,7 @@ def reconcile_attach(ctx: Optional["ProbeContext"], request: Dict) -> Dict:
     return out
 
 
-# ---- the probe context (needs a B200) ------------------------------------------------
+# ---- the probe context (needs an H100) -----------------------------------------------
 class ProbeContext:
     """Long-lived probe context: resident sweep buffers, streams, events.
 

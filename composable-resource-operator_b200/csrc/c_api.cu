@@ -63,7 +63,7 @@ int on_exception() noexcept {
 
 extern "C" {
 
-const char* cro_version(void) { return "croprobe 0.2.0 (sm_100a, abi 2)"; }
+const char* cro_version(void) { return "croprobe 0.2.0 (sm_90a, abi 2)"; }
 
 const char* cro_strerror(int code) {
     switch (code) {

@@ -1099,7 +1099,7 @@ void Cluster::Run(long long max_reconciles) {
         while ((!req_queue_.empty() || !res_queue_.empty()) && n < max_reconciles) {
             // Look for finished probes every 100 us of reconciling.  (Round 1 polled when n % 4 == 0 — but n advances
             // by two per turn while both queues hold work, so an odd n never hit a multiple of four again and finished
-            // probes sat uncollected until a queue drained: one ~200 ms hole per GPU at the start of a storm.)
+            // probes sat uncollected until a queue drained: a hole per GPU at the start of a storm.)
             const auto now_poll = clk::now();
             if (now_poll - last_poll_ >= std::chrono::microseconds(100)) {
                 last_poll_ = now_poll;

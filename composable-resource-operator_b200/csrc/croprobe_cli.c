@@ -57,7 +57,7 @@ int main(int argc, char **argv) {
     opts.flags = CRO_F_LAZY_ALLOC | CRO_F_DEGRADE_ON_OOM;
     if (wants_probe) {
         /* The hot-plug path: one device, identity from /proc (NVML's first call costs more than the probe), and a
-         * 1 GiB first sweep unless told otherwise — it already runs at ~7 TB/s and shortens everything before it. */
+         * 1 GiB first sweep unless told otherwise — far beyond the L2, and it shortens everything before it. */
         opts.sweep_bytes = (argc > 3 ? (uint64_t)strtoull(argv[3], NULL, 10) : 1024ull) << 20;
         if (!(cold && argc > 4 && strcmp(argv[4], "nvml") == 0)) opts.flags |= CRO_F_NO_NVML;
         if (strncmp(argv[2], "GPU-", 4) == 0) {

@@ -402,7 +402,8 @@ bool ScanNvml(std::vector<NvmlGpu>* out, std::string* err) {
         if (getUuid(dev, uuid, sizeof uuid) != 0) continue;
         g.uuid = uuid;
         if (getMinor(dev, &minor) == 0) g.minor = (int)minor;
-        if (getPci(dev, &pci) == 0) g.bus_id = pci.busId;
+        // a device whose PCI info NVML will not give (some virtualised hosts): nvidia-smi prints "[N/A]" for it
+        g.bus_id = getPci(dev, &pci) == 0 ? std::string(pci.busId) : std::string("[N/A]");
         if (getClock) {
             unsigned c = 0;
             if (getClock(dev, /*NVML_CLOCK_SM*/ 1, &c) == 0) g.sm_clock_mhz = c;

@@ -68,15 +68,15 @@ struct ProcGpu {
 // Scans <root>/driver/nvidia/gpus/*/information (root defaults to /proc).
 std::vector<ProcGpu> ScanProc(const std::string& proc_root);
 // The registry's directory listing alone — "<name>:<inode>:<ctime>" per GPU, sorted, joined by '|' — without opening
-// any `information` file: reading those goes through the driver and its locks (measured ~14 ms per read while
-// nvidia-smi polls, 100+ ms for a whole 8-GPU box), listing and stat-ing the directory does not.  A GPU that leaves or
+// any `information` file: reading those goes through the driver and its locks (slow while
+// nvidia-smi polls, and slower for a whole 8-GPU box), listing and stat-ing the directory does not.  A GPU that leaves or
 // joins the bus changes the listing; a re-created entry is a new inode object with new times even when procfs hands it
 // its old inode number.  Empty string: the registry directory does not exist.
 std::string ProcRegistryListing(const std::string& proc_root);
 
 struct NvmlGpu {
     std::string uuid;      // "GPU-..."
-    std::string bus_id;    // nvmlPciInfo_t.busId, "00000000:1F:00.0"
+    std::string bus_id;    // nvmlPciInfo_t.busId, "00000000:1F:00.0"; "[N/A]", as nvidia-smi prints it, when NVML refuses
     int minor = -1;
     unsigned sm_clock_mhz = 0, mem_clock_mhz = 0;
 };

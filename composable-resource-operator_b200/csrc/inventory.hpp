@@ -6,7 +6,7 @@
 // runtime: its device list is fixed at cuInit.  So the probe context keeps two things apart:
 //   * the devices it can probe IN PROCESS (its CUDA contexts, fixed at cro_probe_init), and
 //   * the node's inventory, re-read on every enumeration / visibility query from the driver's own registry
-//     (/proc/driver/nvidia/gpus/*/information — a directory walk, ~0.06 ms — with NVML re-initialised only when
+//     (/proc/driver/nvidia/gpus/*/information — a directory walk — with NVML re-initialised only when
 //     that walk shows a change).
 // A GPU composed after init shows up in the inventory flagged CRO_DEV_NEEDS_HELPER and is probed by a one-shot helper
 // process (croprobe-cli, which runs its own cuInit); a GPU drained / removed from the bus drops out of the inventory

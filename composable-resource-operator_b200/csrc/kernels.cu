@@ -1,4 +1,4 @@
-// kernels.cu — hand-written sm_100a kernels of the post-attach HBM / NVLink probe.
+// kernels.cu — hand-written sm_90a kernels of the post-attach HBM / NVLink probe.
 //
 // The reference has no device code at all (its check is the UUID membership
 // test at internal/utils/gpus.go:54-86); these kernels are new work in that
@@ -43,6 +43,18 @@ __device__ __forceinline__ uint4 ldg_stream(const uint4* p) {
     return r;
 }
 
+// L2 eviction-priority policies for the bulk copies and the 32-byte loads (streaming data is touched once).
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_last() {
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+
 // Batched streaming loads: ONE asm block so ptxas cannot interleave the
 // consumers between the loads — every thread keeps the whole batch (128 B) in
 // flight.  STRIDE is the byte distance between a thread's consecutive vectors.
@@ -64,18 +76,24 @@ __device__ __forceinline__ void ldg128_x8(const void* p, unsigned long long (&a)
         : "l"(p), "n"(STRIDE), "n"(2 * STRIDE), "n"(3 * STRIDE), "n"(4 * STRIDE), "n"(5 * STRIDE),
           "n"(6 * STRIDE), "n"(7 * STRIDE));
 }
-// 256-bit flavour (sm_100+: LDG.E.256): four 32-byte vectors per thread.
+// 32-byte flavour: four 32-byte vectors per thread, each fetched as two adjacent 128-bit loads (sm_90 has no
+// 256-bit LDG), all eight in flight at once, under an L2 evict_first policy (`policy`, from createpolicy).
 template <int STRIDE>
-__device__ __forceinline__ void ldg256_x4(const void* p, unsigned long long (&w)[16]) {
+__device__ __forceinline__ void ldg256_x4(const void* p, uint64_t policy, unsigned long long (&w)[16]) {
     asm volatile(
-        "ld.global.nc.L1::no_allocate.L2::evict_first.v4.u64 {%0,%1,%2,%3}, [%16];\n"
-        "ld.global.nc.L1::no_allocate.L2::evict_first.v4.u64 {%4,%5,%6,%7}, [%16+%17];\n"
-        "ld.global.nc.L1::no_allocate.L2::evict_first.v4.u64 {%8,%9,%10,%11}, [%16+%18];\n"
-        "ld.global.nc.L1::no_allocate.L2::evict_first.v4.u64 {%12,%13,%14,%15}, [%16+%19];\n"
+        "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%0,%1}, [%16], %23;\n"
+        "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%2,%3}, [%16+16], %23;\n"
+        "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%4,%5}, [%16+%17], %23;\n"
+        "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%6,%7}, [%16+%20], %23;\n"
+        "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%8,%9}, [%16+%18], %23;\n"
+        "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%10,%11}, [%16+%21], %23;\n"
+        "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%12,%13}, [%16+%19], %23;\n"
+        "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%14,%15}, [%16+%22], %23;\n"
         : "=l"(w[0]), "=l"(w[1]), "=l"(w[2]), "=l"(w[3]), "=l"(w[4]), "=l"(w[5]), "=l"(w[6]),
           "=l"(w[7]), "=l"(w[8]), "=l"(w[9]), "=l"(w[10]), "=l"(w[11]), "=l"(w[12]), "=l"(w[13]),
           "=l"(w[14]), "=l"(w[15])
-        : "l"(p), "n"(STRIDE), "n"(2 * STRIDE), "n"(3 * STRIDE));
+        : "l"(p), "n"(STRIDE), "n"(2 * STRIDE), "n"(3 * STRIDE), "n"(STRIDE + 16), "n"(2 * STRIDE + 16),
+          "n"(3 * STRIDE + 16), "l"(policy));
 }
 
 __device__ __forceinline__ void stg_stream(uint4* p, const uint4& v) {
@@ -136,17 +154,6 @@ __device__ __forceinline__ void tma_store_1d(void* gdst, const void* smem_src, u
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst),
                  "r"(smem_u32(smem_src)), "r"(bytes)
                  : "memory");
-}
-// L2 eviction-priority policies for the bulk copies (streaming data is touched once).
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-    return p;
 }
 __device__ __forceinline__ void tma_load_1d_hint(void* smem_dst, const void* gsrc, uint32_t bytes,
                                                  uint64_t* bar, uint64_t policy) {
@@ -343,13 +350,14 @@ hbm_read_ldg_kernel(const uint4* __restrict__ base, unsigned long long n_vec, co
     Acc A, B;
     constexpr unsigned long long tile_vecs = (unsigned long long)THREADS * 8;  // 128 B / thread
     const unsigned long long n_tiles = n_vec / tile_vecs;
+    const uint64_t pol = WIDE ? l2_policy_evict_first() : 0;
     for (unsigned long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         if (WIDE) {
             // thread t owns 32-byte vectors t, t+T, t+2T, t+3T of the tile (two 16-byte vectors each)
             const unsigned long long v0 = tile * tile_vecs + 2ull * threadIdx.x;
             const unsigned char* p = reinterpret_cast<const unsigned char*>(base + v0);
             unsigned long long w[16];
-            ldg256_x4<THREADS * 32>(p, w);
+            ldg256_x4<THREADS * 32>(p, pol, w);
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const unsigned long long v = v0 + 2ull * j * THREADS;
@@ -972,12 +980,10 @@ cudaError_t plan_kernels(int device, KernelPlan* plan) {
         plan->copy_fused = {sms * (occ > 0 ? occ : 1), (int)plan->fused_threads, smem};
     }
     // An SM changes its L1 / shared-memory split only when it is empty, so a kernel that asks for the default split
-    // keeps the copy's CTA (128 KiB of shared memory) off every SM it occupies — measured: the first copy sweep waited
-    // for the whole generator.  The generator and the kernels it may run beside therefore ask for the SAME split, the
-    // largest shared memory.  That includes the fill: in cro_probe_all it runs beside the generator of the NVLink prefix
-    // (measured: the full-box HBM phase is 9.96 ms with it, 10.56 ms without, tools/r02_ab.py).  Not the LDG kernels:
-    // they never run beside a generator, and the smallest L1 costs them 12 % (7.30 -> 6.42 TB/s at 4 GiB,
-    // profiles/r02_fused_copy_first_look.jsonl vs r02_size_sweep.jsonl).
+    // keeps the copy's CTA (128 KiB of shared memory) off every SM it occupies, and the first copy sweep waits for the
+    // whole generator.  The generator and the kernels it may run beside therefore ask for the SAME split, the largest
+    // shared memory.  That includes the fill: in cro_probe_all it runs beside the generator of the NVLink prefix.  Not
+    // the LDG kernels: they never run beside a generator, and they want the L1 the smallest split would take away.
     for (const void* fn : {(const void*)hbm_expected_kernel, (const void*)hbm_read_tma_kernel, (const void*)hbm_copy_fused_kernel,
                            (const void*)hbm_copy_tma_kernel, (const void*)probe_finalize_kernel})
         if ((e = cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)) != cudaSuccess)
@@ -991,8 +997,7 @@ cudaError_t plan_kernels(int device, KernelPlan* plan) {
         return e;
     // The generator runs BESIDE the copy sweeps: it may not fill the SM, or the copy's CTA (160 threads, 128 KiB of
     // shared memory) would have to wait for it to drain; and the fewer of its warps compete with the copy's consumer
-    // warps for issue slots the better.  Measured per probe (S = 4 GiB): 9.69 ms with 1 CTA of 256 threads per SM,
-    // 10.13 with 2, 10.32 with 4, 10.57 with the generator in line (profiles/r02_expect_overlap.md).
+    // warps for issue slots the better: one CTA of 256 threads per SM by default (CRO_EXPECT_CTAS).
     plan->expect = {sms * std::min<int>(occ > 0 ? occ : 1, (int)env::get("CRO_EXPECT_CTAS")), 256, 0};
     return cudaSuccess;
 }
@@ -1006,7 +1011,7 @@ static int clamp_grid(int planned, uint64_t bytes, uint64_t tile_bytes) {
 cudaError_t launch_fill(const KernelPlan& p, void* base, uint64_t bytes, const Params& pr,
                         const SweepScratch& sc, SweepOut* out, cudaStream_t st) {
     // Few tiles per CTA: with a fixed grid a 16 GiB fill strides 14 tiles per CTA, the SMs drift apart and the DRAM
-    // window spreads (7.50 TB/s at 4 GiB but 7.16 at 16 GiB and 6.76 at 32 GiB); the grid therefore grows with the sweep.
+    // window spreads and the rate drops as the sweep grows; the grid therefore grows with the sweep.
     constexpr uint64_t kTile = (uint64_t)kFillThreads * kFillUnroll * 16;
     const uint64_t tiles = (bytes + kTile - 1) / kTile;
     const int planned = (int)std::min<uint64_t>(std::max<uint64_t>((uint64_t)p.fill.grid, tiles / 4), 0x7FFFFFFFull);
@@ -1017,9 +1022,6 @@ cudaError_t launch_fill(const KernelPlan& p, void* base, uint64_t bytes, const P
 
 cudaError_t launch_read(const KernelPlan& p, unsigned variant, const void* base, uint64_t bytes,
                         const Params& pr, const SweepScratch& sc, SweepOut* out, cudaStream_t st) {
-    // 256-bit loads need a 32-byte aligned base; half B of a region whose S is an odd multiple of 16 bytes is only
-    // 16-byte aligned (found by the ragged-size parity tests): such a sweep takes the 128-bit flavour.
-    if (variant == READ_LDG256 && (reinterpret_cast<uintptr_t>(base) & 31u)) variant = READ_LDG;
     if (variant == READ_TMA) {
         hbm_read_tma_kernel<<<clamp_grid(p.read_tma.grid, bytes, p.read_tile), p.read_tma.block, p.read_tma.smem, st>>>(
             static_cast<const unsigned char*>(base), bytes, p.read_tile, p.read_stages, p.read_chunk,

@@ -1,4 +1,4 @@
-// kernels.cuh — launch wrappers for the sm_100a probe kernels.
+// kernels.cuh — launch wrappers for the sm_90a probe kernels.
 //
 // No reference counterpart: the reference's post-attach check is a UUID string
 // match (internal/utils/gpus.go:54-86); these kernels are the strong check that

@@ -185,7 +185,8 @@ Reply QueryGpu(const std::string& lib, const std::string& query) {
         snprintf(d.gpu_uuid, sizeof d.gpu_uuid, "%.47s", uuid);
         PciInfo p;
         memset(&p, 0, sizeof p);
-        if (s->pci(dev, &p) == kSuccess) snprintf(d.pci_bus_id, sizeof d.pci_bus_id, "%.23s", p.busId);
+        // nvidia-smi spells a bus id NVML will not give (some virtualised hosts) "[N/A]"
+        snprintf(d.pci_bus_id, sizeof d.pci_bus_id, "%.23s", s->pci(dev, &p) == kSuccess ? p.busId : "[N/A]");
         unsigned minor = 0;
         if (s->minor && s->minor(dev, &minor) == kSuccess) d.device_minor = (int)minor;
         char name[96] = {0};

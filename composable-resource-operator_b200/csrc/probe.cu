@@ -31,10 +31,9 @@ namespace {
 constexpr uint64_t kDefaultSweep = 4ull << 30;
 constexpr uint64_t kDefaultP2P = 1ull << 30;
 constexpr uint64_t kDefaultSeedBase = 0x00C0FFEE00000000ull;
-// 1024 hops: the mean hop latency — and every pair's own value — is the same to 0.1 % at 1 Ki, 4 Ki, 16 Ki and 64 Ki hops
-// (8 GPUs: 1779.4 / 1780.0 / 1780.4 / 1780.6 ns; 2 GPUs: 1860.4 / 1862.7 / 1861.7 / 1861.6; profiles/r02_latency_vs_hops.md),
-// while 64 Ki hops of ~1.8 us would be 122 ms, three times the rest of the full-box probe.  SURVEY.md §8d's 64 Ki is one
-// cro_set_latency_hops / latency_hops away, and bench.py runs all four lengths every time.
+// 1024 hops: a dependent chase of that length already averages over the hop-to-hop jitter, while 64 Ki hops of a
+// microsecond-scale peer load would cost more than the rest of the full-box probe.  SURVEY.md §8d's 64 Ki is one
+// cro_set_latency_hops / latency_hops away, and bench.py runs 1 Ki, 4 Ki, 16 Ki and 64 Ki every time on several GPUs.
 constexpr uint32_t kDefaultHops = 1024;
 
 #define CU_TRY(ctx, expr)                                                              \
@@ -67,7 +66,7 @@ int ensure_region(cro_ctx* c, Device* d) {
     CU_TRY(c, cudaSetDevice(d->ordinal));
     // A device that is already in use may not have 2*S free (the reference's own pre-check for that
     // is CheckNoGPULoads, internal/utils/gpus.go:88).  Degrade: halve S down to 64 MiB — still far
-    // beyond the 126 MB L2 when doubled — and report the size actually swept in the result.
+    // beyond the 50 MB L2 when doubled — and report the size actually swept in the result.
     const uint64_t asked = d->sweep_bytes;
     cudaError_t e = cudaErrorMemoryAllocation;
     for (uint64_t s = asked;; s = (s / 2) & ~(uint64_t)15) {
@@ -154,13 +153,14 @@ void free_scratch(SweepScratch* sc) {
 }  // namespace
 
 uint32_t resolve_read_variant(uint32_t v, uint64_t bytes) {
-    // AUTO: the TMA ring has the higher asymptote (7.47 vs 7.36 TB/s at 4 GiB) but ~5.5 us more constant cost per launch
-    // (ring ramp and drain, profiles/r02_fixed_cost.md), so small sweeps go to plain 256-bit LDG.  Whole probes, median of
-    // 30 (profiles/r02_auto_threshold.jsonl): 256 MiB 732 us with LDG.256 vs 755 with TMA, 512 MiB 1342 vs 1357, 1 GiB
-    // 2594 vs 2551, 2 GiB 5133 vs 5104 — the crossover sits between 512 MiB and 1 GiB.
+    // AUTO: the TMA ring has the higher asymptote but a larger constant cost per launch (ring ramp and drain), so small
+    // sweeps go to plain 128-bit LDG.  Whole probes on an H100 SXM (700 W), median of 21: 64 MiB 438 us with LDG vs 457
+    // with TMA, 128 MiB 791 vs 803, 256 MiB 1502 vs 1494, 1 GiB 5702 vs 5627 — the crossover sits between 128 and
+    // 256 MiB (profiles/h100_700w_read_variants.jsonl; a 400 W card agrees, h100_400w_read_variants.jsonl).  The 32-byte
+    // LDG flavour lost to one or the other at every size from 64 MiB to 4 GiB.
     if (v == CRO_READ_AUTO) {
         v = env::get("CRO_READ_VARIANT");
-        if (v == CRO_READ_AUTO) v = bytes <= (512ull << 20) ? CRO_READ_LDG256 : CRO_READ_TMA;
+        if (v == CRO_READ_AUTO) v = bytes <= (128ull << 20) ? CRO_READ_LDG : CRO_READ_TMA;
     }
     return (v == READ_LDG || v == READ_TMA || v == READ_LDG256) ? v : (uint32_t)READ_TMA;
 }
@@ -291,8 +291,8 @@ int ctx_create(const cro_opts* o, cro_ctx** out) {
         for (int i = 0; i < n_cuda && i < CRO_MAX_DEVICES; ++i) ordinals.push_back(i);
     }
 
-    // Identity: /proc first (a directory walk, ~0.06 ms), NVML only when asked to (its first call costs
-    // tens of ms and serialises across processes) — CRO_F_NO_NVML keeps it off the hot-plug path entirely.
+    // Identity: /proc first (a directory walk), NVML only when asked to (its first call is slow and serialises
+    // across processes) — CRO_F_NO_NVML keeps it off the hot-plug path entirely.
     const std::vector<identity::ProcGpu> proc = identity::ScanProc(c->proc_root);
     std::vector<identity::NvmlGpu> nvml;
     bool have_nvml = false;
@@ -841,8 +841,7 @@ static int probe_finish(cro_ctx* c, Device* d, Lane& L, cro_probe_result* r) {
         c->m_probe_failures++;
         c->set_error(describe_failure(d, *r));
         // What the memory itself reported: uncorrected volatile ECC errors (nvmlDeviceGetTotalEccErrors).
-        // NVML calls serialise across processes (measured: ~2 ms each with 4 ranks probing, enough to skew the
-        // ranks' all-gather), so the warm probe reuses the count read at init / at the last full-box probe and
+        // NVML calls serialise across processes (with several ranks probing, enough to skew the ranks' all-gather), so the warm probe reuses the count read at init / at the last full-box probe and
         // only a FAILED probe pays for a fresh read — which then also goes into the device-resident copies.
         const uint32_t before = d->ecc_uncorrected;
         refresh_ecc(c, d);
@@ -1091,12 +1090,12 @@ int ctx_inventory(cro_ctx* c, std::vector<cro_dev_info>* out, bool force) {
     for (auto& d : c->devs) mine.push_back(d->info);
     std::unique_lock<std::mutex> g(c->inv_mu);
     const bool nvml_ok = !(c->opts.flags & CRO_F_NO_NVML);
-    // Every call looks at the node: the registry's directory listing (readdir + stat, ~10 us, no driver lock).  The
+    // Every call looks at the node: the registry's directory listing (readdir + stat, no driver lock).  The
     // `information` files are read again
     //   * at once, when that listing differs from the last one or the caller insists (it was told about a UUID the
     //     list lacks);
     //   * in the BACKGROUND every 30 s — the reference's own requeue period (composableresource_controller.go:223,285)
-    //     — because each such read goes through the driver's locks (100+ ms for a full box while nvidia-smi polls) and
+    //     — because each such read goes through the driver's locks (slow for a full box while nvidia-smi polls) and
     //     a reconcile must not pay for a refresh that will almost always confirm what is known.
     std::string key = identity::ProcRegistryListing(c->proc_root);
     const bool have_proc = !key.empty();
@@ -1136,7 +1135,7 @@ int ctx_inventory(cro_ctx* c, std::vector<cro_dev_info>* out, bool force) {
 int ctx_probe_uuid(cro_ctx* c, const char* uuid, cro_probe_result* out) {
     if (!uuid || !out) return CRO_ERR_INVALID_ARG;
     const std::string want = uuid;
-    uint64_t sweep = 1ull << 30;              // helper default: 1 GiB already sweeps at ~7 TB/s and starts ~4x sooner
+    uint64_t sweep = 1ull << 30;              // helper default: 1 GiB is far beyond the L2 and starts ~4x sooner than 4 GiB
     if (!c) env::reload(nullptr);            // no context ever validated the environment for this caller
     int deadline = (int)env::get("CRO_HELPER_TIMEOUT_MS");
     if (c) {
@@ -1526,8 +1525,8 @@ int ctx_probe_all(cro_ctx* c, cro_probe_result* out, int cap, int* n_out) {
     }
     c->fullbox.enqueue_ns = now_ns() - t_call;
 
-    // While the GPUs work: a fresh ECC read per device (NVML, 3–5 ms each — on the critical path it would cost the box
-    // more than the NVLink rounds of one pair; and eight of them can outlast the 36 ms the GPUs need, so a device is
+    // While the GPUs work: a fresh ECC read per device (NVML, milliseconds each — on the critical path it would cost the
+    // box more than the NVLink rounds of one pair, and eight of them can outlast the GPUs' own work, so a device is
     // asked at most once a second).  The structs being gathered right now carry the count staged before this call; a
     // count that moved is staged for the next probe, and a FAILING probe re-reads it at once anyway.
     std::vector<int> restage;

@@ -1,5 +1,5 @@
 /*
- * croprobe.h — C ABI of libcroprobe, the B200-native post-attach device probe
+ * croprobe.h — C ABI of libcroprobe, the H100-native post-attach device probe
  * and spec-emit path for the composable-resource operator.
  *
  * This header is the drop-in boundary (SURVEY.md §8b).  Everything here is
@@ -63,7 +63,7 @@ extern "C" {
                                           words [0, S/8), half B [S/8, 2S/8)) */
 
 /* read-sweep kernel variants */
-#define CRO_READ_AUTO   0u   /* by sweep size: 256-bit LDG up to 512 MiB, the TMA ring above (measured crossover) */
+#define CRO_READ_AUTO   0u   /* by sweep size: 128-bit LDG up to 128 MiB, the TMA ring above (measured crossover) */
 #define CRO_READ_LDG    1u   /* ld.global.nc.L1::no_allocate 128-bit, unrolled      */
 #define CRO_READ_TMA    2u   /* cp.async.bulk (1-D TMA) smem ring + LDS.128 reduce  */
 #define CRO_COPY_AUTO   0u
@@ -71,7 +71,7 @@ extern "C" {
 #define CRO_COPY_TMA    2u   /* bulk load -> smem -> bulk store, no register pass   */
 #define CRO_COPY_TMA_FUSED 3u /* the same, and consumer warps fold every tile out of shared memory: the sweep
                                 yields the checksum of its source as read (the probe's default)          */
-#define CRO_READ_LDG256 3u   /* 256-bit LDG flavour                                  */
+#define CRO_READ_LDG256 3u   /* 32-byte LDG flavour: two adjacent 128-bit loads, L2 evict_first */
 
 #define CRO_MAX_DEVICES 16
 
@@ -619,7 +619,7 @@ int  cro_local_node_op(cro_ctx *ctx, const char *request_json, char *buf, size_t
  * -q (:970), and with allow_mutation: -i <uuid> -pm 0|1 (:267), drain -p <bus> -m 0|1 (:269), drain -p <bus> -r (:311) —
  * are answered through NVML inside this process when libnvidia-ml is there ("how": "native": no child process, no
  * second NVML init), with nvidia-smi's stdout and exit code (the two queries are pinned byte for byte against the real
- * nvidia-smi on a B200 box; the three mutating texts are not — the reference never parses them).  "native_nvml": false
+ * nvidia-smi on a GPU box; the three mutating texts are not — the reference never parses them).  "native_nvml": false
  * spawns instead; "nvml_lib": "<path>" names another libnvidia-ml (tests).  Both keys work in cro_local_node_op too.
  * Reply: {"how": "spawned"|"skipped (dry run)"|"native", "failed": bool, "exec_err", "stdout", "stderr"}. */
 int  cro_local_exec(const char *request_json, char *buf, size_t cap, size_t *len);

@@ -1,7 +1,7 @@
 """Re-verifies tests/golden/reference_kats.json against the reference tree.
 
-Only meaningful where /root/reference is mounted (the dev container); the GPU
-box has no reference tree and never runs this.  For each vector, every
+Needs a checkout of the reference, given as the first argument; the test
+suite does not run this.  For each vector, every
 expected error / id string must occur verbatim in the cited file.
 """
 import json
@@ -9,7 +9,7 @@ import os
 import re
 import sys
 
-REF = sys.argv[1] if len(sys.argv) > 1 else "/root/reference"
+REF = sys.argv[1]
 HERE = os.path.dirname(os.path.abspath(__file__))
 kats = json.load(open(os.path.join(HERE, "reference_kats.json")))
 cache = {}

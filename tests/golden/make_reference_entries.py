@@ -1,5 +1,5 @@
 """Extract the EXPECTATIONS of the reference's ComposableResource table tests into a fixture.
-(container only: reads /root/reference; the output tests/golden/reference_entries.json travels)
+(reads the reference checkout named by $CRO_REFERENCE; the output tests/golden/reference_entries.json travels)
 
 For every Entry(...) of internal/controller/composableresource_controller_test.go this records
   line, title, the Describe block it sits in, tenant/cluster uuid (they select the fake fabric's
@@ -14,7 +14,7 @@ import os
 import re
 import sys
 
-SRC = "/root/reference/internal/controller/composableresource_controller_test.go"
+SRC = os.path.join(os.environ["CRO_REFERENCE"], "internal", "controller", "composableresource_controller_test.go")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "reference_entries.json")
 
 STR = r'"((?:[^"\\]|\\.)*)"'

@@ -1,5 +1,5 @@
 """Extracts the reference's wire / status struct DECLARATIONS — field order, Go types, json tags, omitempty — from its Go
-source and writes tests/golden/wire_structs.json.  Run from the repo root (needs /root/reference):
+source and writes tests/golden/wire_structs.json.  Run from the repo root with $CRO_REFERENCE naming a checkout of the reference:
 
     python tests/golden/make_wire_structs.py            # (re)write the fixture
     python tests/golden/make_wire_structs.py --check    # exit 1 if the committed fixture differs from the reference
@@ -12,7 +12,7 @@ import os
 import re
 import sys
 
-REF = "/root/reference"
+REF = os.environ["CRO_REFERENCE"]
 FILES = ["internal/cdi/fti/fm/api/common.go", "internal/cdi/fti/fm/api/scale_up.go", "internal/cdi/fti/fm/api/scale_down.go",
          "internal/cdi/fti/fm/api/get.go", "internal/cdi/fti/cm/api/machine.go", "internal/cdi/fti/cm/client.go",
          "internal/cdi/sunfish/client.go", "internal/cdi/client.go", "api/v1alpha1/composableresource_types.go",

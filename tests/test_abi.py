@@ -38,16 +38,16 @@ def test_result_struct_layout(cro):
         assert getattr(R, k).offset == v, k
 
 
-def test_library_has_sm100a_code_and_blackwell_instructions():
+def test_library_has_sm90a_code_and_hopper_instructions():
     so = os.path.join(ROOT, "composable-resource-operator_b200", "libcroprobe.so")
     out = subprocess.run(["cuobjdump", "-lelf", so], capture_output=True, text=True)
     if out.returncode != 0:
         pytest.skip("cuobjdump unavailable")
-    assert "sm_100a" in out.stdout
+    assert "sm_90a" in out.stdout and "sm_100" not in out.stdout
     sass = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
     assert "UBLKCP" in sass, "1-D TMA bulk copies must be present (cp.async.bulk)"
     assert "SYNCS" in sass, "mbarrier instructions must be present"
-    assert "LDG.E" in sass and ".256" in sass, "256-bit global loads must be present"
+    assert "LDG.E.NA.128.CONSTANT" in sass, "128-bit read-only, no-L1-allocate global loads must be present"
 
 
 @pytest.mark.skipif(os.path.exists("/dev/nvidiactl"), reason="a GPU is present")
@@ -61,7 +61,7 @@ def test_no_gpu_fails_loudly(cro):
 def test_strerror_and_version(cro):
     assert cro.strerror(0) == "ok"
     assert cro.strerror(cro.ERR_CHECKSUM) == "hbm checksum mismatch"
-    assert "sm_100a" in cro.version()
+    assert "sm_90a" in cro.version()
 
 
 def build_c_harness():

@@ -2,11 +2,12 @@
 (reference: internal/utils/gpus.go:125,134 compute apps; :970 drain -q; :267,269,311 the three mutating commands).
 
 This container has no NVML, so the CPU tests load tests/fake_nvml.c as the library; the texts they expect for the two
-QUERIES are the ones captured from the real nvidia-smi on a B200 box (tests/golden/nvidia_smi_texts.json, made by
+QUERIES are the ones captured from the real nvidia-smi on a GPU box (tests/golden/nvidia_smi_texts.json, made by
 tools/smi_texts.sh).  The GPU test compares the native answers with the box's real nvidia-smi byte for byte."""
 import json
 import os
 import subprocess
+import sys
 
 import pytest
 
@@ -157,6 +158,10 @@ def test_native_answers_equal_the_real_nvidia_smi(cro):
 def test_query_gpu_without_a_probe_context(cro, fake_lib, node):
     out = cro.local_exec([SMI, "--query-gpu=device_minor,gpu_uuid,pci.bus_id", FMT], nvml_lib=fake_lib)
     assert out["how"] == "native" and out["stdout"] == "0, %s, 00000000:40:00.0\n1, %s, 00000000:41:00.0\n" % (A, B)
+    # a host whose NVML will not give PCI info (NVML_ERROR_NOT_SUPPORTED): nvidia-smi prints "[N/A]" for the bus id
+    (node / "fail").write_text("nvmlDeviceGetPciInfo_v3 3\n")
+    out = cro.local_exec([SMI, "--query-gpu=gpu_uuid,pci.bus_id", FMT], nvml_lib=fake_lib)
+    assert out["how"] == "native" and out["stdout"] == "%s, [N/A]\n%s, [N/A]\n" % (A, B)
     # a field this library does not know is nvidia-smi's to answer
     out = cro.local_exec([SMI, "--query-gpu=temperature.gpu", FMT], nvml_lib=fake_lib)
     assert out["how"] == "spawned"
@@ -202,3 +207,28 @@ def test_a_refused_maintenance_mode_stops_the_drain_where_the_reference_stops(cr
     assert res["error"] == ("detach command 'set maintenance mode' failed: 'command terminated with exit code 255', stderr: '', "
                             "stdout: 'Failed to set the GPU drain state: Insufficient Permissions\n'")
     assert calls(node) == ["set_persistence %s 0" % A]          # no remove after the refusal
+
+
+@pytest.mark.gpu
+def test_probe_context_identity_follows_nvml_bus_id(cro, fake_lib, tmp_path):
+    """A context takes the bus id from NVML when NVML knows the device, and spells it "[N/A]" — nvidia-smi's answer — when
+    NVML refuses the PCI info.  A fresh process loads tests/fake_nvml.c as libnvidia-ml.so.1, listing this GPU's UUID."""
+    with cro.ProbeContext(sweep_bytes=1 << 20, devices=[0], flags=cro.F_LAZY_ALLOC | cro.F_NO_NVML) as c:
+        uuid = c.own_devices()[0].gpu_uuid.decode()
+    libdir = tmp_path / "lib"
+    libdir.mkdir()
+    os.symlink(fake_lib, str(libdir / "libnvidia-ml.so.1"))
+    state = tmp_path / "state"
+    state.mkdir()
+    (state / "gpus").write_text("%s 00000000:4A:00.0 1\n" % uuid)
+    root = os.path.dirname(HERE)
+    child = ("import importlib, sys; sys.path.insert(0, %r); cro = importlib.import_module('composable-resource-operator_b200')\n"
+             "with cro.ProbeContext(sweep_bytes=1 << 20, devices=[0], flags=cro.F_LAZY_ALLOC) as c:\n"
+             "    print(cro.emit_csv(c.own_devices(), 'gpu_uuid,pci.bus_id'), end='')\n" % root)
+    env = dict(os.environ, LD_LIBRARY_PATH=str(libdir) + os.pathsep + os.environ.get("LD_LIBRARY_PATH", ""), FAKE_NVML_DIR=str(state))
+    for fail, want in (("", "00000000:4A:00.0"), ("nvmlDeviceGetPciInfo_v3 3\n", "[N/A]")):
+        (state / "fail").write_text(fail)
+        out = subprocess.run([sys.executable, "-c", child], env=env, capture_output=True, text=True, timeout=120)
+        assert out.returncode == 0, out.stderr[-1500:]
+        assert out.stdout == "%s, %s\n" % (uuid, want), out.stdout
+

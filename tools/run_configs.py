@@ -1,7 +1,7 @@
 """Runs BASELINE.json configs 3, 4 and 5 on the box's GPUs (single process, as a Go operator would) and prints
 one JSON object per config.  Config 2 is bench.py; config 1 is `bench.py --impl reference`.
 
-  config 3  8xB200 full-box compose: cro_probe_all (concurrent probes + NVLink rounds + one NCCL all-gather)
+  config 3  8xH100 full-box compose: cro_probe_all (concurrent probes + NVLink rounds + one NCCL all-gather)
   config 4  reconcile storm: 1000 synthetic ComposabilityRequests over the box's GPUs, warm probe contexts
   config 5  attach/detach churn: 100 cycles x 4-GPU compose / decompose, probe each attach
 

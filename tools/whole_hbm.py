@@ -1,6 +1,6 @@
-"""One probe over (nearly) the whole HBM of a B200: S = 84 GiB per half, a 168 GiB region of the 180 GB part
-(falls back to 80 / 72 / 64 GiB if the allocation is refused).  Every sweep against the C oracle's closed form — word
-indices run to 2^33.4.  JSON line on stdout."""
+"""One probe over (nearly) the whole HBM of an H100: S = 36 GiB per half, a 72 GiB region of the 80 GB part
+(falls back to 34 / 32 / 28 GiB if the allocation is refused).  Every sweep against the C oracle's closed form — word
+indices run past 2^32.  JSON line on stdout."""
 import importlib
 import json
 import os
@@ -17,7 +17,7 @@ cro = importlib.import_module("composable-resource-operator_b200")
 import oracle  # noqa: E402  (the checker)
 
 co = oracle.COracle()
-for gib in (84, 80, 72, 64):
+for gib in (36, 34, 32, 28):
     S = gib << 30
     try:
         ctx = cro.ProbeContext(sweep_bytes=S, devices=[0])
