@@ -339,7 +339,8 @@ int cro_validate_env(const char* name, const char* value, char* err_buf, size_t 
         copy_out("unknown knob " + S(name), err_buf, err_cap, nullptr);
         return CRO_ERR_UNSUPPORTED;
     }
-    if (env::reload(&why)) return CRO_OK;
+    env::Values checked;                      // a check only: no context's knobs change
+    if (env::read(&checked, &why)) return CRO_OK;
     copy_out(why, err_buf, err_cap, nullptr);
     return CRO_ERR_INVALID_ARG;
 } CRO_API_CATCH

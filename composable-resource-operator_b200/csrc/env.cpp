@@ -4,8 +4,6 @@
 
 #include <cstdlib>
 #include <cstring>
-#include <mutex>
-#include <vector>
 
 namespace cro {
 namespace env {
@@ -47,12 +45,10 @@ const Knob kKnobs[] = {
 };
 constexpr int kN = (int)(sizeof kKnobs / sizeof kKnobs[0]);
 
-std::mutex g_mu;
-unsigned g_val[kN];
-bool g_loaded = false;
-
-void load_defaults_locked() {
-    for (int i = 0; i < kN; ++i) g_val[i] = kKnobs[i].dflt;
+int index_of(const char* name) {
+    for (int i = 0; i < kN; ++i)
+        if (strcmp(kKnobs[i].name, name) == 0) return i;
+    return -1;
 }
 }  // namespace
 
@@ -61,9 +57,13 @@ const Knob* table(int* n_out) {
     return kKnobs;
 }
 
+std::string refusal(const char* name, const std::string& text) {
+    return std::string("the env variable ") + name + " has an invalid value: '" + text + "'";
+}
+
 bool parse(const Knob& k, const char* text, unsigned* out, std::string* err) {
     auto bad = [&]() {
-        if (err) *err = std::string("the env variable ") + k.name + " has an invalid value: '" + (text ? text : "") + "'";
+        if (err) *err = refusal(k.name, text ? text : "");
         return false;
     };
     if (!text || !*text) {
@@ -82,41 +82,32 @@ bool parse(const Knob& k, const char* text, unsigned* out, std::string* err) {
     return true;
 }
 
-bool reload(std::string* err) {
-    unsigned fresh[kN];
+Values::Values() {
+    static_assert(kN <= kMax, "Values::kMax is smaller than the knob table");
+    for (int i = 0; i < kN; ++i) v_[i] = kKnobs[i].dflt;
+}
+
+unsigned Values::get(const char* name) const {
+    const int i = index_of(name);
+    return i < 0 ? 0u : v_[i];
+}
+
+bool read(Values* out, std::string* err) {
+    Values fresh;
     for (int i = 0; i < kN; ++i)
-        if (!parse(kKnobs[i], getenv(kKnobs[i].name), &fresh[i], err)) return false;
-    // the ring must fit the 227 KB a CTA may own
-    auto at = [&](const char* name) {
-        for (int i = 0; i < kN; ++i)
-            if (strcmp(kKnobs[i].name, name) == 0) return i;
-        return 0;
-    };
+        if (!parse(kKnobs[i], getenv(kKnobs[i].name), &fresh.v_[i], err)) return false;
+    // the ring must fit the shared memory a CTA may own, next to the ring kernels' own
     const char* rings[3][2] = {{"CRO_TMA_READ_TILE", "CRO_TMA_READ_STAGES"}, {"CRO_TMA_COPY_TILE", "CRO_TMA_COPY_STAGES"},
                                {"CRO_FUSED_TILE", "CRO_FUSED_STAGES"}};
     for (auto& r : rings) {
-        const int t = at(r[0]), s = at(r[1]);
-        if ((unsigned long long)fresh[t] * fresh[s] > 227ull * 1024 - 1024) {
+        if ((unsigned long long)fresh.get(r[0]) * fresh.get(r[1]) > kRingMaxBytes) {
             const char* v = getenv(r[0]);
-            if (err) *err = std::string("the env variable ") + r[0] + " has an invalid value: '" + (v ? v : "") + "'";
+            if (err) *err = refusal(r[0], v ? v : "");
             return false;
         }
     }
-    std::lock_guard<std::mutex> g(g_mu);
-    memcpy(g_val, fresh, sizeof fresh);
-    g_loaded = true;
+    *out = fresh;
     return true;
-}
-
-unsigned get(const char* name) {
-    std::lock_guard<std::mutex> g(g_mu);
-    if (!g_loaded) {
-        load_defaults_locked();
-        g_loaded = true;
-    }
-    for (int i = 0; i < kN; ++i)
-        if (strcmp(kKnobs[i].name, name) == 0) return g_val[i];
-    return 0;
 }
 
 }  // namespace env

@@ -18,8 +18,6 @@
 // No tensor cores: there is no contraction anywhere on this path.
 #include "kernels.cuh"
 
-#include "env.hpp"
-
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -910,74 +908,88 @@ constexpr int kReadThreads = 512;
 constexpr int kCopyThreads = 512, kCopyUnroll = 8;
 }  // namespace
 
-cudaError_t plan_kernels(int device, KernelPlan* plan) {
+cudaError_t plan_kernels(int device, const env::Values& knobs, KernelPlan* plan, std::string* why) {
     cudaError_t e;
-    int sms = 0;
+    int sms = 0, optin = 0;
     if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device)) != cudaSuccess)
+        return e;
+    if ((e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device)) != cudaSuccess)
         return e;
     plan->sm_count = sms;
     int occ = 0;
+    auto knob = [&](const char* name) { return knobs.get(name); };
 
     auto fill = hbm_fill_kernel<kFillThreads, kFillUnroll>;
     if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fill, kFillThreads, 0)) != cudaSuccess)
         return e;
-    plan->fill = {sms * (occ > 0 ? occ : 1) * (int)env::get("CRO_FILL_WAVES"), kFillThreads, 0};
+    plan->fill = {sms * (occ > 0 ? occ : 1) * (int)knob("CRO_FILL_WAVES"), kFillThreads, 0};
 
     auto rd = hbm_read_ldg_kernel<kReadThreads, false>;
     if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, rd, kReadThreads, 0)) != cudaSuccess)
         return e;
-    plan->read_ldg = {sms * (occ > 0 ? occ : 1) * (int)env::get("CRO_READ_WAVES"), kReadThreads, 0};
+    plan->read_ldg = {sms * (occ > 0 ? occ : 1) * (int)knob("CRO_READ_WAVES"), kReadThreads, 0};
     auto rdw = hbm_read_ldg_kernel<kReadThreads, true>;
     if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, rdw, kReadThreads, 0)) != cudaSuccess)
         return e;
-    plan->read_ldg256 = {sms * (occ > 0 ? occ : 1) * (int)env::get("CRO_READ_WAVES"), kReadThreads, 0};
+    plan->read_ldg256 = {sms * (occ > 0 ? occ : 1) * (int)knob("CRO_READ_WAVES"), kReadThreads, 0};
 
     auto cp = hbm_copy_ldg_kernel<kCopyThreads, kCopyUnroll>;
     if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cp, kCopyThreads, 0)) != cudaSuccess)
         return e;
-    plan->copy_ldg = {sms * (occ > 0 ? occ : 1) * (int)env::get("CRO_COPY_WAVES"), kCopyThreads, 0};
+    plan->copy_ldg = {sms * (occ > 0 ? occ : 1) * (int)knob("CRO_COPY_WAVES"), kCopyThreads, 0};
 
+    // A ring kernel's dynamic shared-memory ceiling belongs to the function in the whole process, not to a context: it
+    // is set to everything the device lets a CTA own beside the kernel's static shared memory, the same value for every
+    // context, so a context planned with a small ring cannot shrink it under another one's larger ring.  Launches and
+    // occupancy use the context's own ring.  A ring that does not fit, or fits no CTA on an SM, is refused by its tile
+    // knob.
+    auto plan_ring = [&](const void* fn, const char* tile_knob, size_t ring, int threads) -> cudaError_t {
+        cudaFuncAttributes fa;
+        cudaError_t r;
+        if ((r = cudaFuncGetAttributes(&fa, fn)) != cudaSuccess) return r;
+        const size_t room = (size_t)optin > fa.sharedSizeBytes ? (size_t)optin - fa.sharedSizeBytes : 0;
+        if (ring > room) {
+            *why = env::refusal(tile_knob, std::to_string(knob(tile_knob)));
+            return cudaErrorInvalidValue;
+        }
+        if ((r = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)room)) != cudaSuccess) return r;
+        if ((r = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, threads, ring)) != cudaSuccess) return r;
+        if (occ < 1) {
+            *why = env::refusal(tile_knob, std::to_string(knob(tile_knob)));
+            return cudaErrorInvalidValue;
+        }
+        return cudaSuccess;
+    };
     {
-        plan->read_tile = env::get("CRO_TMA_READ_TILE");
-        plan->read_stages = env::get("CRO_TMA_READ_STAGES");
-        plan->read_chunk = (env::get("CRO_TMA_READ_CHUNK") & 0xFFFFu) | (env::get("CRO_TMA_READ_HINT") << 16);
-        plan->read_dyn = env::get("CRO_TMA_READ_DYN");
-        const int threads = (int)env::get("CRO_TMA_READ_THREADS");
+        plan->read_tile = knob("CRO_TMA_READ_TILE");
+        plan->read_stages = knob("CRO_TMA_READ_STAGES");
+        plan->read_chunk = (knob("CRO_TMA_READ_CHUNK") & 0xFFFFu) | (knob("CRO_TMA_READ_HINT") << 16);
+        plan->read_dyn = knob("CRO_TMA_READ_DYN");
+        const int threads = (int)knob("CRO_TMA_READ_THREADS");
         const size_t smem = (size_t)plan->read_tile * plan->read_stages;
-        if ((e = cudaFuncSetAttribute(hbm_read_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)smem)) != cudaSuccess)
+        if ((e = plan_ring((const void*)hbm_read_tma_kernel, "CRO_TMA_READ_TILE", smem, threads)) != cudaSuccess)
             return e;
-        if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, hbm_read_tma_kernel, threads, smem)) != cudaSuccess)
-            return e;
-        plan->read_tma = {sms * (occ > 0 ? occ : 1) * (int)env::get("CRO_TMA_READ_WAVES"), threads, smem};
+        plan->read_tma = {sms * occ * (int)knob("CRO_TMA_READ_WAVES"), threads, smem};
     }
     {
-        plan->copy_tile = env::get("CRO_TMA_COPY_TILE");
-        plan->copy_stages = env::get("CRO_TMA_COPY_STAGES");
-        plan->copy_chunk = (env::get("CRO_TMA_COPY_CHUNK") & 0xFFFFu) | (env::get("CRO_TMA_COPY_HINT") << 16);
-        plan->copy_dyn = env::get("CRO_TMA_COPY_DYN");
+        plan->copy_tile = knob("CRO_TMA_COPY_TILE");
+        plan->copy_stages = knob("CRO_TMA_COPY_STAGES");
+        plan->copy_chunk = (knob("CRO_TMA_COPY_CHUNK") & 0xFFFFu) | (knob("CRO_TMA_COPY_HINT") << 16);
+        plan->copy_dyn = knob("CRO_TMA_COPY_DYN");
         const size_t smem = (size_t)plan->copy_tile * plan->copy_stages;
-        if ((e = cudaFuncSetAttribute(hbm_copy_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)smem)) != cudaSuccess)
+        if ((e = plan_ring((const void*)hbm_copy_tma_kernel, "CRO_TMA_COPY_TILE", smem, 32)) != cudaSuccess)
             return e;
-        if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, hbm_copy_tma_kernel, 32, smem)) !=
-            cudaSuccess)
-            return e;
-        plan->copy_tma = {sms * (occ > 0 ? occ : 1) * (int)env::get("CRO_TMA_COPY_WAVES"), 32, smem};
+        plan->copy_tma = {sms * occ * (int)knob("CRO_TMA_COPY_WAVES"), 32, smem};
     }
     {
-        plan->fused_tile = env::get("CRO_FUSED_TILE");
-        plan->fused_stages = env::get("CRO_FUSED_STAGES");
-        plan->fused_chunk = env::get("CRO_FUSED_CHUNK") & 0xFFFFu;
-        plan->fused_threads = env::get("CRO_FUSED_THREADS");
+        plan->fused_tile = knob("CRO_FUSED_TILE");
+        plan->fused_stages = knob("CRO_FUSED_STAGES");
+        plan->fused_chunk = knob("CRO_FUSED_CHUNK") & 0xFFFFu;
+        plan->fused_threads = knob("CRO_FUSED_THREADS");
         const size_t smem = (size_t)plan->fused_tile * plan->fused_stages;
-        if ((e = cudaFuncSetAttribute(hbm_copy_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)smem)) != cudaSuccess)
+        if ((e = plan_ring((const void*)hbm_copy_fused_kernel, "CRO_FUSED_TILE", smem, (int)plan->fused_threads)) != cudaSuccess)
             return e;
-        if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, hbm_copy_fused_kernel,
-                                                               (int)plan->fused_threads, smem)) != cudaSuccess)
-            return e;
-        plan->copy_fused = {sms * (occ > 0 ? occ : 1), (int)plan->fused_threads, smem};
+        plan->copy_fused = {sms * occ, (int)plan->fused_threads, smem};
     }
     // An SM changes its L1 / shared-memory split only when it is empty, so a kernel that asks for the default split
     // keeps the copy's CTA (128 KiB of shared memory) off every SM it occupies, and the first copy sweep waits for the
@@ -988,7 +1000,7 @@ cudaError_t plan_kernels(int device, KernelPlan* plan) {
                            (const void*)hbm_copy_tma_kernel, (const void*)probe_finalize_kernel})
         if ((e = cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)) != cudaSuccess)
             return e;
-    if (env::get("CRO_CARVEOUT_FILL"))     // the fill: it does run beside a generator in cro_probe_all (the p2p prefix's)
+    if (knob("CRO_CARVEOUT_FILL"))     // the fill: it does run beside a generator in cro_probe_all (the p2p prefix's)
         if ((e = cudaFuncSetAttribute((const void*)hbm_fill_kernel<kFillThreads, kFillUnroll>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                       cudaSharedmemCarveoutMaxShared)) != cudaSuccess)
             return e;
@@ -998,7 +1010,7 @@ cudaError_t plan_kernels(int device, KernelPlan* plan) {
     // The generator runs BESIDE the copy sweeps: it may not fill the SM, or the copy's CTA (160 threads, 128 KiB of
     // shared memory) would have to wait for it to drain; and the fewer of its warps compete with the copy's consumer
     // warps for issue slots the better: one CTA of 256 threads per SM by default (CRO_EXPECT_CTAS).
-    plan->expect = {sms * std::min<int>(occ > 0 ? occ : 1, (int)env::get("CRO_EXPECT_CTAS")), 256, 0};
+    plan->expect = {sms * std::min<int>(occ > 0 ? occ : 1, (int)knob("CRO_EXPECT_CTAS")), 256, 0};
     return cudaSuccess;
 }
 

@@ -8,7 +8,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <string>
+
 #include "../../include/croprobe.h"
+#include "env.hpp"
 
 namespace cro {
 
@@ -70,12 +73,14 @@ enum : unsigned { READ_LDG = 1, READ_TMA = 2, READ_LDG256 = 3, COPY_LDG = 1, COP
 struct KernelPlan {
     LaunchCfg fill, read_ldg, read_ldg256, read_tma, copy_ldg, copy_tma, copy_fused, expect;
     int sm_count;
-    // tuning knobs, read from the environment ONCE per device (validated; see env.hpp)
+    // tuning knobs, from the owning context's validated snapshot (see env.hpp)
     unsigned read_tile, read_stages, read_chunk, read_dyn;
     unsigned copy_tile, copy_stages, copy_chunk, copy_dyn;
     unsigned fused_tile, fused_stages, fused_chunk, fused_threads;
 };
-cudaError_t plan_kernels(int device, KernelPlan* plan);
+// A ring (tile * stages) that does not fit the device next to the kernel's static shared memory, or that leaves no
+// room for one CTA per SM, is refused: *why gets the knob's refusal sentence and the call returns cudaErrorInvalidValue.
+cudaError_t plan_kernels(int device, const env::Values& knobs, KernelPlan* plan, std::string* why);
 
 // Seed and stamp of a launch: `pp` (device pointer) when non-null — the captured graph's kernels read the 16 bytes
 // the host refreshed — else the immediate `imm`.

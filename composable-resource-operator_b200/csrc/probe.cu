@@ -152,21 +152,21 @@ void free_scratch(SweepScratch* sc) {
 
 }  // namespace
 
-uint32_t resolve_read_variant(uint32_t v, uint64_t bytes) {
+uint32_t resolve_read_variant(uint32_t v, uint64_t bytes, const env::Values& knobs) {
     // AUTO: the TMA ring has the higher asymptote but a larger constant cost per launch (ring ramp and drain), so small
     // sweeps go to plain 128-bit LDG.  Whole probes on an H100 SXM (700 W), median of 21: 64 MiB 438 us with LDG vs 457
     // with TMA, 128 MiB 791 vs 803, 256 MiB 1502 vs 1494, 1 GiB 5702 vs 5627 — the crossover sits between 128 and
     // 256 MiB (profiles/h100_700w_read_variants.jsonl; a 400 W card agrees, h100_400w_read_variants.jsonl).  The 32-byte
     // LDG flavour lost to one or the other at every size from 64 MiB to 4 GiB.
     if (v == CRO_READ_AUTO) {
-        v = env::get("CRO_READ_VARIANT");
+        v = knobs.get("CRO_READ_VARIANT");
         if (v == CRO_READ_AUTO) v = bytes <= (128ull << 20) ? CRO_READ_LDG : CRO_READ_TMA;
     }
     return (v == READ_LDG || v == READ_TMA || v == READ_LDG256) ? v : (uint32_t)READ_TMA;
 }
-uint32_t resolve_copy_variant(uint32_t v) {
+uint32_t resolve_copy_variant(uint32_t v, const env::Values& knobs) {
     if (v == CRO_COPY_AUTO) {
-        v = env::get("CRO_COPY_VARIANT");
+        v = knobs.get("CRO_COPY_VARIANT");
         if (v == CRO_COPY_AUTO) v = CRO_COPY_TMA_FUSED;
     }
     return (v == COPY_LDG || v == COPY_TMA || v == COPY_TMA_FUSED) ? v : (uint32_t)COPY_TMA_FUSED;
@@ -256,13 +256,13 @@ int ctx_create(const cro_opts* o, cro_ctx** out) {
     };
     {
         // the CRO_* knobs, validated the way the reference validates its own environment
-        // (internal/controller/composableresource_adapter.go:42-45)
+        // (internal/controller/composableresource_adapter.go:42-45), and kept: the context never reads them again
         std::string why;
-        if (!env::reload(&why)) {
+        if (!env::read(&c->knobs, &why)) {
             c->set_error(why);
             return CRO_ERR_INVALID_ARG;
         }
-        c->nvtx = env::get("CRO_NVTX") != 0;
+        c->nvtx = c->knobs.get("CRO_NVTX") != 0;
         if (const char* pr = getenv("CRO_PROC_ROOT"))
             if (*pr) c->proc_root = pr;
     }
@@ -364,7 +364,14 @@ int ctx_create(const cro_opts* o, cro_ctx** out) {
         CU_TRY(c.get(), cudaEventCreate(&d->ev1));
         for (cudaEvent_t* ev : {&d->ev_fork, &d->ev_join, &d->ev_hbm_done, &d->ev_aux_done, &d->ev_chase_ready})
             CU_TRY(c.get(), cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
-        CU_TRY(c.get(), plan_kernels(d->ordinal, &d->plan));
+        {
+            std::string why;
+            const cudaError_t pe = plan_kernels(d->ordinal, c->knobs, &d->plan, &why);
+            if (pe != cudaSuccess) {     // a ring the device cannot hold is the knob's fault, not CUDA's
+                c->set_error(why.empty() ? std::string("plan_kernels: ") + cudaGetErrorString(pe) : why);
+                return why.empty() ? CRO_ERR_CUDA : CRO_ERR_INVALID_ARG;
+            }
+        }
         phase("kernel plan (module load)");
         const int max_grid = std::max({d->plan.fill.grid, d->plan.read_ldg.grid, d->plan.read_ldg256.grid,
                                        d->plan.read_tma.grid, d->plan.copy_fused.grid, d->plan.expect.grid, 1});
@@ -514,7 +521,7 @@ int ctx_read(cro_ctx* c, int idx, uint32_t variant, uint32_t iters, bool dst_hal
              cro_sweep_result* out) {
     Device* d = dev_at(c, idx);
     if (!d || !out || iters == 0) return CRO_ERR_INVALID_ARG;
-    variant = resolve_read_variant(variant, d->sweep_bytes);
+    variant = resolve_read_variant(variant, d->sweep_bytes, c->knobs);
     std::lock_guard<std::mutex> g(d->mu);
     drain_pending(c, d);
     CU_TRY(c, cudaSetDevice(d->ordinal));
@@ -543,7 +550,7 @@ int ctx_read(cro_ctx* c, int idx, uint32_t variant, uint32_t iters, bool dst_hal
 int ctx_copy(cro_ctx* c, int idx, uint32_t variant, uint32_t iters, cro_sweep_result* out) {
     Device* d = dev_at(c, idx);
     if (!d || !out || iters == 0) return CRO_ERR_INVALID_ARG;
-    variant = resolve_copy_variant(variant);
+    variant = resolve_copy_variant(variant, c->knobs);
     std::lock_guard<std::mutex> g(d->mu);
     drain_pending(c, d);
     CU_TRY(c, cudaSetDevice(d->ordinal));
@@ -646,8 +653,8 @@ static int probe_enqueue(cro_ctx* c, Device* d, Lane& L) {
     CU_TRY(c, cudaSetDevice(d->ordinal));
     int rc = ensure_region(c, d);
     if (rc) return rc;
-    const uint32_t rv = resolve_read_variant(o.read_variant, d->sweep_bytes);
-    const uint32_t cv = resolve_copy_variant(o.copy_variant);
+    const uint32_t rv = resolve_read_variant(o.read_variant, d->sweep_bytes, c->knobs);
+    const uint32_t cv = resolve_copy_variant(o.copy_variant, c->knobs);
     const uint32_t R = o.read_sweeps;
     const uint32_t C = (o.flags & CRO_F_SKIP_COPY) ? 0 : o.copy_sweeps;
     if (d->tmpl.sweep_bytes != d->sweep_bytes) {      // ensure_region degraded S
@@ -662,7 +669,7 @@ static int probe_enqueue(cro_ctx* c, Device* d, Lane& L) {
         L.evpool.push_back(e);
     }
     std::vector<cudaEvent_t>& ev = L.evpool;
-    const bool overlap = env::get("CRO_EXPECT_OVERLAP") != 0;
+    const bool overlap = c->knobs.get("CRO_EXPECT_OVERLAP") != 0;
     unsigned char* half[2] = {d->region, d->region + d->sweep_bytes};
     const Params gp = graph_params(L);
 
@@ -735,7 +742,7 @@ static int probe_enqueue(cro_ctx* c, Device* d, Lane& L) {
     const uint64_t graph_key = ((uint64_t)rv << 48) ^ ((uint64_t)cv << 40) ^ ((uint64_t)R << 24) ^ ((uint64_t)C << 8) ^
                                (overlap ? 1u : 0u) ^ (d->sweep_bytes << 1) ^
                                ((o.flags & CRO_F_TEST_INJECT) ? ((uint64_t)o.test_inject_after << 56) ^ (o.test_inject_word * 0x9E3779B97F4A7C15ull) ^ o.test_inject_mask : 0);
-    if (env::get("CRO_USE_GRAPH") && !L.graph_failed) {
+    if (c->knobs.get("CRO_USE_GRAPH") && !L.graph_failed) {
         if (L.graph_exec && L.graph_key != graph_key) {
             cudaGraphExecDestroy(L.graph_exec);
             L.graph_exec = nullptr;
@@ -1136,8 +1143,10 @@ int ctx_probe_uuid(cro_ctx* c, const char* uuid, cro_probe_result* out) {
     if (!uuid || !out) return CRO_ERR_INVALID_ARG;
     const std::string want = uuid;
     uint64_t sweep = 1ull << 30;              // helper default: 1 GiB is far beyond the L2 and starts ~4x sooner than 4 GiB
-    if (!c) env::reload(nullptr);            // no context ever validated the environment for this caller
-    int deadline = (int)env::get("CRO_HELPER_TIMEOUT_MS");
+    env::Values knobs;                        // no context: this caller's environment, defaults where it is illegal
+    if (c) knobs = c->knobs;
+    else env::read(&knobs, nullptr);
+    int deadline = (int)knobs.get("CRO_HELPER_TIMEOUT_MS");
     if (c) {
         std::vector<cro_dev_info> inv;
         int rc = ctx_inventory(c, &inv);
@@ -1384,8 +1393,8 @@ int ctx_probe_all(cro_ctx* c, cro_probe_result* out, int cap, int* n_out) {
     // Per round and device (partner p):  [wait p's HBM phase, p's previous re-read]  READ p's half A over the
     // link -> PUSH my prefix into p's half B -> [wait p's push]  RE-READ my own half B locally.  Both directions
     // of a pair run at once; nothing waits on the host.
-    const bool unidir = env::get("CRO_P2P_UNIDIR") != 0;
-    const unsigned rvp = env::get("CRO_P2P_READ_VARIANT"), wvp = env::get("CRO_P2P_WRITE_VARIANT");
+    const bool unidir = c->knobs.get("CRO_P2P_UNIDIR") != 0;
+    const unsigned rvp = c->knobs.get("CRO_P2P_READ_VARIANT"), wvp = c->knobs.get("CRO_P2P_WRITE_VARIANT");
     auto pair_ok = [&](int a, int b) { return a < 8 && b < 8 && c->devs[(size_t)a]->tmpl.p2p_access[b]; };
     auto push_bytes = [&](const Device* a, const Device* b) {
         return std::min<uint64_t>(std::min<uint64_t>(o.p2p_bytes, a->sweep_bytes), b->sweep_bytes);
@@ -1428,7 +1437,7 @@ int ctx_probe_all(cro_ctx* c, cro_probe_result* out, int cap, int* n_out) {
                 CU_TRY(c, cudaSetDevice(b->ordinal));
                 if (push) {
                     CU_TRY(c, cudaStreamWaitEvent(b->stream, a->ev_push_done[r], 0));
-                    CU_TRY(c, launch_read(b->plan, resolve_read_variant(CRO_READ_AUTO, push_bytes(a, b)), b->region + b->sweep_bytes,
+                    CU_TRY(c, launch_read(b->plan, resolve_read_variant(CRO_READ_AUTO, push_bytes(a, b), c->knobs), b->region + b->sweep_bytes,
                                           push_bytes(a, b), imm_params(b), b->scratch, &b->d_out[kSlotP2P0 + 3 * pr.first + 2], b->stream));
                     c->launches++;
                 }

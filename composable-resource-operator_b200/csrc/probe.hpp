@@ -131,6 +131,8 @@ struct cro_ctx {
     bool nccl_ready = false;
     bool peers_enabled = false;
     bool nvtx = true;
+    // the CRO_* knobs as validated by cro_probe_init: everything the context plans and probes with reads these
+    cro::env::Values knobs;
     std::string proc_root = "/proc";   // where the node's /proc is mounted (tests point it at a fake tree)
     // the node's inventory as of the last enumeration (inventory.hpp)
     std::mutex inv_mu;
@@ -190,8 +192,9 @@ int ctx_expected(cro_ctx* c, int idx, cro_sweep_result* out);
 int ctx_inject(cro_ctx* c, int idx, uint64_t word, uint64_t mask);
 int ctx_read_words(cro_ctx* c, int idx, uint64_t first, uint64_t n, uint64_t* out);
 
-uint32_t resolve_read_variant(uint32_t v, uint64_t bytes);
-uint32_t resolve_copy_variant(uint32_t v);
+// CRO_READ_AUTO / CRO_COPY_AUTO resolved with a context's knobs (CRO_READ_VARIANT, CRO_COPY_VARIANT).
+uint32_t resolve_read_variant(uint32_t v, uint64_t bytes, const env::Values& knobs);
+uint32_t resolve_copy_variant(uint32_t v, const env::Values& knobs);
 
 // Host restatement of the latency permutation of one directed pair (Sattolo cycle over kChaseSlots slots,
 // mt19937_64 seeded with minor_src * 8 + minor_dst; SURVEY.md §8d config 3): perm[i] = successor of slot i.

@@ -400,7 +400,8 @@ int  cro_chase_end(int minor_src, int minor_dst, uint32_t hops, uint32_t *end);
 /* The CRO_* environment knobs are validated like the reference validates its own
  * (internal/controller/composableresource_adapter.go:42-45): an illegal value fails cro_probe_init with
  * "the env variable <NAME> has an invalid value: '<v>'".  This checks one (name, value) pair — or, with
- * name == NULL, the process environment as cro_probe_init would — without needing a GPU. */
+ * name == NULL, the process environment as cro_probe_init would — without needing a GPU.  It is a check only:
+ * a context keeps the values it was created with, whatever the environment says later. */
 int  cro_validate_env(const char *name, const char *value, char *err_buf, size_t err_cap);
 /* Kernel launches issued by this context so far (bench "gpu_launches"). */
 uint64_t cro_launch_count(cro_ctx *ctx);

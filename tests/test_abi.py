@@ -64,9 +64,10 @@ def test_strerror_and_version(cro):
     assert "sm_90a" in cro.version()
 
 
-def build_c_harness():
-    """gcc (plain C, not nvcc / g++) against include/croprobe.h, linked to the shared library like cgo does."""
-    exe = os.path.join(ROOT, "tests", "_c_abi_harness")
+def build_c_harness(out_dir):
+    """gcc (plain C, not nvcc / g++) against include/croprobe.h, linked to the shared library like cgo does.  The
+    executable goes to out_dir: the checkout under test may be read-only."""
+    exe = os.path.join(str(out_dir), "c_abi_harness")
     src = os.path.join(ROOT, "tests", "c_abi_harness.c")
     pkg = os.path.join(ROOT, "composable-resource-operator_b200")
     subprocess.check_call(["gcc", "-std=c11", "-Wall", "-Wextra", "-Werror", "-I" + os.path.join(ROOT, "include"), src, "-o", exe,
@@ -74,8 +75,8 @@ def build_c_harness():
     return exe
 
 
-def test_c_harness_links_and_runs_like_cgo(cro):
-    exe = build_c_harness()
+def test_c_harness_links_and_runs_like_cgo(cro, tmp_path):
+    exe = build_c_harness(tmp_path)
     out = subprocess.run([exe], capture_output=True, text=True)
     assert out.returncode == 0, out.stdout + out.stderr
     assert "c abi harness ok" in out.stdout

@@ -1,6 +1,9 @@
 """CRO_* knobs are validated the way the reference validates its environment
 (internal/controller/composableresource_adapter.go:42-45, :64, :67): strict parse, legal range, one wording."""
+import os
 import re
+import shutil
+import subprocess
 
 import pytest
 
@@ -54,3 +57,68 @@ def test_chase_end_matches_the_golden_vectors(cro):
     g = json.load(open(os.path.join(root, "tests", "golden", "pattern_kats.json")))
     for c in g["chase_ends"]:
         assert cro.chase_end(c["minor_src"], c["minor_dst"], c["hops"]) == c["end"], c
+
+
+# An sm_90 CTA may own this much shared memory, static and dynamic together (cudaDevAttrMaxSharedMemoryPerBlockOptin
+# of an H100).
+SMEM_PER_BLOCK_OPTIN = 232448
+RINGS = {          # knob prefix -> ring kernel
+    "CRO_TMA_READ": "hbm_read_tma_kernel",
+    "CRO_TMA_COPY": "hbm_copy_tma_kernel",
+    "CRO_FUSED": "hbm_copy_fused_kernel",
+}
+
+
+def largest_ring_tile(cro, monkeypatch, prefix, stages):
+    """Sets <prefix>_STAGES and the largest <prefix>_TILE the process-environment check accepts at that depth, and
+    returns that tile.  Bisection in 16-byte steps: the tile's own range is [1024, 114688]."""
+    monkeypatch.setenv(prefix + "_STAGES", str(stages))
+    lo, hi = 1024 // 16, 114688 // 16          # 1024-byte tiles fit at every depth
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        monkeypatch.setenv(prefix + "_TILE", str(16 * mid))
+        if cro.validate_env() == "":
+            lo = mid
+        else:
+            hi = mid - 1
+    monkeypatch.setenv(prefix + "_TILE", str(16 * lo))
+    return 16 * lo
+
+
+def ring_kernels_static_smem(cro):
+    """Static shared memory of each ring kernel in the built library, as cudaFuncGetAttributes().sharedSizeBytes
+    reports it.  cuobjdump's SHARED figure also counts the 1 KiB the system reserves per CTA, so that is taken off."""
+    import __graft_entry__ as g
+    nvcc = g._nvcc()
+    tool = os.path.join(os.path.dirname(nvcc), "cuobjdump") if os.path.dirname(nvcc) else shutil.which("cuobjdump")
+    out = subprocess.run([tool, "-res-usage", cro.LIB_PATH], capture_output=True, text=True, check=True).stdout
+    found, fn = {}, None
+    for line in out.splitlines():
+        m = re.match(r"\s*Function (\S+):", line)
+        if m:
+            fn = m.group(1)
+            continue
+        m = re.search(r"\bSHARED:(\d+)", line)
+        if m and fn:
+            for kernel in RINGS.values():
+                if kernel in fn:
+                    found[kernel] = int(m.group(1)) - 1024
+            fn = None
+    assert set(found) == set(RINGS.values()), out
+    return found
+
+
+def test_largest_legal_ring_fits_beside_the_kernels_static_shared_memory(cro, monkeypatch):
+    """Every ring cro_validate_env accepts must be one the device can launch: ring + the kernel's static shared memory
+    within what a CTA may own.  Otherwise a legal knob setting fails at plan time."""
+    static = ring_kernels_static_smem(cro)
+    for prefix, kernel in RINGS.items():
+        assert 0 < static[kernel] <= 2048, (kernel, static[kernel])
+        for stages in (2, 3, 4, 5, 8, 16):
+            tile = largest_ring_tile(cro, monkeypatch, prefix, stages)
+            assert tile * stages + static[kernel] <= SMEM_PER_BLOCK_OPTIN, (prefix, stages, tile, static[kernel])
+            if tile < 114688:                  # one step more is refused, with the tile knob's sentence
+                monkeypatch.setenv(prefix + "_TILE", str(tile + 16))
+                assert cro.validate_env() == "the env variable %s_TILE has an invalid value: '%d'" % (prefix, tile + 16)
+            monkeypatch.delenv(prefix + "_TILE")
+            monkeypatch.delenv(prefix + "_STAGES")

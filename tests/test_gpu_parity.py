@@ -506,10 +506,10 @@ def test_cli_helper_process(cro):
     print("cold vs warm:", cold)
 
 
-def test_c_harness_on_gpu(cro):
+def test_c_harness_runs_a_gpu_probe(cro, tmp_path):
     """The plain-C caller (what cgo compiles to) runs a probe + emit through the same ABI."""
     from test_abi import build_c_harness
-    out = subprocess.run([build_c_harness(), "gpu"], capture_output=True, text=True)
+    out = subprocess.run([build_c_harness(tmp_path), "gpu"], capture_output=True, text=True)
     assert out.returncode == 0, out.stdout + out.stderr
     assert "gpu ok: GPU-" in out.stdout and "cohdi.io/probe-status" in out.stdout
 
