@@ -168,7 +168,14 @@ EXPORTS = [
     "cro_local_node_op", "cro_scan_cmdline_for", "cro_token_from_reply",
     "cro_selftest_exception_barrier", "cro_probe_sweep_times", "cro_p2p_detail_get", "cro_fullbox_times",
     "cro_chase_end", "cro_validate_env", "cro_node_inventory", "cro_probe_uuid", "cro_set_latency_hops", "cro_local_exec", "cro_metrics_text", "cro_describe_wire_type",
+    "cro_selftest_probe_finalize", "cro_selftest_p2p_finalize", "cro_selftest_chase",
 ]
+
+# Slot map of a device's sweep-slot array (cro_sweep_slot, 64 bytes each); the cro_selftest_* hooks take such arrays.
+SLOT_FILL, SLOT_SWEEP0, MAX_SWEEPS_EACH, SLOT_EXPECT, SLOT_PREFIX, SLOT_P2P0 = 0, 1, 30, 62, 63, 64
+SLOT_SCRATCH = SLOT_P2P0 + 3 * MAX_DEVICES
+SLOT_COUNT = SLOT_SCRATCH + 4
+SLOT_BYTES = 64
 
 
 def _load() -> ctypes.CDLL:
@@ -242,6 +249,12 @@ def _load() -> ctypes.CDLL:
         "cro_fabric_list_devices": (i32, [c] + out),
         "cro_token_from_reply": (i32, [c] + out),
         "cro_selftest_exception_barrier": (i32, [i32]),
+        "cro_selftest_probe_finalize": (i32, [vp, i32, ctypes.POINTER(ProbeResult), vp, u64, u64, u64, u32, u32, u32, u32,
+                                              ctypes.POINTER(ProbeResult)]),
+        "cro_selftest_p2p_finalize": (i32, [vp, i32, ctypes.POINTER(ProbeResult), vp, ctypes.POINTER(vp), ctypes.POINTER(u64),
+                                            ctypes.POINTER(u64), ctypes.POINTER(u32), u32, u32, u32, u32, u32, u64, u64]),
+        "cro_selftest_chase": (i32, [vp, i32, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), u32, u32,
+                                     ctypes.POINTER(u64)]),
         "cro_local_node_op": (i32, [vp, c] + out),
         "cro_local_exec": (i32, [c] + out),
         "cro_describe_wire_type": (i32, [c] + out),
@@ -568,6 +581,44 @@ class ProbeContext:
         t = FullBoxTime()
         self._check(lib.cro_fullbox_times(self.handle, ctypes.byref(t)))
         return t
+
+    # ---- test hooks: the verdict kernels on crafted inputs (never used by the probe path) ----
+    def selftest_probe_finalize(self, dev: int, tmpl: bytes, slots: bytes, seed: int, nonce: int, sweep_bytes: int,
+                                read_sweeps: int, copy_sweeps: int, read_variant: int, copy_variant: int) -> bytes:
+        """probe_finalize_kernel over a 512-byte template and SLOT_COUNT packed slots; returns the 512 bytes it wrote."""
+        assert len(tmpl) == 512 and len(slots) == SLOT_COUNT * SLOT_BYTES
+        t, out = ProbeResult.from_buffer_copy(tmpl), ProbeResult()
+        sl = ctypes.create_string_buffer(slots, len(slots))
+        self._check(lib.cro_selftest_probe_finalize(self.handle, dev, ctypes.byref(t), sl, seed, nonce, sweep_bytes,
+                                                    read_sweeps, copy_sweeps, read_variant, copy_variant, ctypes.byref(out)))
+        return bytes(out)
+
+    def selftest_p2p_finalize(self, dev: int, result: bytes, slots: bytes, peer_slots: List[Optional[bytes]],
+                              peer_stamp: List[int], chase_out: List[int], chase_expect: List[int], n: int, self_index: int,
+                              hops: int, have_push: int, push_folded: int, p2p_bytes: int, stamp: int) -> bytes:
+        """p2p_finalize_kernel over a result struct, this device's slots and peer j's slots (None = no such peer);
+        returns the result struct it left."""
+        assert len(result) == 512 and len(slots) == SLOT_COUNT * SLOT_BYTES and len(peer_slots) <= MAX_DEVICES
+        r = ProbeResult.from_buffer_copy(result)
+        sl = ctypes.create_string_buffer(slots, len(slots))
+        keep = [ctypes.create_string_buffer(p, len(p)) if p is not None else None for p in peer_slots]
+        ps = (ctypes.c_void_p * MAX_DEVICES)(*[ctypes.cast(k, ctypes.c_void_p) if k is not None else None for k in keep])
+        st = (ctypes.c_uint64 * MAX_DEVICES)(*peer_stamp)
+        co = (ctypes.c_uint64 * (2 * MAX_DEVICES))(*chase_out)
+        ce = (ctypes.c_uint32 * MAX_DEVICES)(*chase_expect)
+        self._check(lib.cro_selftest_p2p_finalize(self.handle, dev, ctypes.byref(r), sl, ps, st, co, ce, n, self_index, hops,
+                                                  have_push, push_folded, p2p_bytes, stamp))
+        return bytes(r)
+
+    def selftest_chase(self, dev: int, pairs: List[Optional[Tuple[int, int]]], hops: int) -> List[int]:
+        """chase_kernel over tables built for (minor_src, minor_dst) pairs (None = a row without a table);
+        returns the 2 * len(pairs) output words."""
+        n = len(pairs)
+        src = (ctypes.c_int32 * n)(*[p[0] if p is not None else -1 for p in pairs])
+        dst = (ctypes.c_int32 * n)(*[p[1] if p is not None else -1 for p in pairs])
+        out = (ctypes.c_uint64 * (2 * n))()
+        self._check(lib.cro_selftest_chase(self.handle, dev, src, dst, n, hops, out))
+        return list(out)
 
 
 def node_inventory(proc_root: Optional[str], in_process: List[DevInfo]) -> List[DevInfo]:

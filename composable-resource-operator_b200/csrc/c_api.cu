@@ -99,6 +99,28 @@ int cro_selftest_exception_barrier(int kind) try {
     return CRO_OK;
 } CRO_API_CATCH
 
+int cro_selftest_probe_finalize(cro_ctx* ctx, int i, const cro_probe_result* tmpl, const cro_sweep_slot* slots, uint64_t seed,
+                                uint64_t nonce, uint64_t sweep_bytes, uint32_t read_sweeps, uint32_t copy_sweeps,
+                                uint32_t read_variant, uint32_t copy_variant, cro_probe_result* out) try {
+    if (!ctx) return CRO_ERR_INVALID_ARG;
+    ProbeParams pp{};
+    pp.seed = seed;
+    pp.nonce = nonce;
+    return ctx_selftest_probe_finalize(ctx, i, tmpl, slots, pp, sweep_bytes, read_sweeps, copy_sweeps, read_variant, copy_variant, out);
+} CRO_API_CATCH
+int cro_selftest_p2p_finalize(cro_ctx* ctx, int i, cro_probe_result* result, const cro_sweep_slot* slots,
+                              const cro_sweep_slot* const* peer_slots, const uint64_t* peer_stamp, const uint64_t* chase_out,
+                              const uint32_t* chase_expect, uint32_t n, uint32_t self, uint32_t hops, uint32_t have_push,
+                              uint32_t push_folded, uint64_t p2p_bytes, uint64_t stamp) try {
+    if (!ctx) return CRO_ERR_INVALID_ARG;
+    return ctx_selftest_p2p_finalize(ctx, i, result, slots, peer_slots, peer_stamp, chase_out, chase_expect, n, self, hops,
+                                     have_push, push_folded, p2p_bytes, stamp);
+} CRO_API_CATCH
+int cro_selftest_chase(cro_ctx* ctx, int i, const int32_t* minor_src, const int32_t* minor_dst, uint32_t n, uint32_t hops,
+                       uint64_t* out) try {
+    return ctx ? ctx_selftest_chase(ctx, i, minor_src, minor_dst, n, hops, out) : CRO_ERR_INVALID_ARG;
+} CRO_API_CATCH
+
 int cro_probe_init(const cro_opts* opts, cro_ctx** out) try { return ctx_create(opts, out); } CRO_API_CATCH
 void cro_probe_destroy(cro_ctx* ctx) { ctx_destroy(ctx); }
 

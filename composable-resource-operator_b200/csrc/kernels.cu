@@ -278,6 +278,29 @@ __device__ __forceinline__ void publish(unsigned long long x, unsigned long long
     }
 }
 
+// Epilogue of the sweeps that fold nothing (the fill, the plain copies): called by ONE thread per CTA once the CTA's
+// work is done; the last CTA to get here publishes the sweep's %globaltimer window, stamp and word count with a zero
+// checksum, and re-arms the ticket and the timers.
+__device__ __forceinline__ void publish_window(unsigned long long t_start, const SweepScratch sc, SweepOut* out,
+                                               const ProbeParams& imm, const ProbeParams* pp, unsigned long long n_words) {
+    atomicMin(sc.tmin, t_start);
+    atomicMax(sc.tmax, globaltimer_ns());
+    __threadfence();
+    const unsigned ticket = atomicAdd(sc.counter, 1u);
+    if (ticket == gridDim.x - 1) {
+        __threadfence();
+        out->x = 0; out->s = 0; out->w = 0;
+        out->t0 = *((volatile unsigned long long*)sc.tmin);
+        out->t1 = *((volatile unsigned long long*)sc.tmax);
+        out->stamp = pp ? pp->nonce : imm.nonce;
+        out->n_words = n_words;
+        *sc.counter = 0u;
+        *sc.tmin = ~0ull;
+        *sc.tmax = 0ull;
+        __threadfence();
+    }
+}
+
 // ---------------------------------------------------------------------------
 // hbm_fill: S bytes written.  Thread t of a tile stores vectors t, t+T, ...
 // so each warp-level store instruction covers 512 contiguous bytes.
@@ -315,24 +338,7 @@ hbm_fill_kernel(uint4* __restrict__ base, unsigned long long n_vec, const ProbeP
     }
     if (!out) return;
     __syncthreads();
-    if (threadIdx.x == 0) {
-        atomicMin(sc.tmin, t_start);
-        atomicMax(sc.tmax, globaltimer_ns());
-        __threadfence();
-        const unsigned ticket = atomicAdd(sc.counter, 1u);
-        if (ticket == gridDim.x - 1) {
-            __threadfence();
-            out->x = 0; out->s = 0; out->w = 0;
-            out->t0 = *((volatile unsigned long long*)sc.tmin);
-            out->t1 = *((volatile unsigned long long*)sc.tmax);
-            out->stamp = pp ? pp->nonce : imm.nonce;
-            out->n_words = 2 * n_vec;
-            *sc.counter = 0u;
-            *sc.tmin = ~0ull;
-            *sc.tmax = 0ull;
-            __threadfence();
-        }
-    }
+    if (threadIdx.x == 0) publish_window(t_start, sc, out, imm, pp, 2 * n_vec);
 }
 
 // ---------------------------------------------------------------------------
@@ -496,7 +502,10 @@ hbm_read_tma_kernel(const unsigned char* __restrict__ base, unsigned long long b
 template <int THREADS, int UNROLL>
 __global__ void __launch_bounds__(THREADS)
 hbm_copy_ldg_kernel(uint4* __restrict__ dst, const uint4* __restrict__ src,
-                    unsigned long long n_vec) {
+                    unsigned long long n_vec, const ProbeParams imm, const ProbeParams* __restrict__ pp,
+                    SweepScratch sc, SweepOut* out) {
+    unsigned long long t_start = 0;
+    if (threadIdx.x == 0) t_start = globaltimer_ns();
     const unsigned long long tile_vecs = (unsigned long long)THREADS * UNROLL;
     const unsigned long long n_tiles = n_vec / tile_vecs;
     for (unsigned long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -514,21 +523,27 @@ hbm_copy_ldg_kernel(uint4* __restrict__ dst, const uint4* __restrict__ src,
                                 threadIdx.x;
          i < n_vec; i += (unsigned long long)gridDim.x * THREADS)
         stg_stream(dst + i, ldg_stream(src + i));
+    if (!out) return;
+    __syncthreads();
+    if (threadIdx.x == 0) publish_window(t_start, sc, out, imm, pp, 2 * n_vec);
 }
 
 // ---------------------------------------------------------------------------
 // hbm_copy (TMA path): one thread per CTA drives everything.  Tiles go
 // global -> smem (bulk load, mbarrier) -> global (bulk store, bulk group);
-// data never touches the register file.  Moves bytes, checks nothing.
+// data never touches the register file.  Moves bytes, checks nothing; the
+// window it publishes ends once its last bulk store has completed.
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(32, 1)
 hbm_copy_tma_kernel(unsigned char* __restrict__ dst, const unsigned char* __restrict__ src,
                     unsigned long long bytes, unsigned tile_bytes, unsigned stages, unsigned chunk,
-                    unsigned long long* tile_ctr) {
+                    unsigned long long* tile_ctr, const ProbeParams imm, const ProbeParams* __restrict__ pp,
+                    SweepScratch sc, SweepOut* out) {
     extern __shared__ __align__(128) unsigned char ring[];
     __shared__ __align__(8) uint64_t full_bar[16];
     __shared__ unsigned long long tile_of[16];
     if (threadIdx.x != 0) return;
+    const unsigned long long t_start = globaltimer_ns();
     for (unsigned s = 0; s < stages; ++s) mbar_init(&full_bar[s], 1);
     mbar_fence_init();
     // bit 0: evict_first loads, bit 1: evict_first stores, bit 2: evict_last stores
@@ -591,6 +606,7 @@ hbm_copy_tma_kernel(unsigned char* __restrict__ dst, const unsigned char* __rest
         }
     }
     tma_wait_all();
+    if (out) publish_window(t_start, sc, out, imm, pp, bytes >> 3);
 }
 
 // ---------------------------------------------------------------------------
@@ -816,12 +832,13 @@ probe_finalize_kernel(const FinalizeArgs a) {
 
     unsigned long long tc[kMaxSweepsEach], tr[kMaxSweepsEach];
     unsigned verified = 0;
-    // copy sweep i reads what sweep i-1 wrote (sweep 0 reads the fill): its fold IS the check of that data
+    // every copy publishes its slot: a stale one did not run.  The checksumming copy i also folds what sweep i-1 wrote
+    // (sweep 0 reads the fill): its fold IS the check of that data.  A plain copy's data is checked by the next sweep.
     for (unsigned i = 0; i < C; ++i) {
         const SweepOut& s = sl[kSlotSweep0 + i];
         tc[i] = s.t1 - s.t0;
-        if (!a.fused) continue;
         if (s.stamp != nonce || s.n_words != n_words) fail(CRO_FAIL_STALE, 1 + i);
+        else if (!a.fused) continue;
         else if (!same_fold(s, E)) fail(CRO_FAIL_COPY_SRC, i);
         else if (i > 0) ++verified;            // sweep i-1's destination reproduced the pattern
     }
@@ -887,7 +904,8 @@ p2p_finalize_kernel(const P2PFinalizeArgs a) {
         }
         if (a.hops) {
             const unsigned long long end = a.chase_out[2 * j], ns = a.chase_out[2 * j + 1];
-            const unsigned long long x16 = ns * 16ull / a.hops;
+            // ns * 16 would wrap at 2^60 ns and up; such a chase saturates the 32-bit field anyway (hops < 2^32)
+            const unsigned long long x16 = ns > (~0ull >> 4) ? ~0ull : ns * 16ull / a.hops;
             r->p2p_latency_ns_x16[j] = (uint32_t)(x16 > 0xFFFFFFFFull ? 0xFFFFFFFFull : x16);
             if (end != a.chase_expect[j]) { fail(CRO_FAIL_P2P_CHASE, j); ok = false; }
         }
@@ -1064,14 +1082,14 @@ cudaError_t launch_copy(const KernelPlan& p, unsigned variant, void* dst, const 
         }
         hbm_copy_tma_kernel<<<clamp_grid(p.copy_tma.grid, bytes, p.copy_tile), p.copy_tma.block, p.copy_tma.smem, st>>>(
             static_cast<unsigned char*>(dst), static_cast<const unsigned char*>(src), bytes, p.copy_tile,
-            p.copy_stages, p.copy_chunk, ctr);
+            p.copy_stages, p.copy_chunk, ctr, pr.imm, pr.pp, sc, out);
         if (ctr) {
             cudaError_t e = cudaMemsetAsync(ctr, 0, sizeof(unsigned long long), st);   // leave it armed for the self-resetting kernels
             if (e != cudaSuccess) return e;
         }
     } else {
         hbm_copy_ldg_kernel<kCopyThreads, kCopyUnroll><<<clamp_grid(p.copy_ldg.grid, bytes, kCopyThreads * kCopyUnroll * 16), p.copy_ldg.block, 0, st>>>(
-            static_cast<uint4*>(dst), static_cast<const uint4*>(src), bytes >> 4);
+            static_cast<uint4*>(dst), static_cast<const uint4*>(src), bytes >> 4, pr.imm, pr.pp, sc, out);
     }
     return cudaGetLastError();
 }
@@ -1091,6 +1109,11 @@ cudaError_t launch_chase(const ChaseArgs& a, unsigned long long* out, cudaStream
     if (a.n == 0 || a.n > CRO_MAX_DEVICES) return cudaErrorInvalidValue;
     chase_kernel<<<1, 32 * a.n, 0, st>>>(a, out);
     return cudaGetLastError();
+}
+
+cudaError_t arm_chase_out(unsigned long long* out, cudaStream_t st) {
+    static_assert(kChaseArmed == ~0ull, "the armed word is all 0xFF bytes");
+    return cudaMemsetAsync(out, 0xFF, kChaseOutWords * sizeof(unsigned long long), st);
 }
 
 cudaError_t launch_finalize(const FinalizeArgs& a, cudaStream_t st) {

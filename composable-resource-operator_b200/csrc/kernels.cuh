@@ -6,6 +6,7 @@
 // are bit-exact against the CPU restatement the tests hold (see tests/).
 #pragma once
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 
 #include <string>
@@ -30,7 +31,10 @@ struct SweepOut {
     unsigned long long n_words; // words the sweep covered
     unsigned long long pad;
 };
-static_assert(sizeof(SweepOut) == 64, "SweepOut is one 64-byte slot");
+static_assert(sizeof(SweepOut) == 64 && sizeof(SweepOut) == sizeof(cro_sweep_slot), "SweepOut is one 64-byte slot");
+static_assert(offsetof(SweepOut, t0) == offsetof(cro_sweep_slot, t0) && offsetof(SweepOut, stamp) == offsetof(cro_sweep_slot, stamp) &&
+                  offsetof(SweepOut, n_words) == offsetof(cro_sweep_slot, n_words),
+              "SweepOut is the cro_sweep_slot of include/croprobe.h");
 
 // What a probe's kernels read from device memory instead of taking as launch
 // parameters, so that ONE captured CUDA graph serves every probe: the host
@@ -92,8 +96,9 @@ cudaError_t launch_fill(const KernelPlan&, void* base, uint64_t bytes, const Par
                         const SweepScratch&, SweepOut* out, cudaStream_t);
 cudaError_t launch_read(const KernelPlan&, unsigned variant, const void* base, uint64_t bytes,
                         const Params&, const SweepScratch&, SweepOut* out, cudaStream_t);
-// COPY_TMA_FUSED folds every tile it moves (checksum of the SOURCE stream as read) into *out;
-// the other variants leave *out alone (out may be null for them).
+// Every variant publishes *out when out is non-null: the %globaltimer window, the stamp and n_words = bytes / 8.
+// COPY_TMA_FUSED also folds every tile it moves (checksum of the SOURCE stream as read) into it and needs out; the
+// plain variants fold nothing and write a zero checksum, like the fill.
 cudaError_t launch_copy(const KernelPlan&, unsigned variant, void* dst, const void* src, uint64_t bytes,
                         const Params&, const SweepScratch&, SweepOut* out, cudaStream_t);
 cudaError_t launch_expected(const KernelPlan&, uint64_t bytes, const Params&,
@@ -109,16 +114,22 @@ struct ChaseArgs {
     unsigned hops;
 };
 cudaError_t launch_chase(const ChaseArgs& a, unsigned long long* out, cudaStream_t);
+// The chase output before the chase: every word all 0xFF bytes.  No chase ends there (a table has 65536 slots), so a
+// row the chase did not walk fails the end check at any hop count.
+constexpr unsigned long long kChaseArmed = ~0ull;
+constexpr size_t kChaseOutWords = 2 * CRO_MAX_DEVICES;
+cudaError_t arm_chase_out(unsigned long long* out, cudaStream_t);
 
-// Slot map of one device's SweepOut array (d_out).
-constexpr int kSlotFill = 0;
-constexpr int kSlotSweep0 = 1;              // copies first, then reads: 1 .. 1 + C + R
-constexpr int kMaxSweepsEach = 30;
-constexpr int kSlotExpect = 62;             // closed form of the whole region
-constexpr int kSlotPrefix = 63;             // closed form of the first p2p_bytes (what peers must read)
-constexpr int kSlotP2P0 = 64;               // per peer j: 64 + 3j + {0 read, 1 push, 2 receiver re-read}
-constexpr int kSlotScratch = 64 + 3 * CRO_MAX_DEVICES;   // single-sweep entry points
-constexpr int kSlotCount = kSlotScratch + 4;
+// Slot map of one device's SweepOut array (d_out): include/croprobe.h's, which the test hooks share.
+constexpr int kSlotFill = CRO_SLOT_FILL;
+constexpr int kSlotSweep0 = CRO_SLOT_SWEEP0;          // copies first, then reads: 1 .. 1 + C + R
+constexpr int kMaxSweepsEach = CRO_MAX_SWEEPS_EACH;
+constexpr int kSlotExpect = CRO_SLOT_EXPECT;          // closed form of the whole region
+constexpr int kSlotPrefix = CRO_SLOT_PREFIX;          // closed form of the first p2p_bytes (what peers must read)
+constexpr int kSlotP2P0 = CRO_SLOT_P2P0;              // per peer j: 64 + 3j + {0 read, 1 push, 2 receiver re-read}
+constexpr int kSlotScratch = CRO_SLOT_SCRATCH;        // single-sweep entry points
+constexpr int kSlotCount = CRO_SLOT_COUNT;
+static_assert(kSlotSweep0 + 2 * kMaxSweepsEach <= kSlotExpect && kSlotPrefix + 1 == kSlotP2P0, "slot map");
 
 // The probe's verdict, computed on the device: fills *out (the all-gather send buffer) from the template
 // (identity, staged at init), the sweep slots and the closed form.  One CTA.
@@ -132,6 +143,24 @@ struct FinalizeArgs {
     unsigned read_variant, copy_variant;
     unsigned fused;          // copy sweeps carry a checksum of their source stream
 };
+// The arguments of one probe's finalize: `cv` is the resolved copy variant, C the copy sweeps actually run (a probe
+// without copies reports copy variant 0).
+inline FinalizeArgs finalize_args(const cro_probe_result* tmpl, cro_probe_result* out, const SweepOut* slots,
+                                  const ProbeParams* pp, unsigned long long sweep_bytes, unsigned R, unsigned C,
+                                  unsigned rv, unsigned cv) {
+    FinalizeArgs fa{};
+    fa.tmpl = tmpl;
+    fa.out = out;
+    fa.slots = slots;
+    fa.pp = pp;
+    fa.sweep_bytes = sweep_bytes;
+    fa.read_sweeps = R;
+    fa.copy_sweeps = C;
+    fa.read_variant = rv;
+    fa.copy_variant = C ? cv : 0;
+    fa.fused = (cv == COPY_TMA_FUSED) ? 1u : 0u;
+    return fa;
+}
 cudaError_t launch_finalize(const FinalizeArgs& a, cudaStream_t);
 
 // NVLink part of the verdict: folds the per-peer slots of this device (and the peers' slots it must agree with)

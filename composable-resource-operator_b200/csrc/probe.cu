@@ -572,6 +572,7 @@ int ctx_copy(cro_ctx* c, int idx, uint32_t variant, uint32_t iters, cro_sweep_re
     out->bytes = 2 * d->sweep_bytes * iters;
     out->ns = ms_to_ns(ms);
     if (variant == COPY_TMA_FUSED) slot_to_result(d->h_out[kSlotScratch], out);   // checksum of the source as read
+    else out->timer_ns = d->h_out[kSlotScratch].t1 - d->h_out[kSlotScratch].t0;   // the plain copies fold nothing
     out->variant = variant;
     out->launches = iters;
     return CRO_OK;
@@ -713,18 +714,7 @@ static int probe_enqueue(cro_ctx* c, Device* d, Lane& L) {
             if (maybe_inject()) return CRO_ERR_CUDA;
         }
         if (overlap) CU_TRY(c, cudaStreamWaitEvent(d->stream, d->ev_join, 0));
-        FinalizeArgs fa{};
-        fa.tmpl = d->d_tmpl;
-        fa.out = L.d_result;
-        fa.slots = L.d_out;
-        fa.pp = L.d_params;
-        fa.sweep_bytes = d->sweep_bytes;
-        fa.read_sweeps = R;
-        fa.copy_sweeps = C;
-        fa.read_variant = rv;
-        fa.copy_variant = C ? cv : 0;
-        fa.fused = (cv == COPY_TMA_FUSED) ? 1u : 0u;
-        CU_TRY(c, launch_finalize(fa, d->stream));
+        CU_TRY(c, launch_finalize(finalize_args(d->d_tmpl, L.d_result, L.d_out, L.d_params, d->sweep_bytes, R, C, rv, cv), d->stream));
         CU_TRY(c, cudaMemcpyAsync(L.h_result, L.d_result, sizeof(cro_probe_result), cudaMemcpyDeviceToHost, d->stream));
         CU_TRY(c, cudaMemcpyAsync(L.h_out, L.d_out, sizeof(SweepOut) * 64, cudaMemcpyDeviceToHost, d->stream));
         return CRO_OK;
@@ -1229,6 +1219,18 @@ int enable_peers(cro_ctx* c) {
     return CRO_OK;
 }
 
+// One latency table on the current device: permutation `perm` with slot i at table[i*16], the head of its own
+// 128-byte line.
+int upload_chase_table(cro_ctx* c, const std::vector<uint32_t>& perm, unsigned long long** table) {
+    std::vector<unsigned long long> wide(perm.begin(), perm.end());
+    CU_TRY(c, cudaMalloc(table, (size_t)kChaseSlots * 128));
+    CU_TRY(c, cudaMemset(*table, 0, (size_t)kChaseSlots * 128));
+    CU_TRY(c, cudaMemcpy2D(*table, 128, wide.data(), 8, 8, kChaseSlots, cudaMemcpyHostToDevice));
+    // the chase runs on a non-blocking stream, which does not wait for the legacy stream these copies went to
+    CU_TRY(c, cudaStreamSynchronize(0));
+    return CRO_OK;
+}
+
 // Latency permutations: device b holds, for every other device a, the Sattolo cycle a will chase through b's
 // memory (slot i lives at table[i*16], one per 128-byte line), and a remembers where `hops` steps must end.
 int ensure_chase(cro_ctx* c, uint32_t hops) {
@@ -1238,7 +1240,6 @@ int ensure_chase(cro_ctx* c, uint32_t hops) {
     if (built) return CRO_OK;
     Range nv(c, "cro.chase.build");
     std::vector<uint32_t> perm;
-    std::vector<unsigned long long> wide(kChaseSlots);
     for (int b = 0; b < n; ++b) {
         Device* owner = c->devs[(size_t)b].get();
         CU_TRY(c, cudaSetDevice(owner->ordinal));
@@ -1250,11 +1251,8 @@ int ensure_chase(cro_ctx* c, uint32_t hops) {
             const int mb = owner->info.device_minor >= 0 ? owner->info.device_minor : owner->ordinal;
             chase_permutation(ma, mb, &perm);
             if (!owner->d_chase_tables[(size_t)a]) {
-                CU_TRY(c, cudaMalloc(&owner->d_chase_tables[(size_t)a], (size_t)kChaseSlots * 128));
-                CU_TRY(c, cudaMemset(owner->d_chase_tables[(size_t)a], 0, (size_t)kChaseSlots * 128));
-                for (uint32_t i = 0; i < kChaseSlots; ++i) wide[i] = perm[i];
-                // scatter: 8 bytes into the head of every 128-byte line
-                CU_TRY(c, cudaMemcpy2D(owner->d_chase_tables[(size_t)a], 128, wide.data(), 8, 8, kChaseSlots, cudaMemcpyHostToDevice));
+                const int rc = upload_chase_table(c, perm, &owner->d_chase_tables[(size_t)a]);
+                if (rc) return rc;
             }
             if ((int)chaser->chase_expect.size() != n) chaser->chase_expect.assign((size_t)n, 0u);
             uint32_t at = 0;
@@ -1471,7 +1469,7 @@ int ctx_probe_all(cro_ctx* c, cro_probe_result* out, int cap, int* n_out) {
                 CU_TRY(c, cudaStreamWaitEvent(d->stream, c->devs[(size_t)j]->ev_chase_ready, 0));
                 ca.table[j] = c->devs[(size_t)j]->d_chase_tables[(size_t)i];
             }
-            CU_TRY(c, cudaMemsetAsync(d->d_chase_out, 0, 2 * CRO_MAX_DEVICES * sizeof(unsigned long long), d->stream));
+            CU_TRY(c, arm_chase_out(d->d_chase_out, d->stream));   // a row the chase does not walk cannot pass
             CU_TRY(c, launch_chase(ca, d->d_chase_out, d->stream));
             c->launches++;
             P2PFinalizeArgs pa{};
@@ -1601,7 +1599,8 @@ int ctx_probe_all(cro_ctx* c, cro_probe_result* out, int cap, int* n_out) {
                     lo = std::min(lo, s.t0);
                     hi = std::max(hi, s.t1);
                 }
-                c->fullbox.chase_ns = std::max<uint64_t>(c->fullbox.chase_ns, d->h_chase_out[2 * j + 1]);
+                if (pair_ok(i, j))      // the rows of peers it cannot reach keep the armed value
+                    c->fullbox.chase_ns = std::max<uint64_t>(c->fullbox.chase_ns, d->h_chase_out[2 * j + 1]);
             }
             if (hi > lo) c->fullbox.p2p_ns = std::max<uint64_t>(c->fullbox.p2p_ns, hi - lo);
         }
@@ -1643,6 +1642,124 @@ int ctx_p2p_detail(cro_ctx* c, int idx, int peer, cro_p2p_detail* out) {
     out->chase_expect = (size_t)peer < d->chase_expect.size() ? d->chase_expect[(size_t)peer] : 0;
     out->hops = c->opts.latency_hops;
     out->access = idx < 8 && peer < 8 ? d->tmpl.p2p_access[peer] : 0;
+    return CRO_OK;
+}
+
+// ---------------------------------------------------------------------------
+// test hooks: the verdict kernels on caller-given inputs (include/croprobe.h)
+// ---------------------------------------------------------------------------
+namespace {
+// One device allocation for everything a hook stages, freed on every way out.
+struct HookBuffer {
+    void* p = nullptr;
+    ~HookBuffer() { cudaFree(p); }
+};
+}  // namespace
+
+int ctx_selftest_probe_finalize(cro_ctx* c, int idx, const cro_probe_result* tmpl, const cro_sweep_slot* slots,
+                                const ProbeParams& pp, uint64_t sweep_bytes, uint32_t R, uint32_t C, uint32_t rv,
+                                uint32_t cv, cro_probe_result* out) {
+    Device* d = dev_at(c, idx);
+    if (!d || !tmpl || !slots || !out || R > (uint32_t)kMaxSweepsEach || C > (uint32_t)kMaxSweepsEach)
+        return CRO_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> g(d->mu);
+    drain_pending(c, d);
+    CU_TRY(c, cudaSetDevice(d->ordinal));
+    // [template | result | params | slots]
+    constexpr size_t kRes = sizeof(cro_probe_result), kPar = 64, kSlots = sizeof(SweepOut) * kSlotCount;
+    std::vector<unsigned char> h(2 * kRes + kPar + kSlots, 0);
+    memcpy(h.data(), tmpl, kRes);
+    memcpy(h.data() + 2 * kRes, &pp, sizeof pp);
+    memcpy(h.data() + 2 * kRes + kPar, slots, kSlots);
+    HookBuffer b;
+    CU_TRY(c, cudaMalloc(&b.p, h.size()));
+    unsigned char* base = static_cast<unsigned char*>(b.p);
+    CU_TRY(c, cudaMemcpyAsync(base, h.data(), h.size(), cudaMemcpyHostToDevice, d->stream));
+    CU_TRY(c, launch_finalize(finalize_args(reinterpret_cast<const cro_probe_result*>(base), reinterpret_cast<cro_probe_result*>(base + kRes),
+                                            reinterpret_cast<const SweepOut*>(base + 2 * kRes + kPar),
+                                            reinterpret_cast<const ProbeParams*>(base + 2 * kRes), sweep_bytes, R, C, rv, cv),
+                              d->stream));
+    CU_TRY(c, cudaMemcpyAsync(h.data(), base + kRes, kRes, cudaMemcpyDeviceToHost, d->stream));
+    CU_TRY(c, cudaStreamSynchronize(d->stream));
+    memcpy(out, h.data(), kRes);
+    return CRO_OK;
+}
+
+int ctx_selftest_p2p_finalize(cro_ctx* c, int idx, cro_probe_result* result, const cro_sweep_slot* slots,
+                              const cro_sweep_slot* const* peer_slots, const uint64_t* peer_stamp, const uint64_t* chase_out,
+                              const uint32_t* chase_expect, uint32_t n, uint32_t self, uint32_t hops, uint32_t have_push,
+                              uint32_t push_folded, uint64_t p2p_bytes, uint64_t stamp) {
+    Device* d = dev_at(c, idx);
+    if (!d || !result || !slots || !peer_slots || !peer_stamp || !chase_out || !chase_expect || n > CRO_MAX_DEVICES || self >= n)
+        return CRO_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> g(d->mu);
+    drain_pending(c, d);
+    CU_TRY(c, cudaSetDevice(d->ordinal));
+    // [result | chase output | this device's slots | peer j's slots, for each j]
+    constexpr size_t kRes = sizeof(cro_probe_result), kChase = kChaseOutWords * sizeof(unsigned long long);
+    constexpr size_t kSlots = sizeof(SweepOut) * kSlotCount;
+    std::vector<unsigned char> h(kRes + kChase + (1 + CRO_MAX_DEVICES) * kSlots, 0);
+    memcpy(h.data(), result, kRes);
+    memcpy(h.data() + kRes, chase_out, kChase);
+    memcpy(h.data() + kRes + kChase, slots, kSlots);
+    for (int j = 0; j < CRO_MAX_DEVICES; ++j)
+        if (peer_slots[j]) memcpy(h.data() + kRes + kChase + (size_t)(1 + j) * kSlots, peer_slots[j], kSlots);
+    HookBuffer b;
+    CU_TRY(c, cudaMalloc(&b.p, h.size()));
+    unsigned char* base = static_cast<unsigned char*>(b.p);
+    CU_TRY(c, cudaMemcpyAsync(base, h.data(), h.size(), cudaMemcpyHostToDevice, d->stream));
+    P2PFinalizeArgs pa{};
+    pa.out = reinterpret_cast<cro_probe_result*>(base);
+    pa.chase_out = reinterpret_cast<const unsigned long long*>(base + kRes);
+    pa.slots = reinterpret_cast<const SweepOut*>(base + kRes + kChase);
+    for (int j = 0; j < CRO_MAX_DEVICES; ++j) {
+        if (peer_slots[j]) pa.peer_slots[j] = reinterpret_cast<const SweepOut*>(base + kRes + kChase + (size_t)(1 + j) * kSlots);
+        pa.peer_stamp[j] = peer_stamp[j];
+        pa.chase_expect[j] = chase_expect[j];
+    }
+    pa.n = n;
+    pa.self = self;
+    pa.hops = hops;
+    pa.have_push = have_push;
+    pa.push_folded = push_folded;
+    pa.p2p_bytes = p2p_bytes;
+    pa.stamp = stamp;
+    CU_TRY(c, launch_p2p_finalize(pa, d->stream));
+    CU_TRY(c, cudaMemcpyAsync(h.data(), base, kRes, cudaMemcpyDeviceToHost, d->stream));
+    CU_TRY(c, cudaStreamSynchronize(d->stream));
+    memcpy(result, h.data(), kRes);
+    return CRO_OK;
+}
+
+int ctx_selftest_chase(cro_ctx* c, int idx, const int32_t* minor_src, const int32_t* minor_dst, uint32_t n, uint32_t hops,
+                       uint64_t* out) {
+    Device* d = dev_at(c, idx);
+    if (!d || !minor_src || !minor_dst || !out || n == 0 || n > CRO_MAX_DEVICES) return CRO_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> g(d->mu);
+    drain_pending(c, d);
+    CU_TRY(c, cudaSetDevice(d->ordinal));
+    struct Tables {
+        unsigned long long* t[CRO_MAX_DEVICES] = {};
+        ~Tables() { for (unsigned long long* p : t) cudaFree(p); }
+    } tables;
+    HookBuffer b;
+    CU_TRY(c, cudaMalloc(&b.p, kChaseOutWords * sizeof(unsigned long long)));
+    ChaseArgs ca{};
+    ca.n = n;
+    ca.hops = hops;
+    std::vector<uint32_t> perm;
+    for (uint32_t j = 0; j < n; ++j) {
+        if (minor_src[j] < 0) continue;      // a null row: no table, the warp walks nothing
+        chase_permutation(minor_src[j], minor_dst[j], &perm);
+        const int rc = upload_chase_table(c, perm, &tables.t[j]);
+        if (rc) return rc;
+        ca.table[j] = tables.t[j];
+    }
+    unsigned long long* dout = static_cast<unsigned long long*>(b.p);
+    CU_TRY(c, arm_chase_out(dout, d->stream));
+    CU_TRY(c, launch_chase(ca, dout, d->stream));
+    CU_TRY(c, cudaMemcpyAsync(out, dout, 2 * (size_t)n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, d->stream));
+    CU_TRY(c, cudaStreamSynchronize(d->stream));
     return CRO_OK;
 }
 

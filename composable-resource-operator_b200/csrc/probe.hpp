@@ -192,6 +192,17 @@ int ctx_expected(cro_ctx* c, int idx, cro_sweep_result* out);
 int ctx_inject(cro_ctx* c, int idx, uint64_t word, uint64_t mask);
 int ctx_read_words(cro_ctx* c, int idx, uint64_t first, uint64_t n, uint64_t* out);
 
+// test hooks (include/croprobe.h, cro_selftest_*): the verdict kernels and the chase on caller-given inputs
+int ctx_selftest_probe_finalize(cro_ctx* c, int idx, const cro_probe_result* tmpl, const cro_sweep_slot* slots,
+                                const ProbeParams& pp, uint64_t sweep_bytes, uint32_t R, uint32_t C, uint32_t rv,
+                                uint32_t cv, cro_probe_result* out);
+int ctx_selftest_p2p_finalize(cro_ctx* c, int idx, cro_probe_result* result, const cro_sweep_slot* slots,
+                              const cro_sweep_slot* const* peer_slots, const uint64_t* peer_stamp, const uint64_t* chase_out,
+                              const uint32_t* chase_expect, uint32_t n, uint32_t self, uint32_t hops, uint32_t have_push,
+                              uint32_t push_folded, uint64_t p2p_bytes, uint64_t stamp);
+int ctx_selftest_chase(cro_ctx* c, int idx, const int32_t* minor_src, const int32_t* minor_dst, uint32_t n, uint32_t hops,
+                       uint64_t* out);
+
 // CRO_READ_AUTO / CRO_COPY_AUTO resolved with a context's knobs (CRO_READ_VARIANT, CRO_COPY_VARIANT).
 uint32_t resolve_read_variant(uint32_t v, uint64_t bytes, const env::Values& knobs);
 uint32_t resolve_copy_variant(uint32_t v, const env::Values& knobs);

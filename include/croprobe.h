@@ -152,7 +152,8 @@ typedef struct cro_probe_result {
     uint64_t sweep_bytes;          /*  96 */
     uint64_t seed;                 /* 104  effective pattern seed of THIS probe:
                                            (seed_base | minor) + nonce * 0xD1B54A32D192ED03 */
-    uint64_t checksum_xor;         /* 112  of the first read sweep (or of the sweep that failed) */
+    uint64_t checksum_xor;         /* 112  of read sweep 0 — or, when the first check that failed is a read sweep's
+                                           (stale or wrong), of that read sweep */
     uint64_t checksum_sum;         /* 120 */
     uint64_t fill_ns;              /* 128  sweep times: %globaltimer, first CTA start .. last CTA end */
     uint64_t read_best_ns;         /* 136 */
@@ -166,7 +167,7 @@ typedef struct cro_probe_result {
                                            cro_probe_all and after any failed probe */
     uint64_t p2p_read_ns[8];       /* 184  time to read p2p_bytes out of peer j's HBM over NVLink */
     uint64_t p2p_checksum_xor[8];  /* 248 */
-    uint32_t p2p_latency_ns_x16[8];/* 312  mean hop latency x16 (fixed point)        */
+    uint32_t p2p_latency_ns_x16[8];/* 312  mean hop latency x16 (fixed point): min(chase ns * 16 / hops, 2^32 - 1) */
     uint8_t  p2p_access[8];        /* 344  cudaDeviceCanAccessPeer                   */
     uint64_t p2p_bytes;            /* 352 */
     uint64_t expect_xor;           /* 360  closed-form checksum computed on the device
@@ -174,10 +175,12 @@ typedef struct cro_probe_result {
     uint64_t expect_sum;           /* 368 */
     uint64_t expect_wsum;          /* 376 */
     uint64_t checksum_wsum;        /* 384 */
-    uint64_t copy_checksum_xor;    /* 392  checksum of the LAST copy's destination (read back by the first read sweep) */
+    uint64_t copy_checksum_xor;    /* 392  checksum of the LAST copy's destination (read back by the first read sweep);
+                                           written only when the probe ran copy and read sweeps */
     uint64_t copy_checksum_sum;    /* 400 */
     uint64_t copy_checksum_wsum;   /* 408 */
-    uint64_t total_ns;             /* 416  first CTA of the fill .. last CTA of the last sweep */
+    uint64_t total_ns;             /* 416  first CTA of the fill .. last CTA of any sweep (the latest t1 of the fill, copy
+                                           and read slots, minus the fill's t0, modulo 2^64) */
     uint64_t p2p_write_ns[8];      /* 424  time to PUSH p2p_bytes into peer j's scratch half
                                            (posted NVLink writes; the peer re-reads and checks them) */
     uint32_t nonce;                /* 488  probe number on this device (0 = first probe of the context) */
@@ -188,9 +191,15 @@ typedef struct cro_probe_result {
     uint8_t  read_sweeps;          /* 496 */
     uint8_t  copy_sweeps;          /* 497 */
     uint8_t  copy_verified;        /* 498  copy sweeps whose destination was re-read and matched the closed form
-                                           (sweep k+1 folds what sweep k wrote; the first read sweep folds the last) */
-    uint8_t  fail_code;            /* 499  CRO_FAIL_*: which check failed first (0 = none) */
-    uint8_t  fail_index;           /* 500  sweep number / peer index of that check */
+                                           (sweep k+1 folds what sweep k wrote; the first read sweep folds the last).
+                                           Counted per passing check, also after an earlier failure: every checksumming
+                                           copy k >= 1 that passed, plus read sweep 0 if it passed and copies ran */
+    uint8_t  fail_code;            /* 499  CRO_FAIL_*: which check failed first (0 = none), in the order: closed form,
+                                           fill stamp, each copy sweep (stamp, then fold when it checksums), each read
+                                           sweep (stamp, then fold); p2p_finalize adds its peer checks after all of them */
+    uint8_t  fail_index;           /* 500  CRO_FAIL_STALE: the sweep's number in launch order (0 fill, 1.. copies, then
+                                           reads); CRO_FAIL_COPY_SRC / CRO_FAIL_READ: the copy / read sweep's own index;
+                                           CRO_FAIL_EXPECT: 0, or the peer whose prefix slot is stale; peer checks: the peer */
     uint8_t  p2p_ok;               /* 501  bit j: NVLink read of, push into and chase through peer j all verified */
     uint8_t  reserved8[2];         /* 502 */
     uint64_t t_start_ns;           /* 504  %globaltimer when the probe's first CTA started */
@@ -641,6 +650,50 @@ int  cro_last_error(cro_ctx *ctx, char *buf, size_t cap);
  * barrier made of it; any other kind returns CRO_OK without throwing. */
 int  cro_selftest_exception_barrier(int kind);
 const char *cro_version(void);
+
+/* ---- test hooks: the verdict kernels on caller-given inputs ---------------- */
+/* Test-only: nothing on the probe path calls these.  Each takes the device's mutex, lets any probe still in flight on
+ * it finish first, runs one kernel on buffers of its own (never a probe's slots or result struct) and frees them before
+ * returning. */
+
+/* One sweep's result slot as the kernels write it into a device's slot array: 64 bytes. */
+typedef struct cro_sweep_slot {
+    uint64_t x, s, w;              /* checksum triple of what the sweep folded (zero for the fill and the plain copies) */
+    uint64_t t0, t1;               /* %globaltimer window: first CTA start, last CTA end                                */
+    uint64_t stamp;                /* nonce of the probe whose kernel wrote the slot                                     */
+    uint64_t n_words;              /* 64-bit words the sweep covered                                                     */
+    uint64_t pad;
+} cro_sweep_slot;
+
+/* Slot map of one device's slot array. */
+#define CRO_SLOT_FILL           0
+#define CRO_SLOT_SWEEP0         1   /* copy sweeps first, then read sweeps: 1 .. 1 + C + R                   */
+#define CRO_MAX_SWEEPS_EACH    30   /* at most this many copy sweeps and this many read sweeps               */
+#define CRO_SLOT_EXPECT        62   /* closed form of the whole region                                       */
+#define CRO_SLOT_PREFIX        63   /* closed form of the first p2p_bytes (what the peers must read)         */
+#define CRO_SLOT_P2P0          64   /* per peer j: 64 + 3j + {0 read of j, 1 push into j, 2 re-read of j's push} */
+#define CRO_SLOT_SCRATCH       (CRO_SLOT_P2P0 + 3 * CRO_MAX_DEVICES)   /* the single-sweep entry points       */
+#define CRO_SLOT_COUNT         (CRO_SLOT_SCRATCH + 4)
+
+/* Runs probe_finalize_kernel on device dev_index over tmpl (the identity template), slots[CRO_SLOT_COUNT] and the probe
+ * parameters given, and writes the 512 bytes it produced to *out.  copy_variant is the resolved CRO_COPY_* of the copy
+ * sweeps; read_sweeps and copy_sweeps are at most CRO_MAX_SWEEPS_EACH. */
+int  cro_selftest_probe_finalize(cro_ctx *ctx, int dev_index, const cro_probe_result *tmpl, const cro_sweep_slot *slots,
+                                 uint64_t seed, uint64_t nonce, uint64_t sweep_bytes, uint32_t read_sweeps,
+                                 uint32_t copy_sweeps, uint32_t read_variant, uint32_t copy_variant, cro_probe_result *out);
+/* Runs p2p_finalize_kernel on device dev_index: *result (what probe_finalize wrote) is updated in place.
+ * slots[CRO_SLOT_COUNT] is this device's slot array; peer_slots[j] points at peer j's (CRO_SLOT_COUNT slots) or is NULL
+ * for no such peer; peer_stamp, chase_expect: CRO_MAX_DEVICES entries; chase_out: 2 * CRO_MAX_DEVICES words
+ * ([2j] end slot, [2j+1] ns).  n <= CRO_MAX_DEVICES, self < n. */
+int  cro_selftest_p2p_finalize(cro_ctx *ctx, int dev_index, cro_probe_result *result, const cro_sweep_slot *slots,
+                               const cro_sweep_slot *const *peer_slots, const uint64_t *peer_stamp,
+                               const uint64_t *chase_out, const uint32_t *chase_expect, uint32_t n, uint32_t self,
+                               uint32_t hops, uint32_t have_push, uint32_t push_folded, uint64_t p2p_bytes, uint64_t stamp);
+/* Builds, on device dev_index, the latency permutation of the directed pair (minor_src[j], minor_dst[j]) for each of
+ * n <= CRO_MAX_DEVICES rows (a row with minor_src[j] < 0 gets no table), arms the chase output as the probe does, runs
+ * chase_kernel for `hops` hops and copies the 2 * n output words to out ([2j] end slot, [2j+1] ns). */
+int  cro_selftest_chase(cro_ctx *ctx, int dev_index, const int32_t *minor_src, const int32_t *minor_dst, uint32_t n,
+                        uint32_t hops, uint64_t *out);
 
 #ifdef __cplusplus
 }

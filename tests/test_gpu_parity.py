@@ -165,30 +165,63 @@ def test_probe_result_fields(cro, coracle, ctx_small):
     assert r.total_ns >= r.fill_ns + 3 * r.read_best_ns + 2 * r.copy_best_ns
 
 
+RAGGED = (3 << 20) + 16 * 7
+
+
 def test_device_written_struct_equals_host_assembly(cro, coracle, ctx_small):
     """The 512-byte struct is written by the finalize kernel.  Rebuild it on the host from the same raw material —
     identity from the enumeration, checksums from the oracle, times from the per-sweep %globaltimer windows — and
     compare field by field; the CUDA-event times of the same sweeps must agree with the device's own timers."""
-    r = ctx_small.probe_device(0)
-    d = ctx_small.own_devices()[0]
-    times = ctx_small.sweep_times(0)
-    assert [t.kind for t in times] == [0] + [1] * r.copy_sweeps + [2] * r.read_sweeps
-    want = coracle.checksum(r.seed, 0, r.sweep_bytes // 8)
+    assert_struct_equals_host_assembly(cro, coracle, ctx_small, 0, 0, 2, 3, 64 << 20)
+
+
+# (read variant, copy variant, copy sweeps (0: CRO_F_SKIP_COPY), read sweeps, S): every read x copy variant pair, and
+# the shapes without copies, with one of each and with the most of each
+@pytest.mark.parametrize("rv,cv,C,R,S", [(rv, cv, 2, 3, RAGGED) for rv in VARIANTS for cv in COPY_VARIANTS] +
+                         [(0, 0, 0, 2, RAGGED), (1, 3, 1, 1, RAGGED), (2, 1, 30, 30, RAGGED)])
+def test_device_written_struct_equals_host_assembly_at_every_variant_and_shape(cro, coracle, rv, cv, C, R, S):
+    """The same field-by-field comparison for the plain copies (whose sweeps publish their own timer windows too),
+    every read variant, and the probe shapes at the edges of the slot map."""
+    flags = cro.F_SKIP_COPY if C == 0 else 0
+    with cro.ProbeContext(sweep_bytes=S, devices=[0], flags=flags, read_sweeps=R, copy_sweeps=C or 1, read_variant=rv,
+                          copy_variant=cv) as c:
+        assert_struct_equals_host_assembly(cro, coracle, c, rv, cv, C, R, S)
+
+
+def assert_struct_equals_host_assembly(cro, coracle, c, rv, cv, C, R, S):
+    """One probe on context c (read / copy variants rv / cv as asked, 0 = automatic; C copy and R read sweeps; S bytes),
+    its struct compared with the host's assembly of the same probe."""
+    r = c.probe_device(0)
+    d = c.own_devices()[0]
+    times = c.sweep_times(0)
+    assert [t.kind for t in times] == [0] + [1] * C + [2] * R
+    want = coracle.checksum(r.seed, 0, S // 8)
     reads = sorted(t.timer_ns for t in times if t.kind == 2)
     copies = sorted(t.timer_ns for t in times if t.kind == 1)
+    cv_used = cv or cro.COPY_TMA_FUSED
     host = {
         "abi_version": 2, "status": 0, "cuda_ordinal": d.cuda_ordinal, "device_minor": d.device_minor,
         "gpu_uuid": d.gpu_uuid, "pci_bus_id": d.pci_bus_id, "hbm_bytes_total": d.hbm_bytes_total,
-        "sweep_bytes": 64 << 20, "checksum_xor": want[0], "checksum_sum": want[1], "checksum_wsum": want[2],
+        "sweep_bytes": S, "checksum_xor": want[0], "checksum_sum": want[1], "checksum_wsum": want[2],
         "expect_xor": want[0], "expect_sum": want[1], "expect_wsum": want[2],
-        "copy_checksum_xor": want[0], "copy_checksum_sum": want[1], "copy_checksum_wsum": want[2],
+        "copy_checksum_xor": want[0] if C else 0, "copy_checksum_sum": want[1] if C else 0,
+        "copy_checksum_wsum": want[2] if C else 0,
         "fill_ns": times[0].timer_ns, "read_best_ns": reads[0], "read_median_ns": reads[len(reads) // 2],
-        "copy_best_ns": copies[0], "copy_median_ns": copies[len(copies) // 2],
-        "sm_count": d.sm_count, "read_sweeps": 3, "copy_sweeps": 2, "copy_verified": 2, "fail_code": 0, "fail_index": 0,
-        "rank": 0, "world": 1, "read_variant": cro.READ_LDG, "copy_variant": cro.COPY_TMA_FUSED, "p2p_ok": 0,
+        "copy_best_ns": copies[0] if C else 0, "copy_median_ns": copies[len(copies) // 2] if C else 0,
+        "sm_count": d.sm_count, "read_sweeps": R, "copy_sweeps": C, "fail_code": 0, "fail_index": 0,
+        # the checksumming copy k >= 1 verifies copy k-1's destination; read sweep 0 verifies the last copy's
+        "copy_verified": (C if cv_used == cro.COPY_TMA_FUSED else 1) if C else 0,
+        "rank": 0, "world": 1, "read_variant": rv or cro.READ_LDG, "copy_variant": cv_used if C else 0, "p2p_ok": 0,
     }
-    for k, v in host.items():
-        assert getattr(r, k) == v, (k, getattr(r, k), v)
+    bad = {k: (getattr(r, k), v) for k, v in host.items() if getattr(r, k) != v}
+    # the fill's first CTA .. the last sweep's last CTA: at least every sweep's own window (they run one after the
+    # other on one stream), at most the events around all of them
+    lo, hi = sum(t.timer_ns for t in times), sum(t.event_ns for t in times) * 1.02 + 2000
+    if not lo <= r.total_ns <= hi:
+        bad["total_ns"] = (r.total_ns, (lo, hi))
+    # every sweep publishes its own %globaltimer window
+    bad.update({"timer_ns of sweep (%d, %d)" % (t.kind, t.index): (t.timer_ns, "> 0") for t in times if t.timer_ns == 0})
+    assert not bad, bad
     assert list(r.p2p_read_ns) == [0] * 8 and list(r.p2p_write_ns) == [0] * 8
     for t in times:       # the two clocks watch the same kernels: events add launch latency, never lose time
         assert t.timer_ns <= t.event_ns * 1.02 + 2000 and t.event_ns <= t.timer_ns * 1.25 + 20000, (t.kind, t.index, t.timer_ns, t.event_ns)
@@ -669,22 +702,41 @@ def test_metrics_text_is_prometheus_exposition(cro):
         assert all(k.split("{")[0] in families for k in vals)      # every sample belongs to a declared family
 
 
-@pytest.mark.parametrize("after,half,code,index,verified", [
-    (0, 0, "FAIL_COPY_SRC", 0, 0),     # the fill is corrupted: copy 0 reads something else than the pattern
-    (1, 1, "FAIL_COPY_SRC", 1, 0),     # copy 0's destination (B) is corrupted: copy 1, which reads it, says so
-    (2, 0, "FAIL_COPY_SRC", 2, 1),     # copy 1's destination (A): copy 0's was fine (1 verified), copy 2 trips
-    (3, 1, "FAIL_READ", 0, 2),         # the last copy's destination (B): read sweep 0 re-reads it
-    (4, 0, "FAIL_READ", 1, 3),         # after read 0: half A, read by read sweep 1
-    (5, 0, "FAIL_NONE", 0, 3),         # after the last sweep that reads half A: nobody looks again — and nothing was written
+def _inject_row(copies, after, half, code, index, verified):
+    """One fault-injection case; the three-copy rows keep their ids of old (after-half-code-index-verified), the other
+    shapes carry their copy count in front."""
+    tail = "%d-%d-%s-%d-%d" % (after, half, code, index, verified)
+    return pytest.param(copies, after, half, code, index, verified, id=tail if copies == 3 else "C%d-%s" % (copies, tail))
+
+
+@pytest.mark.parametrize("copies,after,half,code,index,verified", [
+    # fill, 3 copies (A->B, B->A, A->B), 2 reads (B, A)
+    _inject_row(3, 0, 0, "FAIL_COPY_SRC", 0, 0),     # the fill is corrupted: copy 0 reads something else than the pattern
+    _inject_row(3, 1, 1, "FAIL_COPY_SRC", 1, 0),     # copy 0's destination (B) is corrupted: copy 1, which reads it, says so
+    _inject_row(3, 2, 0, "FAIL_COPY_SRC", 2, 1),     # copy 1's destination (A): copy 0's was fine (1 verified), copy 2 trips
+    _inject_row(3, 3, 1, "FAIL_READ", 0, 2),         # the last copy's destination (B): read sweep 0 re-reads it
+    _inject_row(3, 4, 0, "FAIL_READ", 1, 3),         # after read 0: half A, read by read sweep 1
+    _inject_row(3, 5, 0, "FAIL_NONE", 0, 3),         # after the last sweep that reads half A: nobody looks again — and nothing was written
+    # fill, 2 copies (A->B, B->A), 2 reads (A, B)
+    _inject_row(2, 0, 0, "FAIL_COPY_SRC", 0, 0),     # the fill: copy 0 trips, and the corruption travels on through every sweep
+    _inject_row(2, 1, 1, "FAIL_COPY_SRC", 1, 0),     # copy 0's destination (B): copy 1 trips, read 0 re-reads its copy of it
+    _inject_row(2, 2, 0, "FAIL_READ", 0, 1),         # the last copy's destination (A): read sweep 0
+    _inject_row(2, 2, 1, "FAIL_READ", 1, 2),         # B after the last copy: only read sweep 1 looks at it
+    _inject_row(2, 3, 1, "FAIL_READ", 1, 2),         # after read 0: half B, read by read sweep 1
+    # fill, no copies (CRO_F_SKIP_COPY), 2 reads (A, A)
+    _inject_row(0, 0, 0, "FAIL_READ", 0, 0),         # the fill: read sweep 0
+    _inject_row(0, 1, 0, "FAIL_READ", 1, 0),         # after read 0: read sweep 1
+    _inject_row(0, 0, 1, "FAIL_NONE", 0, 0),         # half B: no sweep of a probe without copies reads it
 ])
-def test_device_side_verdict_names_the_sweep_that_caught_it(cro, coracle, after, half, code, index, verified):
+def test_device_side_verdict_names_the_sweep_that_caught_it(cro, coracle, copies, after, half, code, index, verified):
     """Fault injection INSIDE the probe (a one-word XOR kernel behind a chosen sweep of the captured graph): the finalize
-    kernel's verdict must name the first sweep that read the corrupted half, and count the copies verified before it.
-    Probe shape: fill, 3 copies (A->B, B->A, A->B), 2 reads (B, A)."""
+    kernel's verdict must name the first sweep that read the corrupted half, and count the copies verified before it."""
     S = 32 << 20
     n = S // 8
     word = half * n + 123457
-    with cro.ProbeContext(sweep_bytes=S, devices=[0], read_sweeps=2, copy_sweeps=3, inject=(after, word, 1 << 33)) as c:
+    flags = cro.F_SKIP_COPY if copies == 0 else 0
+    with cro.ProbeContext(sweep_bytes=S, devices=[0], flags=flags, read_sweeps=2, copy_sweeps=copies or 1,
+                          inject=(after, word, 1 << 33)) as c:
         r = c.probe_device(0, allow_checksum_error=True)
         want = coracle.checksum(r.seed, 0, n)
         assert r.expect == want
