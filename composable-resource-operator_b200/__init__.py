@@ -146,8 +146,45 @@ class FullBoxTime(ctypes.Structure):
 
 GATHER_HOST, GATHER_NCCL, GATHER_DEGRADED = 0, 1, 2
 
+# fault locator (cro_locate_faults)
+LOCATE_RETEST = 1
+LOCATE_RECORDS, LOCATE_PASSES, LOCATE_GRANULE_BYTES = 4096, 3, 2 << 20
+FAULTS_NONE, FAULTS_UNCLASSIFIED, FAULTS_NOT_REPRODUCED, FAULTS_PERSISTENT = 0, 1, 2, 3
+
+
+class LocateOpts(ctypes.Structure):
+    _fields_ = [("flags", ctypes.c_uint32), ("reserved0", ctypes.c_uint32),
+                ("test_force_first", ctypes.c_uint64), ("test_force_count", ctypes.c_uint64),
+                ("test_force_and", ctypes.c_uint64), ("test_force_or", ctypes.c_uint64)]
+
+
+class FaultWord(ctypes.Structure):
+    """One located word: region index (half B starts at S / 8), expected and actual value, bit p = pass p saw it."""
+    _fields_ = [("word_index", ctypes.c_uint64), ("expected", ctypes.c_uint64), ("actual", ctypes.c_uint64),
+                ("passes", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+class LocatePass(ctypes.Structure):
+    _fields_ = [("halves", ctypes.c_uint32), ("skipped", ctypes.c_uint32), ("seed", ctypes.c_uint64 * 2),
+                ("invert", ctypes.c_uint64), ("words_scanned", ctypes.c_uint64), ("mismatches", ctypes.c_uint64),
+                ("recorded", ctypes.c_uint64), ("granules", ctypes.c_uint64), ("scan_ns", ctypes.c_uint64),
+                ("fold_xor", ctypes.c_uint64 * 2), ("fold_sum", ctypes.c_uint64 * 2), ("fold_wsum", ctypes.c_uint64 * 2)]
+
+    def fold(self, h: int) -> Tuple[int, int, int]:
+        """Checksum (xor, sum, weighted sum) of half h as the pass read it."""
+        return (self.fold_xor[h], self.fold_sum[h], self.fold_wsum[h])
+
+
+class FaultReport(ctypes.Structure):
+    """cro_fault_report: what cro_locate_faults found, per pass and over all passes."""
+    _fields_ = [("status", ctypes.c_int32), ("verdict", ctypes.c_uint32), ("n_passes", ctypes.c_uint32),
+                ("complete", ctypes.c_uint32), ("sweep_bytes", ctypes.c_uint64), ("retest_seed", ctypes.c_uint64),
+                ("located", ctypes.c_uint64), ("recorded", ctypes.c_uint64), ("flip_or", ctypes.c_uint64),
+                ("bit_flips", ctypes.c_uint64 * 64), ("pass_", LocatePass * LOCATE_PASSES)]
+
 
 assert ctypes.sizeof(ProbeResult) == 512, ctypes.sizeof(ProbeResult)
+assert ctypes.sizeof(FaultReport) == 928 and ctypes.sizeof(LocatePass) == 120, ctypes.sizeof(FaultReport)
 
 # Every symbol include/croprobe.h declares; tests check the library exports all of them.
 EXPORTS = [
@@ -169,6 +206,7 @@ EXPORTS = [
     "cro_selftest_exception_barrier", "cro_probe_sweep_times", "cro_p2p_detail_get", "cro_fullbox_times",
     "cro_chase_end", "cro_validate_env", "cro_node_inventory", "cro_probe_uuid", "cro_set_latency_hops", "cro_local_exec", "cro_metrics_text", "cro_describe_wire_type",
     "cro_selftest_probe_finalize", "cro_selftest_p2p_finalize", "cro_selftest_chase",
+    "cro_locate_faults", "cro_emit_fault_annotations_json",
 ]
 
 # Slot map of a device's sweep-slot array (cro_sweep_slot, 64 bytes each); the cro_selftest_* hooks take such arrays.
@@ -255,6 +293,9 @@ def _load() -> ctypes.CDLL:
                                             ctypes.POINTER(u64), ctypes.POINTER(u32), u32, u32, u32, u32, u32, u64, u64]),
         "cro_selftest_chase": (i32, [vp, i32, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), u32, u32,
                                      ctypes.POINTER(u64)]),
+        "cro_locate_faults": (i32, [vp, i32, ctypes.POINTER(LocateOpts), ctypes.POINTER(FaultReport), ctypes.POINTER(FaultWord),
+                                    i32, ctypes.POINTER(i32)]),
+        "cro_emit_fault_annotations_json": (i32, [ctypes.POINTER(FaultReport), ctypes.POINTER(FaultWord), i32] + out),
         "cro_local_node_op": (i32, [vp, c] + out),
         "cro_local_exec": (i32, [c] + out),
         "cro_describe_wire_type": (i32, [c] + out),
@@ -377,6 +418,12 @@ def emit_sunfish_request(name: str, count: int, proc_type: str, model: str) -> s
 
 def emit_probe_annotations_json(r: ProbeResult) -> str:
     return _text(lib.cro_emit_probe_annotations_json, ctypes.byref(r))
+
+
+def emit_fault_annotations_json(report: FaultReport, words: List[FaultWord]) -> str:
+    """Additive cohdi.io/probe-fault-* annotations of a locate_faults report (Go-marshalled map[string]string)."""
+    arr = (FaultWord * max(1, len(words)))(*words)
+    return _text(lib.cro_emit_fault_annotations_json, ctypes.byref(report), arr, len(words))
 
 
 def fm_parse_scale_up_response(body: str, name: str, res_type: str, model: str) -> Tuple[str, str, str]:
@@ -552,6 +599,23 @@ class ProbeContext:
         arr = (ctypes.c_uint64 * n)()
         self._check(lib.cro_read_words(self.handle, dev, first, n, arr))
         return list(arr)
+
+    def locate_faults(self, dev: int = 0, retest: bool = True, cap: int = 256,
+                      force: Optional[Tuple[int, int, int, int]] = None) -> Tuple[FaultReport, List[FaultWord]]:
+        """cro_locate_faults: which words of the sweep region differ from their pattern, typically right after a probe
+        returned ERR_CHECKSUM.  Pass 0 compares what the region holds now; retest adds the fresh-pattern and complement
+        passes.  force = (first, count, and_mask, or_mask) is the test-only stand-in for stuck cells, applied after
+        each retest fill.  Returns the report (its status is OK or ERR_CHECKSUM) and up to `cap` words by index."""
+        o = LocateOpts()
+        o.flags = LOCATE_RETEST if retest else 0
+        if force is not None:
+            o.test_force_first, o.test_force_count, o.test_force_and, o.test_force_or = force
+        rep = FaultReport()
+        arr = (FaultWord * max(1, cap))()
+        n = ctypes.c_int()
+        self._check(lib.cro_locate_faults(self.handle, dev, ctypes.byref(o), ctypes.byref(rep), arr, cap, ctypes.byref(n)),
+                    allow=(ERR_CHECKSUM,))
+        return rep, [arr[i] for i in range(n.value)]
 
     def launch_count(self) -> int:
         return int(lib.cro_launch_count(self.handle))

@@ -38,6 +38,10 @@ static_assert(offsetof(cro_probe_result, nonce) == 488, "layout");
 static_assert(offsetof(cro_probe_result, t_start_ns) == 504, "layout");
 static_assert(sizeof(cro_fullbox_time) == 64 && offsetof(cro_fullbox_time, gather) == 56, "cro_fullbox_time layout");
 static_assert(sizeof(cro_sweep_result) == 56, "layout");
+static_assert(sizeof(cro_locate_opts) == 40 && sizeof(cro_fault_word) == 32, "locator layout");
+static_assert(sizeof(cro_locate_pass) == 120 && offsetof(cro_locate_pass, fold_xor) == 72, "locator layout");
+static_assert(sizeof(cro_fault_report) == 928 && offsetof(cro_fault_report, bit_flips) == 56 &&
+                  offsetof(cro_fault_report, pass) == 568, "locator layout");
 
 using namespace cro::capi;
 
@@ -260,6 +264,21 @@ int cro_inject_fault(cro_ctx* ctx, int i, uint64_t word, uint64_t mask) try {
 int cro_read_words(cro_ctx* ctx, int i, uint64_t first, uint64_t n, uint64_t* out) try {
     return ctx ? ctx_read_words(ctx, i, first, n, out) : CRO_ERR_INVALID_ARG;
 } CRO_API_CATCH
+int cro_locate_faults(cro_ctx* ctx, int i, const cro_locate_opts* opts, cro_fault_report* out, cro_fault_word* words, int cap,
+                      int* n) try {
+    if (!ctx || !out || !n || cap < 0 || (cap > 0 && !words)) return CRO_ERR_INVALID_ARG;
+    *n = 0;
+    cro_locate_opts o{};
+    if (opts) o = *opts;
+    std::vector<cro_fault_word> found;
+    const int rc = ctx_locate(ctx, i, o, out, &found);
+    const size_t k = std::min(found.size(), (size_t)cap);
+    for (size_t j = 0; j < k; ++j) words[j] = found[j];
+    out->recorded = k;
+    if (k < found.size()) out->complete = 0;        // the caller's list misses some located words
+    *n = (int)k;
+    return rc;
+} CRO_API_CATCH
 int cro_device_seed(cro_ctx* ctx, int i, uint64_t* seed) try {
     if (!ctx || !seed || i < 0 || i >= (int)ctx->devs.size()) return CRO_ERR_INVALID_ARG;
     std::lock_guard<std::mutex> g(ctx->devs[(size_t)i]->mu);
@@ -461,6 +480,35 @@ int cro_emit_probe_annotations_json(const cro_probe_result* r, char* buf, size_t
     if (!r) return CRO_ERR_INVALID_ARG;
     gojson::Writer w;
     w.string_map(probe_annotations(*r));
+    return copy_out(w.str(), buf, cap, len);
+} CRO_API_CATCH
+
+int cro_emit_fault_annotations_json(const cro_fault_report* r, const cro_fault_word* words, int n, char* buf, size_t cap,
+                                    size_t* len) try {
+    if (!r || n < 0 || (n > 0 && !words)) return CRO_ERR_INVALID_ARG;
+    static const char* const kVerdict[] = {"none", "unclassified", "not-reproduced", "persistent"};
+    std::map<std::string, std::string> m;
+    m["cohdi.io/probe-fault-verdict"] = kVerdict[fault_verdict(*r)];
+    std::string mism, gran, bits, ws;
+    const uint32_t np = std::min<uint32_t>(r->n_passes, CRO_LOCATE_PASSES);
+    for (uint32_t p = 0; p < np; ++p) {
+        const std::string sep = p ? "," : "";
+        mism += sep + std::to_string(p) + ":" + std::to_string(r->pass[p].mismatches);
+        gran += sep + std::to_string(p) + ":" + std::to_string(r->pass[p].granules);
+    }
+    m["cohdi.io/probe-fault-mismatches"] = mism;
+    m["cohdi.io/probe-fault-granules"] = gran;
+    for (int b = 0; b < 64; ++b)
+        if (r->bit_flips[b]) bits += (bits.empty() ? "" : ",") + std::to_string(b);
+    if (!bits.empty()) m["cohdi.io/probe-fault-bits"] = bits;
+    for (int k = 0; k < n && k < 8; ++k) {
+        char idx[24];
+        snprintf(idx, sizeof idx, "%llx", (unsigned long long)words[k].word_index);
+        ws += (k ? "," : "") + std::string(idx) + ":" + hex16(words[k].expected ^ words[k].actual);
+    }
+    if (!ws.empty()) m["cohdi.io/probe-fault-words"] = ws;
+    gojson::Writer w;
+    w.string_map(m);
     return copy_out(w.str(), buf, cap, len);
 } CRO_API_CATCH
 

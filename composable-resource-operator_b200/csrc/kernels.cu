@@ -9,6 +9,8 @@
 //   hbm_copy_fused    2S bytes moved    + the same checksum of the source stream, folded out of shared memory
 //   hbm_copy_*        2S bytes moved    (plain variants, kept for comparison)
 //   hbm_expected      0 bytes           the same checksum from the closed form
+//   hbm_locate        S bytes read      the read sweep's checksum + every word compared with its closed form
+//                                       (the fault locator, cro_locate_faults; not part of the probe)
 //   chase             pointer chase over peer-resident permutations (latency)
 //   probe_finalize / p2p_finalize       the verdict: the 512-byte result struct is written on the device
 //
@@ -307,11 +309,13 @@ __device__ __forceinline__ void publish_window(unsigned long long t_start, const
 // The CTAs also keep the sweep's %globaltimer window (first start, last store
 // issued) so the device-written result needs no host-side event arithmetic.
 // ---------------------------------------------------------------------------
-template <int THREADS, int UNROLL>
+// INVERT (the fault locator's complement retest) stores ~pattern; the probe's instantiation keeps the plain pattern.
+template <int THREADS, int UNROLL, bool INVERT = false>
 __global__ void __launch_bounds__(THREADS)
 hbm_fill_kernel(uint4* __restrict__ base, unsigned long long n_vec, const ProbeParams imm,
                 const ProbeParams* __restrict__ pp, SweepScratch sc, SweepOut* out) {
     const unsigned long long seed = pp ? pp->seed : imm.seed;
+    constexpr unsigned long long inv = INVERT ? ~0ull : 0ull;
     unsigned long long t_start = 0;
     if (threadIdx.x == 0) t_start = globaltimer_ns();
     const unsigned long long tile_vecs = (unsigned long long)THREADS * UNROLL;
@@ -321,8 +325,8 @@ hbm_fill_kernel(uint4* __restrict__ base, unsigned long long n_vec, const ProbeP
 #pragma unroll
         for (int j = 0; j < UNROLL; ++j) {
             const unsigned long long v = v0 + (unsigned long long)j * THREADS;
-            const unsigned long long a = pattern_word(seed, 2 * v);
-            const unsigned long long b = pattern_word(seed, 2 * v + 1);
+            const unsigned long long a = pattern_word(seed, 2 * v) ^ inv;
+            const unsigned long long b = pattern_word(seed, 2 * v + 1) ^ inv;
             stg_stream(base + v, make_uint4((unsigned)a, (unsigned)(a >> 32), (unsigned)b,
                                             (unsigned)(b >> 32)));
         }
@@ -331,8 +335,8 @@ hbm_fill_kernel(uint4* __restrict__ base, unsigned long long n_vec, const ProbeP
     for (unsigned long long v = n_tiles * tile_vecs + (unsigned long long)blockIdx.x * THREADS +
                                 threadIdx.x;
          v < n_vec; v += (unsigned long long)gridDim.x * THREADS) {
-        const unsigned long long a = pattern_word(seed, 2 * v);
-        const unsigned long long b = pattern_word(seed, 2 * v + 1);
+        const unsigned long long a = pattern_word(seed, 2 * v) ^ inv;
+        const unsigned long long b = pattern_word(seed, 2 * v + 1) ^ inv;
         stg_stream(base + v,
                    make_uint4((unsigned)a, (unsigned)(a >> 32), (unsigned)b, (unsigned)(b >> 32)));
     }
@@ -386,6 +390,158 @@ hbm_read_ldg_kernel(const uint4* __restrict__ base, unsigned long long n_vec, co
         fold2(A, lo64(v), hi64(v), 4 * i + 1);
     }
     publish(acc_x(A) ^ acc_x(B), A.s + B.s, acc_w(A) + acc_w(B), t_start, sc, out, imm, pp, 2 * n_vec);
+}
+
+// ---------------------------------------------------------------------------
+// hbm_locate: the fault locator's compare pass over one half.  The loads and
+// the fold are the LDG read sweep's; each word is also XORed with its expected
+// value, regenerated in registers.  A warp whose words all match takes no other
+// step.  Otherwise the warp (converged: every caller's loop is warp-uniform)
+// records its mismatches with warp-aggregated updates:
+//   count      one shared-memory add per warp, one global add per CTA at the end
+//   records    one atomicAdd per warp claims a run of slots, only while the
+//              buffer has room (a plain load checks first: a full buffer costs
+//              no atomics, so a half that mismatches everywhere does not
+//              serialise on the claim counter)
+//   bit flips  per flipped bit position of the warp: a warp sum into shared
+//              memory, flushed once per CTA
+//   granules   a warp's words span < 2 MiB, so at most two granules: the warp
+//              min and max, set with atomicOr only when not already set
+// ---------------------------------------------------------------------------
+struct LocateCtx {
+    LocateBufs b;
+    unsigned long long word0, seed, invert;
+    unsigned long long* s_bits;     // shared, 64 entries
+    unsigned long long* s_count;    // shared
+};
+
+__device__ __forceinline__ void mark_granule(unsigned long long* bitmap, unsigned g) {
+    unsigned long long* p = bitmap + (g >> 6);
+    const unsigned long long bit = 1ull << (g & 63u);
+    if (!(*reinterpret_cast<volatile unsigned long long*>(p) & bit)) atomicOr(p, bit);
+}
+
+// d[k] = actual ^ expected of the lane's word k; bit k of m: word k mismatches.  Word k is half word
+// 2 * (v0 + (k / 2) * vstride) + (k & 1).  The whole warp calls this (some lane has m != 0).
+template <int K>
+__device__ __forceinline__ void locate_record(const unsigned long long (&d)[K], unsigned m, unsigned long long v0,
+                                              unsigned long long vstride, const LocateCtx& L) {
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned n_lane = __popc(m);
+    const unsigned n_warp = __reduce_add_sync(0xffffffffu, n_lane);
+    unsigned incl = n_lane;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= (unsigned)o) incl += t;
+    }
+    unsigned long long base = kLocateRecords;
+    if (lane == 0) {
+        atomicAdd(L.s_count, (unsigned long long)n_warp);
+        if (*reinterpret_cast<volatile unsigned long long*>(&L.b.ctr->claims) < kLocateRecords)
+            base = atomicAdd(&L.b.ctr->claims, (unsigned long long)n_warp);
+    }
+    base = __shfl_sync(0xffffffffu, base, 0) + (incl - n_lane);
+    unsigned long long flips = 0;
+    unsigned gmin = ~0u, gmax = 0;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        if (!((m >> k) & 1u)) continue;
+        const unsigned long long w = 2 * (v0 + (unsigned long long)(k >> 1) * vstride) + (k & 1);
+        if (base < kLocateRecords) {
+            const unsigned long long e = pattern_word(L.seed, w) ^ L.invert;
+            L.b.rec[base] = LocateRecord{L.word0 + w, e, e ^ d[k]};
+        }
+        ++base;
+        flips |= d[k];
+        const unsigned g = (unsigned)(((L.word0 + w) * 8ull) >> kLocateGranuleShift);
+        gmin = min(gmin, g);
+        gmax = max(gmax, g);
+    }
+    gmin = __reduce_min_sync(0xffffffffu, gmin);
+    gmax = __reduce_max_sync(0xffffffffu, gmax);
+    if (lane == 0) {
+        mark_granule(L.b.granules, gmin);
+        if (gmax != gmin) mark_granule(L.b.granules, gmax);
+    }
+    unsigned long long wor = (unsigned long long)__reduce_or_sync(0xffffffffu, (unsigned)flips) |
+                             ((unsigned long long)__reduce_or_sync(0xffffffffu, (unsigned)(flips >> 32)) << 32);
+    while (wor) {                       // warp-uniform
+        const int bit = __ffsll((long long)wor) - 1;
+        wor &= wor - 1;
+        unsigned c = 0;
+#pragma unroll
+        for (int k = 0; k < K; ++k) c += ((m >> k) & 1u) ? (unsigned)((d[k] >> bit) & 1ull) : 0u;
+        c = __reduce_add_sync(0xffffffffu, c);
+        if (lane == 0) atomicAdd(&L.s_bits[bit], (unsigned long long)c);
+    }
+}
+
+template <int THREADS>
+__global__ void __launch_bounds__(THREADS)
+hbm_locate_kernel(const uint4* __restrict__ base, unsigned long long n_vec, unsigned long long word0,
+                  unsigned long long seed, unsigned long long invert, LocateBufs lb, const ProbeParams imm,
+                  SweepScratch sc, SweepOut* out) {
+    __shared__ unsigned long long s_bits[64];
+    __shared__ unsigned long long s_count;
+    const unsigned long long t_start = globaltimer_ns();
+    for (unsigned i = threadIdx.x; i < 64; i += THREADS) s_bits[i] = 0;
+    if (threadIdx.x == 0) s_count = 0;
+    __syncthreads();
+    const LocateCtx L{lb, word0, seed, invert, s_bits, &s_count};
+    Acc A, B;
+    constexpr unsigned long long tile_vecs = (unsigned long long)THREADS * 8;  // 128 B / thread
+    const unsigned long long n_tiles = n_vec / tile_vecs;
+    for (unsigned long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const unsigned long long v0 = tile * tile_vecs + threadIdx.x;
+        unsigned long long a[8], b[8];
+        ldg128_x8<THREADS * 16>(base + v0, a, b);
+#pragma unroll
+        for (int j = 0; j < 8; j += 2) {
+            fold2(A, a[j], b[j], 4 * (v0 + (unsigned long long)j * THREADS) + 1);
+            fold2(B, a[j + 1], b[j + 1], 4 * (v0 + (unsigned long long)(j + 1) * THREADS) + 1);
+        }
+        unsigned long long d[16];
+        unsigned m = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const unsigned long long v = v0 + (unsigned long long)j * THREADS;
+            d[2 * j] = a[j] ^ pattern_word(seed, 2 * v) ^ invert;
+            d[2 * j + 1] = b[j] ^ pattern_word(seed, 2 * v + 1) ^ invert;
+            m |= (d[2 * j] != 0 ? 1u : 0u) << (2 * j);
+            m |= (d[2 * j + 1] != 0 ? 1u : 0u) << (2 * j + 1);
+        }
+        if (__ballot_sync(0xffffffffu, m != 0)) locate_record<16>(d, m, v0, THREADS, L);
+    }
+    // ragged tail: warp-uniform trip count, so the ballot sees the whole warp
+    const unsigned lane = threadIdx.x & 31u;
+    for (unsigned long long vw = n_tiles * tile_vecs + (unsigned long long)blockIdx.x * THREADS + (threadIdx.x - lane);
+         vw < n_vec; vw += (unsigned long long)gridDim.x * THREADS) {
+        const unsigned long long v = vw + lane;
+        unsigned long long d[2] = {0, 0};
+        unsigned m = 0;
+        if (v < n_vec) {
+            const uint4 q = ldg_stream(base + v);
+            fold2(A, lo64(q), hi64(q), 4 * v + 1);
+            d[0] = lo64(q) ^ pattern_word(seed, 2 * v) ^ invert;
+            d[1] = hi64(q) ^ pattern_word(seed, 2 * v + 1) ^ invert;
+            m = (d[0] != 0 ? 1u : 0u) | (d[1] != 0 ? 2u : 0u);
+        }
+        if (__ballot_sync(0xffffffffu, m != 0)) locate_record<2>(d, m, v, 0, L);
+    }
+    __syncthreads();
+    if (s_count) {                      // CTA-uniform: read after the barrier
+        if (threadIdx.x == 0) atomicAdd(&lb.ctr->mismatches, s_count);
+        if (threadIdx.x < 64 && s_bits[threadIdx.x]) atomicAdd(&lb.ctr->bits[threadIdx.x], s_bits[threadIdx.x]);
+    }
+    publish(acc_x(A) ^ acc_x(B), A.s + B.s, acc_w(A) + acc_w(B), t_start, sc, out, imm, nullptr, 2 * n_vec);
+}
+
+__global__ void force_words_kernel(unsigned long long* base, unsigned long long first, unsigned long long count,
+                                   unsigned long long and_mask, unsigned long long or_mask) {
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < count;
+         i += (unsigned long long)gridDim.x * blockDim.x)
+        base[first + i] = (base[first + i] & and_mask) | or_mask;
 }
 
 // Consumer side shared by the TMA read kernel and the checksumming copy: folds
@@ -950,6 +1106,10 @@ cudaError_t plan_kernels(int device, const env::Values& knobs, KernelPlan* plan,
     if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, rdw, kReadThreads, 0)) != cudaSuccess)
         return e;
     plan->read_ldg256 = {sms * (occ > 0 ? occ : 1) * (int)knob("CRO_READ_WAVES"), kReadThreads, 0};
+    auto loc = hbm_locate_kernel<kReadThreads>;
+    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, loc, kReadThreads, 0)) != cudaSuccess)
+        return e;
+    plan->locate = {sms * (occ > 0 ? occ : 1) * (int)knob("CRO_READ_WAVES"), kReadThreads, 0};
 
     auto cp = hbm_copy_ldg_kernel<kCopyThreads, kCopyUnroll>;
     if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cp, kCopyThreads, 0)) != cudaSuccess)
@@ -1039,14 +1199,34 @@ static int clamp_grid(int planned, uint64_t bytes, uint64_t tile_bytes) {
 }
 
 cudaError_t launch_fill(const KernelPlan& p, void* base, uint64_t bytes, const Params& pr,
-                        const SweepScratch& sc, SweepOut* out, cudaStream_t st) {
+                        const SweepScratch& sc, SweepOut* out, cudaStream_t st, bool invert) {
     // Few tiles per CTA: with a fixed grid a 16 GiB fill strides 14 tiles per CTA, the SMs drift apart and the DRAM
     // window spreads and the rate drops as the sweep grows; the grid therefore grows with the sweep.
     constexpr uint64_t kTile = (uint64_t)kFillThreads * kFillUnroll * 16;
     const uint64_t tiles = (bytes + kTile - 1) / kTile;
     const int planned = (int)std::min<uint64_t>(std::max<uint64_t>((uint64_t)p.fill.grid, tiles / 4), 0x7FFFFFFFull);
-    hbm_fill_kernel<kFillThreads, kFillUnroll><<<clamp_grid(planned, bytes, kTile), p.fill.block, 0, st>>>(
-        static_cast<uint4*>(base), bytes >> 4, pr.imm, pr.pp, sc, out);
+    if (invert)
+        hbm_fill_kernel<kFillThreads, kFillUnroll, true><<<clamp_grid(planned, bytes, kTile), p.fill.block, 0, st>>>(
+            static_cast<uint4*>(base), bytes >> 4, pr.imm, pr.pp, sc, out);
+    else
+        hbm_fill_kernel<kFillThreads, kFillUnroll><<<clamp_grid(planned, bytes, kTile), p.fill.block, 0, st>>>(
+            static_cast<uint4*>(base), bytes >> 4, pr.imm, pr.pp, sc, out);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_locate(const KernelPlan& p, const void* half, uint64_t bytes, uint64_t word0, uint64_t seed,
+                          uint64_t invert, const LocateBufs& lb, const SweepScratch& sc, SweepOut* out, cudaStream_t st) {
+    hbm_locate_kernel<kReadThreads><<<clamp_grid(p.locate.grid, bytes, kReadThreads * 128), p.locate.block, 0, st>>>(
+        static_cast<const uint4*>(half), bytes >> 4, word0, seed, invert, lb, ProbeParams{seed, 0}, sc, out);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_force_words(void* base, uint64_t first, uint64_t count, uint64_t and_mask, uint64_t or_mask,
+                               int sm_count, cudaStream_t st) {
+    if (count == 0) return cudaSuccess;
+    const uint64_t blocks = std::min<uint64_t>((count + 255) / 256, (uint64_t)std::max(sm_count, 1) * 8);
+    force_words_kernel<<<(unsigned)blocks, 256, 0, st>>>(static_cast<unsigned long long*>(base), first, count, and_mask,
+                                                        or_mask);
     return cudaGetLastError();
 }
 

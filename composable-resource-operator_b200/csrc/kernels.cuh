@@ -75,7 +75,7 @@ enum : unsigned { READ_LDG = 1, READ_TMA = 2, READ_LDG256 = 3, COPY_LDG = 1, COP
 
 // One-time per-device setup (smem carve-outs, occupancy → persistent grid size).
 struct KernelPlan {
-    LaunchCfg fill, read_ldg, read_ldg256, read_tma, copy_ldg, copy_tma, copy_fused, expect;
+    LaunchCfg fill, read_ldg, read_ldg256, read_tma, copy_ldg, copy_tma, copy_fused, expect, locate;
     int sm_count;
     // tuning knobs, from the owning context's validated snapshot (see env.hpp)
     unsigned read_tile, read_stages, read_chunk, read_dyn;
@@ -92,8 +92,9 @@ struct Params {
     ProbeParams imm;
     const ProbeParams* pp;
 };
+// invert: write the bitwise complement of the pattern (the fault locator's second retest pass; the probe never does).
 cudaError_t launch_fill(const KernelPlan&, void* base, uint64_t bytes, const Params&,
-                        const SweepScratch&, SweepOut* out, cudaStream_t);
+                        const SweepScratch&, SweepOut* out, cudaStream_t, bool invert = false);
 cudaError_t launch_read(const KernelPlan&, unsigned variant, const void* base, uint64_t bytes,
                         const Params&, const SweepScratch&, SweepOut* out, cudaStream_t);
 // Every variant publishes *out when out is non-null: the %globaltimer window, the stamp and n_words = bytes / 8.
@@ -104,6 +105,31 @@ cudaError_t launch_copy(const KernelPlan&, unsigned variant, void* dst, const vo
 cudaError_t launch_expected(const KernelPlan&, uint64_t bytes, const Params&,
                             const SweepScratch&, SweepOut* out, cudaStream_t);
 cudaError_t launch_xor_word(void* base, uint64_t word_index, uint64_t mask, cudaStream_t);
+
+// Fault locator (cro_locate_faults).  One compare pass over one half: every word is checked against
+// pattern_word(seed, i) ^ invert (i counted from the half's start, as the probe's copies keep it), the half is folded
+// into *out like a read sweep, and every mismatch is counted into the pass's LocateCounters and bitmap, and recorded
+// while the pass's record buffer has room.
+constexpr unsigned kLocateRecords = CRO_LOCATE_RECORDS;
+constexpr unsigned kLocateGranuleShift = 21;               // 2 MiB granules of the region
+struct LocateRecord {
+    unsigned long long word, expected, actual;             // word: region index (half B starts at S / 8)
+};
+struct LocateCounters {
+    unsigned long long mismatches;                          // exact
+    unsigned long long claims;                              // record slots claimed (may run past kLocateRecords)
+    unsigned long long bits[64];                            // mismatching words with bit b flipped
+};
+struct LocateBufs {
+    LocateCounters* ctr;
+    LocateRecord* rec;                                      // kLocateRecords entries
+    unsigned long long* granules;                           // bit g: granule g of the region holds a mismatch
+};
+cudaError_t launch_locate(const KernelPlan&, const void* half, uint64_t bytes, uint64_t word0, uint64_t seed,
+                          uint64_t invert, const LocateBufs&, const SweepScratch&, SweepOut* out, cudaStream_t);
+// word = (word & and_mask) | or_mask over region words [first, first + count): the locator's test hook.
+cudaError_t launch_force_words(void* base, uint64_t first, uint64_t count, uint64_t and_mask, uint64_t or_mask,
+                               int sm_count, cudaStream_t);
 
 // Pointer chase for NVLink latency: warp j of the one CTA follows `hops` dependent ld.relaxed.sys loads through
 // table[j] (one 8-byte slot per 128-byte line, peer-resident); out[2j] = final index, out[2j+1] = %globaltimer ns.

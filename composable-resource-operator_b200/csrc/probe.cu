@@ -15,6 +15,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <random>
 #include <thread>
 
@@ -88,7 +89,15 @@ int ensure_region(cro_ctx* c, Device* d) {
         }
     }
     d->filled = false;
+    d->half_known[0] = d->half_known[1] = false;
     return CRO_OK;
+}
+
+// Half A now holds the pattern of seed_cur (a fill, or a probe's fill).
+void half_a_filled(Device* d) {
+    d->filled = true;
+    d->half_known[0] = true;
+    d->half_seed[0] = d->seed_cur;
 }
 
 int ensure_filled(cro_ctx* c, Device* d) {
@@ -97,7 +106,7 @@ int ensure_filled(cro_ctx* c, Device* d) {
     if (d->filled) return CRO_OK;
     CU_TRY(c, launch_fill(d->plan, d->region, d->sweep_bytes, imm_params(d), d->scratch, nullptr, d->stream));
     c->launches++;
-    d->filled = true;
+    half_a_filled(d);
     return CRO_OK;
 }
 
@@ -437,6 +446,9 @@ Device::~Device() {
     free_scratch(&scratch);
     free_scratch(&scratch_aux);
     free_scratch(&scratch_pfx);
+    free_scratch(&scratch_loc);
+    cudaFree(d_locate);
+    if (h_locate) cudaFreeHost(h_locate);
     for (Lane& L : lanes) {
         cudaFree(L.d_out);
         if (L.h_out) cudaFreeHost(L.h_out);
@@ -504,7 +516,7 @@ int ctx_fill(cro_ctx* c, int idx, uint32_t iters, cro_sweep_result* out) {
         CU_TRY(c, launch_fill(d->plan, d->region, d->sweep_bytes, imm_params(d), d->scratch, &d->d_out[kSlotScratch], d->stream));
     CU_TRY(c, cudaEventRecord(d->ev1, d->stream));
     c->launches += iters;
-    d->filled = true;
+    half_a_filled(d);
     CU_TRY(c, cudaMemcpyAsync(&d->h_out[kSlotScratch], &d->d_out[kSlotScratch], sizeof(SweepOut), cudaMemcpyDeviceToHost, d->stream));
     if ((rc = wait_stream(c, d))) return rc;
     float ms = 0;
@@ -563,6 +575,8 @@ int ctx_copy(cro_ctx* c, int idx, uint32_t variant, uint32_t iters, cro_sweep_re
                               d->scratch, &d->d_out[kSlotScratch], d->stream));
     CU_TRY(c, cudaEventRecord(d->ev1, d->stream));
     c->launches += iters;
+    d->half_known[1] = d->half_known[0];          // B is a copy of A
+    d->half_seed[1] = d->half_seed[0];
     CU_TRY(c, cudaMemcpyAsync(&d->h_out[kSlotScratch], &d->d_out[kSlotScratch], sizeof(SweepOut), cudaMemcpyDeviceToHost,
                               d->stream));
     if ((rc = wait_stream(c, d))) return rc;
@@ -630,6 +644,193 @@ int ctx_read_words(cro_ctx* c, int idx, uint64_t first, uint64_t n, uint64_t* ou
     CU_TRY(c, cudaMemcpyAsync(out, d->region + first * 8, n * 8, cudaMemcpyDeviceToHost, d->stream));
     CU_TRY(c, cudaStreamSynchronize(d->stream));
     return CRO_OK;
+}
+
+// ---------------------------------------------------------------------------
+// fault locator (cro_locate_faults)
+// ---------------------------------------------------------------------------
+namespace {
+// The retest pattern's seed: seed_dev + 2^63.  A probe's seed is seed_dev + nonce * kNonceStride with kNonceStride odd,
+// which equals it only for nonce 2^63: no probe of the context shares the retest's pattern.
+constexpr uint64_t kRetestSeedOffset = 1ull << 63;
+constexpr int kLocateSlots = 2 * CRO_LOCATE_PASSES + CRO_LOCATE_PASSES;   // [2p + h] compare sweeps, then closed forms
+
+// Byte offsets in d_locate: counters and granule bitmaps (zeroed per call), result slots, records.
+struct LocateLayout {
+    size_t ctr, gran, zero_bytes, slots, rec, total;
+    uint64_t gran_words;          // bitmap words per pass
+};
+LocateLayout locate_layout(uint64_t S) {
+    LocateLayout L{};
+    const uint64_t granules = (2 * S + CRO_LOCATE_GRANULE_BYTES - 1) / CRO_LOCATE_GRANULE_BYTES;
+    L.gran_words = (granules + 63) / 64;
+    L.ctr = 0;
+    L.gran = CRO_LOCATE_PASSES * sizeof(LocateCounters);
+    L.zero_bytes = L.gran + CRO_LOCATE_PASSES * L.gran_words * 8;
+    L.slots = (L.zero_bytes + 63) & ~(size_t)63;
+    L.rec = L.slots + kLocateSlots * sizeof(SweepOut);
+    L.total = L.rec + CRO_LOCATE_PASSES * (size_t)kLocateRecords * sizeof(LocateRecord);
+    return L;
+}
+
+// Closed form of the complement of a pattern over n words, from the pattern's: ~p = -1 - p, and the weights
+// 2i + 1 of n words sum to n^2.
+SweepOut complement_fold(SweepOut f, uint64_t n) {
+    f.x ^= (n & 1) ? ~0ull : 0ull;
+    f.s = 0 - n - f.s;
+    f.w = 0 - n * n - f.w;
+    return f;
+}
+}  // namespace
+
+uint32_t fault_verdict(const cro_fault_report& r) {
+    const uint32_t np = std::min<uint32_t>(r.n_passes, CRO_LOCATE_PASSES);
+    for (uint32_t p = 1; p < np; ++p)
+        if (r.pass[p].mismatches) return CRO_FAULTS_PERSISTENT;
+    if (np == 0 || r.pass[0].mismatches == 0) return CRO_FAULTS_NONE;
+    return np > 1 ? CRO_FAULTS_NOT_REPRODUCED : CRO_FAULTS_UNCLASSIFIED;
+}
+
+int ctx_locate(cro_ctx* c, int idx, const cro_locate_opts& o, cro_fault_report* rep, std::vector<cro_fault_word>* words) {
+    memset(rep, 0, sizeof *rep);
+    words->clear();
+    Device* d = dev_at(c, idx);
+    if (!d) {
+        c->set_error("dev_index " + std::to_string(idx) + " is not a device of this context (a GPU probed through the helper "
+                     "process has no resident region to locate faults in)");
+        return rep->status = CRO_ERR_INVALID_ARG;
+    }
+    if (o.flags & ~CRO_LOCATE_RETEST) return rep->status = CRO_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> g(d->mu);
+    drain_pending(c, d);
+    int rc = [&]() -> int {
+        CU_TRY(c, cudaSetDevice(d->ordinal));
+        int r = ensure_region(c, d);
+        if (r) return r;
+        const uint64_t S = d->sweep_bytes, n = S / 8;
+        if (o.test_force_count && (o.test_force_first >= 2 * n || o.test_force_count > 2 * n - o.test_force_first))
+            return CRO_ERR_INVALID_ARG;
+        const LocateLayout lay = locate_layout(S);
+        if (!d->locate_bytes) {       // next to the region, never at its expense: no room is an error of this call
+            if (!d->d_locate) CU_TRY(c, cudaMalloc(&d->d_locate, lay.total));
+            if (!d->h_locate) CU_TRY(c, cudaMallocHost(&d->h_locate, lay.total));
+            if (!d->scratch_loc.partials &&
+                (r = alloc_scratch(c, &d->scratch_loc, std::max({d->plan.locate.grid, d->plan.expect.grid, 1}))))
+                return r;
+            d->locate_bytes = lay.total;
+        }
+        unsigned char* dl = d->d_locate;
+        LocateCounters* ctr = reinterpret_cast<LocateCounters*>(dl + lay.ctr);
+        unsigned long long* gran = reinterpret_cast<unsigned long long*>(dl + lay.gran);
+        SweepOut* slots = reinterpret_cast<SweepOut*>(dl + lay.slots);
+        LocateRecord* rec = reinterpret_cast<LocateRecord*>(dl + lay.rec);
+        CU_TRY(c, cudaMemsetAsync(dl, 0, lay.zero_bytes, d->stream));
+
+        const bool retest = (o.flags & CRO_LOCATE_RETEST) != 0;
+        const uint32_t np = retest ? CRO_LOCATE_PASSES : 1;
+        const uint64_t rseed = d->seed_dev + kRetestSeedOffset;
+        rep->sweep_bytes = S;
+        rep->n_passes = np;
+        rep->retest_seed = retest ? rseed : 0;
+        unsigned char* half[2] = {d->region, d->region + S};
+        std::vector<uint64_t> cf_seeds;      // closed forms to generate, one per distinct seed
+        for (uint32_t p = 0; p < np; ++p) {
+            cro_locate_pass& P = rep->pass[p];
+            P.invert = p == 2 ? ~0ull : 0ull;
+            if (p == 0) {
+                for (int h = 0; h < 2; ++h) {
+                    if (d->half_known[h]) { P.halves |= 1u << h; P.seed[h] = d->half_seed[h]; }
+                    else P.skipped |= 1u << h;
+                }
+            } else {
+                P.halves = 3;
+                P.seed[0] = P.seed[1] = rseed;
+                const Params fp{ProbeParams{rseed, d->nonce_cur}, nullptr};
+                for (int h = 0; h < 2; ++h)
+                    CU_TRY(c, launch_fill(d->plan, half[h], S, fp, d->scratch_loc, nullptr, d->stream, p == 2));
+                CU_TRY(c, launch_force_words(d->region, o.test_force_first, o.test_force_count, o.test_force_and,
+                                             o.test_force_or, d->plan.sm_count, d->stream));
+                c->launches += 2 + (o.test_force_count ? 1 : 0);
+                d->half_known[0] = d->half_known[1] = false;   // the probe's pattern is gone
+                d->filled = false;
+            }
+            const LocateBufs lb{ctr + p, rec + (size_t)p * kLocateRecords, gran + p * lay.gran_words};
+            for (int h = 0; h < 2; ++h) {
+                if (!(P.halves >> h & 1u)) continue;
+                CU_TRY(c, launch_locate(d->plan, half[h], S, h * n, P.seed[h], P.invert, lb, d->scratch_loc,
+                                        &slots[2 * p + h], d->stream));
+                c->launches++;
+                if (std::find(cf_seeds.begin(), cf_seeds.end(), P.seed[h]) == cf_seeds.end()) cf_seeds.push_back(P.seed[h]);
+            }
+        }
+        for (size_t k = 0; k < cf_seeds.size(); ++k) {
+            CU_TRY(c, launch_expected(d->plan, S, Params{ProbeParams{cf_seeds[k], d->nonce_cur}, nullptr}, d->scratch_loc,
+                                      &slots[2 * CRO_LOCATE_PASSES + k], d->stream));
+            c->launches++;
+        }
+        CU_TRY(c, cudaMemcpyAsync(d->h_locate, dl, lay.total, cudaMemcpyDeviceToHost, d->stream));
+        if ((r = wait_stream(c, d))) return r;
+
+        // host side: per-pass counts, the merged word list, and the check that the located words explain each
+        // compared half's checksum exactly
+        const unsigned char* hl = d->h_locate;
+        const LocateCounters* hc = reinterpret_cast<const LocateCounters*>(hl + lay.ctr);
+        const unsigned long long* hg = reinterpret_cast<const unsigned long long*>(hl + lay.gran);
+        const SweepOut* hs = reinterpret_cast<const SweepOut*>(hl + lay.slots);
+        const LocateRecord* hr = reinterpret_cast<const LocateRecord*>(hl + lay.rec);
+        std::map<uint64_t, cro_fault_word> merged;
+        bool complete = true;
+        for (uint32_t p = 0; p < np; ++p) {
+            cro_locate_pass& P = rep->pass[p];
+            P.mismatches = hc[p].mismatches;
+            P.recorded = std::min<uint64_t>(hc[p].claims, kLocateRecords);
+            if (P.recorded != P.mismatches) complete = false;
+            for (int b = 0; b < 64; ++b) rep->bit_flips[b] += hc[p].bits[b];
+            for (uint64_t k = 0; k < lay.gran_words; ++k) P.granules += (uint64_t)__builtin_popcountll(hg[p * lay.gran_words + k]);
+            uint64_t dx[2] = {0, 0}, ds[2] = {0, 0}, dw[2] = {0, 0};
+            for (uint64_t k = 0; k < P.recorded; ++k) {
+                const LocateRecord& R = hr[(size_t)p * kLocateRecords + k];
+                const int h = R.word >= n ? 1 : 0;
+                const uint64_t i = R.word - h * n, delta = R.actual - R.expected;
+                dx[h] ^= R.actual ^ R.expected;
+                ds[h] += delta;
+                dw[h] += delta * (2 * i + 1);
+                auto it = merged.find(R.word);
+                if (it == merged.end()) merged[R.word] = cro_fault_word{R.word, R.expected, R.actual, 1u << p, 0};
+                else it->second.passes |= 1u << p;
+            }
+            for (int h = 0; h < 2; ++h) {
+                if (!(P.halves >> h & 1u)) continue;
+                const SweepOut& s = hs[2 * p + h];
+                P.words_scanned += s.n_words;
+                P.scan_ns += s.t1 - s.t0;
+                P.fold_xor[h] = s.x;
+                P.fold_sum[h] = s.s;
+                P.fold_wsum[h] = s.w;
+                const size_t k = (size_t)(std::find(cf_seeds.begin(), cf_seeds.end(), P.seed[h]) - cf_seeds.begin());
+                SweepOut cf = hs[2 * CRO_LOCATE_PASSES + k];
+                if (P.invert) cf = complement_fold(cf, n);
+                if ((s.x ^ cf.x) != dx[h] || s.s - cf.s != ds[h] || s.w - cf.w != dw[h]) complete = false;
+            }
+        }
+        for (int b = 0; b < 64; ++b)
+            if (rep->bit_flips[b]) rep->flip_or |= 1ull << b;
+        rep->located = merged.size();
+        for (const auto& kv : merged) words->push_back(kv.second);
+        rep->complete = complete ? 1u : 0u;
+        return CRO_OK;
+    }();
+    if (rc) {
+        const uint64_t keep_S = rep->sweep_bytes;
+        memset(rep, 0, sizeof *rep);
+        rep->sweep_bytes = keep_S;
+        words->clear();
+        return rep->status = rc;
+    }
+    rep->verdict = fault_verdict(*rep);
+    bool any = false;
+    for (uint32_t p = 0; p < rep->n_passes; ++p) any |= rep->pass[p].mismatches != 0;
+    return rep->status = any ? CRO_ERR_CHECKSUM : CRO_OK;
 }
 
 // ---------------------------------------------------------------------------
@@ -768,7 +969,11 @@ static int probe_enqueue(cro_ctx* c, Device* d, Lane& L) {
         if (irc) return irc;
     }
     CU_TRY(c, cudaEventRecord(L.ev_done, d->stream));
-    d->filled = true;
+    half_a_filled(d);
+    if (C > 0) {                    // copy 0 wrote the pattern into B; the ping-pong keeps it in both halves
+        d->half_known[1] = true;
+        d->half_seed[1] = d->seed_cur;
+    }
     c->launches += 3 + R + C;       // fill + closed form + sweeps + finalize
     L.events = k;
     L.reads = R;
@@ -1434,6 +1639,7 @@ int ctx_probe_all(cro_ctx* c, cro_probe_result* out, int cap, int* n_out) {
                 if (!pair_ok(pr.first, pr.second)) continue;
                 CU_TRY(c, cudaSetDevice(b->ordinal));
                 if (push) {
+                    b->half_known[1] = false;                        // its prefix now holds a's pattern
                     CU_TRY(c, cudaStreamWaitEvent(b->stream, a->ev_push_done[r], 0));
                     CU_TRY(c, launch_read(b->plan, resolve_read_variant(CRO_READ_AUTO, push_bytes(a, b), c->knobs), b->region + b->sweep_bytes,
                                           push_bytes(a, b), imm_params(b), b->scratch, &b->d_out[kSlotP2P0 + 3 * pr.first + 2], b->stream));

@@ -66,6 +66,15 @@ struct Device {
     uint64_t nonce_cur = 0;            // ... and its nonce
     uint64_t nonce_next = 0;           // nonce the next probe takes
     bool filled = false;
+    // What each half (0 = A, 1 = B) holds, for the fault locator's post-mortem pass: a pattern of seed half_seed[h]
+    // when half_known[h], else nothing it can compare against (never written, a peer's push, a locator retest).
+    bool half_known[2] = {false, false};
+    uint64_t half_seed[2] = {0, 0};
+    // fault locator (ctx_locate): counters, records, granule bitmaps and result slots, allocated at its first call
+    unsigned char* d_locate = nullptr;
+    unsigned char* h_locate = nullptr;     // pinned mirror
+    size_t locate_bytes = 0;
+    SweepScratch scratch_loc{};
     KernelPlan plan{};
     SweepScratch scratch{}, scratch_aux{}, scratch_pfx{};   // main stream / closed form / p2p prefix closed form
     // lane 0's buffers under their old names: the synchronous probe, the single sweeps and cro_probe_all use lane 0
@@ -191,6 +200,11 @@ int ctx_copy(cro_ctx* c, int idx, uint32_t variant, uint32_t iters, cro_sweep_re
 int ctx_expected(cro_ctx* c, int idx, cro_sweep_result* out);
 int ctx_inject(cro_ctx* c, int idx, uint64_t word, uint64_t mask);
 int ctx_read_words(cro_ctx* c, int idx, uint64_t first, uint64_t n, uint64_t* out);
+
+// Fault locator (include/croprobe.h, cro_locate_faults): *words gets every located word, sorted by region index.
+int ctx_locate(cro_ctx* c, int idx, const cro_locate_opts& o, cro_fault_report* rep, std::vector<cro_fault_word>* words);
+// CRO_FAULTS_* of a report, from its per-pass mismatch counts.
+uint32_t fault_verdict(const cro_fault_report& r);
 
 // test hooks (include/croprobe.h, cro_selftest_*): the verdict kernels and the chase on caller-given inputs
 int ctx_selftest_probe_finalize(cro_ctx* c, int idx, const cro_probe_result* tmpl, const cro_sweep_slot* slots,

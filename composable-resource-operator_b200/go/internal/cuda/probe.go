@@ -193,6 +193,77 @@ func (c *Context) ProbeUUID(deviceID string) (r ProbeResult, found bool, err err
 	return convert(&res), true, nil
 }
 
+// FaultReport is the summary of cro_fault_report an operator acts on: detach,
+// retry, or flag the GPU for RMA.
+type FaultReport struct {
+	Verdict     uint32    // CRO_FAULTS_*
+	Complete    bool      // every mismatch is listed and explains the checksums exactly
+	Mismatches  [3]uint64 // per pass: 0 post-mortem, 1 fresh pattern, 2 its complement
+	Granules    [3]uint64 // 2 MiB granules with a mismatch, per pass
+	FlipOr      uint64    // OR of every mismatch's flipped bits
+	RetestSeed  uint64
+	Words       []FaultWord
+	Annotations string // Go-marshalled map[string]string of cohdi.io/probe-fault-* keys
+}
+
+// FaultWord is one located word (cro_fault_word).
+type FaultWord struct {
+	Index    uint64 // region word index: half A first, then half B
+	Expected uint64
+	Actual   uint64
+	Passes   uint32 // bit p: pass p saw it
+}
+
+// LocateFaults runs cro_locate_faults on the in-process device whose UUID is
+// deviceID, typically right after its probe failed with CRO_ERR_CHECKSUM.
+// retest adds the fresh-pattern and complement passes that tell a stuck cell
+// from a one-off error.  A device probed through the helper process has no
+// resident region here and is an error.
+func (c *Context) LocateFaults(deviceID string, retest bool) (FaultReport, error) {
+	var devs [C.CRO_MAX_DEVICES]C.cro_dev_info
+	var n C.int
+	if rc := C.cro_enumerate(c.h, &devs[0], C.CRO_MAX_DEVICES, &n); rc != C.CRO_OK {
+		return FaultReport{}, errorOf(c.h, rc)
+	}
+	idx := C.int(-1)
+	for i := 0; i < int(n); i++ {
+		if C.GoString(&devs[i].gpu_uuid[0]) == deviceID && devs[i].flags&C.CRO_DEV_IN_PROCESS != 0 {
+			idx = C.int(devs[i].dev_index)
+		}
+	}
+	if idx < 0 {
+		return FaultReport{}, fmt.Errorf("cuda fault locator: %s is not a device of this context", deviceID)
+	}
+	var opts C.cro_locate_opts
+	if retest {
+		opts.flags = C.CRO_LOCATE_RETEST
+	}
+	var rep C.cro_fault_report
+	var words [256]C.cro_fault_word
+	var got C.int
+	rc := C.cro_locate_faults(c.h, idx, &opts, &rep, &words[0], 256, &got)
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM {
+		return FaultReport{}, errorOf(c.h, rc)
+	}
+	out := FaultReport{Verdict: uint32(rep.verdict), Complete: rep.complete != 0, FlipOr: uint64(rep.flip_or),
+		RetestSeed: uint64(rep.retest_seed)}
+	for p := 0; p < 3; p++ {
+		out.Mismatches[p] = uint64(rep.pass[p].mismatches)
+		out.Granules[p] = uint64(rep.pass[p].granules)
+	}
+	for i := 0; i < int(got); i++ {
+		w := words[i]
+		out.Words = append(out.Words, FaultWord{uint64(w.word_index), uint64(w.expected), uint64(w.actual), uint32(w.passes)})
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_fault_annotations_json(&rep, &words[0], got, buf, 4096, &ln) == C.CRO_OK {
+		out.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return out, nil
+}
+
 // MetricsText is the Prometheus text exposition of the context's counters and
 // per-GPU gauges; a prometheus.Collector registered with
 // sigs.k8s.io/controller-runtime/pkg/metrics.Registry (cmd/main.go:66,119-125

@@ -415,6 +415,93 @@ int  cro_validate_env(const char *name, const char *value, char *err_buf, size_t
 /* Kernel launches issued by this context so far (bench "gpu_launches"). */
 uint64_t cro_launch_count(cro_ctx *ctx);
 
+/* ---- fault locator: where a failed probe's bad words are ------------------- */
+
+/*
+ * After a probe failed (typically CRO_ERR_CHECKSUM), names the words behind it.  Nothing of the probe changes: the
+ * locator runs only when called.  It takes the device's mutex and lets probes still in flight finish first (their
+ * results stay collectable with cro_probe_end).
+ *
+ * Pass 0 (post-mortem) compares each half of the sweep region, as the last operation left it, with the pattern the
+ * context knows that half holds; it writes nothing.  A half that holds no known pattern is skipped (after
+ * cro_probe_all with the NVLink push leg half B holds a peer's prefix; a probe without copy sweeps leaves half B as it
+ * was).  With CRO_LOCATE_RETEST two more passes follow: pass 1 fills both halves with a fresh pattern (retest seed: the
+ * device seed + 2^63, a seed no probe nonce reaches) and compares, pass 2 does the same with the bitwise complement.
+ * Every bit cell is then written and read back as 0 and as 1, so a stuck-at bit mismatches in exactly one of passes
+ * 1 and 2.  The retest consumes no probe nonce; afterwards both halves hold no known pattern and the single-sweep
+ * entry points refill half A first.
+ *
+ * Word indices are the region's, as for cro_inject_fault / cro_read_words: [0, S/8) half A, [S/8, S/4) half B.
+ * Word i of either half is expected to hold pattern_word(seed, i) (XOR all ones in pass 2).
+ */
+#define CRO_LOCATE_RETEST        0x1u
+#define CRO_LOCATE_RECORDS       4096     /* word records the device keeps per pass; counts stay exact beyond */
+#define CRO_LOCATE_PASSES        3
+#define CRO_LOCATE_GRANULE_BYTES (2u << 20)
+
+#define CRO_FAULTS_NONE           0u      /* no pass found a mismatch                                          */
+#define CRO_FAULTS_UNCLASSIFIED   1u      /* pass 0 found mismatches and no retest ran                          */
+#define CRO_FAULTS_NOT_REPRODUCED 2u      /* pass 0 found mismatches, the retest found none: a transient error, or
+                                             a write that went wrong once                                        */
+#define CRO_FAULTS_PERSISTENT     3u      /* a retest pass found a mismatch: cells that do not hold what is written */
+
+typedef struct cro_locate_opts {
+    uint32_t flags;                /* CRO_LOCATE_*                                                          */
+    uint32_t reserved0;
+    /* test only: after each retest fill, word = (word & test_force_and) | test_force_or for the region words
+       [test_force_first, test_force_first + test_force_count) — a stand-in for stuck cells or a fault storm */
+    uint64_t test_force_first;
+    uint64_t test_force_count;
+    uint64_t test_force_and;
+    uint64_t test_force_or;
+} cro_locate_opts;
+
+typedef struct cro_fault_word {
+    uint64_t word_index;           /* region index                                                          */
+    uint64_t expected;             /* from the first pass that saw the word                                 */
+    uint64_t actual;
+    uint32_t passes;               /* bit p: pass p found the word wrong                                    */
+    uint32_t reserved;
+} cro_fault_word;
+
+typedef struct cro_locate_pass {
+    uint32_t halves;               /*   0  bit h: half h (0 = A, 1 = B) was compared                        */
+    uint32_t skipped;              /*   4  bit h: half h was not compared, it holds no known pattern          */
+    uint64_t seed[2];              /*   8  seed half h was compared against (0 = not compared)                */
+    uint64_t invert;               /*  24  XOR on the pattern: 0, all ones in pass 2                          */
+    uint64_t words_scanned;        /*  32 */
+    uint64_t mismatches;           /*  40  exact                                                             */
+    uint64_t recorded;             /*  48  mismatches the device recorded (<= CRO_LOCATE_RECORDS)            */
+    uint64_t granules;             /*  56  CRO_LOCATE_GRANULE_BYTES granules of the region with a mismatch     */
+    uint64_t scan_ns;              /*  64  %globaltimer windows of the pass's compare sweeps, summed          */
+    uint64_t fold_xor[2];          /*  72  checksum of half h as read (xor, sum, wsum as for a read sweep)    */
+    uint64_t fold_sum[2];          /*  88 */
+    uint64_t fold_wsum[2];         /* 104 */
+} cro_locate_pass;                 /* 120 bytes */
+
+typedef struct cro_fault_report {
+    int32_t  status;               /*   0  the return value: CRO_OK when nothing mismatched, else CRO_ERR_CHECKSUM */
+    uint32_t verdict;              /*   4  CRO_FAULTS_*                                                      */
+    uint32_t n_passes;             /*   8  1, or 3 with CRO_LOCATE_RETEST                                     */
+    uint32_t complete;             /*  12  1: every mismatch of every pass is in the caller's list, and for each
+                                              compared half the located words' deltas reproduce the difference
+                                              between its folded checksum and the half's closed form (xor, sum and
+                                              weighted sum) — the compare path missed nothing the checksum saw     */
+    uint64_t sweep_bytes;          /*  16  S                                                                 */
+    uint64_t retest_seed;          /*  24  0 without CRO_LOCATE_RETEST                                        */
+    uint64_t located;              /*  32  distinct words the device recorded over all passes                 */
+    uint64_t recorded;             /*  40  words written to the caller's list (*n)                             */
+    uint64_t flip_or;              /*  48  OR of every mismatch's actual ^ expected                            */
+    uint64_t bit_flips[64];        /*  56  mismatches (over all passes) with bit b flipped                     */
+    cro_locate_pass pass[CRO_LOCATE_PASSES];   /* 568 */
+} cro_fault_report;                /* 928 bytes */
+
+/* words[0 .. cap) receives the located words sorted by word_index, *n how many were written.  Devices probed through
+ * the helper process (cro_probe_uuid of a GPU attached after init) cannot be located: dev_index is an in-process
+ * device.  opts may be NULL (pass 0 only). */
+int  cro_locate_faults(cro_ctx *ctx, int dev_index, const cro_locate_opts *opts,
+                       cro_fault_report *out, cro_fault_word *words, int cap, int *n);
+
 /* ---- emit: encoding/json-compatible writers ------------------------------ */
 
 /* ComposableResourceStatus (api/v1alpha1/composableresource_types.go:36-41):
@@ -446,6 +533,14 @@ int  cro_emit_sunfish_request(const char *name, long long count, const char *pro
 /* Additive probe annotations (cohdi.io/probe-*), a Go-marshalled
  * map[string]string (keys sorted).  Never mixed into the status bytes. */
 int  cro_emit_probe_annotations_json(const cro_probe_result *r, char *buf, size_t cap, size_t *len);
+
+/* Additive fault annotations (cohdi.io/probe-fault-*) of a cro_locate_faults report, the same Go-marshalled map:
+ * -verdict ("none" | "unclassified" | "not-reproduced" | "persistent", from the report's per-pass counts),
+ * -mismatches and -granules ("<pass>:<count>" per pass run, comma-separated), -bits (flipped bit positions,
+ * ascending; only when a bit flipped) and -words (the first 8 of words[0 .. n) as "<index hex>:<flip mask hex16>";
+ * only when n > 0). */
+int  cro_emit_fault_annotations_json(const cro_fault_report *report, const cro_fault_word *words, int n,
+                                     char *buf, size_t cap, size_t *len);
 
 /* (deviceID, CDIDeviceID) from an FM ScaleUpResponse body, with the
  * res_op_status gate of internal/cdi/fti/fm/client.go:184-213.  On the error
