@@ -183,8 +183,75 @@ class FaultReport(ctypes.Structure):
                 ("bit_flips", ctypes.c_uint64 * 64), ("pass_", LocatePass * LOCATE_PASSES)]
 
 
+# host link probe (cro_probe_host_link, cro_pci_link_path)
+(LINK_LEG_CE_D2H, LINK_LEG_SM_H2D, LINK_LEG_CE_H2D, LINK_LEG_SM_D2H, LINK_LEG_SM_DUPLEX_H2D, LINK_LEG_SM_DUPLEX_D2H,
+ LINK_LEG_CE_DUPLEX_H2D, LINK_LEG_CE_DUPLEX_D2H) = range(8)
+LINK_LEGS = 8
+(LINK_CHECK_D2H_COPY, LINK_CHECK_H2D_COPY, LINK_CHECK_SM_WRITE, LINK_CHECK_DUPLEX_WRITE, LINK_CHECK_DUPLEX_D2H_COPY,
+ LINK_CHECK_CHASE) = range(6)
+LINK_CHECKS, LINK_WORD_CHECKS, LINK_NO_FAIL, LINK_RECORDS = 6, 5, 0xFFFFFFFF, 4096
+LINK_DEGRADED_SPEED, LINK_DEGRADED_WIDTH, LINK_DEGRADED_PATH, LINK_DEGRADED_BOTTLENECK = 1, 2, 4, 8
+PCI_MAX_HOPS = 8
+
+
+class PciHop(ctypes.Structure):
+    """One PCI function on the path: sysfs bdf, current / max link speed (tenths of a GT/s, 0 unknown) and width."""
+    _fields_ = [("bdf", ctypes.c_char * 16), ("cur_speed", ctypes.c_uint32), ("cur_width", ctypes.c_uint32),
+                ("max_speed", ctypes.c_uint32), ("max_width", ctypes.c_uint32)]
+
+
+class PciPath(ctypes.Structure):
+    """cro_pci_path: hop[0] is the device, then each ancestor with link files up to the root bus."""
+    _fields_ = [("numa_node", ctypes.c_int32), ("n_hops", ctypes.c_uint32), ("bottleneck", ctypes.c_uint32),
+                ("truncated", ctypes.c_uint32), ("hop", PciHop * PCI_MAX_HOPS)]
+
+
+class LinkOpts(ctypes.Structure):
+    _fields_ = [("bytes", ctypes.c_uint64), ("hops", ctypes.c_uint32), ("ctas", ctypes.c_uint32),
+                ("test_inject_check", ctypes.c_int32), ("reserved0", ctypes.c_uint32),
+                ("test_inject_word", ctypes.c_uint64), ("test_inject_mask", ctypes.c_uint64)]
+
+
+class LinkFault(ctypes.Structure):
+    """One mismatching word: the check, its index in the buffer that check verified, expected, actual, and the same
+    index of the host buffer involved (equal to actual: the corruption reached host memory)."""
+    _fields_ = [("check", ctypes.c_uint32), ("reserved", ctypes.c_uint32), ("word_index", ctypes.c_uint64),
+                ("expected", ctypes.c_uint64), ("actual", ctypes.c_uint64), ("host_value", ctypes.c_uint64)]
+
+
+class LinkLeg(ctypes.Structure):
+    _fields_ = [("bytes", ctypes.c_uint64), ("ns", ctypes.c_uint64), ("timer_ns", ctypes.c_uint64)]
+
+
+class LinkCheck(ctypes.Structure):
+    _fields_ = [("words", ctypes.c_uint64), ("mismatches", ctypes.c_uint64), ("recorded", ctypes.c_uint64),
+                ("seed", ctypes.c_uint64), ("fold_xor", ctypes.c_uint64), ("fold_sum", ctypes.c_uint64),
+                ("fold_wsum", ctypes.c_uint64), ("expect_xor", ctypes.c_uint64), ("expect_sum", ctypes.c_uint64),
+                ("expect_wsum", ctypes.c_uint64)]
+
+    @property
+    def fold(self) -> Tuple[int, int, int]:
+        return (self.fold_xor, self.fold_sum, self.fold_wsum)
+
+    @property
+    def expect(self) -> Tuple[int, int, int]:
+        return (self.expect_xor, self.expect_sum, self.expect_wsum)
+
+
+class LinkResult(ctypes.Structure):
+    """cro_link_result: legs, checks, chase, path, NUMA placement and replay counters of one host link probe."""
+    _fields_ = [("status", ctypes.c_int32), ("first_fail", ctypes.c_uint32), ("bytes", ctypes.c_uint64),
+                ("seed", ctypes.c_uint64 * 3), ("call", ctypes.c_uint64), ("leg", LinkLeg * LINK_LEGS),
+                ("ce_duplex_span_ns", ctypes.c_uint64), ("check", LinkCheck * LINK_WORD_CHECKS),
+                ("chase_hops", ctypes.c_uint32), ("chase_end", ctypes.c_uint32), ("chase_expect", ctypes.c_uint32),
+                ("chase_minor", ctypes.c_uint32), ("chase_ns", ctypes.c_uint64), ("dev_numa", ctypes.c_int32),
+                ("host_numa", ctypes.c_int32 * 3), ("no_nvml", ctypes.c_uint32), ("degraded", ctypes.c_uint32),
+                ("replays_before", ctypes.c_uint64), ("replays_after", ctypes.c_uint64), ("path", PciPath)]
+
+
 assert ctypes.sizeof(ProbeResult) == 512, ctypes.sizeof(ProbeResult)
 assert ctypes.sizeof(FaultReport) == 928 and ctypes.sizeof(LocatePass) == 120, ctypes.sizeof(FaultReport)
+assert ctypes.sizeof(LinkResult) == 984 and ctypes.sizeof(PciPath) == 272, ctypes.sizeof(LinkResult)
 
 # Every symbol include/croprobe.h declares; tests check the library exports all of them.
 EXPORTS = [
@@ -207,6 +274,7 @@ EXPORTS = [
     "cro_chase_end", "cro_validate_env", "cro_node_inventory", "cro_probe_uuid", "cro_set_latency_hops", "cro_local_exec", "cro_metrics_text", "cro_describe_wire_type",
     "cro_selftest_probe_finalize", "cro_selftest_p2p_finalize", "cro_selftest_chase",
     "cro_locate_faults", "cro_emit_fault_annotations_json",
+    "cro_probe_host_link", "cro_pci_link_path", "cro_emit_link_annotations_json",
 ]
 
 # Slot map of a device's sweep-slot array (cro_sweep_slot, 64 bytes each); the cro_selftest_* hooks take such arrays.
@@ -296,6 +364,10 @@ def _load() -> ctypes.CDLL:
         "cro_locate_faults": (i32, [vp, i32, ctypes.POINTER(LocateOpts), ctypes.POINTER(FaultReport), ctypes.POINTER(FaultWord),
                                     i32, ctypes.POINTER(i32)]),
         "cro_emit_fault_annotations_json": (i32, [ctypes.POINTER(FaultReport), ctypes.POINTER(FaultWord), i32] + out),
+        "cro_probe_host_link": (i32, [vp, i32, ctypes.POINTER(LinkOpts), ctypes.POINTER(LinkResult), ctypes.POINTER(LinkFault),
+                                      i32, ctypes.POINTER(i32)]),
+        "cro_pci_link_path": (i32, [c, c, ctypes.POINTER(PciPath)]),
+        "cro_emit_link_annotations_json": (i32, [ctypes.POINTER(LinkResult)] + out),
         "cro_local_node_op": (i32, [vp, c] + out),
         "cro_local_exec": (i32, [c] + out),
         "cro_describe_wire_type": (i32, [c] + out),
@@ -424,6 +496,20 @@ def emit_fault_annotations_json(report: FaultReport, words: List[FaultWord]) -> 
     """Additive cohdi.io/probe-fault-* annotations of a locate_faults report (Go-marshalled map[string]string)."""
     arr = (FaultWord * max(1, len(words)))(*words)
     return _text(lib.cro_emit_fault_annotations_json, ctypes.byref(report), arr, len(words))
+
+
+def emit_link_annotations_json(r: LinkResult) -> str:
+    """Additive cohdi.io/probe-link-* annotations of a probe_host_link result (Go-marshalled map[string]string)."""
+    return _text(lib.cro_emit_link_annotations_json, ctypes.byref(r))
+
+
+def pci_link_path(bus_id: str, sys_root: Optional[str] = None) -> PciPath:
+    """cro_pci_link_path: the device's PCIe path as sysfs under sys_root (default /sys) describes it.  No GPU needed."""
+    p = PciPath()
+    rc = lib.cro_pci_link_path(_b(sys_root), _b(bus_id), ctypes.byref(p))
+    if rc != OK:
+        raise ProbeError(rc)
+    return p
 
 
 def fm_parse_scale_up_response(body: str, name: str, res_type: str, model: str) -> Tuple[str, str, str]:
@@ -616,6 +702,24 @@ class ProbeContext:
         self._check(lib.cro_locate_faults(self.handle, dev, ctypes.byref(o), ctypes.byref(rep), arr, cap, ctypes.byref(n)),
                     allow=(ERR_CHECKSUM,))
         return rep, [arr[i] for i in range(n.value)]
+
+    def probe_host_link(self, dev: int = 0, bytes: int = 0, hops: int = 0, inject: Optional[Tuple[int, int, int]] = None,
+                        cap: int = 256, ctas: int = 0) -> Tuple[LinkResult, List[LinkFault]]:
+        """cro_probe_host_link: moves fresh patterns over the device's PCIe link in both directions (copy engines and
+        SMs, each direction alone and both at once), checks every byte, chases through host memory and reads the
+        link's path from sysfs.  bytes = 0: min(256 MiB, S); hops = 0: 1024; ctas = 0: the default grid of the SM
+        legs.  inject = (check, word, mask) is the test-only fault.  Returns the result (its status is OK or
+        ERR_CHECKSUM) and up to `cap` mismatching words."""
+        o = LinkOpts()
+        o.bytes, o.hops, o.ctas = bytes, hops, ctas
+        if inject is not None:
+            o.test_inject_check, o.test_inject_word, o.test_inject_mask = inject
+        r = LinkResult()
+        arr = (LinkFault * max(1, cap))()
+        n = ctypes.c_int()
+        self._check(lib.cro_probe_host_link(self.handle, dev, ctypes.byref(o), ctypes.byref(r), arr, cap, ctypes.byref(n)),
+                    allow=(ERR_CHECKSUM,))
+        return r, [arr[i] for i in range(n.value)]
 
     def launch_count(self) -> int:
         return int(lib.cro_launch_count(self.handle))

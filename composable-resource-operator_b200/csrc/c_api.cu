@@ -20,6 +20,7 @@
 #include "env.hpp"
 #include "inventory.hpp"
 #include "gotypes.hpp"
+#include "pcilink.hpp"
 #include <memory>
 #include <new>
 #include <stdexcept>
@@ -42,6 +43,15 @@ static_assert(sizeof(cro_locate_opts) == 40 && sizeof(cro_fault_word) == 32, "lo
 static_assert(sizeof(cro_locate_pass) == 120 && offsetof(cro_locate_pass, fold_xor) == 72, "locator layout");
 static_assert(sizeof(cro_fault_report) == 928 && offsetof(cro_fault_report, bit_flips) == 56 &&
                   offsetof(cro_fault_report, pass) == 568, "locator layout");
+static_assert(sizeof(cro_pci_hop) == 32 && sizeof(cro_pci_path) == 272 && offsetof(cro_pci_path, hop) == 16, "link layout");
+static_assert(sizeof(cro_link_opts) == 40 && sizeof(cro_link_fault) == 40 && sizeof(cro_link_leg) == 24 &&
+                  sizeof(cro_link_check) == 80, "link layout");
+static_assert(sizeof(cro_link_result) == 984 && offsetof(cro_link_result, leg) == 48 &&
+                  offsetof(cro_link_result, ce_duplex_span_ns) == 240 && offsetof(cro_link_result, check) == 248 &&
+                  offsetof(cro_link_result, chase_hops) == 648 && offsetof(cro_link_result, chase_ns) == 664 &&
+                  offsetof(cro_link_result, dev_numa) == 672 && offsetof(cro_link_result, no_nvml) == 688 &&
+                  offsetof(cro_link_result, replays_before) == 696 && offsetof(cro_link_result, path) == 712,
+              "link layout");
 
 using namespace cro::capi;
 
@@ -279,6 +289,23 @@ int cro_locate_faults(cro_ctx* ctx, int i, const cro_locate_opts* opts, cro_faul
     *n = (int)k;
     return rc;
 } CRO_API_CATCH
+int cro_probe_host_link(cro_ctx* ctx, int i, const cro_link_opts* opts, cro_link_result* out, cro_link_fault* faults, int cap,
+                        int* n) try {
+    if (!ctx || !out || !n || cap < 0 || (cap > 0 && !faults)) return CRO_ERR_INVALID_ARG;
+    *n = 0;
+    cro_link_opts o{};
+    if (opts) o = *opts;
+    std::vector<cro_link_fault> found;
+    const int rc = ctx_probe_host_link(ctx, i, o, out, &found);
+    const size_t k = std::min(found.size(), (size_t)cap);
+    for (size_t j = 0; j < k; ++j) faults[j] = found[j];
+    *n = (int)k;
+    return rc;
+} CRO_API_CATCH
+int cro_pci_link_path(const char* sys_root, const char* pci_bus_id, cro_pci_path* out) try {
+    if (!pci_bus_id || !out) return CRO_ERR_INVALID_ARG;
+    return pcilink::ReadPath(sys_root && *sys_root ? sys_root : "/sys", pci_bus_id, out);
+} CRO_API_CATCH
 int cro_device_seed(cro_ctx* ctx, int i, uint64_t* seed) try {
     if (!ctx || !seed || i < 0 || i >= (int)ctx->devs.size()) return CRO_ERR_INVALID_ARG;
     std::lock_guard<std::mutex> g(ctx->devs[(size_t)i]->mu);
@@ -507,6 +534,50 @@ int cro_emit_fault_annotations_json(const cro_fault_report* r, const cro_fault_w
         ws += (k ? "," : "") + std::string(idx) + ":" + hex16(words[k].expected ^ words[k].actual);
     }
     if (!ws.empty()) m["cohdi.io/probe-fault-words"] = ws;
+    gojson::Writer w;
+    w.string_map(m);
+    return copy_out(w.str(), buf, cap, len);
+} CRO_API_CATCH
+
+static std::string link_speed(uint32_t tenths) {
+    if (!tenths) return "unknown";
+    return std::to_string(tenths / 10) + "." + std::to_string(tenths % 10) + "GT/s";
+}
+static std::string mbps(uint64_t bytes, uint64_t ns) {
+    // bytes * 1000 / ns without overflow: 128-bit intermediate
+    return std::to_string(ns ? (uint64_t)((unsigned __int128)bytes * 1000u / ns) : 0ull);
+}
+
+int cro_emit_link_annotations_json(const cro_link_result* r, char* buf, size_t cap, size_t* len) try {
+    if (!r) return CRO_ERR_INVALID_ARG;
+    static const char* const kCheck[CRO_LINK_CHECKS] = {"d2h-copy", "h2d-copy", "sm-write", "duplex-write", "duplex-d2h-copy",
+                                                         "chase"};
+    static const char* const kDegraded[4] = {"speed", "width", "path", "bottleneck"};
+    std::map<std::string, std::string> m;
+    const std::string p = "cohdi.io/probe-link-";
+    m[p + "verdict"] = r->first_fail < CRO_LINK_CHECKS ? std::string("corrupt:") + kCheck[r->first_fail]
+                       : r->status == CRO_OK       ? "ok"
+                                                   : "error";
+    const cro_link_leg* L = r->leg;
+    m[p + "h2d-mbps"] = mbps(L[CRO_LINK_LEG_CE_H2D].bytes, L[CRO_LINK_LEG_CE_H2D].ns);
+    m[p + "d2h-mbps"] = mbps(L[CRO_LINK_LEG_CE_D2H].bytes, L[CRO_LINK_LEG_CE_D2H].ns);
+    m[p + "duplex-mbps"] = mbps(L[CRO_LINK_LEG_CE_DUPLEX_H2D].bytes + L[CRO_LINK_LEG_CE_DUPLEX_D2H].bytes, r->ce_duplex_span_ns);
+    m[p + "sm-h2d-mbps"] = mbps(L[CRO_LINK_LEG_SM_H2D].bytes, L[CRO_LINK_LEG_SM_H2D].ns);
+    m[p + "sm-d2h-mbps"] = mbps(L[CRO_LINK_LEG_SM_D2H].bytes, L[CRO_LINK_LEG_SM_D2H].ns);
+    m[p + "latency-ns"] = std::to_string(r->chase_hops ? r->chase_ns / r->chase_hops : 0ull);
+    const cro_pci_hop& g = r->path.hop[0];
+    m[p + "link"] = link_speed(g.cur_speed) + " x" + std::to_string(g.cur_width) + " / " + link_speed(g.max_speed) + " x" +
+                    std::to_string(g.max_width);
+    if ((r->degraded & CRO_LINK_DEGRADED_BOTTLENECK) && r->path.bottleneck < CRO_PCI_MAX_HOPS) {
+        const cro_pci_hop& b = r->path.hop[r->path.bottleneck];
+        m[p + "bottleneck"] = std::string(b.bdf, strnlen(b.bdf, sizeof b.bdf)) + " " + link_speed(b.cur_speed) + " x" +
+                              std::to_string(b.cur_width);
+    }
+    std::string deg;
+    for (int b = 0; b < 4; ++b)
+        if (r->degraded >> b & 1u) deg += (deg.empty() ? "" : ",") + std::string(kDegraded[b]);
+    if (!deg.empty()) m[p + "degraded"] = deg;
+    if (!r->no_nvml) m[p + "replays"] = std::to_string(r->replays_after - r->replays_before);
     gojson::Writer w;
     w.string_map(m);
     return copy_out(w.str(), buf, cap, len);

@@ -442,5 +442,31 @@ bool NvmlEccUncorrected(const std::string& gpu_uuid, unsigned long long* out) {
     return s.ecc(dev, /*NVML_MEMORY_ERROR_TYPE_UNCORRECTED*/ 1, /*NVML_VOLATILE_ECC*/ 0, out) == 0;
 }
 
+// The same process-wide session for the host link probe's replay counter.
+bool NvmlPcieReplays(const std::string& gpu_uuid, unsigned long long* out) {
+    struct Session {
+        int (*byUuid)(const char*, nvmlDevice_t*) = nullptr;
+        int (*replays)(nvmlDevice_t, unsigned*) = nullptr;
+        bool ok = false;
+    };
+    static Session s;
+    static std::once_flag once;
+    std::call_once(once, [] {
+        void* h = dlopen("libnvidia-ml.so.1", RTLD_NOW | RTLD_LOCAL);
+        if (!h) return;
+        auto init = (int (*)())dlsym(h, "nvmlInit_v2");
+        s.byUuid = (int (*)(const char*, nvmlDevice_t*))dlsym(h, "nvmlDeviceGetHandleByUUID");
+        s.replays = (int (*)(nvmlDevice_t, unsigned*))dlsym(h, "nvmlDeviceGetPcieReplayCounter");
+        s.ok = init && s.byUuid && s.replays && init() == 0;
+    });
+    if (!s.ok) return false;
+    nvmlDevice_t dev = nullptr;
+    if (s.byUuid(gpu_uuid.c_str(), &dev) != 0) return false;
+    unsigned v = 0;
+    if (s.replays(dev, &v) != 0) return false;
+    *out = v;
+    return true;
+}
+
 }  // namespace identity
 }  // namespace cro

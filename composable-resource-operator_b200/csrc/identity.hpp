@@ -85,6 +85,9 @@ bool ScanNvml(std::vector<NvmlGpu>* out, std::string* err);
 // Uncorrected volatile ECC errors of the device since the driver was loaded
 // (nvmlDeviceGetTotalEccErrors); false when NVML or ECC reporting is unavailable.
 bool NvmlEccUncorrected(const std::string& gpu_uuid, unsigned long long* out);
+// PCIe replays of the device's link since the driver was loaded (nvmlDeviceGetPcieReplayCounter); false when NVML or
+// the symbol is missing or the device refuses.
+bool NvmlPcieReplays(const std::string& gpu_uuid, unsigned long long* out);
 
 }  // namespace identity
 }  // namespace cro

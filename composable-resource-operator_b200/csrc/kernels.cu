@@ -11,6 +11,8 @@
 //   hbm_expected      0 bytes           the same checksum from the closed form
 //   hbm_locate        S bytes read      the read sweep's checksum + every word compared with its closed form
 //                                       (the fault locator, cro_locate_faults; not part of the probe)
+//   link_stream       L bytes over PCIe mapped pinned host memory, read (fold + compare) and / or written
+//                                       (the host link probe, cro_probe_host_link; not part of the probe)
 //   chase             pointer chase over peer-resident permutations (latency)
 //   probe_finalize / p2p_finalize       the verdict: the 512-byte result struct is written on the device
 //
@@ -535,6 +537,141 @@ hbm_locate_kernel(const uint4* __restrict__ base, unsigned long long n_vec, unsi
         if (threadIdx.x < 64 && s_bits[threadIdx.x]) atomicAdd(&lb.ctr->bits[threadIdx.x], s_bits[threadIdx.x]);
     }
     publish(acc_x(A) ^ acc_x(B), A.s + B.s, acc_w(A) + acc_w(B), t_start, sc, out, imm, nullptr, 2 * n_vec);
+}
+
+// ---------------------------------------------------------------------------
+// link_stream: the host link probe's SM legs over mapped pinned host memory.
+// Warps [0, rd.warps) of a CTA read (fold + compare, the locator's ballot and
+// warp-aggregated records), warps [rd.warps, rd.warps + wr.warps) write; one
+// launch with both roles keeps both directions of the link busy from the same
+// SMs.  Warp tiles are 32 lanes x 8 vectors (4 KiB): every warp-level access
+// covers 512 contiguous bytes.  Each role's CTA partial and window go through
+// its own scratch; the last CTA of a role publishes the role's slot.
+// ---------------------------------------------------------------------------
+__device__ __forceinline__ void link_publish(const LinkRole& r, unsigned long long x, unsigned long long s,
+                                             unsigned long long w, unsigned long long t0, unsigned long long t1,
+                                             unsigned long long stamp) {
+    const SweepScratch& sc = r.sc;
+    sc.partials[blockIdx.x] = make_ulonglong4(x, s, w, 0ull);
+    atomicMin(sc.tmin, t0);
+    atomicMax(sc.tmax, t1);
+    __threadfence();
+    if (atomicAdd(sc.counter, 1u) != gridDim.x - 1) return;
+    __threadfence();
+    x = 0; s = 0; w = 0;
+    for (unsigned i = 0; i < gridDim.x; ++i) {
+        const ulonglong2* q = reinterpret_cast<const ulonglong2*>(&sc.partials[i]);
+        const ulonglong2 p0 = __ldcg(q), p1 = __ldcg(q + 1);
+        x ^= p0.x; s += p0.y; w += p1.x;
+    }
+    r.out->x = x;
+    r.out->s = s;
+    r.out->w = w;
+    r.out->t0 = *((volatile unsigned long long*)sc.tmin);
+    r.out->t1 = *((volatile unsigned long long*)sc.tmax);
+    r.out->stamp = stamp;
+    r.out->n_words = r.bytes >> 3;
+    *sc.counter = 0u;
+    *sc.tmin = ~0ull;
+    *sc.tmax = 0ull;
+    __threadfence();
+}
+
+__global__ void __launch_bounds__(64 * kLinkWarps)
+link_stream_kernel(const LinkRole rd, const LinkRole wr, LocateBufs lb, unsigned long long stamp) {
+    __shared__ unsigned long long s_bits[64];
+    __shared__ unsigned long long s_count;
+    __shared__ unsigned long long s_x[kLinkWarps], s_s[kLinkWarps], s_w[kLinkWarps];
+    __shared__ unsigned long long s_t0[2], s_t1[2];
+    const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+    for (unsigned i = threadIdx.x; i < 64; i += blockDim.x) s_bits[i] = 0;
+    if (threadIdx.x < 2) { s_t0[threadIdx.x] = ~0ull; s_t1[threadIdx.x] = 0; }
+    if (threadIdx.x == 0) s_count = 0;
+    __syncthreads();
+    const unsigned long long t_start = globaltimer_ns();
+    constexpr unsigned long long tile_vecs = 32 * 8;
+    const bool reader = warp < rd.warps;
+    if (reader) {
+        const uint4* base = static_cast<const uint4*>(rd.buf);
+        const unsigned long long n_vec = rd.bytes >> 4, seed = rd.seed;
+        const LocateCtx L{lb, 0ull, seed, 0ull, s_bits, &s_count};
+        const unsigned long long gw = (unsigned long long)blockIdx.x * rd.warps + warp, nw = (unsigned long long)gridDim.x * rd.warps;
+        const unsigned long long n_tiles = n_vec / tile_vecs;
+        Acc A, B;
+        for (unsigned long long tile = gw; tile < n_tiles; tile += nw) {
+            const unsigned long long v0 = tile * tile_vecs + lane;
+            unsigned long long a[8], b[8];
+            ldg128_x8<32 * 16>(base + v0, a, b);
+            unsigned long long d[16];
+            unsigned m = 0;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const unsigned long long v = v0 + (unsigned long long)j * 32;
+                fold2((j & 1) ? B : A, a[j], b[j], 4 * v + 1);
+                d[2 * j] = a[j] ^ pattern_word(seed, 2 * v);
+                d[2 * j + 1] = b[j] ^ pattern_word(seed, 2 * v + 1);
+                m |= (d[2 * j] != 0 ? 1u : 0u) << (2 * j);
+                m |= (d[2 * j + 1] != 0 ? 1u : 0u) << (2 * j + 1);
+            }
+            if (__ballot_sync(0xffffffffu, m != 0)) locate_record<16>(d, m, v0, 32, L);
+        }
+        // ragged tail: warp-uniform trip count, so the ballot sees the whole warp
+        for (unsigned long long vw = n_tiles * tile_vecs + gw * 32; vw < n_vec; vw += nw * 32) {
+            const unsigned long long v = vw + lane;
+            unsigned long long d[2] = {0, 0};
+            unsigned m = 0;
+            if (v < n_vec) {
+                const uint4 q = ldg_stream(base + v);
+                fold2(A, lo64(q), hi64(q), 4 * v + 1);
+                d[0] = lo64(q) ^ pattern_word(seed, 2 * v);
+                d[1] = hi64(q) ^ pattern_word(seed, 2 * v + 1);
+                m = (d[0] != 0 ? 1u : 0u) | (d[1] != 0 ? 2u : 0u);
+            }
+            if (__ballot_sync(0xffffffffu, m != 0)) locate_record<2>(d, m, v, 0, L);
+        }
+        unsigned long long x = acc_x(A) ^ acc_x(B), s = A.s + B.s, w = acc_w(A) + acc_w(B);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            x ^= __shfl_xor_sync(0xffffffffu, x, o);
+            s += __shfl_xor_sync(0xffffffffu, s, o);
+            w += __shfl_xor_sync(0xffffffffu, w, o);
+        }
+        if (lane == 0) { s_x[warp] = x; s_s[warp] = s; s_w[warp] = w; }
+    } else {
+        uint4* base = static_cast<uint4*>(wr.buf);
+        const unsigned long long n_vec = wr.bytes >> 4, seed = wr.seed;
+        const unsigned long long gw = (unsigned long long)blockIdx.x * wr.warps + (warp - rd.warps),
+                                 nw = (unsigned long long)gridDim.x * wr.warps;
+        const unsigned long long n_tiles = n_vec / tile_vecs;
+        for (unsigned long long tile = gw; tile < n_tiles; tile += nw) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const unsigned long long v = tile * tile_vecs + lane + (unsigned long long)j * 32;
+                const unsigned long long a = pattern_word(seed, 2 * v), b = pattern_word(seed, 2 * v + 1);
+                stg_stream(base + v, make_uint4((unsigned)a, (unsigned)(a >> 32), (unsigned)b, (unsigned)(b >> 32)));
+            }
+        }
+        for (unsigned long long v = n_tiles * tile_vecs + gw * 32 + lane; v < n_vec; v += nw * 32) {
+            const unsigned long long a = pattern_word(seed, 2 * v), b = pattern_word(seed, 2 * v + 1);
+            stg_stream(base + v, make_uint4((unsigned)a, (unsigned)(a >> 32), (unsigned)b, (unsigned)(b >> 32)));
+        }
+    }
+    const unsigned long long t_end = globaltimer_ns();
+    if (lane == 0) {
+        atomicMin(&s_t0[reader ? 0 : 1], t_start);
+        atomicMax(&s_t1[reader ? 0 : 1], t_end);
+    }
+    __syncthreads();
+    if (rd.warps && s_count) {          // CTA-uniform: read after the barrier
+        if (threadIdx.x == 0) atomicAdd(&lb.ctr->mismatches, s_count);
+        if (threadIdx.x < 64 && s_bits[threadIdx.x]) atomicAdd(&lb.ctr->bits[threadIdx.x], s_bits[threadIdx.x]);
+    }
+    if (threadIdx.x == 0 && rd.warps) {
+        unsigned long long x = 0, s = 0, w = 0;
+        for (unsigned k = 0; k < rd.warps; ++k) { x ^= s_x[k]; s += s_s[k]; w += s_w[k]; }
+        link_publish(rd, x, s, w, s_t0[0], s_t1[0], stamp);
+    }
+    if (threadIdx.x == 32 * rd.warps && wr.warps) link_publish(wr, 0, 0, 0, s_t0[1], s_t1[1], stamp);
 }
 
 __global__ void force_words_kernel(unsigned long long* base, unsigned long long first, unsigned long long count,
@@ -1080,6 +1217,8 @@ namespace {
 constexpr int kFillThreads = 512, kFillUnroll = 4;
 constexpr int kReadThreads = 512;
 constexpr int kCopyThreads = 512, kCopyUnroll = 8;
+// Grid of the host link probe's SM legs (8 warps per role and CTA): see DESIGN.md "host link" for the measurement.
+constexpr int kLinkDefaultCtas = 32;
 }  // namespace
 
 cudaError_t plan_kernels(int device, const env::Values& knobs, KernelPlan* plan, std::string* why) {
@@ -1110,6 +1249,7 @@ cudaError_t plan_kernels(int device, const env::Values& knobs, KernelPlan* plan,
     if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, loc, kReadThreads, 0)) != cudaSuccess)
         return e;
     plan->locate = {sms * (occ > 0 ? occ : 1) * (int)knob("CRO_READ_WAVES"), kReadThreads, 0};
+    plan->link_grid = kLinkDefaultCtas;
 
     auto cp = hbm_copy_ldg_kernel<kCopyThreads, kCopyUnroll>;
     if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cp, kCopyThreads, 0)) != cudaSuccess)
@@ -1227,6 +1367,15 @@ cudaError_t launch_force_words(void* base, uint64_t first, uint64_t count, uint6
     const uint64_t blocks = std::min<uint64_t>((count + 255) / 256, (uint64_t)std::max(sm_count, 1) * 8);
     force_words_kernel<<<(unsigned)blocks, 256, 0, st>>>(static_cast<unsigned long long*>(base), first, count, and_mask,
                                                         or_mask);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_link_stream(const LinkRole& rd, const LinkRole& wr, const LocateBufs& lb, int grid, uint64_t stamp,
+                               cudaStream_t st) {
+    if ((rd.warps != 0 && rd.warps != kLinkWarps) || (wr.warps != 0 && wr.warps != kLinkWarps) || !(rd.warps | wr.warps) ||
+        grid < 1)
+        return cudaErrorInvalidValue;
+    link_stream_kernel<<<grid, 32 * (rd.warps + wr.warps), 0, st>>>(rd, wr, lb, stamp);
     return cudaGetLastError();
 }
 

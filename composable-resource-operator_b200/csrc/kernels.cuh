@@ -76,6 +76,7 @@ enum : unsigned { READ_LDG = 1, READ_TMA = 2, READ_LDG256 = 3, COPY_LDG = 1, COP
 // One-time per-device setup (smem carve-outs, occupancy → persistent grid size).
 struct KernelPlan {
     LaunchCfg fill, read_ldg, read_ldg256, read_tma, copy_ldg, copy_tma, copy_fused, expect, locate;
+    int link_grid;                 // default grid of the host link probe's SM legs
     int sm_count;
     // tuning knobs, from the owning context's validated snapshot (see env.hpp)
     unsigned read_tile, read_stages, read_chunk, read_dyn;
@@ -130,6 +131,23 @@ cudaError_t launch_locate(const KernelPlan&, const void* half, uint64_t bytes, u
 // word = (word & and_mask) | or_mask over region words [first, first + count): the locator's test hook.
 cudaError_t launch_force_words(void* base, uint64_t first, uint64_t count, uint64_t and_mask, uint64_t or_mask,
                                int sm_count, cudaStream_t);
+
+// Host link probe (cro_probe_host_link): one launch streams over mapped pinned host memory with two roles, each a
+// number of warps of every CTA (0 warps: the role is off).  The read role folds its buffer like a read sweep and
+// compares every word with pattern_word(seed, i), i the buffer's own word index, counting and recording mismatches as
+// the locator does (LocateBufs, word0 = 0, no granule above L); the write role stores pattern_word(seed, i).  Each role
+// publishes its own SweepOut: %globaltimer window, stamp, n_words, and the fold (read) or a zero checksum (write).
+constexpr int kLinkWarps = 8;                               // warps per role and CTA
+struct LinkRole {
+    void* buf;                                              // device address of the mapped host buffer
+    uint64_t bytes;                                         // multiple of 16
+    uint64_t seed;
+    SweepScratch sc;                                        // the role's own reduction scratch (grid entries)
+    SweepOut* out;
+    unsigned warps;                                         // 0 or kLinkWarps
+};
+cudaError_t launch_link_stream(const LinkRole& rd, const LinkRole& wr, const LocateBufs& lb, int grid, uint64_t stamp,
+                               cudaStream_t);
 
 // Pointer chase for NVLink latency: warp j of the one CTA follows `hops` dependent ld.relaxed.sys loads through
 // table[j] (one 8-byte slot per 128-byte line, peer-resident); out[2j] = final index, out[2j+1] = %globaltimer ns.

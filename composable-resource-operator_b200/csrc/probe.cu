@@ -24,6 +24,7 @@
 #include "env.hpp"
 #include "identity.hpp"
 #include "inventory.hpp"
+#include "pcilink.hpp"
 
 namespace cro {
 
@@ -274,6 +275,8 @@ int ctx_create(const cro_opts* o, cro_ctx** out) {
         c->nvtx = c->knobs.get("CRO_NVTX") != 0;
         if (const char* pr = getenv("CRO_PROC_ROOT"))
             if (*pr) c->proc_root = pr;
+        if (const char* sr = getenv("CRO_SYS_ROOT"))
+            if (*sr) c->sys_root = sr;
     }
 
     phase("options + environment");
@@ -449,6 +452,14 @@ Device::~Device() {
     free_scratch(&scratch_loc);
     cudaFree(d_locate);
     if (h_locate) cudaFreeHost(h_locate);
+    for (int b = 0; b < 2; ++b) {
+        free_scratch(&scratch_link[b]);
+        if (h_link[b]) { cudaHostUnregister(h_link[b]); pcilink::Unmap(h_link[b], link_cap); }
+    }
+    if (h_link_chase) { cudaHostUnregister(h_link_chase); pcilink::Unmap(h_link_chase, (size_t)kChaseSlots * 128); }
+    cudaFree(d_link);
+    if (h_link_out) cudaFreeHost(h_link_out);
+    for (cudaEvent_t e : ev_link) cudaEventDestroy(e);
     for (Lane& L : lanes) {
         cudaFree(L.d_out);
         if (L.h_out) cudaFreeHost(L.h_out);
@@ -831,6 +842,343 @@ int ctx_locate(cro_ctx* c, int idx, const cro_locate_opts& o, cro_fault_report* 
     bool any = false;
     for (uint32_t p = 0; p < rep->n_passes; ++p) any |= rep->pass[p].mismatches != 0;
     return rep->status = any ? CRO_ERR_CHECKSUM : CRO_OK;
+}
+
+// ---------------------------------------------------------------------------
+// host link probe (cro_probe_host_link)
+// ---------------------------------------------------------------------------
+namespace {
+// Pattern j of call k: seed_dev + 2^62 + (3k + j) * kNonceStride.  A probe's seed seed_dev + nonce * kNonceStride equals
+// it only when (nonce - 3k - j) * kNonceStride = 2^62 (mod 2^64); the stride is odd, hence invertible, and 2^62 times
+// an odd number is 2^62 or 3 * 2^62 (mod 2^64), so nonce = 3k + j + 2^62 or + 3 * 2^62: no nonce below 2^62 while
+// 3k + 2 < 2^62.  The locator's retest seed seed_dev + 2^63 would need (3k + j) * kNonceStride = 2^62 (mod 2^64),
+// i.e. 3k + j >= 2^62 by the same argument.  Distinct (k, j) give distinct seeds, so no call passes on the bytes an
+// earlier call left behind.
+constexpr uint64_t kLinkSeedOffset = 1ull << 62;
+constexpr uint64_t kLinkDefaultBytes = 256ull << 20;
+constexpr uint32_t kLinkDefaultHops = 1024;
+constexpr uint32_t kLinkMaxCtas = 4096;
+constexpr int kLinkEvents = 14;
+// d_link slots: [k] the fold of word check k, then the two write roles (SM_D2H, the duplex's), then the closed forms
+// of P1, P2, P3
+constexpr int kLSlotWrite = CRO_LINK_WORD_CHECKS, kLSlotExpect = kLSlotWrite + 2, kLSlots = kLSlotExpect + 3;
+// Per word check: which pattern (0..2 = P1..P3) its buffer must hold, and which host buffer (0 = H0, 1 = H1) it involved.
+constexpr int kCheckPattern[CRO_LINK_WORD_CHECKS] = {0, 0, 1, 2, 0};
+constexpr int kCheckHost[CRO_LINK_WORD_CHECKS] = {0, 0, 1, 0, 1};
+
+// Byte offsets in d_link: counters, granule bitmaps and slots (zeroed per call), records, chase output.
+struct LinkLayout {
+    size_t ctr, gran, slots, zero_bytes, rec, chase, total;
+    uint64_t gran_words;          // bitmap words per check
+};
+LinkLayout link_layout(uint64_t S) {
+    LinkLayout L{};
+    L.gran_words = ((S + CRO_LOCATE_GRANULE_BYTES - 1) / CRO_LOCATE_GRANULE_BYTES + 63) / 64;
+    L.ctr = 0;
+    L.gran = CRO_LINK_WORD_CHECKS * sizeof(LocateCounters);
+    L.slots = (L.gran + CRO_LINK_WORD_CHECKS * L.gran_words * 8 + 63) & ~(size_t)63;
+    L.zero_bytes = L.slots + kLSlots * sizeof(SweepOut);
+    L.rec = L.zero_bytes;
+    L.chase = L.rec + CRO_LINK_WORD_CHECKS * (size_t)kLocateRecords * sizeof(LocateRecord);
+    L.total = L.chase + kChaseOutWords * sizeof(unsigned long long);
+    return L;
+}
+
+// Pinned, mapped host memory of `bytes` on `node` (pcilink::MapOnNode, then cudaHostRegister); nullptr on failure.
+unsigned char* map_pinned(size_t bytes, int node) {
+    void* p = pcilink::MapOnNode(bytes, node);
+    if (!p) return nullptr;
+    if (cudaHostRegister(p, bytes, cudaHostRegisterMapped | cudaHostRegisterPortable) != cudaSuccess) {
+        cudaGetLastError();
+        pcilink::Unmap(p, bytes);
+        return nullptr;
+    }
+    return static_cast<unsigned char*>(p);
+}
+void unmap_pinned(unsigned char*& p, size_t bytes) {
+    if (!p) return;
+    cudaHostUnregister(p);
+    pcilink::Unmap(p, bytes);
+    p = nullptr;
+}
+}  // namespace
+
+int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_result* r, std::vector<cro_link_fault>* faults) {
+    memset(r, 0, sizeof *r);
+    r->first_fail = CRO_LINK_NO_FAIL;
+    r->dev_numa = r->host_numa[0] = r->host_numa[1] = r->host_numa[2] = -1;
+    r->path.numa_node = -1;
+    faults->clear();
+    Device* d = dev_at(c, idx);
+    if (!d) {
+        c->set_error("dev_index " + std::to_string(idx) + " is not a device of this context (a GPU probed through the helper "
+                     "process has no resident region to probe its host link from)");
+        return r->status = CRO_ERR_INVALID_ARG;
+    }
+    std::lock_guard<std::mutex> g(d->mu);
+    drain_pending(c, d);
+    int rc = [&]() -> int {
+        CU_TRY(c, cudaSetDevice(d->ordinal));
+        int e = ensure_region(c, d);
+        if (e) return e;
+        const uint64_t S = d->sweep_bytes;
+        const uint64_t L = o.bytes ? o.bytes : std::min(kLinkDefaultBytes, S);
+        const uint32_t hops = o.hops ? o.hops : kLinkDefaultHops;
+        if (L < 16 || L % 16 || L > S || hops > (1u << 24) || o.ctas > kLinkMaxCtas ||
+            (o.test_inject_mask && (o.test_inject_check < 0 || o.test_inject_check >= CRO_LINK_WORD_CHECKS ||
+                                    o.test_inject_word >= L / 8))) {
+            c->set_error("host link probe: L = " + std::to_string(L) + " must be a multiple of 16 in [16, " + std::to_string(S) +
+                         "], hops at most 2^24, ctas at most " + std::to_string(kLinkMaxCtas) +
+                         ", and an injection must name a word check (0..4) and a word below L / 8");
+            return CRO_ERR_INVALID_ARG;
+        }
+        const int grid = o.ctas ? (int)o.ctas : d->plan.link_grid;
+        const uint64_t n = L / 8;
+        cro_pci_path before_path;
+        // the PCI location as the CUDA driver reports it: the identity sources may not know it (NVML answers "[N/A]"
+        // on some virtualised hosts)
+        char bus_id[32] = {};
+        if (cudaDeviceGetPCIBusId(bus_id, sizeof bus_id, d->ordinal) != cudaSuccess) {
+            cudaGetLastError();
+            snprintf(bus_id, sizeof bus_id, "%s", d->info.pci_bus_id);
+        }
+        const int node = pcilink::ReadPath(c->sys_root, bus_id, &before_path) == CRO_OK ? before_path.numa_node : -1;
+
+        // first call (or a larger L): host buffers, chase table, device-side buffers, events
+        if (d->link_cap < L) {
+            for (unsigned char*& h : d->h_link) unmap_pinned(h, d->link_cap);
+            d->link_cap = 0;
+            for (unsigned char*& h : d->h_link)
+                if (!(h = map_pinned(L, node))) {
+                    for (unsigned char*& q : d->h_link) unmap_pinned(q, L);
+                    c->set_error("host link probe: could not allocate and pin " + std::to_string(L) + " bytes of host memory");
+                    return CRO_ERR_OOM;
+                }
+            d->link_cap = L;
+        }
+        if (!d->h_link_chase) {
+            unsigned char* t = map_pinned((size_t)kChaseSlots * 128, node);
+            if (!t) {
+                c->set_error("host link probe: could not allocate and pin the chase table");
+                return CRO_ERR_OOM;
+            }
+            std::vector<uint32_t> perm;
+            chase_permutation(d->info.device_minor, d->info.device_minor, &perm);
+            d->h_link_chase = reinterpret_cast<unsigned long long*>(t);
+            for (uint32_t i = 0; i < kChaseSlots; ++i) d->h_link_chase[(size_t)i * 16] = perm[i];
+        }
+        const LinkLayout lay = link_layout(S);
+        if (!d->link_bytes) {
+            if (!d->d_link) CU_TRY(c, cudaMalloc(&d->d_link, lay.total));
+            if (!d->h_link_out) CU_TRY(c, cudaMallocHost(&d->h_link_out, lay.total));
+            const int max_grid = std::max({(int)kLinkMaxCtas, d->plan.locate.grid, d->plan.expect.grid, 1});
+            for (SweepScratch& sc : d->scratch_link)
+                if (!sc.partials && (e = alloc_scratch(c, &sc, max_grid))) return e;
+            while (d->ev_link.size() < (size_t)kLinkEvents) {
+                cudaEvent_t ev;
+                CU_TRY(c, cudaEventCreate(&ev));
+                d->ev_link.push_back(ev);
+            }
+            d->link_bytes = lay.total;
+        }
+        unsigned char* H[2] = {d->h_link[0], d->h_link[1]};
+        void* dH[2];
+        for (int b = 0; b < 2; ++b) CU_TRY(c, cudaHostGetDevicePointer(&dH[b], H[b], 0));
+        void* dchase = nullptr;
+        CU_TRY(c, cudaHostGetDevicePointer(&dchase, d->h_link_chase, 0));
+        unsigned char* dl = d->d_link;
+        LocateCounters* ctr = reinterpret_cast<LocateCounters*>(dl + lay.ctr);
+        unsigned long long* gran = reinterpret_cast<unsigned long long*>(dl + lay.gran);
+        SweepOut* slots = reinterpret_cast<SweepOut*>(dl + lay.slots);
+        LocateRecord* rec = reinterpret_cast<LocateRecord*>(dl + lay.rec);
+        unsigned long long* chase_out = reinterpret_cast<unsigned long long*>(dl + lay.chase);
+        auto lb = [&](int k) { return LocateBufs{ctr + k, rec + (size_t)k * kLocateRecords, gran + k * lay.gran_words}; };
+        const std::vector<cudaEvent_t>& ev = d->ev_link;
+        cudaStream_t st = d->stream;
+        unsigned char* A = d->region;
+        unsigned char* B = d->region + S;
+
+        const uint64_t k = d->link_calls++;
+        uint64_t P[3];
+        for (int j = 0; j < 3; ++j) P[j] = d->seed_dev + kLinkSeedOffset + (3 * k + (uint64_t)j) * kNonceStride;
+        r->bytes = L;
+        r->call = k;
+        for (int j = 0; j < 3; ++j) r->seed[j] = P[j];
+        r->chase_hops = hops;
+        r->chase_minor = (uint32_t)d->info.device_minor;
+        const std::string uuid = d->info.gpu_uuid;
+        unsigned long long rp = 0;
+        r->no_nvml = 1;
+        if (!(c->opts.flags & CRO_F_NO_NVML) && identity::NvmlPcieReplays(uuid, &rp)) {
+            r->no_nvml = 0;
+            r->replays_before = rp;
+        }
+
+        const bool inj = o.test_inject_mask != 0;
+        auto inject_host = [&](int check) -> int {      // the CPU flips the pinned word once the leg is done
+            if (!inj || o.test_inject_check != check) return CRO_OK;
+            const int rc2 = wait_stream(c, d);
+            if (rc2) return rc2;
+            reinterpret_cast<volatile uint64_t*>(H[kCheckHost[check]])[o.test_inject_word] ^= o.test_inject_mask;
+            return CRO_OK;
+        };
+        auto inject_b = [&](int check) -> int {
+            if (!inj || o.test_inject_check != check) return CRO_OK;
+            CU_TRY(c, launch_xor_word(B, o.test_inject_word, o.test_inject_mask, st));
+            c->launches++;
+            return CRO_OK;
+        };
+        // Records of the given checks, with the host buffer's word read now: the callers run this once the checks are
+        // done and before a later leg rewrites that buffer.
+        auto harvest = [&](std::initializer_list<int> checks) -> int {
+            CU_TRY(c, cudaMemcpyAsync(d->h_link_out, dl, lay.total, cudaMemcpyDeviceToHost, st));
+            const int rc2 = wait_stream(c, d);
+            if (rc2) return rc2;
+            const LocateCounters* hc = reinterpret_cast<const LocateCounters*>(d->h_link_out + lay.ctr);
+            const LocateRecord* hr = reinterpret_cast<const LocateRecord*>(d->h_link_out + lay.rec);
+            for (int ck : checks) {
+                cro_link_check& C = r->check[ck];
+                C.mismatches = hc[ck].mismatches;
+                C.recorded = std::min<uint64_t>(hc[ck].claims, kLocateRecords);
+                std::vector<cro_link_fault> f;
+                const volatile uint64_t* hb = reinterpret_cast<const volatile uint64_t*>(H[kCheckHost[ck]]);
+                for (uint64_t j = 0; j < C.recorded; ++j) {
+                    const LocateRecord& R = hr[(size_t)ck * kLocateRecords + j];
+                    f.push_back(cro_link_fault{(uint32_t)ck, 0, R.word, R.expected, R.actual, R.word < n ? hb[R.word] : 0});
+                }
+                std::sort(f.begin(), f.end(), [](const cro_link_fault& a, const cro_link_fault& b) { return a.word_index < b.word_index; });
+                faults->insert(faults->end(), f.begin(), f.end());
+            }
+            return CRO_OK;
+        };
+        auto role = [&](void* buf, int pat, int scratch, SweepOut* out) {
+            return LinkRole{buf, L, P[pat], d->scratch_link[scratch], out, (unsigned)kLinkWarps};
+        };
+        const LinkRole off{nullptr, 0, 0, SweepScratch{}, nullptr, 0};
+
+        CU_TRY(c, cudaMemsetAsync(dl, 0, lay.zero_bytes, st));
+        // A[0, L) <- P1, and the closed forms of P1..P3 over L
+        CU_TRY(c, launch_fill(d->plan, A, L, Params{ProbeParams{P[0], k}, nullptr}, d->scratch_link[0], nullptr, st));
+        d->half_known[0] = d->half_known[1] = false;      // both halves now hold the link probe's patterns
+        d->filled = false;
+        for (int j = 0; j < 3; ++j)
+            CU_TRY(c, launch_expected(d->plan, L, Params{ProbeParams{P[j], k}, nullptr}, d->scratch_link[0],
+                                      &slots[kLSlotExpect + j], st));
+        c->launches += 4;
+        // CE d2h, then the SMs read H0 (check 0)
+        CU_TRY(c, cudaEventRecord(ev[0], st));
+        CU_TRY(c, cudaMemcpyAsync(H[0], A, L, cudaMemcpyDeviceToHost, st));
+        CU_TRY(c, cudaEventRecord(ev[1], st));
+        if ((e = inject_host(CRO_LINK_CHECK_D2H_COPY))) return e;
+        CU_TRY(c, cudaEventRecord(ev[2], st));
+        CU_TRY(c, launch_link_stream(role(dH[0], 0, 0, &slots[0]), off, lb(0), grid, k, st));
+        CU_TRY(c, cudaEventRecord(ev[3], st));
+        // CE h2d H0 -> B, checked in HBM (check 1)
+        CU_TRY(c, cudaEventRecord(ev[4], st));
+        CU_TRY(c, cudaMemcpyAsync(B, H[0], L, cudaMemcpyHostToDevice, st));
+        CU_TRY(c, cudaEventRecord(ev[5], st));
+        if ((e = inject_b(CRO_LINK_CHECK_H2D_COPY))) return e;
+        CU_TRY(c, launch_locate(d->plan, B, L, 0, P[0], 0, lb(1), d->scratch_link[0], &slots[1], st));
+        c->launches += 2;
+        if ((e = harvest({0, 1}))) return e;              // before the duplex launch rewrites H0
+        // SMs write P2 into H1
+        CU_TRY(c, cudaEventRecord(ev[6], st));
+        CU_TRY(c, launch_link_stream(off, role(dH[1], 1, 1, &slots[kLSlotWrite]), lb(2), grid, k, st));
+        CU_TRY(c, cudaEventRecord(ev[7], st));
+        if ((e = inject_host(CRO_LINK_CHECK_SM_WRITE))) return e;
+        // SM duplex: read H1 against P2 (check 2) and write P3 into H0, one launch
+        CU_TRY(c, cudaEventRecord(ev[8], st));
+        CU_TRY(c, launch_link_stream(role(dH[1], 1, 0, &slots[2]), role(dH[0], 2, 1, &slots[kLSlotWrite + 1]), lb(2), grid,
+                                     k, st));
+        CU_TRY(c, cudaEventRecord(ev[9], st));
+        c->launches += 2;
+        if ((e = harvest({2}))) return e;                 // before the CE duplex rewrites H1
+        // CE duplex: H0 -> B on the device stream and A -> H1 on aux, at once
+        CU_TRY(c, cudaEventRecord(ev[10], st));
+        CU_TRY(c, cudaStreamWaitEvent(d->aux, ev[10], 0));
+        CU_TRY(c, cudaMemcpyAsync(B, H[0], L, cudaMemcpyHostToDevice, st));
+        CU_TRY(c, cudaEventRecord(ev[11], st));
+        CU_TRY(c, cudaEventRecord(ev[12], d->aux));
+        CU_TRY(c, cudaMemcpyAsync(H[1], A, L, cudaMemcpyDeviceToHost, d->aux));
+        CU_TRY(c, cudaEventRecord(ev[13], d->aux));
+        CU_TRY(c, cudaStreamWaitEvent(st, ev[13], 0));
+        // an idle GPU trains its link down: sample the path while both copies are in flight
+        if (pcilink::ReadPath(c->sys_root, bus_id, &r->path) == CRO_OK) {
+            r->dev_numa = r->path.numa_node;
+            r->degraded = pcilink::Degraded(r->path);
+        }
+        if ((e = wait_stream(c, d))) return e;
+        if ((e = inject_b(CRO_LINK_CHECK_DUPLEX_WRITE))) return e;
+        if ((e = inject_host(CRO_LINK_CHECK_DUPLEX_D2H_COPY))) return e;
+        // check 3: B against P3; check 4: the SMs read H1 against P1 (verification only, untimed)
+        CU_TRY(c, launch_locate(d->plan, B, L, 0, P[2], 0, lb(3), d->scratch_link[0], &slots[3], st));
+        CU_TRY(c, launch_link_stream(role(dH[1], 0, 0, &slots[4]), off, lb(4), grid, k, st));
+        // latency: one warp chases the self pair's permutation through host memory (check 5)
+        ChaseArgs ca{};
+        ca.n = 1;
+        ca.hops = hops;
+        ca.table[0] = static_cast<const unsigned long long*>(dchase);
+        CU_TRY(c, arm_chase_out(chase_out, st));
+        CU_TRY(c, launch_chase(ca, chase_out, st));
+        c->launches += 3;
+        if ((e = harvest({3, 4}))) return e;
+        if (!r->no_nvml && identity::NvmlPcieReplays(uuid, &rp)) r->replays_after = rp;
+        else if (!r->no_nvml) { r->no_nvml = 1; r->replays_before = 0; }
+
+        auto span = [&](int a, int b) -> uint64_t {
+            float ms = 0;
+            return cudaEventElapsedTime(&ms, ev[(size_t)a], ev[(size_t)b]) == cudaSuccess ? ms_to_ns(ms) : 0;
+        };
+        const SweepOut* hs = reinterpret_cast<const SweepOut*>(d->h_link_out + lay.slots);
+        auto window = [](const SweepOut& s) -> uint64_t { return s.t1 > s.t0 ? s.t1 - s.t0 : 0; };
+        const int ev_of[CRO_LINK_LEGS][2] = {{0, 1}, {2, 3}, {4, 5}, {6, 7}, {8, 9}, {8, 9}, {10, 11}, {12, 13}};
+        const SweepOut* timer_of[CRO_LINK_LEGS] = {nullptr, &hs[0], nullptr, &hs[kLSlotWrite], &hs[2], &hs[kLSlotWrite + 1],
+                                                   nullptr, nullptr};
+        for (int lg = 0; lg < CRO_LINK_LEGS; ++lg) {
+            r->leg[lg].bytes = L;
+            r->leg[lg].ns = span(ev_of[lg][0], ev_of[lg][1]);
+            r->leg[lg].timer_ns = timer_of[lg] ? window(*timer_of[lg]) : 0;
+        }
+        r->ce_duplex_span_ns = std::max(span(10, 11), span(10, 13));
+        for (int ck = 0; ck < CRO_LINK_WORD_CHECKS; ++ck) {
+            cro_link_check& C = r->check[ck];
+            const SweepOut& s = hs[ck];
+            const SweepOut& cf = hs[kLSlotExpect + kCheckPattern[ck]];
+            C.words = n;
+            C.seed = P[kCheckPattern[ck]];
+            C.fold_xor = s.x;
+            C.fold_sum = s.s;
+            C.fold_wsum = s.w;
+            C.expect_xor = cf.x;
+            C.expect_sum = cf.s;
+            C.expect_wsum = cf.w;
+            const bool bad = C.mismatches != 0 || s.n_words != n || cf.n_words != n || s.x != cf.x || s.s != cf.s || s.w != cf.w;
+            if (bad && r->first_fail == CRO_LINK_NO_FAIL) r->first_fail = (uint32_t)ck;
+        }
+        const unsigned long long* hco = reinterpret_cast<const unsigned long long*>(d->h_link_out + lay.chase);
+        std::vector<uint32_t> perm;
+        chase_permutation(d->info.device_minor, d->info.device_minor, &perm);
+        uint32_t at = 0;
+        for (uint32_t h = 0; h < hops; ++h) at = perm[at];
+        r->chase_expect = at;
+        r->chase_end = (uint32_t)hco[0];
+        r->chase_ns = hco[0] == kChaseArmed ? 0 : hco[1];
+        if (hco[0] != at && r->first_fail == CRO_LINK_NO_FAIL) r->first_fail = CRO_LINK_CHECK_CHASE;
+        for (int b = 0; b < 2; ++b) r->host_numa[b] = pcilink::NodeOf(H[b]);
+        r->host_numa[2] = pcilink::NodeOf(d->h_link_chase);
+        return CRO_OK;
+    }();
+    if (rc) {
+        const uint64_t keep_L = r->bytes;
+        memset(r, 0, sizeof *r);
+        r->bytes = keep_L;
+        r->first_fail = CRO_LINK_NO_FAIL;
+        r->dev_numa = r->host_numa[0] = r->host_numa[1] = r->host_numa[2] = -1;
+        r->path.numa_node = -1;
+        faults->clear();
+        return r->status = rc;
+    }
+    return r->status = r->first_fail == CRO_LINK_NO_FAIL ? CRO_OK : CRO_ERR_CHECKSUM;
 }
 
 // ---------------------------------------------------------------------------

@@ -75,6 +75,18 @@ struct Device {
     unsigned char* h_locate = nullptr;     // pinned mirror
     size_t locate_bytes = 0;
     SweepScratch scratch_loc{};
+    // host link probe (ctx_probe_host_link), allocated at its first call: pinned host buffers H0 and H1 (link_cap bytes
+    // each, mapped into the device's address space) and the 8 MiB chase table, all from pcilink::MapOnNode; the
+    // device-side counters, records and slots; two role scratches; timing events
+    unsigned char* h_link[2] = {nullptr, nullptr};
+    uint64_t link_cap = 0;
+    unsigned long long* h_link_chase = nullptr;
+    unsigned char* d_link = nullptr;
+    unsigned char* h_link_out = nullptr;   // pinned mirror of d_link
+    size_t link_bytes = 0;
+    SweepScratch scratch_link[2]{};
+    std::vector<cudaEvent_t> ev_link;
+    uint64_t link_calls = 0;               // k of the next call: its seeds
     KernelPlan plan{};
     SweepScratch scratch{}, scratch_aux{}, scratch_pfx{};   // main stream / closed form / p2p prefix closed form
     // lane 0's buffers under their old names: the synchronous probe, the single sweeps and cro_probe_all use lane 0
@@ -143,6 +155,7 @@ struct cro_ctx {
     // the CRO_* knobs as validated by cro_probe_init: everything the context plans and probes with reads these
     cro::env::Values knobs;
     std::string proc_root = "/proc";   // where the node's /proc is mounted (tests point it at a fake tree)
+    std::string sys_root = "/sys";     // where the node's sysfs is mounted (CRO_SYS_ROOT): the host link probe's path
     // the node's inventory as of the last enumeration (inventory.hpp)
     std::mutex inv_mu;
     std::string inv_key;               // uuid/minor set the cached list was built from
@@ -205,6 +218,9 @@ int ctx_read_words(cro_ctx* c, int idx, uint64_t first, uint64_t n, uint64_t* ou
 int ctx_locate(cro_ctx* c, int idx, const cro_locate_opts& o, cro_fault_report* rep, std::vector<cro_fault_word>* words);
 // CRO_FAULTS_* of a report, from its per-pass mismatch counts.
 uint32_t fault_verdict(const cro_fault_report& r);
+
+// Host link probe (include/croprobe.h, cro_probe_host_link): *faults gets every recorded mismatch, by check, then index.
+int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_result* r, std::vector<cro_link_fault>* faults);
 
 // test hooks (include/croprobe.h, cro_selftest_*): the verdict kernels and the chase on caller-given inputs
 int ctx_selftest_probe_finalize(cro_ctx* c, int idx, const cro_probe_result* tmpl, const cro_sweep_slot* slots,

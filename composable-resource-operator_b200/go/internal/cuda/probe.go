@@ -264,6 +264,79 @@ func (c *Context) LocateFaults(deviceID string, retest bool) (FaultReport, error
 	return out, nil
 }
 
+// LinkResult is the summary of cro_link_result an operator reads after
+// composing a GPU: whether every byte crossed the PCIe link intact, at what
+// rates, and how the link trained.
+type LinkResult struct {
+	OK          bool
+	FirstFail   uint32            // CRO_LINK_CHECK_*, CRO_LINK_NO_FAIL when every check passed
+	Bytes       uint64            // L
+	LegBytes    [8]uint64         // per CRO_LINK_LEG_*
+	LegNs       [8]uint64         // CUDA events around each leg
+	DuplexNs    uint64            // span of the copy-engine duplex leg
+	ChaseNs     uint64            // chase through host memory, all hops
+	ChaseHops   uint32
+	Degraded    uint32            // CRO_LINK_DEGRADED_*
+	Faults      []LinkFault
+	Annotations string // Go-marshalled map[string]string of cohdi.io/probe-link-* keys
+}
+
+// LinkFault is one mismatching word (cro_link_fault).
+type LinkFault struct {
+	Check     uint32
+	Index     uint64 // word index in the buffer the check verified
+	Expected  uint64
+	Actual    uint64
+	HostValue uint64 // the host buffer's word: equal to Actual, the corruption reached host memory
+}
+
+// ProbeHostLink runs cro_probe_host_link with its defaults on the in-process
+// device whose UUID is deviceID, typically once after a passing HBM probe of a
+// freshly composed GPU.  A device probed through the helper process is an
+// error, as for LocateFaults.
+func (c *Context) ProbeHostLink(deviceID string) (LinkResult, error) {
+	var devs [C.CRO_MAX_DEVICES]C.cro_dev_info
+	var n C.int
+	if rc := C.cro_enumerate(c.h, &devs[0], C.CRO_MAX_DEVICES, &n); rc != C.CRO_OK {
+		return LinkResult{}, errorOf(c.h, rc)
+	}
+	idx := C.int(-1)
+	for i := 0; i < int(n); i++ {
+		if C.GoString(&devs[i].gpu_uuid[0]) == deviceID && devs[i].flags&C.CRO_DEV_IN_PROCESS != 0 {
+			idx = C.int(devs[i].dev_index)
+		}
+	}
+	if idx < 0 {
+		return LinkResult{}, fmt.Errorf("cuda host link probe: %s is not a device of this context", deviceID)
+	}
+	var res C.cro_link_result
+	var faults [256]C.cro_link_fault
+	var got C.int
+	rc := C.cro_probe_host_link(c.h, idx, nil, &res, &faults[0], 256, &got)
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM {
+		return LinkResult{}, errorOf(c.h, rc)
+	}
+	out := LinkResult{OK: rc == C.CRO_OK, FirstFail: uint32(res.first_fail), Bytes: uint64(res.bytes),
+		DuplexNs: uint64(res.ce_duplex_span_ns), ChaseNs: uint64(res.chase_ns), ChaseHops: uint32(res.chase_hops),
+		Degraded: uint32(res.degraded)}
+	for g := 0; g < int(C.CRO_LINK_LEGS); g++ {
+		out.LegBytes[g] = uint64(res.leg[g].bytes)
+		out.LegNs[g] = uint64(res.leg[g].ns)
+	}
+	for i := 0; i < int(got); i++ {
+		f := faults[i]
+		out.Faults = append(out.Faults, LinkFault{uint32(f.check), uint64(f.word_index), uint64(f.expected), uint64(f.actual),
+			uint64(f.host_value)})
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_link_annotations_json(&res, buf, 4096, &ln) == C.CRO_OK {
+		out.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return out, nil
+}
+
 // MetricsText is the Prometheus text exposition of the context's counters and
 // per-GPU gauges; a prometheus.Collector registered with
 // sigs.k8s.io/controller-runtime/pkg/metrics.Registry (cmd/main.go:66,119-125

@@ -502,6 +502,162 @@ typedef struct cro_fault_report {
 int  cro_locate_faults(cro_ctx *ctx, int dev_index, const cro_locate_opts *opts,
                        cro_fault_report *out, cro_fault_word *words, int cap, int *n);
 
+/* ---- host link: the PCIe path between the host and a composed GPU ------------ */
+
+/*
+ * The PCIe path a fabric composes is the one part of an attached GPU the HBM probe never exercises.  The link probe
+ * moves a fresh pattern across it in both directions, with the copy engines and with the SMs (loads and stores to
+ * mapped pinned host memory), each direction alone and both at once, checks every byte that crossed, times a
+ * dependent pointer chase through host memory, and reads the link's trained speed and width, and those of every hop
+ * above it, from sysfs.  It runs only when called and changes nothing of the probe.
+ *
+ * The call takes the device's mutex and lets probes still in flight finish first (their results stay collectable with
+ * cro_probe_end).  It uses the first L bytes of the sweep region's half A and half B and allocates no device memory
+ * beyond a few small result buffers; on its first call it allocates two pinned host buffers H0, H1 of L bytes (grown
+ * when a later call asks for more) and an 8 MiB chase table, placed on the device's NUMA node when sysfs names one.
+ * Afterwards neither half holds a known pattern: the next single sweep refills half A, and cro_locate_faults' pass 0
+ * skips both halves.
+ *
+ * Three fresh patterns per call (P1, P2, P3 of seed[]), and each step's bytes are checked by a later step:
+ *   leg CE_D2H          copy engine A -> H0 (A filled with P1)          checked by check 0
+ *   leg SM_H2D          SMs read H0 over the link                        = check 0 (H0 against P1)
+ *   leg CE_H2D          copy engine H0 -> B                              check 1 (B[0, L) against P1)
+ *   leg SM_D2H          SMs write P2 into H1                             check 2
+ *   legs SM_DUPLEX_*    one launch: SMs read H1 (= check 2, against P2) and write P3 into H0 at once
+ *   legs CE_DUPLEX_*    copy engines H0 -> B and A -> H1 at once         check 3 (B against P3), check 4 (H1 against P1)
+ *   leg  latency        chase through the host-resident table            check 5 (end slot)
+ * An injected fault (test_inject_*) of check 0 sits in H0 and therefore also reaches check 1 (B is copied from H0);
+ * one of checks 1 to 4 reaches only that check.
+ */
+#define CRO_LINK_LEG_CE_D2H         0
+#define CRO_LINK_LEG_SM_H2D         1
+#define CRO_LINK_LEG_CE_H2D         2
+#define CRO_LINK_LEG_SM_D2H         3
+#define CRO_LINK_LEG_SM_DUPLEX_H2D  4
+#define CRO_LINK_LEG_SM_DUPLEX_D2H  5
+#define CRO_LINK_LEG_CE_DUPLEX_H2D  6
+#define CRO_LINK_LEG_CE_DUPLEX_D2H  7
+#define CRO_LINK_LEGS               8
+
+#define CRO_LINK_CHECK_D2H_COPY        0   /* H0 (CE copy of A) read by the SMs, against P1              */
+#define CRO_LINK_CHECK_H2D_COPY        1   /* B[0, L) (CE copy of H0) against P1                         */
+#define CRO_LINK_CHECK_SM_WRITE        2   /* H1 (SM stores) read by the duplex launch, against P2       */
+#define CRO_LINK_CHECK_DUPLEX_WRITE    3   /* B[0, L) (duplex SM stores to H0, then CE H0 -> B) against P3 */
+#define CRO_LINK_CHECK_DUPLEX_D2H_COPY 4   /* H1 (CE copy of A during the CE duplex) read by the SMs, P1 */
+#define CRO_LINK_CHECK_CHASE           5   /* the chase ended on the slot the host walk names            */
+#define CRO_LINK_CHECKS                6
+#define CRO_LINK_WORD_CHECKS           5   /* checks 0..4 compare words                                  */
+#define CRO_LINK_NO_FAIL               0xFFFFFFFFu
+#define CRO_LINK_RECORDS               CRO_LOCATE_RECORDS   /* word records the device keeps per check     */
+
+/* degraded: reported, never changes the status */
+#define CRO_LINK_DEGRADED_SPEED       0x1u  /* the GPU's link runs below its max speed                    */
+#define CRO_LINK_DEGRADED_WIDTH       0x2u  /* the GPU's link runs below its max width                    */
+#define CRO_LINK_DEGRADED_PATH        0x4u  /* a hop above the GPU runs below its own max speed or width  */
+#define CRO_LINK_DEGRADED_BOTTLENECK  0x8u  /* a hop above the GPU is slower (speed x width) than its link */
+
+#define CRO_PCI_MAX_HOPS 8
+
+typedef struct cro_pci_hop {
+    char     bdf[16];              /*   0  sysfs spelling "0000:1f:00.0"                                    */
+    uint32_t cur_speed;            /*  16  tenths of a GT/s (320 = 32.0 GT/s); 0: "Unknown" or no file       */
+    uint32_t cur_width;            /*  20  lanes; 0: no file                                                */
+    uint32_t max_speed;            /*  24 */
+    uint32_t max_width;            /*  28 */
+} cro_pci_hop;                     /* 32 bytes */
+
+typedef struct cro_pci_path {
+    int32_t  numa_node;            /*   0  the device's numa_node (-1: none, or no file)                     */
+    uint32_t n_hops;               /*   4  entries of hop[]: the device, then each ancestor that is a PCI
+                                              function with link files, up to the root bus                     */
+    uint32_t bottleneck;           /*   8  index in hop[] of the least cur_speed * cur_width among hops whose
+                                              speed and width are known (the lowest such index on a tie; 0 when
+                                              none is known)                                                  */
+    uint32_t truncated;            /*  12  1: the path had more than CRO_PCI_MAX_HOPS hops                     */
+    cro_pci_hop hop[CRO_PCI_MAX_HOPS];   /* 16 */
+} cro_pci_path;                    /* 272 bytes */
+
+typedef struct cro_link_opts {
+    uint64_t bytes;                /*   0  L: 0 = min(256 MiB, S); else a multiple of 16 with 16 <= L <= S     */
+    uint32_t hops;                 /*   8  chase length: 0 = 1024, at most 2^24                                */
+    uint32_t ctas;                 /*  12  grid of the SM legs: 0 = the default (DESIGN.md "host link")        */
+    /* test only: with test_inject_mask != 0, word test_inject_word of the buffer check test_inject_check (0..4)
+       verifies is XORed with the mask after that check's leg and before the check runs */
+    int32_t  test_inject_check;    /*  16 */
+    uint32_t reserved0;            /*  20 */
+    uint64_t test_inject_word;     /*  24 */
+    uint64_t test_inject_mask;     /*  32 */
+} cro_link_opts;                   /* 40 bytes */
+
+typedef struct cro_link_fault {
+    uint32_t check;                /*   0  CRO_LINK_CHECK_*                                                  */
+    uint32_t reserved;             /*   4 */
+    uint64_t word_index;           /*   8  index in the buffer the check verified (word 0 = its first word)   */
+    uint64_t expected;             /*  16 */
+    uint64_t actual;               /*  24 */
+    uint64_t host_value;           /*  32  word_index of the host buffer involved (see cro_probe_host_link)   */
+} cro_link_fault;                  /* 40 bytes */
+
+typedef struct cro_link_leg {
+    uint64_t bytes;                /*   0  bytes the leg moved (L)                                           */
+    uint64_t ns;                   /*   8  CUDA events around the leg (both duplex SM legs: the one launch)    */
+    uint64_t timer_ns;             /*  16  SM legs: the role's own %globaltimer window; 0 for copy engines     */
+} cro_link_leg;                    /* 24 bytes */
+
+typedef struct cro_link_check {
+    uint64_t words;                /*   0  words compared (L / 8)                                            */
+    uint64_t mismatches;           /*   8  exact                                                            */
+    uint64_t recorded;             /*  16  mismatches the device recorded (<= CRO_LINK_RECORDS)              */
+    uint64_t seed;                 /*  24  pattern the buffer must hold: word i = pattern_word(seed, i)       */
+    uint64_t fold_xor;             /*  32  the buffer as read: xor, sum, weighted sum as for a read sweep     */
+    uint64_t fold_sum;             /*  40 */
+    uint64_t fold_wsum;            /*  48 */
+    uint64_t expect_xor;           /*  56  closed form of the pattern over the same words                    */
+    uint64_t expect_sum;           /*  64 */
+    uint64_t expect_wsum;          /*  72 */
+} cro_link_check;                  /* 80 bytes */
+
+typedef struct cro_link_result {
+    int32_t  status;               /*   0  the return value                                                  */
+    uint32_t first_fail;           /*   4  lowest failing CRO_LINK_CHECK_*, or CRO_LINK_NO_FAIL               */
+    uint64_t bytes;                /*   8  L                                                                 */
+    uint64_t seed[3];              /*  16  P1, P2, P3: seed_dev + 2^62 + (3k + j) * 0xD1B54A32D192ED03         */
+    uint64_t call;                 /*  40  k: the call's number on this device, from 0                       */
+    cro_link_leg leg[CRO_LINK_LEGS];   /* 48  CRO_LINK_LEG_*                                                */
+    uint64_t ce_duplex_span_ns;    /* 240  first CE duplex start .. last CE duplex end (CUDA events)          */
+    cro_link_check check[CRO_LINK_WORD_CHECKS];   /* 248 */
+    uint32_t chase_hops;           /* 648 */
+    uint32_t chase_end;            /* 652  slot the chase ended on                                         */
+    uint32_t chase_expect;         /* 656  slot the host walk of the same permutation ends on               */
+    uint32_t chase_minor;          /* 660  the table is the self pair (minor, minor) of cro_chase_end        */
+    uint64_t chase_ns;             /* 664  the chase kernel's %globaltimer window                           */
+    int32_t  dev_numa;             /* 672  path.numa_node                                                   */
+    int32_t  host_numa[3];         /* 676  node the pages of H0, H1, the chase table landed on (first page;
+                                              -1: unknown, e.g. a seccomp profile refuses get_mempolicy)       */
+    uint32_t no_nvml;              /* 688  1: replay counters not read (CRO_F_NO_NVML, or NVML / the symbol is
+                                              missing, or the device refused)                                  */
+    uint32_t degraded;             /* 692  CRO_LINK_DEGRADED_*, from path                                     */
+    uint64_t replays_before;       /* 696  nvmlDeviceGetPcieReplayCounter before the legs and after them       */
+    uint64_t replays_after;        /* 704 */
+    cro_pci_path path;             /* 712  sampled while the CE duplex leg was in flight (an idle GPU lowers its
+                                              link speed)                                                      */
+} cro_link_result;                 /* 984 bytes */
+
+/* faults[0 .. cap) receives the mismatching words (by check, then word index), *n how many were written.
+ * host_value is the same index of the host buffer the check involved (H0 for checks 0, 1, 3; H1 for checks 2, 4),
+ * read by the CPU once the check ran and before any later leg rewrote that buffer: equal to actual, the corruption
+ * reached host memory; equal to expected, it happened on the device side of the transfer.
+ * CRO_OK: every check passed; CRO_ERR_CHECKSUM: a check mismatched (a chase that ended on the wrong slot included).
+ * dev_index must be an in-process device (as for cro_locate_faults).  opts may be NULL: defaults. */
+int  cro_probe_host_link(cro_ctx *ctx, int dev_index, const cro_link_opts *opts,
+                         cro_link_result *out, cro_link_fault *faults, int cap, int *n);
+
+/* The PCIe path of pci_bus_id ("00000000:1F:00.0" or "0000:1f:00.0") under sys_root (NULL: "/sys"), from
+ * <sys_root>/bus/pci/devices/<bdf>: current / max link speed and width and numa_node of the device and of every
+ * ancestor on its real path that has link files.  Reads sysfs only; no context, no CUDA.  CRO_ERR_INVALID_ARG: a bus
+ * id that parses as neither spelling; CRO_ERR_NO_DEVICE: no such device under sys_root. */
+int  cro_pci_link_path(const char *sys_root, const char *pci_bus_id, cro_pci_path *out);
+
 /* ---- emit: encoding/json-compatible writers ------------------------------ */
 
 /* ComposableResourceStatus (api/v1alpha1/composableresource_types.go:36-41):
@@ -541,6 +697,16 @@ int  cro_emit_probe_annotations_json(const cro_probe_result *r, char *buf, size_
  * only when n > 0). */
 int  cro_emit_fault_annotations_json(const cro_fault_report *report, const cro_fault_word *words, int n,
                                      char *buf, size_t cap, size_t *len);
+
+/* Additive host-link annotations (cohdi.io/probe-link-*) of a cro_probe_host_link result, the same Go-marshalled map,
+ * integers and fixed spellings only (MB/s = bytes * 1000 / ns, integer division; 0 when ns is 0):
+ * -verdict ("ok" | "corrupt:<check>" with <check> one of d2h-copy, h2d-copy, sm-write, duplex-write, duplex-d2h-copy,
+ * chase | "error" for a call that failed otherwise), -h2d-mbps and -d2h-mbps (copy-engine legs), -duplex-mbps (both
+ * copy-engine duplex legs' bytes over their span), -sm-h2d-mbps and -sm-d2h-mbps, -latency-ns (chase ns / hops),
+ * -link ("<cur speed> x<cur width> / <max speed> x<max width>" of the GPU, a speed as "32.0GT/s" or "unknown"),
+ * and only when they apply: -bottleneck ("<bdf> <speed> x<width>", with CRO_LINK_DEGRADED_BOTTLENECK), -degraded (the
+ * flags' names speed, width, path, bottleneck, comma-separated) and -replays (the counter delta, when NVML answered). */
+int  cro_emit_link_annotations_json(const cro_link_result *r, char *buf, size_t cap, size_t *len);
 
 /* (deviceID, CDIDeviceID) from an FM ScaleUpResponse body, with the
  * res_op_status gate of internal/cdi/fti/fm/client.go:184-213.  On the error
