@@ -249,7 +249,60 @@ class LinkResult(ctypes.Structure):
                 ("replays_before", ctypes.c_uint64), ("replays_after", ctypes.c_uint64), ("path", PciPath)]
 
 
+# SM compute probe (cro_probe_compute, cro_compute_expected)
+COMPUTE_M, COMPUTE_N, COMPUTE_K = 128, 256, 256
+COMPUTE_LEG_S8, COMPUTE_LEG_BF16, COMPUTE_LEG_E4M3, COMPUTE_LEG_FFMA, COMPUTE_LEG_IMAD = range(5)
+COMPUTE_LEGS, COMPUTE_ALL_LEGS = 5, 0x1F
+COMPUTE_ANSWER_S8, COMPUTE_ANSWER_SMALL = 0, 1
+COMPUTE_RECORDS, COMPUTE_MAX_SMS = 4096, 256
+COMPUTE_MAX_ITERATIONS, COMPUTE_MAX_ALU_ITERATIONS, COMPUTE_MAX_ROUNDS = 65536, 1024, 64
+COMPUTE_NONE, COMPUTE_SM, COMPUTE_ALL = 0, 1, 2
+COMPUTE_PERSISTENT, COMPUTE_INTERMITTENT = 1, 2
+
+
+class ComputeOpts(ctypes.Structure):
+    _fields_ = [("iterations", ctypes.c_uint32), ("alu_iterations", ctypes.c_uint32), ("legs", ctypes.c_uint32),
+                ("max_rounds", ctypes.c_uint32), ("test_inject_leg", ctypes.c_int32), ("test_inject_sm", ctypes.c_int32),
+                ("test_inject_iteration", ctypes.c_uint32), ("test_inject_row", ctypes.c_int32),
+                ("test_inject_col", ctypes.c_int32), ("test_inject_mask", ctypes.c_uint32)]
+
+
+class ComputeLeg(ctypes.Structure):
+    _fields_ = [("iterations", ctypes.c_uint32), ("rounds", ctypes.c_uint32), ("ops", ctypes.c_uint64),
+                ("ns", ctypes.c_uint64), ("timer_ns", ctypes.c_uint64), ("sms_covered", ctypes.c_uint32),
+                ("complete", ctypes.c_uint32), ("mismatches", ctypes.c_uint64), ("fold_mismatches", ctypes.c_uint64),
+                ("recorded", ctypes.c_uint64), ("failed_sms", ctypes.c_uint32), ("unpublished", ctypes.c_uint32),
+                ("ctas", ctypes.c_uint32), ("slowest_sm", ctypes.c_uint32), ("slow_permille", ctypes.c_uint32),
+                ("reserved", ctypes.c_uint32), ("fold", ctypes.c_uint64), ("expect_fold", ctypes.c_uint64)]
+
+
+class ComputeResult(ctypes.Structure):
+    """cro_compute_result: status, verdict and per-leg counts, coverage and times of one compute probe call."""
+    _fields_ = [("status", ctypes.c_int32), ("verdict", ctypes.c_uint32), ("seed", ctypes.c_uint64),
+                ("call", ctypes.c_uint64), ("sm_count", ctypes.c_uint32), ("legs", ctypes.c_uint32),
+                ("host_ref_ns", ctypes.c_uint64), ("nsmid", ctypes.c_uint32), ("bad_sms", ctypes.c_uint32),
+                ("bad_sm", ctypes.c_uint16 * 16), ("leg", ComputeLeg * COMPUTE_LEGS)]
+
+
+class ComputeSmLeg(ctypes.Structure):
+    _fields_ = [("mismatches", ctypes.c_uint64), ("fold_mismatches", ctypes.c_uint64), ("ns", ctypes.c_uint64),
+                ("cycles", ctypes.c_uint64), ("ctas", ctypes.c_uint32), ("mark", ctypes.c_uint32)]
+
+
+class ComputeSm(ctypes.Structure):
+    """One SM seen by a compute probe call, with its counts, times and COMPUTE_PERSISTENT / _INTERMITTENT mark per leg."""
+    _fields_ = [("smid", ctypes.c_uint32), ("reserved", ctypes.c_uint32), ("leg", ComputeSmLeg * COMPUTE_LEGS)]
+
+
+class ComputeFault(ctypes.Structure):
+    """One wrong element of a last iteration's answer: leg, SM, row, column, expected and actual (float legs after
+    rounding to int32)."""
+    _fields_ = [("leg", ctypes.c_uint32), ("smid", ctypes.c_uint32), ("row", ctypes.c_uint32), ("col", ctypes.c_uint32),
+                ("expected", ctypes.c_int32), ("actual", ctypes.c_int32)]
+
+
 assert ctypes.sizeof(ProbeResult) == 512, ctypes.sizeof(ProbeResult)
+assert ctypes.sizeof(ComputeResult) == 600 and ctypes.sizeof(ComputeSm) == 208, ctypes.sizeof(ComputeResult)
 assert ctypes.sizeof(FaultReport) == 928 and ctypes.sizeof(LocatePass) == 120, ctypes.sizeof(FaultReport)
 assert ctypes.sizeof(LinkResult) == 984 and ctypes.sizeof(PciPath) == 272, ctypes.sizeof(LinkResult)
 
@@ -275,6 +328,7 @@ EXPORTS = [
     "cro_selftest_probe_finalize", "cro_selftest_p2p_finalize", "cro_selftest_chase",
     "cro_locate_faults", "cro_emit_fault_annotations_json",
     "cro_probe_host_link", "cro_pci_link_path", "cro_emit_link_annotations_json",
+    "cro_probe_compute", "cro_compute_expected", "cro_emit_compute_annotations_json",
 ]
 
 # Slot map of a device's sweep-slot array (cro_sweep_slot, 64 bytes each); the cro_selftest_* hooks take such arrays.
@@ -368,6 +422,11 @@ def _load() -> ctypes.CDLL:
                                       i32, ctypes.POINTER(i32)]),
         "cro_pci_link_path": (i32, [c, c, ctypes.POINTER(PciPath)]),
         "cro_emit_link_annotations_json": (i32, [ctypes.POINTER(LinkResult)] + out),
+        "cro_probe_compute": (i32, [vp, i32, ctypes.POINTER(ComputeOpts), ctypes.POINTER(ComputeResult),
+                                    ctypes.POINTER(ComputeSm), i32, ctypes.POINTER(i32), ctypes.POINTER(ComputeFault), i32,
+                                    ctypes.POINTER(i32)]),
+        "cro_compute_expected": (i32, [i32, u64, ctypes.POINTER(ctypes.c_int32)]),
+        "cro_emit_compute_annotations_json": (i32, [ctypes.POINTER(ComputeResult)] + out),
         "cro_local_node_op": (i32, [vp, c] + out),
         "cro_local_exec": (i32, [c] + out),
         "cro_describe_wire_type": (i32, [c] + out),
@@ -501,6 +560,21 @@ def emit_fault_annotations_json(report: FaultReport, words: List[FaultWord]) -> 
 def emit_link_annotations_json(r: LinkResult) -> str:
     """Additive cohdi.io/probe-link-* annotations of a probe_host_link result (Go-marshalled map[string]string)."""
     return _text(lib.cro_emit_link_annotations_json, ctypes.byref(r))
+
+
+def emit_compute_annotations_json(r: ComputeResult) -> str:
+    """Additive cohdi.io/probe-compute-* annotations of a probe_compute result (Go-marshalled map[string]string)."""
+    return _text(lib.cro_emit_compute_annotations_json, ctypes.byref(r))
+
+
+def compute_expected(answer: int, seed: int) -> List[int]:
+    """cro_compute_expected: the COMPUTE_ANSWER_S8 / _SMALL answer tile of the operands of `seed`, COMPUTE_M * COMPUTE_N
+    int32 values, row-major (host arithmetic, no GPU)."""
+    arr = (ctypes.c_int32 * (COMPUTE_M * COMPUTE_N))()
+    rc = lib.cro_compute_expected(answer, seed, arr)
+    if rc != OK:
+        raise ProbeError(rc, "cro_compute_expected")
+    return list(arr)
 
 
 def pci_link_path(bus_id: str, sys_root: Optional[str] = None) -> PciPath:
@@ -720,6 +794,26 @@ class ProbeContext:
         self._check(lib.cro_probe_host_link(self.handle, dev, ctypes.byref(o), ctypes.byref(r), arr, cap, ctypes.byref(n)),
                     allow=(ERR_CHECKSUM,))
         return r, [arr[i] for i in range(n.value)]
+
+    def probe_compute(self, dev: int = 0, iterations: int = 0, alu_iterations: int = 0, legs: int = COMPUTE_ALL_LEGS,
+                      max_rounds: int = 0, inject: Optional[Tuple[int, int, int, int, int, int]] = None,
+                      cap: int = 256) -> Tuple[ComputeResult, List[ComputeSm], List[ComputeFault]]:
+        """cro_probe_compute: every SM computes the answer tile with its tensor cores (s8, bf16, e4m3) and CUDA cores
+        (FFMA, IMAD) and checks it exactly.  iterations = 0 / alu_iterations = 0 / max_rounds = 0: the defaults.
+        inject = (leg, sm, iteration, row, col, mask) is the test-only wrong answer (sm, row, col: -1 for every one).
+        Returns the result (its status is OK or ERR_CHECKSUM), one entry per SM seen and up to `cap` element records."""
+        o = ComputeOpts()
+        o.iterations, o.alu_iterations, o.legs, o.max_rounds = iterations, alu_iterations, legs, max_rounds
+        if inject is not None:
+            (o.test_inject_leg, o.test_inject_sm, o.test_inject_iteration, o.test_inject_row, o.test_inject_col,
+             o.test_inject_mask) = inject
+        r = ComputeResult()
+        sms = (ComputeSm * COMPUTE_MAX_SMS)()
+        arr = (ComputeFault * max(1, cap))()
+        n_sms, n = ctypes.c_int(), ctypes.c_int()
+        self._check(lib.cro_probe_compute(self.handle, dev, ctypes.byref(o), ctypes.byref(r), sms, COMPUTE_MAX_SMS,
+                                          ctypes.byref(n_sms), arr, cap, ctypes.byref(n)), allow=(ERR_CHECKSUM,))
+        return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
 
     def launch_count(self) -> int:
         return int(lib.cro_launch_count(self.handle))

@@ -21,6 +21,7 @@
 #include "inventory.hpp"
 #include "gotypes.hpp"
 #include "pcilink.hpp"
+#include "compute.hpp"
 #include <memory>
 #include <new>
 #include <stdexcept>
@@ -52,6 +53,12 @@ static_assert(sizeof(cro_link_result) == 984 && offsetof(cro_link_result, leg) =
                   offsetof(cro_link_result, dev_numa) == 672 && offsetof(cro_link_result, no_nvml) == 688 &&
                   offsetof(cro_link_result, replays_before) == 696 && offsetof(cro_link_result, path) == 712,
               "link layout");
+static_assert(sizeof(cro_compute_opts) == 40 && sizeof(cro_compute_leg) == 104 && sizeof(cro_compute_sm_leg) == 40 &&
+                  sizeof(cro_compute_sm) == 208 && sizeof(cro_compute_fault) == 24, "compute layout");
+static_assert(sizeof(cro_compute_result) == 600 && offsetof(cro_compute_result, host_ref_ns) == 32 &&
+                  offsetof(cro_compute_result, bad_sm) == 48 && offsetof(cro_compute_result, leg) == 80 &&
+                  offsetof(cro_compute_leg, fold) == 88,
+              "compute layout");
 
 using namespace cro::capi;
 
@@ -301,6 +308,26 @@ int cro_probe_host_link(cro_ctx* ctx, int i, const cro_link_opts* opts, cro_link
     for (size_t j = 0; j < k; ++j) faults[j] = found[j];
     *n = (int)k;
     return rc;
+} CRO_API_CATCH
+int cro_probe_compute(cro_ctx* ctx, int i, const cro_compute_opts* opts, cro_compute_result* out, cro_compute_sm* sms,
+                      int sms_cap, int* n_sms, cro_compute_fault* faults, int cap, int* n) try {
+    if (!ctx || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
+        return CRO_ERR_INVALID_ARG;
+    *n = *n_sms = 0;
+    cro_compute_opts o{};
+    if (opts) o = *opts;
+    std::vector<cro_compute_sm> seen;
+    std::vector<cro_compute_fault> found;
+    const int rc = ctx_probe_compute(ctx, i, o, out, &seen, &found);
+    const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
+    for (size_t j = 0; j < ks; ++j) sms[j] = seen[j];
+    for (size_t j = 0; j < kf; ++j) faults[j] = found[j];
+    *n_sms = (int)ks;
+    *n = (int)kf;
+    return rc;
+} CRO_API_CATCH
+int cro_compute_expected(int answer, uint64_t seed, int32_t* out) try {
+    return compute::Expected(answer, seed, out);
 } CRO_API_CATCH
 int cro_pci_link_path(const char* sys_root, const char* pci_bus_id, cro_pci_path* out) try {
     if (!pci_bus_id || !out) return CRO_ERR_INVALID_ARG;
@@ -578,6 +605,45 @@ int cro_emit_link_annotations_json(const cro_link_result* r, char* buf, size_t c
         if (r->degraded >> b & 1u) deg += (deg.empty() ? "" : ",") + std::string(kDegraded[b]);
     if (!deg.empty()) m[p + "degraded"] = deg;
     if (!r->no_nvml) m[p + "replays"] = std::to_string(r->replays_after - r->replays_before);
+    gojson::Writer w;
+    w.string_map(m);
+    return copy_out(w.str(), buf, cap, len);
+} CRO_API_CATCH
+
+int cro_emit_compute_annotations_json(const cro_compute_result* r, char* buf, size_t cap, size_t* len) try {
+    if (!r) return CRO_ERR_INVALID_ARG;
+    static const char* const kLeg[CRO_COMPUTE_LEGS] = {"s8", "bf16", "e4m3", "ffma", "imad"};
+    std::map<std::string, std::string> m;
+    const std::string p = "cohdi.io/probe-compute-";
+    m[p + "verdict"] = r->status == CRO_OK                                                ? "ok"
+                       : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_COMPUTE_SM  ? "sm"
+                       : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_COMPUTE_ALL ? "all"
+                                                                                        : "error";
+    uint32_t covered = 0xFFFFFFFFu, worst = CRO_COMPUTE_LEGS;
+    std::string failed;
+    for (int l = 0; l < CRO_COMPUTE_LEGS; ++l) {
+        if (!(r->legs >> l & 1u)) continue;
+        const cro_compute_leg& L = r->leg[l];
+        covered = std::min(covered, L.sms_covered);
+        if (L.mismatches || L.fold_mismatches || L.unpublished) failed += (failed.empty() ? "" : ",") + std::string(kLeg[l]);
+        if (worst == CRO_COMPUTE_LEGS || L.slow_permille > r->leg[worst].slow_permille) worst = (uint32_t)l;
+    }
+    m[p + "sms"] = std::to_string(covered == 0xFFFFFFFFu ? 0u : covered) + "/" + std::to_string(r->sm_count);
+    if (r->bad_sms) {
+        std::string ids;
+        for (uint32_t j = 0; j < std::min<uint32_t>(r->bad_sms, 16); ++j) ids += (j ? "," : "") + std::to_string(r->bad_sm[j]);
+        m[p + "bad-sms"] = ids;
+    }
+    if (!failed.empty()) m[p + "failed-legs"] = failed;
+    auto rate = [&](int l) {
+        const cro_compute_leg& L = r->leg[l];
+        return std::to_string(L.ns ? L.ops / L.ns : 0ull);
+    };
+    m[p + "s8-gops"] = rate(CRO_COMPUTE_LEG_S8);
+    m[p + "bf16-gflops"] = rate(CRO_COMPUTE_LEG_BF16);
+    m[p + "e4m3-gflops"] = rate(CRO_COMPUTE_LEG_E4M3);
+    if (worst < CRO_COMPUTE_LEGS)
+        m[p + "slowest-sm"] = std::to_string(r->leg[worst].slowest_sm) + " " + std::to_string(r->leg[worst].slow_permille);
     gojson::Writer w;
     w.string_map(m);
     return copy_out(w.str(), buf, cap, len);

@@ -14,17 +14,24 @@
 //   link_stream       L bytes over PCIe mapped pinned host memory, read (fold + compare) and / or written
 //                                       (the host link probe, cro_probe_host_link; not part of the probe)
 //   chase             pointer chase over peer-resident permutations (latency)
+//   compute_probe     0 bytes           the answer tile D = A * B on every SM, tensor cores and CUDA cores, checked
+//                                       exactly (the compute probe, cro_probe_compute; not part of the probe)
 //   probe_finalize / p2p_finalize       the verdict: the 512-byte result struct is written on the device
 //
 // Two data paths per sweep: 128-bit ld.global.nc / st.global vector accesses
 // (also used on peer-mapped pointers for the NVLink probe), and 1-D TMA bulk
 // copies (cp.async.bulk + mbarrier) through a shared-memory ring.
-// No tensor cores: there is no contraction anywhere on this path.
+// The probe path has no tensor cores: there is no contraction on it.  The compute
+// probe uses them on purpose: checking them is its job.
 #include "kernels.cuh"
+
+#include <cuda_bf16.h>
+#include <cuda_fp8.h>
 
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
+#include <type_traits>
 
 namespace cro {
 
@@ -1211,6 +1218,367 @@ p2p_finalize_kernel(const P2PFinalizeArgs a) {
 }
 
 // ---------------------------------------------------------------------------
+// compute_probe: every SM computes the answer tile D = A * B (M x N x K of
+// include/croprobe.h) `iterations` times from operands it generates into its own
+// shared memory, and checks what it got (the compute probe, cro_probe_compute;
+// not part of the HBM probe).  One template per leg:
+//   S8, BF16, E4M3   wgmma.mma_async m64n256 (IGMMA / HGMMA / QGMMA), each of the
+//                    two warpgroups owning 64 rows, chained over K with scale-d = 0
+//                    on the first instruction of every iteration
+//   FFMA, IMAD       the same accumulator fragment computed by scalar FMA / IMAD
+//                    chains on the CUDA cores
+// Operands sit in the canonical K-major no-swizzle layout the wgmma shared-memory
+// descriptors read: core matrices of 8 rows x 16 bytes (128 contiguous bytes, row
+// r at +16 r); the core matrices along K of one 8-row group side by side (leading
+// byte offset 128); 8-row groups 8 * K * elem bytes apart (stride byte offset).
+// B is held transposed (N rows of K), as the K-major form requires.
+// After each iteration every thread adds sum_j value_j * (2j + 1) to a running
+// fold (float values after cvt.rni.s32.f32); at the end it compares the fold with
+// iterations * the fold of the expected values, and the last answer element by
+// element with the expected tile (global memory, L2-resident, shared by all CTAs).
+// Mismatches are recorded with the locator's idiom: a ballot keeps clean warps off
+// the atomics, one atomicAdd per warp claims a run of record slots, and only while
+// a plain load shows room.
+// ---------------------------------------------------------------------------
+constexpr unsigned kCM = CRO_COMPUTE_M, kCN = CRO_COMPUTE_N, kCK = CRO_COMPUTE_K;
+constexpr size_t kComputeSmem = (size_t)(kCM + kCN) * kCK * 2;     // the bf16 operands: 192 KiB, one CTA per SM
+
+template <unsigned LEG> struct ComputeLeg {
+    static constexpr bool kTensor = LEG <= CRO_COMPUTE_LEG_E4M3;
+    static constexpr bool kFloat = LEG == CRO_COMPUTE_LEG_BF16 || LEG == CRO_COMPUTE_LEG_E4M3 || LEG == CRO_COMPUTE_LEG_FFMA;
+    static constexpr unsigned kElem = (LEG == CRO_COMPUTE_LEG_BF16 || LEG == CRO_COMPUTE_LEG_FFMA) ? 2 : 1;   // bytes
+    using Acc = typename std::conditional<kFloat, float, int>::type;
+};
+
+// Byte offset of element (row, k) of a K-major operand with kCK elements per row.
+template <unsigned ELEM>
+__device__ __forceinline__ unsigned kmajor_off(unsigned row, unsigned k) {
+    const unsigned kb = k * ELEM;
+    return (row >> 3) * (8u * kCK * ELEM) + (kb >> 4) * 128u + (row & 7u) * 16u + (kb & 15u);
+}
+
+// wgmma shared-memory descriptor, no swizzle: start address, leading byte offset 128, stride byte offset sbo.
+__device__ __forceinline__ unsigned long long wgmma_desc(unsigned addr, unsigned sbo) {
+    return (unsigned long long)((addr & 0x3FFFFu) >> 4) | ((unsigned long long)(128u >> 4) << 16) |
+           ((unsigned long long)(sbo >> 4) << 32);
+}
+
+__device__ __forceinline__ void wgmma_s8(int (&d)[128], unsigned long long da, unsigned long long db, int scale_d) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+        "}, %128, %129, p;\n}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]),
+          "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]),
+          "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]),
+          "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]),
+          "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]),
+          "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]),
+          "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]),
+          "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]),
+          "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
+        : "l"(da), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_bf16(float (&d)[128], unsigned long long da, unsigned long long db, int scale_d) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+        "}, %128, %129, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(da), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_e4m3(float (&d)[128], unsigned long long da, unsigned long long db, int scale_d) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n256k32.f32.e4m3.e4m3 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+        "}, %128, %129, p, 1, 1;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(da), "l"(db), "r"(scale_d));
+}
+
+// The operand byte read as each leg's element type: s8 as int8; small-int (byte & 7) - 4 as bf16 or e4m3.
+template <unsigned LEG>
+__device__ __forceinline__ void store_operand(unsigned char* p, unsigned byte) {
+    if constexpr (LEG == CRO_COMPUTE_LEG_S8 || LEG == CRO_COMPUTE_LEG_IMAD) {
+        *p = (unsigned char)byte;
+    } else if constexpr (LEG == CRO_COMPUTE_LEG_E4M3) {
+        *p = (unsigned char)__nv_cvt_float_to_fp8((float)((int)(byte & 7u) - 4), __NV_SATFINITE, __NV_E4M3);
+    } else {
+        *reinterpret_cast<__nv_bfloat16*>(p) = __float2bfloat16_rn((float)((int)(byte & 7u) - 4));
+    }
+}
+
+template <unsigned LEG>
+__device__ __forceinline__ int compute_value(typename ComputeLeg<LEG>::Acc v) {
+    if constexpr (ComputeLeg<LEG>::kFloat) return __float2int_rn(v);      // cvt.rni.s32.f32: exact for these integers
+    else return v;
+}
+
+// Element k (0 .. 16 / ELEM - 1) of 16 operand bytes, as the ALU legs multiply it.
+template <unsigned LEG>
+__device__ __forceinline__ typename ComputeLeg<LEG>::Acc alu_elem(const unsigned (&w)[4], int k) {
+    if constexpr (LEG == CRO_COMPUTE_LEG_FFMA) {
+        const unsigned x = w[k >> 1];
+        return __uint_as_float((k & 1) ? (x & 0xFFFF0000u) : (x << 16));
+    } else {
+        return (int)(signed char)(w[k >> 2] >> (8 * (k & 3)));
+    }
+}
+
+// Records the warp's mismatching elements of chunk C (accumulator values 32 C .. 32 C + 31; bit q of m: value
+// 32 C + q mismatches).  The whole warp calls this (some lane has m != 0).
+template <unsigned LEG, int C>
+__device__ __forceinline__ void compute_record(const typename ComputeLeg<LEG>::Acc (&acc)[128], unsigned m, unsigned r0,
+                                               unsigned c0, unsigned smid, const ComputeArgs& a) {
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned n_lane = __popc(m);
+    const unsigned n_warp = __reduce_add_sync(0xffffffffu, n_lane);
+    unsigned incl = n_lane;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= (unsigned)o) incl += t;
+    }
+    unsigned long long base = CRO_COMPUTE_RECORDS;
+    if (lane == 0 && *reinterpret_cast<volatile unsigned long long*>(a.claims) < CRO_COMPUTE_RECORDS)
+        base = atomicAdd(a.claims, (unsigned long long)n_warp);
+    base = __shfl_sync(0xffffffffu, base, 0) + (incl - n_lane);
+#pragma unroll
+    for (int q = 0; q < 32; ++q) {
+        const int j = 32 * C + q;
+        if (!((m >> q) & 1u)) continue;
+        if (base < CRO_COMPUTE_RECORDS) {
+            const unsigned row = r0 + 8u * ((j >> 1) & 1), col = 8u * (j >> 2) + c0 + (j & 1);
+            a.rec[base] = cro_compute_fault{LEG, smid, row, col, __ldg(a.expect + row * kCN + col),
+                                            compute_value<LEG>(acc[j])};
+        }
+        ++base;
+    }
+}
+
+template <unsigned LEG, int C>
+__device__ __forceinline__ unsigned compute_compare(const typename ComputeLeg<LEG>::Acc (&acc)[128], unsigned r0, unsigned c0,
+                                                    unsigned smid, const ComputeArgs& a, unsigned long long* efold) {
+    unsigned m = 0;
+#pragma unroll
+    for (int q = 0; q < 32; ++q) {
+        const int j = 32 * C + q;
+        const unsigned row = r0 + 8u * ((j >> 1) & 1), col = 8u * (j >> 2) + c0 + (j & 1);
+        const int e = __ldg(a.expect + row * kCN + col);
+        *efold += (unsigned long long)(long long)e * (unsigned long long)(2 * j + 1);
+        if (compute_value<LEG>(acc[j]) != e) m |= 1u << q;
+    }
+    if (__ballot_sync(0xffffffffu, m != 0)) compute_record<LEG, C>(acc, m, r0, c0, smid, a);
+    return __popc(m);
+}
+
+template <unsigned LEG>
+__global__ void __launch_bounds__(kComputeThreads, 1) compute_probe_kernel(const ComputeArgs a) {
+    using L = ComputeLeg<LEG>;
+    using Acc = typename L::Acc;
+    constexpr unsigned ELEM = L::kElem;
+    extern __shared__ __align__(128) unsigned char cmp_smem[];
+    __shared__ unsigned long long s_mism, s_fold_mism, s_fold;
+    unsigned char* const sA = cmp_smem;
+    unsigned char* const sB = cmp_smem + kCM * kCK * ELEM;
+    const unsigned tid = threadIdx.x;
+    if (tid == 0) s_mism = s_fold_mism = s_fold = 0;
+
+    // operands: element e is byte e % 8 of pattern_word(seed, e / 8); A[m][k] at e = m * K + k, B[k][n] at
+    // e = M * K + k * N + n
+    for (unsigned w = tid; w < (kCM * kCK + kCK * kCN) / 8; w += kComputeThreads) {
+        const unsigned long long v = pattern_word(a.seed, w);
+#pragma unroll
+        for (unsigned b = 0; b < 8; ++b) {
+            const unsigned e = 8 * w + b;
+            const unsigned byte = (unsigned)(v >> (8 * b)) & 0xFFu;
+            if (e < kCM * kCK) store_operand<LEG>(sA + kmajor_off<ELEM>(e / kCK, e % kCK), byte);
+            else store_operand<LEG>(sB + kmajor_off<ELEM>((e - kCM * kCK) % kCN, (e - kCM * kCK) / kCN), byte);
+        }
+    }
+    if constexpr (L::kTensor) asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+    __syncthreads();
+
+    unsigned smid, nsmid;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+    asm volatile("mov.u32 %0, %%nsmid;" : "=r"(nsmid));
+    const unsigned wg = tid >> 7, lane = tid & 31u;
+    const unsigned r0 = 64u * wg + 16u * ((tid >> 5) & 3u) + (lane >> 2), c0 = 2u * (lane & 3u);
+    // the injection, resolved once: this thread's iteration to inject after (all ones: none) and rows it owns
+    const unsigned rowsel = (a.inj_row < 0) ? 3u : ((unsigned)a.inj_row == r0 ? 1u : (unsigned)a.inj_row == r0 + 8 ? 2u : 0u);
+    const unsigned inj_it = (a.inj_mask && rowsel && (a.inj_sm < 0 || (unsigned)a.inj_sm == smid)) ? a.inj_iter : ~0u;
+
+    Acc acc[128];
+#pragma unroll
+    for (int j = 0; j < 128; ++j) acc[j] = 0;
+    unsigned long long run = 0;
+    const unsigned long long t0 = globaltimer_ns();
+    const long long k0 = clock64();
+    for (unsigned it = 0; it < a.iterations; ++it) {
+        if constexpr (L::kTensor) {
+            constexpr unsigned SBO = 8u * kCK * ELEM;
+            const unsigned long long da = wgmma_desc(smem_u32(sA) + wg * 64u * kCK * ELEM, SBO);
+            const unsigned long long db = wgmma_desc(smem_u32(sB), SBO);
+            asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory");
+#pragma unroll
+            for (unsigned s = 0; s < kCK * ELEM / 32; ++s) {      // 32 bytes of K per instruction: +256 bytes, >> 4
+                if constexpr (LEG == CRO_COMPUTE_LEG_S8) wgmma_s8(acc, da + 16u * s, db + 16u * s, s != 0);
+                else if constexpr (LEG == CRO_COMPUTE_LEG_BF16) wgmma_bf16(acc, da + 16u * s, db + 16u * s, s != 0);
+                else wgmma_e4m3(acc, da + 16u * s, db + 16u * s, s != 0);
+            }
+            asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory");
+            asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory");
+#pragma unroll
+            for (int j = 0; j < 128; ++j) {
+                if constexpr (L::kFloat) asm volatile("" : "+f"(acc[j])::"memory");
+                else asm volatile("" : "+r"(acc[j])::"memory");
+            }
+        } else {
+#pragma unroll
+            for (int j = 0; j < 128; ++j) acc[j] = 0;
+            constexpr int KC = 16 / ELEM;                          // elements per 16-byte core-matrix row
+#pragma unroll 1
+            for (unsigned kc = 0; kc < kCK; kc += KC) {
+                const uint4 x0 = *reinterpret_cast<const uint4*>(sA + kmajor_off<ELEM>(r0, kc));
+                const uint4 x1 = *reinterpret_cast<const uint4*>(sA + kmajor_off<ELEM>(r0 + 8, kc));
+                const unsigned a0[4] = {x0.x, x0.y, x0.z, x0.w}, a1[4] = {x1.x, x1.y, x1.z, x1.w};
+#pragma unroll
+                for (int g = 0; g < 32; ++g) {
+                    const uint4 y0 = *reinterpret_cast<const uint4*>(sB + kmajor_off<ELEM>(8u * g + c0, kc));
+                    const uint4 y1 = *reinterpret_cast<const uint4*>(sB + kmajor_off<ELEM>(8u * g + c0 + 1, kc));
+                    const unsigned b0[4] = {y0.x, y0.y, y0.z, y0.w}, b1[4] = {y1.x, y1.y, y1.z, y1.w};
+#pragma unroll
+                    for (int k = 0; k < KC; ++k) {
+                        const Acc p = alu_elem<LEG>(a0, k), q = alu_elem<LEG>(a1, k);
+                        const Acc u = alu_elem<LEG>(b0, k), v = alu_elem<LEG>(b1, k);
+                        if constexpr (L::kFloat) {
+                            acc[4 * g] = fmaf(p, u, acc[4 * g]);
+                            acc[4 * g + 1] = fmaf(p, v, acc[4 * g + 1]);
+                            acc[4 * g + 2] = fmaf(q, u, acc[4 * g + 2]);
+                            acc[4 * g + 3] = fmaf(q, v, acc[4 * g + 3]);
+                        } else {
+                            acc[4 * g] += p * u;
+                            acc[4 * g + 1] += p * v;
+                            acc[4 * g + 2] += q * u;
+                            acc[4 * g + 3] += q * v;
+                        }
+                    }
+                }
+            }
+        }
+        if (it == inj_it) {                                        // test only: one compare on the clean path
+#pragma unroll
+            for (int j = 0; j < 128; ++j) {
+                const unsigned col = 8u * (j >> 2) + c0 + (j & 1);
+                if (((rowsel >> ((j >> 1) & 1)) & 1u) && (a.inj_col < 0 || (unsigned)a.inj_col == col)) {
+                    if constexpr (L::kFloat) acc[j] = __uint_as_float(__float_as_uint(acc[j]) ^ a.inj_mask);
+                    else acc[j] ^= (int)a.inj_mask;
+                }
+            }
+        }
+        __syncwarp();
+        unsigned long long f = 0;
+#pragma unroll
+        for (int j = 0; j < 128; ++j)
+            f += (unsigned long long)(long long)compute_value<LEG>(acc[j]) * (unsigned long long)(2 * j + 1);
+        run += f;
+    }
+    const long long k1 = clock64();
+    const unsigned long long t1 = globaltimer_ns();
+
+    unsigned long long efold = 0;
+    unsigned mism = compute_compare<LEG, 0>(acc, r0, c0, smid, a, &efold);
+    mism += compute_compare<LEG, 1>(acc, r0, c0, smid, a, &efold);
+    mism += compute_compare<LEG, 2>(acc, r0, c0, smid, a, &efold);
+    mism += compute_compare<LEG, 3>(acc, r0, c0, smid, a, &efold);
+    const unsigned fold_bad = run != (unsigned long long)a.iterations * efold ? 1u : 0u;
+    const unsigned wm = __reduce_add_sync(0xffffffffu, mism), wf = __reduce_add_sync(0xffffffffu, fold_bad);
+    if (lane == 0 && (wm | wf)) {
+        atomicAdd(&s_mism, (unsigned long long)wm);
+        atomicAdd(&s_fold_mism, (unsigned long long)wf);
+    }
+    atomicAdd(&s_fold, run);
+    __syncthreads();
+    if (tid == 0) {
+        if (smid < CRO_COMPUTE_MAX_SMS) atomicOr(a.sm_bits + (smid >> 6), 1ull << (smid & 63u));
+        ComputeCta& o = a.cta[blockIdx.x];
+        o.t0 = t0;
+        o.t1 = t1;
+        o.cycles = (unsigned long long)(k1 - k0);
+        o.mismatches = s_mism;
+        o.fold_mismatches = s_fold_mism;
+        o.fold = s_fold;
+        o.smid = smid;
+        o.nsmid = nsmid;
+        o.stamp = a.stamp;
+    }
+}
+
+// ---------------------------------------------------------------------------
 // host side: plan + launch wrappers
 // ---------------------------------------------------------------------------
 namespace {
@@ -1452,6 +1820,20 @@ cudaError_t launch_finalize(const FinalizeArgs& a, cudaStream_t st) {
 
 cudaError_t launch_p2p_finalize(const P2PFinalizeArgs& a, cudaStream_t st) {
     p2p_finalize_kernel<<<1, 32, 0, st>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_compute(unsigned leg, const ComputeArgs& a, int grid, cudaStream_t st) {
+    void (*k)(ComputeArgs) = leg == CRO_COMPUTE_LEG_S8     ? compute_probe_kernel<CRO_COMPUTE_LEG_S8>
+                             : leg == CRO_COMPUTE_LEG_BF16 ? compute_probe_kernel<CRO_COMPUTE_LEG_BF16>
+                             : leg == CRO_COMPUTE_LEG_E4M3 ? compute_probe_kernel<CRO_COMPUTE_LEG_E4M3>
+                             : leg == CRO_COMPUTE_LEG_FFMA ? compute_probe_kernel<CRO_COMPUTE_LEG_FFMA>
+                             : leg == CRO_COMPUTE_LEG_IMAD ? compute_probe_kernel<CRO_COMPUTE_LEG_IMAD>
+                                                           : nullptr;
+    if (!k || grid < 1) return cudaErrorInvalidValue;
+    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kComputeSmem);
+    if (e != cudaSuccess) return e;
+    k<<<grid, kComputeThreads, kComputeSmem, st>>>(a);
     return cudaGetLastError();
 }
 

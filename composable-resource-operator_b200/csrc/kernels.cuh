@@ -149,6 +149,35 @@ struct LinkRole {
 cudaError_t launch_link_stream(const LinkRole& rd, const LinkRole& wr, const LocateBufs& lb, int grid, uint64_t stamp,
                                cudaStream_t);
 
+// SM compute probe (cro_probe_compute): one launch of leg `leg` (CRO_COMPUTE_LEG_*) runs `grid` CTAs of 256 threads,
+// one per SM.  Each CTA generates the call's operands into its shared memory, computes the answer tile `iterations`
+// times, folds every iteration and compares the last one element by element with *expect (M x N int32, row-major).
+// It publishes one ComputeCta (stamp last written = the call number), ORs its %smid into sm_bits and records its
+// mismatching elements while the record buffer has room (*claims counts the slots claimed, possibly past the end).
+struct ComputeCta {
+    unsigned long long stamp;                   // the call number; all ones (armed) = the CTA did not publish
+    unsigned long long t0, t1;                  // %globaltimer around the iterations
+    unsigned long long cycles;                  // %clock64 around the iterations
+    unsigned long long mismatches;              // elements of the last iteration that differ
+    unsigned long long fold_mismatches;         // threads whose running fold differs
+    unsigned long long fold;                    // every thread's running fold, summed
+    unsigned smid, nsmid;
+};
+static_assert(sizeof(ComputeCta) == 64, "one 64-byte record per CTA");
+struct ComputeArgs {
+    const int* expect;
+    ComputeCta* cta;                            // grid entries
+    unsigned long long* sm_bits;                // CRO_COMPUTE_MAX_SMS / 64 words
+    cro_compute_fault* rec;                     // CRO_COMPUTE_RECORDS entries
+    unsigned long long* claims;
+    unsigned long long seed, stamp;
+    unsigned iterations;
+    int inj_sm, inj_row, inj_col;               // -1: every SM / row / column
+    unsigned inj_iter, inj_mask;                // inj_mask 0: nothing is injected in this launch
+};
+constexpr int kComputeThreads = 256;            // two warpgroups of 64 rows each
+cudaError_t launch_compute(unsigned leg, const ComputeArgs& a, int grid, cudaStream_t);
+
 // Pointer chase for NVLink latency: warp j of the one CTA follows `hops` dependent ld.relaxed.sys loads through
 // table[j] (one 8-byte slot per 128-byte line, peer-resident); out[2j] = final index, out[2j+1] = %globaltimer ns.
 struct ChaseArgs {

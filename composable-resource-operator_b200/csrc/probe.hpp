@@ -87,6 +87,7 @@ struct Device {
     SweepScratch scratch_link[2]{};
     std::vector<cudaEvent_t> ev_link;
     uint64_t link_calls = 0;               // k of the next call: its seeds
+    uint64_t compute_calls = 0;            // k of the next compute probe call (ctx_probe_compute): its operand seed
     KernelPlan plan{};
     SweepScratch scratch{}, scratch_aux{}, scratch_pfx{};   // main stream / closed form / p2p prefix closed form
     // lane 0's buffers under their old names: the synchronous probe, the single sweeps and cro_probe_all use lane 0
@@ -221,6 +222,11 @@ uint32_t fault_verdict(const cro_fault_report& r);
 
 // Host link probe (include/croprobe.h, cro_probe_host_link): *faults gets every recorded mismatch, by check, then index.
 int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_result* r, std::vector<cro_link_fault>* faults);
+
+// SM compute probe (include/croprobe.h, cro_probe_compute): *sms gets one entry per SM seen, by SM id; *faults every
+// recorded element, by (leg, smid, row, col).
+int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_compute_result* r, std::vector<cro_compute_sm>* sms,
+                      std::vector<cro_compute_fault>* faults);
 
 // test hooks (include/croprobe.h, cro_selftest_*): the verdict kernels and the chase on caller-given inputs
 int ctx_selftest_probe_finalize(cro_ctx* c, int idx, const cro_probe_result* tmpl, const cro_sweep_slot* slots,

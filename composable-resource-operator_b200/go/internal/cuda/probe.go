@@ -337,6 +337,80 @@ func (c *Context) ProbeHostLink(deviceID string) (LinkResult, error) {
 	return out, nil
 }
 
+// ComputeResult is the summary of cro_compute_result an operator reads: whether
+// every SM computed the exact answer on its tensor cores and CUDA cores, and
+// which SMs did not.
+type ComputeResult struct {
+	OK          bool
+	Verdict     uint32            // CRO_COMPUTE_NONE / _SM / _ALL
+	SMCount     uint32
+	Covered     [5]uint32         // SMs seen per CRO_COMPUTE_LEG_*
+	Mismatches  [5]uint64         // wrong elements of the last iteration, per leg
+	BadSMs      []uint32          // SMs that failed any leg, ascending
+	Faults      []ComputeFault
+	Annotations string // Go-marshalled map[string]string of cohdi.io/probe-compute-* keys
+}
+
+// ComputeFault is one wrong element (cro_compute_fault).
+type ComputeFault struct {
+	Leg, SM, Row, Col uint32
+	Expected, Actual  int32
+}
+
+// ProbeCompute runs cro_probe_compute with its defaults on the in-process
+// device whose UUID is deviceID: after a passing HBM probe of a freshly composed
+// GPU, and after a locator verdict of not-reproduced.  A device probed through
+// the helper process is an error, as for LocateFaults.
+func (c *Context) ProbeCompute(deviceID string) (ComputeResult, error) {
+	var devs [C.CRO_MAX_DEVICES]C.cro_dev_info
+	var n C.int
+	if rc := C.cro_enumerate(c.h, &devs[0], C.CRO_MAX_DEVICES, &n); rc != C.CRO_OK {
+		return ComputeResult{}, errorOf(c.h, rc)
+	}
+	idx := C.int(-1)
+	for i := 0; i < int(n); i++ {
+		if C.GoString(&devs[i].gpu_uuid[0]) == deviceID && devs[i].flags&C.CRO_DEV_IN_PROCESS != 0 {
+			idx = C.int(devs[i].dev_index)
+		}
+	}
+	if idx < 0 {
+		return ComputeResult{}, fmt.Errorf("cuda compute probe: %s is not a device of this context", deviceID)
+	}
+	var res C.cro_compute_result
+	sms := make([]C.cro_compute_sm, C.CRO_COMPUTE_MAX_SMS)
+	var faults [256]C.cro_compute_fault
+	var nSMs, got C.int
+	rc := C.cro_probe_compute(c.h, idx, nil, &res, &sms[0], C.CRO_COMPUTE_MAX_SMS, &nSMs, &faults[0], 256, &got)
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM {
+		return ComputeResult{}, errorOf(c.h, rc)
+	}
+	out := ComputeResult{OK: rc == C.CRO_OK, Verdict: uint32(res.verdict), SMCount: uint32(res.sm_count)}
+	for l := 0; l < int(C.CRO_COMPUTE_LEGS); l++ {
+		out.Covered[l] = uint32(res.leg[l].sms_covered)
+		out.Mismatches[l] = uint64(res.leg[l].mismatches)
+	}
+	for i := 0; i < int(nSMs); i++ {
+		for l := 0; l < int(C.CRO_COMPUTE_LEGS); l++ {
+			if sms[i].leg[l].mark != 0 {
+				out.BadSMs = append(out.BadSMs, uint32(sms[i].smid))
+				break
+			}
+		}
+	}
+	for i := 0; i < int(got); i++ {
+		f := faults[i]
+		out.Faults = append(out.Faults, ComputeFault{uint32(f.leg), uint32(f.smid), uint32(f.row), uint32(f.col),
+			int32(f.expected), int32(f.actual)})
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_compute_annotations_json(&res, buf, 4096, &ln) == C.CRO_OK {
+		out.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return out, nil
+}
+
 // MetricsText is the Prometheus text exposition of the context's counters and
 // per-GPU gauges; a prometheus.Collector registered with
 // sigs.k8s.io/controller-runtime/pkg/metrics.Registry (cmd/main.go:66,119-125

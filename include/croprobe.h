@@ -658,6 +658,147 @@ int  cro_probe_host_link(cro_ctx *ctx, int dev_index, const cro_link_opts *opts,
  * id that parses as neither spelling; CRO_ERR_NO_DEVICE: no such device under sys_root. */
 int  cro_pci_link_path(const char *sys_root, const char *pci_bus_id, cro_pci_path *out);
 
+/* ---- SM compute: every SM's tensor cores and ALUs against an exact answer ----- */
+
+/*
+ * The HBM probe and the host link probe check memory and the PCIe path; nothing there checks that the SMs compute right
+ * answers.  The compute probe has every SM compute one answer tile D = A * B (M x N x K below) many times, with its
+ * tensor cores (wgmma: s8, bf16, e4m3) and with its CUDA cores (an FFMA chain and an IMAD chain), and compares what it
+ * got with the answer the library computed on the host.  A wrong answer is attributed to the SM (%smid) that produced
+ * it.  It runs only when called and changes nothing of the probe: it takes the device's mutex, lets probes still in
+ * flight finish first (their results stay collectable with cro_probe_end), and never touches the sweep region, so the
+ * fault locator's pass 0 still compares both halves afterwards.  It allocates only its own small buffers (the two
+ * expected tiles, the per-CTA records and the fault records) and frees them before returning.
+ *
+ * Operands of call k on a device: seed = seed_dev + 2^61 + k * 0xD1B54A32D192ED03 (seed_dev = seed_base | minor).
+ * Element e is byte (e mod 8) of pattern_word(seed, e / 8) (little-endian: byte b is bits 8b..8b+7), with
+ *   e = m * 256 + k           for A[m][k]    (0 <= m < M, 0 <= k < K)
+ *   e = 32768 + k * 256 + n   for B[k][n]    (0 <= n < N)
+ * and two readings of that byte:
+ *   s8         the byte as int8_t                                   (legs S8, IMAD:  the "s8 answer")
+ *   small-int  (byte & 7) - 4, an integer in -4 .. 3                 (legs BF16, E4M3, FFMA: the "small-int answer")
+ * The answer is D[m][n] = sum over k of A[m][k] * B[k][n], exact in any order of accumulation (DESIGN.md "The compute
+ * probe"); float legs are compared after cvt.rni.s32.f32.
+ *
+ * Every CTA (one per SM, 256 threads: two warpgroups of 64 rows each) computes the whole tile `iterations` times.
+ * Thread t holds 128 accumulator values, value j (0 <= j < 128) being the element
+ *   row = 64 * (t / 128) + 16 * ((t / 32) % 4) + (t % 32) / 4 + 8 * ((j / 2) % 2),   col = 8 * (j / 4) + 2 * (t % 4) + j % 2
+ * (the wgmma m64n256 accumulator fragment; the ALU legs use the same mapping).  After each iteration the thread adds
+ * fold = sum over j of value_j * (2j + 1) (mod 2^64, values as int32) to a running sum, and at the end compares it with
+ * iterations * fold(expected values): a mismatch counts as a fold mismatch.  The last iteration's values are compared
+ * element by element with the expected tile: mismatches are counted exactly and recorded while there is room.
+ */
+#define CRO_COMPUTE_M             128
+#define CRO_COMPUTE_N             256
+#define CRO_COMPUTE_K             256
+#define CRO_COMPUTE_LEG_S8        0       /* wgmma .s32.s8.s8 (IGMMA), s8 answer                      */
+#define CRO_COMPUTE_LEG_BF16      1       /* wgmma .f32.bf16.bf16 (HGMMA), small-int answer            */
+#define CRO_COMPUTE_LEG_E4M3      2       /* wgmma .f32.e4m3.e4m3 (QGMMA), small-int answer            */
+#define CRO_COMPUTE_LEG_FFMA      3       /* FP32 FFMA chain on the CUDA cores, small-int answer        */
+#define CRO_COMPUTE_LEG_IMAD      4       /* INT32 IMAD chain on the CUDA cores, s8 answer              */
+#define CRO_COMPUTE_LEGS          5
+#define CRO_COMPUTE_ALL_LEGS      0x1Fu   /* bit l: leg l                                              */
+#define CRO_COMPUTE_ANSWER_S8     0
+#define CRO_COMPUTE_ANSWER_SMALL  1
+#define CRO_COMPUTE_RECORDS       4096    /* element records the device keeps per leg; counts stay exact beyond */
+#define CRO_COMPUTE_MAX_SMS       256     /* SM ids the coverage bitmaps hold; a larger %nsmid fails the call    */
+#define CRO_COMPUTE_MAX_ITERATIONS      65536
+#define CRO_COMPUTE_MAX_ALU_ITERATIONS  1024
+#define CRO_COMPUTE_MAX_ROUNDS    64
+
+#define CRO_COMPUTE_NONE          0u      /* no SM failed                                               */
+#define CRO_COMPUTE_SM            1u      /* a strict subset of the covered SMs failed: act on those SMs  */
+#define CRO_COMPUTE_ALL           2u      /* every covered SM failed some leg, or a launched CTA did not publish:
+                                             a common cause (operands, expected answer, launch), not one SM */
+
+#define CRO_COMPUTE_PERSISTENT    1u      /* cro_compute_sm_leg.mark: the last iteration's answer was wrong */
+#define CRO_COMPUTE_INTERMITTENT  2u      /* only the fold was wrong: an earlier iteration, right again by the last */
+
+typedef struct cro_compute_opts {
+    uint32_t iterations;           /*   0  tensor legs: 0 = the default (DESIGN.md), at most CRO_COMPUTE_MAX_ITERATIONS  */
+    uint32_t alu_iterations;       /*   4  FFMA / IMAD legs: 0 = 4, at most CRO_COMPUTE_MAX_ALU_ITERATIONS              */
+    uint32_t legs;                 /*   8  CRO_COMPUTE_ALL_LEGS bits; 0 = all                                            */
+    uint32_t max_rounds;           /*  12  launches per leg while fewer than sm_count SMs were seen: 0 = 4               */
+    /* test only: with test_inject_mask != 0, in each CTA of leg test_inject_leg whose %smid is test_inject_sm (-1: every
+       SM), the mask is XORed into accumulator element (test_inject_row, test_inject_col) (-1: every row / column) after
+       iteration test_inject_iteration's answer is complete and before its fold — a software stand-in for a wrong answer */
+    int32_t  test_inject_leg;      /*  16 */
+    int32_t  test_inject_sm;       /*  20 */
+    uint32_t test_inject_iteration;/*  24 */
+    int32_t  test_inject_row;      /*  28 */
+    int32_t  test_inject_col;      /*  32 */
+    uint32_t test_inject_mask;     /*  36 */
+} cro_compute_opts;                /*  40 bytes */
+
+typedef struct cro_compute_leg {
+    uint32_t iterations;           /*   0  per CTA                                                              */
+    uint32_t rounds;               /*   4  launches                                                             */
+    uint64_t ops;                  /*   8  2 * M * N * K * iterations per CTA launched, summed                  */
+    uint64_t ns;                   /*  16  CUDA events around the launches, summed over rounds                 */
+    uint64_t timer_ns;             /*  24  %globaltimer: first CTA start .. last CTA end, summed over rounds    */
+    uint32_t sms_covered;          /*  32  distinct SMs that ran a CTA of the leg                              */
+    uint32_t complete;             /*  36  1: sms_covered == sm_count                                           */
+    uint64_t mismatches;           /*  40  elements of the last iteration's answer that differ, exact          */
+    uint64_t fold_mismatches;      /*  48  threads whose running fold differs                                   */
+    uint64_t recorded;             /*  56  mismatches the device recorded (<= CRO_COMPUTE_RECORDS)              */
+    uint32_t failed_sms;           /*  64  distinct SMs with a mismatch or a fold mismatch                       */
+    uint32_t unpublished;          /*  68  CTAs launched that published no record                              */
+    uint32_t ctas;                 /*  72  CTAs launched, over all rounds                                      */
+    uint32_t slowest_sm;           /*  76  the SM with the most %clock64 cycles per iteration                    */
+    uint32_t slow_permille;        /*  80  its cycles per iteration over the median SM's, x 1000 (report only)   */
+    uint32_t reserved;             /*  84 */
+    uint64_t fold;                 /*  88  running fold summed over the threads of the CTA on the lowest SM id   */
+    uint64_t expect_fold;          /*  96  iterations * the same sum over the expected answer                    */
+} cro_compute_leg;                 /* 104 bytes */
+
+typedef struct cro_compute_result {
+    int32_t  status;               /*   0  the return value: CRO_OK, or CRO_ERR_CHECKSUM on any mismatch or missing publish */
+    uint32_t verdict;              /*   4  CRO_COMPUTE_NONE / _SM / _ALL                                        */
+    uint64_t seed;                 /*   8  operand seed of this call                                           */
+    uint64_t call;                 /*  16  k: the call's number on this device, from 0                         */
+    uint32_t sm_count;             /*  24  multiprocessors the device reports                                   */
+    uint32_t legs;                 /*  28  legs run (CRO_COMPUTE_ALL_LEGS bits)                                 */
+    uint64_t host_ref_ns;          /*  32  host time to compute both expected answers                          */
+    uint32_t nsmid;                /*  40  %nsmid as the kernels read it                                       */
+    uint32_t bad_sms;              /*  44  distinct SMs that failed any leg                                     */
+    uint16_t bad_sm[16];           /*  48  the first 16 of them, ascending                                     */
+    cro_compute_leg leg[CRO_COMPUTE_LEGS];   /*  80 */
+} cro_compute_result;              /* 600 bytes */
+
+typedef struct cro_compute_sm_leg {
+    uint64_t mismatches;           /*   0 */
+    uint64_t fold_mismatches;      /*   8 */
+    uint64_t ns;                   /*  16  %globaltimer windows of the leg's CTAs on this SM, summed           */
+    uint64_t cycles;               /*  24  %clock64 cycles of the same CTAs, summed                            */
+    uint32_t ctas;                 /*  32  CTAs of the leg that ran on this SM (0: not seen in this leg)       */
+    uint32_t mark;                 /*  36  0, CRO_COMPUTE_PERSISTENT or CRO_COMPUTE_INTERMITTENT                */
+} cro_compute_sm_leg;              /*  40 bytes */
+
+typedef struct cro_compute_sm {
+    uint32_t smid;                 /*   0 */
+    uint32_t reserved;             /*   4 */
+    cro_compute_sm_leg leg[CRO_COMPUTE_LEGS];   /* 8 */
+} cro_compute_sm;                  /* 208 bytes */
+
+typedef struct cro_compute_fault {
+    uint32_t leg;                  /*   0  CRO_COMPUTE_LEG_*                                                    */
+    uint32_t smid;                 /*   4 */
+    uint32_t row;                  /*   8 */
+    uint32_t col;                  /*  12 */
+    int32_t  expected;             /*  16 */
+    int32_t  actual;               /*  20  as compared: float legs after cvt.rni.s32.f32                        */
+} cro_compute_fault;               /*  24 bytes */
+
+/* sms[0 .. sms_cap) receives one entry per SM seen, by SM id (*n_sms how many were written); faults[0 .. cap) the
+ * element records sorted by (leg, smid, row, col) (*n how many).  dev_index must be an in-process device (as for
+ * cro_locate_faults).  opts may be NULL: defaults.  Incomplete coverage never changes the status. */
+int  cro_probe_compute(cro_ctx *ctx, int dev_index, const cro_compute_opts *opts, cro_compute_result *out,
+                       cro_compute_sm *sms, int sms_cap, int *n_sms, cro_compute_fault *faults, int cap, int *n);
+
+/* The expected answer the call uploads: answer CRO_COMPUTE_ANSWER_S8 or _SMALL of the operands of `seed`, as
+ * CRO_COMPUTE_M * CRO_COMPUTE_N int32 values, row-major.  Host arithmetic only; no context. */
+int  cro_compute_expected(int answer, uint64_t seed, int32_t *out);
+
 /* ---- emit: encoding/json-compatible writers ------------------------------ */
 
 /* ComposableResourceStatus (api/v1alpha1/composableresource_types.go:36-41):
@@ -707,6 +848,15 @@ int  cro_emit_fault_annotations_json(const cro_fault_report *report, const cro_f
  * and only when they apply: -bottleneck ("<bdf> <speed> x<width>", with CRO_LINK_DEGRADED_BOTTLENECK), -degraded (the
  * flags' names speed, width, path, bottleneck, comma-separated) and -replays (the counter delta, when NVML answered). */
 int  cro_emit_link_annotations_json(const cro_link_result *r, char *buf, size_t cap, size_t *len);
+
+/* Additive compute annotations (cohdi.io/probe-compute-*) of a cro_probe_compute result, the same Go-marshalled map,
+ * integers and fixed spellings only: -verdict ("ok" for CRO_OK; "sm" or "all" for CRO_ERR_CHECKSUM with that verdict;
+ * "error" otherwise), -sms ("<covered>/<sm_count>", the least sms_covered over the legs run), -bad-sms (bad_sm[0 ..
+ * min(bad_sms, 16)) ascending, comma-separated; only when bad_sms > 0), -failed-legs (s8, bf16, e4m3, ffma, imad of
+ * the legs with a mismatch, a fold mismatch or an unpublished CTA, comma-separated; only when there are any),
+ * -s8-gops, -bf16-gflops, -e4m3-gflops (ops / ns, integer division; 0 when ns is 0) and -slowest-sm ("<id>
+ * <permille>" of the leg run with the largest slow_permille, the lowest leg on a tie). */
+int  cro_emit_compute_annotations_json(const cro_compute_result *r, char *buf, size_t cap, size_t *len);
 
 /* (deviceID, CDIDeviceID) from an FM ScaleUpResponse body, with the
  * res_op_status gate of internal/cdi/fti/fm/client.go:184-213.  On the error
