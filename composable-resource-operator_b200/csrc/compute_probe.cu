@@ -1,0 +1,228 @@
+// compute_probe.cu — the SM compute probe (cro_probe_compute): every SM's tensor cores and ALUs against an exact answer.
+#include <map>
+#include <tuple>
+
+#include "compute.hpp"
+#include "probe_internal.hpp"
+
+namespace cro {
+
+namespace {
+// Operands of call k: seed_dev + 2^61 + k * kNonceStride.  No other seed of the device reaches it while every count
+// stays below 2^61.  The stride is odd, hence invertible mod 2^64, and 2^61 times an odd number is c * 2^61 with c odd
+// (mod 2^64), which as a signed difference is +-2^61 or +-3 * 2^61.
+//   probe nonce n:       seed_dev + n * stride equals it only when (n - k) * stride = 2^61, i.e. n - k = c * 2^61: n or
+//                        k must be at least 2^61;
+//   locator retest:      seed_dev + 2^63 needs k * stride = 2^63 - 2^61 = 3 * 2^61, so k = c * 2^61 >= 2^61;
+//   link pattern 3k'+j:  seed_dev + 2^62 + (3k' + j) * stride needs (k - 3k' - j) * stride = 2^61, so k or 3k' + j is
+//                        at least 2^61.
+// Distinct calls get distinct seeds, so no call passes on the operands an earlier call used.
+constexpr uint64_t kComputeSeedOffset = 1ull << 61;
+// Tensor legs: iterations per CTA when the caller gives none (DESIGN.md "The compute probe" for the measurement).
+constexpr uint32_t kComputeDefaultIterations = 256;
+constexpr uint32_t kComputeDefaultAluIterations = 4;
+constexpr uint32_t kComputeDefaultRounds = 4;
+constexpr uint64_t kComputeOps = 2ull * CRO_COMPUTE_M * CRO_COMPUTE_N * CRO_COMPUTE_K;   // one tile, one iteration
+constexpr int kSmWords = CRO_COMPUTE_MAX_SMS / 64;
+
+// The result of a call that computed nothing: zeroes but for what the call had settled before it stopped (`from`'s
+// seed, call number, SM count and legs).
+void blank_result(cro_compute_result* r, const cro_compute_result from, std::vector<cro_compute_sm>* sms,
+                  std::vector<cro_compute_fault>* faults) {
+    memset(r, 0, sizeof *r);
+    r->seed = from.seed;
+    r->call = from.call;
+    r->sm_count = from.sm_count;
+    r->legs = from.legs;
+    sms->clear();
+    faults->clear();
+}
+}  // namespace
+
+int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_compute_result* r, std::vector<cro_compute_sm>* sms,
+                      std::vector<cro_compute_fault>* faults) {
+    blank_result(r, cro_compute_result{}, sms, faults);
+    Device* d = dev_at(c, idx);
+    if (!d) return r->status = unknown_device(c, idx, "a GPU probed through the helper process cannot be given kernels from here");
+    const uint32_t legs = o.legs ? o.legs : CRO_COMPUTE_ALL_LEGS;
+    const uint32_t ti = o.iterations ? o.iterations : kComputeDefaultIterations;
+    const uint32_t ai = o.alu_iterations ? o.alu_iterations : kComputeDefaultAluIterations;
+    const uint32_t iters[CRO_COMPUTE_LEGS] = {ti, ti, ti, ai, ai};   // s8, bf16, e4m3 tensor legs; ffma, imad ALU legs
+    const uint32_t max_rounds = o.max_rounds ? o.max_rounds : kComputeDefaultRounds;
+    const bool inj = o.test_inject_mask != 0;
+    if ((legs & ~CRO_COMPUTE_ALL_LEGS) || iters[0] > CRO_COMPUTE_MAX_ITERATIONS || iters[3] > CRO_COMPUTE_MAX_ALU_ITERATIONS ||
+        max_rounds > CRO_COMPUTE_MAX_ROUNDS ||
+        (inj && (o.test_inject_leg < 0 || o.test_inject_leg >= CRO_COMPUTE_LEGS || o.test_inject_sm < -1 ||
+                 o.test_inject_sm >= CRO_COMPUTE_MAX_SMS || o.test_inject_row < -1 || o.test_inject_row >= CRO_COMPUTE_M ||
+                 o.test_inject_col < -1 || o.test_inject_col >= CRO_COMPUTE_N ||
+                 o.test_inject_iteration >= iters[o.test_inject_leg]))) {
+        c->set_error("compute probe: legs must be CRO_COMPUTE_ALL_LEGS bits, iterations at most " +
+                     std::to_string(CRO_COMPUTE_MAX_ITERATIONS) + ", alu_iterations at most " +
+                     std::to_string(CRO_COMPUTE_MAX_ALU_ITERATIONS) + ", max_rounds at most " +
+                     std::to_string(CRO_COMPUTE_MAX_ROUNDS) + ", and an injection must name a leg, an SM id below " +
+                     std::to_string(CRO_COMPUTE_MAX_SMS) + " (or -1), a row, a column (or -1) and an iteration the leg runs");
+        return r->status = CRO_ERR_INVALID_ARG;
+    }
+    DeviceGuard g = enter_device(c, idx);
+    if (g.rc) return r->status = g.rc;
+    std::map<uint32_t, cro_compute_sm> per_sm;
+    cudaEvent_t ev[2] = {nullptr, nullptr};     // the call's own, destroyed on every way out
+    int rc = [&]() -> int {
+        const int grid = d->plan.sm_count;
+        const uint64_t k = d->compute_calls++;
+        const uint64_t seed = d->seed_dev + kComputeSeedOffset + k * kNonceStride;
+        r->seed = seed;
+        r->call = k;
+        r->sm_count = (uint32_t)grid;
+        r->legs = legs;
+        std::vector<int32_t> tiles(2 * (size_t)compute::kTile);
+        const uint64_t h0 = now_ns();
+        compute::Expected(CRO_COMPUTE_ANSWER_S8, seed, tiles.data());
+        compute::Expected(CRO_COMPUTE_ANSWER_SMALL, seed, tiles.data() + compute::kTile);
+        r->host_ref_ns = now_ns() - h0;
+        const uint64_t cta_fold[2] = {compute::CtaFold(tiles.data()), compute::CtaFold(tiles.data() + compute::kTile)};
+
+        // [tiles][per leg: sm bitmap, claims][per leg: records][CTA records], allocated per call
+        const size_t tile_bytes = tiles.size() * sizeof(int32_t);
+        const size_t ctr_off = tile_bytes, ctr_bytes = (size_t)CRO_COMPUTE_LEGS * (kSmWords + 1) * 8;
+        const size_t rec_off = ctr_off + ctr_bytes, rec_bytes = (size_t)CRO_COMPUTE_LEGS * CRO_COMPUTE_RECORDS * sizeof(cro_compute_fault);
+        const size_t cta_off = (rec_off + rec_bytes + 63) & ~(size_t)63, cta_bytes = (size_t)grid * sizeof(ComputeCta);
+        DeviceMem<unsigned char> b;
+        CU_TRY(c, cudaMalloc(&b.p, cta_off + cta_bytes));
+        for (cudaEvent_t& x : ev) CU_TRY(c, cudaEventCreate(&x));
+        cudaStream_t st = d->stream;
+        CU_TRY(c, cudaMemcpyAsync(b.p, tiles.data(), tile_bytes, cudaMemcpyHostToDevice, st));
+        CU_TRY(c, cudaMemsetAsync(b.p + ctr_off, 0, ctr_bytes, st));
+        unsigned long long* ctr = reinterpret_cast<unsigned long long*>(b.p + ctr_off);
+        ComputeCta* cta = reinterpret_cast<ComputeCta*>(b.p + cta_off);
+        std::vector<ComputeCta> hc((size_t)grid);
+        unsigned long long hbits[kSmWords + 1];
+
+        for (uint32_t leg = 0; leg < CRO_COMPUTE_LEGS; ++leg) {
+            if (!(legs >> leg & 1u)) continue;
+            cro_compute_leg& R = r->leg[leg];
+            const int answer = (leg == CRO_COMPUTE_LEG_S8 || leg == CRO_COMPUTE_LEG_IMAD) ? 0 : 1;
+            ComputeArgs a{};
+            a.expect = reinterpret_cast<const int*>(b.p) + (size_t)answer * compute::kTile;
+            a.cta = cta;
+            a.sm_bits = ctr + (size_t)leg * (kSmWords + 1);
+            a.claims = a.sm_bits + kSmWords;
+            a.rec = reinterpret_cast<cro_compute_fault*>(b.p + rec_off) + (size_t)leg * CRO_COMPUTE_RECORDS;
+            a.seed = seed;
+            a.stamp = k;
+            a.iterations = iters[leg];
+            a.inj_sm = o.test_inject_sm;
+            a.inj_row = o.test_inject_row;
+            a.inj_col = o.test_inject_col;
+            a.inj_iter = o.test_inject_iteration;
+            a.inj_mask = (inj && (uint32_t)o.test_inject_leg == leg) ? o.test_inject_mask : 0u;
+            R.iterations = iters[leg];
+            R.expect_fold = (uint64_t)iters[leg] * cta_fold[answer];
+            uint32_t fold_sm = ~0u;
+            do {
+                CU_TRY(c, cudaMemsetAsync(cta, 0xFF, cta_bytes, st));        // armed: a CTA that does not publish stays so
+                CU_TRY(c, cudaEventRecord(ev[0], st));
+                CU_TRY(c, launch_compute(leg, a, grid, st));
+                CU_TRY(c, cudaEventRecord(ev[1], st));
+                c->launches++;
+                CU_TRY(c, cudaMemcpyAsync(hc.data(), cta, cta_bytes, cudaMemcpyDeviceToHost, st));
+                CU_TRY(c, cudaMemcpyAsync(hbits, a.sm_bits, sizeof hbits, cudaMemcpyDeviceToHost, st));
+                const int e = wait_stream(c, d);
+                if (e) return e;
+                float ms = 0;
+                CU_TRY(c, cudaEventElapsedTime(&ms, ev[0], ev[1]));
+                R.ns += ms_to_ns(ms);
+                R.rounds++;
+                R.ctas += (uint32_t)grid;
+                R.ops += kComputeOps * iters[leg] * (uint64_t)grid;
+                uint64_t t0 = ~0ull, t1 = 0;
+                for (const ComputeCta& x : hc) {
+                    if (x.stamp != k) {
+                        R.unpublished++;
+                        continue;
+                    }
+                    if (x.nsmid > CRO_COMPUTE_MAX_SMS) {
+                        c->set_error("compute probe: the device reports %nsmid = " + std::to_string(x.nsmid) +
+                                     ", more SM ids than the " + std::to_string(CRO_COMPUTE_MAX_SMS) + " the coverage bitmaps hold");
+                        return CRO_ERR_UNSUPPORTED;
+                    }
+                    r->nsmid = x.nsmid;
+                    t0 = std::min<uint64_t>(t0, x.t0);
+                    t1 = std::max<uint64_t>(t1, x.t1);
+                    cro_compute_sm& S = per_sm[x.smid];
+                    S.smid = x.smid;
+                    cro_compute_sm_leg& SL = S.leg[leg];
+                    SL.ctas++;
+                    SL.mismatches += x.mismatches;
+                    SL.fold_mismatches += x.fold_mismatches;
+                    SL.ns += x.t1 > x.t0 ? x.t1 - x.t0 : 0;
+                    SL.cycles += x.cycles;
+                    R.mismatches += x.mismatches;
+                    R.fold_mismatches += x.fold_mismatches;
+                    if (x.smid < fold_sm) {
+                        fold_sm = x.smid;
+                        R.fold = x.fold;
+                    }
+                }
+                if (t1 > t0) R.timer_ns += t1 - t0;
+                R.sms_covered = 0;
+                for (int w = 0; w < kSmWords; ++w) R.sms_covered += (uint32_t)__builtin_popcountll(hbits[w]);
+            } while (R.sms_covered < (uint32_t)grid && R.rounds < max_rounds);
+            R.complete = R.sms_covered >= (uint32_t)grid ? 1u : 0u;
+            R.recorded = std::min<uint64_t>(hbits[kSmWords], CRO_COMPUTE_RECORDS);
+            if (R.recorded) {
+                std::vector<cro_compute_fault> f((size_t)R.recorded);
+                CU_TRY(c, cudaMemcpy(f.data(), a.rec, f.size() * sizeof(cro_compute_fault), cudaMemcpyDeviceToHost));
+                faults->insert(faults->end(), f.begin(), f.end());
+            }
+            // per SM: marks, failed SMs, and the slowest SM's cycles per iteration against the median
+            std::vector<std::pair<uint64_t, uint32_t>> per_iter;
+            for (auto& kv : per_sm) {
+                cro_compute_sm_leg& SL = kv.second.leg[leg];
+                if (!SL.ctas) continue;
+                SL.mark = SL.mismatches ? CRO_COMPUTE_PERSISTENT : SL.fold_mismatches ? CRO_COMPUTE_INTERMITTENT : 0u;
+                if (SL.mark) R.failed_sms++;
+                per_iter.push_back({SL.cycles / ((uint64_t)SL.ctas * iters[leg]), kv.first});
+            }
+            if (!per_iter.empty()) {
+                std::vector<uint64_t> v;
+                for (auto& p : per_iter) v.push_back(p.first);
+                std::sort(v.begin(), v.end());
+                const uint64_t median = v[v.size() / 2];
+                auto worst = per_iter.front();
+                for (auto& p : per_iter)
+                    if (p.first > worst.first) worst = p;
+                R.slowest_sm = worst.second;
+                R.slow_permille = median ? (uint32_t)std::min<uint64_t>(worst.first * 1000 / median, 0xFFFFFFFFu) : 0u;
+            }
+        }
+        return CRO_OK;
+    }();
+    for (cudaEvent_t x : ev)
+        if (x) cudaEventDestroy(x);
+    if (rc) {
+        blank_result(r, *r, sms, faults);
+        return r->status = rc;
+    }
+    bool all = false, any = false;
+    for (uint32_t leg = 0; leg < CRO_COMPUTE_LEGS; ++leg) {
+        const cro_compute_leg& R = r->leg[leg];
+        if (!(r->legs >> leg & 1u)) continue;
+        if (R.unpublished || (R.failed_sms && R.failed_sms == R.sms_covered)) all = true;
+        if (R.unpublished || R.failed_sms) any = true;
+    }
+    for (auto& kv : per_sm) {
+        bool bad = false;
+        for (const cro_compute_sm_leg& SL : kv.second.leg) bad = bad || SL.mark != 0;
+        if (bad && r->bad_sms < 16) r->bad_sm[r->bad_sms] = (uint16_t)kv.first;
+        if (bad) r->bad_sms++;
+        sms->push_back(kv.second);
+    }
+    std::sort(faults->begin(), faults->end(), [](const cro_compute_fault& x, const cro_compute_fault& y) {
+        return std::make_tuple(x.leg, x.smid, x.row, x.col) < std::make_tuple(y.leg, y.smid, y.row, y.col);
+    });
+    r->verdict = all ? CRO_COMPUTE_ALL : any ? CRO_COMPUTE_SM : CRO_COMPUTE_NONE;
+    return r->status = any ? CRO_ERR_CHECKSUM : CRO_OK;
+}
+
+}  // namespace cro

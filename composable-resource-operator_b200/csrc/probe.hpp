@@ -47,6 +47,9 @@ struct Lane {
     std::chrono::steady_clock::time_point since{};
 };
 
+class MismatchBuffer;   // probe_internal.hpp
+struct LinkState;
+
 struct Device {
     int ordinal = -1;              // CUDA ordinal
     int index = -1;                // rank: position in the minor-sorted list
@@ -70,23 +73,9 @@ struct Device {
     // when half_known[h], else nothing it can compare against (never written, a peer's push, a locator retest).
     bool half_known[2] = {false, false};
     uint64_t half_seed[2] = {0, 0};
-    // fault locator (ctx_locate): counters, records, granule bitmaps and result slots, allocated at its first call
-    unsigned char* d_locate = nullptr;
-    unsigned char* h_locate = nullptr;     // pinned mirror
-    size_t locate_bytes = 0;
-    SweepScratch scratch_loc{};
-    // host link probe (ctx_probe_host_link), allocated at its first call: pinned host buffers H0 and H1 (link_cap bytes
-    // each, mapped into the device's address space) and the 8 MiB chase table, all from pcilink::MapOnNode; the
-    // device-side counters, records and slots; two role scratches; timing events
-    unsigned char* h_link[2] = {nullptr, nullptr};
-    uint64_t link_cap = 0;
-    unsigned long long* h_link_chase = nullptr;
-    unsigned char* d_link = nullptr;
-    unsigned char* h_link_out = nullptr;   // pinned mirror of d_link
-    size_t link_bytes = 0;
-    SweepScratch scratch_link[2]{};
-    std::vector<cudaEvent_t> ev_link;
-    uint64_t link_calls = 0;               // k of the next call: its seeds
+    std::unique_ptr<MismatchBuffer> locate;   // fault locator (ctx_locate), made at its first call
+    std::unique_ptr<LinkState> link;       // host link probe (ctx_probe_host_link), made at its first call
+    uint64_t link_calls = 0;               // k of the next host link probe call: its seeds
     uint64_t compute_calls = 0;            // k of the next compute probe call (ctx_probe_compute): its operand seed
     KernelPlan plan{};
     SweepScratch scratch{}, scratch_aux{}, scratch_pfx{};   // main stream / closed form / p2p prefix closed form
@@ -119,8 +108,9 @@ struct Device {
     Device() = default;
     Device(const Device&) = delete;
     Device& operator=(const Device&) = delete;
-    // Releases every CUDA object this device owns (probe.cu).  Runs for half-built devices too,
-    // so a cro_probe_init that fails midway (OOM on the sweep region) leaks nothing.
+    // Releases every CUDA object this device owns (probe.cu; the probes' own state goes with its owners, after the
+    // streams are synchronised).  Runs for half-built devices too, so a cro_probe_init that fails midway (OOM on the
+    // sweep region) leaks nothing.
     ~Device();
 };
 
