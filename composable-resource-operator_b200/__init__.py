@@ -301,10 +301,67 @@ class ComputeFault(ctypes.Structure):
                 ("expected", ctypes.c_int32), ("actual", ctypes.c_int32)]
 
 
+# whole-HBM scan (cro_scan_hbm, cro_scan_hbm_uuid, cro_read_hbm_health)
+SCAN_CHUNK_BYTES, SCAN_RESERVE_BYTES, SCAN_MAX_CHUNKS, SCAN_PASSES, SCAN_ELEMENTS = 2 << 30, 1 << 30, 128, 2, 4
+(SCAN_HEALTH_ECC_CORRECTED_DURING, SCAN_HEALTH_ECC_UNCORRECTED_DURING, SCAN_HEALTH_REMAP_PENDING,
+ SCAN_HEALTH_REMAP_FAILURE) = 1, 2, 4, 8
+HBM_NVML_ECC_CORRECTED, HBM_NVML_ECC_UNCORRECTED, HBM_NVML_REMAP, HBM_NVML_HISTOGRAM = 1, 2, 4, 8
+
+
+class ScanOpts(ctypes.Structure):
+    _fields_ = [("max_bytes", ctypes.c_uint64), ("reserve_bytes", ctypes.c_uint64), ("seed", ctypes.c_uint64),
+                ("deadline_ms", ctypes.c_int32), ("reserved0", ctypes.c_uint32), ("test_chunk_bytes", ctypes.c_uint64),
+                ("test_force_first", ctypes.c_uint64), ("test_force_count", ctypes.c_uint64),
+                ("test_force_and", ctypes.c_uint64), ("test_force_or", ctypes.c_uint64)]
+
+
+class HbmHealth(ctypes.Structure):
+    """cro_hbm_health: NVML's DRAM ECC counts and row-remapping state; `nvml` has a HBM_NVML_* bit per read answered."""
+    _fields_ = [("nvml", ctypes.c_uint32), ("remap_corrected", ctypes.c_uint32), ("remap_uncorrected", ctypes.c_uint32),
+                ("remap_pending", ctypes.c_uint32), ("remap_failure", ctypes.c_uint32), ("histogram", ctypes.c_uint32 * 5),
+                ("ecc_corrected", ctypes.c_uint64), ("ecc_uncorrected", ctypes.c_uint64)]
+
+
+class ScanPass(ctypes.Structure):
+    _fields_ = [("invert", ctypes.c_uint64), ("words_scanned", ctypes.c_uint64), ("mismatches", ctypes.c_uint64),
+                ("recorded", ctypes.c_uint64), ("granules", ctypes.c_uint64), ("bit_flips", ctypes.c_uint64 * 64)]
+
+
+class ScanChunk(ctypes.Structure):
+    _fields_ = [("word0", ctypes.c_uint64), ("bytes", ctypes.c_uint64), ("fold_xor", ctypes.c_uint64 * 2),
+                ("fold_sum", ctypes.c_uint64 * 2), ("fold_wsum", ctypes.c_uint64 * 2), ("expect_xor", ctypes.c_uint64),
+                ("expect_sum", ctypes.c_uint64), ("expect_wsum", ctypes.c_uint64)]
+
+    def fold(self, p: int) -> Tuple[int, int, int]:
+        """Checksum (xor, sum, weighted sum) of the chunk as compare pass p read it."""
+        return (self.fold_xor[p], self.fold_sum[p], self.fold_wsum[p])
+
+    @property
+    def expect(self) -> Tuple[int, int, int]:
+        return (self.expect_xor, self.expect_sum, self.expect_wsum)
+
+
+class ScanReport(ctypes.Structure):
+    """cro_scan_report: sizes, seed, per-pass counts, per-chunk folds, element times and NVML health of one scan."""
+    _fields_ = [("status", ctypes.c_int32), ("cuda_error", ctypes.c_int32), ("health", ctypes.c_uint32),
+                ("complete", ctypes.c_uint32), ("seed", ctypes.c_uint64), ("total_bytes", ctypes.c_uint64),
+                ("free_bytes", ctypes.c_uint64), ("held_bytes", ctypes.c_uint64), ("covered_bytes", ctypes.c_uint64),
+                ("n_chunks", ctypes.c_uint32), ("elements_done", ctypes.c_uint32), ("located", ctypes.c_uint64),
+                ("recorded", ctypes.c_uint64), ("flip_or", ctypes.c_uint64), ("element_ns", ctypes.c_uint64 * SCAN_ELEMENTS),
+                ("alloc_ns", ctypes.c_uint64), ("nvml_ns", ctypes.c_uint64), ("wall_ns", ctypes.c_uint64),
+                ("helper_ns", ctypes.c_uint64), ("before", HbmHealth), ("after", HbmHealth),
+                ("pass_", ScanPass * SCAN_PASSES), ("chunk", ScanChunk * SCAN_MAX_CHUNKS)]
+
+    def place(self, w: "FaultWord") -> Tuple[int, int]:
+        """(chunk number, word offset in the chunk) of a scan word."""
+        return w.reserved, w.word_index - self.chunk[w.reserved].word0
+
+
 assert ctypes.sizeof(ProbeResult) == 512, ctypes.sizeof(ProbeResult)
 assert ctypes.sizeof(ComputeResult) == 600 and ctypes.sizeof(ComputeSm) == 208, ctypes.sizeof(ComputeResult)
 assert ctypes.sizeof(FaultReport) == 928 and ctypes.sizeof(LocatePass) == 120, ctypes.sizeof(FaultReport)
 assert ctypes.sizeof(LinkResult) == 984 and ctypes.sizeof(PciPath) == 272, ctypes.sizeof(LinkResult)
+assert ctypes.sizeof(ScanReport) == 12632 and ctypes.sizeof(ScanOpts) == 72, ctypes.sizeof(ScanReport)
 
 # Every symbol include/croprobe.h declares; tests check the library exports all of them.
 EXPORTS = [
@@ -329,6 +386,7 @@ EXPORTS = [
     "cro_locate_faults", "cro_emit_fault_annotations_json",
     "cro_probe_host_link", "cro_pci_link_path", "cro_emit_link_annotations_json",
     "cro_probe_compute", "cro_compute_expected", "cro_emit_compute_annotations_json",
+    "cro_scan_hbm", "cro_scan_hbm_uuid", "cro_read_hbm_health", "cro_emit_scan_annotations_json",
 ]
 
 # Slot map of a device's sweep-slot array (cro_sweep_slot, 64 bytes each); the cro_selftest_* hooks take such arrays.
@@ -427,6 +485,12 @@ def _load() -> ctypes.CDLL:
                                     ctypes.POINTER(i32)]),
         "cro_compute_expected": (i32, [i32, u64, ctypes.POINTER(ctypes.c_int32)]),
         "cro_emit_compute_annotations_json": (i32, [ctypes.POINTER(ComputeResult)] + out),
+        "cro_scan_hbm": (i32, [vp, i32, ctypes.POINTER(ScanOpts), ctypes.POINTER(ScanReport), ctypes.POINTER(FaultWord), i32,
+                               ctypes.POINTER(i32)]),
+        "cro_scan_hbm_uuid": (i32, [vp, c, ctypes.POINTER(ScanOpts), ctypes.POINTER(ScanReport), ctypes.POINTER(FaultWord), i32,
+                                    ctypes.POINTER(i32)]),
+        "cro_read_hbm_health": (i32, [c, ctypes.POINTER(HbmHealth)]),
+        "cro_emit_scan_annotations_json": (i32, [ctypes.POINTER(ScanReport)] + out),
         "cro_local_node_op": (i32, [vp, c] + out),
         "cro_local_exec": (i32, [c] + out),
         "cro_describe_wire_type": (i32, [c] + out),
@@ -565,6 +629,47 @@ def emit_link_annotations_json(r: LinkResult) -> str:
 def emit_compute_annotations_json(r: ComputeResult) -> str:
     """Additive cohdi.io/probe-compute-* annotations of a probe_compute result (Go-marshalled map[string]string)."""
     return _text(lib.cro_emit_compute_annotations_json, ctypes.byref(r))
+
+
+def emit_scan_annotations_json(r: ScanReport) -> str:
+    """Additive cohdi.io/hbm-scan-* annotations of a scan report (Go-marshalled map[string]string)."""
+    return _text(lib.cro_emit_scan_annotations_json, ctypes.byref(r))
+
+
+def read_hbm_health(uuid: str) -> HbmHealth:
+    """cro_read_hbm_health: the GPU's DRAM ECC counts and row-remapping state from NVML (no context, no CUDA)."""
+    h = HbmHealth()
+    rc = lib.cro_read_hbm_health(_b(uuid), ctypes.byref(h))
+    if rc != OK:
+        raise ProbeError(rc, "cro_read_hbm_health")
+    return h
+
+
+def _scan_opts(max_bytes: int, reserve_bytes: int, seed: int, deadline_ms: int, chunk_bytes: int,
+               force: Optional[Tuple[int, int, int, int]]) -> ScanOpts:
+    o = ScanOpts()
+    o.max_bytes, o.reserve_bytes, o.seed, o.deadline_ms, o.test_chunk_bytes = max_bytes, reserve_bytes, seed, deadline_ms, chunk_bytes
+    if force is not None:
+        o.test_force_first, o.test_force_count, o.test_force_and, o.test_force_or = force
+    return o
+
+
+def scan_hbm_uuid(ctx: Optional["ProbeContext"], uuid: str, max_bytes: int = 0, reserve_bytes: int = 0, seed: int = 0,
+                  deadline_ms: int = 0, cap: int = 256, chunk_bytes: int = 0,
+                  force: Optional[Tuple[int, int, int, int]] = None) -> Tuple[ScanReport, List[FaultWord]]:
+    """cro_scan_hbm_uuid: the whole-HBM scan of any GPU on the node, run by the helper process (ctx may be None).
+    Returns the report (its status is OK, ERR_CHECKSUM or ERR_CUDA) and up to `cap` mismatching words."""
+    o = _scan_opts(max_bytes, reserve_bytes, seed, deadline_ms, chunk_bytes, force)
+    rep = ScanReport()
+    arr = (FaultWord * max(1, cap))()
+    n = ctypes.c_int()
+    handle = ctx.handle if ctx is not None else None
+    rc = lib.cro_scan_hbm_uuid(handle, _b(uuid), ctypes.byref(o), ctypes.byref(rep), arr, cap, ctypes.byref(n))
+    if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
+        buf = ctypes.create_string_buffer(1024)
+        lib.cro_last_error(handle, buf, 1024)
+        raise ProbeError(rc, buf.value.decode("utf-8", "replace"))
+    return rep, [arr[i] for i in range(n.value)]
 
 
 def compute_expected(answer: int, seed: int) -> List[int]:
@@ -814,6 +919,21 @@ class ProbeContext:
         self._check(lib.cro_probe_compute(self.handle, dev, ctypes.byref(o), ctypes.byref(r), sms, COMPUTE_MAX_SMS,
                                           ctypes.byref(n_sms), arr, cap, ctypes.byref(n)), allow=(ERR_CHECKSUM,))
         return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
+
+    def scan_hbm(self, dev: int = 0, max_bytes: int = 0, reserve_bytes: int = 0, seed: int = 0, cap: int = 256,
+                 chunk_bytes: int = 0, force: Optional[Tuple[int, int, int, int]] = None) -> Tuple[ScanReport, List[FaultWord]]:
+        """cro_scan_hbm: fills every chunk of the free memory this process can allocate (min(max_bytes, free -
+        reserve_bytes); 0 = all / 1 GiB) with a pattern, compares, fills its complement, compares.  seed = 0: a fresh
+        one, reported.  chunk_bytes and force = (first, count, and_mask, or_mask) are the test-only chunk size and stuck
+        cells.  Returns the report (its status is OK, ERR_CHECKSUM or ERR_CUDA) and up to `cap` mismatching words;
+        report.place(word) is its (chunk, offset)."""
+        o = _scan_opts(max_bytes, reserve_bytes, seed, 0, chunk_bytes, force)
+        rep = ScanReport()
+        arr = (FaultWord * max(1, cap))()
+        n = ctypes.c_int()
+        self._check(lib.cro_scan_hbm(self.handle, dev, ctypes.byref(o), ctypes.byref(rep), arr, cap, ctypes.byref(n)),
+                    allow=(ERR_CHECKSUM, ERR_CUDA))
+        return rep, [arr[i] for i in range(n.value)]
 
     def launch_count(self) -> int:
         return int(lib.cro_launch_count(self.handle))

@@ -60,6 +60,13 @@ static_assert(sizeof(cro_compute_result) == 600 && offsetof(cro_compute_result, 
                   offsetof(cro_compute_leg, fold) == 88,
               "compute layout");
 
+static_assert(sizeof(cro_scan_opts) == 72 && sizeof(cro_hbm_health) == 56 && sizeof(cro_scan_pass) == 552 &&
+                  sizeof(cro_scan_chunk) == 88, "scan layout");
+static_assert(sizeof(cro_scan_report) == 12632 && offsetof(cro_scan_report, element_ns) == 88 &&
+                  offsetof(cro_scan_report, before) == 152 && offsetof(cro_scan_report, pass) == 264 &&
+                  offsetof(cro_scan_report, chunk) == 1368 && offsetof(cro_hbm_health, ecc_corrected) == 40,
+              "scan layout");
+
 using namespace cro::capi;
 
 
@@ -325,6 +332,42 @@ int cro_probe_compute(cro_ctx* ctx, int i, const cro_compute_opts* opts, cro_com
     *n_sms = (int)ks;
     *n = (int)kf;
     return rc;
+} CRO_API_CATCH
+// The scan's two forms share the copy-out: words[0 .. cap), recorded and complete as cro_locate_faults sets them.
+static int scan_out(int rc, const std::vector<cro_fault_word>& found, cro_scan_report* out, cro_fault_word* words, int cap, int* n) {
+    const size_t k = std::min(found.size(), (size_t)cap);
+    for (size_t j = 0; j < k; ++j) words[j] = found[j];
+    out->recorded = k;
+    if (k < found.size()) out->complete = 0;        // the caller's list misses some words
+    *n = (int)k;
+    return rc;
+}
+int cro_scan_hbm(cro_ctx* ctx, int i, const cro_scan_opts* opts, cro_scan_report* out, cro_fault_word* words, int cap, int* n) try {
+    if (!ctx || !out || !n || cap < 0 || (cap > 0 && !words)) return CRO_ERR_INVALID_ARG;
+    *n = 0;
+    cro_scan_opts o{};
+    if (opts) o = *opts;
+    std::vector<cro_fault_word> found;
+    const int rc = ctx_scan_hbm(ctx, i, o, out, &found);
+    return scan_out(rc, found, out, words, cap, n);
+} CRO_API_CATCH
+int cro_scan_hbm_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_scan_opts* opts, cro_scan_report* out, cro_fault_word* words,
+                      int cap, int* n) try {
+    if (!gpu_uuid || !out || !n || cap < 0 || (cap > 0 && !words)) return CRO_ERR_INVALID_ARG;
+    *n = 0;
+    cro_scan_opts o{};
+    if (opts) o = *opts;
+    std::vector<cro_fault_word> found;
+    const int rc = ctx_scan_hbm_uuid(ctx, gpu_uuid, o, out, &found, cap);
+    const uint32_t complete = out->complete;
+    scan_out(rc, found, out, words, cap, n);
+    out->complete = complete && found.size() <= (size_t)cap;
+    return rc;
+} CRO_API_CATCH
+int cro_read_hbm_health(const char* gpu_uuid, cro_hbm_health* out) try {
+    if (!gpu_uuid || !out) return CRO_ERR_INVALID_ARG;
+    identity::NvmlHbmHealth(gpu_uuid, true, out);
+    return CRO_OK;
 } CRO_API_CATCH
 int cro_compute_expected(int answer, uint64_t seed, int32_t* out) try {
     return compute::Expected(answer, seed, out);
@@ -644,6 +687,44 @@ int cro_emit_compute_annotations_json(const cro_compute_result* r, char* buf, si
     m[p + "e4m3-gflops"] = rate(CRO_COMPUTE_LEG_E4M3);
     if (worst < CRO_COMPUTE_LEGS)
         m[p + "slowest-sm"] = std::to_string(r->leg[worst].slowest_sm) + " " + std::to_string(r->leg[worst].slow_permille);
+    gojson::Writer w;
+    w.string_map(m);
+    return copy_out(w.str(), buf, cap, len);
+} CRO_API_CATCH
+
+int cro_emit_scan_annotations_json(const cro_scan_report* r, char* buf, size_t cap, size_t* len) try {
+    if (!r) return CRO_ERR_INVALID_ARG;
+    static const char* const kHealth[4] = {"ecc-corrected", "ecc-uncorrected", "remap-pending", "remap-failure"};
+    std::map<std::string, std::string> m;
+    const std::string p = "cohdi.io/hbm-scan-";
+    m[p + "verdict"] = r->status == CRO_OK            ? "ok"
+                       : r->status == CRO_ERR_CHECKSUM ? "corrupt"
+                       : r->status == CRO_ERR_CUDA     ? "cuda-error:" + std::to_string(r->cuda_error)
+                                                       : "error";
+    m[p + "covered-bytes"] = std::to_string(r->covered_bytes);
+    m[p + "free-bytes"] = std::to_string(r->free_bytes);
+    m[p + "seed"] = hex16(r->seed);
+    m[p + "mismatches"] = std::to_string(r->pass[0].mismatches) + "," + std::to_string(r->pass[1].mismatches);
+    m[p + "granules"] = std::to_string(r->pass[0].granules) + "," + std::to_string(r->pass[1].granules);
+    uint64_t ns = 0;
+    for (uint64_t e : r->element_ns) ns += e;
+    m[p + "gbs"] = std::to_string(ns ? (uint64_t)((unsigned __int128)r->covered_bytes * 4u / ns) : 0ull);
+    std::string bits, health;
+    for (int b = 0; b < 64; ++b)
+        if (r->pass[0].bit_flips[b] || r->pass[1].bit_flips[b]) bits += (bits.empty() ? "" : ",") + std::to_string(b);
+    if (!bits.empty()) m[p + "bits"] = bits;
+    for (int b = 0; b < 4; ++b)
+        if (r->health >> b & 1u) health += (health.empty() ? "" : ",") + std::string(kHealth[b]);
+    if (!health.empty()) m[p + "health"] = health;
+    const cro_hbm_health &B = r->before, &A = r->after;
+    if (B.nvml & A.nvml & CRO_HBM_NVML_ECC_CORRECTED) m[p + "ecc-corrected"] = std::to_string(A.ecc_corrected - B.ecc_corrected);
+    if (B.nvml & A.nvml & CRO_HBM_NVML_ECC_UNCORRECTED) m[p + "ecc-uncorrected"] = std::to_string(A.ecc_uncorrected - B.ecc_uncorrected);
+    if (A.nvml & CRO_HBM_NVML_REMAP) m[p + "remapped"] = std::to_string(A.remap_corrected) + "," + std::to_string(A.remap_uncorrected);
+    if (A.nvml & CRO_HBM_NVML_HISTOGRAM) {
+        std::string h;
+        for (int b = 0; b < 5; ++b) h += (b ? "," : "") + std::to_string(A.histogram[b]);
+        m[p + "remap-histogram"] = h;
+    }
     gojson::Writer w;
     w.string_map(m);
     return copy_out(w.str(), buf, cap, len);

@@ -13,6 +13,12 @@
  *   croprobe-cli probe <uuid|index> [sweep_MiB]      one full probe; JSON annotations on stdout, exit 0 iff status ok
  *   croprobe-cli probe-raw <uuid> [sweep_MiB]        the same, the 512-byte cro_probe_result on stdout (for the library)
  *   croprobe-cli cold <uuid|index> [sweep_MiB] [nvml] timings: init, first (cold) probe, second (warm) probe
+ *   croprobe-cli scan <uuid|index> [max_MiB]         whole-HBM scan of the free memory (all of it but 1 GiB unless
+ *                                                    max_MiB bounds it); JSON annotations, exit 0 iff status ok
+ *   croprobe-cli scan-raw <uuid> <max_bytes> <reserve_bytes> <seed> <chunk_bytes> <force_first> <force_count>
+ *                         <force_and> <force_or> <cap>
+ *                                                    the same with every cro_scan_opts field; cro_scan_report and
+ *                                                    its `recorded` cro_fault_word records (at most cap) on stdout
  * Exit 3: the device is not visible to this (fresh) process — the reference's found=false.
  *
  * Plain C against include/croprobe.h — the same surface the cgo shim binds.
@@ -42,24 +48,35 @@ static int fail(cro_ctx *ctx, const char *what, int rc) {
 int main(int argc, char **argv) {
     if (argc < 2) {
         fprintf(stderr, "usage: croprobe-cli csv <query> | enumerate | probe <uuid|index> [sweep_MiB] | probe-raw <uuid> [sweep_MiB] | "
-                        "cold <uuid|index> [sweep_MiB] [nvml]\n");
+                        "cold <uuid|index> [sweep_MiB] [nvml] | scan <uuid|index> [max_MiB] | scan-raw <uuid> <max> <reserve> <seed> <chunk> "
+                        "<first> <count> <and> <or> <cap>\n");
         return 64;
     }
     const double t_start = now_s();
     const char *cmd = argv[1];
     const int raw = strcmp(cmd, "probe-raw") == 0;
     const int cold = strcmp(cmd, "cold") == 0;
+    const int scan_raw = strcmp(cmd, "scan-raw") == 0;
+    const int wants_scan = scan_raw || strcmp(cmd, "scan") == 0;
     const int wants_probe = raw || cold || strcmp(cmd, "probe") == 0;
-    if (wants_probe && argc < 3) return 64;
+    if ((wants_probe || wants_scan) && argc < 3) return 64;
+    if (scan_raw && argc != 12) return 64;
     cro_opts opts;
     memset(&opts, 0, sizeof opts);
     opts.abi_version = CRO_ABI_VERSION;
     opts.flags = CRO_F_LAZY_ALLOC | CRO_F_DEGRADE_ON_OOM;
+    if (wants_scan) {
+        /* no sweep region (the scan allocates its own chunks) and NVML, whose DRAM health record the scan reads */
+        opts.flags = CRO_F_LAZY_ALLOC;
+        opts.sweep_bytes = 64ull << 20;
+    }
     if (wants_probe) {
         /* The hot-plug path: one device, identity from /proc (NVML's first call costs more than the probe), and a
          * 1 GiB first sweep unless told otherwise — far beyond the L2, and it shortens everything before it. */
         opts.sweep_bytes = (argc > 3 ? (uint64_t)strtoull(argv[3], NULL, 10) : 1024ull) << 20;
         if (!(cold && argc > 4 && strcmp(argv[4], "nvml") == 0)) opts.flags |= CRO_F_NO_NVML;
+    }
+    if (wants_probe || wants_scan) {
         if (strncmp(argv[2], "GPU-", 4) == 0) {
             /* before ANY CUDA call: this process's cuInit must enumerate that one GPU only (one primary context
              * instead of eight on a full box) */
@@ -78,7 +95,7 @@ int main(int argc, char **argv) {
         printf("No devices were found\n");
         return 0;
     }
-    if (rc == CRO_ERR_NO_DEVICE && wants_probe && strncmp(argv[2], "GPU-", 4) == 0) {
+    if (rc == CRO_ERR_NO_DEVICE && (wants_probe || wants_scan) && strncmp(argv[2], "GPU-", 4) == 0) {
         fprintf(stderr, "croprobe-cli: device '%s' is not visible\n", argv[2]);   /* found=0, like gpus.go:896-898 */
         return 3;
     }
@@ -104,7 +121,7 @@ int main(int argc, char **argv) {
                    devs[i].dev_index, devs[i].device_minor, devs[i].gpu_uuid, devs[i].pci_bus_id, devs[i].name,
                    (devs[i].flags & CRO_DEV_IN_PROCESS) ? "true" : "false");
         printf("]\n");
-    } else if (wants_probe) {
+    } else if (wants_probe || wants_scan) {
         int idx = -1;
         for (int i = 0; i < n; ++i)
             if ((devs[i].flags & CRO_DEV_IN_PROCESS) && (strcmp(devs[i].gpu_uuid, argv[2]) == 0 || strncmp(argv[2], "GPU-", 4) != 0))
@@ -113,6 +130,37 @@ int main(int argc, char **argv) {
             fprintf(stderr, "croprobe-cli: device '%s' is not visible\n", argv[2]);
             cro_probe_destroy(ctx);
             return 3;
+        }
+        if (wants_scan) {
+            cro_scan_opts so;
+            memset(&so, 0, sizeof so);
+            int cap = 256;
+            if (scan_raw) {
+                uint64_t *f[] = {&so.max_bytes, &so.reserve_bytes, &so.seed, &so.test_chunk_bytes, &so.test_force_first,
+                                 &so.test_force_count, &so.test_force_and, &so.test_force_or};
+                for (int k = 0; k < 8; ++k) *f[k] = (uint64_t)strtoull(argv[3 + k], NULL, 10);
+                cap = atoi(argv[11]);
+            } else if (argc > 3) {
+                so.max_bytes = (uint64_t)strtoull(argv[3], NULL, 10) << 20;
+            }
+            static cro_scan_report sr;
+            cro_fault_word *words = (cro_fault_word *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *words);
+            int got = 0;
+            if (!words) return 2;
+            rc = cro_scan_hbm(ctx, idx, &so, &sr, words, cap, &got);
+            if (scan_raw) {
+                /* the report whatever its status: the library reads why from it */
+                if (fwrite(&sr, sizeof sr, 1, stdout) != 1 || (got && fwrite(words, sizeof *words, (size_t)got, stdout) != (size_t)got))
+                    return 2;
+                fflush(stdout);
+                _exit(sr.status == CRO_OK ? 0 : 1);    /* the chunks go with the process */
+            }
+            if (rc != CRO_OK && rc != CRO_ERR_CHECKSUM && rc != CRO_ERR_CUDA) return fail(ctx, "cro_scan_hbm", rc);
+            if ((rc = cro_emit_scan_annotations_json(&sr, buf, sizeof buf, &len)) != CRO_OK) return fail(ctx, "emit", rc);
+            printf("%s\n", buf);
+            free(words);
+            cro_probe_destroy(ctx);
+            return sr.status == CRO_OK ? 0 : 1;
         }
         cro_probe_result r;
         const double t1 = now_s();

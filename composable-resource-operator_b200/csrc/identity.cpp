@@ -417,16 +417,24 @@ bool ScanNvml(std::vector<NvmlGpu>* out, std::string* err) {
     return ok;
 }
 
-// One NVML session for the life of the process (init is reference-counted, so the
-// init/shutdown pairs of ScanNvml still balance): the per-probe ECC read must not pay
-// nvmlInit every time.
-bool NvmlEccUncorrected(const std::string& gpu_uuid, unsigned long long* out) {
-    struct Session {
-        int (*byUuid)(const char*, nvmlDevice_t*) = nullptr;
-        int (*ecc)(nvmlDevice_t, int, int, unsigned long long*) = nullptr;
-        bool ok = false;
-    };
-    static Session s;
+// One NVML session for the life of the process (init is reference-counted, so the init/shutdown pairs of ScanNvml
+// still balance): the per-probe ECC read, the link probe's replay counter and the scan's memory health must not pay
+// nvmlInit every time.  A reader whose symbol the library lacks answers false.
+namespace {
+struct NvmlRemapHistogram {  // nvmlRowRemapperHistogramValues_t
+    unsigned max, high, partial, low, none;
+};
+struct NvmlSession {
+    int (*byUuid)(const char*, nvmlDevice_t*) = nullptr;
+    int (*ecc)(nvmlDevice_t, int, int, unsigned long long*) = nullptr;
+    int (*replays)(nvmlDevice_t, unsigned*) = nullptr;
+    int (*memErrors)(nvmlDevice_t, int, int, int, unsigned long long*) = nullptr;
+    int (*remapped)(nvmlDevice_t, unsigned*, unsigned*, unsigned*, unsigned*) = nullptr;
+    int (*histogram)(nvmlDevice_t, NvmlRemapHistogram*) = nullptr;
+    bool ok = false;
+};
+const NvmlSession& nvml_session() {
+    static NvmlSession s;
     static std::once_flag once;
     std::call_once(once, [] {
         void* h = dlopen("libnvidia-ml.so.1", RTLD_NOW | RTLD_LOCAL);
@@ -434,38 +442,62 @@ bool NvmlEccUncorrected(const std::string& gpu_uuid, unsigned long long* out) {
         auto init = (int (*)())dlsym(h, "nvmlInit_v2");
         s.byUuid = (int (*)(const char*, nvmlDevice_t*))dlsym(h, "nvmlDeviceGetHandleByUUID");
         s.ecc = (int (*)(nvmlDevice_t, int, int, unsigned long long*))dlsym(h, "nvmlDeviceGetTotalEccErrors");
-        s.ok = init && s.byUuid && s.ecc && init() == 0;
+        s.replays = (int (*)(nvmlDevice_t, unsigned*))dlsym(h, "nvmlDeviceGetPcieReplayCounter");
+        s.memErrors = (int (*)(nvmlDevice_t, int, int, int, unsigned long long*))dlsym(h, "nvmlDeviceGetMemoryErrorCounter");
+        s.remapped = (int (*)(nvmlDevice_t, unsigned*, unsigned*, unsigned*, unsigned*))dlsym(h, "nvmlDeviceGetRemappedRows");
+        s.histogram = (int (*)(nvmlDevice_t, NvmlRemapHistogram*))dlsym(h, "nvmlDeviceGetRowRemapperHistogram");
+        s.ok = init && s.byUuid && init() == 0;
     });
-    if (!s.ok) return false;
+    return s;
+}
+bool nvml_device(const NvmlSession& s, const std::string& gpu_uuid, nvmlDevice_t* dev) {
+    return s.ok && s.byUuid(gpu_uuid.c_str(), dev) == 0;
+}
+}  // namespace
+
+bool NvmlEccUncorrected(const std::string& gpu_uuid, unsigned long long* out) {
+    const NvmlSession& s = nvml_session();
     nvmlDevice_t dev = nullptr;
-    if (s.byUuid(gpu_uuid.c_str(), &dev) != 0) return false;
+    if (!s.ecc || !nvml_device(s, gpu_uuid, &dev)) return false;
     return s.ecc(dev, /*NVML_MEMORY_ERROR_TYPE_UNCORRECTED*/ 1, /*NVML_VOLATILE_ECC*/ 0, out) == 0;
 }
 
-// The same process-wide session for the host link probe's replay counter.
 bool NvmlPcieReplays(const std::string& gpu_uuid, unsigned long long* out) {
-    struct Session {
-        int (*byUuid)(const char*, nvmlDevice_t*) = nullptr;
-        int (*replays)(nvmlDevice_t, unsigned*) = nullptr;
-        bool ok = false;
-    };
-    static Session s;
-    static std::once_flag once;
-    std::call_once(once, [] {
-        void* h = dlopen("libnvidia-ml.so.1", RTLD_NOW | RTLD_LOCAL);
-        if (!h) return;
-        auto init = (int (*)())dlsym(h, "nvmlInit_v2");
-        s.byUuid = (int (*)(const char*, nvmlDevice_t*))dlsym(h, "nvmlDeviceGetHandleByUUID");
-        s.replays = (int (*)(nvmlDevice_t, unsigned*))dlsym(h, "nvmlDeviceGetPcieReplayCounter");
-        s.ok = init && s.byUuid && s.replays && init() == 0;
-    });
-    if (!s.ok) return false;
+    const NvmlSession& s = nvml_session();
     nvmlDevice_t dev = nullptr;
-    if (s.byUuid(gpu_uuid.c_str(), &dev) != 0) return false;
+    if (!s.replays || !nvml_device(s, gpu_uuid, &dev)) return false;
     unsigned v = 0;
     if (s.replays(dev, &v) != 0) return false;
     *out = v;
     return true;
+}
+
+void NvmlHbmHealth(const std::string& gpu_uuid, bool histogram, cro_hbm_health* out) {
+    memset(out, 0, sizeof *out);
+    const NvmlSession& s = nvml_session();
+    nvmlDevice_t dev = nullptr;
+    if (!nvml_device(s, gpu_uuid, &dev)) return;
+    if (s.memErrors) {
+        // NVML_MEMORY_ERROR_TYPE_CORRECTED 0 / _UNCORRECTED 1, NVML_VOLATILE_ECC 0, NVML_MEMORY_LOCATION_DRAM 2
+        unsigned long long v = 0;
+        if (s.memErrors(dev, 0, 0, 2, &v) == 0) { out->ecc_corrected = v; out->nvml |= CRO_HBM_NVML_ECC_CORRECTED; }
+        v = 0;
+        if (s.memErrors(dev, 1, 0, 2, &v) == 0) { out->ecc_uncorrected = v; out->nvml |= CRO_HBM_NVML_ECC_UNCORRECTED; }
+    }
+    unsigned corr = 0, unc = 0, pending = 0, failure = 0;
+    if (s.remapped && s.remapped(dev, &corr, &unc, &pending, &failure) == 0) {
+        out->remap_corrected = corr;
+        out->remap_uncorrected = unc;
+        out->remap_pending = pending ? 1u : 0u;
+        out->remap_failure = failure ? 1u : 0u;
+        out->nvml |= CRO_HBM_NVML_REMAP;
+    }
+    NvmlRemapHistogram h{};
+    if (histogram && s.histogram && s.histogram(dev, &h) == 0) {
+        const unsigned v[5] = {h.max, h.high, h.partial, h.low, h.none};
+        memcpy(out->histogram, v, sizeof v);
+        out->nvml |= CRO_HBM_NVML_HISTOGRAM;
+    }
 }
 
 }  // namespace identity

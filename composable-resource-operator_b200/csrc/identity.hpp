@@ -88,6 +88,10 @@ bool NvmlEccUncorrected(const std::string& gpu_uuid, unsigned long long* out);
 // PCIe replays of the device's link since the driver was loaded (nvmlDeviceGetPcieReplayCounter); false when NVML or
 // the symbol is missing or the device refuses.
 bool NvmlPcieReplays(const std::string& gpu_uuid, unsigned long long* out);
+// The device's DRAM health record: volatile DRAM ECC counts (nvmlDeviceGetMemoryErrorCounter), remapped rows
+// (nvmlDeviceGetRemappedRows) and, with `histogram`, the row remapper's histogram.  out->nvml has a CRO_HBM_NVML_* bit
+// per read NVML answered; a refused read leaves its fields 0.
+void NvmlHbmHealth(const std::string& gpu_uuid, bool histogram, cro_hbm_health* out);
 
 }  // namespace identity
 }  // namespace cro

@@ -107,11 +107,12 @@ std::string DefaultHelperPath() {
     return "croprobe-cli";
 }
 
-int RunHelper(const std::string& helper_path, const std::string& uuid, uint64_t sweep_bytes, int deadline_ms,
-              cro_probe_result* out, std::string* err) {
+int RunHelperRaw(const std::string& helper_path, const std::string& what, const std::string& uuid,
+                 const std::vector<std::string>& args, int deadline_ms, size_t head, size_t rec, size_t max_rec,
+                 uint64_t (*count)(const unsigned char* head), std::string* out, std::string* err) {
     const std::string helper = helper_path.empty() ? DefaultHelperPath() : helper_path;
     if (access(helper.c_str(), X_OK) != 0) {
-        if (err) *err = "probe helper '" + helper + "' is not executable";
+        if (err) *err = what + " '" + helper + "' is not executable";
         return CRO_ERR_EXEC;
     }
     int fds[2];
@@ -119,7 +120,6 @@ int RunHelper(const std::string& helper_path, const std::string& uuid, uint64_t 
         if (err) *err = std::string("pipe: ") + strerror(errno);
         return CRO_ERR_EXEC;
     }
-    const std::string mib = std::to_string(std::max<uint64_t>(1, sweep_bytes >> 20));
     // posix_spawn, not fork: the host process is multi-threaded (CUDA's own threads at least), and the child's
     // environment — CUDA_VISIBLE_DEVICES=<uuid>, so that the helper's cuInit sees this one GPU and nothing else — is
     // built here, before the spawn, instead of with setenv() in a forked child (not async-signal-safe).
@@ -130,23 +130,25 @@ int RunHelper(const std::string& helper_path, const std::string& uuid, uint64_t 
     std::vector<char*> envp;
     for (std::string& e : env_store) envp.push_back(const_cast<char*>(e.c_str()));
     envp.push_back(nullptr);
-    const char* argv[] = {helper.c_str(), "probe-raw", uuid.c_str(), mib.c_str(), nullptr};
+    std::vector<const char*> argv = {helper.c_str()};
+    for (const std::string& a : args) argv.push_back(a.c_str());
+    argv.push_back(nullptr);
     posix_spawn_file_actions_t fa;
     posix_spawn_file_actions_init(&fa);
     posix_spawn_file_actions_adddup2(&fa, fds[1], 1);
     posix_spawn_file_actions_addclose(&fa, fds[0]);
     posix_spawn_file_actions_addclose(&fa, fds[1]);
     pid_t pid = 0;
-    const int src = posix_spawn(&pid, helper.c_str(), &fa, nullptr, const_cast<char* const*>(argv), envp.data());
+    const int src = posix_spawn(&pid, helper.c_str(), &fa, nullptr, const_cast<char* const*>(argv.data()), envp.data());
     posix_spawn_file_actions_destroy(&fa);
     if (src != 0) {
         close(fds[0]); close(fds[1]);
-        if (err) *err = std::string("posix_spawn of the probe helper: ") + strerror(src);
+        if (err) *err = "posix_spawn of the " + what + ": " + strerror(src);
         return CRO_ERR_EXEC;
     }
     close(fds[1]);
-    unsigned char buf[sizeof(cro_probe_result)];
-    size_t got = 0;
+    const size_t cap = head + rec * max_rec;
+    out->clear();
     bool timed_out = false;
     const auto until = std::chrono::steady_clock::now() + std::chrono::milliseconds(deadline_ms > 0 ? deadline_ms : 30000);
     for (;;) {
@@ -157,20 +159,18 @@ int RunHelper(const std::string& helper_path, const std::string& uuid, uint64_t 
         if (pr < 0 && errno == EINTR) continue;
         if (pr < 0) break;
         if (pr == 0) continue;
-        unsigned char tmp[1024];
+        unsigned char tmp[4096];
         const ssize_t n = read(fds[0], tmp, sizeof tmp);
         if (n < 0 && errno == EINTR) continue;
         if (n <= 0) break;                                     // EOF: the helper is done
-        const size_t take = std::min<size_t>((size_t)n, sizeof buf - got);
-        memcpy(buf + got, tmp, take);
-        got += take;
+        out->append(reinterpret_cast<const char*>(tmp), std::min<size_t>((size_t)n, cap - out->size()));
     }
     close(fds[0]);
     int status = 0;
     if (timed_out) {
         kill(pid, SIGKILL);
         waitpid(pid, &status, 0);
-        if (err) *err = "probe helper for " + uuid + " exceeded its deadline of " + std::to_string(deadline_ms) + " ms and was killed";
+        if (err) *err = what + " for " + uuid + " exceeded its deadline of " + std::to_string(deadline_ms) + " ms and was killed";
         return CRO_ERR_DEADLINE;
     }
     // the pipe is closed; give the process until the deadline to exit, then reap it
@@ -190,11 +190,22 @@ int RunHelper(const std::string& helper_path, const std::string& uuid, uint64_t 
         if (err) *err = "device '" + uuid + "' is not visible to a fresh CUDA process";
         return CRO_ERR_NO_DEVICE;
     }
-    if (got != sizeof buf || (code != 0 && code != 1)) {
-        if (err) *err = "probe helper for " + uuid + " failed (exit " + std::to_string(code) + ", " + std::to_string(got) + " result bytes)";
+    const uint64_t n_rec = out->size() >= head && count ? count(reinterpret_cast<const unsigned char*>(out->data())) : 0;
+    if (out->size() < head || n_rec > max_rec || out->size() != head + rec * n_rec || (code != 0 && code != 1)) {
+        if (err) *err = what + " for " + uuid + " failed (exit " + std::to_string(code) + ", " + std::to_string(out->size()) + " result bytes)";
         return CRO_ERR_EXEC;
     }
-    memcpy(out, buf, sizeof buf);
+    return CRO_OK;
+}
+
+int RunHelper(const std::string& helper_path, const std::string& uuid, uint64_t sweep_bytes, int deadline_ms,
+              cro_probe_result* out, std::string* err) {
+    const std::string mib = std::to_string(std::max<uint64_t>(1, sweep_bytes >> 20));
+    std::string got;
+    const int rc = RunHelperRaw(helper_path, "probe helper", uuid, {"probe-raw", uuid, mib}, deadline_ms, sizeof *out, 0, 0,
+                                nullptr, &got, err);
+    if (rc != CRO_OK) return rc;
+    memcpy(out, got.data(), sizeof *out);
     if (out->abi_version != CRO_ABI_VERSION) {
         if (err) *err = "probe helper speaks another ABI version";
         return CRO_ERR_ABI_MISMATCH;

@@ -51,6 +51,15 @@ bool ProcRegistryExists(const std::string& proc_root);
 int RunHelper(const std::string& helper_path, const std::string& uuid, uint64_t sweep_bytes, int deadline_ms,
               cro_probe_result* out, std::string* err);
 
+// What RunHelper and the scan helper share: `<helper> <args...>` with CUDA_VISIBLE_DEVICES=<uuid>, its stdout read into
+// *out under deadline_ms (SIGKILL + reap on expiry).  The output is a head of `head` bytes followed by count(head)
+// records of `rec` bytes (count may be null when there is no tail), at most max_rec of them.  CRO_OK when the helper
+// exited 0 or 1 with exactly that; CRO_ERR_NO_DEVICE (exit 3), CRO_ERR_DEADLINE, CRO_ERR_EXEC otherwise, *err naming
+// `what` ("probe helper", "scan helper").
+int RunHelperRaw(const std::string& helper_path, const std::string& what, const std::string& uuid,
+                 const std::vector<std::string>& args, int deadline_ms, size_t head, size_t rec, size_t max_rec,
+                 uint64_t (*count)(const unsigned char* head), std::string* out, std::string* err);
+
 std::string DefaultHelperPath();
 
 }  // namespace inventory

@@ -11,15 +11,6 @@ namespace {
 constexpr uint64_t kRetestSeedOffset = 1ull << 63;
 constexpr int kLocateSlots = 2 * CRO_LOCATE_PASSES + CRO_LOCATE_PASSES;   // [2p + h] compare sweeps, then closed forms
 
-// Closed form of the complement of a pattern over n words, from the pattern's: ~p = -1 - p, and the weights
-// 2i + 1 of n words sum to n^2.
-SweepOut complement_fold(SweepOut f, uint64_t n) {
-    f.x ^= (n & 1) ? ~0ull : 0ull;
-    f.s = 0 - n - f.s;
-    f.w = 0 - n * n - f.w;
-    return f;
-}
-
 // The report of a call that located nothing: zeroes but for the sweep size it got to (0 before it knew it).
 void blank_report(cro_fault_report* rep, std::vector<cro_fault_word>* words, uint64_t sweep_bytes) {
     memset(rep, 0, sizeof *rep);

@@ -822,6 +822,23 @@ int ctx_inventory(cro_ctx* c, std::vector<cro_dev_info>* out, bool force) {
     return CRO_OK;
 }
 
+int find_on_node(cro_ctx* c, const std::string& uuid, cro_dev_info* hit) {
+    std::vector<cro_dev_info> inv;
+    int rc = ctx_inventory(c, &inv);
+    if (rc) return rc;
+    for (int attempt = 0; attempt < 2; ++attempt) {
+        // told about a UUID the cached list lacks: look again, properly, before saying "not on this node"
+        if (attempt == 1 && (rc = ctx_inventory(c, &inv, true))) return rc;
+        for (const auto& d : inv)
+            if (uuid == std::string(d.gpu_uuid, strnlen(d.gpu_uuid, sizeof d.gpu_uuid))) {
+                *hit = d;
+                return CRO_OK;
+            }
+    }
+    c->set_error("device '" + uuid + "' is not on this node");
+    return CRO_ERR_NO_DEVICE;
+}
+
 int ctx_probe_uuid(cro_ctx* c, const char* uuid, cro_probe_result* out) {
     if (!uuid || !out) return CRO_ERR_INVALID_ARG;
     const std::string want = uuid;
@@ -831,21 +848,10 @@ int ctx_probe_uuid(cro_ctx* c, const char* uuid, cro_probe_result* out) {
     else env::read(&knobs, nullptr);
     int deadline = (int)knobs.get("CRO_HELPER_TIMEOUT_MS");
     if (c) {
-        std::vector<cro_dev_info> inv;
-        int rc = ctx_inventory(c, &inv);
+        cro_dev_info hit{};
+        const int rc = find_on_node(c, want, &hit);
         if (rc) return rc;
-        const cro_dev_info* hit = nullptr;
-        for (int attempt = 0; attempt < 2 && !hit; ++attempt) {
-            // told about a UUID the cached list lacks: look again, properly, before saying "not on this node"
-            if (attempt == 1 && (rc = ctx_inventory(c, &inv, true))) return rc;
-            for (const auto& d : inv)
-                if (want == std::string(d.gpu_uuid, strnlen(d.gpu_uuid, sizeof d.gpu_uuid))) hit = &d;
-        }
-        if (!hit) {
-            c->set_error("device '" + want + "' is not on this node");
-            return CRO_ERR_NO_DEVICE;
-        }
-        if (hit->flags & CRO_DEV_IN_PROCESS) return ctx_probe_device(c, hit->dev_index, out);
+        if (hit.flags & CRO_DEV_IN_PROCESS) return ctx_probe_device(c, hit.dev_index, out);
         sweep = std::min<uint64_t>(c->opts.sweep_bytes, sweep);
         if (c->opts.deadline_ms > 0) deadline = c->opts.deadline_ms;
     }

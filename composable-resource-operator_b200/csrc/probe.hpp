@@ -195,6 +195,9 @@ int ctx_sweep_times(cro_ctx* c, int idx, cro_sweep_time* out, int cap, int* n);
 int ctx_inventory(cro_ctx* c, std::vector<cro_dev_info>* out, bool force = false);
 // Probe by UUID: in-process device, helper process for one attached after init, CRO_ERR_NO_DEVICE when not on the node.
 int ctx_probe_uuid(cro_ctx* c, const char* uuid, cro_probe_result* out);
+// The node's inventory entry of a UUID (looked up twice, the second time with a forced re-read); CRO_ERR_NO_DEVICE with
+// the error text set when the node does not list it.
+int find_on_node(cro_ctx* c, const std::string& uuid, cro_dev_info* hit);
 int ctx_p2p_detail(cro_ctx* c, int idx, int peer, cro_p2p_detail* out);
 
 // single sweeps (each takes the device mutex)
@@ -217,6 +220,14 @@ int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_re
 // recorded element, by (leg, smid, row, col).
 int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_compute_result* r, std::vector<cro_compute_sm>* sms,
                       std::vector<cro_compute_fault>* faults);
+
+// Whole-HBM scan (include/croprobe.h, cro_scan_hbm / cro_scan_hbm_uuid, hbm_scan.cu): *words gets every recorded word,
+// merged by scan index.  The uuid form runs `croprobe-cli scan-raw` and asks it for at most cap words.
+int ctx_scan_hbm(cro_ctx* c, int idx, const cro_scan_opts& o, cro_scan_report* rep, std::vector<cro_fault_word>* words);
+int ctx_scan_hbm_uuid(cro_ctx* c, const char* uuid, const cro_scan_opts& o, cro_scan_report* rep, std::vector<cro_fault_word>* words,
+                      int cap);
+// CRO_SCAN_HEALTH_* of the NVML reads before E0 and after E3.
+uint32_t scan_health(const cro_hbm_health& before, const cro_hbm_health& after);
 
 // test hooks (include/croprobe.h, cro_selftest_*): the verdict kernels and the chase on caller-given inputs
 int ctx_selftest_probe_finalize(cro_ctx* c, int idx, const cro_probe_result* tmpl, const cro_sweep_slot* slots,

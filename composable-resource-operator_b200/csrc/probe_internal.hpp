@@ -218,6 +218,15 @@ int probe_enqueue(cro_ctx* c, Device* d, Lane& L);
 // 128-byte line.
 int upload_chase_table(cro_ctx* c, const std::vector<uint32_t>& perm, unsigned long long** table);
 
+// Closed form of the complement of a pattern over n words, from the pattern's: ~p = -1 - p, and the weights
+// 2i + 1 of n words sum to n^2.
+inline SweepOut complement_fold(SweepOut f, uint64_t n) {
+    f.x ^= (n & 1) ? ~0ull : 0ull;
+    f.s = 0 - n - f.s;
+    f.w = 0 - n * n - f.w;
+    return f;
+}
+
 // Device memory of one call, freed on every way out.
 template <class T>
 struct DeviceMem {

@@ -411,6 +411,107 @@ func (c *Context) ProbeCompute(deviceID string) (ComputeResult, error) {
 	return out, nil
 }
 
+// ScanResult is the summary of cro_scan_report an operator reads: whether every
+// free byte of the GPU's memory held what was written, how much was covered,
+// and the memory's own health record from NVML.
+type ScanResult struct {
+	Status       int32     // CRO_OK, CRO_ERR_CHECKSUM or CRO_ERR_CUDA
+	CudaError    int32     // cudaError_t of a failed element (CRO_ERR_CUDA)
+	Health       uint32    // CRO_SCAN_HEALTH_* bits; never change Status
+	Seed         uint64
+	CoveredBytes uint64
+	FreeBytes    uint64
+	Mismatches   [2]uint64 // per compare pass: 0 against the pattern, 1 against its complement
+	Words        []ScanWord
+	Annotations  string // Go-marshalled map[string]string of cohdi.io/hbm-scan-* keys
+}
+
+// ScanWord is one mismatching scan word (cro_fault_word of a scan).
+type ScanWord struct {
+	Index    uint64 // scan word index
+	Expected uint64
+	Actual   uint64
+	Passes   uint32 // bit p: compare pass p saw it
+	Chunk    uint32
+	Offset   uint64 // word offset in the chunk
+}
+
+func scanResult(rep *C.cro_scan_report, words []C.cro_fault_word, got C.int) ScanResult {
+	out := ScanResult{Status: int32(rep.status), CudaError: int32(rep.cuda_error), Health: uint32(rep.health),
+		Seed: uint64(rep.seed), CoveredBytes: uint64(rep.covered_bytes), FreeBytes: uint64(rep.free_bytes)}
+	for p := 0; p < 2; p++ {
+		out.Mismatches[p] = uint64(rep.pass[p].mismatches)
+	}
+	for i := 0; i < int(got); i++ {
+		w := words[i]
+		k := uint32(w.reserved)
+		out.Words = append(out.Words, ScanWord{uint64(w.word_index), uint64(w.expected), uint64(w.actual), uint32(w.passes), k,
+			uint64(w.word_index) - uint64(rep.chunk[k].word0)})
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_scan_annotations_json(rep, buf, 4096, &ln) == C.CRO_OK {
+		out.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return out
+}
+
+// ScanHBMByUUID runs cro_scan_hbm_uuid: the whole-HBM scan of any GPU on the
+// node through the helper process, the form to call before handing a freshly
+// composed GPU to a tenant.  maxBytes 0 scans all free memory but 1 GiB.  A
+// memory fault (CRO_ERR_CUDA) or a mismatch is a result, not an error; found is
+// false when the node does not list the GPU.
+func (c *Context) ScanHBMByUUID(deviceID string, maxBytes uint64) (r ScanResult, found bool, err error) {
+	id := C.CString(deviceID)
+	defer C.free(unsafe.Pointer(id))
+	var opts C.cro_scan_opts
+	opts.max_bytes = C.uint64_t(maxBytes)
+	rep := (*C.cro_scan_report)(C.malloc(C.size_t(unsafe.Sizeof(C.cro_scan_report{}))))
+	defer C.free(unsafe.Pointer(rep))
+	var words [256]C.cro_fault_word
+	var got C.int
+	rc := C.cro_scan_hbm_uuid(c.h, id, &opts, rep, &words[0], 256, &got)
+	if rc == C.CRO_ERR_NO_DEVICE {
+		return r, false, nil
+	}
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM && rc != C.CRO_ERR_CUDA {
+		return r, true, errorOf(c.h, rc)
+	}
+	return scanResult(rep, words[:], got), true, nil
+}
+
+// ScanHBM runs cro_scan_hbm on the in-process device whose UUID is deviceID:
+// the memory this process can allocate beside what it holds.  ScanHBMByUUID is
+// the form an operator should call (INTEGRATION.md "The HBM scan").
+func (c *Context) ScanHBM(deviceID string, maxBytes uint64) (ScanResult, error) {
+	var devs [C.CRO_MAX_DEVICES]C.cro_dev_info
+	var n C.int
+	if rc := C.cro_enumerate(c.h, &devs[0], C.CRO_MAX_DEVICES, &n); rc != C.CRO_OK {
+		return ScanResult{}, errorOf(c.h, rc)
+	}
+	idx := C.int(-1)
+	for i := 0; i < int(n); i++ {
+		if C.GoString(&devs[i].gpu_uuid[0]) == deviceID && devs[i].flags&C.CRO_DEV_IN_PROCESS != 0 {
+			idx = C.int(devs[i].dev_index)
+		}
+	}
+	if idx < 0 {
+		return ScanResult{}, fmt.Errorf("cuda hbm scan: %s is not a device of this context", deviceID)
+	}
+	var opts C.cro_scan_opts
+	opts.max_bytes = C.uint64_t(maxBytes)
+	rep := (*C.cro_scan_report)(C.malloc(C.size_t(unsafe.Sizeof(C.cro_scan_report{}))))
+	defer C.free(unsafe.Pointer(rep))
+	var words [256]C.cro_fault_word
+	var got C.int
+	rc := C.cro_scan_hbm(c.h, idx, &opts, rep, &words[0], 256, &got)
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM && rc != C.CRO_ERR_CUDA {
+		return ScanResult{}, errorOf(c.h, rc)
+	}
+	return scanResult(rep, words[:], got), nil
+}
+
 // MetricsText is the Prometheus text exposition of the context's counters and
 // per-GPU gauges; a prometheus.Collector registered with
 // sigs.k8s.io/controller-runtime/pkg/metrics.Registry (cmd/main.go:66,119-125

@@ -799,6 +799,144 @@ int  cro_probe_compute(cro_ctx *ctx, int dev_index, const cro_compute_opts *opts
  * CRO_COMPUTE_M * CRO_COMPUTE_N int32 values, row-major.  Host arithmetic only; no context. */
 int  cro_compute_expected(int answer, uint64_t seed, int32_t *out);
 
+/* ---- whole-HBM scan: every free byte of a GPU's memory, and its DRAM health record ---- */
+
+/*
+ * The probe sweeps 2·S bytes (8 GiB by default); the scan tests the memory nobody holds.  It allocates cudaMalloc
+ * chunks of CRO_SCAN_CHUNK_BYTES (the last one ragged) until it covers min(max_bytes, free - reserve_bytes) or an
+ * allocation fails, runs four elements over ALL chunks each before the next element starts
+ *   E0 fill P     E1 compare with P     E2 fill ~P     E3 compare with ~P
+ * and frees the chunks on every way out.  Every bit cell is written and read back as 0 and as 1, so a stuck-at bit
+ * mismatches in exactly one of the two compare passes (pass 0 = E1, pass 1 = E3), and a write that lands in the wrong
+ * place anywhere is seen by the compare that follows.  Reading every location also turns latent weak cells into the
+ * ECC and row-remapping events the scan reads from NVML before E0 and after E3.
+ *
+ * Scan word index: the chunks concatenated in allocation order; chunk k starts at word chunk[k].word0.  Word j holds
+ * pattern_word(seed, j) after E0 and its complement after E2.  The seed is opts->seed, or (0) one derived from the
+ * clock and reported, so no two calls share a pattern.
+ *
+ * Two forms.  cro_scan_hbm_uuid is the one an operator calls (INTEGRATION.md "The HBM scan"): the helper process
+ * (`croprobe-cli scan-raw`, a fresh cuInit that sees only that GPU) reaches GPUs attached after cro_probe_init, can
+ * take nearly all free memory and returns it by exiting, and an uncorrectable ECC error that takes down the CUDA
+ * context which touched the memory costs the helper, not the caller's context.  cro_scan_hbm scans beside what this
+ * process already holds; it takes the device's mutex and lets probes still in flight finish first (their results
+ * stay collectable with cro_probe_end), and never touches the sweep region.
+ *
+ * status: CRO_ERR_CHECKSUM when a compare pass found a mismatch; CRO_ERR_CUDA when a CUDA call failed during the
+ * elements (cuda_error holds the cudaError_t, e.g. cudaErrorECCUncorrectable: the memory faulted; the NVML "after"
+ * read still happens and the report is filled as far as the scan got); CRO_ERR_OOM when not one chunk could be
+ * allocated (nothing is then allocated at all).  The health bits never change the status: what counts as unhealthy
+ * is the caller's call.
+ */
+#define CRO_SCAN_CHUNK_BYTES      (2ull << 30)
+#define CRO_SCAN_RESERVE_BYTES    (1ull << 30)   /* default reserve_bytes                                        */
+#define CRO_SCAN_MAX_CHUNKS       128            /* allocation also ends after this many chunks (256 GiB by default) */
+#define CRO_SCAN_PASSES           2              /* compare passes: 0 = E1 (pattern), 1 = E3 (complement)          */
+#define CRO_SCAN_ELEMENTS         4
+
+/* cro_scan_report.health: reported, never changes the status */
+#define CRO_SCAN_HEALTH_ECC_CORRECTED_DURING    0x1u   /* the volatile DRAM corrected count rose during the scan    */
+#define CRO_SCAN_HEALTH_ECC_UNCORRECTED_DURING  0x2u   /* the volatile DRAM uncorrected count rose during the scan  */
+#define CRO_SCAN_HEALTH_REMAP_PENDING           0x4u   /* a row remap waits for a GPU reset to take effect          */
+#define CRO_SCAN_HEALTH_REMAP_FAILURE           0x8u   /* a remap failed: a bank has no spare rows left             */
+
+/* cro_hbm_health.nvml: which reads NVML answered (a field NVML refused stays 0) */
+#define CRO_HBM_NVML_ECC_CORRECTED    0x1u   /* nvmlDeviceGetMemoryErrorCounter, corrected, volatile, DRAM      */
+#define CRO_HBM_NVML_ECC_UNCORRECTED  0x2u   /* ... uncorrected                                                */
+#define CRO_HBM_NVML_REMAP            0x4u   /* nvmlDeviceGetRemappedRows                                       */
+#define CRO_HBM_NVML_HISTOGRAM        0x8u   /* nvmlDeviceGetRowRemapperHistogram                               */
+
+typedef struct cro_scan_opts {
+    uint64_t max_bytes;            /*   0  0: all free memory but reserve_bytes                                  */
+    uint64_t reserve_bytes;        /*   8  free memory left alone: 0 = CRO_SCAN_RESERVE_BYTES                     */
+    uint64_t seed;                 /*  16  0: derived from the clock (reported)                                   */
+    int32_t  deadline_ms;          /*  24  cro_scan_hbm_uuid: the helper's deadline; 0 = CRO_HELPER_TIMEOUT_MS     */
+    uint32_t reserved0;            /*  28  0 */
+    /* test only: chunk size (0 = CRO_SCAN_CHUNK_BYTES; a multiple of 16), so a small scan has several chunks */
+    uint64_t test_chunk_bytes;     /*  32 */
+    /* test only: after E0 and after E2, word = (word & test_force_and) | test_force_or for the scan words
+       [test_force_first, test_force_first + test_force_count), split per chunk — a stand-in for stuck cells */
+    uint64_t test_force_first;     /*  40 */
+    uint64_t test_force_count;     /*  48 */
+    uint64_t test_force_and;       /*  56 */
+    uint64_t test_force_or;        /*  64 */
+} cro_scan_opts;                   /*  72 bytes */
+
+typedef struct cro_hbm_health {
+    uint32_t nvml;                 /*   0  CRO_HBM_NVML_* of the reads NVML answered                              */
+    uint32_t remap_corrected;      /*   4  rows remapped for corrected errors                                    */
+    uint32_t remap_uncorrected;    /*   8  rows remapped for uncorrected errors                                  */
+    uint32_t remap_pending;        /*  12  1: a remap waits for a GPU reset                                      */
+    uint32_t remap_failure;        /*  16  1: a remap failed                                                     */
+    uint32_t histogram[5];         /*  20  banks with max, high, partial, low, no spare rows left (after E3 only) */
+    uint64_t ecc_corrected;        /*  40  volatile DRAM ECC counts                                              */
+    uint64_t ecc_uncorrected;      /*  48 */
+} cro_hbm_health;                  /*  56 bytes */
+
+typedef struct cro_scan_pass {
+    uint64_t invert;               /*   0  0 for pass 0 (E1), all ones for pass 1 (E3)                           */
+    uint64_t words_scanned;        /*   8 */
+    uint64_t mismatches;           /*  16  exact                                                                 */
+    uint64_t recorded;             /*  24  mismatches the device recorded (<= CRO_LOCATE_RECORDS)                */
+    uint64_t granules;             /*  32  CRO_LOCATE_GRANULE_BYTES granules of the scan with a mismatch          */
+    uint64_t bit_flips[64];        /*  40  mismatches with bit b flipped                                         */
+} cro_scan_pass;                   /* 552 bytes */
+
+typedef struct cro_scan_chunk {
+    uint64_t word0;                /*   0  scan index of the chunk's first word                                  */
+    uint64_t bytes;                /*   8 */
+    uint64_t fold_xor[2];          /*  16  the chunk as compare pass p read it (xor, sum, wsum as for a read
+                                              sweep of pattern seed + word0: weights count from the chunk's start) */
+    uint64_t fold_sum[2];          /*  32 */
+    uint64_t fold_wsum[2];         /*  48 */
+    uint64_t expect_xor;           /*  64  closed form of pattern_word(seed + word0, i) over the chunk (pass 0's;
+                                              pass 1 compares against its complement)                           */
+    uint64_t expect_sum;           /*  72 */
+    uint64_t expect_wsum;          /*  80 */
+} cro_scan_chunk;                  /*  88 bytes */
+
+typedef struct cro_scan_report {
+    int32_t  status;               /*    0  the return value                                                     */
+    int32_t  cuda_error;           /*    4  cudaError_t of the CUDA call that failed during the elements; 0: none  */
+    uint32_t health;               /*    8  CRO_SCAN_HEALTH_*                                                    */
+    uint32_t complete;             /*   12  1: every mismatch of both passes is in the caller's list, and for each
+                                               chunk the listed deltas reproduce its fold minus its closed form    */
+    uint64_t seed;                 /*   16 */
+    uint64_t total_bytes;          /*   24  the device's memory                                                   */
+    uint64_t free_bytes;           /*   32  free when the call started                                            */
+    uint64_t held_bytes;           /*   40  this context's sweep region on the device (0 in the helper)           */
+    uint64_t covered_bytes;        /*   48  bytes scanned: the chunks' sum                                        */
+    uint32_t n_chunks;             /*   56 */
+    uint32_t elements_done;        /*   60  elements that completed: 4 for a whole scan                          */
+    uint64_t located;              /*   64  distinct words the device recorded over both passes                  */
+    uint64_t recorded;             /*   72  words written to the caller's list (*n)                              */
+    uint64_t flip_or;              /*   80  OR of every mismatch's actual ^ expected                             */
+    uint64_t element_ns[CRO_SCAN_ELEMENTS];   /*   88  CUDA events around each element                       */
+    uint64_t alloc_ns;             /*  120  host time to allocate the chunks (and free them)                      */
+    uint64_t nvml_ns;              /*  128  host time of both NVML reads                                          */
+    uint64_t wall_ns;              /*  136  the whole scan call                                                  */
+    uint64_t helper_ns;            /*  144  cro_scan_hbm_uuid: spawn of the helper to its exit; 0 in process      */
+    cro_hbm_health before;         /*  152  read before E0 (no histogram)                                       */
+    cro_hbm_health after;          /*  208  read after E3, or after the element that failed                      */
+    cro_scan_pass pass[CRO_SCAN_PASSES];      /*  264 */
+    cro_scan_chunk chunk[CRO_SCAN_MAX_CHUNKS]; /* 1368 */
+} cro_scan_report;                 /* 12632 bytes */
+
+/* words[0 .. cap) receives the mismatching words merged by scan index (*n how many): word_index is the scan index,
+ * passes bit p that compare pass p saw it, and `reserved` the word's chunk number k (its offset in the chunk is
+ * word_index - chunk[k].word0).  Device addresses mean nothing outside the call and are not reported.  opts may be NULL
+ * (defaults).  cro_scan_hbm: dev_index is an in-process device.  cro_scan_hbm_uuid: ctx may be NULL; a UUID the node
+ * does not list is CRO_ERR_NO_DEVICE; a GPU that is also an in-process device of ctx is held under that device's mutex
+ * while the helper runs, so no probe of it runs beside the scan. */
+int  cro_scan_hbm(cro_ctx *ctx, int dev_index, const cro_scan_opts *opts,
+                  cro_scan_report *out, cro_fault_word *words, int cap, int *n);
+int  cro_scan_hbm_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_scan_opts *opts,
+                       cro_scan_report *out, cro_fault_word *words, int cap, int *n);
+
+/* The device's DRAM health record from NVML, as the scan reads it after E3 (with the histogram): no context, no CUDA.
+ * CRO_OK whatever NVML answered (out->nvml says which reads it did); CRO_ERR_INVALID_ARG for a NULL argument. */
+int  cro_read_hbm_health(const char *gpu_uuid, cro_hbm_health *out);
+
 /* ---- emit: encoding/json-compatible writers ------------------------------ */
 
 /* ComposableResourceStatus (api/v1alpha1/composableresource_types.go:36-41):
@@ -857,6 +995,17 @@ int  cro_emit_link_annotations_json(const cro_link_result *r, char *buf, size_t 
  * -s8-gops, -bf16-gflops, -e4m3-gflops (ops / ns, integer division; 0 when ns is 0) and -slowest-sm ("<id>
  * <permille>" of the leg run with the largest slow_permille, the lowest leg on a tie). */
 int  cro_emit_compute_annotations_json(const cro_compute_result *r, char *buf, size_t cap, size_t *len);
+
+/* Additive HBM scan annotations (cohdi.io/hbm-scan-*) of a cro_scan_hbm / cro_scan_hbm_uuid report, the same
+ * Go-marshalled map, integers and fixed spellings only: -verdict ("ok" for CRO_OK, "corrupt" for CRO_ERR_CHECKSUM,
+ * "cuda-error:<cuda_error>" for CRO_ERR_CUDA, "error" otherwise), -covered-bytes, -free-bytes, -seed (hex16),
+ * -mismatches ("<pass 0>,<pass 1>") and -granules (the same), -gbs (4 * covered_bytes over the elements' summed ns, in
+ * GB/s, integer division; 0 when that is 0), -bits (flipped bit positions, ascending; only when a bit flipped),
+ * -health (the flags' names ecc-corrected, ecc-uncorrected, remap-pending, remap-failure, comma-separated; only when
+ * any is set), and only when NVML answered the read: -ecc-corrected and -ecc-uncorrected (the deltas, after -
+ * before, when both reads answered), -remapped ("<corrected>,<uncorrected>" rows after E3) and -remap-histogram ("max,
+ * high, partial, low, none" without spaces). */
+int  cro_emit_scan_annotations_json(const cro_scan_report *r, char *buf, size_t cap, size_t *len);
 
 /* (deviceID, CDIDeviceID) from an FM ScaleUpResponse body, with the
  * res_op_status gate of internal/cdi/fti/fm/client.go:184-213.  On the error
