@@ -357,6 +357,35 @@ class ScanReport(ctypes.Structure):
         return w.reserved, w.word_index - self.chunk[w.reserved].word0
 
 
+# test hook: one sweep kernel between guard bands (cro_selftest_sweep)
+(SELFTEST_SWEEP_FILL, SELFTEST_SWEEP_COPY_LDG, SELFTEST_SWEEP_COPY_TMA, SELFTEST_SWEEP_COPY_FUSED, SELFTEST_SWEEP_READ_LDG,
+ SELFTEST_SWEEP_READ_TMA, SELFTEST_SWEEP_READ_LDG256, SELFTEST_SWEEP_LOCATE, SELFTEST_SWEEP_FORCE_WORDS,
+ SELFTEST_SWEEP_LINK_READ, SELFTEST_SWEEP_LINK_WRITE) = range(1, 12)
+SELFTEST_LAYOUT_SRC_DST, SELFTEST_LAYOUT_DST_SRC, SELFTEST_LAYOUT_APART = 1, 2, 3
+SELFTEST_GUARD_BYTES, SELFTEST_F_INTERIORS = 2 << 20, 1
+
+
+class SelftestSweepOpts(ctypes.Structure):
+    _fields_ = [("kernel", ctypes.c_uint32), ("layout", ctypes.c_uint32), ("offset", ctypes.c_uint64),
+                ("bytes", ctypes.c_uint64), ("seed", ctypes.c_uint64), ("canary", ctypes.c_uint64),
+                ("invert", ctypes.c_uint64), ("word0", ctypes.c_uint64), ("force_first", ctypes.c_uint64 * 2),
+                ("force_count", ctypes.c_uint64 * 2), ("force_and", ctypes.c_uint64 * 2), ("force_or", ctypes.c_uint64 * 2),
+                ("flags", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+class SelftestSweepOut(ctypes.Structure):
+    """cro_selftest_sweep_out: the kernel's slot, the buffer's size and interiors, each interior's fold after the
+    kernel, and the word-checking kernels' counters and granules."""
+    _fields_ = [("sweep", SweepResult), ("buf_bytes", ctypes.c_uint64), ("at", ctypes.c_uint64 * 2),
+                ("after_xor", ctypes.c_uint64 * 2), ("after_sum", ctypes.c_uint64 * 2), ("after_wsum", ctypes.c_uint64 * 2),
+                ("mismatches", ctypes.c_uint64), ("claims", ctypes.c_uint64), ("granules", ctypes.c_uint64),
+                ("granule_min", ctypes.c_uint64), ("granule_max", ctypes.c_uint64)]
+
+    def after(self, k: int) -> Tuple[int, int, int]:
+        """Checksum (xor, sum, weighted sum) of interior k once the kernel was done."""
+        return (self.after_xor[k], self.after_sum[k], self.after_wsum[k])
+
+
 assert ctypes.sizeof(ProbeResult) == 512, ctypes.sizeof(ProbeResult)
 assert ctypes.sizeof(ComputeResult) == 600 and ctypes.sizeof(ComputeSm) == 208, ctypes.sizeof(ComputeResult)
 assert ctypes.sizeof(FaultReport) == 928 and ctypes.sizeof(LocatePass) == 120, ctypes.sizeof(FaultReport)
@@ -382,7 +411,7 @@ EXPORTS = [
     "cro_local_node_op", "cro_scan_cmdline_for", "cro_token_from_reply",
     "cro_selftest_exception_barrier", "cro_probe_sweep_times", "cro_p2p_detail_get", "cro_fullbox_times",
     "cro_chase_end", "cro_validate_env", "cro_node_inventory", "cro_probe_uuid", "cro_set_latency_hops", "cro_local_exec", "cro_metrics_text", "cro_describe_wire_type",
-    "cro_selftest_probe_finalize", "cro_selftest_p2p_finalize", "cro_selftest_chase",
+    "cro_selftest_probe_finalize", "cro_selftest_p2p_finalize", "cro_selftest_chase", "cro_selftest_sweep",
     "cro_locate_faults", "cro_emit_fault_annotations_json",
     "cro_probe_host_link", "cro_pci_link_path", "cro_emit_link_annotations_json",
     "cro_probe_compute", "cro_compute_expected", "cro_emit_compute_annotations_json",
@@ -473,6 +502,8 @@ def _load() -> ctypes.CDLL:
                                             ctypes.POINTER(u64), ctypes.POINTER(u32), u32, u32, u32, u32, u32, u64, u64]),
         "cro_selftest_chase": (i32, [vp, i32, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), u32, u32,
                                      ctypes.POINTER(u64)]),
+        "cro_selftest_sweep": (i32, [vp, i32, ctypes.POINTER(SelftestSweepOpts), ctypes.POINTER(SelftestSweepOut), vp, u64,
+                                     ctypes.POINTER(FaultWord), i32, ctypes.POINTER(i32)]),
         "cro_locate_faults": (i32, [vp, i32, ctypes.POINTER(LocateOpts), ctypes.POINTER(FaultReport), ctypes.POINTER(FaultWord),
                                     i32, ctypes.POINTER(i32)]),
         "cro_emit_fault_annotations_json": (i32, [ctypes.POINTER(FaultReport), ctypes.POINTER(FaultWord), i32] + out),
@@ -1001,6 +1032,31 @@ class ProbeContext:
         out = (ctypes.c_uint64 * (2 * n))()
         self._check(lib.cro_selftest_chase(self.handle, dev, src, dst, n, hops, out))
         return list(out)
+
+    def selftest_sweep(self, dev: int, kernel: int, bytes: int, offset: int = 0, layout: int = 0, seed: int = 0,
+                       canary: int = 0, invert: int = 0, word0: int = 0, force: List[Tuple[int, int, int, int]] = (),
+                       interiors: bool = False, alloc=bytearray, cap: int = 16):
+        """One SELFTEST_SWEEP_* kernel on a buffer of the hook's own: guards holding canary words (word j of guard g:
+        pattern_word(canary, g * 2^32 + j)) around the interior(s), a copy's in the SELFTEST_LAYOUT_* given.  force: up
+        to two (first, count, and_mask, or_mask) interior ranges.  Returns (SelftestSweepOut, the buffer as alloc(buf_bytes) made it, with the guards and,
+        if interiors, the interiors at their offsets, and up to `cap` of the kernel's records by word)."""
+        o = SelftestSweepOpts()
+        o.kernel, o.layout, o.offset, o.bytes, o.seed, o.canary = kernel, layout, offset, bytes, seed, canary
+        o.invert, o.word0 = invert, word0
+        for r, (first, count, and_mask, or_mask) in enumerate(force):
+            o.force_first[r], o.force_count[r], o.force_and[r], o.force_or[r] = first, count, and_mask, or_mask
+        o.flags = SELFTEST_F_INTERIORS if interiors else 0
+        out = SelftestSweepOut()
+        arr = (FaultWord * max(1, cap))()
+        n = ctypes.c_int()
+        self._check(lib.cro_selftest_sweep(self.handle, dev, ctypes.byref(o), ctypes.byref(out), None, 0, arr, cap,
+                                           ctypes.byref(n)), allow=(ERR_BUFFER_SMALL,))
+        buf = alloc(out.buf_bytes)
+        raw = (ctypes.c_char * out.buf_bytes).from_buffer(buf)
+        self._check(lib.cro_selftest_sweep(self.handle, dev, ctypes.byref(o), ctypes.byref(out), raw, out.buf_bytes, arr,
+                                           cap, ctypes.byref(n)))
+        del raw                                   # release the export: the caller may resize a bytearray
+        return out, buf, [arr[i] for i in range(n.value)]
 
 
 def node_inventory(proc_root: Optional[str], in_process: List[DevInfo]) -> List[DevInfo]:

@@ -66,6 +66,9 @@ static_assert(sizeof(cro_scan_report) == 12632 && offsetof(cro_scan_report, elem
                   offsetof(cro_scan_report, before) == 152 && offsetof(cro_scan_report, pass) == 264 &&
                   offsetof(cro_scan_report, chunk) == 1368 && offsetof(cro_hbm_health, ecc_corrected) == 40,
               "scan layout");
+static_assert(sizeof(cro_selftest_sweep_opts) == 128 && offsetof(cro_selftest_sweep_opts, force_or) == 104 &&
+                  sizeof(cro_selftest_sweep_out) == 168 && offsetof(cro_selftest_sweep_out, mismatches) == 128,
+              "selftest sweep layout");
 
 using namespace cro::capi;
 
@@ -147,6 +150,10 @@ int cro_selftest_p2p_finalize(cro_ctx* ctx, int i, cro_probe_result* result, con
 int cro_selftest_chase(cro_ctx* ctx, int i, const int32_t* minor_src, const int32_t* minor_dst, uint32_t n, uint32_t hops,
                        uint64_t* out) try {
     return ctx ? ctx_selftest_chase(ctx, i, minor_src, minor_dst, n, hops, out) : CRO_ERR_INVALID_ARG;
+} CRO_API_CATCH
+int cro_selftest_sweep(cro_ctx* ctx, int i, const cro_selftest_sweep_opts* opts, cro_selftest_sweep_out* out, void* buf,
+                       uint64_t cap_bytes, cro_fault_word* words, int cap, int* n) try {
+    return ctx ? ctx_selftest_sweep(ctx, i, opts, out, buf, cap_bytes, words, cap, n) : CRO_ERR_INVALID_ARG;
 } CRO_API_CATCH
 
 int cro_probe_init(const cro_opts* opts, cro_ctx** out) try { return ctx_create(opts, out); } CRO_API_CATCH

@@ -239,6 +239,9 @@ int ctx_selftest_p2p_finalize(cro_ctx* c, int idx, cro_probe_result* result, con
                               uint32_t push_folded, uint64_t p2p_bytes, uint64_t stamp);
 int ctx_selftest_chase(cro_ctx* c, int idx, const int32_t* minor_src, const int32_t* minor_dst, uint32_t n, uint32_t hops,
                        uint64_t* out);
+// One sweep kernel on a guarded buffer of the hook's own (cro_selftest_sweep).
+int ctx_selftest_sweep(cro_ctx* c, int idx, const cro_selftest_sweep_opts* o, cro_selftest_sweep_out* out, void* buf,
+                       uint64_t cap_bytes, cro_fault_word* words, int cap, int* n_words);
 
 // CRO_READ_AUTO / CRO_COPY_AUTO resolved with a context's knobs (CRO_READ_VARIANT, CRO_COPY_VARIANT).
 uint32_t resolve_read_variant(uint32_t v, uint64_t bytes, const env::Values& knobs);

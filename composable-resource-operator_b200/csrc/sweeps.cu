@@ -213,4 +213,227 @@ int ctx_selftest_chase(cro_ctx* c, int idx, const int32_t* minor_src, const int3
     return CRO_OK;
 }
 
+// ---------------------------------------------------------------------------
+// test hook: one sweep kernel between guard bands (include/croprobe.h, cro_selftest_sweep)
+// ---------------------------------------------------------------------------
+namespace {
+
+constexpr uint64_t kGuard = CRO_SELFTEST_GUARD_BYTES;
+constexpr uint64_t kMaxHookBytes = 1ull << 40;
+constexpr uint64_t kMaxHookWords = 1ull << 37;      // locate: word0 + interior words, so the granule bitmap stays small
+
+uint64_t round_up(uint64_t v, uint64_t a) { return (v + a - 1) / a * a; }
+
+bool is_copy(uint32_t k) { return k >= CRO_SELFTEST_SWEEP_COPY_LDG && k <= CRO_SELFTEST_SWEEP_COPY_FUSED; }
+bool is_link(uint32_t k) { return k == CRO_SELFTEST_SWEEP_LINK_READ || k == CRO_SELFTEST_SWEEP_LINK_WRITE; }
+
+// The hook's buffer: `total` bytes (a multiple of the guard), interior k at byte at[k].  Every interior starts `offset`
+// past a guard boundary; what the interiors leave of [0, total) is guard, at least kGuard of it on each side.
+struct HookLayout {
+    uint64_t total = 0;
+    uint64_t at[2] = {0, 0};
+    int interiors = 1;
+};
+
+HookLayout hook_layout(const cro_selftest_sweep_opts& o) {
+    HookLayout L;
+    const uint64_t first = kGuard + o.offset;
+    if (o.layout == CRO_SELFTEST_LAYOUT_APART) {
+        L.interiors = 2;
+        L.at[0] = first;
+        L.at[1] = round_up(first + o.bytes, kGuard) + kGuard + o.offset;
+        L.total = round_up(L.at[1] + o.bytes, kGuard) + kGuard;
+    } else if (o.layout != 0) {
+        L.interiors = 2;
+        const int src = o.layout == CRO_SELFTEST_LAYOUT_SRC_DST ? 0 : 1;
+        L.at[src] = first;
+        L.at[1 - src] = first + o.bytes;
+        L.total = round_up(first + 2 * o.bytes, kGuard) + kGuard;
+    } else {
+        L.at[0] = L.at[1] = first;
+        L.total = round_up(first + o.bytes, kGuard) + kGuard;
+    }
+    return L;
+}
+
+// (start, bytes) of every guard, in buffer order (adjacent interiors have none between them).
+std::vector<std::pair<uint64_t, uint64_t>> hook_guards(const HookLayout& L, uint64_t bytes) {
+    uint64_t lo[2] = {std::min(L.at[0], L.at[1]), std::max(L.at[0], L.at[1])};
+    std::vector<std::pair<uint64_t, uint64_t>> g;
+    uint64_t from = 0;
+    for (int k = 0; k < L.interiors; ++k) {
+        if (lo[k] > from) g.push_back({from, lo[k] - from});
+        from = lo[k] + bytes;
+    }
+    g.push_back({from, L.total - from});
+    return g;
+}
+
+// Why the options are refused, or nullptr.
+const char* hook_refusal(const cro_selftest_sweep_opts& o) {
+    const uint32_t k = o.kernel;
+    if (k < CRO_SELFTEST_SWEEP_FILL || k > CRO_SELFTEST_SWEEP_LINK_WRITE) return "unknown kernel";
+    if (is_copy(k) ? (o.layout < CRO_SELFTEST_LAYOUT_SRC_DST || o.layout > CRO_SELFTEST_LAYOUT_APART) : o.layout != 0)
+        return "a copy takes a layout and no other kernel does";
+    if (o.offset % 16 || o.offset >= kGuard) return "the offset must be a multiple of 16 below the guard";
+    if (o.bytes < 16 || o.bytes % 16 || o.bytes > kMaxHookBytes) return "the interior must be a multiple of 16 bytes in [16, 2^40]";
+    const bool inverts = k == CRO_SELFTEST_SWEEP_FILL || k == CRO_SELFTEST_SWEEP_LOCATE;
+    if (o.invert != 0 && !(inverts && o.invert == ~0ull)) return "invert is 0, or all ones for the fill and locate";
+    if (k == CRO_SELFTEST_SWEEP_LOCATE ? o.word0 > kMaxHookWords - o.bytes / 8 : o.word0 != 0)
+        return "word0 is locate's, with word0 + bytes / 8 at most 2^37";
+    const uint64_t n = o.bytes / 8;
+    for (int r = 0; r < 2; ++r) {
+        if (!o.force_count[r]) continue;
+        if (o.force_first[r] >= n || o.force_count[r] > n - o.force_first[r]) return "a force range must lie in the interior";
+        if (k != CRO_SELFTEST_SWEEP_LOCATE && !(k == CRO_SELFTEST_SWEEP_FORCE_WORDS && r == 0))
+            return "force ranges are locate's, and force_words' range 0";
+    }
+    if ((o.flags & ~CRO_SELFTEST_F_INTERIORS) || o.reserved) return "unknown flags";
+    return nullptr;
+}
+
+// Mapped pinned host memory of one call, freed on every way out.
+struct HostMem {
+    void* p = nullptr;
+    HostMem() = default;
+    HostMem(const HostMem&) = delete;
+    HostMem& operator=(const HostMem&) = delete;
+    ~HostMem() { if (p) cudaFreeHost(p); }
+};
+
+}  // namespace
+
+int ctx_selftest_sweep(cro_ctx* c, int idx, const cro_selftest_sweep_opts* o, cro_selftest_sweep_out* out, void* buf,
+                       uint64_t cap_bytes, cro_fault_word* words, int cap, int* n_words) {
+    if (out) memset(out, 0, sizeof *out);
+    if (n_words) *n_words = 0;
+    const char* why = !o || !out || !n_words || cap < 0 || (cap > 0 && !words) ? "null or negative argument" : hook_refusal(*o);
+    HookLayout L;
+    if (!why) {
+        L = hook_layout(*o);
+        out->buf_bytes = L.total;
+        if (dev_at(c, idx) && cap_bytes < L.total) return CRO_ERR_BUFFER_SMALL;
+        if (!buf) why = "null buffer";
+    }
+    if (why) c->set_error(std::string("cro_selftest_sweep: ") + why);
+    DeviceGuard g = enter_device(c, idx, !why);
+    if (g.rc) return g.rc;
+    Device* d = g.d;
+    const uint32_t kernel = o->kernel;
+    const uint64_t bytes = o->bytes;
+    const bool host = is_link(kernel);
+    cudaStream_t st = d->stream;
+
+    // the buffer, its guard boundaries 2 MiB-aligned (device memory, or mapped host memory for the link rows)
+    DeviceMem<unsigned char> dmem;
+    HostMem hmem;
+    unsigned char* base = nullptr;       // device address
+    unsigned char* hbase = nullptr;      // host address (link rows)
+    if (host) {
+        CU_TRY(c, cudaHostAlloc(&hmem.p, L.total + kGuard, cudaHostAllocMapped));
+        void* dp = nullptr;
+        CU_TRY(c, cudaHostGetDevicePointer(&dp, hmem.p, 0));
+        const uint64_t skew = round_up((uint64_t)(uintptr_t)hmem.p, kGuard) - (uint64_t)(uintptr_t)hmem.p;
+        hbase = static_cast<unsigned char*>(hmem.p) + skew;
+        base = static_cast<unsigned char*>(dp) + skew;
+    } else {
+        CU_TRY(c, cudaMalloc(&dmem.p, L.total + kGuard));
+        base = dmem.p + (round_up((uint64_t)(uintptr_t)dmem.p, kGuard) - (uint64_t)(uintptr_t)dmem.p);
+    }
+    // the kernel's counters, records and granule bitmap (one granule to spare past the interior, so a stray record there
+    // shows), the interiors' folds after it, and the reduction scratch
+    MismatchBuffer mb;
+    const KernelPlan& p = d->plan;
+    const int grid = std::max({p.read_ldg.grid, p.read_ldg256.grid, p.read_tma.grid, p.copy_fused.grid, p.locate.grid, p.link_grid, 1});
+    const uint64_t covered = (kernel == CRO_SELFTEST_SWEEP_LOCATE ? o->word0 * 8 : 0) + bytes + CRO_LOCATE_GRANULE_BYTES;
+    int rc = mb.ensure(c, 1, covered, 2, 0, grid, 1);
+    if (rc || (rc = mb.zero(c, st))) return rc;
+    const MismatchView dv = mb.dev();
+    const SweepScratch& sc = mb.scratch[0];
+
+    // guard g: the canary stream from word g * 2^32, so no guard repeats another's words (a stray copy from one guard
+    // into the same place of the next shows); the interior: what the kernel's row asks for
+    const Params pat{ProbeParams{o->seed, 0}, nullptr};
+    const std::vector<std::pair<uint64_t, uint64_t>> guards = hook_guards(L, bytes);
+    for (size_t gi = 0; gi < guards.size(); ++gi) {
+        const Params canary{ProbeParams{o->canary + (gi << 32), 0}, nullptr};
+        CU_TRY(c, launch_fill(p, base + guards[gi].first, guards[gi].second, canary, sc, nullptr, st));
+        c->launches++;
+    }
+    // what the kernel reads holds the pattern (^ invert); what it writes holds the complement of what it should write,
+    // so every word it misses shows
+    unsigned char* in0 = base + L.at[0];
+    unsigned char* in1 = base + L.at[1];
+    const bool writes = kernel == CRO_SELFTEST_SWEEP_FILL || kernel == CRO_SELFTEST_SWEEP_LINK_WRITE;
+    CU_TRY(c, launch_fill(p, in0, bytes, pat, sc, nullptr, st, (o->invert != 0) != writes));
+    if (is_copy(kernel)) CU_TRY(c, launch_fill(p, in1, bytes, pat, sc, nullptr, st, true));
+    c->launches += is_copy(kernel) ? 2 : 1;
+    if (kernel == CRO_SELFTEST_SWEEP_LOCATE)
+        for (int r = 0; r < 2; ++r) {
+            CU_TRY(c, launch_force_words(in0, o->force_first[r], o->force_count[r], o->force_and[r], o->force_or[r], p.sm_count, st));
+            c->launches += o->force_count[r] ? 1 : 0;
+        }
+
+    // the kernel, timed and waited for as the single sweeps are; a kernel that publishes no slot leaves it zero
+    SweepOut* slot = &d->d_out[kSlotScratch];
+    CU_TRY(c, cudaMemsetAsync(slot, 0, sizeof(SweepOut), st));
+    const uint32_t rv = kernel - CRO_SELFTEST_SWEEP_READ_LDG + READ_LDG, cv = kernel - CRO_SELFTEST_SWEEP_COPY_LDG + COPY_LDG;
+    const LinkRole off{nullptr, 0, 0, SweepScratch{}, nullptr, 0}, role{in0, bytes, o->seed, sc, slot, (unsigned)kLinkWarps};
+    auto run = [&]() -> cudaError_t {
+        switch (kernel) {
+            case CRO_SELFTEST_SWEEP_FILL: return launch_fill(p, in0, bytes, pat, sc, slot, st, o->invert != 0);
+            case CRO_SELFTEST_SWEEP_LOCATE: return launch_locate(p, in0, bytes, o->word0, o->seed, o->invert, dv.check(0), sc, slot, st);
+            case CRO_SELFTEST_SWEEP_FORCE_WORDS:
+                return launch_force_words(in0, o->force_first[0], o->force_count[0], o->force_and[0], o->force_or[0], p.sm_count, st);
+            case CRO_SELFTEST_SWEEP_LINK_READ: return launch_link_stream(role, off, dv.check(0), p.link_grid, 0, st);
+            case CRO_SELFTEST_SWEEP_LINK_WRITE: return launch_link_stream(off, role, dv.check(0), p.link_grid, 0, st);
+            default: return is_copy(kernel) ? launch_copy(p, cv, in1, in0, bytes, pat, sc, slot, st) : launch_read(p, rv, in0, bytes, pat, sc, slot, st);
+        }
+    };
+    const bool reads = kernel >= CRO_SELFTEST_SWEEP_READ_LDG && kernel <= CRO_SELFTEST_SWEEP_READ_LDG256;
+    const bool fold = reads || kernel == CRO_SELFTEST_SWEEP_COPY_FUSED || kernel == CRO_SELFTEST_SWEEP_LOCATE ||
+                      kernel == CRO_SELFTEST_SWEEP_LINK_READ;
+    if ((rc = timed_sweep(c, d, 1, is_copy(kernel) ? 2 * bytes : bytes, reads ? rv : is_copy(kernel) ? cv : 0, run, [] {}, fold,
+                          /*deadline=*/true, &out->sweep)))
+        return rc;
+
+    // each interior folded by the LDG read, the counters fetched, the guards (and interiors) copied back
+    for (int k = 0; k < L.interiors; ++k) CU_TRY(c, launch_read(p, READ_LDG, base + L.at[k], bytes, pat, sc, &dv.slots[k], st));
+    c->launches += L.interiors;
+    if ((rc = mb.fetch(c, st))) return rc;
+    std::vector<std::pair<uint64_t, uint64_t>> back = guards;
+    if (o->flags & CRO_SELFTEST_F_INTERIORS)
+        for (int k = 0; k < L.interiors; ++k) back.push_back({L.at[k], bytes});
+    unsigned char* hbuf = static_cast<unsigned char*>(buf);
+    if (!host)
+        for (const auto& seg : back) CU_TRY(c, cudaMemcpyAsync(hbuf + seg.first, base + seg.first, seg.second, cudaMemcpyDeviceToHost, st));
+    if ((rc = wait_stream(c, d))) return rc;
+    if (host)
+        for (const auto& seg : back) memcpy(hbuf + seg.first, hbase + seg.first, seg.second);
+
+    const MismatchView hv = mb.host();
+    for (int k = 0; k < 2; ++k) {
+        const SweepOut& s = hv.slots[k < L.interiors ? k : 0];
+        out->at[k] = L.at[k];
+        out->after_xor[k] = s.x;
+        out->after_sum[k] = s.s;
+        out->after_wsum[k] = s.w;
+    }
+    out->mismatches = hv.ctr[0].mismatches;
+    out->claims = hv.ctr[0].claims;
+    for (uint64_t w = 0; w < hv.gran_words; ++w)
+        for (unsigned long long bits = hv.gran[w]; bits; bits &= bits - 1) {
+            const uint64_t gi = w * 64 + (uint64_t)__builtin_ctzll(bits);
+            if (!out->granules++) out->granule_min = gi;
+            out->granule_max = gi;
+        }
+    std::vector<cro_fault_word> rec;
+    for (uint64_t j = 0; j < std::min<uint64_t>(hv.ctr[0].claims, kLocateRecords); ++j)
+        rec.push_back(cro_fault_word{hv.rec[j].word, hv.rec[j].expected, hv.rec[j].actual, 1u, 0u});
+    std::sort(rec.begin(), rec.end(), [](const cro_fault_word& a, const cro_fault_word& b) { return a.word_index < b.word_index; });
+    *n_words = (int)std::min<size_t>(rec.size(), (size_t)cap);
+    std::copy(rec.begin(), rec.begin() + *n_words, words);
+    return CRO_OK;
+}
+
 }  // namespace cro

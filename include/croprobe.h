@@ -1255,6 +1255,75 @@ int  cro_selftest_p2p_finalize(cro_ctx *ctx, int dev_index, cro_probe_result *re
 int  cro_selftest_chase(cro_ctx *ctx, int dev_index, const int32_t *minor_src, const int32_t *minor_dst, uint32_t n,
                         uint32_t hops, uint64_t *out);
 
+/* Kernels cro_selftest_sweep runs (cro_selftest_sweep_opts.kernel). */
+#define CRO_SELFTEST_SWEEP_FILL         1   /* the pattern of seed, or its complement (invert), over the other one   */
+#define CRO_SELFTEST_SWEEP_COPY_LDG     2   /* copies: the source holds the pattern of seed, the destination its     */
+                                            /* complement                                                            */
+#define CRO_SELFTEST_SWEEP_COPY_TMA     3
+#define CRO_SELFTEST_SWEEP_COPY_FUSED   4
+#define CRO_SELFTEST_SWEEP_READ_LDG     5   /* reads and locate: the interior holds the pattern of seed (^ invert)    */
+#define CRO_SELFTEST_SWEEP_READ_TMA     6
+#define CRO_SELFTEST_SWEEP_READ_LDG256  7
+#define CRO_SELFTEST_SWEEP_LOCATE       8   /* compared with pattern_word(seed, i) ^ invert, recorded as word0 + i    */
+#define CRO_SELFTEST_SWEEP_FORCE_WORDS  9   /* force range 0 of an interior holding the pattern of seed              */
+#define CRO_SELFTEST_SWEEP_LINK_READ   10   /* link_stream's read role over a host interior holding the pattern     */
+#define CRO_SELFTEST_SWEEP_LINK_WRITE  11   /* link_stream's write role: the pattern of seed into a host interior    */
+                                            /* holding its complement                                                */
+/* Where a copy's two interiors lie (cro_selftest_sweep_opts.layout; 0 for every other kernel). */
+#define CRO_SELFTEST_LAYOUT_SRC_DST     1   /* [guard | src | dst | guard]: the probe's A -> B                       */
+#define CRO_SELFTEST_LAYOUT_DST_SRC     2   /* [guard | dst | src | guard]: the probe's B -> A                       */
+#define CRO_SELFTEST_LAYOUT_APART       3   /* [guard | src | guard | dst | guard]                                    */
+#define CRO_SELFTEST_GUARD_BYTES  (2u << 20) /* the least a guard holds: more than any ring (tile * stages) a knob takes */
+#define CRO_SELFTEST_F_INTERIORS        1u  /* copy the interiors back too, not only the guards                       */
+
+typedef struct cro_selftest_sweep_opts {
+    uint32_t kernel;               /*   0  CRO_SELFTEST_SWEEP_*                                                  */
+    uint32_t layout;               /*   4  CRO_SELFTEST_LAYOUT_* of a copy, else 0                               */
+    uint64_t offset;               /*   8  each interior starts this far past a 2 MiB boundary: a multiple of 16  */
+    uint64_t bytes;                /*  16  of each interior: a multiple of 16, at least 16                       */
+    uint64_t seed;                 /*  24  the interior's pattern                                               */
+    uint64_t canary;               /*  32  the guards' pattern: word j of guard g (counted from the buffer's     */
+                                   /*      start) holds pattern_word(canary, g * 2^32 + j)                      */
+    uint64_t invert;               /*  40  fill, locate: XOR on the pattern (0 or all ones)                      */
+    uint64_t word0;                /*  48  locate: scan index of the interior's first word; word0 + bytes / 8 <= 2^37 */
+    uint64_t force_first[2];       /*  56  interior word ranges set to (word & and) | or once the interior is   */
+    uint64_t force_count[2];       /*  72  prepared: locate only, both ranges; force_words: range 0 is the       */
+    uint64_t force_and[2];         /*  88  kernel's own and range 1 stays empty; any other kernel: both empty    */
+    uint64_t force_or[2];          /* 104  (count 0 = no range)                                                 */
+    uint32_t flags;                /* 120  CRO_SELFTEST_F_*                                                      */
+    uint32_t reserved;             /* 124  0                                                                     */
+} cro_selftest_sweep_opts;
+
+typedef struct cro_selftest_sweep_out {
+    cro_sweep_result sweep;        /*   0  the kernel's slot: its fold (reads, fused copy, locate, link read),    */
+                                   /*      window, bytes (2 * bytes for a copy) and variant (reads and copies)    */
+    uint64_t buf_bytes;            /*  56  the buffer: guards and interiors                                     */
+    uint64_t at[2];                /*  64  byte offset in it of interior 0 (a copy's source) and interior 1 (a   */
+                                   /*      copy's destination; the one interior again for every other kernel)   */
+    uint64_t after_xor[2];         /*  80  each interior's fold once the kernel is done, by the LDG read sweep   */
+    uint64_t after_sum[2];         /*  96                                                                        */
+    uint64_t after_wsum[2];        /* 112                                                                        */
+    uint64_t mismatches;           /* 128  locate, link read: the kernel's exact count                          */
+    uint64_t claims;               /* 136  ... and the record slots it claimed                                  */
+    uint64_t granules;             /* 144  ... and the granule bits it set (the locator's CRO_LOCATE_GRANULE_BYTES) */
+    uint64_t granule_min;          /* 152  lowest and highest granule set (0 when none)                         */
+    uint64_t granule_max;          /* 160                                                                        */
+} cro_selftest_sweep_out;
+
+/* Runs one sweep kernel of device dev_index, through the launch plan the context's CRO_* knobs made, on a fresh buffer of
+ * its own (device memory; mapped pinned host memory for the link rows) laid out as guards around the interior(s):
+ * [guard | interior | guard], or a copy's layout.  A guard is at least CRO_SELFTEST_GUARD_BYTES, so a kernel that
+ * strays past its interior by up to a ring lands in the hook's own allocation.  Before the kernel each guard is filled
+ * with its canary words (opts->canary) and each interior is prepared as the kernel's row above says: what the kernel
+ * writes starts as the complement of what it should write, so a word it misses shows.  The kernel runs once between the context's timing
+ * events and is waited for with the context's deadline (CRO_ERR_DEADLINE).  Then each interior is folded by the LDG
+ * read, the guards (and with CRO_SELFTEST_F_INTERIORS the interiors) are copied to buf at their buffer offsets, and
+ * words[0 .. *n) gets the kernel's records (locate, link read), by word, at most cap of them.  A buffer shorter than
+ * the layout (cap_bytes < out->buf_bytes) is CRO_ERR_BUFFER_SMALL with out->buf_bytes set, before anything runs.
+ * Never touches the sweep region; everything it allocates is freed before it returns. */
+int  cro_selftest_sweep(cro_ctx *ctx, int dev_index, const cro_selftest_sweep_opts *opts, cro_selftest_sweep_out *out,
+                        void *buf, uint64_t cap_bytes, cro_fault_word *words, int cap, int *n);
+
 #ifdef __cplusplus
 }
 #endif
