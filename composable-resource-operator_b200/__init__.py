@@ -357,6 +357,87 @@ class ScanReport(ctypes.Structure):
         return w.reserved, w.word_index - self.chunk[w.reserved].word0
 
 
+# SRAM probe (cro_probe_sram, cro_probe_sram_uuid, cro_read_sram_health)
+SRAM_SMEM, SRAM_DSMEM, SRAM_LEGS = 0, 1, 2
+SRAM_LEG_SMEM, SRAM_LEG_DSMEM, SRAM_ALL_LEGS = 1, 2, 3
+SRAM_ELEMENTS, SRAM_RECORDS, SRAM_MAX_SMS, SRAM_MAX_ITERATIONS, SRAM_MAX_ROUNDS, SRAM_MAX_PAIRS = 6, 4096, 256, 4096, 64, 8
+SRAM_NONE, SRAM_SM, SRAM_LINK, SRAM_ALL = 0, 1, 2, 3
+SRAM_PERSISTENT, SRAM_INTERMITTENT = 1, 2
+SRAM_DIR_LOCAL, SRAM_DIR_READ, SRAM_DIR_WRITE = 0, 1, 2
+SRAM_HEALTH_CORRECTED_DURING, SRAM_HEALTH_UNCORRECTED_DURING, SRAM_HEALTH_THRESHOLD_EXCEEDED = 1, 2, 4
+SRAM_NVML_ECC_CORRECTED, SRAM_NVML_ECC_UNCORRECTED, SRAM_NVML_STATUS = 1, 2, 4
+
+
+class SramOpts(ctypes.Structure):
+    _fields_ = [("legs", ctypes.c_uint32), ("iterations", ctypes.c_uint32), ("cluster", ctypes.c_uint32),
+                ("max_rounds", ctypes.c_uint32), ("deadline_ms", ctypes.c_int32), ("test_inject_leg", ctypes.c_int32),
+                ("test_inject_sm", ctypes.c_int32), ("test_inject_element", ctypes.c_uint32),
+                ("test_inject_iteration", ctypes.c_uint32), ("test_inject_word", ctypes.c_int32),
+                ("test_inject_mask", ctypes.c_uint64)]
+
+
+class SramHealth(ctypes.Structure):
+    """cro_sram_health: NVML's volatile SRAM ECC counts and field-diag threshold flag; `nvml` has a SRAM_NVML_* bit per
+    read answered."""
+    _fields_ = [("nvml", ctypes.c_uint32), ("threshold_exceeded", ctypes.c_uint32), ("ecc_corrected", ctypes.c_uint64),
+                ("ecc_uncorrected", ctypes.c_uint64)]
+
+
+class SramPair(ctypes.Structure):
+    """A network pair that failed: `from` (the reader or the writer, by `direction`) and the owner of the words."""
+    _fields_ = [("from_", ctypes.c_uint16), ("owner", ctypes.c_uint16), ("direction", ctypes.c_uint32)]
+
+
+class SramLeg(ctypes.Structure):
+    _fields_ = [("iterations", ctypes.c_uint32), ("rounds", ctypes.c_uint32), ("bytes", ctypes.c_uint64),
+                ("ns", ctypes.c_uint64), ("timer_ns", ctypes.c_uint64), ("sms_covered", ctypes.c_uint32),
+                ("complete", ctypes.c_uint32), ("mismatches", ctypes.c_uint64 * SRAM_ELEMENTS),
+                ("fold_mismatches", ctypes.c_uint64), ("recorded", ctypes.c_uint64), ("failed_sms", ctypes.c_uint32),
+                ("unpublished", ctypes.c_uint32), ("ctas", ctypes.c_uint32), ("cluster", ctypes.c_uint32),
+                ("fold_xor", ctypes.c_uint64), ("fold_sum", ctypes.c_uint64), ("fold_wsum", ctypes.c_uint64),
+                ("expect_xor", ctypes.c_uint64), ("expect_sum", ctypes.c_uint64), ("expect_wsum", ctypes.c_uint64)]
+
+    @property
+    def fold(self) -> Tuple[int, int, int]:
+        return (self.fold_xor, self.fold_sum, self.fold_wsum)
+
+    @property
+    def expect(self) -> Tuple[int, int, int]:
+        return (self.expect_xor, self.expect_sum, self.expect_wsum)
+
+
+class SramResult(ctypes.Structure):
+    """cro_sram_result: status, verdict, bad SMs and pairs, per-leg counts, coverage and times, and NVML's SRAM health of
+    one SRAM probe call."""
+    _fields_ = [("status", ctypes.c_int32), ("verdict", ctypes.c_uint32), ("seed", ctypes.c_uint64),
+                ("call", ctypes.c_uint64), ("sm_count", ctypes.c_uint32), ("legs", ctypes.c_uint32),
+                ("nsmid", ctypes.c_uint32), ("cuda_error", ctypes.c_int32), ("bytes_per_sm", ctypes.c_uint64),
+                ("health", ctypes.c_uint32), ("bad_sms", ctypes.c_uint32), ("bad_sm", ctypes.c_uint16 * 16),
+                ("bad_pairs", ctypes.c_uint32), ("sms_listed", ctypes.c_uint32), ("bad_pair", SramPair * SRAM_MAX_PAIRS),
+                ("recorded", ctypes.c_uint64), ("wall_ns", ctypes.c_uint64), ("helper_ns", ctypes.c_uint64),
+                ("before", SramHealth), ("after", SramHealth), ("leg", SramLeg * SRAM_LEGS)]
+
+
+class SramSmLeg(ctypes.Structure):
+    _fields_ = [("mismatches", ctypes.c_uint64 * SRAM_ELEMENTS), ("fold_mismatches", ctypes.c_uint64),
+                ("ns", ctypes.c_uint64), ("cycles", ctypes.c_uint64), ("ctas", ctypes.c_uint32), ("mark", ctypes.c_uint32)]
+
+
+class SramSm(ctypes.Structure):
+    """One SM seen by an SRAM probe call, with its per-element counts, times and SRAM_PERSISTENT / _INTERMITTENT mark
+    per leg."""
+    _fields_ = [("smid", ctypes.c_uint32), ("reserved", ctypes.c_uint32), ("leg", SramSmLeg * SRAM_LEGS)]
+
+
+class SramFault(ctypes.Structure):
+    """One failed compare: leg, element, iteration, the SM that compared, the other SM of a network pair, the direction,
+    the word's offset, expected and actual."""
+    _fields_ = [("leg", ctypes.c_uint32), ("element", ctypes.c_uint32), ("iteration", ctypes.c_uint32),
+                ("smid", ctypes.c_uint32), ("peer_smid", ctypes.c_uint32), ("direction", ctypes.c_uint32),
+                ("word", ctypes.c_uint32), ("reserved", ctypes.c_uint32), ("expected", ctypes.c_uint64),
+                ("actual", ctypes.c_uint64)]
+
+
 # test hook: one sweep kernel between guard bands (cro_selftest_sweep)
 (SELFTEST_SWEEP_FILL, SELFTEST_SWEEP_COPY_LDG, SELFTEST_SWEEP_COPY_TMA, SELFTEST_SWEEP_COPY_FUSED, SELFTEST_SWEEP_READ_LDG,
  SELFTEST_SWEEP_READ_TMA, SELFTEST_SWEEP_READ_LDG256, SELFTEST_SWEEP_LOCATE, SELFTEST_SWEEP_FORCE_WORDS,
@@ -391,6 +472,7 @@ assert ctypes.sizeof(ComputeResult) == 600 and ctypes.sizeof(ComputeSm) == 208, 
 assert ctypes.sizeof(FaultReport) == 928 and ctypes.sizeof(LocatePass) == 120, ctypes.sizeof(FaultReport)
 assert ctypes.sizeof(LinkResult) == 984 and ctypes.sizeof(PciPath) == 272, ctypes.sizeof(LinkResult)
 assert ctypes.sizeof(ScanReport) == 12632 and ctypes.sizeof(ScanOpts) == 72, ctypes.sizeof(ScanReport)
+assert ctypes.sizeof(SramResult) == 568 and ctypes.sizeof(SramSm) == 168 and ctypes.sizeof(SramFault) == 48, ctypes.sizeof(SramResult)
 
 # Every symbol include/croprobe.h declares; tests check the library exports all of them.
 EXPORTS = [
@@ -416,6 +498,7 @@ EXPORTS = [
     "cro_probe_host_link", "cro_pci_link_path", "cro_emit_link_annotations_json",
     "cro_probe_compute", "cro_compute_expected", "cro_emit_compute_annotations_json",
     "cro_scan_hbm", "cro_scan_hbm_uuid", "cro_read_hbm_health", "cro_emit_scan_annotations_json",
+    "cro_probe_sram", "cro_probe_sram_uuid", "cro_read_sram_health", "cro_emit_sram_annotations_json",
 ]
 
 # Slot map of a device's sweep-slot array (cro_sweep_slot, 64 bytes each); the cro_selftest_* hooks take such arrays.
@@ -522,6 +605,12 @@ def _load() -> ctypes.CDLL:
                                     ctypes.POINTER(i32)]),
         "cro_read_hbm_health": (i32, [c, ctypes.POINTER(HbmHealth)]),
         "cro_emit_scan_annotations_json": (i32, [ctypes.POINTER(ScanReport)] + out),
+        "cro_probe_sram": (i32, [vp, i32, ctypes.POINTER(SramOpts), ctypes.POINTER(SramResult), ctypes.POINTER(SramSm), i32,
+                                 ctypes.POINTER(i32), ctypes.POINTER(SramFault), i32, ctypes.POINTER(i32)]),
+        "cro_probe_sram_uuid": (i32, [vp, c, ctypes.POINTER(SramOpts), ctypes.POINTER(SramResult), ctypes.POINTER(SramSm), i32,
+                                      ctypes.POINTER(i32), ctypes.POINTER(SramFault), i32, ctypes.POINTER(i32)]),
+        "cro_read_sram_health": (i32, [c, ctypes.POINTER(SramHealth)]),
+        "cro_emit_sram_annotations_json": (i32, [ctypes.POINTER(SramResult)] + out),
         "cro_local_node_op": (i32, [vp, c] + out),
         "cro_local_exec": (i32, [c] + out),
         "cro_describe_wire_type": (i32, [c] + out),
@@ -674,6 +763,50 @@ def read_hbm_health(uuid: str) -> HbmHealth:
     if rc != OK:
         raise ProbeError(rc, "cro_read_hbm_health")
     return h
+
+
+def emit_sram_annotations_json(r: SramResult) -> str:
+    """Additive cohdi.io/probe-sram-* annotations of an SRAM probe result (Go-marshalled map[string]string)."""
+    return _text(lib.cro_emit_sram_annotations_json, ctypes.byref(r))
+
+
+def read_sram_health(uuid: str) -> SramHealth:
+    """cro_read_sram_health: the GPU's volatile SRAM ECC counts and threshold flag from NVML (no context, no CUDA)."""
+    h = SramHealth()
+    rc = lib.cro_read_sram_health(_b(uuid), ctypes.byref(h))
+    if rc != OK:
+        raise ProbeError(rc, "cro_read_sram_health")
+    return h
+
+
+def _sram_opts(legs: int, iterations: int, cluster: int, max_rounds: int, deadline_ms: int,
+               inject: Optional[Tuple[int, int, int, int, int, int]]) -> SramOpts:
+    o = SramOpts()
+    o.legs, o.iterations, o.cluster, o.max_rounds, o.deadline_ms = legs, iterations, cluster, max_rounds, deadline_ms
+    if inject is not None:
+        (o.test_inject_leg, o.test_inject_sm, o.test_inject_element, o.test_inject_iteration, o.test_inject_word,
+         o.test_inject_mask) = inject
+    return o
+
+
+def probe_sram_uuid(ctx: Optional["ProbeContext"], uuid: str, legs: int = SRAM_ALL_LEGS, iterations: int = 0, cluster: int = 0,
+                    max_rounds: int = 0, deadline_ms: int = 0, inject: Optional[Tuple[int, int, int, int, int, int]] = None,
+                    cap: int = 256) -> Tuple[SramResult, List[SramSm], List[SramFault]]:
+    """cro_probe_sram_uuid: the SRAM probe of any GPU on the node, run by the helper process (ctx may be None).
+    Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up to `cap` records."""
+    o = _sram_opts(legs, iterations, cluster, max_rounds, deadline_ms, inject)
+    r = SramResult()
+    sms = (SramSm * SRAM_MAX_SMS)()
+    arr = (SramFault * max(1, cap))()
+    n_sms, n = ctypes.c_int(), ctypes.c_int()
+    handle = ctx.handle if ctx is not None else None
+    rc = lib.cro_probe_sram_uuid(handle, _b(uuid), ctypes.byref(o), ctypes.byref(r), sms, SRAM_MAX_SMS, ctypes.byref(n_sms),
+                                 arr, cap, ctypes.byref(n))
+    if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
+        buf = ctypes.create_string_buffer(1024)
+        lib.cro_last_error(handle, buf, 1024)
+        raise ProbeError(rc, buf.value.decode("utf-8", "replace"))
+    return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
 
 
 def _scan_opts(max_bytes: int, reserve_bytes: int, seed: int, deadline_ms: int, chunk_bytes: int,
@@ -965,6 +1098,23 @@ class ProbeContext:
         self._check(lib.cro_scan_hbm(self.handle, dev, ctypes.byref(o), ctypes.byref(rep), arr, cap, ctypes.byref(n)),
                     allow=(ERR_CHECKSUM, ERR_CUDA))
         return rep, [arr[i] for i in range(n.value)]
+
+    def probe_sram(self, dev: int = 0, legs: int = SRAM_ALL_LEGS, iterations: int = 0, cluster: int = 0, max_rounds: int = 0,
+                   inject: Optional[Tuple[int, int, int, int, int, int]] = None,
+                   cap: int = 256) -> Tuple[SramResult, List[SramSm], List[SramFault]]:
+        """cro_probe_sram: March C- over every SM's shared memory (SRAM_LEG_SMEM) and the words of each cluster written
+        and read across the SM-to-SM network (SRAM_LEG_DSMEM, `cluster` CTAs: 2, 4 or 8).  iterations = 0 / cluster = 0 /
+        max_rounds = 0: the defaults.  inject = (leg, sm, element, iteration, word, mask) is the test-only stand-in for a
+        bad cell (sm, word: -1 for every one).  Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry
+        per SM seen and up to `cap` word records."""
+        o = _sram_opts(legs, iterations, cluster, max_rounds, 0, inject)
+        r = SramResult()
+        sms = (SramSm * SRAM_MAX_SMS)()
+        arr = (SramFault * max(1, cap))()
+        n_sms, n = ctypes.c_int(), ctypes.c_int()
+        self._check(lib.cro_probe_sram(self.handle, dev, ctypes.byref(o), ctypes.byref(r), sms, SRAM_MAX_SMS, ctypes.byref(n_sms),
+                                       arr, cap, ctypes.byref(n)), allow=(ERR_CHECKSUM, ERR_CUDA))
+        return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
 
     def launch_count(self) -> int:
         return int(lib.cro_launch_count(self.handle))

@@ -66,6 +66,13 @@ static_assert(sizeof(cro_scan_report) == 12632 && offsetof(cro_scan_report, elem
                   offsetof(cro_scan_report, before) == 152 && offsetof(cro_scan_report, pass) == 264 &&
                   offsetof(cro_scan_report, chunk) == 1368 && offsetof(cro_hbm_health, ecc_corrected) == 40,
               "scan layout");
+static_assert(sizeof(cro_sram_opts) == 48 && sizeof(cro_sram_health) == 24 && sizeof(cro_sram_pair) == 8 &&
+                  sizeof(cro_sram_leg) == 168 && offsetof(cro_sram_leg, fold_xor) == 120 && sizeof(cro_sram_sm_leg) == 80 &&
+                  sizeof(cro_sram_sm) == 168 && sizeof(cro_sram_fault) == 48, "sram layout");
+static_assert(sizeof(cro_sram_result) == 568 && offsetof(cro_sram_result, bad_sm) == 56 && offsetof(cro_sram_result, bad_pair) == 96 &&
+                  offsetof(cro_sram_result, recorded) == 160 && offsetof(cro_sram_result, before) == 184 &&
+                  offsetof(cro_sram_result, leg) == 232,
+              "sram layout");
 static_assert(sizeof(cro_selftest_sweep_opts) == 128 && offsetof(cro_selftest_sweep_opts, force_or) == 104 &&
                   sizeof(cro_selftest_sweep_out) == 168 && offsetof(cro_selftest_sweep_out, mismatches) == 128,
               "selftest sweep layout");
@@ -374,6 +381,48 @@ int cro_scan_hbm_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_scan_opts* o
 int cro_read_hbm_health(const char* gpu_uuid, cro_hbm_health* out) try {
     if (!gpu_uuid || !out) return CRO_ERR_INVALID_ARG;
     identity::NvmlHbmHealth(gpu_uuid, true, out);
+    return CRO_OK;
+} CRO_API_CATCH
+// The SRAM probe's two forms share the copy-out: sms[0 .. sms_cap) and faults[0 .. cap), and what was written in
+// sms_listed and recorded.
+static int sram_out(int rc, const std::vector<cro_sram_sm>& seen, const std::vector<cro_sram_fault>& found, cro_sram_result* out,
+                    cro_sram_sm* sms, int sms_cap, int* n_sms, cro_sram_fault* faults, int cap, int* n) {
+    const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
+    for (size_t j = 0; j < ks; ++j) sms[j] = seen[j];
+    for (size_t j = 0; j < kf; ++j) faults[j] = found[j];
+    out->sms_listed = (uint32_t)ks;
+    out->recorded = kf;
+    *n_sms = (int)ks;
+    *n = (int)kf;
+    return rc;
+}
+int cro_probe_sram(cro_ctx* ctx, int i, const cro_sram_opts* opts, cro_sram_result* out, cro_sram_sm* sms, int sms_cap,
+                   int* n_sms, cro_sram_fault* faults, int cap, int* n) try {
+    if (!ctx || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
+        return CRO_ERR_INVALID_ARG;
+    *n = *n_sms = 0;
+    cro_sram_opts o{};
+    if (opts) o = *opts;
+    std::vector<cro_sram_sm> seen;
+    std::vector<cro_sram_fault> found;
+    const int rc = ctx_probe_sram(ctx, i, o, out, &seen, &found);
+    return sram_out(rc, seen, found, out, sms, sms_cap, n_sms, faults, cap, n);
+} CRO_API_CATCH
+int cro_probe_sram_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_sram_opts* opts, cro_sram_result* out, cro_sram_sm* sms,
+                        int sms_cap, int* n_sms, cro_sram_fault* faults, int cap, int* n) try {
+    if (!gpu_uuid || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
+        return CRO_ERR_INVALID_ARG;
+    *n = *n_sms = 0;
+    cro_sram_opts o{};
+    if (opts) o = *opts;
+    std::vector<cro_sram_sm> seen;
+    std::vector<cro_sram_fault> found;
+    const int rc = ctx_probe_sram_uuid(ctx, gpu_uuid, o, out, &seen, &found, cap);
+    return sram_out(rc, seen, found, out, sms, sms_cap, n_sms, faults, cap, n);
+} CRO_API_CATCH
+int cro_read_sram_health(const char* gpu_uuid, cro_sram_health* out) try {
+    if (!gpu_uuid || !out) return CRO_ERR_INVALID_ARG;
+    identity::NvmlSramHealth(gpu_uuid, true, out);
     return CRO_OK;
 } CRO_API_CATCH
 int cro_compute_expected(int answer, uint64_t seed, int32_t* out) try {
@@ -732,6 +781,48 @@ int cro_emit_scan_annotations_json(const cro_scan_report* r, char* buf, size_t c
         for (int b = 0; b < 5; ++b) h += (b ? "," : "") + std::to_string(A.histogram[b]);
         m[p + "remap-histogram"] = h;
     }
+    gojson::Writer w;
+    w.string_map(m);
+    return copy_out(w.str(), buf, cap, len);
+} CRO_API_CATCH
+
+int cro_emit_sram_annotations_json(const cro_sram_result* r, char* buf, size_t cap, size_t* len) try {
+    if (!r) return CRO_ERR_INVALID_ARG;
+    static const char* const kHealth[3] = {"corrected", "uncorrected", "threshold-exceeded"};
+    std::map<std::string, std::string> m;
+    const std::string p = "cohdi.io/probe-sram-";
+    m[p + "verdict"] = r->status == CRO_OK                                                ? "ok"
+                       : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_SRAM_SM   ? "sm"
+                       : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_SRAM_LINK ? "link"
+                       : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_SRAM_ALL  ? "all"
+                       : r->status == CRO_ERR_CUDA ? "cuda-error:" + std::to_string(r->cuda_error)
+                                                   : "error";
+    uint32_t covered = 0xFFFFFFFFu;
+    for (int l = 0; l < CRO_SRAM_LEGS; ++l)
+        if (r->legs >> l & 1u) covered = std::min(covered, r->leg[l].sms_covered);
+    m[p + "sms"] = std::to_string(covered == 0xFFFFFFFFu ? 0u : covered) + "/" + std::to_string(r->sm_count);
+    if (r->bad_sms) {
+        std::string ids;
+        for (uint32_t j = 0; j < std::min<uint32_t>(r->bad_sms, 16); ++j) ids += (j ? "," : "") + std::to_string(r->bad_sm[j]);
+        m[p + "bad-sms"] = ids;
+    }
+    if (r->bad_pairs) {
+        std::string ps;
+        for (uint32_t j = 0; j < std::min<uint32_t>(r->bad_pairs, CRO_SRAM_MAX_PAIRS); ++j) {
+            const cro_sram_pair& q = r->bad_pair[j];
+            ps += (j ? "," : "") + std::to_string(q.from) + "-" + std::to_string(q.owner) +
+                  (q.direction == CRO_SRAM_DIR_READ ? ":r" : ":w");
+        }
+        m[p + "bad-pairs"] = ps;
+    }
+    m[p + "bytes-per-sm"] = std::to_string(r->bytes_per_sm);
+    std::string health;
+    for (int b = 0; b < 3; ++b)
+        if (r->health >> b & 1u) health += (health.empty() ? "" : ",") + std::string(kHealth[b]);
+    if (!health.empty()) m[p + "health"] = health;
+    const cro_sram_health &B = r->before, &A = r->after;
+    if (B.nvml & A.nvml & CRO_SRAM_NVML_ECC_CORRECTED) m[p + "ecc-corrected"] = std::to_string(A.ecc_corrected - B.ecc_corrected);
+    if (B.nvml & A.nvml & CRO_SRAM_NVML_ECC_UNCORRECTED) m[p + "ecc-uncorrected"] = std::to_string(A.ecc_uncorrected - B.ecc_uncorrected);
     gojson::Writer w;
     w.string_map(m);
     return copy_out(w.str(), buf, cap, len);

@@ -119,20 +119,12 @@ int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_comput
             R.iterations = iters[leg];
             R.expect_fold = (uint64_t)iters[leg] * cta_fold[answer];
             uint32_t fold_sm = ~0u;
-            do {
-                CU_TRY(c, cudaMemsetAsync(cta, 0xFF, cta_bytes, st));        // armed: a CTA that does not publish stays so
-                CU_TRY(c, cudaEventRecord(ev[0], st));
-                CU_TRY(c, launch_compute(leg, a, grid, st));
-                CU_TRY(c, cudaEventRecord(ev[1], st));
-                c->launches++;
-                CU_TRY(c, cudaMemcpyAsync(hc.data(), cta, cta_bytes, cudaMemcpyDeviceToHost, st));
-                CU_TRY(c, cudaMemcpyAsync(hbits, a.sm_bits, sizeof hbits, cudaMemcpyDeviceToHost, st));
-                const int e = wait_stream(c, d);
-                if (e) return e;
-                float ms = 0;
-                CU_TRY(c, cudaEventElapsedTime(&ms, ev[0], ev[1]));
-                R.ns += ms_to_ns(ms);
-                R.rounds++;
+            auto launch = [&] { return launch_compute(leg, a, grid, st); };
+            auto fetch = [&] {
+                cudaError_t e = cudaMemcpyAsync(hc.data(), cta, cta_bytes, cudaMemcpyDeviceToHost, st);
+                return e ? e : cudaMemcpyAsync(hbits, a.sm_bits, sizeof hbits, cudaMemcpyDeviceToHost, st);
+            };
+            auto take = [&](uint32_t* covered) -> int {
                 R.ctas += (uint32_t)grid;
                 R.ops += kComputeOps * iters[leg] * (uint64_t)grid;
                 uint64_t t0 = ~0ull, t1 = 0;
@@ -167,7 +159,11 @@ int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_comput
                 if (t1 > t0) R.timer_ns += t1 - t0;
                 R.sms_covered = 0;
                 for (int w = 0; w < kSmWords; ++w) R.sms_covered += (uint32_t)__builtin_popcountll(hbits[w]);
-            } while (R.sms_covered < (uint32_t)grid && R.rounds < max_rounds);
+                *covered = R.sms_covered;
+                return CRO_OK;
+            };
+            const int e = coverage_rounds(c, d, ev, cta, cta_bytes, (uint32_t)grid, max_rounds, &R.rounds, &R.ns, launch, fetch, take);
+            if (e) return e;
             R.complete = R.sms_covered >= (uint32_t)grid ? 1u : 0u;
             R.recorded = std::min<uint64_t>(hbits[kSmWords], CRO_COMPUTE_RECORDS);
             if (R.recorded) {

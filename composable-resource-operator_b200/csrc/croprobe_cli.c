@@ -19,6 +19,11 @@
  *                         <force_and> <force_or> <cap>
  *                                                    the same with every cro_scan_opts field; cro_scan_report and
  *                                                    its `recorded` cro_fault_word records (at most cap) on stdout
+ *   croprobe-cli sram-raw <uuid> <legs> <iterations> <cluster> <max_rounds> <inject_leg> <inject_sm> <inject_element>
+ *                         <inject_iteration> <inject_word> <inject_mask> <cap>
+ *                                                    the SRAM probe with every cro_sram_opts field; cro_sram_result,
+ *                                                    CRO_SRAM_MAX_SMS cro_sram_sm entries (sms_listed of them filled)
+ *                                                    and its `recorded` cro_sram_fault records (at most cap) on stdout
  * Exit 3: the device is not visible to this (fresh) process — the reference's found=false.
  *
  * Plain C against include/croprobe.h — the same surface the cgo shim binds.
@@ -49,7 +54,8 @@ int main(int argc, char **argv) {
     if (argc < 2) {
         fprintf(stderr, "usage: croprobe-cli csv <query> | enumerate | probe <uuid|index> [sweep_MiB] | probe-raw <uuid> [sweep_MiB] | "
                         "cold <uuid|index> [sweep_MiB] [nvml] | scan <uuid|index> [max_MiB] | scan-raw <uuid> <max> <reserve> <seed> <chunk> "
-                        "<first> <count> <and> <or> <cap>\n");
+                        "<first> <count> <and> <or> <cap> | sram-raw <uuid> <legs> <iterations> <cluster> <rounds> <leg> <sm> <element> <iteration> "
+                        "<word> <mask> <cap>\n");
         return 64;
     }
     const double t_start = now_s();
@@ -57,16 +63,18 @@ int main(int argc, char **argv) {
     const int raw = strcmp(cmd, "probe-raw") == 0;
     const int cold = strcmp(cmd, "cold") == 0;
     const int scan_raw = strcmp(cmd, "scan-raw") == 0;
-    const int wants_scan = scan_raw || strcmp(cmd, "scan") == 0;
+    const int sram_raw = strcmp(cmd, "sram-raw") == 0;
+    const int wants_scan = scan_raw || sram_raw || strcmp(cmd, "scan") == 0;
     const int wants_probe = raw || cold || strcmp(cmd, "probe") == 0;
     if ((wants_probe || wants_scan) && argc < 3) return 64;
     if (scan_raw && argc != 12) return 64;
+    if (sram_raw && argc != 14) return 64;
     cro_opts opts;
     memset(&opts, 0, sizeof opts);
     opts.abi_version = CRO_ABI_VERSION;
     opts.flags = CRO_F_LAZY_ALLOC | CRO_F_DEGRADE_ON_OOM;
     if (wants_scan) {
-        /* no sweep region (the scan allocates its own chunks) and NVML, whose DRAM health record the scan reads */
+        /* no sweep region (the scan allocates its own chunks) and NVML, whose DRAM / SRAM health record these read */
         opts.flags = CRO_F_LAZY_ALLOC;
         opts.sweep_bytes = 64ull << 20;
     }
@@ -130,6 +138,33 @@ int main(int argc, char **argv) {
             fprintf(stderr, "croprobe-cli: device '%s' is not visible\n", argv[2]);
             cro_probe_destroy(ctx);
             return 3;
+        }
+        if (sram_raw) {
+            cro_sram_opts so;
+            memset(&so, 0, sizeof so);
+            so.legs = (uint32_t)strtoul(argv[3], NULL, 10);
+            so.iterations = (uint32_t)strtoul(argv[4], NULL, 10);
+            so.cluster = (uint32_t)strtoul(argv[5], NULL, 10);
+            so.max_rounds = (uint32_t)strtoul(argv[6], NULL, 10);
+            so.test_inject_leg = atoi(argv[7]);
+            so.test_inject_sm = atoi(argv[8]);
+            so.test_inject_element = (uint32_t)strtoul(argv[9], NULL, 10);
+            so.test_inject_iteration = (uint32_t)strtoul(argv[10], NULL, 10);
+            so.test_inject_word = atoi(argv[11]);
+            so.test_inject_mask = (uint64_t)strtoull(argv[12], NULL, 10);
+            const int cap = atoi(argv[13]);
+            static cro_sram_result sr;
+            static cro_sram_sm sms[CRO_SRAM_MAX_SMS];
+            cro_sram_fault *faults = (cro_sram_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
+            int n_sms = 0, got = 0;
+            if (!faults) return 2;
+            cro_probe_sram(ctx, idx, &so, &sr, sms, CRO_SRAM_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
+            /* the result whatever its status: the library reads why from it */
+            if (fwrite(&sr, sizeof sr, 1, stdout) != 1 || fwrite(sms, sizeof sms, 1, stdout) != 1 ||
+                (got && fwrite(faults, sizeof *faults, (size_t)got, stdout) != (size_t)got))
+                return 2;
+            fflush(stdout);
+            _exit(sr.status == CRO_OK ? 0 : 1);
         }
         if (wants_scan) {
             cro_scan_opts so;

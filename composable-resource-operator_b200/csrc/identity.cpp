@@ -418,12 +418,21 @@ bool ScanNvml(std::vector<NvmlGpu>* out, std::string* err) {
 }
 
 // One NVML session for the life of the process (init is reference-counted, so the init/shutdown pairs of ScanNvml
-// still balance): the per-probe ECC read, the link probe's replay counter and the scan's memory health must not pay
-// nvmlInit every time.  A reader whose symbol the library lacks answers false.
+// still balance): the per-probe ECC read, the link probe's replay counter and the scan's and SRAM probe's memory health
+// must not pay nvmlInit every time.  A reader whose symbol the library lacks answers false.
 namespace {
 struct NvmlRemapHistogram {  // nvmlRowRemapperHistogramValues_t
     unsigned max, high, partial, low, none;
 };
+struct NvmlSramStatus {  // nvmlEccSramErrorStatus_v1_t
+    unsigned version;
+    unsigned long long aggregateUncParity, aggregateUncSecDed, aggregateCor, volatileUncParity, volatileUncSecDed,
+        volatileCor, aggregateUncBucketL2, aggregateUncBucketSm, aggregateUncBucketPcie, aggregateUncBucketMcu,
+        aggregateUncBucketOther;
+    unsigned bThresholdExceeded;
+};
+static_assert(sizeof(NvmlSramStatus) == 104, "nvmlEccSramErrorStatus_v1_t");
+constexpr unsigned kNvmlSramStatusV1 = (unsigned)sizeof(NvmlSramStatus) | (1u << 24);   // NVML_STRUCT_VERSION(.., 1)
 struct NvmlSession {
     int (*byUuid)(const char*, nvmlDevice_t*) = nullptr;
     int (*ecc)(nvmlDevice_t, int, int, unsigned long long*) = nullptr;
@@ -431,6 +440,7 @@ struct NvmlSession {
     int (*memErrors)(nvmlDevice_t, int, int, int, unsigned long long*) = nullptr;
     int (*remapped)(nvmlDevice_t, unsigned*, unsigned*, unsigned*, unsigned*) = nullptr;
     int (*histogram)(nvmlDevice_t, NvmlRemapHistogram*) = nullptr;
+    int (*sramStatus)(nvmlDevice_t, NvmlSramStatus*) = nullptr;
     bool ok = false;
 };
 const NvmlSession& nvml_session() {
@@ -446,6 +456,7 @@ const NvmlSession& nvml_session() {
         s.memErrors = (int (*)(nvmlDevice_t, int, int, int, unsigned long long*))dlsym(h, "nvmlDeviceGetMemoryErrorCounter");
         s.remapped = (int (*)(nvmlDevice_t, unsigned*, unsigned*, unsigned*, unsigned*))dlsym(h, "nvmlDeviceGetRemappedRows");
         s.histogram = (int (*)(nvmlDevice_t, NvmlRemapHistogram*))dlsym(h, "nvmlDeviceGetRowRemapperHistogram");
+        s.sramStatus = (int (*)(nvmlDevice_t, NvmlSramStatus*))dlsym(h, "nvmlDeviceGetSramEccErrorStatus");
         s.ok = init && s.byUuid && init() == 0;
     });
     return s;
@@ -497,6 +508,26 @@ void NvmlHbmHealth(const std::string& gpu_uuid, bool histogram, cro_hbm_health* 
         const unsigned v[5] = {h.max, h.high, h.partial, h.low, h.none};
         memcpy(out->histogram, v, sizeof v);
         out->nvml |= CRO_HBM_NVML_HISTOGRAM;
+    }
+}
+
+void NvmlSramHealth(const std::string& gpu_uuid, bool status, cro_sram_health* out) {
+    memset(out, 0, sizeof *out);
+    const NvmlSession& s = nvml_session();
+    nvmlDevice_t dev = nullptr;
+    if (!nvml_device(s, gpu_uuid, &dev)) return;
+    if (s.memErrors) {
+        // NVML_MEMORY_ERROR_TYPE_CORRECTED 0 / _UNCORRECTED 1, NVML_VOLATILE_ECC 0, NVML_MEMORY_LOCATION_SRAM 7
+        unsigned long long v = 0;
+        if (s.memErrors(dev, 0, 0, 7, &v) == 0) { out->ecc_corrected = v; out->nvml |= CRO_SRAM_NVML_ECC_CORRECTED; }
+        v = 0;
+        if (s.memErrors(dev, 1, 0, 7, &v) == 0) { out->ecc_uncorrected = v; out->nvml |= CRO_SRAM_NVML_ECC_UNCORRECTED; }
+    }
+    NvmlSramStatus st{};
+    st.version = kNvmlSramStatusV1;
+    if (status && s.sramStatus && s.sramStatus(dev, &st) == 0) {
+        out->threshold_exceeded = st.bThresholdExceeded ? 1u : 0u;
+        out->nvml |= CRO_SRAM_NVML_STATUS;
     }
 }
 

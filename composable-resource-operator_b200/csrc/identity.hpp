@@ -92,6 +92,10 @@ bool NvmlPcieReplays(const std::string& gpu_uuid, unsigned long long* out);
 // (nvmlDeviceGetRemappedRows) and, with `histogram`, the row remapper's histogram.  out->nvml has a CRO_HBM_NVML_* bit
 // per read NVML answered; a refused read leaves its fields 0.
 void NvmlHbmHealth(const std::string& gpu_uuid, bool histogram, cro_hbm_health* out);
+// The device's SRAM health record: volatile SRAM ECC counts (nvmlDeviceGetMemoryErrorCounter) and, with `status`, the
+// field-diag threshold flag of nvmlDeviceGetSramEccErrorStatus (looked up by name: older drivers lack it).
+// out->nvml has a CRO_SRAM_NVML_* bit per read NVML answered.
+void NvmlSramHealth(const std::string& gpu_uuid, bool status, cro_sram_health* out);
 
 }  // namespace identity
 }  // namespace cro

@@ -24,6 +24,7 @@
 // The probe path has no tensor cores: there is no contraction on it.  The compute
 // probe uses them on purpose: checking them is its job.
 #include "kernels.cuh"
+#include "warp_claim.cuh"
 
 #include <cuda_bf16.h>
 #include <cuda_fp8.h>
@@ -436,21 +437,8 @@ template <int K>
 __device__ __forceinline__ void locate_record(const unsigned long long (&d)[K], unsigned m, unsigned long long v0,
                                               unsigned long long vstride, const LocateCtx& L) {
     const unsigned lane = threadIdx.x & 31u;
-    const unsigned n_lane = __popc(m);
-    const unsigned n_warp = __reduce_add_sync(0xffffffffu, n_lane);
-    unsigned incl = n_lane;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= (unsigned)o) incl += t;
-    }
-    unsigned long long base = kLocateRecords;
-    if (lane == 0) {
-        atomicAdd(L.s_count, (unsigned long long)n_warp);
-        if (*reinterpret_cast<volatile unsigned long long*>(&L.b.ctr->claims) < kLocateRecords)
-            base = atomicAdd(&L.b.ctr->claims, (unsigned long long)n_warp);
-    }
-    base = __shfl_sync(0xffffffffu, base, 0) + (incl - n_lane);
+    unsigned long long base = warp_claim(__popc(m), &L.b.ctr->claims, kLocateRecords,
+                                         [&](unsigned n_warp) { atomicAdd(L.s_count, (unsigned long long)n_warp); });
     unsigned long long flips = 0;
     unsigned gmin = ~0u, gmax = 0;
 #pragma unroll
@@ -1394,19 +1382,7 @@ __device__ __forceinline__ typename ComputeLeg<LEG>::Acc alu_elem(const unsigned
 template <unsigned LEG, int C>
 __device__ __forceinline__ void compute_record(const typename ComputeLeg<LEG>::Acc (&acc)[128], unsigned m, unsigned r0,
                                                unsigned c0, unsigned smid, const ComputeArgs& a) {
-    const unsigned lane = threadIdx.x & 31u;
-    const unsigned n_lane = __popc(m);
-    const unsigned n_warp = __reduce_add_sync(0xffffffffu, n_lane);
-    unsigned incl = n_lane;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= (unsigned)o) incl += t;
-    }
-    unsigned long long base = CRO_COMPUTE_RECORDS;
-    if (lane == 0 && *reinterpret_cast<volatile unsigned long long*>(a.claims) < CRO_COMPUTE_RECORDS)
-        base = atomicAdd(a.claims, (unsigned long long)n_warp);
-    base = __shfl_sync(0xffffffffu, base, 0) + (incl - n_lane);
+    unsigned long long base = warp_claim(__popc(m), a.claims, CRO_COMPUTE_RECORDS, [](unsigned) {});
 #pragma unroll
     for (int q = 0; q < 32; ++q) {
         const int j = 32 * C + q;

@@ -178,6 +178,49 @@ struct ComputeArgs {
 constexpr int kComputeThreads = 256;            // two warpgroups of 64 rows each
 cudaError_t launch_compute(unsigned leg, const ComputeArgs& a, int grid, cudaStream_t);
 
+// SRAM probe (cro_probe_sram, sram_kernels.cu).  Local leg: `grid` CTAs of kSramThreads, each marching its own
+// n_words of dynamic shared memory (March C-, include/croprobe.h).  Network leg: clusters of `cluster` CTAs, rank r
+// with seed + r * kNonceStride.  Each CTA publishes one SramCta (stamp last = the call number) and records its
+// mismatching words while the leg's record buffer has room (*claims counts the slots claimed, possibly past the end).
+struct SramCta {
+    unsigned long long stamp;                   // the call number; all ones (armed) = the CTA did not publish
+    unsigned long long t0, t1;                  // %globaltimer around the iterations
+    unsigned long long cycles;                  // %clock64 around the iterations
+    unsigned long long count[CRO_SRAM_ELEMENTS];  // compares that failed, per element
+    unsigned long long last;                    // ... of them in the last iteration
+    unsigned long long fold_x, fold_s, fold_w;  // local: M5 fold over every iteration
+    unsigned smid, nsmid, rank, block;          // rank in the cluster (0 for the local leg), blockIdx.x
+};
+static_assert(sizeof(SramCta) == 128, "per-CTA record");
+struct SramRecord {
+    unsigned element, iteration, smid;          // smid: the CTA whose compare failed
+    unsigned peer_block;                        // network: blockIdx.x of the owner (D1) or the writer (D3)
+    unsigned round, word;                       // round: the launch's round number, to resolve peer_block
+    unsigned long long expected, actual;
+};
+static_assert(sizeof(SramRecord) == 40, "word record");
+struct SramArgs {
+    SramCta* cta;                               // grid entries
+    SramRecord* rec;                            // CRO_SRAM_RECORDS entries
+    unsigned long long* claims;
+    unsigned long long seed, stamp;
+    unsigned n_words;                           // a multiple of 32 (the march loops stay warp-uniform)
+    unsigned iterations;
+    unsigned round;
+    int inj_sm, inj_word;                       // -1: every SM / word
+    unsigned inj_element, inj_iter;
+    unsigned long long inj_mask;                // 0: nothing is injected in this launch
+};
+constexpr int kSramThreads = 1024;
+// The words each CTA marches on the current device: its opt-in shared memory per block less the kernels' static
+// shared memory, rounded down to 32 words.  Sets both kernels' dynamic shared memory to that and the carve-out to
+// the most shared memory.
+cudaError_t sram_plan(int device, unsigned* n_words);
+cudaError_t launch_sram_smem(const SramArgs& a, int grid, cudaStream_t);
+cudaError_t launch_sram_dsmem(const SramArgs& a, int grid, unsigned cluster, cudaStream_t);
+// Clusters of `cluster` CTAs the device can hold at once with the leg's shared memory (0: none fits).
+cudaError_t sram_max_clusters(unsigned cluster, unsigned n_words, int* clusters);
+
 // Pointer chase for NVLink latency: warp j of the one CTA follows `hops` dependent ld.relaxed.sys loads through
 // table[j] (one 8-byte slot per 128-byte line, peer-resident); out[2j] = final index, out[2j+1] = %globaltimer ns.
 struct ChaseArgs {

@@ -77,6 +77,7 @@ struct Device {
     std::unique_ptr<LinkState> link;       // host link probe (ctx_probe_host_link), made at its first call
     uint64_t link_calls = 0;               // k of the next host link probe call: its seeds
     uint64_t compute_calls = 0;            // k of the next compute probe call (ctx_probe_compute): its operand seed
+    uint64_t sram_calls = 0;               // k of the next SRAM probe call (ctx_probe_sram): its seeds
     KernelPlan plan{};
     SweepScratch scratch{}, scratch_aux{}, scratch_pfx{};   // main stream / closed form / p2p prefix closed form
     // lane 0's buffers under their old names: the synchronous probe, the single sweeps and cro_probe_all use lane 0
@@ -228,6 +229,16 @@ int ctx_scan_hbm_uuid(cro_ctx* c, const char* uuid, const cro_scan_opts& o, cro_
                       int cap);
 // CRO_SCAN_HEALTH_* of the NVML reads before E0 and after E3.
 uint32_t scan_health(const cro_hbm_health& before, const cro_hbm_health& after);
+
+// SRAM probe (include/croprobe.h, cro_probe_sram / cro_probe_sram_uuid, sram_probe.cu): *sms gets one entry per SM
+// seen, by SM id; *faults every recorded word, by (leg, element, smid, iteration, word).  The uuid form runs
+// `croprobe-cli sram-raw` and asks it for at most cap words.
+int ctx_probe_sram(cro_ctx* c, int idx, const cro_sram_opts& o, cro_sram_result* r, std::vector<cro_sram_sm>* sms,
+                   std::vector<cro_sram_fault>* faults);
+int ctx_probe_sram_uuid(cro_ctx* c, const char* uuid, const cro_sram_opts& o, cro_sram_result* r, std::vector<cro_sram_sm>* sms,
+                        std::vector<cro_sram_fault>* faults, int cap);
+// CRO_SRAM_HEALTH_* of the NVML reads before the first leg and after the last.
+uint32_t sram_health(const cro_sram_health& before, const cro_sram_health& after);
 
 // test hooks (include/croprobe.h, cro_selftest_*): the verdict kernels and the chase on caller-given inputs
 int ctx_selftest_probe_finalize(cro_ctx* c, int idx, const cro_probe_result* tmpl, const cro_sweep_slot* slots,

@@ -237,6 +237,34 @@ struct DeviceMem {
     ~DeviceMem() { cudaFree(p); }
 };
 
+// The per-SM probes' coverage loop (the compute and SRAM probes): one launch per round, relaunched while fewer than
+// `want` SMs were seen and fewer than max_rounds rounds ran.  Each round arms the CTA records (all ones: a CTA that
+// does not publish stays so), times launch() with ev, then fetch() enqueues the copies back, the stream is waited for
+// and take(&covered) reads the round's records and says how many distinct SMs were seen so far.  *ns sums the rounds'
+// event times.
+template <class Launch, class Fetch, class Take>
+int coverage_rounds(cro_ctx* c, Device* d, cudaEvent_t (&ev)[2], void* cta, size_t cta_bytes, uint32_t want, uint32_t max_rounds,
+                    uint32_t* rounds, uint64_t* ns, Launch launch, Fetch fetch, Take take) {
+    uint32_t covered = 0;
+    do {
+        CU_TRY(c, cudaMemsetAsync(cta, 0xFF, cta_bytes, d->stream));
+        CU_TRY(c, cudaEventRecord(ev[0], d->stream));
+        CU_TRY(c, launch());
+        CU_TRY(c, cudaEventRecord(ev[1], d->stream));
+        c->launches++;
+        CU_TRY(c, fetch());
+        const int e = wait_stream(c, d);
+        if (e) return e;
+        float ms = 0;
+        CU_TRY(c, cudaEventElapsedTime(&ms, ev[0], ev[1]));
+        *ns += ms_to_ns(ms);
+        ++*rounds;
+        const int rc = take(&covered);
+        if (rc) return rc;
+    } while (covered < want && *rounds < max_rounds);
+    return CRO_OK;
+}
+
 // The typed parts of one copy of a MismatchBuffer: the device block or its host mirror.
 struct MismatchView {
     LocateCounters* ctr;               // [check]

@@ -1,0 +1,377 @@
+// sram_probe.cu — the SRAM probe (cro_probe_sram, cro_probe_sram_uuid): every SM's shared memory marched as 0 and as
+// 1, the SM-to-SM network of a cluster written and read across, and the SRAM ECC record NVML keeps for them.
+#include <map>
+#include <set>
+#include <tuple>
+
+#include "inventory.hpp"
+#include "probe_internal.hpp"
+
+namespace cro {
+
+namespace {
+// Seeds of call k: seed_dev + 2^60 + (8k + r) * kNonceStride for cluster rank r < 8 (r = 0: the local leg's, the one
+// reported).  No other seed of the device reaches them while every count stays below 2^57.  The stride is odd, hence
+// invertible mod 2^64, and 2^60 times an odd number is c * 2^60 with c odd (mod 2^64), which as a signed difference is
+// an odd multiple of 2^60, at least 2^60 in size:
+//   probe nonce n:       seed_dev + n * stride needs (8k + r - n) * stride = -2^60: n or 8k + r is at least 2^60;
+//   locator retest:      seed_dev + 2^63 needs (8k + r) * stride = 2^63 - 2^60 = 7 * 2^60, so 8k + r >= 2^60;
+//   link pattern 3k'+j:  seed_dev + 2^62 + (3k' + j) * stride needs (8k + r - 3k' - j) * stride = 3 * 2^60, so
+//                        8k + r or 3k' + j is at least 2^60;
+//   compute call k':     seed_dev + 2^61 + k' * stride needs (8k + r - k') * stride = 2^60, so 8k + r or k' >= 2^60.
+// Distinct (k, r) give distinct seeds: no call passes on what an earlier call, or another rank, left in shared memory,
+// which no launch clears.
+constexpr uint64_t kSramSeedOffset = 1ull << 60;
+constexpr uint64_t kSramSeedsPerCall = 8;           // the largest cluster
+// Iterations per CTA and launches per leg when the caller gives none.  On an H100 80GB HBM3 at a 400 W limit
+// (profiles/h100_400w_sram_rate.jsonl) a local launch of 64 iterations takes 2.9 ms and a network launch at C = 2
+// 1.8 ms, and one round of each covers all 132 SMs: about 5 ms a call for every cell written and read back 64 times
+// each way.  The time grows linearly with iterations (DESIGN.md "The SRAM probe").
+constexpr uint32_t kSramDefaultIterations = 64;
+constexpr uint32_t kSramDefaultRounds = 4;
+constexpr uint32_t kSramDefaultCluster = 2;
+
+// The result of a call that marched nothing: zeroes but for what the call had settled before it stopped.
+void blank_result(cro_sram_result* r, const cro_sram_result& from, std::vector<cro_sram_sm>* sms, std::vector<cro_sram_fault>* faults) {
+    const cro_sram_result keep = from;
+    memset(r, 0, sizeof *r);
+    r->seed = keep.seed;
+    r->call = keep.call;
+    r->sm_count = keep.sm_count;
+    r->legs = keep.legs;
+    r->bytes_per_sm = keep.bytes_per_sm;
+    r->cuda_error = keep.cuda_error;
+    r->before = keep.before;
+    r->after = keep.after;
+    r->health = keep.health;
+    sms->clear();
+    faults->clear();
+}
+
+// What every CTA's M5 fold must be: the read-sweep checksum of pattern_word(seed, 0 .. n) once per iteration (xor of
+// the iterations' folds, sums summed).
+void closed_form(uint64_t seed, uint32_t n, uint32_t iterations, cro_sram_leg* L) {
+    uint64_t x = 0, s = 0, w = 0;
+    for (uint64_t i = 0; i < n; ++i) {
+        const uint64_t v = pattern_word(seed, i);
+        x ^= v;
+        s += v;
+        w += v * (2 * i + 1);
+    }
+    L->expect_xor = (iterations & 1) ? x : 0;
+    L->expect_sum = s * iterations;
+    L->expect_wsum = w * iterations;
+}
+
+bool valid_injection(const cro_sram_opts& o, uint32_t iterations) {
+    if (!o.test_inject_mask) return true;
+    const bool el = o.test_inject_leg == CRO_SRAM_SMEM ? (o.test_inject_element >= 1 && o.test_inject_element <= 5)
+                    : o.test_inject_leg == CRO_SRAM_DSMEM ? (o.test_inject_element == 1 || o.test_inject_element == 2)
+                                                          : false;
+    return el && o.test_inject_sm >= -1 && o.test_inject_sm < CRO_SRAM_MAX_SMS && o.test_inject_iteration < iterations &&
+           o.test_inject_word >= -1;
+}
+}  // namespace
+
+uint32_t sram_health(const cro_sram_health& b, const cro_sram_health& a) {
+    uint32_t h = 0;
+    if ((b.nvml & a.nvml & CRO_SRAM_NVML_ECC_CORRECTED) && a.ecc_corrected > b.ecc_corrected) h |= CRO_SRAM_HEALTH_CORRECTED_DURING;
+    if ((b.nvml & a.nvml & CRO_SRAM_NVML_ECC_UNCORRECTED) && a.ecc_uncorrected > b.ecc_uncorrected) h |= CRO_SRAM_HEALTH_UNCORRECTED_DURING;
+    if ((a.nvml & CRO_SRAM_NVML_STATUS) && a.threshold_exceeded) h |= CRO_SRAM_HEALTH_THRESHOLD_EXCEEDED;
+    return h;
+}
+
+int ctx_probe_sram(cro_ctx* c, int idx, const cro_sram_opts& o, cro_sram_result* r, std::vector<cro_sram_sm>* sms,
+                   std::vector<cro_sram_fault>* faults) {
+    const uint64_t t_call = now_ns();
+    blank_result(r, cro_sram_result{}, sms, faults);
+    Device* d = dev_at(c, idx);
+    if (!d) return r->status = unknown_device(c, idx, "a GPU attached after init is probed through the helper process, cro_probe_sram_uuid");
+    const uint32_t legs = o.legs ? o.legs : CRO_SRAM_ALL_LEGS;
+    const uint32_t iters = o.iterations ? o.iterations : kSramDefaultIterations;
+    const uint32_t cluster = o.cluster ? o.cluster : kSramDefaultCluster;
+    const uint32_t max_rounds = o.max_rounds ? o.max_rounds : kSramDefaultRounds;
+    if ((legs & ~CRO_SRAM_ALL_LEGS) || iters > CRO_SRAM_MAX_ITERATIONS || (cluster != 2 && cluster != 4 && cluster != 8) ||
+        max_rounds > CRO_SRAM_MAX_ROUNDS || !valid_injection(o, iters)) {
+        c->set_error("SRAM probe: legs must be CRO_SRAM_ALL_LEGS bits, iterations at most " + std::to_string(CRO_SRAM_MAX_ITERATIONS) +
+                     ", cluster 2, 4 or 8, max_rounds at most " + std::to_string(CRO_SRAM_MAX_ROUNDS) +
+                     ", and an injection must name a leg, an element it has (local 1 .. 5, network 1 or 2), an SM id below " +
+                     std::to_string(CRO_SRAM_MAX_SMS) + " (or -1), an iteration the call runs and a word (or -1)");
+        return r->status = CRO_ERR_INVALID_ARG;
+    }
+    DeviceGuard g = enter_device(c, idx);
+    if (g.rc) return r->status = g.rc;
+    Range nv(c, "cro.probe_sram");
+    const std::string uuid(d->info.gpu_uuid, strnlen(d->info.gpu_uuid, sizeof d->info.gpu_uuid));
+    const bool nvml = !(c->opts.flags & CRO_F_NO_NVML);
+    std::map<uint32_t, cro_sram_sm> per_sm;
+    std::map<uint32_t, uint64_t> last[CRO_SRAM_LEGS];       // per SM: failed compares of the last iteration
+    std::vector<SramRecord> recs[CRO_SRAM_LEGS];
+    std::vector<std::vector<uint32_t>> block_smid;          // network leg, per round: blockIdx.x -> %smid (~0u: silent)
+    bool marched = false;
+    cudaEvent_t ev[2] = {nullptr, nullptr};                  // the call's own, destroyed on every way out
+    int rc = [&]() -> int {
+        const int sm_count = d->plan.sm_count;
+        unsigned n_words = 0;
+        CU_TRY(c, sram_plan(d->ordinal, &n_words));
+        if (o.test_inject_mask && o.test_inject_word >= (int)n_words) {
+            c->set_error("SRAM probe: injection word " + std::to_string(o.test_inject_word) + " is past the " +
+                         std::to_string(n_words) + " words each CTA marches");
+            return CRO_ERR_INVALID_ARG;
+        }
+        int clusters = 0;
+        if (legs & CRO_SRAM_LEG_DSMEM) {
+            CU_TRY(c, sram_max_clusters(cluster, n_words, &clusters));
+            if (clusters < 1) {
+                c->set_error("SRAM probe: the device cannot place one cluster of " + std::to_string(cluster) + " CTAs with " +
+                             std::to_string(8ull * n_words) + " bytes of shared memory each");
+                return CRO_ERR_UNSUPPORTED;
+            }
+        }
+        const int net_grid = clusters * (int)cluster, max_grid = std::max(sm_count, net_grid);
+        const uint64_t k = d->sram_calls++;
+        const uint64_t seed = d->seed_dev + kSramSeedOffset + k * kSramSeedsPerCall * kNonceStride;
+        r->seed = seed;
+        r->call = k;
+        r->sm_count = (uint32_t)sm_count;
+        r->legs = legs;
+        r->bytes_per_sm = 8ull * n_words;
+
+        // [claims per leg][records per leg][CTA records], allocated per call
+        const size_t rec_off = 64, rec_bytes = (size_t)CRO_SRAM_LEGS * CRO_SRAM_RECORDS * sizeof(SramRecord);
+        const size_t cta_off = (rec_off + rec_bytes + 63) & ~(size_t)63;
+        DeviceMem<unsigned char> b;
+        CU_TRY(c, cudaMalloc(&b.p, cta_off + (size_t)max_grid * sizeof(SramCta)));
+        for (cudaEvent_t& x : ev) CU_TRY(c, cudaEventCreate(&x));
+        cudaStream_t st = d->stream;
+        CU_TRY(c, cudaMemsetAsync(b.p, 0, rec_off, st));
+        unsigned long long* claims = reinterpret_cast<unsigned long long*>(b.p);
+        SramRecord* rec = reinterpret_cast<SramRecord*>(b.p + rec_off);
+        SramCta* cta = reinterpret_cast<SramCta*>(b.p + cta_off);
+        std::vector<SramCta> hc((size_t)max_grid);
+        if (nvml) identity::NvmlSramHealth(uuid, false, &r->before);
+        marched = true;
+
+        for (uint32_t leg = 0; leg < CRO_SRAM_LEGS; ++leg) {
+            if (!(legs >> leg & 1u)) continue;
+            cro_sram_leg& R = r->leg[leg];
+            const bool net = leg == CRO_SRAM_DSMEM;
+            const int grid = net ? net_grid : sm_count;
+            SramArgs a{};
+            a.cta = cta;
+            a.rec = rec + (size_t)leg * CRO_SRAM_RECORDS;
+            a.claims = claims + leg;
+            a.seed = seed;
+            a.stamp = k;
+            a.n_words = n_words;
+            a.iterations = iters;
+            a.inj_sm = o.test_inject_sm;
+            a.inj_word = o.test_inject_word;
+            a.inj_element = o.test_inject_element;
+            a.inj_iter = o.test_inject_iteration;
+            a.inj_mask = o.test_inject_leg == (int)leg ? o.test_inject_mask : 0ull;
+            R.iterations = iters;
+            R.cluster = net ? cluster : 0u;
+            if (!net) closed_form(seed, n_words, iters, &R);
+            // local: M0 and M5 touch every word once, M1 .. M4 twice; network: D0, D2, D3 once and D1 once per peer
+            const uint64_t cta_bytes_moved = 8ull * n_words * iters * (net ? cluster + 2 : 10);
+            const size_t cta_bytes = (size_t)grid * sizeof(SramCta);
+            std::set<uint32_t> seen;
+            uint32_t fold_sm = ~0u;
+            auto launch = [&] {
+                a.round = R.rounds;
+                return net ? launch_sram_dsmem(a, grid, cluster, st) : launch_sram_smem(a, grid, st);
+            };
+            auto fetch = [&] { return cudaMemcpyAsync(hc.data(), cta, cta_bytes, cudaMemcpyDeviceToHost, st); };
+            auto take = [&](uint32_t* covered) -> int {
+                R.ctas += (uint32_t)grid;
+                R.bytes += cta_bytes_moved * (uint64_t)grid;
+                if (net) block_smid.emplace_back((size_t)grid, ~0u);
+                uint64_t t0 = ~0ull, t1 = 0;
+                for (int j = 0; j < grid; ++j) {
+                    const SramCta& x = hc[(size_t)j];
+                    if (x.stamp != k) {
+                        R.unpublished++;
+                        continue;
+                    }
+                    if (x.nsmid > CRO_SRAM_MAX_SMS) {
+                        c->set_error("SRAM probe: the device reports %nsmid = " + std::to_string(x.nsmid) + ", more SM ids than the " +
+                                     std::to_string(CRO_SRAM_MAX_SMS) + " the result holds");
+                        return CRO_ERR_UNSUPPORTED;
+                    }
+                    r->nsmid = x.nsmid;
+                    t0 = std::min<uint64_t>(t0, x.t0);
+                    t1 = std::max<uint64_t>(t1, x.t1);
+                    if (net) block_smid.back()[(size_t)j] = x.smid;
+                    seen.insert(x.smid);
+                    cro_sram_sm& S = per_sm[x.smid];
+                    S.smid = x.smid;
+                    cro_sram_sm_leg& SL = S.leg[leg];
+                    SL.ctas++;
+                    for (int e = 0; e < CRO_SRAM_ELEMENTS; ++e) {
+                        SL.mismatches[e] += x.count[e];
+                        R.mismatches[e] += x.count[e];
+                    }
+                    last[leg][x.smid] += x.last;
+                    SL.ns += x.t1 > x.t0 ? x.t1 - x.t0 : 0;
+                    SL.cycles += x.cycles;
+                    if (net) continue;
+                    const bool fold_bad = x.fold_x != R.expect_xor || x.fold_s != R.expect_sum || x.fold_w != R.expect_wsum;
+                    SL.fold_mismatches += fold_bad ? 1 : 0;
+                    R.fold_mismatches += fold_bad ? 1 : 0;
+                    if (x.smid < fold_sm) {
+                        fold_sm = x.smid;
+                        R.fold_xor = x.fold_x;
+                        R.fold_sum = x.fold_s;
+                        R.fold_wsum = x.fold_w;
+                    }
+                }
+                if (t1 > t0) R.timer_ns += t1 - t0;
+                *covered = R.sms_covered = (uint32_t)seen.size();
+                return CRO_OK;
+            };
+            const int e = coverage_rounds(c, d, ev, cta, cta_bytes, (uint32_t)sm_count, max_rounds, &R.rounds, &R.ns, launch, fetch, take);
+            if (e) return e;
+            R.complete = R.sms_covered >= (uint32_t)sm_count ? 1u : 0u;
+            unsigned long long n_claims = 0;
+            CU_TRY(c, cudaMemcpy(&n_claims, a.claims, sizeof n_claims, cudaMemcpyDeviceToHost));
+            R.recorded = std::min<uint64_t>(n_claims, CRO_SRAM_RECORDS);
+            recs[leg].resize((size_t)R.recorded);
+            if (R.recorded) CU_TRY(c, cudaMemcpy(recs[leg].data(), a.rec, recs[leg].size() * sizeof(SramRecord), cudaMemcpyDeviceToHost));
+            for (auto& kv : per_sm) {
+                cro_sram_sm_leg& SL = kv.second.leg[leg];
+                if (!SL.ctas) continue;
+                uint64_t any = SL.fold_mismatches;
+                for (uint64_t m : SL.mismatches) any += m;
+                SL.mark = last[leg][kv.first] ? CRO_SRAM_PERSISTENT : any ? CRO_SRAM_INTERMITTENT : 0u;
+                if (SL.mark) R.failed_sms++;
+            }
+        }
+        return CRO_OK;
+    }();
+    for (cudaEvent_t x : ev)
+        if (x) cudaEventDestroy(x);
+    if (rc == CRO_ERR_CUDA) r->cuda_error = (int32_t)cudaGetLastError();
+    if (marched && nvml) identity::NvmlSramHealth(uuid, true, &r->after);
+    r->health = sram_health(r->before, r->after);
+    if (rc) {
+        blank_result(r, *r, sms, faults);
+        r->wall_ns = now_ns() - t_call;
+        return r->status = rc;
+    }
+
+    // the word records, the owner or writer resolved from the CTAs' own records of the same round
+    for (uint32_t leg = 0; leg < CRO_SRAM_LEGS; ++leg)
+        for (const SramRecord& q : recs[leg]) {
+            cro_sram_fault f{};
+            f.leg = leg;
+            f.element = q.element;
+            f.iteration = q.iteration;
+            f.smid = q.smid;
+            f.word = q.word;
+            f.expected = q.expected;
+            f.actual = q.actual;
+            if (leg == CRO_SRAM_SMEM) {
+                f.peer_smid = q.smid;
+                f.direction = CRO_SRAM_DIR_LOCAL;
+            } else {
+                f.direction = q.element == 1 ? CRO_SRAM_DIR_READ : CRO_SRAM_DIR_WRITE;
+                f.peer_smid = q.round < block_smid.size() && q.peer_block < block_smid[q.round].size() ? block_smid[q.round][q.peer_block] : ~0u;
+            }
+            faults->push_back(f);
+        }
+    std::sort(faults->begin(), faults->end(), [](const cro_sram_fault& x, const cro_sram_fault& y) {
+        return std::make_tuple(x.leg, x.element, x.smid, x.iteration, x.word) < std::make_tuple(y.leg, y.element, y.smid, y.iteration, y.word);
+    });
+
+    // verdict: SMs that failed the local leg, then network pairs between SMs that passed it
+    std::set<uint32_t> local_bad;
+    for (auto& kv : per_sm) {
+        if (kv.second.leg[CRO_SRAM_SMEM].mark) local_bad.insert(kv.first);
+        sms->push_back(kv.second);
+    }
+    std::set<std::tuple<uint32_t, uint32_t, uint32_t>> pairs;      // (direction, from, owner)
+    for (const cro_sram_fault& f : *faults) {
+        if (f.leg != CRO_SRAM_DSMEM || local_bad.count(f.smid) || local_bad.count(f.peer_smid)) continue;
+        if (f.direction == CRO_SRAM_DIR_READ) pairs.insert({f.direction, f.smid, f.peer_smid});
+        else pairs.insert({f.direction, f.peer_smid, f.smid});
+    }
+    bool all = false, any = false;
+    for (uint32_t leg = 0; leg < CRO_SRAM_LEGS; ++leg) {
+        const cro_sram_leg& R = r->leg[leg];
+        if (!(r->legs >> leg & 1u)) continue;
+        if (R.unpublished || (R.failed_sms && R.failed_sms == R.sms_covered)) all = true;
+        if (R.unpublished || R.failed_sms) any = true;
+    }
+    for (uint32_t s : local_bad) {
+        if (r->bad_sms < 16) r->bad_sm[r->bad_sms] = (uint16_t)s;
+        r->bad_sms++;
+    }
+    for (const auto& p : pairs) {
+        if (r->bad_pairs < CRO_SRAM_MAX_PAIRS)
+            r->bad_pair[r->bad_pairs] = cro_sram_pair{(uint16_t)std::get<1>(p), (uint16_t)std::get<2>(p), std::get<0>(p)};
+        r->bad_pairs++;
+    }
+    r->verdict = all ? CRO_SRAM_ALL : !local_bad.empty() ? CRO_SRAM_SM : any ? CRO_SRAM_LINK : CRO_SRAM_NONE;
+    r->wall_ns = now_ns() - t_call;
+    return r->status = any ? CRO_ERR_CHECKSUM : CRO_OK;
+}
+
+namespace {
+uint64_t sram_tail_count(const unsigned char* head) {
+    return reinterpret_cast<const cro_sram_result*>(head)->recorded;
+}
+}  // namespace
+
+int ctx_probe_sram_uuid(cro_ctx* c, const char* uuid, const cro_sram_opts& o, cro_sram_result* r, std::vector<cro_sram_sm>* sms,
+                        std::vector<cro_sram_fault>* faults, int cap) {
+    const uint64_t t_call = now_ns();
+    blank_result(r, cro_sram_result{}, sms, faults);
+    if (!uuid) return r->status = CRO_ERR_INVALID_ARG;
+    const std::string want = uuid;
+    env::Values knobs;                        // no context: this caller's environment, defaults where it is illegal
+    if (c) knobs = c->knobs;
+    else env::read(&knobs, nullptr);
+    const int deadline = o.deadline_ms > 0 ? o.deadline_ms : (int)knobs.get("CRO_HELPER_TIMEOUT_MS");
+    DeviceGuard g;
+    if (c) {
+        cro_dev_info hit{};
+        int rc = find_on_node(c, want, &hit);
+        if (rc) return r->status = rc;
+        if (hit.flags & CRO_DEV_IN_PROCESS) {     // no probe of this GPU runs beside the helper
+            g = enter_device(c, hit.dev_index);
+            if (g.rc) return r->status = g.rc;
+        }
+    }
+    auto num = [](int64_t v) { return std::to_string(v); };
+    const std::vector<std::string> args = {"sram-raw", want, num(o.legs), num(o.iterations), num(o.cluster), num(o.max_rounds),
+                                           num(o.test_inject_leg), num(o.test_inject_sm), num(o.test_inject_element),
+                                           num(o.test_inject_iteration), num(o.test_inject_word), std::to_string(o.test_inject_mask),
+                                           num(cap)};
+    const size_t head = sizeof *r + CRO_SRAM_MAX_SMS * sizeof(cro_sram_sm);
+    std::string got, err;
+    if (c && c->nvtx) nvtxRangePushA("cro.probe_sram.helper");
+    int rc = inventory::RunHelperRaw("", "SRAM helper", want, args, deadline, head, sizeof(cro_sram_fault), (size_t)cap,
+                                     sram_tail_count, &got, &err);
+    if (c && c->nvtx) nvtxRangePop();
+    const uint64_t helper_ns = now_ns() - t_call;
+    if (rc == CRO_OK) {
+        memcpy(r, got.data(), sizeof *r);
+        const cro_sram_sm* s = reinterpret_cast<const cro_sram_sm*>(got.data() + sizeof *r);
+        sms->assign(s, s + std::min<uint32_t>(r->sms_listed, CRO_SRAM_MAX_SMS));
+        const cro_sram_fault* f = reinterpret_cast<const cro_sram_fault*>(got.data() + head);
+        faults->assign(f, f + r->recorded);
+        r->helper_ns = helper_ns;
+        rc = r->status;
+        if (rc != CRO_OK && rc != CRO_ERR_CHECKSUM) err = "SRAM helper for " + want + ": " + cro_strerror(rc);
+    } else {
+        r->status = rc;
+    }
+    if (rc != CRO_OK && !err.empty()) {
+        if (c) c->set_error(err);
+        else set_thread_error(err);
+    }
+    return rc;
+}
+
+}  // namespace cro

@@ -512,6 +512,112 @@ func (c *Context) ScanHBM(deviceID string, maxBytes uint64) (ScanResult, error) 
 	return scanResult(rep, words[:], got), nil
 }
 
+// SRAMResult is the summary of cro_sram_result an operator reads: whether every
+// SM's shared memory and the SM-to-SM network held what was written, which SMs
+// or pairs did not, and the SRAM ECC record from NVML.
+type SRAMResult struct {
+	Status      int32     // CRO_OK, CRO_ERR_CHECKSUM or CRO_ERR_CUDA
+	CudaError   int32     // cudaError_t of a failed launch (CRO_ERR_CUDA)
+	Verdict     uint32    // CRO_SRAM_NONE / _SM / _LINK / _ALL
+	Health      uint32    // CRO_SRAM_HEALTH_* bits; never change Status
+	SMCount     uint32
+	Covered     [2]uint32 // SMs seen per leg: CRO_SRAM_SMEM, CRO_SRAM_DSMEM
+	BytesPerSM  uint64
+	BadSMs      []uint32   // SMs that failed the local leg, ascending (at most 16)
+	BadPairs    []SRAMPair // network pairs whose SMs both passed the local leg (at most 8)
+	Faults      []SRAMFault
+	Annotations string // Go-marshalled map[string]string of cohdi.io/probe-sram-* keys
+}
+
+// SRAMPair is a failed network pair: From read (Direction CRO_SRAM_DIR_READ)
+// or wrote (CRO_SRAM_DIR_WRITE) Owner's shared memory.
+type SRAMPair struct {
+	From, Owner, Direction uint32
+}
+
+// SRAMFault is one failed compare (cro_sram_fault).
+type SRAMFault struct {
+	Leg, Element, Iteration, SM, PeerSM, Direction, Word uint32
+	Expected, Actual                                     uint64
+}
+
+func sramResult(res *C.cro_sram_result, faults []C.cro_sram_fault, got C.int) SRAMResult {
+	out := SRAMResult{Status: int32(res.status), CudaError: int32(res.cuda_error), Verdict: uint32(res.verdict),
+		Health: uint32(res.health), SMCount: uint32(res.sm_count), BytesPerSM: uint64(res.bytes_per_sm)}
+	for l := 0; l < 2; l++ {
+		out.Covered[l] = uint32(res.leg[l].sms_covered)
+	}
+	for i := 0; i < int(res.bad_sms) && i < 16; i++ {
+		out.BadSMs = append(out.BadSMs, uint32(res.bad_sm[i]))
+	}
+	for i := 0; i < int(res.bad_pairs) && i < int(C.CRO_SRAM_MAX_PAIRS); i++ {
+		p := res.bad_pair[i]
+		out.BadPairs = append(out.BadPairs, SRAMPair{uint32(p.from), uint32(p.owner), uint32(p.direction)})
+	}
+	for i := 0; i < int(got); i++ {
+		f := faults[i]
+		out.Faults = append(out.Faults, SRAMFault{uint32(f.leg), uint32(f.element), uint32(f.iteration), uint32(f.smid),
+			uint32(f.peer_smid), uint32(f.direction), uint32(f.word), uint64(f.expected), uint64(f.actual)})
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_sram_annotations_json(res, buf, 4096, &ln) == C.CRO_OK {
+		out.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return out
+}
+
+// ProbeSRAMByUUID runs cro_probe_sram_uuid with its defaults: the SRAM probe of
+// any GPU on the node through the helper process, the form to call on a freshly
+// composed GPU (INTEGRATION.md "The SRAM probe").  A mismatch or a fault
+// (CRO_ERR_CUDA) is a result, not an error; found is false when the node does
+// not list the GPU.
+func (c *Context) ProbeSRAMByUUID(deviceID string) (r SRAMResult, found bool, err error) {
+	id := C.CString(deviceID)
+	defer C.free(unsafe.Pointer(id))
+	var res C.cro_sram_result
+	sms := make([]C.cro_sram_sm, C.CRO_SRAM_MAX_SMS)
+	var faults [256]C.cro_sram_fault
+	var nSMs, got C.int
+	rc := C.cro_probe_sram_uuid(c.h, id, nil, &res, &sms[0], C.CRO_SRAM_MAX_SMS, &nSMs, &faults[0], 256, &got)
+	if rc == C.CRO_ERR_NO_DEVICE {
+		return r, false, nil
+	}
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM && rc != C.CRO_ERR_CUDA {
+		return r, true, errorOf(c.h, rc)
+	}
+	return sramResult(&res, faults[:], got), true, nil
+}
+
+// ProbeSRAM runs cro_probe_sram with its defaults on the in-process device whose
+// UUID is deviceID.  ProbeSRAMByUUID is the form an operator should call.
+func (c *Context) ProbeSRAM(deviceID string) (SRAMResult, error) {
+	var devs [C.CRO_MAX_DEVICES]C.cro_dev_info
+	var n C.int
+	if rc := C.cro_enumerate(c.h, &devs[0], C.CRO_MAX_DEVICES, &n); rc != C.CRO_OK {
+		return SRAMResult{}, errorOf(c.h, rc)
+	}
+	idx := C.int(-1)
+	for i := 0; i < int(n); i++ {
+		if C.GoString(&devs[i].gpu_uuid[0]) == deviceID && devs[i].flags&C.CRO_DEV_IN_PROCESS != 0 {
+			idx = C.int(devs[i].dev_index)
+		}
+	}
+	if idx < 0 {
+		return SRAMResult{}, fmt.Errorf("cuda sram probe: %s is not a device of this context", deviceID)
+	}
+	var res C.cro_sram_result
+	sms := make([]C.cro_sram_sm, C.CRO_SRAM_MAX_SMS)
+	var faults [256]C.cro_sram_fault
+	var nSMs, got C.int
+	rc := C.cro_probe_sram(c.h, idx, nil, &res, &sms[0], C.CRO_SRAM_MAX_SMS, &nSMs, &faults[0], 256, &got)
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM && rc != C.CRO_ERR_CUDA {
+		return SRAMResult{}, errorOf(c.h, rc)
+	}
+	return sramResult(&res, faults[:], got), nil
+}
+
 // MetricsText is the Prometheus text exposition of the context's counters and
 // per-GPU gauges; a prometheus.Collector registered with
 // sigs.k8s.io/controller-runtime/pkg/metrics.Registry (cmd/main.go:66,119-125

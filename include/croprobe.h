@@ -937,6 +937,204 @@ int  cro_scan_hbm_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_scan_opts *
  * CRO_OK whatever NVML answered (out->nvml says which reads it did); CRO_ERR_INVALID_ARG for a NULL argument. */
 int  cro_read_hbm_health(const char *gpu_uuid, cro_hbm_health *out);
 
+/* ---- SRAM: every SM's shared memory and the SM-to-SM network, and the SRAM ECC record ---- */
+
+/*
+ * The probe, the scan and the compute probe keep operands in shared memory, but only as pseudo-random bytes: a bad cell
+ * shows as a wrong fold or a wrong tile, and the compute probe cannot tell a bad SM's arithmetic from its memory.  The
+ * SRAM probe writes every shared-memory word it can reach as 0 and as 1, reads it back and names the SM it belongs to.
+ *
+ * Local leg (CRO_SRAM_SMEM): one CTA per SM with the device's opt-in maximum of dynamic shared memory (bytes_per_sm,
+ * 64-bit words w = 0 .. n - 1; thread t of T owns words t, t + T, ...).  Each iteration runs March C- with P(w) =
+ * pattern_word(seed, w) and Q(w) = ~P(w):
+ *   M0 write P;  M1 ascending: read P, write Q;  M2 ascending: read Q, write P;
+ *   M3 descending: read P, write Q;  M4 descending: read Q, write P;  M5 read P
+ * with a CTA barrier between elements.  The order holds per word and per thread; between words of different threads
+ * it is not enforced.  Every read is compared (mismatches counted exactly per element, recorded while there is room);
+ * M5's reads are also folded (xor, sum, sum of v * (2w + 1), over every iteration: xor of the iterations' folds, sums
+ * summed) and the library compares each CTA's fold with the closed form.
+ *
+ * Network leg (CRO_SRAM_DSMEM): clusters of `cluster` CTAs (2, 4 or 8), as many as the device places at once, each CTA
+ * with the local leg's shared memory.  The CTA of cluster rank r owns P_r(w) = pattern_word(seed + r * 0xD1B54A32D192ED03,
+ * w), so a word read from the wrong peer mismatches.  Each iteration:
+ *   D0 write P_r locally;  D1 read every peer's words over the network (mapa + ld.shared::cluster) against its P;
+ *   D2 write Q of peer (r + 1) mod C into that peer (st.shared::cluster);  D3 read the own words locally against Q_r
+ * with a cluster barrier between elements.  A D1 mismatch is a remote-read fault of (reader, owner); a D3 mismatch a
+ * remote-write fault of (writer, owner).  Whether the network path carries ECC or parity is not documented: the
+ * compare is end to end either way.
+ *
+ * Seeds: call k on a device uses seed = seed_dev + 2^60 + 8 * k * 0xD1B54A32D192ED03 (rank r adds r times the
+ * stride), so no call passes on what an earlier call left in shared memory.  Each leg is relaunched while fewer than
+ * sm_count SMs took part, up to max_rounds launches; short coverage is reported (complete = 0), never an error.  It
+ * runs only when called: it takes the device's mutex, lets probes in flight finish first (their results stay
+ * collectable) and never touches the sweep region.
+ *
+ * status: CRO_ERR_CHECKSUM on any mismatch, fold mismatch or CTA that did not publish; CRO_ERR_CUDA when a launch
+ * failed (cuda_error holds the cudaError_t, e.g. 214 for an uncorrectable ECC error); CRO_ERR_UNSUPPORTED when the
+ * device cannot place one cluster of the asked size.  The NVML SRAM health read before the first leg and after the
+ * last never changes the status.
+ */
+#define CRO_SRAM_SMEM             0       /* leg index: the local march                                     */
+#define CRO_SRAM_DSMEM            1       /* leg index: the SM-to-SM network                                */
+#define CRO_SRAM_LEGS             2
+#define CRO_SRAM_LEG_SMEM         0x1u    /* cro_sram_opts.legs bits                                        */
+#define CRO_SRAM_LEG_DSMEM        0x2u
+#define CRO_SRAM_ALL_LEGS         0x3u
+#define CRO_SRAM_ELEMENTS         6       /* per-element counts: M0 .. M5 (local), D0 .. D3 (network)       */
+#define CRO_SRAM_RECORDS          4096    /* word records the device keeps per leg; counts stay exact beyond */
+#define CRO_SRAM_MAX_SMS          256     /* SM ids the results hold; a larger %nsmid fails the call         */
+#define CRO_SRAM_MAX_ITERATIONS   4096
+#define CRO_SRAM_MAX_ROUNDS       64
+#define CRO_SRAM_MAX_PAIRS        8       /* network pairs listed in the result                             */
+
+#define CRO_SRAM_NONE             0u      /* nothing failed                                                  */
+#define CRO_SRAM_SM               1u      /* a strict subset of the covered SMs failed the local leg          */
+#define CRO_SRAM_LINK             2u      /* network faults between SMs that both passed the local leg        */
+#define CRO_SRAM_ALL              3u      /* every covered SM failed a leg, or a launched CTA did not publish  */
+
+#define CRO_SRAM_PERSISTENT       1u      /* cro_sram_sm_leg.mark: the last iteration's compare failed         */
+#define CRO_SRAM_INTERMITTENT     2u      /* an earlier iteration failed, or only the fold did                 */
+
+#define CRO_SRAM_DIR_LOCAL        0u      /* cro_sram_fault.direction */
+#define CRO_SRAM_DIR_READ         1u      /* D1: smid read peer_smid's words */
+#define CRO_SRAM_DIR_WRITE        2u      /* D3: peer_smid wrote smid's words */
+
+/* cro_sram_result.health: reported, never changes the status */
+#define CRO_SRAM_HEALTH_CORRECTED_DURING    0x1u   /* the volatile SRAM corrected count rose during the call       */
+#define CRO_SRAM_HEALTH_UNCORRECTED_DURING  0x2u   /* the volatile SRAM uncorrected count rose during the call     */
+#define CRO_SRAM_HEALTH_THRESHOLD_EXCEEDED  0x4u   /* NVML's SRAM error status: the field-diag threshold is exceeded */
+
+/* cro_sram_health.nvml: which reads NVML answered (a field NVML refused stays 0) */
+#define CRO_SRAM_NVML_ECC_CORRECTED    0x1u   /* nvmlDeviceGetMemoryErrorCounter, corrected, volatile, SRAM       */
+#define CRO_SRAM_NVML_ECC_UNCORRECTED  0x2u   /* ... uncorrected                                                  */
+#define CRO_SRAM_NVML_STATUS           0x4u   /* nvmlDeviceGetSramEccErrorStatus (absent from older drivers)       */
+
+typedef struct cro_sram_opts {
+    uint32_t legs;                 /*   0  CRO_SRAM_LEG_* bits; 0 = both                                          */
+    uint32_t iterations;           /*   4  per CTA, both legs: 0 = the default (DESIGN.md), at most MAX_ITERATIONS */
+    uint32_t cluster;              /*   8  network leg: CTAs per cluster, 2, 4 or 8; 0 = 2                        */
+    uint32_t max_rounds;           /*  12  launches per leg while fewer than sm_count SMs took part: 0 = 4         */
+    int32_t  deadline_ms;          /*  16  cro_probe_sram_uuid: the helper's deadline; 0 = CRO_HELPER_TIMEOUT_MS   */
+    /* test only: with test_inject_mask != 0, in each CTA of leg test_inject_leg (CRO_SRAM_SMEM / _DSMEM) whose %smid
+       is test_inject_sm (-1: every SM), the mask is XORed into the word test_inject_word (-1: every word) of element
+       test_inject_element in iteration test_inject_iteration: local leg, elements 1 .. 5, into the value read before
+       the compare; network leg, element 1 into the value D1 read, element 2 into the value D2 writes.  A software
+       stand-in for a bad cell: nothing is provoked in the hardware. */
+    int32_t  test_inject_leg;      /*  20 */
+    int32_t  test_inject_sm;       /*  24 */
+    uint32_t test_inject_element;  /*  28 */
+    uint32_t test_inject_iteration;/*  32 */
+    int32_t  test_inject_word;     /*  36 */
+    uint64_t test_inject_mask;     /*  40 */
+} cro_sram_opts;                   /*  48 bytes */
+
+typedef struct cro_sram_health {
+    uint32_t nvml;                 /*   0  CRO_SRAM_NVML_* of the reads NVML answered                              */
+    uint32_t threshold_exceeded;   /*   4  nvmlEccSramErrorStatus_t.bThresholdExceeded (after the last leg only)   */
+    uint64_t ecc_corrected;        /*   8  volatile SRAM ECC counts                                               */
+    uint64_t ecc_uncorrected;      /*  16 */
+} cro_sram_health;                 /*  24 bytes */
+
+typedef struct cro_sram_pair {
+    uint16_t from;                 /*   0  the reader (CRO_SRAM_DIR_READ) or the writer (CRO_SRAM_DIR_WRITE)       */
+    uint16_t owner;                /*   2  the SM whose shared memory holds the words                             */
+    uint32_t direction;            /*   4  CRO_SRAM_DIR_READ / _WRITE                                            */
+} cro_sram_pair;                   /*   8 bytes */
+
+typedef struct cro_sram_leg {
+    uint32_t iterations;           /*   0  per CTA                                                               */
+    uint32_t rounds;               /*   4  launches                                                              */
+    uint64_t bytes;                /*   8  shared-memory bytes read and written by the CTAs launched (reads over the
+                                              network included)                                                 */
+    uint64_t ns;                   /*  16  CUDA events around the launches, summed over rounds                  */
+    uint64_t timer_ns;             /*  24  %globaltimer: first CTA start .. last CTA end, summed over rounds     */
+    uint32_t sms_covered;          /*  32  distinct SMs that ran a CTA of the leg (network: took part in a cluster) */
+    uint32_t complete;             /*  36  1: sms_covered == sm_count                                            */
+    uint64_t mismatches[CRO_SRAM_ELEMENTS];   /*  40  per element, exact (local M1 .. M5; network D1, D3)         */
+    uint64_t fold_mismatches;      /*  88  local: CTAs whose M5 fold differs from the closed form               */
+    uint64_t recorded;             /*  96  mismatches the device recorded (<= CRO_SRAM_RECORDS)                  */
+    uint32_t failed_sms;           /* 104  distinct SMs with a mark                                             */
+    uint32_t unpublished;          /* 108  CTAs launched that published no record                              */
+    uint32_t ctas;                 /* 112  CTAs launched, over all rounds                                       */
+    uint32_t cluster;              /* 116  network: CTAs per cluster; 0 for the local leg                      */
+    uint64_t fold_xor;             /* 120  local: M5 fold of the CTA on the lowest SM id                         */
+    uint64_t fold_sum;             /* 128 */
+    uint64_t fold_wsum;            /* 136 */
+    uint64_t expect_xor;           /* 144  local: the closed form every CTA's fold must equal                    */
+    uint64_t expect_sum;           /* 152 */
+    uint64_t expect_wsum;          /* 160 */
+} cro_sram_leg;                    /* 168 bytes */
+
+typedef struct cro_sram_result {
+    int32_t  status;               /*   0  the return value                                                      */
+    uint32_t verdict;              /*   4  CRO_SRAM_NONE / _SM / _LINK / _ALL                                     */
+    uint64_t seed;                 /*   8  seed of this call (rank 0's)                                          */
+    uint64_t call;                 /*  16  k: the call's number on this device, from 0                          */
+    uint32_t sm_count;             /*  24  multiprocessors the device reports                                    */
+    uint32_t legs;                 /*  28  legs run (CRO_SRAM_LEG_* bits)                                        */
+    uint32_t nsmid;                /*  32  %nsmid as the kernels read it                                        */
+    int32_t  cuda_error;           /*  36  cudaError_t of the launch that failed; 0: none                        */
+    uint64_t bytes_per_sm;         /*  40  shared-memory bytes each CTA marches                                  */
+    uint32_t health;               /*  48  CRO_SRAM_HEALTH_*                                                    */
+    uint32_t bad_sms;              /*  52  distinct SMs that failed the local leg                                */
+    uint16_t bad_sm[16];           /*  56  the first 16 of them, ascending                                      */
+    uint32_t bad_pairs;            /*  88  distinct network pairs recorded whose SMs both passed the local leg   */
+    uint32_t sms_listed;           /*  92  entries written to the caller's per-SM list                          */
+    cro_sram_pair bad_pair[CRO_SRAM_MAX_PAIRS];   /*  96  the first of them, by (direction, from, owner)          */
+    uint64_t recorded;             /* 160  word records written to the caller's list (*n)                       */
+    uint64_t wall_ns;              /* 168  the whole call                                                       */
+    uint64_t helper_ns;            /* 176  cro_probe_sram_uuid: spawn of the helper to its exit; 0 in process   */
+    cro_sram_health before;        /* 184  read before the first leg                                            */
+    cro_sram_health after;         /* 208  read after the last leg (with the threshold flag)                    */
+    cro_sram_leg leg[CRO_SRAM_LEGS];         /* 232 */
+} cro_sram_result;                 /* 568 bytes */
+
+typedef struct cro_sram_sm_leg {
+    uint64_t mismatches[CRO_SRAM_ELEMENTS];   /*   0  compares of this SM's CTAs that failed, per element          */
+    uint64_t fold_mismatches;      /*  48 */
+    uint64_t ns;                   /*  56  %globaltimer windows of the leg's CTAs on this SM, summed            */
+    uint64_t cycles;               /*  64  %clock64 cycles of the same CTAs, summed                             */
+    uint32_t ctas;                 /*  72  CTAs of the leg that ran on this SM (0: not seen in this leg)        */
+    uint32_t mark;                 /*  76  0, CRO_SRAM_PERSISTENT or CRO_SRAM_INTERMITTENT                      */
+} cro_sram_sm_leg;                 /*  80 bytes */
+
+typedef struct cro_sram_sm {
+    uint32_t smid;                 /*   0 */
+    uint32_t reserved;             /*   4 */
+    cro_sram_sm_leg leg[CRO_SRAM_LEGS];      /*   8 */
+} cro_sram_sm;                     /* 168 bytes */
+
+typedef struct cro_sram_fault {
+    uint32_t leg;                  /*   0  CRO_SRAM_SMEM / _DSMEM                                               */
+    uint32_t element;              /*   4  local 1 .. 5 (M1 .. M5); network 1 (D1) or 3 (D3)                     */
+    uint32_t iteration;            /*   8 */
+    uint32_t smid;                 /*  12  the SM whose compare failed: the local SM, the D1 reader, the D3 owner  */
+    uint32_t peer_smid;            /*  16  network: the D1 owner or the D3 writer (from the CTAs' own records);
+                                              local: smid                                                      */
+    uint32_t direction;            /*  20  CRO_SRAM_DIR_*                                                       */
+    uint32_t word;                 /*  24  word offset in the owner's shared memory                             */
+    uint32_t reserved;             /*  28 */
+    uint64_t expected;             /*  32 */
+    uint64_t actual;               /*  40 */
+} cro_sram_fault;                  /*  48 bytes */
+
+/* sms[0 .. sms_cap) receives one entry per SM seen, by SM id (*n_sms how many); faults[0 .. cap) the word records
+ * sorted by (leg, element, smid, iteration, word) (*n how many).  opts may be NULL: defaults.  cro_probe_sram:
+ * dev_index is an in-process device.  cro_probe_sram_uuid runs `croprobe-cli sram-raw` (a fresh cuInit that sees only
+ * that GPU): it reaches GPUs attached after cro_probe_init, and an uncorrectable SRAM error, which takes down the CUDA
+ * context that hit it, costs the helper, not the caller's context (INTEGRATION.md "The SRAM probe").  ctx may be NULL;
+ * a UUID the node does not list is CRO_ERR_NO_DEVICE; a GPU that is also an in-process device of ctx is held under
+ * that device's mutex while the helper runs. */
+int  cro_probe_sram(cro_ctx *ctx, int dev_index, const cro_sram_opts *opts, cro_sram_result *out,
+                    cro_sram_sm *sms, int sms_cap, int *n_sms, cro_sram_fault *faults, int cap, int *n);
+int  cro_probe_sram_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_sram_opts *opts, cro_sram_result *out,
+                         cro_sram_sm *sms, int sms_cap, int *n_sms, cro_sram_fault *faults, int cap, int *n);
+
+/* The device's SRAM health record from NVML, as the probe reads it after the last leg (with the threshold flag): no
+ * context, no CUDA.  CRO_OK whatever NVML answered (out->nvml says which reads it did); CRO_ERR_INVALID_ARG for a
+ * NULL argument. */
+int  cro_read_sram_health(const char *gpu_uuid, cro_sram_health *out);
+
 /* ---- emit: encoding/json-compatible writers ------------------------------ */
 
 /* ComposableResourceStatus (api/v1alpha1/composableresource_types.go:36-41):
@@ -1006,6 +1204,16 @@ int  cro_emit_compute_annotations_json(const cro_compute_result *r, char *buf, s
  * before, when both reads answered), -remapped ("<corrected>,<uncorrected>" rows after E3) and -remap-histogram ("max,
  * high, partial, low, none" without spaces). */
 int  cro_emit_scan_annotations_json(const cro_scan_report *r, char *buf, size_t cap, size_t *len);
+
+/* Additive SRAM annotations (cohdi.io/probe-sram-*) of a cro_probe_sram / cro_probe_sram_uuid result, the same
+ * Go-marshalled map, integers and fixed spellings only: -verdict ("ok" for CRO_OK; "sm", "link" or "all" for
+ * CRO_ERR_CHECKSUM with that verdict; "cuda-error:<cuda_error>" for CRO_ERR_CUDA; "error" otherwise), -sms
+ * ("<covered>/<sm_count>", the least sms_covered over the legs run), -bad-sms (bad_sm[0 .. min(bad_sms, 16)),
+ * comma-separated; only when bad_sms > 0), -bad-pairs (bad_pair[0 .. min(bad_pairs, 8)) as "<from>-<owner>:<r|w>",
+ * comma-separated; only when bad_pairs > 0), -bytes-per-sm, -health (the flags' names corrected, uncorrected,
+ * threshold-exceeded, comma-separated; only when any is set), and -ecc-corrected and -ecc-uncorrected (the deltas,
+ * after - before; only when both reads answered). */
+int  cro_emit_sram_annotations_json(const cro_sram_result *r, char *buf, size_t cap, size_t *len);
 
 /* (deviceID, CDIDeviceID) from an FM ScaleUpResponse body, with the
  * res_op_status gate of internal/cdi/fti/fm/client.go:184-213.  On the error
