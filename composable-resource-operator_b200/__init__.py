@@ -495,8 +495,8 @@ EXPORTS = [
     "cro_chase_end", "cro_validate_env", "cro_node_inventory", "cro_probe_uuid", "cro_set_latency_hops", "cro_local_exec", "cro_metrics_text", "cro_describe_wire_type",
     "cro_selftest_probe_finalize", "cro_selftest_p2p_finalize", "cro_selftest_chase", "cro_selftest_sweep",
     "cro_locate_faults", "cro_emit_fault_annotations_json",
-    "cro_probe_host_link", "cro_pci_link_path", "cro_emit_link_annotations_json",
-    "cro_probe_compute", "cro_compute_expected", "cro_emit_compute_annotations_json",
+    "cro_probe_host_link", "cro_probe_host_link_uuid", "cro_pci_link_path", "cro_emit_link_annotations_json",
+    "cro_probe_compute", "cro_probe_compute_uuid", "cro_compute_expected", "cro_emit_compute_annotations_json",
     "cro_scan_hbm", "cro_scan_hbm_uuid", "cro_read_hbm_health", "cro_emit_scan_annotations_json",
     "cro_probe_sram", "cro_probe_sram_uuid", "cro_read_sram_health", "cro_emit_sram_annotations_json",
 ]
@@ -592,11 +592,16 @@ def _load() -> ctypes.CDLL:
         "cro_emit_fault_annotations_json": (i32, [ctypes.POINTER(FaultReport), ctypes.POINTER(FaultWord), i32] + out),
         "cro_probe_host_link": (i32, [vp, i32, ctypes.POINTER(LinkOpts), ctypes.POINTER(LinkResult), ctypes.POINTER(LinkFault),
                                       i32, ctypes.POINTER(i32)]),
+        "cro_probe_host_link_uuid": (i32, [vp, c, ctypes.POINTER(LinkOpts), i32, ctypes.POINTER(LinkResult),
+                                           ctypes.POINTER(LinkFault), i32, ctypes.POINTER(i32), ctypes.POINTER(u64)]),
         "cro_pci_link_path": (i32, [c, c, ctypes.POINTER(PciPath)]),
         "cro_emit_link_annotations_json": (i32, [ctypes.POINTER(LinkResult)] + out),
         "cro_probe_compute": (i32, [vp, i32, ctypes.POINTER(ComputeOpts), ctypes.POINTER(ComputeResult),
                                     ctypes.POINTER(ComputeSm), i32, ctypes.POINTER(i32), ctypes.POINTER(ComputeFault), i32,
                                     ctypes.POINTER(i32)]),
+        "cro_probe_compute_uuid": (i32, [vp, c, ctypes.POINTER(ComputeOpts), i32, ctypes.POINTER(ComputeResult),
+                                         ctypes.POINTER(ComputeSm), i32, ctypes.POINTER(i32), ctypes.POINTER(ComputeFault), i32,
+                                         ctypes.POINTER(i32), ctypes.POINTER(u64)]),
         "cro_compute_expected": (i32, [i32, u64, ctypes.POINTER(ctypes.c_int32)]),
         "cro_emit_compute_annotations_json": (i32, [ctypes.POINTER(ComputeResult)] + out),
         "cro_scan_hbm": (i32, [vp, i32, ctypes.POINTER(ScanOpts), ctypes.POINTER(ScanReport), ctypes.POINTER(FaultWord), i32,
@@ -807,6 +812,68 @@ def probe_sram_uuid(ctx: Optional["ProbeContext"], uuid: str, legs: int = SRAM_A
         lib.cro_last_error(handle, buf, 1024)
         raise ProbeError(rc, buf.value.decode("utf-8", "replace"))
     return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
+
+
+def _helper_error(rc: int, handle) -> "ProbeError":
+    buf = ctypes.create_string_buffer(1024)
+    lib.cro_last_error(handle, buf, 1024)
+    return ProbeError(rc, buf.value.decode("utf-8", "replace"))
+
+
+def _link_opts(bytes: int, hops: int, ctas: int, inject: Optional[Tuple[int, int, int]]) -> LinkOpts:
+    o = LinkOpts()
+    o.bytes, o.hops, o.ctas = bytes, hops, ctas
+    if inject is not None:
+        o.test_inject_check, o.test_inject_word, o.test_inject_mask = inject
+    return o
+
+
+def probe_host_link_uuid(ctx: Optional["ProbeContext"], uuid: str, bytes: int = 0, hops: int = 0, ctas: int = 0,
+                         deadline_ms: int = 0, inject: Optional[Tuple[int, int, int]] = None,
+                         cap: int = 256) -> Tuple[LinkResult, List[LinkFault], int]:
+    """cro_probe_host_link_uuid: the host link probe of any GPU on the node, run by the helper process (ctx may be
+    None).  bytes = 0: 256 MiB (the helper's sweep region is L).  Returns the result (its status is OK, ERR_CHECKSUM or
+    ERR_CUDA), up to `cap` mismatching words and the helper's spawn-to-exit time in ns."""
+    o = _link_opts(bytes, hops, ctas, inject)
+    r = LinkResult()
+    arr = (LinkFault * max(1, cap))()
+    n, ns = ctypes.c_int(), ctypes.c_uint64()
+    handle = ctx.handle if ctx is not None else None
+    rc = lib.cro_probe_host_link_uuid(handle, _b(uuid), ctypes.byref(o), deadline_ms, ctypes.byref(r), arr, cap, ctypes.byref(n),
+                                      ctypes.byref(ns))
+    if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
+        raise _helper_error(rc, handle)
+    return r, [arr[i] for i in range(n.value)], ns.value
+
+
+def _compute_opts(iterations: int, alu_iterations: int, legs: int, max_rounds: int,
+                  inject: Optional[Tuple[int, int, int, int, int, int]]) -> ComputeOpts:
+    o = ComputeOpts()
+    o.iterations, o.alu_iterations, o.legs, o.max_rounds = iterations, alu_iterations, legs, max_rounds
+    if inject is not None:
+        (o.test_inject_leg, o.test_inject_sm, o.test_inject_iteration, o.test_inject_row, o.test_inject_col,
+         o.test_inject_mask) = inject
+    return o
+
+
+def probe_compute_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: int = 0, alu_iterations: int = 0,
+                       legs: int = COMPUTE_ALL_LEGS, max_rounds: int = 0, deadline_ms: int = 0,
+                       inject: Optional[Tuple[int, int, int, int, int, int]] = None,
+                       cap: int = 256) -> Tuple[ComputeResult, List[ComputeSm], List[ComputeFault], int]:
+    """cro_probe_compute_uuid: the compute probe of any GPU on the node, run by the helper process (ctx may be None).
+    Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen, up to `cap` element records
+    and the helper's spawn-to-exit time in ns."""
+    o = _compute_opts(iterations, alu_iterations, legs, max_rounds, inject)
+    r = ComputeResult()
+    sms = (ComputeSm * COMPUTE_MAX_SMS)()
+    arr = (ComputeFault * max(1, cap))()
+    n_sms, n, ns = ctypes.c_int(), ctypes.c_int(), ctypes.c_uint64()
+    handle = ctx.handle if ctx is not None else None
+    rc = lib.cro_probe_compute_uuid(handle, _b(uuid), ctypes.byref(o), deadline_ms, ctypes.byref(r), sms, COMPUTE_MAX_SMS,
+                                    ctypes.byref(n_sms), arr, cap, ctypes.byref(n), ctypes.byref(ns))
+    if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
+        raise _helper_error(rc, handle)
+    return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)], ns.value
 
 
 def _scan_opts(max_bytes: int, reserve_bytes: int, seed: int, deadline_ms: int, chunk_bytes: int,
@@ -1053,10 +1120,7 @@ class ProbeContext:
         link's path from sysfs.  bytes = 0: min(256 MiB, S); hops = 0: 1024; ctas = 0: the default grid of the SM
         legs.  inject = (check, word, mask) is the test-only fault.  Returns the result (its status is OK or
         ERR_CHECKSUM) and up to `cap` mismatching words."""
-        o = LinkOpts()
-        o.bytes, o.hops, o.ctas = bytes, hops, ctas
-        if inject is not None:
-            o.test_inject_check, o.test_inject_word, o.test_inject_mask = inject
+        o = _link_opts(bytes, hops, ctas, inject)
         r = LinkResult()
         arr = (LinkFault * max(1, cap))()
         n = ctypes.c_int()
@@ -1071,11 +1135,7 @@ class ProbeContext:
         (FFMA, IMAD) and checks it exactly.  iterations = 0 / alu_iterations = 0 / max_rounds = 0: the defaults.
         inject = (leg, sm, iteration, row, col, mask) is the test-only wrong answer (sm, row, col: -1 for every one).
         Returns the result (its status is OK or ERR_CHECKSUM), one entry per SM seen and up to `cap` element records."""
-        o = ComputeOpts()
-        o.iterations, o.alu_iterations, o.legs, o.max_rounds = iterations, alu_iterations, legs, max_rounds
-        if inject is not None:
-            (o.test_inject_leg, o.test_inject_sm, o.test_inject_iteration, o.test_inject_row, o.test_inject_col,
-             o.test_inject_mask) = inject
+        o = _compute_opts(iterations, alu_iterations, legs, max_rounds, inject)
         r = ComputeResult()
         sms = (ComputeSm * COMPUTE_MAX_SMS)()
         arr = (ComputeFault * max(1, cap))()

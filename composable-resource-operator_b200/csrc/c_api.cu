@@ -330,6 +330,32 @@ int cro_probe_host_link(cro_ctx* ctx, int i, const cro_link_opts* opts, cro_link
     *n = (int)k;
     return rc;
 } CRO_API_CATCH
+int cro_probe_host_link_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_link_opts* opts, int deadline_ms, cro_link_result* out,
+                             cro_link_fault* faults, int cap, int* n, uint64_t* helper_ns) try {
+    if (!gpu_uuid || !out || !n || cap < 0 || (cap > 0 && !faults)) return CRO_ERR_INVALID_ARG;
+    *n = 0;
+    if (helper_ns) *helper_ns = 0;
+    cro_link_opts o{};
+    if (opts) o = *opts;
+    std::vector<cro_link_fault> found;
+    uint64_t ns = 0;
+    const int rc = ctx_probe_host_link_uuid(ctx, gpu_uuid, o, deadline_ms, out, &found, cap, &ns);
+    const size_t k = std::min(found.size(), (size_t)cap);
+    for (size_t j = 0; j < k; ++j) faults[j] = found[j];
+    *n = (int)k;
+    if (helper_ns) *helper_ns = ns;
+    return rc;
+} CRO_API_CATCH
+// The compute probe's two forms share the copy-out: sms[0 .. sms_cap) and faults[0 .. cap).
+static int compute_out(int rc, const std::vector<cro_compute_sm>& seen, const std::vector<cro_compute_fault>& found,
+                       cro_compute_sm* sms, int sms_cap, int* n_sms, cro_compute_fault* faults, int cap, int* n) {
+    const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
+    for (size_t j = 0; j < ks; ++j) sms[j] = seen[j];
+    for (size_t j = 0; j < kf; ++j) faults[j] = found[j];
+    *n_sms = (int)ks;
+    *n = (int)kf;
+    return rc;
+}
 int cro_probe_compute(cro_ctx* ctx, int i, const cro_compute_opts* opts, cro_compute_result* out, cro_compute_sm* sms,
                       int sms_cap, int* n_sms, cro_compute_fault* faults, int cap, int* n) try {
     if (!ctx || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
@@ -340,12 +366,23 @@ int cro_probe_compute(cro_ctx* ctx, int i, const cro_compute_opts* opts, cro_com
     std::vector<cro_compute_sm> seen;
     std::vector<cro_compute_fault> found;
     const int rc = ctx_probe_compute(ctx, i, o, out, &seen, &found);
-    const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
-    for (size_t j = 0; j < ks; ++j) sms[j] = seen[j];
-    for (size_t j = 0; j < kf; ++j) faults[j] = found[j];
-    *n_sms = (int)ks;
-    *n = (int)kf;
-    return rc;
+    return compute_out(rc, seen, found, sms, sms_cap, n_sms, faults, cap, n);
+} CRO_API_CATCH
+int cro_probe_compute_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_compute_opts* opts, int deadline_ms,
+                           cro_compute_result* out, cro_compute_sm* sms, int sms_cap, int* n_sms, cro_compute_fault* faults,
+                           int cap, int* n, uint64_t* helper_ns) try {
+    if (!gpu_uuid || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
+        return CRO_ERR_INVALID_ARG;
+    *n = *n_sms = 0;
+    if (helper_ns) *helper_ns = 0;
+    cro_compute_opts o{};
+    if (opts) o = *opts;
+    std::vector<cro_compute_sm> seen;
+    std::vector<cro_compute_fault> found;
+    uint64_t ns = 0;
+    const int rc = ctx_probe_compute_uuid(ctx, gpu_uuid, o, deadline_ms, out, &seen, &found, cap, &ns);
+    if (helper_ns) *helper_ns = ns;
+    return compute_out(rc, seen, found, sms, sms_cap, n_sms, faults, cap, n);
 } CRO_API_CATCH
 // The scan's two forms share the copy-out: words[0 .. cap), recorded and complete as cro_locate_faults sets them.
 static int scan_out(int rc, const std::vector<cro_fault_word>& found, cro_scan_report* out, cro_fault_word* words, int cap, int* n) {

@@ -37,6 +37,27 @@ void blank_result(cro_compute_result* r, const cro_compute_result from, std::vec
     sms->clear();
     faults->clear();
 }
+
+// Why the options are refused ("" when they pass): both forms' argument checks.
+std::string compute_opts_error(const cro_compute_opts& o) {
+    const uint32_t legs = o.legs ? o.legs : CRO_COMPUTE_ALL_LEGS;
+    const uint32_t ti = o.iterations ? o.iterations : kComputeDefaultIterations;
+    const uint32_t ai = o.alu_iterations ? o.alu_iterations : kComputeDefaultAluIterations;
+    const uint32_t iters[CRO_COMPUTE_LEGS] = {ti, ti, ti, ai, ai};
+    const uint32_t max_rounds = o.max_rounds ? o.max_rounds : kComputeDefaultRounds;
+    if ((legs & ~CRO_COMPUTE_ALL_LEGS) || iters[0] > CRO_COMPUTE_MAX_ITERATIONS || iters[3] > CRO_COMPUTE_MAX_ALU_ITERATIONS ||
+        max_rounds > CRO_COMPUTE_MAX_ROUNDS ||
+        (o.test_inject_mask &&
+         (o.test_inject_leg < 0 || o.test_inject_leg >= CRO_COMPUTE_LEGS || o.test_inject_sm < -1 ||
+          o.test_inject_sm >= CRO_COMPUTE_MAX_SMS || o.test_inject_row < -1 || o.test_inject_row >= CRO_COMPUTE_M ||
+          o.test_inject_col < -1 || o.test_inject_col >= CRO_COMPUTE_N || o.test_inject_iteration >= iters[o.test_inject_leg])))
+        return "compute probe: legs must be CRO_COMPUTE_ALL_LEGS bits, iterations at most " +
+               std::to_string(CRO_COMPUTE_MAX_ITERATIONS) + ", alu_iterations at most " +
+               std::to_string(CRO_COMPUTE_MAX_ALU_ITERATIONS) + ", max_rounds at most " +
+               std::to_string(CRO_COMPUTE_MAX_ROUNDS) + ", and an injection must name a leg, an SM id below " +
+               std::to_string(CRO_COMPUTE_MAX_SMS) + " (or -1), a row, a column (or -1) and an iteration the leg runs";
+    return "";
+}
 }  // namespace
 
 int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_compute_result* r, std::vector<cro_compute_sm>* sms,
@@ -48,21 +69,13 @@ int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_comput
     const uint32_t ti = o.iterations ? o.iterations : kComputeDefaultIterations;
     const uint32_t ai = o.alu_iterations ? o.alu_iterations : kComputeDefaultAluIterations;
     const uint32_t iters[CRO_COMPUTE_LEGS] = {ti, ti, ti, ai, ai};   // s8, bf16, e4m3 tensor legs; ffma, imad ALU legs
-    const uint32_t max_rounds = o.max_rounds ? o.max_rounds : kComputeDefaultRounds;
     const bool inj = o.test_inject_mask != 0;
-    if ((legs & ~CRO_COMPUTE_ALL_LEGS) || iters[0] > CRO_COMPUTE_MAX_ITERATIONS || iters[3] > CRO_COMPUTE_MAX_ALU_ITERATIONS ||
-        max_rounds > CRO_COMPUTE_MAX_ROUNDS ||
-        (inj && (o.test_inject_leg < 0 || o.test_inject_leg >= CRO_COMPUTE_LEGS || o.test_inject_sm < -1 ||
-                 o.test_inject_sm >= CRO_COMPUTE_MAX_SMS || o.test_inject_row < -1 || o.test_inject_row >= CRO_COMPUTE_M ||
-                 o.test_inject_col < -1 || o.test_inject_col >= CRO_COMPUTE_N ||
-                 o.test_inject_iteration >= iters[o.test_inject_leg]))) {
-        c->set_error("compute probe: legs must be CRO_COMPUTE_ALL_LEGS bits, iterations at most " +
-                     std::to_string(CRO_COMPUTE_MAX_ITERATIONS) + ", alu_iterations at most " +
-                     std::to_string(CRO_COMPUTE_MAX_ALU_ITERATIONS) + ", max_rounds at most " +
-                     std::to_string(CRO_COMPUTE_MAX_ROUNDS) + ", and an injection must name a leg, an SM id below " +
-                     std::to_string(CRO_COMPUTE_MAX_SMS) + " (or -1), a row, a column (or -1) and an iteration the leg runs");
+    const std::string why = compute_opts_error(o);
+    if (!why.empty()) {
+        c->set_error(why);
         return r->status = CRO_ERR_INVALID_ARG;
     }
+    const uint32_t max_rounds = o.max_rounds ? o.max_rounds : kComputeDefaultRounds;
     DeviceGuard g = enter_device(c, idx);
     if (g.rc) return r->status = g.rc;
     std::map<uint32_t, cro_compute_sm> per_sm;
@@ -219,6 +232,53 @@ int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_comput
     });
     r->verdict = all ? CRO_COMPUTE_ALL : any ? CRO_COMPUTE_SM : CRO_COMPUTE_NONE;
     return r->status = any ? CRO_ERR_CHECKSUM : CRO_OK;
+}
+
+namespace {
+// compute-raw's stdout: the result, the helper's own counts n_sms and n, CRO_COMPUTE_MAX_SMS per-SM entries (n_sms of
+// them filled), then n faults.  An n_sms the entries cannot hold makes the output malformed.
+constexpr size_t kComputeCounts = sizeof(cro_compute_result);
+constexpr size_t kComputeSms = kComputeCounts + 2 * sizeof(uint64_t);
+constexpr size_t kComputeHead = kComputeSms + CRO_COMPUTE_MAX_SMS * sizeof(cro_compute_sm);
+uint64_t compute_count(const unsigned char* head, int which) {
+    uint64_t v;
+    memcpy(&v, head + kComputeCounts + which * sizeof v, sizeof v);
+    return v;
+}
+uint64_t compute_tail_count(const unsigned char* head) {
+    return compute_count(head, 0) > CRO_COMPUTE_MAX_SMS ? ~0ull : compute_count(head, 1);
+}
+}  // namespace
+
+int ctx_probe_compute_uuid(cro_ctx* c, const char* uuid, const cro_compute_opts& o, int deadline_ms, cro_compute_result* r,
+                           std::vector<cro_compute_sm>* sms, std::vector<cro_compute_fault>* faults, int cap, uint64_t* helper_ns) {
+    blank_result(r, cro_compute_result{}, sms, faults);
+    *helper_ns = 0;
+    if (!uuid) return r->status = CRO_ERR_INVALID_ARG;
+    const std::string why = compute_opts_error(o);
+    if (!why.empty()) {
+        set_call_error(c, why);
+        return r->status = CRO_ERR_INVALID_ARG;
+    }
+    const std::string want = uuid;
+    auto num = [](int64_t v) { return std::to_string(v); };
+    const std::vector<std::string> args = {"compute-raw", want, std::to_string(helper_seed_base(c)), num(o.iterations),
+                                           num(o.alu_iterations), num(o.legs), num(o.max_rounds), num(o.test_inject_leg),
+                                           num(o.test_inject_sm), num(o.test_inject_iteration), num(o.test_inject_row),
+                                           num(o.test_inject_col), num(o.test_inject_mask), num(cap)};
+    std::string got;
+    int rc = run_probe_helper(c, want, "compute helper", "cro.probe_compute.helper", args, deadline_ms, kComputeHead,
+                              sizeof(cro_compute_fault), (size_t)cap, compute_tail_count, &got, helper_ns);
+    if (rc != CRO_OK) return r->status = rc;
+    const unsigned char* head = reinterpret_cast<const unsigned char*>(got.data());
+    memcpy(r, head, sizeof *r);
+    const cro_compute_sm* s = reinterpret_cast<const cro_compute_sm*>(head + kComputeSms);
+    sms->assign(s, s + compute_count(head, 0));
+    const cro_compute_fault* f = reinterpret_cast<const cro_compute_fault*>(head + kComputeHead);
+    faults->assign(f, f + compute_count(head, 1));
+    rc = r->status;
+    if (rc != CRO_OK && rc != CRO_ERR_CHECKSUM) set_call_error(c, "compute helper for " + want + ": " + cro_strerror(rc));
+    return rc;
 }
 
 }  // namespace cro

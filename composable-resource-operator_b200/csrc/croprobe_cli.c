@@ -24,7 +24,23 @@
  *                                                    the SRAM probe with every cro_sram_opts field; cro_sram_result,
  *                                                    CRO_SRAM_MAX_SMS cro_sram_sm entries (sms_listed of them filled)
  *                                                    and its `recorded` cro_sram_fault records (at most cap) on stdout
- * Exit 3: the device is not visible to this (fresh) process — the reference's found=false.
+ *   croprobe-cli link-raw <uuid> <seed_base> <bytes> <hops> <ctas> <inject_check> <inject_word> <inject_mask> <cap>
+ *                                                    the host link probe with every cro_link_opts field, its sweep
+ *                                                    region L (256 MiB when bytes is 0) and NVML on for the replay
+ *                                                    counters; cro_link_result, a uint64_t n, then n cro_link_fault
+ *                                                    records (at most cap) on stdout
+ *   croprobe-cli compute-raw <uuid> <seed_base> <iterations> <alu_iterations> <legs> <max_rounds> <inject_leg>
+ *                            <inject_sm> <inject_iteration> <inject_row> <inject_col> <inject_mask> <cap>
+ *                                                    the compute probe with every cro_compute_opts field, no sweep
+ *                                                    region and no NVML; cro_compute_result, uint64_t n_sms and n,
+ *                                                    CRO_COMPUTE_MAX_SMS cro_compute_sm entries (n_sms of them filled),
+ *                                                    then n cro_compute_fault records (at most cap) on stdout
+ *   link-raw and compute-raw take cro_opts.seed_base from argv (the device seed is seed_base | minor, as in process), so
+ *   that the library can give every helper call fresh patterns and operands; their counts are the helper's own,
+ *   because neither result says how many records follow.
+ * Exit 3: the device is not visible to this (fresh) process — the reference's found=false.  The raw commands exit 0
+ * iff the probe's status is CRO_OK, 1 for any other status (the result on stdout says which), 64 for a wrong argument
+ * count.
  *
  * Plain C against include/croprobe.h — the same surface the cgo shim binds.
  */
@@ -55,7 +71,9 @@ int main(int argc, char **argv) {
         fprintf(stderr, "usage: croprobe-cli csv <query> | enumerate | probe <uuid|index> [sweep_MiB] | probe-raw <uuid> [sweep_MiB] | "
                         "cold <uuid|index> [sweep_MiB] [nvml] | scan <uuid|index> [max_MiB] | scan-raw <uuid> <max> <reserve> <seed> <chunk> "
                         "<first> <count> <and> <or> <cap> | sram-raw <uuid> <legs> <iterations> <cluster> <rounds> <leg> <sm> <element> <iteration> "
-                        "<word> <mask> <cap>\n");
+                        "<word> <mask> <cap> | link-raw <uuid> <seed_base> <bytes> <hops> <ctas> <check> <word> <mask> <cap> | "
+                        "compute-raw <uuid> <seed_base> <iterations> <alu_iterations> <legs> <rounds> <leg> <sm> <iteration> <row> <col> "
+                        "<mask> <cap>\n");
         return 64;
     }
     const double t_start = now_s();
@@ -64,11 +82,16 @@ int main(int argc, char **argv) {
     const int cold = strcmp(cmd, "cold") == 0;
     const int scan_raw = strcmp(cmd, "scan-raw") == 0;
     const int sram_raw = strcmp(cmd, "sram-raw") == 0;
-    const int wants_scan = scan_raw || sram_raw || strcmp(cmd, "scan") == 0;
+    const int link_raw = strcmp(cmd, "link-raw") == 0;
+    const int compute_raw = strcmp(cmd, "compute-raw") == 0;
+    /* the commands that run one check of one device by their own, not the HBM probe */
+    const int wants_scan = scan_raw || sram_raw || link_raw || compute_raw || strcmp(cmd, "scan") == 0;
     const int wants_probe = raw || cold || strcmp(cmd, "probe") == 0;
     if ((wants_probe || wants_scan) && argc < 3) return 64;
     if (scan_raw && argc != 12) return 64;
     if (sram_raw && argc != 14) return 64;
+    if (link_raw && argc != 11) return 64;
+    if (compute_raw && argc != 15) return 64;
     cro_opts opts;
     memset(&opts, 0, sizeof opts);
     opts.abi_version = CRO_ABI_VERSION;
@@ -78,6 +101,13 @@ int main(int argc, char **argv) {
         opts.flags = CRO_F_LAZY_ALLOC;
         opts.sweep_bytes = 64ull << 20;
     }
+    if (compute_raw) opts.flags |= CRO_F_NO_NVML;       /* no health record to read, and NVML's first call is slow */
+    if (link_raw) {
+        /* a region of exactly L (the probe checks L <= S; no halving on a full GPU), and NVML for the replay counters */
+        opts.flags = CRO_F_LAZY_ALLOC;
+        opts.sweep_bytes = strtoull(argv[4], NULL, 10) ? (uint64_t)strtoull(argv[4], NULL, 10) : 256ull << 20;
+    }
+    if (link_raw || compute_raw) opts.seed_base = (uint64_t)strtoull(argv[3], NULL, 10);
     if (wants_probe) {
         /* The hot-plug path: one device, identity from /proc (NVML's first call costs more than the probe), and a
          * 1 GiB first sweep unless told otherwise — far beyond the L2, and it shortens everything before it. */
@@ -165,6 +195,57 @@ int main(int argc, char **argv) {
                 return 2;
             fflush(stdout);
             _exit(sr.status == CRO_OK ? 0 : 1);
+        }
+        if (link_raw) {
+            cro_link_opts lo;
+            memset(&lo, 0, sizeof lo);
+            lo.bytes = (uint64_t)strtoull(argv[4], NULL, 10);
+            lo.hops = (uint32_t)strtoul(argv[5], NULL, 10);
+            lo.ctas = (uint32_t)strtoul(argv[6], NULL, 10);
+            lo.test_inject_check = atoi(argv[7]);
+            lo.test_inject_word = (uint64_t)strtoull(argv[8], NULL, 10);
+            lo.test_inject_mask = (uint64_t)strtoull(argv[9], NULL, 10);
+            const int cap = atoi(argv[10]);
+            static cro_link_result lr;
+            cro_link_fault *faults = (cro_link_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
+            int got = 0;
+            if (!faults) return 2;
+            cro_probe_host_link(ctx, idx, &lo, &lr, faults, cap > 0 ? cap : 0, &got);
+            const uint64_t n_out = (uint64_t)got;
+            /* the result whatever its status: the library reads why from it */
+            if (fwrite(&lr, sizeof lr, 1, stdout) != 1 || fwrite(&n_out, sizeof n_out, 1, stdout) != 1 ||
+                (got && fwrite(faults, sizeof *faults, (size_t)got, stdout) != (size_t)got))
+                return 2;
+            fflush(stdout);
+            _exit(lr.status == CRO_OK ? 0 : 1);    /* the pinned buffers and the region go with the process */
+        }
+        if (compute_raw) {
+            cro_compute_opts co;
+            memset(&co, 0, sizeof co);
+            co.iterations = (uint32_t)strtoul(argv[4], NULL, 10);
+            co.alu_iterations = (uint32_t)strtoul(argv[5], NULL, 10);
+            co.legs = (uint32_t)strtoul(argv[6], NULL, 10);
+            co.max_rounds = (uint32_t)strtoul(argv[7], NULL, 10);
+            co.test_inject_leg = atoi(argv[8]);
+            co.test_inject_sm = atoi(argv[9]);
+            co.test_inject_iteration = (uint32_t)strtoul(argv[10], NULL, 10);
+            co.test_inject_row = atoi(argv[11]);
+            co.test_inject_col = atoi(argv[12]);
+            co.test_inject_mask = (uint32_t)strtoul(argv[13], NULL, 10);
+            const int cap = atoi(argv[14]);
+            static cro_compute_result cr;
+            static cro_compute_sm sms[CRO_COMPUTE_MAX_SMS];
+            cro_compute_fault *faults = (cro_compute_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
+            int n_sms = 0, got = 0;
+            if (!faults) return 2;
+            cro_probe_compute(ctx, idx, &co, &cr, sms, CRO_COMPUTE_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
+            const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)got};
+            /* the result whatever its status: the library reads why from it */
+            if (fwrite(&cr, sizeof cr, 1, stdout) != 1 || fwrite(counts, sizeof counts, 1, stdout) != 1 ||
+                fwrite(sms, sizeof sms, 1, stdout) != 1 || (got && fwrite(faults, sizeof *faults, (size_t)got, stdout) != (size_t)got))
+                return 2;
+            fflush(stdout);
+            _exit(cr.status == CRO_OK ? 0 : 1);
         }
         if (wants_scan) {
             cro_scan_opts so;

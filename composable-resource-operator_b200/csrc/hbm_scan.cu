@@ -11,16 +11,15 @@
 
 namespace cro {
 
-namespace {
-constexpr int kCfSlot0 = CRO_SCAN_PASSES * CRO_SCAN_MAX_CHUNKS;   // slots [p * MAX + k] compare folds, then closed forms
-
-// A seed no earlier call shares: the wall clock, the process and a per-process call count through splitmix.
 uint64_t fresh_seed() {
     static std::atomic<uint64_t> calls{0};
     const uint64_t t = (uint64_t)std::chrono::system_clock::now().time_since_epoch().count();
     const uint64_t s = pattern_word(t ^ ((uint64_t)getpid() << 40), calls.fetch_add(1) * kNonceStride);
     return s ? s : 1;     // 0 asks for a fresh seed: never report it as the one used
 }
+
+namespace {
+constexpr int kCfSlot0 = CRO_SCAN_PASSES * CRO_SCAN_MAX_CHUNKS;   // slots [p * MAX + k] compare folds, then closed forms
 
 void blank_report(cro_scan_report* rep, std::vector<cro_fault_word>* words) {
     memset(rep, 0, sizeof *rep);

@@ -53,6 +53,19 @@ void unmap_pinned(unsigned char*& p, size_t bytes) {
     pcilink::Unmap(p, bytes);
     p = nullptr;
 }
+
+// Why the options are refused for a sweep region of S bytes ("" when they pass): both forms' argument checks.
+std::string link_opts_error(const cro_link_opts& o, uint64_t S) {
+    const uint64_t L = o.bytes ? o.bytes : std::min(kLinkDefaultBytes, S);
+    const uint32_t hops = o.hops ? o.hops : kLinkDefaultHops;
+    if (L < 16 || L % 16 || L > S || hops > (1u << 24) || o.ctas > kLinkMaxCtas ||
+        (o.test_inject_mask && (o.test_inject_check < 0 || o.test_inject_check >= CRO_LINK_WORD_CHECKS ||
+                                o.test_inject_word >= L / 8)))
+        return "host link probe: L = " + std::to_string(L) + " must be a multiple of 16 in [16, " + std::to_string(S) +
+               "], hops at most 2^24, ctas at most " + std::to_string(kLinkMaxCtas) +
+               ", and an injection must name a word check (0..4) and a word below L / 8";
+    return "";
+}
 }  // namespace
 
 LinkState::~LinkState() {
@@ -74,12 +87,9 @@ int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_re
         const uint64_t S = d->sweep_bytes;
         const uint64_t L = o.bytes ? o.bytes : std::min(kLinkDefaultBytes, S);
         const uint32_t hops = o.hops ? o.hops : kLinkDefaultHops;
-        if (L < 16 || L % 16 || L > S || hops > (1u << 24) || o.ctas > kLinkMaxCtas ||
-            (o.test_inject_mask && (o.test_inject_check < 0 || o.test_inject_check >= CRO_LINK_WORD_CHECKS ||
-                                    o.test_inject_word >= L / 8))) {
-            c->set_error("host link probe: L = " + std::to_string(L) + " must be a multiple of 16 in [16, " + std::to_string(S) +
-                         "], hops at most 2^24, ctas at most " + std::to_string(kLinkMaxCtas) +
-                         ", and an injection must name a word check (0..4) and a word below L / 8");
+        const std::string why = link_opts_error(o, S);
+        if (!why.empty()) {
+            c->set_error(why);
             return CRO_ERR_INVALID_ARG;
         }
         const int grid = o.ctas ? (int)o.ctas : d->plan.link_grid;
@@ -303,6 +313,44 @@ int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_re
         return r->status = rc;
     }
     return r->status = r->first_fail == CRO_LINK_NO_FAIL ? CRO_OK : CRO_ERR_CHECKSUM;
+}
+
+namespace {
+// link-raw's stdout: the result, the helper's own fault count n, then n faults.
+uint64_t link_tail_count(const unsigned char* head) {
+    uint64_t n;
+    memcpy(&n, head + sizeof(cro_link_result), sizeof n);
+    return n;
+}
+}  // namespace
+
+int ctx_probe_host_link_uuid(cro_ctx* c, const char* uuid, const cro_link_opts& o, int deadline_ms, cro_link_result* r,
+                             std::vector<cro_link_fault>* faults, int cap, uint64_t* helper_ns) {
+    blank_result(r, faults, 0);
+    *helper_ns = 0;
+    if (!uuid) return r->status = CRO_ERR_INVALID_ARG;
+    // the helper's sweep region is L, or the default L when none is given: refuse here what it would refuse there
+    const std::string why = link_opts_error(o, o.bytes ? o.bytes : kLinkDefaultBytes);
+    if (!why.empty()) {
+        set_call_error(c, why);
+        return r->status = CRO_ERR_INVALID_ARG;
+    }
+    const std::string want = uuid;
+    auto num = [](uint64_t v) { return std::to_string(v); };
+    const std::vector<std::string> args = {"link-raw", want, num(helper_seed_base(c)), num(o.bytes), num(o.hops), num(o.ctas),
+                                           std::to_string(o.test_inject_check), num(o.test_inject_word), num(o.test_inject_mask),
+                                           num((uint64_t)cap)};
+    const size_t head = sizeof *r + sizeof(uint64_t);
+    std::string got;
+    int rc = run_probe_helper(c, want, "link helper", "cro.probe_host_link.helper", args, deadline_ms, head, sizeof(cro_link_fault),
+                              (size_t)cap, link_tail_count, &got, helper_ns);
+    if (rc != CRO_OK) return r->status = rc;
+    memcpy(r, got.data(), sizeof *r);
+    const cro_link_fault* f = reinterpret_cast<const cro_link_fault*>(got.data() + head);
+    faults->assign(f, f + link_tail_count(reinterpret_cast<const unsigned char*>(got.data())));
+    rc = r->status;
+    if (rc != CRO_OK && rc != CRO_ERR_CHECKSUM) set_call_error(c, "link helper for " + want + ": " + cro_strerror(rc));
+    return rc;
 }
 
 }  // namespace cro

@@ -870,4 +870,42 @@ int ctx_probe_uuid(cro_ctx* c, const char* uuid, cro_probe_result* out) {
     return rc;
 }
 
+void set_call_error(cro_ctx* c, const std::string& m) {
+    if (c) c->set_error(m);
+    else set_thread_error(m);
+}
+
+uint64_t helper_seed_base(cro_ctx* c) {
+    if (c) return c->opts.seed_base + ((c->helper_seeds.fetch_add(1) + 1) << 8);
+    const uint64_t s = fresh_seed() & ~0xFFull;
+    return s ? s : 0x100;         // 0 would ask the helper for the default base
+}
+
+int run_probe_helper(cro_ctx* c, const std::string& uuid, const std::string& what, const char* range,
+                     const std::vector<std::string>& args, int deadline_ms, size_t head, size_t rec, size_t cap,
+                     uint64_t (*count)(const unsigned char* head), std::string* got, uint64_t* helper_ns) {
+    env::Values knobs;                        // no context: this caller's environment, defaults where it is illegal
+    if (c) knobs = c->knobs;
+    else env::read(&knobs, nullptr);
+    const int deadline = deadline_ms > 0 ? deadline_ms : (int)knobs.get("CRO_HELPER_TIMEOUT_MS");
+    DeviceGuard g;
+    if (c) {
+        cro_dev_info hit{};
+        const int rc = find_on_node(c, uuid, &hit);
+        if (rc) return rc;
+        if (hit.flags & CRO_DEV_IN_PROCESS) {     // no probe of this GPU runs beside the helper
+            g = enter_device(c, hit.dev_index);
+            if (g.rc) return g.rc;
+        }
+    }
+    std::string err;
+    if (c && c->nvtx) nvtxRangePushA(range);
+    const uint64_t t_spawn = now_ns();
+    const int rc = inventory::RunHelperRaw("", what, uuid, args, deadline, head, rec, cap, count, got, &err);
+    *helper_ns = now_ns() - t_spawn;
+    if (c && c->nvtx) nvtxRangePop();
+    if (rc != CRO_OK && !err.empty()) set_call_error(c, err);
+    return rc;
+}
+
 }  // namespace cro

@@ -136,6 +136,8 @@ struct cro_ctx {
     std::atomic<uint64_t> launches{0};
     // gauges / counters behind cro_metrics_text (the operator's Prometheus registry, cmd/main.go:66,119-125)
     std::atomic<uint64_t> m_probes{0}, m_probe_failures{0}, m_fullbox{0}, m_helper_probes{0}, m_helper_failures{0};
+    // helper calls of the host link and compute probes' uuid forms so far: the seed base of each (helper_seed_base)
+    std::atomic<uint64_t> helper_seeds{0};
     std::mutex err_mu;
     std::string last_error;
     std::mutex all_mu;                 // serialises cro_probe_all
@@ -214,13 +216,35 @@ int ctx_locate(cro_ctx* c, int idx, const cro_locate_opts& o, cro_fault_report* 
 // CRO_FAULTS_* of a report, from its per-pass mismatch counts.
 uint32_t fault_verdict(const cro_fault_report& r);
 
-// Host link probe (include/croprobe.h, cro_probe_host_link): *faults gets every recorded mismatch, by check, then index.
+// Host link probe (include/croprobe.h, cro_probe_host_link / cro_probe_host_link_uuid): *faults gets every recorded
+// mismatch, by check, then index.  The uuid form runs `croprobe-cli link-raw` and asks it for at most cap faults;
+// *helper_ns is the helper's spawn to exit.
 int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_result* r, std::vector<cro_link_fault>* faults);
+int ctx_probe_host_link_uuid(cro_ctx* c, const char* uuid, const cro_link_opts& o, int deadline_ms, cro_link_result* r,
+                             std::vector<cro_link_fault>* faults, int cap, uint64_t* helper_ns);
 
-// SM compute probe (include/croprobe.h, cro_probe_compute): *sms gets one entry per SM seen, by SM id; *faults every
-// recorded element, by (leg, smid, row, col).
+// SM compute probe (include/croprobe.h, cro_probe_compute / cro_probe_compute_uuid): *sms gets one entry per SM seen, by
+// SM id; *faults every recorded element, by (leg, smid, row, col).  The uuid form runs `croprobe-cli compute-raw` and
+// asks it for at most cap faults; *helper_ns is the helper's spawn to exit.
 int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_compute_result* r, std::vector<cro_compute_sm>* sms,
                       std::vector<cro_compute_fault>* faults);
+int ctx_probe_compute_uuid(cro_ctx* c, const char* uuid, const cro_compute_opts& o, int deadline_ms, cro_compute_result* r,
+                           std::vector<cro_compute_sm>* sms, std::vector<cro_compute_fault>* faults, int cap, uint64_t* helper_ns);
+
+// The helper run behind the host link and compute probes' uuid forms.  Bad options are refused by the caller first.
+// With a context, the node must list the GPU (CRO_ERR_NO_DEVICE otherwise) and a GPU that is also an in-process device
+// is held under its device guard while the helper runs.  Then `croprobe-cli args...` runs as inventory::RunHelperRaw
+// runs it ("<what> for <uuid> ..." in its errors) and its stdout lands in *got.  *helper_ns: spawn to exit.  An error
+// goes to the context, or to the calling thread without one.
+int run_probe_helper(cro_ctx* c, const std::string& uuid, const std::string& what, const char* range,
+                     const std::vector<std::string>& args, int deadline_ms, size_t head, size_t rec, size_t cap,
+                     uint64_t (*count)(const unsigned char* head), std::string* got, uint64_t* helper_ns);
+// The cro_opts.seed_base a helper of those forms gets: with a context, its seed_base + (h << 8) for the context's h-th
+// such call (h from 1, so no helper repeats the context's own seeds); without one, a clock-derived base.  The low byte
+// is clear either way: the helper ORs the minor into it.
+uint64_t helper_seed_base(cro_ctx* c);
+// Sets an error text on the context, or on the calling thread without one.
+void set_call_error(cro_ctx* c, const std::string& m);
 
 // Whole-HBM scan (include/croprobe.h, cro_scan_hbm / cro_scan_hbm_uuid, hbm_scan.cu): *words gets every recorded word,
 // merged by scan index.  The uuid form runs `croprobe-cli scan-raw` and asks it for at most cap words.

@@ -37,6 +37,10 @@ struct Range {
     ~Range() { if (on) nvtxRangePop(); }
 };
 
+// A seed no earlier call shares: the wall clock, the process and a per-process call count through splitmix; never 0
+// (hbm_scan.cu).
+uint64_t fresh_seed();
+
 inline Params imm_params(const Device* d) { return Params{ProbeParams{d->seed_cur, d->nonce_cur}, nullptr}; }
 inline uint64_t seed_of(const Device* d, uint64_t nonce) { return d->seed_dev + nonce * kNonceStride; }
 

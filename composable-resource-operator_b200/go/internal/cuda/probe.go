@@ -290,10 +290,52 @@ type LinkFault struct {
 	HostValue uint64 // the host buffer's word: equal to Actual, the corruption reached host memory
 }
 
+func linkResult(res *C.cro_link_result, faults []C.cro_link_fault, got C.int) LinkResult {
+	out := LinkResult{OK: res.status == C.CRO_OK, FirstFail: uint32(res.first_fail), Bytes: uint64(res.bytes),
+		DuplexNs: uint64(res.ce_duplex_span_ns), ChaseNs: uint64(res.chase_ns), ChaseHops: uint32(res.chase_hops),
+		Degraded: uint32(res.degraded)}
+	for g := 0; g < int(C.CRO_LINK_LEGS); g++ {
+		out.LegBytes[g] = uint64(res.leg[g].bytes)
+		out.LegNs[g] = uint64(res.leg[g].ns)
+	}
+	for i := 0; i < int(got); i++ {
+		f := faults[i]
+		out.Faults = append(out.Faults, LinkFault{uint32(f.check), uint64(f.word_index), uint64(f.expected), uint64(f.actual),
+			uint64(f.host_value)})
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_link_annotations_json(res, buf, 4096, &ln) == C.CRO_OK {
+		out.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return out
+}
+
+// ProbeHostLinkByUUID runs cro_probe_host_link_uuid with its defaults: the host
+// link probe of any GPU on the node through the helper process, the form an
+// operator calls once after a passing HBM probe of a freshly composed GPU
+// (INTEGRATION.md §2).  A mismatch is a result, not an error; found is false
+// when the node does not list the GPU.
+func (c *Context) ProbeHostLinkByUUID(deviceID string) (r LinkResult, found bool, err error) {
+	id := C.CString(deviceID)
+	defer C.free(unsafe.Pointer(id))
+	var res C.cro_link_result
+	var faults [256]C.cro_link_fault
+	var got C.int
+	rc := C.cro_probe_host_link_uuid(c.h, id, nil, 0, &res, &faults[0], 256, &got, nil)
+	if rc == C.CRO_ERR_NO_DEVICE {
+		return r, false, nil
+	}
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM {
+		return r, true, errorOf(c.h, rc)
+	}
+	return linkResult(&res, faults[:], got), true, nil
+}
+
 // ProbeHostLink runs cro_probe_host_link with its defaults on the in-process
-// device whose UUID is deviceID, typically once after a passing HBM probe of a
-// freshly composed GPU.  A device probed through the helper process is an
-// error, as for LocateFaults.
+// device whose UUID is deviceID.  ProbeHostLinkByUUID is the form an operator
+// should call: it also reaches a GPU composed after the manager started.
 func (c *Context) ProbeHostLink(deviceID string) (LinkResult, error) {
 	var devs [C.CRO_MAX_DEVICES]C.cro_dev_info
 	var n C.int
@@ -316,25 +358,7 @@ func (c *Context) ProbeHostLink(deviceID string) (LinkResult, error) {
 	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM {
 		return LinkResult{}, errorOf(c.h, rc)
 	}
-	out := LinkResult{OK: rc == C.CRO_OK, FirstFail: uint32(res.first_fail), Bytes: uint64(res.bytes),
-		DuplexNs: uint64(res.ce_duplex_span_ns), ChaseNs: uint64(res.chase_ns), ChaseHops: uint32(res.chase_hops),
-		Degraded: uint32(res.degraded)}
-	for g := 0; g < int(C.CRO_LINK_LEGS); g++ {
-		out.LegBytes[g] = uint64(res.leg[g].bytes)
-		out.LegNs[g] = uint64(res.leg[g].ns)
-	}
-	for i := 0; i < int(got); i++ {
-		f := faults[i]
-		out.Faults = append(out.Faults, LinkFault{uint32(f.check), uint64(f.word_index), uint64(f.expected), uint64(f.actual),
-			uint64(f.host_value)})
-	}
-	buf := (*C.char)(C.malloc(4096))
-	defer C.free(unsafe.Pointer(buf))
-	var ln C.size_t
-	if C.cro_emit_link_annotations_json(&res, buf, 4096, &ln) == C.CRO_OK {
-		out.Annotations = C.GoStringN(buf, C.int(ln))
-	}
-	return out, nil
+	return linkResult(&res, faults[:], got), nil
 }
 
 // ComputeResult is the summary of cro_compute_result an operator reads: whether
@@ -357,10 +381,61 @@ type ComputeFault struct {
 	Expected, Actual  int32
 }
 
+func computeResult(res *C.cro_compute_result, sms []C.cro_compute_sm, nSMs C.int, faults []C.cro_compute_fault,
+	got C.int) ComputeResult {
+	out := ComputeResult{OK: res.status == C.CRO_OK, Verdict: uint32(res.verdict), SMCount: uint32(res.sm_count)}
+	for l := 0; l < int(C.CRO_COMPUTE_LEGS); l++ {
+		out.Covered[l] = uint32(res.leg[l].sms_covered)
+		out.Mismatches[l] = uint64(res.leg[l].mismatches)
+	}
+	for i := 0; i < int(nSMs); i++ {
+		for l := 0; l < int(C.CRO_COMPUTE_LEGS); l++ {
+			if sms[i].leg[l].mark != 0 {
+				out.BadSMs = append(out.BadSMs, uint32(sms[i].smid))
+				break
+			}
+		}
+	}
+	for i := 0; i < int(got); i++ {
+		f := faults[i]
+		out.Faults = append(out.Faults, ComputeFault{uint32(f.leg), uint32(f.smid), uint32(f.row), uint32(f.col),
+			int32(f.expected), int32(f.actual)})
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_compute_annotations_json(res, buf, 4096, &ln) == C.CRO_OK {
+		out.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return out
+}
+
+// ProbeComputeByUUID runs cro_probe_compute_uuid with its defaults: the compute
+// probe of any GPU on the node through the helper process, the form an operator
+// calls after a passing HBM probe of a freshly composed GPU and after a locator
+// verdict of not-reproduced (INTEGRATION.md §2).  A mismatch or a failed launch
+// (CRO_ERR_CUDA) is a result, not an error; found is false when the node does
+// not list the GPU.
+func (c *Context) ProbeComputeByUUID(deviceID string) (r ComputeResult, found bool, err error) {
+	id := C.CString(deviceID)
+	defer C.free(unsafe.Pointer(id))
+	var res C.cro_compute_result
+	sms := make([]C.cro_compute_sm, C.CRO_COMPUTE_MAX_SMS)
+	var faults [256]C.cro_compute_fault
+	var nSMs, got C.int
+	rc := C.cro_probe_compute_uuid(c.h, id, nil, 0, &res, &sms[0], C.CRO_COMPUTE_MAX_SMS, &nSMs, &faults[0], 256, &got, nil)
+	if rc == C.CRO_ERR_NO_DEVICE {
+		return r, false, nil
+	}
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM && rc != C.CRO_ERR_CUDA {
+		return r, true, errorOf(c.h, rc)
+	}
+	return computeResult(&res, sms, nSMs, faults[:], got), true, nil
+}
+
 // ProbeCompute runs cro_probe_compute with its defaults on the in-process
-// device whose UUID is deviceID: after a passing HBM probe of a freshly composed
-// GPU, and after a locator verdict of not-reproduced.  A device probed through
-// the helper process is an error, as for LocateFaults.
+// device whose UUID is deviceID.  ProbeComputeByUUID is the form an operator
+// should call: it also reaches a GPU composed after the manager started.
 func (c *Context) ProbeCompute(deviceID string) (ComputeResult, error) {
 	var devs [C.CRO_MAX_DEVICES]C.cro_dev_info
 	var n C.int
@@ -384,31 +459,7 @@ func (c *Context) ProbeCompute(deviceID string) (ComputeResult, error) {
 	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM {
 		return ComputeResult{}, errorOf(c.h, rc)
 	}
-	out := ComputeResult{OK: rc == C.CRO_OK, Verdict: uint32(res.verdict), SMCount: uint32(res.sm_count)}
-	for l := 0; l < int(C.CRO_COMPUTE_LEGS); l++ {
-		out.Covered[l] = uint32(res.leg[l].sms_covered)
-		out.Mismatches[l] = uint64(res.leg[l].mismatches)
-	}
-	for i := 0; i < int(nSMs); i++ {
-		for l := 0; l < int(C.CRO_COMPUTE_LEGS); l++ {
-			if sms[i].leg[l].mark != 0 {
-				out.BadSMs = append(out.BadSMs, uint32(sms[i].smid))
-				break
-			}
-		}
-	}
-	for i := 0; i < int(got); i++ {
-		f := faults[i]
-		out.Faults = append(out.Faults, ComputeFault{uint32(f.leg), uint32(f.smid), uint32(f.row), uint32(f.col),
-			int32(f.expected), int32(f.actual)})
-	}
-	buf := (*C.char)(C.malloc(4096))
-	defer C.free(unsafe.Pointer(buf))
-	var ln C.size_t
-	if C.cro_emit_compute_annotations_json(&res, buf, 4096, &ln) == C.CRO_OK {
-		out.Annotations = C.GoStringN(buf, C.int(ln))
-	}
-	return out, nil
+	return computeResult(&res, sms, nSMs, faults[:], got), nil
 }
 
 // ScanResult is the summary of cro_scan_report an operator reads: whether every

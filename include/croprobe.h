@@ -652,6 +652,21 @@ typedef struct cro_link_result {
 int  cro_probe_host_link(cro_ctx *ctx, int dev_index, const cro_link_opts *opts,
                          cro_link_result *out, cro_link_fault *faults, int cap, int *n);
 
+/* The same probe of any GPU on the node, run by `croprobe-cli link-raw` (a fresh cuInit that sees only that GPU): the
+ * form an operator calls (INTEGRATION.md §2).  It reaches GPUs attached after cro_probe_init, and an uncorrectable error
+ * in the memory it uses costs the helper, not the caller's context.  The helper's sweep region is L (256 MiB when
+ * opts->bytes is 0, the in-process default of a 4 GiB region), so L <= S always holds; every other option is checked as
+ * in process, before any helper starts.  ctx may be NULL; a UUID the node does not list, or one the helper cannot see, is
+ * CRO_ERR_NO_DEVICE; a GPU that is also an in-process device of ctx is held under that device's mutex while the helper
+ * runs (probes in flight finish first and stay collectable; its sweep region is not touched, so the fault locator's
+ * pass 0 still compares both halves).  deadline_ms 0: CRO_HELPER_TIMEOUT_MS; a helper past it is killed
+ * (CRO_ERR_DEADLINE).  *helper_ns (may be NULL): the helper's spawn to exit.  The result and faults are what the
+ * in-process call on that GPU writes; the seeds come from a base drawn per helper call (ctx's seed_base + (h << 8) for
+ * its h-th such call, from 1, or one from the clock without ctx), and call is 0.  Malformed output or a crash:
+ * CRO_ERR_EXEC. */
+int  cro_probe_host_link_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_link_opts *opts, int deadline_ms,
+                              cro_link_result *out, cro_link_fault *faults, int cap, int *n, uint64_t *helper_ns);
+
 /* The PCIe path of pci_bus_id ("00000000:1F:00.0" or "0000:1f:00.0") under sys_root (NULL: "/sys"), from
  * <sys_root>/bus/pci/devices/<bdf>: current / max link speed and width and numa_node of the device and of every
  * ancestor on its real path that has link files.  Reads sysfs only; no context, no CUDA.  CRO_ERR_INVALID_ARG: a bus
@@ -794,6 +809,14 @@ typedef struct cro_compute_fault {
  * cro_locate_faults).  opts may be NULL: defaults.  Incomplete coverage never changes the status. */
 int  cro_probe_compute(cro_ctx *ctx, int dev_index, const cro_compute_opts *opts, cro_compute_result *out,
                        cro_compute_sm *sms, int sms_cap, int *n_sms, cro_compute_fault *faults, int cap, int *n);
+
+/* The same probe of any GPU on the node, run by `croprobe-cli compute-raw` (a fresh cuInit that sees only that GPU):
+ * the form an operator calls (INTEGRATION.md §2).  Options are checked as in process, before any helper starts; ctx,
+ * deadline_ms, *helper_ns, the seed base and the return codes are as for cro_probe_host_link_uuid (a failed launch:
+ * CRO_ERR_CUDA, the helper's status). */
+int  cro_probe_compute_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_compute_opts *opts, int deadline_ms,
+                            cro_compute_result *out, cro_compute_sm *sms, int sms_cap, int *n_sms,
+                            cro_compute_fault *faults, int cap, int *n, uint64_t *helper_ns);
 
 /* The expected answer the call uploads: answer CRO_COMPUTE_ANSWER_S8 or _SMALL of the operands of `seed`, as
  * CRO_COMPUTE_M * CRO_COMPUTE_N int32 values, row-major.  Host arithmetic only; no context. */

@@ -7,7 +7,12 @@ launches of the leg, so the operand generation and the compare are inside it).  
 tile's M = 128 is two m64 row blocks, one warpgroup each, and a third warpgroup's 128 accumulator registers per thread
 do not fit (384 threads x ~208 registers > the SM's 65536).  PyTorch: torch.matmul in bf16, torch._scaled_mm in e4m3
 and torch._int_mm in int8 on 8192^3, CUDA events, median of 21 after 3 warm-up calls.  The card's name, power limit and
-max SM clock come from a read-only nvidia-smi query in the same run."""
+max SM clock come from a read-only nvidia-smi query in the same run.
+
+--helper: instead, the helper form (cro_probe_compute_uuid) against the in-process form at the default settings:
+HELPER_ROUNDS calls of each, alternating, in one context over cuda:0.  One line, appended to --out: the median, least
+and largest spawn-to-exit time of the helper, the in-process call's wall time, and per leg the median rate inside the
+helper and in process."""
 import argparse
 import importlib
 import json
@@ -23,6 +28,8 @@ ROUNDS = 21
 ITERATIONS = [16, 64, 256, 1024, 4096]
 TENSOR = [("s8", cro.COMPUTE_LEG_S8), ("bf16", cro.COMPUTE_LEG_BF16), ("e4m3", cro.COMPUTE_LEG_E4M3)]
 G = 8192
+HELPER_ROUNDS = 9
+LEG_NAMES = ["s8", "bf16", "e4m3", "ffma", "imad"]
 
 
 def med(xs):
@@ -57,9 +64,38 @@ def torch_gemms():
     return out
 
 
+def helper_rates(gpu: str, power: str, clock: str) -> dict:
+    with cro.ProbeContext(sweep_bytes=64 << 20, devices=[0]) as ctx:
+        uuid = ctx.own_devices()[0].gpu_uuid.decode()
+        ctx.probe_compute(0)                                         # warm-up: modules loaded, clocks up
+        cro.probe_compute_uuid(ctx, uuid)
+        inproc, helper, spawn, walls = [], [], [], []
+        for _ in range(HELPER_ROUNDS):
+            t = time.perf_counter_ns()
+            r, _s, _f = ctx.probe_compute(0)
+            walls.append(time.perf_counter_ns() - t)
+            assert r.status == cro.OK
+            inproc.append(r)
+            r, _s, _f, ns = cro.probe_compute_uuid(ctx, uuid)
+            assert r.status == cro.OK
+            helper.append(r)
+            spawn.append(ns)
+    out = {"gpu": gpu, "power_limit": power, "clocks_max_sm": clock, "probe": "compute", "rounds": HELPER_ROUNDS,
+           "iterations": r.leg[0].iterations, "alu_iterations": r.leg[cro.COMPUTE_LEG_FFMA].iterations,
+           "helper_ns_median": med(spawn), "helper_ns_min": min(spawn), "helper_ns_max": max(spawn),
+           "in_process_wall_ns_median": med(walls),
+           "host_ref_ns_median": {"helper": med([r.host_ref_ns for r in helper]), "in_process": med([r.host_ref_ns for r in inproc])}}
+    for leg, name in enumerate(LEG_NAMES):
+        out[name + "_rate_median"] = {"helper": med([r.leg[leg].ops // r.leg[leg].ns for r in helper]),
+                                      "in_process": med([r.leg[leg].ops // r.leg[leg].ns for r in inproc])}
+    return out
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--out-dir", default=os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "profiles"))
+    ap.add_argument("--helper", action="store_true", help="the helper form against the in-process form")
+    ap.add_argument("--out", default=None, help="--helper: append the line to this file")
     args = ap.parse_args()
     lines = []
 
@@ -71,6 +107,12 @@ def main() -> None:
     gpu, power, clock = subprocess.run(
         ["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
         capture_output=True, text=True, check=True).stdout.strip().split(", ")
+    if args.helper:
+        emit(helper_rates(gpu, power, clock))
+        if args.out:
+            with open(args.out, "a") as f:
+                f.write("\n".join(lines) + "\n")
+        return
     best = {}
     with cro.ProbeContext(sweep_bytes=64 << 20, devices=[0]) as ctx:
         ctx.probe_compute(0, iterations=16, alu_iterations=1)       # warm-up: modules loaded, clocks up

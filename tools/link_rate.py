@@ -4,7 +4,11 @@ one line per grid point, then the summary line.
 First the grid of the SM legs: for each CTA count, 3 calls, median MB/s of the SM h2d, d2h and duplex legs (events).
 Then 21 calls at the default grid, median per leg.  The GPU's name and power limit come from nvidia-smi in the same
 run, and the trained link (current and max speed and width, sampled during the copy-engine duplex leg) from the
-result itself."""
+result itself.
+
+--helper: instead, the helper form (cro_probe_host_link_uuid) against the in-process form at L = 256 MiB, the helper's
+default: HELPER_ROUNDS calls of each, alternating, in one context over cuda:0.  One line: the median, least and largest
+spawn-to-exit time of the helper, and per leg the median MB/s inside the helper and in process."""
 import argparse
 import importlib
 import json
@@ -18,6 +22,8 @@ cro = importlib.import_module("composable-resource-operator_b200")
 L = 1 << 30
 ROUNDS = 21
 GRIDS = [1, 2, 4, 8, 16, 32, 66, 132]
+HELPER_L = 256 << 20
+HELPER_ROUNDS = 9
 LEGS = ["ce_d2h", "sm_h2d", "ce_h2d", "sm_d2h", "sm_duplex_h2d", "sm_duplex_d2h", "ce_duplex_h2d", "ce_duplex_d2h"]
 
 
@@ -33,9 +39,36 @@ def speed(t):
     return "unknown" if t == 0 else "%d.%dGT/s" % (t // 10, t % 10)
 
 
+def helper_rates(gpu: str, power: str) -> dict:
+    with cro.ProbeContext(sweep_bytes=HELPER_L, devices=[0]) as ctx:
+        uuid = ctx.own_devices()[0].gpu_uuid.decode()
+        ctx.probe_host_link(0, bytes=HELPER_L)                      # warm-up: host buffers pinned, link trained up
+        cro.probe_host_link_uuid(ctx, uuid, bytes=HELPER_L)
+        inproc, helper, spawn = [], [], []
+        for _ in range(HELPER_ROUNDS):
+            r, _f = ctx.probe_host_link(0, bytes=HELPER_L)
+            assert r.status == cro.OK, r.first_fail
+            inproc.append(r)
+            r, _f, ns = cro.probe_host_link_uuid(ctx, uuid, bytes=HELPER_L)
+            assert r.status == cro.OK, r.first_fail
+            helper.append(r)
+            spawn.append(ns)
+    out = {"gpu": gpu, "power_limit": power, "probe": "host_link", "bytes": HELPER_L, "rounds": HELPER_ROUNDS,
+           "helper_ns_median": med(spawn), "helper_ns_min": min(spawn), "helper_ns_max": max(spawn),
+           "legs_ns_median": {"helper": med([sum(g.ns for g in r.leg) for r in helper]),
+                              "in_process": med([sum(g.ns for g in r.leg) for r in inproc])}}
+    for i, name in enumerate(LEGS):
+        out[name + "_mbps_median"] = {"helper": med([mbps(r.leg[i].bytes, r.leg[i].ns) for r in helper]),
+                                      "in_process": med([mbps(r.leg[i].bytes, r.leg[i].ns) for r in inproc])}
+    out["latency_ns_median"] = {"helper": med([r.chase_ns // r.chase_hops for r in helper]),
+                                "in_process": med([r.chase_ns // r.chase_hops for r in inproc])}
+    return out
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
+    ap.add_argument("--helper", action="store_true", help="the helper form against the in-process form")
     args = ap.parse_args()
     lines = []
 
@@ -45,6 +78,12 @@ def main() -> None:
 
     gpu, power = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
                                 capture_output=True, text=True, check=True).stdout.strip().split(", ")
+    if args.helper:
+        emit(json.dumps(helper_rates(gpu, power)))
+        if args.out:
+            with open(args.out, "a") as f:
+                f.write("\n".join(lines) + "\n")
+        return
     with cro.ProbeContext(sweep_bytes=L, devices=[0]) as ctx:
         assert ctx.probe_device(0).status == cro.OK
         for _ in range(2):       # warm-up: host buffers allocated and pinned, link trained up
