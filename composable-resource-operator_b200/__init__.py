@@ -438,6 +438,81 @@ class SramFault(ctypes.Structure):
                 ("actual", ctypes.c_uint64)]
 
 
+# L2 probe (cro_probe_l2, cro_read_l2_health, cro_selftest_l2_classify)
+L2_BLOCK_BYTES, L2_MIN_BYTES, L2_MAX_L2_MULTIPLE, L2_ELEMENTS, L2_RECORDS, L2_MAX_SMS = 16384, 1 << 20, 8, 6, 4096, 256
+L2_MAX_ITERATIONS, L2_MAX_A1_COUNTERS, L2_MAX_A2_COUNTERS, L2_MAX_LINES, L2_MAX_COUNTERS = 256, 1 << 20, 8192, 8, 8
+L2_MARCH, L2_A1, L2_A2 = 0, 1, 2
+L2_NONE, L2_SM, L2_LINE, L2_ATOMIC, L2_ALL = 0, 1, 2, 3, 4
+L2_PERSISTENT, L2_INTERMITTENT = 1, 2
+(L2_HEALTH_SRAM_CORRECTED_DURING, L2_HEALTH_SRAM_UNCORRECTED_DURING, L2_HEALTH_L2_CORRECTED_DURING,
+ L2_HEALTH_L2_UNCORRECTED_DURING, L2_HEALTH_THRESHOLD_EXCEEDED, L2_HEALTH_L2_BUCKET) = 1, 2, 4, 8, 16, 32
+L2_NVML_SRAM_CORRECTED, L2_NVML_SRAM_UNCORRECTED, L2_NVML_L2_CORRECTED, L2_NVML_L2_UNCORRECTED, L2_NVML_STATUS = 1, 2, 4, 8, 16
+
+
+class L2Opts(ctypes.Structure):
+    _fields_ = [("bytes", ctypes.c_uint64), ("iterations", ctypes.c_uint32), ("a1_counters", ctypes.c_uint32),
+                ("a2_counters", ctypes.c_uint32), ("deadline_ms", ctypes.c_int32), ("test_inject_leg", ctypes.c_int32),
+                ("test_inject_sm", ctypes.c_int32), ("test_inject_element", ctypes.c_int32),
+                ("test_inject_iteration", ctypes.c_uint32), ("test_inject_word", ctypes.c_int64),
+                ("test_inject_mask", ctypes.c_uint64)]
+
+
+class L2Health(ctypes.Structure):
+    """cro_l2_health: NVML's volatile SRAM and L2 ECC counts, and the SRAM error status's threshold flag and L2 bucket;
+    `nvml` has an L2_NVML_* bit per read answered."""
+    _fields_ = [("nvml", ctypes.c_uint32), ("threshold_exceeded", ctypes.c_uint32), ("sram_corrected", ctypes.c_uint64),
+                ("sram_uncorrected", ctypes.c_uint64), ("l2_corrected", ctypes.c_uint64), ("l2_uncorrected", ctypes.c_uint64),
+                ("unc_bucket_l2", ctypes.c_uint64)]
+
+
+class L2Result(ctypes.Structure):
+    """cro_l2_result: status, verdict, bad SMs, lines and counters, exact counts, the M5 fold against its closed form,
+    times and NVML health of one L2 probe call."""
+    _fields_ = [("status", ctypes.c_int32), ("verdict", ctypes.c_uint32), ("seed", ctypes.c_uint64),
+                ("seed_atomic", ctypes.c_uint64), ("call", ctypes.c_uint64), ("bytes", ctypes.c_uint64),
+                ("sm_count", ctypes.c_uint32), ("nsmid", ctypes.c_uint32), ("ctas", ctypes.c_uint32), ("blocks", ctypes.c_uint32),
+                ("delta", ctypes.c_uint32), ("iterations", ctypes.c_uint32), ("cuda_error", ctypes.c_int32),
+                ("health", ctypes.c_uint32), ("sms_covered", ctypes.c_uint32), ("unpublished", ctypes.c_uint32),
+                ("mismatches", ctypes.c_uint64 * L2_ELEMENTS), ("recorded", ctypes.c_uint64), ("overflow", ctypes.c_uint32),
+                ("sms_listed", ctypes.c_uint32), ("bad_sms", ctypes.c_uint32), ("bad_lines", ctypes.c_uint32),
+                ("bad_sm", ctypes.c_uint16 * 16), ("bad_line", ctypes.c_uint64 * L2_MAX_LINES),
+                ("fold_xor", ctypes.c_uint64), ("fold_sum", ctypes.c_uint64), ("fold_wsum", ctypes.c_uint64),
+                ("expect_xor", ctypes.c_uint64), ("expect_sum", ctypes.c_uint64), ("expect_wsum", ctypes.c_uint64),
+                ("fold_ok", ctypes.c_uint32), ("a1_counters", ctypes.c_uint32), ("a2_counters", ctypes.c_uint32),
+                ("a2_tickets", ctypes.c_uint32), ("a1_bad", ctypes.c_uint64), ("a2_holes", ctypes.c_uint64),
+                ("a2_bad", ctypes.c_uint64), ("a1_bad_counter", ctypes.c_uint32 * L2_MAX_COUNTERS),
+                ("a2_bad_counter", ctypes.c_uint32 * L2_MAX_COUNTERS), ("element_ns", ctypes.c_uint64 * L2_ELEMENTS),
+                ("march_ns", ctypes.c_uint64), ("march_bytes", ctypes.c_uint64), ("a1_ns", ctypes.c_uint64),
+                ("a1_check_ns", ctypes.c_uint64), ("a2_ns", ctypes.c_uint64), ("a2_check_ns", ctypes.c_uint64),
+                ("l2_bytes", ctypes.c_uint64), ("wall_ns", ctypes.c_uint64), ("helper_ns", ctypes.c_uint64),
+                ("before", L2Health), ("after", L2Health)]
+
+    @property
+    def fold(self) -> Tuple[int, int, int]:
+        return (self.fold_xor, self.fold_sum, self.fold_wsum)
+
+    @property
+    def expect(self) -> Tuple[int, int, int]:
+        return (self.expect_xor, self.expect_sum, self.expect_wsum)
+
+
+class L2Sm(ctypes.Structure):
+    """One SM seen by an L2 probe call: its launches, the reads it saw wrong per element (and in the last iteration),
+    the words it read per element and its L2_PERSISTENT / _INTERMITTENT mark."""
+    _fields_ = [("smid", ctypes.c_uint32), ("mark", ctypes.c_uint32), ("launches", ctypes.c_uint32),
+                ("reserved", ctypes.c_uint32), ("mismatches", ctypes.c_uint64 * L2_ELEMENTS), ("last", ctypes.c_uint64),
+                ("words_read", ctypes.c_uint64 * L2_ELEMENTS), ("ns", ctypes.c_uint64)]
+
+
+class L2Fault(ctypes.Structure):
+    """One failed compare: element, iteration, the reader's SM and CTA, the writer's CTA and SM, the word, expected,
+    actual and whether the word is a line fault."""
+    _fields_ = [("element", ctypes.c_uint32), ("iteration", ctypes.c_uint32), ("smid", ctypes.c_uint32),
+                ("cta", ctypes.c_uint32), ("writer_cta", ctypes.c_uint32), ("writer_smid", ctypes.c_uint32),
+                ("word", ctypes.c_uint64), ("expected", ctypes.c_uint64), ("actual", ctypes.c_uint64),
+                ("line", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
 # test hook: one sweep kernel between guard bands (cro_selftest_sweep)
 (SELFTEST_SWEEP_FILL, SELFTEST_SWEEP_COPY_LDG, SELFTEST_SWEEP_COPY_TMA, SELFTEST_SWEEP_COPY_FUSED, SELFTEST_SWEEP_READ_LDG,
  SELFTEST_SWEEP_READ_TMA, SELFTEST_SWEEP_READ_LDG256, SELFTEST_SWEEP_LOCATE, SELFTEST_SWEEP_FORCE_WORDS,
@@ -473,6 +548,7 @@ assert ctypes.sizeof(FaultReport) == 928 and ctypes.sizeof(LocatePass) == 120, c
 assert ctypes.sizeof(LinkResult) == 984 and ctypes.sizeof(PciPath) == 272, ctypes.sizeof(LinkResult)
 assert ctypes.sizeof(ScanReport) == 12632 and ctypes.sizeof(ScanOpts) == 72, ctypes.sizeof(ScanReport)
 assert ctypes.sizeof(SramResult) == 568 and ctypes.sizeof(SramSm) == 168 and ctypes.sizeof(SramFault) == 48, ctypes.sizeof(SramResult)
+assert ctypes.sizeof(L2Result) == 616 and ctypes.sizeof(L2Sm) == 128 and ctypes.sizeof(L2Fault) == 56, ctypes.sizeof(L2Result)
 
 # Every symbol include/croprobe.h declares; tests check the library exports all of them.
 EXPORTS = [
@@ -499,6 +575,7 @@ EXPORTS = [
     "cro_probe_compute", "cro_probe_compute_uuid", "cro_compute_expected", "cro_emit_compute_annotations_json",
     "cro_scan_hbm", "cro_scan_hbm_uuid", "cro_read_hbm_health", "cro_emit_scan_annotations_json",
     "cro_probe_sram", "cro_probe_sram_uuid", "cro_read_sram_health", "cro_emit_sram_annotations_json",
+    "cro_probe_l2", "cro_probe_l2_uuid", "cro_read_l2_health", "cro_emit_l2_annotations_json", "cro_selftest_l2_classify",
 ]
 
 # Slot map of a device's sweep-slot array (cro_sweep_slot, 64 bytes each); the cro_selftest_* hooks take such arrays.
@@ -616,6 +693,13 @@ def _load() -> ctypes.CDLL:
                                       ctypes.POINTER(i32), ctypes.POINTER(SramFault), i32, ctypes.POINTER(i32)]),
         "cro_read_sram_health": (i32, [c, ctypes.POINTER(SramHealth)]),
         "cro_emit_sram_annotations_json": (i32, [ctypes.POINTER(SramResult)] + out),
+        "cro_probe_l2": (i32, [vp, i32, ctypes.POINTER(L2Opts), ctypes.POINTER(L2Result), ctypes.POINTER(L2Sm), i32,
+                               ctypes.POINTER(i32), ctypes.POINTER(L2Fault), i32, ctypes.POINTER(i32)]),
+        "cro_probe_l2_uuid": (i32, [vp, c, ctypes.POINTER(L2Opts), ctypes.POINTER(L2Result), ctypes.POINTER(L2Sm), i32,
+                                    ctypes.POINTER(i32), ctypes.POINTER(L2Fault), i32, ctypes.POINTER(i32)]),
+        "cro_read_l2_health": (i32, [c, ctypes.POINTER(L2Health)]),
+        "cro_emit_l2_annotations_json": (i32, [ctypes.POINTER(L2Result)] + out),
+        "cro_selftest_l2_classify": (i32, [ctypes.POINTER(L2Result), ctypes.POINTER(L2Sm), i32, ctypes.POINTER(L2Fault), i32]),
         "cro_local_node_op": (i32, [vp, c] + out),
         "cro_local_exec": (i32, [c] + out),
         "cro_describe_wire_type": (i32, [c] + out),
@@ -782,6 +866,62 @@ def read_sram_health(uuid: str) -> SramHealth:
     if rc != OK:
         raise ProbeError(rc, "cro_read_sram_health")
     return h
+
+
+def emit_l2_annotations_json(r: L2Result) -> str:
+    """Additive cohdi.io/probe-l2-* annotations of an L2 probe result (Go-marshalled map[string]string)."""
+    return _text(lib.cro_emit_l2_annotations_json, ctypes.byref(r))
+
+
+def read_l2_health(uuid: str) -> L2Health:
+    """cro_read_l2_health: the GPU's volatile SRAM and L2 ECC counts and SRAM error status from NVML (no context, no
+    CUDA)."""
+    h = L2Health()
+    rc = lib.cro_read_l2_health(_b(uuid), ctypes.byref(h))
+    if rc != OK:
+        raise ProbeError(rc, "cro_read_l2_health")
+    return h
+
+
+def _l2_opts(bytes: int, iterations: int, a1_counters: int, a2_counters: int, deadline_ms: int,
+             inject: Optional[Tuple[int, int, int, int, int, int]]) -> L2Opts:
+    o = L2Opts()
+    o.bytes, o.iterations, o.a1_counters, o.a2_counters, o.deadline_ms = bytes, iterations, a1_counters, a2_counters, deadline_ms
+    if inject is not None:
+        (o.test_inject_leg, o.test_inject_sm, o.test_inject_element, o.test_inject_iteration, o.test_inject_word,
+         o.test_inject_mask) = inject
+    return o
+
+
+def probe_l2_uuid(ctx: Optional["ProbeContext"], uuid: str, bytes: int = 0, iterations: int = 0, a1_counters: int = 0,
+                  a2_counters: int = 0, deadline_ms: int = 0, inject: Optional[Tuple[int, int, int, int, int, int]] = None,
+                  cap: int = 256) -> Tuple[L2Result, List[L2Sm], List[L2Fault]]:
+    """cro_probe_l2_uuid: the L2 probe of any GPU on the node, run by the helper process (ctx may be None).
+    Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up to `cap` records."""
+    o = _l2_opts(bytes, iterations, a1_counters, a2_counters, deadline_ms, inject)
+    r = L2Result()
+    sms = (L2Sm * L2_MAX_SMS)()
+    arr = (L2Fault * max(1, cap))()
+    n_sms, n = ctypes.c_int(), ctypes.c_int()
+    handle = ctx.handle if ctx is not None else None
+    rc = lib.cro_probe_l2_uuid(handle, _b(uuid), ctypes.byref(o), ctypes.byref(r), sms, L2_MAX_SMS, ctypes.byref(n_sms),
+                               arr, cap, ctypes.byref(n))
+    if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
+        buf = ctypes.create_string_buffer(1024)
+        lib.cro_last_error(handle, buf, 1024)
+        raise ProbeError(rc, buf.value.decode("utf-8", "replace"))
+    return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
+
+
+def selftest_l2_classify(r: L2Result, sms: List[L2Sm], faults: List[L2Fault]) -> Tuple[L2Result, List[L2Sm], List[L2Fault]]:
+    """cro_selftest_l2_classify: the L2 probe's classification of the given counts and records, on copies."""
+    out = L2Result.from_buffer_copy(r)
+    s = (L2Sm * max(1, len(sms)))(*sms)
+    f = (L2Fault * max(1, len(faults)))(*faults)
+    rc = lib.cro_selftest_l2_classify(ctypes.byref(out), s, len(sms), f, len(faults))
+    if rc != OK:
+        raise ProbeError(rc, "cro_selftest_l2_classify")
+    return out, list(s[:len(sms)]), list(f[:len(faults)])
 
 
 def _sram_opts(legs: int, iterations: int, cluster: int, max_rounds: int, deadline_ms: int,
@@ -1174,6 +1314,23 @@ class ProbeContext:
         n_sms, n = ctypes.c_int(), ctypes.c_int()
         self._check(lib.cro_probe_sram(self.handle, dev, ctypes.byref(o), ctypes.byref(r), sms, SRAM_MAX_SMS, ctypes.byref(n_sms),
                                        arr, cap, ctypes.byref(n)), allow=(ERR_CHECKSUM, ERR_CUDA))
+        return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
+
+    def probe_l2(self, dev: int = 0, bytes: int = 0, iterations: int = 0, a1_counters: int = 0, a2_counters: int = 0,
+                 inject: Optional[Tuple[int, int, int, int, int, int]] = None,
+                 cap: int = 256) -> Tuple[L2Result, List[L2Sm], List[L2Fault]]:
+        """cro_probe_l2: March C- over an L2-resident buffer of `bytes` whose blocks change SM from element to element,
+        and the L2 atomic units' A1 (red.add / red.xor) and A2 (atom.add tickets) legs.  0: the defaults.
+        inject = (leg, sm, element, iteration, word, mask) is the test-only stand-in for a fault (L2_MARCH: sm, element,
+        word -1 for every one; L2_A1 / L2_A2: word is the counter).  Returns the result (its status is OK,
+        ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up to `cap` word records."""
+        o = _l2_opts(bytes, iterations, a1_counters, a2_counters, 0, inject)
+        r = L2Result()
+        sms = (L2Sm * L2_MAX_SMS)()
+        arr = (L2Fault * max(1, cap))()
+        n_sms, n = ctypes.c_int(), ctypes.c_int()
+        self._check(lib.cro_probe_l2(self.handle, dev, ctypes.byref(o), ctypes.byref(r), sms, L2_MAX_SMS, ctypes.byref(n_sms),
+                                     arr, cap, ctypes.byref(n)), allow=(ERR_CHECKSUM, ERR_CUDA))
         return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
 
     def launch_count(self) -> int:

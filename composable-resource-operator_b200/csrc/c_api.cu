@@ -73,6 +73,11 @@ static_assert(sizeof(cro_sram_result) == 568 && offsetof(cro_sram_result, bad_sm
                   offsetof(cro_sram_result, recorded) == 160 && offsetof(cro_sram_result, before) == 184 &&
                   offsetof(cro_sram_result, leg) == 232,
               "sram layout");
+static_assert(sizeof(cro_l2_opts) == 56 && sizeof(cro_l2_health) == 48 && sizeof(cro_l2_sm) == 128 && sizeof(cro_l2_fault) == 56 &&
+                  sizeof(cro_l2_result) == 616 && offsetof(cro_l2_result, mismatches) == 80 &&
+                  offsetof(cro_l2_result, bad_line) == 184 && offsetof(cro_l2_result, a1_bad) == 312 &&
+                  offsetof(cro_l2_result, element_ns) == 400 && offsetof(cro_l2_result, before) == 520,
+              "l2 layout");
 static_assert(sizeof(cro_selftest_sweep_opts) == 128 && offsetof(cro_selftest_sweep_opts, force_or) == 104 &&
                   sizeof(cro_selftest_sweep_out) == 168 && offsetof(cro_selftest_sweep_out, mismatches) == 128,
               "selftest sweep layout");
@@ -460,6 +465,53 @@ int cro_probe_sram_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_sram_opts*
 int cro_read_sram_health(const char* gpu_uuid, cro_sram_health* out) try {
     if (!gpu_uuid || !out) return CRO_ERR_INVALID_ARG;
     identity::NvmlSramHealth(gpu_uuid, true, out);
+    return CRO_OK;
+} CRO_API_CATCH
+// The L2 probe's two forms share the copy-out: sms[0 .. sms_cap) and faults[0 .. cap), and what was written in
+// sms_listed and recorded.
+static int l2_out(int rc, const std::vector<cro_l2_sm>& seen, const std::vector<cro_l2_fault>& found, cro_l2_result* out,
+                  cro_l2_sm* sms, int sms_cap, int* n_sms, cro_l2_fault* faults, int cap, int* n) {
+    const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
+    for (size_t j = 0; j < ks; ++j) sms[j] = seen[j];
+    for (size_t j = 0; j < kf; ++j) faults[j] = found[j];
+    out->sms_listed = (uint32_t)ks;
+    out->recorded = kf;
+    *n_sms = (int)ks;
+    *n = (int)kf;
+    return rc;
+}
+int cro_probe_l2(cro_ctx* ctx, int i, const cro_l2_opts* opts, cro_l2_result* out, cro_l2_sm* sms, int sms_cap, int* n_sms,
+                 cro_l2_fault* faults, int cap, int* n) try {
+    if (!ctx || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
+        return CRO_ERR_INVALID_ARG;
+    *n = *n_sms = 0;
+    cro_l2_opts o{};
+    if (opts) o = *opts;
+    std::vector<cro_l2_sm> seen;
+    std::vector<cro_l2_fault> found;
+    const int rc = ctx_probe_l2(ctx, i, o, out, &seen, &found);
+    return l2_out(rc, seen, found, out, sms, sms_cap, n_sms, faults, cap, n);
+} CRO_API_CATCH
+int cro_probe_l2_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_l2_opts* opts, cro_l2_result* out, cro_l2_sm* sms,
+                      int sms_cap, int* n_sms, cro_l2_fault* faults, int cap, int* n) try {
+    if (!gpu_uuid || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
+        return CRO_ERR_INVALID_ARG;
+    *n = *n_sms = 0;
+    cro_l2_opts o{};
+    if (opts) o = *opts;
+    std::vector<cro_l2_sm> seen;
+    std::vector<cro_l2_fault> found;
+    const int rc = ctx_probe_l2_uuid(ctx, gpu_uuid, o, out, &seen, &found, cap);
+    return l2_out(rc, seen, found, out, sms, sms_cap, n_sms, faults, cap, n);
+} CRO_API_CATCH
+int cro_read_l2_health(const char* gpu_uuid, cro_l2_health* out) try {
+    if (!gpu_uuid || !out) return CRO_ERR_INVALID_ARG;
+    identity::NvmlL2Health(gpu_uuid, true, out);
+    return CRO_OK;
+} CRO_API_CATCH
+int cro_selftest_l2_classify(cro_l2_result* r, cro_l2_sm* sms, int n_sms, cro_l2_fault* faults, int n) try {
+    if (!r || n_sms < 0 || n < 0 || (n_sms > 0 && !sms) || (n > 0 && !faults)) return CRO_ERR_INVALID_ARG;
+    l2_classify(r, sms, (size_t)n_sms, faults, (size_t)n);
     return CRO_OK;
 } CRO_API_CATCH
 int cro_compute_expected(int answer, uint64_t seed, int32_t* out) try {
@@ -860,6 +912,41 @@ int cro_emit_sram_annotations_json(const cro_sram_result* r, char* buf, size_t c
     const cro_sram_health &B = r->before, &A = r->after;
     if (B.nvml & A.nvml & CRO_SRAM_NVML_ECC_CORRECTED) m[p + "ecc-corrected"] = std::to_string(A.ecc_corrected - B.ecc_corrected);
     if (B.nvml & A.nvml & CRO_SRAM_NVML_ECC_UNCORRECTED) m[p + "ecc-uncorrected"] = std::to_string(A.ecc_uncorrected - B.ecc_uncorrected);
+    gojson::Writer w;
+    w.string_map(m);
+    return copy_out(w.str(), buf, cap, len);
+} CRO_API_CATCH
+
+int cro_emit_l2_annotations_json(const cro_l2_result* r, char* buf, size_t cap, size_t* len) try {
+    if (!r) return CRO_ERR_INVALID_ARG;
+    static const char* const kHealth[6] = {"sram-corrected", "sram-uncorrected", "l2-corrected", "l2-uncorrected",
+                                           "threshold-exceeded", "l2-bucket"};
+    static const char* const kVerdict[5] = {"", "sm", "line", "atomic", "all"};
+    std::map<std::string, std::string> m;
+    const std::string p = "cohdi.io/probe-l2-";
+    m[p + "verdict"] = r->status == CRO_OK                                                           ? "ok"
+                       : r->status == CRO_ERR_CHECKSUM && r->verdict >= 1 && r->verdict <= CRO_L2_ALL ? kVerdict[r->verdict]
+                       : r->status == CRO_ERR_CUDA ? "cuda-error:" + std::to_string(r->cuda_error)
+                                                   : "error";
+    m[p + "sms"] = std::to_string(r->sms_covered) + "/" + std::to_string(r->sm_count);
+    m[p + "bytes"] = std::to_string(r->bytes);
+    m[p + "iterations"] = std::to_string(r->iterations);
+    m[p + "march-gbs"] = std::to_string(r->march_ns ? r->march_bytes / r->march_ns : 0ull);
+    auto list = [](const auto* v, uint64_t n) {
+        std::string s;
+        for (uint64_t j = 0; j < n; ++j) s += (j ? "," : "") + std::to_string(v[j]);
+        return s;
+    };
+    if (r->bad_sms) m[p + "bad-sms"] = list(r->bad_sm, std::min<uint64_t>(r->bad_sms, 16));
+    if (r->bad_lines) m[p + "bad-lines"] = list(r->bad_line, std::min<uint64_t>(r->bad_lines, CRO_L2_MAX_LINES));
+    if (r->a1_bad) m[p + "a1-bad-counters"] = list(r->a1_bad_counter, std::min<uint64_t>(r->a1_bad, CRO_L2_MAX_COUNTERS));
+    if (r->a2_bad) m[p + "a2-bad-counters"] = list(r->a2_bad_counter, std::min<uint64_t>(r->a2_bad, CRO_L2_MAX_COUNTERS));
+    if (r->a2_holes) m[p + "a2-holes"] = std::to_string(r->a2_holes);
+    if (r->overflow) m[p + "overflow"] = "1";
+    std::string health;
+    for (int b = 0; b < 6; ++b)
+        if (r->health >> b & 1u) health += (health.empty() ? "" : ",") + std::string(kHealth[b]);
+    if (!health.empty()) m[p + "health"] = health;
     gojson::Writer w;
     w.string_map(m);
     return copy_out(w.str(), buf, cap, len);

@@ -531,5 +531,31 @@ void NvmlSramHealth(const std::string& gpu_uuid, bool status, cro_sram_health* o
     }
 }
 
+void NvmlL2Health(const std::string& gpu_uuid, bool status, cro_l2_health* out) {
+    memset(out, 0, sizeof *out);
+    const NvmlSession& s = nvml_session();
+    nvmlDevice_t dev = nullptr;
+    if (!nvml_device(s, gpu_uuid, &dev)) return;
+    if (s.memErrors) {
+        // NVML_MEMORY_ERROR_TYPE_CORRECTED 0 / _UNCORRECTED 1, NVML_VOLATILE_ECC 0, NVML_MEMORY_LOCATION_SRAM 7 and
+        // NVML_MEMORY_LOCATION_L2_CACHE 1 (which a Hopper driver may refuse: its L2 errors are counted as SRAM's)
+        unsigned long long v = 0;
+        if (s.memErrors(dev, 0, 0, 7, &v) == 0) { out->sram_corrected = v; out->nvml |= CRO_L2_NVML_SRAM_CORRECTED; }
+        v = 0;
+        if (s.memErrors(dev, 1, 0, 7, &v) == 0) { out->sram_uncorrected = v; out->nvml |= CRO_L2_NVML_SRAM_UNCORRECTED; }
+        v = 0;
+        if (s.memErrors(dev, 0, 0, 1, &v) == 0) { out->l2_corrected = v; out->nvml |= CRO_L2_NVML_L2_CORRECTED; }
+        v = 0;
+        if (s.memErrors(dev, 1, 0, 1, &v) == 0) { out->l2_uncorrected = v; out->nvml |= CRO_L2_NVML_L2_UNCORRECTED; }
+    }
+    NvmlSramStatus st{};
+    st.version = kNvmlSramStatusV1;
+    if (status && s.sramStatus && s.sramStatus(dev, &st) == 0) {
+        out->threshold_exceeded = st.bThresholdExceeded ? 1u : 0u;
+        out->unc_bucket_l2 = st.aggregateUncBucketL2;
+        out->nvml |= CRO_L2_NVML_STATUS;
+    }
+}
+
 }  // namespace identity
 }  // namespace cro

@@ -96,6 +96,10 @@ void NvmlHbmHealth(const std::string& gpu_uuid, bool histogram, cro_hbm_health* 
 // field-diag threshold flag of nvmlDeviceGetSramEccErrorStatus (looked up by name: older drivers lack it).
 // out->nvml has a CRO_SRAM_NVML_* bit per read NVML answered.
 void NvmlSramHealth(const std::string& gpu_uuid, bool status, cro_sram_health* out);
+// The record the L2 probe reads: volatile SRAM and L2 ECC counts (nvmlDeviceGetMemoryErrorCounter, locations 7 and 1)
+// and, with `status`, nvmlDeviceGetSramEccErrorStatus's threshold flag and aggregate uncorrectable L2 bucket.
+// out->nvml has a CRO_L2_NVML_* bit per read NVML answered.
+void NvmlL2Health(const std::string& gpu_uuid, bool status, cro_l2_health* out);
 
 }  // namespace identity
 }  // namespace cro

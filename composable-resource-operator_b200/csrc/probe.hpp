@@ -78,6 +78,7 @@ struct Device {
     uint64_t link_calls = 0;               // k of the next host link probe call: its seeds
     uint64_t compute_calls = 0;            // k of the next compute probe call (ctx_probe_compute): its operand seed
     uint64_t sram_calls = 0;               // k of the next SRAM probe call (ctx_probe_sram): its seeds
+    uint64_t l2_calls = 0;                 // k of the next L2 probe call (ctx_probe_l2): its seeds
     KernelPlan plan{};
     SweepScratch scratch{}, scratch_aux{}, scratch_pfx{};   // main stream / closed form / p2p prefix closed form
     // lane 0's buffers under their old names: the synchronous probe, the single sweeps and cro_probe_all use lane 0
@@ -263,6 +264,29 @@ int ctx_probe_sram_uuid(cro_ctx* c, const char* uuid, const cro_sram_opts& o, cr
                         std::vector<cro_sram_fault>* faults, int cap);
 // CRO_SRAM_HEALTH_* of the NVML reads before the first leg and after the last.
 uint32_t sram_health(const cro_sram_health& before, const cro_sram_health& after);
+
+// L2 probe (include/croprobe.h, cro_probe_l2, l2_probe.cu): *sms gets one entry per SM seen, by SM id; *faults every
+// recorded word, by (word, iteration, element, smid).
+int ctx_probe_l2(cro_ctx* c, int idx, const cro_l2_opts& o, cro_l2_result* r, std::vector<cro_l2_sm>* sms,
+                 std::vector<cro_l2_fault>* faults);
+// The uuid form runs `croprobe-cli l2-raw` with a fresh seed base (helper_seed_base) and asks it for at most cap words.
+int ctx_probe_l2_uuid(cro_ctx* c, const char* uuid, const cro_l2_opts& o, cro_l2_result* r, std::vector<cro_l2_sm>* sms,
+                      std::vector<cro_l2_fault>* faults, int cap);
+// The options with their defaults filled in.
+struct L2Settings {
+    uint64_t bytes;
+    uint32_t iterations, a1, a2;
+};
+// Checks a call's options against a device whose L2 holds l2_size bytes (0: not known here, W's upper bound is left to
+// the helper), filling *p; false with *why set when they are refused.  Both forms call it before anything is launched
+// or spawned; `helper` says which (only the helper form takes a deadline).
+bool l2_check_args(const cro_l2_opts& o, uint64_t l2_size, bool helper, L2Settings* p, std::string* why);
+// The rotation step of G CTAs (0: G < 5, no step puts M1 .. M5 of a word on five CTAs).
+uint32_t l2_delta(uint32_t G);
+// CRO_L2_HEALTH_* of the NVML reads before and after the call.
+uint32_t l2_health(const cro_l2_health& before, const cro_l2_health& after);
+// The verdict, bad SMs and lines, marks and line flags of a call's counts and records (cro_selftest_l2_classify).
+void l2_classify(cro_l2_result* r, cro_l2_sm* sms, size_t n_sms, cro_l2_fault* faults, size_t n);
 
 // test hooks (include/croprobe.h, cro_selftest_*): the verdict kernels and the chase on caller-given inputs
 int ctx_selftest_probe_finalize(cro_ctx* c, int idx, const cro_probe_result* tmpl, const cro_sweep_slot* slots,

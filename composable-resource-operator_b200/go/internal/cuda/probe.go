@@ -669,6 +669,115 @@ func (c *Context) ProbeSRAM(deviceID string) (SRAMResult, error) {
 	return sramResult(&res, faults[:], got), nil
 }
 
+// L2Result is the summary of cro_l2_result an operator reads: whether the
+// L2-resident buffer held what each SM wrote when another SM read it back,
+// whether the L2 atomic units gave the right answers, which SMs, buffer offsets
+// or counters did not, and the SRAM / L2 ECC record from NVML.
+type L2Result struct {
+	Status        int32  // CRO_OK, CRO_ERR_CHECKSUM or CRO_ERR_CUDA
+	CudaError     int32  // cudaError_t of a failed launch (CRO_ERR_CUDA)
+	Verdict       uint32 // CRO_L2_NONE / _SM / _LINE / _ATOMIC / _ALL
+	Health        uint32 // CRO_L2_HEALTH_* bits; never change Status
+	SMCount       uint32
+	Covered       uint32 // SMs that read words of the buffer
+	Bytes         uint64 // W
+	Overflow      bool   // more mismatches than records kept; counts stay exact
+	BadSMs        []uint32
+	BadLines      []uint64 // byte offsets into the call's buffer (at most 8)
+	A1BadCounters []uint32
+	A2BadCounters []uint32
+	A2Holes       uint64
+	Faults        []L2Fault
+	Annotations   string // Go-marshalled map[string]string of cohdi.io/probe-l2-* keys
+}
+
+// L2Fault is one failed compare (cro_l2_fault).
+type L2Fault struct {
+	Element, Iteration, SM, CTA, WriterCTA, WriterSM uint32
+	Word, Expected, Actual                           uint64
+	Line                                             bool
+}
+
+func l2Result(res *C.cro_l2_result, faults []C.cro_l2_fault, got C.int) L2Result {
+	out := L2Result{Status: int32(res.status), CudaError: int32(res.cuda_error), Verdict: uint32(res.verdict),
+		Health: uint32(res.health), SMCount: uint32(res.sm_count), Covered: uint32(res.sms_covered),
+		Bytes: uint64(res.bytes), Overflow: res.overflow != 0, A2Holes: uint64(res.a2_holes)}
+	for i := 0; i < int(res.bad_sms) && i < 16; i++ {
+		out.BadSMs = append(out.BadSMs, uint32(res.bad_sm[i]))
+	}
+	for i := 0; i < int(res.bad_lines) && i < int(C.CRO_L2_MAX_LINES); i++ {
+		out.BadLines = append(out.BadLines, uint64(res.bad_line[i]))
+	}
+	for i := 0; i < int(res.a1_bad) && i < int(C.CRO_L2_MAX_COUNTERS); i++ {
+		out.A1BadCounters = append(out.A1BadCounters, uint32(res.a1_bad_counter[i]))
+	}
+	for i := 0; i < int(res.a2_bad) && i < int(C.CRO_L2_MAX_COUNTERS); i++ {
+		out.A2BadCounters = append(out.A2BadCounters, uint32(res.a2_bad_counter[i]))
+	}
+	for i := 0; i < int(got); i++ {
+		f := faults[i]
+		out.Faults = append(out.Faults, L2Fault{uint32(f.element), uint32(f.iteration), uint32(f.smid), uint32(f.cta),
+			uint32(f.writer_cta), uint32(f.writer_smid), uint64(f.word), uint64(f.expected), uint64(f.actual), f.line != 0})
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_l2_annotations_json(res, buf, 4096, &ln) == C.CRO_OK {
+		out.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return out
+}
+
+// ProbeL2ByUUID runs cro_probe_l2_uuid with its defaults: the L2 probe of any
+// GPU on the node through the helper process, the form to call on a freshly
+// composed GPU (INTEGRATION.md "The L2 probe").  A mismatch or a fault
+// (CRO_ERR_CUDA) is a result, not an error; found is false when the node does
+// not list the GPU.
+func (c *Context) ProbeL2ByUUID(deviceID string) (r L2Result, found bool, err error) {
+	id := C.CString(deviceID)
+	defer C.free(unsafe.Pointer(id))
+	var res C.cro_l2_result
+	sms := make([]C.cro_l2_sm, C.CRO_L2_MAX_SMS)
+	var faults [256]C.cro_l2_fault
+	var nSMs, got C.int
+	rc := C.cro_probe_l2_uuid(c.h, id, nil, &res, &sms[0], C.CRO_L2_MAX_SMS, &nSMs, &faults[0], 256, &got)
+	if rc == C.CRO_ERR_NO_DEVICE {
+		return r, false, nil
+	}
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM && rc != C.CRO_ERR_CUDA {
+		return r, true, errorOf(c.h, rc)
+	}
+	return l2Result(&res, faults[:], got), true, nil
+}
+
+// ProbeL2 runs cro_probe_l2 with its defaults on the in-process device whose
+// UUID is deviceID.  ProbeL2ByUUID is the form an operator should call.
+func (c *Context) ProbeL2(deviceID string) (L2Result, error) {
+	var devs [C.CRO_MAX_DEVICES]C.cro_dev_info
+	var n C.int
+	if rc := C.cro_enumerate(c.h, &devs[0], C.CRO_MAX_DEVICES, &n); rc != C.CRO_OK {
+		return L2Result{}, errorOf(c.h, rc)
+	}
+	idx := C.int(-1)
+	for i := 0; i < int(n); i++ {
+		if C.GoString(&devs[i].gpu_uuid[0]) == deviceID && devs[i].flags&C.CRO_DEV_IN_PROCESS != 0 {
+			idx = C.int(devs[i].dev_index)
+		}
+	}
+	if idx < 0 {
+		return L2Result{}, fmt.Errorf("cuda l2 probe: %s is not a device of this context", deviceID)
+	}
+	var res C.cro_l2_result
+	sms := make([]C.cro_l2_sm, C.CRO_L2_MAX_SMS)
+	var faults [256]C.cro_l2_fault
+	var nSMs, got C.int
+	rc := C.cro_probe_l2(c.h, idx, nil, &res, &sms[0], C.CRO_L2_MAX_SMS, &nSMs, &faults[0], 256, &got)
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM && rc != C.CRO_ERR_CUDA {
+		return L2Result{}, errorOf(c.h, rc)
+	}
+	return l2Result(&res, faults[:], got), nil
+}
+
 // MetricsText is the Prometheus text exposition of the context's counters and
 // per-GPU gauges; a prometheus.Collector registered with
 // sigs.k8s.io/controller-runtime/pkg/metrics.Registry (cmd/main.go:66,119-125

@@ -1158,6 +1158,225 @@ int  cro_probe_sram_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_sram_opts
  * NULL argument. */
 int  cro_read_sram_health(const char *gpu_uuid, cro_sram_health *out);
 
+/* ---- L2: the L2 cache, the crossbar between the SMs and its slices, and the L2 atomic units ---- */
+
+/*
+ * The probe's sweeps stream through the L2 once under evict-first hints, and no kernel reads back on purpose what
+ * another SM wrote, so an L2 or crossbar fault either shows as an HBM fault or not at all.  The L2 probe keeps a buffer
+ * of `bytes` (W) resident in the L2 and marches it from SM to SM, then checks the L2's atomic units against answers
+ * computed without atomics.
+ *
+ * March: one CTA per SM (G = sm_count CTAs, forced by the kernel's shared-memory request) over the buffer's 64-bit
+ * words, cut into blocks of CRO_L2_BLOCK_BYTES.  Each iteration runs March C- with P(w) = pattern_word(seed, w) and
+ * Q(w) = ~P(w):
+ *   M0 write P;  M1 ascending: read P, write Q;  M2 ascending: read Q, write P;
+ *   M3 descending: read P, write Q;  M4 descending: read Q, write P;  M5 read P
+ * and each element is its own launch: the stream orders the elements, no kernel waits for another CTA.  Block b is
+ * handled in element e by CTA (b + e * delta) mod G, with delta chosen so that M1 .. M5 of one word run on five
+ * different CTAs: every word is written by one CTA and read back by another, through the L2 and the crossbar.  Every
+ * access is a 128-bit ld/st.relaxed.gpu with an L2::evict_last cache policy: L1 is bypassed, the persisting-L2
+ * set-aside is not touched.  Every read is compared (mismatches counted exactly per element and per CTA, recorded up to
+ * CRO_L2_RECORDS a call with the reader's %smid and the CTA that wrote the word); M5's reads are also folded (xor, sum,
+ * sum of v * (2w + 1) by global word index) and the CTAs' folds, combined, must equal the closed form once per
+ * iteration.  Each CTA publishes a record per launch (the call number, %smid, %globaltimer window, counts); a CTA that
+ * did not publish fails the call.
+ *
+ * Atomics: A1, every CTA j adds (red.add.u64) and xors (red.xor.b64) pattern_word(seed_atomic, j * n + i) into
+ * counter i < a1_counters; a checker kernel without atomics recomputes every counter's sum and xor.  A2, for each of
+ * a2_counters counters on its own 128-byte line, one warp of every CTA takes atom.add.u32 tickets and stores what it
+ * got back; the checker marks each ticket present and counts holes (a duplicate or wrong ticket leaves one), and
+ * checks the final value is 32 * G.
+ *
+ * Seeds: call k on a device uses seed = seed_dev + 2^59 + 2k * 0xD1B54A32D192ED03 for the march and the next stride
+ * for the atomics.  Runs only when called: it takes the device's mutex, lets probes in flight finish first (their
+ * results stay collectable), allocates its buffers per call and never touches the sweep region.
+ *
+ * Verdict: a word seen wrong by two or more reader SMs is a line fault (the storage at that offset: the L2 line or the
+ * HBM behind it, which the probe cannot tell apart); a word seen wrong by one SM is that reader's fault.  CRO_L2_ALL
+ * when a CTA did not publish, every SM that read in an element where a read went wrong saw a wrong word, or the
+ * fold failed with every compare passing;
+ * else CRO_L2_LINE when there are line faults; else CRO_L2_SM; else CRO_L2_ATOMIC when only A1 or A2 failed.  When
+ * more mismatches happened than were recorded (overflow), the line / SM split rests on the records kept; the counts
+ * stay exact.  status: CRO_ERR_CHECKSUM for any verdict but CRO_L2_NONE; CRO_ERR_CUDA when a launch failed
+ * (cuda_error holds the cudaError_t).  The NVML health read before and after never changes the status.
+ */
+#define CRO_L2_BLOCK_BYTES        16384u  /* W is a multiple of this                                         */
+#define CRO_L2_MIN_BYTES          (1u << 20)
+#define CRO_L2_MAX_L2_MULTIPLE    8       /* W is at most 8 times cudaDevAttrL2CacheSize                     */
+#define CRO_L2_ELEMENTS           6       /* per-element counts: M0 .. M5                                     */
+#define CRO_L2_RECORDS            4096    /* word records a call keeps; counts stay exact beyond             */
+#define CRO_L2_MAX_SMS            256     /* SM ids the results hold; a larger %nsmid fails the call          */
+#define CRO_L2_MAX_ITERATIONS     256
+#define CRO_L2_MAX_A1_COUNTERS    (1u << 20)
+#define CRO_L2_MAX_A2_COUNTERS    8192
+#define CRO_L2_MAX_LINES          8       /* line offsets listed in the result                               */
+#define CRO_L2_MAX_COUNTERS       8       /* bad counters listed per atomic leg                              */
+
+#define CRO_L2_MARCH              0       /* cro_l2_opts.test_inject_leg */
+#define CRO_L2_A1                 1
+#define CRO_L2_A2                 2
+
+#define CRO_L2_NONE               0u      /* nothing failed                                                  */
+#define CRO_L2_SM                 1u      /* a strict subset of the covered SMs read words wrong, no line fault */
+#define CRO_L2_LINE               2u      /* words seen wrong by two or more SMs                              */
+#define CRO_L2_ATOMIC             3u      /* only A1 or A2 failed                                             */
+#define CRO_L2_ALL                4u      /* a CTA did not publish, every reader of a failing element failed, or only the fold did */
+
+#define CRO_L2_PERSISTENT         1u      /* cro_l2_sm.mark: the SM's compares failed in the last iteration    */
+#define CRO_L2_INTERMITTENT       2u      /* ... only in an earlier one                                        */
+
+/* cro_l2_result.health: reported, never changes the status */
+#define CRO_L2_HEALTH_SRAM_CORRECTED_DURING    0x1u   /* volatile SRAM corrected count rose during the call          */
+#define CRO_L2_HEALTH_SRAM_UNCORRECTED_DURING  0x2u
+#define CRO_L2_HEALTH_L2_CORRECTED_DURING      0x4u   /* volatile L2 corrected count rose (NVML may never answer)    */
+#define CRO_L2_HEALTH_L2_UNCORRECTED_DURING    0x8u
+#define CRO_L2_HEALTH_THRESHOLD_EXCEEDED       0x10u  /* NVML's SRAM error status: the field-diag threshold           */
+#define CRO_L2_HEALTH_L2_BUCKET                0x20u  /* ... and its aggregate uncorrectable L2 bucket is not 0       */
+
+/* cro_l2_health.nvml: which reads NVML answered (a field NVML refused stays 0) */
+#define CRO_L2_NVML_SRAM_CORRECTED    0x1u    /* nvmlDeviceGetMemoryErrorCounter, volatile, SRAM (location 7)     */
+#define CRO_L2_NVML_SRAM_UNCORRECTED  0x2u
+#define CRO_L2_NVML_L2_CORRECTED      0x4u    /* ... L2 cache (location 1)                                        */
+#define CRO_L2_NVML_L2_UNCORRECTED    0x8u
+#define CRO_L2_NVML_STATUS            0x10u   /* nvmlDeviceGetSramEccErrorStatus (absent from older drivers)       */
+
+typedef struct cro_l2_opts {
+    uint64_t bytes;                /*   0  W: 0 = the default (DESIGN.md), else a multiple of CRO_L2_BLOCK_BYTES in
+                                              [CRO_L2_MIN_BYTES, 8 * the device's L2 size]                       */
+    uint32_t iterations;           /*   8  0 = the default, at most CRO_L2_MAX_ITERATIONS                          */
+    uint32_t a1_counters;          /*  12  0 = 65536, at most CRO_L2_MAX_A1_COUNTERS                               */
+    uint32_t a2_counters;          /*  16  0 = 1024, at most CRO_L2_MAX_A2_COUNTERS                                */
+    int32_t  deadline_ms;          /*  20  cro_probe_l2_uuid: the helper's deadline; 0 = CRO_HELPER_TIMEOUT_MS.
+                                              cro_probe_l2 waits for the stream as every in-process probe does
+                                              (cro_opts.deadline_ms) and refuses a value other than 0          */
+    /* test only: with test_inject_mask != 0.  Leg CRO_L2_MARCH: in each CTA whose %smid is test_inject_sm (-1: every
+       SM), the mask is XORed into the value read of word test_inject_word (-1: every word) in element
+       test_inject_element (1 .. 5; -1: every reading element) of iteration test_inject_iteration.  CRO_L2_A1: CTA 0's
+       contribution to counter test_inject_word is XORed with the mask.  CRO_L2_A2: the ticket lane 0 of CTA 0 stores
+       for counter test_inject_word is XORed with the mask's low 32 bits (a mask whose low 32 bits are 0 is refused).
+       A software stand-in: nothing is provoked in the hardware. */
+    int32_t  test_inject_leg;      /*  24 */
+    int32_t  test_inject_sm;       /*  28 */
+    int32_t  test_inject_element;  /*  32 */
+    uint32_t test_inject_iteration;/*  36 */
+    int64_t  test_inject_word;     /*  40 */
+    uint64_t test_inject_mask;     /*  48 */
+} cro_l2_opts;                     /*  56 bytes */
+
+typedef struct cro_l2_health {
+    uint32_t nvml;                 /*   0  CRO_L2_NVML_* of the reads NVML answered                               */
+    uint32_t threshold_exceeded;   /*   4  nvmlEccSramErrorStatus_t.bThresholdExceeded (after the call only)       */
+    uint64_t sram_corrected;       /*   8  volatile SRAM ECC counts                                               */
+    uint64_t sram_uncorrected;     /*  16 */
+    uint64_t l2_corrected;         /*  24  volatile L2 ECC counts                                                 */
+    uint64_t l2_uncorrected;       /*  32 */
+    uint64_t unc_bucket_l2;        /*  40  nvmlEccSramErrorStatus_t.aggregateUncBucketL2 (after the call only)     */
+} cro_l2_health;                   /*  48 bytes */
+
+typedef struct cro_l2_result {
+    int32_t  status;               /*   0  the return value                                                      */
+    uint32_t verdict;              /*   4  CRO_L2_NONE / _SM / _LINE / _ATOMIC / _ALL                            */
+    uint64_t seed;                 /*   8  the march's seed                                                      */
+    uint64_t seed_atomic;          /*  16  A1's seed                                                             */
+    uint64_t call;                 /*  24  k: the call's number on this device, from 0                          */
+    uint64_t bytes;                /*  32  W                                                                     */
+    uint32_t sm_count;             /*  40  multiprocessors the device reports                                    */
+    uint32_t nsmid;                /*  44  %nsmid as the kernels read it                                        */
+    uint32_t ctas;                 /*  48  G: CTAs per launch                                                    */
+    uint32_t blocks;               /*  52  W / CRO_L2_BLOCK_BYTES                                                */
+    uint32_t delta;                /*  56  the rotation step between elements                                    */
+    uint32_t iterations;           /*  60 */
+    int32_t  cuda_error;           /*  64  cudaError_t of the launch that failed; 0: none                        */
+    uint32_t health;               /*  68  CRO_L2_HEALTH_*                                                      */
+    uint32_t sms_covered;          /*  72  distinct SMs that read words of the buffer (a CTA that owns no block in
+                                              an element reads nothing there)                                  */
+    uint32_t unpublished;          /*  76  march CTAs (over all launches) and checker CTAs that published nothing */
+    uint64_t mismatches[CRO_L2_ELEMENTS];    /*  80  per element, exact                                         */
+    uint64_t recorded;             /* 128  word records written to the caller's list (*n)                       */
+    uint32_t overflow;             /* 136  1: more mismatches than the device kept records of                   */
+    uint32_t sms_listed;           /* 140  entries written to the caller's per-SM list                          */
+    uint32_t bad_sms;              /* 144  distinct SMs with a word only they saw wrong                         */
+    uint32_t bad_lines;            /* 148  distinct words seen wrong by two or more SMs                          */
+    uint16_t bad_sm[16];           /* 152  the first 16 bad SMs, ascending                                      */
+    uint64_t bad_line[CRO_L2_MAX_LINES];     /* 184  byte offsets of the first line faults in this call's buffer   */
+    uint64_t fold_xor;             /* 248  M5 fold of every CTA over every iteration                             */
+    uint64_t fold_sum;             /* 256 */
+    uint64_t fold_wsum;            /* 264 */
+    uint64_t expect_xor;           /* 272  iterations x the closed form of pattern_word(seed, 0 .. W / 8)         */
+    uint64_t expect_sum;           /* 280 */
+    uint64_t expect_wsum;          /* 288 */
+    uint32_t fold_ok;              /* 296  1: the fold equals the closed form                                   */
+    uint32_t a1_counters;          /* 300 */
+    uint32_t a2_counters;          /* 304 */
+    uint32_t a2_tickets;           /* 308  32 * G: what every A2 counter must end at                             */
+    uint64_t a1_bad;               /* 312  A1 counters whose sum or xor differs                                  */
+    uint64_t a2_holes;             /* 320  tickets missing over all A2 counters                                  */
+    uint64_t a2_bad;               /* 328  A2 counters with a hole or a wrong final value                        */
+    uint32_t a1_bad_counter[CRO_L2_MAX_COUNTERS];   /* 336  the first of them, ascending                          */
+    uint32_t a2_bad_counter[CRO_L2_MAX_COUNTERS];   /* 368 */
+    uint64_t element_ns[CRO_L2_ELEMENTS];    /* 400  %globaltimer: first CTA start .. last CTA end, per element,
+                                                       summed over iterations                                 */
+    uint64_t march_ns;             /* 448  CUDA events around the march's launches                               */
+    uint64_t march_bytes;          /* 456  bytes read and written by the march                                   */
+    uint64_t a1_ns;                /* 464  CUDA events: A1's kernel, its checker, A2's kernel, its checker         */
+    uint64_t a1_check_ns;          /* 472 */
+    uint64_t a2_ns;                /* 480 */
+    uint64_t a2_check_ns;          /* 488 */
+    uint64_t l2_bytes;             /* 496  cudaDevAttrL2CacheSize                                                */
+    uint64_t wall_ns;              /* 504  the whole call                                                       */
+    uint64_t helper_ns;            /* 512  0 in process                                                         */
+    cro_l2_health before;          /* 520  read before the first launch                                         */
+    cro_l2_health after;           /* 568  read after the last (with the SRAM error status)                      */
+} cro_l2_result;                   /* 616 bytes */
+
+typedef struct cro_l2_sm {
+    uint32_t smid;                 /*   0 */
+    uint32_t mark;                 /*   4  0, CRO_L2_PERSISTENT or CRO_L2_INTERMITTENT (bad SMs only)           */
+    uint32_t launches;             /*   8  march CTAs that ran on this SM                                       */
+    uint32_t reserved;             /*  12 */
+    uint64_t mismatches[CRO_L2_ELEMENTS];    /*  16  reads this SM saw wrong, per element                       */
+    uint64_t last;                 /*  64  ... of them in the last iteration                                    */
+    uint64_t words_read[CRO_L2_ELEMENTS];    /*  72  words this SM read, per element, by the rotation              */
+    uint64_t ns;                   /* 120  %globaltimer windows of its CTAs, summed                             */
+} cro_l2_sm;                       /* 128 bytes */
+
+typedef struct cro_l2_fault {
+    uint32_t element;              /*   0  1 .. 5 */
+    uint32_t iteration;            /*   4 */
+    uint32_t smid;                 /*   8  the reader                                                           */
+    uint32_t cta;                  /*  12  the reader's CTA                                                      */
+    uint32_t writer_cta;           /*  16  the CTA that wrote the word in the element before                     */
+    uint32_t writer_smid;          /*  20  its SM, from its published record (0xFFFFFFFF: it did not publish)    */
+    uint64_t word;                 /*  24  word index in this call's buffer (byte offset / 8)                    */
+    uint64_t expected;             /*  32 */
+    uint64_t actual;               /*  40 */
+    uint32_t line;                 /*  48  1: the word was seen wrong by two or more SMs                         */
+    uint32_t reserved;             /*  52 */
+} cro_l2_fault;                    /*  56 bytes */
+
+/* sms[0 .. sms_cap) receives one entry per SM seen, by SM id (*n_sms how many); faults[0 .. cap) the word records
+ * sorted by (word, iteration, element) (*n how many).  opts may be NULL: defaults.  cro_probe_l2: dev_index is an
+ * in-process device.  cro_probe_l2_uuid runs `croprobe-cli l2-raw` (a fresh cuInit that sees only that GPU), so it
+ * reaches GPUs attached after cro_probe_init; ctx may be NULL; a UUID the node does not list is CRO_ERR_NO_DEVICE; a
+ * GPU that is also an in-process device of ctx is held under that device's mutex while the helper runs.  Every helper
+ * call gets a fresh cro_opts.seed_base (the context's seed_base + (h << 8) for its h-th helper call, or one from the
+ * clock without a context), so its call 0 uses seeds no earlier call used.  Options are refused before any spawn with
+ * the in-process error text, all but W's upper bound, which needs the device and which the helper checks. */
+int  cro_probe_l2(cro_ctx *ctx, int dev_index, const cro_l2_opts *opts, cro_l2_result *out,
+                  cro_l2_sm *sms, int sms_cap, int *n_sms, cro_l2_fault *faults, int cap, int *n);
+int  cro_probe_l2_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_l2_opts *opts, cro_l2_result *out,
+                       cro_l2_sm *sms, int sms_cap, int *n_sms, cro_l2_fault *faults, int cap, int *n);
+
+/* The device's SRAM and L2 health record from NVML, as the probe reads it after the call (with the SRAM error
+ * status): no context, no CUDA.  CRO_OK whatever NVML answered; CRO_ERR_INVALID_ARG for a NULL argument. */
+int  cro_read_l2_health(const char *gpu_uuid, cro_l2_health *out);
+
+/* Test hook: the probe's classification, a pure function.  Reads from *r unpublished, fold_ok, mismatches[5], a1_bad
+ * and a2_bad; from sms[] smid, mismatches, last and words_read; and
+ * the records faults[0 .. n) (element, iteration, smid, word).  Writes r's verdict, status, bad_sms, bad_sm,
+ * bad_lines and bad_line, each sms[].mark and each faults[].line, as cro_probe_l2 does. */
+int  cro_selftest_l2_classify(cro_l2_result *r, cro_l2_sm *sms, int n_sms, cro_l2_fault *faults, int n);
+
 /* ---- emit: encoding/json-compatible writers ------------------------------ */
 
 /* ComposableResourceStatus (api/v1alpha1/composableresource_types.go:36-41):
@@ -1237,6 +1456,16 @@ int  cro_emit_scan_annotations_json(const cro_scan_report *r, char *buf, size_t 
  * threshold-exceeded, comma-separated; only when any is set), and -ecc-corrected and -ecc-uncorrected (the deltas,
  * after - before; only when both reads answered). */
 int  cro_emit_sram_annotations_json(const cro_sram_result *r, char *buf, size_t cap, size_t *len);
+
+/* Additive L2 annotations (cohdi.io/probe-l2-*) of a cro_probe_l2 result, the same Go-marshalled map, integers and
+ * fixed spellings only: -verdict ("ok" for CRO_OK; "sm", "line", "atomic" or "all" for CRO_ERR_CHECKSUM with that
+ * verdict; "cuda-error:<cuda_error>" for CRO_ERR_CUDA; "error" otherwise), -sms ("<sms_covered>/<sm_count>"), -bytes,
+ * -iterations, -march-gbs (march_bytes / march_ns, integer division; 0 when march_ns is 0), and only when they apply:
+ * -bad-sms (bad_sm[0 .. min(bad_sms, 16)), comma-separated), -bad-lines (bad_line[0 .. min(bad_lines, 8)), decimal
+ * byte offsets, comma-separated), -a1-bad-counters and -a2-bad-counters (the listed counters, at most 8, comma-
+ * separated; when a1_bad / a2_bad > 0), -a2-holes (when a2_holes > 0), -overflow ("1"), -health (the flags' names
+ * sram-corrected, sram-uncorrected, l2-corrected, l2-uncorrected, threshold-exceeded, l2-bucket, comma-separated). */
+int  cro_emit_l2_annotations_json(const cro_l2_result *r, char *buf, size_t cap, size_t *len);
 
 /* (deviceID, CDIDeviceID) from an FM ScaleUpResponse body, with the
  * res_op_status gate of internal/cdi/fti/fm/client.go:184-213.  On the error
