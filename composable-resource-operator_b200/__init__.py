@@ -301,6 +301,43 @@ class ComputeFault(ctypes.Structure):
                 ("expected", ctypes.c_int32), ("actual", ctypes.c_int32)]
 
 
+# SM precision probe (cro_probe_precision, cro_precision_expected); verdicts and marks are COMPUTE_*
+PRECISION_LEG_F64, PRECISION_LEG_DFMA, PRECISION_LEG_TF32, PRECISION_LEG_F16, PRECISION_LEG_F16ACC, PRECISION_LEG_E5M2, \
+    PRECISION_LEG_HFMA2 = range(7)
+PRECISION_LEGS, PRECISION_ALL_LEGS = 7, 0x7F
+PRECISION_ANSWER_WIDE, PRECISION_ANSWER_SMALL128, PRECISION_ANSWER_SMALL, PRECISION_ANSWER_NARROW = range(4)
+PRECISION_ANSWERS = 4
+PRECISION_M, PRECISION_N, PRECISION_K, PRECISION_F64_N, PRECISION_F64_K, PRECISION_TF32_K = 128, 256, 256, 64, 128, 128
+PRECISION_RECORDS, PRECISION_MAX_SMS = 4096, 256
+PRECISION_MAX_ITERATIONS, PRECISION_MAX_ALU_ITERATIONS, PRECISION_MAX_ROUNDS = 65536, 4096, 64
+
+
+class PrecisionOpts(ctypes.Structure):
+    _fields_ = [("iterations", ctypes.c_uint32), ("alu_iterations", ctypes.c_uint32), ("legs", ctypes.c_uint32),
+                ("max_rounds", ctypes.c_uint32), ("test_inject_leg", ctypes.c_int32), ("test_inject_sm", ctypes.c_int32),
+                ("test_inject_iteration", ctypes.c_uint32), ("test_inject_row", ctypes.c_int32),
+                ("test_inject_col", ctypes.c_int32), ("reserved", ctypes.c_uint32), ("test_inject_mask", ctypes.c_uint64)]
+
+
+class PrecisionResult(ctypes.Structure):
+    """cro_precision_result: status, verdict and per-leg counts, coverage and times of one precision probe call."""
+    _fields_ = [("status", ctypes.c_int32), ("verdict", ctypes.c_uint32), ("seed", ctypes.c_uint64),
+                ("call", ctypes.c_uint64), ("sm_count", ctypes.c_uint32), ("legs", ctypes.c_uint32),
+                ("host_ref_ns", ctypes.c_uint64), ("nsmid", ctypes.c_uint32), ("bad_sms", ctypes.c_uint32),
+                ("bad_sm", ctypes.c_uint16 * 16), ("leg", ComputeLeg * PRECISION_LEGS)]
+
+
+class PrecisionSm(ctypes.Structure):
+    """One SM seen by a precision probe call, with its counts, times and COMPUTE_PERSISTENT / _INTERMITTENT mark per leg."""
+    _fields_ = [("smid", ctypes.c_uint32), ("reserved", ctypes.c_uint32), ("leg", ComputeSmLeg * PRECISION_LEGS)]
+
+
+class PrecisionFault(ctypes.Structure):
+    """One wrong element of a last iteration's answer: leg, SM, row, column, the exact answer and the raw bits got."""
+    _fields_ = [("leg", ctypes.c_uint32), ("smid", ctypes.c_uint32), ("row", ctypes.c_uint32), ("col", ctypes.c_uint32),
+                ("expected", ctypes.c_int64), ("actual_bits", ctypes.c_uint64)]
+
+
 # whole-HBM scan (cro_scan_hbm, cro_scan_hbm_uuid, cro_read_hbm_health)
 SCAN_CHUNK_BYTES, SCAN_RESERVE_BYTES, SCAN_MAX_CHUNKS, SCAN_PASSES, SCAN_ELEMENTS = 2 << 30, 1 << 30, 128, 2, 4
 (SCAN_HEALTH_ECC_CORRECTED_DURING, SCAN_HEALTH_ECC_UNCORRECTED_DURING, SCAN_HEALTH_REMAP_PENDING,
@@ -544,6 +581,8 @@ class SelftestSweepOut(ctypes.Structure):
 
 assert ctypes.sizeof(ProbeResult) == 512, ctypes.sizeof(ProbeResult)
 assert ctypes.sizeof(ComputeResult) == 600 and ctypes.sizeof(ComputeSm) == 208, ctypes.sizeof(ComputeResult)
+assert ctypes.sizeof(PrecisionResult) == 808 and ctypes.sizeof(PrecisionSm) == 288 and ctypes.sizeof(PrecisionFault) == 32 \
+    and ctypes.sizeof(PrecisionOpts) == 48, ctypes.sizeof(PrecisionResult)
 assert ctypes.sizeof(FaultReport) == 928 and ctypes.sizeof(LocatePass) == 120, ctypes.sizeof(FaultReport)
 assert ctypes.sizeof(LinkResult) == 984 and ctypes.sizeof(PciPath) == 272, ctypes.sizeof(LinkResult)
 assert ctypes.sizeof(ScanReport) == 12632 and ctypes.sizeof(ScanOpts) == 72, ctypes.sizeof(ScanReport)
@@ -573,6 +612,7 @@ EXPORTS = [
     "cro_locate_faults", "cro_emit_fault_annotations_json",
     "cro_probe_host_link", "cro_probe_host_link_uuid", "cro_pci_link_path", "cro_emit_link_annotations_json",
     "cro_probe_compute", "cro_probe_compute_uuid", "cro_compute_expected", "cro_emit_compute_annotations_json",
+    "cro_probe_precision", "cro_probe_precision_uuid", "cro_precision_expected", "cro_emit_precision_annotations_json",
     "cro_scan_hbm", "cro_scan_hbm_uuid", "cro_read_hbm_health", "cro_emit_scan_annotations_json",
     "cro_probe_sram", "cro_probe_sram_uuid", "cro_read_sram_health", "cro_emit_sram_annotations_json",
     "cro_probe_l2", "cro_probe_l2_uuid", "cro_read_l2_health", "cro_emit_l2_annotations_json", "cro_selftest_l2_classify",
@@ -681,6 +721,14 @@ def _load() -> ctypes.CDLL:
                                          ctypes.POINTER(i32), ctypes.POINTER(u64)]),
         "cro_compute_expected": (i32, [i32, u64, ctypes.POINTER(ctypes.c_int32)]),
         "cro_emit_compute_annotations_json": (i32, [ctypes.POINTER(ComputeResult)] + out),
+        "cro_probe_precision": (i32, [vp, i32, ctypes.POINTER(PrecisionOpts), ctypes.POINTER(PrecisionResult),
+                                      ctypes.POINTER(PrecisionSm), i32, ctypes.POINTER(i32), ctypes.POINTER(PrecisionFault), i32,
+                                      ctypes.POINTER(i32)]),
+        "cro_probe_precision_uuid": (i32, [vp, c, ctypes.POINTER(PrecisionOpts), i32, ctypes.POINTER(PrecisionResult),
+                                           ctypes.POINTER(PrecisionSm), i32, ctypes.POINTER(i32), ctypes.POINTER(PrecisionFault),
+                                           i32, ctypes.POINTER(i32), ctypes.POINTER(u64)]),
+        "cro_precision_expected": (i32, [i32, u64, ctypes.POINTER(ctypes.c_int64)]),
+        "cro_emit_precision_annotations_json": (i32, [ctypes.POINTER(PrecisionResult)] + out),
         "cro_scan_hbm": (i32, [vp, i32, ctypes.POINTER(ScanOpts), ctypes.POINTER(ScanReport), ctypes.POINTER(FaultWord), i32,
                                ctypes.POINTER(i32)]),
         "cro_scan_hbm_uuid": (i32, [vp, c, ctypes.POINTER(ScanOpts), ctypes.POINTER(ScanReport), ctypes.POINTER(FaultWord), i32,
@@ -838,6 +886,11 @@ def emit_link_annotations_json(r: LinkResult) -> str:
 def emit_compute_annotations_json(r: ComputeResult) -> str:
     """Additive cohdi.io/probe-compute-* annotations of a probe_compute result (Go-marshalled map[string]string)."""
     return _text(lib.cro_emit_compute_annotations_json, ctypes.byref(r))
+
+
+def emit_precision_annotations_json(r: PrecisionResult) -> str:
+    """Additive cohdi.io/probe-precision-* annotations of a probe_precision result (Go-marshalled map[string]string)."""
+    return _text(lib.cro_emit_precision_annotations_json, ctypes.byref(r))
 
 
 def emit_scan_annotations_json(r: ScanReport) -> str:
@@ -1016,6 +1069,36 @@ def probe_compute_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: int
     return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)], ns.value
 
 
+def _precision_opts(iterations: int, alu_iterations: int, legs: int, max_rounds: int,
+                    inject: Optional[Tuple[int, int, int, int, int, int]]) -> PrecisionOpts:
+    o = PrecisionOpts()
+    o.iterations, o.alu_iterations, o.legs, o.max_rounds = iterations, alu_iterations, legs, max_rounds
+    if inject is not None:
+        (o.test_inject_leg, o.test_inject_sm, o.test_inject_iteration, o.test_inject_row, o.test_inject_col,
+         o.test_inject_mask) = inject
+    return o
+
+
+def probe_precision_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: int = 0, alu_iterations: int = 0,
+                         legs: int = PRECISION_ALL_LEGS, max_rounds: int = 0, deadline_ms: int = 0,
+                         inject: Optional[Tuple[int, int, int, int, int, int]] = None,
+                         cap: int = 256) -> Tuple[PrecisionResult, List[PrecisionSm], List[PrecisionFault], int]:
+    """cro_probe_precision_uuid: the precision probe of any GPU on the node, run by the helper process (ctx may be None).
+    Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen, up to `cap` element records
+    and the helper's spawn-to-exit time in ns."""
+    o = _precision_opts(iterations, alu_iterations, legs, max_rounds, inject)
+    r = PrecisionResult()
+    sms = (PrecisionSm * PRECISION_MAX_SMS)()
+    arr = (PrecisionFault * max(1, cap))()
+    n_sms, n, ns = ctypes.c_int(), ctypes.c_int(), ctypes.c_uint64()
+    handle = ctx.handle if ctx is not None else None
+    rc = lib.cro_probe_precision_uuid(handle, _b(uuid), ctypes.byref(o), deadline_ms, ctypes.byref(r), sms, PRECISION_MAX_SMS,
+                                      ctypes.byref(n_sms), arr, cap, ctypes.byref(n), ctypes.byref(ns))
+    if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
+        raise _helper_error(rc, handle)
+    return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)], ns.value
+
+
 def _scan_opts(max_bytes: int, reserve_bytes: int, seed: int, deadline_ms: int, chunk_bytes: int,
                force: Optional[Tuple[int, int, int, int]]) -> ScanOpts:
     o = ScanOpts()
@@ -1041,6 +1124,16 @@ def scan_hbm_uuid(ctx: Optional["ProbeContext"], uuid: str, max_bytes: int = 0, 
         lib.cro_last_error(handle, buf, 1024)
         raise ProbeError(rc, buf.value.decode("utf-8", "replace"))
     return rep, [arr[i] for i in range(n.value)]
+
+
+def precision_expected(answer: int, seed: int) -> List[int]:
+    """cro_precision_expected: the PRECISION_ANSWER_* answer tile of the operands of `seed`, int64 values, row-major
+    (PRECISION_M x PRECISION_F64_N for the wide answer, PRECISION_M x PRECISION_N otherwise; host arithmetic, no GPU)."""
+    arr = (ctypes.c_int64 * (PRECISION_M * PRECISION_N))()
+    rc = lib.cro_precision_expected(answer, seed, arr)
+    if rc != OK:
+        raise ProbeError(rc, "cro_precision_expected")
+    return list(arr)[:PRECISION_M * (PRECISION_F64_N if answer == PRECISION_ANSWER_WIDE else PRECISION_N)]
 
 
 def compute_expected(answer: int, seed: int) -> List[int]:
@@ -1282,6 +1375,23 @@ class ProbeContext:
         n_sms, n = ctypes.c_int(), ctypes.c_int()
         self._check(lib.cro_probe_compute(self.handle, dev, ctypes.byref(o), ctypes.byref(r), sms, COMPUTE_MAX_SMS,
                                           ctypes.byref(n_sms), arr, cap, ctypes.byref(n)), allow=(ERR_CHECKSUM,))
+        return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
+
+    def probe_precision(self, dev: int = 0, iterations: int = 0, alu_iterations: int = 0, legs: int = PRECISION_ALL_LEGS,
+                        max_rounds: int = 0, inject: Optional[Tuple[int, int, int, int, int, int]] = None,
+                        cap: int = 256) -> Tuple[PrecisionResult, List[PrecisionSm], List[PrecisionFault]]:
+        """cro_probe_precision: every SM computes its answer tiles in FP64 (DMMA, DFMA), TF32, FP16 (f32 and f16
+        accumulation, HFMA2) and E5M2 and checks each value bit for bit.  iterations (F64, TF32, F16, F16ACC, E5M2) /
+        alu_iterations (DFMA, HFMA2) / max_rounds = 0: the defaults.  inject = (leg, sm, iteration, row, col, mask) is the
+        test-only wrong answer (sm, row, col: -1 for every one; mask up to the leg's element width).  Returns the result
+        (its status is OK or ERR_CHECKSUM), one entry per SM seen and up to `cap` element records."""
+        o = _precision_opts(iterations, alu_iterations, legs, max_rounds, inject)
+        r = PrecisionResult()
+        sms = (PrecisionSm * PRECISION_MAX_SMS)()
+        arr = (PrecisionFault * max(1, cap))()
+        n_sms, n = ctypes.c_int(), ctypes.c_int()
+        self._check(lib.cro_probe_precision(self.handle, dev, ctypes.byref(o), ctypes.byref(r), sms, PRECISION_MAX_SMS,
+                                            ctypes.byref(n_sms), arr, cap, ctypes.byref(n)), allow=(ERR_CHECKSUM,))
         return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
 
     def scan_hbm(self, dev: int = 0, max_bytes: int = 0, reserve_bytes: int = 0, seed: int = 0, cap: int = 256,

@@ -59,6 +59,11 @@ static_assert(sizeof(cro_compute_result) == 600 && offsetof(cro_compute_result, 
                   offsetof(cro_compute_result, bad_sm) == 48 && offsetof(cro_compute_result, leg) == 80 &&
                   offsetof(cro_compute_leg, fold) == 88,
               "compute layout");
+static_assert(sizeof(cro_precision_opts) == 48 && offsetof(cro_precision_opts, test_inject_mask) == 40 &&
+                  sizeof(cro_precision_result) == 808 && offsetof(cro_precision_result, leg) == 80 &&
+                  sizeof(cro_precision_sm) == 288 && sizeof(cro_precision_fault) == 32 &&
+                  offsetof(cro_precision_fault, actual_bits) == 24,
+              "precision layout");
 
 static_assert(sizeof(cro_scan_opts) == 72 && sizeof(cro_hbm_health) == 56 && sizeof(cro_scan_pass) == 552 &&
                   sizeof(cro_scan_chunk) == 88, "scan layout");
@@ -389,6 +394,44 @@ int cro_probe_compute_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_compute
     if (helper_ns) *helper_ns = ns;
     return compute_out(rc, seen, found, sms, sms_cap, n_sms, faults, cap, n);
 } CRO_API_CATCH
+// The precision probe's two forms share the copy-out: sms[0 .. sms_cap) and faults[0 .. cap).
+static int precision_out(int rc, const std::vector<cro_precision_sm>& seen, const std::vector<cro_precision_fault>& found,
+                         cro_precision_sm* sms, int sms_cap, int* n_sms, cro_precision_fault* faults, int cap, int* n) {
+    const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
+    for (size_t j = 0; j < ks; ++j) sms[j] = seen[j];
+    for (size_t j = 0; j < kf; ++j) faults[j] = found[j];
+    *n_sms = (int)ks;
+    *n = (int)kf;
+    return rc;
+}
+int cro_probe_precision(cro_ctx* ctx, int i, const cro_precision_opts* opts, cro_precision_result* out, cro_precision_sm* sms,
+                        int sms_cap, int* n_sms, cro_precision_fault* faults, int cap, int* n) try {
+    if (!ctx || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
+        return CRO_ERR_INVALID_ARG;
+    *n = *n_sms = 0;
+    cro_precision_opts o{};
+    if (opts) o = *opts;
+    std::vector<cro_precision_sm> seen;
+    std::vector<cro_precision_fault> found;
+    const int rc = ctx_probe_precision(ctx, i, o, out, &seen, &found);
+    return precision_out(rc, seen, found, sms, sms_cap, n_sms, faults, cap, n);
+} CRO_API_CATCH
+int cro_probe_precision_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_precision_opts* opts, int deadline_ms,
+                             cro_precision_result* out, cro_precision_sm* sms, int sms_cap, int* n_sms,
+                             cro_precision_fault* faults, int cap, int* n, uint64_t* helper_ns) try {
+    if (!gpu_uuid || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
+        return CRO_ERR_INVALID_ARG;
+    *n = *n_sms = 0;
+    if (helper_ns) *helper_ns = 0;
+    cro_precision_opts o{};
+    if (opts) o = *opts;
+    std::vector<cro_precision_sm> seen;
+    std::vector<cro_precision_fault> found;
+    uint64_t ns = 0;
+    const int rc = ctx_probe_precision_uuid(ctx, gpu_uuid, o, deadline_ms, out, &seen, &found, cap, &ns);
+    if (helper_ns) *helper_ns = ns;
+    return precision_out(rc, seen, found, sms, sms_cap, n_sms, faults, cap, n);
+} CRO_API_CATCH
 // The scan's two forms share the copy-out: words[0 .. cap), recorded and complete as cro_locate_faults sets them.
 static int scan_out(int rc, const std::vector<cro_fault_word>& found, cro_scan_report* out, cro_fault_word* words, int cap, int* n) {
     const size_t k = std::min(found.size(), (size_t)cap);
@@ -516,6 +559,9 @@ int cro_selftest_l2_classify(cro_l2_result* r, cro_l2_sm* sms, int n_sms, cro_l2
 } CRO_API_CATCH
 int cro_compute_expected(int answer, uint64_t seed, int32_t* out) try {
     return compute::Expected(answer, seed, out);
+} CRO_API_CATCH
+int cro_precision_expected(int answer, uint64_t seed, int64_t* out) try {
+    return precision::Expected(answer, seed, out);
 } CRO_API_CATCH
 int cro_pci_link_path(const char* sys_root, const char* pci_bus_id, cro_pci_path* out) try {
     if (!pci_bus_id || !out) return CRO_ERR_INVALID_ARG;
@@ -831,6 +877,42 @@ int cro_emit_compute_annotations_json(const cro_compute_result* r, char* buf, si
     m[p + "bf16-gflops"] = rate(CRO_COMPUTE_LEG_BF16);
     m[p + "e4m3-gflops"] = rate(CRO_COMPUTE_LEG_E4M3);
     if (worst < CRO_COMPUTE_LEGS)
+        m[p + "slowest-sm"] = std::to_string(r->leg[worst].slowest_sm) + " " + std::to_string(r->leg[worst].slow_permille);
+    gojson::Writer w;
+    w.string_map(m);
+    return copy_out(w.str(), buf, cap, len);
+} CRO_API_CATCH
+
+int cro_emit_precision_annotations_json(const cro_precision_result* r, char* buf, size_t cap, size_t* len) try {
+    if (!r) return CRO_ERR_INVALID_ARG;
+    static const char* const kLeg[CRO_PRECISION_LEGS] = {"f64", "dfma", "tf32", "f16", "f16acc", "e5m2", "hfma2"};
+    std::map<std::string, std::string> m;
+    const std::string p = "cohdi.io/probe-precision-";
+    m[p + "verdict"] = r->status == CRO_OK                                                ? "ok"
+                       : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_COMPUTE_SM  ? "sm"
+                       : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_COMPUTE_ALL ? "all"
+                                                                                        : "error";
+    uint32_t covered = 0xFFFFFFFFu, worst = CRO_PRECISION_LEGS;
+    std::string failed;
+    for (int l = 0; l < CRO_PRECISION_LEGS; ++l) {
+        if (!(r->legs >> l & 1u)) continue;
+        const cro_compute_leg& L = r->leg[l];
+        covered = std::min(covered, L.sms_covered);
+        if (L.mismatches || L.fold_mismatches || L.unpublished) failed += (failed.empty() ? "" : ",") + std::string(kLeg[l]);
+        if (worst == CRO_PRECISION_LEGS || L.slow_permille > r->leg[worst].slow_permille) worst = (uint32_t)l;
+    }
+    m[p + "sms"] = std::to_string(covered == 0xFFFFFFFFu ? 0u : covered) + "/" + std::to_string(r->sm_count);
+    if (r->bad_sms) {
+        std::string ids;
+        for (uint32_t j = 0; j < std::min<uint32_t>(r->bad_sms, 16); ++j) ids += (j ? "," : "") + std::to_string(r->bad_sm[j]);
+        m[p + "bad-sms"] = ids;
+    }
+    if (!failed.empty()) m[p + "failed-legs"] = failed;
+    for (int l : {CRO_PRECISION_LEG_F64, CRO_PRECISION_LEG_TF32, CRO_PRECISION_LEG_F16, CRO_PRECISION_LEG_F16ACC, CRO_PRECISION_LEG_E5M2}) {
+        const cro_compute_leg& L = r->leg[l];
+        m[p + kLeg[l] + "-gflops"] = std::to_string(L.ns ? L.ops / L.ns : 0ull);
+    }
+    if (worst < CRO_PRECISION_LEGS)
         m[p + "slowest-sm"] = std::to_string(r->leg[worst].slowest_sm) + " " + std::to_string(r->leg[worst].slow_permille);
     gojson::Writer w;
     w.string_map(m);

@@ -1,9 +1,6 @@
 // compute_probe.cu — the SM compute probe (cro_probe_compute): every SM's tensor cores and ALUs against an exact answer.
-#include <map>
-#include <tuple>
-
 #include "compute.hpp"
-#include "probe_internal.hpp"
+#include "sm_legs.hpp"
 
 namespace cro {
 
@@ -138,42 +135,8 @@ int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_comput
                 return e ? e : cudaMemcpyAsync(hbits, a.sm_bits, sizeof hbits, cudaMemcpyDeviceToHost, st);
             };
             auto take = [&](uint32_t* covered) -> int {
-                R.ctas += (uint32_t)grid;
-                R.ops += kComputeOps * iters[leg] * (uint64_t)grid;
-                uint64_t t0 = ~0ull, t1 = 0;
-                for (const ComputeCta& x : hc) {
-                    if (x.stamp != k) {
-                        R.unpublished++;
-                        continue;
-                    }
-                    if (x.nsmid > CRO_COMPUTE_MAX_SMS) {
-                        c->set_error("compute probe: the device reports %nsmid = " + std::to_string(x.nsmid) +
-                                     ", more SM ids than the " + std::to_string(CRO_COMPUTE_MAX_SMS) + " the coverage bitmaps hold");
-                        return CRO_ERR_UNSUPPORTED;
-                    }
-                    r->nsmid = x.nsmid;
-                    t0 = std::min<uint64_t>(t0, x.t0);
-                    t1 = std::max<uint64_t>(t1, x.t1);
-                    cro_compute_sm& S = per_sm[x.smid];
-                    S.smid = x.smid;
-                    cro_compute_sm_leg& SL = S.leg[leg];
-                    SL.ctas++;
-                    SL.mismatches += x.mismatches;
-                    SL.fold_mismatches += x.fold_mismatches;
-                    SL.ns += x.t1 > x.t0 ? x.t1 - x.t0 : 0;
-                    SL.cycles += x.cycles;
-                    R.mismatches += x.mismatches;
-                    R.fold_mismatches += x.fold_mismatches;
-                    if (x.smid < fold_sm) {
-                        fold_sm = x.smid;
-                        R.fold = x.fold;
-                    }
-                }
-                if (t1 > t0) R.timer_ns += t1 - t0;
-                R.sms_covered = 0;
-                for (int w = 0; w < kSmWords; ++w) R.sms_covered += (uint32_t)__builtin_popcountll(hbits[w]);
-                *covered = R.sms_covered;
-                return CRO_OK;
+                return take_leg_round(c, "compute probe", hc, k, leg, kComputeOps * iters[leg] * (uint64_t)grid, hbits, kSmWords,
+                                      CRO_COMPUTE_MAX_SMS, R, &r->nsmid, &fold_sm, per_sm, covered);
             };
             const int e = coverage_rounds(c, d, ev, cta, cta_bytes, (uint32_t)grid, max_rounds, &R.rounds, &R.ns, launch, fetch, take);
             if (e) return e;
@@ -184,26 +147,7 @@ int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_comput
                 CU_TRY(c, cudaMemcpy(f.data(), a.rec, f.size() * sizeof(cro_compute_fault), cudaMemcpyDeviceToHost));
                 faults->insert(faults->end(), f.begin(), f.end());
             }
-            // per SM: marks, failed SMs, and the slowest SM's cycles per iteration against the median
-            std::vector<std::pair<uint64_t, uint32_t>> per_iter;
-            for (auto& kv : per_sm) {
-                cro_compute_sm_leg& SL = kv.second.leg[leg];
-                if (!SL.ctas) continue;
-                SL.mark = SL.mismatches ? CRO_COMPUTE_PERSISTENT : SL.fold_mismatches ? CRO_COMPUTE_INTERMITTENT : 0u;
-                if (SL.mark) R.failed_sms++;
-                per_iter.push_back({SL.cycles / ((uint64_t)SL.ctas * iters[leg]), kv.first});
-            }
-            if (!per_iter.empty()) {
-                std::vector<uint64_t> v;
-                for (auto& p : per_iter) v.push_back(p.first);
-                std::sort(v.begin(), v.end());
-                const uint64_t median = v[v.size() / 2];
-                auto worst = per_iter.front();
-                for (auto& p : per_iter)
-                    if (p.first > worst.first) worst = p;
-                R.slowest_sm = worst.second;
-                R.slow_permille = median ? (uint32_t)std::min<uint64_t>(worst.first * 1000 / median, 0xFFFFFFFFu) : 0u;
-            }
+            finish_leg(R, per_sm, leg, iters[leg]);
         }
         return CRO_OK;
     }();
@@ -213,25 +157,7 @@ int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_comput
         blank_result(r, *r, sms, faults);
         return r->status = rc;
     }
-    bool all = false, any = false;
-    for (uint32_t leg = 0; leg < CRO_COMPUTE_LEGS; ++leg) {
-        const cro_compute_leg& R = r->leg[leg];
-        if (!(r->legs >> leg & 1u)) continue;
-        if (R.unpublished || (R.failed_sms && R.failed_sms == R.sms_covered)) all = true;
-        if (R.unpublished || R.failed_sms) any = true;
-    }
-    for (auto& kv : per_sm) {
-        bool bad = false;
-        for (const cro_compute_sm_leg& SL : kv.second.leg) bad = bad || SL.mark != 0;
-        if (bad && r->bad_sms < 16) r->bad_sm[r->bad_sms] = (uint16_t)kv.first;
-        if (bad) r->bad_sms++;
-        sms->push_back(kv.second);
-    }
-    std::sort(faults->begin(), faults->end(), [](const cro_compute_fault& x, const cro_compute_fault& y) {
-        return std::make_tuple(x.leg, x.smid, x.row, x.col) < std::make_tuple(y.leg, y.smid, y.row, y.col);
-    });
-    r->verdict = all ? CRO_COMPUTE_ALL : any ? CRO_COMPUTE_SM : CRO_COMPUTE_NONE;
-    return r->status = any ? CRO_ERR_CHECKSUM : CRO_OK;
+    return close_call(r, CRO_COMPUTE_LEGS, per_sm, sms, faults);
 }
 
 namespace {

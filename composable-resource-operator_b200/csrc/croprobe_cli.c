@@ -35,13 +35,19 @@
  *                                                    region and no NVML; cro_compute_result, uint64_t n_sms and n,
  *                                                    CRO_COMPUTE_MAX_SMS cro_compute_sm entries (n_sms of them filled),
  *                                                    then n cro_compute_fault records (at most cap) on stdout
+ *   croprobe-cli precision-raw <uuid> <seed_base> <iterations> <alu_iterations> <legs> <max_rounds> <inject_leg>
+ *                              <inject_sm> <inject_iteration> <inject_row> <inject_col> <inject_mask> <cap>
+ *                                                    the precision probe with every cro_precision_opts field, as
+ *                                                    compute-raw: cro_precision_result, uint64_t n_sms and n,
+ *                                                    CRO_PRECISION_MAX_SMS cro_precision_sm entries, then n
+ *                                                    cro_precision_fault records (at most cap) on stdout
  *   croprobe-cli l2-raw <uuid> <seed_base> <bytes> <iterations> <a1_counters> <a2_counters> <inject_leg> <inject_sm>
  *                       <inject_element> <inject_iteration> <inject_word> <inject_mask> <cap>
  *                                                    the L2 probe with every cro_l2_opts field but the deadline, NVML on
  *                                                    for its health record; cro_l2_result, uint64_t n_sms and n,
  *                                                    CRO_L2_MAX_SMS cro_l2_sm entries (n_sms of them filled), then n
  *                                                    cro_l2_fault records (at most cap) on stdout
- *   link-raw, compute-raw and l2-raw take cro_opts.seed_base from argv (the device seed is seed_base | minor, as in process), so
+ *   link-raw, compute-raw, precision-raw and l2-raw take cro_opts.seed_base from argv (the device seed is seed_base | minor, as in process), so
  *   that the library can give every helper call fresh patterns and operands; their counts are the helper's own,
  *   because neither result says how many records follow.
  * Exit 3: the device is not visible to this (fresh) process — the reference's found=false.  The raw commands exit 0
@@ -79,7 +85,8 @@ int main(int argc, char **argv) {
                         "<first> <count> <and> <or> <cap> | sram-raw <uuid> <legs> <iterations> <cluster> <rounds> <leg> <sm> <element> <iteration> "
                         "<word> <mask> <cap> | link-raw <uuid> <seed_base> <bytes> <hops> <ctas> <check> <word> <mask> <cap> | "
                         "compute-raw <uuid> <seed_base> <iterations> <alu_iterations> <legs> <rounds> <leg> <sm> <iteration> <row> <col> "
-                        "<mask> <cap> | l2-raw <uuid> <seed_base> <bytes> <iterations> <a1> <a2> <leg> <sm> <element> <iteration> <word> <mask> <cap>\n");
+                        "<mask> <cap> | precision-raw <uuid> <seed_base> <iterations> <alu_iterations> <legs> <rounds> <leg> <sm> <iteration> <row> "
+                        "<col> <mask> <cap> | l2-raw <uuid> <seed_base> <bytes> <iterations> <a1> <a2> <leg> <sm> <element> <iteration> <word> <mask> <cap>\n");
         return 64;
     }
     const double t_start = now_s();
@@ -91,8 +98,9 @@ int main(int argc, char **argv) {
     const int link_raw = strcmp(cmd, "link-raw") == 0;
     const int compute_raw = strcmp(cmd, "compute-raw") == 0;
     const int l2_raw = strcmp(cmd, "l2-raw") == 0;
+    const int precision_raw = strcmp(cmd, "precision-raw") == 0;
     /* the commands that run one check of one device by their own, not the HBM probe */
-    const int wants_scan = scan_raw || sram_raw || link_raw || compute_raw || l2_raw || strcmp(cmd, "scan") == 0;
+    const int wants_scan = scan_raw || sram_raw || link_raw || compute_raw || precision_raw || l2_raw || strcmp(cmd, "scan") == 0;
     const int wants_probe = raw || cold || strcmp(cmd, "probe") == 0;
     if ((wants_probe || wants_scan) && argc < 3) return 64;
     if (scan_raw && argc != 12) return 64;
@@ -100,6 +108,7 @@ int main(int argc, char **argv) {
     if (link_raw && argc != 11) return 64;
     if (compute_raw && argc != 15) return 64;
     if (l2_raw && argc != 15) return 64;
+    if (precision_raw && argc != 15) return 64;
     cro_opts opts;
     memset(&opts, 0, sizeof opts);
     opts.abi_version = CRO_ABI_VERSION;
@@ -109,13 +118,13 @@ int main(int argc, char **argv) {
         opts.flags = CRO_F_LAZY_ALLOC;
         opts.sweep_bytes = 64ull << 20;
     }
-    if (compute_raw) opts.flags |= CRO_F_NO_NVML;       /* no health record to read, and NVML's first call is slow */
+    if (compute_raw || precision_raw) opts.flags |= CRO_F_NO_NVML;       /* no health record to read, and NVML's first call is slow */
     if (link_raw) {
         /* a region of exactly L (the probe checks L <= S; no halving on a full GPU), and NVML for the replay counters */
         opts.flags = CRO_F_LAZY_ALLOC;
         opts.sweep_bytes = strtoull(argv[4], NULL, 10) ? (uint64_t)strtoull(argv[4], NULL, 10) : 256ull << 20;
     }
-    if (link_raw || compute_raw || l2_raw) opts.seed_base = (uint64_t)strtoull(argv[3], NULL, 10);
+    if (link_raw || compute_raw || precision_raw || l2_raw) opts.seed_base = (uint64_t)strtoull(argv[3], NULL, 10);
     if (wants_probe) {
         /* The hot-plug path: one device, identity from /proc (NVML's first call costs more than the probe), and a
          * 1 GiB first sweep unless told otherwise — far beyond the L2, and it shortens everything before it. */
@@ -282,6 +291,34 @@ int main(int argc, char **argv) {
                 return 2;
             fflush(stdout);
             _exit(cr.status == CRO_OK ? 0 : 1);
+        }
+        if (precision_raw) {
+            cro_precision_opts po;
+            memset(&po, 0, sizeof po);
+            po.iterations = (uint32_t)strtoul(argv[4], NULL, 10);
+            po.alu_iterations = (uint32_t)strtoul(argv[5], NULL, 10);
+            po.legs = (uint32_t)strtoul(argv[6], NULL, 10);
+            po.max_rounds = (uint32_t)strtoul(argv[7], NULL, 10);
+            po.test_inject_leg = atoi(argv[8]);
+            po.test_inject_sm = atoi(argv[9]);
+            po.test_inject_iteration = (uint32_t)strtoul(argv[10], NULL, 10);
+            po.test_inject_row = atoi(argv[11]);
+            po.test_inject_col = atoi(argv[12]);
+            po.test_inject_mask = (uint64_t)strtoull(argv[13], NULL, 10);
+            const int cap = atoi(argv[14]);
+            static cro_precision_result pr;
+            static cro_precision_sm sms[CRO_PRECISION_MAX_SMS];
+            cro_precision_fault *faults = (cro_precision_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
+            int n_sms = 0, got = 0;
+            if (!faults) return 2;
+            cro_probe_precision(ctx, idx, &po, &pr, sms, CRO_PRECISION_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
+            const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)got};
+            /* the result whatever its status: the library reads why from it */
+            if (fwrite(&pr, sizeof pr, 1, stdout) != 1 || fwrite(counts, sizeof counts, 1, stdout) != 1 ||
+                fwrite(sms, sizeof sms, 1, stdout) != 1 || (got && fwrite(faults, sizeof *faults, (size_t)got, stdout) != (size_t)got))
+                return 2;
+            fflush(stdout);
+            _exit(pr.status == CRO_OK ? 0 : 1);
         }
         if (wants_scan) {
             cro_scan_opts so;

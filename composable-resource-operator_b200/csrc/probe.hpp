@@ -79,6 +79,7 @@ struct Device {
     uint64_t compute_calls = 0;            // k of the next compute probe call (ctx_probe_compute): its operand seed
     uint64_t sram_calls = 0;               // k of the next SRAM probe call (ctx_probe_sram): its seeds
     uint64_t l2_calls = 0;                 // k of the next L2 probe call (ctx_probe_l2): its seeds
+    uint64_t precision_calls = 0;          // k of the next precision probe call (ctx_probe_precision): its operand seed
     KernelPlan plan{};
     SweepScratch scratch{}, scratch_aux{}, scratch_pfx{};   // main stream / closed form / p2p prefix closed form
     // lane 0's buffers under their old names: the synchronous probe, the single sweeps and cro_probe_all use lane 0
@@ -231,6 +232,19 @@ int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_comput
                       std::vector<cro_compute_fault>* faults);
 int ctx_probe_compute_uuid(cro_ctx* c, const char* uuid, const cro_compute_opts& o, int deadline_ms, cro_compute_result* r,
                            std::vector<cro_compute_sm>* sms, std::vector<cro_compute_fault>* faults, int cap, uint64_t* helper_ns);
+
+// SM precision probe (include/croprobe.h, cro_probe_precision / cro_probe_precision_uuid, precision_probe.cu): as the
+// compute probe's two forms; the uuid form runs `croprobe-cli precision-raw`.
+int ctx_probe_precision(cro_ctx* c, int idx, const cro_precision_opts& o, cro_precision_result* r,
+                        std::vector<cro_precision_sm>* sms, std::vector<cro_precision_fault>* faults);
+int ctx_probe_precision_uuid(cro_ctx* c, const char* uuid, const cro_precision_opts& o, int deadline_ms, cro_precision_result* r,
+                             std::vector<cro_precision_sm>* sms, std::vector<cro_precision_fault>* faults, int cap,
+                             uint64_t* helper_ns);
+namespace precision {
+// The answer tile of the operands of `seed` (include/croprobe.h): answer CRO_PRECISION_ANSWER_*, M x N int64 values,
+// row-major.  CRO_ERR_INVALID_ARG for another answer.
+int Expected(int answer, uint64_t seed, int64_t* out);
+}  // namespace precision
 
 // The helper run behind the host link and compute probes' uuid forms.  Bad options are refused by the caller first.
 // With a context, the node must list the GPU (CRO_ERR_NO_DEVICE otherwise) and a GPU that is also an in-process device

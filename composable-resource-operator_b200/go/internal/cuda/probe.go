@@ -462,6 +462,110 @@ func (c *Context) ProbeCompute(deviceID string) (ComputeResult, error) {
 	return computeResult(&res, sms, nSMs, faults[:], got), nil
 }
 
+// PrecisionResult is the summary of cro_precision_result an operator reads:
+// whether every SM computed the exact answer, bit for bit, in FP64 (DMMA,
+// DFMA), TF32, FP16 (f32 and f16 accumulation, HFMA2) and E5M2, and which SMs
+// did not.
+type PrecisionResult struct {
+	OK          bool
+	Verdict     uint32            // CRO_COMPUTE_NONE / _SM / _ALL
+	SMCount     uint32
+	Covered     [7]uint32         // SMs seen per CRO_PRECISION_LEG_*
+	Mismatches  [7]uint64         // wrong elements of the last iteration, per leg
+	BadSMs      []uint32          // SMs that failed any leg, ascending
+	Faults      []PrecisionFault
+	Annotations string // Go-marshalled map[string]string of cohdi.io/probe-precision-* keys
+}
+
+// PrecisionFault is one wrong element (cro_precision_fault): the exact answer
+// and the accumulator's raw bits.
+type PrecisionFault struct {
+	Leg, SM, Row, Col uint32
+	Expected          int64
+	ActualBits        uint64
+}
+
+func precisionResult(res *C.cro_precision_result, sms []C.cro_precision_sm, nSMs C.int, faults []C.cro_precision_fault,
+	got C.int) PrecisionResult {
+	out := PrecisionResult{OK: res.status == C.CRO_OK, Verdict: uint32(res.verdict), SMCount: uint32(res.sm_count)}
+	for l := 0; l < int(C.CRO_PRECISION_LEGS); l++ {
+		out.Covered[l] = uint32(res.leg[l].sms_covered)
+		out.Mismatches[l] = uint64(res.leg[l].mismatches)
+	}
+	for i := 0; i < int(nSMs); i++ {
+		for l := 0; l < int(C.CRO_PRECISION_LEGS); l++ {
+			if sms[i].leg[l].mark != 0 {
+				out.BadSMs = append(out.BadSMs, uint32(sms[i].smid))
+				break
+			}
+		}
+	}
+	for i := 0; i < int(got); i++ {
+		f := faults[i]
+		out.Faults = append(out.Faults, PrecisionFault{uint32(f.leg), uint32(f.smid), uint32(f.row), uint32(f.col),
+			int64(f.expected), uint64(f.actual_bits)})
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_precision_annotations_json(res, buf, 4096, &ln) == C.CRO_OK {
+		out.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return out
+}
+
+// ProbePrecisionByUUID runs cro_probe_precision_uuid with its defaults: the
+// precision probe of any GPU on the node through the helper process, the form
+// an operator calls next to the compute probe, after a passing HBM probe of a
+// freshly composed GPU and before it goes to an FP64 or FP16 tenant
+// (INTEGRATION.md §2f).  A mismatch or a failed launch (CRO_ERR_CUDA) is a
+// result, not an error; found is false when the node does not list the GPU.
+func (c *Context) ProbePrecisionByUUID(deviceID string) (r PrecisionResult, found bool, err error) {
+	id := C.CString(deviceID)
+	defer C.free(unsafe.Pointer(id))
+	var res C.cro_precision_result
+	sms := make([]C.cro_precision_sm, C.CRO_PRECISION_MAX_SMS)
+	var faults [256]C.cro_precision_fault
+	var nSMs, got C.int
+	rc := C.cro_probe_precision_uuid(c.h, id, nil, 0, &res, &sms[0], C.CRO_PRECISION_MAX_SMS, &nSMs, &faults[0], 256, &got, nil)
+	if rc == C.CRO_ERR_NO_DEVICE {
+		return r, false, nil
+	}
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM && rc != C.CRO_ERR_CUDA {
+		return r, true, errorOf(c.h, rc)
+	}
+	return precisionResult(&res, sms, nSMs, faults[:], got), true, nil
+}
+
+// ProbePrecision runs cro_probe_precision with its defaults on the in-process
+// device whose UUID is deviceID.  ProbePrecisionByUUID is the form an operator
+// should call: it also reaches a GPU composed after the manager started.
+func (c *Context) ProbePrecision(deviceID string) (PrecisionResult, error) {
+	var devs [C.CRO_MAX_DEVICES]C.cro_dev_info
+	var n C.int
+	if rc := C.cro_enumerate(c.h, &devs[0], C.CRO_MAX_DEVICES, &n); rc != C.CRO_OK {
+		return PrecisionResult{}, errorOf(c.h, rc)
+	}
+	idx := C.int(-1)
+	for i := 0; i < int(n); i++ {
+		if C.GoString(&devs[i].gpu_uuid[0]) == deviceID && devs[i].flags&C.CRO_DEV_IN_PROCESS != 0 {
+			idx = C.int(devs[i].dev_index)
+		}
+	}
+	if idx < 0 {
+		return PrecisionResult{}, fmt.Errorf("cuda precision probe: %s is not a device of this context", deviceID)
+	}
+	var res C.cro_precision_result
+	sms := make([]C.cro_precision_sm, C.CRO_PRECISION_MAX_SMS)
+	var faults [256]C.cro_precision_fault
+	var nSMs, got C.int
+	rc := C.cro_probe_precision(c.h, idx, nil, &res, &sms[0], C.CRO_PRECISION_MAX_SMS, &nSMs, &faults[0], 256, &got)
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM {
+		return PrecisionResult{}, errorOf(c.h, rc)
+	}
+	return precisionResult(&res, sms, nSMs, faults[:], got), nil
+}
+
 // ScanResult is the summary of cro_scan_report an operator reads: whether every
 // free byte of the GPU's memory held what was written, how much was covered,
 // and the memory's own health record from NVML.

@@ -822,6 +822,134 @@ int  cro_probe_compute_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_comput
  * CRO_COMPUTE_M * CRO_COMPUTE_N int32 values, row-major.  Host arithmetic only; no context. */
 int  cro_compute_expected(int answer, uint64_t seed, int32_t *out);
 
+/* ---- SM precision: every SM's FP64, TF32, FP16 and E5M2 arithmetic against an exact answer, bit for bit ---- */
+
+/*
+ * The compute probe checks s8, bf16 and e4m3 tensor cores and FP32 / INT32 CUDA cores, and compares float answers after
+ * rounding them to int32.  The precision probe checks the formats it leaves out, one leg each, on every SM: the FP64
+ * tensor cores (DMMA) and CUDA cores (DFMA), TF32 and FP16 tensor cores with f32 accumulation, FP16 tensor cores with
+ * f16 accumulation, E5M2 tensor cores, and the FP16 CUDA cores (HFMA2).  It is shaped like the compute probe (one CTA
+ * per SM, one launch per leg, the same verdicts, marks, coverage rounds and slowest-SM report, and the same guarantees:
+ * the device's mutex, probes in flight finish first, the sweep region untouched) but compares tighter: every value
+ * must be IEEE-equal to the exact answer encoded in the leg's own type, and the fold adds the value's bit pattern, so
+ * a flipped fraction bit fails even where it is worth far less than 0.5.
+ *
+ * Operands of call k on a device: seed = seed_dev + 2^58 + k * 0xD1B54A32D192ED03.  With the leg's M, N and K, element
+ *   e = m * K + k             for A[m][k]
+ *   e = M * K + k * N + n     for B[k][n]
+ * is read one of three ways:
+ *   small-int  (byte & 7) - 4 in -4 .. 3, byte = byte (e mod 8) of pattern_word(seed, e / 8)      (TF32, F16, E5M2)
+ *   narrow     (byte & 3) - 2 in -2 .. 1, the same byte                                             (F16ACC, HFMA2)
+ *   wide       the low 20 bits of pattern_word(seed, e), sign-extended: -2^19 .. 2^19 - 1          (F64, DFMA)
+ * Each answer D[m][n] = sum over k of A[m][k] * B[k][n] is exact in any order of accumulation (DESIGN.md "The precision
+ * probe"): small-int partial sums stay within 16 K <= 4096 (exact with 13 significant bits; every operand is exact in
+ * tf32, f16 and e5m2), narrow ones within 4 * 256 = 1024 (exact in f16's 11), wide ones within 2^38 * 128 = 2^45
+ * (exact in f64's 53).
+ *
+ * Legs (M x N x K; every CTA has 256 threads and holds the whole tile in shared memory):
+ *   F64     mma.sync m16n8k16 .f64 (DMMA)        128 x  64 x 128   wide answer; warp w owns rows 16w .. 16w + 15
+ *   DFMA    DFMA chains, the F64 fragment        128 x  64 x 128   wide answer
+ *   TF32    wgmma m64n256k8 .f32.tf32 (HGMMA)    128 x 256 x 128   small-int answer at K = 128
+ *   F16     wgmma m64n256k16 .f32.f16 (HGMMA)    128 x 256 x 256   small-int answer
+ *   F16ACC  wgmma m64n256k16 .f16.f16 (HGMMA)    128 x 256 x 256   narrow answer, f16 accumulators
+ *   E5M2    wgmma m64n256k32 .f32.e5m2 (QGMMA)   128 x 256 x 256   small-int answer
+ *   HFMA2   HFMA2 chains, f16 accumulators       128 x 256 x 256   narrow answer; (col, col + 1) pairs packed
+ * Thread t holds V values (V = 32 for F64 / DFMA, 128 otherwise); value j is the element
+ *   row = r0(t) + 8 * ((j / 2) % 2),   col = 8 * (j / 4) + 2 * (t % 4) + j % 2
+ * with r0(t) = 16 * (t / 32) + (t % 32) / 4 for F64 / DFMA and 64 * (t / 128) + 16 * ((t / 32) % 4) + (t % 32) / 4
+ * otherwise (the mma / wgmma accumulator fragments; the CUDA-core legs use the same mapping).
+ *
+ * Compare: a value is right when it is IEEE-equal to its expected integer converted to the leg's type (exact for these
+ * bounds, so -0 equals 0 and any fraction fails).  Fold: after every iteration the thread adds canon(v) * (2e + 1)
+ * (mod 2^64) over its values, with canon(v) the value's bit pattern (64, 32 or 16 bits, zero-extended; -0 taken as 0)
+ * and e = row * N + col; at the end it compares the running sum with iterations * the same sum over the expected
+ * values.  The fold of a whole CTA is layout-free: the sum over every element of the tile.
+ */
+#define CRO_PRECISION_LEG_F64       0
+#define CRO_PRECISION_LEG_DFMA      1
+#define CRO_PRECISION_LEG_TF32      2
+#define CRO_PRECISION_LEG_F16       3
+#define CRO_PRECISION_LEG_F16ACC    4
+#define CRO_PRECISION_LEG_E5M2      5
+#define CRO_PRECISION_LEG_HFMA2     6
+#define CRO_PRECISION_LEGS          7
+#define CRO_PRECISION_ALL_LEGS      0x7Fu   /* bit l: leg l */
+#define CRO_PRECISION_ANSWER_WIDE   0       /* 128 x 64, K = 128: F64, DFMA      */
+#define CRO_PRECISION_ANSWER_SMALL128 1     /* 128 x 256, K = 128: TF32          */
+#define CRO_PRECISION_ANSWER_SMALL  2       /* 128 x 256, K = 256: F16, E5M2     */
+#define CRO_PRECISION_ANSWER_NARROW 3       /* 128 x 256, K = 256: F16ACC, HFMA2 */
+#define CRO_PRECISION_ANSWERS       4
+#define CRO_PRECISION_M             128
+#define CRO_PRECISION_N             256     /* F64 / DFMA: CRO_PRECISION_F64_N */
+#define CRO_PRECISION_K             256     /* F64 / DFMA / TF32: 128           */
+#define CRO_PRECISION_F64_N         64
+#define CRO_PRECISION_F64_K         128
+#define CRO_PRECISION_TF32_K        128
+#define CRO_PRECISION_RECORDS       4096    /* element records the device keeps per leg; counts stay exact beyond */
+#define CRO_PRECISION_MAX_SMS       256
+#define CRO_PRECISION_MAX_ITERATIONS      65536
+#define CRO_PRECISION_MAX_ALU_ITERATIONS  4096
+#define CRO_PRECISION_MAX_ROUNDS    64
+/* verdicts: CRO_COMPUTE_NONE / _SM / _ALL; marks: CRO_COMPUTE_PERSISTENT / _INTERMITTENT */
+
+typedef struct cro_precision_opts {
+    uint32_t iterations;           /*   0  F64, TF32, F16, F16ACC, E5M2: 0 = the default, at most CRO_PRECISION_MAX_ITERATIONS */
+    uint32_t alu_iterations;       /*   4  DFMA, HFMA2: 0 = the default, at most CRO_PRECISION_MAX_ALU_ITERATIONS             */
+    uint32_t legs;                 /*   8  CRO_PRECISION_ALL_LEGS bits; 0 = all                                                */
+    uint32_t max_rounds;           /*  12  launches per leg while fewer than sm_count SMs were seen: 0 = 4                     */
+    /* test only: as cro_compute_opts, the mask XORed into the element's own bits (64 for F64 / DFMA, 32 for the f32
+       accumulators, 16 for F16ACC / HFMA2; a mask wider than the leg's element is refused) */
+    int32_t  test_inject_leg;      /*  16 */
+    int32_t  test_inject_sm;       /*  20 */
+    uint32_t test_inject_iteration;/*  24 */
+    int32_t  test_inject_row;      /*  28 */
+    int32_t  test_inject_col;      /*  32 */
+    uint32_t reserved;             /*  36 */
+    uint64_t test_inject_mask;     /*  40 */
+} cro_precision_opts;              /*  48 bytes */
+
+typedef struct cro_precision_result {
+    int32_t  status;               /*   0  CRO_OK, or CRO_ERR_CHECKSUM on any mismatch or missing publish       */
+    uint32_t verdict;              /*   4  CRO_COMPUTE_NONE / _SM / _ALL                                        */
+    uint64_t seed;                 /*   8  operand seed of this call                                           */
+    uint64_t call;                 /*  16  k: the call's number on this device, from 0                         */
+    uint32_t sm_count;             /*  24 */
+    uint32_t legs;                 /*  28  legs run (CRO_PRECISION_ALL_LEGS bits)                               */
+    uint64_t host_ref_ns;          /*  32  host time to compute the four expected answers                       */
+    uint32_t nsmid;                /*  40 */
+    uint32_t bad_sms;              /*  44 */
+    uint16_t bad_sm[16];           /*  48 */
+    cro_compute_leg leg[CRO_PRECISION_LEGS];   /*  80  ops: 2 * M * N * K * iterations per CTA, the leg's own shape */
+} cro_precision_result;            /* 808 bytes */
+
+typedef struct cro_precision_sm {
+    uint32_t smid;                 /*   0 */
+    uint32_t reserved;             /*   4 */
+    cro_compute_sm_leg leg[CRO_PRECISION_LEGS];   /* 8 */
+} cro_precision_sm;                /* 288 bytes */
+
+typedef struct cro_precision_fault {
+    uint32_t leg;                  /*   0  CRO_PRECISION_LEG_*                                                  */
+    uint32_t smid;                 /*   4 */
+    uint32_t row;                  /*   8 */
+    uint32_t col;                  /*  12 */
+    int64_t  expected;             /*  16  the exact answer                                                     */
+    uint64_t actual_bits;          /*  24  the accumulator's raw bits (64, 32 or 16 of them, zero-extended)      */
+} cro_precision_fault;             /*  32 bytes */
+
+/* As cro_probe_compute: sms one entry per SM seen, faults sorted by (leg, smid, row, col). */
+int  cro_probe_precision(cro_ctx *ctx, int dev_index, const cro_precision_opts *opts, cro_precision_result *out,
+                         cro_precision_sm *sms, int sms_cap, int *n_sms, cro_precision_fault *faults, int cap, int *n);
+
+/* The same probe of any GPU on the node, run by `croprobe-cli precision-raw`; as cro_probe_compute_uuid. */
+int  cro_probe_precision_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_precision_opts *opts, int deadline_ms,
+                              cro_precision_result *out, cro_precision_sm *sms, int sms_cap, int *n_sms,
+                              cro_precision_fault *faults, int cap, int *n, uint64_t *helper_ns);
+
+/* The expected answer a call uploads: answer CRO_PRECISION_ANSWER_* of the operands of `seed`, as M * N int64 values
+ * (128 x 64 for _WIDE, 128 x 256 otherwise), row-major.  Host arithmetic only; no context. */
+int  cro_precision_expected(int answer, uint64_t seed, int64_t *out);
+
 /* ---- whole-HBM scan: every free byte of a GPU's memory, and its DRAM health record ---- */
 
 /*
@@ -1435,6 +1563,11 @@ int  cro_emit_link_annotations_json(const cro_link_result *r, char *buf, size_t 
  * -s8-gops, -bf16-gflops, -e4m3-gflops (ops / ns, integer division; 0 when ns is 0) and -slowest-sm ("<id>
  * <permille>" of the leg run with the largest slow_permille, the lowest leg on a tie). */
 int  cro_emit_compute_annotations_json(const cro_compute_result *r, char *buf, size_t cap, size_t *len);
+
+/* Additive precision annotations (cohdi.io/probe-precision-*) of a cro_probe_precision result, spelled as the compute
+ * probe's: -verdict, -sms, -bad-sms, -failed-legs (f64, dfma, tf32, f16, f16acc, e5m2, hfma2), -f64-gflops,
+ * -tf32-gflops, -f16-gflops, -f16acc-gflops, -e5m2-gflops (ops / ns, integer division; 0 when ns is 0) and -slowest-sm. */
+int  cro_emit_precision_annotations_json(const cro_precision_result *r, char *buf, size_t cap, size_t *len);
 
 /* Additive HBM scan annotations (cohdi.io/hbm-scan-*) of a cro_scan_hbm / cro_scan_hbm_uuid report, the same
  * Go-marshalled map, integers and fixed spellings only: -verdict ("ok" for CRO_OK, "corrupt" for CRO_ERR_CHECKSUM,
