@@ -952,18 +952,11 @@ def probe_l2_uuid(ctx: Optional["ProbeContext"], uuid: str, bytes: int = 0, iter
     """cro_probe_l2_uuid: the L2 probe of any GPU on the node, run by the helper process (ctx may be None).
     Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up to `cap` records."""
     o = _l2_opts(bytes, iterations, a1_counters, a2_counters, deadline_ms, inject)
-    r = L2Result()
-    sms = (L2Sm * L2_MAX_SMS)()
-    arr = (L2Fault * max(1, cap))()
-    n_sms, n = ctypes.c_int(), ctypes.c_int()
     handle = ctx.handle if ctx is not None else None
-    rc = lib.cro_probe_l2_uuid(handle, _b(uuid), ctypes.byref(o), ctypes.byref(r), sms, L2_MAX_SMS, ctypes.byref(n_sms),
-                               arr, cap, ctypes.byref(n))
+    rc, out = _per_sm(lib.cro_probe_l2_uuid, (handle, _b(uuid), ctypes.byref(o)), L2Result, L2Sm, L2_MAX_SMS, L2Fault, cap)
     if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
-        buf = ctypes.create_string_buffer(1024)
-        lib.cro_last_error(handle, buf, 1024)
-        raise ProbeError(rc, buf.value.decode("utf-8", "replace"))
-    return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
+        raise _helper_error(rc, handle)
+    return out
 
 
 def selftest_l2_classify(r: L2Result, sms: List[L2Sm], faults: List[L2Fault]) -> Tuple[L2Result, List[L2Sm], List[L2Fault]]:
@@ -993,24 +986,30 @@ def probe_sram_uuid(ctx: Optional["ProbeContext"], uuid: str, legs: int = SRAM_A
     """cro_probe_sram_uuid: the SRAM probe of any GPU on the node, run by the helper process (ctx may be None).
     Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up to `cap` records."""
     o = _sram_opts(legs, iterations, cluster, max_rounds, deadline_ms, inject)
-    r = SramResult()
-    sms = (SramSm * SRAM_MAX_SMS)()
-    arr = (SramFault * max(1, cap))()
-    n_sms, n = ctypes.c_int(), ctypes.c_int()
     handle = ctx.handle if ctx is not None else None
-    rc = lib.cro_probe_sram_uuid(handle, _b(uuid), ctypes.byref(o), ctypes.byref(r), sms, SRAM_MAX_SMS, ctypes.byref(n_sms),
-                                 arr, cap, ctypes.byref(n))
+    rc, out = _per_sm(lib.cro_probe_sram_uuid, (handle, _b(uuid), ctypes.byref(o)), SramResult, SramSm, SRAM_MAX_SMS, SramFault,
+                      cap)
     if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
-        buf = ctypes.create_string_buffer(1024)
-        lib.cro_last_error(handle, buf, 1024)
-        raise ProbeError(rc, buf.value.decode("utf-8", "replace"))
-    return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
+        raise _helper_error(rc, handle)
+    return out
 
 
 def _helper_error(rc: int, handle) -> "ProbeError":
     buf = ctypes.create_string_buffer(1024)
     lib.cro_last_error(handle, buf, 1024)
     return ProbeError(rc, buf.value.decode("utf-8", "replace"))
+
+
+def _per_sm(fn, head: tuple, result, sm, max_sms: int, fault, cap: int, tail: tuple = ()):
+    """One call of a per-SM probe (compute, precision, SRAM, L2; in process or by UUID):
+    fn(*head, result, sms, max_sms, n_sms, faults, cap, n, *tail) on fresh arrays.  Returns the return code and
+    (result, the SM entries, the faults)."""
+    r = result()
+    sms = (sm * max_sms)()
+    arr = (fault * max(1, cap))()
+    n_sms, n = ctypes.c_int(), ctypes.c_int()
+    rc = fn(*head, ctypes.byref(r), sms, max_sms, ctypes.byref(n_sms), arr, cap, ctypes.byref(n), *tail)
+    return rc, (r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)])
 
 
 def _link_opts(bytes: int, hops: int, ctas: int, inject: Optional[Tuple[int, int, int]]) -> LinkOpts:
@@ -1057,16 +1056,13 @@ def probe_compute_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: int
     Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen, up to `cap` element records
     and the helper's spawn-to-exit time in ns."""
     o = _compute_opts(iterations, alu_iterations, legs, max_rounds, inject)
-    r = ComputeResult()
-    sms = (ComputeSm * COMPUTE_MAX_SMS)()
-    arr = (ComputeFault * max(1, cap))()
-    n_sms, n, ns = ctypes.c_int(), ctypes.c_int(), ctypes.c_uint64()
+    ns = ctypes.c_uint64()
     handle = ctx.handle if ctx is not None else None
-    rc = lib.cro_probe_compute_uuid(handle, _b(uuid), ctypes.byref(o), deadline_ms, ctypes.byref(r), sms, COMPUTE_MAX_SMS,
-                                    ctypes.byref(n_sms), arr, cap, ctypes.byref(n), ctypes.byref(ns))
+    rc, out = _per_sm(lib.cro_probe_compute_uuid, (handle, _b(uuid), ctypes.byref(o), deadline_ms), ComputeResult, ComputeSm,
+                      COMPUTE_MAX_SMS, ComputeFault, cap, (ctypes.byref(ns),))
     if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
         raise _helper_error(rc, handle)
-    return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)], ns.value
+    return out + (ns.value,)
 
 
 def _precision_opts(iterations: int, alu_iterations: int, legs: int, max_rounds: int,
@@ -1087,16 +1083,13 @@ def probe_precision_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: i
     Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen, up to `cap` element records
     and the helper's spawn-to-exit time in ns."""
     o = _precision_opts(iterations, alu_iterations, legs, max_rounds, inject)
-    r = PrecisionResult()
-    sms = (PrecisionSm * PRECISION_MAX_SMS)()
-    arr = (PrecisionFault * max(1, cap))()
-    n_sms, n, ns = ctypes.c_int(), ctypes.c_int(), ctypes.c_uint64()
+    ns = ctypes.c_uint64()
     handle = ctx.handle if ctx is not None else None
-    rc = lib.cro_probe_precision_uuid(handle, _b(uuid), ctypes.byref(o), deadline_ms, ctypes.byref(r), sms, PRECISION_MAX_SMS,
-                                      ctypes.byref(n_sms), arr, cap, ctypes.byref(n), ctypes.byref(ns))
+    rc, out = _per_sm(lib.cro_probe_precision_uuid, (handle, _b(uuid), ctypes.byref(o), deadline_ms), PrecisionResult,
+                      PrecisionSm, PRECISION_MAX_SMS, PrecisionFault, cap, (ctypes.byref(ns),))
     if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
         raise _helper_error(rc, handle)
-    return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)], ns.value
+    return out + (ns.value,)
 
 
 def _scan_opts(max_bytes: int, reserve_bytes: int, seed: int, deadline_ms: int, chunk_bytes: int,
@@ -1120,9 +1113,7 @@ def scan_hbm_uuid(ctx: Optional["ProbeContext"], uuid: str, max_bytes: int = 0, 
     handle = ctx.handle if ctx is not None else None
     rc = lib.cro_scan_hbm_uuid(handle, _b(uuid), ctypes.byref(o), ctypes.byref(rep), arr, cap, ctypes.byref(n))
     if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
-        buf = ctypes.create_string_buffer(1024)
-        lib.cro_last_error(handle, buf, 1024)
-        raise ProbeError(rc, buf.value.decode("utf-8", "replace"))
+        raise _helper_error(rc, handle)
     return rep, [arr[i] for i in range(n.value)]
 
 
@@ -1369,13 +1360,10 @@ class ProbeContext:
         inject = (leg, sm, iteration, row, col, mask) is the test-only wrong answer (sm, row, col: -1 for every one).
         Returns the result (its status is OK or ERR_CHECKSUM), one entry per SM seen and up to `cap` element records."""
         o = _compute_opts(iterations, alu_iterations, legs, max_rounds, inject)
-        r = ComputeResult()
-        sms = (ComputeSm * COMPUTE_MAX_SMS)()
-        arr = (ComputeFault * max(1, cap))()
-        n_sms, n = ctypes.c_int(), ctypes.c_int()
-        self._check(lib.cro_probe_compute(self.handle, dev, ctypes.byref(o), ctypes.byref(r), sms, COMPUTE_MAX_SMS,
-                                          ctypes.byref(n_sms), arr, cap, ctypes.byref(n)), allow=(ERR_CHECKSUM,))
-        return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
+        rc, out = _per_sm(lib.cro_probe_compute, (self.handle, dev, ctypes.byref(o)), ComputeResult, ComputeSm, COMPUTE_MAX_SMS,
+                          ComputeFault, cap)
+        self._check(rc, allow=(ERR_CHECKSUM,))
+        return out
 
     def probe_precision(self, dev: int = 0, iterations: int = 0, alu_iterations: int = 0, legs: int = PRECISION_ALL_LEGS,
                         max_rounds: int = 0, inject: Optional[Tuple[int, int, int, int, int, int]] = None,
@@ -1386,13 +1374,10 @@ class ProbeContext:
         test-only wrong answer (sm, row, col: -1 for every one; mask up to the leg's element width).  Returns the result
         (its status is OK or ERR_CHECKSUM), one entry per SM seen and up to `cap` element records."""
         o = _precision_opts(iterations, alu_iterations, legs, max_rounds, inject)
-        r = PrecisionResult()
-        sms = (PrecisionSm * PRECISION_MAX_SMS)()
-        arr = (PrecisionFault * max(1, cap))()
-        n_sms, n = ctypes.c_int(), ctypes.c_int()
-        self._check(lib.cro_probe_precision(self.handle, dev, ctypes.byref(o), ctypes.byref(r), sms, PRECISION_MAX_SMS,
-                                            ctypes.byref(n_sms), arr, cap, ctypes.byref(n)), allow=(ERR_CHECKSUM,))
-        return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
+        rc, out = _per_sm(lib.cro_probe_precision, (self.handle, dev, ctypes.byref(o)), PrecisionResult, PrecisionSm,
+                          PRECISION_MAX_SMS, PrecisionFault, cap)
+        self._check(rc, allow=(ERR_CHECKSUM,))
+        return out
 
     def scan_hbm(self, dev: int = 0, max_bytes: int = 0, reserve_bytes: int = 0, seed: int = 0, cap: int = 256,
                  chunk_bytes: int = 0, force: Optional[Tuple[int, int, int, int]] = None) -> Tuple[ScanReport, List[FaultWord]]:
@@ -1418,13 +1403,9 @@ class ProbeContext:
         bad cell (sm, word: -1 for every one).  Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry
         per SM seen and up to `cap` word records."""
         o = _sram_opts(legs, iterations, cluster, max_rounds, 0, inject)
-        r = SramResult()
-        sms = (SramSm * SRAM_MAX_SMS)()
-        arr = (SramFault * max(1, cap))()
-        n_sms, n = ctypes.c_int(), ctypes.c_int()
-        self._check(lib.cro_probe_sram(self.handle, dev, ctypes.byref(o), ctypes.byref(r), sms, SRAM_MAX_SMS, ctypes.byref(n_sms),
-                                       arr, cap, ctypes.byref(n)), allow=(ERR_CHECKSUM, ERR_CUDA))
-        return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
+        rc, out = _per_sm(lib.cro_probe_sram, (self.handle, dev, ctypes.byref(o)), SramResult, SramSm, SRAM_MAX_SMS, SramFault, cap)
+        self._check(rc, allow=(ERR_CHECKSUM, ERR_CUDA))
+        return out
 
     def probe_l2(self, dev: int = 0, bytes: int = 0, iterations: int = 0, a1_counters: int = 0, a2_counters: int = 0,
                  inject: Optional[Tuple[int, int, int, int, int, int]] = None,
@@ -1435,13 +1416,9 @@ class ProbeContext:
         word -1 for every one; L2_A1 / L2_A2: word is the counter).  Returns the result (its status is OK,
         ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up to `cap` word records."""
         o = _l2_opts(bytes, iterations, a1_counters, a2_counters, 0, inject)
-        r = L2Result()
-        sms = (L2Sm * L2_MAX_SMS)()
-        arr = (L2Fault * max(1, cap))()
-        n_sms, n = ctypes.c_int(), ctypes.c_int()
-        self._check(lib.cro_probe_l2(self.handle, dev, ctypes.byref(o), ctypes.byref(r), sms, L2_MAX_SMS, ctypes.byref(n_sms),
-                                     arr, cap, ctypes.byref(n)), allow=(ERR_CHECKSUM, ERR_CUDA))
-        return r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)]
+        rc, out = _per_sm(lib.cro_probe_l2, (self.handle, dev, ctypes.byref(o)), L2Result, L2Sm, L2_MAX_SMS, L2Fault, cap)
+        self._check(rc, allow=(ERR_CHECKSUM, ERR_CUDA))
+        return out
 
     def launch_count(self) -> int:
         return int(lib.cro_launch_count(self.handle))

@@ -106,6 +106,43 @@ int on_exception() noexcept {
         return CRO_ERR_INTERNAL;
     }
 }
+
+// The four per-SM probes (compute, precision, SRAM, L2), in process and by UUID, share their C side: the argument
+// check (target: the context, or the GPU's UUID), opts' defaults, *n_sms and *n zeroed, then run(o, &seen, &found)
+// and sms[0 .. sms_cap) and faults[0 .. cap) copied out.  copied is false when the arguments were refused: nothing
+// ran and nothing was written.
+struct PerSmCopy {
+    int rc;
+    bool copied;
+    size_t sms, faults;
+};
+template <class Opts, class Sm, class Fault, class Run>
+PerSmCopy per_sm_call(const void* target, const void* out, const Opts* opts, Sm* sms, int sms_cap, int* n_sms,
+                      Fault* faults, int cap, int* n, Run run) {
+    if (!target || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
+        return {CRO_ERR_INVALID_ARG, false, 0, 0};
+    *n = *n_sms = 0;
+    Opts o{};
+    if (opts) o = *opts;
+    std::vector<Sm> seen;
+    std::vector<Fault> found;
+    const int rc = run(o, &seen, &found);
+    const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
+    for (size_t j = 0; j < ks; ++j) sms[j] = seen[j];
+    for (size_t j = 0; j < kf; ++j) faults[j] = found[j];
+    *n_sms = (int)ks;
+    *n = (int)kf;
+    return {rc, true, ks, kf};
+}
+// The SRAM and L2 results also say how much the caller got: sms_listed and recorded.
+template <class Result>
+int listed(const PerSmCopy& k, Result* out) {
+    if (k.copied) {
+        out->sms_listed = (uint32_t)k.sms;
+        out->recorded = k.faults;
+    }
+    return k.rc;
+}
 }  // namespace capi
 }  // namespace cro
 
@@ -356,81 +393,39 @@ int cro_probe_host_link_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_link_
     if (helper_ns) *helper_ns = ns;
     return rc;
 } CRO_API_CATCH
-// The compute probe's two forms share the copy-out: sms[0 .. sms_cap) and faults[0 .. cap).
-static int compute_out(int rc, const std::vector<cro_compute_sm>& seen, const std::vector<cro_compute_fault>& found,
-                       cro_compute_sm* sms, int sms_cap, int* n_sms, cro_compute_fault* faults, int cap, int* n) {
-    const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
-    for (size_t j = 0; j < ks; ++j) sms[j] = seen[j];
-    for (size_t j = 0; j < kf; ++j) faults[j] = found[j];
-    *n_sms = (int)ks;
-    *n = (int)kf;
-    return rc;
-}
 int cro_probe_compute(cro_ctx* ctx, int i, const cro_compute_opts* opts, cro_compute_result* out, cro_compute_sm* sms,
                       int sms_cap, int* n_sms, cro_compute_fault* faults, int cap, int* n) try {
-    if (!ctx || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
-        return CRO_ERR_INVALID_ARG;
-    *n = *n_sms = 0;
-    cro_compute_opts o{};
-    if (opts) o = *opts;
-    std::vector<cro_compute_sm> seen;
-    std::vector<cro_compute_fault> found;
-    const int rc = ctx_probe_compute(ctx, i, o, out, &seen, &found);
-    return compute_out(rc, seen, found, sms, sms_cap, n_sms, faults, cap, n);
+    return per_sm_call(ctx, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_compute_opts& o, auto* seen, auto* found) {
+        return ctx_probe_compute(ctx, i, o, out, seen, found);
+    }).rc;
 } CRO_API_CATCH
 int cro_probe_compute_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_compute_opts* opts, int deadline_ms,
                            cro_compute_result* out, cro_compute_sm* sms, int sms_cap, int* n_sms, cro_compute_fault* faults,
                            int cap, int* n, uint64_t* helper_ns) try {
-    if (!gpu_uuid || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
-        return CRO_ERR_INVALID_ARG;
-    *n = *n_sms = 0;
-    if (helper_ns) *helper_ns = 0;
-    cro_compute_opts o{};
-    if (opts) o = *opts;
-    std::vector<cro_compute_sm> seen;
-    std::vector<cro_compute_fault> found;
-    uint64_t ns = 0;
-    const int rc = ctx_probe_compute_uuid(ctx, gpu_uuid, o, deadline_ms, out, &seen, &found, cap, &ns);
-    if (helper_ns) *helper_ns = ns;
-    return compute_out(rc, seen, found, sms, sms_cap, n_sms, faults, cap, n);
+    return per_sm_call(gpu_uuid, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_compute_opts& o, auto* seen, auto* found) {
+        uint64_t ns = 0;
+        if (helper_ns) *helper_ns = 0;
+        const int rc = ctx_probe_compute_uuid(ctx, gpu_uuid, o, deadline_ms, out, seen, found, cap, &ns);
+        if (helper_ns) *helper_ns = ns;
+        return rc;
+    }).rc;
 } CRO_API_CATCH
-// The precision probe's two forms share the copy-out: sms[0 .. sms_cap) and faults[0 .. cap).
-static int precision_out(int rc, const std::vector<cro_precision_sm>& seen, const std::vector<cro_precision_fault>& found,
-                         cro_precision_sm* sms, int sms_cap, int* n_sms, cro_precision_fault* faults, int cap, int* n) {
-    const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
-    for (size_t j = 0; j < ks; ++j) sms[j] = seen[j];
-    for (size_t j = 0; j < kf; ++j) faults[j] = found[j];
-    *n_sms = (int)ks;
-    *n = (int)kf;
-    return rc;
-}
 int cro_probe_precision(cro_ctx* ctx, int i, const cro_precision_opts* opts, cro_precision_result* out, cro_precision_sm* sms,
                         int sms_cap, int* n_sms, cro_precision_fault* faults, int cap, int* n) try {
-    if (!ctx || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
-        return CRO_ERR_INVALID_ARG;
-    *n = *n_sms = 0;
-    cro_precision_opts o{};
-    if (opts) o = *opts;
-    std::vector<cro_precision_sm> seen;
-    std::vector<cro_precision_fault> found;
-    const int rc = ctx_probe_precision(ctx, i, o, out, &seen, &found);
-    return precision_out(rc, seen, found, sms, sms_cap, n_sms, faults, cap, n);
+    return per_sm_call(ctx, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_precision_opts& o, auto* seen, auto* found) {
+        return ctx_probe_precision(ctx, i, o, out, seen, found);
+    }).rc;
 } CRO_API_CATCH
 int cro_probe_precision_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_precision_opts* opts, int deadline_ms,
                              cro_precision_result* out, cro_precision_sm* sms, int sms_cap, int* n_sms,
                              cro_precision_fault* faults, int cap, int* n, uint64_t* helper_ns) try {
-    if (!gpu_uuid || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
-        return CRO_ERR_INVALID_ARG;
-    *n = *n_sms = 0;
-    if (helper_ns) *helper_ns = 0;
-    cro_precision_opts o{};
-    if (opts) o = *opts;
-    std::vector<cro_precision_sm> seen;
-    std::vector<cro_precision_fault> found;
-    uint64_t ns = 0;
-    const int rc = ctx_probe_precision_uuid(ctx, gpu_uuid, o, deadline_ms, out, &seen, &found, cap, &ns);
-    if (helper_ns) *helper_ns = ns;
-    return precision_out(rc, seen, found, sms, sms_cap, n_sms, faults, cap, n);
+    return per_sm_call(gpu_uuid, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_precision_opts& o, auto* seen, auto* found) {
+        uint64_t ns = 0;
+        if (helper_ns) *helper_ns = 0;
+        const int rc = ctx_probe_precision_uuid(ctx, gpu_uuid, o, deadline_ms, out, seen, found, cap, &ns);
+        if (helper_ns) *helper_ns = ns;
+        return rc;
+    }).rc;
 } CRO_API_CATCH
 // The scan's two forms share the copy-out: words[0 .. cap), recorded and complete as cro_locate_faults sets them.
 static int scan_out(int rc, const std::vector<cro_fault_word>& found, cro_scan_report* out, cro_fault_word* words, int cap, int* n) {
@@ -468,84 +463,34 @@ int cro_read_hbm_health(const char* gpu_uuid, cro_hbm_health* out) try {
     identity::NvmlHbmHealth(gpu_uuid, true, out);
     return CRO_OK;
 } CRO_API_CATCH
-// The SRAM probe's two forms share the copy-out: sms[0 .. sms_cap) and faults[0 .. cap), and what was written in
-// sms_listed and recorded.
-static int sram_out(int rc, const std::vector<cro_sram_sm>& seen, const std::vector<cro_sram_fault>& found, cro_sram_result* out,
-                    cro_sram_sm* sms, int sms_cap, int* n_sms, cro_sram_fault* faults, int cap, int* n) {
-    const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
-    for (size_t j = 0; j < ks; ++j) sms[j] = seen[j];
-    for (size_t j = 0; j < kf; ++j) faults[j] = found[j];
-    out->sms_listed = (uint32_t)ks;
-    out->recorded = kf;
-    *n_sms = (int)ks;
-    *n = (int)kf;
-    return rc;
-}
 int cro_probe_sram(cro_ctx* ctx, int i, const cro_sram_opts* opts, cro_sram_result* out, cro_sram_sm* sms, int sms_cap,
                    int* n_sms, cro_sram_fault* faults, int cap, int* n) try {
-    if (!ctx || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
-        return CRO_ERR_INVALID_ARG;
-    *n = *n_sms = 0;
-    cro_sram_opts o{};
-    if (opts) o = *opts;
-    std::vector<cro_sram_sm> seen;
-    std::vector<cro_sram_fault> found;
-    const int rc = ctx_probe_sram(ctx, i, o, out, &seen, &found);
-    return sram_out(rc, seen, found, out, sms, sms_cap, n_sms, faults, cap, n);
+    return listed(per_sm_call(ctx, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_sram_opts& o, auto* seen, auto* found) {
+        return ctx_probe_sram(ctx, i, o, out, seen, found);
+    }), out);
 } CRO_API_CATCH
 int cro_probe_sram_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_sram_opts* opts, cro_sram_result* out, cro_sram_sm* sms,
                         int sms_cap, int* n_sms, cro_sram_fault* faults, int cap, int* n) try {
-    if (!gpu_uuid || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
-        return CRO_ERR_INVALID_ARG;
-    *n = *n_sms = 0;
-    cro_sram_opts o{};
-    if (opts) o = *opts;
-    std::vector<cro_sram_sm> seen;
-    std::vector<cro_sram_fault> found;
-    const int rc = ctx_probe_sram_uuid(ctx, gpu_uuid, o, out, &seen, &found, cap);
-    return sram_out(rc, seen, found, out, sms, sms_cap, n_sms, faults, cap, n);
+    return listed(per_sm_call(gpu_uuid, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_sram_opts& o, auto* seen, auto* found) {
+        return ctx_probe_sram_uuid(ctx, gpu_uuid, o, out, seen, found, cap);
+    }), out);
 } CRO_API_CATCH
 int cro_read_sram_health(const char* gpu_uuid, cro_sram_health* out) try {
     if (!gpu_uuid || !out) return CRO_ERR_INVALID_ARG;
     identity::NvmlSramHealth(gpu_uuid, true, out);
     return CRO_OK;
 } CRO_API_CATCH
-// The L2 probe's two forms share the copy-out: sms[0 .. sms_cap) and faults[0 .. cap), and what was written in
-// sms_listed and recorded.
-static int l2_out(int rc, const std::vector<cro_l2_sm>& seen, const std::vector<cro_l2_fault>& found, cro_l2_result* out,
-                  cro_l2_sm* sms, int sms_cap, int* n_sms, cro_l2_fault* faults, int cap, int* n) {
-    const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
-    for (size_t j = 0; j < ks; ++j) sms[j] = seen[j];
-    for (size_t j = 0; j < kf; ++j) faults[j] = found[j];
-    out->sms_listed = (uint32_t)ks;
-    out->recorded = kf;
-    *n_sms = (int)ks;
-    *n = (int)kf;
-    return rc;
-}
 int cro_probe_l2(cro_ctx* ctx, int i, const cro_l2_opts* opts, cro_l2_result* out, cro_l2_sm* sms, int sms_cap, int* n_sms,
                  cro_l2_fault* faults, int cap, int* n) try {
-    if (!ctx || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
-        return CRO_ERR_INVALID_ARG;
-    *n = *n_sms = 0;
-    cro_l2_opts o{};
-    if (opts) o = *opts;
-    std::vector<cro_l2_sm> seen;
-    std::vector<cro_l2_fault> found;
-    const int rc = ctx_probe_l2(ctx, i, o, out, &seen, &found);
-    return l2_out(rc, seen, found, out, sms, sms_cap, n_sms, faults, cap, n);
+    return listed(per_sm_call(ctx, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_l2_opts& o, auto* seen, auto* found) {
+        return ctx_probe_l2(ctx, i, o, out, seen, found);
+    }), out);
 } CRO_API_CATCH
 int cro_probe_l2_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_l2_opts* opts, cro_l2_result* out, cro_l2_sm* sms,
                       int sms_cap, int* n_sms, cro_l2_fault* faults, int cap, int* n) try {
-    if (!gpu_uuid || !out || !n || !n_sms || cap < 0 || sms_cap < 0 || (cap > 0 && !faults) || (sms_cap > 0 && !sms))
-        return CRO_ERR_INVALID_ARG;
-    *n = *n_sms = 0;
-    cro_l2_opts o{};
-    if (opts) o = *opts;
-    std::vector<cro_l2_sm> seen;
-    std::vector<cro_l2_fault> found;
-    const int rc = ctx_probe_l2_uuid(ctx, gpu_uuid, o, out, &seen, &found, cap);
-    return l2_out(rc, seen, found, out, sms, sms_cap, n_sms, faults, cap, n);
+    return listed(per_sm_call(gpu_uuid, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_l2_opts& o, auto* seen, auto* found) {
+        return ctx_probe_l2_uuid(ctx, gpu_uuid, o, out, seen, found, cap);
+    }), out);
 } CRO_API_CATCH
 int cro_read_l2_health(const char* gpu_uuid, cro_l2_health* out) try {
     if (!gpu_uuid || !out) return CRO_ERR_INVALID_ARG;

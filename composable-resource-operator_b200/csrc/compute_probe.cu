@@ -160,22 +160,6 @@ int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_comput
     return close_call(r, CRO_COMPUTE_LEGS, per_sm, sms, faults);
 }
 
-namespace {
-// compute-raw's stdout: the result, the helper's own counts n_sms and n, CRO_COMPUTE_MAX_SMS per-SM entries (n_sms of
-// them filled), then n faults.  An n_sms the entries cannot hold makes the output malformed.
-constexpr size_t kComputeCounts = sizeof(cro_compute_result);
-constexpr size_t kComputeSms = kComputeCounts + 2 * sizeof(uint64_t);
-constexpr size_t kComputeHead = kComputeSms + CRO_COMPUTE_MAX_SMS * sizeof(cro_compute_sm);
-uint64_t compute_count(const unsigned char* head, int which) {
-    uint64_t v;
-    memcpy(&v, head + kComputeCounts + which * sizeof v, sizeof v);
-    return v;
-}
-uint64_t compute_tail_count(const unsigned char* head) {
-    return compute_count(head, 0) > CRO_COMPUTE_MAX_SMS ? ~0ull : compute_count(head, 1);
-}
-}  // namespace
-
 int ctx_probe_compute_uuid(cro_ctx* c, const char* uuid, const cro_compute_opts& o, int deadline_ms, cro_compute_result* r,
                            std::vector<cro_compute_sm>* sms, std::vector<cro_compute_fault>* faults, int cap, uint64_t* helper_ns) {
     blank_result(r, cro_compute_result{}, sms, faults);
@@ -192,19 +176,13 @@ int ctx_probe_compute_uuid(cro_ctx* c, const char* uuid, const cro_compute_opts&
                                            num(o.alu_iterations), num(o.legs), num(o.max_rounds), num(o.test_inject_leg),
                                            num(o.test_inject_sm), num(o.test_inject_iteration), num(o.test_inject_row),
                                            num(o.test_inject_col), num(o.test_inject_mask), num(cap)};
+    using Frame = SmFrame<cro_compute_result, cro_compute_sm, cro_compute_fault, CRO_COMPUTE_MAX_SMS>;
     std::string got;
-    int rc = run_probe_helper(c, want, "compute helper", "cro.probe_compute.helper", args, deadline_ms, kComputeHead,
-                              sizeof(cro_compute_fault), (size_t)cap, compute_tail_count, &got, helper_ns);
+    const int rc = run_probe_helper(c, want, "compute helper", "cro.probe_compute.helper", args, deadline_ms, Frame::kHead,
+                                    sizeof(cro_compute_fault), (size_t)cap, Frame::tail, &got, helper_ns);
     if (rc != CRO_OK) return r->status = rc;
-    const unsigned char* head = reinterpret_cast<const unsigned char*>(got.data());
-    memcpy(r, head, sizeof *r);
-    const cro_compute_sm* s = reinterpret_cast<const cro_compute_sm*>(head + kComputeSms);
-    sms->assign(s, s + compute_count(head, 0));
-    const cro_compute_fault* f = reinterpret_cast<const cro_compute_fault*>(head + kComputeHead);
-    faults->assign(f, f + compute_count(head, 1));
-    rc = r->status;
-    if (rc != CRO_OK && rc != CRO_ERR_CHECKSUM) set_call_error(c, "compute helper for " + want + ": " + cro_strerror(rc));
-    return rc;
+    Frame::read(got, r, sms, faults);
+    return r->status;
 }
 
 }  // namespace cro

@@ -78,6 +78,199 @@ static int fail(cro_ctx *ctx, const char *what, int rc) {
     return 2;
 }
 
+static char buf[1 << 16];
+
+/* A raw command's stdout, the result whatever its status (the library reads why from it): the result, n_counts counts
+ * of the helper's own, the per-SM block and n records of rec_bytes each, the empty parts left out.  Then it exits 0 iff
+ * the status is CRO_OK and 1 for any other, skipping the teardown (it costs as much as a probe): the process's buffers
+ * and allocations go with it.  2 when stdout takes less. */
+static int write_frame(const void *result, size_t result_bytes, const uint64_t *counts, size_t n_counts, const void *sms,
+                       size_t sms_bytes, const void *records, size_t rec_bytes, int n, int status) {
+    if (fwrite(result, result_bytes, 1, stdout) != 1 || (n_counts && fwrite(counts, sizeof *counts, n_counts, stdout) != n_counts) ||
+        (sms_bytes && fwrite(sms, sms_bytes, 1, stdout) != 1) || (n > 0 && fwrite(records, rec_bytes, (size_t)n, stdout) != (size_t)n))
+        return 2;
+    fflush(stdout);
+    _exit(status == CRO_OK ? 0 : 1);
+}
+
+/* The raw commands: each fills its probe's options from argv, runs the probe on device idx and writes its frame. */
+static int scan_raw(cro_ctx *ctx, int idx, char **argv) {
+    cro_scan_opts so;
+    memset(&so, 0, sizeof so);
+    uint64_t *f[] = {&so.max_bytes, &so.reserve_bytes, &so.seed, &so.test_chunk_bytes, &so.test_force_first,
+                     &so.test_force_count, &so.test_force_and, &so.test_force_or};
+    for (int k = 0; k < 8; ++k) *f[k] = (uint64_t)strtoull(argv[3 + k], NULL, 10);
+    const int cap = atoi(argv[11]);
+    static cro_scan_report sr;
+    cro_fault_word *words = (cro_fault_word *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *words);
+    int got = 0;
+    if (!words) return 2;
+    cro_scan_hbm(ctx, idx, &so, &sr, words, cap, &got);
+    return write_frame(&sr, sizeof sr, NULL, 0, NULL, 0, words, sizeof *words, got, sr.status);
+}
+
+static int sram_raw(cro_ctx *ctx, int idx, char **argv) {
+    cro_sram_opts so;
+    memset(&so, 0, sizeof so);
+    so.legs = (uint32_t)strtoul(argv[3], NULL, 10);
+    so.iterations = (uint32_t)strtoul(argv[4], NULL, 10);
+    so.cluster = (uint32_t)strtoul(argv[5], NULL, 10);
+    so.max_rounds = (uint32_t)strtoul(argv[6], NULL, 10);
+    so.test_inject_leg = atoi(argv[7]);
+    so.test_inject_sm = atoi(argv[8]);
+    so.test_inject_element = (uint32_t)strtoul(argv[9], NULL, 10);
+    so.test_inject_iteration = (uint32_t)strtoul(argv[10], NULL, 10);
+    so.test_inject_word = atoi(argv[11]);
+    so.test_inject_mask = (uint64_t)strtoull(argv[12], NULL, 10);
+    const int cap = atoi(argv[13]);
+    static cro_sram_result sr;
+    static cro_sram_sm sms[CRO_SRAM_MAX_SMS];
+    cro_sram_fault *faults = (cro_sram_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
+    int n_sms = 0, got = 0;
+    if (!faults) return 2;
+    cro_probe_sram(ctx, idx, &so, &sr, sms, CRO_SRAM_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
+    return write_frame(&sr, sizeof sr, NULL, 0, sms, sizeof sms, faults, sizeof *faults, got, sr.status);
+}
+
+static int link_raw(cro_ctx *ctx, int idx, char **argv) {
+    cro_link_opts lo;
+    memset(&lo, 0, sizeof lo);
+    lo.bytes = (uint64_t)strtoull(argv[4], NULL, 10);
+    lo.hops = (uint32_t)strtoul(argv[5], NULL, 10);
+    lo.ctas = (uint32_t)strtoul(argv[6], NULL, 10);
+    lo.test_inject_check = atoi(argv[7]);
+    lo.test_inject_word = (uint64_t)strtoull(argv[8], NULL, 10);
+    lo.test_inject_mask = (uint64_t)strtoull(argv[9], NULL, 10);
+    const int cap = atoi(argv[10]);
+    static cro_link_result lr;
+    cro_link_fault *faults = (cro_link_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
+    int got = 0;
+    if (!faults) return 2;
+    cro_probe_host_link(ctx, idx, &lo, &lr, faults, cap > 0 ? cap : 0, &got);
+    const uint64_t n_out = (uint64_t)got;
+    return write_frame(&lr, sizeof lr, &n_out, 1, NULL, 0, faults, sizeof *faults, got, lr.status);
+}
+
+static int compute_raw(cro_ctx *ctx, int idx, char **argv) {
+    cro_compute_opts co;
+    memset(&co, 0, sizeof co);
+    co.iterations = (uint32_t)strtoul(argv[4], NULL, 10);
+    co.alu_iterations = (uint32_t)strtoul(argv[5], NULL, 10);
+    co.legs = (uint32_t)strtoul(argv[6], NULL, 10);
+    co.max_rounds = (uint32_t)strtoul(argv[7], NULL, 10);
+    co.test_inject_leg = atoi(argv[8]);
+    co.test_inject_sm = atoi(argv[9]);
+    co.test_inject_iteration = (uint32_t)strtoul(argv[10], NULL, 10);
+    co.test_inject_row = atoi(argv[11]);
+    co.test_inject_col = atoi(argv[12]);
+    co.test_inject_mask = (uint32_t)strtoul(argv[13], NULL, 10);
+    const int cap = atoi(argv[14]);
+    static cro_compute_result cr;
+    static cro_compute_sm sms[CRO_COMPUTE_MAX_SMS];
+    cro_compute_fault *faults = (cro_compute_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
+    int n_sms = 0, got = 0;
+    if (!faults) return 2;
+    cro_probe_compute(ctx, idx, &co, &cr, sms, CRO_COMPUTE_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
+    const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)got};
+    return write_frame(&cr, sizeof cr, counts, 2, sms, sizeof sms, faults, sizeof *faults, got, cr.status);
+}
+
+static int precision_raw(cro_ctx *ctx, int idx, char **argv) {
+    cro_precision_opts po;
+    memset(&po, 0, sizeof po);
+    po.iterations = (uint32_t)strtoul(argv[4], NULL, 10);
+    po.alu_iterations = (uint32_t)strtoul(argv[5], NULL, 10);
+    po.legs = (uint32_t)strtoul(argv[6], NULL, 10);
+    po.max_rounds = (uint32_t)strtoul(argv[7], NULL, 10);
+    po.test_inject_leg = atoi(argv[8]);
+    po.test_inject_sm = atoi(argv[9]);
+    po.test_inject_iteration = (uint32_t)strtoul(argv[10], NULL, 10);
+    po.test_inject_row = atoi(argv[11]);
+    po.test_inject_col = atoi(argv[12]);
+    po.test_inject_mask = (uint64_t)strtoull(argv[13], NULL, 10);
+    const int cap = atoi(argv[14]);
+    static cro_precision_result pr;
+    static cro_precision_sm sms[CRO_PRECISION_MAX_SMS];
+    cro_precision_fault *faults = (cro_precision_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
+    int n_sms = 0, got = 0;
+    if (!faults) return 2;
+    cro_probe_precision(ctx, idx, &po, &pr, sms, CRO_PRECISION_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
+    const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)got};
+    return write_frame(&pr, sizeof pr, counts, 2, sms, sizeof sms, faults, sizeof *faults, got, pr.status);
+}
+
+static int l2_raw(cro_ctx *ctx, int idx, char **argv) {
+    cro_l2_opts lo;
+    memset(&lo, 0, sizeof lo);
+    lo.bytes = (uint64_t)strtoull(argv[4], NULL, 10);
+    lo.iterations = (uint32_t)strtoul(argv[5], NULL, 10);
+    lo.a1_counters = (uint32_t)strtoul(argv[6], NULL, 10);
+    lo.a2_counters = (uint32_t)strtoul(argv[7], NULL, 10);
+    lo.test_inject_leg = atoi(argv[8]);
+    lo.test_inject_sm = atoi(argv[9]);
+    lo.test_inject_element = atoi(argv[10]);
+    lo.test_inject_iteration = (uint32_t)strtoul(argv[11], NULL, 10);
+    lo.test_inject_word = (int64_t)strtoll(argv[12], NULL, 10);
+    lo.test_inject_mask = (uint64_t)strtoull(argv[13], NULL, 10);
+    const int cap = atoi(argv[14]);
+    static cro_l2_result lr;
+    static cro_l2_sm sms[CRO_L2_MAX_SMS];
+    cro_l2_fault *faults = (cro_l2_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
+    int n_sms = 0, got = 0;
+    if (!faults) return 2;
+    cro_probe_l2(ctx, idx, &lo, &lr, sms, CRO_L2_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
+    const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)got};
+    return write_frame(&lr, sizeof lr, counts, 2, sms, sizeof sms, faults, sizeof *faults, got, lr.status);
+}
+
+/* `scan`: the whole-HBM scan of the free memory (all of it but 1 GiB unless argv[3], in MiB, bounds it) as JSON. */
+static int scan_json(cro_ctx *ctx, int idx, char **argv) {
+    cro_scan_opts so;
+    memset(&so, 0, sizeof so);
+    if (argv[3]) so.max_bytes = (uint64_t)strtoull(argv[3], NULL, 10) << 20;
+    static cro_scan_report sr;
+    cro_fault_word *words = (cro_fault_word *)calloc(256, sizeof *words);
+    int got = 0;
+    size_t len = 0;
+    if (!words) return 2;
+    int rc = cro_scan_hbm(ctx, idx, &so, &sr, words, 256, &got);
+    if (rc != CRO_OK && rc != CRO_ERR_CHECKSUM && rc != CRO_ERR_CUDA) return fail(ctx, "cro_scan_hbm", rc);
+    if ((rc = cro_emit_scan_annotations_json(&sr, buf, sizeof buf, &len)) != CRO_OK) return fail(ctx, "emit", rc);
+    printf("%s\n", buf);
+    free(words);
+    cro_probe_destroy(ctx);
+    return sr.status == CRO_OK ? 0 : 1;
+}
+
+/* The commands that take a device (argv[2]): their argc (0: at least 3, the rest optional), cro_opts.flags and sweep
+ * region, whether argv[3] is cro_opts.seed_base, and what runs once the device is found (NULL: main's own probe). */
+static const struct command {
+    const char *name;
+    int argc;
+    uint32_t flags;
+    uint64_t sweep_mib;
+    int seeded;
+    int (*run)(cro_ctx *ctx, int idx, char **argv);
+} commands[] = {
+    /* the hot-plug path: one device, identity from /proc (NVML's first call costs more than the probe), and a 1 GiB
+     * first sweep unless argv[3] says otherwise — far beyond the L2, and it shortens everything before it */
+    {"probe", 0, CRO_F_LAZY_ALLOC | CRO_F_DEGRADE_ON_OOM | CRO_F_NO_NVML, 1024, 0, NULL},
+    {"probe-raw", 0, CRO_F_LAZY_ALLOC | CRO_F_DEGRADE_ON_OOM | CRO_F_NO_NVML, 1024, 0, NULL},
+    {"cold", 0, CRO_F_LAZY_ALLOC | CRO_F_DEGRADE_ON_OOM | CRO_F_NO_NVML, 1024, 0, NULL},
+    /* one check of one device by their own, not the HBM probe: no sweep region (the scan allocates its own chunks) and
+     * NVML, whose DRAM / SRAM / L2 health record these read */
+    {"scan", 0, CRO_F_LAZY_ALLOC, 64, 0, scan_json},
+    {"scan-raw", 12, CRO_F_LAZY_ALLOC, 64, 0, scan_raw},
+    {"sram-raw", 14, CRO_F_LAZY_ALLOC, 64, 0, sram_raw},
+    {"l2-raw", 15, CRO_F_LAZY_ALLOC, 64, 1, l2_raw},
+    /* a region of exactly L, argv[4] (the probe checks L <= S; no halving on a full GPU), and NVML for the replay
+     * counters */
+    {"link-raw", 11, CRO_F_LAZY_ALLOC, 256, 1, link_raw},
+    /* no health record to read, and NVML's first call is slow */
+    {"compute-raw", 15, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, 1, compute_raw},
+    {"precision-raw", 15, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, 1, precision_raw},
+};
+
 int main(int argc, char **argv) {
     if (argc < 2) {
         fprintf(stderr, "usage: croprobe-cli csv <query> | enumerate | probe <uuid|index> [sweep_MiB] | probe-raw <uuid> [sweep_MiB] | "
@@ -91,47 +284,22 @@ int main(int argc, char **argv) {
     }
     const double t_start = now_s();
     const char *cmd = argv[1];
-    const int raw = strcmp(cmd, "probe-raw") == 0;
+    const struct command *c = NULL;
+    for (size_t k = 0; k < sizeof commands / sizeof *commands; ++k)
+        if (strcmp(cmd, commands[k].name) == 0) c = &commands[k];
+    if (c && (argc < 3 || (c->argc && argc != c->argc))) return 64;
     const int cold = strcmp(cmd, "cold") == 0;
-    const int scan_raw = strcmp(cmd, "scan-raw") == 0;
-    const int sram_raw = strcmp(cmd, "sram-raw") == 0;
-    const int link_raw = strcmp(cmd, "link-raw") == 0;
-    const int compute_raw = strcmp(cmd, "compute-raw") == 0;
-    const int l2_raw = strcmp(cmd, "l2-raw") == 0;
-    const int precision_raw = strcmp(cmd, "precision-raw") == 0;
-    /* the commands that run one check of one device by their own, not the HBM probe */
-    const int wants_scan = scan_raw || sram_raw || link_raw || compute_raw || precision_raw || l2_raw || strcmp(cmd, "scan") == 0;
-    const int wants_probe = raw || cold || strcmp(cmd, "probe") == 0;
-    if ((wants_probe || wants_scan) && argc < 3) return 64;
-    if (scan_raw && argc != 12) return 64;
-    if (sram_raw && argc != 14) return 64;
-    if (link_raw && argc != 11) return 64;
-    if (compute_raw && argc != 15) return 64;
-    if (l2_raw && argc != 15) return 64;
-    if (precision_raw && argc != 15) return 64;
     cro_opts opts;
     memset(&opts, 0, sizeof opts);
     opts.abi_version = CRO_ABI_VERSION;
     opts.flags = CRO_F_LAZY_ALLOC | CRO_F_DEGRADE_ON_OOM;
-    if (wants_scan) {
-        /* no sweep region (the scan allocates its own chunks) and NVML, whose DRAM / SRAM health record these read */
-        opts.flags = CRO_F_LAZY_ALLOC;
-        opts.sweep_bytes = 64ull << 20;
-    }
-    if (compute_raw || precision_raw) opts.flags |= CRO_F_NO_NVML;       /* no health record to read, and NVML's first call is slow */
-    if (link_raw) {
-        /* a region of exactly L (the probe checks L <= S; no halving on a full GPU), and NVML for the replay counters */
-        opts.flags = CRO_F_LAZY_ALLOC;
-        opts.sweep_bytes = strtoull(argv[4], NULL, 10) ? (uint64_t)strtoull(argv[4], NULL, 10) : 256ull << 20;
-    }
-    if (link_raw || compute_raw || precision_raw || l2_raw) opts.seed_base = (uint64_t)strtoull(argv[3], NULL, 10);
-    if (wants_probe) {
-        /* The hot-plug path: one device, identity from /proc (NVML's first call costs more than the probe), and a
-         * 1 GiB first sweep unless told otherwise — far beyond the L2, and it shortens everything before it. */
-        opts.sweep_bytes = (argc > 3 ? (uint64_t)strtoull(argv[3], NULL, 10) : 1024ull) << 20;
-        if (!(cold && argc > 4 && strcmp(argv[4], "nvml") == 0)) opts.flags |= CRO_F_NO_NVML;
-    }
-    if (wants_probe || wants_scan) {
+    if (c) {
+        opts.flags = c->flags;
+        opts.sweep_bytes = c->sweep_mib << 20;
+        if (c->seeded) opts.seed_base = (uint64_t)strtoull(argv[3], NULL, 10);
+        if (!c->run && argc > 3) opts.sweep_bytes = (uint64_t)strtoull(argv[3], NULL, 10) << 20;    /* the probe's sweep_MiB */
+        if (cold && argc > 4 && strcmp(argv[4], "nvml") == 0) opts.flags &= ~CRO_F_NO_NVML;
+        if (c->run == link_raw && strtoull(argv[4], NULL, 10)) opts.sweep_bytes = (uint64_t)strtoull(argv[4], NULL, 10);  /* L */
         if (strncmp(argv[2], "GPU-", 4) == 0) {
             /* before ANY CUDA call: this process's cuInit must enumerate that one GPU only (one primary context
              * instead of eight on a full box) */
@@ -150,7 +318,7 @@ int main(int argc, char **argv) {
         printf("No devices were found\n");
         return 0;
     }
-    if (rc == CRO_ERR_NO_DEVICE && (wants_probe || wants_scan) && strncmp(argv[2], "GPU-", 4) == 0) {
+    if (rc == CRO_ERR_NO_DEVICE && c && strncmp(argv[2], "GPU-", 4) == 0) {
         fprintf(stderr, "croprobe-cli: device '%s' is not visible\n", argv[2]);   /* found=0, like gpus.go:896-898 */
         return 3;
     }
@@ -160,7 +328,6 @@ int main(int argc, char **argv) {
     cro_dev_info devs[CRO_MAX_DEVICES];
     int n = 0;
     if ((rc = cro_enumerate(ctx, devs, CRO_MAX_DEVICES, &n)) != CRO_OK) return fail(ctx, "cro_enumerate", rc);
-    static char buf[1 << 16];
     size_t len = 0;
 
     if (strcmp(cmd, "csv") == 0) {
@@ -176,7 +343,7 @@ int main(int argc, char **argv) {
                    devs[i].dev_index, devs[i].device_minor, devs[i].gpu_uuid, devs[i].pci_bus_id, devs[i].name,
                    (devs[i].flags & CRO_DEV_IN_PROCESS) ? "true" : "false");
         printf("]\n");
-    } else if (wants_probe || wants_scan) {
+    } else if (c) {
         int idx = -1;
         for (int i = 0; i < n; ++i)
             if ((devs[i].flags & CRO_DEV_IN_PROCESS) && (strcmp(devs[i].gpu_uuid, argv[2]) == 0 || strncmp(argv[2], "GPU-", 4) != 0))
@@ -186,171 +353,7 @@ int main(int argc, char **argv) {
             cro_probe_destroy(ctx);
             return 3;
         }
-        if (sram_raw) {
-            cro_sram_opts so;
-            memset(&so, 0, sizeof so);
-            so.legs = (uint32_t)strtoul(argv[3], NULL, 10);
-            so.iterations = (uint32_t)strtoul(argv[4], NULL, 10);
-            so.cluster = (uint32_t)strtoul(argv[5], NULL, 10);
-            so.max_rounds = (uint32_t)strtoul(argv[6], NULL, 10);
-            so.test_inject_leg = atoi(argv[7]);
-            so.test_inject_sm = atoi(argv[8]);
-            so.test_inject_element = (uint32_t)strtoul(argv[9], NULL, 10);
-            so.test_inject_iteration = (uint32_t)strtoul(argv[10], NULL, 10);
-            so.test_inject_word = atoi(argv[11]);
-            so.test_inject_mask = (uint64_t)strtoull(argv[12], NULL, 10);
-            const int cap = atoi(argv[13]);
-            static cro_sram_result sr;
-            static cro_sram_sm sms[CRO_SRAM_MAX_SMS];
-            cro_sram_fault *faults = (cro_sram_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
-            int n_sms = 0, got = 0;
-            if (!faults) return 2;
-            cro_probe_sram(ctx, idx, &so, &sr, sms, CRO_SRAM_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
-            /* the result whatever its status: the library reads why from it */
-            if (fwrite(&sr, sizeof sr, 1, stdout) != 1 || fwrite(sms, sizeof sms, 1, stdout) != 1 ||
-                (got && fwrite(faults, sizeof *faults, (size_t)got, stdout) != (size_t)got))
-                return 2;
-            fflush(stdout);
-            _exit(sr.status == CRO_OK ? 0 : 1);
-        }
-        if (l2_raw) {
-            cro_l2_opts lo;
-            memset(&lo, 0, sizeof lo);
-            lo.bytes = (uint64_t)strtoull(argv[4], NULL, 10);
-            lo.iterations = (uint32_t)strtoul(argv[5], NULL, 10);
-            lo.a1_counters = (uint32_t)strtoul(argv[6], NULL, 10);
-            lo.a2_counters = (uint32_t)strtoul(argv[7], NULL, 10);
-            lo.test_inject_leg = atoi(argv[8]);
-            lo.test_inject_sm = atoi(argv[9]);
-            lo.test_inject_element = atoi(argv[10]);
-            lo.test_inject_iteration = (uint32_t)strtoul(argv[11], NULL, 10);
-            lo.test_inject_word = (int64_t)strtoll(argv[12], NULL, 10);
-            lo.test_inject_mask = (uint64_t)strtoull(argv[13], NULL, 10);
-            const int cap = atoi(argv[14]);
-            static cro_l2_result lr;
-            static cro_l2_sm sms[CRO_L2_MAX_SMS];
-            cro_l2_fault *faults = (cro_l2_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
-            int n_sms = 0, got = 0;
-            if (!faults) return 2;
-            cro_probe_l2(ctx, idx, &lo, &lr, sms, CRO_L2_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
-            const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)got};
-            /* the result whatever its status: the library reads why from it */
-            if (fwrite(&lr, sizeof lr, 1, stdout) != 1 || fwrite(counts, sizeof counts, 1, stdout) != 1 ||
-                fwrite(sms, sizeof sms, 1, stdout) != 1 || (got && fwrite(faults, sizeof *faults, (size_t)got, stdout) != (size_t)got))
-                return 2;
-            fflush(stdout);
-            _exit(lr.status == CRO_OK ? 0 : 1);
-        }
-        if (link_raw) {
-            cro_link_opts lo;
-            memset(&lo, 0, sizeof lo);
-            lo.bytes = (uint64_t)strtoull(argv[4], NULL, 10);
-            lo.hops = (uint32_t)strtoul(argv[5], NULL, 10);
-            lo.ctas = (uint32_t)strtoul(argv[6], NULL, 10);
-            lo.test_inject_check = atoi(argv[7]);
-            lo.test_inject_word = (uint64_t)strtoull(argv[8], NULL, 10);
-            lo.test_inject_mask = (uint64_t)strtoull(argv[9], NULL, 10);
-            const int cap = atoi(argv[10]);
-            static cro_link_result lr;
-            cro_link_fault *faults = (cro_link_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
-            int got = 0;
-            if (!faults) return 2;
-            cro_probe_host_link(ctx, idx, &lo, &lr, faults, cap > 0 ? cap : 0, &got);
-            const uint64_t n_out = (uint64_t)got;
-            /* the result whatever its status: the library reads why from it */
-            if (fwrite(&lr, sizeof lr, 1, stdout) != 1 || fwrite(&n_out, sizeof n_out, 1, stdout) != 1 ||
-                (got && fwrite(faults, sizeof *faults, (size_t)got, stdout) != (size_t)got))
-                return 2;
-            fflush(stdout);
-            _exit(lr.status == CRO_OK ? 0 : 1);    /* the pinned buffers and the region go with the process */
-        }
-        if (compute_raw) {
-            cro_compute_opts co;
-            memset(&co, 0, sizeof co);
-            co.iterations = (uint32_t)strtoul(argv[4], NULL, 10);
-            co.alu_iterations = (uint32_t)strtoul(argv[5], NULL, 10);
-            co.legs = (uint32_t)strtoul(argv[6], NULL, 10);
-            co.max_rounds = (uint32_t)strtoul(argv[7], NULL, 10);
-            co.test_inject_leg = atoi(argv[8]);
-            co.test_inject_sm = atoi(argv[9]);
-            co.test_inject_iteration = (uint32_t)strtoul(argv[10], NULL, 10);
-            co.test_inject_row = atoi(argv[11]);
-            co.test_inject_col = atoi(argv[12]);
-            co.test_inject_mask = (uint32_t)strtoul(argv[13], NULL, 10);
-            const int cap = atoi(argv[14]);
-            static cro_compute_result cr;
-            static cro_compute_sm sms[CRO_COMPUTE_MAX_SMS];
-            cro_compute_fault *faults = (cro_compute_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
-            int n_sms = 0, got = 0;
-            if (!faults) return 2;
-            cro_probe_compute(ctx, idx, &co, &cr, sms, CRO_COMPUTE_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
-            const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)got};
-            /* the result whatever its status: the library reads why from it */
-            if (fwrite(&cr, sizeof cr, 1, stdout) != 1 || fwrite(counts, sizeof counts, 1, stdout) != 1 ||
-                fwrite(sms, sizeof sms, 1, stdout) != 1 || (got && fwrite(faults, sizeof *faults, (size_t)got, stdout) != (size_t)got))
-                return 2;
-            fflush(stdout);
-            _exit(cr.status == CRO_OK ? 0 : 1);
-        }
-        if (precision_raw) {
-            cro_precision_opts po;
-            memset(&po, 0, sizeof po);
-            po.iterations = (uint32_t)strtoul(argv[4], NULL, 10);
-            po.alu_iterations = (uint32_t)strtoul(argv[5], NULL, 10);
-            po.legs = (uint32_t)strtoul(argv[6], NULL, 10);
-            po.max_rounds = (uint32_t)strtoul(argv[7], NULL, 10);
-            po.test_inject_leg = atoi(argv[8]);
-            po.test_inject_sm = atoi(argv[9]);
-            po.test_inject_iteration = (uint32_t)strtoul(argv[10], NULL, 10);
-            po.test_inject_row = atoi(argv[11]);
-            po.test_inject_col = atoi(argv[12]);
-            po.test_inject_mask = (uint64_t)strtoull(argv[13], NULL, 10);
-            const int cap = atoi(argv[14]);
-            static cro_precision_result pr;
-            static cro_precision_sm sms[CRO_PRECISION_MAX_SMS];
-            cro_precision_fault *faults = (cro_precision_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
-            int n_sms = 0, got = 0;
-            if (!faults) return 2;
-            cro_probe_precision(ctx, idx, &po, &pr, sms, CRO_PRECISION_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
-            const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)got};
-            /* the result whatever its status: the library reads why from it */
-            if (fwrite(&pr, sizeof pr, 1, stdout) != 1 || fwrite(counts, sizeof counts, 1, stdout) != 1 ||
-                fwrite(sms, sizeof sms, 1, stdout) != 1 || (got && fwrite(faults, sizeof *faults, (size_t)got, stdout) != (size_t)got))
-                return 2;
-            fflush(stdout);
-            _exit(pr.status == CRO_OK ? 0 : 1);
-        }
-        if (wants_scan) {
-            cro_scan_opts so;
-            memset(&so, 0, sizeof so);
-            int cap = 256;
-            if (scan_raw) {
-                uint64_t *f[] = {&so.max_bytes, &so.reserve_bytes, &so.seed, &so.test_chunk_bytes, &so.test_force_first,
-                                 &so.test_force_count, &so.test_force_and, &so.test_force_or};
-                for (int k = 0; k < 8; ++k) *f[k] = (uint64_t)strtoull(argv[3 + k], NULL, 10);
-                cap = atoi(argv[11]);
-            } else if (argc > 3) {
-                so.max_bytes = (uint64_t)strtoull(argv[3], NULL, 10) << 20;
-            }
-            static cro_scan_report sr;
-            cro_fault_word *words = (cro_fault_word *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *words);
-            int got = 0;
-            if (!words) return 2;
-            rc = cro_scan_hbm(ctx, idx, &so, &sr, words, cap, &got);
-            if (scan_raw) {
-                /* the report whatever its status: the library reads why from it */
-                if (fwrite(&sr, sizeof sr, 1, stdout) != 1 || (got && fwrite(words, sizeof *words, (size_t)got, stdout) != (size_t)got))
-                    return 2;
-                fflush(stdout);
-                _exit(sr.status == CRO_OK ? 0 : 1);    /* the chunks go with the process */
-            }
-            if (rc != CRO_OK && rc != CRO_ERR_CHECKSUM && rc != CRO_ERR_CUDA) return fail(ctx, "cro_scan_hbm", rc);
-            if ((rc = cro_emit_scan_annotations_json(&sr, buf, sizeof buf, &len)) != CRO_OK) return fail(ctx, "emit", rc);
-            printf("%s\n", buf);
-            free(words);
-            cro_probe_destroy(ctx);
-            return sr.status == CRO_OK ? 0 : 1;
-        }
+        if (c->run) return c->run(ctx, idx, argv);
         cro_probe_result r;
         const double t1 = now_s();
         rc = cro_probe_device(ctx, idx, &r);
@@ -366,14 +369,12 @@ int main(int argc, char **argv) {
                    "\"cold_total_s\":%.4f,\"cold_probes_per_s\":%.2f,\"warm_probes_per_s\":%.2f,\"nvml\":%s,\"status\":%d}\n",
                    r.gpu_uuid, (unsigned long long)r.sweep_bytes, t_init, t_cold, t_warm, total,
                    1.0 / total, 1.0 / t_warm, (opts.flags & CRO_F_NO_NVML) ? "false" : "true", rc2 ? rc2 : r.status);
-        } else if (raw) {
-            if (fwrite(&r, sizeof r, 1, stdout) != 1) return 2;
-            fflush(stdout);
+        } else if (strcmp(cmd, "probe-raw") == 0) {
+            return write_frame(&r, sizeof r, NULL, 0, NULL, 0, NULL, 0, 0, r.status);
         } else {
             if ((rc = cro_emit_probe_annotations_json(&r, buf, sizeof buf, &len)) != CRO_OK) return fail(ctx, "emit", rc);
             printf("%s\n", buf);
         }
-        if (raw) _exit(r.status == CRO_OK ? 0 : 1);    /* the verdict is out: skip the teardown (it costs as much as the probe) */
         cro_probe_destroy(ctx);
         return r.status == CRO_OK ? 0 : 1;
     } else {

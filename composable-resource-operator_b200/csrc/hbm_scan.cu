@@ -6,7 +6,6 @@
 #include <atomic>
 #include <map>
 
-#include "inventory.hpp"
 #include "probe_internal.hpp"
 
 namespace cro {
@@ -281,49 +280,23 @@ uint64_t scan_tail_count(const unsigned char* head) {
 
 int ctx_scan_hbm_uuid(cro_ctx* c, const char* uuid, const cro_scan_opts& o, cro_scan_report* rep, std::vector<cro_fault_word>* words,
                       int cap) {
-    const uint64_t t_call = now_ns();
     blank_report(rep, words);
     if (!uuid) return rep->status = CRO_ERR_INVALID_ARG;
     const std::string want = uuid;
-    env::Values knobs;                        // no context: this caller's environment, defaults where it is illegal
-    if (c) knobs = c->knobs;
-    else env::read(&knobs, nullptr);
-    const int deadline = o.deadline_ms > 0 ? o.deadline_ms : (int)knobs.get("CRO_HELPER_TIMEOUT_MS");
-    DeviceGuard g;
-    if (c) {
-        cro_dev_info hit{};
-        int rc = find_on_node(c, want, &hit);
-        if (rc) return rep->status = rc;
-        if (hit.flags & CRO_DEV_IN_PROCESS) {     // no probe of this GPU runs beside the scan
-            g = enter_device(c, hit.dev_index);
-            if (g.rc) return rep->status = g.rc;
-        }
-    }
     auto num = [](uint64_t v) { return std::to_string(v); };
     const std::vector<std::string> args = {"scan-raw", want, num(o.max_bytes), num(o.reserve_bytes), num(o.seed), num(o.test_chunk_bytes),
                                            num(o.test_force_first), num(o.test_force_count), num(o.test_force_and),
                                            num(o.test_force_or), num((uint64_t)cap)};
-    std::string got, err;
-    if (c && c->nvtx) nvtxRangePushA("cro.scan_hbm.helper");
-    int rc = inventory::RunHelperRaw("", "scan helper", want, args, deadline, sizeof *rep, sizeof(cro_fault_word), (size_t)cap,
-                                     scan_tail_count, &got, &err);
-    if (c && c->nvtx) nvtxRangePop();
-    const uint64_t helper_ns = now_ns() - t_call;
-    if (rc == CRO_OK) {
-        memcpy(rep, got.data(), sizeof *rep);
-        const cro_fault_word* w = reinterpret_cast<const cro_fault_word*>(got.data() + sizeof *rep);
-        words->assign(w, w + rep->recorded);
-        rep->helper_ns = helper_ns;
-        rc = rep->status;
-        if (rc != CRO_OK && rc != CRO_ERR_CHECKSUM) err = "scan helper for " + want + ": " + cro_strerror(rc);
-    } else {
-        rep->status = rc;
-    }
-    if (rc != CRO_OK && !err.empty()) {
-        if (c) c->set_error(err);
-        else set_thread_error(err);
-    }
-    return rc;
+    std::string got;
+    uint64_t helper_ns = 0;
+    const int rc = run_probe_helper(c, want, "scan helper", "cro.scan_hbm.helper", args, o.deadline_ms, sizeof *rep,
+                                    sizeof(cro_fault_word), (size_t)cap, scan_tail_count, &got, &helper_ns);
+    if (rc != CRO_OK) return rep->status = rc;
+    memcpy(rep, got.data(), sizeof *rep);
+    const cro_fault_word* w = reinterpret_cast<const cro_fault_word*>(got.data() + sizeof *rep);
+    words->assign(w, w + rep->recorded);
+    rep->helper_ns = helper_ns;
+    return rep->status;
 }
 
 }  // namespace cro

@@ -342,15 +342,13 @@ int ctx_probe_host_link_uuid(cro_ctx* c, const char* uuid, const cro_link_opts& 
                                            num((uint64_t)cap)};
     const size_t head = sizeof *r + sizeof(uint64_t);
     std::string got;
-    int rc = run_probe_helper(c, want, "link helper", "cro.probe_host_link.helper", args, deadline_ms, head, sizeof(cro_link_fault),
-                              (size_t)cap, link_tail_count, &got, helper_ns);
+    const int rc = run_probe_helper(c, want, "link helper", "cro.probe_host_link.helper", args, deadline_ms, head,
+                                    sizeof(cro_link_fault), (size_t)cap, link_tail_count, &got, helper_ns);
     if (rc != CRO_OK) return r->status = rc;
     memcpy(r, got.data(), sizeof *r);
     const cro_link_fault* f = reinterpret_cast<const cro_link_fault*>(got.data() + head);
     faults->assign(f, f + link_tail_count(reinterpret_cast<const unsigned char*>(got.data())));
-    rc = r->status;
-    if (rc != CRO_OK && rc != CRO_ERR_CHECKSUM) set_call_error(c, "link helper for " + want + ": " + cro_strerror(rc));
-    return rc;
+    return r->status;
 }
 
 }  // namespace cro

@@ -405,20 +405,6 @@ int ctx_probe_l2(cro_ctx* c, int idx, const cro_l2_opts& o, cro_l2_result* r, st
     return r->status;
 }
 
-namespace {
-// l2-raw's stdout (croprobe_cli.c): the result, the helper's own counts n_sms and n, CRO_L2_MAX_SMS per-SM entries
-// (n_sms of them filled), then n faults.  An n_sms the entries cannot hold makes the output malformed.
-constexpr size_t kL2Counts = sizeof(cro_l2_result);
-constexpr size_t kL2Sms = kL2Counts + 2 * sizeof(uint64_t);
-constexpr size_t kL2Head = kL2Sms + CRO_L2_MAX_SMS * sizeof(cro_l2_sm);
-uint64_t l2_count(const unsigned char* head, int which) {
-    uint64_t v;
-    memcpy(&v, head + kL2Counts + which * sizeof v, sizeof v);
-    return v;
-}
-uint64_t l2_tail_count(const unsigned char* head) { return l2_count(head, 0) > CRO_L2_MAX_SMS ? ~0ull : l2_count(head, 1); }
-}  // namespace
-
 int ctx_probe_l2_uuid(cro_ctx* c, const char* uuid, const cro_l2_opts& o, cro_l2_result* r, std::vector<cro_l2_sm>* sms,
                       std::vector<cro_l2_fault>* faults, int cap) {
     blank_result(r, cro_l2_result{}, sms, faults);
@@ -435,21 +421,15 @@ int ctx_probe_l2_uuid(cro_ctx* c, const char* uuid, const cro_l2_opts& o, cro_l2
                                            num(o.iterations), num(o.a1_counters), num(o.a2_counters), num(o.test_inject_leg),
                                            num(o.test_inject_sm), num(o.test_inject_element), num(o.test_inject_iteration),
                                            num(o.test_inject_word), std::to_string(o.test_inject_mask), num(cap)};
+    using Frame = SmFrame<cro_l2_result, cro_l2_sm, cro_l2_fault, CRO_L2_MAX_SMS>;
     std::string got;
     uint64_t helper_ns = 0;
-    int rc = run_probe_helper(c, want, "L2 helper", "cro.probe_l2.helper", args, o.deadline_ms, kL2Head, sizeof(cro_l2_fault),
-                              (size_t)cap, l2_tail_count, &got, &helper_ns);
+    const int rc = run_probe_helper(c, want, "L2 helper", "cro.probe_l2.helper", args, o.deadline_ms, Frame::kHead,
+                                    sizeof(cro_l2_fault), (size_t)cap, Frame::tail, &got, &helper_ns);
     if (rc != CRO_OK) return r->status = rc;
-    const unsigned char* head = reinterpret_cast<const unsigned char*>(got.data());
-    memcpy(r, head, sizeof *r);
-    const cro_l2_sm* s = reinterpret_cast<const cro_l2_sm*>(head + kL2Sms);
-    sms->assign(s, s + l2_count(head, 0));
-    const cro_l2_fault* f = reinterpret_cast<const cro_l2_fault*>(head + kL2Head);
-    faults->assign(f, f + l2_count(head, 1));
+    Frame::read(got, r, sms, faults);
     r->helper_ns = helper_ns;
-    rc = r->status;
-    if (rc != CRO_OK && rc != CRO_ERR_CHECKSUM) set_call_error(c, "L2 helper for " + want + ": " + cro_strerror(rc));
-    return rc;
+    return r->status;
 }
 
 }  // namespace cro

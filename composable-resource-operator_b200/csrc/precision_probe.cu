@@ -262,22 +262,6 @@ int ctx_probe_precision(cro_ctx* c, int idx, const cro_precision_opts& o, cro_pr
     return close_call(r, CRO_PRECISION_LEGS, per_sm, sms, faults);
 }
 
-namespace {
-// precision-raw's stdout: the result, the helper's own counts n_sms and n, CRO_PRECISION_MAX_SMS per-SM entries (n_sms
-// of them filled), then n faults.  An n_sms the entries cannot hold makes the output malformed.
-constexpr size_t kPrecisionCounts = sizeof(cro_precision_result);
-constexpr size_t kPrecisionSms = kPrecisionCounts + 2 * sizeof(uint64_t);
-constexpr size_t kPrecisionHead = kPrecisionSms + CRO_PRECISION_MAX_SMS * sizeof(cro_precision_sm);
-uint64_t precision_count(const unsigned char* head, int which) {
-    uint64_t v;
-    memcpy(&v, head + kPrecisionCounts + which * sizeof v, sizeof v);
-    return v;
-}
-uint64_t precision_tail_count(const unsigned char* head) {
-    return precision_count(head, 0) > CRO_PRECISION_MAX_SMS ? ~0ull : precision_count(head, 1);
-}
-}  // namespace
-
 int ctx_probe_precision_uuid(cro_ctx* c, const char* uuid, const cro_precision_opts& o, int deadline_ms, cro_precision_result* r,
                              std::vector<cro_precision_sm>* sms, std::vector<cro_precision_fault>* faults, int cap,
                              uint64_t* helper_ns) {
@@ -295,19 +279,13 @@ int ctx_probe_precision_uuid(cro_ctx* c, const char* uuid, const cro_precision_o
                                            num(o.alu_iterations), num(o.legs), num(o.max_rounds), num(o.test_inject_leg),
                                            num(o.test_inject_sm), num(o.test_inject_iteration), num(o.test_inject_row),
                                            num(o.test_inject_col), std::to_string(o.test_inject_mask), num(cap)};
+    using Frame = SmFrame<cro_precision_result, cro_precision_sm, cro_precision_fault, CRO_PRECISION_MAX_SMS>;
     std::string got;
-    int rc = run_probe_helper(c, want, "precision helper", "cro.probe_precision.helper", args, deadline_ms, kPrecisionHead,
-                              sizeof(cro_precision_fault), (size_t)cap, precision_tail_count, &got, helper_ns);
+    const int rc = run_probe_helper(c, want, "precision helper", "cro.probe_precision.helper", args, deadline_ms, Frame::kHead,
+                                    sizeof(cro_precision_fault), (size_t)cap, Frame::tail, &got, helper_ns);
     if (rc != CRO_OK) return r->status = rc;
-    const unsigned char* head = reinterpret_cast<const unsigned char*>(got.data());
-    memcpy(r, head, sizeof *r);
-    const cro_precision_sm* s = reinterpret_cast<const cro_precision_sm*>(head + kPrecisionSms);
-    sms->assign(s, s + precision_count(head, 0));
-    const cro_precision_fault* f = reinterpret_cast<const cro_precision_fault*>(head + kPrecisionHead);
-    faults->assign(f, f + precision_count(head, 1));
-    rc = r->status;
-    if (rc != CRO_OK && rc != CRO_ERR_CHECKSUM) set_call_error(c, "precision helper for " + want + ": " + cro_strerror(rc));
-    return rc;
+    Frame::read(got, r, sms, faults);
+    return r->status;
 }
 
 }  // namespace cro

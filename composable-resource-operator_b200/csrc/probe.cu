@@ -9,9 +9,11 @@
 #include <dlfcn.h>
 #include <unistd.h>
 
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <random>
+#include <type_traits>
 
 #include "env.hpp"
 #include "inventory.hpp"
@@ -881,6 +883,13 @@ uint64_t helper_seed_base(cro_ctx* c) {
     return s ? s : 0x100;         // 0 would ask the helper for the default base
 }
 
+// run_probe_helper reads a helper result's status from the first four bytes of its frame.
+template <class R>
+constexpr bool status_first() { return offsetof(R, status) == 0 && std::is_same<decltype(R::status), int32_t>::value; }
+static_assert(status_first<cro_link_result>() && status_first<cro_compute_result>() && status_first<cro_precision_result>() &&
+                  status_first<cro_scan_report>() && status_first<cro_sram_result>() && status_first<cro_l2_result>(),
+              "every helper result begins with its int32_t status");
+
 int run_probe_helper(cro_ctx* c, const std::string& uuid, const std::string& what, const char* range,
                      const std::vector<std::string>& args, int deadline_ms, size_t head, size_t rec, size_t cap,
                      uint64_t (*count)(const unsigned char* head), std::string* got, uint64_t* helper_ns) {
@@ -904,8 +913,14 @@ int run_probe_helper(cro_ctx* c, const std::string& uuid, const std::string& wha
     const int rc = inventory::RunHelperRaw("", what, uuid, args, deadline, head, rec, cap, count, got, &err);
     *helper_ns = now_ns() - t_spawn;
     if (c && c->nvtx) nvtxRangePop();
-    if (rc != CRO_OK && !err.empty()) set_call_error(c, err);
-    return rc;
+    if (rc != CRO_OK) {
+        if (!err.empty()) set_call_error(c, err);
+        return rc;
+    }
+    int32_t status;
+    memcpy(&status, got->data(), sizeof status);
+    if (status != CRO_OK && status != CRO_ERR_CHECKSUM) set_call_error(c, what + " for " + uuid + ": " + cro_strerror(status));
+    return CRO_OK;
 }
 
 }  // namespace cro

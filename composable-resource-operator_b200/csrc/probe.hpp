@@ -11,6 +11,7 @@
 
 #include <atomic>
 #include <chrono>
+#include <cstring>
 #include <deque>
 #include <memory>
 #include <mutex>
@@ -138,7 +139,7 @@ struct cro_ctx {
     std::atomic<uint64_t> launches{0};
     // gauges / counters behind cro_metrics_text (the operator's Prometheus registry, cmd/main.go:66,119-125)
     std::atomic<uint64_t> m_probes{0}, m_probe_failures{0}, m_fullbox{0}, m_helper_probes{0}, m_helper_failures{0};
-    // helper calls of the host link and compute probes' uuid forms so far: the seed base of each (helper_seed_base)
+    // helper calls that took a seed base so far: the seed base of each (helper_seed_base)
     std::atomic<uint64_t> helper_seeds{0};
     std::mutex err_mu;
     std::string last_error;
@@ -246,17 +247,44 @@ namespace precision {
 int Expected(int answer, uint64_t seed, int64_t* out);
 }  // namespace precision
 
-// The helper run behind the host link and compute probes' uuid forms.  Bad options are refused by the caller first.
-// With a context, the node must list the GPU (CRO_ERR_NO_DEVICE otherwise) and a GPU that is also an in-process device
-// is held under its device guard while the helper runs.  Then `croprobe-cli args...` runs as inventory::RunHelperRaw
-// runs it ("<what> for <uuid> ..." in its errors) and its stdout lands in *got.  *helper_ns: spawn to exit.  An error
-// goes to the context, or to the calling thread without one.
+// The helper run behind the uuid forms of the host link, compute, precision, scan, SRAM and L2 probes.  Bad options
+// are refused by the caller first.  With a context, the node must list the GPU (CRO_ERR_NO_DEVICE otherwise) and a GPU
+// that is also an in-process device is held under its device guard while the helper runs.  Then `croprobe-cli args...`
+// runs as inventory::RunHelperRaw runs it ("<what> for <uuid> ..." in its errors) and its stdout lands in *got.
+// *helper_ns: spawn to exit.  CRO_OK means *got is a whole frame; the result's status, its first field, is the call's
+// status then, and one other than CRO_OK or CRO_ERR_CHECKSUM is an error too.  An error goes to the context, or to the
+// calling thread without one.
 int run_probe_helper(cro_ctx* c, const std::string& uuid, const std::string& what, const char* range,
                      const std::vector<std::string>& args, int deadline_ms, size_t head, size_t rec, size_t cap,
                      uint64_t (*count)(const unsigned char* head), std::string* got, uint64_t* helper_ns);
-// The cro_opts.seed_base a helper of those forms gets: with a context, its seed_base + (h << 8) for the context's h-th
-// such call (h from 1, so no helper repeats the context's own seeds); without one, a clock-derived base.  The low byte
-// is clear either way: the helper ORs the minor into it.
+// The stdout of compute-raw, precision-raw and l2-raw: the Result, the helper's own counts n_sms and n (uint64_t),
+// MAX_SMS Sm entries (n_sms of them filled), then n Fault records.  An n_sms the entries cannot hold makes the output
+// malformed.
+template <class Result, class Sm, class Fault, size_t MAX_SMS>
+struct SmFrame {
+    static constexpr size_t kCounts = sizeof(Result);
+    static constexpr size_t kSms = kCounts + 2 * sizeof(uint64_t);
+    static constexpr size_t kHead = kSms + MAX_SMS * sizeof(Sm);
+    static uint64_t count(const unsigned char* head, int which) {
+        uint64_t v;
+        memcpy(&v, head + kCounts + which * sizeof v, sizeof v);
+        return v;
+    }
+    // The record count run_probe_helper's count argument gives RunHelperRaw.
+    static uint64_t tail(const unsigned char* head) { return count(head, 0) > MAX_SMS ? ~0ull : count(head, 1); }
+    // Unpacks a frame run_probe_helper accepted.
+    static void read(const std::string& got, Result* r, std::vector<Sm>* sms, std::vector<Fault>* faults) {
+        const unsigned char* head = reinterpret_cast<const unsigned char*>(got.data());
+        memcpy(r, head, sizeof *r);
+        const Sm* s = reinterpret_cast<const Sm*>(head + kSms);
+        sms->assign(s, s + count(head, 0));
+        const Fault* f = reinterpret_cast<const Fault*>(head + kHead);
+        faults->assign(f, f + count(head, 1));
+    }
+};
+// The cro_opts.seed_base a helper of the link, compute, precision and L2 forms gets: with a context, its seed_base +
+// (h << 8) for the context's h-th such call (h from 1, so no helper repeats the context's own seeds); without one, a
+// clock-derived base.  The low byte is clear either way: the helper ORs the minor into it.
 uint64_t helper_seed_base(cro_ctx* c);
 // Sets an error text on the context, or on the calling thread without one.
 void set_call_error(cro_ctx* c, const std::string& m);

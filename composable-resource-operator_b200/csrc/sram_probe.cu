@@ -4,7 +4,6 @@
 #include <set>
 #include <tuple>
 
-#include "inventory.hpp"
 #include "probe_internal.hpp"
 
 namespace cro {
@@ -325,53 +324,27 @@ uint64_t sram_tail_count(const unsigned char* head) {
 
 int ctx_probe_sram_uuid(cro_ctx* c, const char* uuid, const cro_sram_opts& o, cro_sram_result* r, std::vector<cro_sram_sm>* sms,
                         std::vector<cro_sram_fault>* faults, int cap) {
-    const uint64_t t_call = now_ns();
     blank_result(r, cro_sram_result{}, sms, faults);
     if (!uuid) return r->status = CRO_ERR_INVALID_ARG;
     const std::string want = uuid;
-    env::Values knobs;                        // no context: this caller's environment, defaults where it is illegal
-    if (c) knobs = c->knobs;
-    else env::read(&knobs, nullptr);
-    const int deadline = o.deadline_ms > 0 ? o.deadline_ms : (int)knobs.get("CRO_HELPER_TIMEOUT_MS");
-    DeviceGuard g;
-    if (c) {
-        cro_dev_info hit{};
-        int rc = find_on_node(c, want, &hit);
-        if (rc) return r->status = rc;
-        if (hit.flags & CRO_DEV_IN_PROCESS) {     // no probe of this GPU runs beside the helper
-            g = enter_device(c, hit.dev_index);
-            if (g.rc) return r->status = g.rc;
-        }
-    }
     auto num = [](int64_t v) { return std::to_string(v); };
     const std::vector<std::string> args = {"sram-raw", want, num(o.legs), num(o.iterations), num(o.cluster), num(o.max_rounds),
                                            num(o.test_inject_leg), num(o.test_inject_sm), num(o.test_inject_element),
                                            num(o.test_inject_iteration), num(o.test_inject_word), std::to_string(o.test_inject_mask),
                                            num(cap)};
     const size_t head = sizeof *r + CRO_SRAM_MAX_SMS * sizeof(cro_sram_sm);
-    std::string got, err;
-    if (c && c->nvtx) nvtxRangePushA("cro.probe_sram.helper");
-    int rc = inventory::RunHelperRaw("", "SRAM helper", want, args, deadline, head, sizeof(cro_sram_fault), (size_t)cap,
-                                     sram_tail_count, &got, &err);
-    if (c && c->nvtx) nvtxRangePop();
-    const uint64_t helper_ns = now_ns() - t_call;
-    if (rc == CRO_OK) {
-        memcpy(r, got.data(), sizeof *r);
-        const cro_sram_sm* s = reinterpret_cast<const cro_sram_sm*>(got.data() + sizeof *r);
-        sms->assign(s, s + std::min<uint32_t>(r->sms_listed, CRO_SRAM_MAX_SMS));
-        const cro_sram_fault* f = reinterpret_cast<const cro_sram_fault*>(got.data() + head);
-        faults->assign(f, f + r->recorded);
-        r->helper_ns = helper_ns;
-        rc = r->status;
-        if (rc != CRO_OK && rc != CRO_ERR_CHECKSUM) err = "SRAM helper for " + want + ": " + cro_strerror(rc);
-    } else {
-        r->status = rc;
-    }
-    if (rc != CRO_OK && !err.empty()) {
-        if (c) c->set_error(err);
-        else set_thread_error(err);
-    }
-    return rc;
+    std::string got;
+    uint64_t helper_ns = 0;
+    const int rc = run_probe_helper(c, want, "SRAM helper", "cro.probe_sram.helper", args, o.deadline_ms, head,
+                                    sizeof(cro_sram_fault), (size_t)cap, sram_tail_count, &got, &helper_ns);
+    if (rc != CRO_OK) return r->status = rc;
+    memcpy(r, got.data(), sizeof *r);
+    const cro_sram_sm* s = reinterpret_cast<const cro_sram_sm*>(got.data() + sizeof *r);
+    sms->assign(s, s + std::min<uint32_t>(r->sms_listed, CRO_SRAM_MAX_SMS));
+    const cro_sram_fault* f = reinterpret_cast<const cro_sram_fault*>(got.data() + head);
+    faults->assign(f, f + r->recorded);
+    r->helper_ns = helper_ns;
+    return r->status;
 }
 
 }  // namespace cro
