@@ -8,13 +8,6 @@
 namespace cro {
 
 namespace {
-// Pattern j of call k: seed_dev + 2^62 + (3k + j) * kNonceStride.  A probe's seed seed_dev + nonce * kNonceStride equals
-// it only when (nonce - 3k - j) * kNonceStride = 2^62 (mod 2^64); the stride is odd, hence invertible, and 2^62 times
-// an odd number is 2^62 or 3 * 2^62 (mod 2^64), so nonce = 3k + j + 2^62 or + 3 * 2^62: no nonce below 2^62 while
-// 3k + 2 < 2^62.  The locator's retest seed seed_dev + 2^63 would need (3k + j) * kNonceStride = 2^62 (mod 2^64),
-// i.e. 3k + j >= 2^62 by the same argument.  Distinct (k, j) give distinct seeds, so no call passes on the bytes an
-// earlier call left behind.
-constexpr uint64_t kLinkSeedOffset = 1ull << 62;
 constexpr uint64_t kLinkDefaultBytes = 256ull << 20;
 constexpr uint32_t kLinkDefaultHops = 1024;
 constexpr uint32_t kLinkMaxCtas = 4096;
@@ -145,7 +138,7 @@ int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_re
 
         const uint64_t k = d->link_calls++;
         uint64_t P[3];
-        for (int j = 0; j < 3; ++j) P[j] = d->seed_dev + kLinkSeedOffset + (3 * k + (uint64_t)j) * kNonceStride;
+        for (int j = 0; j < 3; ++j) P[j] = space_seed(d, kSeedLink, k, (uint64_t)j);
         r->bytes = L;
         r->call = k;
         for (int j = 0; j < 3; ++j) r->seed[j] = P[j];

@@ -24,6 +24,7 @@
 // The probe path has no tensor cores: there is no contraction on it.  The compute
 // probe uses them on purpose: checking them is its job.
 #include "kernels.cuh"
+#include "sm_tile.cuh"
 #include "warp_claim.cuh"
 
 #include <cuda_bf16.h>
@@ -39,12 +40,6 @@ namespace cro {
 // ---------------------------------------------------------------------------
 // small PTX helpers
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-
 __device__ __forceinline__ uint4 ldg_stream(const uint4* p) {
     uint4 r;
     asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
@@ -117,10 +112,6 @@ __device__ __forceinline__ unsigned long long lo64(const uint4& v) {
 }
 __device__ __forceinline__ unsigned long long hi64(const uint4& v) {
     return (unsigned long long)v.z | ((unsigned long long)v.w << 32);
-}
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-    return (uint32_t)__cvta_generic_to_shared(p);
 }
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -1216,10 +1207,8 @@ p2p_finalize_kernel(const P2PFinalizeArgs a) {
 //   FFMA, IMAD       the same accumulator fragment computed by scalar FMA / IMAD
 //                    chains on the CUDA cores
 // Operands sit in the canonical K-major no-swizzle layout the wgmma shared-memory
-// descriptors read: core matrices of 8 rows x 16 bytes (128 contiguous bytes, row
-// r at +16 r); the core matrices along K of one 8-row group side by side (leading
-// byte offset 128); 8-row groups 8 * K * elem bytes apart (stride byte offset).
-// B is held transposed (N rows of K), as the K-major form requires.
+// descriptors read (kmajor_off, sm_tile.cuh).  B is held transposed (N rows of K),
+// as the K-major form requires.
 // After each iteration every thread adds sum_j value_j * (2j + 1) to a running
 // fold (float values after cvt.rni.s32.f32); at the end it compares the fold with
 // iterations * the fold of the expected values, and the last answer element by
@@ -1238,115 +1227,9 @@ template <unsigned LEG> struct ComputeLeg {
     using Acc = typename std::conditional<kFloat, float, int>::type;
 };
 
-// Byte offset of element (row, k) of a K-major operand with kCK elements per row.
-template <unsigned ELEM>
-__device__ __forceinline__ unsigned kmajor_off(unsigned row, unsigned k) {
-    const unsigned kb = k * ELEM;
-    return (row >> 3) * (8u * kCK * ELEM) + (kb >> 4) * 128u + (row & 7u) * 16u + (kb & 15u);
-}
-
-// wgmma shared-memory descriptor, no swizzle: start address, leading byte offset 128, stride byte offset sbo.
-__device__ __forceinline__ unsigned long long wgmma_desc(unsigned addr, unsigned sbo) {
-    return (unsigned long long)((addr & 0x3FFFFu) >> 4) | ((unsigned long long)(128u >> 4) << 16) |
-           ((unsigned long long)(sbo >> 4) << 32);
-}
-
-__device__ __forceinline__ void wgmma_s8(int (&d)[128], unsigned long long da, unsigned long long db, int scale_d) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
-        "wgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 "
-        "{"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
-        "}, %128, %129, p;\n}\n"
-        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
-          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
-          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
-          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
-          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
-          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
-          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
-          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]),
-          "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]),
-          "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]),
-          "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]),
-          "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]),
-          "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]),
-          "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]),
-          "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]),
-          "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
-        : "l"(da), "l"(db), "r"(scale_d));
-}
-__device__ __forceinline__ void wgmma_bf16(float (&d)[128], unsigned long long da, unsigned long long db, int scale_d) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
-        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
-        "{"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
-        "}, %128, %129, p, 1, 1, 0, 0;\n}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-        : "l"(da), "l"(db), "r"(scale_d));
-}
-__device__ __forceinline__ void wgmma_e4m3(float (&d)[128], unsigned long long da, unsigned long long db, int scale_d) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
-        "wgmma.mma_async.sync.aligned.m64n256k32.f32.e4m3.e4m3 "
-        "{"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
-        "}, %128, %129, p, 1, 1;\n}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-        : "l"(da), "l"(db), "r"(scale_d));
-}
+SM_TILE_WGMMA(wgmma_s8, int, 128, "+r", "m64n256k32.s32.s8.s8", "")
+SM_TILE_WGMMA(wgmma_bf16, float, 128, "+f", "m64n256k16.f32.bf16.bf16", ", 1, 1, 0, 0")
+SM_TILE_WGMMA(wgmma_e4m3, float, 128, "+f", "m64n256k32.f32.e4m3.e4m3", ", 1, 1")
 
 // The operand byte read as each leg's element type: s8 as int8; small-int (byte & 7) - 4 as bf16 or e4m3.
 template <unsigned LEG>
@@ -1432,8 +1315,8 @@ __global__ void __launch_bounds__(kComputeThreads, 1) compute_probe_kernel(const
         for (unsigned b = 0; b < 8; ++b) {
             const unsigned e = 8 * w + b;
             const unsigned byte = (unsigned)(v >> (8 * b)) & 0xFFu;
-            if (e < kCM * kCK) store_operand<LEG>(sA + kmajor_off<ELEM>(e / kCK, e % kCK), byte);
-            else store_operand<LEG>(sB + kmajor_off<ELEM>((e - kCM * kCK) % kCN, (e - kCM * kCK) / kCN), byte);
+            if (e < kCM * kCK) store_operand<LEG>(sA + kmajor_off<ELEM, kCK>(e / kCK, e % kCK), byte);
+            else store_operand<LEG>(sB + kmajor_off<ELEM, kCK>((e - kCM * kCK) % kCN, (e - kCM * kCK) / kCN), byte);
         }
     }
     if constexpr (L::kTensor) asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
@@ -1444,9 +1327,7 @@ __global__ void __launch_bounds__(kComputeThreads, 1) compute_probe_kernel(const
     asm volatile("mov.u32 %0, %%nsmid;" : "=r"(nsmid));
     const unsigned wg = tid >> 7, lane = tid & 31u;
     const unsigned r0 = 64u * wg + 16u * ((tid >> 5) & 3u) + (lane >> 2), c0 = 2u * (lane & 3u);
-    // the injection, resolved once: this thread's iteration to inject after (all ones: none) and rows it owns
-    const unsigned rowsel = (a.inj_row < 0) ? 3u : ((unsigned)a.inj_row == r0 ? 1u : (unsigned)a.inj_row == r0 + 8 ? 2u : 0u);
-    const unsigned inj_it = (a.inj_mask && rowsel && (a.inj_sm < 0 || (unsigned)a.inj_sm == smid)) ? a.inj_iter : ~0u;
+    const Injection inj = resolve_injection(a, r0, smid);
 
     Acc acc[128];
 #pragma unroll
@@ -1479,13 +1360,13 @@ __global__ void __launch_bounds__(kComputeThreads, 1) compute_probe_kernel(const
             constexpr int KC = 16 / ELEM;                          // elements per 16-byte core-matrix row
 #pragma unroll 1
             for (unsigned kc = 0; kc < kCK; kc += KC) {
-                const uint4 x0 = *reinterpret_cast<const uint4*>(sA + kmajor_off<ELEM>(r0, kc));
-                const uint4 x1 = *reinterpret_cast<const uint4*>(sA + kmajor_off<ELEM>(r0 + 8, kc));
+                const uint4 x0 = *reinterpret_cast<const uint4*>(sA + kmajor_off<ELEM, kCK>(r0, kc));
+                const uint4 x1 = *reinterpret_cast<const uint4*>(sA + kmajor_off<ELEM, kCK>(r0 + 8, kc));
                 const unsigned a0[4] = {x0.x, x0.y, x0.z, x0.w}, a1[4] = {x1.x, x1.y, x1.z, x1.w};
 #pragma unroll
                 for (int g = 0; g < 32; ++g) {
-                    const uint4 y0 = *reinterpret_cast<const uint4*>(sB + kmajor_off<ELEM>(8u * g + c0, kc));
-                    const uint4 y1 = *reinterpret_cast<const uint4*>(sB + kmajor_off<ELEM>(8u * g + c0 + 1, kc));
+                    const uint4 y0 = *reinterpret_cast<const uint4*>(sB + kmajor_off<ELEM, kCK>(8u * g + c0, kc));
+                    const uint4 y1 = *reinterpret_cast<const uint4*>(sB + kmajor_off<ELEM, kCK>(8u * g + c0 + 1, kc));
                     const unsigned b0[4] = {y0.x, y0.y, y0.z, y0.w}, b1[4] = {y1.x, y1.y, y1.z, y1.w};
 #pragma unroll
                     for (int k = 0; k < KC; ++k) {
@@ -1506,11 +1387,11 @@ __global__ void __launch_bounds__(kComputeThreads, 1) compute_probe_kernel(const
                 }
             }
         }
-        if (it == inj_it) {                                        // test only: one compare on the clean path
+        if (it == inj.iter) {                                        // test only: one compare on the clean path
 #pragma unroll
             for (int j = 0; j < 128; ++j) {
                 const unsigned col = 8u * (j >> 2) + c0 + (j & 1);
-                if (((rowsel >> ((j >> 1) & 1)) & 1u) && (a.inj_col < 0 || (unsigned)a.inj_col == col)) {
+                if (((inj.rows >> ((j >> 1) & 1)) & 1u) && (a.inj_col < 0 || (unsigned)a.inj_col == col)) {
                     if constexpr (L::kFloat) acc[j] = __uint_as_float(__float_as_uint(acc[j]) ^ a.inj_mask);
                     else acc[j] ^= (int)a.inj_mask;
                 }
@@ -1532,26 +1413,7 @@ __global__ void __launch_bounds__(kComputeThreads, 1) compute_probe_kernel(const
     mism += compute_compare<LEG, 2>(acc, r0, c0, smid, a, &efold);
     mism += compute_compare<LEG, 3>(acc, r0, c0, smid, a, &efold);
     const unsigned fold_bad = run != (unsigned long long)a.iterations * efold ? 1u : 0u;
-    const unsigned wm = __reduce_add_sync(0xffffffffu, mism), wf = __reduce_add_sync(0xffffffffu, fold_bad);
-    if (lane == 0 && (wm | wf)) {
-        atomicAdd(&s_mism, (unsigned long long)wm);
-        atomicAdd(&s_fold_mism, (unsigned long long)wf);
-    }
-    atomicAdd(&s_fold, run);
-    __syncthreads();
-    if (tid == 0) {
-        if (smid < CRO_COMPUTE_MAX_SMS) atomicOr(a.sm_bits + (smid >> 6), 1ull << (smid & 63u));
-        ComputeCta& o = a.cta[blockIdx.x];
-        o.t0 = t0;
-        o.t1 = t1;
-        o.cycles = (unsigned long long)(k1 - k0);
-        o.mismatches = s_mism;
-        o.fold_mismatches = s_fold_mism;
-        o.fold = s_fold;
-        o.smid = smid;
-        o.nsmid = nsmid;
-        o.stamp = a.stamp;
-    }
+    publish_cta<CRO_COMPUTE_MAX_SMS>(a, mism, fold_bad, run, t0, t1, k0, k1, smid, nsmid, s_mism, s_fold_mism, s_fold);
 }
 
 // ---------------------------------------------------------------------------

@@ -10,18 +10,6 @@
 namespace cro {
 
 namespace {
-// Seeds of call k: seed_dev + 2^59 + (2k + m) * kNonceStride, m = 0 for the march and 1 for the atomics.  No other seed
-// of the device reaches them while every count stays below 2^58.  The stride is odd, hence invertible mod 2^64, and
-// each offset below is an odd multiple of 2^59, which times the stride's inverse is again an odd multiple of 2^59 (mod
-// 2^64), at least 2^59 in size as a signed difference:
-//   probe nonce n:       seed_dev + n * stride needs (2k + m - n) * stride = -2^59: n or 2k + m is at least 2^58;
-//   locator retest:      seed_dev + 2^63 needs (2k + m) * stride = 2^63 - 2^59 = 15 * 2^59, so 2k + m >= 2^58;
-//   link pattern 3k'+j:  seed_dev + 2^62 + (3k' + j) * stride needs (2k + m - 3k' - j) * stride = 7 * 2^59;
-//   compute call k':     seed_dev + 2^61 + k' * stride needs (2k + m - k') * stride = 3 * 2^59;
-//   SRAM call k', rank r: seed_dev + 2^60 + (8k' + r) * stride needs (2k + m - 8k' - r) * stride = 2^59;
-// each of which asks for a count of at least 2^58.  Distinct (k, m) give distinct seeds: no call passes on what an
-// earlier call left in its buffer, which the next cudaMalloc may hand back unchanged.
-constexpr uint64_t kL2SeedOffset = 1ull << 59;
 // W and iterations when the caller gives none.  On an H100 80GB HBM3 at a 700 W limit (profiles/h100_700w_l2_rate.jsonl)
 // the read-and-write elements M1 .. M4 move 4.1-4.3 TB/s at W = 24 and 32 MiB, and M1, M2 and M4 fall to 2.7-2.8 TB/s
 // at 48 and 64 MiB, under the 3.1 TB/s the locator reads HBM at: 32 MiB is the largest measured size that stays in the
@@ -196,8 +184,8 @@ int ctx_probe_l2(cro_ctx* c, int idx, const cro_l2_opts& o, cro_l2_result* r, st
         CU_TRY(c, l2_plan(d->ordinal, &dyn));
         const uint64_t k = d->l2_calls++;
         const uint64_t launches = (uint64_t)p.iterations * CRO_L2_ELEMENTS;
-        r->seed = d->seed_dev + kL2SeedOffset + 2 * k * kNonceStride;
-        r->seed_atomic = r->seed + kNonceStride;
+        r->seed = space_seed(d, kSeedL2, k, 0);
+        r->seed_atomic = space_seed(d, kSeedL2, k, 1);
         r->call = k;
         r->bytes = p.bytes;
         r->sm_count = G;

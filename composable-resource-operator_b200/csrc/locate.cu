@@ -6,9 +6,6 @@
 namespace cro {
 
 namespace {
-// The retest pattern's seed: seed_dev + 2^63.  A probe's seed is seed_dev + nonce * kNonceStride with kNonceStride odd,
-// which equals it only for nonce 2^63: no probe of the context shares the retest's pattern.
-constexpr uint64_t kRetestSeedOffset = 1ull << 63;
 constexpr int kLocateSlots = 2 * CRO_LOCATE_PASSES + CRO_LOCATE_PASSES;   // [2p + h] compare sweeps, then closed forms
 
 // The report of a call that located nothing: zeroes but for the sweep size it got to (0 before it knew it).
@@ -50,7 +47,7 @@ int ctx_locate(cro_ctx* c, int idx, const cro_locate_opts& o, cro_fault_report* 
 
         const bool retest = (o.flags & CRO_LOCATE_RETEST) != 0;
         const uint32_t np = retest ? CRO_LOCATE_PASSES : 1;
-        const uint64_t rseed = d->seed_dev + kRetestSeedOffset;
+        const uint64_t rseed = space_seed(d, kSeedRetest, 0);
         rep->sweep_bytes = S;
         rep->n_passes = np;
         rep->retest_seed = retest ? rseed : 0;

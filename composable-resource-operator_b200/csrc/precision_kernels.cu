@@ -7,8 +7,7 @@
 //   TF32, F16,   wgmma.mma_async m64n256 (HGMMA / QGMMA), each of the two warpgroups owning 64 rows, chained over K
 //   F16ACC, E5M2 with scale-d = 0 on the first instruction of every iteration (F16ACC: 64 f16x2 accumulators)
 //   HFMA2        the F16ACC fragment computed by HFMA2 chains, f16 accumulators, (col, col + 1) packed
-// The wgmma legs keep their operands in the canonical K-major no-swizzle layout (as the compute probe's kernels in
-// kernels.cu: core matrices of 8 rows x 16 bytes, leading byte offset 128, stride byte offset 8 * K * elem); B is held
+// The wgmma legs keep their operands in the canonical K-major no-swizzle layout (kmajor_off, sm_tile.cuh); B is held
 // transposed (N rows of K).  The F64 legs keep A and B^T row-major with rows of K + 4 doubles, so that the eight rows
 // a fragment load touches fall on distinct banks.
 // After each iteration every thread adds sum_j canon(value_j) * (2e_j + 1) to a running fold (e_j = row * N + col); at
@@ -21,19 +20,12 @@
 #include <type_traits>
 
 #include "precision_kernels.cuh"
+#include "sm_tile.cuh"
 #include "warp_claim.cuh"
 
 namespace cro {
 
 namespace {
-
-__device__ __forceinline__ unsigned long long timer_ns() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-
-__device__ __forceinline__ unsigned smem_addr(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 
 template <unsigned LEG> struct PLeg {
     static constexpr bool kF64 = LEG == CRO_PRECISION_LEG_F64 || LEG == CRO_PRECISION_LEG_DFMA;   // the F64 fragment
@@ -55,53 +47,10 @@ static_assert(PLeg<CRO_PRECISION_LEG_F64>::kSmem <= 227 * 1024 && PLeg<CRO_PRECI
                   PLeg<CRO_PRECISION_LEG_F16>::kSmem <= 227 * 1024,
               "one CTA's operands fit an H100 SM's shared memory");
 
-// Byte offset of element (row, k) of a K-major operand with K elements of ELEM bytes per row.
-template <unsigned ELEM, unsigned K>
-__device__ __forceinline__ unsigned kmajor(unsigned row, unsigned k) {
-    const unsigned kb = k * ELEM;
-    return (row >> 3) * (8u * K * ELEM) + (kb >> 4) * 128u + (row & 7u) * 16u + (kb & 15u);
-}
-
-// wgmma shared-memory descriptor, no swizzle: start address, leading byte offset 128, stride byte offset sbo.
-__device__ __forceinline__ unsigned long long desc(unsigned addr, unsigned sbo) {
-    return (unsigned long long)((addr & 0x3FFFFu) >> 4) | ((unsigned long long)(128u >> 4) << 16) |
-           ((unsigned long long)(sbo >> 4) << 32);
-}
-
-#define PREC_R128                                                                                                        \
-    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "      \
-    "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "  \
-    "%47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, "  \
-    "%70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, "  \
-    "%93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, "    \
-    "%113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}"
-#define PREC_R64                                                                                                         \
-    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "      \
-    "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "  \
-    "%47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
-#define PREC_8(c, b)                                                                                                     \
-    c(d[b]), c(d[b + 1]), c(d[b + 2]), c(d[b + 3]), c(d[b + 4]), c(d[b + 5]), c(d[b + 6]), c(d[b + 7])
-#define PREC_64(c, b) PREC_8(c, b), PREC_8(c, b + 8), PREC_8(c, b + 16), PREC_8(c, b + 24), PREC_8(c, b + 32),            \
-                      PREC_8(c, b + 40), PREC_8(c, b + 48), PREC_8(c, b + 56)
-
-// One wgmma of 32 bytes of K.  `tail` is the instruction's scale / transpose immediates.
-#define PREC_WGMMA_F32(name, shape, tail)                                                                                \
-    __device__ __forceinline__ void name(float (&d)[128], unsigned long long da, unsigned long long db, int scale_d) {   \
-        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\nwgmma.mma_async.sync.aligned." shape " " PREC_R128      \
-                     ", %128, %129, p, " tail ";\n}\n"                                                                 \
-                     : PREC_64("+f", 0), PREC_64("+f", 64)                                                              \
-                     : "l"(da), "l"(db), "r"(scale_d));                                                                 \
-    }
-PREC_WGMMA_F32(wgmma_tf32, "m64n256k8.f32.tf32.tf32", "1, 1")
-PREC_WGMMA_F32(wgmma_f16, "m64n256k16.f32.f16.f16", "1, 1, 0, 0")
-PREC_WGMMA_F32(wgmma_e5m2, "m64n256k32.f32.e5m2.e5m2", "1, 1")
-
-__device__ __forceinline__ void wgmma_f16acc(unsigned (&d)[64], unsigned long long da, unsigned long long db, int scale_d) {
-    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\nwgmma.mma_async.sync.aligned.m64n256k16.f16.f16.f16 " PREC_R64
-                 ", %64, %65, p, 1, 1, 0, 0;\n}\n"
-                 : PREC_64("+r", 0)
-                 : "l"(da), "l"(db), "r"(scale_d));
-}
+SM_TILE_WGMMA(wgmma_tf32, float, 128, "+f", "m64n256k8.f32.tf32.tf32", ", 1, 1")
+SM_TILE_WGMMA(wgmma_f16, float, 128, "+f", "m64n256k16.f32.f16.f16", ", 1, 1, 0, 0")
+SM_TILE_WGMMA(wgmma_e5m2, float, 128, "+f", "m64n256k32.f32.e5m2.e5m2", ", 1, 1")
+SM_TILE_WGMMA(wgmma_f16acc, unsigned, 64, "+r", "m64n256k16.f16.f16.f16", ", 1, 1, 0, 0")
 
 // d += a * b for one 16 x 8 x 16 tile of the F64 leg (DMMA).
 __device__ __forceinline__ void dmma(double* d, const double (&a)[8], const double (&b)[4]) {
@@ -210,7 +159,7 @@ __global__ void __launch_bounds__(kPrecisionThreads, 1) precision_kernel(const P
         const unsigned m = e < M * K ? e / K : (e - M * K) % N, k = e < M * K ? e % K : (e - M * K) / N;
         unsigned char* base = e < M * K ? sA : sB;
         if constexpr (L::kF64) store_operand<LEG>(base + ((size_t)m * LD + k) * 8, v);
-        else store_operand<LEG>(base + kmajor<ELEM, K>(m, k), v);
+        else store_operand<LEG>(base + kmajor_off<ELEM, K>(m, k), v);
     };
     if constexpr (L::kF64) {
         for (unsigned e = tid; e < M * K + K * N; e += kPrecisionThreads)       // wide: 20 low bits, sign-extended
@@ -233,16 +182,14 @@ __global__ void __launch_bounds__(kPrecisionThreads, 1) precision_kernel(const P
     asm volatile("mov.u32 %0, %%nsmid;" : "=r"(nsmid));
     const unsigned wg = tid >> 7, warp = tid >> 5, lane = tid & 31u;
     const unsigned r0 = (L::kF64 ? 16u * warp : 64u * wg + 16u * (warp & 3u)) + (lane >> 2), c0 = 2u * (lane & 3u);
-    // the injection, resolved once: this thread's iteration to inject after (all ones: none) and rows it owns
-    const unsigned rowsel = (a.inj_row < 0) ? 3u : ((unsigned)a.inj_row == r0 ? 1u : (unsigned)a.inj_row == r0 + 8 ? 2u : 0u);
-    const unsigned inj_it = (a.inj_mask && rowsel && (a.inj_sm < 0 || (unsigned)a.inj_sm == smid)) ? a.inj_iter : ~0u;
+    const Injection inj = resolve_injection(a, r0, smid);
 
     Acc acc[L::kRegs];
 #pragma unroll
     for (int j = 0; j < (int)L::kRegs; ++j) acc[j] = 0;
     const unsigned w0 = 2u * (r0 * N + c0) + 1u;                   // value j's weight 2e + 1 is w0 + a constant
     unsigned long long run = 0;
-    const unsigned long long t0 = timer_ns();
+    const unsigned long long t0 = globaltimer_ns();
     const long long k0 = clock64();
     for (unsigned it = 0; it < a.iterations; ++it) {
         if constexpr (LEG == CRO_PRECISION_LEG_F64) {
@@ -292,13 +239,13 @@ __global__ void __launch_bounds__(kPrecisionThreads, 1) precision_kernel(const P
             for (int j = 0; j < 64; ++j) acc[j] = 0;
 #pragma unroll 1
             for (unsigned kc = 0; kc < K; kc += 8) {                 // 8 halves: one 16-byte core-matrix row
-                const uint4 x0 = *reinterpret_cast<const uint4*>(sA + kmajor<2, K>(r0, kc));
-                const uint4 x1 = *reinterpret_cast<const uint4*>(sA + kmajor<2, K>(r0 + 8, kc));
+                const uint4 x0 = *reinterpret_cast<const uint4*>(sA + kmajor_off<2, K>(r0, kc));
+                const uint4 x1 = *reinterpret_cast<const uint4*>(sA + kmajor_off<2, K>(r0 + 8, kc));
                 const unsigned a0[4] = {x0.x, x0.y, x0.z, x0.w}, a1[4] = {x1.x, x1.y, x1.z, x1.w};
 #pragma unroll
                 for (int g = 0; g < 32; ++g) {
-                    const uint4 y0 = *reinterpret_cast<const uint4*>(sB + kmajor<2, K>(8u * g + c0, kc));
-                    const uint4 y1 = *reinterpret_cast<const uint4*>(sB + kmajor<2, K>(8u * g + c0 + 1, kc));
+                    const uint4 y0 = *reinterpret_cast<const uint4*>(sB + kmajor_off<2, K>(8u * g + c0, kc));
+                    const uint4 y1 = *reinterpret_cast<const uint4*>(sB + kmajor_off<2, K>(8u * g + c0 + 1, kc));
                     const unsigned b0[4] = {y0.x, y0.y, y0.z, y0.w}, b1[4] = {y1.x, y1.y, y1.z, y1.w};
 #pragma unroll
                     for (int k = 0; k < 8; ++k) {
@@ -312,8 +259,8 @@ __global__ void __launch_bounds__(kPrecisionThreads, 1) precision_kernel(const P
             }
         } else {
             constexpr unsigned SBO = 8u * K * ELEM;
-            const unsigned long long da = desc(smem_addr(sA) + wg * 64u * K * ELEM, SBO);
-            const unsigned long long db = desc(smem_addr(sB), SBO);
+            const unsigned long long da = wgmma_desc(smem_u32(sA) + wg * 64u * K * ELEM, SBO);
+            const unsigned long long db = wgmma_desc(smem_u32(sB), SBO);
             asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory");
 #pragma unroll
             for (unsigned s = 0; s < K * ELEM / 32; ++s) {            // 32 bytes of K per instruction: +256 bytes, >> 4
@@ -330,11 +277,11 @@ __global__ void __launch_bounds__(kPrecisionThreads, 1) precision_kernel(const P
                 else asm volatile("" : "+f"(acc[j])::"memory");
             }
         }
-        if (it == inj_it) {                                        // test only: one compare on the clean path
+        if (it == inj.iter) {                                        // test only: one compare on the clean path
 #pragma unroll
             for (int j = 0; j < (int)L::kVals; ++j) {
                 const unsigned col = 8u * (j >> 2) + c0 + (j & 1);
-                if (((rowsel >> ((j >> 1) & 1)) & 1u) && (a.inj_col < 0 || (unsigned)a.inj_col == col)) inject<LEG>(acc, j, a.inj_mask);
+                if (((inj.rows >> ((j >> 1) & 1)) & 1u) && (a.inj_col < 0 || (unsigned)a.inj_col == col)) inject<LEG>(acc, j, a.inj_mask);
             }
         }
         __syncwarp();
@@ -345,7 +292,7 @@ __global__ void __launch_bounds__(kPrecisionThreads, 1) precision_kernel(const P
         run += f;
     }
     const long long k1 = clock64();
-    const unsigned long long t1 = timer_ns();
+    const unsigned long long t1 = globaltimer_ns();
 
     unsigned long long efold = 0;
     unsigned mism = compare<LEG, 0>(acc, r0, c0, smid, a, &efold);
@@ -355,26 +302,7 @@ __global__ void __launch_bounds__(kPrecisionThreads, 1) precision_kernel(const P
         mism += compare<LEG, 3>(acc, r0, c0, smid, a, &efold);
     }
     const unsigned fold_bad = run != (unsigned long long)a.iterations * efold ? 1u : 0u;
-    const unsigned wm = __reduce_add_sync(0xffffffffu, mism), wf = __reduce_add_sync(0xffffffffu, fold_bad);
-    if (lane == 0 && (wm | wf)) {
-        atomicAdd(&s_mism, (unsigned long long)wm);
-        atomicAdd(&s_fold_mism, (unsigned long long)wf);
-    }
-    atomicAdd(&s_fold, run);
-    __syncthreads();
-    if (tid == 0) {
-        if (smid < CRO_PRECISION_MAX_SMS) atomicOr(a.sm_bits + (smid >> 6), 1ull << (smid & 63u));
-        ComputeCta& o = a.cta[blockIdx.x];
-        o.t0 = t0;
-        o.t1 = t1;
-        o.cycles = (unsigned long long)(k1 - k0);
-        o.mismatches = s_mism;
-        o.fold_mismatches = s_fold_mism;
-        o.fold = s_fold;
-        o.smid = smid;
-        o.nsmid = nsmid;
-        o.stamp = a.stamp;
-    }
+    publish_cta<CRO_PRECISION_MAX_SMS>(a, mism, fold_bad, run, t0, t1, k0, k1, smid, nsmid, s_mism, s_fold_mism, s_fold);
 }
 
 template <unsigned LEG>

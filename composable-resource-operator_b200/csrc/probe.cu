@@ -434,7 +434,7 @@ int probe_enqueue(cro_ctx* c, Device* d, Lane& L) {
 
     // this probe's seed: the host refreshes the 16 bytes the graph's first node copies to the device
     const uint64_t nonce = d->nonce_next++;
-    L.h_params->seed = seed_of(d, nonce);
+    L.h_params->seed = space_seed(d, kSeedNonce, nonce);
     L.h_params->nonce = nonce;
     d->seed_cur = L.h_params->seed;
     d->nonce_cur = nonce;

@@ -42,7 +42,29 @@ struct Range {
 uint64_t fresh_seed();
 
 inline Params imm_params(const Device* d) { return Params{ProbeParams{d->seed_cur, d->nonce_cur}, nullptr}; }
-inline uint64_t seed_of(const Device* d, uint64_t nonce) { return d->seed_dev + nonce * kNonceStride; }
+
+// The seed spaces of a device: seed j of call k in a space is seed_dev + offset + (per_call * k + j) * kNonceStride.
+// No seed of one space is a seed of another while every count per_call * k + j stays below 2^58.  kNonceStride is
+// odd, hence invertible mod 2^64, so seeds of offsets O != O' and counts n, n' are equal only when (n - n') *
+// kNonceStride = O' - O (mod 2^64).  Every offset is 0 or a power of two from 2^58 up, so O' - O is a nonzero multiple
+// of 2^58 mod 2^64, and so is n - n' (an odd factor keeps the power of two in a number): n or n' is at least 2^58.
+// Within a space distinct counts give distinct seeds, so no call passes on what an earlier call left behind.
+enum SeedSpace { kSeedNonce, kSeedRetest, kSeedLink, kSeedCompute, kSeedSram, kSeedL2, kSeedPrecision };
+struct SeedSpaceInfo {
+    uint64_t offset, per_call;
+};
+constexpr SeedSpaceInfo kSeedSpaces[] = {
+    {0, 1},             // kSeedNonce: probe nonce k (the HBM probe's pattern)
+    {1ull << 63, 1},    // kSeedRetest: the fault locator's retest pattern (k = 0)
+    {1ull << 62, 3},    // kSeedLink: host link patterns P1 .. P3
+    {1ull << 61, 1},    // kSeedCompute: compute probe operands
+    {1ull << 60, 8},    // kSeedSram: SRAM probe, one per cluster rank (the largest cluster)
+    {1ull << 59, 2},    // kSeedL2: L2 probe march (j = 0) and atomics (j = 1)
+    {1ull << 58, 1},    // kSeedPrecision: precision probe operands
+};
+inline uint64_t space_seed(const Device* d, SeedSpace s, uint64_t k, uint64_t j = 0) {
+    return d->seed_dev + kSeedSpaces[s].offset + (kSeedSpaces[s].per_call * k + j) * kNonceStride;
+}
 
 inline Device* dev_at(cro_ctx* c, int idx) {
     if (!c || idx < 0 || idx >= (int)c->devs.size()) return nullptr;

@@ -9,19 +9,6 @@
 namespace cro {
 
 namespace {
-// Seeds of call k: seed_dev + 2^60 + (8k + r) * kNonceStride for cluster rank r < 8 (r = 0: the local leg's, the one
-// reported).  No other seed of the device reaches them while every count stays below 2^57.  The stride is odd, hence
-// invertible mod 2^64, and 2^60 times an odd number is c * 2^60 with c odd (mod 2^64), which as a signed difference is
-// an odd multiple of 2^60, at least 2^60 in size:
-//   probe nonce n:       seed_dev + n * stride needs (8k + r - n) * stride = -2^60: n or 8k + r is at least 2^60;
-//   locator retest:      seed_dev + 2^63 needs (8k + r) * stride = 2^63 - 2^60 = 7 * 2^60, so 8k + r >= 2^60;
-//   link pattern 3k'+j:  seed_dev + 2^62 + (3k' + j) * stride needs (8k + r - 3k' - j) * stride = 3 * 2^60, so
-//                        8k + r or 3k' + j is at least 2^60;
-//   compute call k':     seed_dev + 2^61 + k' * stride needs (8k + r - k') * stride = 2^60, so 8k + r or k' >= 2^60.
-// Distinct (k, r) give distinct seeds: no call passes on what an earlier call, or another rank, left in shared memory,
-// which no launch clears.
-constexpr uint64_t kSramSeedOffset = 1ull << 60;
-constexpr uint64_t kSramSeedsPerCall = 8;           // the largest cluster
 // Iterations per CTA and launches per leg when the caller gives none.  On an H100 80GB HBM3 at a 400 W limit
 // (profiles/h100_400w_sram_rate.jsonl) a local launch of 64 iterations takes 2.9 ms and a network launch at C = 2
 // 1.8 ms, and one round of each covers all 132 SMs: about 5 ms a call for every cell written and read back 64 times
@@ -129,7 +116,7 @@ int ctx_probe_sram(cro_ctx* c, int idx, const cro_sram_opts& o, cro_sram_result*
         }
         const int net_grid = clusters * (int)cluster, max_grid = std::max(sm_count, net_grid);
         const uint64_t k = d->sram_calls++;
-        const uint64_t seed = d->seed_dev + kSramSeedOffset + k * kSramSeedsPerCall * kNonceStride;
+        const uint64_t seed = space_seed(d, kSeedSram, k);     // rank r's: seed + r * kNonceStride
         r->seed = seed;
         r->call = k;
         r->sm_count = (uint32_t)sm_count;

@@ -370,3 +370,19 @@ def test_no_precision_kernel_spills(tmp_path):
     spills = re.findall(r"(\d+) bytes spill stores, (\d+) bytes spill loads", out)
     assert len([e for e in entries if "precision_kernel" in e]) == 7 and len(spills) >= 7, out
     assert all(s == ("0", "0") for s in spills), out
+
+
+def _sass_pin():
+    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
+    import make_kernel_sass
+    return make_kernel_sass, json.load(open(os.path.join(ROOT, "tests", "golden", "precision_sass.json")))
+
+
+@pytest.mark.skipif(_tool("cuobjdump") is None or _tool("nvcc") is None, reason="the CUDA tools are not installed")
+def test_precision_kernels_sass_and_ptxas_are_pinned(cro):
+    # every precision kernel's machine code and resources as recorded (tests/golden/make_kernel_sass.py)
+    mk, want = _sass_pin()
+    got = mk.sass_digests(mk.obj_of("precision_kernels.cu"))
+    assert sorted(got) == sorted(want["sass_sha256"])
+    assert got == want["sass_sha256"], [k for k in got if got[k] != want["sass_sha256"][k]]
+    assert mk.ptxas_lines("precision_kernels.cu") == want["ptxas"]
