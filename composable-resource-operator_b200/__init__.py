@@ -550,6 +550,33 @@ class L2Fault(ctypes.Structure):
                 ("line", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
 
 
+# test hooks: the compute, precision and SRAM probes' classification of caller-given rounds
+# (cro_selftest_sm_legs_classify, cro_selftest_sram_classify)
+SM_LEGS_COMPUTE, SM_LEGS_PRECISION = 0, 1
+
+
+class SmCta(ctypes.Structure):
+    """cro_sm_cta: what one CTA of a compute or precision leg publishes at the end of a round."""
+    _fields_ = [("stamp", ctypes.c_uint64), ("t0", ctypes.c_uint64), ("t1", ctypes.c_uint64), ("cycles", ctypes.c_uint64),
+                ("mismatches", ctypes.c_uint64), ("fold_mismatches", ctypes.c_uint64), ("fold", ctypes.c_uint64),
+                ("smid", ctypes.c_uint32), ("nsmid", ctypes.c_uint32)]
+
+
+class SramCta(ctypes.Structure):
+    """cro_sram_cta: what one CTA of an SRAM leg publishes at the end of a round."""
+    _fields_ = [("stamp", ctypes.c_uint64), ("t0", ctypes.c_uint64), ("t1", ctypes.c_uint64), ("cycles", ctypes.c_uint64),
+                ("count", ctypes.c_uint64 * SRAM_ELEMENTS), ("last", ctypes.c_uint64), ("fold_x", ctypes.c_uint64),
+                ("fold_s", ctypes.c_uint64), ("fold_w", ctypes.c_uint64), ("smid", ctypes.c_uint32), ("nsmid", ctypes.c_uint32),
+                ("rank", ctypes.c_uint32), ("block", ctypes.c_uint32)]
+
+
+class SramRecord(ctypes.Structure):
+    """cro_sram_record: one word record of an SRAM leg as the device keeps it (peer_block resolved through `round`)."""
+    _fields_ = [("element", ctypes.c_uint32), ("iteration", ctypes.c_uint32), ("smid", ctypes.c_uint32),
+                ("peer_block", ctypes.c_uint32), ("round", ctypes.c_uint32), ("word", ctypes.c_uint32),
+                ("expected", ctypes.c_uint64), ("actual", ctypes.c_uint64)]
+
+
 # test hook: one sweep kernel between guard bands (cro_selftest_sweep)
 (SELFTEST_SWEEP_FILL, SELFTEST_SWEEP_COPY_LDG, SELFTEST_SWEEP_COPY_TMA, SELFTEST_SWEEP_COPY_FUSED, SELFTEST_SWEEP_READ_LDG,
  SELFTEST_SWEEP_READ_TMA, SELFTEST_SWEEP_READ_LDG256, SELFTEST_SWEEP_LOCATE, SELFTEST_SWEEP_FORCE_WORDS,
@@ -588,6 +615,7 @@ assert ctypes.sizeof(LinkResult) == 984 and ctypes.sizeof(PciPath) == 272, ctype
 assert ctypes.sizeof(ScanReport) == 12632 and ctypes.sizeof(ScanOpts) == 72, ctypes.sizeof(ScanReport)
 assert ctypes.sizeof(SramResult) == 568 and ctypes.sizeof(SramSm) == 168 and ctypes.sizeof(SramFault) == 48, ctypes.sizeof(SramResult)
 assert ctypes.sizeof(L2Result) == 616 and ctypes.sizeof(L2Sm) == 128 and ctypes.sizeof(L2Fault) == 56, ctypes.sizeof(L2Result)
+assert ctypes.sizeof(SmCta) == 64 and ctypes.sizeof(SramCta) == 128 and ctypes.sizeof(SramRecord) == 40, ctypes.sizeof(SramCta)
 
 # Every symbol include/croprobe.h declares; tests check the library exports all of them.
 EXPORTS = [
@@ -616,6 +644,7 @@ EXPORTS = [
     "cro_scan_hbm", "cro_scan_hbm_uuid", "cro_read_hbm_health", "cro_emit_scan_annotations_json",
     "cro_probe_sram", "cro_probe_sram_uuid", "cro_read_sram_health", "cro_emit_sram_annotations_json",
     "cro_probe_l2", "cro_probe_l2_uuid", "cro_read_l2_health", "cro_emit_l2_annotations_json", "cro_selftest_l2_classify",
+    "cro_selftest_sm_legs_classify", "cro_selftest_sram_classify",
 ]
 
 # Slot map of a device's sweep-slot array (cro_sweep_slot, 64 bytes each); the cro_selftest_* hooks take such arrays.
@@ -748,6 +777,13 @@ def _load() -> ctypes.CDLL:
         "cro_read_l2_health": (i32, [c, ctypes.POINTER(L2Health)]),
         "cro_emit_l2_annotations_json": (i32, [ctypes.POINTER(L2Result)] + out),
         "cro_selftest_l2_classify": (i32, [ctypes.POINTER(L2Result), ctypes.POINTER(L2Sm), i32, ctypes.POINTER(L2Fault), i32]),
+        "cro_selftest_sm_legs_classify": (i32, [i32, u32, ctypes.POINTER(u32), u32, u64, ctypes.POINTER(u32),
+                                                ctypes.POINTER(SmCta), ctypes.POINTER(u64), ctypes.POINTER(u64), vp, vp, vp, i32,
+                                                ctypes.POINTER(i32), vp, i32, ctypes.POINTER(i32)]),
+        "cro_selftest_sram_classify": (i32, [u32, u32, u32, u64, u32, u32, u32, u64, ctypes.POINTER(u32),
+                                             ctypes.POINTER(SramCta), ctypes.POINTER(u64), ctypes.POINTER(SramRecord),
+                                             ctypes.POINTER(SramResult), ctypes.POINTER(SramSm), i32, ctypes.POINTER(i32),
+                                             ctypes.POINTER(SramFault), i32, ctypes.POINTER(i32)]),
         "cro_local_node_op": (i32, [vp, c] + out),
         "cro_local_exec": (i32, [c] + out),
         "cro_describe_wire_type": (i32, [c] + out),
@@ -968,6 +1004,57 @@ def selftest_l2_classify(r: L2Result, sms: List[L2Sm], faults: List[L2Fault]) ->
     if rc != OK:
         raise ProbeError(rc, "cro_selftest_l2_classify")
     return out, list(s[:len(sms)]), list(f[:len(faults)])
+
+
+def _legs_rounds(n_legs: int, legs: int, rounds, claims, records, cta, words: int, fault):
+    """The flat arrays of the selftest hooks: per leg of `legs`, rounds[l] as (CTA records, coverage words) pairs and
+    records[l]; `words` 0 means the rounds carry no coverage words."""
+    ran = [l for l in range(n_legs) if legs >> l & 1]
+    ctas = [x for l in ran for got, _ in rounds[l] for x in got]
+    bits = [b for l in ran for _, got in rounds[l] for b in got]
+    recs = [x for l in ran for x in records[l]]
+    assert all(len(got) == words for l in ran for _, got in rounds[l])
+    return ((ctypes.c_uint32 * n_legs)(*[len(rounds[l]) if l in ran else 0 for l in range(n_legs)]),
+            (cta * max(1, len(ctas)))(*ctas), (ctypes.c_uint64 * max(1, len(bits)))(*bits),
+            (ctypes.c_uint64 * n_legs)(*claims), (fault * max(1, len(recs)))(*recs))
+
+
+def selftest_sm_legs_classify(probe: int, iterations: List[int], grid: int, call: int, rounds, claims: List[int],
+                              records, legs: int = 0):
+    """cro_selftest_sm_legs_classify: the compute (SM_LEGS_COMPUTE) or precision probe's classification of call `call`
+    on `grid` SMs.  Per leg l (every list is indexed by leg; legs 0: all): rounds[l] a list of (grid SmCta, the
+    COMPUTE_MAX_SMS // 64 coverage words) per round, claims[l] and records[l] (ComputeFault / PrecisionFault, the first
+    min(claims[l], RECORDS)).  Returns (result, SM entries, faults); the result's status may be OK, ERR_CHECKSUM or
+    ERR_UNSUPPORTED."""
+    compute = probe == SM_LEGS_COMPUTE
+    n_legs = COMPUTE_LEGS if compute else PRECISION_LEGS
+    result, sm, fault = (ComputeResult, ComputeSm, ComputeFault) if compute else (PrecisionResult, PrecisionSm, PrecisionFault)
+    ran = legs or (1 << n_legs) - 1
+    nr, ctas, bits, cl, recs = _legs_rounds(n_legs, ran, rounds, claims, records, SmCta, COMPUTE_MAX_SMS // 64, fault)
+    it = (ctypes.c_uint32 * n_legs)(*iterations)
+    cap = sum(len(records[l]) for l in range(n_legs) if ran >> l & 1)
+    rc, out = _per_sm(lib.cro_selftest_sm_legs_classify, (probe, legs, it, grid, call, nr, ctas, bits, cl,
+                                                          recs), result, sm, COMPUTE_MAX_SMS, fault, cap)
+    if rc not in (OK, ERR_CHECKSUM, ERR_UNSUPPORTED):
+        raise ProbeError(rc, "cro_selftest_sm_legs_classify")
+    return out
+
+
+def selftest_sram_classify(iterations: int, n_words: int, seed: int, cluster: int, sm_count: int, net_grid: int, call: int,
+                           rounds, claims: List[int], records, legs: int = 0):
+    """cro_selftest_sram_classify: the SRAM probe's classification of call `call`.  Per leg l (legs 0: both): rounds[l] a
+    list of rounds, each a list of SramCta (sm_count of them for the local leg, net_grid for the network leg),
+    claims[l] and records[l] (SramRecord, the first min(claims[l], SRAM_RECORDS)).  Returns (result, SM entries,
+    faults); the result's status may be OK, ERR_CHECKSUM or ERR_UNSUPPORTED."""
+    ran = legs or SRAM_ALL_LEGS
+    nr, ctas, _, cl, recs = _legs_rounds(SRAM_LEGS, ran, [[(x, []) for x in r] for r in rounds], claims, records, SramCta, 0,
+                                         SramRecord)
+    cap = sum(len(records[l]) for l in range(SRAM_LEGS) if ran >> l & 1)
+    rc, out = _per_sm(lib.cro_selftest_sram_classify, (legs, iterations, n_words, seed, cluster, sm_count, net_grid, call, nr,
+                                                       ctas, cl, recs), SramResult, SramSm, SRAM_MAX_SMS, SramFault, cap)
+    if rc not in (OK, ERR_CHECKSUM, ERR_UNSUPPORTED):
+        raise ProbeError(rc, "cro_selftest_sram_classify")
+    return out
 
 
 def _sram_opts(legs: int, iterations: int, cluster: int, max_rounds: int, deadline_ms: int,

@@ -502,6 +502,80 @@ int cro_selftest_l2_classify(cro_l2_result* r, cro_l2_sm* sms, int n_sms, cro_l2
     l2_classify(r, sms, (size_t)n_sms, faults, (size_t)n);
     return CRO_OK;
 } CRO_API_CATCH
+int cro_selftest_sm_legs_classify(int probe, uint32_t legs, const uint32_t* iterations, uint32_t grid, uint64_t call,
+                                  const uint32_t* rounds, const cro_sm_cta* ctas, const uint64_t* sm_bits, const uint64_t* claims,
+                                  const void* records, void* out, void* sms, int sms_cap, int* n_sms, void* faults, int cap,
+                                  int* n) try {
+    const uint32_t n_legs = probe == CRO_SM_LEGS_COMPUTE ? CRO_COMPUTE_LEGS : CRO_PRECISION_LEGS;
+    const uint32_t max_records = probe == CRO_SM_LEGS_COMPUTE ? CRO_COMPUTE_RECORDS : CRO_PRECISION_RECORDS;
+    const uint32_t all = (1u << n_legs) - 1;
+    if (legs == 0) legs = all;
+    if ((probe != CRO_SM_LEGS_COMPUTE && probe != CRO_SM_LEGS_PRECISION) || (legs & ~all) || !iterations || !rounds || !claims ||
+        grid == 0 || !out || !n_sms || !n || sms_cap < 0 || cap < 0 || (sms_cap > 0 && !sms) || (cap > 0 && !faults))
+        return CRO_ERR_INVALID_ARG;
+    uint64_t n_rounds = 0, n_records = 0;
+    for (uint32_t l = 0; l < n_legs; ++l) {
+        if (!(legs >> l & 1u)) continue;
+        if (!iterations[l]) return CRO_ERR_INVALID_ARG;
+        n_rounds += rounds[l];
+        n_records += std::min<uint64_t>(claims[l], max_records);
+    }
+    if ((n_rounds && (!ctas || !sm_bits)) || (n_records && !records)) return CRO_ERR_INVALID_ARG;
+    *n = *n_sms = 0;
+    auto copy_out = [&](int rc, const auto& seen, const auto& found, auto* s, auto* f) {
+        const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
+        std::copy(seen.begin(), seen.begin() + ks, s);
+        std::copy(found.begin(), found.begin() + kf, f);
+        *n_sms = (int)ks;
+        *n = (int)kf;
+        return rc;
+    };
+    if (probe == CRO_SM_LEGS_COMPUTE) {
+        std::vector<cro_compute_sm> seen;
+        std::vector<cro_compute_fault> found;
+        const int rc = classify_compute(legs, iterations, grid, call, rounds, ctas, sm_bits, claims,
+                                        static_cast<const cro_compute_fault*>(records), static_cast<cro_compute_result*>(out),
+                                        &seen, &found);
+        return copy_out(rc, seen, found, static_cast<cro_compute_sm*>(sms), static_cast<cro_compute_fault*>(faults));
+    }
+    std::vector<cro_precision_sm> seen;
+    std::vector<cro_precision_fault> found;
+    const int rc = classify_precision(legs, iterations, grid, call, rounds, ctas, sm_bits, claims,
+                                      static_cast<const cro_precision_fault*>(records), static_cast<cro_precision_result*>(out),
+                                      &seen, &found);
+    return copy_out(rc, seen, found, static_cast<cro_precision_sm*>(sms), static_cast<cro_precision_fault*>(faults));
+} CRO_API_CATCH
+int cro_selftest_sram_classify(uint32_t legs, uint32_t iterations, uint32_t n_words, uint64_t seed, uint32_t cluster,
+                               uint32_t sm_count, uint32_t net_grid, uint64_t call, const uint32_t* rounds, const cro_sram_cta* ctas,
+                               const uint64_t* claims, const cro_sram_record* records, cro_sram_result* out, cro_sram_sm* sms,
+                               int sms_cap, int* n_sms, cro_sram_fault* faults, int cap, int* n) try {
+    if (legs == 0) legs = CRO_SRAM_ALL_LEGS;
+    const bool net = legs & CRO_SRAM_LEG_DSMEM;
+    if ((legs & ~CRO_SRAM_ALL_LEGS) || iterations == 0 || iterations > CRO_SRAM_MAX_ITERATIONS ||
+        (cluster != 2 && cluster != 4 && cluster != 8) || sm_count == 0 || (net && (net_grid == 0 || net_grid % cluster)) ||
+        !rounds || !claims || !out || !n_sms || !n || sms_cap < 0 || cap < 0 || (sms_cap > 0 && !sms) || (cap > 0 && !faults))
+        return CRO_ERR_INVALID_ARG;
+    uint64_t n_ctas = 0, n_records = 0;
+    for (uint32_t l = 0; l < CRO_SRAM_LEGS; ++l) {
+        if (!(legs >> l & 1u)) continue;
+        n_ctas += (uint64_t)rounds[l] * (l == CRO_SRAM_DSMEM ? net_grid : sm_count);
+        n_records += std::min<uint64_t>(claims[l], CRO_SRAM_RECORDS);
+    }
+    if ((n_ctas && !ctas) || (n_records && !records)) return CRO_ERR_INVALID_ARG;
+    *n = *n_sms = 0;
+    std::vector<cro_sram_sm> seen;
+    std::vector<cro_sram_fault> found;
+    const int rc = classify_sram(legs, iterations, n_words, seed, cluster, sm_count, net_grid, call, rounds, ctas, claims, records,
+                                 out, &seen, &found);
+    const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
+    std::copy(seen.begin(), seen.begin() + ks, sms);
+    std::copy(found.begin(), found.begin() + kf, faults);
+    *n_sms = (int)ks;
+    *n = (int)kf;
+    out->sms_listed = (uint32_t)ks;
+    out->recorded = kf;
+    return rc;
+} CRO_API_CATCH
 int cro_compute_expected(int answer, uint64_t seed, int32_t* out) try {
     return compute::Expected(answer, seed, out);
 } CRO_API_CATCH

@@ -64,4 +64,10 @@ int ctx_probe_compute_uuid(cro_ctx* c, const char* uuid, const cro_compute_opts&
     return probe_sm_legs_uuid<ComputeProbe>(c, uuid, o, deadline_ms, r, sms, faults, cap, helper_ns);
 }
 
+int classify_compute(uint32_t legs, const uint32_t* iterations, uint32_t grid, uint64_t k, const uint32_t* rounds,
+                     const cro_sm_cta* ctas, const uint64_t* sm_bits, const uint64_t* claims, const cro_compute_fault* records,
+                     cro_compute_result* r, std::vector<cro_compute_sm>* sms, std::vector<cro_compute_fault>* faults) {
+    return classify_sm_legs<ComputeProbe>(legs, iterations, grid, k, rounds, ctas, sm_bits, claims, records, r, sms, faults);
+}
+
 }  // namespace cro

@@ -165,4 +165,10 @@ int ctx_probe_precision_uuid(cro_ctx* c, const char* uuid, const cro_precision_o
     return probe_sm_legs_uuid<PrecisionProbe>(c, uuid, o, deadline_ms, r, sms, faults, cap, helper_ns);
 }
 
+int classify_precision(uint32_t legs, const uint32_t* iterations, uint32_t grid, uint64_t k, const uint32_t* rounds,
+                       const cro_sm_cta* ctas, const uint64_t* sm_bits, const uint64_t* claims, const cro_precision_fault* records,
+                       cro_precision_result* r, std::vector<cro_precision_sm>* sms, std::vector<cro_precision_fault>* faults) {
+    return classify_sm_legs<PrecisionProbe>(legs, iterations, grid, k, rounds, ctas, sm_bits, claims, records, r, sms, faults);
+}
+
 }  // namespace cro

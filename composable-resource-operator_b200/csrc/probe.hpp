@@ -241,6 +241,13 @@ int ctx_probe_precision(cro_ctx* c, int idx, const cro_precision_opts& o, cro_pr
 int ctx_probe_precision_uuid(cro_ctx* c, const char* uuid, const cro_precision_opts& o, int deadline_ms, cro_precision_result* r,
                              std::vector<cro_precision_sm>* sms, std::vector<cro_precision_fault>* faults, int cap,
                              uint64_t* helper_ns);
+// cro_selftest_sm_legs_classify: each probe's classification of the caller's rounds and records (sm_legs.hpp).
+int classify_compute(uint32_t legs, const uint32_t* iterations, uint32_t grid, uint64_t k, const uint32_t* rounds,
+                     const cro_sm_cta* ctas, const uint64_t* sm_bits, const uint64_t* claims, const cro_compute_fault* records,
+                     cro_compute_result* r, std::vector<cro_compute_sm>* sms, std::vector<cro_compute_fault>* faults);
+int classify_precision(uint32_t legs, const uint32_t* iterations, uint32_t grid, uint64_t k, const uint32_t* rounds,
+                       const cro_sm_cta* ctas, const uint64_t* sm_bits, const uint64_t* claims, const cro_precision_fault* records,
+                       cro_precision_result* r, std::vector<cro_precision_sm>* sms, std::vector<cro_precision_fault>* faults);
 namespace precision {
 // The answer tile of the operands of `seed` (include/croprobe.h): answer CRO_PRECISION_ANSWER_*, M x N int64 values,
 // row-major.  CRO_ERR_INVALID_ARG for another answer.
@@ -306,6 +313,11 @@ int ctx_probe_sram_uuid(cro_ctx* c, const char* uuid, const cro_sram_opts& o, cr
                         std::vector<cro_sram_fault>* faults, int cap);
 // CRO_SRAM_HEALTH_* of the NVML reads before the first leg and after the last.
 uint32_t sram_health(const cro_sram_health& before, const cro_sram_health& after);
+// cro_selftest_sram_classify: the probe's classification of the caller's rounds and records, as ctx_probe_sram makes it.
+int classify_sram(uint32_t legs, uint32_t iterations, uint32_t n_words, uint64_t seed, uint32_t cluster, uint32_t sm_count,
+                  uint32_t net_grid, uint64_t k, const uint32_t* rounds, const cro_sram_cta* ctas, const uint64_t* claims,
+                  const cro_sram_record* records, cro_sram_result* r, std::vector<cro_sram_sm>* sms,
+                  std::vector<cro_sram_fault>* faults);
 
 // L2 probe (include/croprobe.h, cro_probe_l2, l2_probe.cu): *sms gets one entry per SM seen, by SM id; *faults every
 // recorded word, by (word, iteration, element, smid).

@@ -13,6 +13,16 @@
 
 namespace cro {
 
+// cro_sm_cta is the public mirror of ComputeCta (cro_selftest_sm_legs_classify hands the records over as they are).
+static_assert(sizeof(cro_sm_cta) == sizeof(ComputeCta) && offsetof(cro_sm_cta, stamp) == offsetof(ComputeCta, stamp) &&
+                  offsetof(cro_sm_cta, t0) == offsetof(ComputeCta, t0) && offsetof(cro_sm_cta, t1) == offsetof(ComputeCta, t1) &&
+                  offsetof(cro_sm_cta, cycles) == offsetof(ComputeCta, cycles) &&
+                  offsetof(cro_sm_cta, mismatches) == offsetof(ComputeCta, mismatches) &&
+                  offsetof(cro_sm_cta, fold_mismatches) == offsetof(ComputeCta, fold_mismatches) &&
+                  offsetof(cro_sm_cta, fold) == offsetof(ComputeCta, fold) && offsetof(cro_sm_cta, smid) == offsetof(ComputeCta, smid) &&
+                  offsetof(cro_sm_cta, nsmid) == offsetof(ComputeCta, nsmid),
+              "cro_sm_cta mirrors ComputeCta");
+
 // One round of leg `leg` of call k: the CTA records hc (grid of them, each ops / grid operations) into R and per_sm,
 // and the round's coverage bitmap (sm_words words) into R.sms_covered and *covered.  A CTA whose stamp is not k did not
 // publish.  *fold_sm tracks the lowest SM id seen, whose CTA's fold R.fold reports.  CRO_ERR_UNSUPPORTED (with the
@@ -30,8 +40,8 @@ int take_leg_round(cro_ctx* c, const char* who, const std::vector<ComputeCta>& h
             continue;
         }
         if (x.nsmid > max_sms) {
-            c->set_error(std::string(who) + ": the device reports %nsmid = " + std::to_string(x.nsmid) + ", more SM ids than the " +
-                         std::to_string(max_sms) + " the coverage bitmaps hold");
+            set_call_error(c, std::string(who) + ": the device reports %nsmid = " + std::to_string(x.nsmid) +
+                                  ", more SM ids than the " + std::to_string(max_sms) + " the coverage bitmaps hold");
             return CRO_ERR_UNSUPPORTED;
         }
         *nsmid = x.nsmid;
@@ -107,6 +117,35 @@ int close_call(Result* r, uint32_t n_legs, const std::map<uint32_t, Sm>& per_sm,
     });
     r->verdict = all ? CRO_COMPUTE_ALL : any ? CRO_COMPUTE_SM : CRO_COMPUTE_NONE;
     return r->status = any ? CRO_ERR_CHECKSUM : CRO_OK;
+}
+
+// One leg of call k once it is launched: rounds(take) runs its coverage rounds, calling take(&covered) with each round's
+// grid CTA records in hc and its coverage bitmap, then the claims count, in hbits; then the leg's coverage, the records
+// copy_faults(dst, n) copies in (the first min(claims, P::kRecords)) and the marks of finish_leg.  The in-process call
+// and cro_selftest_sm_legs_classify both run every leg through here.
+template <class P, class Rounds, class CopyFaults>
+int take_leg(cro_ctx* c, const char* who, const std::vector<ComputeCta>& hc, const unsigned long long* hbits, uint64_t k,
+             uint32_t leg, uint32_t iterations, cro_compute_leg& R, uint32_t* nsmid, std::map<uint32_t, typename P::Sm>& per_sm,
+             std::vector<typename P::Fault>* faults, Rounds rounds, CopyFaults copy_faults) {
+    constexpr int kSmWords = P::kMaxSms / 64;
+    const uint32_t grid = (uint32_t)hc.size();
+    uint32_t fold_sm = ~0u;
+    auto take = [&](uint32_t* covered) -> int {
+        return take_leg_round(c, who, hc, k, leg, P::ops(leg) * iterations * (uint64_t)grid, hbits, kSmWords, P::kMaxSms, R,
+                              nsmid, &fold_sm, per_sm, covered);
+    };
+    const int e = rounds(take);
+    if (e) return e;
+    R.complete = R.sms_covered >= grid ? 1u : 0u;
+    R.recorded = std::min<uint64_t>(hbits[kSmWords], P::kRecords);
+    if (R.recorded) {
+        std::vector<typename P::Fault> f((size_t)R.recorded);
+        const int ef = copy_faults(f.data(), f.size());
+        if (ef) return ef;
+        faults->insert(faults->end(), f.begin(), f.end());
+    }
+    finish_leg(R, per_sm, leg, iterations);
+    return CRO_OK;
 }
 
 // What a probe P gives the calls below:
@@ -220,31 +259,77 @@ int probe_sm_legs(cro_ctx* c, int idx, const typename P::Opts& o, typename P::Re
             a.inj_mask = (inj && (uint32_t)o.test_inject_leg == leg) ? o.test_inject_mask : 0;
             R.iterations = iters[leg];
             R.expect_fold = (uint64_t)iters[leg] * fold[answer];
-            uint32_t fold_sm = ~0u;
             auto launch = [&] { return P::launch(leg, a, grid, st); };
             auto fetch = [&] {
                 cudaError_t e = cudaMemcpyAsync(hc.data(), cta, cta_bytes, cudaMemcpyDeviceToHost, st);
                 return e ? e : cudaMemcpyAsync(hbits, a.sm_bits, sizeof hbits, cudaMemcpyDeviceToHost, st);
             };
-            auto take = [&](uint32_t* covered) -> int {
-                return take_leg_round(c, who.c_str(), hc, k, leg, P::ops(leg) * iters[leg] * (uint64_t)grid, hbits, kSmWords,
-                                      P::kMaxSms, R, &r->nsmid, &fold_sm, per_sm, covered);
+            auto rounds = [&](auto take) {
+                return coverage_rounds(c, d, ev, cta, cta_bytes, (uint32_t)grid, max_rounds, &R.rounds, &R.ns, launch, fetch, take);
             };
-            const int e = coverage_rounds(c, d, ev, cta, cta_bytes, (uint32_t)grid, max_rounds, &R.rounds, &R.ns, launch, fetch, take);
+            auto copy_faults = [&](Fault* f, size_t n) -> int {
+                CU_TRY(c, cudaMemcpy(f, a.rec, n * sizeof(Fault), cudaMemcpyDeviceToHost));
+                return CRO_OK;
+            };
+            const int e = take_leg<P>(c, who.c_str(), hc, hbits, k, leg, iters[leg], R, &r->nsmid, per_sm, faults, rounds, copy_faults);
             if (e) return e;
-            R.complete = R.sms_covered >= (uint32_t)grid ? 1u : 0u;
-            R.recorded = std::min<uint64_t>(hbits[kSmWords], P::kRecords);
-            if (R.recorded) {
-                std::vector<Fault> f((size_t)R.recorded);
-                CU_TRY(c, cudaMemcpy(f.data(), a.rec, f.size() * sizeof(Fault), cudaMemcpyDeviceToHost));
-                faults->insert(faults->end(), f.begin(), f.end());
-            }
-            finish_leg(R, per_sm, leg, iters[leg]);
         }
         return CRO_OK;
     }();
     for (cudaEvent_t x : ev)
         if (x) cudaEventDestroy(x);
+    if (rc) {
+        blank_result(r, *r, sms, faults);
+        return r->status = rc;
+    }
+    return close_call(r, P::kLegs, per_sm, sms, faults);
+}
+
+// cro_selftest_sm_legs_classify: call k of a device of `grid` SMs as the in-process call classifies it, from the
+// caller's rounds instead of launches.  Leg l of `legs` ran rounds[l] rounds (grid records of ctas and kMaxSms / 64
+// words of sm_bits each, in leg order) and left claims[l] claims and min(claims[l], kRecords) records.
+template <class P>
+int classify_sm_legs(uint32_t legs, const uint32_t* iterations, uint32_t grid, uint64_t k, const uint32_t* rounds,
+                     const cro_sm_cta* ctas, const uint64_t* sm_bits, const uint64_t* claims, const typename P::Fault* records,
+                     typename P::Result* r, std::vector<typename P::Sm>* sms, std::vector<typename P::Fault>* faults) {
+    using Fault = typename P::Fault;
+    constexpr int kSmWords = P::kMaxSms / 64;
+    blank_result(r, typename P::Result{}, sms, faults);
+    r->call = k;
+    r->sm_count = grid;
+    r->legs = legs;
+    const std::string who = std::string(P::kName) + " probe";
+    std::map<uint32_t, typename P::Sm> per_sm;
+    std::vector<ComputeCta> hc((size_t)grid);
+    unsigned long long hbits[kSmWords + 1];
+    const int rc = [&]() -> int {
+        for (uint32_t leg = 0; leg < P::kLegs; ++leg) {
+            if (!(legs >> leg & 1u)) continue;
+            cro_compute_leg& R = r->leg[leg];
+            R.iterations = iterations[leg];
+            hbits[kSmWords] = claims[leg];
+            auto each_round = [&](auto take) -> int {
+                for (uint32_t j = 0; j < rounds[leg]; ++j, ctas += grid, sm_bits += kSmWords) {
+                    memcpy(hc.data(), ctas, (size_t)grid * sizeof(ComputeCta));
+                    memcpy(hbits, sm_bits, kSmWords * sizeof(uint64_t));
+                    ++R.rounds;
+                    uint32_t covered = 0;
+                    const int e = take(&covered);
+                    if (e) return e;
+                }
+                return CRO_OK;
+            };
+            auto copy_faults = [&](Fault* f, size_t n) -> int {
+                std::copy(records, records + n, f);
+                records += n;
+                return CRO_OK;
+            };
+            const int e = take_leg<P>(nullptr, who.c_str(), hc, hbits, k, leg, iterations[leg], R, &r->nsmid, per_sm, faults,
+                                      each_round, copy_faults);
+            if (e) return e;
+        }
+        return CRO_OK;
+    }();
     if (rc) {
         blank_result(r, *r, sms, faults);
         return r->status = rc;

@@ -759,10 +759,16 @@ typedef struct cro_compute_leg {
     uint32_t failed_sms;           /*  64  distinct SMs with a mismatch or a fold mismatch                       */
     uint32_t unpublished;          /*  68  CTAs launched that published no record                              */
     uint32_t ctas;                 /*  72  CTAs launched, over all rounds                                      */
-    uint32_t slowest_sm;           /*  76  the SM with the most %clock64 cycles per iteration                    */
-    uint32_t slow_permille;        /*  80  its cycles per iteration over the median SM's, x 1000 (report only)   */
+    uint32_t slowest_sm;           /*  76  the SM with the most %clock64 cycles per iteration (cycles summed over
+                                              its CTAs / (CTAs * iterations), integer division); on a tie the
+                                              lowest SM id                                                     */
+    uint32_t slow_permille;        /*  80  its cycles per iteration over the median SM's, x 1000, integer division,
+                                              capped at 2^32 - 1 (report only).  The median of n SMs is the
+                                              (n / 2)-th of their values sorted ascending, from 0: the upper one for
+                                              an even n.  0 when the median is 0                               */
     uint32_t reserved;             /*  84 */
-    uint64_t fold;                 /*  88  running fold summed over the threads of the CTA on the lowest SM id   */
+    uint64_t fold;                 /*  88  running fold summed over the threads of the CTA on the lowest SM id
+                                              (the first such CTA to publish, by round and then by CTA index) */
     uint64_t expect_fold;          /*  96  iterations * the same sum over the expected answer                    */
 } cro_compute_leg;                 /* 104 bytes */
 
@@ -1208,7 +1214,8 @@ typedef struct cro_sram_leg {
     uint32_t unpublished;          /* 108  CTAs launched that published no record                              */
     uint32_t ctas;                 /* 112  CTAs launched, over all rounds                                       */
     uint32_t cluster;              /* 116  network: CTAs per cluster; 0 for the local leg                      */
-    uint64_t fold_xor;             /* 120  local: M5 fold of the CTA on the lowest SM id                         */
+    uint64_t fold_xor;             /* 120  local: M5 fold of the CTA on the lowest SM id (the first such CTA to
+                                              publish, by round and then by CTA index)                          */
     uint64_t fold_sum;             /* 128 */
     uint64_t fold_wsum;            /* 136 */
     uint64_t expect_xor;           /* 144  local: the closed form every CTA's fold must equal                    */
@@ -1504,6 +1511,79 @@ int  cro_read_l2_health(const char *gpu_uuid, cro_l2_health *out);
  * the records faults[0 .. n) (element, iteration, smid, word).  Writes r's verdict, status, bad_sms, bad_sm,
  * bad_lines and bad_line, each sms[].mark and each faults[].line, as cro_probe_l2 does. */
 int  cro_selftest_l2_classify(cro_l2_result *r, cro_l2_sm *sms, int n_sms, cro_l2_fault *faults, int n);
+
+/* What one CTA of a compute or precision leg publishes at the end of a round. */
+typedef struct cro_sm_cta {
+    uint64_t stamp;                /*   0  the call number k; any other value: the CTA did not publish            */
+    uint64_t t0, t1;               /*   8  %globaltimer around the iterations                                     */
+    uint64_t cycles;               /*  24  %clock64 around the iterations                                         */
+    uint64_t mismatches;           /*  32  elements of the last iteration that differ                             */
+    uint64_t fold_mismatches;      /*  40  threads whose running fold differs                                     */
+    uint64_t fold;                 /*  48  every thread's running fold, summed                                    */
+    uint32_t smid;                 /*  56 */
+    uint32_t nsmid;                /*  60 */
+} cro_sm_cta;                      /*  64 bytes */
+
+#define CRO_SM_LEGS_COMPUTE       0   /* cro_selftest_sm_legs_classify: the compute probe   */
+#define CRO_SM_LEGS_PRECISION     1   /* ... the precision probe                           */
+
+/* Test hook: the compute (probe CRO_SM_LEGS_COMPUTE: out a cro_compute_result, sms cro_compute_sm, records and faults
+ * cro_compute_fault) or precision probe's (CRO_SM_LEGS_PRECISION: the cro_precision_* types) classification of call
+ * `call` on a device of `grid` SMs, from caller-given rounds instead of launches.  legs: the legs that ran (0: all).
+ * Per leg l of them: iterations[l] (>= 1) per CTA, rounds[l] rounds, each of `grid` records of ctas and of the
+ * CRO_COMPUTE_MAX_SMS / 64 words of sm_bits (the leg's coverage bitmap after that round), and claims[l] record claims,
+ * of which the first min(claims[l], CRO_COMPUTE_RECORDS) are in `records`; ctas, sm_bits and records run in leg order.
+ * Every array is indexed by leg (CRO_COMPUTE_LEGS or CRO_PRECISION_LEGS entries).  Writes out, sms[0 .. sms_cap) and
+ * faults[0 .. cap) (*n_sms, *n how many) exactly as the in-process call does, all but what needs the device: seed,
+ * host_ref_ns, ns and expect_fold stay 0, and rounds is rounds[l].  Returns out->status (CRO_ERR_UNSUPPORTED with a
+ * blanked result for a %nsmid above CRO_COMPUTE_MAX_SMS), or CRO_ERR_INVALID_ARG for a NULL array it needs, a negative
+ * cap, grid 0, an unknown probe or leg, or a leg of 0 iterations. */
+int  cro_selftest_sm_legs_classify(int probe, uint32_t legs, const uint32_t *iterations, uint32_t grid, uint64_t call,
+                                   const uint32_t *rounds, const cro_sm_cta *ctas, const uint64_t *sm_bits,
+                                   const uint64_t *claims, const void *records, void *out, void *sms, int sms_cap,
+                                   int *n_sms, void *faults, int cap, int *n);
+
+/* What one CTA of an SRAM leg publishes at the end of a round, and one word record of a leg. */
+typedef struct cro_sram_cta {
+    uint64_t stamp;                /*   0  the call number k; any other value: the CTA did not publish            */
+    uint64_t t0, t1;               /*   8  %globaltimer around the iterations                                     */
+    uint64_t cycles;               /*  24  %clock64 around the iterations                                         */
+    uint64_t count[CRO_SRAM_ELEMENTS];   /*  32  compares that failed, per element                              */
+    uint64_t last;                 /*  80  ... of them in the last iteration                                      */
+    uint64_t fold_x, fold_s, fold_w;     /*  88  local: the M5 fold over every iteration                        */
+    uint32_t smid;                 /* 112 */
+    uint32_t nsmid;                /* 116 */
+    uint32_t rank;                 /* 120  rank in the cluster (0 for the local leg)                              */
+    uint32_t block;                /* 124  blockIdx.x                                                             */
+} cro_sram_cta;                    /* 128 bytes */
+
+typedef struct cro_sram_record {
+    uint32_t element;              /*   0  local 1 .. 5; network 1 (D1) or 3 (D3)                                 */
+    uint32_t iteration;            /*   4 */
+    uint32_t smid;                 /*   8  the CTA whose compare failed                                           */
+    uint32_t peer_block;           /*  12  network: blockIdx.x of the owner (D1) or the writer (D3)               */
+    uint32_t round;                /*  16  the launch's round, whose CTA records resolve peer_block               */
+    uint32_t word;                 /*  20 */
+    uint64_t expected;             /*  24 */
+    uint64_t actual;               /*  32 */
+} cro_sram_record;                 /*  40 bytes */
+
+/* Test hook: the SRAM probe's classification of call `call` (seed `seed`, n_words words per CTA, `iterations` per CTA,
+ * network clusters of `cluster`) on a device of sm_count SMs, from caller-given rounds instead of launches.  legs: the
+ * CRO_SRAM_LEG_* bits that ran (0: both).  Per leg l of them: rounds[l] rounds of sm_count (local) or net_grid
+ * (network) records of ctas, and claims[l] record claims, of which the first min(claims[l], CRO_SRAM_RECORDS) are in
+ * `records`; ctas and records run in leg order.  The local fold is checked against the library's own closed form.
+ * Writes out, sms[0 .. sms_cap) and faults[0 .. cap) (*n_sms, *n, out->sms_listed, out->recorded) exactly as
+ * cro_probe_sram does, all but what needs the device: ns, wall_ns, health, before and after stay 0, and rounds is
+ * rounds[l].  Returns out->status (CRO_ERR_UNSUPPORTED with a blanked result for a %nsmid above CRO_SRAM_MAX_SMS), or
+ * CRO_ERR_INVALID_ARG for a NULL array it needs, a negative cap, sm_count 0, a network leg of grid 0 or a grid that is
+ * not whole clusters, legs outside CRO_SRAM_ALL_LEGS, a cluster other than 2, 4 or 8, or iterations 0 or above
+ * CRO_SRAM_MAX_ITERATIONS. */
+int  cro_selftest_sram_classify(uint32_t legs, uint32_t iterations, uint32_t n_words, uint64_t seed, uint32_t cluster,
+                                uint32_t sm_count, uint32_t net_grid, uint64_t call, const uint32_t *rounds,
+                                const cro_sram_cta *ctas, const uint64_t *claims, const cro_sram_record *records,
+                                cro_sram_result *out, cro_sram_sm *sms, int sms_cap, int *n_sms, cro_sram_fault *faults,
+                                int cap, int *n);
 
 /* ---- emit: encoding/json-compatible writers ------------------------------ */
 

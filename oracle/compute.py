@@ -15,12 +15,14 @@ from typing import Dict
 
 import numpy as np
 
+import sm_legs
 from oracle import go_marshal_string_map, pattern_words_np
 
 M, N, K = 128, 256, 256
 S8, SMALL = 0, 1
 LEG_NAMES = ["s8", "bf16", "e4m3", "ffma", "imad"]
 LEG_ANSWER = [S8, SMALL, SMALL, SMALL, S8]
+LEGS, RECORDS = 5, 4096
 OK, ERR_CHECKSUM = 0, -6
 NONE, SM, ALL = 0, 1, 2
 U64 = (1 << 64) - 1
@@ -128,3 +130,8 @@ def annotations(r: Dict) -> Dict[str, str]:
 
 def annotations_json(r: Dict) -> bytes:
     return go_marshal_string_map(annotations(r)).encode()
+
+
+def classify(call: Dict):
+    """The classification of a call's rounds and records (oracle/sm_legs.py): every leg computes one M x N x K tile."""
+    return sm_legs.classify(call, LEGS, [2 * M * N * K] * LEGS, RECORDS)

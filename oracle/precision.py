@@ -10,6 +10,7 @@ from typing import Dict
 
 import numpy as np
 
+import sm_legs
 from oracle import go_marshal_string_map, pattern_words_np
 
 WIDE, SMALL128, SMALL, NARROW = range(4)
@@ -18,6 +19,7 @@ BOUND = {WIDE: 1 << 45, SMALL128: 16 * 128, SMALL: 16 * 256, NARROW: 4 * 256}   
 LEG_NAMES = ["f64", "dfma", "tf32", "f16", "f16acc", "e5m2", "hfma2"]
 LEG_ANSWER = [WIDE, WIDE, SMALL128, SMALL, NARROW, SMALL, NARROW]
 LEG_BITS = [64, 64, 32, 32, 16, 32, 16]
+LEGS, RECORDS = 7, 4096
 RATE_LEGS = [(0, "f64-gflops"), (2, "tf32-gflops"), (3, "f16-gflops"), (4, "f16acc-gflops"), (5, "e5m2-gflops")]
 OK, ERR_CHECKSUM = 0, -6
 NONE, SM, ALL = 0, 1, 2
@@ -100,3 +102,9 @@ def annotations(r: Dict) -> Dict[str, str]:
 
 def annotations_json(r: Dict) -> bytes:
     return go_marshal_string_map(annotations(r)).encode()
+
+
+def classify(call: Dict):
+    """The classification of a call's rounds and records (oracle/sm_legs.py): leg l computes its answer's M x N x K."""
+    ops = [2 * SHAPE[a][0] * SHAPE[a][1] * SHAPE[a][2] for a in LEG_ANSWER]
+    return sm_legs.classify(call, LEGS, ops, RECORDS)

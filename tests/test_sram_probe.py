@@ -1,6 +1,7 @@
 """The SRAM probe (cro_probe_sram, cro_probe_sram_uuid) on one H100, against the C oracle's checksums.
 
 Faults come only from the probe's software injection (test_inject_*); nothing here repeats a call to catch a real one."""
+import collections
 import json
 
 import pytest
@@ -163,6 +164,73 @@ def test_network_write_injection_names_the_writer_and_owner(cro, ctx, clean):
     assert [(p.from_, p.owner, p.direction) for p in r.bad_pair[:r.bad_pairs]] == [(smid, o, cro.SRAM_DIR_WRITE) for o in owners]
     assert json.loads(cro.emit_sram_annotations_json(r))["cohdi.io/probe-sram-bad-pairs"] == \
         ",".join("%d-%d:w" % (smid, o) for o in owners)
+
+
+def multi_round_target(cro, ctx, cluster):
+    """A clean network call at this cluster size, and the SM that ran the most of its CTAs (at least two, so some of
+    its records come from rounds after the first)."""
+    r, sms, faults = ctx.probe_sram(0, legs=cro.SRAM_LEG_DSMEM, iterations=2, cluster=cluster)
+    assert r.status == cro.OK and not faults
+    target = max(sms, key=lambda s: (s.leg[1].ctas, -s.smid))
+    print("cluster %d: %d/%d SMs covered in %d rounds; SM %d ran %d network CTAs" % (
+        cluster, r.leg[1].sms_covered, r.sm_count, r.leg[1].rounds, target.smid, target.leg[1].ctas))
+    assert r.leg[1].rounds >= 2 and target.leg[1].ctas >= 2, "every SM ran one network CTA at this cluster size"
+    return target.smid
+
+
+def network_sms(sms):
+    return {s.smid for s in sms if s.leg[1].ctas}
+
+
+@pytest.mark.parametrize("cluster", [4, 8])
+def test_network_read_injection_over_several_rounds(cro, ctx, cluster):
+    """D1 of every network CTA on the target reads word w of each of its C - 1 peers wrong: each record names the
+    owner that the record's own round placed at peer_block."""
+    smid, w = multi_round_target(cro, ctx, cluster), 513
+    r, sms, faults = ctx.probe_sram(0, legs=cro.SRAM_LEG_DSMEM, iterations=2, cluster=cluster,
+                                    inject=(cro.SRAM_DSMEM, smid, 1, 1, w, BIT))
+    (entry,) = [s for s in sms if s.smid == smid]
+    ctas = entry.leg[1].ctas
+    print("cluster %d read injection: SM %d ran %d network CTAs in %d rounds" % (cluster, smid, ctas, r.leg[1].rounds))
+    assert ctas >= 1 and r.leg[1].unpublished == 0
+    assert r.status == cro.ERR_CHECKSUM and r.verdict == cro.SRAM_LINK and r.bad_sms == 0
+    L = r.leg[1]
+    assert list(L.mismatches) == [0, (cluster - 1) * ctas, 0, 0, 0, 0] and L.recorded == len(faults) == (cluster - 1) * ctas
+    ranks = collections.Counter()
+    for f in faults:
+        assert (f.leg, f.element, f.direction, f.smid, f.word, f.iteration) == (1, 1, cro.SRAM_DIR_READ, smid, w, 1)
+        assert f.peer_smid != smid and f.peer_smid in network_sms(sms) and f.actual == f.expected ^ BIT
+        (rank,) = [q for q in range(cluster) if pattern((r.seed + q * STRIDE) & MASK, w) == f.expected]
+        ranks[rank] += 1
+    assert max(ranks.values()) <= ctas and len(ranks) >= cluster - 1
+    owners = sorted({f.peer_smid for f in faults})
+    assert r.bad_pairs == len(owners)
+    assert [(p.from_, p.owner, p.direction) for p in r.bad_pair[:min(r.bad_pairs, cro.SRAM_MAX_PAIRS)]] == \
+        [(smid, o, cro.SRAM_DIR_READ) for o in owners][:cro.SRAM_MAX_PAIRS]
+    assert json.loads(cro.emit_sram_annotations_json(r))["cohdi.io/probe-sram-verdict"] == "link"
+
+
+@pytest.mark.parametrize("cluster", [4, 8])
+def test_network_write_injection_over_several_rounds(cro, ctx, cluster):
+    """D2 of every network CTA on the target writes word w of its next peer wrong; that peer's D3 finds it and names
+    its previous rank's SM, resolved through the record's own round, as the writer."""
+    smid, w = multi_round_target(cro, ctx, cluster), 2047
+    r, sms, faults = ctx.probe_sram(0, legs=cro.SRAM_LEG_DSMEM, iterations=2, cluster=cluster,
+                                    inject=(cro.SRAM_DSMEM, smid, 2, 0, w, BIT))
+    (entry,) = [s for s in sms if s.smid == smid]
+    ctas = entry.leg[1].ctas
+    print("cluster %d write injection: SM %d ran %d network CTAs in %d rounds" % (cluster, smid, ctas, r.leg[1].rounds))
+    assert ctas >= 1 and r.leg[1].unpublished == 0
+    assert r.status == cro.ERR_CHECKSUM and r.verdict == cro.SRAM_LINK and r.bad_sms == 0
+    assert list(r.leg[1].mismatches) == [0, 0, 0, ctas, 0, 0] and len(faults) == ctas
+    for f in faults:
+        assert (f.leg, f.element, f.direction, f.peer_smid, f.word, f.iteration) == (1, 3, cro.SRAM_DIR_WRITE, smid, w, 0)
+        assert f.smid != smid and f.smid in network_sms(sms) and f.actual == f.expected ^ BIT
+        assert any(f.expected == pattern((r.seed + q * STRIDE) & MASK, w) ^ MASK for q in range(cluster))
+    owners = sorted({f.smid for f in faults})
+    assert r.bad_pairs == len(owners)
+    assert [(p.from_, p.owner, p.direction) for p in r.bad_pair[:min(r.bad_pairs, cro.SRAM_MAX_PAIRS)]] == \
+        [(smid, o, cro.SRAM_DIR_WRITE) for o in owners][:cro.SRAM_MAX_PAIRS]
 
 
 def test_injection_into_every_sm_is_a_common_cause(cro, ctx):
