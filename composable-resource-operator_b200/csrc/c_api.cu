@@ -107,6 +107,16 @@ int on_exception() noexcept {
     }
 }
 
+// Every record-returning entry point copies its records out the same way: the first min(v.size(), cap) of v to
+// to[], their count to *n, and returns that count.
+template <class T>
+size_t copy_capped(const std::vector<T>& v, T* to, int cap, int* n) {
+    const size_t k = std::min(v.size(), (size_t)cap);
+    std::copy(v.begin(), v.begin() + k, to);
+    *n = (int)k;
+    return k;
+}
+
 // The four per-SM probes (compute, precision, SRAM, L2), in process and by UUID, share their C side: the argument
 // check (target: the context, or the GPU's UUID), opts' defaults, *n_sms and *n zeroed, then run(o, &seen, &found)
 // and sms[0 .. sms_cap) and faults[0 .. cap) copied out.  copied is false when the arguments were refused: nothing
@@ -127,12 +137,7 @@ PerSmCopy per_sm_call(const void* target, const void* out, const Opts* opts, Sm*
     std::vector<Sm> seen;
     std::vector<Fault> found;
     const int rc = run(o, &seen, &found);
-    const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
-    for (size_t j = 0; j < ks; ++j) sms[j] = seen[j];
-    for (size_t j = 0; j < kf; ++j) faults[j] = found[j];
-    *n_sms = (int)ks;
-    *n = (int)kf;
-    return {rc, true, ks, kf};
+    return {rc, true, copy_capped(seen, sms, sms_cap, n_sms), copy_capped(found, faults, cap, n)};
 }
 // The SRAM and L2 results also say how much the caller got: sms_listed and recorded.
 template <class Result>
@@ -357,11 +362,8 @@ int cro_locate_faults(cro_ctx* ctx, int i, const cro_locate_opts* opts, cro_faul
     if (opts) o = *opts;
     std::vector<cro_fault_word> found;
     const int rc = ctx_locate(ctx, i, o, out, &found);
-    const size_t k = std::min(found.size(), (size_t)cap);
-    for (size_t j = 0; j < k; ++j) words[j] = found[j];
-    out->recorded = k;
-    if (k < found.size()) out->complete = 0;        // the caller's list misses some located words
-    *n = (int)k;
+    out->recorded = copy_capped(found, words, cap, n);
+    if (out->recorded < found.size()) out->complete = 0;        // the caller's list misses some located words
     return rc;
 } CRO_API_CATCH
 int cro_probe_host_link(cro_ctx* ctx, int i, const cro_link_opts* opts, cro_link_result* out, cro_link_fault* faults, int cap,
@@ -372,9 +374,7 @@ int cro_probe_host_link(cro_ctx* ctx, int i, const cro_link_opts* opts, cro_link
     if (opts) o = *opts;
     std::vector<cro_link_fault> found;
     const int rc = ctx_probe_host_link(ctx, i, o, out, &found);
-    const size_t k = std::min(found.size(), (size_t)cap);
-    for (size_t j = 0; j < k; ++j) faults[j] = found[j];
-    *n = (int)k;
+    copy_capped(found, faults, cap, n);
     return rc;
 } CRO_API_CATCH
 int cro_probe_host_link_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_link_opts* opts, int deadline_ms, cro_link_result* out,
@@ -387,9 +387,7 @@ int cro_probe_host_link_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_link_
     std::vector<cro_link_fault> found;
     uint64_t ns = 0;
     const int rc = ctx_probe_host_link_uuid(ctx, gpu_uuid, o, deadline_ms, out, &found, cap, &ns);
-    const size_t k = std::min(found.size(), (size_t)cap);
-    for (size_t j = 0; j < k; ++j) faults[j] = found[j];
-    *n = (int)k;
+    copy_capped(found, faults, cap, n);
     if (helper_ns) *helper_ns = ns;
     return rc;
 } CRO_API_CATCH
@@ -427,15 +425,6 @@ int cro_probe_precision_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_preci
         return rc;
     }).rc;
 } CRO_API_CATCH
-// The scan's two forms share the copy-out: words[0 .. cap), recorded and complete as cro_locate_faults sets them.
-static int scan_out(int rc, const std::vector<cro_fault_word>& found, cro_scan_report* out, cro_fault_word* words, int cap, int* n) {
-    const size_t k = std::min(found.size(), (size_t)cap);
-    for (size_t j = 0; j < k; ++j) words[j] = found[j];
-    out->recorded = k;
-    if (k < found.size()) out->complete = 0;        // the caller's list misses some words
-    *n = (int)k;
-    return rc;
-}
 int cro_scan_hbm(cro_ctx* ctx, int i, const cro_scan_opts* opts, cro_scan_report* out, cro_fault_word* words, int cap, int* n) try {
     if (!ctx || !out || !n || cap < 0 || (cap > 0 && !words)) return CRO_ERR_INVALID_ARG;
     *n = 0;
@@ -443,7 +432,9 @@ int cro_scan_hbm(cro_ctx* ctx, int i, const cro_scan_opts* opts, cro_scan_report
     if (opts) o = *opts;
     std::vector<cro_fault_word> found;
     const int rc = ctx_scan_hbm(ctx, i, o, out, &found);
-    return scan_out(rc, found, out, words, cap, n);
+    out->recorded = copy_capped(found, words, cap, n);
+    if (out->recorded < found.size()) out->complete = 0;        // the caller's list misses some words
+    return rc;
 } CRO_API_CATCH
 int cro_scan_hbm_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_scan_opts* opts, cro_scan_report* out, cro_fault_word* words,
                       int cap, int* n) try {
@@ -453,9 +444,8 @@ int cro_scan_hbm_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_scan_opts* o
     if (opts) o = *opts;
     std::vector<cro_fault_word> found;
     const int rc = ctx_scan_hbm_uuid(ctx, gpu_uuid, o, out, &found, cap);
-    const uint32_t complete = out->complete;
-    scan_out(rc, found, out, words, cap, n);
-    out->complete = complete && found.size() <= (size_t)cap;
+    out->recorded = copy_capped(found, words, cap, n);
+    out->complete = out->complete && found.size() <= (size_t)cap;
     return rc;
 } CRO_API_CATCH
 int cro_read_hbm_health(const char* gpu_uuid, cro_hbm_health* out) try {
@@ -522,28 +512,24 @@ int cro_selftest_sm_legs_classify(int probe, uint32_t legs, const uint32_t* iter
     }
     if ((n_rounds && (!ctas || !sm_bits)) || (n_records && !records)) return CRO_ERR_INVALID_ARG;
     *n = *n_sms = 0;
-    auto copy_out = [&](int rc, const auto& seen, const auto& found, auto* s, auto* f) {
-        const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
-        std::copy(seen.begin(), seen.begin() + ks, s);
-        std::copy(found.begin(), found.begin() + kf, f);
-        *n_sms = (int)ks;
-        *n = (int)kf;
-        return rc;
-    };
     if (probe == CRO_SM_LEGS_COMPUTE) {
         std::vector<cro_compute_sm> seen;
         std::vector<cro_compute_fault> found;
         const int rc = classify_compute(legs, iterations, grid, call, rounds, ctas, sm_bits, claims,
                                         static_cast<const cro_compute_fault*>(records), static_cast<cro_compute_result*>(out),
                                         &seen, &found);
-        return copy_out(rc, seen, found, static_cast<cro_compute_sm*>(sms), static_cast<cro_compute_fault*>(faults));
+        copy_capped(seen, static_cast<cro_compute_sm*>(sms), sms_cap, n_sms);
+        copy_capped(found, static_cast<cro_compute_fault*>(faults), cap, n);
+        return rc;
     }
     std::vector<cro_precision_sm> seen;
     std::vector<cro_precision_fault> found;
     const int rc = classify_precision(legs, iterations, grid, call, rounds, ctas, sm_bits, claims,
                                       static_cast<const cro_precision_fault*>(records), static_cast<cro_precision_result*>(out),
                                       &seen, &found);
-    return copy_out(rc, seen, found, static_cast<cro_precision_sm*>(sms), static_cast<cro_precision_fault*>(faults));
+    copy_capped(seen, static_cast<cro_precision_sm*>(sms), sms_cap, n_sms);
+    copy_capped(found, static_cast<cro_precision_fault*>(faults), cap, n);
+    return rc;
 } CRO_API_CATCH
 int cro_selftest_sram_classify(uint32_t legs, uint32_t iterations, uint32_t n_words, uint64_t seed, uint32_t cluster,
                                uint32_t sm_count, uint32_t net_grid, uint64_t call, const uint32_t* rounds, const cro_sram_cta* ctas,
@@ -567,14 +553,7 @@ int cro_selftest_sram_classify(uint32_t legs, uint32_t iterations, uint32_t n_wo
     std::vector<cro_sram_fault> found;
     const int rc = classify_sram(legs, iterations, n_words, seed, cluster, sm_count, net_grid, call, rounds, ctas, claims, records,
                                  out, &seen, &found);
-    const size_t ks = std::min(seen.size(), (size_t)sms_cap), kf = std::min(found.size(), (size_t)cap);
-    std::copy(seen.begin(), seen.begin() + ks, sms);
-    std::copy(found.begin(), found.begin() + kf, faults);
-    *n_sms = (int)ks;
-    *n = (int)kf;
-    out->sms_listed = (uint32_t)ks;
-    out->recorded = kf;
-    return rc;
+    return listed({rc, true, copy_capped(seen, sms, sms_cap, n_sms), copy_capped(found, faults, cap, n)}, out);
 } CRO_API_CATCH
 int cro_compute_expected(int answer, uint64_t seed, int32_t* out) try {
     return compute::Expected(answer, seed, out);
@@ -746,6 +725,98 @@ int cro_emit_sunfish_request(const char* name, long long count, const char* proc
 } CRO_API_CATCH
 
 }  // extern "C" (reopened below)
+
+// ---- annotation helpers: each emitter names its own keys and builds their values from these ----
+
+using Annotations = std::map<std::string, std::string>;
+
+static int emit(const Annotations& m, char* buf, size_t cap, size_t* len) {
+    gojson::Writer w;
+    w.string_map(m);
+    return copy_out(w.str(), buf, cap, len);
+}
+// "f(0),f(1),...,f(n-1)"
+template <class F>
+static std::string join(uint64_t n, F f) {
+    std::string s;
+    for (uint64_t j = 0; j < n; ++j) s += (j ? "," : "") + f(j);
+    return s;
+}
+// The first n values of v, in decimal.
+template <class T>
+static std::string join(const T* v, uint64_t n) {
+    return join(n, [&](uint64_t j) { return std::to_string(v[j]); });
+}
+// The bit numbers b < 64 for which flipped(b) holds, comma-joined.
+template <class F>
+static std::string bit_numbers(F flipped) {
+    std::string s;
+    for (int b = 0; b < 64; ++b)
+        if (flipped(b)) s += (s.empty() ? "" : ",") + std::to_string(b);
+    return s;
+}
+// names[b] for each bit b < n set in mask, comma-joined.
+static std::string bit_names(uint32_t mask, const char* const* names, int n) {
+    std::string s;
+    for (int b = 0; b < n; ++b)
+        if (mask >> b & 1u) s += (s.empty() ? "" : ",") + std::string(names[b]);
+    return s;
+}
+// A list-valued key is written only when its list has an entry.
+static void put_list(Annotations& m, const std::string& key, const std::string& list) {
+    if (!list.empty()) m[key] = list;
+}
+// The least sms_covered over the legs run: the "sms" key's numerator, 0 when no leg ran.
+template <class Leg>
+static uint32_t min_covered(uint32_t legs, const Leg* leg, int n_legs) {
+    uint32_t covered = 0xFFFFFFFFu;
+    for (int l = 0; l < n_legs; ++l)
+        if (legs >> l & 1u) covered = std::min(covered, leg[l].sms_covered);
+    return covered == 0xFFFFFFFFu ? 0u : covered;
+}
+// How much each ECC count grew over the call, for a count NVML gave both before and after it.
+template <class Health>
+static void ecc_delta(Annotations& m, const std::string& p, const Health& B, const Health& A, uint32_t corrected_bit,
+                      uint32_t uncorrected_bit) {
+    if (B.nvml & A.nvml & corrected_bit) m[p + "ecc-corrected"] = std::to_string(A.ecc_corrected - B.ecc_corrected);
+    if (B.nvml & A.nvml & uncorrected_bit) m[p + "ecc-uncorrected"] = std::to_string(A.ecc_uncorrected - B.ecc_uncorrected);
+}
+static std::string cuda_error(int32_t e) { return "cuda-error:" + std::to_string(e); }
+
+// The compute and precision results both hold a cro_compute_leg per leg.  Their annotations differ only in the key
+// prefix p, the leg names and which legs report a rate under which key.
+struct LegRate {
+    int leg;
+    const char* key;
+};
+template <class Result>
+static int emit_sm_legs(const Result& r, const std::string& p, const char* const* leg_name, int n_legs,
+                        std::initializer_list<LegRate> rates, char* buf, size_t cap, size_t* len) {
+    Annotations m;
+    m[p + "verdict"] = r.status == CRO_OK                                               ? "ok"
+                       : r.status == CRO_ERR_CHECKSUM && r.verdict == CRO_COMPUTE_SM  ? "sm"
+                       : r.status == CRO_ERR_CHECKSUM && r.verdict == CRO_COMPUTE_ALL ? "all"
+                                                                                      : "error";
+    m[p + "sms"] = std::to_string(min_covered(r.legs, r.leg, n_legs)) + "/" + std::to_string(r.sm_count);
+    if (r.bad_sms) m[p + "bad-sms"] = join(r.bad_sm, std::min<uint32_t>(r.bad_sms, 16));
+    uint32_t failed = 0;
+    int worst = n_legs;     // the first leg with the largest slow_permille
+    for (int l = 0; l < n_legs; ++l) {
+        if (!(r.legs >> l & 1u)) continue;
+        const cro_compute_leg& L = r.leg[l];
+        if (L.mismatches || L.fold_mismatches || L.unpublished) failed |= 1u << l;
+        if (worst == n_legs || L.slow_permille > r.leg[worst].slow_permille) worst = l;
+    }
+    put_list(m, p + "failed-legs", bit_names(failed, leg_name, n_legs));
+    for (const LegRate& q : rates) {
+        const cro_compute_leg& L = r.leg[q.leg];
+        m[p + q.key] = std::to_string(L.ns ? L.ops / L.ns : 0ull);
+    }
+    if (worst < n_legs)
+        m[p + "slowest-sm"] = std::to_string(r.leg[worst].slowest_sm) + " " + std::to_string(r.leg[worst].slow_permille);
+    return emit(m, buf, cap, len);
+}
+
 std::map<std::string, std::string> cro::capi::probe_annotations(const cro_probe_result& r) {
     std::map<std::string, std::string> m;
     m["cohdi.io/probe-status"] = cro_strerror(r.status);
@@ -785,38 +856,27 @@ extern "C" {
 
 int cro_emit_probe_annotations_json(const cro_probe_result* r, char* buf, size_t cap, size_t* len) try {
     if (!r) return CRO_ERR_INVALID_ARG;
-    gojson::Writer w;
-    w.string_map(probe_annotations(*r));
-    return copy_out(w.str(), buf, cap, len);
+    return emit(probe_annotations(*r), buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_fault_annotations_json(const cro_fault_report* r, const cro_fault_word* words, int n, char* buf, size_t cap,
                                     size_t* len) try {
     if (!r || n < 0 || (n > 0 && !words)) return CRO_ERR_INVALID_ARG;
     static const char* const kVerdict[] = {"none", "unclassified", "not-reproduced", "persistent"};
-    std::map<std::string, std::string> m;
+    Annotations m;
     m["cohdi.io/probe-fault-verdict"] = kVerdict[fault_verdict(*r)];
-    std::string mism, gran, bits, ws;
     const uint32_t np = std::min<uint32_t>(r->n_passes, CRO_LOCATE_PASSES);
-    for (uint32_t p = 0; p < np; ++p) {
-        const std::string sep = p ? "," : "";
-        mism += sep + std::to_string(p) + ":" + std::to_string(r->pass[p].mismatches);
-        gran += sep + std::to_string(p) + ":" + std::to_string(r->pass[p].granules);
-    }
-    m["cohdi.io/probe-fault-mismatches"] = mism;
-    m["cohdi.io/probe-fault-granules"] = gran;
-    for (int b = 0; b < 64; ++b)
-        if (r->bit_flips[b]) bits += (bits.empty() ? "" : ",") + std::to_string(b);
-    if (!bits.empty()) m["cohdi.io/probe-fault-bits"] = bits;
-    for (int k = 0; k < n && k < 8; ++k) {
-        char idx[24];
-        snprintf(idx, sizeof idx, "%llx", (unsigned long long)words[k].word_index);
-        ws += (k ? "," : "") + std::string(idx) + ":" + hex16(words[k].expected ^ words[k].actual);
-    }
-    if (!ws.empty()) m["cohdi.io/probe-fault-words"] = ws;
-    gojson::Writer w;
-    w.string_map(m);
-    return copy_out(w.str(), buf, cap, len);
+    m["cohdi.io/probe-fault-mismatches"] =
+        join(np, [&](uint64_t p) { return std::to_string(p) + ":" + std::to_string(r->pass[p].mismatches); });
+    m["cohdi.io/probe-fault-granules"] =
+        join(np, [&](uint64_t p) { return std::to_string(p) + ":" + std::to_string(r->pass[p].granules); });
+    put_list(m, "cohdi.io/probe-fault-bits", bit_numbers([&](int b) { return r->bit_flips[b] != 0; }));
+    put_list(m, "cohdi.io/probe-fault-words", join(std::min(n, 8), [&](uint64_t k) {
+                 char idx[24];
+                 snprintf(idx, sizeof idx, "%llx", (unsigned long long)words[k].word_index);
+                 return std::string(idx) + ":" + hex16(words[k].expected ^ words[k].actual);
+             }));
+    return emit(m, buf, cap, len);
 } CRO_API_CATCH
 
 static std::string link_speed(uint32_t tenths) {
@@ -833,7 +893,7 @@ int cro_emit_link_annotations_json(const cro_link_result* r, char* buf, size_t c
     static const char* const kCheck[CRO_LINK_CHECKS] = {"d2h-copy", "h2d-copy", "sm-write", "duplex-write", "duplex-d2h-copy",
                                                          "chase"};
     static const char* const kDegraded[4] = {"speed", "width", "path", "bottleneck"};
-    std::map<std::string, std::string> m;
+    Annotations m;
     const std::string p = "cohdi.io/probe-link-";
     m[p + "verdict"] = r->first_fail < CRO_LINK_CHECKS ? std::string("corrupt:") + kCheck[r->first_fail]
                        : r->status == CRO_OK       ? "ok"
@@ -853,99 +913,37 @@ int cro_emit_link_annotations_json(const cro_link_result* r, char* buf, size_t c
         m[p + "bottleneck"] = std::string(b.bdf, strnlen(b.bdf, sizeof b.bdf)) + " " + link_speed(b.cur_speed) + " x" +
                               std::to_string(b.cur_width);
     }
-    std::string deg;
-    for (int b = 0; b < 4; ++b)
-        if (r->degraded >> b & 1u) deg += (deg.empty() ? "" : ",") + std::string(kDegraded[b]);
-    if (!deg.empty()) m[p + "degraded"] = deg;
+    put_list(m, p + "degraded", bit_names(r->degraded, kDegraded, 4));
     if (!r->no_nvml) m[p + "replays"] = std::to_string(r->replays_after - r->replays_before);
-    gojson::Writer w;
-    w.string_map(m);
-    return copy_out(w.str(), buf, cap, len);
+    return emit(m, buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_compute_annotations_json(const cro_compute_result* r, char* buf, size_t cap, size_t* len) try {
-    if (!r) return CRO_ERR_INVALID_ARG;
     static const char* const kLeg[CRO_COMPUTE_LEGS] = {"s8", "bf16", "e4m3", "ffma", "imad"};
-    std::map<std::string, std::string> m;
-    const std::string p = "cohdi.io/probe-compute-";
-    m[p + "verdict"] = r->status == CRO_OK                                                ? "ok"
-                       : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_COMPUTE_SM  ? "sm"
-                       : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_COMPUTE_ALL ? "all"
-                                                                                        : "error";
-    uint32_t covered = 0xFFFFFFFFu, worst = CRO_COMPUTE_LEGS;
-    std::string failed;
-    for (int l = 0; l < CRO_COMPUTE_LEGS; ++l) {
-        if (!(r->legs >> l & 1u)) continue;
-        const cro_compute_leg& L = r->leg[l];
-        covered = std::min(covered, L.sms_covered);
-        if (L.mismatches || L.fold_mismatches || L.unpublished) failed += (failed.empty() ? "" : ",") + std::string(kLeg[l]);
-        if (worst == CRO_COMPUTE_LEGS || L.slow_permille > r->leg[worst].slow_permille) worst = (uint32_t)l;
-    }
-    m[p + "sms"] = std::to_string(covered == 0xFFFFFFFFu ? 0u : covered) + "/" + std::to_string(r->sm_count);
-    if (r->bad_sms) {
-        std::string ids;
-        for (uint32_t j = 0; j < std::min<uint32_t>(r->bad_sms, 16); ++j) ids += (j ? "," : "") + std::to_string(r->bad_sm[j]);
-        m[p + "bad-sms"] = ids;
-    }
-    if (!failed.empty()) m[p + "failed-legs"] = failed;
-    auto rate = [&](int l) {
-        const cro_compute_leg& L = r->leg[l];
-        return std::to_string(L.ns ? L.ops / L.ns : 0ull);
-    };
-    m[p + "s8-gops"] = rate(CRO_COMPUTE_LEG_S8);
-    m[p + "bf16-gflops"] = rate(CRO_COMPUTE_LEG_BF16);
-    m[p + "e4m3-gflops"] = rate(CRO_COMPUTE_LEG_E4M3);
-    if (worst < CRO_COMPUTE_LEGS)
-        m[p + "slowest-sm"] = std::to_string(r->leg[worst].slowest_sm) + " " + std::to_string(r->leg[worst].slow_permille);
-    gojson::Writer w;
-    w.string_map(m);
-    return copy_out(w.str(), buf, cap, len);
+    if (!r) return CRO_ERR_INVALID_ARG;
+    return emit_sm_legs(*r, "cohdi.io/probe-compute-", kLeg, CRO_COMPUTE_LEGS,
+                        {{CRO_COMPUTE_LEG_S8, "s8-gops"}, {CRO_COMPUTE_LEG_BF16, "bf16-gflops"}, {CRO_COMPUTE_LEG_E4M3, "e4m3-gflops"}},
+                        buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_precision_annotations_json(const cro_precision_result* r, char* buf, size_t cap, size_t* len) try {
-    if (!r) return CRO_ERR_INVALID_ARG;
     static const char* const kLeg[CRO_PRECISION_LEGS] = {"f64", "dfma", "tf32", "f16", "f16acc", "e5m2", "hfma2"};
-    std::map<std::string, std::string> m;
-    const std::string p = "cohdi.io/probe-precision-";
-    m[p + "verdict"] = r->status == CRO_OK                                                ? "ok"
-                       : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_COMPUTE_SM  ? "sm"
-                       : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_COMPUTE_ALL ? "all"
-                                                                                        : "error";
-    uint32_t covered = 0xFFFFFFFFu, worst = CRO_PRECISION_LEGS;
-    std::string failed;
-    for (int l = 0; l < CRO_PRECISION_LEGS; ++l) {
-        if (!(r->legs >> l & 1u)) continue;
-        const cro_compute_leg& L = r->leg[l];
-        covered = std::min(covered, L.sms_covered);
-        if (L.mismatches || L.fold_mismatches || L.unpublished) failed += (failed.empty() ? "" : ",") + std::string(kLeg[l]);
-        if (worst == CRO_PRECISION_LEGS || L.slow_permille > r->leg[worst].slow_permille) worst = (uint32_t)l;
-    }
-    m[p + "sms"] = std::to_string(covered == 0xFFFFFFFFu ? 0u : covered) + "/" + std::to_string(r->sm_count);
-    if (r->bad_sms) {
-        std::string ids;
-        for (uint32_t j = 0; j < std::min<uint32_t>(r->bad_sms, 16); ++j) ids += (j ? "," : "") + std::to_string(r->bad_sm[j]);
-        m[p + "bad-sms"] = ids;
-    }
-    if (!failed.empty()) m[p + "failed-legs"] = failed;
-    for (int l : {CRO_PRECISION_LEG_F64, CRO_PRECISION_LEG_TF32, CRO_PRECISION_LEG_F16, CRO_PRECISION_LEG_F16ACC, CRO_PRECISION_LEG_E5M2}) {
-        const cro_compute_leg& L = r->leg[l];
-        m[p + kLeg[l] + "-gflops"] = std::to_string(L.ns ? L.ops / L.ns : 0ull);
-    }
-    if (worst < CRO_PRECISION_LEGS)
-        m[p + "slowest-sm"] = std::to_string(r->leg[worst].slowest_sm) + " " + std::to_string(r->leg[worst].slow_permille);
-    gojson::Writer w;
-    w.string_map(m);
-    return copy_out(w.str(), buf, cap, len);
+    if (!r) return CRO_ERR_INVALID_ARG;
+    return emit_sm_legs(*r, "cohdi.io/probe-precision-", kLeg, CRO_PRECISION_LEGS,
+                        {{CRO_PRECISION_LEG_F64, "f64-gflops"}, {CRO_PRECISION_LEG_TF32, "tf32-gflops"},
+                         {CRO_PRECISION_LEG_F16, "f16-gflops"}, {CRO_PRECISION_LEG_F16ACC, "f16acc-gflops"},
+                         {CRO_PRECISION_LEG_E5M2, "e5m2-gflops"}},
+                        buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_scan_annotations_json(const cro_scan_report* r, char* buf, size_t cap, size_t* len) try {
     if (!r) return CRO_ERR_INVALID_ARG;
     static const char* const kHealth[4] = {"ecc-corrected", "ecc-uncorrected", "remap-pending", "remap-failure"};
-    std::map<std::string, std::string> m;
+    Annotations m;
     const std::string p = "cohdi.io/hbm-scan-";
     m[p + "verdict"] = r->status == CRO_OK            ? "ok"
                        : r->status == CRO_ERR_CHECKSUM ? "corrupt"
-                       : r->status == CRO_ERR_CUDA     ? "cuda-error:" + std::to_string(r->cuda_error)
+                       : r->status == CRO_ERR_CUDA     ? cuda_error(r->cuda_error)
                                                        : "error";
     m[p + "covered-bytes"] = std::to_string(r->covered_bytes);
     m[p + "free-bytes"] = std::to_string(r->free_bytes);
@@ -955,67 +953,37 @@ int cro_emit_scan_annotations_json(const cro_scan_report* r, char* buf, size_t c
     uint64_t ns = 0;
     for (uint64_t e : r->element_ns) ns += e;
     m[p + "gbs"] = std::to_string(ns ? (uint64_t)((unsigned __int128)r->covered_bytes * 4u / ns) : 0ull);
-    std::string bits, health;
-    for (int b = 0; b < 64; ++b)
-        if (r->pass[0].bit_flips[b] || r->pass[1].bit_flips[b]) bits += (bits.empty() ? "" : ",") + std::to_string(b);
-    if (!bits.empty()) m[p + "bits"] = bits;
-    for (int b = 0; b < 4; ++b)
-        if (r->health >> b & 1u) health += (health.empty() ? "" : ",") + std::string(kHealth[b]);
-    if (!health.empty()) m[p + "health"] = health;
-    const cro_hbm_health &B = r->before, &A = r->after;
-    if (B.nvml & A.nvml & CRO_HBM_NVML_ECC_CORRECTED) m[p + "ecc-corrected"] = std::to_string(A.ecc_corrected - B.ecc_corrected);
-    if (B.nvml & A.nvml & CRO_HBM_NVML_ECC_UNCORRECTED) m[p + "ecc-uncorrected"] = std::to_string(A.ecc_uncorrected - B.ecc_uncorrected);
+    put_list(m, p + "bits", bit_numbers([&](int b) { return r->pass[0].bit_flips[b] || r->pass[1].bit_flips[b]; }));
+    put_list(m, p + "health", bit_names(r->health, kHealth, 4));
+    const cro_hbm_health& A = r->after;
+    ecc_delta(m, p, r->before, A, CRO_HBM_NVML_ECC_CORRECTED, CRO_HBM_NVML_ECC_UNCORRECTED);
     if (A.nvml & CRO_HBM_NVML_REMAP) m[p + "remapped"] = std::to_string(A.remap_corrected) + "," + std::to_string(A.remap_uncorrected);
-    if (A.nvml & CRO_HBM_NVML_HISTOGRAM) {
-        std::string h;
-        for (int b = 0; b < 5; ++b) h += (b ? "," : "") + std::to_string(A.histogram[b]);
-        m[p + "remap-histogram"] = h;
-    }
-    gojson::Writer w;
-    w.string_map(m);
-    return copy_out(w.str(), buf, cap, len);
+    if (A.nvml & CRO_HBM_NVML_HISTOGRAM) m[p + "remap-histogram"] = join(A.histogram, 5);
+    return emit(m, buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_sram_annotations_json(const cro_sram_result* r, char* buf, size_t cap, size_t* len) try {
     if (!r) return CRO_ERR_INVALID_ARG;
     static const char* const kHealth[3] = {"corrected", "uncorrected", "threshold-exceeded"};
-    std::map<std::string, std::string> m;
+    Annotations m;
     const std::string p = "cohdi.io/probe-sram-";
     m[p + "verdict"] = r->status == CRO_OK                                                ? "ok"
                        : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_SRAM_SM   ? "sm"
                        : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_SRAM_LINK ? "link"
                        : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_SRAM_ALL  ? "all"
-                       : r->status == CRO_ERR_CUDA ? "cuda-error:" + std::to_string(r->cuda_error)
+                       : r->status == CRO_ERR_CUDA ? cuda_error(r->cuda_error)
                                                    : "error";
-    uint32_t covered = 0xFFFFFFFFu;
-    for (int l = 0; l < CRO_SRAM_LEGS; ++l)
-        if (r->legs >> l & 1u) covered = std::min(covered, r->leg[l].sms_covered);
-    m[p + "sms"] = std::to_string(covered == 0xFFFFFFFFu ? 0u : covered) + "/" + std::to_string(r->sm_count);
-    if (r->bad_sms) {
-        std::string ids;
-        for (uint32_t j = 0; j < std::min<uint32_t>(r->bad_sms, 16); ++j) ids += (j ? "," : "") + std::to_string(r->bad_sm[j]);
-        m[p + "bad-sms"] = ids;
-    }
-    if (r->bad_pairs) {
-        std::string ps;
-        for (uint32_t j = 0; j < std::min<uint32_t>(r->bad_pairs, CRO_SRAM_MAX_PAIRS); ++j) {
+    m[p + "sms"] = std::to_string(min_covered(r->legs, r->leg, CRO_SRAM_LEGS)) + "/" + std::to_string(r->sm_count);
+    if (r->bad_sms) m[p + "bad-sms"] = join(r->bad_sm, std::min<uint32_t>(r->bad_sms, 16));
+    if (r->bad_pairs)
+        m[p + "bad-pairs"] = join(std::min<uint32_t>(r->bad_pairs, CRO_SRAM_MAX_PAIRS), [&](uint64_t j) {
             const cro_sram_pair& q = r->bad_pair[j];
-            ps += (j ? "," : "") + std::to_string(q.from) + "-" + std::to_string(q.owner) +
-                  (q.direction == CRO_SRAM_DIR_READ ? ":r" : ":w");
-        }
-        m[p + "bad-pairs"] = ps;
-    }
+            return std::to_string(q.from) + "-" + std::to_string(q.owner) + (q.direction == CRO_SRAM_DIR_READ ? ":r" : ":w");
+        });
     m[p + "bytes-per-sm"] = std::to_string(r->bytes_per_sm);
-    std::string health;
-    for (int b = 0; b < 3; ++b)
-        if (r->health >> b & 1u) health += (health.empty() ? "" : ",") + std::string(kHealth[b]);
-    if (!health.empty()) m[p + "health"] = health;
-    const cro_sram_health &B = r->before, &A = r->after;
-    if (B.nvml & A.nvml & CRO_SRAM_NVML_ECC_CORRECTED) m[p + "ecc-corrected"] = std::to_string(A.ecc_corrected - B.ecc_corrected);
-    if (B.nvml & A.nvml & CRO_SRAM_NVML_ECC_UNCORRECTED) m[p + "ecc-uncorrected"] = std::to_string(A.ecc_uncorrected - B.ecc_uncorrected);
-    gojson::Writer w;
-    w.string_map(m);
-    return copy_out(w.str(), buf, cap, len);
+    put_list(m, p + "health", bit_names(r->health, kHealth, 3));
+    ecc_delta(m, p, r->before, r->after, CRO_SRAM_NVML_ECC_CORRECTED, CRO_SRAM_NVML_ECC_UNCORRECTED);
+    return emit(m, buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_l2_annotations_json(const cro_l2_result* r, char* buf, size_t cap, size_t* len) try {
@@ -1023,34 +991,24 @@ int cro_emit_l2_annotations_json(const cro_l2_result* r, char* buf, size_t cap, 
     static const char* const kHealth[6] = {"sram-corrected", "sram-uncorrected", "l2-corrected", "l2-uncorrected",
                                            "threshold-exceeded", "l2-bucket"};
     static const char* const kVerdict[5] = {"", "sm", "line", "atomic", "all"};
-    std::map<std::string, std::string> m;
+    Annotations m;
     const std::string p = "cohdi.io/probe-l2-";
     m[p + "verdict"] = r->status == CRO_OK                                                           ? "ok"
                        : r->status == CRO_ERR_CHECKSUM && r->verdict >= 1 && r->verdict <= CRO_L2_ALL ? kVerdict[r->verdict]
-                       : r->status == CRO_ERR_CUDA ? "cuda-error:" + std::to_string(r->cuda_error)
+                       : r->status == CRO_ERR_CUDA ? cuda_error(r->cuda_error)
                                                    : "error";
     m[p + "sms"] = std::to_string(r->sms_covered) + "/" + std::to_string(r->sm_count);
     m[p + "bytes"] = std::to_string(r->bytes);
     m[p + "iterations"] = std::to_string(r->iterations);
     m[p + "march-gbs"] = std::to_string(r->march_ns ? r->march_bytes / r->march_ns : 0ull);
-    auto list = [](const auto* v, uint64_t n) {
-        std::string s;
-        for (uint64_t j = 0; j < n; ++j) s += (j ? "," : "") + std::to_string(v[j]);
-        return s;
-    };
-    if (r->bad_sms) m[p + "bad-sms"] = list(r->bad_sm, std::min<uint64_t>(r->bad_sms, 16));
-    if (r->bad_lines) m[p + "bad-lines"] = list(r->bad_line, std::min<uint64_t>(r->bad_lines, CRO_L2_MAX_LINES));
-    if (r->a1_bad) m[p + "a1-bad-counters"] = list(r->a1_bad_counter, std::min<uint64_t>(r->a1_bad, CRO_L2_MAX_COUNTERS));
-    if (r->a2_bad) m[p + "a2-bad-counters"] = list(r->a2_bad_counter, std::min<uint64_t>(r->a2_bad, CRO_L2_MAX_COUNTERS));
+    if (r->bad_sms) m[p + "bad-sms"] = join(r->bad_sm, std::min<uint64_t>(r->bad_sms, 16));
+    if (r->bad_lines) m[p + "bad-lines"] = join(r->bad_line, std::min<uint64_t>(r->bad_lines, CRO_L2_MAX_LINES));
+    if (r->a1_bad) m[p + "a1-bad-counters"] = join(r->a1_bad_counter, std::min<uint64_t>(r->a1_bad, CRO_L2_MAX_COUNTERS));
+    if (r->a2_bad) m[p + "a2-bad-counters"] = join(r->a2_bad_counter, std::min<uint64_t>(r->a2_bad, CRO_L2_MAX_COUNTERS));
     if (r->a2_holes) m[p + "a2-holes"] = std::to_string(r->a2_holes);
     if (r->overflow) m[p + "overflow"] = "1";
-    std::string health;
-    for (int b = 0; b < 6; ++b)
-        if (r->health >> b & 1u) health += (health.empty() ? "" : ",") + std::string(kHealth[b]);
-    if (!health.empty()) m[p + "health"] = health;
-    gojson::Writer w;
-    w.string_map(m);
-    return copy_out(w.str(), buf, cap, len);
+    put_list(m, p + "health", bit_names(r->health, kHealth, 6));
+    return emit(m, buf, cap, len);
 } CRO_API_CATCH
 
 int cro_fm_parse_scale_up_response(const char* body, const char* resource_name, const char* res_type,
