@@ -645,7 +645,31 @@ EXPORTS = [
     "cro_probe_sram", "cro_probe_sram_uuid", "cro_read_sram_health", "cro_emit_sram_annotations_json",
     "cro_probe_l2", "cro_probe_l2_uuid", "cro_read_l2_health", "cro_emit_l2_annotations_json", "cro_selftest_l2_classify",
     "cro_selftest_sm_legs_classify", "cro_selftest_sram_classify",
+    "cro_selftest_locate_collect", "cro_selftest_scan_collect", "cro_selftest_link_classify",
 ]
+
+# test hooks: the word checks' reports from caller-given device output
+# (cro_selftest_locate_collect, cro_selftest_scan_collect, cro_selftest_link_classify)
+class LocateCounters(ctypes.Structure):
+    """cro_locate_counters: a word-checking kernel's exact counts of one pass or check."""
+    _fields_ = [("mismatches", ctypes.c_uint64), ("claims", ctypes.c_uint64), ("bits", ctypes.c_uint64 * 64)]
+
+
+class LocateRecord(ctypes.Structure):
+    """cro_locate_record: one word a word-checking kernel recorded."""
+    _fields_ = [("word", ctypes.c_uint64), ("expected", ctypes.c_uint64), ("actual", ctypes.c_uint64)]
+
+
+class SweepSlot(ctypes.Structure):
+    """cro_sweep_slot: one sweep's result slot as the kernels write it."""
+    _fields_ = [("x", ctypes.c_uint64), ("s", ctypes.c_uint64), ("w", ctypes.c_uint64), ("t0", ctypes.c_uint64),
+                ("t1", ctypes.c_uint64), ("stamp", ctypes.c_uint64), ("n_words", ctypes.c_uint64), ("pad", ctypes.c_uint64)]
+
+
+LINK_SLOTS = LINK_WORD_CHECKS + 5             # [k] check k's fold, two write roles, the closed forms of P1, P2, P3
+SCAN_SLOTS = SCAN_PASSES * SCAN_MAX_CHUNKS + SCAN_MAX_CHUNKS
+LOCATE_SLOTS = 3 * LOCATE_PASSES
+assert ctypes.sizeof(LocateCounters) == 528 and ctypes.sizeof(LocateRecord) == 24 and ctypes.sizeof(SweepSlot) == 64
 
 # Slot map of a device's sweep-slot array (cro_sweep_slot, 64 bytes each); the cro_selftest_* hooks take such arrays.
 SLOT_FILL, SLOT_SWEEP0, MAX_SWEEPS_EACH, SLOT_EXPECT, SLOT_PREFIX, SLOT_P2P0 = 0, 1, 30, 62, 63, 64
@@ -784,6 +808,16 @@ def _load() -> ctypes.CDLL:
                                              ctypes.POINTER(SramCta), ctypes.POINTER(u64), ctypes.POINTER(SramRecord),
                                              ctypes.POINTER(SramResult), ctypes.POINTER(SramSm), i32, ctypes.POINTER(i32),
                                              ctypes.POINTER(SramFault), i32, ctypes.POINTER(i32)]),
+        "cro_selftest_locate_collect": (i32, [u64, ctypes.POINTER(LocatePass), u32, ctypes.POINTER(LocateCounters),
+                                              ctypes.POINTER(LocateRecord), ctypes.POINTER(u64), u64, ctypes.POINTER(SweepSlot),
+                                              ctypes.POINTER(FaultReport), ctypes.POINTER(FaultWord), i32, ctypes.POINTER(i32)]),
+        "cro_selftest_scan_collect": (i32, [i32, ctypes.POINTER(LocateCounters), ctypes.POINTER(LocateRecord),
+                                            ctypes.POINTER(u64), u64, ctypes.POINTER(SweepSlot), ctypes.POINTER(ScanReport),
+                                            ctypes.POINTER(FaultWord), i32, ctypes.POINTER(i32)]),
+        "cro_selftest_link_classify": (i32, [u64, ctypes.POINTER(u64), u32, u32, ctypes.POINTER(LocateCounters),
+                                             ctypes.POINTER(LocateRecord), ctypes.POINTER(u64), ctypes.POINTER(SweepSlot),
+                                             ctypes.POINTER(u64), ctypes.POINTER(LinkResult), ctypes.POINTER(LinkFault), i32,
+                                             ctypes.POINTER(i32)]),
         "cro_local_node_op": (i32, [vp, c] + out),
         "cro_local_exec": (i32, [c] + out),
         "cro_describe_wire_type": (i32, [c] + out),
@@ -1055,6 +1089,69 @@ def selftest_sram_classify(iterations: int, n_words: int, seed: int, cluster: in
     if rc not in (OK, ERR_CHECKSUM, ERR_UNSUPPORTED):
         raise ProbeError(rc, "cro_selftest_sram_classify")
     return out
+
+
+def _word_checks(counters: List[LocateCounters], records, granules=None):
+    """The flat arrays of the word-check hooks: counters, records[k] (the first min(claims, LOCATE_RECORDS) of each) in
+    order, and granules[k] (each the same number of words) in order."""
+    recs = [x for r in records for x in r]
+    assert [len(r) for r in records] == [min(c.claims, LOCATE_RECORDS) for c in counters]
+    gw = len(granules[0]) if granules else 0
+    bits = [b for g in granules or [] for b in g]
+    assert len(bits) == gw * len(counters)
+    return ((LocateCounters * len(counters))(*counters), (LocateRecord * max(1, len(recs)))(*recs),
+            (ctypes.c_uint64 * max(1, len(bits)))(*bits), gw)
+
+
+def selftest_locate_collect(sweep_bytes: int, passes: List[LocatePass], counters: List[LocateCounters], records,
+                            granules, slots: List[SweepSlot], cap: Optional[int] = None):
+    """cro_selftest_locate_collect: the fault locator's report of len(passes) passes over a region of sweep_bytes, from
+    pass p's counters[p], records[p] and granule words granules[p], and the LOCATE_SLOTS slots.  Returns (report,
+    words); cap defaults to every located word."""
+    ctr, recs, gran, gw = _word_checks(counters, records, granules)
+    cap = sum(len(r) for r in records) if cap is None else cap
+    out, words, n = FaultReport(), (FaultWord * max(1, cap))(), ctypes.c_int()
+    rc = lib.cro_selftest_locate_collect(sweep_bytes, (LocatePass * len(passes))(*passes), len(passes), ctr, recs, gran, gw,
+                                         (SweepSlot * LOCATE_SLOTS)(*slots), ctypes.byref(out), words, cap, ctypes.byref(n))
+    if rc not in (OK, ERR_CHECKSUM):
+        raise ProbeError(rc, "cro_selftest_locate_collect")
+    return out, list(words[:n.value])
+
+
+def selftest_scan_collect(chunks: List[Tuple[int, int]], elements_done: int, cuda_error: int, counters: List[LocateCounters],
+                          records, granules, slots: List[SweepSlot], cap: Optional[int] = None):
+    """cro_selftest_scan_collect: the scan's report over chunks [(word0, bytes)] after elements_done elements (and the
+    CUDA error that stopped them, 0: none), from pass p's counters[p], records[p] and granule words granules[p], and
+    the SCAN_SLOTS slots.  Returns (report, words); cap defaults to every recorded word."""
+    ctr, recs, gran, gw = _word_checks(counters, records, granules)
+    cap = sum(len(r) for r in records) if cap is None else cap
+    out, words, n = ScanReport(), (FaultWord * max(1, cap))(), ctypes.c_int()
+    out.n_chunks, out.elements_done = len(chunks), elements_done
+    for k, (word0, nbytes) in enumerate(chunks):
+        out.chunk[k].word0, out.chunk[k].bytes = word0, nbytes
+    rc = lib.cro_selftest_scan_collect(cuda_error, ctr, recs, gran, gw, (SweepSlot * SCAN_SLOTS)(*slots), ctypes.byref(out),
+                                       words, cap, ctypes.byref(n))
+    if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
+        raise ProbeError(rc, "cro_selftest_scan_collect")
+    return out, list(words[:n.value])
+
+
+def selftest_link_classify(bytes: int, seeds: List[int], minor: int, hops: int, counters: List[LocateCounters], records,
+                           host: List[List[int]], slots: List[SweepSlot], chase_out: List[int], cap: Optional[int] = None):
+    """cro_selftest_link_classify: the host link probe's word checks and chase of a call of L = bytes, from check k's
+    counters[k], records[k] and host buffer host[k] (L / 8 words as the CPU read them), the LINK_SLOTS slots and the
+    chase output (end slot, ns).  Returns (result, faults); cap defaults to every recorded fault."""
+    ctr, recs, _, _ = _word_checks(counters, records)
+    assert all(len(h) == bytes // 8 for h in host) and len(host) == LINK_WORD_CHECKS
+    cap = sum(len(r) for r in records) if cap is None else cap
+    out, faults, n = LinkResult(), (LinkFault * max(1, cap))(), ctypes.c_int()
+    hw = (ctypes.c_uint64 * (LINK_WORD_CHECKS * (bytes // 8)))(*[w for h in host for w in h])
+    rc = lib.cro_selftest_link_classify(bytes, (ctypes.c_uint64 * 3)(*seeds), minor, hops, ctr, recs, hw,
+                                        (SweepSlot * LINK_SLOTS)(*slots), (ctypes.c_uint64 * 2)(*chase_out), ctypes.byref(out),
+                                        faults, cap, ctypes.byref(n))
+    if rc not in (OK, ERR_CHECKSUM):
+        raise ProbeError(rc, "cro_selftest_link_classify")
+    return out, list(faults[:n.value])
 
 
 def _sram_opts(legs: int, iterations: int, cluster: int, max_rounds: int, deadline_ms: int,

@@ -83,6 +83,12 @@ static_assert(sizeof(cro_l2_opts) == 56 && sizeof(cro_l2_health) == 48 && sizeof
                   offsetof(cro_l2_result, bad_line) == 184 && offsetof(cro_l2_result, a1_bad) == 312 &&
                   offsetof(cro_l2_result, element_ns) == 400 && offsetof(cro_l2_result, before) == 520,
               "l2 layout");
+static_assert(sizeof(cro_locate_counters) == sizeof(LocateCounters) && offsetof(cro_locate_counters, claims) == offsetof(LocateCounters, claims) &&
+                  offsetof(cro_locate_counters, bits) == offsetof(LocateCounters, bits) && sizeof(cro_locate_counters) == 528,
+              "cro_locate_counters is the word checks' LocateCounters");
+static_assert(sizeof(cro_locate_record) == sizeof(LocateRecord) && offsetof(cro_locate_record, expected) == offsetof(LocateRecord, expected) &&
+                  offsetof(cro_locate_record, actual) == offsetof(LocateRecord, actual) && sizeof(cro_locate_record) == 24,
+              "cro_locate_record is the word checks' LocateRecord");
 static_assert(sizeof(cro_selftest_sweep_opts) == 128 && offsetof(cro_selftest_sweep_opts, force_or) == 104 &&
                   sizeof(cro_selftest_sweep_out) == 168 && offsetof(cro_selftest_sweep_out, mismatches) == 128,
               "selftest sweep layout");
@@ -554,6 +560,61 @@ int cro_selftest_sram_classify(uint32_t legs, uint32_t iterations, uint32_t n_wo
     const int rc = classify_sram(legs, iterations, n_words, seed, cluster, sm_count, net_grid, call, rounds, ctas, claims, records,
                                  out, &seen, &found);
     return listed({rc, true, copy_capped(seen, sms, sms_cap, n_sms), copy_capped(found, faults, cap, n)}, out);
+} CRO_API_CATCH
+// The word checks' records before min(claims, CRO_LOCATE_RECORDS) of each of k counters.
+static uint64_t records_of(const cro_locate_counters* ctr, int k) {
+    uint64_t n = 0;
+    for (int i = 0; i < k; ++i) n += std::min<uint64_t>(ctr[i].claims, CRO_LOCATE_RECORDS);
+    return n;
+}
+static constexpr uint64_t kMaxGranuleWords = (1ull << 37) * 8 / CRO_LOCATE_GRANULE_BYTES / 64;   // 2^37 words
+int cro_selftest_locate_collect(uint64_t sweep_bytes, const cro_locate_pass* passes, uint32_t n_passes, const cro_locate_counters* ctr,
+                                const cro_locate_record* records, const uint64_t* granules, uint64_t granule_words,
+                                const cro_sweep_slot* slots, cro_fault_report* out, cro_fault_word* words, int cap, int* n) try {
+    if (!passes || !ctr || !slots || !out || !n || cap < 0 || (cap > 0 && !words) || sweep_bytes == 0 || sweep_bytes % 8 ||
+        n_passes == 0 || n_passes > CRO_LOCATE_PASSES || granule_words > kMaxGranuleWords || (granule_words && !granules))
+        return CRO_ERR_INVALID_ARG;
+    for (uint32_t p = 0; p < n_passes; ++p)
+        if ((passes[p].halves | passes[p].skipped) & ~3u) return CRO_ERR_INVALID_ARG;
+    if (records_of(ctr, (int)n_passes) && !records) return CRO_ERR_INVALID_ARG;
+    *n = 0;
+    std::vector<cro_fault_word> found;
+    const int rc = selftest_locate_collect(sweep_bytes, passes, n_passes, ctr, records, granules, granule_words, slots, out, &found);
+    out->recorded = copy_capped(found, words, cap, n);
+    if (out->recorded < found.size()) out->complete = 0;        // as cro_locate_faults
+    return rc;
+} CRO_API_CATCH
+int cro_selftest_scan_collect(int32_t cuda_error, const cro_locate_counters* ctr, const cro_locate_record* records,
+                              const uint64_t* granules, uint64_t granule_words, const cro_sweep_slot* slots, cro_scan_report* out,
+                              cro_fault_word* words, int cap, int* n) try {
+    if (!ctr || !slots || !out || !n || cap < 0 || (cap > 0 && !words) || granule_words > kMaxGranuleWords ||
+        (granule_words && !granules) || out->n_chunks == 0 || out->n_chunks > CRO_SCAN_MAX_CHUNKS ||
+        out->elements_done > CRO_SCAN_ELEMENTS || (records_of(ctr, CRO_SCAN_PASSES) && !records))
+        return CRO_ERR_INVALID_ARG;
+    uint64_t at = 0;
+    for (uint32_t k = 0; k < out->n_chunks; ++k) {
+        const cro_scan_chunk& K = out->chunk[k];
+        if (K.word0 != at || K.bytes == 0 || K.bytes % 8 || K.bytes / 8 > (1ull << 37) - at) return CRO_ERR_INVALID_ARG;
+        at += K.bytes / 8;
+    }
+    *n = 0;
+    std::vector<cro_fault_word> found;
+    const int rc = selftest_scan_collect(cuda_error, ctr, records, granules, granule_words, slots, out, &found);
+    out->recorded = copy_capped(found, words, cap, n);
+    if (out->recorded < found.size()) out->complete = 0;        // as cro_scan_hbm
+    return rc;
+} CRO_API_CATCH
+int cro_selftest_link_classify(uint64_t bytes, const uint64_t* seeds, uint32_t minor, uint32_t hops, const cro_locate_counters* ctr,
+                               const cro_locate_record* records, const uint64_t* host, const cro_sweep_slot* slots,
+                               const uint64_t* chase_out, cro_link_result* out, cro_link_fault* faults, int cap, int* n) try {
+    if (!seeds || !ctr || !host || !slots || !chase_out || !out || !n || cap < 0 || (cap > 0 && !faults) || bytes < 16 ||
+        bytes % 16 || hops == 0 || hops > (1u << 24) || (records_of(ctr, CRO_LINK_WORD_CHECKS) && !records))
+        return CRO_ERR_INVALID_ARG;
+    *n = 0;
+    std::vector<cro_link_fault> found;
+    const int rc = selftest_link_classify(bytes, seeds, minor, hops, ctr, records, host, slots, chase_out, out, &found);
+    copy_capped(found, faults, cap, n);
+    return rc;
 } CRO_API_CATCH
 int cro_compute_expected(int answer, uint64_t seed, int32_t* out) try {
     return compute::Expected(answer, seed, out);

@@ -98,7 +98,6 @@ void collect(const MismatchView& hv, bool have_cf, cro_scan_report* rep, std::ve
             dx[k] ^= R.actual ^ R.expected;
             ds[k] += delta;
             dw[k] += delta * (2 * i + 1);
-            rep->flip_or |= R.actual ^ R.expected;
             auto it = merged.find(R.word);
             if (it == merged.end()) merged[R.word] = cro_fault_word{R.word, R.expected, R.actual, 1u << p, k};
             else it->second.passes |= 1u << p;
@@ -116,12 +115,58 @@ void collect(const MismatchView& hv, bool have_cf, cro_scan_report* rep, std::ve
             else cf = complement_fold(cf, K.bytes / 8);
             if ((s.x ^ cf.x) != dx[k] || s.s - cf.s != ds[k] || s.w - cf.w != dw[k]) complete = false;
         }
+        // from the exact counters: a bit flipped only in words past the record cap counts too
+        for (int b = 0; b < 64; ++b)
+            if (P.bit_flips[b]) rep->flip_or |= 1ull << b;
     }
     rep->located = merged.size();
     for (const auto& kv : merged) words->push_back(kv.second);
     rep->complete = complete ? 1u : 0u;
 }
+
+// The end of a scan whose elements ran (elements_done of them, elem_err the CUDA error that stopped them): the passes
+// collected from hv (nullptr: the counters could not be fetched) as far as the scan got — nothing below E2 after an
+// error — and the status.  The closed forms ran only when no element failed.
+int finish_scan(const MismatchView* hv, cudaError_t elem_err, cro_scan_report* rep, std::vector<cro_fault_word>* words) {
+    if (hv && !(elem_err && rep->elements_done < 2)) collect(*hv, !elem_err, rep, words);
+    if (elem_err) {
+        rep->cuda_error = (int32_t)elem_err;
+        return CRO_ERR_CUDA;
+    }
+    for (const cro_scan_pass& P : rep->pass)
+        if (P.mismatches) return CRO_ERR_CHECKSUM;
+    return CRO_OK;
+}
 }  // namespace
+
+int selftest_scan_collect(int32_t cuda_error, const cro_locate_counters* ctr, const cro_locate_record* records,
+                          const uint64_t* granules, uint64_t granule_words, const cro_sweep_slot* slots, cro_scan_report* rep,
+                          std::vector<cro_fault_word>* words) {
+    const cro_scan_report in = *rep;
+    blank_report(rep, words);
+    rep->n_chunks = in.n_chunks;
+    rep->elements_done = in.elements_done;
+    for (uint32_t k = 0; k < in.n_chunks; ++k) {
+        rep->chunk[k].word0 = in.chunk[k].word0;
+        rep->chunk[k].bytes = in.chunk[k].bytes;
+        rep->covered_bytes += in.chunk[k].bytes;
+    }
+    // the device's layout: kLocateRecords records per pass, the compare slots then the closed forms
+    std::vector<LocateCounters> c(CRO_SCAN_PASSES);
+    std::vector<LocateRecord> rec((size_t)CRO_SCAN_PASSES * kLocateRecords);
+    std::vector<unsigned long long> gran(CRO_SCAN_PASSES * granule_words);
+    std::vector<SweepOut> s(kCfSlot0 + CRO_SCAN_MAX_CHUNKS);
+    memcpy(c.data(), ctr, sizeof(LocateCounters) * CRO_SCAN_PASSES);
+    for (int p = 0; p < CRO_SCAN_PASSES; ++p) {
+        const uint64_t k = std::min<uint64_t>(ctr[p].claims, kLocateRecords);
+        if (k) memcpy(&rec[(size_t)p * kLocateRecords], records, k * sizeof *records);
+        records += k;
+    }
+    if (granule_words) memcpy(gran.data(), granules, CRO_SCAN_PASSES * granule_words * 8);
+    memcpy(s.data(), slots, s.size() * sizeof *slots);
+    const MismatchView hv{c.data(), gran.data(), s.data(), rec.data(), nullptr, granule_words};
+    return rep->status = finish_scan(&hv, (cudaError_t)cuda_error, rep, words);
+}
 
 uint32_t scan_health(const cro_hbm_health& b, const cro_hbm_health& a) {
     uint32_t h = 0;
@@ -232,34 +277,23 @@ int ctx_scan_hbm(cro_ctx* c, int idx, const cro_scan_opts& o, cro_scan_report* r
         rep->health = scan_health(rep->before, rep->after);
 
         // the closed forms (ALU only) once every element ran; the counters as far as the scan got
-        bool have_cf = false;
-        if (!elem_err) {
-            for (uint32_t k = 0; k < rep->n_chunks && !elem_err; ++k) {
-                elem_err = launch_expected(d->plan, rep->chunk[k].bytes, Params{ProbeParams{rep->seed + rep->chunk[k].word0, 0}, nullptr},
-                                           sc, &dv.slots[kCfSlot0 + k], d->stream);
-                c->launches++;
-            }
-            have_cf = !elem_err;
+        for (uint32_t k = 0; k < rep->n_chunks && !elem_err; ++k) {
+            elem_err = launch_expected(d->plan, rep->chunk[k].bytes, Params{ProbeParams{rep->seed + rep->chunk[k].word0, 0}, nullptr},
+                                       sc, &dv.slots[kCfSlot0 + k], d->stream);
+            c->launches++;
         }
-        if (elem_err && rep->elements_done < 2) return CRO_OK;
+        if (elem_err && rep->elements_done < 2) return finish_scan(nullptr, elem_err, rep, words);
         if (mb.fetch(c, d->stream) != CRO_OK || cudaStreamSynchronize(d->stream) != cudaSuccess) {
             if (!elem_err) elem_err = cudaGetLastError();
             if (!elem_err) elem_err = cudaErrorUnknown;
-            return CRO_OK;
+            return finish_scan(nullptr, elem_err, rep, words);
         }
-        collect(mb.host(), have_cf, rep, words);
-        return CRO_OK;
+        const MismatchView hv = mb.host();
+        return finish_scan(&hv, elem_err, rep, words);
     }();
     const uint64_t t_free = now_ns();
     ch.release();
     rep->alloc_ns += now_ns() - t_free;
-    if (!rc && elem_err) {
-        rep->cuda_error = (int32_t)elem_err;
-        rc = CRO_ERR_CUDA;
-    }
-    if (!rc) {
-        for (const cro_scan_pass& P : rep->pass) rc = rc ? rc : (P.mismatches ? CRO_ERR_CHECKSUM : CRO_OK);
-    }
     if (rc == CRO_ERR_OOM || rc == CRO_ERR_INVALID_ARG) {
         // nothing was scanned: keep what says why (the sizes), drop the rest
         const cro_scan_report keep = *rep;

@@ -59,7 +59,81 @@ std::string link_opts_error(const cro_link_opts& o, uint64_t S) {
                ", and an injection must name a word check (0..4) and a word below L / 8";
     return "";
 }
+
+// Word check ck's counts and records once it ran (hv, the host mirror after the fetch), each record with word
+// word_index of the host buffer the check involved (hb, n = L / 8 words, read now), appended to *faults by word index.
+void take_link_check(const MismatchView& hv, int ck, const volatile uint64_t* hb, uint64_t n, cro_link_result* r,
+                     std::vector<cro_link_fault>* faults) {
+    cro_link_check& C = r->check[ck];
+    C.mismatches = hv.ctr[ck].mismatches;
+    C.recorded = std::min<uint64_t>(hv.ctr[ck].claims, kLocateRecords);
+    std::vector<cro_link_fault> f;
+    for (uint64_t j = 0; j < C.recorded; ++j) {
+        const LocateRecord& R = hv.rec[(size_t)ck * kLocateRecords + j];
+        f.push_back(cro_link_fault{(uint32_t)ck, 0, R.word, R.expected, R.actual, R.word < n ? hb[R.word] : 0});
+    }
+    std::sort(f.begin(), f.end(), [](const cro_link_fault& a, const cro_link_fault& b) { return a.word_index < b.word_index; });
+    faults->insert(faults->end(), f.begin(), f.end());
+}
+
+// The verdict once every check was taken: each word check's fold against the closed form of its pattern (both over
+// n = L / 8 words, the pattern seeds r->seed), then the chase's end (hco: the chase output words) against the host walk
+// of hops steps through the (minor, minor) permutation.  first_fail is the lowest check that failed.
+void classify_link(const MismatchView& hv, const unsigned long long* hco, int minor, uint32_t hops, cro_link_result* r) {
+    const uint64_t n = r->bytes / 8;
+    for (int ck = 0; ck < CRO_LINK_WORD_CHECKS; ++ck) {
+        cro_link_check& C = r->check[ck];
+        const SweepOut& s = hv.slots[ck];
+        const SweepOut& cf = hv.slots[kLSlotExpect + kCheckPattern[ck]];
+        C.words = n;
+        C.seed = r->seed[kCheckPattern[ck]];
+        C.fold_xor = s.x;
+        C.fold_sum = s.s;
+        C.fold_wsum = s.w;
+        C.expect_xor = cf.x;
+        C.expect_sum = cf.s;
+        C.expect_wsum = cf.w;
+        const bool bad = C.mismatches != 0 || s.n_words != n || cf.n_words != n || s.x != cf.x || s.s != cf.s || s.w != cf.w;
+        if (bad && r->first_fail == CRO_LINK_NO_FAIL) r->first_fail = (uint32_t)ck;
+    }
+    std::vector<uint32_t> perm;
+    chase_permutation(minor, minor, &perm);
+    uint32_t at = 0;
+    for (uint32_t h = 0; h < hops; ++h) at = perm[at];
+    r->chase_expect = at;
+    r->chase_end = (uint32_t)hco[0];
+    r->chase_ns = hco[0] == kChaseArmed ? 0 : hco[1];
+    if (hco[0] != at && r->first_fail == CRO_LINK_NO_FAIL) r->first_fail = CRO_LINK_CHECK_CHASE;
+}
+
+int link_status(const cro_link_result& r) { return r.first_fail == CRO_LINK_NO_FAIL ? CRO_OK : CRO_ERR_CHECKSUM; }
 }  // namespace
+
+int selftest_link_classify(uint64_t bytes, const uint64_t* seeds, uint32_t minor, uint32_t hops, const cro_locate_counters* ctr,
+                           const cro_locate_record* records, const uint64_t* host, const cro_sweep_slot* slots,
+                           const uint64_t* chase_out, cro_link_result* r, std::vector<cro_link_fault>* faults) {
+    blank_result(r, faults, bytes);
+    const uint64_t n = bytes / 8;
+    for (int j = 0; j < 3; ++j) r->seed[j] = seeds[j];
+    r->chase_hops = hops;
+    r->chase_minor = minor;
+    // the device's layout: kLocateRecords records per check, then the result slots
+    std::vector<LocateCounters> c(CRO_LINK_WORD_CHECKS);
+    std::vector<LocateRecord> rec((size_t)CRO_LINK_WORD_CHECKS * kLocateRecords);
+    std::vector<SweepOut> s(kLSlots);
+    memcpy(c.data(), ctr, sizeof(LocateCounters) * CRO_LINK_WORD_CHECKS);
+    for (int ck = 0; ck < CRO_LINK_WORD_CHECKS; ++ck) {
+        const uint64_t k = std::min<uint64_t>(ctr[ck].claims, kLocateRecords);
+        if (k) memcpy(&rec[(size_t)ck * kLocateRecords], records, k * sizeof *records);
+        records += k;
+    }
+    memcpy(s.data(), slots, kLSlots * sizeof *slots);
+    const MismatchView hv{c.data(), nullptr, s.data(), rec.data(), nullptr, 0};
+    for (int ck = 0; ck < CRO_LINK_WORD_CHECKS; ++ck) take_link_check(hv, ck, host + ck * n, n, r, faults);
+    const unsigned long long co[2] = {chase_out[0], chase_out[1]};
+    classify_link(hv, co, (int)minor, hops, r);
+    return r->status = link_status(*r);
+}
 
 LinkState::~LinkState() {
     for (unsigned char*& h : host) unmap_pinned(h, cap);
@@ -171,19 +245,8 @@ int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_re
         auto harvest = [&](std::initializer_list<int> checks) -> int {
             int rc2 = mb.fetch(c, st);
             if (rc2 || (rc2 = wait_stream(c, d))) return rc2;
-            for (int ck : checks) {
-                cro_link_check& C = r->check[ck];
-                C.mismatches = hv.ctr[ck].mismatches;
-                C.recorded = std::min<uint64_t>(hv.ctr[ck].claims, kLocateRecords);
-                std::vector<cro_link_fault> f;
-                const volatile uint64_t* hb = reinterpret_cast<const volatile uint64_t*>(ls.host[kCheckHost[ck]]);
-                for (uint64_t j = 0; j < C.recorded; ++j) {
-                    const LocateRecord& R = hv.rec[(size_t)ck * kLocateRecords + j];
-                    f.push_back(cro_link_fault{(uint32_t)ck, 0, R.word, R.expected, R.actual, R.word < n ? hb[R.word] : 0});
-                }
-                std::sort(f.begin(), f.end(), [](const cro_link_fault& a, const cro_link_fault& b) { return a.word_index < b.word_index; });
-                faults->insert(faults->end(), f.begin(), f.end());
-            }
+            for (int ck : checks)
+                take_link_check(hv, ck, reinterpret_cast<const volatile uint64_t*>(ls.host[kCheckHost[ck]]), n, r, faults);
             return CRO_OK;
         };
         auto role = [&](void* buf, int pat, int scratch, SweepOut* out) {
@@ -273,30 +336,7 @@ int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_re
             r->leg[lg].timer_ns = timer_of[lg] >= 0 ? window(hv.slots[timer_of[lg]]) : 0;
         }
         r->ce_duplex_span_ns = std::max(span(10, 11), span(10, 13));
-        for (int ck = 0; ck < CRO_LINK_WORD_CHECKS; ++ck) {
-            cro_link_check& C = r->check[ck];
-            const SweepOut& s = hv.slots[ck];
-            const SweepOut& cf = hv.slots[kLSlotExpect + kCheckPattern[ck]];
-            C.words = n;
-            C.seed = P[kCheckPattern[ck]];
-            C.fold_xor = s.x;
-            C.fold_sum = s.s;
-            C.fold_wsum = s.w;
-            C.expect_xor = cf.x;
-            C.expect_sum = cf.s;
-            C.expect_wsum = cf.w;
-            const bool bad = C.mismatches != 0 || s.n_words != n || cf.n_words != n || s.x != cf.x || s.s != cf.s || s.w != cf.w;
-            if (bad && r->first_fail == CRO_LINK_NO_FAIL) r->first_fail = (uint32_t)ck;
-        }
-        const unsigned long long* hco = reinterpret_cast<const unsigned long long*>(hv.tail);
-        std::vector<uint32_t> perm;
-        chase_permutation(d->info.device_minor, d->info.device_minor, &perm);
-        uint32_t at = 0;
-        for (uint32_t h = 0; h < hops; ++h) at = perm[at];
-        r->chase_expect = at;
-        r->chase_end = (uint32_t)hco[0];
-        r->chase_ns = hco[0] == kChaseArmed ? 0 : hco[1];
-        if (hco[0] != at && r->first_fail == CRO_LINK_NO_FAIL) r->first_fail = CRO_LINK_CHECK_CHASE;
+        classify_link(hv, reinterpret_cast<const unsigned long long*>(hv.tail), d->info.device_minor, hops, r);
         for (int b = 0; b < 2; ++b) r->host_numa[b] = pcilink::NodeOf(ls.host[b]);
         r->host_numa[2] = pcilink::NodeOf(ls.chase);
         return CRO_OK;
@@ -305,7 +345,7 @@ int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_re
         blank_result(r, faults, r->bytes);
         return r->status = rc;
     }
-    return r->status = r->first_fail == CRO_LINK_NO_FAIL ? CRO_OK : CRO_ERR_CHECKSUM;
+    return r->status = link_status(*r);
 }
 
 namespace {

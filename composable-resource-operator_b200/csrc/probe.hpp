@@ -218,6 +218,12 @@ int ctx_read_words(cro_ctx* c, int idx, uint64_t first, uint64_t n, uint64_t* ou
 int ctx_locate(cro_ctx* c, int idx, const cro_locate_opts& o, cro_fault_report* rep, std::vector<cro_fault_word>* words);
 // CRO_FAULTS_* of a report, from its per-pass mismatch counts.
 uint32_t fault_verdict(const cro_fault_report& r);
+// cro_selftest_locate_collect: the locator's report from the caller's counters, records, bitmaps and slots, as
+// ctx_locate makes it from its kernels' (CRO_ERR_INVALID_ARG when the compared halves have more than
+// CRO_LOCATE_PASSES distinct seeds).
+int selftest_locate_collect(uint64_t sweep_bytes, const cro_locate_pass* passes, uint32_t n_passes, const cro_locate_counters* ctr,
+                            const cro_locate_record* records, const uint64_t* granules, uint64_t granule_words,
+                            const cro_sweep_slot* slots, cro_fault_report* rep, std::vector<cro_fault_word>* words);
 
 // Host link probe (include/croprobe.h, cro_probe_host_link / cro_probe_host_link_uuid): *faults gets every recorded
 // mismatch, by check, then index.  The uuid form runs `croprobe-cli link-raw` and asks it for at most cap faults;
@@ -225,6 +231,11 @@ uint32_t fault_verdict(const cro_fault_report& r);
 int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_result* r, std::vector<cro_link_fault>* faults);
 int ctx_probe_host_link_uuid(cro_ctx* c, const char* uuid, const cro_link_opts& o, int deadline_ms, cro_link_result* r,
                              std::vector<cro_link_fault>* faults, int cap, uint64_t* helper_ns);
+// cro_selftest_link_classify: the probe's takes and classification of the caller's counters, records, host words,
+// slots and chase output, as ctx_probe_host_link makes them from its kernels'.
+int selftest_link_classify(uint64_t bytes, const uint64_t* seeds, uint32_t minor, uint32_t hops, const cro_locate_counters* ctr,
+                           const cro_locate_record* records, const uint64_t* host, const cro_sweep_slot* slots,
+                           const uint64_t* chase_out, cro_link_result* r, std::vector<cro_link_fault>* faults);
 
 // SM compute probe (include/croprobe.h, cro_probe_compute / cro_probe_compute_uuid): *sms gets one entry per SM seen, by
 // SM id; *faults every recorded element, by (leg, smid, row, col).  The uuid form runs `croprobe-cli compute-raw` and
@@ -303,6 +314,12 @@ int ctx_scan_hbm_uuid(cro_ctx* c, const char* uuid, const cro_scan_opts& o, cro_
                       int cap);
 // CRO_SCAN_HEALTH_* of the NVML reads before E0 and after E3.
 uint32_t scan_health(const cro_hbm_health& before, const cro_hbm_health& after);
+// cro_selftest_scan_collect: the scan's passes, words and status from the caller's counters, records, bitmaps and
+// slots, as ctx_scan_hbm makes them from its kernels'.  *rep gives n_chunks, elements_done and the chunks' word0 and
+// bytes.
+int selftest_scan_collect(int32_t cuda_error, const cro_locate_counters* ctr, const cro_locate_record* records,
+                          const uint64_t* granules, uint64_t granule_words, const cro_sweep_slot* slots, cro_scan_report* rep,
+                          std::vector<cro_fault_word>* words);
 
 // SRAM probe (include/croprobe.h, cro_probe_sram / cro_probe_sram_uuid, sram_probe.cu): *sms gets one entry per SM
 // seen, by SM id; *faults every recorded word, by (leg, element, smid, iteration, word).  The uuid form runs

@@ -1997,6 +1997,67 @@ typedef struct cro_selftest_sweep_out {
 int  cro_selftest_sweep(cro_ctx *ctx, int dev_index, const cro_selftest_sweep_opts *opts, cro_selftest_sweep_out *out,
                         void *buf, uint64_t cap_bytes, cro_fault_word *words, int cap, int *n);
 
+/* ---- test hooks: the word checks' reports from caller-given device output ------------------------------------- */
+/* Pure functions, no context: the host code that turns what the word-checking kernels (the locator's compare, the
+ * link probe's read role) wrote into a report, run on the caller's copy of it. */
+
+/* What a word-checking kernel keeps per pass or check: exact counts, and records while there is room. */
+typedef struct cro_locate_counters {
+    uint64_t mismatches;           /*   0  exact                                                                  */
+    uint64_t claims;               /*   8  record slots claimed (may run past CRO_LOCATE_RECORDS)                 */
+    uint64_t bits[64];             /*  16  mismatching words with bit b flipped                                   */
+} cro_locate_counters;             /* 528 bytes */
+
+typedef struct cro_locate_record {
+    uint64_t word;                 /*   0  region, scan or buffer index                                           */
+    uint64_t expected;             /*   8 */
+    uint64_t actual;               /*  16 */
+} cro_locate_record;               /*  24 bytes */
+
+/* The fault locator's report (cro_locate_faults) of a call on a sweep region of sweep_bytes (a multiple of 8) with
+ * n_passes passes (1 .. CRO_LOCATE_PASSES), from caller-given compare output instead of launches.  passes[p] gives pass
+ * p's halves, skipped, seed and invert (nothing else of it is read).  Per pass p: ctr[p], the first
+ * min(ctr[p].claims, CRO_LOCATE_RECORDS) records of `records` (in pass order), granule_words words of `granules` (in
+ * pass order; at most 8192, the bitmap of 2^37 words).  slots[0 .. 2 * CRO_LOCATE_PASSES + CRO_LOCATE_PASSES) as the
+ * device lays them out: [2p + h] the compare of half h in pass p, then [2 * CRO_LOCATE_PASSES + k] the closed form of
+ * the k-th distinct seed of a compared half, counted in pass then half order.  Writes out and words[0 .. cap) (*n) as
+ * cro_locate_faults does (retest_seed stays 0).  Returns out->status, or CRO_ERR_INVALID_ARG for a NULL array it needs,
+ * a negative cap, sweep_bytes 0 or not a multiple of 8, n_passes out of range, halves or skipped beyond bits 0 and 1,
+ * more than CRO_LOCATE_PASSES distinct seeds, or granule_words above 8192. */
+int  cro_selftest_locate_collect(uint64_t sweep_bytes, const cro_locate_pass *passes, uint32_t n_passes,
+                                 const cro_locate_counters *ctr, const cro_locate_record *records, const uint64_t *granules,
+                                 uint64_t granule_words, const cro_sweep_slot *slots, cro_fault_report *out,
+                                 cro_fault_word *words, int cap, int *n);
+
+/* The whole-HBM scan's report (cro_scan_hbm) from caller-given compare output.  *out gives the call's n_chunks (1 ..
+ * CRO_SCAN_MAX_CHUNKS), elements_done (0 .. CRO_SCAN_ELEMENTS) and each chunk's word0 and bytes: the chunks must lie
+ * back to back from word 0, each a non-zero multiple of 8 bytes, and end by word 2^37; the rest of *out is blanked,
+ * and covered_bytes is the chunks' sum.  cuda_error: the cudaError_t that stopped the elements (0: none; the closed
+ * forms ran only without one).  Per pass p of CRO_SCAN_PASSES: ctr[p], the first min(ctr[p].claims, CRO_LOCATE_RECORDS) records of `records`
+ * (in pass order) and granule_words words of `granules` (at most 8192).  slots: CRO_SCAN_PASSES * CRO_SCAN_MAX_CHUNKS +
+ * CRO_SCAN_MAX_CHUNKS, [p * CRO_SCAN_MAX_CHUNKS + k] the compare of chunk k in pass p, then [CRO_SCAN_PASSES *
+ * CRO_SCAN_MAX_CHUNKS + k] chunk k's closed form.  Writes out and words[0 .. cap) (*n) as cro_scan_hbm does; the
+ * sizes, seed, times and health stay 0.  Returns out->status, or CRO_ERR_INVALID_ARG for a NULL array it needs, a
+ * negative cap or an out-of-range count or chunk. */
+int  cro_selftest_scan_collect(int32_t cuda_error, const cro_locate_counters *ctr, const cro_locate_record *records,
+                               const uint64_t *granules, uint64_t granule_words, const cro_sweep_slot *slots,
+                               cro_scan_report *out, cro_fault_word *words, int cap, int *n);
+
+/* The host link probe's word checks and chase (cro_probe_host_link) of a call of L = bytes (a multiple of 16, at least
+ * 16) with patterns seeds[3] (P1, P2, P3) and a chase of hops (1 .. 2^24) steps through the (minor, minor)
+ * permutation, from caller-given device output.  Per word check k: ctr[k], the first min(ctr[k].claims,
+ * CRO_LINK_RECORDS) records of `records` (in check order), and host[k * L / 8 .. (k + 1) * L / 8): the host buffer
+ * check k involved as the CPU read it once k ran.  slots: CRO_LINK_WORD_CHECKS + 5 as the device lays them out: [k]
+ * the fold of check k, [5] and [6] the write roles (not read), [7 + j] the closed form of pattern j.  chase_out: the
+ * chase kernel's two words, end slot and ns (all ones: armed, the chase did not publish).  Writes out and
+ * faults[0 .. cap) (*n) as cro_probe_host_link does, all but what needs the device: the legs, call, NUMA nodes,
+ * replays and path stay blank.  Returns out->status, or CRO_ERR_INVALID_ARG for a NULL array it needs, a negative cap,
+ * or bytes or hops out of range. */
+int  cro_selftest_link_classify(uint64_t bytes, const uint64_t *seeds, uint32_t minor, uint32_t hops,
+                                const cro_locate_counters *ctr, const cro_locate_record *records, const uint64_t *host,
+                                const cro_sweep_slot *slots, const uint64_t *chase_out, cro_link_result *out,
+                                cro_link_fault *faults, int cap, int *n);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,15 +7,112 @@ and words a list of (word_index, expected, actual).
 Verdict rule (include/croprobe.h, CRO_FAULTS_*): a retest pass (1 or 2) that ran and found a mismatch makes the
 faults persistent; otherwise mismatches in pass 0 are "not reproduced" when a retest ran and "unclassified" when none
 did; no mismatch anywhere is "none".  Only the first min(n_passes, 3) passes count.
+
+collect() restates the report cro_locate_faults makes from what its compare kernels wrote (cro_selftest_locate_collect).
 """
 from __future__ import annotations
 
-from typing import Dict, Sequence, Tuple
+from typing import Dict, List, Sequence, Tuple
 
 from oracle import go_marshal_string_map
 
 PASSES = 3
+RECORDS = 4096
+OK, ERR_CHECKSUM = 0, -6
+U64 = (1 << 64) - 1
 NONE, UNCLASSIFIED, NOT_REPRODUCED, PERSISTENT = 0, 1, 2, 3
+
+
+def complement_fold(f: Tuple[int, int, int], n: int) -> Tuple[int, int, int]:
+    """The closed form of the complement of a pattern over n words from the pattern's: ~p = -1 - p, and the weights
+    2i + 1 of n words sum to n^2."""
+    return f[0] ^ (U64 if n & 1 else 0), (-n - f[1]) & U64, (-n * n - f[2]) & U64
+
+
+def deltas(records, index) -> Tuple[int, int, int]:
+    """What the records change in a fold: xor, sum and weighted sum of actual - expected, each record at the position
+    index(word) of its own sweep."""
+    dx = ds = dw = 0
+    for r in records:
+        d = (r["actual"] - r["expected"]) & U64
+        dx ^= r["actual"] ^ r["expected"]
+        ds = (ds + d) & U64
+        dw = (dw + d * (2 * index(r["word"]) + 1)) & U64
+    return dx, ds, dw
+
+
+def explained(slot: Dict, cf: Tuple[int, int, int], d: Tuple[int, int, int]) -> bool:
+    """The fold in `slot` is the closed form cf changed by exactly the deltas d."""
+    return (slot["x"] ^ cf[0], (slot["s"] - cf[1]) & U64, (slot["w"] - cf[2]) & U64) == d
+
+
+def merge(records_by_pass, chunk_of=lambda w: 0) -> List[Dict]:
+    """Every recorded word once, by index: expected and actual from the first record of it (in pass order), bit p of
+    passes for each pass that recorded it, reserved = chunk_of(word)."""
+    words = {}
+    for p, recs in enumerate(records_by_pass):
+        for r in recs:
+            w = words.setdefault(r["word"], dict(word_index=r["word"], expected=r["expected"], actual=r["actual"], passes=0,
+                                                 reserved=chunk_of(r["word"])))
+            w["passes"] |= 1 << p
+    return [words[k] for k in sorted(words)]
+
+
+def collect(call: Dict) -> Tuple[Dict, List[Dict]]:
+    """The report and word list cro_locate_faults makes of its passes.  call: {"sweep_bytes", "passes": [{"halves",
+    "skipped", "seed": [2], "invert"}] (one per pass), "counters": [{"mismatches", "claims", "bits": [64]}],
+    "records": [[{"word", "expected", "actual"}]] (the first min(claims, RECORDS) of each pass), "granules": [[words]],
+    "slots": [9 slots {"x", "s", "w", "t0", "t1", "n_words", ...}], "cap"}.
+
+    From include/croprobe.h: half h of the region holds words [h * n, (h + 1) * n), n = S / 8, and word i of a half
+    is compared with pattern_word(seed[h], i) ^ invert.  The device's slots are [2p + h] for the compare of half h in
+    pass p, then one closed form per distinct seed of a compared half, in pass then half order; a pass with invert
+    compares against the complement's closed form.  complete: every pass recorded all its mismatches, each compared
+    half's fold differs from its closed form by exactly its records' deltas (weights from the half's start), and the
+    caller's list holds every located word."""
+    n = call["sweep_bytes"] // 8
+    np_ = len(call["passes"])
+    seeds = []
+    for P in call["passes"]:
+        for h in range(2):
+            if P["halves"] >> h & 1 and P["seed"][h] not in seeds:
+                seeds.append(P["seed"][h])
+    complete = True
+    bit_flips = [0] * 64
+    passes = []
+    for p, (P, c, recs) in enumerate(zip(call["passes"], call["counters"], call["records"])):
+        recorded = min(c["claims"], RECORDS)
+        assert len(recs) == recorded
+        complete &= recorded == c["mismatches"]
+        bit_flips = [(a + b) & U64 for a, b in zip(bit_flips, c["bits"])]
+        out = dict(halves=P["halves"], skipped=P["skipped"], seed=list(P["seed"]), invert=P["invert"], words_scanned=0,
+                   mismatches=c["mismatches"], recorded=recorded, granules=sum(bin(g).count("1") for g in call["granules"][p]),
+                   scan_ns=0, fold_xor=[0, 0], fold_sum=[0, 0], fold_wsum=[0, 0])
+        for h in range(2):
+            if not P["halves"] >> h & 1:
+                continue
+            s = call["slots"][2 * p + h]
+            out["words_scanned"] = (out["words_scanned"] + s["n_words"]) & U64
+            out["scan_ns"] = (out["scan_ns"] + s["t1"] - s["t0"]) & U64
+            out["fold_xor"][h], out["fold_sum"][h], out["fold_wsum"][h] = s["x"], s["s"], s["w"]
+            c_ = call["slots"][2 * PASSES + seeds.index(P["seed"][h])]
+            cf = (c_["x"], c_["s"], c_["w"])
+            if P["invert"]:
+                cf = complement_fold(cf, n)
+            mine = [r for r in recs if (r["word"] >= n) == (h == 1)]
+            complete &= explained(s, cf, deltas(mine, lambda w: w - h * n))
+        passes.append(out)
+    blank = dict(halves=0, skipped=0, seed=[0, 0], invert=0, words_scanned=0, mismatches=0, recorded=0, granules=0,
+                 scan_ns=0, fold_xor=[0, 0], fold_sum=[0, 0], fold_wsum=[0, 0])
+    passes += [dict(blank) for _ in range(PASSES - np_)]
+    words = merge(call["records"])
+    listed = words[:call["cap"]]
+    r = dict(status=ERR_CHECKSUM if any(P["mismatches"] for P in passes[:np_]) else OK, n_passes=np_,
+             complete=int(complete and len(listed) == len(words)), sweep_bytes=call["sweep_bytes"], retest_seed=0,
+             located=len(words), recorded=len(listed), flip_or=sum(1 << b for b in range(64) if bit_flips[b]),
+             bit_flips=bit_flips, pass_=passes)
+    r["verdict"] = verdict(dict(n_passes=np_, **{"pass": passes}))
+    return r, listed
 VERDICT_TEXT = {NONE: "none", UNCLASSIFIED: "unclassified", NOT_REPRODUCED: "not-reproduced", PERSISTENT: "persistent"}
 WORDS_SHOWN = 8
 

@@ -1,5 +1,6 @@
-"""Restatement of the host link probe's annotations (cro_emit_link_annotations_json) and of the PCIe path rules
-(cro_pci_link_path: bottleneck and degraded flags).
+"""Restatement of the host link probe's annotations (cro_emit_link_annotations_json), of the PCIe path rules
+(cro_pci_link_path: bottleneck and degraded flags) and of the word checks' and the chase's verdict (classify,
+cro_selftest_link_classify).
 
 Pure Python over a result given as plain values, so the emitter can be held to it without a GPU.  A result is a dict:
   {"status": int, "first_fail": int, "leg": [{"bytes": int, "ns": int}] * 8, "ce_duplex_span_ns": int,
@@ -13,7 +14,7 @@ legs over their span; latency is chase ns // hops; a speed in tenths of a GT/s p
 """
 from __future__ import annotations
 
-from typing import Dict, List
+from typing import Callable, Dict, List, Tuple
 
 from oracle import go_marshal_string_map
 
@@ -64,6 +65,51 @@ def annotations(r: Dict) -> Dict[str, str]:
 def annotations_json(r: Dict) -> bytes:
     """The bytes json.Marshal of the annotation map gives (keys sorted)."""
     return go_marshal_string_map(annotations(r)).encode()
+
+
+CHECK_PATTERN = [0, 0, 1, 2, 0]     # P1, P1, P2, P3, P1: the pattern word check k's buffer must hold
+WORD_CHECKS, CHECK_CHASE, NO_FAIL, RECORDS = 5, 5, 0xFFFFFFFF, 4096
+SLOT_EXPECT = WORD_CHECKS + 2       # slots: [k] check k's fold, the two write roles, then the closed forms of P1..P3
+OK, ERR_CHECKSUM = 0, -6
+
+
+def classify(call: Dict, chase_end: Callable[[int, int, int], int]) -> Tuple[Dict, List[Dict]]:
+    """The word checks' and the chase's part of the result, and the faults, that cro_probe_host_link makes of what its
+    kernels wrote (cro_selftest_link_classify).  call: {"bytes", "seeds": [3], "minor", "hops", "counters": [5 x
+    {"mismatches", "claims"}], "records": [5 x [{"word", "expected", "actual"}]] (the first min(claims, RECORDS) of
+    each check), "host": [5 x [L / 8 words]], "slots": [10 slots {"x", "s", "w", "n_words", ...}], "chase_out": [end,
+    ns], "cap"}.  chase_end(minor_src, minor_dst, hops): the host walk of the latency permutation.
+
+    From include/croprobe.h: check k must hold pattern_word(seed, i) for its pattern's seed over L / 8 words; it fails
+    when it counted a mismatch, or its fold or closed form covered another number of words, or its fold is not the
+    closed form.  The chase fails when it did not end on the host walk's slot (an armed output, all ones, never does
+    and reports no time).  first_fail is the lowest failing check.  The faults run by check, then word index, and
+    host_value is word word_index of the host buffer the check involved, 0 past L / 8."""
+    n = call["bytes"] // 8
+    first_fail = NO_FAIL
+    checks, found = [], []
+    for k in range(WORD_CHECKS):
+        c, recs = call["counters"][k], call["records"][k]
+        assert len(recs) == min(c["claims"], RECORDS)
+        s, cf = call["slots"][k], call["slots"][SLOT_EXPECT + CHECK_PATTERN[k]]
+        checks.append(dict(words=n, mismatches=c["mismatches"], recorded=len(recs), seed=call["seeds"][CHECK_PATTERN[k]],
+                           fold_xor=s["x"], fold_sum=s["s"], fold_wsum=s["w"], expect_xor=cf["x"], expect_sum=cf["s"],
+                           expect_wsum=cf["w"]))
+        bad = c["mismatches"] != 0 or s["n_words"] != n or cf["n_words"] != n or (s["x"], s["s"], s["w"]) != (
+            cf["x"], cf["s"], cf["w"])
+        if bad and first_fail == NO_FAIL:
+            first_fail = k
+        found += [dict(check=k, reserved=0, word_index=r["word"], expected=r["expected"], actual=r["actual"],
+                       host_value=call["host"][k][r["word"]] if r["word"] < n else 0)
+                  for r in sorted(recs, key=lambda r: r["word"])]
+    expect = chase_end(call["minor"], call["minor"], call["hops"])
+    end, ns = call["chase_out"]
+    if end != expect and first_fail == NO_FAIL:
+        first_fail = CHECK_CHASE
+    r = dict(status=OK if first_fail == NO_FAIL else ERR_CHECKSUM, first_fail=first_fail, bytes=call["bytes"],
+             seed=list(call["seeds"]), check=checks, chase_hops=call["hops"], chase_end=end & 0xFFFFFFFF,
+             chase_expect=expect, chase_minor=call["minor"], chase_ns=0 if end == U64 else ns)
+    return r, found[:call["cap"]]
 
 
 def bottleneck(hops: List[Dict]) -> int:

@@ -1,5 +1,6 @@
 """Restatement of the whole-HBM scan's verdict, health bits and annotations (cro_scan_hbm, scan_health,
-cro_emit_scan_annotations_json), and of what a stuck-at force does to the scan's two compare passes.
+cro_emit_scan_annotations_json), of its report from what the compare passes wrote (collect, cro_selftest_scan_collect),
+and of what a stuck-at force does to the scan's two compare passes.
 
 Pure Python over a report given as plain values, so the emitter can be held to it without a GPU.  A report is a dict:
   {"status": int, "cuda_error": int, "health": int, "seed": int, "covered_bytes": int, "free_bytes": int,
@@ -14,13 +15,15 @@ sum is 0; an NVML field prints only when the read that fills it answered (both r
 """
 from __future__ import annotations
 
-from typing import Dict, List
+from typing import Dict, List, Tuple
 
 import numpy as np
 
+import faults
 from oracle import go_marshal_string_map, pattern_words_np
 
 OK, ERR_CUDA, ERR_CHECKSUM = 0, -4, -6
+SCAN_PASSES, SCAN_ELEMENTS, SCAN_MAX_CHUNKS, RECORDS = 2, 4, 128, 4096
 ECC_CORRECTED_DURING, ECC_UNCORRECTED_DURING, REMAP_PENDING, REMAP_FAILURE = 1, 2, 4, 8
 HEALTH_NAMES = ["ecc-corrected", "ecc-uncorrected", "remap-pending", "remap-failure"]
 NVML_ECC_CORRECTED, NVML_ECC_UNCORRECTED, NVML_REMAP, NVML_HISTOGRAM = 1, 2, 4, 8
@@ -76,6 +79,61 @@ def annotations(r: Dict) -> Dict[str, str]:
 
 def annotations_json(r: Dict) -> bytes:
     return go_marshal_string_map(annotations(r)).encode("utf-8")
+
+
+def collect(call: Dict) -> Tuple[Dict, List[Dict]]:
+    """The report fields and word list cro_scan_hbm makes of its compare passes (cro_selftest_scan_collect).  call:
+    {"chunks": [(word0, bytes)], "elements_done", "cuda_error", "counters": [2 x {"mismatches", "claims", "bits"}],
+    "records": [2 x [{"word", "expected", "actual"}]] (the first min(claims, RECORDS) of each pass), "granules":
+    [2 x [words]], "slots": [SCAN_SLOTS slots {"x", "s", "w", "n_words", ...}], "cap"}.
+
+    From include/croprobe.h: compare pass p is element E(2p + 1), so it is reported only when that element completed,
+    and after a CUDA error that stopped the scan before E2 nothing is.  Scan word j lies in the chunk k with
+    word0_k <= j < word0_(k+1); chunk k is folded with weights from its own start and compared with its own closed form
+    (pass 1: the complement's, over the chunk's own words), which exists only when no element failed.  flip_or has
+    every bit that any reported mismatch flipped: the exact bit counters say which.  status: CRO_ERR_CUDA (cuda_error
+    kept) after an error, else CRO_ERR_CHECKSUM when a reported pass mismatched."""
+    starts = [w0 for w0, _ in call["chunks"]]
+    done, err = call["elements_done"], call["cuda_error"]
+    have_cf = err == 0
+
+    def chunk_of(w):
+        return max(k for k, w0 in enumerate(starts) if w0 <= w)
+    chunks = [dict(word0=w0, bytes=b, fold_xor=[0, 0], fold_sum=[0, 0], fold_wsum=[0, 0], expect_xor=0, expect_sum=0,
+                   expect_wsum=0) for w0, b in call["chunks"]]
+    passes = [dict(invert=0, words_scanned=0, mismatches=0, recorded=0, granules=0, bit_flips=[0] * 64)
+              for _ in range(SCAN_PASSES)]
+    ran = [] if err and done < 2 else [p for p in range(SCAN_PASSES) if 2 * p + 1 < done]
+    complete = have_cf and done == SCAN_ELEMENTS and not (err and done < 2)
+    for p in ran:
+        c, recs = call["counters"][p], call["records"][p]
+        P = passes[p]
+        P.update(invert=U64 if p else 0, mismatches=c["mismatches"], recorded=min(c["claims"], RECORDS),
+                 granules=sum(bin(g).count("1") for g in call["granules"][p]), bit_flips=list(c["bits"]))
+        assert len(recs) == P["recorded"]
+        complete &= P["recorded"] == P["mismatches"]
+        for k, K in enumerate(chunks):
+            s = call["slots"][p * SCAN_MAX_CHUNKS + k]
+            P["words_scanned"] = (P["words_scanned"] + s["n_words"]) & U64
+            K["fold_xor"][p], K["fold_sum"][p], K["fold_wsum"][p] = s["x"], s["s"], s["w"]
+            if not have_cf:
+                continue
+            c_ = call["slots"][SCAN_PASSES * SCAN_MAX_CHUNKS + k]
+            cf = (c_["x"], c_["s"], c_["w"])
+            if p == 0:
+                K["expect_xor"], K["expect_sum"], K["expect_wsum"] = cf
+            else:
+                cf = faults.complement_fold(cf, K["bytes"] // 8)
+            mine = [r for r in recs if chunk_of(r["word"]) == k]
+            complete &= faults.explained(s, cf, faults.deltas(mine, lambda w: w - K["word0"]))
+    words = faults.merge([call["records"][p] if p in ran else [] for p in range(SCAN_PASSES)], chunk_of)
+    listed = words[:call["cap"]]
+    status = ERR_CUDA if err else ERR_CHECKSUM if any(P["mismatches"] for P in passes) else OK
+    flips = [any(P["bit_flips"][b] for P in passes) for b in range(64)]
+    r = dict(status=status, cuda_error=err, complete=int(complete and len(listed) == len(words)),
+             covered_bytes=sum(b for _, b in call["chunks"]), n_chunks=len(chunks), elements_done=done, located=len(words),
+             recorded=len(listed), flip_or=sum(1 << b for b in range(64) if flips[b]), pass_=passes, chunk=chunks)
+    return r, listed
 
 
 def forced_mismatches(seed: int, first: int, count: int, and_mask: int, or_mask: int) -> List[Dict]:

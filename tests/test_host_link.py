@@ -36,10 +36,23 @@ def seeds(ctx, k):
     return [(dev + (1 << 62) + (3 * k + j) * STRIDE) & MASK for j in range(3)]
 
 
-@pytest.mark.parametrize("L", [64 * MiB, 256 * MiB, RAGGED], ids=["64MiB", "256MiB", "3MiB+112B"])
-def test_clean_call(cro, coracle, ctx, L):
+# The SM legs' grids beside the default: one CTA, a few, one per SM and the most ctas takes.  At 4096 CTAs and L = 16 B
+# every warp but one has nothing to do and the ragged tail does all the work.
+GRID_SIZES = [(16, "16B"), (4096 + 16, "4KiB+16B"), (RAGGED, "3MiB+112B"), (64 * MiB, "64MiB")]
+GRID_CTAS = [1, 7, "sm_count", 4096]
+GRIDS = [(L, c, "%s-ctas%s" % (name, c)) for L, name in GRID_SIZES for c in GRID_CTAS]
+
+
+def grid(ctx, ctas):
+    return ctx.own_devices()[0].sm_count if ctas == "sm_count" else ctas
+
+
+@pytest.mark.parametrize("L,ctas", [pytest.param(64 * MiB, 0, id="64MiB"), pytest.param(256 * MiB, 0, id="256MiB"),
+                                    pytest.param(RAGGED, 0, id="3MiB+112B")] +
+                         [pytest.param(L, c, id=name) for L, c, name in GRIDS])
+def test_clean_call(cro, coracle, ctx, L, ctas):
     n = L // 8
-    r, faults = ctx.probe_host_link(0, bytes=L)
+    r, faults = ctx.probe_host_link(0, bytes=L, ctas=grid(ctx, ctas))
     assert r.status == cro.OK and r.first_fail == cro.LINK_NO_FAIL and faults == []
     assert r.bytes == L and list(r.seed) == seeds(ctx, r.call)
     want = [coracle.checksum(r.seed[j], 0, n, threads=16) for j in range(3)]
@@ -57,19 +70,23 @@ def test_clean_call(cro, coracle, ctx, L):
     assert r.chase_ns > 0
     ann = json.loads(cro.emit_link_annotations_json(r))
     assert ann["cohdi.io/probe-link-verdict"] == "ok"
-    assert int(ann["cohdi.io/probe-link-h2d-mbps"]) > 0 and int(ann["cohdi.io/probe-link-duplex-mbps"]) > 0
-    r2, _ = ctx.probe_host_link(0, bytes=L)
+    if L >= 4096:          # the rates are whole MB/s: 16 B in the tens of microseconds a leg takes rounds to 0
+        assert int(ann["cohdi.io/probe-link-h2d-mbps"]) > 0 and int(ann["cohdi.io/probe-link-duplex-mbps"]) > 0
+    r2, _ = ctx.probe_host_link(0, bytes=L, ctas=grid(ctx, ctas))
     assert r2.status == cro.OK and r2.call == r.call + 1 and not set(r2.seed) & set(r.seed)
 
 
-@pytest.mark.parametrize("check", range(5))
-@pytest.mark.parametrize("where", ["first", "middle", "last"])
-def test_injected_fault_is_found_where_it_reaches(cro, coracle, ctx, check, where):
-    L = 64 * MiB
+# at the default grid and 64 MiB, every check and place; per grid of GRIDS, the last word of checks 0 and 2 (the SMs
+# read a host buffer there)
+@pytest.mark.parametrize("where,check,L,ctas",
+                         [pytest.param(w, k, 64 * MiB, 0, id="%s-%d" % (w, k)) for w in ["first", "middle", "last"]
+                          for k in range(5)] +
+                         [pytest.param("last", k, L, c, id="last-%d-%s" % (k, name)) for L, c, name in GRIDS for k in (0, 2)])
+def test_injected_fault_is_found_where_it_reaches(cro, coracle, ctx, where, check, L, ctas):
     n = L // 8
     word = {"first": 0, "middle": n // 2 + 3, "last": n - 1}[where]
     mask = (1 << 63) | (1 << 17) | 1
-    r, faults = ctx.probe_host_link(0, bytes=L, inject=(check, word, mask))
+    r, faults = ctx.probe_host_link(0, bytes=L, inject=(check, word, mask), ctas=grid(ctx, ctas))
     assert r.status == cro.ERR_CHECKSUM and r.first_fail == min(REACHES[check])
     assert {f.check for f in faults} == REACHES[check], [(f.check, f.word_index) for f in faults]
     for k in range(cro.LINK_WORD_CHECKS):

@@ -215,6 +215,55 @@ def test_sweep_footprint(cro, coracle, monkeypatch, name, label):
     assert not fails, "\n".join(["S = %d bytes, tile %d, %d stages" % (S, T, D)] + fails)
 
 
+STRADDLE = (1 << 32) - 3              # locate's words 0 .. 5 of an interior from here lie on both sides of 2^32
+HIGH_SIZES = [(16, "16B"), (4096 + 16, "4KiB+16B"), ((3 << 20) + 112, "3MiB+112B"), (64 << 20, "64MiB")]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("n_bytes", [s for s, _ in HIGH_SIZES], ids=[i for _, i in HIGH_SIZES])
+def test_locate_past_word_2_32(cro, coracle, n_bytes):
+    """The LOCATE row at scan indices past 2^32 (an 80 GB scan reaches 2^33): a warp whose words straddle 2^32, a range
+    above it, and the last words below 2^37, the highest index the granule bitmap takes.  Records and granules carry the
+    absolute index; the fold and the compare count from the interior's start."""
+    n = n_bytes // 8
+    want = coracle.checksum(SEED, 0, n, threads=os.cpu_count() or 1)
+    fails = []
+    with cro.ProbeContext(sweep_bytes=1 << 20, devices=[0], flags=cro.F_LAZY_ALLOC, deadline_ms=DEADLINE_MS) as c:
+        for word0 in (STRADDLE, (1 << 32) + (1 << 18), (1 << 37) - n):
+            for invert in (0, MASK):
+                fold = _complement_fold(want, n) if invert else want
+                clean = lambda: _pattern(n) ^ np.uint64(invert)          # noqa: E731
+                name = "locate word0 %#x, invert %#x" % (word0, invert)
+                r = Row(c, name + ", clean", cro.SELFTEST_SWEEP_LOCATE, n_bytes, 0, word0=word0, invert=invert)
+                r.fold(fold)
+                r.counts(0)
+                r.interior(0, clean, fold)
+                fails += r.fails
+                # the first and last words, and at STRADDLE words 0 .. 5 as well
+                ranges = [(0, 6 if word0 == STRADDLE and n >= 6 else 1), (n - 1, 1)]
+                idx = sorted({i for first, count in ranges for i in range(first, first + count)})
+                olds = [oracle.pattern_word(SEED, i) ^ invert for i in idx]
+                changed = [(i, o, _forced(o)) for i, o in zip(idx, olds) if _forced(o) != o]
+                grans = sorted({(word0 + i) * 8 // cro.LOCATE_GRANULE_BYTES for i, _, _ in changed})
+
+                def forced():
+                    w = clean().copy()
+                    w[[i for i, _, _ in changed]] = [f for _, _, f in changed]
+                    return w
+                r = Row(c, name + ", forced %s" % idx, cro.SELFTEST_SWEEP_LOCATE, n_bytes, 0, word0=word0, invert=invert,
+                        force=[(f, k, FORCE_AND, FORCE_OR) for f, k in ranges])
+                r.fold(_changed_fold(fold, changed))
+                r.counts(len(changed), (len(grans), grans[0], grans[-1]))
+                r.interior(0, forced, _changed_fold(fold, changed))
+                got = [(w.word_index, w.expected, w.actual, w.passes) for w in r.words]
+                if got != [(word0 + i, o, f, 1) for i, o, f in changed]:
+                    r.fail("records %s" % [tuple(hex(v) for v in g) for g in got])
+                if word0 == (1 << 37) - n and r.out.granule_max != (1 << 19) - 1:
+                    r.fail("the last granule below 2^37 words is %d" % r.out.granule_max)
+                fails += r.fails
+    assert not fails, "\n".join(fails)
+
+
 @pytest.mark.gpu
 def test_invalid_arguments_are_refused(cro):
     with cro.ProbeContext(sweep_bytes=1 << 20, devices=[0], flags=cro.F_LAZY_ALLOC, deadline_ms=DEADLINE_MS) as c:
