@@ -615,6 +615,42 @@ assert ctypes.sizeof(LinkResult) == 984 and ctypes.sizeof(PciPath) == 272, ctype
 assert ctypes.sizeof(ScanReport) == 12632 and ctypes.sizeof(ScanOpts) == 72, ctypes.sizeof(ScanReport)
 assert ctypes.sizeof(SramResult) == 568 and ctypes.sizeof(SramSm) == 168 and ctypes.sizeof(SramFault) == 48, ctypes.sizeof(SramResult)
 assert ctypes.sizeof(L2Result) == 616 and ctypes.sizeof(L2Sm) == 128 and ctypes.sizeof(L2Fault) == 56, ctypes.sizeof(L2Result)
+# health check (cro_check_health, cro_check_health_uuid): the six checks in one call
+HEALTH_COMPUTE, HEALTH_PRECISION, HEALTH_SRAM, HEALTH_L2, HEALTH_LINK, HEALTH_SCAN = 0x01, 0x02, 0x04, 0x08, 0x10, 0x20
+HEALTH_ALL = 0x3F
+HEALTH_CHECKS = 6
+HEALTH_NAMES = ("compute", "precision", "sram", "l2", "link", "scan")      # bit c, in run order
+
+
+class HealthOpts(ctypes.Structure):
+    """cro_health_opts: the checks to run (0: all) and each check's own options (zeroed: its defaults)."""
+    _fields_ = [("checks", ctypes.c_uint32), ("reserved0", ctypes.c_uint32), ("compute", ComputeOpts),
+                ("precision", PrecisionOpts), ("sram", SramOpts), ("l2", L2Opts), ("link", LinkOpts), ("scan", ScanOpts)]
+
+
+class HealthResult(ctypes.Structure):
+    """cro_health_result: the call's summary and each check's own result."""
+    _fields_ = [("status", ctypes.c_int32), ("checks", ctypes.c_uint32), ("ran", ctypes.c_uint32), ("failed", ctypes.c_uint32),
+                ("errored", ctypes.c_uint32), ("not_run", ctypes.c_uint32), ("incomplete", ctypes.c_uint32),
+                ("reserved0", ctypes.c_uint32), ("check_status", ctypes.c_int32 * HEALTH_CHECKS),
+                ("check_ns", ctypes.c_uint64 * HEALTH_CHECKS), ("seed_base", ctypes.c_uint64), ("helper_ns", ctypes.c_uint64),
+                ("compute", ComputeResult), ("precision", PrecisionResult), ("sram", SramResult), ("l2", L2Result),
+                ("link", LinkResult), ("scan", ScanReport)]
+
+
+# (name, element type) of each list of cro_health_records, in order
+HEALTH_LISTS = [("compute_sms", ComputeSm), ("compute_faults", ComputeFault), ("precision_sms", PrecisionSm),
+                ("precision_faults", PrecisionFault), ("sram_sms", SramSm), ("sram_faults", SramFault), ("l2_sms", L2Sm),
+                ("l2_faults", L2Fault), ("link_faults", LinkFault), ("scan_words", FaultWord)]
+
+
+class HealthRecords(ctypes.Structure):
+    """cro_health_records: the caller's {array, cap, n} per list of records."""
+    _fields_ = [f for name, t in HEALTH_LISTS
+                for f in ((name, ctypes.POINTER(t)), (name + "_cap", ctypes.c_int32), (name + "_n", ctypes.c_int32))]
+
+
+assert ctypes.sizeof(HealthOpts) == 312 and ctypes.sizeof(HealthResult) == 16328 and ctypes.sizeof(HealthRecords) == 160
 assert ctypes.sizeof(SmCta) == 64 and ctypes.sizeof(SramCta) == 128 and ctypes.sizeof(SramRecord) == 40, ctypes.sizeof(SramCta)
 
 # Every symbol include/croprobe.h declares; tests check the library exports all of them.
@@ -646,6 +682,7 @@ EXPORTS = [
     "cro_probe_l2", "cro_probe_l2_uuid", "cro_read_l2_health", "cro_emit_l2_annotations_json", "cro_selftest_l2_classify",
     "cro_selftest_sm_legs_classify", "cro_selftest_sram_classify",
     "cro_selftest_locate_collect", "cro_selftest_scan_collect", "cro_selftest_link_classify",
+    "cro_check_health", "cro_check_health_uuid", "cro_selftest_health_classify", "cro_emit_health_annotations_json",
 ]
 
 # test hooks: the word checks' reports from caller-given device output
@@ -818,6 +855,12 @@ def _load() -> ctypes.CDLL:
                                              ctypes.POINTER(LocateRecord), ctypes.POINTER(u64), ctypes.POINTER(SweepSlot),
                                              ctypes.POINTER(u64), ctypes.POINTER(LinkResult), ctypes.POINTER(LinkFault), i32,
                                              ctypes.POINTER(i32)]),
+        "cro_check_health": (i32, [vp, i32, ctypes.POINTER(HealthOpts), ctypes.POINTER(HealthResult), ctypes.POINTER(HealthRecords)]),
+        "cro_check_health_uuid": (i32, [vp, c, ctypes.POINTER(HealthOpts), i32, ctypes.POINTER(HealthResult),
+                                        ctypes.POINTER(HealthRecords), ctypes.POINTER(u64)]),
+        "cro_selftest_health_classify": (i32, [u32, ctypes.POINTER(ctypes.c_int32), i32, ctypes.POINTER(HealthResult),
+                                               ctypes.POINTER(u32)]),
+        "cro_emit_health_annotations_json": (i32, [ctypes.POINTER(HealthResult)] + out),
         "cro_local_node_op": (i32, [vp, c] + out),
         "cro_local_exec": (i32, [c] + out),
         "cro_describe_wire_type": (i32, [c] + out),
@@ -1301,6 +1344,79 @@ def scan_hbm_uuid(ctx: Optional["ProbeContext"], uuid: str, max_bytes: int = 0, 
     return rep, [arr[i] for i in range(n.value)]
 
 
+def emit_health_annotations_json(r: HealthResult) -> str:
+    """Every ran check's own annotations and the cohdi.io/probe-health-* keys of a health result (one Go-marshalled
+    map[string]string)."""
+    return _text(lib.cro_emit_health_annotations_json, ctypes.byref(r))
+
+
+def selftest_health_classify(checks: int, statuses: List[int]) -> Tuple[HealthResult, int]:
+    """cro_selftest_health_classify: the stop and status rules for the selection `checks` (0: all) after the first
+    len(statuses) checks to run returned `statuses`.  Returns the summary (status, checks, ran, failed, errored, not_run,
+    check_status) and the HEALTH_* bit of the check to run next (0: none is left)."""
+    out, nxt = HealthResult(), ctypes.c_uint32()
+    rc = lib.cro_selftest_health_classify(checks, (ctypes.c_int32 * max(1, len(statuses)))(*statuses), len(statuses),
+                                          ctypes.byref(out), ctypes.byref(nxt))
+    if rc != OK:
+        raise ProbeError(rc, "cro_selftest_health_classify")
+    return out, nxt.value
+
+
+def _health_opts(checks: int, compute=None, precision=None, sram=None, l2=None, link=None, scan=None) -> HealthOpts:
+    """HealthOpts from the checks and each check's options, given as its struct or as a dict of the keyword arguments
+    its own helper form takes (None: defaults)."""
+    o = HealthOpts()
+    o.checks = checks
+    makers = {"compute": lambda a: _compute_opts(a.get("iterations", 0), a.get("alu_iterations", 0), a.get("legs", 0),
+                                                 a.get("max_rounds", 0), a.get("inject")),
+              "precision": lambda a: _precision_opts(a.get("iterations", 0), a.get("alu_iterations", 0), a.get("legs", 0),
+                                                     a.get("max_rounds", 0), a.get("inject")),
+              "sram": lambda a: _sram_opts(a.get("legs", 0), a.get("iterations", 0), a.get("cluster", 0), a.get("max_rounds", 0),
+                                           a.get("deadline_ms", 0), a.get("inject")),
+              "l2": lambda a: _l2_opts(a.get("bytes", 0), a.get("iterations", 0), a.get("a1_counters", 0), a.get("a2_counters", 0),
+                                       a.get("deadline_ms", 0), a.get("inject")),
+              "link": lambda a: _link_opts(a.get("bytes", 0), a.get("hops", 0), a.get("ctas", 0), a.get("inject")),
+              "scan": lambda a: _scan_opts(a.get("max_bytes", 0), a.get("reserve_bytes", 0), a.get("seed", 0), a.get("deadline_ms", 0),
+                                           a.get("chunk_bytes", 0), a.get("force"))}
+    for name, given in (("compute", compute), ("precision", precision), ("sram", sram), ("l2", l2), ("link", link), ("scan", scan)):
+        if given is not None:
+            setattr(o, name, makers[name](given) if isinstance(given, dict) else given)
+    return o
+
+
+def _health_call(fn, head: tuple, tail: tuple, caps: Dict[str, int]):
+    """fn(*head, result, records, *tail) with fresh arrays: caps[name] entries per list (per-SM lists default to
+    every SM, the others to 256).  Returns the return code, the result and {list name: its records}."""
+    r, rec, keep = HealthResult(), HealthRecords(), []
+    for name, t in HEALTH_LISTS:
+        cap = caps.get(name, 256 if not name.endswith("_sms") else COMPUTE_MAX_SMS)
+        arr = (t * max(1, cap))()
+        keep.append(arr)
+        setattr(rec, name, ctypes.cast(arr, ctypes.POINTER(t)))
+        setattr(rec, name + "_cap", cap)
+    rc = fn(*head, ctypes.byref(r), ctypes.byref(rec), *tail)
+    records = {name: [getattr(rec, name)[i] for i in range(getattr(rec, name + "_n"))] for name, _ in HEALTH_LISTS}
+    return rc, r, records
+
+
+def check_health_uuid(ctx: Optional["ProbeContext"], uuid: str, checks: int = 0, compute=None, precision=None, sram=None, l2=None,
+                      link=None, scan=None, deadline_ms: int = 0, caps: Optional[Dict[str, int]] = None
+                      ) -> Tuple[HealthResult, Dict[str, list], int]:
+    """cro_check_health_uuid: the selected checks (0: all six) of any GPU on the node in one helper process (ctx may be
+    None).  Each check's options: its struct, or a dict of the keyword arguments its own helper form takes (None:
+    defaults).  caps: records asked for per list (HEALTH_LISTS names).  Returns the result (its status is OK,
+    ERR_CHECKSUM, or the first other status a check returned), {list name: records} and the helper's spawn-to-exit ns.
+    Raises ProbeError when no check ran: options refused, or no result from the helper."""
+    o = _health_opts(checks, compute, precision, sram, l2, link, scan)
+    ns = ctypes.c_uint64()
+    handle = ctx.handle if ctx is not None else None
+    rc, r, records = _health_call(lib.cro_check_health_uuid, (handle, _b(uuid), ctypes.byref(o), deadline_ms), (ctypes.byref(ns),),
+                                  caps or {})
+    if rc != OK and r.ran == 0:         # refused, or the helper gave no result: no check ran
+        raise _helper_error(rc, handle)
+    return r, records, ns.value
+
+
 def precision_expected(answer: int, seed: int) -> List[int]:
     """cro_precision_expected: the PRECISION_ANSWER_* answer tile of the operands of `seed`, int64 values, row-major
     (PRECISION_M x PRECISION_F64_N for the wide answer, PRECISION_M x PRECISION_N otherwise; host arithmetic, no GPU)."""
@@ -1603,6 +1719,16 @@ class ProbeContext:
         rc, out = _per_sm(lib.cro_probe_l2, (self.handle, dev, ctypes.byref(o)), L2Result, L2Sm, L2_MAX_SMS, L2Fault, cap)
         self._check(rc, allow=(ERR_CHECKSUM, ERR_CUDA))
         return out
+
+    def check_health(self, dev: int = 0, checks: int = 0, compute=None, precision=None, sram=None, l2=None, link=None, scan=None,
+                     caps: Optional[Dict[str, int]] = None) -> Tuple[HealthResult, Dict[str, list]]:
+        """cro_check_health: the selected checks (0: all six) on in-process device `dev`, each through its own in-process
+        call, with the options check_health_uuid takes.  Returns the result and {list name: records}."""
+        o = _health_opts(checks, compute, precision, sram, l2, link, scan)
+        rc, r, records = _health_call(lib.cro_check_health, (self.handle, dev, ctypes.byref(o)), (), caps or {})
+        if r.ran == 0:
+            self._check(rc)
+        return r, records
 
     def launch_count(self) -> int:
         return int(lib.cro_launch_count(self.handle))

@@ -83,6 +83,19 @@ static_assert(sizeof(cro_l2_opts) == 56 && sizeof(cro_l2_health) == 48 && sizeof
                   offsetof(cro_l2_result, bad_line) == 184 && offsetof(cro_l2_result, a1_bad) == 312 &&
                   offsetof(cro_l2_result, element_ns) == 400 && offsetof(cro_l2_result, before) == 520,
               "l2 layout");
+static_assert(sizeof(cro_health_opts) == 312 && offsetof(cro_health_opts, compute) == 8 && offsetof(cro_health_opts, precision) == 48 &&
+                  offsetof(cro_health_opts, sram) == 96 && offsetof(cro_health_opts, l2) == 144 &&
+                  offsetof(cro_health_opts, link) == 200 && offsetof(cro_health_opts, scan) == 240,
+              "health layout");
+static_assert(sizeof(cro_health_result) == 16328 && offsetof(cro_health_result, check_status) == 32 &&
+                  offsetof(cro_health_result, check_ns) == 56 && offsetof(cro_health_result, seed_base) == 104 &&
+                  offsetof(cro_health_result, compute) == 120 && offsetof(cro_health_result, precision) == 720 &&
+                  offsetof(cro_health_result, sram) == 1528 && offsetof(cro_health_result, l2) == 2096 &&
+                  offsetof(cro_health_result, link) == 2712 && offsetof(cro_health_result, scan) == 3696,
+              "health layout");
+static_assert(sizeof(cro_health_records) == 160 && offsetof(cro_health_records, precision_sms) == 32 &&
+                  offsetof(cro_health_records, link_faults) == 128 && offsetof(cro_health_records, scan_words_n) == 156,
+              "health layout");
 static_assert(sizeof(cro_locate_counters) == sizeof(LocateCounters) && offsetof(cro_locate_counters, claims) == offsetof(LocateCounters, claims) &&
                   offsetof(cro_locate_counters, bits) == offsetof(LocateCounters, bits) && sizeof(cro_locate_counters) == 528,
               "cro_locate_counters is the word checks' LocateCounters");
@@ -616,6 +629,83 @@ int cro_selftest_link_classify(uint64_t bytes, const uint64_t* seeds, uint32_t m
     copy_capped(found, faults, cap, n);
     return rc;
 } CRO_API_CATCH
+// The caller's record arrays of a health call: every cap not negative and every array with a cap present.
+static bool records_ok(const cro_health_records* r) {
+    if (!r) return true;
+    const std::pair<const void*, int32_t> lists[] = {
+        {r->compute_sms, r->compute_sms_cap}, {r->compute_faults, r->compute_faults_cap}, {r->precision_sms, r->precision_sms_cap},
+        {r->precision_faults, r->precision_faults_cap}, {r->sram_sms, r->sram_sms_cap}, {r->sram_faults, r->sram_faults_cap},
+        {r->l2_sms, r->l2_sms_cap}, {r->l2_faults, r->l2_faults_cap}, {r->link_faults, r->link_faults_cap},
+        {r->scan_words, r->scan_words_cap}};
+    for (const auto& l : lists)
+        if (l.second < 0 || (l.second > 0 && !l.first)) return false;
+    return true;
+}
+// A health call's records copied out to the caller's arrays (none without them), and what the SRAM, L2 and scan
+// results say the caller got, as their own calls say it.
+static void copy_health(const HealthRecords& v, cro_health_result* out, cro_health_records* r) {
+    cro_health_records none{};
+    if (!r) r = &none;
+    copy_capped(v.compute_sms, r->compute_sms, r->compute_sms_cap, &r->compute_sms_n);
+    copy_capped(v.compute_faults, r->compute_faults, r->compute_faults_cap, &r->compute_faults_n);
+    copy_capped(v.precision_sms, r->precision_sms, r->precision_sms_cap, &r->precision_sms_n);
+    copy_capped(v.precision_faults, r->precision_faults, r->precision_faults_cap, &r->precision_faults_n);
+    const size_t sram_sms = copy_capped(v.sram_sms, r->sram_sms, r->sram_sms_cap, &r->sram_sms_n);
+    const size_t sram_faults = copy_capped(v.sram_faults, r->sram_faults, r->sram_faults_cap, &r->sram_faults_n);
+    const size_t l2_sms = copy_capped(v.l2_sms, r->l2_sms, r->l2_sms_cap, &r->l2_sms_n);
+    const size_t l2_faults = copy_capped(v.l2_faults, r->l2_faults, r->l2_faults_cap, &r->l2_faults_n);
+    copy_capped(v.link_faults, r->link_faults, r->link_faults_cap, &r->link_faults_n);
+    const size_t words = copy_capped(v.scan_words, r->scan_words, r->scan_words_cap, &r->scan_words_n);
+    if (out->ran & CRO_HEALTH_SRAM) listed(PerSmCopy{CRO_OK, true, sram_sms, sram_faults}, &out->sram);
+    if (out->ran & CRO_HEALTH_L2) listed(PerSmCopy{CRO_OK, true, l2_sms, l2_faults}, &out->l2);
+    if (out->ran & CRO_HEALTH_SCAN) {
+        out->scan.complete = out->scan.complete && words == v.scan_words.size();
+        out->scan.recorded = words;
+    }
+}
+int cro_check_health(cro_ctx* ctx, int i, const cro_health_opts* opts, cro_health_result* out, cro_health_records* rec) try {
+    if (!ctx || !out || !records_ok(rec)) return CRO_ERR_INVALID_ARG;
+    cro_health_opts o{};
+    if (opts) o = *opts;
+    const std::string why = health_opts_error(o);
+    if (!why.empty() || i < 0 || i >= (int)ctx->devs.size()) {
+        ctx->set_error(why.empty() ? "health check: device index " + std::to_string(i) + " is not an in-process device" : why);
+        *out = cro_health_result{};
+        out->checks = o.checks ? o.checks : CRO_HEALTH_ALL;
+        return out->status = CRO_ERR_INVALID_ARG;
+    }
+    HealthRecords v;
+    const int rc = ctx_check_health(ctx, i, o, out, &v);
+    copy_health(v, out, rec);
+    return rc;
+} CRO_API_CATCH
+int cro_check_health_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_health_opts* opts, int deadline_ms, cro_health_result* out,
+                          cro_health_records* rec, uint64_t* helper_ns) try {
+    if (!gpu_uuid || !out || !records_ok(rec)) return CRO_ERR_INVALID_ARG;
+    if (helper_ns) *helper_ns = 0;
+    cro_health_opts o{};
+    if (opts) o = *opts;
+    HealthCaps caps{};
+    if (rec)
+        caps = HealthCaps{{rec->compute_faults_cap, rec->precision_faults_cap, rec->sram_faults_cap, rec->l2_faults_cap,
+                           rec->link_faults_cap, rec->scan_words_cap}};
+    HealthRecords v;
+    uint64_t ns = 0;
+    const int rc = ctx_check_health_uuid(ctx, gpu_uuid, o, deadline_ms, caps, out, &v, &ns);
+    copy_health(v, out, rec);
+    if (helper_ns) *helper_ns = ns;
+    return rc;
+} CRO_API_CATCH
+int cro_selftest_health_classify(uint32_t checks, const int32_t* statuses, int n, cro_health_result* out, uint32_t* next) try {
+    if (checks == 0) checks = CRO_HEALTH_ALL;
+    if ((checks & ~CRO_HEALTH_ALL) || n < 0 || (n > 0 && !statuses) || !out || !next) return CRO_ERR_INVALID_ARG;
+    cro_health_result r = *out;
+    const int c = health_step(checks, statuses, n, &r);
+    if (c < 0) return CRO_ERR_INVALID_ARG;
+    *out = r;
+    *next = c < CRO_HEALTH_CHECKS ? 1u << c : 0u;
+    return CRO_OK;
+} CRO_API_CATCH
 int cro_compute_expected(int answer, uint64_t seed, int32_t* out) try {
     return compute::Expected(answer, seed, out);
 } CRO_API_CATCH
@@ -827,14 +917,6 @@ static std::string bit_names(uint32_t mask, const char* const* names, int n) {
 static void put_list(Annotations& m, const std::string& key, const std::string& list) {
     if (!list.empty()) m[key] = list;
 }
-// The least sms_covered over the legs run: the "sms" key's numerator, 0 when no leg ran.
-template <class Leg>
-static uint32_t min_covered(uint32_t legs, const Leg* leg, int n_legs) {
-    uint32_t covered = 0xFFFFFFFFu;
-    for (int l = 0; l < n_legs; ++l)
-        if (legs >> l & 1u) covered = std::min(covered, leg[l].sms_covered);
-    return covered == 0xFFFFFFFFu ? 0u : covered;
-}
 // How much each ECC count grew over the call, for a count NVML gave both before and after it.
 template <class Health>
 static void ecc_delta(Annotations& m, const std::string& p, const Health& B, const Health& A, uint32_t corrected_bit,
@@ -851,8 +933,8 @@ struct LegRate {
     const char* key;
 };
 template <class Result>
-static int emit_sm_legs(const Result& r, const std::string& p, const char* const* leg_name, int n_legs,
-                        std::initializer_list<LegRate> rates, char* buf, size_t cap, size_t* len) {
+static Annotations sm_legs_annotations(const Result& r, const std::string& p, const char* const* leg_name, int n_legs,
+                                       std::initializer_list<LegRate> rates) {
     Annotations m;
     m[p + "verdict"] = r.status == CRO_OK                                               ? "ok"
                        : r.status == CRO_ERR_CHECKSUM && r.verdict == CRO_COMPUTE_SM  ? "sm"
@@ -875,7 +957,7 @@ static int emit_sm_legs(const Result& r, const std::string& p, const char* const
     }
     if (worst < n_legs)
         m[p + "slowest-sm"] = std::to_string(r.leg[worst].slowest_sm) + " " + std::to_string(r.leg[worst].slow_permille);
-    return emit(m, buf, cap, len);
+    return m;
 }
 
 std::map<std::string, std::string> cro::capi::probe_annotations(const cro_probe_result& r) {
@@ -913,6 +995,160 @@ std::map<std::string, std::string> cro::capi::probe_annotations(const cro_probe_
     return m;
 }
 
+static std::string link_speed(uint32_t tenths) {
+    if (!tenths) return "unknown";
+    return std::to_string(tenths / 10) + "." + std::to_string(tenths % 10) + "GT/s";
+}
+static std::string mbps(uint64_t bytes, uint64_t ns) {
+    // bytes * 1000 / ns without overflow: 128-bit intermediate
+    return std::to_string(ns ? (uint64_t)((unsigned __int128)bytes * 1000u / ns) : 0ull);
+}
+
+static Annotations link_annotations(const cro_link_result& r) {
+    static const char* const kCheck[CRO_LINK_CHECKS] = {"d2h-copy", "h2d-copy", "sm-write", "duplex-write", "duplex-d2h-copy",
+                                                         "chase"};
+    static const char* const kDegraded[4] = {"speed", "width", "path", "bottleneck"};
+    Annotations m;
+    const std::string p = "cohdi.io/probe-link-";
+    m[p + "verdict"] = r.first_fail < CRO_LINK_CHECKS ? std::string("corrupt:") + kCheck[r.first_fail]
+                       : r.status == CRO_OK       ? "ok"
+                                                   : "error";
+    const cro_link_leg* L = r.leg;
+    m[p + "h2d-mbps"] = mbps(L[CRO_LINK_LEG_CE_H2D].bytes, L[CRO_LINK_LEG_CE_H2D].ns);
+    m[p + "d2h-mbps"] = mbps(L[CRO_LINK_LEG_CE_D2H].bytes, L[CRO_LINK_LEG_CE_D2H].ns);
+    m[p + "duplex-mbps"] = mbps(L[CRO_LINK_LEG_CE_DUPLEX_H2D].bytes + L[CRO_LINK_LEG_CE_DUPLEX_D2H].bytes, r.ce_duplex_span_ns);
+    m[p + "sm-h2d-mbps"] = mbps(L[CRO_LINK_LEG_SM_H2D].bytes, L[CRO_LINK_LEG_SM_H2D].ns);
+    m[p + "sm-d2h-mbps"] = mbps(L[CRO_LINK_LEG_SM_D2H].bytes, L[CRO_LINK_LEG_SM_D2H].ns);
+    m[p + "latency-ns"] = std::to_string(r.chase_hops ? r.chase_ns / r.chase_hops : 0ull);
+    const cro_pci_hop& g = r.path.hop[0];
+    m[p + "link"] = link_speed(g.cur_speed) + " x" + std::to_string(g.cur_width) + " / " + link_speed(g.max_speed) + " x" +
+                    std::to_string(g.max_width);
+    if ((r.degraded & CRO_LINK_DEGRADED_BOTTLENECK) && r.path.bottleneck < CRO_PCI_MAX_HOPS) {
+        const cro_pci_hop& b = r.path.hop[r.path.bottleneck];
+        m[p + "bottleneck"] = std::string(b.bdf, strnlen(b.bdf, sizeof b.bdf)) + " " + link_speed(b.cur_speed) + " x" +
+                              std::to_string(b.cur_width);
+    }
+    put_list(m, p + "degraded", bit_names(r.degraded, kDegraded, 4));
+    if (!r.no_nvml) m[p + "replays"] = std::to_string(r.replays_after - r.replays_before);
+    return m;
+}
+
+static Annotations scan_annotations(const cro_scan_report& r) {
+    static const char* const kHealth[4] = {"ecc-corrected", "ecc-uncorrected", "remap-pending", "remap-failure"};
+    Annotations m;
+    const std::string p = "cohdi.io/hbm-scan-";
+    m[p + "verdict"] = r.status == CRO_OK            ? "ok"
+                       : r.status == CRO_ERR_CHECKSUM ? "corrupt"
+                       : r.status == CRO_ERR_CUDA     ? cuda_error(r.cuda_error)
+                                                       : "error";
+    m[p + "covered-bytes"] = std::to_string(r.covered_bytes);
+    m[p + "free-bytes"] = std::to_string(r.free_bytes);
+    m[p + "seed"] = hex16(r.seed);
+    m[p + "mismatches"] = std::to_string(r.pass[0].mismatches) + "," + std::to_string(r.pass[1].mismatches);
+    m[p + "granules"] = std::to_string(r.pass[0].granules) + "," + std::to_string(r.pass[1].granules);
+    uint64_t ns = 0;
+    for (uint64_t e : r.element_ns) ns += e;
+    m[p + "gbs"] = std::to_string(ns ? (uint64_t)((unsigned __int128)r.covered_bytes * 4u / ns) : 0ull);
+    put_list(m, p + "bits", bit_numbers([&](int b) { return r.pass[0].bit_flips[b] || r.pass[1].bit_flips[b]; }));
+    put_list(m, p + "health", bit_names(r.health, kHealth, 4));
+    const cro_hbm_health& A = r.after;
+    ecc_delta(m, p, r.before, A, CRO_HBM_NVML_ECC_CORRECTED, CRO_HBM_NVML_ECC_UNCORRECTED);
+    if (A.nvml & CRO_HBM_NVML_REMAP) m[p + "remapped"] = std::to_string(A.remap_corrected) + "," + std::to_string(A.remap_uncorrected);
+    if (A.nvml & CRO_HBM_NVML_HISTOGRAM) m[p + "remap-histogram"] = join(A.histogram, 5);
+    return m;
+}
+
+static Annotations sram_annotations(const cro_sram_result& r) {
+    static const char* const kHealth[3] = {"corrected", "uncorrected", "threshold-exceeded"};
+    Annotations m;
+    const std::string p = "cohdi.io/probe-sram-";
+    m[p + "verdict"] = r.status == CRO_OK                                                ? "ok"
+                       : r.status == CRO_ERR_CHECKSUM && r.verdict == CRO_SRAM_SM   ? "sm"
+                       : r.status == CRO_ERR_CHECKSUM && r.verdict == CRO_SRAM_LINK ? "link"
+                       : r.status == CRO_ERR_CHECKSUM && r.verdict == CRO_SRAM_ALL  ? "all"
+                       : r.status == CRO_ERR_CUDA ? cuda_error(r.cuda_error)
+                                                   : "error";
+    m[p + "sms"] = std::to_string(min_covered(r.legs, r.leg, CRO_SRAM_LEGS)) + "/" + std::to_string(r.sm_count);
+    if (r.bad_sms) m[p + "bad-sms"] = join(r.bad_sm, std::min<uint32_t>(r.bad_sms, 16));
+    if (r.bad_pairs)
+        m[p + "bad-pairs"] = join(std::min<uint32_t>(r.bad_pairs, CRO_SRAM_MAX_PAIRS), [&](uint64_t j) {
+            const cro_sram_pair& q = r.bad_pair[j];
+            return std::to_string(q.from) + "-" + std::to_string(q.owner) + (q.direction == CRO_SRAM_DIR_READ ? ":r" : ":w");
+        });
+    m[p + "bytes-per-sm"] = std::to_string(r.bytes_per_sm);
+    put_list(m, p + "health", bit_names(r.health, kHealth, 3));
+    ecc_delta(m, p, r.before, r.after, CRO_SRAM_NVML_ECC_CORRECTED, CRO_SRAM_NVML_ECC_UNCORRECTED);
+    return m;
+}
+
+static Annotations l2_annotations(const cro_l2_result& r) {
+    static const char* const kHealth[6] = {"sram-corrected", "sram-uncorrected", "l2-corrected", "l2-uncorrected",
+                                           "threshold-exceeded", "l2-bucket"};
+    static const char* const kVerdict[5] = {"", "sm", "line", "atomic", "all"};
+    Annotations m;
+    const std::string p = "cohdi.io/probe-l2-";
+    m[p + "verdict"] = r.status == CRO_OK                                                           ? "ok"
+                       : r.status == CRO_ERR_CHECKSUM && r.verdict >= 1 && r.verdict <= CRO_L2_ALL ? kVerdict[r.verdict]
+                       : r.status == CRO_ERR_CUDA ? cuda_error(r.cuda_error)
+                                                   : "error";
+    m[p + "sms"] = std::to_string(r.sms_covered) + "/" + std::to_string(r.sm_count);
+    m[p + "bytes"] = std::to_string(r.bytes);
+    m[p + "iterations"] = std::to_string(r.iterations);
+    m[p + "march-gbs"] = std::to_string(r.march_ns ? r.march_bytes / r.march_ns : 0ull);
+    if (r.bad_sms) m[p + "bad-sms"] = join(r.bad_sm, std::min<uint64_t>(r.bad_sms, 16));
+    if (r.bad_lines) m[p + "bad-lines"] = join(r.bad_line, std::min<uint64_t>(r.bad_lines, CRO_L2_MAX_LINES));
+    if (r.a1_bad) m[p + "a1-bad-counters"] = join(r.a1_bad_counter, std::min<uint64_t>(r.a1_bad, CRO_L2_MAX_COUNTERS));
+    if (r.a2_bad) m[p + "a2-bad-counters"] = join(r.a2_bad_counter, std::min<uint64_t>(r.a2_bad, CRO_L2_MAX_COUNTERS));
+    if (r.a2_holes) m[p + "a2-holes"] = std::to_string(r.a2_holes);
+    if (r.overflow) m[p + "overflow"] = "1";
+    put_list(m, p + "health", bit_names(r.health, kHealth, 6));
+    return m;
+}
+
+static Annotations compute_annotations(const cro_compute_result& r) {
+    static const char* const kLeg[CRO_COMPUTE_LEGS] = {"s8", "bf16", "e4m3", "ffma", "imad"};
+    return sm_legs_annotations(r, "cohdi.io/probe-compute-", kLeg, CRO_COMPUTE_LEGS,
+                               {{CRO_COMPUTE_LEG_S8, "s8-gops"}, {CRO_COMPUTE_LEG_BF16, "bf16-gflops"}, {CRO_COMPUTE_LEG_E4M3, "e4m3-gflops"}});
+}
+
+static Annotations precision_annotations(const cro_precision_result& r) {
+    static const char* const kLeg[CRO_PRECISION_LEGS] = {"f64", "dfma", "tf32", "f16", "f16acc", "e5m2", "hfma2"};
+    return sm_legs_annotations(r, "cohdi.io/probe-precision-", kLeg, CRO_PRECISION_LEGS,
+                               {{CRO_PRECISION_LEG_F64, "f64-gflops"}, {CRO_PRECISION_LEG_TF32, "tf32-gflops"},
+                                {CRO_PRECISION_LEG_F16, "f16-gflops"}, {CRO_PRECISION_LEG_F16ACC, "f16acc-gflops"},
+                                {CRO_PRECISION_LEG_E5M2, "e5m2-gflops"}});
+}
+
+// The health check's annotations: each check that ran, its own keys unchanged, and the call's cohdi.io/probe-health-*.
+static Annotations health_annotations(const cro_health_result& r) {
+    static const char* const kName[CRO_HEALTH_CHECKS] = {"compute", "precision", "sram", "l2", "link", "scan"};
+    const int32_t cuda[CRO_HEALTH_CHECKS] = {0, 0, r.sram.cuda_error, r.l2.cuda_error, 0, r.scan.cuda_error};
+    Annotations m;
+    auto add = [&](const Annotations& a) { m.insert(a.begin(), a.end()); };
+    if (r.ran & CRO_HEALTH_COMPUTE) add(compute_annotations(r.compute));
+    if (r.ran & CRO_HEALTH_PRECISION) add(precision_annotations(r.precision));
+    if (r.ran & CRO_HEALTH_SRAM) add(sram_annotations(r.sram));
+    if (r.ran & CRO_HEALTH_L2) add(l2_annotations(r.l2));
+    if (r.ran & CRO_HEALTH_LINK) add(link_annotations(r.link));
+    if (r.ran & CRO_HEALTH_SCAN) add(scan_annotations(r.scan));
+    const std::string p = "cohdi.io/probe-health-";
+    std::string verdict = r.status == CRO_OK ? "ok" : r.status == CRO_ERR_CHECKSUM ? "fail" : "error";
+    for (int c = 0; c < CRO_HEALTH_CHECKS && r.status == CRO_ERR_CUDA; ++c)
+        if ((r.ran >> c & 1u) && r.check_status[c] == CRO_ERR_CUDA) {
+            verdict = cuda_error(cuda[c]);
+            break;
+        }
+    m[p + "verdict"] = verdict;
+    put_list(m, p + "failed", bit_names(r.failed, kName, CRO_HEALTH_CHECKS));
+    put_list(m, p + "errors", bit_names(r.errored, kName, CRO_HEALTH_CHECKS));
+    put_list(m, p + "not-run", bit_names(r.not_run, kName, CRO_HEALTH_CHECKS));
+    put_list(m, p + "incomplete", bit_names(r.incomplete, kName, CRO_HEALTH_CHECKS));
+    uint64_t ns = r.helper_ns;
+    for (int c = 0; c < CRO_HEALTH_CHECKS && !r.helper_ns; ++c) ns += r.check_ns[c];
+    m[p + "ms"] = std::to_string(ns / 1000000u);
+    return m;
+}
+
 extern "C" {
 
 int cro_emit_probe_annotations_json(const cro_probe_result* r, char* buf, size_t cap, size_t* len) try {
@@ -940,136 +1176,39 @@ int cro_emit_fault_annotations_json(const cro_fault_report* r, const cro_fault_w
     return emit(m, buf, cap, len);
 } CRO_API_CATCH
 
-static std::string link_speed(uint32_t tenths) {
-    if (!tenths) return "unknown";
-    return std::to_string(tenths / 10) + "." + std::to_string(tenths % 10) + "GT/s";
-}
-static std::string mbps(uint64_t bytes, uint64_t ns) {
-    // bytes * 1000 / ns without overflow: 128-bit intermediate
-    return std::to_string(ns ? (uint64_t)((unsigned __int128)bytes * 1000u / ns) : 0ull);
-}
-
 int cro_emit_link_annotations_json(const cro_link_result* r, char* buf, size_t cap, size_t* len) try {
     if (!r) return CRO_ERR_INVALID_ARG;
-    static const char* const kCheck[CRO_LINK_CHECKS] = {"d2h-copy", "h2d-copy", "sm-write", "duplex-write", "duplex-d2h-copy",
-                                                         "chase"};
-    static const char* const kDegraded[4] = {"speed", "width", "path", "bottleneck"};
-    Annotations m;
-    const std::string p = "cohdi.io/probe-link-";
-    m[p + "verdict"] = r->first_fail < CRO_LINK_CHECKS ? std::string("corrupt:") + kCheck[r->first_fail]
-                       : r->status == CRO_OK       ? "ok"
-                                                   : "error";
-    const cro_link_leg* L = r->leg;
-    m[p + "h2d-mbps"] = mbps(L[CRO_LINK_LEG_CE_H2D].bytes, L[CRO_LINK_LEG_CE_H2D].ns);
-    m[p + "d2h-mbps"] = mbps(L[CRO_LINK_LEG_CE_D2H].bytes, L[CRO_LINK_LEG_CE_D2H].ns);
-    m[p + "duplex-mbps"] = mbps(L[CRO_LINK_LEG_CE_DUPLEX_H2D].bytes + L[CRO_LINK_LEG_CE_DUPLEX_D2H].bytes, r->ce_duplex_span_ns);
-    m[p + "sm-h2d-mbps"] = mbps(L[CRO_LINK_LEG_SM_H2D].bytes, L[CRO_LINK_LEG_SM_H2D].ns);
-    m[p + "sm-d2h-mbps"] = mbps(L[CRO_LINK_LEG_SM_D2H].bytes, L[CRO_LINK_LEG_SM_D2H].ns);
-    m[p + "latency-ns"] = std::to_string(r->chase_hops ? r->chase_ns / r->chase_hops : 0ull);
-    const cro_pci_hop& g = r->path.hop[0];
-    m[p + "link"] = link_speed(g.cur_speed) + " x" + std::to_string(g.cur_width) + " / " + link_speed(g.max_speed) + " x" +
-                    std::to_string(g.max_width);
-    if ((r->degraded & CRO_LINK_DEGRADED_BOTTLENECK) && r->path.bottleneck < CRO_PCI_MAX_HOPS) {
-        const cro_pci_hop& b = r->path.hop[r->path.bottleneck];
-        m[p + "bottleneck"] = std::string(b.bdf, strnlen(b.bdf, sizeof b.bdf)) + " " + link_speed(b.cur_speed) + " x" +
-                              std::to_string(b.cur_width);
-    }
-    put_list(m, p + "degraded", bit_names(r->degraded, kDegraded, 4));
-    if (!r->no_nvml) m[p + "replays"] = std::to_string(r->replays_after - r->replays_before);
-    return emit(m, buf, cap, len);
+    return emit(link_annotations(*r), buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_compute_annotations_json(const cro_compute_result* r, char* buf, size_t cap, size_t* len) try {
-    static const char* const kLeg[CRO_COMPUTE_LEGS] = {"s8", "bf16", "e4m3", "ffma", "imad"};
     if (!r) return CRO_ERR_INVALID_ARG;
-    return emit_sm_legs(*r, "cohdi.io/probe-compute-", kLeg, CRO_COMPUTE_LEGS,
-                        {{CRO_COMPUTE_LEG_S8, "s8-gops"}, {CRO_COMPUTE_LEG_BF16, "bf16-gflops"}, {CRO_COMPUTE_LEG_E4M3, "e4m3-gflops"}},
-                        buf, cap, len);
+    return emit(compute_annotations(*r), buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_precision_annotations_json(const cro_precision_result* r, char* buf, size_t cap, size_t* len) try {
-    static const char* const kLeg[CRO_PRECISION_LEGS] = {"f64", "dfma", "tf32", "f16", "f16acc", "e5m2", "hfma2"};
     if (!r) return CRO_ERR_INVALID_ARG;
-    return emit_sm_legs(*r, "cohdi.io/probe-precision-", kLeg, CRO_PRECISION_LEGS,
-                        {{CRO_PRECISION_LEG_F64, "f64-gflops"}, {CRO_PRECISION_LEG_TF32, "tf32-gflops"},
-                         {CRO_PRECISION_LEG_F16, "f16-gflops"}, {CRO_PRECISION_LEG_F16ACC, "f16acc-gflops"},
-                         {CRO_PRECISION_LEG_E5M2, "e5m2-gflops"}},
-                        buf, cap, len);
+    return emit(precision_annotations(*r), buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_scan_annotations_json(const cro_scan_report* r, char* buf, size_t cap, size_t* len) try {
     if (!r) return CRO_ERR_INVALID_ARG;
-    static const char* const kHealth[4] = {"ecc-corrected", "ecc-uncorrected", "remap-pending", "remap-failure"};
-    Annotations m;
-    const std::string p = "cohdi.io/hbm-scan-";
-    m[p + "verdict"] = r->status == CRO_OK            ? "ok"
-                       : r->status == CRO_ERR_CHECKSUM ? "corrupt"
-                       : r->status == CRO_ERR_CUDA     ? cuda_error(r->cuda_error)
-                                                       : "error";
-    m[p + "covered-bytes"] = std::to_string(r->covered_bytes);
-    m[p + "free-bytes"] = std::to_string(r->free_bytes);
-    m[p + "seed"] = hex16(r->seed);
-    m[p + "mismatches"] = std::to_string(r->pass[0].mismatches) + "," + std::to_string(r->pass[1].mismatches);
-    m[p + "granules"] = std::to_string(r->pass[0].granules) + "," + std::to_string(r->pass[1].granules);
-    uint64_t ns = 0;
-    for (uint64_t e : r->element_ns) ns += e;
-    m[p + "gbs"] = std::to_string(ns ? (uint64_t)((unsigned __int128)r->covered_bytes * 4u / ns) : 0ull);
-    put_list(m, p + "bits", bit_numbers([&](int b) { return r->pass[0].bit_flips[b] || r->pass[1].bit_flips[b]; }));
-    put_list(m, p + "health", bit_names(r->health, kHealth, 4));
-    const cro_hbm_health& A = r->after;
-    ecc_delta(m, p, r->before, A, CRO_HBM_NVML_ECC_CORRECTED, CRO_HBM_NVML_ECC_UNCORRECTED);
-    if (A.nvml & CRO_HBM_NVML_REMAP) m[p + "remapped"] = std::to_string(A.remap_corrected) + "," + std::to_string(A.remap_uncorrected);
-    if (A.nvml & CRO_HBM_NVML_HISTOGRAM) m[p + "remap-histogram"] = join(A.histogram, 5);
-    return emit(m, buf, cap, len);
+    return emit(scan_annotations(*r), buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_sram_annotations_json(const cro_sram_result* r, char* buf, size_t cap, size_t* len) try {
     if (!r) return CRO_ERR_INVALID_ARG;
-    static const char* const kHealth[3] = {"corrected", "uncorrected", "threshold-exceeded"};
-    Annotations m;
-    const std::string p = "cohdi.io/probe-sram-";
-    m[p + "verdict"] = r->status == CRO_OK                                                ? "ok"
-                       : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_SRAM_SM   ? "sm"
-                       : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_SRAM_LINK ? "link"
-                       : r->status == CRO_ERR_CHECKSUM && r->verdict == CRO_SRAM_ALL  ? "all"
-                       : r->status == CRO_ERR_CUDA ? cuda_error(r->cuda_error)
-                                                   : "error";
-    m[p + "sms"] = std::to_string(min_covered(r->legs, r->leg, CRO_SRAM_LEGS)) + "/" + std::to_string(r->sm_count);
-    if (r->bad_sms) m[p + "bad-sms"] = join(r->bad_sm, std::min<uint32_t>(r->bad_sms, 16));
-    if (r->bad_pairs)
-        m[p + "bad-pairs"] = join(std::min<uint32_t>(r->bad_pairs, CRO_SRAM_MAX_PAIRS), [&](uint64_t j) {
-            const cro_sram_pair& q = r->bad_pair[j];
-            return std::to_string(q.from) + "-" + std::to_string(q.owner) + (q.direction == CRO_SRAM_DIR_READ ? ":r" : ":w");
-        });
-    m[p + "bytes-per-sm"] = std::to_string(r->bytes_per_sm);
-    put_list(m, p + "health", bit_names(r->health, kHealth, 3));
-    ecc_delta(m, p, r->before, r->after, CRO_SRAM_NVML_ECC_CORRECTED, CRO_SRAM_NVML_ECC_UNCORRECTED);
-    return emit(m, buf, cap, len);
+    return emit(sram_annotations(*r), buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_l2_annotations_json(const cro_l2_result* r, char* buf, size_t cap, size_t* len) try {
     if (!r) return CRO_ERR_INVALID_ARG;
-    static const char* const kHealth[6] = {"sram-corrected", "sram-uncorrected", "l2-corrected", "l2-uncorrected",
-                                           "threshold-exceeded", "l2-bucket"};
-    static const char* const kVerdict[5] = {"", "sm", "line", "atomic", "all"};
-    Annotations m;
-    const std::string p = "cohdi.io/probe-l2-";
-    m[p + "verdict"] = r->status == CRO_OK                                                           ? "ok"
-                       : r->status == CRO_ERR_CHECKSUM && r->verdict >= 1 && r->verdict <= CRO_L2_ALL ? kVerdict[r->verdict]
-                       : r->status == CRO_ERR_CUDA ? cuda_error(r->cuda_error)
-                                                   : "error";
-    m[p + "sms"] = std::to_string(r->sms_covered) + "/" + std::to_string(r->sm_count);
-    m[p + "bytes"] = std::to_string(r->bytes);
-    m[p + "iterations"] = std::to_string(r->iterations);
-    m[p + "march-gbs"] = std::to_string(r->march_ns ? r->march_bytes / r->march_ns : 0ull);
-    if (r->bad_sms) m[p + "bad-sms"] = join(r->bad_sm, std::min<uint64_t>(r->bad_sms, 16));
-    if (r->bad_lines) m[p + "bad-lines"] = join(r->bad_line, std::min<uint64_t>(r->bad_lines, CRO_L2_MAX_LINES));
-    if (r->a1_bad) m[p + "a1-bad-counters"] = join(r->a1_bad_counter, std::min<uint64_t>(r->a1_bad, CRO_L2_MAX_COUNTERS));
-    if (r->a2_bad) m[p + "a2-bad-counters"] = join(r->a2_bad_counter, std::min<uint64_t>(r->a2_bad, CRO_L2_MAX_COUNTERS));
-    if (r->a2_holes) m[p + "a2-holes"] = std::to_string(r->a2_holes);
-    if (r->overflow) m[p + "overflow"] = "1";
-    put_list(m, p + "health", bit_names(r->health, kHealth, 6));
-    return emit(m, buf, cap, len);
+    return emit(l2_annotations(*r), buf, cap, len);
+} CRO_API_CATCH
+
+int cro_emit_health_annotations_json(const cro_health_result* r, char* buf, size_t cap, size_t* len) try {
+    if (!r) return CRO_ERR_INVALID_ARG;
+    return emit(health_annotations(*r), buf, cap, len);
 } CRO_API_CATCH
 
 int cro_fm_parse_scale_up_response(const char* body, const char* resource_name, const char* res_type,

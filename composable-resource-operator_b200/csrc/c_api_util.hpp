@@ -52,6 +52,16 @@ inline std::string hex16(uint64_t v) {
 int on_exception() noexcept;
 #define CRO_API_CATCH catch (...) { return ::cro::capi::on_exception(); }
 
+// The least sms_covered over the legs run: the "sms" annotation's numerator and what makes a health check incomplete;
+// 0 when no leg ran.
+template <class Leg>
+uint32_t min_covered(uint32_t legs, const Leg* leg, int n_legs) {
+    uint32_t covered = 0xFFFFFFFFu;
+    for (int l = 0; l < n_legs; ++l)
+        if (legs >> l & 1u) covered = covered < leg[l].sms_covered ? covered : leg[l].sms_covered;
+    return covered == 0xFFFFFFFFu ? 0u : covered;
+}
+
 // cohdi.io/probe-* annotations of one result (defined in c_api.cu)
 std::map<std::string, std::string> probe_annotations(const cro_probe_result& r);
 

@@ -59,6 +59,8 @@ int ctx_probe_compute(cro_ctx* c, int idx, const cro_compute_opts& o, cro_comput
     return probe_sm_legs<ComputeProbe>(c, idx, o, r, sms, faults);
 }
 
+std::string compute_opts_error(const cro_compute_opts& o) { return ComputeProbe::opts_error(o); }
+
 int ctx_probe_compute_uuid(cro_ctx* c, const char* uuid, const cro_compute_opts& o, int deadline_ms, cro_compute_result* r,
                            std::vector<cro_compute_sm>* sms, std::vector<cro_compute_fault>* faults, int cap, uint64_t* helper_ns) {
     return probe_sm_legs_uuid<ComputeProbe>(c, uuid, o, deadline_ms, r, sms, faults, cap, helper_ns);

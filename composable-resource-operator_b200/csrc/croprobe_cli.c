@@ -47,7 +47,14 @@
  *                                                    for its health record; cro_l2_result, uint64_t n_sms and n,
  *                                                    CRO_L2_MAX_SMS cro_l2_sm entries (n_sms of them filled), then n
  *                                                    cro_l2_fault records (at most cap) on stdout
- *   link-raw, compute-raw, precision-raw and l2-raw take cro_opts.seed_base from argv (the device seed is seed_base | minor, as in process), so
+ *   croprobe-cli health-raw <uuid> <seed_base> <checks> <compute-raw's options and cap> <precision-raw's> <sram-raw's>
+ *                           <l2-raw's> <link-raw's> <scan-raw's>
+ *                                                    the health check (cro_check_health) with every option of every
+ *                                                    check, each as its own -raw command takes them after the uuid (and
+ *                                                    the seed base), its sweep region L, NVML on; the cro_health_result,
+ *                                                    then each check that ran, in run order, as its own -raw writes it
+ *   croprobe-cli health <uuid|index>                 the health check with defaults; JSON annotations, exit 0 iff ok
+ *   link-raw, compute-raw, precision-raw, l2-raw and health-raw take cro_opts.seed_base from argv (the device seed is seed_base | minor, as in process), so
  *   that the library can give every helper call fresh patterns and operands; their counts are the helper's own,
  *   because neither result says how many records follow.
  * Exit 3: the device is not visible to this (fresh) process — the reference's found=false.  The raw commands exit 0
@@ -80,48 +87,130 @@ static int fail(cro_ctx *ctx, const char *what, int rc) {
 
 static char buf[1 << 16];
 
-/* A raw command's stdout, the result whatever its status (the library reads why from it): the result, n_counts counts
- * of the helper's own, the per-SM block and n records of rec_bytes each, the empty parts left out.  Then it exits 0 iff
- * the status is CRO_OK and 1 for any other, skipping the teardown (it costs as much as a probe): the process's buffers
- * and allocations go with it.  2 when stdout takes less. */
-static int write_frame(const void *result, size_t result_bytes, const uint64_t *counts, size_t n_counts, const void *sms,
-                       size_t sms_bytes, const void *records, size_t rec_bytes, int n, int status) {
+/* A raw command's stdout, the result whatever its status (the library reads why from it): one frame per result, each
+ * the result, n_counts counts of the helper's own, the per-SM block and n records of rec_bytes each, the empty parts
+ * left out (put_frame: 0, or 2 when stdout takes less).  Then end_frames exits 0 iff the status is CRO_OK and 1 for any
+ * other, skipping the teardown (it costs as much as a probe): the process's buffers and allocations go with it. */
+static int put_frame(const void *result, size_t result_bytes, const uint64_t *counts, size_t n_counts, const void *sms,
+                     size_t sms_bytes, const void *records, size_t rec_bytes, int n) {
     if (fwrite(result, result_bytes, 1, stdout) != 1 || (n_counts && fwrite(counts, sizeof *counts, n_counts, stdout) != n_counts) ||
         (sms_bytes && fwrite(sms, sms_bytes, 1, stdout) != 1) || (n > 0 && fwrite(records, rec_bytes, (size_t)n, stdout) != (size_t)n))
         return 2;
+    return 0;
+}
+static int end_frames(int status) {
     fflush(stdout);
     _exit(status == CRO_OK ? 0 : 1);
+}
+
+/* Each check's frame, as its -raw command and health-raw write it: compute, precision and L2 with the counts n_sms and
+ * n and the whole per-SM block, SRAM with the block (the result says how many records follow), link with n, the scan
+ * with its words only. */
+static int put_compute(const cro_compute_result *r, const cro_compute_sm *sms, int n_sms, const cro_compute_fault *f, int n) {
+    const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)n};
+    return put_frame(r, sizeof *r, counts, 2, sms, CRO_COMPUTE_MAX_SMS * sizeof *sms, f, sizeof *f, n);
+}
+static int put_precision(const cro_precision_result *r, const cro_precision_sm *sms, int n_sms, const cro_precision_fault *f,
+                         int n) {
+    const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)n};
+    return put_frame(r, sizeof *r, counts, 2, sms, CRO_PRECISION_MAX_SMS * sizeof *sms, f, sizeof *f, n);
+}
+static int put_l2(const cro_l2_result *r, const cro_l2_sm *sms, int n_sms, const cro_l2_fault *f, int n) {
+    const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)n};
+    return put_frame(r, sizeof *r, counts, 2, sms, CRO_L2_MAX_SMS * sizeof *sms, f, sizeof *f, n);
+}
+static int put_sram(const cro_sram_result *r, const cro_sram_sm *sms, const cro_sram_fault *f, int n) {
+    return put_frame(r, sizeof *r, NULL, 0, sms, CRO_SRAM_MAX_SMS * sizeof *sms, f, sizeof *f, n);
+}
+static int put_link(const cro_link_result *r, const cro_link_fault *f, int n) {
+    const uint64_t n_out = (uint64_t)n;
+    return put_frame(r, sizeof *r, &n_out, 1, NULL, 0, f, sizeof *f, n);
+}
+static int put_scan(const cro_scan_report *r, const cro_fault_word *w, int n) {
+    return put_frame(r, sizeof *r, NULL, 0, NULL, 0, w, sizeof *w, n);
+}
+
+/* Each check's options from argv, a[0] its first, in the order its -raw command takes them. */
+static void scan_opts_at(char **a, cro_scan_opts *so) {
+    uint64_t *f[] = {&so->max_bytes, &so->reserve_bytes, &so->seed, &so->test_chunk_bytes, &so->test_force_first,
+                     &so->test_force_count, &so->test_force_and, &so->test_force_or};
+    for (int k = 0; k < 8; ++k) *f[k] = (uint64_t)strtoull(a[k], NULL, 10);
+}
+static void sram_opts_at(char **a, cro_sram_opts *so) {
+    so->legs = (uint32_t)strtoul(a[0], NULL, 10);
+    so->iterations = (uint32_t)strtoul(a[1], NULL, 10);
+    so->cluster = (uint32_t)strtoul(a[2], NULL, 10);
+    so->max_rounds = (uint32_t)strtoul(a[3], NULL, 10);
+    so->test_inject_leg = atoi(a[4]);
+    so->test_inject_sm = atoi(a[5]);
+    so->test_inject_element = (uint32_t)strtoul(a[6], NULL, 10);
+    so->test_inject_iteration = (uint32_t)strtoul(a[7], NULL, 10);
+    so->test_inject_word = atoi(a[8]);
+    so->test_inject_mask = (uint64_t)strtoull(a[9], NULL, 10);
+}
+static void link_opts_at(char **a, cro_link_opts *lo) {
+    lo->bytes = (uint64_t)strtoull(a[0], NULL, 10);
+    lo->hops = (uint32_t)strtoul(a[1], NULL, 10);
+    lo->ctas = (uint32_t)strtoul(a[2], NULL, 10);
+    lo->test_inject_check = atoi(a[3]);
+    lo->test_inject_word = (uint64_t)strtoull(a[4], NULL, 10);
+    lo->test_inject_mask = (uint64_t)strtoull(a[5], NULL, 10);
+}
+static void compute_opts_at(char **a, cro_compute_opts *co) {
+    co->iterations = (uint32_t)strtoul(a[0], NULL, 10);
+    co->alu_iterations = (uint32_t)strtoul(a[1], NULL, 10);
+    co->legs = (uint32_t)strtoul(a[2], NULL, 10);
+    co->max_rounds = (uint32_t)strtoul(a[3], NULL, 10);
+    co->test_inject_leg = atoi(a[4]);
+    co->test_inject_sm = atoi(a[5]);
+    co->test_inject_iteration = (uint32_t)strtoul(a[6], NULL, 10);
+    co->test_inject_row = atoi(a[7]);
+    co->test_inject_col = atoi(a[8]);
+    co->test_inject_mask = (uint32_t)strtoul(a[9], NULL, 10);
+}
+static void precision_opts_at(char **a, cro_precision_opts *po) {
+    po->iterations = (uint32_t)strtoul(a[0], NULL, 10);
+    po->alu_iterations = (uint32_t)strtoul(a[1], NULL, 10);
+    po->legs = (uint32_t)strtoul(a[2], NULL, 10);
+    po->max_rounds = (uint32_t)strtoul(a[3], NULL, 10);
+    po->test_inject_leg = atoi(a[4]);
+    po->test_inject_sm = atoi(a[5]);
+    po->test_inject_iteration = (uint32_t)strtoul(a[6], NULL, 10);
+    po->test_inject_row = atoi(a[7]);
+    po->test_inject_col = atoi(a[8]);
+    po->test_inject_mask = (uint64_t)strtoull(a[9], NULL, 10);
+}
+static void l2_opts_at(char **a, cro_l2_opts *lo) {
+    lo->bytes = (uint64_t)strtoull(a[0], NULL, 10);
+    lo->iterations = (uint32_t)strtoul(a[1], NULL, 10);
+    lo->a1_counters = (uint32_t)strtoul(a[2], NULL, 10);
+    lo->a2_counters = (uint32_t)strtoul(a[3], NULL, 10);
+    lo->test_inject_leg = atoi(a[4]);
+    lo->test_inject_sm = atoi(a[5]);
+    lo->test_inject_element = atoi(a[6]);
+    lo->test_inject_iteration = (uint32_t)strtoul(a[7], NULL, 10);
+    lo->test_inject_word = (int64_t)strtoll(a[8], NULL, 10);
+    lo->test_inject_mask = (uint64_t)strtoull(a[9], NULL, 10);
 }
 
 /* The raw commands: each fills its probe's options from argv, runs the probe on device idx and writes its frame. */
 static int scan_raw(cro_ctx *ctx, int idx, char **argv) {
     cro_scan_opts so;
     memset(&so, 0, sizeof so);
-    uint64_t *f[] = {&so.max_bytes, &so.reserve_bytes, &so.seed, &so.test_chunk_bytes, &so.test_force_first,
-                     &so.test_force_count, &so.test_force_and, &so.test_force_or};
-    for (int k = 0; k < 8; ++k) *f[k] = (uint64_t)strtoull(argv[3 + k], NULL, 10);
+    scan_opts_at(argv + 3, &so);
     const int cap = atoi(argv[11]);
     static cro_scan_report sr;
     cro_fault_word *words = (cro_fault_word *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *words);
     int got = 0;
     if (!words) return 2;
     cro_scan_hbm(ctx, idx, &so, &sr, words, cap, &got);
-    return write_frame(&sr, sizeof sr, NULL, 0, NULL, 0, words, sizeof *words, got, sr.status);
+    return put_scan(&sr, words, got) ? 2 : end_frames(sr.status);
 }
 
 static int sram_raw(cro_ctx *ctx, int idx, char **argv) {
     cro_sram_opts so;
     memset(&so, 0, sizeof so);
-    so.legs = (uint32_t)strtoul(argv[3], NULL, 10);
-    so.iterations = (uint32_t)strtoul(argv[4], NULL, 10);
-    so.cluster = (uint32_t)strtoul(argv[5], NULL, 10);
-    so.max_rounds = (uint32_t)strtoul(argv[6], NULL, 10);
-    so.test_inject_leg = atoi(argv[7]);
-    so.test_inject_sm = atoi(argv[8]);
-    so.test_inject_element = (uint32_t)strtoul(argv[9], NULL, 10);
-    so.test_inject_iteration = (uint32_t)strtoul(argv[10], NULL, 10);
-    so.test_inject_word = atoi(argv[11]);
-    so.test_inject_mask = (uint64_t)strtoull(argv[12], NULL, 10);
+    sram_opts_at(argv + 3, &so);
     const int cap = atoi(argv[13]);
     static cro_sram_result sr;
     static cro_sram_sm sms[CRO_SRAM_MAX_SMS];
@@ -129,41 +218,26 @@ static int sram_raw(cro_ctx *ctx, int idx, char **argv) {
     int n_sms = 0, got = 0;
     if (!faults) return 2;
     cro_probe_sram(ctx, idx, &so, &sr, sms, CRO_SRAM_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
-    return write_frame(&sr, sizeof sr, NULL, 0, sms, sizeof sms, faults, sizeof *faults, got, sr.status);
+    return put_sram(&sr, sms, faults, got) ? 2 : end_frames(sr.status);
 }
 
 static int link_raw(cro_ctx *ctx, int idx, char **argv) {
     cro_link_opts lo;
     memset(&lo, 0, sizeof lo);
-    lo.bytes = (uint64_t)strtoull(argv[4], NULL, 10);
-    lo.hops = (uint32_t)strtoul(argv[5], NULL, 10);
-    lo.ctas = (uint32_t)strtoul(argv[6], NULL, 10);
-    lo.test_inject_check = atoi(argv[7]);
-    lo.test_inject_word = (uint64_t)strtoull(argv[8], NULL, 10);
-    lo.test_inject_mask = (uint64_t)strtoull(argv[9], NULL, 10);
+    link_opts_at(argv + 4, &lo);
     const int cap = atoi(argv[10]);
     static cro_link_result lr;
     cro_link_fault *faults = (cro_link_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
     int got = 0;
     if (!faults) return 2;
     cro_probe_host_link(ctx, idx, &lo, &lr, faults, cap > 0 ? cap : 0, &got);
-    const uint64_t n_out = (uint64_t)got;
-    return write_frame(&lr, sizeof lr, &n_out, 1, NULL, 0, faults, sizeof *faults, got, lr.status);
+    return put_link(&lr, faults, got) ? 2 : end_frames(lr.status);
 }
 
 static int compute_raw(cro_ctx *ctx, int idx, char **argv) {
     cro_compute_opts co;
     memset(&co, 0, sizeof co);
-    co.iterations = (uint32_t)strtoul(argv[4], NULL, 10);
-    co.alu_iterations = (uint32_t)strtoul(argv[5], NULL, 10);
-    co.legs = (uint32_t)strtoul(argv[6], NULL, 10);
-    co.max_rounds = (uint32_t)strtoul(argv[7], NULL, 10);
-    co.test_inject_leg = atoi(argv[8]);
-    co.test_inject_sm = atoi(argv[9]);
-    co.test_inject_iteration = (uint32_t)strtoul(argv[10], NULL, 10);
-    co.test_inject_row = atoi(argv[11]);
-    co.test_inject_col = atoi(argv[12]);
-    co.test_inject_mask = (uint32_t)strtoul(argv[13], NULL, 10);
+    compute_opts_at(argv + 4, &co);
     const int cap = atoi(argv[14]);
     static cro_compute_result cr;
     static cro_compute_sm sms[CRO_COMPUTE_MAX_SMS];
@@ -171,23 +245,13 @@ static int compute_raw(cro_ctx *ctx, int idx, char **argv) {
     int n_sms = 0, got = 0;
     if (!faults) return 2;
     cro_probe_compute(ctx, idx, &co, &cr, sms, CRO_COMPUTE_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
-    const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)got};
-    return write_frame(&cr, sizeof cr, counts, 2, sms, sizeof sms, faults, sizeof *faults, got, cr.status);
+    return put_compute(&cr, sms, n_sms, faults, got) ? 2 : end_frames(cr.status);
 }
 
 static int precision_raw(cro_ctx *ctx, int idx, char **argv) {
     cro_precision_opts po;
     memset(&po, 0, sizeof po);
-    po.iterations = (uint32_t)strtoul(argv[4], NULL, 10);
-    po.alu_iterations = (uint32_t)strtoul(argv[5], NULL, 10);
-    po.legs = (uint32_t)strtoul(argv[6], NULL, 10);
-    po.max_rounds = (uint32_t)strtoul(argv[7], NULL, 10);
-    po.test_inject_leg = atoi(argv[8]);
-    po.test_inject_sm = atoi(argv[9]);
-    po.test_inject_iteration = (uint32_t)strtoul(argv[10], NULL, 10);
-    po.test_inject_row = atoi(argv[11]);
-    po.test_inject_col = atoi(argv[12]);
-    po.test_inject_mask = (uint64_t)strtoull(argv[13], NULL, 10);
+    precision_opts_at(argv + 4, &po);
     const int cap = atoi(argv[14]);
     static cro_precision_result pr;
     static cro_precision_sm sms[CRO_PRECISION_MAX_SMS];
@@ -195,23 +259,13 @@ static int precision_raw(cro_ctx *ctx, int idx, char **argv) {
     int n_sms = 0, got = 0;
     if (!faults) return 2;
     cro_probe_precision(ctx, idx, &po, &pr, sms, CRO_PRECISION_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
-    const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)got};
-    return write_frame(&pr, sizeof pr, counts, 2, sms, sizeof sms, faults, sizeof *faults, got, pr.status);
+    return put_precision(&pr, sms, n_sms, faults, got) ? 2 : end_frames(pr.status);
 }
 
 static int l2_raw(cro_ctx *ctx, int idx, char **argv) {
     cro_l2_opts lo;
     memset(&lo, 0, sizeof lo);
-    lo.bytes = (uint64_t)strtoull(argv[4], NULL, 10);
-    lo.iterations = (uint32_t)strtoul(argv[5], NULL, 10);
-    lo.a1_counters = (uint32_t)strtoul(argv[6], NULL, 10);
-    lo.a2_counters = (uint32_t)strtoul(argv[7], NULL, 10);
-    lo.test_inject_leg = atoi(argv[8]);
-    lo.test_inject_sm = atoi(argv[9]);
-    lo.test_inject_element = atoi(argv[10]);
-    lo.test_inject_iteration = (uint32_t)strtoul(argv[11], NULL, 10);
-    lo.test_inject_word = (int64_t)strtoll(argv[12], NULL, 10);
-    lo.test_inject_mask = (uint64_t)strtoull(argv[13], NULL, 10);
+    l2_opts_at(argv + 4, &lo);
     const int cap = atoi(argv[14]);
     static cro_l2_result lr;
     static cro_l2_sm sms[CRO_L2_MAX_SMS];
@@ -219,8 +273,7 @@ static int l2_raw(cro_ctx *ctx, int idx, char **argv) {
     int n_sms = 0, got = 0;
     if (!faults) return 2;
     cro_probe_l2(ctx, idx, &lo, &lr, sms, CRO_L2_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
-    const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)got};
-    return write_frame(&lr, sizeof lr, counts, 2, sms, sizeof sms, faults, sizeof *faults, got, lr.status);
+    return put_l2(&lr, sms, n_sms, faults, got) ? 2 : end_frames(lr.status);
 }
 
 /* `scan`: the whole-HBM scan of the free memory (all of it but 1 GiB unless argv[3], in MiB, bounds it) as JSON. */
@@ -240,6 +293,78 @@ static int scan_json(cro_ctx *ctx, int idx, char **argv) {
     free(words);
     cro_probe_destroy(ctx);
     return sr.status == CRO_OK ? 0 : 1;
+}
+
+/* health-raw's argv: each check's options from its first, then its cap.  The link check's L is argv[H_LINK]. */
+enum { H_COMPUTE = 5, H_PRECISION = 16, H_SRAM = 27, H_L2 = 38, H_LINK = 49, H_SCAN = 56, H_ARGC = 65 };
+
+/* `health-raw`: cro_check_health, then its result and each check that ran as its own frame. */
+static int health_raw(cro_ctx *ctx, int idx, char **argv) {
+    static cro_health_opts ho;
+    static cro_health_result hr;
+    static cro_compute_sm csms[CRO_COMPUTE_MAX_SMS];
+    static cro_precision_sm psms[CRO_PRECISION_MAX_SMS];
+    static cro_sram_sm ssms[CRO_SRAM_MAX_SMS];
+    static cro_l2_sm lsms[CRO_L2_MAX_SMS];
+    memset(&ho, 0, sizeof ho);
+    ho.checks = (uint32_t)strtoul(argv[4], NULL, 10);
+    compute_opts_at(argv + H_COMPUTE, &ho.compute);
+    precision_opts_at(argv + H_PRECISION, &ho.precision);
+    sram_opts_at(argv + H_SRAM, &ho.sram);
+    l2_opts_at(argv + H_L2, &ho.l2);
+    link_opts_at(argv + H_LINK, &ho.link);
+    scan_opts_at(argv + H_SCAN, &ho.scan);
+    int cap[6] = {atoi(argv[H_COMPUTE + 10]), atoi(argv[H_PRECISION + 10]), atoi(argv[H_SRAM + 10]), atoi(argv[H_L2 + 10]),
+                  atoi(argv[H_LINK + 6]), atoi(argv[H_SCAN + 8])};
+    for (int k = 0; k < 6; ++k) cap[k] = cap[k] > 0 ? cap[k] : 0;
+    cro_health_records rec;
+    memset(&rec, 0, sizeof rec);
+    rec.compute_sms = csms;
+    rec.compute_sms_cap = CRO_COMPUTE_MAX_SMS;
+    rec.precision_sms = psms;
+    rec.precision_sms_cap = CRO_PRECISION_MAX_SMS;
+    rec.sram_sms = ssms;
+    rec.sram_sms_cap = CRO_SRAM_MAX_SMS;
+    rec.l2_sms = lsms;
+    rec.l2_sms_cap = CRO_L2_MAX_SMS;
+    rec.compute_faults = calloc((size_t)cap[0] + 1, sizeof *rec.compute_faults);
+    rec.precision_faults = calloc((size_t)cap[1] + 1, sizeof *rec.precision_faults);
+    rec.sram_faults = calloc((size_t)cap[2] + 1, sizeof *rec.sram_faults);
+    rec.l2_faults = calloc((size_t)cap[3] + 1, sizeof *rec.l2_faults);
+    rec.link_faults = calloc((size_t)cap[4] + 1, sizeof *rec.link_faults);
+    rec.scan_words = calloc((size_t)cap[5] + 1, sizeof *rec.scan_words);
+    if (!rec.compute_faults || !rec.precision_faults || !rec.sram_faults || !rec.l2_faults || !rec.link_faults || !rec.scan_words)
+        return 2;
+    rec.compute_faults_cap = cap[0];
+    rec.precision_faults_cap = cap[1];
+    rec.sram_faults_cap = cap[2];
+    rec.l2_faults_cap = cap[3];
+    rec.link_faults_cap = cap[4];
+    rec.scan_words_cap = cap[5];
+    cro_check_health(ctx, idx, &ho, &hr, &rec);
+    if (put_frame(&hr, sizeof hr, NULL, 0, NULL, 0, NULL, 0, 0) ||
+        ((hr.ran & CRO_HEALTH_COMPUTE) && put_compute(&hr.compute, csms, rec.compute_sms_n, rec.compute_faults, rec.compute_faults_n)) ||
+        ((hr.ran & CRO_HEALTH_PRECISION) &&
+         put_precision(&hr.precision, psms, rec.precision_sms_n, rec.precision_faults, rec.precision_faults_n)) ||
+        ((hr.ran & CRO_HEALTH_SRAM) && put_sram(&hr.sram, ssms, rec.sram_faults, rec.sram_faults_n)) ||
+        ((hr.ran & CRO_HEALTH_L2) && put_l2(&hr.l2, lsms, rec.l2_sms_n, rec.l2_faults, rec.l2_faults_n)) ||
+        ((hr.ran & CRO_HEALTH_LINK) && put_link(&hr.link, rec.link_faults, rec.link_faults_n)) ||
+        ((hr.ran & CRO_HEALTH_SCAN) && put_scan(&hr.scan, rec.scan_words, rec.scan_words_n)))
+        return 2;
+    return end_frames(hr.status);
+}
+
+/* `health`: the health check with defaults; every check's annotations and the call's own as one JSON object. */
+static int health_json(cro_ctx *ctx, int idx, char **argv) {
+    static cro_health_result hr;
+    size_t len = 0;
+    (void)argv;
+    int rc = cro_check_health(ctx, idx, NULL, &hr, NULL);
+    if (rc == CRO_ERR_INVALID_ARG) return fail(ctx, "cro_check_health", rc);
+    if ((rc = cro_emit_health_annotations_json(&hr, buf, sizeof buf, &len)) != CRO_OK) return fail(ctx, "emit", rc);
+    printf("%s\n", buf);
+    cro_probe_destroy(ctx);
+    return hr.status == CRO_OK ? 0 : 1;
 }
 
 /* The commands that take a device (argv[2]): their argc (0: at least 3, the rest optional), cro_opts.flags and sweep
@@ -269,6 +394,10 @@ static const struct command {
     /* no health record to read, and NVML's first call is slow */
     {"compute-raw", 15, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, 1, compute_raw},
     {"precision-raw", 15, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, 1, precision_raw},
+    /* every check of one device: the link check's region (exactly L, argv[49], when it is given) and NVML for the scan's,
+     * SRAM's and L2's health records and the link's replay counters */
+    {"health-raw", H_ARGC, CRO_F_LAZY_ALLOC, 256, 1, health_raw},
+    {"health", 0, CRO_F_LAZY_ALLOC, 256, 0, health_json},
 };
 
 int main(int argc, char **argv) {
@@ -279,7 +408,9 @@ int main(int argc, char **argv) {
                         "<word> <mask> <cap> | link-raw <uuid> <seed_base> <bytes> <hops> <ctas> <check> <word> <mask> <cap> | "
                         "compute-raw <uuid> <seed_base> <iterations> <alu_iterations> <legs> <rounds> <leg> <sm> <iteration> <row> <col> "
                         "<mask> <cap> | precision-raw <uuid> <seed_base> <iterations> <alu_iterations> <legs> <rounds> <leg> <sm> <iteration> <row> "
-                        "<col> <mask> <cap> | l2-raw <uuid> <seed_base> <bytes> <iterations> <a1> <a2> <leg> <sm> <element> <iteration> <word> <mask> <cap>\n");
+                        "<col> <mask> <cap> | l2-raw <uuid> <seed_base> <bytes> <iterations> <a1> <a2> <leg> <sm> <element> <iteration> <word> <mask> <cap> | "
+                        "health-raw <uuid> <seed_base> <checks> <compute-raw, precision-raw, sram-raw, l2-raw, link-raw, scan-raw options "
+                        "and caps> | health <uuid|index>\n");
         return 64;
     }
     const double t_start = now_s();
@@ -300,6 +431,7 @@ int main(int argc, char **argv) {
         if (!c->run && argc > 3) opts.sweep_bytes = (uint64_t)strtoull(argv[3], NULL, 10) << 20;    /* the probe's sweep_MiB */
         if (cold && argc > 4 && strcmp(argv[4], "nvml") == 0) opts.flags &= ~CRO_F_NO_NVML;
         if (c->run == link_raw && strtoull(argv[4], NULL, 10)) opts.sweep_bytes = (uint64_t)strtoull(argv[4], NULL, 10);  /* L */
+        if (c->run == health_raw && strtoull(argv[H_LINK], NULL, 10)) opts.sweep_bytes = (uint64_t)strtoull(argv[H_LINK], NULL, 10);
         if (strncmp(argv[2], "GPU-", 4) == 0) {
             /* before ANY CUDA call: this process's cuInit must enumerate that one GPU only (one primary context
              * instead of eight on a full box) */
@@ -370,7 +502,7 @@ int main(int argc, char **argv) {
                    r.gpu_uuid, (unsigned long long)r.sweep_bytes, t_init, t_cold, t_warm, total,
                    1.0 / total, 1.0 / t_warm, (opts.flags & CRO_F_NO_NVML) ? "false" : "true", rc2 ? rc2 : r.status);
         } else if (strcmp(cmd, "probe-raw") == 0) {
-            return write_frame(&r, sizeof r, NULL, 0, NULL, 0, NULL, 0, 0, r.status);
+            return put_frame(&r, sizeof r, NULL, 0, NULL, 0, NULL, 0, 0) ? 2 : end_frames(r.status);
         } else {
             if ((rc = cro_emit_probe_annotations_json(&r, buf, sizeof buf, &len)) != CRO_OK) return fail(ctx, "emit", rc);
             printf("%s\n", buf);

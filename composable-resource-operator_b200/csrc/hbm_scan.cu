@@ -179,14 +179,20 @@ uint32_t scan_health(const cro_hbm_health& b, const cro_hbm_health& a) {
     return h;
 }
 
+std::string scan_opts_error(const cro_scan_opts& o) {
+    const uint64_t chunk_bytes = o.test_chunk_bytes ? o.test_chunk_bytes : CRO_SCAN_CHUNK_BYTES;
+    return chunk_bytes % 16 || o.reserved0 ? "scan chunk size must be a multiple of 16 bytes and reserved0 zero" : "";
+}
+
 int ctx_scan_hbm(cro_ctx* c, int idx, const cro_scan_opts& o, cro_scan_report* rep, std::vector<cro_fault_word>* words) {
     const uint64_t t_call = now_ns();
     blank_report(rep, words);
     Device* d = dev_at(c, idx);
     if (!d) return rep->status = unknown_device(c, idx, "a GPU attached after init is scanned through the helper process, cro_scan_hbm_uuid");
     const uint64_t chunk_bytes = o.test_chunk_bytes ? o.test_chunk_bytes : CRO_SCAN_CHUNK_BYTES;
-    if (chunk_bytes % 16 || o.reserved0) {
-        c->set_error("scan chunk size must be a multiple of 16 bytes and reserved0 zero");
+    const std::string why = scan_opts_error(o);
+    if (!why.empty()) {
+        c->set_error(why);
         return rep->status = CRO_ERR_INVALID_ARG;
     }
     DeviceGuard g = enter_device(c, idx);
@@ -307,7 +313,7 @@ int ctx_scan_hbm(cro_ctx* c, int idx, const cro_scan_opts& o, cro_scan_report* r
 }
 
 namespace {
-uint64_t scan_tail_count(const unsigned char* head) {
+uint64_t scan_tail_count(const unsigned char* head, size_t) {
     return reinterpret_cast<const cro_scan_report*>(head)->recorded;
 }
 }  // namespace

@@ -348,9 +348,12 @@ int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_re
     return r->status = link_status(*r);
 }
 
+// The helper's sweep region is L, or the default L when none is given: refuse here what it would refuse there.
+std::string link_helper_opts_error(const cro_link_opts& o) { return link_opts_error(o, o.bytes ? o.bytes : kLinkDefaultBytes); }
+
 namespace {
 // link-raw's stdout: the result, the helper's own fault count n, then n faults.
-uint64_t link_tail_count(const unsigned char* head) {
+uint64_t link_tail_count(const unsigned char* head, size_t) {
     uint64_t n;
     memcpy(&n, head + sizeof(cro_link_result), sizeof n);
     return n;
@@ -362,8 +365,7 @@ int ctx_probe_host_link_uuid(cro_ctx* c, const char* uuid, const cro_link_opts& 
     blank_result(r, faults, 0);
     *helper_ns = 0;
     if (!uuid) return r->status = CRO_ERR_INVALID_ARG;
-    // the helper's sweep region is L, or the default L when none is given: refuse here what it would refuse there
-    const std::string why = link_opts_error(o, o.bytes ? o.bytes : kLinkDefaultBytes);
+    const std::string why = link_helper_opts_error(o);
     if (!why.empty()) {
         set_call_error(c, why);
         return r->status = CRO_ERR_INVALID_ARG;
@@ -380,7 +382,7 @@ int ctx_probe_host_link_uuid(cro_ctx* c, const char* uuid, const cro_link_opts& 
     if (rc != CRO_OK) return r->status = rc;
     memcpy(r, got.data(), sizeof *r);
     const cro_link_fault* f = reinterpret_cast<const cro_link_fault*>(got.data() + head);
-    faults->assign(f, f + link_tail_count(reinterpret_cast<const unsigned char*>(got.data())));
+    faults->assign(f, f + link_tail_count(reinterpret_cast<const unsigned char*>(got.data()), got.size()));
     return r->status;
 }
 

@@ -109,7 +109,7 @@ std::string DefaultHelperPath() {
 
 int RunHelperRaw(const std::string& helper_path, const std::string& what, const std::string& uuid,
                  const std::vector<std::string>& args, int deadline_ms, size_t head, size_t rec, size_t max_rec,
-                 uint64_t (*count)(const unsigned char* head), std::string* out, std::string* err) {
+                 uint64_t (*count)(const unsigned char* out, size_t size), std::string* out, std::string* err) {
     const std::string helper = helper_path.empty() ? DefaultHelperPath() : helper_path;
     if (access(helper.c_str(), X_OK) != 0) {
         if (err) *err = what + " '" + helper + "' is not executable";
@@ -190,7 +190,7 @@ int RunHelperRaw(const std::string& helper_path, const std::string& what, const 
         if (err) *err = "device '" + uuid + "' is not visible to a fresh CUDA process";
         return CRO_ERR_NO_DEVICE;
     }
-    const uint64_t n_rec = out->size() >= head && count ? count(reinterpret_cast<const unsigned char*>(out->data())) : 0;
+    const uint64_t n_rec = out->size() >= head && count ? count(reinterpret_cast<const unsigned char*>(out->data()), out->size()) : 0;
     if (out->size() < head || n_rec > max_rec || out->size() != head + rec * n_rec || (code != 0 && code != 1)) {
         if (err) *err = what + " for " + uuid + " failed (exit " + std::to_string(code) + ", " + std::to_string(out->size()) + " result bytes)";
         return CRO_ERR_EXEC;

@@ -159,6 +159,8 @@ int ctx_probe_precision(cro_ctx* c, int idx, const cro_precision_opts& o, cro_pr
     return probe_sm_legs<PrecisionProbe>(c, idx, o, r, sms, faults);
 }
 
+std::string precision_opts_error(const cro_precision_opts& o) { return PrecisionProbe::opts_error(o); }
+
 int ctx_probe_precision_uuid(cro_ctx* c, const char* uuid, const cro_precision_opts& o, int deadline_ms, cro_precision_result* r,
                              std::vector<cro_precision_sm>* sms, std::vector<cro_precision_fault>* faults, int cap,
                              uint64_t* helper_ns) {

@@ -892,7 +892,7 @@ static_assert(status_first<cro_link_result>() && status_first<cro_compute_result
 
 int run_probe_helper(cro_ctx* c, const std::string& uuid, const std::string& what, const char* range,
                      const std::vector<std::string>& args, int deadline_ms, size_t head, size_t rec, size_t cap,
-                     uint64_t (*count)(const unsigned char* head), std::string* got, uint64_t* helper_ns) {
+                     uint64_t (*count)(const unsigned char* out, size_t size), std::string* got, uint64_t* helper_ns) {
     env::Values knobs;                        // no context: this caller's environment, defaults where it is illegal
     if (c) knobs = c->knobs;
     else env::read(&knobs, nullptr);

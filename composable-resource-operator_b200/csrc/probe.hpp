@@ -274,7 +274,7 @@ int Expected(int answer, uint64_t seed, int64_t* out);
 // calling thread without one.
 int run_probe_helper(cro_ctx* c, const std::string& uuid, const std::string& what, const char* range,
                      const std::vector<std::string>& args, int deadline_ms, size_t head, size_t rec, size_t cap,
-                     uint64_t (*count)(const unsigned char* head), std::string* got, uint64_t* helper_ns);
+                     uint64_t (*count)(const unsigned char* out, size_t size), std::string* got, uint64_t* helper_ns);
 // The stdout of compute-raw, precision-raw and l2-raw: the Result, the helper's own counts n_sms and n (uint64_t),
 // MAX_SMS Sm entries (n_sms of them filled), then n Fault records.  An n_sms the entries cannot hold makes the output
 // malformed.
@@ -289,7 +289,7 @@ struct SmFrame {
         return v;
     }
     // The record count run_probe_helper's count argument gives RunHelperRaw.
-    static uint64_t tail(const unsigned char* head) { return count(head, 0) > MAX_SMS ? ~0ull : count(head, 1); }
+    static uint64_t tail(const unsigned char* head, size_t) { return count(head, 0) > MAX_SMS ? ~0ull : count(head, 1); }
     // Unpacks a frame run_probe_helper accepted.
     static void read(const std::string& got, Result* r, std::vector<Sm>* sms, std::vector<Fault>* faults) {
         const unsigned char* head = reinterpret_cast<const unsigned char*>(got.data());
@@ -320,6 +320,14 @@ uint32_t scan_health(const cro_hbm_health& before, const cro_hbm_health& after);
 int selftest_scan_collect(int32_t cuda_error, const cro_locate_counters* ctr, const cro_locate_record* records,
                           const uint64_t* granules, uint64_t granule_words, const cro_sweep_slot* slots, cro_scan_report* rep,
                           std::vector<cro_fault_word>* words);
+
+// Each check's argument check, as its calls make it: why the options are refused ("" when they pass).  The link
+// check's is its helper form's (L against a region of L); the L2 check's is l2_check_args.
+std::string compute_opts_error(const cro_compute_opts& o);
+std::string precision_opts_error(const cro_precision_opts& o);
+std::string sram_opts_error(const cro_sram_opts& o);
+std::string link_helper_opts_error(const cro_link_opts& o);
+std::string scan_opts_error(const cro_scan_opts& o);
 
 // SRAM probe (include/croprobe.h, cro_probe_sram / cro_probe_sram_uuid, sram_probe.cu): *sms gets one entry per SM
 // seen, by SM id; *faults every recorded word, by (leg, element, smid, iteration, word).  The uuid form runs
@@ -358,6 +366,36 @@ uint32_t l2_delta(uint32_t G);
 uint32_t l2_health(const cro_l2_health& before, const cro_l2_health& after);
 // The verdict, bad SMs and lines, marks and line flags of a call's counts and records (cro_selftest_l2_classify).
 void l2_classify(cro_l2_result* r, cro_l2_sm* sms, size_t n_sms, cro_l2_fault* faults, size_t n);
+
+// Health check (include/croprobe.h, cro_check_health / cro_check_health_uuid, health.cpp): every record each check
+// found, as its own call lists them.
+struct HealthRecords {
+    std::vector<cro_compute_sm> compute_sms;
+    std::vector<cro_compute_fault> compute_faults;
+    std::vector<cro_precision_sm> precision_sms;
+    std::vector<cro_precision_fault> precision_faults;
+    std::vector<cro_sram_sm> sram_sms;
+    std::vector<cro_sram_fault> sram_faults;
+    std::vector<cro_l2_sm> l2_sms;
+    std::vector<cro_l2_fault> l2_faults;
+    std::vector<cro_link_fault> link_faults;
+    std::vector<cro_fault_word> scan_words;
+};
+// The record caps the helper is asked for, in run order: compute, precision, SRAM, L2 faults, link faults, scan words.
+struct HealthCaps {
+    int faults[CRO_HEALTH_CHECKS];
+};
+// The stop and status rules (cro_selftest_health_classify): checks is the selection, status[0 .. n) what the first n
+// checks to run returned.  Writes r's status, checks, ran, failed, errored, not_run and check_status; returns the index
+// of the check to run next, CRO_HEALTH_CHECKS when none is left, or -1 when the rules let fewer than n checks run.
+int health_step(uint32_t checks, const int32_t* status, int n, cro_health_result* r);
+// Why a health call's options are refused before anything runs ("" when they pass): check bits, sub-option deadlines
+// and each selected check's own argument check.
+std::string health_opts_error(const cro_health_opts& o);
+int ctx_check_health(cro_ctx* c, int idx, const cro_health_opts& o, cro_health_result* r, HealthRecords* rec);
+// The uuid form runs `croprobe-cli health-raw` with a fresh seed base and asks it for at most caps records per list.
+int ctx_check_health_uuid(cro_ctx* c, const char* uuid, const cro_health_opts& o, int deadline_ms, const HealthCaps& caps,
+                          cro_health_result* r, HealthRecords* rec, uint64_t* helper_ns);
 
 // test hooks (include/croprobe.h, cro_selftest_*): the verdict kernels and the chase on caller-given inputs
 int ctx_selftest_probe_finalize(cro_ctx* c, int idx, const cro_probe_result* tmpl, const cro_sweep_slot* slots,

@@ -239,6 +239,20 @@ uint32_t sram_health(const cro_sram_health& b, const cro_sram_health& a) {
     return h;
 }
 
+std::string sram_opts_error(const cro_sram_opts& o) {
+    const uint32_t legs = o.legs ? o.legs : CRO_SRAM_ALL_LEGS;
+    const uint32_t iters = o.iterations ? o.iterations : kSramDefaultIterations;
+    const uint32_t cluster = o.cluster ? o.cluster : kSramDefaultCluster;
+    const uint32_t max_rounds = o.max_rounds ? o.max_rounds : kSramDefaultRounds;
+    if ((legs & ~CRO_SRAM_ALL_LEGS) || iters > CRO_SRAM_MAX_ITERATIONS || (cluster != 2 && cluster != 4 && cluster != 8) ||
+        max_rounds > CRO_SRAM_MAX_ROUNDS || !valid_injection(o, iters))
+        return "SRAM probe: legs must be CRO_SRAM_ALL_LEGS bits, iterations at most " + std::to_string(CRO_SRAM_MAX_ITERATIONS) +
+               ", cluster 2, 4 or 8, max_rounds at most " + std::to_string(CRO_SRAM_MAX_ROUNDS) +
+               ", and an injection must name a leg, an element it has (local 1 .. 5, network 1 or 2), an SM id below " +
+               std::to_string(CRO_SRAM_MAX_SMS) + " (or -1), an iteration the call runs and a word (or -1)";
+    return "";
+}
+
 int ctx_probe_sram(cro_ctx* c, int idx, const cro_sram_opts& o, cro_sram_result* r, std::vector<cro_sram_sm>* sms,
                    std::vector<cro_sram_fault>* faults) {
     const uint64_t t_call = now_ns();
@@ -249,12 +263,9 @@ int ctx_probe_sram(cro_ctx* c, int idx, const cro_sram_opts& o, cro_sram_result*
     const uint32_t iters = o.iterations ? o.iterations : kSramDefaultIterations;
     const uint32_t cluster = o.cluster ? o.cluster : kSramDefaultCluster;
     const uint32_t max_rounds = o.max_rounds ? o.max_rounds : kSramDefaultRounds;
-    if ((legs & ~CRO_SRAM_ALL_LEGS) || iters > CRO_SRAM_MAX_ITERATIONS || (cluster != 2 && cluster != 4 && cluster != 8) ||
-        max_rounds > CRO_SRAM_MAX_ROUNDS || !valid_injection(o, iters)) {
-        c->set_error("SRAM probe: legs must be CRO_SRAM_ALL_LEGS bits, iterations at most " + std::to_string(CRO_SRAM_MAX_ITERATIONS) +
-                     ", cluster 2, 4 or 8, max_rounds at most " + std::to_string(CRO_SRAM_MAX_ROUNDS) +
-                     ", and an injection must name a leg, an element it has (local 1 .. 5, network 1 or 2), an SM id below " +
-                     std::to_string(CRO_SRAM_MAX_SMS) + " (or -1), an iteration the call runs and a word (or -1)");
+    const std::string why = sram_opts_error(o);
+    if (!why.empty()) {
+        c->set_error(why);
         return r->status = CRO_ERR_INVALID_ARG;
     }
     DeviceGuard g = enter_device(c, idx);
@@ -404,7 +415,7 @@ int classify_sram(uint32_t legs, uint32_t iterations, uint32_t n_words, uint64_t
 }
 
 namespace {
-uint64_t sram_tail_count(const unsigned char* head) {
+uint64_t sram_tail_count(const unsigned char* head, size_t) {
     return reinterpret_cast<const cro_sram_result*>(head)->recorded;
 }
 }  // namespace

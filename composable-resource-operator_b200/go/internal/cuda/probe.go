@@ -882,6 +882,102 @@ func (c *Context) ProbeL2(deviceID string) (L2Result, error) {
 	return l2Result(&res, faults[:], got), nil
 }
 
+// HealthResult is the summary of cro_health_result an operator reads: the
+// call's status and which checks failed, errored, did not run or fell short of
+// every SM, each check that ran as its own Go result, and every annotation.
+type HealthResult struct {
+	Status      int32  // CRO_OK, CRO_ERR_CHECKSUM, or the first other status a check returned
+	Ran         uint32 // CRO_HEALTH_* bits
+	Failed      uint32 // ... that returned CRO_ERR_CHECKSUM
+	Errored     uint32 // ... that returned another status but CRO_OK
+	NotRun      uint32 // selected, but after a check that returned CRO_ERR_CUDA
+	Incomplete  uint32 // ran on fewer SMs than the device has; never changes Status
+	HelperNs    uint64 // the helper's spawn to exit
+	Compute     ComputeResult
+	Precision   PrecisionResult
+	SRAM        SRAMResult
+	L2          L2Result
+	Link        LinkResult
+	Scan        ScanResult
+	Annotations string // Go-marshalled map[string]string: every ran check's keys and cohdi.io/probe-health-*
+}
+
+// CheckHealthByUUID runs cro_check_health_uuid: the selected checks (checks 0:
+// all six) of any GPU on the node in one helper process, each with its defaults,
+// the form to call once after the first passing HBM probe of a freshly composed
+// GPU (INTEGRATION.md §2g).  A failed check is a result, not an error; found is
+// false when the node does not list the GPU.
+func (c *Context) CheckHealthByUUID(deviceID string, checks uint32) (r HealthResult, found bool, err error) {
+	id := C.CString(deviceID)
+	defer C.free(unsafe.Pointer(id))
+	var opts C.cro_health_opts
+	opts.checks = C.uint32_t(checks)
+	// the result and the record arrays live in C memory: the records struct the call takes holds pointers to them
+	res := (*C.cro_health_result)(C.malloc(C.size_t(unsafe.Sizeof(C.cro_health_result{}))))
+	defer C.free(unsafe.Pointer(res))
+	rec := (*C.cro_health_records)(C.malloc(C.size_t(unsafe.Sizeof(C.cro_health_records{}))))
+	defer C.free(unsafe.Pointer(rec))
+	*rec = C.cro_health_records{} // the SRAM and L2 per-SM lists stay NULL with cap 0
+	alloc := func(n int, size uintptr) unsafe.Pointer { return C.malloc(C.size_t(n) * C.size_t(size)) }
+	rec.compute_sms = (*C.cro_compute_sm)(alloc(int(C.CRO_COMPUTE_MAX_SMS), unsafe.Sizeof(C.cro_compute_sm{})))
+	rec.compute_sms_cap = C.CRO_COMPUTE_MAX_SMS
+	rec.compute_faults = (*C.cro_compute_fault)(alloc(256, unsafe.Sizeof(C.cro_compute_fault{})))
+	rec.compute_faults_cap = 256
+	rec.precision_sms = (*C.cro_precision_sm)(alloc(int(C.CRO_PRECISION_MAX_SMS), unsafe.Sizeof(C.cro_precision_sm{})))
+	rec.precision_sms_cap = C.CRO_PRECISION_MAX_SMS
+	rec.precision_faults = (*C.cro_precision_fault)(alloc(256, unsafe.Sizeof(C.cro_precision_fault{})))
+	rec.precision_faults_cap = 256
+	rec.sram_faults = (*C.cro_sram_fault)(alloc(256, unsafe.Sizeof(C.cro_sram_fault{})))
+	rec.sram_faults_cap = 256
+	rec.l2_faults = (*C.cro_l2_fault)(alloc(256, unsafe.Sizeof(C.cro_l2_fault{})))
+	rec.l2_faults_cap = 256
+	rec.link_faults = (*C.cro_link_fault)(alloc(256, unsafe.Sizeof(C.cro_link_fault{})))
+	rec.link_faults_cap = 256
+	rec.scan_words = (*C.cro_fault_word)(alloc(256, unsafe.Sizeof(C.cro_fault_word{})))
+	rec.scan_words_cap = 256
+	for _, p := range []unsafe.Pointer{unsafe.Pointer(rec.compute_sms), unsafe.Pointer(rec.compute_faults),
+		unsafe.Pointer(rec.precision_sms), unsafe.Pointer(rec.precision_faults), unsafe.Pointer(rec.sram_faults),
+		unsafe.Pointer(rec.l2_faults), unsafe.Pointer(rec.link_faults), unsafe.Pointer(rec.scan_words)} {
+		defer C.free(p)
+	}
+	rc := C.cro_check_health_uuid(c.h, id, &opts, 0, res, rec, nil)
+	if rc == C.CRO_ERR_NO_DEVICE {
+		return r, false, nil
+	}
+	if rc != C.CRO_OK && res.ran == 0 {
+		return r, true, errorOf(c.h, rc)
+	}
+	r = HealthResult{Status: int32(res.status), Ran: uint32(res.ran), Failed: uint32(res.failed), Errored: uint32(res.errored),
+		NotRun: uint32(res.not_run), Incomplete: uint32(res.incomplete), HelperNs: uint64(res.helper_ns)}
+	if r.Ran&C.CRO_HEALTH_COMPUTE != 0 {
+		r.Compute = computeResult(&res.compute, unsafe.Slice(rec.compute_sms, C.CRO_COMPUTE_MAX_SMS), rec.compute_sms_n,
+			unsafe.Slice(rec.compute_faults, 256), rec.compute_faults_n)
+	}
+	if r.Ran&C.CRO_HEALTH_PRECISION != 0 {
+		r.Precision = precisionResult(&res.precision, unsafe.Slice(rec.precision_sms, C.CRO_PRECISION_MAX_SMS), rec.precision_sms_n,
+			unsafe.Slice(rec.precision_faults, 256), rec.precision_faults_n)
+	}
+	if r.Ran&C.CRO_HEALTH_SRAM != 0 {
+		r.SRAM = sramResult(&res.sram, unsafe.Slice(rec.sram_faults, 256), rec.sram_faults_n)
+	}
+	if r.Ran&C.CRO_HEALTH_L2 != 0 {
+		r.L2 = l2Result(&res.l2, unsafe.Slice(rec.l2_faults, 256), rec.l2_faults_n)
+	}
+	if r.Ran&C.CRO_HEALTH_LINK != 0 {
+		r.Link = linkResult(&res.link, unsafe.Slice(rec.link_faults, 256), rec.link_faults_n)
+	}
+	if r.Ran&C.CRO_HEALTH_SCAN != 0 {
+		r.Scan = scanResult(&res.scan, unsafe.Slice(rec.scan_words, 256), rec.scan_words_n)
+	}
+	buf := (*C.char)(C.malloc(65536))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_health_annotations_json(res, buf, 65536, &ln) == C.CRO_OK {
+		r.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return r, true, nil
+}
+
 // MetricsText is the Prometheus text exposition of the context's counters and
 // per-GPU gauges; a prometheus.Collector registered with
 // sigs.k8s.io/controller-runtime/pkg/metrics.Registry (cmd/main.go:66,119-125

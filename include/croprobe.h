@@ -1585,6 +1585,133 @@ int  cro_selftest_sram_classify(uint32_t legs, uint32_t iterations, uint32_t n_w
                                 cro_sram_result *out, cro_sram_sm *sms, int sms_cap, int *n_sms, cro_sram_fault *faults,
                                 int cap, int *n);
 
+/* ---- health: a composed GPU's six checks in one call ---- */
+
+/*
+ * Accepting a freshly composed GPU takes the compute, precision, SRAM, L2, host link and whole-HBM checks.  Through
+ * their single helper forms that is six helper processes, each paying its own cuInit, primary context and NVML start,
+ * and six verdicts to combine.  The health check runs the selected checks in one call, on one device, in this fixed
+ * order (bit c of CRO_HEALTH_* is check c, and c is also its place in the order):
+ *   compute, precision, SRAM, L2    cheap and SM-local, so first
+ *   host link                       the sweep region (L bytes in the helper) and pinned host memory
+ *   scan                            all free memory but reserve_bytes, and the check most likely to meet an
+ *                                   uncorrectable ECC error: last
+ * Stop rule: once a check returns CRO_ERR_CUDA, no later check runs (a sticky error fails every later launch in the
+ * process); each is reported in not_run.  Any other status (CRO_ERR_OOM, CRO_ERR_CHECKSUM, ...) does not stop it.
+ * Status of the call: CRO_ERR_CHECKSUM when any check returned it (corruption found is never transient); else the first
+ * status other than CRO_OK in run order; else CRO_OK.  Short coverage and the health bits never change it, as in each
+ * probe.  Each check runs with its own options, checked by its own argument check; there are no new knobs.
+ */
+#define CRO_HEALTH_COMPUTE        0x01u
+#define CRO_HEALTH_PRECISION      0x02u
+#define CRO_HEALTH_SRAM           0x04u
+#define CRO_HEALTH_L2             0x08u
+#define CRO_HEALTH_LINK           0x10u
+#define CRO_HEALTH_SCAN           0x20u
+#define CRO_HEALTH_ALL            0x3Fu
+#define CRO_HEALTH_CHECKS         6
+
+typedef struct cro_health_opts {
+    uint32_t checks;               /*   0  CRO_HEALTH_* bits; 0 = CRO_HEALTH_ALL                                   */
+    uint32_t reserved0;            /*   4  0 */
+    /* each check's own options (a zeroed struct: that check's defaults).  The call has one deadline: a non-zero
+       sram.deadline_ms, l2.deadline_ms or scan.deadline_ms is refused */
+    cro_compute_opts   compute;    /*   8 */
+    cro_precision_opts precision;  /*  48 */
+    cro_sram_opts      sram;       /*  96 */
+    cro_l2_opts        l2;         /* 144 */
+    cro_link_opts      link;       /* 200 */
+    cro_scan_opts      scan;       /* 240 */
+} cro_health_opts;                 /* 312 bytes */
+
+typedef struct cro_health_result {
+    int32_t  status;               /*   0  the return value (rules above)                                         */
+    uint32_t checks;               /*   4  the checks selected                                                    */
+    uint32_t ran;                  /*   8  checks that ran                                                        */
+    uint32_t failed;               /*  12  ... and returned CRO_ERR_CHECKSUM                                      */
+    uint32_t errored;              /*  16  ... and returned another status but CRO_OK                             */
+    uint32_t not_run;              /*  20  selected, but after a check that returned CRO_ERR_CUDA                 */
+    uint32_t incomplete;           /*  24  compute, precision, SRAM, L2 that ran with their least sms_covered over
+                                              the legs run below sm_count (link and scan have no coverage)    */
+    uint32_t reserved0;            /*  28 */
+    int32_t  check_status[CRO_HEALTH_CHECKS];   /*  32  the status each check returned; 0 when it did not run      */
+    uint64_t check_ns[CRO_HEALTH_CHECKS];       /*  56  host wall clock of each check that ran                     */
+    uint64_t seed_base;            /* 104  cro_opts.seed_base of the context the checks ran in                     */
+    uint64_t helper_ns;            /* 112  cro_check_health_uuid: spawn of the helper to its exit; 0 in process    */
+    cro_compute_result   compute;  /* 120  each check's own result (blank when it did not run)                     */
+    cro_precision_result precision;/* 720 */
+    cro_sram_result      sram;     /* 1528 */
+    cro_l2_result        l2;       /* 2096 */
+    cro_link_result      link;     /* 2712 */
+    cro_scan_report      scan;     /* 3696 */
+} cro_health_result;               /* 16328 bytes */
+
+/* The caller's record arrays, one {array, cap, n} per list: the per-SM entries and faults of the compute, precision,
+ * SRAM and L2 checks, the link faults and the scan words, each as that check's own call writes them (its first cap
+ * records; n: how many were written).  An array may be NULL with cap 0.  The SRAM and L2 results' sms_listed and
+ * recorded, and the scan's recorded and complete, say what the caller got, as in their own calls. */
+typedef struct cro_health_records {
+    cro_compute_sm      *compute_sms;       /*   0 */
+    int32_t              compute_sms_cap;   /*   8 */
+    int32_t              compute_sms_n;     /*  12 */
+    cro_compute_fault   *compute_faults;    /*  16 */
+    int32_t              compute_faults_cap;/*  24 */
+    int32_t              compute_faults_n;  /*  28 */
+    cro_precision_sm    *precision_sms;     /*  32 */
+    int32_t              precision_sms_cap; /*  40 */
+    int32_t              precision_sms_n;   /*  44 */
+    cro_precision_fault *precision_faults;  /*  48 */
+    int32_t              precision_faults_cap; /* 56 */
+    int32_t              precision_faults_n;   /* 60 */
+    cro_sram_sm         *sram_sms;          /*  64 */
+    int32_t              sram_sms_cap;      /*  72 */
+    int32_t              sram_sms_n;        /*  76 */
+    cro_sram_fault      *sram_faults;       /*  80 */
+    int32_t              sram_faults_cap;   /*  88 */
+    int32_t              sram_faults_n;     /*  92 */
+    cro_l2_sm           *l2_sms;            /*  96 */
+    int32_t              l2_sms_cap;        /* 104 */
+    int32_t              l2_sms_n;          /* 108 */
+    cro_l2_fault        *l2_faults;         /* 112 */
+    int32_t              l2_faults_cap;     /* 120 */
+    int32_t              l2_faults_n;       /* 124 */
+    cro_link_fault      *link_faults;       /* 128 */
+    int32_t              link_faults_cap;   /* 136 */
+    int32_t              link_faults_n;     /* 140 */
+    cro_fault_word      *scan_words;        /* 144 */
+    int32_t              scan_words_cap;    /* 152 */
+    int32_t              scan_words_n;      /* 156 */
+} cro_health_records;              /* 160 bytes (64-bit pointers) */
+
+/* In process: the selected checks on in-process device dev_index, each through its own in-process call, in order.
+ * opts may be NULL (every check, defaults); rec may be NULL (no records).  Returns out->status, or CRO_ERR_INVALID_ARG
+ * before anything runs for a NULL ctx or out, check bits outside CRO_HEALTH_ALL, a sub-option deadline, a selected
+ * check's options its own argument check refuses, or a negative cap or a NULL array with a cap.  The result is filled
+ * whatever the status. */
+int  cro_check_health(cro_ctx *ctx, int dev_index, const cro_health_opts *opts, cro_health_result *out,
+                      cro_health_records *rec);
+
+/* The form an operator calls (INTEGRATION.md §2g): the same checks of any GPU on the node in one helper process,
+ * `croprobe-cli health-raw` (a fresh cuInit that sees only that GPU).  ctx may be NULL; a UUID the node does not list,
+ * or one the helper cannot see, is CRO_ERR_NO_DEVICE; a GPU that is also an in-process device of ctx is held under
+ * that device's mutex while the helper runs.  Options are refused before any helper starts, as cro_check_health
+ * refuses them (the link check's L against the helper's region of L; the L2 buffer's upper bound, which needs the
+ * device, is the helper's to check).  deadline_ms 0: CRO_HELPER_TIMEOUT_MS; a helper past it is killed
+ * (CRO_ERR_DEADLINE).  The helper gets one fresh cro_opts.seed_base per call (ctx's seed_base + (h << 8) for its h-th
+ * helper call, or one from the clock without ctx), reported in out->seed_base; every check starts at call 0 of its own
+ * seed space, so no seed of one call is a seed of another; the scan keeps its own seed option (0: the clock).
+ * Malformed output or a crash: CRO_ERR_EXEC.  out is filled whatever the helper's status (CRO_ERR_CUDA included);
+ * *helper_ns (may be NULL) and out->helper_ns: the helper's spawn to exit. */
+int  cro_check_health_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_health_opts *opts, int deadline_ms,
+                           cro_health_result *out, cro_health_records *rec, uint64_t *helper_ns);
+
+/* Test hook: the stop and status rules, a pure function.  checks: the selection (0: all); statuses[0 .. n): what the
+ * first n checks to run returned, in run order.  Writes out's status, checks, ran, failed, errored, not_run and
+ * check_status (the rest untouched) and *next: the CRO_HEALTH_* bit of the check to run next, 0 when none is left.
+ * CRO_ERR_INVALID_ARG for bits outside CRO_HEALTH_ALL, a NULL array it needs, or more statuses than checks the rules
+ * let run. */
+int  cro_selftest_health_classify(uint32_t checks, const int32_t *statuses, int n, cro_health_result *out, uint32_t *next);
+
 /* ---- emit: encoding/json-compatible writers ------------------------------ */
 
 /* ComposableResourceStatus (api/v1alpha1/composableresource_types.go:36-41):
@@ -1679,6 +1806,14 @@ int  cro_emit_sram_annotations_json(const cro_sram_result *r, char *buf, size_t 
  * separated; when a1_bad / a2_bad > 0), -a2-holes (when a2_holes > 0), -overflow ("1"), -health (the flags' names
  * sram-corrected, sram-uncorrected, l2-corrected, l2-uncorrected, threshold-exceeded, l2-bucket, comma-separated). */
 int  cro_emit_l2_annotations_json(const cro_l2_result *r, char *buf, size_t cap, size_t *len);
+
+/* Annotations of a health result, one Go-marshalled map: every check that ran contributes its own annotations,
+ * unchanged (cro_emit_*_annotations_json of its result), and the call adds cohdi.io/probe-health-*: -verdict ("ok" for
+ * CRO_OK; "fail" for CRO_ERR_CHECKSUM; "cuda-error:<n>" for CRO_ERR_CUDA, n the cuda_error of the first check that
+ * returned it, 0 for one whose result carries none; "error" otherwise), -failed, -errors, -not-run and -incomplete (the
+ * names compute, precision, sram, l2, link, scan of those checks, in run order, comma-separated; each only when it
+ * names any) and -ms (helper_ns, or the checks' summed check_ns when helper_ns is 0, in ms, integer division). */
+int  cro_emit_health_annotations_json(const cro_health_result *r, char *buf, size_t cap, size_t *len);
 
 /* (deviceID, CDIDeviceID) from an FM ScaleUpResponse body, with the
  * res_op_status gate of internal/cdi/fti/fm/client.go:184-213.  On the error
