@@ -338,6 +338,43 @@ class PrecisionFault(ctypes.Structure):
                 ("expected", ctypes.c_int64), ("actual_bits", ctypes.c_uint64)]
 
 
+# SM sparse probe (cro_probe_sparse, cro_sparse_expected); verdicts and marks are COMPUTE_*
+SPARSE_LEG_S8, SPARSE_LEG_E4M3, SPARSE_LEG_E5M2, SPARSE_LEG_BF16, SPARSE_LEG_F16, SPARSE_LEG_TF32 = range(6)
+SPARSE_LEGS, SPARSE_ALL_LEGS = 6, 0x3F
+SPARSE_ANSWER_S8, SPARSE_ANSWER_SMALL, SPARSE_ANSWER_SMALL256, SPARSE_ANSWER_SMALL128 = range(4)
+SPARSE_ANSWERS = 4
+SPARSE_M, SPARSE_N, SPARSE_K, SPARSE_K16, SPARSE_TF32_K = 128, 256, 512, 256, 128
+SPARSE_RECORDS, SPARSE_MAX_SMS, SPARSE_MAX_ITERATIONS, SPARSE_MAX_ROUNDS = 4096, 256, 65536, 64
+
+
+class SparseOpts(ctypes.Structure):
+    _fields_ = [("iterations", ctypes.c_uint32), ("legs", ctypes.c_uint32), ("max_rounds", ctypes.c_uint32),
+                ("test_inject_leg", ctypes.c_int32), ("test_inject_sm", ctypes.c_int32),
+                ("test_inject_iteration", ctypes.c_uint32), ("test_inject_row", ctypes.c_int32),
+                ("test_inject_col", ctypes.c_int32), ("test_inject_mask", ctypes.c_uint64), ("test_meta", ctypes.c_uint32),
+                ("test_meta_leg", ctypes.c_int32), ("test_meta_sm", ctypes.c_int32), ("test_meta_iteration", ctypes.c_uint32),
+                ("test_meta_row", ctypes.c_uint32), ("test_meta_group", ctypes.c_uint32)]
+
+
+class SparseResult(ctypes.Structure):
+    """cro_sparse_result: status, verdict and per-leg counts, coverage and times of one sparse probe call."""
+    _fields_ = [("status", ctypes.c_int32), ("verdict", ctypes.c_uint32), ("seed", ctypes.c_uint64),
+                ("call", ctypes.c_uint64), ("sm_count", ctypes.c_uint32), ("legs", ctypes.c_uint32),
+                ("host_ref_ns", ctypes.c_uint64), ("nsmid", ctypes.c_uint32), ("bad_sms", ctypes.c_uint32),
+                ("bad_sm", ctypes.c_uint16 * 16), ("leg", ComputeLeg * SPARSE_LEGS)]
+
+
+class SparseSm(ctypes.Structure):
+    """One SM seen by a sparse probe call, with its counts, times and COMPUTE_PERSISTENT / _INTERMITTENT mark per leg."""
+    _fields_ = [("smid", ctypes.c_uint32), ("reserved", ctypes.c_uint32), ("leg", ComputeSmLeg * SPARSE_LEGS)]
+
+
+class SparseFault(ctypes.Structure):
+    """One wrong element of a last iteration's answer: leg, SM, row, column, the exact answer and the raw 32 bits got."""
+    _fields_ = [("leg", ctypes.c_uint32), ("smid", ctypes.c_uint32), ("row", ctypes.c_uint32), ("col", ctypes.c_uint32),
+                ("expected", ctypes.c_int32), ("actual_bits", ctypes.c_uint32)]
+
+
 # whole-HBM scan (cro_scan_hbm, cro_scan_hbm_uuid, cro_read_hbm_health)
 SCAN_CHUNK_BYTES, SCAN_RESERVE_BYTES, SCAN_MAX_CHUNKS, SCAN_PASSES, SCAN_ELEMENTS = 2 << 30, 1 << 30, 128, 2, 4
 (SCAN_HEALTH_ECC_CORRECTED_DURING, SCAN_HEALTH_ECC_UNCORRECTED_DURING, SCAN_HEALTH_REMAP_PENDING,
@@ -552,7 +589,7 @@ class L2Fault(ctypes.Structure):
 
 # test hooks: the compute, precision and SRAM probes' classification of caller-given rounds
 # (cro_selftest_sm_legs_classify, cro_selftest_sram_classify)
-SM_LEGS_COMPUTE, SM_LEGS_PRECISION = 0, 1
+SM_LEGS_COMPUTE, SM_LEGS_PRECISION, SM_LEGS_SPARSE = 0, 1, 3
 
 
 class SmCta(ctypes.Structure):
@@ -610,6 +647,8 @@ assert ctypes.sizeof(ProbeResult) == 512, ctypes.sizeof(ProbeResult)
 assert ctypes.sizeof(ComputeResult) == 600 and ctypes.sizeof(ComputeSm) == 208, ctypes.sizeof(ComputeResult)
 assert ctypes.sizeof(PrecisionResult) == 808 and ctypes.sizeof(PrecisionSm) == 288 and ctypes.sizeof(PrecisionFault) == 32 \
     and ctypes.sizeof(PrecisionOpts) == 48, ctypes.sizeof(PrecisionResult)
+assert ctypes.sizeof(SparseResult) == 704 and ctypes.sizeof(SparseSm) == 248 and ctypes.sizeof(SparseFault) == 24 \
+    and ctypes.sizeof(SparseOpts) == 64, ctypes.sizeof(SparseResult)
 assert ctypes.sizeof(FaultReport) == 928 and ctypes.sizeof(LocatePass) == 120, ctypes.sizeof(FaultReport)
 assert ctypes.sizeof(LinkResult) == 984 and ctypes.sizeof(PciPath) == 272, ctypes.sizeof(LinkResult)
 assert ctypes.sizeof(ScanReport) == 12632 and ctypes.sizeof(ScanOpts) == 72, ctypes.sizeof(ScanReport)
@@ -677,6 +716,7 @@ EXPORTS = [
     "cro_probe_host_link", "cro_probe_host_link_uuid", "cro_pci_link_path", "cro_emit_link_annotations_json",
     "cro_probe_compute", "cro_probe_compute_uuid", "cro_compute_expected", "cro_emit_compute_annotations_json",
     "cro_probe_precision", "cro_probe_precision_uuid", "cro_precision_expected", "cro_emit_precision_annotations_json",
+    "cro_probe_sparse", "cro_probe_sparse_uuid", "cro_sparse_expected", "cro_emit_sparse_annotations_json",
     "cro_scan_hbm", "cro_scan_hbm_uuid", "cro_read_hbm_health", "cro_emit_scan_annotations_json",
     "cro_probe_sram", "cro_probe_sram_uuid", "cro_read_sram_health", "cro_emit_sram_annotations_json",
     "cro_probe_l2", "cro_probe_l2_uuid", "cro_read_l2_health", "cro_emit_l2_annotations_json", "cro_selftest_l2_classify",
@@ -818,6 +858,13 @@ def _load() -> ctypes.CDLL:
                                            ctypes.POINTER(PrecisionSm), i32, ctypes.POINTER(i32), ctypes.POINTER(PrecisionFault),
                                            i32, ctypes.POINTER(i32), ctypes.POINTER(u64)]),
         "cro_precision_expected": (i32, [i32, u64, ctypes.POINTER(ctypes.c_int64)]),
+        "cro_probe_sparse": (i32, [vp, i32, ctypes.POINTER(SparseOpts), ctypes.POINTER(SparseResult), ctypes.POINTER(SparseSm),
+                                   i32, ctypes.POINTER(i32), ctypes.POINTER(SparseFault), i32, ctypes.POINTER(i32)]),
+        "cro_probe_sparse_uuid": (i32, [vp, c, ctypes.POINTER(SparseOpts), i32, ctypes.POINTER(SparseResult),
+                                        ctypes.POINTER(SparseSm), i32, ctypes.POINTER(i32), ctypes.POINTER(SparseFault), i32,
+                                        ctypes.POINTER(i32), ctypes.POINTER(u64)]),
+        "cro_sparse_expected": (i32, [i32, u64, ctypes.POINTER(ctypes.c_int32)]),
+        "cro_emit_sparse_annotations_json": (i32, [ctypes.POINTER(SparseResult)] + out),
         "cro_emit_precision_annotations_json": (i32, [ctypes.POINTER(PrecisionResult)] + out),
         "cro_scan_hbm": (i32, [vp, i32, ctypes.POINTER(ScanOpts), ctypes.POINTER(ScanReport), ctypes.POINTER(FaultWord), i32,
                                ctypes.POINTER(i32)]),
@@ -1001,6 +1048,11 @@ def emit_compute_annotations_json(r: ComputeResult) -> str:
     return _text(lib.cro_emit_compute_annotations_json, ctypes.byref(r))
 
 
+def emit_sparse_annotations_json(r: SparseResult) -> str:
+    """Additive cohdi.io/probe-sparse-* annotations of a probe_sparse result (Go-marshalled map[string]string)."""
+    return _text(lib.cro_emit_sparse_annotations_json, ctypes.byref(r))
+
+
 def emit_precision_annotations_json(r: PrecisionResult) -> str:
     """Additive cohdi.io/probe-precision-* annotations of a probe_precision result (Go-marshalled map[string]string)."""
     return _text(lib.cro_emit_precision_annotations_json, ctypes.byref(r))
@@ -1098,14 +1150,14 @@ def _legs_rounds(n_legs: int, legs: int, rounds, claims, records, cta, words: in
 
 def selftest_sm_legs_classify(probe: int, iterations: List[int], grid: int, call: int, rounds, claims: List[int],
                               records, legs: int = 0):
-    """cro_selftest_sm_legs_classify: the compute (SM_LEGS_COMPUTE) or precision probe's classification of call `call`
-    on `grid` SMs.  Per leg l (every list is indexed by leg; legs 0: all): rounds[l] a list of (grid SmCta, the
-    COMPUTE_MAX_SMS // 64 coverage words) per round, claims[l] and records[l] (ComputeFault / PrecisionFault, the first
-    min(claims[l], RECORDS)).  Returns (result, SM entries, faults); the result's status may be OK, ERR_CHECKSUM or
-    ERR_UNSUPPORTED."""
-    compute = probe == SM_LEGS_COMPUTE
-    n_legs = COMPUTE_LEGS if compute else PRECISION_LEGS
-    result, sm, fault = (ComputeResult, ComputeSm, ComputeFault) if compute else (PrecisionResult, PrecisionSm, PrecisionFault)
+    """cro_selftest_sm_legs_classify: the compute (SM_LEGS_COMPUTE), precision (SM_LEGS_PRECISION) or sparse
+    (SM_LEGS_SPARSE) probe's classification of call `call` on `grid` SMs.  Per leg l (every list is indexed by leg; legs
+    0: all): rounds[l] a list of (grid SmCta, the COMPUTE_MAX_SMS // 64 coverage words) per round, claims[l] and
+    records[l] (ComputeFault / PrecisionFault / SparseFault, the first min(claims[l], RECORDS)).  Returns (result, SM
+    entries, faults); the result's status may be OK, ERR_CHECKSUM or ERR_UNSUPPORTED."""
+    n_legs, result, sm, fault = {SM_LEGS_COMPUTE: (COMPUTE_LEGS, ComputeResult, ComputeSm, ComputeFault),
+                                 SM_LEGS_SPARSE: (SPARSE_LEGS, SparseResult, SparseSm, SparseFault)}.get(
+        probe, (PRECISION_LEGS, PrecisionResult, PrecisionSm, PrecisionFault))
     ran = legs or (1 << n_legs) - 1
     nr, ctas, bits, cl, recs = _legs_rounds(n_legs, ran, rounds, claims, records, SmCta, COMPUTE_MAX_SMS // 64, fault)
     it = (ctypes.c_uint32 * n_legs)(*iterations)
@@ -1319,6 +1371,36 @@ def probe_precision_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: i
     return out + (ns.value,)
 
 
+def _sparse_opts(iterations: int, legs: int, max_rounds: int, inject: Optional[Tuple[int, int, int, int, int, int]],
+                 meta: Optional[Tuple[int, int, int, int, int]]) -> SparseOpts:
+    o = SparseOpts()
+    o.iterations, o.legs, o.max_rounds = iterations, legs, max_rounds
+    if inject is not None:
+        (o.test_inject_leg, o.test_inject_sm, o.test_inject_iteration, o.test_inject_row, o.test_inject_col,
+         o.test_inject_mask) = inject
+    if meta is not None:
+        o.test_meta = 1
+        o.test_meta_leg, o.test_meta_sm, o.test_meta_iteration, o.test_meta_row, o.test_meta_group = meta
+    return o
+
+
+def probe_sparse_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: int = 0, legs: int = SPARSE_ALL_LEGS,
+                      max_rounds: int = 0, deadline_ms: int = 0, inject: Optional[Tuple[int, int, int, int, int, int]] = None,
+                      meta: Optional[Tuple[int, int, int, int, int]] = None,
+                      cap: int = 256) -> Tuple[SparseResult, List[SparseSm], List[SparseFault], int]:
+    """cro_probe_sparse_uuid: the sparse probe of any GPU on the node, run by the helper process (ctx may be None).
+    Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen, up to `cap` element records
+    and the helper's spawn-to-exit time in ns."""
+    o = _sparse_opts(iterations, legs, max_rounds, inject, meta)
+    ns = ctypes.c_uint64()
+    handle = ctx.handle if ctx is not None else None
+    rc, out = _per_sm(lib.cro_probe_sparse_uuid, (handle, _b(uuid), ctypes.byref(o), deadline_ms), SparseResult, SparseSm,
+                      SPARSE_MAX_SMS, SparseFault, cap, (ctypes.byref(ns),))
+    if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
+        raise _helper_error(rc, handle)
+    return out + (ns.value,)
+
+
 def _scan_opts(max_bytes: int, reserve_bytes: int, seed: int, deadline_ms: int, chunk_bytes: int,
                force: Optional[Tuple[int, int, int, int]]) -> ScanOpts:
     o = ScanOpts()
@@ -1415,6 +1497,16 @@ def check_health_uuid(ctx: Optional["ProbeContext"], uuid: str, checks: int = 0,
     if rc != OK and r.ran == 0:         # refused, or the helper gave no result: no check ran
         raise _helper_error(rc, handle)
     return r, records, ns.value
+
+
+def sparse_expected(answer: int, seed: int) -> List[int]:
+    """cro_sparse_expected: the SPARSE_ANSWER_* answer tile of the operands of `seed`, SPARSE_M x SPARSE_N int32
+    values, row-major (host arithmetic, no GPU)."""
+    arr = (ctypes.c_int32 * (SPARSE_M * SPARSE_N))()
+    rc = lib.cro_sparse_expected(answer, seed, arr)
+    if rc != OK:
+        raise ProbeError(rc, "cro_sparse_expected")
+    return list(arr)
 
 
 def precision_expected(answer: int, seed: int) -> List[int]:
@@ -1676,6 +1768,21 @@ class ProbeContext:
         o = _precision_opts(iterations, alu_iterations, legs, max_rounds, inject)
         rc, out = _per_sm(lib.cro_probe_precision, (self.handle, dev, ctypes.byref(o)), PrecisionResult, PrecisionSm,
                           PRECISION_MAX_SMS, PrecisionFault, cap)
+        self._check(rc, allow=(ERR_CHECKSUM,))
+        return out
+
+    def probe_sparse(self, dev: int = 0, iterations: int = 0, legs: int = SPARSE_ALL_LEGS, max_rounds: int = 0,
+                     inject: Optional[Tuple[int, int, int, int, int, int]] = None,
+                     meta: Optional[Tuple[int, int, int, int, int]] = None,
+                     cap: int = 256) -> Tuple[SparseResult, List[SparseSm], List[SparseFault]]:
+        """cro_probe_sparse: every SM computes its answer tiles with 2:4 structured-sparsity wgmma in s8, E4M3, E5M2,
+        BF16, F16 and TF32 (1:2) and checks each value exactly.  iterations / max_rounds = 0: the defaults.  inject =
+        (leg, sm, iteration, row, col, mask) is the test-only accumulator XOR (sm, row, col: -1 for every one; mask at
+        most 32 bits); meta = (leg, sm, iteration, row, group) the test-only metadata substitution (sm -1: every SM).
+        Returns the result (its status is OK or ERR_CHECKSUM), one entry per SM seen and up to `cap` element records."""
+        o = _sparse_opts(iterations, legs, max_rounds, inject, meta)
+        rc, out = _per_sm(lib.cro_probe_sparse, (self.handle, dev, ctypes.byref(o)), SparseResult, SparseSm, SPARSE_MAX_SMS,
+                          SparseFault, cap)
         self._check(rc, allow=(ERR_CHECKSUM,))
         return out
 

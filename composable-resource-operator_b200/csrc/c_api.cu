@@ -64,6 +64,11 @@ static_assert(sizeof(cro_precision_opts) == 48 && offsetof(cro_precision_opts, t
                   sizeof(cro_precision_sm) == 288 && sizeof(cro_precision_fault) == 32 &&
                   offsetof(cro_precision_fault, actual_bits) == 24,
               "precision layout");
+static_assert(sizeof(cro_sparse_opts) == 64 && offsetof(cro_sparse_opts, test_inject_mask) == 32 &&
+                  offsetof(cro_sparse_opts, test_meta_group) == 60 && sizeof(cro_sparse_result) == 704 &&
+                  offsetof(cro_sparse_result, leg) == 80 && sizeof(cro_sparse_sm) == 248 && sizeof(cro_sparse_fault) == 24 &&
+                  offsetof(cro_sparse_fault, actual_bits) == 20,
+              "sparse layout");
 
 static_assert(sizeof(cro_scan_opts) == 72 && sizeof(cro_hbm_health) == 56 && sizeof(cro_scan_pass) == 552 &&
                   sizeof(cro_scan_chunk) == 88, "scan layout");
@@ -444,6 +449,23 @@ int cro_probe_precision_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_preci
         return rc;
     }).rc;
 } CRO_API_CATCH
+int cro_probe_sparse(cro_ctx* ctx, int i, const cro_sparse_opts* opts, cro_sparse_result* out, cro_sparse_sm* sms, int sms_cap,
+                     int* n_sms, cro_sparse_fault* faults, int cap, int* n) try {
+    return per_sm_call(ctx, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_sparse_opts& o, auto* seen, auto* found) {
+        return ctx_probe_sparse(ctx, i, o, out, seen, found);
+    }).rc;
+} CRO_API_CATCH
+int cro_probe_sparse_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_sparse_opts* opts, int deadline_ms, cro_sparse_result* out,
+                          cro_sparse_sm* sms, int sms_cap, int* n_sms, cro_sparse_fault* faults, int cap, int* n,
+                          uint64_t* helper_ns) try {
+    return per_sm_call(gpu_uuid, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_sparse_opts& o, auto* seen, auto* found) {
+        uint64_t ns = 0;
+        if (helper_ns) *helper_ns = 0;
+        const int rc = ctx_probe_sparse_uuid(ctx, gpu_uuid, o, deadline_ms, out, seen, found, cap, &ns);
+        if (helper_ns) *helper_ns = ns;
+        return rc;
+    }).rc;
+} CRO_API_CATCH
 int cro_scan_hbm(cro_ctx* ctx, int i, const cro_scan_opts* opts, cro_scan_report* out, cro_fault_word* words, int cap, int* n) try {
     if (!ctx || !out || !n || cap < 0 || (cap > 0 && !words)) return CRO_ERR_INVALID_ARG;
     *n = 0;
@@ -515,12 +537,16 @@ int cro_selftest_sm_legs_classify(int probe, uint32_t legs, const uint32_t* iter
                                   const uint32_t* rounds, const cro_sm_cta* ctas, const uint64_t* sm_bits, const uint64_t* claims,
                                   const void* records, void* out, void* sms, int sms_cap, int* n_sms, void* faults, int cap,
                                   int* n) try {
-    const uint32_t n_legs = probe == CRO_SM_LEGS_COMPUTE ? CRO_COMPUTE_LEGS : CRO_PRECISION_LEGS;
-    const uint32_t max_records = probe == CRO_SM_LEGS_COMPUTE ? CRO_COMPUTE_RECORDS : CRO_PRECISION_RECORDS;
+    const uint32_t n_legs = probe == CRO_SM_LEGS_COMPUTE  ? CRO_COMPUTE_LEGS
+                            : probe == CRO_SM_LEGS_SPARSE ? CRO_SPARSE_LEGS
+                                                          : CRO_PRECISION_LEGS;
+    const uint32_t max_records = probe == CRO_SM_LEGS_COMPUTE ? CRO_COMPUTE_RECORDS
+                                 : probe == CRO_SM_LEGS_SPARSE ? CRO_SPARSE_RECORDS
+                                                               : CRO_PRECISION_RECORDS;
     const uint32_t all = (1u << n_legs) - 1;
     if (legs == 0) legs = all;
-    if ((probe != CRO_SM_LEGS_COMPUTE && probe != CRO_SM_LEGS_PRECISION) || (legs & ~all) || !iterations || !rounds || !claims ||
-        grid == 0 || !out || !n_sms || !n || sms_cap < 0 || cap < 0 || (sms_cap > 0 && !sms) || (cap > 0 && !faults))
+    if ((probe != CRO_SM_LEGS_COMPUTE && probe != CRO_SM_LEGS_PRECISION && probe != CRO_SM_LEGS_SPARSE) || (legs & ~all) ||
+        !iterations || !rounds || !claims || grid == 0 || !out || !n_sms || !n || sms_cap < 0 || cap < 0 || (sms_cap > 0 && !sms) || (cap > 0 && !faults))
         return CRO_ERR_INVALID_ARG;
     uint64_t n_rounds = 0, n_records = 0;
     for (uint32_t l = 0; l < n_legs; ++l) {
@@ -539,6 +565,16 @@ int cro_selftest_sm_legs_classify(int probe, uint32_t legs, const uint32_t* iter
                                         &seen, &found);
         copy_capped(seen, static_cast<cro_compute_sm*>(sms), sms_cap, n_sms);
         copy_capped(found, static_cast<cro_compute_fault*>(faults), cap, n);
+        return rc;
+    }
+    if (probe == CRO_SM_LEGS_SPARSE) {
+        std::vector<cro_sparse_sm> seen;
+        std::vector<cro_sparse_fault> found;
+        const int rc = classify_sparse(legs, iterations, grid, call, rounds, ctas, sm_bits, claims,
+                                       static_cast<const cro_sparse_fault*>(records), static_cast<cro_sparse_result*>(out), &seen,
+                                       &found);
+        copy_capped(seen, static_cast<cro_sparse_sm*>(sms), sms_cap, n_sms);
+        copy_capped(found, static_cast<cro_sparse_fault*>(faults), cap, n);
         return rc;
     }
     std::vector<cro_precision_sm> seen;
@@ -711,6 +747,9 @@ int cro_compute_expected(int answer, uint64_t seed, int32_t* out) try {
 } CRO_API_CATCH
 int cro_precision_expected(int answer, uint64_t seed, int64_t* out) try {
     return precision::Expected(answer, seed, out);
+} CRO_API_CATCH
+int cro_sparse_expected(int answer, uint64_t seed, int32_t* out) try {
+    return sparse::Expected(answer, seed, out);
 } CRO_API_CATCH
 int cro_pci_link_path(const char* sys_root, const char* pci_bus_id, cro_pci_path* out) try {
     if (!pci_bus_id || !out) return CRO_ERR_INVALID_ARG;
@@ -926,7 +965,7 @@ static void ecc_delta(Annotations& m, const std::string& p, const Health& B, con
 }
 static std::string cuda_error(int32_t e) { return "cuda-error:" + std::to_string(e); }
 
-// The compute and precision results both hold a cro_compute_leg per leg.  Their annotations differ only in the key
+// The compute, precision and sparse results all hold a cro_compute_leg per leg.  Their annotations differ only in the key
 // prefix p, the leg names and which legs report a rate under which key.
 struct LegRate {
     int leg;
@@ -1119,6 +1158,14 @@ static Annotations precision_annotations(const cro_precision_result& r) {
                                 {CRO_PRECISION_LEG_E5M2, "e5m2-gflops"}});
 }
 
+static Annotations sparse_annotations(const cro_sparse_result& r) {
+    static const char* const kLeg[CRO_SPARSE_LEGS] = {"s8", "e4m3", "e5m2", "bf16", "f16", "tf32"};
+    return sm_legs_annotations(r, "cohdi.io/probe-sparse-", kLeg, CRO_SPARSE_LEGS,
+                               {{CRO_SPARSE_LEG_S8, "s8-gops"}, {CRO_SPARSE_LEG_E4M3, "e4m3-gflops"},
+                                {CRO_SPARSE_LEG_E5M2, "e5m2-gflops"}, {CRO_SPARSE_LEG_BF16, "bf16-gflops"},
+                                {CRO_SPARSE_LEG_F16, "f16-gflops"}, {CRO_SPARSE_LEG_TF32, "tf32-gflops"}});
+}
+
 // The health check's annotations: each check that ran, its own keys unchanged, and the call's cohdi.io/probe-health-*.
 static Annotations health_annotations(const cro_health_result& r) {
     static const char* const kName[CRO_HEALTH_CHECKS] = {"compute", "precision", "sram", "l2", "link", "scan"};
@@ -1189,6 +1236,11 @@ int cro_emit_compute_annotations_json(const cro_compute_result* r, char* buf, si
 int cro_emit_precision_annotations_json(const cro_precision_result* r, char* buf, size_t cap, size_t* len) try {
     if (!r) return CRO_ERR_INVALID_ARG;
     return emit(precision_annotations(*r), buf, cap, len);
+} CRO_API_CATCH
+
+int cro_emit_sparse_annotations_json(const cro_sparse_result* r, char* buf, size_t cap, size_t* len) try {
+    if (!r) return CRO_ERR_INVALID_ARG;
+    return emit(sparse_annotations(*r), buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_scan_annotations_json(const cro_scan_report* r, char* buf, size_t cap, size_t* len) try {

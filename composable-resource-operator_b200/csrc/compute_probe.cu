@@ -33,6 +33,9 @@ struct ComputeProbe {
     static uint64_t ops(uint32_t) { return 2ull * CRO_COMPUTE_M * CRO_COMPUTE_N * CRO_COMPUTE_K; }
     static cudaError_t launch(uint32_t leg, const ComputeArgs& a, int grid, cudaStream_t st) { return launch_compute(leg, a, grid, st); }
 
+    static void test_args(const cro_compute_opts&, uint32_t, ComputeArgs*) {}
+    static std::vector<std::string> helper_args(const cro_compute_opts& o) { return dense_helper_args(o); }
+
     static std::string opts_error(const cro_compute_opts& o) {
         const uint32_t legs = o.legs ? o.legs : CRO_COMPUTE_ALL_LEGS;
         uint32_t iters[CRO_COMPUTE_LEGS];

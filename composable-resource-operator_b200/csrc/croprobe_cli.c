@@ -41,6 +41,13 @@
  *                                                    compute-raw: cro_precision_result, uint64_t n_sms and n,
  *                                                    CRO_PRECISION_MAX_SMS cro_precision_sm entries, then n
  *                                                    cro_precision_fault records (at most cap) on stdout
+ *   croprobe-cli sparse-raw <uuid> <seed_base> <iterations> <legs> <max_rounds> <inject_leg> <inject_sm>
+ *                           <inject_iteration> <inject_row> <inject_col> <inject_mask> <meta> <meta_leg> <meta_sm>
+ *                           <meta_iteration> <meta_row> <meta_group> <cap>
+ *                                                    the sparse probe with every cro_sparse_opts field, as compute-raw:
+ *                                                    cro_sparse_result, uint64_t n_sms and n, CRO_SPARSE_MAX_SMS
+ *                                                    cro_sparse_sm entries, then n cro_sparse_fault records (at most
+ *                                                    cap) on stdout
  *   croprobe-cli l2-raw <uuid> <seed_base> <bytes> <iterations> <a1_counters> <a2_counters> <inject_leg> <inject_sm>
  *                       <inject_element> <inject_iteration> <inject_word> <inject_mask> <cap>
  *                                                    the L2 probe with every cro_l2_opts field but the deadline, NVML on
@@ -54,9 +61,9 @@
  *                                                    the seed base), its sweep region L, NVML on; the cro_health_result,
  *                                                    then each check that ran, in run order, as its own -raw writes it
  *   croprobe-cli health <uuid|index>                 the health check with defaults; JSON annotations, exit 0 iff ok
- *   link-raw, compute-raw, precision-raw, l2-raw and health-raw take cro_opts.seed_base from argv (the device seed is seed_base | minor, as in process), so
- *   that the library can give every helper call fresh patterns and operands; their counts are the helper's own,
- *   because neither result says how many records follow.
+ *   link-raw, compute-raw, precision-raw, sparse-raw, l2-raw and health-raw take cro_opts.seed_base from argv (the
+ *   device seed is seed_base | minor, as in process), so that the library can give every helper call fresh patterns
+ *   and operands; their counts are the helper's own, because neither result says how many records follow.
  * Exit 3: the device is not visible to this (fresh) process — the reference's found=false.  The raw commands exit 0
  * iff the probe's status is CRO_OK, 1 for any other status (the result on stdout says which), 64 for a wrong argument
  * count.
@@ -114,6 +121,10 @@ static int put_precision(const cro_precision_result *r, const cro_precision_sm *
                          int n) {
     const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)n};
     return put_frame(r, sizeof *r, counts, 2, sms, CRO_PRECISION_MAX_SMS * sizeof *sms, f, sizeof *f, n);
+}
+static int put_sparse(const cro_sparse_result *r, const cro_sparse_sm *sms, int n_sms, const cro_sparse_fault *f, int n) {
+    const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)n};
+    return put_frame(r, sizeof *r, counts, 2, sms, CRO_SPARSE_MAX_SMS * sizeof *sms, f, sizeof *f, n);
 }
 static int put_l2(const cro_l2_result *r, const cro_l2_sm *sms, int n_sms, const cro_l2_fault *f, int n) {
     const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)n};
@@ -262,6 +273,35 @@ static int precision_raw(cro_ctx *ctx, int idx, char **argv) {
     return put_precision(&pr, sms, n_sms, faults, got) ? 2 : end_frames(pr.status);
 }
 
+static int sparse_raw(cro_ctx *ctx, int idx, char **argv) {
+    char **a = argv + 4;
+    cro_sparse_opts so;
+    memset(&so, 0, sizeof so);
+    so.iterations = (uint32_t)strtoul(a[0], NULL, 10);
+    so.legs = (uint32_t)strtoul(a[1], NULL, 10);
+    so.max_rounds = (uint32_t)strtoul(a[2], NULL, 10);
+    so.test_inject_leg = atoi(a[3]);
+    so.test_inject_sm = atoi(a[4]);
+    so.test_inject_iteration = (uint32_t)strtoul(a[5], NULL, 10);
+    so.test_inject_row = atoi(a[6]);
+    so.test_inject_col = atoi(a[7]);
+    so.test_inject_mask = strtoull(a[8], NULL, 10);
+    so.test_meta = (uint32_t)strtoul(a[9], NULL, 10);
+    so.test_meta_leg = atoi(a[10]);
+    so.test_meta_sm = atoi(a[11]);
+    so.test_meta_iteration = (uint32_t)strtoul(a[12], NULL, 10);
+    so.test_meta_row = (uint32_t)strtoul(a[13], NULL, 10);
+    so.test_meta_group = (uint32_t)strtoul(a[14], NULL, 10);
+    const int cap = atoi(argv[19]);
+    static cro_sparse_result sr;
+    static cro_sparse_sm sms[CRO_SPARSE_MAX_SMS];
+    cro_sparse_fault *faults = (cro_sparse_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
+    int n_sms = 0, got = 0;
+    if (!faults) return 2;
+    cro_probe_sparse(ctx, idx, &so, &sr, sms, CRO_SPARSE_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
+    return put_sparse(&sr, sms, n_sms, faults, got) ? 2 : end_frames(sr.status);
+}
+
 static int l2_raw(cro_ctx *ctx, int idx, char **argv) {
     cro_l2_opts lo;
     memset(&lo, 0, sizeof lo);
@@ -394,6 +434,7 @@ static const struct command {
     /* no health record to read, and NVML's first call is slow */
     {"compute-raw", 15, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, 1, compute_raw},
     {"precision-raw", 15, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, 1, precision_raw},
+    {"sparse-raw", 20, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, 1, sparse_raw},
     /* every check of one device: the link check's region (exactly L, argv[49], when it is given) and NVML for the scan's,
      * SRAM's and L2's health records and the link's replay counters */
     {"health-raw", H_ARGC, CRO_F_LAZY_ALLOC, 256, 1, health_raw},
@@ -408,7 +449,8 @@ int main(int argc, char **argv) {
                         "<word> <mask> <cap> | link-raw <uuid> <seed_base> <bytes> <hops> <ctas> <check> <word> <mask> <cap> | "
                         "compute-raw <uuid> <seed_base> <iterations> <alu_iterations> <legs> <rounds> <leg> <sm> <iteration> <row> <col> "
                         "<mask> <cap> | precision-raw <uuid> <seed_base> <iterations> <alu_iterations> <legs> <rounds> <leg> <sm> <iteration> <row> "
-                        "<col> <mask> <cap> | l2-raw <uuid> <seed_base> <bytes> <iterations> <a1> <a2> <leg> <sm> <element> <iteration> <word> <mask> <cap> | "
+                        "<col> <mask> <cap> | sparse-raw <uuid> <seed_base> <iterations> <legs> <rounds> <leg> <sm> <iteration> <row> <col> "
+                        "<mask> <meta> <meta_leg> <meta_sm> <meta_iteration> <meta_row> <meta_group> <cap> | l2-raw <uuid> <seed_base> <bytes> <iterations> <a1> <a2> <leg> <sm> <element> <iteration> <word> <mask> <cap> | "
                         "health-raw <uuid> <seed_base> <checks> <compute-raw, precision-raw, sram-raw, l2-raw, link-raw, scan-raw options "
                         "and caps> | health <uuid|index>\n");
         return 64;

@@ -130,6 +130,9 @@ struct PrecisionProbe {
     }
     static cudaError_t launch(uint32_t leg, const PrecisionArgs& a, int grid, cudaStream_t st) { return launch_precision(leg, a, grid, st); }
 
+    static void test_args(const cro_precision_opts&, uint32_t, PrecisionArgs*) {}
+    static std::vector<std::string> helper_args(const cro_precision_opts& o) { return dense_helper_args(o); }
+
     static std::string opts_error(const cro_precision_opts& o) {
         const uint32_t legs = o.legs ? o.legs : CRO_PRECISION_ALL_LEGS;
         uint32_t iters[CRO_PRECISION_LEGS];

@@ -81,6 +81,7 @@ struct Device {
     uint64_t sram_calls = 0;               // k of the next SRAM probe call (ctx_probe_sram): its seeds
     uint64_t l2_calls = 0;                 // k of the next L2 probe call (ctx_probe_l2): its seeds
     uint64_t precision_calls = 0;          // k of the next precision probe call (ctx_probe_precision): its operand seed
+    uint64_t sparse_calls = 0;             // k of the next sparse probe call (ctx_probe_sparse): its operand seed
     KernelPlan plan{};
     SweepScratch scratch{}, scratch_aux{}, scratch_pfx{};   // main stream / closed form / p2p prefix closed form
     // lane 0's buffers under their old names: the synchronous probe, the single sweeps and cro_probe_all use lane 0
@@ -259,6 +260,20 @@ int classify_compute(uint32_t legs, const uint32_t* iterations, uint32_t grid, u
 int classify_precision(uint32_t legs, const uint32_t* iterations, uint32_t grid, uint64_t k, const uint32_t* rounds,
                        const cro_sm_cta* ctas, const uint64_t* sm_bits, const uint64_t* claims, const cro_precision_fault* records,
                        cro_precision_result* r, std::vector<cro_precision_sm>* sms, std::vector<cro_precision_fault>* faults);
+// SM sparse probe (include/croprobe.h, cro_probe_sparse / cro_probe_sparse_uuid, sparse_probe.cu): as the compute
+// probe's two forms; the uuid form runs `croprobe-cli sparse-raw`.
+int ctx_probe_sparse(cro_ctx* c, int idx, const cro_sparse_opts& o, cro_sparse_result* r, std::vector<cro_sparse_sm>* sms,
+                     std::vector<cro_sparse_fault>* faults);
+int ctx_probe_sparse_uuid(cro_ctx* c, const char* uuid, const cro_sparse_opts& o, int deadline_ms, cro_sparse_result* r,
+                          std::vector<cro_sparse_sm>* sms, std::vector<cro_sparse_fault>* faults, int cap, uint64_t* helper_ns);
+int classify_sparse(uint32_t legs, const uint32_t* iterations, uint32_t grid, uint64_t k, const uint32_t* rounds,
+                    const cro_sm_cta* ctas, const uint64_t* sm_bits, const uint64_t* claims, const cro_sparse_fault* records,
+                    cro_sparse_result* r, std::vector<cro_sparse_sm>* sms, std::vector<cro_sparse_fault>* faults);
+namespace sparse {
+// The answer tile of the operands of `seed` (include/croprobe.h): answer CRO_SPARSE_ANSWER_*, M x N int32 values,
+// row-major.  CRO_ERR_INVALID_ARG for another answer.
+int Expected(int answer, uint64_t seed, int32_t* out);
+}  // namespace sparse
 namespace precision {
 // The answer tile of the operands of `seed` (include/croprobe.h): answer CRO_PRECISION_ANSWER_*, M x N int64 values,
 // row-major.  CRO_ERR_INVALID_ARG for another answer.

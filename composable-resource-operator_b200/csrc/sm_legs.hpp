@@ -1,7 +1,8 @@
-// sm_legs.hpp — the host side the per-SM arithmetic probes (the compute probe, compute_probe.cu, and the precision
-// probe, precision_probe.cu) share: what one round's CTA records add to a leg and to its SMs, the marks and the slowest
-// SM of a finished leg, the call's verdict, and the in-process and helper forms of a call.  Sm is cro_compute_sm or
-// cro_precision_sm (smid and leg[], one cro_compute_sm_leg per leg); the leg totals are a cro_compute_leg in both.
+// sm_legs.hpp — the host side the per-SM arithmetic probes (the compute probe, compute_probe.cu, the precision probe,
+// precision_probe.cu, and the sparse probe, sparse_probe.cu) share: what one round's CTA records add to a leg and to
+// its SMs, the marks and the slowest SM of a finished leg, the call's verdict, and the in-process and helper forms of a
+// call.  Sm is cro_compute_sm, cro_precision_sm or cro_sparse_sm (smid and leg[], one cro_compute_sm_leg per leg); the
+// leg totals are a cro_compute_leg in all three.
 #pragma once
 #include <algorithm>
 #include <map>
@@ -151,14 +152,18 @@ int take_leg(cro_ctx* c, const char* who, const std::vector<ComputeCta>& hc, con
 // What a probe P gives the calls below:
 //   Opts, Result, Sm, Fault, Args    its option, result, per-SM, record and kernel argument types
 //   Tile                             the element type of its answer tiles (Args::expect points into them)
-//   kName                            "compute", "precision": "<kName> probe" in error texts, croprobe-cli <kName>-raw
+//   kName                            "compute", "precision", "sparse": "<kName> probe" in error texts, croprobe-cli
+//                                    <kName>-raw
 //   kLegs, kAllLegs, kMaxSms, kRecords, kAnswers, kCalls (its call counter in Device), kSeeds (its seed space)
-//   kDefaultIterations, kDefaultAluIterations, kDefaultRounds, kAluLeg[leg] (the leg runs alu_iterations)
+//   kDefaultIterations, kDefaultRounds, kAluLeg[leg] (the leg runs alu_iterations; with any such leg, Opts has
+//                                    alu_iterations and P kDefaultAluIterations)
 //   elements(answer), expected(answer, seed, out), fold(answer, tile)   an answer's tile: size, values, the fold one
 //                                                                       iteration of a CTA adds when all is right
 //   answer(leg), ops(leg)            a leg's answer and operations per CTA and iteration
 //   launch(leg, args, grid, stream)  one launch of a leg
 //   opts_error(opts)                 why the options are refused ("" when they pass), both forms' argument check
+//   test_args(opts, leg, &args)      the launch's test fields beyond the accumulator injection (none: an empty body)
+//   helper_args(opts)                the option fields of the helper's argv, between the seed base and the cap
 
 // The result of a call that computed nothing: zeroes but for what the call had settled before it stopped (`from`'s
 // seed, call number, SM count and legs).
@@ -173,12 +178,33 @@ void blank_result(Result* r, const Result from, std::vector<Sm>* sms, std::vecto
     faults->clear();
 }
 
+template <class P>
+constexpr bool has_alu_legs() {
+    for (bool alu : P::kAluLeg)
+        if (alu) return true;
+    return false;
+}
+
 // Iterations per CTA of each leg: the options' or the defaults.
 template <class P>
 void leg_iterations(const typename P::Opts& o, uint32_t (&iters)[P::kLegs]) {
     const uint32_t ti = o.iterations ? o.iterations : P::kDefaultIterations;
-    const uint32_t ai = o.alu_iterations ? o.alu_iterations : P::kDefaultAluIterations;
-    for (uint32_t l = 0; l < P::kLegs; ++l) iters[l] = P::kAluLeg[l] ? ai : ti;
+    for (uint32_t l = 0; l < P::kLegs; ++l) iters[l] = ti;
+    if constexpr (has_alu_legs<P>()) {
+        const uint32_t ai = o.alu_iterations ? o.alu_iterations : P::kDefaultAluIterations;
+        for (uint32_t l = 0; l < P::kLegs; ++l)
+            if (P::kAluLeg[l]) iters[l] = ai;
+    }
+}
+
+// The option fields of compute-raw's and precision-raw's argv.
+template <class Opts>
+std::vector<std::string> dense_helper_args(const Opts& o) {
+    using std::to_string;
+    return {to_string(o.iterations),      to_string(o.alu_iterations),        to_string(o.legs),
+            to_string(o.max_rounds),      to_string(o.test_inject_leg),       to_string(o.test_inject_sm),
+            to_string(o.test_inject_iteration), to_string(o.test_inject_row), to_string(o.test_inject_col),
+            to_string(o.test_inject_mask)};
 }
 
 // The in-process form: call k of the device gets the seed space_seed(d, P::kSeeds, k), its answer tiles computed here
@@ -257,6 +283,7 @@ int probe_sm_legs(cro_ctx* c, int idx, const typename P::Opts& o, typename P::Re
             a.inj_col = o.test_inject_col;
             a.inj_iter = o.test_inject_iteration;
             a.inj_mask = (inj && (uint32_t)o.test_inject_leg == leg) ? o.test_inject_mask : 0;
+            P::test_args(o, leg, &a);
             R.iterations = iters[leg];
             R.expect_fold = (uint64_t)iters[leg] * fold[answer];
             auto launch = [&] { return P::launch(leg, a, grid, st); };
@@ -337,7 +364,8 @@ int classify_sm_legs(uint32_t legs, const uint32_t* iterations, uint32_t grid, u
     return close_call(r, P::kLegs, per_sm, sms, faults);
 }
 
-// The helper form: `croprobe-cli <kName>-raw` with a fresh seed base (helper_seed_base), the options and cap on argv.
+// The helper form: `croprobe-cli <kName>-raw` with a fresh seed base (helper_seed_base), the options (helper_args) and
+// cap on argv.
 template <class P>
 int probe_sm_legs_uuid(cro_ctx* c, const char* uuid, const typename P::Opts& o, int deadline_ms, typename P::Result* r,
                        std::vector<typename P::Sm>* sms, std::vector<typename P::Fault>* faults, int cap, uint64_t* helper_ns) {
@@ -351,11 +379,10 @@ int probe_sm_legs_uuid(cro_ctx* c, const char* uuid, const typename P::Opts& o, 
     }
     const std::string want = uuid, name = P::kName;
     using std::to_string;
-    const std::vector<std::string> args = {name + "-raw", want, to_string(helper_seed_base(c)), to_string(o.iterations),
-                                           to_string(o.alu_iterations), to_string(o.legs), to_string(o.max_rounds),
-                                           to_string(o.test_inject_leg), to_string(o.test_inject_sm),
-                                           to_string(o.test_inject_iteration), to_string(o.test_inject_row),
-                                           to_string(o.test_inject_col), to_string(o.test_inject_mask), to_string(cap)};
+    std::vector<std::string> args = {name + "-raw", want, to_string(helper_seed_base(c))};
+    const std::vector<std::string> fields = P::helper_args(o);
+    args.insert(args.end(), fields.begin(), fields.end());
+    args.push_back(to_string(cap));
     using Frame = SmFrame<typename P::Result, typename P::Sm, typename P::Fault, P::kMaxSms>;
     std::string got;
     const int rc = run_probe_helper(c, want, name + " helper", ("cro.probe_" + name + ".helper").c_str(), args, deadline_ms,

@@ -1,7 +1,7 @@
-// sm_tile.cuh — what the per-SM arithmetic kernels share (the compute probe's, kernels.cu, and the precision probe's,
-// precision_kernels.cu): the PTX helpers, the K-major operand layout and its wgmma descriptor, the wgmma wrappers, the
-// injection each thread resolves once, and the CTA epilogue that publishes a ComputeCta.  kernels.cu's sweep kernels
-// use the same timer and shared-address helpers.
+// sm_tile.cuh — what the per-SM arithmetic kernels share (the compute probe's, kernels.cu, the precision probe's,
+// precision_kernels.cu, and the sparse probe's, sparse_kernels.cu): the PTX helpers, the K-major operand layout and its
+// wgmma descriptor, the wgmma wrappers, the injection each thread resolves once, and the CTA epilogue that publishes a
+// ComputeCta.  kernels.cu's sweep kernels use the same timer and shared-address helpers.
 #pragma once
 #include "kernels.cuh"
 
@@ -34,14 +34,15 @@ __device__ __forceinline__ unsigned long long wgmma_desc(unsigned addr, unsigned
 
 // The accumulator operands of a wgmma with 128 or 64 registers per thread: the instruction's register list followed
 // by its descriptor and scale-d operands (SM_TILE_ACC*), the index of the scale-d input (SM_TILE_SCALE*), and the
-// output bindings d[0 ..] under constraint c (SM_TILE_OUT*).
-#define SM_TILE_ACC128                                                                                                   \
+// output bindings d[0 ..] under constraint c (SM_TILE_OUT*).  SM_TILE_REGS128 is the register list alone.
+#define SM_TILE_ACC128 SM_TILE_REGS128 ", %128, %129, p"
+#define SM_TILE_REGS128                                                                                                  \
     "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "      \
     "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "  \
     "%47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, "  \
     "%70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, "  \
     "%93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, "    \
-    "%113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p"
+    "%113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}"
 #define SM_TILE_ACC64                                                                                                    \
     "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "      \
     "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "  \
@@ -63,6 +64,18 @@ __device__ __forceinline__ unsigned long long wgmma_desc(unsigned addr, unsigned
                      " " SM_TILE_ACC##N tail ";\n}\n"                                                                   \
                      : SM_TILE_OUT##N(c)                                                                                \
                      : "l"(da), "l"(db), "r"(scale_d));                                                                 \
+    }
+
+// name(d, da, db, meta, scale_d): one wgmma.mma_async.sp `shape` (sparse A) on 128 accumulators of type Acc bound as c,
+// with the sparsity metadata register meta and sparsity selector `sel` (an immediate, "0" or "1"), scale-d off when
+// scale_d is 0.  `tail` is as for SM_TILE_WGMMA.
+#define SM_TILE_WGMMA_SP(name, Acc, c, shape, sel, tail)                                                                 \
+    __device__ __forceinline__ void name(Acc (&d)[128], unsigned long long da, unsigned long long db, unsigned meta,     \
+                                         int scale_d) {                                                                 \
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %131, 0;\nwgmma.mma_async.sp.sync.aligned." shape " "          \
+                     SM_TILE_REGS128 ", %128, %129, %130, " sel ", p" tail ";\n}\n"                                     \
+                     : SM_TILE_OUT128(c)                                                                                \
+                     : "l"(da), "l"(db), "r"(meta), "r"(scale_d));                                                      \
     }
 
 // The injection of a launch (a.inj_*), resolved once by the thread owning rows r0 and r0 + 8 of SM smid: which of its

@@ -566,6 +566,75 @@ func (c *Context) ProbePrecision(deviceID string) (PrecisionResult, error) {
 	return precisionResult(&res, sms, nSMs, faults[:], got), nil
 }
 
+// SparseResult is the summary of cro_sparse_result an operator reads: whether
+// every SM computed the exact answer with 2:4 structured-sparsity wgmma in s8,
+// E4M3, E5M2, BF16, F16 and TF32 (1:2), and which SMs did not.
+type SparseResult struct {
+	OK          bool
+	Verdict     uint32            // CRO_COMPUTE_NONE / _SM / _ALL
+	SMCount     uint32
+	Covered     [6]uint32         // SMs seen per CRO_SPARSE_LEG_*
+	Mismatches  [6]uint64         // wrong elements of the last iteration, per leg
+	BadSMs      []uint32          // SMs that failed any leg, ascending
+	Faults      []SparseFault
+	Annotations string // Go-marshalled map[string]string of cohdi.io/probe-sparse-* keys
+}
+
+// SparseFault is one wrong element (cro_sparse_fault): the exact answer and
+// the accumulator's raw 32 bits (int32 for S8, f32 otherwise).
+type SparseFault struct {
+	Leg, SM, Row, Col uint32
+	Expected          int32
+	ActualBits        uint32
+}
+
+// ProbeSparseByUUID runs cro_probe_sparse_uuid with its defaults: the sparse
+// probe of any GPU on the node through the helper process, the form an
+// operator calls next to the compute and precision probes, before a freshly
+// composed GPU goes to a tenant running 2:4-pruned inference (INTEGRATION.md
+// §2h).  A mismatch or a failed launch (CRO_ERR_CUDA) is a result, not an
+// error; found is false when the node does not list the GPU.
+func (c *Context) ProbeSparseByUUID(deviceID string) (r SparseResult, found bool, err error) {
+	id := C.CString(deviceID)
+	defer C.free(unsafe.Pointer(id))
+	var res C.cro_sparse_result
+	sms := make([]C.cro_sparse_sm, C.CRO_SPARSE_MAX_SMS)
+	var faults [256]C.cro_sparse_fault
+	var nSMs, got C.int
+	rc := C.cro_probe_sparse_uuid(c.h, id, nil, 0, &res, &sms[0], C.CRO_SPARSE_MAX_SMS, &nSMs, &faults[0], 256, &got, nil)
+	if rc == C.CRO_ERR_NO_DEVICE {
+		return r, false, nil
+	}
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM && rc != C.CRO_ERR_CUDA {
+		return r, true, errorOf(c.h, rc)
+	}
+	r = SparseResult{OK: res.status == C.CRO_OK, Verdict: uint32(res.verdict), SMCount: uint32(res.sm_count)}
+	for l := 0; l < int(C.CRO_SPARSE_LEGS); l++ {
+		r.Covered[l] = uint32(res.leg[l].sms_covered)
+		r.Mismatches[l] = uint64(res.leg[l].mismatches)
+	}
+	for i := 0; i < int(nSMs); i++ {
+		for l := 0; l < int(C.CRO_SPARSE_LEGS); l++ {
+			if sms[i].leg[l].mark != 0 {
+				r.BadSMs = append(r.BadSMs, uint32(sms[i].smid))
+				break
+			}
+		}
+	}
+	for i := 0; i < int(got); i++ {
+		f := faults[i]
+		r.Faults = append(r.Faults, SparseFault{uint32(f.leg), uint32(f.smid), uint32(f.row), uint32(f.col),
+			int32(f.expected), uint32(f.actual_bits)})
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_sparse_annotations_json(&res, buf, 4096, &ln) == C.CRO_OK {
+		r.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return r, true, nil
+}
+
 // ScanResult is the summary of cro_scan_report an operator reads: whether every
 // free byte of the GPU's memory held what was written, how much was covered,
 // and the memory's own health record from NVML.

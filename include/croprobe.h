@@ -956,6 +956,139 @@ int  cro_probe_precision_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_prec
  * (128 x 64 for _WIDE, 128 x 256 otherwise), row-major.  Host arithmetic only; no context. */
 int  cro_precision_expected(int answer, uint64_t seed, int64_t *out);
 
+/* ---- SM sparse: every SM's 2:4 structured-sparsity tensor cores against an exact answer ---- */
+
+/*
+ * The compute and precision probes issue only dense wgmma.  In the sparse datapath (wgmma.mma_async.sp: IGMMA.SP,
+ * QGMMA.SP, HGMMA.SP) the tensor core reads a compressed A operand and a metadata register that says which rows of B
+ * each kept value meets; a fault in the metadata decode or the sparse operand routing wrongs only sparse work.  The
+ * sparse probe runs that path on every SM, one leg per format, shaped like the precision probe (one CTA per SM, one
+ * launch per leg, the same verdicts, marks, coverage rounds, slowest-SM report and guarantees: the device's mutex,
+ * probes in flight finish first, the sweep region untouched).
+ *
+ * Operands of call k on a device: seed = seed_dev + 2^57 + k * 0xD1B54A32D192ED03.  The logical A is M x K, sparse:
+ * in every group of G consecutive K positions of a row (G = 4, TF32: G = 2) two are kept (TF32: one); the compressed A
+ * holds the kept values, M x K/2, the lower kept index first.  With the leg's K, byte e means byte (e mod 8) of
+ * pattern_word(seed, e / 8), and
+ *   e = m * K/2 + c                                 for compressed A[m][c]
+ *   e = M * K/2 + k * N + n                         for B[k][n]
+ *   e = M * K/2 + K * N + m * ceil(K / G / P) + g / P    for the pair of group g of row m: (g + byte e) mod P
+ * P is the number of legal pairs: 6 for G = 4, in the order (0,1) (0,2) (0,3) (1,2) (1,3) (2,3), and 2 for TF32,
+ * (0) (1).  Every run of P consecutive groups of a row holds each pair once, so every pair appears in every call.  The
+ * metadata nibble of a pair (i, j) is i | j << 2; TF32's (0) and (1) are 0x4 and 0xE.  Values are read
+ *   s8         (int8_t)byte; a kept value of 0 is taken as 1                                  (S8)
+ *   small-int  (byte & 7) - 4 in -4 .. 3; a kept value v >= 0 is taken as v + 1 (so -4 .. 4, never 0)
+ *                                                                              (E4M3, E5M2, BF16, F16, TF32)
+ * so a kept value is never 0 and a wrong index changes the answer wherever the two rows of B differ.  D[m][n] = sum
+ * over the kept (k, value) of row m of value * B[k][n] is exact in any order of accumulation (DESIGN.md "The sparse
+ * probe"): K/2 products, each at most 2^14 (s8) or 16 (small-int), keep every partial sum within 2^22 (s8, int32) and
+ * 4096 (small-int, exact in f32's 24 bits; every operand is exact in e4m3, e5m2, bf16, f16 and tf32).
+ *
+ * Legs (M x N x logical K; every CTA has 256 threads, two warpgroups of 64 rows, and holds the compressed A and B^T,
+ * K-major, in 160 KiB of shared memory; eight .sp instructions per warpgroup per iteration):
+ *   S8    wgmma.sp m64n256k64 .s32.s8.s8 (IGMMA.SP)      128 x 256 x 512   s8 answer
+ *   E4M3  wgmma.sp m64n256k64 .f32.e4m3 (QGMMA.SP)       128 x 256 x 512   small-int answer at K = 512
+ *   E5M2  wgmma.sp m64n256k64 .f32.e5m2 (QGMMA.SP)       128 x 256 x 512   small-int answer at K = 512
+ *   BF16  wgmma.sp m64n256k32 .f32.bf16 (HGMMA.SP)       128 x 256 x 256   small-int answer at K = 256
+ *   F16   wgmma.sp m64n256k32 .f32.f16 (HGMMA.SP)        128 x 256 x 256   small-int answer at K = 256
+ *   TF32  wgmma.sp m64n256k16 .f32.tf32 (HGMMA.SP)       128 x 256 x 128   small-int answer at K = 128, 1:2
+ * BF16, F16 and TF32 alternate sparsity selector 0 and 1 over their eight K steps (the FP8 and s8 forms take only 0).
+ * Thread t holds 128 values; value j is the element row = r0(t) + 8 * ((j / 2) % 2), col = 8 * (j / 4) + 2 * (t % 4)
+ * + j % 2 with r0(t) = 64 * (t / 128) + 16 * ((t / 32) % 4) + (t % 32) / 4, the wgmma accumulator fragment.
+ *
+ * Compare: S8 values must equal the expected int32; the other legs' must be IEEE-equal to it as an f32.  Fold: after
+ * every iteration the thread adds canon(v) * (2e + 1) (mod 2^64) over its values, canon(v) the value's 32 bits (the
+ * f32 legs take -0 as 0), e = row * N + col; at the end it compares the running sum with iterations * the same sum
+ * over the expected values.
+ */
+#define CRO_SPARSE_LEG_S8           0
+#define CRO_SPARSE_LEG_E4M3         1
+#define CRO_SPARSE_LEG_E5M2         2
+#define CRO_SPARSE_LEG_BF16         3
+#define CRO_SPARSE_LEG_F16          4
+#define CRO_SPARSE_LEG_TF32         5
+#define CRO_SPARSE_LEGS             6
+#define CRO_SPARSE_ALL_LEGS         0x3Fu   /* bit l: leg l */
+#define CRO_SPARSE_ANSWER_S8        0       /* K = 512, s8: S8                   */
+#define CRO_SPARSE_ANSWER_SMALL     1       /* K = 512, small-int: E4M3, E5M2    */
+#define CRO_SPARSE_ANSWER_SMALL256  2       /* K = 256, small-int: BF16, F16     */
+#define CRO_SPARSE_ANSWER_SMALL128  3       /* K = 128, small-int, 1:2: TF32     */
+#define CRO_SPARSE_ANSWERS          4
+#define CRO_SPARSE_M                128
+#define CRO_SPARSE_N                256
+#define CRO_SPARSE_K                512     /* logical K of S8, E4M3, E5M2 */
+#define CRO_SPARSE_K16              256     /* ... of BF16, F16            */
+#define CRO_SPARSE_TF32_K           128     /* ... of TF32                 */
+#define CRO_SPARSE_RECORDS          4096    /* element records the device keeps per leg; counts stay exact beyond */
+#define CRO_SPARSE_MAX_SMS          256
+#define CRO_SPARSE_MAX_ITERATIONS   65536
+#define CRO_SPARSE_MAX_ROUNDS       64
+/* verdicts: CRO_COMPUTE_NONE / _SM / _ALL; marks: CRO_COMPUTE_PERSISTENT / _INTERMITTENT */
+
+typedef struct cro_sparse_opts {
+    uint32_t iterations;           /*   0  0 = the default, at most CRO_SPARSE_MAX_ITERATIONS                    */
+    uint32_t legs;                 /*   4  CRO_SPARSE_ALL_LEGS bits; 0 = all                                     */
+    uint32_t max_rounds;           /*   8  launches per leg while fewer than sm_count SMs were seen: 0 = 4       */
+    /* test only: as cro_precision_opts, the mask XORed into the accumulator's 32 bits after the iteration */
+    int32_t  test_inject_leg;      /*  12 */
+    int32_t  test_inject_sm;       /*  16 */
+    uint32_t test_inject_iteration;/*  20 */
+    int32_t  test_inject_row;      /*  24 */
+    int32_t  test_inject_col;      /*  28 */
+    uint64_t test_inject_mask;     /*  32  0: no accumulator injection; at most 32 bits wide                     */
+    /* test only: a metadata substitution.  In iteration test_meta_iteration on SM test_meta_sm (-1: every SM), leg
+       test_meta_leg gives group test_meta_group of row test_meta_row the next legal pair in the order above (the
+       last wraps to the first), the kept values unchanged: a legal pattern the tensor core decodes to a wrong answer */
+    uint32_t test_meta;            /*  40  0: none; 1: substitute                                                */
+    int32_t  test_meta_leg;        /*  44 */
+    int32_t  test_meta_sm;         /*  48 */
+    uint32_t test_meta_iteration;  /*  52 */
+    uint32_t test_meta_row;        /*  56  below CRO_SPARSE_M                                                   */
+    uint32_t test_meta_group;      /*  60  below K / G of the leg (128 for S8 / E4M3 / E5M2, 64 otherwise)       */
+} cro_sparse_opts;                 /*  64 bytes */
+
+typedef struct cro_sparse_result {
+    int32_t  status;               /*   0  CRO_OK, or CRO_ERR_CHECKSUM on any mismatch or missing publish       */
+    uint32_t verdict;              /*   4  CRO_COMPUTE_NONE / _SM / _ALL                                        */
+    uint64_t seed;                 /*   8  operand seed of this call                                           */
+    uint64_t call;                 /*  16  k: the call's number on this device, from 0                         */
+    uint32_t sm_count;             /*  24 */
+    uint32_t legs;                 /*  28  legs run (CRO_SPARSE_ALL_LEGS bits)                                  */
+    uint64_t host_ref_ns;          /*  32  host time to compute the four expected answers                       */
+    uint32_t nsmid;                /*  40 */
+    uint32_t bad_sms;              /*  44 */
+    uint16_t bad_sm[16];           /*  48 */
+    cro_compute_leg leg[CRO_SPARSE_LEGS];   /*  80  ops: 2 * M * N * logical K * iterations per CTA (dense-equivalent) */
+} cro_sparse_result;               /* 704 bytes */
+
+typedef struct cro_sparse_sm {
+    uint32_t smid;                 /*   0 */
+    uint32_t reserved;             /*   4 */
+    cro_compute_sm_leg leg[CRO_SPARSE_LEGS];   /* 8 */
+} cro_sparse_sm;                   /* 248 bytes */
+
+typedef struct cro_sparse_fault {
+    uint32_t leg;                  /*   0  CRO_SPARSE_LEG_*                                                     */
+    uint32_t smid;                 /*   4 */
+    uint32_t row;                  /*   8 */
+    uint32_t col;                  /*  12 */
+    int32_t  expected;             /*  16  the exact answer                                                     */
+    uint32_t actual_bits;          /*  20  the accumulator's raw 32 bits (int32 for S8, f32 otherwise)          */
+} cro_sparse_fault;                /*  24 bytes */
+
+/* As cro_probe_compute: sms one entry per SM seen, faults sorted by (leg, smid, row, col). */
+int  cro_probe_sparse(cro_ctx *ctx, int dev_index, const cro_sparse_opts *opts, cro_sparse_result *out,
+                      cro_sparse_sm *sms, int sms_cap, int *n_sms, cro_sparse_fault *faults, int cap, int *n);
+
+/* The same probe of any GPU on the node, run by `croprobe-cli sparse-raw`; as cro_probe_compute_uuid. */
+int  cro_probe_sparse_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_sparse_opts *opts, int deadline_ms,
+                           cro_sparse_result *out, cro_sparse_sm *sms, int sms_cap, int *n_sms,
+                           cro_sparse_fault *faults, int cap, int *n, uint64_t *helper_ns);
+
+/* The expected answer a call uploads: answer CRO_SPARSE_ANSWER_* of the operands of `seed`, as CRO_SPARSE_M *
+ * CRO_SPARSE_N int32 values, row-major.  Host arithmetic only; no context. */
+int  cro_sparse_expected(int answer, uint64_t seed, int32_t *out);
+
 /* ---- whole-HBM scan: every free byte of a GPU's memory, and its DRAM health record ---- */
 
 /*
@@ -1526,14 +1659,16 @@ typedef struct cro_sm_cta {
 
 #define CRO_SM_LEGS_COMPUTE       0   /* cro_selftest_sm_legs_classify: the compute probe   */
 #define CRO_SM_LEGS_PRECISION     1   /* ... the precision probe                           */
+#define CRO_SM_LEGS_SPARSE        3   /* ... the sparse probe (cro_sparse_* types); 2 names no probe and is refused */
 
 /* Test hook: the compute (probe CRO_SM_LEGS_COMPUTE: out a cro_compute_result, sms cro_compute_sm, records and faults
- * cro_compute_fault) or precision probe's (CRO_SM_LEGS_PRECISION: the cro_precision_* types) classification of call
- * `call` on a device of `grid` SMs, from caller-given rounds instead of launches.  legs: the legs that ran (0: all).
- * Per leg l of them: iterations[l] (>= 1) per CTA, rounds[l] rounds, each of `grid` records of ctas and of the
- * CRO_COMPUTE_MAX_SMS / 64 words of sm_bits (the leg's coverage bitmap after that round), and claims[l] record claims,
- * of which the first min(claims[l], CRO_COMPUTE_RECORDS) are in `records`; ctas, sm_bits and records run in leg order.
- * Every array is indexed by leg (CRO_COMPUTE_LEGS or CRO_PRECISION_LEGS entries).  Writes out, sms[0 .. sms_cap) and
+ * cro_compute_fault), precision (CRO_SM_LEGS_PRECISION: the cro_precision_* types) or sparse probe's
+ * (CRO_SM_LEGS_SPARSE: the cro_sparse_* types) classification of call `call` on a device of `grid` SMs, from
+ * caller-given rounds instead of launches.  legs: the legs that ran (0: all).  Per leg l of them: iterations[l] (>= 1)
+ * per CTA, rounds[l] rounds, each of `grid` records of ctas and of the CRO_COMPUTE_MAX_SMS / 64 words of sm_bits (the
+ * leg's coverage bitmap after that round), and claims[l] record claims, of which the first min(claims[l],
+ * CRO_COMPUTE_RECORDS) are in `records`; ctas, sm_bits and records run in leg order.  Every array is indexed by leg
+ * (CRO_COMPUTE_LEGS, CRO_PRECISION_LEGS or CRO_SPARSE_LEGS entries).  Writes out, sms[0 .. sms_cap) and
  * faults[0 .. cap) (*n_sms, *n how many) exactly as the in-process call does, all but what needs the device: seed,
  * host_ref_ns, ns and expect_fold stay 0, and rounds is rounds[l].  Returns out->status (CRO_ERR_UNSUPPORTED with a
  * blanked result for a %nsmid above CRO_COMPUTE_MAX_SMS), or CRO_ERR_INVALID_ARG for a NULL array it needs, a negative
@@ -1775,6 +1910,12 @@ int  cro_emit_compute_annotations_json(const cro_compute_result *r, char *buf, s
  * probe's: -verdict, -sms, -bad-sms, -failed-legs (f64, dfma, tf32, f16, f16acc, e5m2, hfma2), -f64-gflops,
  * -tf32-gflops, -f16-gflops, -f16acc-gflops, -e5m2-gflops (ops / ns, integer division; 0 when ns is 0) and -slowest-sm. */
 int  cro_emit_precision_annotations_json(const cro_precision_result *r, char *buf, size_t cap, size_t *len);
+
+/* Additive sparse annotations (cohdi.io/probe-sparse-*) of a cro_probe_sparse result, spelled as the compute probe's:
+ * -verdict, -sms, -bad-sms, -failed-legs (s8, e4m3, e5m2, bf16, f16, tf32), -s8-gops, -e4m3-gflops, -e5m2-gflops,
+ * -bf16-gflops, -f16-gflops, -tf32-gflops (dense-equivalent ops / ns, integer division; 0 when ns is 0) and
+ * -slowest-sm. */
+int  cro_emit_sparse_annotations_json(const cro_sparse_result *r, char *buf, size_t cap, size_t *len);
 
 /* Additive HBM scan annotations (cohdi.io/hbm-scan-*) of a cro_scan_hbm / cro_scan_hbm_uuid report, the same
  * Go-marshalled map, integers and fixed spellings only: -verdict ("ok" for CRO_OK, "corrupt" for CRO_ERR_CHECKSUM,
