@@ -15,6 +15,7 @@ struct ComputeProbe {
     using Args = ComputeArgs;
     using Tile = int32_t;
     static constexpr const char* kName = "compute";
+    static constexpr const cro_wire& kWire = cro_wire_compute;
     static constexpr uint32_t kLegs = CRO_COMPUTE_LEGS, kAllLegs = CRO_COMPUTE_ALL_LEGS, kMaxSms = CRO_COMPUTE_MAX_SMS;
     static constexpr uint32_t kRecords = CRO_COMPUTE_RECORDS;
     static constexpr int kAnswers = 2;      // CRO_COMPUTE_ANSWER_S8, _SMALL
@@ -34,7 +35,6 @@ struct ComputeProbe {
     static cudaError_t launch(uint32_t leg, const ComputeArgs& a, int grid, cudaStream_t st) { return launch_compute(leg, a, grid, st); }
 
     static void test_args(const cro_compute_opts&, uint32_t, ComputeArgs*) {}
-    static std::vector<std::string> helper_args(const cro_compute_opts& o) { return dense_helper_args(o); }
 
     static std::string opts_error(const cro_compute_opts& o) {
         const uint32_t legs = o.legs ? o.legs : CRO_COMPUTE_ALL_LEGS;

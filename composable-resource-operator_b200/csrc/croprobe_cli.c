@@ -78,6 +78,7 @@
 #include <unistd.h>
 
 #include "croprobe.h"
+#include "helper_wire.h"
 
 static double now_s(void) {
     struct timespec ts;
@@ -94,14 +95,17 @@ static int fail(cro_ctx *ctx, const char *what, int rc) {
 
 static char buf[1 << 16];
 
-/* A raw command's stdout, the result whatever its status (the library reads why from it): one frame per result, each
- * the result, n_counts counts of the helper's own, the per-SM block and n records of rec_bytes each, the empty parts
- * left out (put_frame: 0, or 2 when stdout takes less).  Then end_frames exits 0 iff the status is CRO_OK and 1 for any
- * other, skipping the teardown (it costs as much as a probe): the process's buffers and allocations go with it. */
-static int put_frame(const void *result, size_t result_bytes, const uint64_t *counts, size_t n_counts, const void *sms,
-                     size_t sms_bytes, const void *records, size_t rec_bytes, int n) {
-    if (fwrite(result, result_bytes, 1, stdout) != 1 || (n_counts && fwrite(counts, sizeof *counts, n_counts, stdout) != n_counts) ||
-        (sms_bytes && fwrite(sms, sms_bytes, 1, stdout) != 1) || (n > 0 && fwrite(records, rec_bytes, (size_t)n, stdout) != (size_t)n))
+/* A raw command's stdout, the result whatever its status (the library reads why from it): one frame per result, laid
+ * out as its cro_wire_frame says, the counts the result does not hold written after it (put_frame: 0, or 2 when stdout
+ * takes less).  Then end_frames exits 0 iff the status is CRO_OK and 1 for any other, skipping the teardown (it costs as
+ * much as a probe): the process's buffers and allocations go with it. */
+static int put_frame(const cro_wire_frame *w, const void *result, const void *sms, uint64_t n_sms, const void *records, uint64_t n) {
+    unsigned char counts[2 * sizeof(uint64_t)] = {0};
+    if (w->n_sms_width && w->n_sms_at >= w->result) memcpy(counts + (w->n_sms_at - w->result), &n_sms, w->n_sms_width);
+    if (w->n_width && w->n_at >= w->result) memcpy(counts + (w->n_at - w->result), &n, w->n_width);
+    const size_t sms_bytes = (size_t)w->max_sms * w->sm;
+    if (fwrite(result, w->result, 1, stdout) != 1 || (w->counts && fwrite(counts, sizeof(uint64_t), w->counts, stdout) != w->counts) ||
+        (sms_bytes && fwrite(sms, sms_bytes, 1, stdout) != 1) || (n && fwrite(records, w->rec, (size_t)n, stdout) != (size_t)n))
         return 2;
     return 0;
 }
@@ -110,210 +114,95 @@ static int end_frames(int status) {
     _exit(status == CRO_OK ? 0 : 1);
 }
 
-/* Each check's frame, as its -raw command and health-raw write it: compute, precision and L2 with the counts n_sms and
- * n and the whole per-SM block, SRAM with the block (the result says how many records follow), link with n, the scan
- * with its words only. */
-static int put_compute(const cro_compute_result *r, const cro_compute_sm *sms, int n_sms, const cro_compute_fault *f, int n) {
-    const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)n};
-    return put_frame(r, sizeof *r, counts, 2, sms, CRO_COMPUTE_MAX_SMS * sizeof *sms, f, sizeof *f, n);
+/* w's options from argv, a[0] its first, into opts; the cap that follows them. */
+static int opts_at(const cro_wire *w, char **a, void *opts) {
+    for (uint32_t i = 0; i < w->n_fields; ++i) cro_wire_parse(w, i, a[i], opts);
+    return atoi(a[w->n_fields]);
 }
-static int put_precision(const cro_precision_result *r, const cro_precision_sm *sms, int n_sms, const cro_precision_fault *f,
-                         int n) {
-    const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)n};
-    return put_frame(r, sizeof *r, counts, 2, sms, CRO_PRECISION_MAX_SMS * sizeof *sms, f, sizeof *f, n);
-}
-static int put_sparse(const cro_sparse_result *r, const cro_sparse_sm *sms, int n_sms, const cro_sparse_fault *f, int n) {
-    const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)n};
-    return put_frame(r, sizeof *r, counts, 2, sms, CRO_SPARSE_MAX_SMS * sizeof *sms, f, sizeof *f, n);
-}
-static int put_l2(const cro_l2_result *r, const cro_l2_sm *sms, int n_sms, const cro_l2_fault *f, int n) {
-    const uint64_t counts[2] = {(uint64_t)n_sms, (uint64_t)n};
-    return put_frame(r, sizeof *r, counts, 2, sms, CRO_L2_MAX_SMS * sizeof *sms, f, sizeof *f, n);
-}
-static int put_sram(const cro_sram_result *r, const cro_sram_sm *sms, const cro_sram_fault *f, int n) {
-    return put_frame(r, sizeof *r, NULL, 0, sms, CRO_SRAM_MAX_SMS * sizeof *sms, f, sizeof *f, n);
-}
-static int put_link(const cro_link_result *r, const cro_link_fault *f, int n) {
-    const uint64_t n_out = (uint64_t)n;
-    return put_frame(r, sizeof *r, &n_out, 1, NULL, 0, f, sizeof *f, n);
-}
-static int put_scan(const cro_scan_report *r, const cro_fault_word *w, int n) {
-    return put_frame(r, sizeof *r, NULL, 0, NULL, 0, w, sizeof *w, n);
-}
-
-/* Each check's options from argv, a[0] its first, in the order its -raw command takes them. */
-static void scan_opts_at(char **a, cro_scan_opts *so) {
-    uint64_t *f[] = {&so->max_bytes, &so->reserve_bytes, &so->seed, &so->test_chunk_bytes, &so->test_force_first,
-                     &so->test_force_count, &so->test_force_and, &so->test_force_or};
-    for (int k = 0; k < 8; ++k) *f[k] = (uint64_t)strtoull(a[k], NULL, 10);
-}
-static void sram_opts_at(char **a, cro_sram_opts *so) {
-    so->legs = (uint32_t)strtoul(a[0], NULL, 10);
-    so->iterations = (uint32_t)strtoul(a[1], NULL, 10);
-    so->cluster = (uint32_t)strtoul(a[2], NULL, 10);
-    so->max_rounds = (uint32_t)strtoul(a[3], NULL, 10);
-    so->test_inject_leg = atoi(a[4]);
-    so->test_inject_sm = atoi(a[5]);
-    so->test_inject_element = (uint32_t)strtoul(a[6], NULL, 10);
-    so->test_inject_iteration = (uint32_t)strtoul(a[7], NULL, 10);
-    so->test_inject_word = atoi(a[8]);
-    so->test_inject_mask = (uint64_t)strtoull(a[9], NULL, 10);
-}
-static void link_opts_at(char **a, cro_link_opts *lo) {
-    lo->bytes = (uint64_t)strtoull(a[0], NULL, 10);
-    lo->hops = (uint32_t)strtoul(a[1], NULL, 10);
-    lo->ctas = (uint32_t)strtoul(a[2], NULL, 10);
-    lo->test_inject_check = atoi(a[3]);
-    lo->test_inject_word = (uint64_t)strtoull(a[4], NULL, 10);
-    lo->test_inject_mask = (uint64_t)strtoull(a[5], NULL, 10);
-}
-static void compute_opts_at(char **a, cro_compute_opts *co) {
-    co->iterations = (uint32_t)strtoul(a[0], NULL, 10);
-    co->alu_iterations = (uint32_t)strtoul(a[1], NULL, 10);
-    co->legs = (uint32_t)strtoul(a[2], NULL, 10);
-    co->max_rounds = (uint32_t)strtoul(a[3], NULL, 10);
-    co->test_inject_leg = atoi(a[4]);
-    co->test_inject_sm = atoi(a[5]);
-    co->test_inject_iteration = (uint32_t)strtoul(a[6], NULL, 10);
-    co->test_inject_row = atoi(a[7]);
-    co->test_inject_col = atoi(a[8]);
-    co->test_inject_mask = (uint32_t)strtoul(a[9], NULL, 10);
-}
-static void precision_opts_at(char **a, cro_precision_opts *po) {
-    po->iterations = (uint32_t)strtoul(a[0], NULL, 10);
-    po->alu_iterations = (uint32_t)strtoul(a[1], NULL, 10);
-    po->legs = (uint32_t)strtoul(a[2], NULL, 10);
-    po->max_rounds = (uint32_t)strtoul(a[3], NULL, 10);
-    po->test_inject_leg = atoi(a[4]);
-    po->test_inject_sm = atoi(a[5]);
-    po->test_inject_iteration = (uint32_t)strtoul(a[6], NULL, 10);
-    po->test_inject_row = atoi(a[7]);
-    po->test_inject_col = atoi(a[8]);
-    po->test_inject_mask = (uint64_t)strtoull(a[9], NULL, 10);
-}
-static void l2_opts_at(char **a, cro_l2_opts *lo) {
-    lo->bytes = (uint64_t)strtoull(a[0], NULL, 10);
-    lo->iterations = (uint32_t)strtoul(a[1], NULL, 10);
-    lo->a1_counters = (uint32_t)strtoul(a[2], NULL, 10);
-    lo->a2_counters = (uint32_t)strtoul(a[3], NULL, 10);
-    lo->test_inject_leg = atoi(a[4]);
-    lo->test_inject_sm = atoi(a[5]);
-    lo->test_inject_element = atoi(a[6]);
-    lo->test_inject_iteration = (uint32_t)strtoul(a[7], NULL, 10);
-    lo->test_inject_word = (int64_t)strtoll(a[8], NULL, 10);
-    lo->test_inject_mask = (uint64_t)strtoull(a[9], NULL, 10);
-}
+/* A raw command's options, after its uuid and seed base. */
+static int raw_opts(const cro_wire *w, char **argv, void *opts) { return opts_at(w, argv + 3 + w->seeded, opts); }
 
 /* The raw commands: each fills its probe's options from argv, runs the probe on device idx and writes its frame. */
 static int scan_raw(cro_ctx *ctx, int idx, char **argv) {
-    cro_scan_opts so;
-    memset(&so, 0, sizeof so);
-    scan_opts_at(argv + 3, &so);
-    const int cap = atoi(argv[11]);
+    static cro_scan_opts so;
+    const int cap = raw_opts(&cro_wire_scan, argv, &so);
     static cro_scan_report sr;
     cro_fault_word *words = (cro_fault_word *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *words);
     int got = 0;
     if (!words) return 2;
     cro_scan_hbm(ctx, idx, &so, &sr, words, cap, &got);
-    return put_scan(&sr, words, got) ? 2 : end_frames(sr.status);
+    return put_frame(&cro_wire_scan.frame, &sr, NULL, 0, words, (uint64_t)got) ? 2 : end_frames(sr.status);
 }
 
 static int sram_raw(cro_ctx *ctx, int idx, char **argv) {
-    cro_sram_opts so;
-    memset(&so, 0, sizeof so);
-    sram_opts_at(argv + 3, &so);
-    const int cap = atoi(argv[13]);
+    static cro_sram_opts so;
+    const int cap = raw_opts(&cro_wire_sram, argv, &so);
     static cro_sram_result sr;
     static cro_sram_sm sms[CRO_SRAM_MAX_SMS];
     cro_sram_fault *faults = (cro_sram_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
     int n_sms = 0, got = 0;
     if (!faults) return 2;
     cro_probe_sram(ctx, idx, &so, &sr, sms, CRO_SRAM_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
-    return put_sram(&sr, sms, faults, got) ? 2 : end_frames(sr.status);
+    return put_frame(&cro_wire_sram.frame, &sr, sms, (uint64_t)n_sms, faults, (uint64_t)got) ? 2 : end_frames(sr.status);
 }
 
 static int link_raw(cro_ctx *ctx, int idx, char **argv) {
-    cro_link_opts lo;
-    memset(&lo, 0, sizeof lo);
-    link_opts_at(argv + 4, &lo);
-    const int cap = atoi(argv[10]);
+    static cro_link_opts lo;
+    const int cap = raw_opts(&cro_wire_link, argv, &lo);
     static cro_link_result lr;
     cro_link_fault *faults = (cro_link_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
     int got = 0;
     if (!faults) return 2;
     cro_probe_host_link(ctx, idx, &lo, &lr, faults, cap > 0 ? cap : 0, &got);
-    return put_link(&lr, faults, got) ? 2 : end_frames(lr.status);
+    return put_frame(&cro_wire_link.frame, &lr, NULL, 0, faults, (uint64_t)got) ? 2 : end_frames(lr.status);
 }
 
 static int compute_raw(cro_ctx *ctx, int idx, char **argv) {
-    cro_compute_opts co;
-    memset(&co, 0, sizeof co);
-    compute_opts_at(argv + 4, &co);
-    const int cap = atoi(argv[14]);
+    static cro_compute_opts co;
+    const int cap = raw_opts(&cro_wire_compute, argv, &co);
     static cro_compute_result cr;
     static cro_compute_sm sms[CRO_COMPUTE_MAX_SMS];
     cro_compute_fault *faults = (cro_compute_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
     int n_sms = 0, got = 0;
     if (!faults) return 2;
     cro_probe_compute(ctx, idx, &co, &cr, sms, CRO_COMPUTE_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
-    return put_compute(&cr, sms, n_sms, faults, got) ? 2 : end_frames(cr.status);
+    return put_frame(&cro_wire_compute.frame, &cr, sms, (uint64_t)n_sms, faults, (uint64_t)got) ? 2 : end_frames(cr.status);
 }
 
 static int precision_raw(cro_ctx *ctx, int idx, char **argv) {
-    cro_precision_opts po;
-    memset(&po, 0, sizeof po);
-    precision_opts_at(argv + 4, &po);
-    const int cap = atoi(argv[14]);
+    static cro_precision_opts po;
+    const int cap = raw_opts(&cro_wire_precision, argv, &po);
     static cro_precision_result pr;
     static cro_precision_sm sms[CRO_PRECISION_MAX_SMS];
     cro_precision_fault *faults = (cro_precision_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
     int n_sms = 0, got = 0;
     if (!faults) return 2;
     cro_probe_precision(ctx, idx, &po, &pr, sms, CRO_PRECISION_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
-    return put_precision(&pr, sms, n_sms, faults, got) ? 2 : end_frames(pr.status);
+    return put_frame(&cro_wire_precision.frame, &pr, sms, (uint64_t)n_sms, faults, (uint64_t)got) ? 2 : end_frames(pr.status);
 }
 
 static int sparse_raw(cro_ctx *ctx, int idx, char **argv) {
-    char **a = argv + 4;
-    cro_sparse_opts so;
-    memset(&so, 0, sizeof so);
-    so.iterations = (uint32_t)strtoul(a[0], NULL, 10);
-    so.legs = (uint32_t)strtoul(a[1], NULL, 10);
-    so.max_rounds = (uint32_t)strtoul(a[2], NULL, 10);
-    so.test_inject_leg = atoi(a[3]);
-    so.test_inject_sm = atoi(a[4]);
-    so.test_inject_iteration = (uint32_t)strtoul(a[5], NULL, 10);
-    so.test_inject_row = atoi(a[6]);
-    so.test_inject_col = atoi(a[7]);
-    so.test_inject_mask = strtoull(a[8], NULL, 10);
-    so.test_meta = (uint32_t)strtoul(a[9], NULL, 10);
-    so.test_meta_leg = atoi(a[10]);
-    so.test_meta_sm = atoi(a[11]);
-    so.test_meta_iteration = (uint32_t)strtoul(a[12], NULL, 10);
-    so.test_meta_row = (uint32_t)strtoul(a[13], NULL, 10);
-    so.test_meta_group = (uint32_t)strtoul(a[14], NULL, 10);
-    const int cap = atoi(argv[19]);
+    static cro_sparse_opts so;
+    const int cap = raw_opts(&cro_wire_sparse, argv, &so);
     static cro_sparse_result sr;
     static cro_sparse_sm sms[CRO_SPARSE_MAX_SMS];
     cro_sparse_fault *faults = (cro_sparse_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
     int n_sms = 0, got = 0;
     if (!faults) return 2;
     cro_probe_sparse(ctx, idx, &so, &sr, sms, CRO_SPARSE_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
-    return put_sparse(&sr, sms, n_sms, faults, got) ? 2 : end_frames(sr.status);
+    return put_frame(&cro_wire_sparse.frame, &sr, sms, (uint64_t)n_sms, faults, (uint64_t)got) ? 2 : end_frames(sr.status);
 }
 
 static int l2_raw(cro_ctx *ctx, int idx, char **argv) {
-    cro_l2_opts lo;
-    memset(&lo, 0, sizeof lo);
-    l2_opts_at(argv + 4, &lo);
-    const int cap = atoi(argv[14]);
+    static cro_l2_opts lo;
+    const int cap = raw_opts(&cro_wire_l2, argv, &lo);
     static cro_l2_result lr;
     static cro_l2_sm sms[CRO_L2_MAX_SMS];
     cro_l2_fault *faults = (cro_l2_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
     int n_sms = 0, got = 0;
     if (!faults) return 2;
     cro_probe_l2(ctx, idx, &lo, &lr, sms, CRO_L2_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
-    return put_l2(&lr, sms, n_sms, faults, got) ? 2 : end_frames(lr.status);
+    return put_frame(&cro_wire_l2.frame, &lr, sms, (uint64_t)n_sms, faults, (uint64_t)got) ? 2 : end_frames(lr.status);
 }
 
 /* `scan`: the whole-HBM scan of the free memory (all of it but 1 GiB unless argv[3], in MiB, bounds it) as JSON. */
@@ -335,9 +224,6 @@ static int scan_json(cro_ctx *ctx, int idx, char **argv) {
     return sr.status == CRO_OK ? 0 : 1;
 }
 
-/* health-raw's argv: each check's options from its first, then its cap.  The link check's L is argv[H_LINK]. */
-enum { H_COMPUTE = 5, H_PRECISION = 16, H_SRAM = 27, H_L2 = 38, H_LINK = 49, H_SCAN = 56, H_ARGC = 65 };
-
 /* `health-raw`: cro_check_health, then its result and each check that ran as its own frame. */
 static int health_raw(cro_ctx *ctx, int idx, char **argv) {
     static cro_health_opts ho;
@@ -346,17 +232,12 @@ static int health_raw(cro_ctx *ctx, int idx, char **argv) {
     static cro_precision_sm psms[CRO_PRECISION_MAX_SMS];
     static cro_sram_sm ssms[CRO_SRAM_MAX_SMS];
     static cro_l2_sm lsms[CRO_L2_MAX_SMS];
-    memset(&ho, 0, sizeof ho);
     ho.checks = (uint32_t)strtoul(argv[4], NULL, 10);
-    compute_opts_at(argv + H_COMPUTE, &ho.compute);
-    precision_opts_at(argv + H_PRECISION, &ho.precision);
-    sram_opts_at(argv + H_SRAM, &ho.sram);
-    l2_opts_at(argv + H_L2, &ho.l2);
-    link_opts_at(argv + H_LINK, &ho.link);
-    scan_opts_at(argv + H_SCAN, &ho.scan);
-    int cap[6] = {atoi(argv[H_COMPUTE + 10]), atoi(argv[H_PRECISION + 10]), atoi(argv[H_SRAM + 10]), atoi(argv[H_L2 + 10]),
-                  atoi(argv[H_LINK + 6]), atoi(argv[H_SCAN + 8])};
-    for (int k = 0; k < 6; ++k) cap[k] = cap[k] > 0 ? cap[k] : 0;
+    int cap[CRO_HEALTH_CHECKS];
+    for (int k = 0; k < CRO_HEALTH_CHECKS; ++k) {
+        cap[k] = opts_at(cro_wire_health[k].wire, argv + cro_wire_health_at(k), (char *)&ho + cro_wire_health[k].opts_at);
+        cap[k] = cap[k] > 0 ? cap[k] : 0;
+    }
     cro_health_records rec;
     memset(&rec, 0, sizeof rec);
     rec.compute_sms = csms;
@@ -382,15 +263,17 @@ static int health_raw(cro_ctx *ctx, int idx, char **argv) {
     rec.link_faults_cap = cap[4];
     rec.scan_words_cap = cap[5];
     cro_check_health(ctx, idx, &ho, &hr, &rec);
-    if (put_frame(&hr, sizeof hr, NULL, 0, NULL, 0, NULL, 0, 0) ||
-        ((hr.ran & CRO_HEALTH_COMPUTE) && put_compute(&hr.compute, csms, rec.compute_sms_n, rec.compute_faults, rec.compute_faults_n)) ||
-        ((hr.ran & CRO_HEALTH_PRECISION) &&
-         put_precision(&hr.precision, psms, rec.precision_sms_n, rec.precision_faults, rec.precision_faults_n)) ||
-        ((hr.ran & CRO_HEALTH_SRAM) && put_sram(&hr.sram, ssms, rec.sram_faults, rec.sram_faults_n)) ||
-        ((hr.ran & CRO_HEALTH_L2) && put_l2(&hr.l2, lsms, rec.l2_sms_n, rec.l2_faults, rec.l2_faults_n)) ||
-        ((hr.ran & CRO_HEALTH_LINK) && put_link(&hr.link, rec.link_faults, rec.link_faults_n)) ||
-        ((hr.ran & CRO_HEALTH_SCAN) && put_scan(&hr.scan, rec.scan_words, rec.scan_words_n)))
-        return 2;
+    const void *sms[CRO_HEALTH_CHECKS] = {csms, psms, ssms, lsms, NULL, NULL};
+    const int n_sms[CRO_HEALTH_CHECKS] = {rec.compute_sms_n, rec.precision_sms_n, rec.sram_sms_n, rec.l2_sms_n, 0, 0};
+    const void *recs[CRO_HEALTH_CHECKS] = {rec.compute_faults, rec.precision_faults, rec.sram_faults,
+                                           rec.l2_faults,      rec.link_faults,      rec.scan_words};
+    const int n[CRO_HEALTH_CHECKS] = {rec.compute_faults_n, rec.precision_faults_n, rec.sram_faults_n,
+                                      rec.l2_faults_n,      rec.link_faults_n,      rec.scan_words_n};
+    if (fwrite(&hr, sizeof hr, 1, stdout) != 1) return 2;
+    for (int k = 0; k < CRO_HEALTH_CHECKS; ++k)
+        if ((hr.ran >> k & 1u) && put_frame(&cro_wire_health[k].wire->frame, (const char *)&hr + cro_wire_health[k].result_at, sms[k],
+                                            (uint64_t)n_sms[k], recs[k], (uint64_t)n[k]))
+            return 2;
     return end_frames(hr.status);
 }
 
@@ -407,38 +290,37 @@ static int health_json(cro_ctx *ctx, int idx, char **argv) {
     return hr.status == CRO_OK ? 0 : 1;
 }
 
-/* The commands that take a device (argv[2]): their argc (0: at least 3, the rest optional), cro_opts.flags and sweep
- * region, whether argv[3] is cro_opts.seed_base, and what runs once the device is found (NULL: main's own probe). */
+/* The commands that take a device (argv[2]): their name, or a raw command's argv and frame (helper_wire.h; NULL: argc at
+ * least 3, the rest optional), cro_opts.flags and sweep region, and what runs once the device is found (NULL: main's own probe). */
 static const struct command {
     const char *name;
-    int argc;
+    const cro_wire *wire;
     uint32_t flags;
     uint64_t sweep_mib;
-    int seeded;
     int (*run)(cro_ctx *ctx, int idx, char **argv);
 } commands[] = {
     /* the hot-plug path: one device, identity from /proc (NVML's first call costs more than the probe), and a 1 GiB
      * first sweep unless argv[3] says otherwise — far beyond the L2, and it shortens everything before it */
-    {"probe", 0, CRO_F_LAZY_ALLOC | CRO_F_DEGRADE_ON_OOM | CRO_F_NO_NVML, 1024, 0, NULL},
-    {"probe-raw", 0, CRO_F_LAZY_ALLOC | CRO_F_DEGRADE_ON_OOM | CRO_F_NO_NVML, 1024, 0, NULL},
-    {"cold", 0, CRO_F_LAZY_ALLOC | CRO_F_DEGRADE_ON_OOM | CRO_F_NO_NVML, 1024, 0, NULL},
+    {"probe", NULL, CRO_F_LAZY_ALLOC | CRO_F_DEGRADE_ON_OOM | CRO_F_NO_NVML, 1024, NULL},
+    {"probe-raw", NULL, CRO_F_LAZY_ALLOC | CRO_F_DEGRADE_ON_OOM | CRO_F_NO_NVML, 1024, NULL},
+    {"cold", NULL, CRO_F_LAZY_ALLOC | CRO_F_DEGRADE_ON_OOM | CRO_F_NO_NVML, 1024, NULL},
     /* one check of one device by their own, not the HBM probe: no sweep region (the scan allocates its own chunks) and
      * NVML, whose DRAM / SRAM / L2 health record these read */
-    {"scan", 0, CRO_F_LAZY_ALLOC, 64, 0, scan_json},
-    {"scan-raw", 12, CRO_F_LAZY_ALLOC, 64, 0, scan_raw},
-    {"sram-raw", 14, CRO_F_LAZY_ALLOC, 64, 0, sram_raw},
-    {"l2-raw", 15, CRO_F_LAZY_ALLOC, 64, 1, l2_raw},
-    /* a region of exactly L, argv[4] (the probe checks L <= S; no halving on a full GPU), and NVML for the replay
-     * counters */
-    {"link-raw", 11, CRO_F_LAZY_ALLOC, 256, 1, link_raw},
+    {"scan", NULL, CRO_F_LAZY_ALLOC, 64, scan_json},
+    {NULL, &cro_wire_scan, CRO_F_LAZY_ALLOC, 64, scan_raw},
+    {NULL, &cro_wire_sram, CRO_F_LAZY_ALLOC, 64, sram_raw},
+    {NULL, &cro_wire_l2, CRO_F_LAZY_ALLOC, 64, l2_raw},
+    /* a region of exactly L, the link's bytes (the probe checks L <= S; no halving on a full GPU), and NVML for the
+     * replay counters */
+    {NULL, &cro_wire_link, CRO_F_LAZY_ALLOC, 256, link_raw},
     /* no health record to read, and NVML's first call is slow */
-    {"compute-raw", 15, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, 1, compute_raw},
-    {"precision-raw", 15, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, 1, precision_raw},
-    {"sparse-raw", 20, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, 1, sparse_raw},
-    /* every check of one device: the link check's region (exactly L, argv[49], when it is given) and NVML for the scan's,
-     * SRAM's and L2's health records and the link's replay counters */
-    {"health-raw", H_ARGC, CRO_F_LAZY_ALLOC, 256, 1, health_raw},
-    {"health", 0, CRO_F_LAZY_ALLOC, 256, 0, health_json},
+    {NULL, &cro_wire_compute, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, compute_raw},
+    {NULL, &cro_wire_precision, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, precision_raw},
+    {NULL, &cro_wire_sparse, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, sparse_raw},
+    /* every check of one device: the link check's region (exactly L when it is given) and NVML for the scan's, SRAM's and
+     * L2's health records and the link's replay counters */
+    {"health-raw", NULL, CRO_F_LAZY_ALLOC, 256, health_raw},
+    {"health", NULL, CRO_F_LAZY_ALLOC, 256, health_json},
 };
 
 int main(int argc, char **argv) {
@@ -459,8 +341,9 @@ int main(int argc, char **argv) {
     const char *cmd = argv[1];
     const struct command *c = NULL;
     for (size_t k = 0; k < sizeof commands / sizeof *commands; ++k)
-        if (strcmp(cmd, commands[k].name) == 0) c = &commands[k];
-    if (c && (argc < 3 || (c->argc && argc != c->argc))) return 64;
+        if (strcmp(cmd, commands[k].wire ? commands[k].wire->cmd : commands[k].name) == 0) c = &commands[k];
+    const int want = !c ? 0 : c->wire ? cro_wire_argc(c->wire) : c->run == health_raw ? cro_wire_health_at(CRO_HEALTH_CHECKS) : 0;
+    if (c && (argc < 3 || (want && argc != want))) return 64;
     const int cold = strcmp(cmd, "cold") == 0;
     cro_opts opts;
     memset(&opts, 0, sizeof opts);
@@ -469,11 +352,12 @@ int main(int argc, char **argv) {
     if (c) {
         opts.flags = c->flags;
         opts.sweep_bytes = c->sweep_mib << 20;
-        if (c->seeded) opts.seed_base = (uint64_t)strtoull(argv[3], NULL, 10);
+        if (c->wire ? c->wire->seeded : c->run == health_raw) opts.seed_base = (uint64_t)strtoull(argv[3], NULL, 10);
         if (!c->run && argc > 3) opts.sweep_bytes = (uint64_t)strtoull(argv[3], NULL, 10) << 20;    /* the probe's sweep_MiB */
         if (cold && argc > 4 && strcmp(argv[4], "nvml") == 0) opts.flags &= ~CRO_F_NO_NVML;
-        if (c->run == link_raw && strtoull(argv[4], NULL, 10)) opts.sweep_bytes = (uint64_t)strtoull(argv[4], NULL, 10);  /* L */
-        if (c->run == health_raw && strtoull(argv[H_LINK], NULL, 10)) opts.sweep_bytes = (uint64_t)strtoull(argv[H_LINK], NULL, 10);
+        /* L: the link's first option (the link is health-raw's fifth check) */
+        const char *link_bytes = c->run == link_raw ? argv[4] : c->run == health_raw ? argv[cro_wire_health_at(4)] : "0";
+        if (strtoull(link_bytes, NULL, 10)) opts.sweep_bytes = (uint64_t)strtoull(link_bytes, NULL, 10);
         if (strncmp(argv[2], "GPU-", 4) == 0) {
             /* before ANY CUDA call: this process's cuInit must enumerate that one GPU only (one primary context
              * instead of eight on a full box) */
@@ -544,7 +428,7 @@ int main(int argc, char **argv) {
                    r.gpu_uuid, (unsigned long long)r.sweep_bytes, t_init, t_cold, t_warm, total,
                    1.0 / total, 1.0 / t_warm, (opts.flags & CRO_F_NO_NVML) ? "false" : "true", rc2 ? rc2 : r.status);
         } else if (strcmp(cmd, "probe-raw") == 0) {
-            return put_frame(&r, sizeof r, NULL, 0, NULL, 0, NULL, 0, 0) ? 2 : end_frames(r.status);
+            return fwrite(&r, sizeof r, 1, stdout) != 1 ? 2 : end_frames(r.status);
         } else {
             if ((rc = cro_emit_probe_annotations_json(&r, buf, sizeof buf, &len)) != CRO_OK) return fail(ctx, "emit", rc);
             printf("%s\n", buf);

@@ -312,30 +312,14 @@ int ctx_scan_hbm(cro_ctx* c, int idx, const cro_scan_opts& o, cro_scan_report* r
     return rep->status = rc;
 }
 
-namespace {
-uint64_t scan_tail_count(const unsigned char* head, size_t) {
-    return reinterpret_cast<const cro_scan_report*>(head)->recorded;
-}
-}  // namespace
-
 int ctx_scan_hbm_uuid(cro_ctx* c, const char* uuid, const cro_scan_opts& o, cro_scan_report* rep, std::vector<cro_fault_word>* words,
                       int cap) {
     blank_report(rep, words);
     if (!uuid) return rep->status = CRO_ERR_INVALID_ARG;
-    const std::string want = uuid;
-    auto num = [](uint64_t v) { return std::to_string(v); };
-    const std::vector<std::string> args = {"scan-raw", want, num(o.max_bytes), num(o.reserve_bytes), num(o.seed), num(o.test_chunk_bytes),
-                                           num(o.test_force_first), num(o.test_force_count), num(o.test_force_and),
-                                           num(o.test_force_or), num((uint64_t)cap)};
-    std::string got;
     uint64_t helper_ns = 0;
-    const int rc = run_probe_helper(c, want, "scan helper", "cro.scan_hbm.helper", args, o.deadline_ms, sizeof *rep,
-                                    sizeof(cro_fault_word), (size_t)cap, scan_tail_count, &got, &helper_ns);
-    if (rc != CRO_OK) return rep->status = rc;
-    memcpy(rep, got.data(), sizeof *rep);
-    const cro_fault_word* w = reinterpret_cast<const cro_fault_word*>(got.data() + sizeof *rep);
-    words->assign(w, w + rep->recorded);
-    rep->helper_ns = helper_ns;
+    if (run_check_helper(c, cro_wire_scan, uuid, "scan helper", "cro.scan_hbm.helper", &o, cap, o.deadline_ms, &helper_ns, rep,
+                         words) == CRO_OK)
+        rep->helper_ns = helper_ns;
     return rep->status;
 }
 

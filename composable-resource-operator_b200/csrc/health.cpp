@@ -89,64 +89,20 @@ int ctx_check_health(cro_ctx* c, int idx, const cro_health_opts& o, cro_health_r
 }
 
 namespace {
-// One check's part of the health-raw frame, laid out as its own -raw command writes it: the result, `counts` uint64_t
-// counts, the per-SM block, then the records.  n_sms and n read a part's counts (n_sms 0 without a per-SM list).
-struct Part {
-    size_t result, counts, sms, rec, max_sms;
-    void (*read)(const unsigned char* part, uint64_t* n_sms, uint64_t* n);
-    size_t head() const { return result + counts * sizeof(uint64_t) + sms; }
-};
-template <class Result, class Sm, class Fault, size_t MAX_SMS>
-Part sm_part() {
-    using F = SmFrame<Result, Sm, Fault, MAX_SMS>;
-    return {sizeof(Result), 2, MAX_SMS * sizeof(Sm), sizeof(Fault), MAX_SMS, [](const unsigned char* p, uint64_t* n_sms, uint64_t* n) {
-                *n_sms = F::count(p, 0);
-                *n = F::count(p, 1);
-            }};
-}
-const Part kParts[CRO_HEALTH_CHECKS] = {
-    sm_part<cro_compute_result, cro_compute_sm, cro_compute_fault, CRO_COMPUTE_MAX_SMS>(),
-    sm_part<cro_precision_result, cro_precision_sm, cro_precision_fault, CRO_PRECISION_MAX_SMS>(),
-    {sizeof(cro_sram_result), 0, CRO_SRAM_MAX_SMS * sizeof(cro_sram_sm), sizeof(cro_sram_fault), CRO_SRAM_MAX_SMS,
-     [](const unsigned char* p, uint64_t* n_sms, uint64_t* n) {
-         const cro_sram_result* r = reinterpret_cast<const cro_sram_result*>(p);
-         *n_sms = r->sms_listed;
-         *n = r->recorded;
-     }},
-    sm_part<cro_l2_result, cro_l2_sm, cro_l2_fault, CRO_L2_MAX_SMS>(),
-    {sizeof(cro_link_result), 1, 0, sizeof(cro_link_fault), 0,
-     [](const unsigned char* p, uint64_t* n_sms, uint64_t* n) {
-         *n_sms = 0;
-         memcpy(n, p + sizeof(cro_link_result), sizeof *n);
-     }},
-    {sizeof(cro_scan_report), 0, 0, sizeof(cro_fault_word), 0, [](const unsigned char* p, uint64_t* n_sms, uint64_t* n) {
-         *n_sms = 0;
-         *n = reinterpret_cast<const cro_scan_report*>(p)->recorded;
-     }},
-};
-
-// The bytes after the health result in a frame of `size` bytes: each ran check's part in run order; ~0 when a part is
-// cut short or lists more per-SM entries than its block holds.
+// The bytes after the health result in a frame of `size` bytes: each ran check's frame in run order; ~0 when one is
+// malformed.
 uint64_t health_tail(const unsigned char* f, size_t size) {
     uint32_t ran;
     memcpy(&ran, f + offsetof(cro_health_result, ran), sizeof ran);
     size_t at = sizeof(cro_health_result);
-    for (int c = 0; c < CRO_HEALTH_CHECKS; ++c) {
-        if (!(ran >> c & 1u)) continue;
-        const Part& p = kParts[c];
-        if (size - at < p.head()) return ~0ull;
-        uint64_t n_sms, n;
-        p.read(f + at, &n_sms, &n);
-        if (n_sms > p.max_sms || n > (size - at - p.head()) / p.rec) return ~0ull;
-        at += p.head() + n * p.rec;
+    for (int k = 0; k < CRO_HEALTH_CHECKS; ++k) {
+        if (!(ran >> k & 1u)) continue;
+        const cro_wire_frame& w = cro_wire_health[k].wire->frame;
+        const uint64_t tail = read_frame(w, f + at, size - at);
+        if (tail == ~0ull) return ~0ull;
+        at += w.result + tail;
     }
     return at - sizeof(cro_health_result);
-}
-
-template <class T>
-void take(const unsigned char* from, uint64_t n, std::vector<T>* to) {
-    const T* t = reinterpret_cast<const T*>(from);
-    to->assign(t, t + n);
 }
 }  // namespace
 
@@ -164,35 +120,16 @@ int ctx_check_health_uuid(cro_ctx* c, const char* uuid, const cro_health_opts& o
         return r->status = CRO_ERR_INVALID_ARG;
     }
     const std::string want = uuid;
-    using std::to_string;
-    auto u = [](uint64_t v) { return to_string(v); };
-    auto i = [](int64_t v) { return to_string(v); };
-    const cro_compute_opts& co = o.compute;
-    const cro_precision_opts& po = o.precision;
-    const cro_sram_opts& so = o.sram;
-    const cro_l2_opts& lo = o.l2;
-    const cro_link_opts& ko = o.link;
-    const cro_scan_opts& xo = o.scan;
     // every option of every check, in run order, each check's as its own -raw command takes them, then its cap
-    const std::vector<std::string> args = {
-        "health-raw", want, u(helper_seed_base(c)), u(checks),
-        u(co.iterations), u(co.alu_iterations), u(co.legs), u(co.max_rounds), i(co.test_inject_leg), i(co.test_inject_sm),
-        u(co.test_inject_iteration), i(co.test_inject_row), i(co.test_inject_col), u(co.test_inject_mask), i(caps.faults[0]),
-        u(po.iterations), u(po.alu_iterations), u(po.legs), u(po.max_rounds), i(po.test_inject_leg), i(po.test_inject_sm),
-        u(po.test_inject_iteration), i(po.test_inject_row), i(po.test_inject_col), u(po.test_inject_mask), i(caps.faults[1]),
-        u(so.legs), u(so.iterations), u(so.cluster), u(so.max_rounds), i(so.test_inject_leg), i(so.test_inject_sm),
-        u(so.test_inject_element), u(so.test_inject_iteration), i(so.test_inject_word), u(so.test_inject_mask), i(caps.faults[2]),
-        u(lo.bytes), u(lo.iterations), u(lo.a1_counters), u(lo.a2_counters), i(lo.test_inject_leg), i(lo.test_inject_sm),
-        i(lo.test_inject_element), u(lo.test_inject_iteration), i(lo.test_inject_word), u(lo.test_inject_mask), i(caps.faults[3]),
-        u(ko.bytes), u(ko.hops), u(ko.ctas), i(ko.test_inject_check), u(ko.test_inject_word), u(ko.test_inject_mask),
-        i(caps.faults[4]),
-        u(xo.max_bytes), u(xo.reserve_bytes), u(xo.seed), u(xo.test_chunk_bytes), u(xo.test_force_first), u(xo.test_force_count),
-        u(xo.test_force_and), u(xo.test_force_or), i(caps.faults[5])};
+    std::vector<std::string> args = {"health-raw", want, std::to_string(helper_seed_base(c)), std::to_string(checks)};
     size_t max_tail = 0;
-    for (int k = 0; k < CRO_HEALTH_CHECKS; ++k)
-        if (checks >> k & 1u) max_tail += kParts[k].head() + (size_t)caps.faults[k] * kParts[k].rec;
+    for (int k = 0; k < CRO_HEALTH_CHECKS; ++k) {
+        const cro_wire& w = *cro_wire_health[k].wire;
+        append_wire_args(w, reinterpret_cast<const char*>(&o) + cro_wire_health[k].opts_at, caps.faults[k], &args);
+        if (checks >> k & 1u) max_tail += cro_wire_head(&w.frame) + (size_t)caps.faults[k] * w.frame.rec;
+    }
     std::string got;
-    const int rc = run_probe_helper(c, want, "health helper", "cro.check_health.helper", args, deadline_ms, sizeof *r, 1, max_tail,
+    const int rc = run_probe_helper(c, want, "health helper", "cro.check_health.helper", args, deadline_ms, sizeof *r, max_tail,
                                     health_tail, &got, helper_ns);
     if (rc != CRO_OK) return r->status = rc;
     const unsigned char* f = reinterpret_cast<const unsigned char*>(got.data());
@@ -201,29 +138,32 @@ int ctx_check_health_uuid(cro_ctx* c, const char* uuid, const cro_health_opts& o
     std::string bad;
     if (r->checks != checks || ((r->ran | r->not_run) & ~checks) || (r->ran & r->not_run)) bad = "checks outside the selection";
     size_t at = sizeof *r;
-    void* held[CRO_HEALTH_CHECKS] = {&r->compute, &r->precision, &r->sram, &r->l2, &r->link, &r->scan};
+    std::vector<unsigned char> no_sms;
     for (int k = 0; k < CRO_HEALTH_CHECKS && bad.empty(); ++k) {
+        const cro_wire_frame& w = cro_wire_health[k].wire->frame;
+        unsigned char* held = reinterpret_cast<unsigned char*>(r) + cro_wire_health[k].result_at;
         if (!(r->ran >> k & 1u)) {
-            memset(held[k], 0, kParts[k].result);       // blank when it did not run
+            memset(held, 0, w.result);       // blank when it did not run
             continue;
         }
-        const Part& p = kParts[k];
         const unsigned char* part = f + at;
-        uint64_t n_sms, n;
-        p.read(part, &n_sms, &n);
-        if (memcmp(part, held[k], p.result) != 0) bad = "a check's result differs from the one the health result holds";
-        else if (n > (uint64_t)caps.faults[k]) bad = "more records than asked for";
-        const unsigned char* sms = part + p.head() - p.sms;
-        const unsigned char* recs = part + p.head();
+        uint64_t tail = 0;
+        size_t n = 0;
+        auto take = [&](auto* recs, auto* sms) {
+            tail = read_frame(w, part, got.size() - at, nullptr, recs, sms);
+            n = recs->size();
+        };
         switch (k) {
-            case 0: take(sms, n_sms, &rec->compute_sms); take(recs, n, &rec->compute_faults); break;
-            case 1: take(sms, n_sms, &rec->precision_sms); take(recs, n, &rec->precision_faults); break;
-            case 2: take(sms, n_sms, &rec->sram_sms); take(recs, n, &rec->sram_faults); break;
-            case 3: take(sms, n_sms, &rec->l2_sms); take(recs, n, &rec->l2_faults); break;
-            case 4: take(recs, n, &rec->link_faults); break;
-            case 5: take(recs, n, &rec->scan_words); break;
+            case 0: take(&rec->compute_faults, &rec->compute_sms); break;
+            case 1: take(&rec->precision_faults, &rec->precision_sms); break;
+            case 2: take(&rec->sram_faults, &rec->sram_sms); break;
+            case 3: take(&rec->l2_faults, &rec->l2_sms); break;
+            case 4: take(&rec->link_faults, &no_sms); break;
+            case 5: take(&rec->scan_words, &no_sms); break;
         }
-        at += p.head() + n * p.rec;
+        if (memcmp(part, held, w.result) != 0) bad = "a check's result differs from the one the health result holds";
+        else if (n > (size_t)caps.faults[k]) bad = "more records than asked for";
+        at += w.result + tail;
     }
     if (!bad.empty()) {
         set_call_error(c, "health helper for " + want + " failed (" + bad + ")");

@@ -351,15 +351,6 @@ int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_re
 // The helper's sweep region is L, or the default L when none is given: refuse here what it would refuse there.
 std::string link_helper_opts_error(const cro_link_opts& o) { return link_opts_error(o, o.bytes ? o.bytes : kLinkDefaultBytes); }
 
-namespace {
-// link-raw's stdout: the result, the helper's own fault count n, then n faults.
-uint64_t link_tail_count(const unsigned char* head, size_t) {
-    uint64_t n;
-    memcpy(&n, head + sizeof(cro_link_result), sizeof n);
-    return n;
-}
-}  // namespace
-
 int ctx_probe_host_link_uuid(cro_ctx* c, const char* uuid, const cro_link_opts& o, int deadline_ms, cro_link_result* r,
                              std::vector<cro_link_fault>* faults, int cap, uint64_t* helper_ns) {
     blank_result(r, faults, 0);
@@ -370,19 +361,7 @@ int ctx_probe_host_link_uuid(cro_ctx* c, const char* uuid, const cro_link_opts& 
         set_call_error(c, why);
         return r->status = CRO_ERR_INVALID_ARG;
     }
-    const std::string want = uuid;
-    auto num = [](uint64_t v) { return std::to_string(v); };
-    const std::vector<std::string> args = {"link-raw", want, num(helper_seed_base(c)), num(o.bytes), num(o.hops), num(o.ctas),
-                                           std::to_string(o.test_inject_check), num(o.test_inject_word), num(o.test_inject_mask),
-                                           num((uint64_t)cap)};
-    const size_t head = sizeof *r + sizeof(uint64_t);
-    std::string got;
-    const int rc = run_probe_helper(c, want, "link helper", "cro.probe_host_link.helper", args, deadline_ms, head,
-                                    sizeof(cro_link_fault), (size_t)cap, link_tail_count, &got, helper_ns);
-    if (rc != CRO_OK) return r->status = rc;
-    memcpy(r, got.data(), sizeof *r);
-    const cro_link_fault* f = reinterpret_cast<const cro_link_fault*>(got.data() + head);
-    faults->assign(f, f + link_tail_count(reinterpret_cast<const unsigned char*>(got.data()), got.size()));
+    run_check_helper(c, cro_wire_link, uuid, "link helper", "cro.probe_host_link.helper", &o, cap, deadline_ms, helper_ns, r, faults);
     return r->status;
 }
 

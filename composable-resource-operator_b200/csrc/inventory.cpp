@@ -108,8 +108,9 @@ std::string DefaultHelperPath() {
 }
 
 int RunHelperRaw(const std::string& helper_path, const std::string& what, const std::string& uuid,
-                 const std::vector<std::string>& args, int deadline_ms, size_t head, size_t rec, size_t max_rec,
-                 uint64_t (*count)(const unsigned char* out, size_t size), std::string* out, std::string* err) {
+                 const std::vector<std::string>& args, int deadline_ms, size_t head, size_t max_tail,
+                 const std::function<uint64_t(const unsigned char* out, size_t size)>& tail, std::string* out,
+                 std::string* err) {
     const std::string helper = helper_path.empty() ? DefaultHelperPath() : helper_path;
     if (access(helper.c_str(), X_OK) != 0) {
         if (err) *err = what + " '" + helper + "' is not executable";
@@ -147,7 +148,7 @@ int RunHelperRaw(const std::string& helper_path, const std::string& what, const 
         return CRO_ERR_EXEC;
     }
     close(fds[1]);
-    const size_t cap = head + rec * max_rec;
+    const size_t cap = head + max_tail;
     out->clear();
     bool timed_out = false;
     const auto until = std::chrono::steady_clock::now() + std::chrono::milliseconds(deadline_ms > 0 ? deadline_ms : 30000);
@@ -190,8 +191,8 @@ int RunHelperRaw(const std::string& helper_path, const std::string& what, const 
         if (err) *err = "device '" + uuid + "' is not visible to a fresh CUDA process";
         return CRO_ERR_NO_DEVICE;
     }
-    const uint64_t n_rec = out->size() >= head && count ? count(reinterpret_cast<const unsigned char*>(out->data()), out->size()) : 0;
-    if (out->size() < head || n_rec > max_rec || out->size() != head + rec * n_rec || (code != 0 && code != 1)) {
+    const uint64_t n_tail = out->size() >= head && tail ? tail(reinterpret_cast<const unsigned char*>(out->data()), out->size()) : 0;
+    if (out->size() < head || n_tail > max_tail || out->size() != head + n_tail || (code != 0 && code != 1)) {
         if (err) *err = what + " for " + uuid + " failed (exit " + std::to_string(code) + ", " + std::to_string(out->size()) + " result bytes)";
         return CRO_ERR_EXEC;
     }
@@ -202,8 +203,8 @@ int RunHelper(const std::string& helper_path, const std::string& uuid, uint64_t 
               cro_probe_result* out, std::string* err) {
     const std::string mib = std::to_string(std::max<uint64_t>(1, sweep_bytes >> 20));
     std::string got;
-    const int rc = RunHelperRaw(helper_path, "probe helper", uuid, {"probe-raw", uuid, mib}, deadline_ms, sizeof *out, 0, 0,
-                                nullptr, &got, err);
+    const int rc = RunHelperRaw(helper_path, "probe helper", uuid, {"probe-raw", uuid, mib}, deadline_ms, sizeof *out, 0, nullptr,
+                                &got, err);
     if (rc != CRO_OK) return rc;
     memcpy(out, got.data(), sizeof *out);
     if (out->abi_version != CRO_ABI_VERSION) {

@@ -403,20 +403,10 @@ int ctx_probe_l2_uuid(cro_ctx* c, const char* uuid, const cro_l2_opts& o, cro_l2
         set_call_error(c, why);
         return r->status = CRO_ERR_INVALID_ARG;
     }
-    const std::string want = uuid;
-    auto num = [](int64_t v) { return std::to_string(v); };
-    const std::vector<std::string> args = {"l2-raw", want, std::to_string(helper_seed_base(c)), std::to_string(o.bytes),
-                                           num(o.iterations), num(o.a1_counters), num(o.a2_counters), num(o.test_inject_leg),
-                                           num(o.test_inject_sm), num(o.test_inject_element), num(o.test_inject_iteration),
-                                           num(o.test_inject_word), std::to_string(o.test_inject_mask), num(cap)};
-    using Frame = SmFrame<cro_l2_result, cro_l2_sm, cro_l2_fault, CRO_L2_MAX_SMS>;
-    std::string got;
     uint64_t helper_ns = 0;
-    const int rc = run_probe_helper(c, want, "L2 helper", "cro.probe_l2.helper", args, o.deadline_ms, Frame::kHead,
-                                    sizeof(cro_l2_fault), (size_t)cap, Frame::tail, &got, &helper_ns);
-    if (rc != CRO_OK) return r->status = rc;
-    Frame::read(got, r, sms, faults);
-    r->helper_ns = helper_ns;
+    if (run_check_helper(c, cro_wire_l2, uuid, "L2 helper", "cro.probe_l2.helper", &o, cap, o.deadline_ms, &helper_ns, r, faults,
+                         sms) == CRO_OK)
+        r->helper_ns = helper_ns;
     return r->status;
 }
 

@@ -110,6 +110,7 @@ struct PrecisionProbe {
     using Args = PrecisionArgs;
     using Tile = int64_t;
     static constexpr const char* kName = "precision";
+    static constexpr const cro_wire& kWire = cro_wire_precision;
     static constexpr uint32_t kLegs = CRO_PRECISION_LEGS, kAllLegs = CRO_PRECISION_ALL_LEGS, kMaxSms = CRO_PRECISION_MAX_SMS;
     static constexpr uint32_t kRecords = CRO_PRECISION_RECORDS;
     static constexpr int kAnswers = CRO_PRECISION_ANSWERS;
@@ -131,7 +132,6 @@ struct PrecisionProbe {
     static cudaError_t launch(uint32_t leg, const PrecisionArgs& a, int grid, cudaStream_t st) { return launch_precision(leg, a, grid, st); }
 
     static void test_args(const cro_precision_opts&, uint32_t, PrecisionArgs*) {}
-    static std::vector<std::string> helper_args(const cro_precision_opts& o) { return dense_helper_args(o); }
 
     static std::string opts_error(const cro_precision_opts& o) {
         const uint32_t legs = o.legs ? o.legs : CRO_PRECISION_ALL_LEGS;

@@ -883,6 +883,15 @@ uint64_t helper_seed_base(cro_ctx* c) {
     return s ? s : 0x100;         // 0 would ask the helper for the default base
 }
 
+void append_wire_args(const cro_wire& w, const void* o, int cap, std::vector<std::string>* args) {
+    char s[24];
+    for (uint32_t i = 0; i < w.n_fields; ++i) {
+        cro_wire_format(&w, i, o, s, sizeof s);
+        args->push_back(s);
+    }
+    args->push_back(std::to_string(cap));
+}
+
 // run_probe_helper reads a helper result's status from the first four bytes of its frame.
 template <class R>
 constexpr bool status_first() { return offsetof(R, status) == 0 && std::is_same<decltype(R::status), int32_t>::value; }
@@ -891,8 +900,9 @@ static_assert(status_first<cro_link_result>() && status_first<cro_compute_result
               "every helper result begins with its int32_t status");
 
 int run_probe_helper(cro_ctx* c, const std::string& uuid, const std::string& what, const char* range,
-                     const std::vector<std::string>& args, int deadline_ms, size_t head, size_t rec, size_t cap,
-                     uint64_t (*count)(const unsigned char* out, size_t size), std::string* got, uint64_t* helper_ns) {
+                     const std::vector<std::string>& args, int deadline_ms, size_t head, size_t max_tail,
+                     const std::function<uint64_t(const unsigned char* out, size_t size)>& tail, std::string* got,
+                     uint64_t* helper_ns) {
     env::Values knobs;                        // no context: this caller's environment, defaults where it is illegal
     if (c) knobs = c->knobs;
     else env::read(&knobs, nullptr);
@@ -910,7 +920,7 @@ int run_probe_helper(cro_ctx* c, const std::string& uuid, const std::string& wha
     std::string err;
     if (c && c->nvtx) nvtxRangePushA(range);
     const uint64_t t_spawn = now_ns();
-    const int rc = inventory::RunHelperRaw("", what, uuid, args, deadline, head, rec, cap, count, got, &err);
+    const int rc = inventory::RunHelperRaw("", what, uuid, args, deadline, head, max_tail, tail, got, &err);
     *helper_ns = now_ns() - t_spawn;
     if (c && c->nvtx) nvtxRangePop();
     if (rc != CRO_OK) {

@@ -13,6 +13,7 @@
 #include <chrono>
 #include <cstring>
 #include <deque>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -20,6 +21,7 @@
 #include <vector>
 
 #include "../../include/croprobe.h"
+#include "helper_wire.h"
 #include "kernels.cuh"
 
 namespace cro {
@@ -280,47 +282,71 @@ namespace precision {
 int Expected(int answer, uint64_t seed, int64_t* out);
 }  // namespace precision
 
-// The helper run behind the uuid forms of the host link, compute, precision, scan, SRAM and L2 probes.  Bad options
-// are refused by the caller first.  With a context, the node must list the GPU (CRO_ERR_NO_DEVICE otherwise) and a GPU
-// that is also an in-process device is held under its device guard while the helper runs.  Then `croprobe-cli args...`
-// runs as inventory::RunHelperRaw runs it ("<what> for <uuid> ..." in its errors) and its stdout lands in *got.
-// *helper_ns: spawn to exit.  CRO_OK means *got is a whole frame; the result's status, its first field, is the call's
-// status then, and one other than CRO_OK or CRO_ERR_CHECKSUM is an error too.  An error goes to the context, or to the
-// calling thread without one.
+// The helper run behind the uuid forms of the host link, compute, precision, sparse, scan, SRAM and L2 probes and the
+// health check.  Bad options are refused by the caller first.  With a context, the node must list the GPU
+// (CRO_ERR_NO_DEVICE otherwise) and a GPU that is also an in-process device is held under its device guard while the
+// helper runs.  Then `croprobe-cli args...` runs as inventory::RunHelperRaw runs it ("<what> for <uuid> ..." in its
+// errors): its stdout, head bytes and then tail(out, size) more, at most max_tail, lands in *got.  *helper_ns: spawn to
+// exit.  CRO_OK means *got is a whole frame; the result's status, its first field, is the call's status then, and one
+// other than CRO_OK or CRO_ERR_CHECKSUM is an error too.  An error goes to the context, or to the calling thread
+// without one.
 int run_probe_helper(cro_ctx* c, const std::string& uuid, const std::string& what, const char* range,
-                     const std::vector<std::string>& args, int deadline_ms, size_t head, size_t rec, size_t cap,
-                     uint64_t (*count)(const unsigned char* out, size_t size), std::string* got, uint64_t* helper_ns);
-// The stdout of compute-raw, precision-raw and l2-raw: the Result, the helper's own counts n_sms and n (uint64_t),
-// MAX_SMS Sm entries (n_sms of them filled), then n Fault records.  An n_sms the entries cannot hold makes the output
-// malformed.
-template <class Result, class Sm, class Fault, size_t MAX_SMS>
-struct SmFrame {
-    static constexpr size_t kCounts = sizeof(Result);
-    static constexpr size_t kSms = kCounts + 2 * sizeof(uint64_t);
-    static constexpr size_t kHead = kSms + MAX_SMS * sizeof(Sm);
-    static uint64_t count(const unsigned char* head, int which) {
-        uint64_t v;
-        memcpy(&v, head + kCounts + which * sizeof v, sizeof v);
-        return v;
+                     const std::vector<std::string>& args, int deadline_ms, size_t head, size_t max_tail,
+                     const std::function<uint64_t(const unsigned char* out, size_t size)>& tail, std::string* got,
+                     uint64_t* helper_ns);
+// One check's frame (helper_wire.h) at f, size bytes from there on: the bytes it takes after its result, or ~0 when it
+// is cut short, lists more per-SM entries than its block holds or more records than follow.  Its result, records and
+// per-SM entries go to whichever of r, recs and sms are given.
+template <class Rec = unsigned char, class Sm = unsigned char>
+uint64_t read_frame(const cro_wire_frame& w, const unsigned char* f, size_t size, void* r = nullptr,
+                    std::vector<Rec>* recs = nullptr, std::vector<Sm>* sms = nullptr) {
+    const size_t head = cro_wire_head(&w);
+    if (size < head) return ~0ull;
+    uint64_t n_sms = 0, n = 0;
+    memcpy(&n_sms, f + w.n_sms_at, w.n_sms_width);
+    memcpy(&n, f + w.n_at, w.n_width);
+    if (n_sms > w.max_sms || n > (size - head) / w.rec) return ~0ull;
+    if (r) memcpy(r, f, w.result);
+    if (sms) {
+        const Sm* s = reinterpret_cast<const Sm*>(f + head - (size_t)w.max_sms * w.sm);
+        sms->assign(s, s + n_sms);
     }
-    // The record count run_probe_helper's count argument gives RunHelperRaw.
-    static uint64_t tail(const unsigned char* head, size_t) { return count(head, 0) > MAX_SMS ? ~0ull : count(head, 1); }
-    // Unpacks a frame run_probe_helper accepted.
-    static void read(const std::string& got, Result* r, std::vector<Sm>* sms, std::vector<Fault>* faults) {
-        const unsigned char* head = reinterpret_cast<const unsigned char*>(got.data());
-        memcpy(r, head, sizeof *r);
-        const Sm* s = reinterpret_cast<const Sm*>(head + kSms);
-        sms->assign(s, s + count(head, 0));
-        const Fault* f = reinterpret_cast<const Fault*>(head + kHead);
-        faults->assign(f, f + count(head, 1));
+    if (recs) {
+        const Rec* x = reinterpret_cast<const Rec*>(f + head);
+        recs->assign(x, x + n);
     }
-};
+    return head - w.result + n * w.rec;
+}
 // The cro_opts.seed_base a helper of the link, compute, precision and L2 forms gets: with a context, its seed_base +
 // (h << 8) for the context's h-th such call (h from 1, so no helper repeats the context's own seeds); without one, a
 // clock-derived base.  The low byte is clear either way: the helper ORs the minor into it.
 uint64_t helper_seed_base(cro_ctx* c);
 // Sets an error text on the context, or on the calling thread without one.
 void set_call_error(cro_ctx* c, const std::string& m);
+// w's option fields of the options at o as argv, then the record cap.
+void append_wire_args(const cro_wire& w, const void* o, int cap, std::vector<std::string>* args);
+// The helper form of one check: `croprobe-cli <w.cmd> <uuid> [<seed base>] <options> <cap>` (a fresh seed base,
+// helper_seed_base, when w is seeded) through run_probe_helper, its frame unpacked into *r, *recs and *sms.  Returns
+// run_probe_helper's code; *r is blank but for its status when that is not CRO_OK.
+template <class Result, class Rec, class Sm = unsigned char>
+int run_check_helper(cro_ctx* c, const cro_wire& w, const std::string& uuid, const std::string& what, const char* range,
+                     const void* opts, int cap, int deadline_ms, uint64_t* helper_ns, Result* r, std::vector<Rec>* recs,
+                     std::vector<Sm>* sms = nullptr) {
+    std::vector<std::string> args = {w.cmd, uuid};
+    if (w.seeded) args.push_back(std::to_string(helper_seed_base(c)));
+    append_wire_args(w, opts, cap, &args);
+    std::string got;
+    const int rc = run_probe_helper(c, uuid, what, range, args, deadline_ms, w.frame.result,
+                                    cro_wire_head(&w.frame) - w.frame.result + (size_t)cap * w.frame.rec,
+                                    [&w](const unsigned char* f, size_t size) { return read_frame(w.frame, f, size); }, &got,
+                                    helper_ns);
+    if (rc != CRO_OK) {
+        r->status = rc;
+        return rc;
+    }
+    read_frame(w.frame, reinterpret_cast<const unsigned char*>(got.data()), got.size(), r, recs, sms);
+    return CRO_OK;
+}
 
 // Whole-HBM scan (include/croprobe.h, cro_scan_hbm / cro_scan_hbm_uuid, hbm_scan.cu): *words gets every recorded word,
 // merged by scan index.  The uuid form runs `croprobe-cli scan-raw` and asks it for at most cap words.

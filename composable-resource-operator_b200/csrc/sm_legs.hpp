@@ -152,8 +152,9 @@ int take_leg(cro_ctx* c, const char* who, const std::vector<ComputeCta>& hc, con
 // What a probe P gives the calls below:
 //   Opts, Result, Sm, Fault, Args    its option, result, per-SM, record and kernel argument types
 //   Tile                             the element type of its answer tiles (Args::expect points into them)
-//   kName                            "compute", "precision", "sparse": "<kName> probe" in error texts, croprobe-cli
-//                                    <kName>-raw
+//   kName                            "compute", "precision", "sparse": "<kName> probe" and "<kName> helper" in error
+//                                    texts
+//   kWire                            its helper command's argv and frame (helper_wire.h), croprobe-cli <kName>-raw
 //   kLegs, kAllLegs, kMaxSms, kRecords, kAnswers, kCalls (its call counter in Device), kSeeds (its seed space)
 //   kDefaultIterations, kDefaultRounds, kAluLeg[leg] (the leg runs alu_iterations; with any such leg, Opts has
 //                                    alu_iterations and P kDefaultAluIterations)
@@ -163,7 +164,6 @@ int take_leg(cro_ctx* c, const char* who, const std::vector<ComputeCta>& hc, con
 //   launch(leg, args, grid, stream)  one launch of a leg
 //   opts_error(opts)                 why the options are refused ("" when they pass), both forms' argument check
 //   test_args(opts, leg, &args)      the launch's test fields beyond the accumulator injection (none: an empty body)
-//   helper_args(opts)                the option fields of the helper's argv, between the seed base and the cap
 
 // The result of a call that computed nothing: zeroes but for what the call had settled before it stopped (`from`'s
 // seed, call number, SM count and legs).
@@ -195,16 +195,6 @@ void leg_iterations(const typename P::Opts& o, uint32_t (&iters)[P::kLegs]) {
         for (uint32_t l = 0; l < P::kLegs; ++l)
             if (P::kAluLeg[l]) iters[l] = ai;
     }
-}
-
-// The option fields of compute-raw's and precision-raw's argv.
-template <class Opts>
-std::vector<std::string> dense_helper_args(const Opts& o) {
-    using std::to_string;
-    return {to_string(o.iterations),      to_string(o.alu_iterations),        to_string(o.legs),
-            to_string(o.max_rounds),      to_string(o.test_inject_leg),       to_string(o.test_inject_sm),
-            to_string(o.test_inject_iteration), to_string(o.test_inject_row), to_string(o.test_inject_col),
-            to_string(o.test_inject_mask)};
 }
 
 // The in-process form: call k of the device gets the seed space_seed(d, P::kSeeds, k), its answer tiles computed here
@@ -364,8 +354,7 @@ int classify_sm_legs(uint32_t legs, const uint32_t* iterations, uint32_t grid, u
     return close_call(r, P::kLegs, per_sm, sms, faults);
 }
 
-// The helper form: `croprobe-cli <kName>-raw` with a fresh seed base (helper_seed_base), the options (helper_args) and
-// cap on argv.
+// The helper form: `croprobe-cli <kName>-raw` with a fresh seed base, the options and cap on argv (run_check_helper).
 template <class P>
 int probe_sm_legs_uuid(cro_ctx* c, const char* uuid, const typename P::Opts& o, int deadline_ms, typename P::Result* r,
                        std::vector<typename P::Sm>* sms, std::vector<typename P::Fault>* faults, int cap, uint64_t* helper_ns) {
@@ -377,18 +366,9 @@ int probe_sm_legs_uuid(cro_ctx* c, const char* uuid, const typename P::Opts& o, 
         set_call_error(c, why);
         return r->status = CRO_ERR_INVALID_ARG;
     }
-    const std::string want = uuid, name = P::kName;
-    using std::to_string;
-    std::vector<std::string> args = {name + "-raw", want, to_string(helper_seed_base(c))};
-    const std::vector<std::string> fields = P::helper_args(o);
-    args.insert(args.end(), fields.begin(), fields.end());
-    args.push_back(to_string(cap));
-    using Frame = SmFrame<typename P::Result, typename P::Sm, typename P::Fault, P::kMaxSms>;
-    std::string got;
-    const int rc = run_probe_helper(c, want, name + " helper", ("cro.probe_" + name + ".helper").c_str(), args, deadline_ms,
-                                    Frame::kHead, sizeof(typename P::Fault), (size_t)cap, Frame::tail, &got, helper_ns);
-    if (rc != CRO_OK) return r->status = rc;
-    Frame::read(got, r, sms, faults);
+    const std::string name = P::kName;
+    run_check_helper(c, P::kWire, uuid, name + " helper", ("cro.probe_" + name + ".helper").c_str(), &o, cap, deadline_ms,
+                     helper_ns, r, faults, sms);
     return r->status;
 }
 

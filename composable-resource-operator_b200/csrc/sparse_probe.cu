@@ -96,6 +96,7 @@ struct SparseProbe {
     using Args = SparseArgs;
     using Tile = int32_t;
     static constexpr const char* kName = "sparse";
+    static constexpr const cro_wire& kWire = cro_wire_sparse;
     static constexpr uint32_t kLegs = CRO_SPARSE_LEGS, kAllLegs = CRO_SPARSE_ALL_LEGS, kMaxSms = CRO_SPARSE_MAX_SMS;
     static constexpr uint32_t kRecords = CRO_SPARSE_RECORDS;
     static constexpr int kAnswers = CRO_SPARSE_ANSWERS;
@@ -122,14 +123,6 @@ struct SparseProbe {
         a->meta_iter = o.test_meta_iteration;
         a->meta_row = o.test_meta_row;
         a->meta_group = o.test_meta_group;
-    }
-    static std::vector<std::string> helper_args(const cro_sparse_opts& o) {
-        using std::to_string;
-        return {to_string(o.iterations),       to_string(o.legs),          to_string(o.max_rounds),
-                to_string(o.test_inject_leg),  to_string(o.test_inject_sm), to_string(o.test_inject_iteration),
-                to_string(o.test_inject_row),  to_string(o.test_inject_col), to_string(o.test_inject_mask),
-                to_string(o.test_meta),        to_string(o.test_meta_leg), to_string(o.test_meta_sm),
-                to_string(o.test_meta_iteration), to_string(o.test_meta_row), to_string(o.test_meta_group)};
     }
 
     static std::string opts_error(const cro_sparse_opts& o) {

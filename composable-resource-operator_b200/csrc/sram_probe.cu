@@ -414,34 +414,14 @@ int classify_sram(uint32_t legs, uint32_t iterations, uint32_t n_words, uint64_t
     return close_sram_call(r, t, sms, faults);
 }
 
-namespace {
-uint64_t sram_tail_count(const unsigned char* head, size_t) {
-    return reinterpret_cast<const cro_sram_result*>(head)->recorded;
-}
-}  // namespace
-
 int ctx_probe_sram_uuid(cro_ctx* c, const char* uuid, const cro_sram_opts& o, cro_sram_result* r, std::vector<cro_sram_sm>* sms,
                         std::vector<cro_sram_fault>* faults, int cap) {
     blank_result(r, cro_sram_result{}, sms, faults);
     if (!uuid) return r->status = CRO_ERR_INVALID_ARG;
-    const std::string want = uuid;
-    auto num = [](int64_t v) { return std::to_string(v); };
-    const std::vector<std::string> args = {"sram-raw", want, num(o.legs), num(o.iterations), num(o.cluster), num(o.max_rounds),
-                                           num(o.test_inject_leg), num(o.test_inject_sm), num(o.test_inject_element),
-                                           num(o.test_inject_iteration), num(o.test_inject_word), std::to_string(o.test_inject_mask),
-                                           num(cap)};
-    const size_t head = sizeof *r + CRO_SRAM_MAX_SMS * sizeof(cro_sram_sm);
-    std::string got;
     uint64_t helper_ns = 0;
-    const int rc = run_probe_helper(c, want, "SRAM helper", "cro.probe_sram.helper", args, o.deadline_ms, head,
-                                    sizeof(cro_sram_fault), (size_t)cap, sram_tail_count, &got, &helper_ns);
-    if (rc != CRO_OK) return r->status = rc;
-    memcpy(r, got.data(), sizeof *r);
-    const cro_sram_sm* s = reinterpret_cast<const cro_sram_sm*>(got.data() + sizeof *r);
-    sms->assign(s, s + std::min<uint32_t>(r->sms_listed, CRO_SRAM_MAX_SMS));
-    const cro_sram_fault* f = reinterpret_cast<const cro_sram_fault*>(got.data() + head);
-    faults->assign(f, f + r->recorded);
-    r->helper_ns = helper_ns;
+    if (run_check_helper(c, cro_wire_sram, uuid, "SRAM helper", "cro.probe_sram.helper", &o, cap, o.deadline_ms, &helper_ns, r,
+                         faults, sms) == CRO_OK)
+        r->helper_ns = helper_ns;
     return r->status;
 }
 

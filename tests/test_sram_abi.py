@@ -295,6 +295,13 @@ def test_sram_helper_failures_are_loud(cro, tmp_path, monkeypatch):
     with pytest.raises(cro.ProbeError) as e:
         cro.probe_sram_uuid(None, U)
     assert e.value.code == cro.ERR_EXEC and "SRAM helper for %s failed" % U in str(e.value)
+    listed = 'struct.pack_into("<II", r, 88, 0, 2)'                                           # more SMs than the block holds
+    assert listed in SRAM_HELPER
+    too_many = (SRAM_HELPER % "").replace(listed, 'struct.pack_into("<II", r, 88, 0, %d)' % (cro.SRAM_MAX_SMS + 1))
+    monkeypatch.setenv("CRO_HELPER_PATH", fake_helper(tmp_path, too_many))
+    with pytest.raises(cro.ProbeError) as e:
+        cro.probe_sram_uuid(None, U)
+    assert e.value.code == cro.ERR_EXEC and "SRAM helper for %s failed" % U in str(e.value)
     monkeypatch.setenv("CRO_HELPER_PATH", fake_helper(tmp_path, "import sys\nsys.exit(3)\n"))
     with pytest.raises(cro.ProbeError) as e:
         cro.probe_sram_uuid(None, U)
