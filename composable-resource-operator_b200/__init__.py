@@ -512,6 +512,74 @@ class SramFault(ctypes.Structure):
                 ("actual", ctypes.c_uint64)]
 
 
+# register-file probe (cro_probe_regfile, cro_probe_regfile_uuid, cro_selftest_regfile_classify)
+REGFILE_SLOTS, REGFILE_THREADS, REGFILE_ELEMENTS, REGFILE_RECORDS, REGFILE_MAX_SMS = 224, 256, 2, 4096, 256
+REGFILE_MAX_ITERATIONS, REGFILE_MAX_ROUNDS = 4096, 64
+REGFILE_NONE, REGFILE_SM, REGFILE_ALL = 0, 1, 2
+REGFILE_PERSISTENT, REGFILE_INTERMITTENT = 1, 2
+
+
+class RegfileOpts(ctypes.Structure):
+    _fields_ = [("iterations", ctypes.c_uint32), ("max_rounds", ctypes.c_uint32), ("deadline_ms", ctypes.c_int32),
+                ("test_inject_sm", ctypes.c_int32), ("test_inject_warp", ctypes.c_int32), ("test_inject_lane", ctypes.c_int32),
+                ("test_inject_slot", ctypes.c_int32), ("test_inject_element", ctypes.c_uint32),
+                ("test_inject_iteration", ctypes.c_uint32), ("test_inject_mask", ctypes.c_uint32)]
+
+
+class RegfileResult(ctypes.Structure):
+    """cro_regfile_result: status, verdict, bad SMs, per-element counts, the fold and its closed form, coverage and
+    times, the kernel's registers and NVML's SRAM health of one register-file probe call."""
+    _fields_ = [("status", ctypes.c_int32), ("verdict", ctypes.c_uint32), ("seed", ctypes.c_uint64), ("call", ctypes.c_uint64),
+                ("sm_count", ctypes.c_uint32), ("nsmid", ctypes.c_uint32), ("cuda_error", ctypes.c_int32),
+                ("health", ctypes.c_uint32), ("iterations", ctypes.c_uint32), ("rounds", ctypes.c_uint32),
+                ("slots", ctypes.c_uint32), ("threads", ctypes.c_uint32), ("num_regs", ctypes.c_uint32),
+                ("regs_per_sm", ctypes.c_uint32), ("sms_covered", ctypes.c_uint32), ("complete", ctypes.c_uint32),
+                ("ctas", ctypes.c_uint32), ("unpublished", ctypes.c_uint32), ("failed_sms", ctypes.c_uint32),
+                ("bad_sms", ctypes.c_uint32), ("bad_sm", ctypes.c_uint16 * 16),
+                ("mismatches", ctypes.c_uint64 * REGFILE_ELEMENTS), ("fold_mismatches", ctypes.c_uint64),
+                ("recorded", ctypes.c_uint64), ("sms_listed", ctypes.c_uint32), ("reserved", ctypes.c_uint32),
+                ("bits_checked", ctypes.c_uint64), ("ns", ctypes.c_uint64), ("timer_ns", ctypes.c_uint64),
+                ("wall_ns", ctypes.c_uint64), ("helper_ns", ctypes.c_uint64), ("fold_xor", ctypes.c_uint64),
+                ("fold_sum", ctypes.c_uint64), ("fold_wsum", ctypes.c_uint64), ("expect_xor", ctypes.c_uint64),
+                ("expect_sum", ctypes.c_uint64), ("expect_wsum", ctypes.c_uint64), ("before", SramHealth),
+                ("after", SramHealth)]
+
+    @property
+    def fold(self) -> Tuple[int, int, int]:
+        return (self.fold_xor, self.fold_sum, self.fold_wsum)
+
+    @property
+    def expect(self) -> Tuple[int, int, int]:
+        return (self.expect_xor, self.expect_sum, self.expect_wsum)
+
+
+class RegfileSm(ctypes.Structure):
+    """One SM seen by a register-file probe call: its per-element counts, fold mismatches, times and REGFILE_PERSISTENT /
+    _INTERMITTENT mark."""
+    _fields_ = [("smid", ctypes.c_uint32), ("mark", ctypes.c_uint32), ("mismatches", ctypes.c_uint64 * REGFILE_ELEMENTS),
+                ("fold_mismatches", ctypes.c_uint64), ("ns", ctypes.c_uint64), ("cycles", ctypes.c_uint64),
+                ("ctas", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+class RegfileFault(ctypes.Structure):
+    """One failed compare: element, iteration, SM, warp, lane, slot, expected and actual word."""
+    _fields_ = [("element", ctypes.c_uint32), ("iteration", ctypes.c_uint32), ("smid", ctypes.c_uint32),
+                ("warp", ctypes.c_uint32), ("lane", ctypes.c_uint32), ("slot", ctypes.c_uint32),
+                ("expected", ctypes.c_uint32), ("actual", ctypes.c_uint32)]
+
+
+class RegfileCta(ctypes.Structure):
+    """cro_regfile_cta: what one CTA of the register-file probe publishes at the end of a round."""
+    _fields_ = [("stamp", ctypes.c_uint64), ("t0", ctypes.c_uint64), ("t1", ctypes.c_uint64), ("cycles", ctypes.c_uint64),
+                ("count", ctypes.c_uint64 * REGFILE_ELEMENTS), ("last", ctypes.c_uint64), ("fold_x", ctypes.c_uint64),
+                ("fold_s", ctypes.c_uint64), ("fold_w", ctypes.c_uint64), ("smid", ctypes.c_uint32), ("nsmid", ctypes.c_uint32),
+                ("block", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+assert ctypes.sizeof(RegfileOpts) == 40 and ctypes.sizeof(RegfileResult) == 296 and ctypes.sizeof(RegfileSm) == 56 \
+    and ctypes.sizeof(RegfileFault) == 32 and ctypes.sizeof(RegfileCta) == 96, ctypes.sizeof(RegfileResult)
+
+
 # L2 probe (cro_probe_l2, cro_read_l2_health, cro_selftest_l2_classify)
 L2_BLOCK_BYTES, L2_MIN_BYTES, L2_MAX_L2_MULTIPLE, L2_ELEMENTS, L2_RECORDS, L2_MAX_SMS = 16384, 1 << 20, 8, 6, 4096, 256
 L2_MAX_ITERATIONS, L2_MAX_A1_COUNTERS, L2_MAX_A2_COUNTERS, L2_MAX_LINES, L2_MAX_COUNTERS = 256, 1 << 20, 8192, 8, 8
@@ -719,6 +787,7 @@ EXPORTS = [
     "cro_probe_sparse", "cro_probe_sparse_uuid", "cro_sparse_expected", "cro_emit_sparse_annotations_json",
     "cro_scan_hbm", "cro_scan_hbm_uuid", "cro_read_hbm_health", "cro_emit_scan_annotations_json",
     "cro_probe_sram", "cro_probe_sram_uuid", "cro_read_sram_health", "cro_emit_sram_annotations_json",
+    "cro_probe_regfile", "cro_probe_regfile_uuid", "cro_emit_regfile_annotations_json", "cro_selftest_regfile_classify",
     "cro_probe_l2", "cro_probe_l2_uuid", "cro_read_l2_health", "cro_emit_l2_annotations_json", "cro_selftest_l2_classify",
     "cro_selftest_sm_legs_classify", "cro_selftest_sram_classify",
     "cro_selftest_locate_collect", "cro_selftest_scan_collect", "cro_selftest_link_classify",
@@ -877,6 +946,16 @@ def _load() -> ctypes.CDLL:
         "cro_probe_sram_uuid": (i32, [vp, c, ctypes.POINTER(SramOpts), ctypes.POINTER(SramResult), ctypes.POINTER(SramSm), i32,
                                       ctypes.POINTER(i32), ctypes.POINTER(SramFault), i32, ctypes.POINTER(i32)]),
         "cro_read_sram_health": (i32, [c, ctypes.POINTER(SramHealth)]),
+        "cro_probe_regfile": (i32, [vp, i32, ctypes.POINTER(RegfileOpts), ctypes.POINTER(RegfileResult), ctypes.POINTER(RegfileSm),
+                                    i32, ctypes.POINTER(i32), ctypes.POINTER(RegfileFault), i32, ctypes.POINTER(i32)]),
+        "cro_probe_regfile_uuid": (i32, [vp, c, ctypes.POINTER(RegfileOpts), ctypes.POINTER(RegfileResult),
+                                         ctypes.POINTER(RegfileSm), i32, ctypes.POINTER(i32), ctypes.POINTER(RegfileFault), i32,
+                                         ctypes.POINTER(i32)]),
+        "cro_emit_regfile_annotations_json": (i32, [ctypes.POINTER(RegfileResult)] + out),
+        "cro_selftest_regfile_classify": (i32, [u32, u64, u32, u64, u32, ctypes.POINTER(RegfileCta), u64,
+                                                ctypes.POINTER(RegfileFault), ctypes.POINTER(RegfileResult),
+                                                ctypes.POINTER(RegfileSm), i32, ctypes.POINTER(i32), ctypes.POINTER(RegfileFault),
+                                                i32, ctypes.POINTER(i32)]),
         "cro_emit_sram_annotations_json": (i32, [ctypes.POINTER(SramResult)] + out),
         "cro_probe_l2": (i32, [vp, i32, ctypes.POINTER(L2Opts), ctypes.POINTER(L2Result), ctypes.POINTER(L2Sm), i32,
                                ctypes.POINTER(i32), ctypes.POINTER(L2Fault), i32, ctypes.POINTER(i32)]),
@@ -1077,6 +1156,11 @@ def emit_sram_annotations_json(r: SramResult) -> str:
     return _text(lib.cro_emit_sram_annotations_json, ctypes.byref(r))
 
 
+def emit_regfile_annotations_json(r: RegfileResult) -> str:
+    """Additive cohdi.io/probe-regfile-* annotations of a register-file probe result (Go-marshalled map[string]string)."""
+    return _text(lib.cro_emit_regfile_annotations_json, ctypes.byref(r))
+
+
 def read_sram_health(uuid: str) -> SramHealth:
     """cro_read_sram_health: the GPU's volatile SRAM ECC counts and threshold flag from NVML (no context, no CUDA)."""
     h = SramHealth()
@@ -1186,6 +1270,23 @@ def selftest_sram_classify(iterations: int, n_words: int, seed: int, cluster: in
     return out
 
 
+def selftest_regfile_classify(iterations: int, seed: int, sm_count: int, call: int, rounds: List[List[RegfileCta]],
+                              claims: int, records: List[RegfileFault], cap: Optional[int] = None):
+    """cro_selftest_regfile_classify: the register-file probe's classification of call `call`: rounds, each a list of
+    sm_count RegfileCta, `claims` record claims and the first min(claims, REGFILE_RECORDS) records.  Returns (result, SM
+    entries, faults); the result's status may be OK, ERR_CHECKSUM or ERR_UNSUPPORTED.  cap defaults to every record."""
+    assert all(len(r) == sm_count for r in rounds) and len(records) == min(claims, REGFILE_RECORDS)
+    flat = [x for r in rounds for x in r]
+    ctas = (RegfileCta * max(1, len(flat)))(*flat)
+    recs = (RegfileFault * max(1, len(records)))(*records)
+    cap = len(records) if cap is None else cap
+    rc, out = _per_sm(lib.cro_selftest_regfile_classify, (iterations, seed, sm_count, call, len(rounds), ctas, claims, recs),
+                      RegfileResult, RegfileSm, REGFILE_MAX_SMS, RegfileFault, cap)
+    if rc not in (OK, ERR_CHECKSUM, ERR_UNSUPPORTED):
+        raise ProbeError(rc, "cro_selftest_regfile_classify")
+    return out
+
+
 def _word_checks(counters: List[LocateCounters], records, granules=None):
     """The flat arrays of the word-check hooks: counters, records[k] (the first min(claims, LOCATE_RECORDS) of each) in
     order, and granules[k] (each the same number of words) in order."""
@@ -1268,6 +1369,31 @@ def probe_sram_uuid(ctx: Optional["ProbeContext"], uuid: str, legs: int = SRAM_A
     handle = ctx.handle if ctx is not None else None
     rc, out = _per_sm(lib.cro_probe_sram_uuid, (handle, _b(uuid), ctypes.byref(o)), SramResult, SramSm, SRAM_MAX_SMS, SramFault,
                       cap)
+    if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
+        raise _helper_error(rc, handle)
+    return out
+
+
+def _regfile_opts(iterations: int, max_rounds: int, deadline_ms: int,
+                  inject: Optional[Tuple[int, int, int, int, int, int, int]]) -> RegfileOpts:
+    o = RegfileOpts()
+    o.iterations, o.max_rounds, o.deadline_ms = iterations, max_rounds, deadline_ms
+    if inject is not None:
+        (o.test_inject_sm, o.test_inject_warp, o.test_inject_lane, o.test_inject_slot, o.test_inject_element,
+         o.test_inject_iteration, o.test_inject_mask) = inject
+    return o
+
+
+def probe_regfile_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: int = 0, max_rounds: int = 0, deadline_ms: int = 0,
+                       inject: Optional[Tuple[int, int, int, int, int, int, int]] = None,
+                       cap: int = 256) -> Tuple[RegfileResult, List[RegfileSm], List[RegfileFault]]:
+    """cro_probe_regfile_uuid: the register-file probe of any GPU on the node, run by the helper process (ctx may be
+    None).  Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up to `cap`
+    records."""
+    o = _regfile_opts(iterations, max_rounds, deadline_ms, inject)
+    handle = ctx.handle if ctx is not None else None
+    rc, out = _per_sm(lib.cro_probe_regfile_uuid, (handle, _b(uuid), ctypes.byref(o)), RegfileResult, RegfileSm, REGFILE_MAX_SMS,
+                      RegfileFault, cap)
     if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
         raise _helper_error(rc, handle)
     return out
@@ -1811,6 +1937,20 @@ class ProbeContext:
         per SM seen and up to `cap` word records."""
         o = _sram_opts(legs, iterations, cluster, max_rounds, 0, inject)
         rc, out = _per_sm(lib.cro_probe_sram, (self.handle, dev, ctypes.byref(o)), SramResult, SramSm, SRAM_MAX_SMS, SramFault, cap)
+        self._check(rc, allow=(ERR_CHECKSUM, ERR_CUDA))
+        return out
+
+    def probe_regfile(self, dev: int = 0, iterations: int = 0, max_rounds: int = 0,
+                      inject: Optional[Tuple[int, int, int, int, int, int, int]] = None,
+                      cap: int = 256) -> Tuple[RegfileResult, List[RegfileSm], List[RegfileFault]]:
+        """cro_probe_regfile: every SM's registers hold REGFILE_SLOTS pattern words per thread, as 0 and as 1, across two
+        barriers, and every word is compared.  iterations = 0 / max_rounds = 0: the defaults.  inject = (sm, warp, lane,
+        slot, element, iteration, mask) is the test-only stand-in for a bad cell (sm, warp, lane, slot: -1 for every
+        one).  Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up to `cap`
+        slot records."""
+        o = _regfile_opts(iterations, max_rounds, 0, inject)
+        rc, out = _per_sm(lib.cro_probe_regfile, (self.handle, dev, ctypes.byref(o)), RegfileResult, RegfileSm, REGFILE_MAX_SMS,
+                          RegfileFault, cap)
         self._check(rc, allow=(ERR_CHECKSUM, ERR_CUDA))
         return out
 

@@ -83,6 +83,11 @@ static_assert(sizeof(cro_sram_result) == 568 && offsetof(cro_sram_result, bad_sm
                   offsetof(cro_sram_result, recorded) == 160 && offsetof(cro_sram_result, before) == 184 &&
                   offsetof(cro_sram_result, leg) == 232,
               "sram layout");
+static_assert(sizeof(cro_regfile_opts) == 40 && sizeof(cro_regfile_result) == 296 && offsetof(cro_regfile_result, bad_sm) == 88 &&
+                  offsetof(cro_regfile_result, mismatches) == 120 && offsetof(cro_regfile_result, fold_xor) == 200 &&
+                  offsetof(cro_regfile_result, before) == 248 && sizeof(cro_regfile_sm) == 56 && sizeof(cro_regfile_fault) == 32 &&
+                  sizeof(cro_regfile_cta) == 96 && offsetof(cro_regfile_cta, smid) == 80,
+              "regfile layout");
 static_assert(sizeof(cro_l2_opts) == 56 && sizeof(cro_l2_health) == 48 && sizeof(cro_l2_sm) == 128 && sizeof(cro_l2_fault) == 56 &&
                   sizeof(cro_l2_result) == 616 && offsetof(cro_l2_result, mismatches) == 80 &&
                   offsetof(cro_l2_result, bad_line) == 184 && offsetof(cro_l2_result, a1_bad) == 312 &&
@@ -510,6 +515,31 @@ int cro_read_sram_health(const char* gpu_uuid, cro_sram_health* out) try {
     if (!gpu_uuid || !out) return CRO_ERR_INVALID_ARG;
     identity::NvmlSramHealth(gpu_uuid, true, out);
     return CRO_OK;
+} CRO_API_CATCH
+int cro_probe_regfile(cro_ctx* ctx, int i, const cro_regfile_opts* opts, cro_regfile_result* out, cro_regfile_sm* sms,
+                      int sms_cap, int* n_sms, cro_regfile_fault* faults, int cap, int* n) try {
+    return listed(per_sm_call(ctx, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_regfile_opts& o, auto* seen, auto* found) {
+        return ctx_probe_regfile(ctx, i, o, out, seen, found);
+    }), out);
+} CRO_API_CATCH
+int cro_probe_regfile_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_regfile_opts* opts, cro_regfile_result* out,
+                           cro_regfile_sm* sms, int sms_cap, int* n_sms, cro_regfile_fault* faults, int cap, int* n) try {
+    return listed(per_sm_call(gpu_uuid, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_regfile_opts& o, auto* seen, auto* found) {
+        return ctx_probe_regfile_uuid(ctx, gpu_uuid, o, out, seen, found, cap);
+    }), out);
+} CRO_API_CATCH
+int cro_selftest_regfile_classify(uint32_t iterations, uint64_t seed, uint32_t sm_count, uint64_t call, uint32_t rounds,
+                                  const cro_regfile_cta* ctas, uint64_t claims, const cro_regfile_fault* records,
+                                  cro_regfile_result* out, cro_regfile_sm* sms, int sms_cap, int* n_sms, cro_regfile_fault* faults,
+                                  int cap, int* n) try {
+    if (iterations == 0 || iterations > CRO_REGFILE_MAX_ITERATIONS || sm_count == 0 || (rounds && !ctas) ||
+        (claims && !records) || !out || !n_sms || !n || sms_cap < 0 || cap < 0 || (sms_cap > 0 && !sms) || (cap > 0 && !faults))
+        return CRO_ERR_INVALID_ARG;
+    *n = *n_sms = 0;
+    std::vector<cro_regfile_sm> seen;
+    std::vector<cro_regfile_fault> found;
+    const int rc = classify_regfile(iterations, seed, sm_count, call, rounds, ctas, claims, records, out, &seen, &found);
+    return listed({rc, true, copy_capped(seen, sms, sms_cap, n_sms), copy_capped(found, faults, cap, n)}, out);
 } CRO_API_CATCH
 int cro_probe_l2(cro_ctx* ctx, int i, const cro_l2_opts* opts, cro_l2_result* out, cro_l2_sm* sms, int sms_cap, int* n_sms,
                  cro_l2_fault* faults, int cap, int* n) try {
@@ -1120,6 +1150,24 @@ static Annotations sram_annotations(const cro_sram_result& r) {
     return m;
 }
 
+static Annotations regfile_annotations(const cro_regfile_result& r) {
+    static const char* const kHealth[3] = {"corrected", "uncorrected", "threshold-exceeded"};
+    Annotations m;
+    const std::string p = "cohdi.io/probe-regfile-";
+    m[p + "verdict"] = r.status == CRO_OK                                                   ? "ok"
+                       : r.status == CRO_ERR_CHECKSUM && r.verdict == CRO_REGFILE_SM  ? "sm"
+                       : r.status == CRO_ERR_CHECKSUM && r.verdict == CRO_REGFILE_ALL ? "all"
+                       : r.status == CRO_ERR_CUDA ? cuda_error(r.cuda_error)
+                                                   : "error";
+    m[p + "sms"] = std::to_string(r.sms_covered) + "/" + std::to_string(r.sm_count);
+    if (r.bad_sms) m[p + "bad-sms"] = join(r.bad_sm, std::min<uint32_t>(r.bad_sms, 16));
+    m[p + "regs"] = std::to_string((uint64_t)r.slots * r.threads) + "/" + std::to_string(r.regs_per_sm);
+    m[p + "iterations"] = std::to_string(r.iterations);
+    put_list(m, p + "health", bit_names(r.health, kHealth, 3));
+    ecc_delta(m, p, r.before, r.after, CRO_SRAM_NVML_ECC_CORRECTED, CRO_SRAM_NVML_ECC_UNCORRECTED);
+    return m;
+}
+
 static Annotations l2_annotations(const cro_l2_result& r) {
     static const char* const kHealth[6] = {"sram-corrected", "sram-uncorrected", "l2-corrected", "l2-uncorrected",
                                            "threshold-exceeded", "l2-bucket"};
@@ -1251,6 +1299,11 @@ int cro_emit_scan_annotations_json(const cro_scan_report* r, char* buf, size_t c
 int cro_emit_sram_annotations_json(const cro_sram_result* r, char* buf, size_t cap, size_t* len) try {
     if (!r) return CRO_ERR_INVALID_ARG;
     return emit(sram_annotations(*r), buf, cap, len);
+} CRO_API_CATCH
+
+int cro_emit_regfile_annotations_json(const cro_regfile_result* r, char* buf, size_t cap, size_t* len) try {
+    if (!r) return CRO_ERR_INVALID_ARG;
+    return emit(regfile_annotations(*r), buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_l2_annotations_json(const cro_l2_result* r, char* buf, size_t cap, size_t* len) try {

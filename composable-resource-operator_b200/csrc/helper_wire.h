@@ -163,6 +163,24 @@ static const cro_wire_field cro_wire_l2_fields[] = {
 static const cro_wire cro_wire_l2 = {"l2-raw", 1, CRO_WIRE_FIELDS(cro_wire_l2_fields),
                                      CRO_WIRE_SM_FRAME(cro_l2_result, cro_l2_sm, cro_l2_fault, CRO_L2_MAX_SMS)};
 
+static const cro_wire_field cro_wire_regfile_fields[] = {
+    CRO_WIRE_FIELD(cro_regfile_opts, iterations),
+    CRO_WIRE_FIELD(cro_regfile_opts, max_rounds),
+    CRO_WIRE_FIELD(cro_regfile_opts, test_inject_sm),
+    CRO_WIRE_FIELD(cro_regfile_opts, test_inject_warp),
+    CRO_WIRE_FIELD(cro_regfile_opts, test_inject_lane),
+    CRO_WIRE_FIELD(cro_regfile_opts, test_inject_slot),
+    CRO_WIRE_FIELD(cro_regfile_opts, test_inject_element),
+    CRO_WIRE_FIELD(cro_regfile_opts, test_inject_iteration),
+    CRO_WIRE_FIELD(cro_regfile_opts, test_inject_mask),
+};
+/* The register-file frame: the result, then CRO_REGFILE_MAX_SMS cro_regfile_sm entries (sms_listed of them filled) and
+ * `recorded` cro_regfile_fault records. */
+static const cro_wire cro_wire_regfile = {"regfile-raw", 1, CRO_WIRE_FIELDS(cro_wire_regfile_fields),
+                                          {sizeof(cro_regfile_result), 0, sizeof(cro_regfile_sm), CRO_REGFILE_MAX_SMS,
+                                           sizeof(cro_regfile_fault), CRO_WIRE_AT(cro_regfile_result, sms_listed),
+                                           CRO_WIRE_AT(cro_regfile_result, recorded)}};
+
 /* health-raw: <uuid> <seed_base> <checks>, then each check's fields and cap in run order (the CRO_HEALTH_* bit order).
  * Its stdout: the cro_health_result, then the frame of each check that ran, in run order.  opts_at and result_at:
  * where the check's options and result are in cro_health_opts and cro_health_result. */

@@ -221,6 +221,25 @@ cudaError_t launch_sram_dsmem(const SramArgs& a, int grid, unsigned cluster, cud
 // Clusters of `cluster` CTAs the device can hold at once with the leg's shared memory (0: none fits).
 cudaError_t sram_max_clusters(unsigned cluster, unsigned n_words, int* clusters);
 
+// Register-file probe (cro_probe_regfile, regfile_kernels.cu): `grid` CTAs of CRO_REGFILE_THREADS, one per SM, each
+// holding CRO_REGFILE_SLOTS pattern words per thread in registers (include/croprobe.h).  Each CTA publishes one
+// cro_regfile_cta (stamp last = the call number) and records its mismatching slots while the record buffer has room
+// (*claims counts the slots claimed, possibly past the end).
+struct RegfileArgs {
+    cro_regfile_cta* cta;                       // grid entries
+    cro_regfile_fault* rec;                     // CRO_REGFILE_RECORDS entries
+    unsigned long long* claims;
+    unsigned long long seed, stamp;             // seed: iteration 0's; iteration i adds i * kNonceStride
+    unsigned iterations;
+    int inj_sm, inj_warp, inj_lane, inj_slot;   // -1: every SM / warp / lane / slot
+    unsigned inj_element, inj_iter;
+    unsigned inj_mask;                          // 0: nothing is injected in this launch
+};
+// Sets the kernel's dynamic shared memory (the source words) and carve-out; *fa gets its attributes (numRegs).
+// cudaErrorInvalidConfiguration when the device's opt-in shared memory per block cannot hold the source.
+cudaError_t regfile_plan(int device, cudaFuncAttributes* fa);
+cudaError_t launch_regfile(const RegfileArgs& a, int grid, cudaStream_t);
+
 // Pointer chase for NVLink latency: warp j of the one CTA follows `hops` dependent ld.relaxed.sys loads through
 // table[j] (one 8-byte slot per 128-byte line, peer-resident); out[2j] = final index, out[2j+1] = %globaltimer ns.
 struct ChaseArgs {

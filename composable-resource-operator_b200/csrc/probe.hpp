@@ -84,6 +84,7 @@ struct Device {
     uint64_t l2_calls = 0;                 // k of the next L2 probe call (ctx_probe_l2): its seeds
     uint64_t precision_calls = 0;          // k of the next precision probe call (ctx_probe_precision): its operand seed
     uint64_t sparse_calls = 0;             // k of the next sparse probe call (ctx_probe_sparse): its operand seed
+    uint64_t regfile_calls = 0;            // k of the next register-file probe call (ctx_probe_regfile): its seeds
     KernelPlan plan{};
     SweepScratch scratch{}, scratch_aux{}, scratch_pfx{};   // main stream / closed form / p2p prefix closed form
     // lane 0's buffers under their old names: the synchronous probe, the single sweeps and cro_probe_all use lane 0
@@ -384,6 +385,20 @@ int classify_sram(uint32_t legs, uint32_t iterations, uint32_t n_words, uint64_t
                   uint32_t net_grid, uint64_t k, const uint32_t* rounds, const cro_sram_cta* ctas, const uint64_t* claims,
                   const cro_sram_record* records, cro_sram_result* r, std::vector<cro_sram_sm>* sms,
                   std::vector<cro_sram_fault>* faults);
+
+// Register-file probe (include/croprobe.h, cro_probe_regfile / cro_probe_regfile_uuid, regfile_probe.cu): *sms gets one
+// entry per SM seen, by SM id; *faults every recorded slot, by (smid, iteration, element, warp, lane, slot).  The uuid
+// form runs `croprobe-cli regfile-raw` with a fresh seed base and asks it for at most cap slots.
+std::string regfile_opts_error(const cro_regfile_opts& o);
+int ctx_probe_regfile(cro_ctx* c, int idx, const cro_regfile_opts& o, cro_regfile_result* r, std::vector<cro_regfile_sm>* sms,
+                      std::vector<cro_regfile_fault>* faults);
+int ctx_probe_regfile_uuid(cro_ctx* c, const char* uuid, const cro_regfile_opts& o, cro_regfile_result* r,
+                           std::vector<cro_regfile_sm>* sms, std::vector<cro_regfile_fault>* faults, int cap);
+// cro_selftest_regfile_classify: the probe's classification of the caller's rounds and records, as ctx_probe_regfile
+// makes it.
+int classify_regfile(uint32_t iterations, uint64_t seed, uint32_t sm_count, uint64_t k, uint32_t rounds,
+                     const cro_regfile_cta* ctas, uint64_t claims, const cro_regfile_fault* records, cro_regfile_result* r,
+                     std::vector<cro_regfile_sm>* sms, std::vector<cro_regfile_fault>* faults);
 
 // L2 probe (include/croprobe.h, cro_probe_l2, l2_probe.cu): *sms gets one entry per SM seen, by SM id; *faults every
 // recorded word, by (word, iteration, element, smid).

@@ -842,6 +842,67 @@ func (c *Context) ProbeSRAM(deviceID string) (SRAMResult, error) {
 	return sramResult(&res, faults[:], got), nil
 }
 
+// RegfileResult is the summary of cro_regfile_result an operator reads: whether
+// every SM's registers held the pattern written into them, which SMs did not,
+// and the SRAM ECC record from NVML.
+type RegfileResult struct {
+	Status      int32  // CRO_OK, CRO_ERR_CHECKSUM or CRO_ERR_CUDA
+	CudaError   int32  // cudaError_t of a failed launch (CRO_ERR_CUDA)
+	Verdict     uint32 // CRO_REGFILE_NONE / _SM / _ALL
+	Health      uint32 // CRO_SRAM_HEALTH_* bits; never change Status
+	SMCount     uint32
+	Covered     uint32
+	RegsHeld    uint32 // registers per SM that held a pattern word (K * T)
+	RegsPerSM   uint32
+	BadSMs      []uint32 // SMs that failed, ascending (at most 16)
+	Faults      []RegfileFault
+	Annotations string // Go-marshalled map[string]string of cohdi.io/probe-regfile-* keys
+}
+
+// RegfileFault is one failed compare (cro_regfile_fault).
+type RegfileFault struct {
+	Element, Iteration, SM, Warp, Lane, Slot, Expected, Actual uint32
+}
+
+// ProbeRegfileByUUID runs cro_probe_regfile_uuid with its defaults: the
+// register-file probe of any GPU on the node through the helper process
+// (INTEGRATION.md "The register-file probe").  A mismatch or a fault
+// (CRO_ERR_CUDA) is a result, not an error; found is false when the node does
+// not list the GPU.
+func (c *Context) ProbeRegfileByUUID(deviceID string) (r RegfileResult, found bool, err error) {
+	id := C.CString(deviceID)
+	defer C.free(unsafe.Pointer(id))
+	var res C.cro_regfile_result
+	sms := make([]C.cro_regfile_sm, C.CRO_REGFILE_MAX_SMS)
+	var faults [256]C.cro_regfile_fault
+	var nSMs, got C.int
+	rc := C.cro_probe_regfile_uuid(c.h, id, nil, &res, &sms[0], C.CRO_REGFILE_MAX_SMS, &nSMs, &faults[0], 256, &got)
+	if rc == C.CRO_ERR_NO_DEVICE {
+		return r, false, nil
+	}
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM && rc != C.CRO_ERR_CUDA {
+		return r, true, errorOf(c.h, rc)
+	}
+	r = RegfileResult{Status: int32(res.status), CudaError: int32(res.cuda_error), Verdict: uint32(res.verdict),
+		Health: uint32(res.health), SMCount: uint32(res.sm_count), Covered: uint32(res.sms_covered),
+		RegsHeld: uint32(res.slots) * uint32(res.threads), RegsPerSM: uint32(res.regs_per_sm)}
+	for i := 0; i < int(res.bad_sms) && i < 16; i++ {
+		r.BadSMs = append(r.BadSMs, uint32(res.bad_sm[i]))
+	}
+	for i := 0; i < int(got); i++ {
+		f := faults[i]
+		r.Faults = append(r.Faults, RegfileFault{uint32(f.element), uint32(f.iteration), uint32(f.smid), uint32(f.warp),
+			uint32(f.lane), uint32(f.slot), uint32(f.expected), uint32(f.actual)})
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_regfile_annotations_json(&res, buf, 4096, &ln) == C.CRO_OK {
+		r.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return r, true, nil
+}
+
 // L2Result is the summary of cro_l2_result an operator reads: whether the
 // L2-resident buffer held what each SM wrote when another SM read it back,
 // whether the L2 atomic units gave the right answers, which SMs, buffer offsets

@@ -1426,7 +1426,184 @@ int  cro_probe_sram_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_sram_opts
  * NULL argument. */
 int  cro_read_sram_health(const char *gpu_uuid, cro_sram_health *out);
 
-/* ---- L2: the L2 cache, the crossbar between the SMs and its slices, and the L2 atomic units ---- */
+/* ---- register file: every SM's 32-bit registers held as 0 and as 1 ---- */
+
+/*
+ * The register file is the largest SRAM on an SM: 65 536 32-bit registers (256 KiB) on an H100 SM.  The compute,
+ * precision and sparse probes hold each operand for a few instructions in whichever registers ptxas picked, so a weak
+ * or coupled register cell that holds no accumulator passes them all.  The register-file probe holds a known pattern
+ * in K = CRO_REGFILE_SLOTS registers of every thread of one CTA per SM and checks every word.
+ *
+ * Shape: one CTA of T = CRO_REGFILE_THREADS threads (8 warps, 2 per SM sub-partition) per SM, launched with
+ * __launch_bounds__(256, 1) at 255 registers per thread: at the sm_90 allocation granularity that is the SM's whole
+ * register file, so no other CTA shares the SM.  K * T = 57 344 of the 65 536 registers (87.5 %) hold pattern words;
+ * at most 255 / 256 are addressable at all (R255 is the zero register), and the rest hold the loop's own state.  K = 224
+ * is the largest multiple of 4 whose source words (4 * K * T = 224 KiB, one per thread and slot) fit the 227 KiB of
+ * shared memory a CTA can have.
+ *
+ * Pattern: iteration i of call k uses seed_i = seed + i * 0xD1B54A32D192ED03, seed = seed_dev + 2^56 + 4096 * k *
+ * 0xD1B54A32D192ED03, and P_i(t, s) = the low 32 bits of pattern_word(seed_i, t * K + s) for thread t and slot s.
+ * Each iteration runs two elements: E0 holds P_i and E1 holds ~P_i, so every held bit is 0 and 1 in every iteration.
+ * One element: the CTA writes the source words to shared memory; barrier; each thread loads its K words into K
+ * registers (fully unrolled 16-byte loads); barrier; the CTA overwrites the source with 0 and publishes the element's
+ * key; barrier; each thread reads the key and compares every slot with the word recomputed from it.  Nothing but the
+ * registers holds the loaded words across the two barriers (tests/test_regfile_abi.py checks the SASS).  Mismatches
+ * are counted exactly per element and recorded while there is room; the last iteration's E1 words are also folded
+ * (xor, sum, sum of v * (2s + 1), over the CTA) and the library compares each CTA's fold with the closed form.
+ *
+ * The verdict and marks follow the SRAM probe's local leg: CRO_REGFILE_ALL when every covered SM failed or a launched
+ * CTA did not publish.  It runs only when called: it takes the device's mutex, lets probes in flight finish first
+ * (their results stay collectable) and never touches the sweep region.  The NVML SRAM ECC record (cro_sram_health) is
+ * read before and after and never changes the status; NVML does not document whether register-file ECC errors count
+ * under its SRAM location.  Which physical register or SM unit a slot maps to is not known; smid is %smid, with the
+ * other probes' caveat.
+ *
+ * status: CRO_ERR_CHECKSUM on any mismatch, fold mismatch or CTA that did not publish; CRO_ERR_CUDA when a launch
+ * failed (cuda_error holds the cudaError_t).
+ */
+#define CRO_REGFILE_SLOTS          224     /* K: registers each thread holds                                  */
+#define CRO_REGFILE_THREADS        256     /* T: threads per CTA                                              */
+#define CRO_REGFILE_ELEMENTS       2       /* E0 (P), E1 (~P)                                                 */
+#define CRO_REGFILE_RECORDS        4096    /* slot records the device keeps; counts stay exact beyond          */
+#define CRO_REGFILE_MAX_SMS        256     /* SM ids the results hold; a larger %nsmid fails the call          */
+#define CRO_REGFILE_MAX_ITERATIONS 4096
+#define CRO_REGFILE_MAX_ROUNDS     64
+
+#define CRO_REGFILE_NONE           0u      /* nothing failed                                                  */
+#define CRO_REGFILE_SM             1u      /* a strict subset of the covered SMs failed                        */
+#define CRO_REGFILE_ALL            2u      /* every covered SM failed, or a launched CTA did not publish       */
+
+#define CRO_REGFILE_PERSISTENT     1u      /* cro_regfile_sm.mark: the last iteration's compare failed          */
+#define CRO_REGFILE_INTERMITTENT   2u      /* an earlier iteration failed, or only the fold did                 */
+
+typedef struct cro_regfile_opts {
+    uint32_t iterations;           /*   0  per CTA: 0 = the default (DESIGN.md), at most MAX_ITERATIONS           */
+    uint32_t max_rounds;           /*   4  launches while fewer than sm_count SMs took part: 0 = 4               */
+    int32_t  deadline_ms;          /*   8  cro_probe_regfile_uuid: the helper's deadline; 0 = CRO_HELPER_TIMEOUT_MS */
+    /* test only: with test_inject_mask != 0, the mask is XORed into the source word that thread (test_inject_warp,
+       test_inject_lane) of the CTA on SM test_inject_sm loads into slot test_inject_slot in element
+       test_inject_element (0 or 1) of iteration test_inject_iteration (-1: every SM, warp, lane or slot), after the
+       word is generated and before it is loaded.  A software stand-in for a bad cell: nothing is provoked in the
+       hardware, and the hold-and-compare code is the same with and without it. */
+    int32_t  test_inject_sm;       /*  12 */
+    int32_t  test_inject_warp;     /*  16 */
+    int32_t  test_inject_lane;     /*  20 */
+    int32_t  test_inject_slot;     /*  24 */
+    uint32_t test_inject_element;  /*  28 */
+    uint32_t test_inject_iteration;/*  32 */
+    uint32_t test_inject_mask;     /*  36 */
+} cro_regfile_opts;                /*  40 bytes */
+
+typedef struct cro_regfile_result {
+    int32_t  status;               /*   0  the return value                                                      */
+    uint32_t verdict;              /*   4  CRO_REGFILE_NONE / _SM / _ALL                                          */
+    uint64_t seed;                 /*   8  seed of this call (iteration i: seed + i * 0xD1B54A32D192ED03)         */
+    uint64_t call;                 /*  16  k: the call's number on this device, from 0                          */
+    uint32_t sm_count;             /*  24  multiprocessors the device reports                                    */
+    uint32_t nsmid;                /*  28  %nsmid as the kernel reads it                                         */
+    int32_t  cuda_error;           /*  32  cudaError_t of the launch that failed; 0: none                        */
+    uint32_t health;               /*  36  CRO_SRAM_HEALTH_* of before and after                                 */
+    uint32_t iterations;           /*  40  per CTA                                                               */
+    uint32_t rounds;               /*  44  launches                                                              */
+    uint32_t slots;                /*  48  K                                                                     */
+    uint32_t threads;              /*  52  T                                                                     */
+    uint32_t num_regs;             /*  56  registers per thread of the kernel (cudaFuncGetAttributes)             */
+    uint32_t regs_per_sm;          /*  60  32-bit registers per SM the device reports                            */
+    uint32_t sms_covered;          /*  64  distinct SMs that ran a CTA                                           */
+    uint32_t complete;             /*  68  1: sms_covered >= sm_count                                            */
+    uint32_t ctas;                 /*  72  CTAs launched, over all rounds                                        */
+    uint32_t unpublished;          /*  76  CTAs launched that published no record                               */
+    uint32_t failed_sms;           /*  80  distinct SMs with a mark                                              */
+    uint32_t bad_sms;              /*  84  = failed_sms                                                          */
+    uint16_t bad_sm[16];           /*  88  the first 16 of them, ascending                                      */
+    uint64_t mismatches[CRO_REGFILE_ELEMENTS];   /* 120  per element, exact                                      */
+    uint64_t fold_mismatches;      /* 136  CTAs whose fold differs from the closed form                         */
+    uint64_t recorded;             /* 144  slot records written to the caller's list (*n)                       */
+    uint32_t sms_listed;           /* 152  entries written to the caller's per-SM list                          */
+    uint32_t reserved;             /* 156 */
+    uint64_t bits_checked;         /* 160  held bits compared: 32 * K * T * 2 * iterations per CTA that published */
+    uint64_t ns;                   /* 168  CUDA events around the launches, summed over rounds                  */
+    uint64_t timer_ns;             /* 176  %globaltimer: first CTA start .. last CTA end, summed over rounds     */
+    uint64_t wall_ns;              /* 184  the whole call                                                       */
+    uint64_t helper_ns;            /* 192  cro_probe_regfile_uuid: spawn of the helper to its exit; 0 in process */
+    uint64_t fold_xor;             /* 200  fold of the CTA on the lowest SM id (the first such CTA to publish)   */
+    uint64_t fold_sum;             /* 208 */
+    uint64_t fold_wsum;            /* 216 */
+    uint64_t expect_xor;           /* 224  the closed form every CTA's fold must equal                          */
+    uint64_t expect_sum;           /* 232 */
+    uint64_t expect_wsum;          /* 240 */
+    cro_sram_health before;        /* 248  read before the first launch                                         */
+    cro_sram_health after;         /* 272  read after the last (with the threshold flag)                        */
+} cro_regfile_result;              /* 296 bytes */
+
+typedef struct cro_regfile_sm {
+    uint32_t smid;                 /*   0 */
+    uint32_t mark;                 /*   4  0, CRO_REGFILE_PERSISTENT or CRO_REGFILE_INTERMITTENT                 */
+    uint64_t mismatches[CRO_REGFILE_ELEMENTS];   /*   8  compares of this SM's CTAs that failed, per element       */
+    uint64_t fold_mismatches;      /*  24 */
+    uint64_t ns;                   /*  32  %globaltimer windows of this SM's CTAs, summed                       */
+    uint64_t cycles;               /*  40  %clock64 cycles of the same CTAs, summed                             */
+    uint32_t ctas;                 /*  48  CTAs that ran on this SM                                             */
+    uint32_t reserved;             /*  52 */
+} cro_regfile_sm;                  /*  56 bytes */
+
+typedef struct cro_regfile_fault {
+    uint32_t element;              /*   0  0 (P) or 1 (~P)                                                      */
+    uint32_t iteration;            /*   4 */
+    uint32_t smid;                 /*   8 */
+    uint32_t warp;                 /*  12  0 .. 7                                                               */
+    uint32_t lane;                 /*  16  0 .. 31                                                              */
+    uint32_t slot;                 /*  20  0 .. K - 1                                                           */
+    uint32_t expected;             /*  24 */
+    uint32_t actual;               /*  28 */
+} cro_regfile_fault;               /*  32 bytes */
+
+/* sms[0 .. sms_cap) receives one entry per SM seen, by SM id (*n_sms how many); faults[0 .. cap) the slot records
+ * sorted by (smid, iteration, element, warp, lane, slot) (*n how many).  opts may be NULL: defaults.
+ * cro_probe_regfile: dev_index is an in-process device.  cro_probe_regfile_uuid runs `croprobe-cli regfile-raw` (a
+ * fresh cuInit that sees only that GPU) with a fresh seed base, as the SRAM probe's uuid form does otherwise. */
+int  cro_probe_regfile(cro_ctx *ctx, int dev_index, const cro_regfile_opts *opts, cro_regfile_result *out,
+                       cro_regfile_sm *sms, int sms_cap, int *n_sms, cro_regfile_fault *faults, int cap, int *n);
+int  cro_probe_regfile_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_regfile_opts *opts, cro_regfile_result *out,
+                            cro_regfile_sm *sms, int sms_cap, int *n_sms, cro_regfile_fault *faults, int cap, int *n);
+
+/* What one CTA publishes at the end of a round. */
+typedef struct cro_regfile_cta {
+    uint64_t stamp;                /*   0  the call number k; any other value: the CTA did not publish            */
+    uint64_t t0, t1;               /*   8  %globaltimer around the iterations                                     */
+    uint64_t cycles;               /*  24  %clock64 around the iterations                                         */
+    uint64_t count[CRO_REGFILE_ELEMENTS];   /*  32  compares that failed, per element                           */
+    uint64_t last;                 /*  48  ... of them in the last iteration                                      */
+    uint64_t fold_x, fold_s, fold_w;        /*  56  the last iteration's E1 fold                                */
+    uint32_t smid;                 /*  80 */
+    uint32_t nsmid;                /*  84 */
+    uint32_t block;                /*  88  blockIdx.x                                                             */
+    uint32_t reserved;             /*  92 */
+} cro_regfile_cta;                 /*  96 bytes */
+
+/* Test hook: the probe's classification of call `call` (seed `seed`, `iterations` per CTA) on a device of sm_count
+ * SMs, from caller-given rounds instead of launches: `rounds` rounds of sm_count records of ctas, and `claims` record
+ * claims, of which the first min(claims, CRO_REGFILE_RECORDS) are in `records`.  The fold is checked against the
+ * library's own closed form.  Writes out, sms[0 .. sms_cap) and faults[0 .. cap) (*n_sms, *n, out->sms_listed,
+ * out->recorded) exactly as cro_probe_regfile does, all but what needs the device: ns, wall_ns, num_regs, regs_per_sm,
+ * health, before and after stay 0.  Returns out->status (CRO_ERR_UNSUPPORTED with a blanked result for a %nsmid above
+ * CRO_REGFILE_MAX_SMS), or CRO_ERR_INVALID_ARG for a NULL array it needs, a negative cap, sm_count 0 or iterations 0 or
+ * above CRO_REGFILE_MAX_ITERATIONS. */
+int  cro_selftest_regfile_classify(uint32_t iterations, uint64_t seed, uint32_t sm_count, uint64_t call, uint32_t rounds,
+                                   const cro_regfile_cta *ctas, uint64_t claims, const cro_regfile_fault *records,
+                                   cro_regfile_result *out, cro_regfile_sm *sms, int sms_cap, int *n_sms,
+                                   cro_regfile_fault *faults, int cap, int *n);
+
+/* Additive register-file annotations (cohdi.io/probe-regfile-*) of a cro_probe_regfile / cro_probe_regfile_uuid
+ * result, the same Go-marshalled map, integers and fixed spellings only: -verdict ("ok" for CRO_OK; "sm" or "all" for
+ * CRO_ERR_CHECKSUM with that verdict; "cuda-error:<cuda_error>" for CRO_ERR_CUDA; "error" otherwise), -sms
+ * ("<sms_covered>/<sm_count>"), -bad-sms (bad_sm[0 .. min(bad_sms, 16)), comma-separated; only when bad_sms > 0),
+ * -regs ("<slots * threads>/<regs_per_sm>"), -iterations, -health (the flags' names corrected, uncorrected,
+ * threshold-exceeded, comma-separated; only when any is set), and -ecc-corrected and -ecc-uncorrected (the deltas,
+ * after - before; only when both reads answered). */
+int  cro_emit_regfile_annotations_json(const cro_regfile_result *r, char *buf, size_t cap, size_t *len);
+
+/* ---- L2:the L2 cache, the crossbar between the SMs and its slices, and the L2 atomic units ---- */
 
 /*
  * The probe's sweeps stream through the L2 once under evict-first hints, and no kernel reads back on purpose what
