@@ -375,6 +375,43 @@ class SparseFault(ctypes.Structure):
                 ("expected", ctypes.c_int32), ("actual_bits", ctypes.c_uint32)]
 
 
+# SM warp-MMA probe (cro_probe_warpmma, cro_warpmma_expected); verdicts and marks are COMPUTE_*
+WARPMMA_LEG_S8, WARPMMA_LEG_F16, WARPMMA_LEG_BF16, WARPMMA_LEG_TF32, WARPMMA_LEG_F16ACC, WARPMMA_LEG_MOVE = range(6)
+WARPMMA_LEGS, WARPMMA_ALL_LEGS = 6, 0x3F
+WARPMMA_ANSWER_S8, WARPMMA_ANSWER_SMALL, WARPMMA_ANSWER_SMALL128, WARPMMA_ANSWER_NARROW, WARPMMA_ANSWER_MOVE = range(5)
+WARPMMA_ANSWERS = 5
+WARPMMA_M, WARPMMA_N, WARPMMA_K, WARPMMA_TF32_K = 128, 256, 256, 128
+WARPMMA_RECORDS, WARPMMA_MAX_SMS, WARPMMA_MAX_ITERATIONS, WARPMMA_MAX_ROUNDS = 4096, 256, 65536, 64
+
+
+class WarpMmaOpts(ctypes.Structure):
+    _fields_ = [("iterations", ctypes.c_uint32), ("legs", ctypes.c_uint32), ("max_rounds", ctypes.c_uint32),
+                ("test_inject_leg", ctypes.c_int32), ("test_inject_sm", ctypes.c_int32),
+                ("test_inject_iteration", ctypes.c_uint32), ("test_inject_row", ctypes.c_int32),
+                ("test_inject_col", ctypes.c_int32), ("test_inject_mask", ctypes.c_uint64), ("test_addr", ctypes.c_uint32),
+                ("test_addr_leg", ctypes.c_int32), ("test_addr_sm", ctypes.c_int32), ("test_addr_iteration", ctypes.c_uint32),
+                ("test_addr_row", ctypes.c_uint32), ("test_addr_kstep", ctypes.c_uint32)]
+
+
+class WarpMmaResult(ctypes.Structure):
+    """cro_warpmma_result: status, verdict and per-leg counts, coverage and times of one warp-MMA probe call."""
+    _fields_ = [("status", ctypes.c_int32), ("verdict", ctypes.c_uint32), ("seed", ctypes.c_uint64),
+                ("call", ctypes.c_uint64), ("sm_count", ctypes.c_uint32), ("legs", ctypes.c_uint32),
+                ("host_ref_ns", ctypes.c_uint64), ("nsmid", ctypes.c_uint32), ("bad_sms", ctypes.c_uint32),
+                ("bad_sm", ctypes.c_uint16 * 16), ("leg", ComputeLeg * WARPMMA_LEGS)]
+
+
+class WarpMmaSm(ctypes.Structure):
+    """One SM seen by a warp-MMA probe call, with its counts, times and COMPUTE_PERSISTENT / _INTERMITTENT mark per leg."""
+    _fields_ = [("smid", ctypes.c_uint32), ("reserved", ctypes.c_uint32), ("leg", ComputeSmLeg * WARPMMA_LEGS)]
+
+
+class WarpMmaFault(ctypes.Structure):
+    """One wrong element of a last iteration's answer: leg, SM, row, column, the exact answer and the raw bits got."""
+    _fields_ = [("leg", ctypes.c_uint32), ("smid", ctypes.c_uint32), ("row", ctypes.c_uint32), ("col", ctypes.c_uint32),
+                ("expected", ctypes.c_int32), ("actual_bits", ctypes.c_uint32)]
+
+
 # whole-HBM scan (cro_scan_hbm, cro_scan_hbm_uuid, cro_read_hbm_health)
 SCAN_CHUNK_BYTES, SCAN_RESERVE_BYTES, SCAN_MAX_CHUNKS, SCAN_PASSES, SCAN_ELEMENTS = 2 << 30, 1 << 30, 128, 2, 4
 (SCAN_HEALTH_ECC_CORRECTED_DURING, SCAN_HEALTH_ECC_UNCORRECTED_DURING, SCAN_HEALTH_REMAP_PENDING,
@@ -657,7 +694,7 @@ class L2Fault(ctypes.Structure):
 
 # test hooks: the compute, precision and SRAM probes' classification of caller-given rounds
 # (cro_selftest_sm_legs_classify, cro_selftest_sram_classify)
-SM_LEGS_COMPUTE, SM_LEGS_PRECISION, SM_LEGS_SPARSE = 0, 1, 3
+SM_LEGS_COMPUTE, SM_LEGS_PRECISION, SM_LEGS_SPARSE, SM_LEGS_WARPMMA = 0, 1, 3, 4
 
 
 class SmCta(ctypes.Structure):
@@ -717,6 +754,8 @@ assert ctypes.sizeof(PrecisionResult) == 808 and ctypes.sizeof(PrecisionSm) == 2
     and ctypes.sizeof(PrecisionOpts) == 48, ctypes.sizeof(PrecisionResult)
 assert ctypes.sizeof(SparseResult) == 704 and ctypes.sizeof(SparseSm) == 248 and ctypes.sizeof(SparseFault) == 24 \
     and ctypes.sizeof(SparseOpts) == 64, ctypes.sizeof(SparseResult)
+assert ctypes.sizeof(WarpMmaResult) == 704 and ctypes.sizeof(WarpMmaSm) == 248 and ctypes.sizeof(WarpMmaFault) == 24 \
+    and ctypes.sizeof(WarpMmaOpts) == 64, ctypes.sizeof(WarpMmaResult)
 assert ctypes.sizeof(FaultReport) == 928 and ctypes.sizeof(LocatePass) == 120, ctypes.sizeof(FaultReport)
 assert ctypes.sizeof(LinkResult) == 984 and ctypes.sizeof(PciPath) == 272, ctypes.sizeof(LinkResult)
 assert ctypes.sizeof(ScanReport) == 12632 and ctypes.sizeof(ScanOpts) == 72, ctypes.sizeof(ScanReport)
@@ -785,6 +824,7 @@ EXPORTS = [
     "cro_probe_compute", "cro_probe_compute_uuid", "cro_compute_expected", "cro_emit_compute_annotations_json",
     "cro_probe_precision", "cro_probe_precision_uuid", "cro_precision_expected", "cro_emit_precision_annotations_json",
     "cro_probe_sparse", "cro_probe_sparse_uuid", "cro_sparse_expected", "cro_emit_sparse_annotations_json",
+    "cro_probe_warpmma", "cro_probe_warpmma_uuid", "cro_warpmma_expected", "cro_emit_warpmma_annotations_json",
     "cro_scan_hbm", "cro_scan_hbm_uuid", "cro_read_hbm_health", "cro_emit_scan_annotations_json",
     "cro_probe_sram", "cro_probe_sram_uuid", "cro_read_sram_health", "cro_emit_sram_annotations_json",
     "cro_probe_regfile", "cro_probe_regfile_uuid", "cro_emit_regfile_annotations_json", "cro_selftest_regfile_classify",
@@ -934,6 +974,14 @@ def _load() -> ctypes.CDLL:
                                         ctypes.POINTER(i32), ctypes.POINTER(u64)]),
         "cro_sparse_expected": (i32, [i32, u64, ctypes.POINTER(ctypes.c_int32)]),
         "cro_emit_sparse_annotations_json": (i32, [ctypes.POINTER(SparseResult)] + out),
+        "cro_probe_warpmma": (i32, [vp, i32, ctypes.POINTER(WarpMmaOpts), ctypes.POINTER(WarpMmaResult),
+                                    ctypes.POINTER(WarpMmaSm), i32, ctypes.POINTER(i32), ctypes.POINTER(WarpMmaFault), i32,
+                                    ctypes.POINTER(i32)]),
+        "cro_probe_warpmma_uuid": (i32, [vp, c, ctypes.POINTER(WarpMmaOpts), i32, ctypes.POINTER(WarpMmaResult),
+                                         ctypes.POINTER(WarpMmaSm), i32, ctypes.POINTER(i32), ctypes.POINTER(WarpMmaFault), i32,
+                                         ctypes.POINTER(i32), ctypes.POINTER(u64)]),
+        "cro_warpmma_expected": (i32, [i32, u64, ctypes.POINTER(ctypes.c_int32)]),
+        "cro_emit_warpmma_annotations_json": (i32, [ctypes.POINTER(WarpMmaResult)] + out),
         "cro_emit_precision_annotations_json": (i32, [ctypes.POINTER(PrecisionResult)] + out),
         "cro_scan_hbm": (i32, [vp, i32, ctypes.POINTER(ScanOpts), ctypes.POINTER(ScanReport), ctypes.POINTER(FaultWord), i32,
                                ctypes.POINTER(i32)]),
@@ -1132,6 +1180,11 @@ def emit_sparse_annotations_json(r: SparseResult) -> str:
     return _text(lib.cro_emit_sparse_annotations_json, ctypes.byref(r))
 
 
+def emit_warpmma_annotations_json(r: WarpMmaResult) -> str:
+    """Additive cohdi.io/probe-warpmma-* annotations of a probe_warpmma result (Go-marshalled map[string]string)."""
+    return _text(lib.cro_emit_warpmma_annotations_json, ctypes.byref(r))
+
+
 def emit_precision_annotations_json(r: PrecisionResult) -> str:
     """Additive cohdi.io/probe-precision-* annotations of a probe_precision result (Go-marshalled map[string]string)."""
     return _text(lib.cro_emit_precision_annotations_json, ctypes.byref(r))
@@ -1234,13 +1287,14 @@ def _legs_rounds(n_legs: int, legs: int, rounds, claims, records, cta, words: in
 
 def selftest_sm_legs_classify(probe: int, iterations: List[int], grid: int, call: int, rounds, claims: List[int],
                               records, legs: int = 0):
-    """cro_selftest_sm_legs_classify: the compute (SM_LEGS_COMPUTE), precision (SM_LEGS_PRECISION) or sparse
-    (SM_LEGS_SPARSE) probe's classification of call `call` on `grid` SMs.  Per leg l (every list is indexed by leg; legs
-    0: all): rounds[l] a list of (grid SmCta, the COMPUTE_MAX_SMS // 64 coverage words) per round, claims[l] and
-    records[l] (ComputeFault / PrecisionFault / SparseFault, the first min(claims[l], RECORDS)).  Returns (result, SM
-    entries, faults); the result's status may be OK, ERR_CHECKSUM or ERR_UNSUPPORTED."""
+    """cro_selftest_sm_legs_classify: the compute (SM_LEGS_COMPUTE), precision (SM_LEGS_PRECISION), sparse
+    (SM_LEGS_SPARSE) or warp-MMA (SM_LEGS_WARPMMA) probe's classification of call `call` on `grid` SMs.  Per leg l (every
+    list is indexed by leg; legs 0: all): rounds[l] a list of (grid SmCta, the COMPUTE_MAX_SMS // 64 coverage words) per
+    round, claims[l] and records[l] (ComputeFault / PrecisionFault / SparseFault / WarpMmaFault, the first min(claims[l],
+    RECORDS)).  Returns (result, SM entries, faults); the result's status may be OK, ERR_CHECKSUM or ERR_UNSUPPORTED."""
     n_legs, result, sm, fault = {SM_LEGS_COMPUTE: (COMPUTE_LEGS, ComputeResult, ComputeSm, ComputeFault),
-                                 SM_LEGS_SPARSE: (SPARSE_LEGS, SparseResult, SparseSm, SparseFault)}.get(
+                                 SM_LEGS_SPARSE: (SPARSE_LEGS, SparseResult, SparseSm, SparseFault),
+                                 SM_LEGS_WARPMMA: (WARPMMA_LEGS, WarpMmaResult, WarpMmaSm, WarpMmaFault)}.get(
         probe, (PRECISION_LEGS, PrecisionResult, PrecisionSm, PrecisionFault))
     ran = legs or (1 << n_legs) - 1
     nr, ctas, bits, cl, recs = _legs_rounds(n_legs, ran, rounds, claims, records, SmCta, COMPUTE_MAX_SMS // 64, fault)
@@ -1527,6 +1581,36 @@ def probe_sparse_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: int 
     return out + (ns.value,)
 
 
+def _warpmma_opts(iterations: int, legs: int, max_rounds: int, inject: Optional[Tuple[int, int, int, int, int, int]],
+                  addr: Optional[Tuple[int, int, int, int, int]]) -> WarpMmaOpts:
+    o = WarpMmaOpts()
+    o.iterations, o.legs, o.max_rounds = iterations, legs, max_rounds
+    if inject is not None:
+        (o.test_inject_leg, o.test_inject_sm, o.test_inject_iteration, o.test_inject_row, o.test_inject_col,
+         o.test_inject_mask) = inject
+    if addr is not None:
+        o.test_addr = 1
+        o.test_addr_leg, o.test_addr_sm, o.test_addr_iteration, o.test_addr_row, o.test_addr_kstep = addr
+    return o
+
+
+def probe_warpmma_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: int = 0, legs: int = WARPMMA_ALL_LEGS,
+                       max_rounds: int = 0, deadline_ms: int = 0, inject: Optional[Tuple[int, int, int, int, int, int]] = None,
+                       addr: Optional[Tuple[int, int, int, int, int]] = None,
+                       cap: int = 256) -> Tuple[WarpMmaResult, List[WarpMmaSm], List[WarpMmaFault], int]:
+    """cro_probe_warpmma_uuid: the warp-MMA probe of any GPU on the node, run by the helper process (ctx may be None).
+    Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen, up to `cap` element records
+    and the helper's spawn-to-exit time in ns."""
+    o = _warpmma_opts(iterations, legs, max_rounds, inject, addr)
+    ns = ctypes.c_uint64()
+    handle = ctx.handle if ctx is not None else None
+    rc, out = _per_sm(lib.cro_probe_warpmma_uuid, (handle, _b(uuid), ctypes.byref(o), deadline_ms), WarpMmaResult, WarpMmaSm,
+                      WARPMMA_MAX_SMS, WarpMmaFault, cap, (ctypes.byref(ns),))
+    if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
+        raise _helper_error(rc, handle)
+    return out + (ns.value,)
+
+
 def _scan_opts(max_bytes: int, reserve_bytes: int, seed: int, deadline_ms: int, chunk_bytes: int,
                force: Optional[Tuple[int, int, int, int]]) -> ScanOpts:
     o = ScanOpts()
@@ -1632,6 +1716,16 @@ def sparse_expected(answer: int, seed: int) -> List[int]:
     rc = lib.cro_sparse_expected(answer, seed, arr)
     if rc != OK:
         raise ProbeError(rc, "cro_sparse_expected")
+    return list(arr)
+
+
+def warpmma_expected(answer: int, seed: int) -> List[int]:
+    """cro_warpmma_expected: the WARPMMA_ANSWER_* answer tile of the operands of `seed`, WARPMMA_M x WARPMMA_N int32
+    values, row-major (host arithmetic, no GPU)."""
+    arr = (ctypes.c_int32 * (WARPMMA_M * WARPMMA_N))()
+    rc = lib.cro_warpmma_expected(answer, seed, arr)
+    if rc != OK:
+        raise ProbeError(rc, "cro_warpmma_expected")
     return list(arr)
 
 
@@ -1909,6 +2003,22 @@ class ProbeContext:
         o = _sparse_opts(iterations, legs, max_rounds, inject, meta)
         rc, out = _per_sm(lib.cro_probe_sparse, (self.handle, dev, ctypes.byref(o)), SparseResult, SparseSm, SPARSE_MAX_SMS,
                           SparseFault, cap)
+        self._check(rc, allow=(ERR_CHECKSUM,))
+        return out
+
+    def probe_warpmma(self, dev: int = 0, iterations: int = 0, legs: int = WARPMMA_ALL_LEGS, max_rounds: int = 0,
+                      inject: Optional[Tuple[int, int, int, int, int, int]] = None,
+                      addr: Optional[Tuple[int, int, int, int, int]] = None,
+                      cap: int = 256) -> Tuple[WarpMmaResult, List[WarpMmaSm], List[WarpMmaFault]]:
+        """cro_probe_warpmma: every SM computes its answer tiles with warp-synchronous mma.sync in s8, F16, BF16, TF32
+        and F16 accumulation from ldmatrix fragments, and moves a tile through ldmatrix, movmatrix and stmatrix, and
+        checks each value exactly.  iterations / max_rounds = 0: the defaults.  inject = (leg, sm, iteration, row, col,
+        mask) is the test-only accumulator XOR (sm, row, col: -1 for every one; mask at most the leg's value width);
+        addr = (leg, sm, iteration, row, kstep) the test-only fragment-address substitution (sm -1: every SM).  Returns
+        the result (its status is OK or ERR_CHECKSUM), one entry per SM seen and up to `cap` element records."""
+        o = _warpmma_opts(iterations, legs, max_rounds, inject, addr)
+        rc, out = _per_sm(lib.cro_probe_warpmma, (self.handle, dev, ctypes.byref(o)), WarpMmaResult, WarpMmaSm,
+                          WARPMMA_MAX_SMS, WarpMmaFault, cap)
         self._check(rc, allow=(ERR_CHECKSUM,))
         return out
 

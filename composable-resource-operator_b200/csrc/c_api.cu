@@ -69,6 +69,11 @@ static_assert(sizeof(cro_sparse_opts) == 64 && offsetof(cro_sparse_opts, test_in
                   offsetof(cro_sparse_result, leg) == 80 && sizeof(cro_sparse_sm) == 248 && sizeof(cro_sparse_fault) == 24 &&
                   offsetof(cro_sparse_fault, actual_bits) == 20,
               "sparse layout");
+static_assert(sizeof(cro_warpmma_opts) == 64 && offsetof(cro_warpmma_opts, test_inject_mask) == 32 &&
+                  offsetof(cro_warpmma_opts, test_addr_kstep) == 60 && sizeof(cro_warpmma_result) == 704 &&
+                  offsetof(cro_warpmma_result, leg) == 80 && sizeof(cro_warpmma_sm) == 248 && sizeof(cro_warpmma_fault) == 24 &&
+                  offsetof(cro_warpmma_fault, actual_bits) == 20,
+              "warpmma layout");
 
 static_assert(sizeof(cro_scan_opts) == 72 && sizeof(cro_hbm_health) == 56 && sizeof(cro_scan_pass) == 552 &&
                   sizeof(cro_scan_chunk) == 88, "scan layout");
@@ -471,6 +476,23 @@ int cro_probe_sparse_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_sparse_o
         return rc;
     }).rc;
 } CRO_API_CATCH
+int cro_probe_warpmma(cro_ctx* ctx, int i, const cro_warpmma_opts* opts, cro_warpmma_result* out, cro_warpmma_sm* sms,
+                      int sms_cap, int* n_sms, cro_warpmma_fault* faults, int cap, int* n) try {
+    return per_sm_call(ctx, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_warpmma_opts& o, auto* seen, auto* found) {
+        return ctx_probe_warpmma(ctx, i, o, out, seen, found);
+    }).rc;
+} CRO_API_CATCH
+int cro_probe_warpmma_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_warpmma_opts* opts, int deadline_ms,
+                           cro_warpmma_result* out, cro_warpmma_sm* sms, int sms_cap, int* n_sms, cro_warpmma_fault* faults,
+                           int cap, int* n, uint64_t* helper_ns) try {
+    return per_sm_call(gpu_uuid, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_warpmma_opts& o, auto* seen, auto* found) {
+        uint64_t ns = 0;
+        if (helper_ns) *helper_ns = 0;
+        const int rc = ctx_probe_warpmma_uuid(ctx, gpu_uuid, o, deadline_ms, out, seen, found, cap, &ns);
+        if (helper_ns) *helper_ns = ns;
+        return rc;
+    }).rc;
+} CRO_API_CATCH
 int cro_scan_hbm(cro_ctx* ctx, int i, const cro_scan_opts* opts, cro_scan_report* out, cro_fault_word* words, int cap, int* n) try {
     if (!ctx || !out || !n || cap < 0 || (cap > 0 && !words)) return CRO_ERR_INVALID_ARG;
     *n = 0;
@@ -567,15 +589,18 @@ int cro_selftest_sm_legs_classify(int probe, uint32_t legs, const uint32_t* iter
                                   const uint32_t* rounds, const cro_sm_cta* ctas, const uint64_t* sm_bits, const uint64_t* claims,
                                   const void* records, void* out, void* sms, int sms_cap, int* n_sms, void* faults, int cap,
                                   int* n) try {
-    const uint32_t n_legs = probe == CRO_SM_LEGS_COMPUTE  ? CRO_COMPUTE_LEGS
-                            : probe == CRO_SM_LEGS_SPARSE ? CRO_SPARSE_LEGS
-                                                          : CRO_PRECISION_LEGS;
-    const uint32_t max_records = probe == CRO_SM_LEGS_COMPUTE ? CRO_COMPUTE_RECORDS
-                                 : probe == CRO_SM_LEGS_SPARSE ? CRO_SPARSE_RECORDS
-                                                               : CRO_PRECISION_RECORDS;
+    const uint32_t n_legs = probe == CRO_SM_LEGS_COMPUTE   ? CRO_COMPUTE_LEGS
+                            : probe == CRO_SM_LEGS_SPARSE  ? CRO_SPARSE_LEGS
+                            : probe == CRO_SM_LEGS_WARPMMA ? CRO_WARPMMA_LEGS
+                                                           : CRO_PRECISION_LEGS;
+    const uint32_t max_records = probe == CRO_SM_LEGS_COMPUTE   ? CRO_COMPUTE_RECORDS
+                                 : probe == CRO_SM_LEGS_SPARSE  ? CRO_SPARSE_RECORDS
+                                 : probe == CRO_SM_LEGS_WARPMMA ? CRO_WARPMMA_RECORDS
+                                                                : CRO_PRECISION_RECORDS;
     const uint32_t all = (1u << n_legs) - 1;
     if (legs == 0) legs = all;
-    if ((probe != CRO_SM_LEGS_COMPUTE && probe != CRO_SM_LEGS_PRECISION && probe != CRO_SM_LEGS_SPARSE) || (legs & ~all) ||
+    if ((probe != CRO_SM_LEGS_COMPUTE && probe != CRO_SM_LEGS_PRECISION && probe != CRO_SM_LEGS_SPARSE &&
+         probe != CRO_SM_LEGS_WARPMMA) || (legs & ~all) ||
         !iterations || !rounds || !claims || grid == 0 || !out || !n_sms || !n || sms_cap < 0 || cap < 0 || (sms_cap > 0 && !sms) || (cap > 0 && !faults))
         return CRO_ERR_INVALID_ARG;
     uint64_t n_rounds = 0, n_records = 0;
@@ -605,6 +630,16 @@ int cro_selftest_sm_legs_classify(int probe, uint32_t legs, const uint32_t* iter
                                        &found);
         copy_capped(seen, static_cast<cro_sparse_sm*>(sms), sms_cap, n_sms);
         copy_capped(found, static_cast<cro_sparse_fault*>(faults), cap, n);
+        return rc;
+    }
+    if (probe == CRO_SM_LEGS_WARPMMA) {
+        std::vector<cro_warpmma_sm> seen;
+        std::vector<cro_warpmma_fault> found;
+        const int rc = classify_warpmma(legs, iterations, grid, call, rounds, ctas, sm_bits, claims,
+                                        static_cast<const cro_warpmma_fault*>(records), static_cast<cro_warpmma_result*>(out), &seen,
+                                        &found);
+        copy_capped(seen, static_cast<cro_warpmma_sm*>(sms), sms_cap, n_sms);
+        copy_capped(found, static_cast<cro_warpmma_fault*>(faults), cap, n);
         return rc;
     }
     std::vector<cro_precision_sm> seen;
@@ -780,6 +815,9 @@ int cro_precision_expected(int answer, uint64_t seed, int64_t* out) try {
 } CRO_API_CATCH
 int cro_sparse_expected(int answer, uint64_t seed, int32_t* out) try {
     return sparse::Expected(answer, seed, out);
+} CRO_API_CATCH
+int cro_warpmma_expected(int answer, uint64_t seed, int32_t* out) try {
+    return warpmma::Expected(answer, seed, out);
 } CRO_API_CATCH
 int cro_pci_link_path(const char* sys_root, const char* pci_bus_id, cro_pci_path* out) try {
     if (!pci_bus_id || !out) return CRO_ERR_INVALID_ARG;
@@ -995,8 +1033,8 @@ static void ecc_delta(Annotations& m, const std::string& p, const Health& B, con
 }
 static std::string cuda_error(int32_t e) { return "cuda-error:" + std::to_string(e); }
 
-// The compute, precision and sparse results all hold a cro_compute_leg per leg.  Their annotations differ only in the key
-// prefix p, the leg names and which legs report a rate under which key.
+// The compute, precision, sparse and warp-MMA results all hold a cro_compute_leg per leg.  Their annotations differ
+// only in the key prefix p, the leg names and which legs report a rate under which key.
 struct LegRate {
     int leg;
     const char* key;
@@ -1214,6 +1252,14 @@ static Annotations sparse_annotations(const cro_sparse_result& r) {
                                 {CRO_SPARSE_LEG_F16, "f16-gflops"}, {CRO_SPARSE_LEG_TF32, "tf32-gflops"}});
 }
 
+static Annotations warpmma_annotations(const cro_warpmma_result& r) {
+    static const char* const kLeg[CRO_WARPMMA_LEGS] = {"s8", "f16", "bf16", "tf32", "f16acc", "move"};
+    return sm_legs_annotations(r, "cohdi.io/probe-warpmma-", kLeg, CRO_WARPMMA_LEGS,
+                               {{CRO_WARPMMA_LEG_S8, "s8-gops"}, {CRO_WARPMMA_LEG_F16, "f16-gflops"},
+                                {CRO_WARPMMA_LEG_BF16, "bf16-gflops"}, {CRO_WARPMMA_LEG_TF32, "tf32-gflops"},
+                                {CRO_WARPMMA_LEG_F16ACC, "f16acc-gflops"}, {CRO_WARPMMA_LEG_MOVE, "move-gelems"}});
+}
+
 // The health check's annotations: each check that ran, its own keys unchanged, and the call's cohdi.io/probe-health-*.
 static Annotations health_annotations(const cro_health_result& r) {
     static const char* const kName[CRO_HEALTH_CHECKS] = {"compute", "precision", "sram", "l2", "link", "scan"};
@@ -1289,6 +1335,11 @@ int cro_emit_precision_annotations_json(const cro_precision_result* r, char* buf
 int cro_emit_sparse_annotations_json(const cro_sparse_result* r, char* buf, size_t cap, size_t* len) try {
     if (!r) return CRO_ERR_INVALID_ARG;
     return emit(sparse_annotations(*r), buf, cap, len);
+} CRO_API_CATCH
+
+int cro_emit_warpmma_annotations_json(const cro_warpmma_result* r, char* buf, size_t cap, size_t* len) try {
+    if (!r) return CRO_ERR_INVALID_ARG;
+    return emit(warpmma_annotations(*r), buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_scan_annotations_json(const cro_scan_report* r, char* buf, size_t cap, size_t* len) try {

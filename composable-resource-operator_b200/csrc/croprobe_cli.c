@@ -48,6 +48,13 @@
  *                                                    cro_sparse_result, uint64_t n_sms and n, CRO_SPARSE_MAX_SMS
  *                                                    cro_sparse_sm entries, then n cro_sparse_fault records (at most
  *                                                    cap) on stdout
+ *   croprobe-cli warpmma-raw <uuid> <seed_base> <iterations> <legs> <max_rounds> <inject_leg> <inject_sm>
+ *                            <inject_iteration> <inject_row> <inject_col> <inject_mask> <addr> <addr_leg> <addr_sm>
+ *                            <addr_iteration> <addr_row> <addr_kstep> <cap>
+ *                                                    the warp-MMA probe with every cro_warpmma_opts field, as
+ *                                                    compute-raw: cro_warpmma_result, uint64_t n_sms and n,
+ *                                                    CRO_WARPMMA_MAX_SMS cro_warpmma_sm entries, then n
+ *                                                    cro_warpmma_fault records (at most cap) on stdout
  *   croprobe-cli l2-raw <uuid> <seed_base> <bytes> <iterations> <a1_counters> <a2_counters> <inject_leg> <inject_sm>
  *                       <inject_element> <inject_iteration> <inject_word> <inject_mask> <cap>
  *                                                    the L2 probe with every cro_l2_opts field but the deadline, NVML on
@@ -68,9 +75,9 @@
  *                                                    the seed base), its sweep region L, NVML on; the cro_health_result,
  *                                                    then each check that ran, in run order, as its own -raw writes it
  *   croprobe-cli health <uuid|index>                 the health check with defaults; JSON annotations, exit 0 iff ok
- *   link-raw, compute-raw, precision-raw, sparse-raw, l2-raw, regfile-raw and health-raw take cro_opts.seed_base from
- *   argv (the device seed is seed_base | minor, as in process), so that the library can give every helper call fresh patterns
- *   and operands; their counts are the helper's own, because neither result says how many records follow.
+ *   link-raw, compute-raw, precision-raw, sparse-raw, warpmma-raw, l2-raw, regfile-raw and health-raw take
+ *   cro_opts.seed_base from argv (the device seed is seed_base | minor, as in process), so that the library can give
+ *   every helper call fresh patterns and operands; their counts are the helper's own, because neither result says how many records follow.
  * Exit 3: the device is not visible to this (fresh) process — the reference's found=false.  The raw commands exit 0
  * iff the probe's status is CRO_OK, 1 for any other status (the result on stdout says which), 64 for a wrong argument
  * count.
@@ -198,6 +205,18 @@ static int sparse_raw(cro_ctx *ctx, int idx, char **argv) {
     if (!faults) return 2;
     cro_probe_sparse(ctx, idx, &so, &sr, sms, CRO_SPARSE_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
     return put_frame(&cro_wire_sparse.frame, &sr, sms, (uint64_t)n_sms, faults, (uint64_t)got) ? 2 : end_frames(sr.status);
+}
+
+static int warpmma_raw(cro_ctx *ctx, int idx, char **argv) {
+    static cro_warpmma_opts wo;
+    const int cap = raw_opts(&cro_wire_warpmma, argv, &wo);
+    static cro_warpmma_result wr;
+    static cro_warpmma_sm sms[CRO_WARPMMA_MAX_SMS];
+    cro_warpmma_fault *faults = (cro_warpmma_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
+    int n_sms = 0, got = 0;
+    if (!faults) return 2;
+    cro_probe_warpmma(ctx, idx, &wo, &wr, sms, CRO_WARPMMA_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
+    return put_frame(&cro_wire_warpmma.frame, &wr, sms, (uint64_t)n_sms, faults, (uint64_t)got) ? 2 : end_frames(wr.status);
 }
 
 static int l2_raw(cro_ctx *ctx, int idx, char **argv) {
@@ -337,6 +356,7 @@ static const struct command {
     {NULL, &cro_wire_compute, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, compute_raw},
     {NULL, &cro_wire_precision, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, precision_raw},
     {NULL, &cro_wire_sparse, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, sparse_raw},
+    {NULL, &cro_wire_warpmma, CRO_F_LAZY_ALLOC | CRO_F_NO_NVML, 64, warpmma_raw},
     /* every check of one device: the link check's region (exactly L when it is given) and NVML for the scan's, SRAM's and
      * L2's health records and the link's replay counters */
     {"health-raw", NULL, CRO_F_LAZY_ALLOC, 256, health_raw},
@@ -352,7 +372,9 @@ int main(int argc, char **argv) {
                         "compute-raw <uuid> <seed_base> <iterations> <alu_iterations> <legs> <rounds> <leg> <sm> <iteration> <row> <col> "
                         "<mask> <cap> | precision-raw <uuid> <seed_base> <iterations> <alu_iterations> <legs> <rounds> <leg> <sm> <iteration> <row> "
                         "<col> <mask> <cap> | sparse-raw <uuid> <seed_base> <iterations> <legs> <rounds> <leg> <sm> <iteration> <row> <col> "
-                        "<mask> <meta> <meta_leg> <meta_sm> <meta_iteration> <meta_row> <meta_group> <cap> | l2-raw <uuid> <seed_base> <bytes> <iterations> <a1> <a2> <leg> <sm> <element> <iteration> <word> <mask> <cap> | "
+                        "<mask> <meta> <meta_leg> <meta_sm> <meta_iteration> <meta_row> <meta_group> <cap> | warpmma-raw <uuid> <seed_base> "
+                        "<iterations> <legs> <rounds> <leg> <sm> <iteration> <row> <col> <mask> <addr> <addr_leg> <addr_sm> <addr_iteration> "
+                        "<addr_row> <addr_kstep> <cap> | l2-raw <uuid> <seed_base> <bytes> <iterations> <a1> <a2> <leg> <sm> <element> <iteration> <word> <mask> <cap> | "
                         "regfile-raw <uuid> <seed_base> <iterations> <rounds> <sm> <warp> <lane> <slot> <element> <iteration> <mask> <cap> | "
                         "health-raw <uuid> <seed_base> <checks> <compute-raw, precision-raw, sram-raw, l2-raw, link-raw, scan-raw options "
                         "and caps> | health <uuid|index>\n");

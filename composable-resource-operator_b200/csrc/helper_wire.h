@@ -41,7 +41,7 @@ typedef struct cro_wire_frame {
     uint32_t n_sms_at, n_sms_width, n_at, n_width;
 } cro_wire_frame;
 
-/* The compute, precision, sparse and L2 frames: the counts n_sms and n follow the result. */
+/* The compute, precision, sparse, warp-MMA and L2 frames: the counts n_sms and n follow the result. */
 #define CRO_WIRE_SM_FRAME(R, S, F, MAX) {sizeof(R), 2, sizeof(S), MAX, sizeof(F), sizeof(R), 8, sizeof(R) + 8, 8}
 
 /* One -raw command: its name, whether argv[3] is cro_opts.seed_base (the device seed is seed_base | minor, as in
@@ -147,6 +147,27 @@ static const cro_wire_field cro_wire_sparse_fields[] = {
 static const cro_wire cro_wire_sparse = {
     "sparse-raw", 1, CRO_WIRE_FIELDS(cro_wire_sparse_fields),
     CRO_WIRE_SM_FRAME(cro_sparse_result, cro_sparse_sm, cro_sparse_fault, CRO_SPARSE_MAX_SMS)};
+
+static const cro_wire_field cro_wire_warpmma_fields[] = {
+    CRO_WIRE_FIELD(cro_warpmma_opts, iterations),
+    CRO_WIRE_FIELD(cro_warpmma_opts, legs),
+    CRO_WIRE_FIELD(cro_warpmma_opts, max_rounds),
+    CRO_WIRE_FIELD(cro_warpmma_opts, test_inject_leg),
+    CRO_WIRE_FIELD(cro_warpmma_opts, test_inject_sm),
+    CRO_WIRE_FIELD(cro_warpmma_opts, test_inject_iteration),
+    CRO_WIRE_FIELD(cro_warpmma_opts, test_inject_row),
+    CRO_WIRE_FIELD(cro_warpmma_opts, test_inject_col),
+    CRO_WIRE_FIELD(cro_warpmma_opts, test_inject_mask),
+    CRO_WIRE_FIELD(cro_warpmma_opts, test_addr),
+    CRO_WIRE_FIELD(cro_warpmma_opts, test_addr_leg),
+    CRO_WIRE_FIELD(cro_warpmma_opts, test_addr_sm),
+    CRO_WIRE_FIELD(cro_warpmma_opts, test_addr_iteration),
+    CRO_WIRE_FIELD(cro_warpmma_opts, test_addr_row),
+    CRO_WIRE_FIELD(cro_warpmma_opts, test_addr_kstep),
+};
+static const cro_wire cro_wire_warpmma = {
+    "warpmma-raw", 1, CRO_WIRE_FIELDS(cro_wire_warpmma_fields),
+    CRO_WIRE_SM_FRAME(cro_warpmma_result, cro_warpmma_sm, cro_warpmma_fault, CRO_WARPMMA_MAX_SMS)};
 
 static const cro_wire_field cro_wire_l2_fields[] = {
     CRO_WIRE_FIELD(cro_l2_opts, bytes),

@@ -85,6 +85,7 @@ struct Device {
     uint64_t precision_calls = 0;          // k of the next precision probe call (ctx_probe_precision): its operand seed
     uint64_t sparse_calls = 0;             // k of the next sparse probe call (ctx_probe_sparse): its operand seed
     uint64_t regfile_calls = 0;            // k of the next register-file probe call (ctx_probe_regfile): its seeds
+    uint64_t warpmma_calls = 0;            // k of the next warp-MMA probe call (ctx_probe_warpmma): its operand seed
     KernelPlan plan{};
     SweepScratch scratch{}, scratch_aux{}, scratch_pfx{};   // main stream / closed form / p2p prefix closed form
     // lane 0's buffers under their old names: the synchronous probe, the single sweeps and cro_probe_all use lane 0
@@ -281,9 +282,25 @@ namespace precision {
 // The answer tile of the operands of `seed` (include/croprobe.h): answer CRO_PRECISION_ANSWER_*, M x N int64 values,
 // row-major.  CRO_ERR_INVALID_ARG for another answer.
 int Expected(int answer, uint64_t seed, int64_t* out);
+// The sum over every element e of an answer's tile of canon(value in its legs' type) * (2e + 1) (mod 2^64).
+uint64_t TileFold(int answer, const int64_t* tile);
 }  // namespace precision
+// SM warp-MMA probe (include/croprobe.h, cro_probe_warpmma / cro_probe_warpmma_uuid, warpmma_probe.cu): as the compute
+// probe's two forms; the uuid form runs `croprobe-cli warpmma-raw`.
+int ctx_probe_warpmma(cro_ctx* c, int idx, const cro_warpmma_opts& o, cro_warpmma_result* r, std::vector<cro_warpmma_sm>* sms,
+                      std::vector<cro_warpmma_fault>* faults);
+int ctx_probe_warpmma_uuid(cro_ctx* c, const char* uuid, const cro_warpmma_opts& o, int deadline_ms, cro_warpmma_result* r,
+                           std::vector<cro_warpmma_sm>* sms, std::vector<cro_warpmma_fault>* faults, int cap, uint64_t* helper_ns);
+int classify_warpmma(uint32_t legs, const uint32_t* iterations, uint32_t grid, uint64_t k, const uint32_t* rounds,
+                     const cro_sm_cta* ctas, const uint64_t* sm_bits, const uint64_t* claims, const cro_warpmma_fault* records,
+                     cro_warpmma_result* r, std::vector<cro_warpmma_sm>* sms, std::vector<cro_warpmma_fault>* faults);
+namespace warpmma {
+// The answer tile of the operands of `seed` (include/croprobe.h): answer CRO_WARPMMA_ANSWER_*, M x N int32 values,
+// row-major.  CRO_ERR_INVALID_ARG for another answer.
+int Expected(int answer, uint64_t seed, int32_t* out);
+}  // namespace warpmma
 
-// The helper run behind the uuid forms of the host link, compute, precision, sparse, scan, SRAM and L2 probes and the
+// The helper run behind the uuid forms of the host link, compute, precision, sparse, warp-MMA, scan, SRAM and L2 probes and the
 // health check.  Bad options are refused by the caller first.  With a context, the node must list the GPU
 // (CRO_ERR_NO_DEVICE otherwise) and a GPU that is also an in-process device is held under its device guard while the
 // helper runs.  Then `croprobe-cli args...` runs as inventory::RunHelperRaw runs it ("<what> for <uuid> ..." in its

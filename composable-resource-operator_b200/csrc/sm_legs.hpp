@@ -1,8 +1,8 @@
 // sm_legs.hpp — the host side the per-SM arithmetic probes (the compute probe, compute_probe.cu, the precision probe,
-// precision_probe.cu, and the sparse probe, sparse_probe.cu) share: what one round's CTA records add to a leg and to
-// its SMs, the marks and the slowest SM of a finished leg, the call's verdict, and the in-process and helper forms of a
-// call.  Sm is cro_compute_sm, cro_precision_sm or cro_sparse_sm (smid and leg[], one cro_compute_sm_leg per leg); the
-// leg totals are a cro_compute_leg in all three.
+// precision_probe.cu, the sparse probe, sparse_probe.cu, and the warp-MMA probe, warpmma_probe.cu) share: what one
+// round's CTA records add to a leg and to its SMs, the marks and the slowest SM of a finished leg, the call's verdict,
+// and the in-process and helper forms of a call.  Sm is cro_compute_sm, cro_precision_sm, cro_sparse_sm or
+// cro_warpmma_sm (smid and leg[], one cro_compute_sm_leg per leg); the leg totals are a cro_compute_leg in all four.
 #pragma once
 #include <algorithm>
 #include <map>
@@ -152,8 +152,8 @@ int take_leg(cro_ctx* c, const char* who, const std::vector<ComputeCta>& hc, con
 // What a probe P gives the calls below:
 //   Opts, Result, Sm, Fault, Args    its option, result, per-SM, record and kernel argument types
 //   Tile                             the element type of its answer tiles (Args::expect points into them)
-//   kName                            "compute", "precision", "sparse": "<kName> probe" and "<kName> helper" in error
-//                                    texts
+//   kName                            "compute", "precision", "sparse", "warpmma": "<kName> probe" and "<kName> helper" in
+//                                    error texts
 //   kWire                            its helper command's argv and frame (helper_wire.h), croprobe-cli <kName>-raw
 //   kLegs, kAllLegs, kMaxSms, kRecords, kAnswers, kCalls (its call counter in Device), kSeeds (its seed space)
 //   kDefaultIterations, kDefaultRounds, kAluLeg[leg] (the leg runs alu_iterations; with any such leg, Opts has

@@ -635,6 +635,78 @@ func (c *Context) ProbeSparseByUUID(deviceID string) (r SparseResult, found bool
 	return r, true, nil
 }
 
+// WarpMMAResult is the summary of cro_warpmma_result an operator reads:
+// whether every SM computed the exact answer with warp-synchronous mma.sync in
+// s8, F16, BF16, TF32 and F16 accumulation from ldmatrix fragments, and moved
+// a tile through ldmatrix, movmatrix and stmatrix intact, and which SMs did not.
+type WarpMMAResult struct {
+	OK          bool
+	Verdict     uint32    // CRO_COMPUTE_NONE / _SM / _ALL
+	SMCount     uint32
+	Covered     [6]uint32 // SMs seen per CRO_WARPMMA_LEG_*
+	Mismatches  [6]uint64 // wrong elements of the last iteration, per leg
+	BadSMs      []uint32  // SMs that failed any leg, ascending
+	Faults      []WarpMMAFault
+	Annotations string // Go-marshalled map[string]string of cohdi.io/probe-warpmma-* keys
+}
+
+// WarpMMAFault is one wrong element (cro_warpmma_fault): the exact answer and
+// the value's raw bits (int32 for S8, f32 for F16 / BF16 / TF32, f16 for
+// F16ACC, the 16-bit word for MOVE).
+type WarpMMAFault struct {
+	Leg, SM, Row, Col uint32
+	Expected          int32
+	ActualBits        uint32
+}
+
+// ProbeWarpMMAByUUID runs cro_probe_warpmma_uuid with its defaults: the
+// warp-MMA probe of any GPU on the node through the helper process, the form
+// an operator calls next to the compute, precision and sparse probes, before a
+// freshly composed GPU goes to a tenant whose kernels drive the tensor cores
+// with mma.sync, such as FlashAttention-2 (INTEGRATION.md §2j).  A mismatch or
+// a failed launch (CRO_ERR_CUDA) is a result, not an error; found is false
+// when the node does not list the GPU.
+func (c *Context) ProbeWarpMMAByUUID(deviceID string) (r WarpMMAResult, found bool, err error) {
+	id := C.CString(deviceID)
+	defer C.free(unsafe.Pointer(id))
+	var res C.cro_warpmma_result
+	sms := make([]C.cro_warpmma_sm, C.CRO_WARPMMA_MAX_SMS)
+	var faults [256]C.cro_warpmma_fault
+	var nSMs, got C.int
+	rc := C.cro_probe_warpmma_uuid(c.h, id, nil, 0, &res, &sms[0], C.CRO_WARPMMA_MAX_SMS, &nSMs, &faults[0], 256, &got, nil)
+	if rc == C.CRO_ERR_NO_DEVICE {
+		return r, false, nil
+	}
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM && rc != C.CRO_ERR_CUDA {
+		return r, true, errorOf(c.h, rc)
+	}
+	r = WarpMMAResult{OK: res.status == C.CRO_OK, Verdict: uint32(res.verdict), SMCount: uint32(res.sm_count)}
+	for l := 0; l < int(C.CRO_WARPMMA_LEGS); l++ {
+		r.Covered[l] = uint32(res.leg[l].sms_covered)
+		r.Mismatches[l] = uint64(res.leg[l].mismatches)
+	}
+	for i := 0; i < int(nSMs); i++ {
+		for l := 0; l < int(C.CRO_WARPMMA_LEGS); l++ {
+			if sms[i].leg[l].mark != 0 {
+				r.BadSMs = append(r.BadSMs, uint32(sms[i].smid))
+				break
+			}
+		}
+	}
+	for i := 0; i < int(got); i++ {
+		f := faults[i]
+		r.Faults = append(r.Faults, WarpMMAFault{uint32(f.leg), uint32(f.smid), uint32(f.row), uint32(f.col),
+			int32(f.expected), uint32(f.actual_bits)})
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_warpmma_annotations_json(&res, buf, 4096, &ln) == C.CRO_OK {
+		r.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return r, true, nil
+}
+
 // ScanResult is the summary of cro_scan_report an operator reads: whether every
 // free byte of the GPU's memory held what was written, how much was covered,
 // and the memory's own health record from NVML.

@@ -1089,6 +1089,146 @@ int  cro_probe_sparse_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_sparse_
  * CRO_SPARSE_N int32 values, row-major.  Host arithmetic only; no context. */
 int  cro_sparse_expected(int answer, uint64_t seed, int32_t *out);
 
+/* ---- SM warp-MMA: every SM's mma.sync tensor-core path and its ldmatrix / stmatrix / movmatrix moves ---- */
+
+/*
+ * The compute, precision and sparse probes drive the tensor cores through wgmma, whose A and B come from shared memory
+ * through a descriptor.  Hopper also runs the warp-synchronous path Ampere-style code uses (CUTLASS 2.x kernels,
+ * FlashAttention-2, many int8 and weight-only GEMMs): mma.sync (HMMA, IMMA) with register operands, put there by
+ * ldmatrix (LDSM), and fragments moved by stmatrix (STSM) and movmatrix (MOVM).  A fault in register-sourced operand
+ * delivery, in the HMMA / IMMA issue path or in the transposing crossbar behind LDSM.T and STSM.T passes every wgmma
+ * check.  The warp-MMA probe runs that path on every SM, one leg per form, shaped like the precision probe (one CTA per
+ * SM, one launch per leg, the same verdicts, marks, coverage rounds, slowest-SM report and guarantees: the device's
+ * mutex, probes in flight finish first, the sweep region untouched).  It issues only forms that are native on sm_90a.
+ *
+ * Operands of call k on a device: seed = seed_dev + 2^55 + k * 0xD1B54A32D192ED03.  The arithmetic legs read the
+ * compute and precision probes' operands: with the leg's K, element
+ *   e = m * K + k                   for A[m][k]
+ *   e = M * K + k * N + n           for B[k][n]
+ * is byte (e mod 8) of pattern_word(seed, e / 8), read as
+ *   s8         (int8_t)byte                         S8: the compute probe's s8 answer (K = 256)
+ *   small-int  (byte & 7) - 4 in -4 .. 3            F16, BF16: the compute probe's small-int answer (K = 256)
+ *                                                   TF32: the precision probe's small-int answer at K = 128
+ *   narrow     (byte & 3) - 2 in -2 .. 1            F16ACC: the precision probe's narrow answer (K = 256)
+ * every partial sum exact in the leg's accumulator (the compute and precision probes' bounds).  The MOVE leg's source
+ * tile S is M x N 16-bit words, S[r][c] = halfword (e mod 4) of pattern_word(seed, e / 4), e = r * N + c (halfword h:
+ * bits 16h .. 16h + 15); its answer is S transposed in each 8 x 8 block: E[8a + i][8b + j] = S[8a + j][8b + i].
+ *
+ * Legs (M x N x K; every CTA has 256 threads and generates its operands into its shared memory, every row padded by
+ * 16 bytes; A is row-major, B is held as B^T [n][k] for S8 and TF32 and as B [k][n] for F16, BF16 and F16ACC):
+ *   S8      mma.sync m16n8k32 .s32.s8.s8 (IMMA.16832.S8.S8)     128 x 256 x 256   B^T by ldmatrix
+ *   F16     mma.sync m16n8k16 .f32.f16 (HMMA.16816.F32)         128 x 256 x 256   B by ldmatrix.trans
+ *   BF16    mma.sync m16n8k16 .f32.bf16 (HMMA.16816.F32.BF16)   128 x 256 x 256   B by ldmatrix.trans
+ *   TF32    mma.sync m16n8k8 .f32.tf32 (HMMA.1688.F32.TF32)     128 x 256 x 128   B^T by ldmatrix
+ *   F16ACC  mma.sync m16n8k16 .f16.f16 (HMMA.16816.F16)         128 x 256 x 256   B by ldmatrix.trans; f16 accumulators
+ *   MOVE    LDSM.16.M88.4, MOVM.16.MT88, STSM.16.MT88.4, LDSM.16.MT88.4, STSM.16.M88.4, LDSM.16.M88.4 on the tile
+ * Every operand reaches an mma.sync through ldmatrix (.x4 for A and B); an instruction reads 32 bytes of K of each row,
+ * the A ldmatrix.x4 of instruction i the 16-byte K segments ("k-steps") 2i and 2i + 1.  Warp w owns rows 16w .. 16w + 15
+ * of the answer.  Thread t holds 128 values (the f16 and MOVE legs two to a register); value j is the element
+ *   row = r0(t) + 8 * ((j / 2) % 2),   col = 8 * (j / 4) + 2 * (t % 4) + j % 2,   r0(t) = 16 * (t / 32) + (t % 32) / 4
+ * (the mma.sync accumulator fragment).  In each iteration the MOVE leg's warp w takes every 16 x 16 sub-tile of its
+ * band through ldmatrix.x4 from S, movmatrix.trans of each register, stmatrix.x4.trans into buffer T (T's blocks equal
+ * S's), ldmatrix.x4.trans from T, stmatrix.x4 into buffer U (each block transposed) and ldmatrix.x4 from U into the
+ * values it compares.
+ *
+ * Compare: S8 values must equal the expected int32; F16, BF16 and TF32 values must be IEEE-equal to it as an f32,
+ * F16ACC values as an f16; MOVE values must equal its 16 bits.  Fold: after every iteration the thread adds canon(v) *
+ * (2e + 1) (mod 2^64) over its values, canon(v) the value's bits (int32, f32, f16 or the raw 16; the f32 and f16 legs
+ * take -0 as 0), e = row * N + col; at the end it compares the running sum with iterations * the same sum over the
+ * expected values.
+ */
+#define CRO_WARPMMA_LEG_S8          0
+#define CRO_WARPMMA_LEG_F16         1
+#define CRO_WARPMMA_LEG_BF16        2
+#define CRO_WARPMMA_LEG_TF32        3
+#define CRO_WARPMMA_LEG_F16ACC      4
+#define CRO_WARPMMA_LEG_MOVE        5
+#define CRO_WARPMMA_LEGS            6
+#define CRO_WARPMMA_ALL_LEGS        0x3Fu   /* bit l: leg l */
+#define CRO_WARPMMA_ANSWER_S8       0       /* K = 256, s8: S8                          */
+#define CRO_WARPMMA_ANSWER_SMALL    1       /* K = 256, small-int: F16, BF16            */
+#define CRO_WARPMMA_ANSWER_SMALL128 2       /* K = 128, small-int: TF32                 */
+#define CRO_WARPMMA_ANSWER_NARROW   3       /* K = 256, narrow: F16ACC                  */
+#define CRO_WARPMMA_ANSWER_MOVE     4       /* the block-transposed 16-bit tile: MOVE   */
+#define CRO_WARPMMA_ANSWERS         5
+#define CRO_WARPMMA_M               128
+#define CRO_WARPMMA_N               256
+#define CRO_WARPMMA_K               256     /* K of S8, F16, BF16, F16ACC */
+#define CRO_WARPMMA_TF32_K          128     /* ... of TF32                */
+#define CRO_WARPMMA_RECORDS         4096    /* element records the device keeps per leg; counts stay exact beyond */
+#define CRO_WARPMMA_MAX_SMS         256
+#define CRO_WARPMMA_MAX_ITERATIONS  65536
+#define CRO_WARPMMA_MAX_ROUNDS      64
+/* verdicts: CRO_COMPUTE_NONE / _SM / _ALL; marks: CRO_COMPUTE_PERSISTENT / _INTERMITTENT */
+
+typedef struct cro_warpmma_opts {
+    uint32_t iterations;           /*   0  0 = the default, at most CRO_WARPMMA_MAX_ITERATIONS                   */
+    uint32_t legs;                 /*   4  CRO_WARPMMA_ALL_LEGS bits; 0 = all                                    */
+    uint32_t max_rounds;           /*   8  launches per leg while fewer than sm_count SMs were seen: 0 = 4       */
+    /* test only: as cro_precision_opts, the mask XORed into the value's own bits (32 for S8, F16, BF16 and TF32, 16
+       for F16ACC and MOVE; a wider mask is refused) after the iteration; in MOVE it goes into the register the
+       stmatrix.x4 into U stores, so the wrong word passes through STSM and LDSM before it is compared */
+    int32_t  test_inject_leg;      /*  12 */
+    int32_t  test_inject_sm;       /*  16 */
+    uint32_t test_inject_iteration;/*  20 */
+    int32_t  test_inject_row;      /*  24 */
+    int32_t  test_inject_col;      /*  28 */
+    uint64_t test_inject_mask;     /*  32  0: no accumulator injection                                           */
+    /* test only: a fragment-address substitution.  In iteration test_addr_iteration on SM test_addr_sm (-1: every
+       SM), leg test_addr_leg (S8 .. F16ACC), the lane that supplies row test_addr_row's address for the A ldmatrix of
+       k-step test_addr_kstep passes the address of row test_addr_row ^ 1 instead: only that row of the answer
+       changes, to D[R][n] + sum over k of that 16-byte segment of (A[R ^ 1][k] - A[R][k]) * B[k][n] */
+    uint32_t test_addr;            /*  40  0: none; 1: substitute                                                */
+    int32_t  test_addr_leg;        /*  44 */
+    int32_t  test_addr_sm;         /*  48 */
+    uint32_t test_addr_iteration;  /*  52 */
+    uint32_t test_addr_row;        /*  56  below CRO_WARPMMA_M                                                  */
+    uint32_t test_addr_kstep;      /*  60  below K * element bytes / 16 (16 for S8, 32 otherwise)                */
+} cro_warpmma_opts;                /*  64 bytes */
+
+typedef struct cro_warpmma_result {
+    int32_t  status;               /*   0  CRO_OK, or CRO_ERR_CHECKSUM on any mismatch or missing publish       */
+    uint32_t verdict;              /*   4  CRO_COMPUTE_NONE / _SM / _ALL                                        */
+    uint64_t seed;                 /*   8  operand seed of this call                                           */
+    uint64_t call;                 /*  16  k: the call's number on this device, from 0                         */
+    uint32_t sm_count;             /*  24 */
+    uint32_t legs;                 /*  28  legs run (CRO_WARPMMA_ALL_LEGS bits)                                 */
+    uint64_t host_ref_ns;          /*  32  host time to compute the five expected answers                       */
+    uint32_t nsmid;                /*  40 */
+    uint32_t bad_sms;              /*  44 */
+    uint16_t bad_sm[16];           /*  48 */
+    cro_compute_leg leg[CRO_WARPMMA_LEGS];   /*  80  ops: 2 * M * N * K * iterations per CTA; MOVE: M * N elements */
+} cro_warpmma_result;              /* 704 bytes */
+
+typedef struct cro_warpmma_sm {
+    uint32_t smid;                 /*   0 */
+    uint32_t reserved;             /*   4 */
+    cro_compute_sm_leg leg[CRO_WARPMMA_LEGS];   /* 8 */
+} cro_warpmma_sm;                  /* 248 bytes */
+
+typedef struct cro_warpmma_fault {
+    uint32_t leg;                  /*   0  CRO_WARPMMA_LEG_*                                                    */
+    uint32_t smid;                 /*   4 */
+    uint32_t row;                  /*   8 */
+    uint32_t col;                  /*  12 */
+    int32_t  expected;             /*  16  the exact answer (MOVE: the 16-bit word, 0 .. 65535)                 */
+    uint32_t actual_bits;          /*  20  the value's raw bits: int32 for S8, f32 for F16 / BF16 / TF32, f16
+                                              for F16ACC, the 16-bit word for MOVE (zero-extended)             */
+} cro_warpmma_fault;               /*  24 bytes */
+
+/* As cro_probe_compute: sms one entry per SM seen, faults sorted by (leg, smid, row, col). */
+int  cro_probe_warpmma(cro_ctx *ctx, int dev_index, const cro_warpmma_opts *opts, cro_warpmma_result *out,
+                       cro_warpmma_sm *sms, int sms_cap, int *n_sms, cro_warpmma_fault *faults, int cap, int *n);
+
+/* The same probe of any GPU on the node, run by `croprobe-cli warpmma-raw`; as cro_probe_compute_uuid. */
+int  cro_probe_warpmma_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_warpmma_opts *opts, int deadline_ms,
+                            cro_warpmma_result *out, cro_warpmma_sm *sms, int sms_cap, int *n_sms,
+                            cro_warpmma_fault *faults, int cap, int *n, uint64_t *helper_ns);
+
+/* The expected answer a call uploads: answer CRO_WARPMMA_ANSWER_* of the operands of `seed`, as CRO_WARPMMA_M *
+ * CRO_WARPMMA_N int32 values, row-major.  Host arithmetic only; no context. */
+int  cro_warpmma_expected(int answer, uint64_t seed, int32_t *out);
+
 /* ---- whole-HBM scan: every free byte of a GPU's memory, and its DRAM health record ---- */
 
 /*
@@ -1837,15 +1977,17 @@ typedef struct cro_sm_cta {
 #define CRO_SM_LEGS_COMPUTE       0   /* cro_selftest_sm_legs_classify: the compute probe   */
 #define CRO_SM_LEGS_PRECISION     1   /* ... the precision probe                           */
 #define CRO_SM_LEGS_SPARSE        3   /* ... the sparse probe (cro_sparse_* types); 2 names no probe and is refused */
+#define CRO_SM_LEGS_WARPMMA       4   /* ... the warp-MMA probe (cro_warpmma_* types)      */
 
 /* Test hook: the compute (probe CRO_SM_LEGS_COMPUTE: out a cro_compute_result, sms cro_compute_sm, records and faults
- * cro_compute_fault), precision (CRO_SM_LEGS_PRECISION: the cro_precision_* types) or sparse probe's
- * (CRO_SM_LEGS_SPARSE: the cro_sparse_* types) classification of call `call` on a device of `grid` SMs, from
- * caller-given rounds instead of launches.  legs: the legs that ran (0: all).  Per leg l of them: iterations[l] (>= 1)
- * per CTA, rounds[l] rounds, each of `grid` records of ctas and of the CRO_COMPUTE_MAX_SMS / 64 words of sm_bits (the
- * leg's coverage bitmap after that round), and claims[l] record claims, of which the first min(claims[l],
- * CRO_COMPUTE_RECORDS) are in `records`; ctas, sm_bits and records run in leg order.  Every array is indexed by leg
- * (CRO_COMPUTE_LEGS, CRO_PRECISION_LEGS or CRO_SPARSE_LEGS entries).  Writes out, sms[0 .. sms_cap) and
+ * cro_compute_fault), precision (CRO_SM_LEGS_PRECISION: the cro_precision_* types), sparse (CRO_SM_LEGS_SPARSE: the
+ * cro_sparse_* types) or warp-MMA probe's (CRO_SM_LEGS_WARPMMA: the cro_warpmma_* types) classification of call `call`
+ * on a device of `grid` SMs, from caller-given rounds instead of launches.  legs: the legs that ran (0: all).  Per leg
+ * l of them: iterations[l] (>= 1) per CTA, rounds[l] rounds, each of `grid` records of ctas and of the
+ * CRO_COMPUTE_MAX_SMS / 64 words of sm_bits (the leg's coverage bitmap after that round), and claims[l] record claims,
+ * of which the first min(claims[l], CRO_COMPUTE_RECORDS) are in `records`; ctas, sm_bits and records run in leg order.
+ * Every array is indexed by leg (CRO_COMPUTE_LEGS, CRO_PRECISION_LEGS, CRO_SPARSE_LEGS or CRO_WARPMMA_LEGS entries).
+ * Writes out, sms[0 .. sms_cap) and
  * faults[0 .. cap) (*n_sms, *n how many) exactly as the in-process call does, all but what needs the device: seed,
  * host_ref_ns, ns and expect_fold stay 0, and rounds is rounds[l].  Returns out->status (CRO_ERR_UNSUPPORTED with a
  * blanked result for a %nsmid above CRO_COMPUTE_MAX_SMS), or CRO_ERR_INVALID_ARG for a NULL array it needs, a negative
@@ -2093,6 +2235,12 @@ int  cro_emit_precision_annotations_json(const cro_precision_result *r, char *bu
  * -bf16-gflops, -f16-gflops, -tf32-gflops (dense-equivalent ops / ns, integer division; 0 when ns is 0) and
  * -slowest-sm. */
 int  cro_emit_sparse_annotations_json(const cro_sparse_result *r, char *buf, size_t cap, size_t *len);
+
+/* Additive warp-MMA annotations (cohdi.io/probe-warpmma-*) of a cro_probe_warpmma result, spelled as the compute
+ * probe's: -verdict, -sms, -bad-sms, -failed-legs (s8, f16, bf16, tf32, f16acc, move), -s8-gops, -f16-gflops,
+ * -bf16-gflops, -tf32-gflops, -f16acc-gflops, -move-gelems (MOVE: tile elements moved per ns; all: ops / ns, integer
+ * division; 0 when ns is 0) and -slowest-sm. */
+int  cro_emit_warpmma_annotations_json(const cro_warpmma_result *r, char *buf, size_t cap, size_t *len);
 
 /* Additive HBM scan annotations (cohdi.io/hbm-scan-*) of a cro_scan_hbm / cro_scan_hbm_uuid report, the same
  * Go-marshalled map, integers and fixed spellings only: -verdict ("ok" for CRO_OK, "corrupt" for CRO_ERR_CHECKSUM,
