@@ -617,6 +617,72 @@ assert ctypes.sizeof(RegfileOpts) == 40 and ctypes.sizeof(RegfileResult) == 296 
     and ctypes.sizeof(RegfileFault) == 32 and ctypes.sizeof(RegfileCta) == 96, ctypes.sizeof(RegfileResult)
 
 
+# cross-lane probe (cro_probe_xlane, cro_probe_xlane_uuid, cro_xlane_expected, cro_selftest_xlane_classify)
+XLANE_LEG_SHFL, XLANE_LEG_VOTE, XLANE_LEG_MATCH, XLANE_LEG_REDUX, XLANE_LEG_ATOMS = range(5)
+XLANE_LEGS, XLANE_ALL_LEGS, XLANE_THREADS, XLANE_WARPS, XLANE_THREAD_RECORDS = 5, 0x1F, 256, 8, 4
+XLANE_RECORDS, XLANE_MAX_SMS, XLANE_MAX_ITERATIONS, XLANE_MAX_ROUNDS = 4096, 256, 4096, 64
+XLANE_SHFL_OPS, XLANE_VOTE_OPS, XLANE_MATCH_OPS, XLANE_REDUX_OPS, XLANE_ATOMS_OPS, XLANE_MAX_OPS = 177, 384, 64, 1296, 60, 1296
+XLANE_OPS = [XLANE_SHFL_OPS, XLANE_VOTE_OPS, XLANE_MATCH_OPS, XLANE_REDUX_OPS, XLANE_ATOMS_OPS]
+XLANE_NONE, XLANE_SM, XLANE_ALL = 0, 1, 2
+XLANE_PERSISTENT, XLANE_INTERMITTENT = 1, 2
+
+
+class XlaneOpts(ctypes.Structure):
+    _fields_ = [("iterations", ctypes.c_uint32), ("legs", ctypes.c_uint32), ("max_rounds", ctypes.c_uint32),
+                ("deadline_ms", ctypes.c_int32), ("test_inject_leg", ctypes.c_int32), ("test_inject_sm", ctypes.c_int32),
+                ("test_inject_warp", ctypes.c_int32), ("test_inject_lane", ctypes.c_int32), ("test_inject_op", ctypes.c_uint32),
+                ("test_inject_iteration", ctypes.c_uint32), ("test_inject_mask", ctypes.c_uint64)]
+
+
+class XlaneResult(ctypes.Structure):
+    """cro_xlane_result: status, verdict, bad SMs, per-leg counts, ops checked, folds and closed forms, coverage and
+    times of one cross-lane probe call."""
+    _fields_ = [("status", ctypes.c_int32), ("verdict", ctypes.c_uint32), ("seed", ctypes.c_uint64), ("call", ctypes.c_uint64),
+                ("sm_count", ctypes.c_uint32), ("nsmid", ctypes.c_uint32), ("cuda_error", ctypes.c_int32), ("legs", ctypes.c_uint32),
+                ("iterations", ctypes.c_uint32), ("rounds", ctypes.c_uint32), ("sms_covered", ctypes.c_uint32),
+                ("complete", ctypes.c_uint32), ("ctas", ctypes.c_uint32), ("unpublished", ctypes.c_uint32),
+                ("threads_unpublished", ctypes.c_uint32), ("failed_sms", ctypes.c_uint32), ("bad_sms", ctypes.c_uint32),
+                ("failed_legs", ctypes.c_uint32), ("bad_sm", ctypes.c_uint16 * 16), ("recorded", ctypes.c_uint64),
+                ("sms_listed", ctypes.c_uint32), ("reserved", ctypes.c_uint32), ("mismatches", ctypes.c_uint64 * XLANE_LEGS),
+                ("ops_checked", ctypes.c_uint64 * XLANE_LEGS), ("fold_mismatches", ctypes.c_uint64 * XLANE_LEGS),
+                ("leg_ns", ctypes.c_uint64 * XLANE_LEGS), ("fold", (ctypes.c_uint64 * 3) * XLANE_LEGS),
+                ("expect", (ctypes.c_uint64 * 3) * XLANE_LEGS), ("ns", ctypes.c_uint64), ("timer_ns", ctypes.c_uint64),
+                ("wall_ns", ctypes.c_uint64), ("helper_ns", ctypes.c_uint64)]
+
+
+class XlaneSm(ctypes.Structure):
+    """One SM seen by a cross-lane probe call: its failed legs, per-leg counts, fold mismatches, times and
+    XLANE_PERSISTENT / _INTERMITTENT mark."""
+    _fields_ = [("smid", ctypes.c_uint32), ("mark", ctypes.c_uint32), ("failed_legs", ctypes.c_uint32), ("ctas", ctypes.c_uint32),
+                ("mismatches", ctypes.c_uint64 * XLANE_LEGS), ("fold_mismatches", ctypes.c_uint64), ("ns", ctypes.c_uint64),
+                ("cycles", ctypes.c_uint64)]
+
+
+class XlaneFault(ctypes.Structure):
+    """One failed compare: leg, op, iteration, SM, warp, lane, the source lane of a shuffle's expected value (peer),
+    expected and actual result."""
+    _fields_ = [("leg", ctypes.c_uint32), ("op", ctypes.c_uint32), ("iteration", ctypes.c_uint32), ("smid", ctypes.c_uint32),
+                ("warp", ctypes.c_uint32), ("lane", ctypes.c_uint32), ("peer", ctypes.c_uint32), ("reserved", ctypes.c_uint32),
+                ("expected", ctypes.c_uint64), ("actual", ctypes.c_uint64)]
+
+
+class XlaneThread(ctypes.Structure):
+    """cro_xlane_thread: what one thread of the cross-lane probe publishes at the end of a launch."""
+    _fields_ = [("stamp", ctypes.c_uint64), ("count", ctypes.c_uint64), ("last", ctypes.c_uint64), ("fold_x", ctypes.c_uint64),
+                ("fold_s", ctypes.c_uint64), ("fold_w", ctypes.c_uint64)]
+
+
+class XlaneCta(ctypes.Structure):
+    """cro_xlane_cta: what thread 0 of a CTA of the cross-lane probe publishes at the end of a launch."""
+    _fields_ = [("stamp", ctypes.c_uint64), ("t0", ctypes.c_uint64), ("t1", ctypes.c_uint64), ("cycles", ctypes.c_uint64),
+                ("smid", ctypes.c_uint32), ("nsmid", ctypes.c_uint32), ("block", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+assert ctypes.sizeof(XlaneOpts) == 48 and ctypes.sizeof(XlaneResult) == 560 and ctypes.sizeof(XlaneSm) == 80 \
+    and ctypes.sizeof(XlaneFault) == 48 and ctypes.sizeof(XlaneThread) == 48 and ctypes.sizeof(XlaneCta) == 48, \
+    ctypes.sizeof(XlaneResult)
+
+
 # L2 probe (cro_probe_l2, cro_read_l2_health, cro_selftest_l2_classify)
 L2_BLOCK_BYTES, L2_MIN_BYTES, L2_MAX_L2_MULTIPLE, L2_ELEMENTS, L2_RECORDS, L2_MAX_SMS = 16384, 1 << 20, 8, 6, 4096, 256
 L2_MAX_ITERATIONS, L2_MAX_A1_COUNTERS, L2_MAX_A2_COUNTERS, L2_MAX_LINES, L2_MAX_COUNTERS = 256, 1 << 20, 8192, 8, 8
@@ -828,6 +894,8 @@ EXPORTS = [
     "cro_scan_hbm", "cro_scan_hbm_uuid", "cro_read_hbm_health", "cro_emit_scan_annotations_json",
     "cro_probe_sram", "cro_probe_sram_uuid", "cro_read_sram_health", "cro_emit_sram_annotations_json",
     "cro_probe_regfile", "cro_probe_regfile_uuid", "cro_emit_regfile_annotations_json", "cro_selftest_regfile_classify",
+    "cro_probe_xlane", "cro_probe_xlane_uuid", "cro_xlane_expected", "cro_emit_xlane_annotations_json",
+    "cro_selftest_xlane_classify",
     "cro_probe_l2", "cro_probe_l2_uuid", "cro_read_l2_health", "cro_emit_l2_annotations_json", "cro_selftest_l2_classify",
     "cro_selftest_sm_legs_classify", "cro_selftest_sram_classify",
     "cro_selftest_locate_collect", "cro_selftest_scan_collect", "cro_selftest_link_classify",
@@ -1005,6 +1073,15 @@ def _load() -> ctypes.CDLL:
                                                 ctypes.POINTER(RegfileSm), i32, ctypes.POINTER(i32), ctypes.POINTER(RegfileFault),
                                                 i32, ctypes.POINTER(i32)]),
         "cro_emit_sram_annotations_json": (i32, [ctypes.POINTER(SramResult)] + out),
+        "cro_probe_xlane": (i32, [vp, i32, ctypes.POINTER(XlaneOpts), ctypes.POINTER(XlaneResult), ctypes.POINTER(XlaneSm),
+                                  i32, ctypes.POINTER(i32), ctypes.POINTER(XlaneFault), i32, ctypes.POINTER(i32)]),
+        "cro_probe_xlane_uuid": (i32, [vp, c, ctypes.POINTER(XlaneOpts), ctypes.POINTER(XlaneResult), ctypes.POINTER(XlaneSm),
+                                       i32, ctypes.POINTER(i32), ctypes.POINTER(XlaneFault), i32, ctypes.POINTER(i32)]),
+        "cro_xlane_expected": (i32, [i32, u64, u32, i32, ctypes.POINTER(u64)]),
+        "cro_emit_xlane_annotations_json": (i32, [ctypes.POINTER(XlaneResult)] + out),
+        "cro_selftest_xlane_classify": (i32, [u32, u32, u64, u32, u64, u32, ctypes.POINTER(XlaneCta), ctypes.POINTER(XlaneThread),
+                                              ctypes.POINTER(XlaneFault), ctypes.POINTER(XlaneResult), ctypes.POINTER(XlaneSm), i32,
+                                              ctypes.POINTER(i32), ctypes.POINTER(XlaneFault), i32, ctypes.POINTER(i32)]),
         "cro_probe_l2": (i32, [vp, i32, ctypes.POINTER(L2Opts), ctypes.POINTER(L2Result), ctypes.POINTER(L2Sm), i32,
                                ctypes.POINTER(i32), ctypes.POINTER(L2Fault), i32, ctypes.POINTER(i32)]),
         "cro_probe_l2_uuid": (i32, [vp, c, ctypes.POINTER(L2Opts), ctypes.POINTER(L2Result), ctypes.POINTER(L2Sm), i32,
@@ -1212,6 +1289,40 @@ def emit_sram_annotations_json(r: SramResult) -> str:
 def emit_regfile_annotations_json(r: RegfileResult) -> str:
     """Additive cohdi.io/probe-regfile-* annotations of a register-file probe result (Go-marshalled map[string]string)."""
     return _text(lib.cro_emit_regfile_annotations_json, ctypes.byref(r))
+
+
+def emit_xlane_annotations_json(r: XlaneResult) -> str:
+    """Additive cohdi.io/probe-xlane-* annotations of a cross-lane probe result (Go-marshalled map[string]string)."""
+    return _text(lib.cro_emit_xlane_annotations_json, ctypes.byref(r))
+
+
+def xlane_expected(leg: int, seed: int, iteration: int, warp: int) -> List[int]:
+    """cro_xlane_expected: every lane's expected result of every op of leg `leg` in iteration `iteration` of a call of
+    seed `seed`, for warp `warp`: a list indexed op * 32 + lane (host arithmetic, no GPU)."""
+    arr = (ctypes.c_uint64 * (XLANE_MAX_OPS * 32))()
+    rc = lib.cro_xlane_expected(leg, seed, iteration, warp, arr)
+    if rc != OK:
+        raise ProbeError(rc, "cro_xlane_expected")
+    return list(arr[:XLANE_OPS[leg] * 32])
+
+
+def selftest_xlane_classify(legs: int, iterations: int, seed: int, sm_count: int, call: int, rounds, cap: Optional[int] = None):
+    """cro_selftest_xlane_classify: the cross-lane probe's classification of call `call`.  rounds[leg index][round] =
+    (sm_count XlaneCta, sm_count * XLANE_THREADS XlaneThread, sm_count * XLANE_THREADS * XLANE_THREAD_RECORDS
+    XlaneFault), for each leg of `legs` in order, every leg the same number of rounds.  Returns (result, SM entries,
+    faults); the result's status may be OK, ERR_CHECKSUM or ERR_UNSUPPORTED.  cap defaults to XLANE_RECORDS."""
+    n_rounds = len(rounds[0]) if rounds else 0
+    assert all(len(r) == n_rounds for r in rounds)
+    flat = [rnd for leg in rounds for rnd in leg]
+    ctas = (XlaneCta * max(1, sm_count * len(flat)))(*[x for rnd in flat for x in rnd[0]])
+    thr = (XlaneThread * max(1, sm_count * XLANE_THREADS * len(flat)))(*[x for rnd in flat for x in rnd[1]])
+    recs = (XlaneFault * max(1, sm_count * XLANE_THREADS * XLANE_THREAD_RECORDS * len(flat)))(*[x for rnd in flat for x in rnd[2]])
+    cap = XLANE_RECORDS if cap is None else cap
+    rc, out = _per_sm(lib.cro_selftest_xlane_classify, (legs, iterations, seed, sm_count, call, n_rounds, ctas, thr, recs),
+                      XlaneResult, XlaneSm, XLANE_MAX_SMS, XlaneFault, cap)
+    if rc not in (OK, ERR_CHECKSUM, ERR_UNSUPPORTED):
+        raise ProbeError(rc, "cro_selftest_xlane_classify")
+    return out
 
 
 def read_sram_health(uuid: str) -> SramHealth:
@@ -1448,6 +1559,30 @@ def probe_regfile_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: int
     handle = ctx.handle if ctx is not None else None
     rc, out = _per_sm(lib.cro_probe_regfile_uuid, (handle, _b(uuid), ctypes.byref(o)), RegfileResult, RegfileSm, REGFILE_MAX_SMS,
                       RegfileFault, cap)
+    if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
+        raise _helper_error(rc, handle)
+    return out
+
+
+def _xlane_opts(iterations: int, legs: int, max_rounds: int, deadline_ms: int,
+                inject: Optional[Tuple[int, int, int, int, int, int, int]]) -> XlaneOpts:
+    o = XlaneOpts()
+    o.iterations, o.legs, o.max_rounds, o.deadline_ms = iterations, legs, max_rounds, deadline_ms
+    if inject is not None:
+        (o.test_inject_leg, o.test_inject_sm, o.test_inject_warp, o.test_inject_lane, o.test_inject_op, o.test_inject_iteration,
+         o.test_inject_mask) = inject
+    return o
+
+
+def probe_xlane_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: int = 0, legs: int = 0, max_rounds: int = 0,
+                     deadline_ms: int = 0, inject: Optional[Tuple[int, int, int, int, int, int, int]] = None,
+                     cap: int = 256) -> Tuple[XlaneResult, List[XlaneSm], List[XlaneFault]]:
+    """cro_probe_xlane_uuid: the cross-lane probe of any GPU on the node, run by the helper process (ctx may be None).
+    Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up to `cap` records."""
+    o = _xlane_opts(iterations, legs, max_rounds, deadline_ms, inject)
+    handle = ctx.handle if ctx is not None else None
+    rc, out = _per_sm(lib.cro_probe_xlane_uuid, (handle, _b(uuid), ctypes.byref(o)), XlaneResult, XlaneSm, XLANE_MAX_SMS,
+                      XlaneFault, cap)
     if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
         raise _helper_error(rc, handle)
     return out
@@ -2061,6 +2196,20 @@ class ProbeContext:
         o = _regfile_opts(iterations, max_rounds, 0, inject)
         rc, out = _per_sm(lib.cro_probe_regfile, (self.handle, dev, ctypes.byref(o)), RegfileResult, RegfileSm, REGFILE_MAX_SMS,
                           RegfileFault, cap)
+        self._check(rc, allow=(ERR_CHECKSUM, ERR_CUDA))
+        return out
+
+    def probe_xlane(self, dev: int = 0, iterations: int = 0, legs: int = 0, max_rounds: int = 0,
+                    inject: Optional[Tuple[int, int, int, int, int, int, int]] = None,
+                    cap: int = 256) -> Tuple[XlaneResult, List[XlaneSm], List[XlaneFault]]:
+        """cro_probe_xlane: every lane of every warp of one CTA per SM checks each shuffle, vote, match, warp-reduce and
+        shared-atomic form of the legs run (legs = 0: all) against an exact answer.  iterations / max_rounds = 0: the
+        defaults.  inject = (leg, sm, warp, lane, op, iteration, mask) is the test-only operand XOR (sm, warp, lane: -1
+        for every one).  Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up
+        to `cap` records."""
+        o = _xlane_opts(iterations, legs, max_rounds, 0, inject)
+        rc, out = _per_sm(lib.cro_probe_xlane, (self.handle, dev, ctypes.byref(o)), XlaneResult, XlaneSm, XLANE_MAX_SMS,
+                          XlaneFault, cap)
         self._check(rc, allow=(ERR_CHECKSUM, ERR_CUDA))
         return out
 

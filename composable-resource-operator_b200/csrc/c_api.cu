@@ -93,6 +93,12 @@ static_assert(sizeof(cro_regfile_opts) == 40 && sizeof(cro_regfile_result) == 29
                   offsetof(cro_regfile_result, before) == 248 && sizeof(cro_regfile_sm) == 56 && sizeof(cro_regfile_fault) == 32 &&
                   sizeof(cro_regfile_cta) == 96 && offsetof(cro_regfile_cta, smid) == 80,
               "regfile layout");
+static_assert(sizeof(cro_xlane_opts) == 48 && offsetof(cro_xlane_opts, test_inject_mask) == 40 && sizeof(cro_xlane_result) == 560 &&
+                  offsetof(cro_xlane_result, bad_sm) == 80 && offsetof(cro_xlane_result, mismatches) == 128 &&
+                  offsetof(cro_xlane_result, fold) == 288 && offsetof(cro_xlane_result, ns) == 528 && sizeof(cro_xlane_sm) == 80 &&
+                  sizeof(cro_xlane_fault) == 48 && offsetof(cro_xlane_fault, expected) == 32 && sizeof(cro_xlane_thread) == 48 &&
+                  sizeof(cro_xlane_cta) == 48 && offsetof(cro_xlane_cta, smid) == 32,
+              "xlane layout");
 static_assert(sizeof(cro_l2_opts) == 56 && sizeof(cro_l2_health) == 48 && sizeof(cro_l2_sm) == 128 && sizeof(cro_l2_fault) == 56 &&
                   sizeof(cro_l2_result) == 616 && offsetof(cro_l2_result, mismatches) == 80 &&
                   offsetof(cro_l2_result, bad_line) == 184 && offsetof(cro_l2_result, a1_bad) == 312 &&
@@ -561,6 +567,37 @@ int cro_selftest_regfile_classify(uint32_t iterations, uint64_t seed, uint32_t s
     std::vector<cro_regfile_sm> seen;
     std::vector<cro_regfile_fault> found;
     const int rc = classify_regfile(iterations, seed, sm_count, call, rounds, ctas, claims, records, out, &seen, &found);
+    return listed({rc, true, copy_capped(seen, sms, sms_cap, n_sms), copy_capped(found, faults, cap, n)}, out);
+} CRO_API_CATCH
+int cro_probe_xlane(cro_ctx* ctx, int i, const cro_xlane_opts* opts, cro_xlane_result* out, cro_xlane_sm* sms, int sms_cap,
+                    int* n_sms, cro_xlane_fault* faults, int cap, int* n) try {
+    return listed(per_sm_call(ctx, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_xlane_opts& o, auto* seen, auto* found) {
+        return ctx_probe_xlane(ctx, i, o, out, seen, found);
+    }), out);
+} CRO_API_CATCH
+int cro_probe_xlane_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_xlane_opts* opts, cro_xlane_result* out, cro_xlane_sm* sms,
+                         int sms_cap, int* n_sms, cro_xlane_fault* faults, int cap, int* n) try {
+    return listed(per_sm_call(gpu_uuid, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_xlane_opts& o, auto* seen, auto* found) {
+        return ctx_probe_xlane_uuid(ctx, gpu_uuid, o, out, seen, found, cap);
+    }), out);
+} CRO_API_CATCH
+int cro_xlane_expected(int leg, uint64_t seed, uint32_t iteration, int warp, uint64_t* out) try {
+    if (leg < 0 || leg >= CRO_XLANE_LEGS || warp < 0 || warp >= CRO_XLANE_WARPS || !out) return CRO_ERR_INVALID_ARG;
+    xlane_expected((unsigned)leg, seed, iteration, (unsigned)warp, out);
+    return CRO_OK;
+} CRO_API_CATCH
+int cro_selftest_xlane_classify(uint32_t legs, uint32_t iterations, uint64_t seed, uint32_t sm_count, uint64_t call, uint32_t rounds,
+                                const cro_xlane_cta* ctas, const cro_xlane_thread* threads, const cro_xlane_fault* records,
+                                cro_xlane_result* out, cro_xlane_sm* sms, int sms_cap, int* n_sms, cro_xlane_fault* faults, int cap,
+                                int* n) try {
+    if (legs == 0 || legs > CRO_XLANE_ALL_LEGS || iterations == 0 || iterations > CRO_XLANE_MAX_ITERATIONS || sm_count == 0 ||
+        (rounds && (!ctas || !threads || !records)) || !out || !n_sms || !n || sms_cap < 0 || cap < 0 || (sms_cap > 0 && !sms) ||
+        (cap > 0 && !faults))
+        return CRO_ERR_INVALID_ARG;
+    *n = *n_sms = 0;
+    std::vector<cro_xlane_sm> seen;
+    std::vector<cro_xlane_fault> found;
+    const int rc = classify_xlane(legs, iterations, seed, sm_count, call, rounds, ctas, threads, records, out, &seen, &found);
     return listed({rc, true, copy_capped(seen, sms, sms_cap, n_sms), copy_capped(found, faults, cap, n)}, out);
 } CRO_API_CATCH
 int cro_probe_l2(cro_ctx* ctx, int i, const cro_l2_opts* opts, cro_l2_result* out, cro_l2_sm* sms, int sms_cap, int* n_sms,
@@ -1206,6 +1243,22 @@ static Annotations regfile_annotations(const cro_regfile_result& r) {
     return m;
 }
 
+static Annotations xlane_annotations(const cro_xlane_result& r) {
+    static const char* const kLegs[CRO_XLANE_LEGS] = {"shfl", "vote", "match", "redux", "atoms"};
+    Annotations m;
+    const std::string p = "cohdi.io/probe-xlane-";
+    m[p + "verdict"] = r.status == CRO_OK                                                 ? "ok"
+                       : r.status == CRO_ERR_CHECKSUM && r.verdict == CRO_XLANE_SM  ? "sm"
+                       : r.status == CRO_ERR_CHECKSUM && r.verdict == CRO_XLANE_ALL ? "all"
+                       : r.status == CRO_ERR_CUDA ? cuda_error(r.cuda_error)
+                                                   : "error";
+    m[p + "sms"] = std::to_string(r.sms_covered) + "/" + std::to_string(r.sm_count);
+    if (r.bad_sms) m[p + "bad-sms"] = join(r.bad_sm, std::min<uint32_t>(r.bad_sms, 16));
+    put_list(m, p + "legs", bit_names(r.failed_legs, kLegs, CRO_XLANE_LEGS));
+    m[p + "iterations"] = std::to_string(r.iterations);
+    return m;
+}
+
 static Annotations l2_annotations(const cro_l2_result& r) {
     static const char* const kHealth[6] = {"sram-corrected", "sram-uncorrected", "l2-corrected", "l2-uncorrected",
                                            "threshold-exceeded", "l2-bucket"};
@@ -1355,6 +1408,11 @@ int cro_emit_sram_annotations_json(const cro_sram_result* r, char* buf, size_t c
 int cro_emit_regfile_annotations_json(const cro_regfile_result* r, char* buf, size_t cap, size_t* len) try {
     if (!r) return CRO_ERR_INVALID_ARG;
     return emit(regfile_annotations(*r), buf, cap, len);
+} CRO_API_CATCH
+
+int cro_emit_xlane_annotations_json(const cro_xlane_result* r, char* buf, size_t cap, size_t* len) try {
+    if (!r) return CRO_ERR_INVALID_ARG;
+    return emit(xlane_annotations(*r), buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_l2_annotations_json(const cro_l2_result* r, char* buf, size_t cap, size_t* len) try {

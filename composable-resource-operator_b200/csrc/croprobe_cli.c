@@ -68,6 +68,12 @@
  *                                                    CRO_REGFILE_MAX_SMS cro_regfile_sm entries (sms_listed of them
  *                                                    filled) and its `recorded` cro_regfile_fault records (at most cap)
  *                                                    on stdout
+ *   croprobe-cli xlane-raw <uuid> <seed_base> <iterations> <legs> <max_rounds> <inject_leg> <inject_sm> <inject_warp>
+ *                          <inject_lane> <inject_op> <inject_iteration> <inject_mask> <cap>
+ *                                                    the cross-lane probe with every cro_xlane_opts field but the
+ *                                                    deadline; cro_xlane_result, CRO_XLANE_MAX_SMS cro_xlane_sm entries
+ *                                                    (sms_listed of them filled) and its `recorded` cro_xlane_fault
+ *                                                    records (at most cap) on stdout
  *   croprobe-cli health-raw <uuid> <seed_base> <checks> <compute-raw's options and cap> <precision-raw's> <sram-raw's>
  *                           <l2-raw's> <link-raw's> <scan-raw's>
  *                                                    the health check (cro_check_health) with every option of every
@@ -75,7 +81,7 @@
  *                                                    the seed base), its sweep region L, NVML on; the cro_health_result,
  *                                                    then each check that ran, in run order, as its own -raw writes it
  *   croprobe-cli health <uuid|index>                 the health check with defaults; JSON annotations, exit 0 iff ok
- *   link-raw, compute-raw, precision-raw, sparse-raw, warpmma-raw, l2-raw, regfile-raw and health-raw take
+ *   link-raw, compute-raw, precision-raw, sparse-raw, warpmma-raw, l2-raw, regfile-raw, xlane-raw and health-raw take
  *   cro_opts.seed_base from argv (the device seed is seed_base | minor, as in process), so that the library can give
  *   every helper call fresh patterns and operands; their counts are the helper's own, because neither result says how many records follow.
  * Exit 3: the device is not visible to this (fresh) process — the reference's found=false.  The raw commands exit 0
@@ -243,6 +249,18 @@ static int regfile_raw(cro_ctx *ctx, int idx, char **argv) {
     return put_frame(&cro_wire_regfile.frame, &rr, sms, (uint64_t)n_sms, faults, (uint64_t)got) ? 2 : end_frames(rr.status);
 }
 
+static int xlane_raw(cro_ctx *ctx, int idx, char **argv) {
+    static cro_xlane_opts xo;
+    const int cap = raw_opts(&cro_wire_xlane, argv, &xo);
+    static cro_xlane_result xr;
+    static cro_xlane_sm sms[CRO_XLANE_MAX_SMS];
+    cro_xlane_fault *faults = (cro_xlane_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
+    int n_sms = 0, got = 0;
+    if (!faults) return 2;
+    cro_probe_xlane(ctx, idx, &xo, &xr, sms, CRO_XLANE_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
+    return put_frame(&cro_wire_xlane.frame, &xr, sms, (uint64_t)n_sms, faults, (uint64_t)got) ? 2 : end_frames(xr.status);
+}
+
 /* `scan`: the whole-HBM scan of the free memory (all of it but 1 GiB unless argv[3], in MiB, bounds it) as JSON. */
 static int scan_json(cro_ctx *ctx, int idx, char **argv) {
     cro_scan_opts so;
@@ -349,6 +367,7 @@ static const struct command {
     {NULL, &cro_wire_sram, CRO_F_LAZY_ALLOC, 64, sram_raw},
     {NULL, &cro_wire_l2, CRO_F_LAZY_ALLOC, 64, l2_raw},
     {NULL, &cro_wire_regfile, CRO_F_LAZY_ALLOC, 64, regfile_raw},
+    {NULL, &cro_wire_xlane, CRO_F_LAZY_ALLOC, 64, xlane_raw},
     /* a region of exactly L, the link's bytes (the probe checks L <= S; no halving on a full GPU), and NVML for the
      * replay counters */
     {NULL, &cro_wire_link, CRO_F_LAZY_ALLOC, 256, link_raw},
@@ -376,6 +395,7 @@ int main(int argc, char **argv) {
                         "<iterations> <legs> <rounds> <leg> <sm> <iteration> <row> <col> <mask> <addr> <addr_leg> <addr_sm> <addr_iteration> "
                         "<addr_row> <addr_kstep> <cap> | l2-raw <uuid> <seed_base> <bytes> <iterations> <a1> <a2> <leg> <sm> <element> <iteration> <word> <mask> <cap> | "
                         "regfile-raw <uuid> <seed_base> <iterations> <rounds> <sm> <warp> <lane> <slot> <element> <iteration> <mask> <cap> | "
+                        "xlane-raw <uuid> <seed_base> <iterations> <legs> <rounds> <leg> <sm> <warp> <lane> <op> <iteration> <mask> <cap> | "
                         "health-raw <uuid> <seed_base> <checks> <compute-raw, precision-raw, sram-raw, l2-raw, link-raw, scan-raw options "
                         "and caps> | health <uuid|index>\n");
         return 64;

@@ -202,6 +202,25 @@ static const cro_wire cro_wire_regfile = {"regfile-raw", 1, CRO_WIRE_FIELDS(cro_
                                            sizeof(cro_regfile_fault), CRO_WIRE_AT(cro_regfile_result, sms_listed),
                                            CRO_WIRE_AT(cro_regfile_result, recorded)}};
 
+static const cro_wire_field cro_wire_xlane_fields[] = {
+    CRO_WIRE_FIELD(cro_xlane_opts, iterations),
+    CRO_WIRE_FIELD(cro_xlane_opts, legs),
+    CRO_WIRE_FIELD(cro_xlane_opts, max_rounds),
+    CRO_WIRE_FIELD(cro_xlane_opts, test_inject_leg),
+    CRO_WIRE_FIELD(cro_xlane_opts, test_inject_sm),
+    CRO_WIRE_FIELD(cro_xlane_opts, test_inject_warp),
+    CRO_WIRE_FIELD(cro_xlane_opts, test_inject_lane),
+    CRO_WIRE_FIELD(cro_xlane_opts, test_inject_op),
+    CRO_WIRE_FIELD(cro_xlane_opts, test_inject_iteration),
+    CRO_WIRE_FIELD(cro_xlane_opts, test_inject_mask),
+};
+/* The cross-lane frame: the result, then CRO_XLANE_MAX_SMS cro_xlane_sm entries (sms_listed of them filled) and
+ * `recorded` cro_xlane_fault records. */
+static const cro_wire cro_wire_xlane = {"xlane-raw", 1, CRO_WIRE_FIELDS(cro_wire_xlane_fields),
+                                        {sizeof(cro_xlane_result), 0, sizeof(cro_xlane_sm), CRO_XLANE_MAX_SMS,
+                                         sizeof(cro_xlane_fault), CRO_WIRE_AT(cro_xlane_result, sms_listed),
+                                         CRO_WIRE_AT(cro_xlane_result, recorded)}};
+
 /* health-raw: <uuid> <seed_base> <checks>, then each check's fields and cap in run order (the CRO_HEALTH_* bit order).
  * Its stdout: the cro_health_result, then the frame of each check that ran, in run order.  opts_at and result_at:
  * where the check's options and result are in cro_health_opts and cro_health_result. */

@@ -86,6 +86,7 @@ struct Device {
     uint64_t sparse_calls = 0;             // k of the next sparse probe call (ctx_probe_sparse): its operand seed
     uint64_t regfile_calls = 0;            // k of the next register-file probe call (ctx_probe_regfile): its seeds
     uint64_t warpmma_calls = 0;            // k of the next warp-MMA probe call (ctx_probe_warpmma): its operand seed
+    uint64_t xlane_calls = 0;              // k of the next cross-lane probe call (ctx_probe_xlane): its seeds
     KernelPlan plan{};
     SweepScratch scratch{}, scratch_aux{}, scratch_pfx{};   // main stream / closed form / p2p prefix closed form
     // lane 0's buffers under their old names: the synchronous probe, the single sweeps and cro_probe_all use lane 0
@@ -416,6 +417,20 @@ int ctx_probe_regfile_uuid(cro_ctx* c, const char* uuid, const cro_regfile_opts&
 int classify_regfile(uint32_t iterations, uint64_t seed, uint32_t sm_count, uint64_t k, uint32_t rounds,
                      const cro_regfile_cta* ctas, uint64_t claims, const cro_regfile_fault* records, cro_regfile_result* r,
                      std::vector<cro_regfile_sm>* sms, std::vector<cro_regfile_fault>* faults);
+
+// Cross-lane probe (include/croprobe.h, cro_probe_xlane / cro_probe_xlane_uuid, xlane_probe.cu): *sms gets one entry
+// per SM seen, by SM id; *faults the records, by (leg, smid, iteration, op, warp, lane), at most CRO_XLANE_RECORDS.  The
+// uuid form runs `croprobe-cli xlane-raw` with a fresh seed base and asks it for at most cap records.
+std::string xlane_opts_error(const cro_xlane_opts& o);
+int ctx_probe_xlane(cro_ctx* c, int idx, const cro_xlane_opts& o, cro_xlane_result* r, std::vector<cro_xlane_sm>* sms,
+                    std::vector<cro_xlane_fault>* faults);
+int ctx_probe_xlane_uuid(cro_ctx* c, const char* uuid, const cro_xlane_opts& o, cro_xlane_result* r,
+                         std::vector<cro_xlane_sm>* sms, std::vector<cro_xlane_fault>* faults, int cap);
+// cro_xlane_expected and cro_selftest_xlane_classify.
+void xlane_expected(unsigned leg, uint64_t seed, uint32_t iteration, unsigned warp, uint64_t* out);
+int classify_xlane(uint32_t legs, uint32_t iterations, uint64_t seed, uint32_t sm_count, uint64_t k, uint32_t rounds,
+                   const cro_xlane_cta* ctas, const cro_xlane_thread* threads, const cro_xlane_fault* records,
+                   cro_xlane_result* r, std::vector<cro_xlane_sm>* sms, std::vector<cro_xlane_fault>* faults);
 
 // L2 probe (include/croprobe.h, cro_probe_l2, l2_probe.cu): *sms gets one entry per SM seen, by SM id; *faults every
 // recorded word, by (word, iteration, element, smid).

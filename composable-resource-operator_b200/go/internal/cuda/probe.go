@@ -975,6 +975,64 @@ func (c *Context) ProbeRegfileByUUID(deviceID string) (r RegfileResult, found bo
 	return r, true, nil
 }
 
+// XlaneResult is the summary of cro_xlane_result an operator reads: whether
+// every SM's shuffle, vote, match, warp-reduce and shared-atomic units gave the
+// right answer on every lane, and which SMs and legs did not.
+type XlaneResult struct {
+	Status      int32  // CRO_OK, CRO_ERR_CHECKSUM or CRO_ERR_CUDA
+	CudaError   int32  // cudaError_t of a failed launch (CRO_ERR_CUDA)
+	Verdict     uint32 // CRO_XLANE_NONE / _SM / _ALL
+	FailedLegs  uint32 // bit per CRO_XLANE_LEG_* that failed
+	SMCount     uint32
+	Covered     uint32
+	BadSMs      []uint32 // SMs that failed, ascending (at most 16)
+	Faults      []XlaneFault
+	Annotations string // Go-marshalled map[string]string of cohdi.io/probe-xlane-* keys
+}
+
+// XlaneFault is one failed compare (cro_xlane_fault).
+type XlaneFault struct {
+	Leg, Op, Iteration, SM, Warp, Lane, Peer uint32
+	Expected, Actual                         uint64
+}
+
+// ProbeXlaneByUUID runs cro_probe_xlane_uuid with its defaults: the cross-lane
+// probe of any GPU on the node through the helper process (INTEGRATION.md
+// "The cross-lane probe").  A mismatch or a fault (CRO_ERR_CUDA) is a result,
+// not an error; found is false when the node does not list the GPU.
+func (c *Context) ProbeXlaneByUUID(deviceID string) (r XlaneResult, found bool, err error) {
+	id := C.CString(deviceID)
+	defer C.free(unsafe.Pointer(id))
+	var res C.cro_xlane_result
+	sms := make([]C.cro_xlane_sm, C.CRO_XLANE_MAX_SMS)
+	var faults [256]C.cro_xlane_fault
+	var nSMs, got C.int
+	rc := C.cro_probe_xlane_uuid(c.h, id, nil, &res, &sms[0], C.CRO_XLANE_MAX_SMS, &nSMs, &faults[0], 256, &got)
+	if rc == C.CRO_ERR_NO_DEVICE {
+		return r, false, nil
+	}
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM && rc != C.CRO_ERR_CUDA {
+		return r, true, errorOf(c.h, rc)
+	}
+	r = XlaneResult{Status: int32(res.status), CudaError: int32(res.cuda_error), Verdict: uint32(res.verdict),
+		FailedLegs: uint32(res.failed_legs), SMCount: uint32(res.sm_count), Covered: uint32(res.sms_covered)}
+	for i := 0; i < int(res.bad_sms) && i < 16; i++ {
+		r.BadSMs = append(r.BadSMs, uint32(res.bad_sm[i]))
+	}
+	for i := 0; i < int(got); i++ {
+		f := faults[i]
+		r.Faults = append(r.Faults, XlaneFault{uint32(f.leg), uint32(f.op), uint32(f.iteration), uint32(f.smid), uint32(f.warp),
+			uint32(f.lane), uint32(f.peer), uint64(f.expected), uint64(f.actual)})
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_xlane_annotations_json(&res, buf, 4096, &ln) == C.CRO_OK {
+		r.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return r, true, nil
+}
+
 // L2Result is the summary of cro_l2_result an operator reads: whether the
 // L2-resident buffer held what each SM wrote when another SM read it back,
 // whether the L2 atomic units gave the right answers, which SMs, buffer offsets

@@ -1743,6 +1743,198 @@ int  cro_selftest_regfile_classify(uint32_t iterations, uint64_t seed, uint32_t 
  * after - before; only when both reads answered). */
 int  cro_emit_regfile_annotations_json(const cro_regfile_result *r, char *buf, size_t cap, size_t *len);
 
+/* ---- cross-lane: every SM's shuffle, vote, match, warp-reduce and shared-atomic units ---- */
+
+/*
+ * Every warp reduction, ballot and record claim runs through a few SM units that move data between the lanes of a
+ * warp (SHFL, VOTE, MATCH, REDUX) and the shared-memory atomic unit (ATOMS); the other probes' own tallies do too.  A
+ * shuffle that reads the wrong lane computes a wrong answer and raises nothing.  The cross-lane probe checks each
+ * instruction form on every lane of every warp of one CTA per SM against an exact answer.
+ *
+ * Shape: one CTA of CRO_XLANE_THREADS threads (8 warps) per SM, with a dynamic shared-memory request that keeps the SM
+ * to one CTA, and one launch per leg.  Iteration i of call k uses seed_i = seed + i * 0xD1B54A32D192ED03, seed =
+ * seed_dev + 2^54 + 4096 * k * 0xD1B54A32D192ED03.  Lane l of warp w takes its operands from pattern_word(seed_i,
+ * key(leg, op, w, l)), so no operand is warp-uniform; each thread computes its expected results from seed_i with
+ * plain integer arithmetic, recomputing its peers' operands rather than asking them.  cro_xlane_expected gives the
+ * same answers on the host; DESIGN.md "The cross-lane probe" lists each leg's ops:
+ *   SHFL   shfl.sync idx (source lane + r, r = 0..31), up and down (every delta at widths 32, 16, 8, 4, 2), bfly
+ *          (every lane mask); the value and the in-range predicate
+ *   VOTE   ballot, any, all, uni over rows 0, ~0, walking one, walking zero and seeded rows
+ *   MATCH  match.any / match.all in .b32 and .b64 over class maps of 1, 2, 3, 32 and seeded class counts
+ *   REDUX  redux.sync add.u32, add.s32, min/max .u32 / .s32, and, or, xor over walking-extreme and seeded rows
+ *   ATOMS  atom.shared add.u32, inc, dec, min/max .u32 / .s32, and, or, xor, exch.b32/.b64, cas.b32/.b64, add.u64,
+ *          each on one word per CTA, per warp, per lane index, and on 32 words of one bank; only results that do not
+ *          depend on the order the threads ran in are checked
+ * The report path uses none of these units: each thread counts its own mismatches, keeps its first
+ * CRO_XLANE_THREAD_RECORDS records in its own slots, folds the last iteration's results and publishes them with plain
+ * stores into its own cro_xlane_thread, stamped with the call number; thread 0 publishes the CTA's cro_xlane_cta.
+ * The host sums the entries, sorts the records and keeps the first CRO_XLANE_RECORDS; counts stay exact.
+ *
+ * Verdict and marks follow the register-file probe: CRO_XLANE_ALL when every covered SM failed, or a launched CTA or
+ * one of its threads did not publish.  The probe runs only when called, lets probes in flight finish first (their
+ * results stay collectable) and never touches the sweep region.  No NVML counter is documented for these units.
+ *
+ * status: CRO_ERR_CHECKSUM on any mismatch, fold mismatch or entry not published; CRO_ERR_CUDA when a launch failed.
+ */
+#define CRO_XLANE_LEG_SHFL         0
+#define CRO_XLANE_LEG_VOTE         1
+#define CRO_XLANE_LEG_MATCH        2
+#define CRO_XLANE_LEG_REDUX        3
+#define CRO_XLANE_LEG_ATOMS        4
+#define CRO_XLANE_LEGS             5
+#define CRO_XLANE_ALL_LEGS         0x1Fu
+#define CRO_XLANE_THREADS          256     /* threads per CTA: 8 warps                                       */
+#define CRO_XLANE_WARPS            8
+#define CRO_XLANE_THREAD_RECORDS   4       /* records each thread keeps                                      */
+#define CRO_XLANE_RECORDS          4096    /* records a result holds; counts stay exact beyond               */
+#define CRO_XLANE_MAX_SMS          256     /* SM ids the results hold; a larger %nsmid fails the call        */
+#define CRO_XLANE_MAX_ITERATIONS   4096
+#define CRO_XLANE_MAX_ROUNDS       64
+#define CRO_XLANE_SHFL_OPS         177     /* idx 32, up 57, down 57, bfly 31                                */
+#define CRO_XLANE_VOTE_OPS         384     /* 96 rows x (ballot, any, all, uni)                              */
+#define CRO_XLANE_MATCH_OPS        64      /* 16 class maps x (any.b32, all.b32, any.b64, all.b64)           */
+#define CRO_XLANE_REDUX_OPS        1296    /* 144 rows x 9 operations                                        */
+#define CRO_XLANE_ATOMS_OPS        60      /* 15 operations x 4 contention shapes                            */
+#define CRO_XLANE_MAX_OPS          1296
+
+#define CRO_XLANE_NONE             0u
+#define CRO_XLANE_SM               1u      /* a strict subset of the covered SMs failed                      */
+#define CRO_XLANE_ALL              2u      /* every covered SM failed, or an entry was not published          */
+
+#define CRO_XLANE_PERSISTENT       1u      /* cro_xlane_sm.mark: a compare of the last iteration failed       */
+#define CRO_XLANE_INTERMITTENT     2u      /* only an earlier iteration failed, or only the fold               */
+
+typedef struct cro_xlane_opts {
+    uint32_t iterations;           /*   0  per CTA and leg: 0 = the default (DESIGN.md), at most MAX_ITERATIONS   */
+    uint32_t legs;                 /*   4  bit per CRO_XLANE_LEG_*: 0 = all                                        */
+    uint32_t max_rounds;           /*   8  launches per leg while fewer than sm_count SMs took part: 0 = 4         */
+    int32_t  deadline_ms;          /*  12  cro_probe_xlane_uuid: the helper's deadline; 0 = CRO_HELPER_TIMEOUT_MS  */
+    /* test only: with test_inject_mask != 0, the mask is XORed into the operand of op test_inject_op of leg
+       test_inject_leg that thread (test_inject_warp, test_inject_lane) of the CTA on SM test_inject_sm gives in
+       iteration test_inject_iteration (-1: every SM, warp or lane), after it is generated and before the
+       instruction.  A software stand-in for a fault: the expected values still come from the key.  ATOMS inc and dec
+       (whose effect under a changed bound depends on the order the threads ran in) are refused. */
+    int32_t  test_inject_leg;      /*  16 */
+    int32_t  test_inject_sm;       /*  20 */
+    int32_t  test_inject_warp;     /*  24 */
+    int32_t  test_inject_lane;     /*  28 */
+    uint32_t test_inject_op;       /*  32 */
+    uint32_t test_inject_iteration;/*  36 */
+    uint64_t test_inject_mask;     /*  40 */
+} cro_xlane_opts;                  /*  48 bytes */
+
+typedef struct cro_xlane_result {
+    int32_t  status;               /*   0  the return value                                                      */
+    uint32_t verdict;              /*   4  CRO_XLANE_NONE / _SM / _ALL                                            */
+    uint64_t seed;                 /*   8  seed of this call (iteration i: seed + i * 0xD1B54A32D192ED03)         */
+    uint64_t call;                 /*  16  k: the call's number on this device, from 0                          */
+    uint32_t sm_count;             /*  24  multiprocessors the device reports                                    */
+    uint32_t nsmid;                /*  28  %nsmid as the kernel reads it                                         */
+    int32_t  cuda_error;           /*  32  cudaError_t of the launch that failed; 0: none                        */
+    uint32_t legs;                 /*  36  legs run                                                              */
+    uint32_t iterations;           /*  40  per CTA and leg                                                       */
+    uint32_t rounds;               /*  44  launches, over every leg                                              */
+    uint32_t sms_covered;          /*  48  distinct SMs that ran a CTA, in the leg run that saw the fewest        */
+    uint32_t complete;             /*  52  1: every leg covered sm_count SMs                                     */
+    uint32_t ctas;                 /*  56  CTAs launched                                                         */
+    uint32_t unpublished;          /*  60  CTAs launched that published no record                               */
+    uint32_t threads_unpublished;  /*  64  threads of published CTAs that published no entry                    */
+    uint32_t failed_sms;           /*  68  distinct SMs with a mark                                              */
+    uint32_t bad_sms;              /*  72  = failed_sms                                                          */
+    uint32_t failed_legs;          /*  76  bit per leg with a mismatch, fold mismatch or unpublished entry       */
+    uint16_t bad_sm[16];           /*  80  the first 16 failed SMs, ascending                                    */
+    uint64_t recorded;             /* 112  records written to the caller's list (*n)                            */
+    uint32_t sms_listed;           /* 120  entries written to the caller's per-SM list                          */
+    uint32_t reserved;             /* 124 */
+    uint64_t mismatches[CRO_XLANE_LEGS];       /* 128  compares that failed, per leg, exact                     */
+    uint64_t ops_checked[CRO_XLANE_LEGS];      /* 168  compares made: ops * 256 * iterations per published CTA  */
+    uint64_t fold_mismatches[CRO_XLANE_LEGS];  /* 208  CTAs whose fold differs from the closed form              */
+    uint64_t leg_ns[CRO_XLANE_LEGS];           /* 248  CUDA events around each leg's launches                    */
+    uint64_t fold[CRO_XLANE_LEGS][3];          /* 288  (xor, sum, weighted sum) of the lowest SM id's CTA         */
+    uint64_t expect[CRO_XLANE_LEGS][3];        /* 408  the closed form every CTA's fold must equal                */
+    uint64_t ns;                   /* 528  CUDA events around the launches, summed                              */
+    uint64_t timer_ns;             /* 536  %globaltimer: first CTA start .. last CTA end, summed over rounds     */
+    uint64_t wall_ns;              /* 544  the whole call                                                       */
+    uint64_t helper_ns;            /* 552  cro_probe_xlane_uuid: spawn of the helper to its exit; 0 in process  */
+} cro_xlane_result;                /* 560 bytes */
+
+typedef struct cro_xlane_sm {
+    uint32_t smid;                 /*   0 */
+    uint32_t mark;                 /*   4  0, CRO_XLANE_PERSISTENT or CRO_XLANE_INTERMITTENT                     */
+    uint32_t failed_legs;          /*   8  bit per leg that failed on this SM                                    */
+    uint32_t ctas;                 /*  12  CTAs that ran on this SM, over every leg                              */
+    uint64_t mismatches[CRO_XLANE_LEGS];   /*  16 */
+    uint64_t fold_mismatches;      /*  56 */
+    uint64_t ns;                   /*  64  %globaltimer windows of this SM's CTAs, summed                       */
+    uint64_t cycles;               /*  72  %clock64 cycles of the same CTAs, summed                             */
+} cro_xlane_sm;                    /*  80 bytes */
+
+typedef struct cro_xlane_fault {
+    uint32_t leg;                  /*   0  CRO_XLANE_LEG_*                                                       */
+    uint32_t op;                   /*   4  the op's index within its leg (DESIGN.md)                              */
+    uint32_t iteration;            /*   8 */
+    uint32_t smid;                 /*  12 */
+    uint32_t warp;                 /*  16 */
+    uint32_t lane;                 /*  20 */
+    uint32_t peer;                 /*  24  SHFL: the source lane of the expected value; other legs all ones     */
+    uint32_t reserved;             /*  28 */
+    uint64_t expected;             /*  32 */
+    uint64_t actual;               /*  40 */
+} cro_xlane_fault;                 /*  48 bytes */
+
+/* What one thread publishes at the end of a launch, with plain stores. */
+typedef struct cro_xlane_thread {
+    uint64_t stamp;                /*   0  the call number k; any other value: the thread did not publish         */
+    uint64_t count;                /*   8  compares that failed                                                   */
+    uint64_t last;                 /*  16  ... of them in the last iteration                                      */
+    uint64_t fold_x, fold_s, fold_w;   /*  24  the last iteration's results: xor, sum, sum of v * (2 op + 1)      */
+} cro_xlane_thread;                /*  48 bytes */
+
+/* What thread 0 of a CTA publishes at the end of a launch. */
+typedef struct cro_xlane_cta {
+    uint64_t stamp;                /*   0  the call number k; any other value: the CTA did not publish            */
+    uint64_t t0, t1;               /*   8  %globaltimer around the iterations                                     */
+    uint64_t cycles;               /*  24  %clock64 around the iterations                                         */
+    uint32_t smid;                 /*  32 */
+    uint32_t nsmid;                /*  36 */
+    uint32_t block;                /*  40  blockIdx.x                                                             */
+    uint32_t reserved;             /*  44 */
+} cro_xlane_cta;                   /*  48 bytes */
+
+/* sms[0 .. sms_cap) receives one entry per SM seen, by SM id (*n_sms how many); faults[0 .. cap) the records sorted
+ * by (leg, smid, iteration, op, warp, lane) (*n how many).  opts may be NULL: defaults.  cro_probe_xlane: dev_index is
+ * an in-process device.  cro_probe_xlane_uuid runs `croprobe-cli xlane-raw` (a fresh cuInit that sees only that GPU)
+ * with a fresh seed base. */
+int  cro_probe_xlane(cro_ctx *ctx, int dev_index, const cro_xlane_opts *opts, cro_xlane_result *out, cro_xlane_sm *sms,
+                     int sms_cap, int *n_sms, cro_xlane_fault *faults, int cap, int *n);
+int  cro_probe_xlane_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_xlane_opts *opts, cro_xlane_result *out,
+                          cro_xlane_sm *sms, int sms_cap, int *n_sms, cro_xlane_fault *faults, int cap, int *n);
+
+/* Every lane's expected result of every op of leg `leg` in iteration `iteration` of a call of seed `seed`, for warp
+ * `warp` (0 .. 7): out[op * 32 + lane], CRO_XLANE_*_OPS ops.  Host arithmetic, no GPU.  CRO_ERR_INVALID_ARG for a leg
+ * or warp out of range or a NULL out. */
+int  cro_xlane_expected(int leg, uint64_t seed, uint32_t iteration, int warp, uint64_t *out);
+
+/* Test hook: the probe's classification of call `call` (seed, iterations) on a device of sm_count SMs from
+ * caller-given launches instead of real ones.  For each leg of `legs` in order, `rounds` rounds, each of sm_count
+ * cro_xlane_cta (ctas), sm_count * CRO_XLANE_THREADS cro_xlane_thread (threads, by block then thread) and
+ * CRO_XLANE_THREAD_RECORDS records per thread (records; the first min(count, CRO_XLANE_THREAD_RECORDS) of each are
+ * read).  The folds are checked against the library's closed form.  Writes out, sms and faults as cro_probe_xlane
+ * does, all but what needs the device (ns, leg_ns, wall_ns stay 0).  Returns out->status (CRO_ERR_UNSUPPORTED with a
+ * blanked result for a %nsmid above CRO_XLANE_MAX_SMS), or CRO_ERR_INVALID_ARG for a NULL array it needs, a negative
+ * cap, sm_count 0, legs out of range, or iterations 0 or above CRO_XLANE_MAX_ITERATIONS. */
+int  cro_selftest_xlane_classify(uint32_t legs, uint32_t iterations, uint64_t seed, uint32_t sm_count, uint64_t call,
+                                 uint32_t rounds, const cro_xlane_cta *ctas, const cro_xlane_thread *threads,
+                                 const cro_xlane_fault *records, cro_xlane_result *out, cro_xlane_sm *sms, int sms_cap,
+                                 int *n_sms, cro_xlane_fault *faults, int cap, int *n);
+
+/* Additive cross-lane annotations (cohdi.io/probe-xlane-*) of a cro_probe_xlane / cro_probe_xlane_uuid result, the
+ * same Go-marshalled map: -verdict ("ok" for CRO_OK; "sm" or "all" for CRO_ERR_CHECKSUM with that verdict;
+ * "cuda-error:<cuda_error>" for CRO_ERR_CUDA; "error" otherwise), -sms ("<sms_covered>/<sm_count>"), -bad-sms
+ * (bad_sm[0 .. min(bad_sms, 16)), comma-separated; only when bad_sms > 0), -legs (the failed legs' names shfl, vote,
+ * match, redux, atoms, comma-separated; only when any failed) and -iterations. */
+int  cro_emit_xlane_annotations_json(const cro_xlane_result *r, char *buf, size_t cap, size_t *len);
+
 /* ---- L2:the L2 cache, the crossbar between the SMs and its slices, and the L2 atomic units ---- */
 
 /*
