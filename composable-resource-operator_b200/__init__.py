@@ -683,6 +683,62 @@ assert ctypes.sizeof(XlaneOpts) == 48 and ctypes.sizeof(XlaneResult) == 560 and 
     ctypes.sizeof(XlaneResult)
 
 
+# ALU probe (cro_probe_alu, cro_probe_alu_uuid, cro_alu_expected, cro_selftest_alu_classify)
+ALU_LEG_LOGIC, ALU_LEG_SHIFT, ALU_LEG_IADD, ALU_LEG_IMUL, ALU_LEG_FLOAT = range(5)
+ALU_LEGS, ALU_ALL_LEGS, ALU_THREADS, ALU_WARPS, ALU_THREAD_RECORDS = 5, 0x1F, 256, 8, 4
+ALU_RECORDS, ALU_MAX_SMS, ALU_MAX_ITERATIONS, ALU_MAX_ROUNDS = 4096, 256, 65536, 64
+ALU_LOGIC_OPS, ALU_SHIFT_OPS, ALU_IADD_OPS, ALU_IMUL_OPS, ALU_FLOAT_OPS, ALU_MAX_OPS = 538, 76, 200, 100, 360, 538
+ALU_OPS = [ALU_LOGIC_OPS, ALU_SHIFT_OPS, ALU_IADD_OPS, ALU_IMUL_OPS, ALU_FLOAT_OPS]
+ALU_NONE, ALU_SM, ALU_ALL = 0, 1, 2
+ALU_PERSISTENT, ALU_INTERMITTENT = 1, 2
+
+
+class AluOpts(ctypes.Structure):
+    _fields_ = [("iterations", ctypes.c_uint32), ("legs", ctypes.c_uint32), ("max_rounds", ctypes.c_uint32),
+                ("deadline_ms", ctypes.c_int32), ("test_inject_leg", ctypes.c_int32), ("test_inject_sm", ctypes.c_int32),
+                ("test_inject_warp", ctypes.c_int32), ("test_inject_lane", ctypes.c_int32), ("test_inject_op", ctypes.c_uint32),
+                ("test_inject_iteration", ctypes.c_uint32), ("test_inject_operand", ctypes.c_uint32), ("reserved", ctypes.c_uint32),
+                ("test_inject_mask", ctypes.c_uint64)]
+
+
+class AluResult(ctypes.Structure):
+    """cro_alu_result: the cross-lane result's fields (status, verdict, bad SMs, per-leg counts, folds, coverage and
+    times) and the time the host took to build the call's table."""
+    _fields_ = XlaneResult._fields_ + [("table_ns", ctypes.c_uint64)]
+
+
+class AluSm(ctypes.Structure):
+    """One SM seen by an ALU probe call: its failed legs, per-leg counts, fold mismatches, times and mark."""
+    _fields_ = XlaneSm._fields_
+
+
+class AluRecord(ctypes.Structure):
+    """cro_alu_record: one table entry, the operands of one (leg, op, warp, lane) and the exact result."""
+    _fields_ = [("in_", ctypes.c_uint64 * 4), ("out", ctypes.c_uint64 * 3), ("reserved", ctypes.c_uint64)]
+
+
+class AluFault(ctypes.Structure):
+    """One failed compare: leg, op, iteration, SM, warp, lane, the table's operands, expected and actual result."""
+    _fields_ = [("leg", ctypes.c_uint32), ("op", ctypes.c_uint32), ("iteration", ctypes.c_uint32), ("smid", ctypes.c_uint32),
+                ("warp", ctypes.c_uint32), ("lane", ctypes.c_uint32), ("reserved", ctypes.c_uint32 * 2), ("in_", ctypes.c_uint64 * 4),
+                ("expected", ctypes.c_uint64 * 3), ("actual", ctypes.c_uint64 * 3)]
+
+
+class AluThread(ctypes.Structure):
+    """cro_alu_thread: what one thread of the ALU probe publishes at the end of a launch."""
+    _fields_ = XlaneThread._fields_
+
+
+class AluCta(ctypes.Structure):
+    """cro_alu_cta: what thread 0 of a CTA of the ALU probe publishes at the end of a launch."""
+    _fields_ = XlaneCta._fields_
+
+
+assert ctypes.sizeof(AluOpts) == 56 and ctypes.sizeof(AluResult) == 568 and ctypes.sizeof(AluSm) == 80 \
+    and ctypes.sizeof(AluRecord) == 64 and ctypes.sizeof(AluFault) == 112 and ctypes.sizeof(AluThread) == 48 \
+    and ctypes.sizeof(AluCta) == 48, ctypes.sizeof(AluResult)
+
+
 # L2 probe (cro_probe_l2, cro_read_l2_health, cro_selftest_l2_classify)
 L2_BLOCK_BYTES, L2_MIN_BYTES, L2_MAX_L2_MULTIPLE, L2_ELEMENTS, L2_RECORDS, L2_MAX_SMS = 16384, 1 << 20, 8, 6, 4096, 256
 L2_MAX_ITERATIONS, L2_MAX_A1_COUNTERS, L2_MAX_A2_COUNTERS, L2_MAX_LINES, L2_MAX_COUNTERS = 256, 1 << 20, 8192, 8, 8
@@ -896,6 +952,7 @@ EXPORTS = [
     "cro_probe_regfile", "cro_probe_regfile_uuid", "cro_emit_regfile_annotations_json", "cro_selftest_regfile_classify",
     "cro_probe_xlane", "cro_probe_xlane_uuid", "cro_xlane_expected", "cro_emit_xlane_annotations_json",
     "cro_selftest_xlane_classify",
+    "cro_probe_alu", "cro_probe_alu_uuid", "cro_alu_expected", "cro_emit_alu_annotations_json", "cro_selftest_alu_classify",
     "cro_probe_l2", "cro_probe_l2_uuid", "cro_read_l2_health", "cro_emit_l2_annotations_json", "cro_selftest_l2_classify",
     "cro_selftest_sm_legs_classify", "cro_selftest_sram_classify",
     "cro_selftest_locate_collect", "cro_selftest_scan_collect", "cro_selftest_link_classify",
@@ -1082,6 +1139,15 @@ def _load() -> ctypes.CDLL:
         "cro_selftest_xlane_classify": (i32, [u32, u32, u64, u32, u64, u32, ctypes.POINTER(XlaneCta), ctypes.POINTER(XlaneThread),
                                               ctypes.POINTER(XlaneFault), ctypes.POINTER(XlaneResult), ctypes.POINTER(XlaneSm), i32,
                                               ctypes.POINTER(i32), ctypes.POINTER(XlaneFault), i32, ctypes.POINTER(i32)]),
+        "cro_probe_alu": (i32, [vp, i32, ctypes.POINTER(AluOpts), ctypes.POINTER(AluResult), ctypes.POINTER(AluSm),
+                                i32, ctypes.POINTER(i32), ctypes.POINTER(AluFault), i32, ctypes.POINTER(i32)]),
+        "cro_probe_alu_uuid": (i32, [vp, c, ctypes.POINTER(AluOpts), ctypes.POINTER(AluResult), ctypes.POINTER(AluSm),
+                                     i32, ctypes.POINTER(i32), ctypes.POINTER(AluFault), i32, ctypes.POINTER(i32)]),
+        "cro_alu_expected": (i32, [i32, u64, i32, ctypes.POINTER(AluRecord)]),
+        "cro_emit_alu_annotations_json": (i32, [ctypes.POINTER(AluResult)] + out),
+        "cro_selftest_alu_classify": (i32, [u32, u32, u64, u32, u64, u32, ctypes.POINTER(AluCta), ctypes.POINTER(AluThread),
+                                            ctypes.POINTER(AluFault), ctypes.POINTER(AluResult), ctypes.POINTER(AluSm), i32,
+                                            ctypes.POINTER(i32), ctypes.POINTER(AluFault), i32, ctypes.POINTER(i32)]),
         "cro_probe_l2": (i32, [vp, i32, ctypes.POINTER(L2Opts), ctypes.POINTER(L2Result), ctypes.POINTER(L2Sm), i32,
                                ctypes.POINTER(i32), ctypes.POINTER(L2Fault), i32, ctypes.POINTER(i32)]),
         "cro_probe_l2_uuid": (i32, [vp, c, ctypes.POINTER(L2Opts), ctypes.POINTER(L2Result), ctypes.POINTER(L2Sm), i32,
@@ -1322,6 +1388,38 @@ def selftest_xlane_classify(legs: int, iterations: int, seed: int, sm_count: int
                       XlaneResult, XlaneSm, XLANE_MAX_SMS, XlaneFault, cap)
     if rc not in (OK, ERR_CHECKSUM, ERR_UNSUPPORTED):
         raise ProbeError(rc, "cro_selftest_xlane_classify")
+    return out
+
+
+def emit_alu_annotations_json(r: AluResult) -> str:
+    """Additive cohdi.io/probe-alu-* annotations of an ALU probe result (Go-marshalled map[string]string)."""
+    return _text(lib.cro_emit_alu_annotations_json, ctypes.byref(r))
+
+
+def alu_expected(leg: int, seed: int, warp: int) -> List[AluRecord]:
+    """cro_alu_expected: the table of a call of seed `seed` for leg `leg` and warp `warp`: a list of AluRecord indexed
+    op * 32 + lane, each the operands and the exact result (host arithmetic, no GPU)."""
+    arr = (AluRecord * (ALU_OPS[leg] * 32))()
+    rc = lib.cro_alu_expected(leg, seed, warp, arr)
+    if rc != OK:
+        raise ProbeError(rc, "cro_alu_expected")
+    return list(arr)
+
+
+def selftest_alu_classify(legs: int, iterations: int, seed: int, sm_count: int, call: int, rounds, cap: Optional[int] = None):
+    """cro_selftest_alu_classify: the ALU probe's classification of call `call`, as selftest_xlane_classify with
+    AluCta, AluThread and AluFault.  Returns (result, SM entries, faults)."""
+    n_rounds = len(rounds[0]) if rounds else 0
+    assert all(len(r) == n_rounds for r in rounds)
+    flat = [rnd for leg in rounds for rnd in leg]
+    ctas = (AluCta * max(1, sm_count * len(flat)))(*[x for rnd in flat for x in rnd[0]])
+    thr = (AluThread * max(1, sm_count * ALU_THREADS * len(flat)))(*[x for rnd in flat for x in rnd[1]])
+    recs = (AluFault * max(1, sm_count * ALU_THREADS * ALU_THREAD_RECORDS * len(flat)))(*[x for rnd in flat for x in rnd[2]])
+    cap = ALU_RECORDS if cap is None else cap
+    rc, out = _per_sm(lib.cro_selftest_alu_classify, (legs, iterations, seed, sm_count, call, n_rounds, ctas, thr, recs),
+                      AluResult, AluSm, ALU_MAX_SMS, AluFault, cap)
+    if rc not in (OK, ERR_CHECKSUM, ERR_UNSUPPORTED):
+        raise ProbeError(rc, "cro_selftest_alu_classify")
     return out
 
 
@@ -1583,6 +1681,29 @@ def probe_xlane_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: int =
     handle = ctx.handle if ctx is not None else None
     rc, out = _per_sm(lib.cro_probe_xlane_uuid, (handle, _b(uuid), ctypes.byref(o)), XlaneResult, XlaneSm, XLANE_MAX_SMS,
                       XlaneFault, cap)
+    if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
+        raise _helper_error(rc, handle)
+    return out
+
+
+def _alu_opts(iterations: int, legs: int, max_rounds: int, deadline_ms: int,
+              inject: Optional[Tuple[int, int, int, int, int, int, int, int]]) -> AluOpts:
+    o = AluOpts()
+    o.iterations, o.legs, o.max_rounds, o.deadline_ms = iterations, legs, max_rounds, deadline_ms
+    if inject is not None:
+        (o.test_inject_leg, o.test_inject_sm, o.test_inject_warp, o.test_inject_lane, o.test_inject_op, o.test_inject_iteration,
+         o.test_inject_operand, o.test_inject_mask) = inject
+    return o
+
+
+def probe_alu_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: int = 0, legs: int = 0, max_rounds: int = 0,
+                   deadline_ms: int = 0, inject: Optional[Tuple[int, int, int, int, int, int, int, int]] = None,
+                   cap: int = 256) -> Tuple[AluResult, List[AluSm], List[AluFault]]:
+    """cro_probe_alu_uuid: the ALU probe of any GPU on the node, run by the helper process (ctx may be None).  Returns
+    the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up to `cap` records."""
+    o = _alu_opts(iterations, legs, max_rounds, deadline_ms, inject)
+    handle = ctx.handle if ctx is not None else None
+    rc, out = _per_sm(lib.cro_probe_alu_uuid, (handle, _b(uuid), ctypes.byref(o)), AluResult, AluSm, ALU_MAX_SMS, AluFault, cap)
     if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
         raise _helper_error(rc, handle)
     return out
@@ -2210,6 +2331,19 @@ class ProbeContext:
         o = _xlane_opts(iterations, legs, max_rounds, 0, inject)
         rc, out = _per_sm(lib.cro_probe_xlane, (self.handle, dev, ctypes.byref(o)), XlaneResult, XlaneSm, XLANE_MAX_SMS,
                           XlaneFault, cap)
+        self._check(rc, allow=(ERR_CHECKSUM, ERR_CUDA))
+        return out
+
+    def probe_alu(self, dev: int = 0, iterations: int = 0, legs: int = 0, max_rounds: int = 0,
+                  inject: Optional[Tuple[int, int, int, int, int, int, int, int]] = None,
+                  cap: int = 256) -> Tuple[AluResult, List[AluSm], List[AluFault]]:
+        """cro_probe_alu: every lane of every warp of one CTA per SM runs each integer, bit-manipulation, DPX and
+        directed-rounding floating-point form of the legs run (legs = 0: all) on the host table's operands and checks
+        the result.  iterations / max_rounds = 0: the defaults.  inject = (leg, sm, warp, lane, op, iteration, operand,
+        mask) is the test-only operand XOR (sm, warp, lane: -1 for every one).  Returns the result (its status is OK,
+        ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up to `cap` records."""
+        o = _alu_opts(iterations, legs, max_rounds, 0, inject)
+        rc, out = _per_sm(lib.cro_probe_alu, (self.handle, dev, ctypes.byref(o)), AluResult, AluSm, ALU_MAX_SMS, AluFault, cap)
         self._check(rc, allow=(ERR_CHECKSUM, ERR_CUDA))
         return out
 

@@ -99,6 +99,11 @@ static_assert(sizeof(cro_xlane_opts) == 48 && offsetof(cro_xlane_opts, test_inje
                   sizeof(cro_xlane_fault) == 48 && offsetof(cro_xlane_fault, expected) == 32 && sizeof(cro_xlane_thread) == 48 &&
                   sizeof(cro_xlane_cta) == 48 && offsetof(cro_xlane_cta, smid) == 32,
               "xlane layout");
+static_assert(sizeof(cro_alu_opts) == 56 && offsetof(cro_alu_opts, test_inject_mask) == 48 && sizeof(cro_alu_result) == 568 &&
+                  offsetof(cro_alu_result, mismatches) == 128 && offsetof(cro_alu_result, table_ns) == 560 && sizeof(cro_alu_sm) == 80 &&
+                  sizeof(cro_alu_record) == 64 && sizeof(cro_alu_fault) == 112 && offsetof(cro_alu_fault, in) == 32 &&
+                  offsetof(cro_alu_fault, actual) == 88 && sizeof(cro_alu_thread) == 48 && sizeof(cro_alu_cta) == 48,
+              "alu layout");
 static_assert(sizeof(cro_l2_opts) == 56 && sizeof(cro_l2_health) == 48 && sizeof(cro_l2_sm) == 128 && sizeof(cro_l2_fault) == 56 &&
                   sizeof(cro_l2_result) == 616 && offsetof(cro_l2_result, mismatches) == 80 &&
                   offsetof(cro_l2_result, bad_line) == 184 && offsetof(cro_l2_result, a1_bad) == 312 &&
@@ -598,6 +603,36 @@ int cro_selftest_xlane_classify(uint32_t legs, uint32_t iterations, uint64_t see
     std::vector<cro_xlane_sm> seen;
     std::vector<cro_xlane_fault> found;
     const int rc = classify_xlane(legs, iterations, seed, sm_count, call, rounds, ctas, threads, records, out, &seen, &found);
+    return listed({rc, true, copy_capped(seen, sms, sms_cap, n_sms), copy_capped(found, faults, cap, n)}, out);
+} CRO_API_CATCH
+int cro_probe_alu(cro_ctx* ctx, int i, const cro_alu_opts* opts, cro_alu_result* out, cro_alu_sm* sms, int sms_cap, int* n_sms,
+                  cro_alu_fault* faults, int cap, int* n) try {
+    return listed(per_sm_call(ctx, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_alu_opts& o, auto* seen, auto* found) {
+        return ctx_probe_alu(ctx, i, o, out, seen, found);
+    }), out);
+} CRO_API_CATCH
+int cro_probe_alu_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_alu_opts* opts, cro_alu_result* out, cro_alu_sm* sms,
+                       int sms_cap, int* n_sms, cro_alu_fault* faults, int cap, int* n) try {
+    return listed(per_sm_call(gpu_uuid, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_alu_opts& o, auto* seen, auto* found) {
+        return ctx_probe_alu_uuid(ctx, gpu_uuid, o, out, seen, found, cap);
+    }), out);
+} CRO_API_CATCH
+int cro_alu_expected(int leg, uint64_t seed, int warp, cro_alu_record* out) try {
+    if (leg < 0 || leg >= CRO_ALU_LEGS || warp < 0 || warp >= CRO_ALU_WARPS || !out) return CRO_ERR_INVALID_ARG;
+    alu_expected((unsigned)leg, seed, (unsigned)warp, out);
+    return CRO_OK;
+} CRO_API_CATCH
+int cro_selftest_alu_classify(uint32_t legs, uint32_t iterations, uint64_t seed, uint32_t sm_count, uint64_t call, uint32_t rounds,
+                              const cro_alu_cta* ctas, const cro_alu_thread* threads, const cro_alu_fault* records, cro_alu_result* out,
+                              cro_alu_sm* sms, int sms_cap, int* n_sms, cro_alu_fault* faults, int cap, int* n) try {
+    if (legs == 0 || legs > CRO_ALU_ALL_LEGS || iterations == 0 || iterations > CRO_ALU_MAX_ITERATIONS || sm_count == 0 ||
+        (rounds && (!ctas || !threads || !records)) || !out || !n_sms || !n || sms_cap < 0 || cap < 0 || (sms_cap > 0 && !sms) ||
+        (cap > 0 && !faults))
+        return CRO_ERR_INVALID_ARG;
+    *n = *n_sms = 0;
+    std::vector<cro_alu_sm> seen;
+    std::vector<cro_alu_fault> found;
+    const int rc = classify_alu(legs, iterations, seed, sm_count, call, rounds, ctas, threads, records, out, &seen, &found);
     return listed({rc, true, copy_capped(seen, sms, sms_cap, n_sms), copy_capped(found, faults, cap, n)}, out);
 } CRO_API_CATCH
 int cro_probe_l2(cro_ctx* ctx, int i, const cro_l2_opts* opts, cro_l2_result* out, cro_l2_sm* sms, int sms_cap, int* n_sms,
@@ -1243,20 +1278,30 @@ static Annotations regfile_annotations(const cro_regfile_result& r) {
     return m;
 }
 
-static Annotations xlane_annotations(const cro_xlane_result& r) {
-    static const char* const kLegs[CRO_XLANE_LEGS] = {"shfl", "vote", "match", "redux", "atoms"};
+// The cross-lane and ALU probes' annotations: the same keys under their own prefix.
+template <class R>
+static Annotations lane_annotations(const R& r, const std::string& p, const char* const* legs, unsigned n_legs, uint32_t sm, uint32_t all) {
     Annotations m;
-    const std::string p = "cohdi.io/probe-xlane-";
     m[p + "verdict"] = r.status == CRO_OK                                                 ? "ok"
-                       : r.status == CRO_ERR_CHECKSUM && r.verdict == CRO_XLANE_SM  ? "sm"
-                       : r.status == CRO_ERR_CHECKSUM && r.verdict == CRO_XLANE_ALL ? "all"
+                       : r.status == CRO_ERR_CHECKSUM && r.verdict == sm ? "sm"
+                       : r.status == CRO_ERR_CHECKSUM && r.verdict == all ? "all"
                        : r.status == CRO_ERR_CUDA ? cuda_error(r.cuda_error)
                                                    : "error";
     m[p + "sms"] = std::to_string(r.sms_covered) + "/" + std::to_string(r.sm_count);
     if (r.bad_sms) m[p + "bad-sms"] = join(r.bad_sm, std::min<uint32_t>(r.bad_sms, 16));
-    put_list(m, p + "legs", bit_names(r.failed_legs, kLegs, CRO_XLANE_LEGS));
+    put_list(m, p + "legs", bit_names(r.failed_legs, legs, n_legs));
     m[p + "iterations"] = std::to_string(r.iterations);
     return m;
+}
+
+static Annotations xlane_annotations(const cro_xlane_result& r) {
+    static const char* const kLegs[CRO_XLANE_LEGS] = {"shfl", "vote", "match", "redux", "atoms"};
+    return lane_annotations(r, "cohdi.io/probe-xlane-", kLegs, CRO_XLANE_LEGS, CRO_XLANE_SM, CRO_XLANE_ALL);
+}
+
+static Annotations alu_annotations(const cro_alu_result& r) {
+    static const char* const kLegs[CRO_ALU_LEGS] = {"logic", "shift", "iadd", "imul", "float"};
+    return lane_annotations(r, "cohdi.io/probe-alu-", kLegs, CRO_ALU_LEGS, CRO_ALU_SM, CRO_ALU_ALL);
 }
 
 static Annotations l2_annotations(const cro_l2_result& r) {
@@ -1413,6 +1458,11 @@ int cro_emit_regfile_annotations_json(const cro_regfile_result* r, char* buf, si
 int cro_emit_xlane_annotations_json(const cro_xlane_result* r, char* buf, size_t cap, size_t* len) try {
     if (!r) return CRO_ERR_INVALID_ARG;
     return emit(xlane_annotations(*r), buf, cap, len);
+} CRO_API_CATCH
+
+int cro_emit_alu_annotations_json(const cro_alu_result* r, char* buf, size_t cap, size_t* len) try {
+    if (!r) return CRO_ERR_INVALID_ARG;
+    return emit(alu_annotations(*r), buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_l2_annotations_json(const cro_l2_result* r, char* buf, size_t cap, size_t* len) try {

@@ -74,6 +74,12 @@
  *                                                    deadline; cro_xlane_result, CRO_XLANE_MAX_SMS cro_xlane_sm entries
  *                                                    (sms_listed of them filled) and its `recorded` cro_xlane_fault
  *                                                    records (at most cap) on stdout
+ *   croprobe-cli alu-raw <uuid> <seed_base> <iterations> <legs> <max_rounds> <inject_leg> <inject_sm> <inject_warp>
+ *                        <inject_lane> <inject_op> <inject_iteration> <inject_operand> <inject_mask> <cap>
+ *                                                    the ALU probe with every cro_alu_opts field but the deadline;
+ *                                                    cro_alu_result, CRO_ALU_MAX_SMS cro_alu_sm entries (sms_listed of
+ *                                                    them filled) and its `recorded` cro_alu_fault records (at most
+ *                                                    cap) on stdout
  *   croprobe-cli health-raw <uuid> <seed_base> <checks> <compute-raw's options and cap> <precision-raw's> <sram-raw's>
  *                           <l2-raw's> <link-raw's> <scan-raw's>
  *                                                    the health check (cro_check_health) with every option of every
@@ -81,7 +87,7 @@
  *                                                    the seed base), its sweep region L, NVML on; the cro_health_result,
  *                                                    then each check that ran, in run order, as its own -raw writes it
  *   croprobe-cli health <uuid|index>                 the health check with defaults; JSON annotations, exit 0 iff ok
- *   link-raw, compute-raw, precision-raw, sparse-raw, warpmma-raw, l2-raw, regfile-raw, xlane-raw and health-raw take
+ *   link-raw, compute-raw, precision-raw, sparse-raw, warpmma-raw, l2-raw, regfile-raw, xlane-raw, alu-raw and health-raw take
  *   cro_opts.seed_base from argv (the device seed is seed_base | minor, as in process), so that the library can give
  *   every helper call fresh patterns and operands; their counts are the helper's own, because neither result says how many records follow.
  * Exit 3: the device is not visible to this (fresh) process — the reference's found=false.  The raw commands exit 0
@@ -261,6 +267,18 @@ static int xlane_raw(cro_ctx *ctx, int idx, char **argv) {
     return put_frame(&cro_wire_xlane.frame, &xr, sms, (uint64_t)n_sms, faults, (uint64_t)got) ? 2 : end_frames(xr.status);
 }
 
+static int alu_raw(cro_ctx *ctx, int idx, char **argv) {
+    static cro_alu_opts ao;
+    const int cap = raw_opts(&cro_wire_alu, argv, &ao);
+    static cro_alu_result ar;
+    static cro_alu_sm sms[CRO_ALU_MAX_SMS];
+    cro_alu_fault *faults = (cro_alu_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
+    int n_sms = 0, got = 0;
+    if (!faults) return 2;
+    cro_probe_alu(ctx, idx, &ao, &ar, sms, CRO_ALU_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
+    return put_frame(&cro_wire_alu.frame, &ar, sms, (uint64_t)n_sms, faults, (uint64_t)got) ? 2 : end_frames(ar.status);
+}
+
 /* `scan`: the whole-HBM scan of the free memory (all of it but 1 GiB unless argv[3], in MiB, bounds it) as JSON. */
 static int scan_json(cro_ctx *ctx, int idx, char **argv) {
     cro_scan_opts so;
@@ -368,6 +386,7 @@ static const struct command {
     {NULL, &cro_wire_l2, CRO_F_LAZY_ALLOC, 64, l2_raw},
     {NULL, &cro_wire_regfile, CRO_F_LAZY_ALLOC, 64, regfile_raw},
     {NULL, &cro_wire_xlane, CRO_F_LAZY_ALLOC, 64, xlane_raw},
+    {NULL, &cro_wire_alu, CRO_F_LAZY_ALLOC, 64, alu_raw},
     /* a region of exactly L, the link's bytes (the probe checks L <= S; no halving on a full GPU), and NVML for the
      * replay counters */
     {NULL, &cro_wire_link, CRO_F_LAZY_ALLOC, 256, link_raw},
@@ -396,6 +415,8 @@ int main(int argc, char **argv) {
                         "<addr_row> <addr_kstep> <cap> | l2-raw <uuid> <seed_base> <bytes> <iterations> <a1> <a2> <leg> <sm> <element> <iteration> <word> <mask> <cap> | "
                         "regfile-raw <uuid> <seed_base> <iterations> <rounds> <sm> <warp> <lane> <slot> <element> <iteration> <mask> <cap> | "
                         "xlane-raw <uuid> <seed_base> <iterations> <legs> <rounds> <leg> <sm> <warp> <lane> <op> <iteration> <mask> <cap> | "
+                        "alu-raw <uuid> <seed_base> <iterations> <legs> <rounds> <leg> <sm> <warp> <lane> <op> <iteration> <operand> <mask> "
+                        "<cap> | "
                         "health-raw <uuid> <seed_base> <checks> <compute-raw, precision-raw, sram-raw, l2-raw, link-raw, scan-raw options "
                         "and caps> | health <uuid|index>\n");
         return 64;

@@ -221,6 +221,25 @@ static const cro_wire cro_wire_xlane = {"xlane-raw", 1, CRO_WIRE_FIELDS(cro_wire
                                          sizeof(cro_xlane_fault), CRO_WIRE_AT(cro_xlane_result, sms_listed),
                                          CRO_WIRE_AT(cro_xlane_result, recorded)}};
 
+static const cro_wire_field cro_wire_alu_fields[] = {
+    CRO_WIRE_FIELD(cro_alu_opts, iterations),
+    CRO_WIRE_FIELD(cro_alu_opts, legs),
+    CRO_WIRE_FIELD(cro_alu_opts, max_rounds),
+    CRO_WIRE_FIELD(cro_alu_opts, test_inject_leg),
+    CRO_WIRE_FIELD(cro_alu_opts, test_inject_sm),
+    CRO_WIRE_FIELD(cro_alu_opts, test_inject_warp),
+    CRO_WIRE_FIELD(cro_alu_opts, test_inject_lane),
+    CRO_WIRE_FIELD(cro_alu_opts, test_inject_op),
+    CRO_WIRE_FIELD(cro_alu_opts, test_inject_iteration),
+    CRO_WIRE_FIELD(cro_alu_opts, test_inject_operand),
+    CRO_WIRE_FIELD(cro_alu_opts, test_inject_mask),
+};
+/* The ALU frame: the result, then CRO_ALU_MAX_SMS cro_alu_sm entries (sms_listed of them filled) and `recorded`
+ * cro_alu_fault records. */
+static const cro_wire cro_wire_alu = {"alu-raw", 1, CRO_WIRE_FIELDS(cro_wire_alu_fields),
+                                      {sizeof(cro_alu_result), 0, sizeof(cro_alu_sm), CRO_ALU_MAX_SMS, sizeof(cro_alu_fault),
+                                       CRO_WIRE_AT(cro_alu_result, sms_listed), CRO_WIRE_AT(cro_alu_result, recorded)}};
+
 /* health-raw: <uuid> <seed_base> <checks>, then each check's fields and cap in run order (the CRO_HEALTH_* bit order).
  * Its stdout: the cro_health_result, then the frame of each check that ran, in run order.  opts_at and result_at:
  * where the check's options and result are in cro_health_opts and cro_health_result. */

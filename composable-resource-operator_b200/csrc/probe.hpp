@@ -87,6 +87,7 @@ struct Device {
     uint64_t regfile_calls = 0;            // k of the next register-file probe call (ctx_probe_regfile): its seeds
     uint64_t warpmma_calls = 0;            // k of the next warp-MMA probe call (ctx_probe_warpmma): its operand seed
     uint64_t xlane_calls = 0;              // k of the next cross-lane probe call (ctx_probe_xlane): its seeds
+    uint64_t alu_calls = 0;                // k of the next ALU probe call (ctx_probe_alu): its table's seed
     KernelPlan plan{};
     SweepScratch scratch{}, scratch_aux{}, scratch_pfx{};   // main stream / closed form / p2p prefix closed form
     // lane 0's buffers under their old names: the synchronous probe, the single sweeps and cro_probe_all use lane 0
@@ -431,6 +432,20 @@ void xlane_expected(unsigned leg, uint64_t seed, uint32_t iteration, unsigned wa
 int classify_xlane(uint32_t legs, uint32_t iterations, uint64_t seed, uint32_t sm_count, uint64_t k, uint32_t rounds,
                    const cro_xlane_cta* ctas, const cro_xlane_thread* threads, const cro_xlane_fault* records,
                    cro_xlane_result* r, std::vector<cro_xlane_sm>* sms, std::vector<cro_xlane_fault>* faults);
+
+// ALU probe (include/croprobe.h, cro_probe_alu / cro_probe_alu_uuid, alu_probe.cu): *sms gets one entry per SM seen,
+// by SM id; *faults the records, by (leg, smid, iteration, op, warp, lane), at most CRO_ALU_RECORDS.  The uuid form
+// runs `croprobe-cli alu-raw` with a fresh seed base and asks it for at most cap records.
+std::string alu_opts_error(const cro_alu_opts& o);
+int ctx_probe_alu(cro_ctx* c, int idx, const cro_alu_opts& o, cro_alu_result* r, std::vector<cro_alu_sm>* sms,
+                  std::vector<cro_alu_fault>* faults);
+int ctx_probe_alu_uuid(cro_ctx* c, const char* uuid, const cro_alu_opts& o, cro_alu_result* r, std::vector<cro_alu_sm>* sms,
+                       std::vector<cro_alu_fault>* faults, int cap);
+// cro_alu_expected and cro_selftest_alu_classify.
+void alu_expected(unsigned leg, uint64_t seed, unsigned warp, cro_alu_record* out);
+int classify_alu(uint32_t legs, uint32_t iterations, uint64_t seed, uint32_t sm_count, uint64_t k, uint32_t rounds,
+                 const cro_alu_cta* ctas, const cro_alu_thread* threads, const cro_alu_fault* records, cro_alu_result* r,
+                 std::vector<cro_alu_sm>* sms, std::vector<cro_alu_fault>* faults);
 
 // L2 probe (include/croprobe.h, cro_probe_l2, l2_probe.cu): *sms gets one entry per SM seen, by SM id; *faults every
 // recorded word, by (word, iteration, element, smid).

@@ -6,6 +6,7 @@
 // CRO_XLANE_THREAD_RECORDS records in its own slots, folds the last iteration's results and publishes them with plain
 // stores; thread 0 publishes the CTA's window.  No ballot gate, warp-aggregated claim, shared tally or global atomic:
 // tests/test_xlane_abi.py checks on the SASS that an instantiation issues only its own leg's cross-lane forms.
+#include "lane_tally.cuh"
 #include "xlane_kernels.cuh"
 
 namespace cro {
@@ -20,28 +21,12 @@ constexpr size_t kSmemBytes = 160u << 10;
 constexpr unsigned kArenaWords = 1024;                  // ATOMS: 8-byte words, then 512 presence bytes
 constexpr unsigned kCasTries = 512;                     // more than any group's size: a correct unit never runs out
 
-__device__ __forceinline__ unsigned long long timer_ns() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-
 // What a thread accumulates for its own entry.
-struct Tally {
-    unsigned long long count = 0, last = 0, fx = 0, fs = 0, fw = 0;
-    cro_xlane_fault* rec;
+struct Tally : LaneCounts<cro_xlane_fault, kR> {
     unsigned leg, smid, warp, lane;
     __device__ __forceinline__ void check(unsigned it, bool lastit, unsigned op, unsigned peer, u64 e, u64 got) {
-        if (got != e) {
-            if (count < kR) rec[count] = cro_xlane_fault{leg, op, it, smid, warp, lane, peer, 0u, e, got};
-            ++count;
-            last += lastit ? 1u : 0u;
-        }
-        if (lastit) {
-            fx ^= got;
-            fs += got;
-            fw += got * (2ull * op + 1ull);
-        }
+        if (got != e) miss(lastit, [&] { return cro_xlane_fault{leg, op, it, smid, warp, lane, peer, 0u, e, got}; });
+        if (lastit) fold(op, got);
     }
 };
 
@@ -304,7 +289,7 @@ __global__ void __launch_bounds__(kT, 1) xlane_kernel(const XlaneArgs a) {
     T.smid = smid;
     T.warp = w;
     T.lane = l;
-    const unsigned long long t0 = timer_ns();
+    const unsigned long long t0 = lane_timer_ns();
     const long long k0 = clock64();
 #pragma unroll 1
     for (unsigned it = 0; it < a.iterations; ++it) {
@@ -318,27 +303,8 @@ __global__ void __launch_bounds__(kT, 1) xlane_kernel(const XlaneArgs a) {
         if (LEG == CRO_XLANE_LEG_ATOMS) leg_atoms(T, seed, it, lastit, w, l, a.inj_op, m, arena);
     }
     const long long k1 = clock64();
-    const unsigned long long t1 = timer_ns();
-    cro_xlane_thread& o = a.thr[me];
-    o.count = T.count;
-    o.last = T.last;
-    o.fold_x = T.fx;
-    o.fold_s = T.fs;
-    o.fold_w = T.fw;
-    __threadfence();
-    o.stamp = a.stamp;
-    if (t == 0) {
-        cro_xlane_cta& c = a.cta[blockIdx.x];
-        c.t0 = t0;
-        c.t1 = t1;
-        c.cycles = (unsigned long long)(k1 - k0);
-        c.smid = smid;
-        c.nsmid = nsmid;
-        c.block = blockIdx.x;
-        c.reserved = 0;
-        __threadfence();
-        c.stamp = a.stamp;
-    }
+    const unsigned long long t1 = lane_timer_ns();
+    T.publish(a.thr[me], a.cta, a.stamp, t0, t1, k0, k1, smid, nsmid);
 }
 
 template <unsigned LEG>

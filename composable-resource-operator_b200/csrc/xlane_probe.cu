@@ -1,10 +1,6 @@
 // xlane_probe.cu — the cross-lane probe (cro_probe_xlane, cro_probe_xlane_uuid): every SM's shuffle, vote, match,
 // warp-reduce and shared-atomic units checked op by op on every lane, one launch per leg.
-#include <map>
-#include <set>
-#include <tuple>
-
-#include "probe_internal.hpp"
+#include "lane_report.hpp"
 #include "xlane_kernels.cuh"
 
 namespace cro {
@@ -56,120 +52,20 @@ void closed_form(uint64_t seed, uint32_t iterations, uint32_t legs, cro_xlane_re
     }
 }
 
-// What a call's rounds leave for its verdict.
-struct XlaneTally {
-    std::map<uint32_t, cro_xlane_sm> per_sm;
-    std::map<uint32_t, uint64_t> last;                      // per SM: failed compares of the last iteration
-    std::set<uint32_t> seen[CRO_XLANE_LEGS];
-    uint32_t fold_sm[CRO_XLANE_LEGS] = {~0u, ~0u, ~0u, ~0u, ~0u};   // the lowest SM seen per leg, whose fold r reports
-    std::vector<cro_xlane_fault> recs;
+// The cross-lane probe's types and constants for the shared report path (lane_report.hpp).
+struct XlaneReport {
+    using Result = cro_xlane_result;
+    using Sm = cro_xlane_sm;
+    using Fault = cro_xlane_fault;
+    using Thread = cro_xlane_thread;
+    using Cta = cro_xlane_cta;
+    static constexpr unsigned kLegs = CRO_XLANE_LEGS, kThreads = CRO_XLANE_THREADS, kThreadRecs = CRO_XLANE_THREAD_RECORDS,
+                              kRecords = CRO_XLANE_RECORDS, kMaxSms = CRO_XLANE_MAX_SMS, kPersistent = CRO_XLANE_PERSISTENT,
+                              kIntermittent = CRO_XLANE_INTERMITTENT, kNone = CRO_XLANE_NONE, kSm = CRO_XLANE_SM, kAll = CRO_XLANE_ALL;
+    static constexpr const char* kName = "cross-lane probe";
+    static unsigned ops(unsigned leg) { return xlane::kOps[leg]; }
 };
-
-bool any_failed(const cro_xlane_thread* ht, int grid, uint64_t k) {
-    for (size_t i = 0; i < (size_t)grid * CRO_XLANE_THREADS; ++i)
-        if (ht[i].stamp == k && ht[i].count) return true;
-    return false;
-}
-
-// One round of leg `leg` of call k: the grid CTAs' entries hc, their threads' entries ht and records hr (read only for
-// threads that failed).  CRO_ERR_UNSUPPORTED (with the error text) when the device reports more SM ids than the
-// result holds.
-int take_xlane_round(cro_ctx* c, unsigned leg, const cro_xlane_cta* hc, const cro_xlane_thread* ht, const cro_xlane_fault* hr,
-                     int grid, uint64_t k, cro_xlane_result* r, XlaneTally& t, uint32_t* covered) {
-    const uint32_t bit = 1u << leg;
-    r->ctas += (uint32_t)grid;
-    uint64_t t0 = ~0ull, t1 = 0;
-    for (int j = 0; j < grid; ++j) {
-        const cro_xlane_cta& x = hc[(size_t)j];
-        if (x.stamp != k) {
-            r->unpublished++;
-            r->failed_legs |= bit;
-            continue;
-        }
-        if (x.nsmid > CRO_XLANE_MAX_SMS) {
-            set_call_error(c, "cross-lane probe: the device reports %nsmid = " + std::to_string(x.nsmid) +
-                                  ", more SM ids than the " + std::to_string(CRO_XLANE_MAX_SMS) + " the result holds");
-            return CRO_ERR_UNSUPPORTED;
-        }
-        r->nsmid = x.nsmid;
-        t0 = std::min<uint64_t>(t0, x.t0);
-        t1 = std::max<uint64_t>(t1, x.t1);
-        t.seen[leg].insert(x.smid);
-        cro_xlane_sm& S = t.per_sm[x.smid];
-        S.smid = x.smid;
-        S.ctas++;
-        S.ns += x.t1 > x.t0 ? x.t1 - x.t0 : 0;
-        S.cycles += x.cycles;
-        uint64_t fx = 0, fs = 0, fw = 0, n = 0;
-        bool silent = false;
-        for (size_t q = 0; q < CRO_XLANE_THREADS; ++q) {
-            const size_t i = (size_t)j * CRO_XLANE_THREADS + q;
-            const cro_xlane_thread& e = ht[i];
-            if (e.stamp != k) {
-                r->threads_unpublished++;
-                silent = true;
-                continue;
-            }
-            n += e.count;
-            t.last[x.smid] += e.last;
-            fx ^= e.fold_x;
-            fs += e.fold_s;
-            fw += e.fold_w;
-            for (size_t m = 0; m < std::min<uint64_t>(e.count, kThreadRecs); ++m) t.recs.push_back(hr[i * kThreadRecs + m]);
-        }
-        S.mismatches[leg] += n;
-        r->mismatches[leg] += n;
-        r->ops_checked[leg] += (uint64_t)xlane::kOps[leg] * CRO_XLANE_THREADS * r->iterations;
-        const bool fold_bad = !silent && (fx != r->expect[leg][0] || fs != r->expect[leg][1] || fw != r->expect[leg][2]);
-        S.fold_mismatches += fold_bad ? 1 : 0;
-        r->fold_mismatches[leg] += fold_bad ? 1 : 0;
-        if (n || fold_bad || silent) {
-            S.failed_legs |= bit;
-            r->failed_legs |= bit;
-        }
-        if (x.smid < t.fold_sm[leg]) {
-            t.fold_sm[leg] = x.smid;
-            r->fold[leg][0] = fx;
-            r->fold[leg][1] = fs;
-            r->fold[leg][2] = fw;
-        }
-    }
-    if (t1 > t0) r->timer_ns += t1 - t0;
-    *covered = (uint32_t)t.seen[leg].size();
-    return CRO_OK;
-}
-
-// The call's end: coverage, each SM's mark (persistent: a compare of the last iteration failed; intermittent: only an
-// earlier one, only the fold, or a thread that did not publish), the records sorted and capped, the bad SMs and the
-// verdict.
-int close_xlane_call(cro_xlane_result* r, XlaneTally& t, std::vector<cro_xlane_sm>* sms, std::vector<cro_xlane_fault>* faults) {
-    uint32_t covered = ~0u;
-    for (unsigned leg = 0; leg < CRO_XLANE_LEGS; ++leg)
-        if (r->legs >> leg & 1u) covered = std::min<uint32_t>(covered, (uint32_t)t.seen[leg].size());
-    r->sms_covered = covered == ~0u ? 0 : covered;
-    r->complete = r->sms_covered >= r->sm_count ? 1u : 0u;
-    for (auto& kv : t.per_sm) {
-        cro_xlane_sm& S = kv.second;
-        S.mark = t.last[kv.first] ? CRO_XLANE_PERSISTENT : S.failed_legs ? CRO_XLANE_INTERMITTENT : 0u;
-        if (S.mark) {
-            if (r->bad_sms < 16) r->bad_sm[r->bad_sms] = (uint16_t)kv.first;
-            r->bad_sms++;
-        }
-        sms->push_back(S);
-    }
-    r->failed_sms = r->bad_sms;
-    *faults = std::move(t.recs);
-    std::stable_sort(faults->begin(), faults->end(), [](const cro_xlane_fault& x, const cro_xlane_fault& y) {
-        return std::make_tuple(x.leg, x.smid, x.iteration, x.op, x.warp, x.lane) <
-               std::make_tuple(y.leg, y.smid, y.iteration, y.op, y.warp, y.lane);
-    });
-    if (faults->size() > CRO_XLANE_RECORDS) faults->resize(CRO_XLANE_RECORDS);
-    const bool silent = r->unpublished || r->threads_unpublished;
-    const bool all = silent || (r->failed_sms && r->failed_sms == t.per_sm.size());
-    const bool any = silent || r->failed_sms;
-    r->verdict = all ? CRO_XLANE_ALL : any ? CRO_XLANE_SM : CRO_XLANE_NONE;
-    return r->status = any ? CRO_ERR_CHECKSUM : CRO_OK;
-}
+using XlaneTally = LaneTally<XlaneReport>;
 
 // The call's settings before anything runs.
 void open_xlane_call(cro_xlane_result* r, uint64_t seed, uint64_t k, uint32_t sm_count, uint32_t legs, uint32_t iters) {
@@ -261,8 +157,8 @@ int ctx_probe_xlane(cro_ctx* c, int idx, const cro_xlane_opts& o, cro_xlane_resu
             auto launch = [&] { return launch_xlane(leg, a, sm_count, st); };
             auto fetch = [&] { return cudaMemcpyAsync(head.data(), b.p, head.size(), cudaMemcpyDeviceToHost, st); };
             auto take = [&](uint32_t* covered) -> int {
-                if (any_failed(ht, sm_count, k)) CU_TRY(c, cudaMemcpy(hr.data(), a.rec, rec_bytes, cudaMemcpyDeviceToHost));
-                return take_xlane_round(c, leg, hc, ht, hr.data(), sm_count, k, r, t, covered);
+                if (lane_any_failed<XlaneReport>(ht, sm_count, k)) CU_TRY(c, cudaMemcpy(hr.data(), a.rec, rec_bytes, cudaMemcpyDeviceToHost));
+                return take_lane_round<XlaneReport>(c, leg, hc, ht, hr.data(), sm_count, k, r, t, covered);
             };
             uint32_t rounds = 0;
             const int e = coverage_rounds(c, d, ev, b.p, head.size(), (uint32_t)sm_count, max_rounds, &rounds, &r->leg_ns[leg], launch,
@@ -281,7 +177,7 @@ int ctx_probe_xlane(cro_ctx* c, int idx, const cro_xlane_opts& o, cro_xlane_resu
         r->wall_ns = now_ns() - t_call;
         return r->status = rc;
     }
-    const int status = close_xlane_call(r, t, sms, faults);
+    const int status = close_lane_call<XlaneReport>(r, t, sms, faults);
     r->wall_ns = now_ns() - t_call;
     return status;
 }
@@ -298,14 +194,14 @@ int classify_xlane(uint32_t legs, uint32_t iterations, uint64_t seed, uint32_t s
         for (uint32_t j = 0; j < rounds; ++j, ctas += sm_count, threads += n_thr, records += n_thr * kThreadRecs) {
             ++r->rounds;
             uint32_t covered = 0;
-            const int e = take_xlane_round(nullptr, leg, ctas, threads, records, (int)sm_count, k, r, t, &covered);
+            const int e = take_lane_round<XlaneReport>(nullptr, leg, ctas, threads, records, (int)sm_count, k, r, t, &covered);
             if (e) {
                 blank_result(r, *r, sms, faults);
                 return r->status = e;
             }
         }
     }
-    return close_xlane_call(r, t, sms, faults);
+    return close_lane_call<XlaneReport>(r, t, sms, faults);
 }
 
 int ctx_probe_xlane_uuid(cro_ctx* c, const char* uuid, const cro_xlane_opts& o, cro_xlane_result* r,

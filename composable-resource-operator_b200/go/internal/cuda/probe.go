@@ -1033,6 +1033,73 @@ func (c *Context) ProbeXlaneByUUID(deviceID string) (r XlaneResult, found bool, 
 	return r, true, nil
 }
 
+// AluResult is the summary of cro_alu_result an operator reads: whether every
+// SM's integer, bit-manipulation, DPX and directed-rounding floating-point
+// instructions gave the exact answer on every lane, and which SMs and legs did not.
+type AluResult struct {
+	Status      int32  // CRO_OK, CRO_ERR_CHECKSUM or CRO_ERR_CUDA
+	CudaError   int32  // cudaError_t of a failed launch (CRO_ERR_CUDA)
+	Verdict     uint32 // CRO_ALU_NONE / _SM / _ALL
+	FailedLegs  uint32 // bit per CRO_ALU_LEG_* that failed
+	SMCount     uint32
+	Covered     uint32
+	BadSMs      []uint32 // SMs that failed, ascending (at most 16)
+	Faults      []AluFault
+	Annotations string // Go-marshalled map[string]string of cohdi.io/probe-alu-* keys
+}
+
+// AluFault is one failed compare (cro_alu_fault): the op, where it ran, its
+// operands as the table holds them, and the expected and actual result words.
+type AluFault struct {
+	Leg, Op, Iteration, SM, Warp, Lane uint32
+	In                                 [4]uint64
+	Expected, Actual                   [3]uint64
+}
+
+// ProbeAluByUUID runs cro_probe_alu_uuid with its defaults: the ALU probe of
+// any GPU on the node through the helper process (INTEGRATION.md "The ALU
+// probe").  A mismatch or a fault (CRO_ERR_CUDA) is a result, not an error;
+// found is false when the node does not list the GPU.
+func (c *Context) ProbeAluByUUID(deviceID string) (r AluResult, found bool, err error) {
+	id := C.CString(deviceID)
+	defer C.free(unsafe.Pointer(id))
+	var res C.cro_alu_result
+	sms := make([]C.cro_alu_sm, C.CRO_ALU_MAX_SMS)
+	var faults [256]C.cro_alu_fault
+	var nSMs, got C.int
+	rc := C.cro_probe_alu_uuid(c.h, id, nil, &res, &sms[0], C.CRO_ALU_MAX_SMS, &nSMs, &faults[0], 256, &got)
+	if rc == C.CRO_ERR_NO_DEVICE {
+		return r, false, nil
+	}
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM && rc != C.CRO_ERR_CUDA {
+		return r, true, errorOf(c.h, rc)
+	}
+	r = AluResult{Status: int32(res.status), CudaError: int32(res.cuda_error), Verdict: uint32(res.verdict),
+		FailedLegs: uint32(res.failed_legs), SMCount: uint32(res.sm_count), Covered: uint32(res.sms_covered)}
+	for i := 0; i < int(res.bad_sms) && i < 16; i++ {
+		r.BadSMs = append(r.BadSMs, uint32(res.bad_sm[i]))
+	}
+	for i := 0; i < int(got); i++ {
+		f := faults[i]
+		a := AluFault{Leg: uint32(f.leg), Op: uint32(f.op), Iteration: uint32(f.iteration), SM: uint32(f.smid),
+			Warp: uint32(f.warp), Lane: uint32(f.lane)}
+		for k := 0; k < 4; k++ {
+			a.In[k] = uint64(f.in[k])
+		}
+		for k := 0; k < 3; k++ {
+			a.Expected[k], a.Actual[k] = uint64(f.expected[k]), uint64(f.actual[k])
+		}
+		r.Faults = append(r.Faults, a)
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_alu_annotations_json(&res, buf, 4096, &ln) == C.CRO_OK {
+		r.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return r, true, nil
+}
+
 // L2Result is the summary of cro_l2_result an operator reads: whether the
 // L2-resident buffer held what each SM wrote when another SM read it back,
 // whether the L2 atomic units gave the right answers, which SMs, buffer offsets

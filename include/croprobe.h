@@ -1935,6 +1935,203 @@ int  cro_selftest_xlane_classify(uint32_t legs, uint32_t iterations, uint64_t se
  * match, redux, atoms, comma-separated; only when any failed) and -iterations. */
 int  cro_emit_xlane_annotations_json(const cro_xlane_result *r, char *buf, size_t cap, size_t *len);
 
+/* ---- ALU: every SM's integer, bit-manipulation, DPX and directed-rounding floating-point instructions ---- */
+
+/*
+ * Address arithmetic, hashing, Philox (IMAD.HI), FP8/int4 packing (PRMT, LOP3), int8 GEMV (IDP.4A), top-k compares and
+ * masks all run on the SM's scalar integer and FP32/FP64 pipes.  A wrong LUT bit, a shift that clamps at the wrong
+ * count or a wrong high word computes a wrong answer and raises nothing.  The ALU probe checks each instruction form
+ * on every lane of every warp of one CTA per SM against an exact answer.
+ *
+ * The device computes no operand and no expected value, since that arithmetic is the unit under test: the host builds
+ * one table per call from the call's seed (seed = seed_dev + 2^53 + k * 0xD1B54A32D192ED03), holding for every (leg,
+ * op, warp, lane) a cro_alu_record with the operands and the exact result, computed in host integer arithmetic
+ * (directed rounding included; no host FPU rounding mode is involved).  cro_alu_expected returns it.  Every iteration
+ * repeats the same table.  Each thread loads its record, runs exactly one instruction form on it and compares the
+ * result with the loaded one.  Op = form * rows + row; DESIGN.md "The ALU probe" lists each leg's forms:
+ *   LOGIC  lop3.b32 at all 256 LUTs; bmsk .clamp / .wrap; brev; popc .b32 / .b64; bfind .u32 / .s32 (and .shiftamt);
+ *          szext .clamp / .wrap .u32 / .s32
+ *   SHIFT  shf .l / .r x .wrap / .clamp; shl .b32 / .b64; shr .b32 / .u32 / .s32 / .b64 / .u64 / .s64; prmt.b32
+ *          with per-lane selectors and in modes .f4e .b4e .rc8 .ecl .ecr .rc16
+ *   IADD   add / sub carry chains over 64 and 128 bits; setp at every integer comparison feeding selp; min / max
+ *          .s32 .u32 .s16x2 .u16x2 (with .relu); the three-operand min / max and add-min / add-max pairs ptxas fuses
+ *          into VIMNMX3 / VIADDMNMX; sad
+ *   IMUL   mul .lo / .hi / .wide .s32 .u32; mad .lo / .hi; mad.cc / madc chains; mul.lo.u64; dp4a and dp2a.lo / .hi
+ *          in all four signedness pairs
+ *   FLOAT  add / sub / mul / fma .f32 at .rn .rz .rm .rp; add / mul / fma .f64 at .rz .rm .rp; min / max .f32
+ *          plain, .NaN and .xorsign.abs; setp.f32 at all 14 comparisons
+ * Only inputs whose result bits the PTX ISA fixes are generated: no NaN out of arithmetic, no mixed-sign zero pair
+ * into min / max.  The report path is the cross-lane probe's: per-thread counts, first CRO_ALU_THREAD_RECORDS
+ * records and a fold of the last iteration, published with plain stores, stamped with the call number.
+ *
+ * Verdict and marks follow the cross-lane probe.  status: CRO_ERR_CHECKSUM on any mismatch, fold mismatch or entry
+ * not published; CRO_ERR_CUDA when a launch failed.
+ */
+#define CRO_ALU_LEG_LOGIC          0
+#define CRO_ALU_LEG_SHIFT          1
+#define CRO_ALU_LEG_IADD           2
+#define CRO_ALU_LEG_IMUL           3
+#define CRO_ALU_LEG_FLOAT          4
+#define CRO_ALU_LEGS               5
+#define CRO_ALU_ALL_LEGS           0x1Fu
+#define CRO_ALU_THREADS            256     /* threads per CTA: 8 warps                                       */
+#define CRO_ALU_WARPS              8
+#define CRO_ALU_THREAD_RECORDS     4       /* records each thread keeps                                      */
+#define CRO_ALU_RECORDS            4096    /* records a result holds; counts stay exact beyond               */
+#define CRO_ALU_MAX_SMS            256     /* SM ids the results hold; a larger %nsmid fails the call        */
+#define CRO_ALU_MAX_ITERATIONS     65536
+#define CRO_ALU_MAX_ROUNDS         64
+#define CRO_ALU_LOGIC_OPS          538     /* 269 forms x 2 rows                                             */
+#define CRO_ALU_SHIFT_OPS          76      /* 19 forms x 4 rows                                              */
+#define CRO_ALU_IADD_OPS           200     /* 50 forms x 4 rows                                              */
+#define CRO_ALU_IMUL_OPS           100     /* 25 forms x 4 rows                                              */
+#define CRO_ALU_FLOAT_OPS          360     /* 45 forms x 8 rows                                              */
+#define CRO_ALU_MAX_OPS            538
+
+#define CRO_ALU_NONE               0u
+#define CRO_ALU_SM                 1u      /* a strict subset of the covered SMs failed                      */
+#define CRO_ALU_ALL                2u      /* every covered SM failed, or an entry was not published          */
+
+#define CRO_ALU_PERSISTENT         1u      /* cro_alu_sm.mark: a compare of the last iteration failed         */
+#define CRO_ALU_INTERMITTENT       2u      /* only an earlier iteration failed, or only the fold               */
+
+typedef struct cro_alu_opts {
+    uint32_t iterations;           /*   0  per CTA and leg: 0 = the default (DESIGN.md), at most MAX_ITERATIONS   */
+    uint32_t legs;                 /*   4  bit per CRO_ALU_LEG_*: 0 = all                                          */
+    uint32_t max_rounds;           /*   8  launches per leg while fewer than sm_count SMs took part: 0 = 4         */
+    int32_t  deadline_ms;          /*  12  cro_probe_alu_uuid: the helper's deadline; 0 = CRO_HELPER_TIMEOUT_MS    */
+    /* test only: with test_inject_mask != 0, the mask is XORed into operand test_inject_operand (in[0 .. 3]) of op
+       test_inject_op of leg test_inject_leg that thread (test_inject_warp, test_inject_lane) of the CTA on SM
+       test_inject_sm uses in iteration test_inject_iteration (-1: every SM, warp or lane), after it is loaded and
+       before the instruction.  A software stand-in for a fault: the expected values still come from the table. */
+    int32_t  test_inject_leg;      /*  16 */
+    int32_t  test_inject_sm;       /*  20 */
+    int32_t  test_inject_warp;     /*  24 */
+    int32_t  test_inject_lane;     /*  28 */
+    uint32_t test_inject_op;       /*  32 */
+    uint32_t test_inject_iteration;/*  36 */
+    uint32_t test_inject_operand;  /*  40  0 .. 3                                                                */
+    uint32_t reserved;             /*  44 */
+    uint64_t test_inject_mask;     /*  48 */
+} cro_alu_opts;                    /*  56 bytes */
+
+typedef struct cro_alu_result {
+    int32_t  status;               /*   0  the return value                                                      */
+    uint32_t verdict;              /*   4  CRO_ALU_NONE / _SM / _ALL                                              */
+    uint64_t seed;                 /*   8  seed of this call's table                                             */
+    uint64_t call;                 /*  16  k: the call's number on this device, from 0                          */
+    uint32_t sm_count;             /*  24  multiprocessors the device reports                                    */
+    uint32_t nsmid;                /*  28  %nsmid as the kernel reads it                                         */
+    int32_t  cuda_error;           /*  32  cudaError_t of the launch that failed; 0: none                        */
+    uint32_t legs;                 /*  36  legs run                                                              */
+    uint32_t iterations;           /*  40  per CTA and leg                                                       */
+    uint32_t rounds;               /*  44  launches, over every leg                                              */
+    uint32_t sms_covered;          /*  48  distinct SMs that ran a CTA, in the leg run that saw the fewest        */
+    uint32_t complete;             /*  52  1: every leg covered sm_count SMs                                     */
+    uint32_t ctas;                 /*  56  CTAs launched                                                         */
+    uint32_t unpublished;          /*  60  CTAs launched that published no record                               */
+    uint32_t threads_unpublished;  /*  64  threads of published CTAs that published no entry                    */
+    uint32_t failed_sms;           /*  68  distinct SMs with a mark                                              */
+    uint32_t bad_sms;              /*  72  = failed_sms                                                          */
+    uint32_t failed_legs;          /*  76  bit per leg with a mismatch, fold mismatch or unpublished entry       */
+    uint16_t bad_sm[16];           /*  80  the first 16 failed SMs, ascending                                    */
+    uint64_t recorded;             /* 112  records written to the caller's list (*n)                            */
+    uint32_t sms_listed;           /* 120  entries written to the caller's per-SM list                          */
+    uint32_t reserved;             /* 124 */
+    uint64_t mismatches[CRO_ALU_LEGS];         /* 128  compares that failed, per leg, exact                     */
+    uint64_t ops_checked[CRO_ALU_LEGS];        /* 168  compares made: ops * 256 * iterations per published CTA  */
+    uint64_t fold_mismatches[CRO_ALU_LEGS];    /* 208  CTAs whose fold differs from the closed form              */
+    uint64_t leg_ns[CRO_ALU_LEGS];             /* 248  CUDA events around each leg's launches                    */
+    uint64_t fold[CRO_ALU_LEGS][3];            /* 288  (xor, sum, weighted sum) of the lowest SM id's CTA         */
+    uint64_t expect[CRO_ALU_LEGS][3];          /* 408  the closed form every CTA's fold must equal                */
+    uint64_t ns;                   /* 528  CUDA events around the launches, summed                              */
+    uint64_t timer_ns;             /* 536  %globaltimer: first CTA start .. last CTA end, summed over rounds     */
+    uint64_t wall_ns;              /* 544  the whole call                                                       */
+    uint64_t helper_ns;            /* 552  cro_probe_alu_uuid: spawn of the helper to its exit; 0 in process    */
+    uint64_t table_ns;             /* 560  building the call's table on the host (part of wall_ns)              */
+} cro_alu_result;                  /* 568 bytes */
+
+typedef struct cro_alu_sm {
+    uint32_t smid;                 /*   0 */
+    uint32_t mark;                 /*   4  0, CRO_ALU_PERSISTENT or CRO_ALU_INTERMITTENT                         */
+    uint32_t failed_legs;          /*   8  bit per leg that failed on this SM                                    */
+    uint32_t ctas;                 /*  12  CTAs that ran on this SM, over every leg                              */
+    uint64_t mismatches[CRO_ALU_LEGS];     /*  16 */
+    uint64_t fold_mismatches;      /*  56 */
+    uint64_t ns;                   /*  64  %globaltimer windows of this SM's CTAs, summed                       */
+    uint64_t cycles;               /*  72  %clock64 cycles of the same CTAs, summed                             */
+} cro_alu_sm;                      /*  80 bytes */
+
+/* One table entry: the operands of one (leg, op, warp, lane) and the exact result.  Which words a form reads and
+ * writes is listed in DESIGN.md "The ALU probe"; unused words are 0. */
+typedef struct cro_alu_record {
+    uint64_t in[4];                /*   0 */
+    uint64_t out[3];               /*  32 */
+    uint64_t reserved;             /*  56 */
+} cro_alu_record;                  /*  64 bytes */
+
+typedef struct cro_alu_fault {
+    uint32_t leg;                  /*   0  CRO_ALU_LEG_*                                                         */
+    uint32_t op;                   /*   4  the op's index within its leg: form * rows + row                      */
+    uint32_t iteration;            /*   8 */
+    uint32_t smid;                 /*  12 */
+    uint32_t warp;                 /*  16 */
+    uint32_t lane;                 /*  20 */
+    uint32_t reserved[2];          /*  24 */
+    uint64_t in[4];                /*  32  the operands as the table holds them                                  */
+    uint64_t expected[3];          /*  64 */
+    uint64_t actual[3];            /*  88 */
+} cro_alu_fault;                   /* 112 bytes */
+
+/* What one thread publishes at the end of a launch, with plain stores. */
+typedef struct cro_alu_thread {
+    uint64_t stamp;                /*   0  the call number k; any other value: the thread did not publish         */
+    uint64_t count;                /*   8  compares that failed                                                   */
+    uint64_t last;                 /*  16  ... of them in the last iteration                                      */
+    uint64_t fold_x, fold_s, fold_w;   /*  24  the last iteration's results v = out[0] + 2 out[1] + 4 out[2]:
+                                             xor, sum, sum of v * (2 op + 1)                                        */
+} cro_alu_thread;                  /*  48 bytes */
+
+/* What thread 0 of a CTA publishes at the end of a launch. */
+typedef struct cro_alu_cta {
+    uint64_t stamp;                /*   0  the call number k; any other value: the CTA did not publish            */
+    uint64_t t0, t1;               /*   8  %globaltimer around the iterations                                     */
+    uint64_t cycles;               /*  24  %clock64 around the iterations                                         */
+    uint32_t smid;                 /*  32 */
+    uint32_t nsmid;                /*  36 */
+    uint32_t block;                /*  40  blockIdx.x                                                             */
+    uint32_t reserved;             /*  44 */
+} cro_alu_cta;                     /*  48 bytes */
+
+/* sms[0 .. sms_cap) receives one entry per SM seen, by SM id (*n_sms how many); faults[0 .. cap) the records sorted
+ * by (leg, smid, iteration, op, warp, lane) (*n how many).  opts may be NULL: defaults.  cro_probe_alu: dev_index is
+ * an in-process device.  cro_probe_alu_uuid runs `croprobe-cli alu-raw` (a fresh cuInit that sees only that GPU)
+ * with a fresh seed base. */
+int  cro_probe_alu(cro_ctx *ctx, int dev_index, const cro_alu_opts *opts, cro_alu_result *out, cro_alu_sm *sms,
+                   int sms_cap, int *n_sms, cro_alu_fault *faults, int cap, int *n);
+int  cro_probe_alu_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_alu_opts *opts, cro_alu_result *out,
+                        cro_alu_sm *sms, int sms_cap, int *n_sms, cro_alu_fault *faults, int cap, int *n);
+
+/* The table of a call of seed `seed` for leg `leg` and warp `warp` (0 .. 7): out[op * 32 + lane], CRO_ALU_*_OPS ops.
+ * Host arithmetic, no GPU.  CRO_ERR_INVALID_ARG for a leg or warp out of range or a NULL out. */
+int  cro_alu_expected(int leg, uint64_t seed, int warp, cro_alu_record *out);
+
+/* Test hook: the probe's classification of call `call` (seed, iterations) on a device of sm_count SMs from
+ * caller-given launches, as cro_selftest_xlane_classify does for the cross-lane probe (ctas, threads by block then
+ * thread, CRO_ALU_THREAD_RECORDS records per thread; the folds are checked against the closed form of the seed's
+ * table).  Returns out->status (CRO_ERR_UNSUPPORTED with a blanked result for a %nsmid above CRO_ALU_MAX_SMS), or
+ * CRO_ERR_INVALID_ARG for a NULL array it needs, a negative cap, sm_count 0, legs out of range, or iterations 0 or
+ * above CRO_ALU_MAX_ITERATIONS. */
+int  cro_selftest_alu_classify(uint32_t legs, uint32_t iterations, uint64_t seed, uint32_t sm_count, uint64_t call,
+                               uint32_t rounds, const cro_alu_cta *ctas, const cro_alu_thread *threads,
+                               const cro_alu_fault *records, cro_alu_result *out, cro_alu_sm *sms, int sms_cap,
+                               int *n_sms, cro_alu_fault *faults, int cap, int *n);
+
+/* Additive ALU annotations (cohdi.io/probe-alu-*) of a cro_probe_alu / cro_probe_alu_uuid result, the same
+ * Go-marshalled map and keys as the cross-lane probe's: -verdict, -sms, -bad-sms, -legs (logic, shift, iadd, imul,
+ * float) and -iterations. */
+int  cro_emit_alu_annotations_json(const cro_alu_result *r, char *buf, size_t cap, size_t *len);
+
 /* ---- L2:the L2 cache, the crossbar between the SMs and its slices, and the L2 atomic units ---- */
 
 /*
