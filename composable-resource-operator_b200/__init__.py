@@ -739,6 +739,85 @@ assert ctypes.sizeof(AluOpts) == 56 and ctypes.sizeof(AluResult) == 568 and ctyp
     and ctypes.sizeof(AluCta) == 48, ctypes.sizeof(AluResult)
 
 
+# Barrier probe (cro_probe_barrier, cro_probe_barrier_uuid, cro_barrier_expected, cro_selftest_barrier_classify)
+BARRIER_LEG_BAR, BARRIER_LEG_MBAR, BARRIER_LEG_CLUSTER = range(3)
+BARRIER_LEGS, BARRIER_ALL_LEGS, BARRIER_THREADS, BARRIER_WARPS, BARRIER_THREAD_RECORDS = 3, 0x7, 256, 8, 4
+BARRIER_RECORDS, BARRIER_MAX_SMS, BARRIER_MAX_ITERATIONS, BARRIER_MAX_ROUNDS, BARRIER_MAX_PAIRS = 4096, 256, 65536, 64, 16
+BARRIER_BAR_OPS, BARRIER_MBAR_OPS, BARRIER_CLUSTER_OPS, BARRIER_MAX_OPS = 64, 8, 17, 64
+BARRIER_OPS = [BARRIER_BAR_OPS, BARRIER_MBAR_OPS, BARRIER_CLUSTER_OPS]
+BARRIER_WAIT_NS = 20000000
+(BARRIER_FORM_POPC, BARRIER_FORM_AND, BARRIER_FORM_OR, BARRIER_FORM_ARRIVE, BARRIER_FORM_TICKET, BARRIER_FORM_COUNT,
+ BARRIER_FORM_DROP, BARRIER_FORM_TX, BARRIER_FORM_CBAR, BARRIER_FORM_ST_B32, BARRIER_FORM_ST_B64, BARRIER_FORM_ST_V2,
+ BARRIER_FORM_ST_V4, BARRIER_FORM_RED_ADD, BARRIER_FORM_RED_ADD64, BARRIER_FORM_RED_MIN, BARRIER_FORM_RED_MAX,
+ BARRIER_FORM_RED_MINS, BARRIER_FORM_RED_MAXS, BARRIER_FORM_RED_AND, BARRIER_FORM_RED_OR, BARRIER_FORM_RED_XOR,
+ BARRIER_FORM_RED_INC, BARRIER_FORM_RED_DEC) = range(24)
+BARRIER_KIND_VALUE, BARRIER_KIND_EARLY, BARRIER_KIND_TICKET, BARRIER_KIND_TIMEOUT = range(4)
+BARRIER_NONE, BARRIER_SM, BARRIER_ALL, BARRIER_LINK = 0, 1, 2, 3
+BARRIER_PERSISTENT, BARRIER_INTERMITTENT = 1, 2
+
+
+class BarrierOpts(ctypes.Structure):
+    _fields_ = [("iterations", ctypes.c_uint32), ("legs", ctypes.c_uint32), ("max_rounds", ctypes.c_uint32),
+                ("deadline_ms", ctypes.c_int32), ("cluster", ctypes.c_uint32), ("test_inject_leg", ctypes.c_int32),
+                ("test_inject_sm", ctypes.c_int32), ("test_inject_warp", ctypes.c_int32), ("test_inject_lane", ctypes.c_int32),
+                ("test_inject_op", ctypes.c_uint32), ("test_inject_iteration", ctypes.c_uint32), ("reserved", ctypes.c_uint32),
+                ("test_inject_mask", ctypes.c_uint64)]
+
+
+class BarrierPair(ctypes.Structure):
+    _fields_ = [("smid", ctypes.c_uint16), ("peer_smid", ctypes.c_uint16)]
+
+
+class BarrierResult(ctypes.Structure):
+    """cro_barrier_result: the cross-lane result's counts for three legs, the cluster size, the kept timeout records,
+    the CLUSTER leg's coverage and failed (SM, peer SM) pairs, times and the host's table build time."""
+    _fields_ = XlaneResult._fields_[:21] + [("cluster", ctypes.c_uint32)] + [
+        ("mismatches", ctypes.c_uint64 * 3), ("ops_checked", ctypes.c_uint64 * 3), ("fold_mismatches", ctypes.c_uint64 * 3),
+        ("leg_ns", ctypes.c_uint64 * 3), ("fold", (ctypes.c_uint64 * 3) * 3), ("expect", (ctypes.c_uint64 * 3) * 3),
+        ("timeouts", ctypes.c_uint64), ("cluster_sms", ctypes.c_uint32), ("bad_pairs", ctypes.c_uint32),
+        ("bad_pair", BarrierPair * 16), ("ns", ctypes.c_uint64), ("timer_ns", ctypes.c_uint64), ("wall_ns", ctypes.c_uint64),
+        ("helper_ns", ctypes.c_uint64), ("table_ns", ctypes.c_uint64)]
+
+
+class BarrierSm(ctypes.Structure):
+    """One SM seen by a barrier probe call: its failed legs, per-leg counts, fold mismatches, times and mark."""
+    _fields_ = [("smid", ctypes.c_uint32), ("mark", ctypes.c_uint32), ("failed_legs", ctypes.c_uint32), ("ctas", ctypes.c_uint32),
+                ("mismatches", ctypes.c_uint64 * 3), ("fold_mismatches", ctypes.c_uint64), ("ns", ctypes.c_uint64),
+                ("cycles", ctypes.c_uint64)]
+
+
+class BarrierRow(ctypes.Structure):
+    """cro_barrier_row: one row of the table."""
+    _fields_ = [("form", ctypes.c_uint32), ("bar", ctypes.c_uint32), ("count", ctypes.c_uint32), ("warps", ctypes.c_uint32),
+                ("producers", ctypes.c_uint32), ("phases", ctypes.c_uint32), ("held", ctypes.c_uint32), ("arriver", ctypes.c_uint32),
+                ("expect", ctypes.c_uint64), ("pred", ctypes.c_uint32 * 8), ("next_rank", ctypes.c_uint8 * 8),
+                ("slot_init", ctypes.c_uint64 * 8), ("slot_expect", ctypes.c_uint64 * 8)]
+
+
+class BarrierFault(ctypes.Structure):
+    """One failed check: leg, row, iteration, SM, warp, lane, kind, barrier id (or form), phase, slot, peer SM,
+    expected and actual."""
+    _fields_ = [("leg", ctypes.c_uint32), ("op", ctypes.c_uint32), ("iteration", ctypes.c_uint32), ("smid", ctypes.c_uint32),
+                ("warp", ctypes.c_uint32), ("lane", ctypes.c_uint32), ("kind", ctypes.c_uint32), ("bar", ctypes.c_uint32),
+                ("phase", ctypes.c_uint32), ("slot", ctypes.c_uint32), ("peer_smid", ctypes.c_uint32), ("reserved", ctypes.c_uint32),
+                ("expected", ctypes.c_uint64), ("actual", ctypes.c_uint64)]
+
+
+class BarrierThread(ctypes.Structure):
+    """cro_barrier_thread: what one thread of the barrier probe publishes at the end of a launch."""
+    _fields_ = XlaneThread._fields_
+
+
+class BarrierCta(ctypes.Structure):
+    """cro_barrier_cta: what thread 0 of a CTA of the barrier probe publishes at the end of a launch."""
+    _fields_ = XlaneCta._fields_
+
+
+assert ctypes.sizeof(BarrierOpts) == 56 and ctypes.sizeof(BarrierResult) == 488 and ctypes.sizeof(BarrierSm) == 64 \
+    and ctypes.sizeof(BarrierRow) == 208 and ctypes.sizeof(BarrierFault) == 64 and ctypes.sizeof(BarrierThread) == 48 \
+    and ctypes.sizeof(BarrierCta) == 48, ctypes.sizeof(BarrierResult)
+
+
 # L2 probe (cro_probe_l2, cro_read_l2_health, cro_selftest_l2_classify)
 L2_BLOCK_BYTES, L2_MIN_BYTES, L2_MAX_L2_MULTIPLE, L2_ELEMENTS, L2_RECORDS, L2_MAX_SMS = 16384, 1 << 20, 8, 6, 4096, 256
 L2_MAX_ITERATIONS, L2_MAX_A1_COUNTERS, L2_MAX_A2_COUNTERS, L2_MAX_LINES, L2_MAX_COUNTERS = 256, 1 << 20, 8192, 8, 8
@@ -953,6 +1032,8 @@ EXPORTS = [
     "cro_probe_xlane", "cro_probe_xlane_uuid", "cro_xlane_expected", "cro_emit_xlane_annotations_json",
     "cro_selftest_xlane_classify",
     "cro_probe_alu", "cro_probe_alu_uuid", "cro_alu_expected", "cro_emit_alu_annotations_json", "cro_selftest_alu_classify",
+    "cro_probe_barrier", "cro_probe_barrier_uuid", "cro_barrier_expected", "cro_emit_barrier_annotations_json",
+    "cro_selftest_barrier_classify",
     "cro_probe_l2", "cro_probe_l2_uuid", "cro_read_l2_health", "cro_emit_l2_annotations_json", "cro_selftest_l2_classify",
     "cro_selftest_sm_legs_classify", "cro_selftest_sram_classify",
     "cro_selftest_locate_collect", "cro_selftest_scan_collect", "cro_selftest_link_classify",
@@ -1148,6 +1229,16 @@ def _load() -> ctypes.CDLL:
         "cro_selftest_alu_classify": (i32, [u32, u32, u64, u32, u64, u32, ctypes.POINTER(AluCta), ctypes.POINTER(AluThread),
                                             ctypes.POINTER(AluFault), ctypes.POINTER(AluResult), ctypes.POINTER(AluSm), i32,
                                             ctypes.POINTER(i32), ctypes.POINTER(AluFault), i32, ctypes.POINTER(i32)]),
+        "cro_probe_barrier": (i32, [vp, i32, ctypes.POINTER(BarrierOpts), ctypes.POINTER(BarrierResult), ctypes.POINTER(BarrierSm),
+                                    i32, ctypes.POINTER(i32), ctypes.POINTER(BarrierFault), i32, ctypes.POINTER(i32)]),
+        "cro_probe_barrier_uuid": (i32, [vp, c, ctypes.POINTER(BarrierOpts), ctypes.POINTER(BarrierResult), ctypes.POINTER(BarrierSm),
+                                         i32, ctypes.POINTER(i32), ctypes.POINTER(BarrierFault), i32, ctypes.POINTER(i32)]),
+        "cro_barrier_expected": (i32, [i32, u64, u32, ctypes.POINTER(BarrierRow), ctypes.POINTER(u64)]),
+        "cro_emit_barrier_annotations_json": (i32, [ctypes.POINTER(BarrierResult)] + out),
+        "cro_selftest_barrier_classify": (i32, [u32, u32, u64, u32, u32, u64, u32, ctypes.POINTER(BarrierCta),
+                                                ctypes.POINTER(BarrierThread), ctypes.POINTER(BarrierFault),
+                                                ctypes.POINTER(BarrierResult), ctypes.POINTER(BarrierSm), i32, ctypes.POINTER(i32),
+                                                ctypes.POINTER(BarrierFault), i32, ctypes.POINTER(i32)]),
         "cro_probe_l2": (i32, [vp, i32, ctypes.POINTER(L2Opts), ctypes.POINTER(L2Result), ctypes.POINTER(L2Sm), i32,
                                ctypes.POINTER(i32), ctypes.POINTER(L2Fault), i32, ctypes.POINTER(i32)]),
         "cro_probe_l2_uuid": (i32, [vp, c, ctypes.POINTER(L2Opts), ctypes.POINTER(L2Result), ctypes.POINTER(L2Sm), i32,
@@ -1420,6 +1511,40 @@ def selftest_alu_classify(legs: int, iterations: int, seed: int, sm_count: int, 
                       AluResult, AluSm, ALU_MAX_SMS, AluFault, cap)
     if rc not in (OK, ERR_CHECKSUM, ERR_UNSUPPORTED):
         raise ProbeError(rc, "cro_selftest_alu_classify")
+    return out
+
+
+def emit_barrier_annotations_json(r: BarrierResult) -> str:
+    """Additive cohdi.io/probe-barrier-* annotations of a barrier probe result (Go-marshalled map[string]string)."""
+    return _text(lib.cro_emit_barrier_annotations_json, ctypes.byref(r))
+
+
+def barrier_expected(leg: int, seed: int, cluster: int = 2) -> Tuple[List[BarrierRow], List[int]]:
+    """cro_barrier_expected: the table of a call of seed `seed` for leg `leg` (cluster: the CLUSTER leg's cluster
+    size): its rows and its words, indexed (row * 256 + thread) * 2 + j (host arithmetic, no GPU)."""
+    rows = (BarrierRow * BARRIER_OPS[leg])()
+    words = (ctypes.c_uint64 * (BARRIER_OPS[leg] * BARRIER_THREADS * 2))()
+    rc = lib.cro_barrier_expected(leg, seed, cluster, rows, words)
+    if rc != OK:
+        raise ProbeError(rc, "cro_barrier_expected")
+    return list(rows), list(words)
+
+
+def selftest_barrier_classify(legs: int, iterations: int, seed: int, cluster: int, sm_count: int, call: int, rounds,
+                              cap: Optional[int] = None):
+    """cro_selftest_barrier_classify: the barrier probe's classification of call `call`, as selftest_xlane_classify
+    with BarrierCta, BarrierThread and BarrierFault.  Returns (result, SM entries, faults)."""
+    n_rounds = len(rounds[0]) if rounds else 0
+    assert all(len(r) == n_rounds for r in rounds)
+    flat = [rnd for leg in rounds for rnd in leg]
+    ctas = (BarrierCta * max(1, sm_count * len(flat)))(*[x for rnd in flat for x in rnd[0]])
+    thr = (BarrierThread * max(1, sm_count * BARRIER_THREADS * len(flat)))(*[x for rnd in flat for x in rnd[1]])
+    recs = (BarrierFault * max(1, sm_count * BARRIER_THREADS * BARRIER_THREAD_RECORDS * len(flat)))(*[x for rnd in flat for x in rnd[2]])
+    cap = BARRIER_RECORDS if cap is None else cap
+    rc, out = _per_sm(lib.cro_selftest_barrier_classify, (legs, iterations, seed, cluster, sm_count, call, n_rounds, ctas, thr, recs),
+                      BarrierResult, BarrierSm, BARRIER_MAX_SMS, BarrierFault, cap)
+    if rc not in (OK, ERR_CHECKSUM, ERR_UNSUPPORTED):
+        raise ProbeError(rc, "cro_selftest_barrier_classify")
     return out
 
 
@@ -1704,6 +1829,30 @@ def probe_alu_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: int = 0
     o = _alu_opts(iterations, legs, max_rounds, deadline_ms, inject)
     handle = ctx.handle if ctx is not None else None
     rc, out = _per_sm(lib.cro_probe_alu_uuid, (handle, _b(uuid), ctypes.byref(o)), AluResult, AluSm, ALU_MAX_SMS, AluFault, cap)
+    if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
+        raise _helper_error(rc, handle)
+    return out
+
+
+def _barrier_opts(iterations: int, legs: int, max_rounds: int, cluster: int, deadline_ms: int,
+                  inject: Optional[Tuple[int, int, int, int, int, int, int]]) -> BarrierOpts:
+    o = BarrierOpts()
+    o.iterations, o.legs, o.max_rounds, o.cluster, o.deadline_ms = iterations, legs, max_rounds, cluster, deadline_ms
+    if inject is not None:
+        (o.test_inject_leg, o.test_inject_sm, o.test_inject_warp, o.test_inject_lane, o.test_inject_op, o.test_inject_iteration,
+         o.test_inject_mask) = inject
+    return o
+
+
+def probe_barrier_uuid(ctx: Optional["ProbeContext"], uuid: str, iterations: int = 0, legs: int = 0, max_rounds: int = 0,
+                       cluster: int = 0, deadline_ms: int = 0, inject: Optional[Tuple[int, int, int, int, int, int, int]] = None,
+                       cap: int = 256) -> Tuple[BarrierResult, List[BarrierSm], List[BarrierFault]]:
+    """cro_probe_barrier_uuid: the barrier probe of any GPU on the node, run by the helper process (ctx may be None).
+    Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up to `cap` records."""
+    o = _barrier_opts(iterations, legs, max_rounds, cluster, deadline_ms, inject)
+    handle = ctx.handle if ctx is not None else None
+    rc, out = _per_sm(lib.cro_probe_barrier_uuid, (handle, _b(uuid), ctypes.byref(o)), BarrierResult, BarrierSm, BARRIER_MAX_SMS,
+                      BarrierFault, cap)
     if rc not in (OK, ERR_CHECKSUM, ERR_CUDA):
         raise _helper_error(rc, handle)
     return out
@@ -2344,6 +2493,20 @@ class ProbeContext:
         ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up to `cap` records."""
         o = _alu_opts(iterations, legs, max_rounds, 0, inject)
         rc, out = _per_sm(lib.cro_probe_alu, (self.handle, dev, ctypes.byref(o)), AluResult, AluSm, ALU_MAX_SMS, AluFault, cap)
+        self._check(rc, allow=(ERR_CHECKSUM, ERR_CUDA))
+        return out
+
+    def probe_barrier(self, dev: int = 0, iterations: int = 0, legs: int = 0, max_rounds: int = 0, cluster: int = 0,
+                      inject: Optional[Tuple[int, int, int, int, int, int, int]] = None,
+                      cap: int = 256) -> Tuple[BarrierResult, List[BarrierSm], List[BarrierFault]]:
+        """cro_probe_barrier: one CTA of 8 warps per SM runs every row of the legs run (legs = 0: all) on the host's
+        table: named barriers, mbarrier phases and transaction counts, and (clusters of `cluster`, 0: 2) cluster
+        barriers with async remote stores.  iterations / max_rounds = 0: the defaults.  inject = (leg, sm, warp, lane,
+        row, iteration, mask) is the test-only XOR into every value that row compares (sm, warp, lane: -1 for every one).
+        Returns the result (its status is OK, ERR_CHECKSUM or ERR_CUDA), one entry per SM seen and up to `cap` records."""
+        o = _barrier_opts(iterations, legs, max_rounds, cluster, 0, inject)
+        rc, out = _per_sm(lib.cro_probe_barrier, (self.handle, dev, ctypes.byref(o)), BarrierResult, BarrierSm, BARRIER_MAX_SMS,
+                          BarrierFault, cap)
         self._check(rc, allow=(ERR_CHECKSUM, ERR_CUDA))
         return out
 

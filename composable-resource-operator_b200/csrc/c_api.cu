@@ -104,6 +104,13 @@ static_assert(sizeof(cro_alu_opts) == 56 && offsetof(cro_alu_opts, test_inject_m
                   sizeof(cro_alu_record) == 64 && sizeof(cro_alu_fault) == 112 && offsetof(cro_alu_fault, in) == 32 &&
                   offsetof(cro_alu_fault, actual) == 88 && sizeof(cro_alu_thread) == 48 && sizeof(cro_alu_cta) == 48,
               "alu layout");
+static_assert(sizeof(cro_barrier_opts) == 56 && offsetof(cro_barrier_opts, test_inject_mask) == 48 && sizeof(cro_barrier_result) == 488 &&
+                  offsetof(cro_barrier_result, mismatches) == 128 && offsetof(cro_barrier_result, timeouts) == 368 &&
+                  offsetof(cro_barrier_result, bad_pair) == 384 && offsetof(cro_barrier_result, table_ns) == 480 &&
+                  sizeof(cro_barrier_sm) == 64 && sizeof(cro_barrier_row) == 208 && offsetof(cro_barrier_row, slot_expect) == 144 &&
+                  sizeof(cro_barrier_fault) == 64 && offsetof(cro_barrier_fault, expected) == 48 && sizeof(cro_barrier_thread) == 48 &&
+                  sizeof(cro_barrier_cta) == 48,
+              "barrier layout");
 static_assert(sizeof(cro_l2_opts) == 56 && sizeof(cro_l2_health) == 48 && sizeof(cro_l2_sm) == 128 && sizeof(cro_l2_fault) == 56 &&
                   sizeof(cro_l2_result) == 616 && offsetof(cro_l2_result, mismatches) == 80 &&
                   offsetof(cro_l2_result, bad_line) == 184 && offsetof(cro_l2_result, a1_bad) == 312 &&
@@ -633,6 +640,38 @@ int cro_selftest_alu_classify(uint32_t legs, uint32_t iterations, uint64_t seed,
     std::vector<cro_alu_sm> seen;
     std::vector<cro_alu_fault> found;
     const int rc = classify_alu(legs, iterations, seed, sm_count, call, rounds, ctas, threads, records, out, &seen, &found);
+    return listed({rc, true, copy_capped(seen, sms, sms_cap, n_sms), copy_capped(found, faults, cap, n)}, out);
+} CRO_API_CATCH
+int cro_probe_barrier(cro_ctx* ctx, int i, const cro_barrier_opts* opts, cro_barrier_result* out, cro_barrier_sm* sms, int sms_cap,
+                      int* n_sms, cro_barrier_fault* faults, int cap, int* n) try {
+    return listed(per_sm_call(ctx, out, opts, sms, sms_cap, n_sms, faults, cap, n, [&](const cro_barrier_opts& o, auto* seen, auto* found) {
+        return ctx_probe_barrier(ctx, i, o, out, seen, found);
+    }), out);
+} CRO_API_CATCH
+int cro_probe_barrier_uuid(cro_ctx* ctx, const char* gpu_uuid, const cro_barrier_opts* opts, cro_barrier_result* out, cro_barrier_sm* sms,
+                           int sms_cap, int* n_sms, cro_barrier_fault* faults, int cap, int* n) try {
+    return listed(per_sm_call(gpu_uuid, out, opts, sms, sms_cap, n_sms, faults, cap, n,
+                              [&](const cro_barrier_opts& o, auto* seen, auto* found) {
+                                  return ctx_probe_barrier_uuid(ctx, gpu_uuid, o, out, seen, found, cap);
+                              }), out);
+} CRO_API_CATCH
+int cro_barrier_expected(int leg, uint64_t seed, uint32_t cluster, cro_barrier_row* rows, uint64_t* words) try {
+    if (leg < 0 || leg >= CRO_BARRIER_LEGS || (cluster != 2 && cluster != 4 && cluster != 8) || !rows || !words) return CRO_ERR_INVALID_ARG;
+    barrier_expected((unsigned)leg, seed, cluster, rows, words);
+    return CRO_OK;
+} CRO_API_CATCH
+int cro_selftest_barrier_classify(uint32_t legs, uint32_t iterations, uint64_t seed, uint32_t cluster, uint32_t sm_count, uint64_t call,
+                                  uint32_t rounds, const cro_barrier_cta* ctas, const cro_barrier_thread* threads,
+                                  const cro_barrier_fault* records, cro_barrier_result* out, cro_barrier_sm* sms, int sms_cap, int* n_sms,
+                                  cro_barrier_fault* faults, int cap, int* n) try {
+    if (legs == 0 || legs > CRO_BARRIER_ALL_LEGS || iterations == 0 || iterations > CRO_BARRIER_MAX_ITERATIONS || sm_count == 0 ||
+        (cluster != 2 && cluster != 4 && cluster != 8) || (rounds && (!ctas || !threads || !records)) || !out || !n_sms || !n ||
+        sms_cap < 0 || cap < 0 || (sms_cap > 0 && !sms) || (cap > 0 && !faults))
+        return CRO_ERR_INVALID_ARG;
+    *n = *n_sms = 0;
+    std::vector<cro_barrier_sm> seen;
+    std::vector<cro_barrier_fault> found;
+    const int rc = classify_barrier(legs, iterations, seed, cluster, sm_count, call, rounds, ctas, threads, records, out, &seen, &found);
     return listed({rc, true, copy_capped(seen, sms, sms_cap, n_sms), copy_capped(found, faults, cap, n)}, out);
 } CRO_API_CATCH
 int cro_probe_l2(cro_ctx* ctx, int i, const cro_l2_opts* opts, cro_l2_result* out, cro_l2_sm* sms, int sms_cap, int* n_sms,
@@ -1304,6 +1343,19 @@ static Annotations alu_annotations(const cro_alu_result& r) {
     return lane_annotations(r, "cohdi.io/probe-alu-", kLegs, CRO_ALU_LEGS, CRO_ALU_SM, CRO_ALU_ALL);
 }
 
+// The cross-lane probe's keys under cohdi.io/probe-barrier-, "link" for a LINK verdict, and the failed pairs.
+static Annotations barrier_annotations(const cro_barrier_result& r) {
+    static const char* const kLegs[CRO_BARRIER_LEGS] = {"bar", "mbar", "cluster"};
+    const std::string p = "cohdi.io/probe-barrier-";
+    Annotations m = lane_annotations(r, p, kLegs, CRO_BARRIER_LEGS, CRO_BARRIER_SM, CRO_BARRIER_ALL);
+    if (r.status == CRO_ERR_CHECKSUM && r.verdict == CRO_BARRIER_LINK) m[p + "verdict"] = "link";
+    std::string pairs;
+    for (uint32_t i = 0; i < std::min<uint32_t>(r.bad_pairs, CRO_BARRIER_MAX_PAIRS); ++i)
+        pairs += (pairs.empty() ? "" : ",") + std::to_string(r.bad_pair[i].smid) + ">" + std::to_string(r.bad_pair[i].peer_smid);
+    put_list(m, p + "bad-pairs", pairs);
+    return m;
+}
+
 static Annotations l2_annotations(const cro_l2_result& r) {
     static const char* const kHealth[6] = {"sram-corrected", "sram-uncorrected", "l2-corrected", "l2-uncorrected",
                                            "threshold-exceeded", "l2-bucket"};
@@ -1463,6 +1515,11 @@ int cro_emit_xlane_annotations_json(const cro_xlane_result* r, char* buf, size_t
 int cro_emit_alu_annotations_json(const cro_alu_result* r, char* buf, size_t cap, size_t* len) try {
     if (!r) return CRO_ERR_INVALID_ARG;
     return emit(alu_annotations(*r), buf, cap, len);
+} CRO_API_CATCH
+
+int cro_emit_barrier_annotations_json(const cro_barrier_result* r, char* buf, size_t cap, size_t* len) try {
+    if (!r) return CRO_ERR_INVALID_ARG;
+    return emit(barrier_annotations(*r), buf, cap, len);
 } CRO_API_CATCH
 
 int cro_emit_l2_annotations_json(const cro_l2_result* r, char* buf, size_t cap, size_t* len) try {

@@ -80,6 +80,12 @@
  *                                                    cro_alu_result, CRO_ALU_MAX_SMS cro_alu_sm entries (sms_listed of
  *                                                    them filled) and its `recorded` cro_alu_fault records (at most
  *                                                    cap) on stdout
+ *   croprobe-cli barrier-raw <uuid> <seed_base> <iterations> <legs> <max_rounds> <cluster> <inject_leg> <inject_sm>
+ *                            <inject_warp> <inject_lane> <inject_op> <inject_iteration> <inject_mask> <cap>
+ *                                                    the barrier probe with every cro_barrier_opts field but the
+ *                                                    deadline; cro_barrier_result, CRO_BARRIER_MAX_SMS cro_barrier_sm
+ *                                                    entries (sms_listed of them filled) and its `recorded`
+ *                                                    cro_barrier_fault records (at most cap) on stdout
  *   croprobe-cli health-raw <uuid> <seed_base> <checks> <compute-raw's options and cap> <precision-raw's> <sram-raw's>
  *                           <l2-raw's> <link-raw's> <scan-raw's>
  *                                                    the health check (cro_check_health) with every option of every
@@ -87,7 +93,7 @@
  *                                                    the seed base), its sweep region L, NVML on; the cro_health_result,
  *                                                    then each check that ran, in run order, as its own -raw writes it
  *   croprobe-cli health <uuid|index>                 the health check with defaults; JSON annotations, exit 0 iff ok
- *   link-raw, compute-raw, precision-raw, sparse-raw, warpmma-raw, l2-raw, regfile-raw, xlane-raw, alu-raw and health-raw take
+ *   link-raw, compute-raw, precision-raw, sparse-raw, warpmma-raw, l2-raw, regfile-raw, xlane-raw, alu-raw, barrier-raw and health-raw take
  *   cro_opts.seed_base from argv (the device seed is seed_base | minor, as in process), so that the library can give
  *   every helper call fresh patterns and operands; their counts are the helper's own, because neither result says how many records follow.
  * Exit 3: the device is not visible to this (fresh) process — the reference's found=false.  The raw commands exit 0
@@ -279,6 +285,18 @@ static int alu_raw(cro_ctx *ctx, int idx, char **argv) {
     return put_frame(&cro_wire_alu.frame, &ar, sms, (uint64_t)n_sms, faults, (uint64_t)got) ? 2 : end_frames(ar.status);
 }
 
+static int barrier_raw(cro_ctx *ctx, int idx, char **argv) {
+    static cro_barrier_opts bo;
+    const int cap = raw_opts(&cro_wire_barrier, argv, &bo);
+    static cro_barrier_result br;
+    static cro_barrier_sm sms[CRO_BARRIER_MAX_SMS];
+    cro_barrier_fault *faults = (cro_barrier_fault *)calloc(cap > 0 ? (size_t)cap : 1, sizeof *faults);
+    int n_sms = 0, got = 0;
+    if (!faults) return 2;
+    cro_probe_barrier(ctx, idx, &bo, &br, sms, CRO_BARRIER_MAX_SMS, &n_sms, faults, cap > 0 ? cap : 0, &got);
+    return put_frame(&cro_wire_barrier.frame, &br, sms, (uint64_t)n_sms, faults, (uint64_t)got) ? 2 : end_frames(br.status);
+}
+
 /* `scan`: the whole-HBM scan of the free memory (all of it but 1 GiB unless argv[3], in MiB, bounds it) as JSON. */
 static int scan_json(cro_ctx *ctx, int idx, char **argv) {
     cro_scan_opts so;
@@ -387,6 +405,7 @@ static const struct command {
     {NULL, &cro_wire_regfile, CRO_F_LAZY_ALLOC, 64, regfile_raw},
     {NULL, &cro_wire_xlane, CRO_F_LAZY_ALLOC, 64, xlane_raw},
     {NULL, &cro_wire_alu, CRO_F_LAZY_ALLOC, 64, alu_raw},
+    {NULL, &cro_wire_barrier, CRO_F_LAZY_ALLOC, 64, barrier_raw},
     /* a region of exactly L, the link's bytes (the probe checks L <= S; no halving on a full GPU), and NVML for the
      * replay counters */
     {NULL, &cro_wire_link, CRO_F_LAZY_ALLOC, 256, link_raw},
@@ -417,6 +436,8 @@ int main(int argc, char **argv) {
                         "xlane-raw <uuid> <seed_base> <iterations> <legs> <rounds> <leg> <sm> <warp> <lane> <op> <iteration> <mask> <cap> | "
                         "alu-raw <uuid> <seed_base> <iterations> <legs> <rounds> <leg> <sm> <warp> <lane> <op> <iteration> <operand> <mask> "
                         "<cap> | "
+                        "barrier-raw <uuid> <seed_base> <iterations> <legs> <rounds> <cluster> <leg> <sm> <warp> <lane> <op> <iteration> "
+                        "<mask> <cap> | "
                         "health-raw <uuid> <seed_base> <checks> <compute-raw, precision-raw, sram-raw, l2-raw, link-raw, scan-raw options "
                         "and caps> | health <uuid|index>\n");
         return 64;

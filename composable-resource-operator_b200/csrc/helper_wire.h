@@ -240,6 +240,26 @@ static const cro_wire cro_wire_alu = {"alu-raw", 1, CRO_WIRE_FIELDS(cro_wire_alu
                                       {sizeof(cro_alu_result), 0, sizeof(cro_alu_sm), CRO_ALU_MAX_SMS, sizeof(cro_alu_fault),
                                        CRO_WIRE_AT(cro_alu_result, sms_listed), CRO_WIRE_AT(cro_alu_result, recorded)}};
 
+static const cro_wire_field cro_wire_barrier_fields[] = {
+    CRO_WIRE_FIELD(cro_barrier_opts, iterations),
+    CRO_WIRE_FIELD(cro_barrier_opts, legs),
+    CRO_WIRE_FIELD(cro_barrier_opts, max_rounds),
+    CRO_WIRE_FIELD(cro_barrier_opts, cluster),
+    CRO_WIRE_FIELD(cro_barrier_opts, test_inject_leg),
+    CRO_WIRE_FIELD(cro_barrier_opts, test_inject_sm),
+    CRO_WIRE_FIELD(cro_barrier_opts, test_inject_warp),
+    CRO_WIRE_FIELD(cro_barrier_opts, test_inject_lane),
+    CRO_WIRE_FIELD(cro_barrier_opts, test_inject_op),
+    CRO_WIRE_FIELD(cro_barrier_opts, test_inject_iteration),
+    CRO_WIRE_FIELD(cro_barrier_opts, test_inject_mask),
+};
+/* The barrier frame: the result, then CRO_BARRIER_MAX_SMS cro_barrier_sm entries (sms_listed of them filled) and
+ * `recorded` cro_barrier_fault records. */
+static const cro_wire cro_wire_barrier = {"barrier-raw", 1, CRO_WIRE_FIELDS(cro_wire_barrier_fields),
+                                          {sizeof(cro_barrier_result), 0, sizeof(cro_barrier_sm), CRO_BARRIER_MAX_SMS,
+                                           sizeof(cro_barrier_fault), CRO_WIRE_AT(cro_barrier_result, sms_listed),
+                                           CRO_WIRE_AT(cro_barrier_result, recorded)}};
+
 /* health-raw: <uuid> <seed_base> <checks>, then each check's fields and cap in run order (the CRO_HEALTH_* bit order).
  * Its stdout: the cro_health_result, then the frame of each check that ran, in run order.  opts_at and result_at:
  * where the check's options and result are in cro_health_opts and cro_health_result. */

@@ -88,6 +88,7 @@ struct Device {
     uint64_t warpmma_calls = 0;            // k of the next warp-MMA probe call (ctx_probe_warpmma): its operand seed
     uint64_t xlane_calls = 0;              // k of the next cross-lane probe call (ctx_probe_xlane): its seeds
     uint64_t alu_calls = 0;                // k of the next ALU probe call (ctx_probe_alu): its table's seed
+    uint64_t barrier_calls = 0;            // k of the next barrier probe call (ctx_probe_barrier): its table's seed
     KernelPlan plan{};
     SweepScratch scratch{}, scratch_aux{}, scratch_pfx{};   // main stream / closed form / p2p prefix closed form
     // lane 0's buffers under their old names: the synchronous probe, the single sweeps and cro_probe_all use lane 0
@@ -446,6 +447,20 @@ void alu_expected(unsigned leg, uint64_t seed, unsigned warp, cro_alu_record* ou
 int classify_alu(uint32_t legs, uint32_t iterations, uint64_t seed, uint32_t sm_count, uint64_t k, uint32_t rounds,
                  const cro_alu_cta* ctas, const cro_alu_thread* threads, const cro_alu_fault* records, cro_alu_result* r,
                  std::vector<cro_alu_sm>* sms, std::vector<cro_alu_fault>* faults);
+
+// Barrier probe (include/croprobe.h, cro_probe_barrier / cro_probe_barrier_uuid, barrier_probe.cu): *sms gets one entry
+// per SM seen, by SM id; *faults the records, by (leg, smid, iteration, op, warp, lane), at most CRO_BARRIER_RECORDS.
+// The uuid form runs `croprobe-cli barrier-raw` with a fresh seed base and asks it for at most cap records.
+std::string barrier_opts_error(const cro_barrier_opts& o);
+int ctx_probe_barrier(cro_ctx* c, int idx, const cro_barrier_opts& o, cro_barrier_result* r, std::vector<cro_barrier_sm>* sms,
+                      std::vector<cro_barrier_fault>* faults);
+int ctx_probe_barrier_uuid(cro_ctx* c, const char* uuid, const cro_barrier_opts& o, cro_barrier_result* r,
+                           std::vector<cro_barrier_sm>* sms, std::vector<cro_barrier_fault>* faults, int cap);
+// cro_barrier_expected and cro_selftest_barrier_classify.
+void barrier_expected(unsigned leg, uint64_t seed, uint32_t cluster, cro_barrier_row* rows, uint64_t* words);
+int classify_barrier(uint32_t legs, uint32_t iterations, uint64_t seed, uint32_t cluster, uint32_t sm_count, uint64_t k, uint32_t rounds,
+                     const cro_barrier_cta* ctas, const cro_barrier_thread* threads, const cro_barrier_fault* records,
+                     cro_barrier_result* r, std::vector<cro_barrier_sm>* sms, std::vector<cro_barrier_fault>* faults);
 
 // L2 probe (include/croprobe.h, cro_probe_l2, l2_probe.cu): *sms gets one entry per SM seen, by SM id; *faults every
 // recorded word, by (word, iteration, element, smid).

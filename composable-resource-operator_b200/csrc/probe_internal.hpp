@@ -44,14 +44,14 @@ uint64_t fresh_seed();
 inline Params imm_params(const Device* d) { return Params{ProbeParams{d->seed_cur, d->nonce_cur}, nullptr}; }
 
 // The seed spaces of a device: seed j of call k in a space is seed_dev + offset + (per_call * k + j) * kNonceStride.
-// No seed of one space is a seed of another while every count per_call * k + j stays below 2^53.  kNonceStride is
+// No seed of one space is a seed of another while every count per_call * k + j stays below 2^52.  kNonceStride is
 // odd, hence invertible mod 2^64, so seeds of offsets O != O' and counts n, n' are equal only when (n - n') *
-// kNonceStride = O' - O (mod 2^64).  Every offset is 0 or a power of two from 2^53 up, so O' - O is a nonzero multiple
-// of 2^53 mod 2^64, and so is n - n' (an odd factor keeps the power of two in a number): n or n' is at least 2^53.  The
-// largest per_call, the register-file probe's 65536, keeps its counts 65536 k + j below 2^53 while k < 2^37.
+// kNonceStride = O' - O (mod 2^64).  Every offset is 0 or a power of two from 2^52 up, so O' - O is a nonzero multiple
+// of 2^52 mod 2^64, and so is n - n' (an odd factor keeps the power of two in a number): n or n' is at least 2^52.  The
+// largest per_call, the register-file probe's 65536, keeps its counts 65536 k + j below 2^52 while k < 2^36.
 // Within a space distinct counts give distinct seeds, so no call passes on what an earlier call left behind.
 enum SeedSpace { kSeedNonce, kSeedRetest, kSeedLink, kSeedCompute, kSeedSram, kSeedL2, kSeedPrecision, kSeedSparse, kSeedRegfile,
-                 kSeedWarpMma, kSeedXlane, kSeedAlu };
+                 kSeedWarpMma, kSeedXlane, kSeedAlu, kSeedBarrier };
 struct SeedSpaceInfo {
     uint64_t offset, per_call;
 };
@@ -68,6 +68,7 @@ constexpr SeedSpaceInfo kSeedSpaces[] = {
     {1ull << 55, 1},    // kSeedWarpMma: warp-MMA probe operands and MOVE tile
     {1ull << 54, CRO_XLANE_MAX_ITERATIONS},     // kSeedXlane: cross-lane probe, one per iteration
     {1ull << 53, 1},    // kSeedAlu: ALU probe table, one per call (every iteration repeats it)
+    {1ull << 52, 1},    // kSeedBarrier: barrier probe table, one per call (every iteration repeats it)
 };
 inline uint64_t space_seed(const Device* d, SeedSpace s, uint64_t k, uint64_t j = 0) {
     return d->seed_dev + kSeedSpaces[s].offset + (kSeedSpaces[s].per_call * k + j) * kNonceStride;

@@ -1100,6 +1100,76 @@ func (c *Context) ProbeAluByUUID(deviceID string) (r AluResult, found bool, err 
 	return r, true, nil
 }
 
+// BarrierResult is the summary of cro_barrier_result an operator reads: whether
+// every SM's named barriers, mbarrier phases and transaction counts, and cluster
+// barriers with async remote stores behaved exactly, and which SMs, legs and
+// (SM, peer SM) pairs did not.
+type BarrierResult struct {
+	Status      int32  // CRO_OK, CRO_ERR_CHECKSUM or CRO_ERR_CUDA
+	CudaError   int32  // cudaError_t of a failed launch (CRO_ERR_CUDA)
+	Verdict     uint32 // CRO_BARRIER_NONE / _SM / _ALL / _LINK
+	FailedLegs  uint32 // bit per CRO_BARRIER_LEG_* that failed
+	SMCount     uint32
+	Covered     uint32
+	Timeouts    uint64      // mbarrier waits that ran out, among the kept records
+	BadSMs      []uint32    // SMs that failed, ascending (at most 16)
+	BadPairs    [][2]uint32 // (SM, peer SM) of the failed CLUSTER records (at most 16)
+	Faults      []BarrierFault
+	Annotations string // Go-marshalled map[string]string of cohdi.io/probe-barrier-* keys
+}
+
+// BarrierFault is one failed check (cro_barrier_fault): the leg and row, where
+// it ran, its kind, barrier id or form, phase and slot, and the expected and
+// actual values.
+type BarrierFault struct {
+	Leg, Op, Iteration, SM, Warp, Lane, Kind, Bar, Phase, Slot, PeerSM uint32
+	Expected, Actual                                                   uint64
+}
+
+// ProbeBarrierByUUID runs cro_probe_barrier_uuid with its defaults: the
+// barrier probe of any GPU on the node through the helper process, whose
+// deadline contains a barrier that never releases (INTEGRATION.md "The barrier
+// probe").  A mismatch or a fault (CRO_ERR_CUDA) is a result, not an error;
+// found is false when the node does not list the GPU.
+func (c *Context) ProbeBarrierByUUID(deviceID string) (r BarrierResult, found bool, err error) {
+	id := C.CString(deviceID)
+	defer C.free(unsafe.Pointer(id))
+	var res C.cro_barrier_result
+	sms := make([]C.cro_barrier_sm, C.CRO_BARRIER_MAX_SMS)
+	var faults [256]C.cro_barrier_fault
+	var nSMs, got C.int
+	rc := C.cro_probe_barrier_uuid(c.h, id, nil, &res, &sms[0], C.CRO_BARRIER_MAX_SMS, &nSMs, &faults[0], 256, &got)
+	if rc == C.CRO_ERR_NO_DEVICE {
+		return r, false, nil
+	}
+	if rc != C.CRO_OK && rc != C.CRO_ERR_CHECKSUM && rc != C.CRO_ERR_CUDA {
+		return r, true, errorOf(c.h, rc)
+	}
+	r = BarrierResult{Status: int32(res.status), CudaError: int32(res.cuda_error), Verdict: uint32(res.verdict),
+		FailedLegs: uint32(res.failed_legs), SMCount: uint32(res.sm_count), Covered: uint32(res.sms_covered),
+		Timeouts: uint64(res.timeouts)}
+	for i := 0; i < int(res.bad_sms) && i < 16; i++ {
+		r.BadSMs = append(r.BadSMs, uint32(res.bad_sm[i]))
+	}
+	for i := 0; i < int(res.bad_pairs) && i < 16; i++ {
+		r.BadPairs = append(r.BadPairs, [2]uint32{uint32(res.bad_pair[i].smid), uint32(res.bad_pair[i].peer_smid)})
+	}
+	for i := 0; i < int(got); i++ {
+		f := faults[i]
+		r.Faults = append(r.Faults, BarrierFault{Leg: uint32(f.leg), Op: uint32(f.op), Iteration: uint32(f.iteration),
+			SM: uint32(f.smid), Warp: uint32(f.warp), Lane: uint32(f.lane), Kind: uint32(f.kind), Bar: uint32(f.bar),
+			Phase: uint32(f.phase), Slot: uint32(f.slot), PeerSM: uint32(f.peer_smid), Expected: uint64(f.expected),
+			Actual: uint64(f.actual)})
+	}
+	buf := (*C.char)(C.malloc(4096))
+	defer C.free(unsafe.Pointer(buf))
+	var ln C.size_t
+	if C.cro_emit_barrier_annotations_json(&res, buf, 4096, &ln) == C.CRO_OK {
+		r.Annotations = C.GoStringN(buf, C.int(ln))
+	}
+	return r, true, nil
+}
+
 // L2Result is the summary of cro_l2_result an operator reads: whether the
 // L2-resident buffer held what each SM wrote when another SM read it back,
 // whether the L2 atomic units gave the right answers, which SMs, buffer offsets

@@ -2132,6 +2132,267 @@ int  cro_selftest_alu_classify(uint32_t legs, uint32_t iterations, uint64_t seed
  * float) and -iterations. */
 int  cro_emit_alu_annotations_json(const cro_alu_result *r, char *buf, size_t cap, size_t *len);
 
+/* ---- Barrier: every SM's named barriers, mbarrier unit (SYNCS) and cluster barriers with async remote stores ---- */
+
+/*
+ * Every pipelined kernel orders its shared-memory stages through the SM's barrier hardware: bar.sync between stages,
+ * mbarrier phases and transaction counts under every TMA ring and warp-specialised producer/consumer loop, and
+ * barrier.cluster with st.async / red.async across a cluster.  A transaction count that goes wrong, a phase that
+ * completes early or a named barrier that releases before every thread arrived lets a consumer read a tile before it
+ * landed: silent corruption blamed on the memory, or a hang.  The barrier probe checks these units on one CTA of 8
+ * warps per SM (one cluster of CTAs for the CLUSTER leg), every check exact and independent of the order the threads
+ * ran in.
+ *
+ * The host builds one table per call from the call's seed (seed = seed_dev + 2^52 + k * 0xD1B54A32D192ED03): per leg
+ * and row a cro_barrier_row (barrier id, thread count, participating warps, predicates, counts, held-back thread,
+ * expected results) and per (row, thread) two words (producer words, arrival counts, byte pieces, stored values,
+ * reduction operands).  cro_barrier_expected returns it.  Every iteration repeats it; the device computes no expected
+ * value.  Legs (DESIGN.md "The barrier probe" lists each row's checks in device order):
+ *   BAR      64 rows, all 16 named-barrier ids: bar.red.popc.u32, bar.red.and.pred and bar.red.or.pred over 32 .. 256
+ *            threads of seeded warp subsets and predicate rows (all, none, a walking one, a walking zero, seeded), and
+ *            bar.arrive producers against bar.sync consumers, each consumer reading every producer's shared word.
+ *   MBAR     8 rows on a freshly initialised mbarrier: arrive.noComplete tickets (pending_count, as a set N+1 .. 2),
+ *            arrive with seeded counts over K consecutive phases, arrive_drop, arrive.expect_tx with complete_tx split
+ *            over several warps.  test_wait.parity must be false while one arrival or byte piece is held back, true
+ *            for the preceding phase, and try_wait.parity true once it is delivered.
+ *   CLUSTER  17 rows across a cluster (2, 4 or 8 CTAs): barrier.cluster.arrive.release / wait.acquire with shared
+ *            words read on the next rank through mapa (and getctarank of the mapped address); st.async .b32 .b64
+ *            .v2.b32 .v4.b32 and red.async add.u32 add.u64 min/max .u32/.s32 and or xor inc dec into the next rank,
+ *            each completing bytes on its mbarrier, whose expect_tx is the exact byte total.
+ * Every mbarrier wait is a try_wait loop bounded by CRO_BARRIER_WAIT_NS of %globaltimer: on expiry it records a
+ * CRO_BARRIER_KIND_TIMEOUT and goes on.  bar.sync, bar.red and barrier.cluster.wait cannot be bounded: a broken
+ * barrier unit can hang the in-process form; the helper form's deadline kills it.  The report path is the
+ * cross-lane probe's (plain stores, no barrier, vote or atomic).
+ *
+ * Verdict: CRO_BARRIER_ALL when every covered SM failed or an entry was not published; CRO_BARRIER_LINK when only
+ * CLUSTER checks failed (bad_pair names each (SM, peer SM) pair); CRO_BARRIER_SM otherwise.  status: CRO_ERR_CHECKSUM
+ * on any mismatch, fold mismatch or entry not published; CRO_ERR_CUDA when a launch failed.
+ */
+#define CRO_BARRIER_LEG_BAR          0
+#define CRO_BARRIER_LEG_MBAR         1
+#define CRO_BARRIER_LEG_CLUSTER      2
+#define CRO_BARRIER_LEGS             3
+#define CRO_BARRIER_ALL_LEGS         0x7u
+#define CRO_BARRIER_THREADS          256     /* threads per CTA: 8 warps                                     */
+#define CRO_BARRIER_WARPS            8
+#define CRO_BARRIER_THREAD_RECORDS   4       /* records each thread keeps                                    */
+#define CRO_BARRIER_RECORDS          4096    /* records a result holds; counts stay exact beyond             */
+#define CRO_BARRIER_MAX_SMS          256     /* SM ids the results hold; a larger %nsmid fails the call      */
+#define CRO_BARRIER_MAX_ITERATIONS   65536
+#define CRO_BARRIER_MAX_ROUNDS       64
+#define CRO_BARRIER_MAX_PAIRS        16
+#define CRO_BARRIER_BAR_OPS          64      /* rows per leg                                                 */
+#define CRO_BARRIER_MBAR_OPS         8
+#define CRO_BARRIER_CLUSTER_OPS      17
+#define CRO_BARRIER_MAX_OPS          64
+#define CRO_BARRIER_WAIT_NS          20000000ull   /* %globaltimer budget of one mbarrier wait: 20 ms, each
+                                                        step of the wait counting at most 1 ms                */
+
+/* cro_barrier_row.form */
+#define CRO_BARRIER_FORM_POPC        0       /* BAR: bar.red.popc.u32                                        */
+#define CRO_BARRIER_FORM_AND         1       /* BAR: bar.red.and.pred                                        */
+#define CRO_BARRIER_FORM_OR          2       /* BAR: bar.red.or.pred                                         */
+#define CRO_BARRIER_FORM_ARRIVE      3       /* BAR: bar.arrive producers, bar.sync consumers                */
+#define CRO_BARRIER_FORM_TICKET      4       /* MBAR: arrive.noComplete tickets                              */
+#define CRO_BARRIER_FORM_COUNT       5       /* MBAR: arrive with seeded counts over K phases                */
+#define CRO_BARRIER_FORM_DROP        6       /* MBAR: arrive_drop, then a phase with fewer arrivals          */
+#define CRO_BARRIER_FORM_TX          7       /* MBAR: arrive.expect_tx and complete_tx pieces over K phases  */
+#define CRO_BARRIER_FORM_CBAR        8       /* CLUSTER: barrier.cluster, mapa reads, getctarank             */
+#define CRO_BARRIER_FORM_ST_B32      9       /* CLUSTER: st.async ... the forms below, in this order         */
+#define CRO_BARRIER_FORM_ST_B64      10
+#define CRO_BARRIER_FORM_ST_V2       11
+#define CRO_BARRIER_FORM_ST_V4       12
+#define CRO_BARRIER_FORM_RED_ADD     13      /* red.async add.u32                                            */
+#define CRO_BARRIER_FORM_RED_ADD64   14      /* add.u64                                                      */
+#define CRO_BARRIER_FORM_RED_MIN     15      /* min.u32                                                      */
+#define CRO_BARRIER_FORM_RED_MAX     16      /* max.u32                                                      */
+#define CRO_BARRIER_FORM_RED_MINS    17      /* min.s32                                                      */
+#define CRO_BARRIER_FORM_RED_MAXS    18      /* max.s32                                                      */
+#define CRO_BARRIER_FORM_RED_AND     19      /* and.b32                                                      */
+#define CRO_BARRIER_FORM_RED_OR      20      /* or.b32                                                       */
+#define CRO_BARRIER_FORM_RED_XOR     21      /* xor.b32                                                      */
+#define CRO_BARRIER_FORM_RED_INC     22      /* inc.u32, one bound no sum reaches                            */
+#define CRO_BARRIER_FORM_RED_DEC     23      /* dec.u32, from a start no count reaches 0 from                */
+
+/* cro_barrier_fault.kind */
+#define CRO_BARRIER_KIND_VALUE       0u      /* a reduction result, a word read or received, a wait's result */
+#define CRO_BARRIER_KIND_EARLY       1u      /* a barrier or phase that released before every thread arrived:
+                                                a stale producer word, or test_wait true while a piece is held */
+#define CRO_BARRIER_KIND_TICKET      2u      /* a pending_count ticket out of range or shared with a thread  */
+#define CRO_BARRIER_KIND_TIMEOUT     3u      /* an mbarrier wait ran out of CRO_BARRIER_WAIT_NS               */
+
+#define CRO_BARRIER_NONE             0u
+#define CRO_BARRIER_SM               1u      /* a strict subset of the covered SMs failed a CTA-local leg    */
+#define CRO_BARRIER_ALL              2u      /* every covered SM failed, or an entry was not published        */
+#define CRO_BARRIER_LINK             3u      /* only CLUSTER checks failed: bad_pair names the pairs          */
+
+#define CRO_BARRIER_PERSISTENT       1u      /* cro_barrier_sm.mark: a check of the last iteration failed     */
+#define CRO_BARRIER_INTERMITTENT     2u      /* only an earlier iteration failed, or only the fold            */
+
+typedef struct cro_barrier_opts {
+    uint32_t iterations;           /*   0  per CTA and leg: 0 = the default (DESIGN.md), at most MAX_ITERATIONS   */
+    uint32_t legs;                 /*   4  bit per CRO_BARRIER_LEG_*: 0 = all                                      */
+    uint32_t max_rounds;           /*   8  launches per leg while fewer than sm_count SMs took part: 0 = 4         */
+    int32_t  deadline_ms;          /*  12  cro_probe_barrier_uuid: the helper's deadline; 0 = CRO_HELPER_TIMEOUT_MS */
+    uint32_t cluster;              /*  16  CTAs per cluster of the CLUSTER leg: 0 = 2; 2, 4 or 8                    */
+    /* test only: with test_inject_mask != 0, the mask is XORed into every value row test_inject_op of leg
+       test_inject_leg compares in thread (test_inject_warp, test_inject_lane) of the CTA on SM test_inject_sm in
+       iteration test_inject_iteration (-1: every SM, warp or lane), after the instruction and before the compare.
+       It never adds or skips an arrival and never changes a count or a byte total. */
+    int32_t  test_inject_leg;      /*  20 */
+    int32_t  test_inject_sm;       /*  24 */
+    int32_t  test_inject_warp;     /*  28 */
+    int32_t  test_inject_lane;     /*  32 */
+    uint32_t test_inject_op;       /*  36 */
+    uint32_t test_inject_iteration;/*  40 */
+    uint32_t reserved;             /*  44 */
+    uint64_t test_inject_mask;     /*  48 */
+} cro_barrier_opts;                /*  56 bytes */
+
+typedef struct cro_barrier_pair {
+    uint16_t smid;                 /*   0  the SM whose check failed                                              */
+    uint16_t peer_smid;            /*   2  the SM of the cluster rank it read from or received from               */
+} cro_barrier_pair;                /*   4 bytes */
+
+typedef struct cro_barrier_result {
+    int32_t  status;               /*   0  the return value                                                      */
+    uint32_t verdict;              /*   4  CRO_BARRIER_NONE / _SM / _ALL / _LINK                                  */
+    uint64_t seed;                 /*   8  seed of this call's table                                             */
+    uint64_t call;                 /*  16  k: the call's number on this device, from 0                          */
+    uint32_t sm_count;             /*  24  multiprocessors the device reports                                    */
+    uint32_t nsmid;                /*  28  %nsmid as the kernel reads it                                         */
+    int32_t  cuda_error;           /*  32  cudaError_t of the launch that failed; 0: none                        */
+    uint32_t legs;                 /*  36  legs run                                                              */
+    uint32_t iterations;           /*  40  per CTA and leg                                                       */
+    uint32_t rounds;               /*  44  launches, over every leg                                              */
+    uint32_t sms_covered;          /*  48  distinct SMs that ran a CTA, in the BAR or MBAR leg run that saw the
+                                              fewest (the CLUSTER leg's when only it ran; its own is cluster_sms) */
+    uint32_t complete;             /*  52  1: sms_covered >= sm_count                                            */
+    uint32_t ctas;                 /*  56  CTAs launched                                                         */
+    uint32_t unpublished;          /*  60  CTAs launched that published no record                               */
+    uint32_t threads_unpublished;  /*  64  threads of published CTAs that published no entry                    */
+    uint32_t failed_sms;           /*  68  distinct SMs with a mark                                              */
+    uint32_t bad_sms;              /*  72  = failed_sms                                                          */
+    uint32_t failed_legs;          /*  76  bit per leg with a mismatch, fold mismatch or unpublished entry       */
+    uint16_t bad_sm[16];           /*  80  the first 16 failed SMs, ascending                                    */
+    uint64_t recorded;             /* 112  records written to the caller's list (*n)                            */
+    uint32_t sms_listed;           /* 120  entries written to the caller's per-SM list                          */
+    uint32_t cluster;              /* 124  CTAs per cluster of the CLUSTER leg (its rounds end at max_rounds or
+                                              at the first round that reaches no new SM)                          */
+    uint64_t mismatches[CRO_BARRIER_LEGS];       /* 128  checks that failed, per leg, exact                    */
+    uint64_t ops_checked[CRO_BARRIER_LEGS];      /* 152  rows run: rows * 256 threads * iterations per CTA     */
+    uint64_t fold_mismatches[CRO_BARRIER_LEGS];  /* 176  CTAs whose fold differs from the closed form          */
+    uint64_t leg_ns[CRO_BARRIER_LEGS];           /* 200  CUDA events around each leg's launches                */
+    uint64_t fold[CRO_BARRIER_LEGS][3];          /* 224  (xor, sum, weighted sum) of the lowest SM id's CTA     */
+    uint64_t expect[CRO_BARRIER_LEGS][3];        /* 296  the closed form every CTA's fold must equal            */
+    uint64_t timeouts;             /* 368  CRO_BARRIER_KIND_TIMEOUT records the threads kept (before the cap)   */
+    uint32_t cluster_sms;          /* 376  distinct SMs the CLUSTER leg covered                                 */
+    uint32_t bad_pairs;            /* 380  distinct (SM, peer SM) pairs of the CLUSTER records the threads kept
+                                              (before the CRO_BARRIER_RECORDS cap)                                */
+    cro_barrier_pair bad_pair[CRO_BARRIER_MAX_PAIRS];   /* 384  the first 16, ascending                        */
+    uint64_t ns;                   /* 448  CUDA events around the launches, summed                              */
+    uint64_t timer_ns;             /* 456  %globaltimer: first CTA start .. last CTA end, summed over rounds     */
+    uint64_t wall_ns;              /* 464  the whole call                                                       */
+    uint64_t helper_ns;            /* 472  cro_probe_barrier_uuid: spawn of the helper to its exit; 0 in process */
+    uint64_t table_ns;             /* 480  building the call's table on the host (part of wall_ns)              */
+} cro_barrier_result;              /* 488 bytes */
+
+typedef struct cro_barrier_sm {
+    uint32_t smid;                 /*   0 */
+    uint32_t mark;                 /*   4  0, CRO_BARRIER_PERSISTENT or CRO_BARRIER_INTERMITTENT                  */
+    uint32_t failed_legs;          /*   8  bit per leg that failed on this SM                                    */
+    uint32_t ctas;                 /*  12  CTAs that ran on this SM, over every leg                              */
+    uint64_t mismatches[CRO_BARRIER_LEGS];   /*  16 */
+    uint64_t fold_mismatches;      /*  40 */
+    uint64_t ns;                   /*  48  %globaltimer windows of this SM's CTAs, summed                       */
+    uint64_t cycles;               /*  56  %clock64 cycles of the same CTAs, summed                             */
+} cro_barrier_sm;                  /*  64 bytes */
+
+/* One row of the table.  Which fields a form reads is listed in DESIGN.md "The barrier probe"; unused fields are 0. */
+typedef struct cro_barrier_row {
+    uint32_t form;                 /*   0  CRO_BARRIER_FORM_*                                                    */
+    uint32_t bar;                  /*   4  BAR: the named barrier id                                             */
+    uint32_t count;                /*   8  BAR: threads at the barrier; MBAR: the mbarrier's init count;
+                                              CLUSTER async: the byte total the receiver expects                  */
+    uint32_t warps;                /*  12  bit per participating warp (ARRIVE: the consumers)                    */
+    uint32_t producers;            /*  16  ARRIVE: bit per producer warp                                         */
+    uint32_t phases;               /*  20  MBAR: consecutive phases                                              */
+    uint32_t held;                 /*  24  MBAR: the thread whose arrival or byte piece is held back              */
+    uint32_t arriver;              /*  28  TX: the thread that arrives with expect_tx; RED: the slots reduced into */
+    uint64_t expect;               /*  32  POPC: the count; AND / OR: 0 or 1                                     */
+    uint32_t pred[8];              /*  40  BAR reductions: bit per thread                                        */
+    uint8_t  next_rank[8];         /*  72  CBAR: getctarank of the next rank's address, per rank                 */
+    uint64_t slot_init[8];         /*  80  RED: each slot's value before the reductions                          */
+    uint64_t slot_expect[8];       /* 144  RED: each slot's value after them                                     */
+} cro_barrier_row;                 /* 208 bytes */
+
+typedef struct cro_barrier_fault {
+    uint32_t leg;                  /*   0  CRO_BARRIER_LEG_*                                                     */
+    uint32_t op;                   /*   4  the row                                                               */
+    uint32_t iteration;            /*   8 */
+    uint32_t smid;                 /*  12 */
+    uint32_t warp;                 /*  16 */
+    uint32_t lane;                 /*  20 */
+    uint32_t kind;                 /*  24  CRO_BARRIER_KIND_*                                                    */
+    uint32_t bar;                  /*  28  BAR: the named barrier id; else the row's form                        */
+    uint32_t phase;                /*  32  MBAR: the phase within the row; else 0                                */
+    uint32_t slot;                 /*  36  which check of the row: the producer thread read, the slot, the wait  */
+    uint32_t peer_smid;            /*  40  CLUSTER: the SM of the rank read from or received from; else smid    */
+    uint32_t reserved;             /*  44 */
+    uint64_t expected;             /*  48 */
+    uint64_t actual;               /*  56 */
+} cro_barrier_fault;               /*  64 bytes */
+
+/* What one thread publishes at the end of a launch, with plain stores. */
+typedef struct cro_barrier_thread {
+    uint64_t stamp;                /*   0  the call number k; any other value: the thread did not publish         */
+    uint64_t count;                /*   8  checks that failed                                                     */
+    uint64_t last;                 /*  16  ... of them in the last iteration                                      */
+    uint64_t fold_x, fold_s, fold_w;   /*  24  the last iteration's checked values v: xor, sum, sum of v * (2 op + 1) */
+} cro_barrier_thread;              /*  48 bytes */
+
+/* What thread 0 of a CTA publishes at the end of a launch. */
+typedef struct cro_barrier_cta {
+    uint64_t stamp;                /*   0  the call number k; any other value: the CTA did not publish            */
+    uint64_t t0, t1;               /*   8  %globaltimer around the iterations                                     */
+    uint64_t cycles;               /*  24  %clock64 around the iterations                                         */
+    uint32_t smid;                 /*  32 */
+    uint32_t nsmid;                /*  36 */
+    uint32_t block;                /*  40  blockIdx.x                                                             */
+    uint32_t reserved;             /*  44 */
+} cro_barrier_cta;                 /*  48 bytes */
+
+/* sms[0 .. sms_cap) receives one entry per SM seen, by SM id (*n_sms how many); faults[0 .. cap) the records sorted
+ * by (leg, smid, iteration, op, warp, lane) (*n how many).  opts may be NULL: defaults.  cro_probe_barrier: dev_index
+ * is an in-process device.  cro_probe_barrier_uuid runs `croprobe-cli barrier-raw` (a fresh cuInit that sees only
+ * that GPU) with a fresh seed base. */
+int  cro_probe_barrier(cro_ctx *ctx, int dev_index, const cro_barrier_opts *opts, cro_barrier_result *out,
+                       cro_barrier_sm *sms, int sms_cap, int *n_sms, cro_barrier_fault *faults, int cap, int *n);
+int  cro_probe_barrier_uuid(cro_ctx *ctx, const char *gpu_uuid, const cro_barrier_opts *opts, cro_barrier_result *out,
+                            cro_barrier_sm *sms, int sms_cap, int *n_sms, cro_barrier_fault *faults, int cap, int *n);
+
+/* The table of a call of seed `seed` for leg `leg` (cluster: the CLUSTER leg's cluster size, 2, 4 or 8):
+ * rows[0 .. CRO_BARRIER_*_OPS) and words[(row * 256 + thread) * 2 + j].  Host arithmetic, no GPU.
+ * CRO_ERR_INVALID_ARG for a leg or cluster out of range or a NULL array. */
+int  cro_barrier_expected(int leg, uint64_t seed, uint32_t cluster, cro_barrier_row *rows, uint64_t *words);
+
+/* Test hook: the probe's classification of call `call` (seed, iterations, cluster) on a device of sm_count SMs from
+ * caller-given launches, as cro_selftest_xlane_classify does for the cross-lane probe (ctas, threads by block then
+ * thread, CRO_BARRIER_THREAD_RECORDS records per thread; the folds are checked against the closed form of the seed's
+ * table), then the LINK pairs.  Returns out->status (CRO_ERR_UNSUPPORTED with a blanked result for a %nsmid above
+ * CRO_BARRIER_MAX_SMS), or CRO_ERR_INVALID_ARG for a NULL array it needs, a negative cap, sm_count 0, legs or cluster
+ * out of range, or iterations 0 or above CRO_BARRIER_MAX_ITERATIONS. */
+int  cro_selftest_barrier_classify(uint32_t legs, uint32_t iterations, uint64_t seed, uint32_t cluster, uint32_t sm_count,
+                                   uint64_t call, uint32_t rounds, const cro_barrier_cta *ctas,
+                                   const cro_barrier_thread *threads, const cro_barrier_fault *records,
+                                   cro_barrier_result *out, cro_barrier_sm *sms, int sms_cap, int *n_sms,
+                                   cro_barrier_fault *faults, int cap, int *n);
+
+/* Additive barrier annotations (cohdi.io/probe-barrier-*) of a cro_probe_barrier / cro_probe_barrier_uuid result, the
+ * cross-lane probe's keys (-verdict, with "link" for CRO_BARRIER_LINK; -sms, -bad-sms, -legs: bar, mbar, cluster;
+ * -iterations) and -bad-pairs ("sm>peer", comma-separated; only when any). */
+int  cro_emit_barrier_annotations_json(const cro_barrier_result *r, char *buf, size_t cap, size_t *len);
+
 /* ---- L2:the L2 cache, the crossbar between the SMs and its slices, and the L2 atomic units ---- */
 
 /*
