@@ -1020,6 +1020,7 @@ EXPORTS = [
     "cro_selftest_exception_barrier", "cro_probe_sweep_times", "cro_p2p_detail_get", "cro_fullbox_times",
     "cro_chase_end", "cro_validate_env", "cro_node_inventory", "cro_probe_uuid", "cro_set_latency_hops", "cro_local_exec", "cro_metrics_text", "cro_describe_wire_type",
     "cro_selftest_probe_finalize", "cro_selftest_p2p_finalize", "cro_selftest_chase", "cro_selftest_sweep",
+    "cro_selftest_p2p_plan",
     "cro_locate_faults", "cro_emit_fault_annotations_json",
     "cro_probe_host_link", "cro_probe_host_link_uuid", "cro_pci_link_path", "cro_emit_link_annotations_json",
     "cro_probe_compute", "cro_probe_compute_uuid", "cro_compute_expected", "cro_emit_compute_annotations_json",
@@ -1068,6 +1069,50 @@ SLOT_FILL, SLOT_SWEEP0, MAX_SWEEPS_EACH, SLOT_EXPECT, SLOT_PREFIX, SLOT_P2P0 = 0
 SLOT_SCRATCH = SLOT_P2P0 + 3 * MAX_DEVICES
 SLOT_COUNT = SLOT_SCRATCH + 4
 SLOT_BYTES = 64
+
+# test hook: the full-box probe's schedule (cro_selftest_p2p_plan)
+P2P_PLAN_OPS, P2P_PLAN_ROUNDS = 4096, 16
+P2P_OP_HBM, P2P_OP_PREFIX, P2P_OP_RECORD, P2P_OP_WAIT, P2P_OP_READ, P2P_OP_PUSH, P2P_OP_REREAD, P2P_OP_CHASE, \
+    P2P_OP_FINALIZE = range(1, 10)
+P2P_EV_HBM, P2P_EV_PUSH, P2P_EV_REREAD, P2P_EV_CHASE = range(1, 5)
+
+
+class P2POp(ctypes.Structure):
+    """cro_p2p_op: one stream operation of the full-box plan."""
+    _fields_ = [("kind", ctypes.c_uint8), ("dev", ctypes.c_uint8), ("peer", ctypes.c_uint8), ("event", ctypes.c_uint8),
+                ("round", ctypes.c_uint16), ("slot", ctypes.c_uint16), ("bytes", ctypes.c_uint64)]
+
+
+class P2PFinalizePlan(ctypes.Structure):
+    """cro_p2p_finalize_plan: one device's p2p_finalize arguments other than pointers, and the peers it checks and chases."""
+    _fields_ = [("n", ctypes.c_uint32), ("self", ctypes.c_uint32), ("have_push", ctypes.c_uint32),
+                ("push_folded", ctypes.c_uint32), ("p2p_bytes", ctypes.c_uint64), ("peer_mask", ctypes.c_uint32),
+                ("chase_mask", ctypes.c_uint32)]
+
+
+class P2PPlan(ctypes.Structure):
+    """cro_p2p_plan: what cro_probe_all enqueues, in order."""
+    _fields_ = [("p2p_bytes", ctypes.c_uint64), ("n_rounds", ctypes.c_uint32), ("n_ops", ctypes.c_uint32),
+                ("n_pairs", ctypes.c_uint8 * P2P_PLAN_ROUNDS), ("pair", (ctypes.c_uint8 * MAX_DEVICES) * P2P_PLAN_ROUNDS),
+                ("fin", P2PFinalizePlan * MAX_DEVICES), ("op", P2POp * P2P_PLAN_OPS)]
+
+
+assert ctypes.sizeof(P2POp) == 16 and ctypes.sizeof(P2PFinalizePlan) == 32 and ctypes.sizeof(P2PPlan) == 66336
+
+
+def selftest_p2p_plan(sweep_bytes: List[int], p2p_bytes: int, access: List[List[int]], flags: int = 0, unidir: bool = False,
+                      write_variant: int = 3) -> P2PPlan:
+    """cro_selftest_p2p_plan: the plan cro_probe_all walks on len(sweep_bytes) devices of those sizes, access[i] being
+    device i's 8 p2p_access bytes, with cro_opts.flags `flags`, the CRO_P2P_UNIDIR knob and CRO_P2P_WRITE_VARIANT."""
+    n = len(sweep_bytes)
+    assert len(access) == n and all(len(row) == 8 for row in access)
+    out = P2PPlan()
+    rc = lib.cro_selftest_p2p_plan(n, (ctypes.c_uint64 * max(1, n))(*sweep_bytes), p2p_bytes,
+                                   (ctypes.c_uint8 * max(8, 8 * n))(*[v for row in access for v in row]), flags, int(unidir),
+                                   write_variant, ctypes.byref(out))
+    if rc != OK:
+        raise ProbeError(rc, "cro_selftest_p2p_plan")
+    return out
 
 
 def _load() -> ctypes.CDLL:
@@ -1147,6 +1192,8 @@ def _load() -> ctypes.CDLL:
                                             ctypes.POINTER(u64), ctypes.POINTER(u32), u32, u32, u32, u32, u32, u64, u64]),
         "cro_selftest_chase": (i32, [vp, i32, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), u32, u32,
                                      ctypes.POINTER(u64)]),
+        "cro_selftest_p2p_plan": (i32, [u32, ctypes.POINTER(u64), u64, ctypes.POINTER(ctypes.c_uint8), u32, u32, u32,
+                                        ctypes.POINTER(P2PPlan)]),
         "cro_selftest_sweep": (i32, [vp, i32, ctypes.POINTER(SelftestSweepOpts), ctypes.POINTER(SelftestSweepOut), vp, u64,
                                      ctypes.POINTER(FaultWord), i32, ctypes.POINTER(i32)]),
         "cro_locate_faults": (i32, [vp, i32, ctypes.POINTER(LocateOpts), ctypes.POINTER(FaultReport), ctypes.POINTER(FaultWord),

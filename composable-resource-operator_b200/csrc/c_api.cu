@@ -262,6 +262,10 @@ int cro_selftest_chase(cro_ctx* ctx, int i, const int32_t* minor_src, const int3
                        uint64_t* out) try {
     return ctx ? ctx_selftest_chase(ctx, i, minor_src, minor_dst, n, hops, out) : CRO_ERR_INVALID_ARG;
 } CRO_API_CATCH
+int cro_selftest_p2p_plan(uint32_t n, const uint64_t* sweep_bytes, uint64_t p2p_bytes, const uint8_t* access, uint32_t flags,
+                          uint32_t unidir, uint32_t write_variant, cro_p2p_plan* out) try {
+    return selftest_p2p_plan(n, sweep_bytes, p2p_bytes, access, flags, unidir, write_variant, out);
+} CRO_API_CATCH
 int cro_selftest_sweep(cro_ctx* ctx, int i, const cro_selftest_sweep_opts* opts, cro_selftest_sweep_out* out, void* buf,
                        uint64_t cap_bytes, cro_fault_word* words, int cap, int* n) try {
     return ctx ? ctx_selftest_sweep(ctx, i, opts, out, buf, cap_bytes, words, cap, n) : CRO_ERR_INVALID_ARG;

@@ -130,6 +130,127 @@ int load_nccl(cro_ctx* c) {
     return CRO_OK;
 }
 
+// One stream operation of the full-box plan, and one device's p2p_finalize arguments other than pointers;
+// cro_p2p_op and cro_p2p_finalize_plan are their public mirrors (cro_selftest_p2p_plan hands them over as they are).
+struct P2POp {
+    uint8_t kind, dev, peer, event;   // CRO_P2P_OP_*, the stream's device, the other device, CRO_P2P_EV_*
+    uint16_t round, slot;
+    uint64_t bytes;
+};
+struct P2PFinalizePlan {
+    uint32_t n, self, have_push, push_folded;
+    uint64_t p2p_bytes;
+    uint32_t peer_mask, chase_mask;
+};
+static_assert(sizeof(cro_p2p_op) == sizeof(P2POp) && offsetof(cro_p2p_op, kind) == offsetof(P2POp, kind) &&
+                  offsetof(cro_p2p_op, dev) == offsetof(P2POp, dev) && offsetof(cro_p2p_op, peer) == offsetof(P2POp, peer) &&
+                  offsetof(cro_p2p_op, event) == offsetof(P2POp, event) && offsetof(cro_p2p_op, round) == offsetof(P2POp, round) &&
+                  offsetof(cro_p2p_op, slot) == offsetof(P2POp, slot) && offsetof(cro_p2p_op, bytes) == offsetof(P2POp, bytes),
+              "cro_p2p_op mirrors P2POp");
+static_assert(sizeof(cro_p2p_finalize_plan) == sizeof(P2PFinalizePlan) &&
+                  offsetof(cro_p2p_finalize_plan, n) == offsetof(P2PFinalizePlan, n) &&
+                  offsetof(cro_p2p_finalize_plan, self) == offsetof(P2PFinalizePlan, self) &&
+                  offsetof(cro_p2p_finalize_plan, have_push) == offsetof(P2PFinalizePlan, have_push) &&
+                  offsetof(cro_p2p_finalize_plan, push_folded) == offsetof(P2PFinalizePlan, push_folded) &&
+                  offsetof(cro_p2p_finalize_plan, p2p_bytes) == offsetof(P2PFinalizePlan, p2p_bytes) &&
+                  offsetof(cro_p2p_finalize_plan, peer_mask) == offsetof(P2PFinalizePlan, peer_mask) &&
+                  offsetof(cro_p2p_finalize_plan, chase_mask) == offsetof(P2PFinalizePlan, chase_mask),
+              "cro_p2p_finalize_plan mirrors P2PFinalizePlan");
+static_assert(sizeof(cro_p2p_plan) == 66336 && offsetof(cro_p2p_plan, fin) == 288 && offsetof(cro_p2p_plan, op) == 800,
+              "cro_p2p_plan layout");
+
+struct P2PPlan {
+    uint64_t p2p_bytes = 0;                                 // P: every leg's bytes, the prefix's and the finalize's
+    std::vector<std::vector<std::pair<int, int>>> rounds;
+    std::vector<P2POp> ops;                                 // in enqueue order; a wait binds to the last record before it
+    P2PFinalizePlan fin[CRO_MAX_DEVICES] = {};
+};
+
+// The full-box probe's schedule (include/croprobe.h, cro_selftest_p2p_plan, states the rules): a pure function of the
+// device count, each device's S after degradation, the options and the access rows (access[8 * i + j]).
+P2PPlan make_p2p_plan(int n, const uint64_t* sweep_bytes, uint64_t p2p_bytes, const uint8_t* access, uint32_t flags, bool unidir,
+                      uint32_t write_variant) {
+    P2PPlan p;
+    const bool nvlink = n > 1 && !(flags & CRO_F_SKIP_P2P);
+    const bool push = nvlink && !(flags & CRO_F_SKIP_P2P_WRITE);
+    auto op = [&](uint8_t kind, int dev, int peer, uint8_t event, size_t round, int slot, uint64_t bytes) {
+        p.ops.push_back(P2POp{kind, (uint8_t)dev, (uint8_t)peer, event, (uint16_t)round, (uint16_t)slot, bytes});
+    };
+    if (nvlink) {
+        // one prefix for the whole call: a pair of unequal sizes would otherwise move, fold and expect different lengths
+        p.p2p_bytes = p2p_bytes;
+        for (int i = 0; i < n; ++i) p.p2p_bytes = std::min(p.p2p_bytes, sweep_bytes[i]);
+    }
+    const uint64_t P = p.p2p_bytes;
+    for (int i = 0; i < n; ++i) {
+        op(CRO_P2P_OP_HBM, i, i, 0, 0, 0, 0);
+        if (!nvlink) continue;
+        op(CRO_P2P_OP_PREFIX, i, i, 0, 0, kSlotPrefix, P);
+        op(CRO_P2P_OP_RECORD, i, i, CRO_P2P_EV_HBM, 0, 0, 0);
+    }
+    if (!nvlink) return p;
+    // a pair is scheduled only when both directions are reachable: one-way access would leave a push unchecked
+    auto linked = [&](int a, int b) { return a < 8 && b < 8 && access[8 * a + b] && access[8 * b + a]; };
+    p.rounds = one_factorisation(n);
+    for (size_t r = 0; r < p.rounds.size(); ++r) {
+        std::vector<std::pair<int, int>> directed;
+        for (const auto& pr : p.rounds[r]) {
+            if (!linked(pr.first, pr.second)) continue;
+            directed.push_back(pr);
+            // CRO_P2P_UNIDIR=1 (measurement only, tools/p2p_variants.py): one direction per pair, to see what the link
+            // gives when its other half is idle; the reverse direction's result slots stay zero
+            if (!unidir) directed.push_back({pr.second, pr.first});
+        }
+        for (const auto& [a, b] : directed) {                   // stage A: read + push
+            op(CRO_P2P_OP_WAIT, a, b, CRO_P2P_EV_HBM, 0, 0, 0);
+            if (r > 0) op(CRO_P2P_OP_WAIT, a, b, CRO_P2P_EV_REREAD, r - 1, 0, 0);
+            op(CRO_P2P_OP_READ, a, b, 0, r, kSlotP2P0 + 3 * b, P);
+            if (push) op(CRO_P2P_OP_PUSH, a, b, 0, r, kSlotP2P0 + 3 * b + 1, P);
+        }
+        // every device publishes both round events, byes and unscheduled pairs included: the next round's pusher waits
+        // on its partner's re-read event of this round, and a device that sat out must not leave a stale one there
+        for (int i = 0; i < n; ++i) op(CRO_P2P_OP_RECORD, i, i, CRO_P2P_EV_PUSH, r, 0, 0);
+        for (const auto& [a, b] : directed) {                   // stage B: the receiver checks what landed
+            if (!push) continue;
+            op(CRO_P2P_OP_WAIT, b, a, CRO_P2P_EV_PUSH, r, 0, 0);
+            op(CRO_P2P_OP_REREAD, b, a, 0, r, kSlotP2P0 + 3 * a + 2, P);
+        }
+        for (int i = 0; i < n; ++i) op(CRO_P2P_OP_RECORD, i, i, CRO_P2P_EV_REREAD, r, 0, 0);
+    }
+    // latency: every device chases all its peers at once (one warp per peer, one load in flight each), after EVERY
+    // device has finished its bandwidth legs so the links are quiet
+    for (int i = 0; i < n; ++i) op(CRO_P2P_OP_RECORD, i, i, CRO_P2P_EV_CHASE, 0, 0, 0);
+    for (int i = 0; i < n; ++i) {
+        for (int j = 0; j < n; ++j)
+            if (j != i) op(CRO_P2P_OP_WAIT, i, j, CRO_P2P_EV_CHASE, 0, 0, 0);
+        op(CRO_P2P_OP_CHASE, i, i, 0, 0, 0, 0);
+        op(CRO_P2P_OP_FINALIZE, i, i, 0, 0, 0, 0);
+        P2PFinalizePlan& f = p.fin[i];
+        f.n = (uint32_t)n;
+        f.self = (uint32_t)i;
+        f.have_push = (push && !unidir) ? 1u : 0u;
+        f.push_folded = write_variant == COPY_TMA_FUSED ? 1u : 0u;   // the plain copies land bytes but fold nothing
+        f.p2p_bytes = P;
+        for (int j = 0; j < n; ++j)
+            if (j != i && linked(i, j)) f.chase_mask |= 1u << j;
+        f.peer_mask = f.chase_mask;
+        if (unidir)     // measurement mode: only the pairs' first devices read; check nothing that did not run
+            for (const auto& rd : p.rounds)
+                for (const auto& pr : rd)
+                    if (pr.second == i) f.peer_mask &= ~(1u << pr.first);
+    }
+    return p;
+}
+
+cudaEvent_t plan_event(Device* d, const P2POp& o) {
+    switch (o.event) {
+        case CRO_P2P_EV_HBM: return d->ev_hbm_done;
+        case CRO_P2P_EV_PUSH: return d->ev_push_done[o.round];
+        case CRO_P2P_EV_REREAD: return d->ev_reread_done[o.round];
+        default: return d->ev_chase_ready;
+    }
+}
+
 }  // namespace
 
 // One call = the full-box probe (BASELINE config 3).  Everything is ENQUEUED first — per-device probe graphs,
@@ -157,7 +278,6 @@ int ctx_probe_all(cro_ctx* c, cro_probe_result* out, int cap, int* n_out) {
         d->lane_head = 0;
     }
     const bool p2p = n > 1 && !(o.flags & CRO_F_SKIP_P2P);
-    const bool push = p2p && !(o.flags & CRO_F_SKIP_P2P_WRITE);
     bool use_nccl = n > 1 && !(o.flags & CRO_F_SKIP_NCCL);
     bool nccl_degraded = false;
     int rc;
@@ -186,11 +306,21 @@ int ctx_probe_all(cro_ctx* c, cro_probe_result* out, int cap, int* n_out) {
             c->nccl_ready = true;
         }
     }
-    const auto rounds = p2p ? one_factorisation(n) : std::vector<std::vector<std::pair<int, int>>>();
+    // the plan needs every device's S after any CRO_F_DEGRADE_ON_OOM halving, so the regions exist before it is made
+    std::vector<uint64_t> sizes((size_t)n);
+    std::vector<uint8_t> access((size_t)n * 8);
+    for (int i = 0; i < n; ++i) {
+        Device* d = c->devs[(size_t)i].get();
+        if ((rc = ensure_region(c, d))) return rc;
+        sizes[(size_t)i] = d->sweep_bytes;
+        memcpy(&access[(size_t)i * 8], d->tmpl.p2p_access, 8);
+    }
+    const unsigned rvp = c->knobs.get("CRO_P2P_READ_VARIANT"), wvp = c->knobs.get("CRO_P2P_WRITE_VARIANT");
+    const P2PPlan plan = make_p2p_plan(n, sizes.data(), o.p2p_bytes, access.data(), o.flags, c->knobs.get("CRO_P2P_UNIDIR") != 0, wvp);
     for (int i = 0; i < n && p2p; ++i) {
         Device* d = c->devs[(size_t)i].get();
         CU_TRY(c, cudaSetDevice(d->ordinal));
-        while (d->ev_push_done.size() < rounds.size()) {
+        while (d->ev_push_done.size() < plan.rounds.size()) {
             cudaEvent_t e1, e2;
             CU_TRY(c, cudaEventCreateWithFlags(&e1, cudaEventDisableTiming));
             CU_TRY(c, cudaEventCreateWithFlags(&e2, cudaEventDisableTiming));
@@ -199,135 +329,92 @@ int ctx_probe_all(cro_ctx* c, cro_probe_result* out, int cap, int* n_out) {
         }
     }
 
-    // ---- phase 1: every device's HBM probe, one graph launch each ---------------------------------------
+    // ---- phases 1 and 2: every device's HBM probe, then the NVLink rounds, 1-factorised so each GPU is in exactly one
+    // pair per round and chained across devices by events, then the chase and the verdict; nothing waits on the host.
+    // Per round and device (partner p):  [wait p's HBM phase, p's previous re-read]  READ p's half A over the link ->
+    // PUSH my prefix into p's half B -> [wait p's push]  RE-READ my own half B locally.
     {
-        Range nv(c, "cro.probe_all.hbm");
-        for (int i = 0; i < n; ++i) {
-            Device* d = c->devs[(size_t)i].get();
-            if ((rc = probe_enqueue(c, d, d->lanes[0]))) return rc;
-            if (p2p) {
-                // what this device's first p2p_bytes must fold to, for the peers that will read them
-                CU_TRY(c, launch_expected(d->plan, std::min<uint64_t>(o.p2p_bytes, d->sweep_bytes), imm_params(d), d->scratch_pfx,
-                                          &d->d_out[kSlotPrefix], d->aux));
-                c->launches++;
-                CU_TRY(c, cudaEventRecord(d->ev_aux_done, d->aux));
-                CU_TRY(c, cudaStreamWaitEvent(d->stream, d->ev_aux_done, 0));
-                CU_TRY(c, cudaEventRecord(d->ev_hbm_done, d->stream));
-            }
-        }
-    }
-
-    // ---- phase 2: NVLink rounds, 1-factorised so each GPU is in exactly one pair per round ----------------
-    // Per round and device (partner p):  [wait p's HBM phase, p's previous re-read]  READ p's half A over the
-    // link -> PUSH my prefix into p's half B -> [wait p's push]  RE-READ my own half B locally.  Both directions
-    // of a pair run at once; nothing waits on the host.
-    const bool unidir = c->knobs.get("CRO_P2P_UNIDIR") != 0;
-    const unsigned rvp = c->knobs.get("CRO_P2P_READ_VARIANT"), wvp = c->knobs.get("CRO_P2P_WRITE_VARIANT");
-    auto pair_ok = [&](int a, int b) { return a < 8 && b < 8 && c->devs[(size_t)a]->tmpl.p2p_access[b]; };
-    auto push_bytes = [&](const Device* a, const Device* b) {
-        return std::min<uint64_t>(std::min<uint64_t>(o.p2p_bytes, a->sweep_bytes), b->sweep_bytes);
-    };
-    if (p2p) {
-        Range nv(c, "cro.probe_all.nvlink");
-        for (size_t r = 0; r < rounds.size(); ++r) {
-            std::vector<std::pair<int, int>> directed;
-            for (const auto& p : rounds[r]) {
-                directed.push_back({p.first, p.second});
-                // CRO_P2P_UNIDIR=1 (measurement only, tools/p2p_variants.py): one direction per pair, to see what the
-                // link gives when its other half is idle; the reverse direction's result slots stay zero
-                if (!unidir) directed.push_back({p.second, p.first});
-            }
-            for (const auto& pr : directed) {                       // stage A: read + push
-                Device* a = c->devs[(size_t)pr.first].get();
-                Device* b = c->devs[(size_t)pr.second].get();
-                if (!pair_ok(pr.first, pr.second)) continue;
-                CU_TRY(c, cudaSetDevice(a->ordinal));
-                CU_TRY(c, cudaStreamWaitEvent(a->stream, b->ev_hbm_done, 0));
-                if (r > 0) CU_TRY(c, cudaStreamWaitEvent(a->stream, b->ev_reread_done[r - 1], 0));
-                // TMA bulk copies straight out of the peer's HBM (cp.async.bulk on the peer-mapped address) into
-                // this GPU's shared memory, checksummed as they land
-                CU_TRY(c, launch_read(a->plan, rvp, b->region, std::min<uint64_t>(o.p2p_bytes, b->sweep_bytes), imm_params(a),
-                                      a->scratch, &a->d_out[kSlotP2P0 + 3 * pr.second], a->stream));
-                c->launches++;
-                if (push) {
-                    // posted NVLink writes: a streams its own prefix through shared memory (bulk load from local
-                    // HBM, bulk store to the peer-mapped address, folded on the way) into half B of b's region
-                    CU_TRY(c, launch_copy(a->plan, wvp, b->region + b->sweep_bytes, a->region, push_bytes(a, b), imm_params(a),
-                                          a->scratch, &a->d_out[kSlotP2P0 + 3 * pr.second + 1], a->stream));
-                    c->launches++;
-                }
-                CU_TRY(c, cudaEventRecord(a->ev_push_done[r], a->stream));
-            }
-            for (const auto& pr : directed) {                       // stage B: the receiver checks what landed
-                Device* a = c->devs[(size_t)pr.first].get();          // pusher
-                Device* b = c->devs[(size_t)pr.second].get();         // receiver
-                if (!pair_ok(pr.first, pr.second)) continue;
-                CU_TRY(c, cudaSetDevice(b->ordinal));
-                if (push) {
-                    b->half_known[1] = false;                        // its prefix now holds a's pattern
-                    CU_TRY(c, cudaStreamWaitEvent(b->stream, a->ev_push_done[r], 0));
-                    CU_TRY(c, launch_read(b->plan, resolve_read_variant(CRO_READ_AUTO, push_bytes(a, b), c->knobs), b->region + b->sweep_bytes,
-                                          push_bytes(a, b), imm_params(b), b->scratch, &b->d_out[kSlotP2P0 + 3 * pr.first + 2], b->stream));
-                    c->launches++;
-                }
-                CU_TRY(c, cudaEventRecord(b->ev_reread_done[r], b->stream));
-            }
-            if (unidir)   // the idle direction's devices still have to publish their round events
-                for (const auto& p : rounds[r]) {
-                    Device* b = c->devs[(size_t)p.second].get();
-                    CU_TRY(c, cudaSetDevice(b->ordinal));
-                    CU_TRY(c, cudaEventRecord(b->ev_push_done[r], b->stream));
-                    Device* a = c->devs[(size_t)p.first].get();
-                    CU_TRY(c, cudaSetDevice(a->ordinal));
-                    CU_TRY(c, cudaEventRecord(a->ev_reread_done[r], a->stream));
-                }
-        }
-        // latency: every device chases all its peers at once (one warp per peer, one load in flight each),
-        // after EVERY device has finished its bandwidth legs so the links are quiet
-        for (int i = 0; i < n; ++i) {
-            Device* d = c->devs[(size_t)i].get();
+        Range nv(c, "cro.probe_all.enqueue");
+        for (const P2POp& op : plan.ops) {
+            Device* d = c->devs[op.dev].get();
+            Device* p = c->devs[op.peer].get();
             CU_TRY(c, cudaSetDevice(d->ordinal));
-            CU_TRY(c, cudaEventRecord(d->ev_chase_ready, d->stream));
-        }
-        for (int i = 0; i < n; ++i) {
-            Device* d = c->devs[(size_t)i].get();
-            CU_TRY(c, cudaSetDevice(d->ordinal));
-            ChaseArgs ca{};
-            ca.n = (unsigned)n;
-            ca.hops = o.latency_hops;
-            for (int j = 0; j < n; ++j) {
-                if (j == i || !pair_ok(i, j)) continue;
-                CU_TRY(c, cudaStreamWaitEvent(d->stream, c->devs[(size_t)j]->ev_chase_ready, 0));
-                ca.table[j] = c->devs[(size_t)j]->d_chase_tables[(size_t)i];
+            switch (op.kind) {
+                case CRO_P2P_OP_HBM:
+                    if ((rc = probe_enqueue(c, d, d->lanes[0]))) return rc;
+                    break;
+                case CRO_P2P_OP_PREFIX:   // what this device's first P bytes must fold to, for the peers that will read them
+                    CU_TRY(c, launch_expected(d->plan, op.bytes, imm_params(d), d->scratch_pfx, &d->d_out[op.slot], d->aux));
+                    c->launches++;
+                    CU_TRY(c, cudaEventRecord(d->ev_aux_done, d->aux));
+                    CU_TRY(c, cudaStreamWaitEvent(d->stream, d->ev_aux_done, 0));
+                    break;
+                case CRO_P2P_OP_RECORD:
+                    CU_TRY(c, cudaEventRecord(plan_event(d, op), d->stream));
+                    break;
+                case CRO_P2P_OP_WAIT:
+                    CU_TRY(c, cudaStreamWaitEvent(d->stream, plan_event(p, op), 0));
+                    break;
+                case CRO_P2P_OP_READ:
+                    // TMA bulk copies straight out of the peer's HBM (cp.async.bulk on the peer-mapped address) into this
+                    // GPU's shared memory, checksummed as they land
+                    CU_TRY(c, launch_read(d->plan, rvp, p->region, op.bytes, imm_params(d), d->scratch, &d->d_out[op.slot], d->stream));
+                    c->launches++;
+                    break;
+                case CRO_P2P_OP_PUSH:
+                    // posted NVLink writes: d streams its own prefix through shared memory (bulk load from local HBM,
+                    // bulk store to the peer-mapped address, folded on the way) into half B of p's region
+                    CU_TRY(c, launch_copy(d->plan, wvp, p->region + p->sweep_bytes, d->region, op.bytes, imm_params(d), d->scratch,
+                                          &d->d_out[op.slot], d->stream));
+                    c->launches++;
+                    break;
+                case CRO_P2P_OP_REREAD:
+                    d->half_known[1] = false;                        // its prefix now holds p's pattern
+                    CU_TRY(c, launch_read(d->plan, resolve_read_variant(CRO_READ_AUTO, op.bytes, c->knobs), d->region + d->sweep_bytes,
+                                          op.bytes, imm_params(d), d->scratch, &d->d_out[op.slot], d->stream));
+                    c->launches++;
+                    break;
+                case CRO_P2P_OP_CHASE: {
+                    ChaseArgs ca{};
+                    ca.n = (unsigned)n;
+                    ca.hops = o.latency_hops;
+                    for (int j = 0; j < n; ++j)
+                        if (plan.fin[op.dev].chase_mask >> j & 1) ca.table[j] = c->devs[(size_t)j]->d_chase_tables[op.dev];
+                    CU_TRY(c, arm_chase_out(d->d_chase_out, d->stream));   // a row the chase does not walk cannot pass
+                    CU_TRY(c, launch_chase(ca, d->d_chase_out, d->stream));
+                    c->launches++;
+                    break;
+                }
+                case CRO_P2P_OP_FINALIZE: {
+                    const P2PFinalizePlan& f = plan.fin[op.dev];
+                    P2PFinalizeArgs pa{};
+                    pa.out = d->d_result;
+                    pa.slots = d->d_out;
+                    pa.chase_out = d->d_chase_out;
+                    pa.n = f.n;
+                    pa.self = f.self;
+                    pa.hops = o.latency_hops;
+                    pa.have_push = f.have_push;
+                    pa.push_folded = f.push_folded;
+                    pa.p2p_bytes = f.p2p_bytes;
+                    pa.stamp = d->nonce_cur;
+                    for (int j = 0; j < n; ++j) {
+                        if (f.peer_mask >> j & 1) {
+                            pa.peer_slots[j] = c->devs[(size_t)j]->d_out;
+                            pa.peer_stamp[j] = c->devs[(size_t)j]->nonce_cur;
+                        }
+                        if (f.chase_mask >> j & 1) pa.chase_expect[j] = d->chase_expect[(size_t)j];
+                    }
+                    CU_TRY(c, launch_p2p_finalize(pa, d->stream));
+                    c->launches++;
+                    CU_TRY(c, cudaMemcpyAsync(d->h_chase_out, d->d_chase_out, 2 * CRO_MAX_DEVICES * sizeof(unsigned long long), cudaMemcpyDeviceToHost, d->stream));
+                    CU_TRY(c, cudaMemcpyAsync(d->h_out, d->d_out, sizeof(SweepOut) * kSlotCount, cudaMemcpyDeviceToHost, d->stream));
+                    break;
+                }
+                default:
+                    c->set_error("full-box plan: unknown op " + std::to_string(op.kind));
+                    return CRO_ERR_INTERNAL;
             }
-            CU_TRY(c, arm_chase_out(d->d_chase_out, d->stream));   // a row the chase does not walk cannot pass
-            CU_TRY(c, launch_chase(ca, d->d_chase_out, d->stream));
-            c->launches++;
-            P2PFinalizeArgs pa{};
-            pa.out = d->d_result;
-            pa.slots = d->d_out;
-            pa.chase_out = d->d_chase_out;
-            pa.n = (unsigned)n;
-            pa.self = (unsigned)i;
-            pa.hops = o.latency_hops;
-            pa.have_push = (push && !unidir) ? 1u : 0u;
-            pa.push_folded = wvp == COPY_TMA_FUSED ? 1u : 0u;   // the plain copies land bytes but fold nothing: only the receiver checks
-            pa.p2p_bytes = o.p2p_bytes;
-            pa.stamp = d->nonce_cur;
-            for (int j = 0; j < n; ++j) {
-                if (j == i || !pair_ok(i, j)) continue;
-                pa.peer_slots[j] = c->devs[(size_t)j]->d_out;
-                pa.peer_stamp[j] = c->devs[(size_t)j]->nonce_cur;
-                pa.chase_expect[j] = d->chase_expect[(size_t)j];
-            }
-            if (unidir)     // measurement mode: only the pairs' first devices read; check nothing that did not run
-                for (const auto& rd : rounds)
-                    for (const auto& p : rd)
-                        if (p.second == i) pa.peer_slots[p.first] = nullptr;
-            CU_TRY(c, launch_p2p_finalize(pa, d->stream));
-            c->launches++;
-            CU_TRY(c, cudaMemcpyAsync(d->h_chase_out, d->d_chase_out, 2 * CRO_MAX_DEVICES * sizeof(unsigned long long), cudaMemcpyDeviceToHost, d->stream));
-            CU_TRY(c, cudaMemcpyAsync(d->h_out, d->d_out, sizeof(SweepOut) * kSlotCount, cudaMemcpyDeviceToHost, d->stream));
         }
     }
 
@@ -430,7 +517,7 @@ int ctx_probe_all(cro_ctx* c, cro_probe_result* out, int cap, int* n_out) {
                     lo = std::min(lo, s.t0);
                     hi = std::max(hi, s.t1);
                 }
-                if (pair_ok(i, j))      // the rows of peers it cannot reach keep the armed value
+                if (plan.fin[i].chase_mask >> j & 1)      // the rows of peers it does not chase keep the armed value
                     c->fullbox.chase_ns = std::max<uint64_t>(c->fullbox.chase_ns, d->h_chase_out[2 * j + 1]);
             }
             if (hi > lo) c->fullbox.p2p_ns = std::max<uint64_t>(c->fullbox.p2p_ns, hi - lo);
@@ -441,11 +528,35 @@ int ctx_probe_all(cro_ctx* c, cro_probe_result* out, int cap, int* n_out) {
         CU_TRY(c, cudaSetDevice(d->ordinal));
         if ((rc = stage_template(c, d))) return rc;
     }
-    c->fullbox.rounds = (uint32_t)rounds.size();
+    c->fullbox.rounds = (uint32_t)plan.rounds.size();
     c->fullbox.host_syncs = host_syncs;
     c->fullbox.gather = use_nccl ? CRO_GATHER_NCCL : nccl_degraded ? CRO_GATHER_DEGRADED : CRO_GATHER_HOST;
     c->fullbox.wall_ns = now_ns() - t_call;
     return worst;
+}
+
+int selftest_p2p_plan(uint32_t n, const uint64_t* sweep_bytes, uint64_t p2p_bytes, const uint8_t* access, uint32_t flags,
+                      uint32_t unidir, uint32_t write_variant, cro_p2p_plan* out) {
+    if (!sweep_bytes || !access || !out || n > CRO_MAX_DEVICES) return CRO_ERR_INVALID_ARG;
+    const P2PPlan p = make_p2p_plan((int)n, sweep_bytes, p2p_bytes, access, flags, unidir != 0, write_variant);
+    if (p.ops.size() > CRO_P2P_PLAN_OPS || p.rounds.size() > CRO_P2P_PLAN_ROUNDS) {
+        set_thread_error("full-box plan larger than cro_p2p_plan holds");
+        return CRO_ERR_INTERNAL;
+    }
+    memset(out, 0, sizeof *out);
+    out->p2p_bytes = p.p2p_bytes;
+    out->n_rounds = (uint32_t)p.rounds.size();
+    out->n_ops = (uint32_t)p.ops.size();
+    for (size_t r = 0; r < p.rounds.size(); ++r) {
+        out->n_pairs[r] = (uint8_t)p.rounds[r].size();
+        for (size_t k = 0; k < p.rounds[r].size(); ++k) {
+            out->pair[r][2 * k] = (uint8_t)p.rounds[r][k].first;
+            out->pair[r][2 * k + 1] = (uint8_t)p.rounds[r][k].second;
+        }
+    }
+    memcpy(out->fin, p.fin, sizeof p.fin);
+    memcpy(out->op, p.ops.data(), p.ops.size() * sizeof(P2POp));
+    return CRO_OK;
 }
 
 int ctx_p2p_detail(cro_ctx* c, int idx, int peer, cro_p2p_detail* out) {

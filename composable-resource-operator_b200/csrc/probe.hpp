@@ -196,6 +196,9 @@ int ctx_create(const cro_opts* o, cro_ctx** out);
 void ctx_destroy(cro_ctx* c);
 int ctx_probe_device(cro_ctx* c, int idx, cro_probe_result* out);
 int ctx_probe_all(cro_ctx* c, cro_probe_result* out, int cap, int* n);
+// cro_selftest_p2p_plan: the plan ctx_probe_all walks, from caller-given sizes, access rows and options (fullbox.cu).
+int selftest_p2p_plan(uint32_t n, const uint64_t* sweep_bytes, uint64_t p2p_bytes, const uint8_t* access, uint32_t flags,
+                      uint32_t unidir, uint32_t write_variant, cro_p2p_plan* out);
 int ctx_probe_begin(cro_ctx* c, int idx);
 int ctx_probe_end(cro_ctx* c, int idx, cro_probe_result* out);
 int ctx_probe_poll(cro_ctx* c, int idx);

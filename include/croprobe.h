@@ -82,7 +82,9 @@ typedef struct cro_opts {
     uint32_t abi_version;          /* must be CRO_ABI_VERSION                               */
     uint32_t flags;                /* CRO_F_*                                               */
     uint64_t sweep_bytes;          /* S, per-device sweep region; default 4 GiB             */
-    uint64_t p2p_bytes;            /* S_p2p per directed pair; default 1 GiB (<= S)         */
+    uint64_t p2p_bytes;            /* S_p2p per directed pair; default 1 GiB (<= S).  A pair
+                                      moves min(p2p_bytes, every device's S after any
+                                      CRO_F_DEGRADE_ON_OOM halving)                          */
     uint64_t seed_base;            /* default 0x00C0FFEE00000000; seed = base | minor       */
     uint32_t read_sweeps;          /* default 5                                             */
     uint32_t copy_sweeps;          /* default 5                                             */
@@ -168,8 +170,11 @@ typedef struct cro_probe_result {
     uint64_t p2p_read_ns[8];       /* 184  time to read p2p_bytes out of peer j's HBM over NVLink */
     uint64_t p2p_checksum_xor[8];  /* 248 */
     uint32_t p2p_latency_ns_x16[8];/* 312  mean hop latency x16 (fixed point): min(chase ns * 16 / hops, 2^32 - 1) */
-    uint8_t  p2p_access[8];        /* 344  cudaDeviceCanAccessPeer                   */
-    uint64_t p2p_bytes;            /* 352 */
+    uint8_t  p2p_access[8];        /* 344  cudaDeviceCanAccessPeer(this device -> j).  cro_probe_all moves bytes between
+                                           two devices and checks them only when both directions are reachable: a peer
+                                           this device reaches one way only shows 1 here and keeps its p2p_ok bit clear */
+    uint64_t p2p_bytes;            /* 352  bytes each pair actually moved per leg: min(cro_opts.p2p_bytes, every
+                                           device's sweep_bytes), the same for every pair of the call */
     uint64_t expect_xor;           /* 360  closed-form checksum computed on the device
                                            by an independent generator kernel        */
     uint64_t expect_sum;           /* 368 */
@@ -200,7 +205,9 @@ typedef struct cro_probe_result {
     uint8_t  fail_index;           /* 500  CRO_FAIL_STALE: the sweep's number in launch order (0 fill, 1.. copies, then
                                            reads); CRO_FAIL_COPY_SRC / CRO_FAIL_READ: the copy / read sweep's own index;
                                            CRO_FAIL_EXPECT: 0, or the peer whose prefix slot is stale; peer checks: the peer */
-    uint8_t  p2p_ok;               /* 501  bit j: NVLink read of, push into and chase through peer j all verified */
+    uint8_t  p2p_ok;               /* 501  bit j: NVLink read of, push into and chase through peer j all verified; clear
+                                           for a peer not reachable both ways (p2p_access of both devices), which is
+                                           never scheduled */
     uint8_t  reserved8[2];         /* 502 */
     uint64_t t_start_ns;           /* 504  %globaltimer when the probe's first CTA started */
 } cro_probe_result;
@@ -3178,6 +3185,79 @@ int  cro_selftest_p2p_finalize(cro_ctx *ctx, int dev_index, cro_probe_result *re
  * chase_kernel for `hops` hops and copies the 2 * n output words to out ([2j] end slot, [2j+1] ns). */
 int  cro_selftest_chase(cro_ctx *ctx, int dev_index, const int32_t *minor_src, const int32_t *minor_dst, uint32_t n,
                         uint32_t hops, uint64_t *out);
+
+/* ---- test hook: the full-box probe's schedule ------------------------------------------------------------------ */
+/* cro_probe_all enqueues by walking one plan, a pure function of the device count, each device's sweep size, the
+ * options and the peer-access matrix; this hook returns that plan without a GPU or a context.
+ *
+ * Rules (DESIGN.md §5):
+ *  - Every device runs its HBM probe.  With the NVLink phase (n >= 2 and no CRO_F_SKIP_P2P), every leg moves
+ *    P = min(p2p_bytes, every device's sweep_bytes) bytes, and each device writes the closed form of its first P
+ *    bytes to CRO_SLOT_PREFIX, then records its HBM event.
+ *  - Rounds: the round-robin 1-factorisation of K_m, m = n rounded up to even, m - 1 rounds.  Round r holds the pairs
+ *    (m-1, r) and ((r+k) mod (m-1), (r-k) mod (m-1)) for k = 1 .. m/2 - 1, in that order; a pair with device m-1 of an
+ *    odd n is a bye and is dropped.
+ *  - A pair (a, b) is scheduled only when both are below 8 and each one's p2p_access row reaches the other.  Then a
+ *    reads b and pushes into b, and, unless unidir, b reads a and pushes into a.  In round r the reader first waits
+ *    for the peer's HBM event and (r > 0) the peer's re-read event of round r-1.  The receiver of a push waits for the
+ *    pusher's push event of round r, then re-reads its own half B.
+ *  - Every device records its push event of round r after the round's reads and pushes, and its re-read event of
+ *    round r after the round's re-reads: every round, byes and unscheduled pairs included.
+ *  - Every device then records its chase event, waits for every other device's chase event, chases every
+ *    scheduled peer and runs p2p_finalize, which gets a slot array for each scheduled peer (under unidir, not for
+ *    a peer that only pushed into it).
+ * A wait binds to the last record of that event enqueued before it, in the plan's op order. */
+#define CRO_P2P_PLAN_OPS     4096   /* op[] capacity: more than the 2256 ops of 16 devices                          */
+#define CRO_P2P_PLAN_ROUNDS    16   /* round capacity: at most 15 rounds                                            */
+
+#define CRO_P2P_OP_HBM        1     /* dev's HBM probe                                                              */
+#define CRO_P2P_OP_PREFIX     2     /* closed form of dev's first `bytes` into its slot `slot`                      */
+#define CRO_P2P_OP_RECORD     3     /* dev records its own event `event` of round `round`                          */
+#define CRO_P2P_OP_WAIT       4     /* dev's stream waits for device peer's event `event` of round `round`          */
+#define CRO_P2P_OP_READ       5     /* dev reads `bytes` of peer's half A over the link into dev's slot `slot`      */
+#define CRO_P2P_OP_PUSH       6     /* dev pushes its first `bytes` into peer's half B, folded into slot `slot`     */
+#define CRO_P2P_OP_REREAD     7     /* dev re-reads `bytes` of its own half B, pushed by peer, into slot `slot`     */
+#define CRO_P2P_OP_CHASE      8     /* dev chases every peer of its finalize's chase_mask                          */
+#define CRO_P2P_OP_FINALIZE   9     /* dev's p2p_finalize with fin[dev]                                            */
+
+#define CRO_P2P_EV_HBM        1     /* events a RECORD or WAIT names; only PUSH and REREAD use `round`              */
+#define CRO_P2P_EV_PUSH       2
+#define CRO_P2P_EV_REREAD     3
+#define CRO_P2P_EV_CHASE      4
+
+typedef struct cro_p2p_op {
+    uint8_t  kind;                 /*   0  CRO_P2P_OP_*                                                              */
+    uint8_t  dev;                  /*   1  the device whose stream runs it                                          */
+    uint8_t  peer;                 /*   2  the other device (RECORD, HBM, PREFIX, CHASE, FINALIZE: dev)              */
+    uint8_t  event;                /*   3  CRO_P2P_EV_* of a RECORD or WAIT, else 0                                  */
+    uint16_t round;                /*   4  round of a leg or of a PUSH / REREAD event, else 0                        */
+    uint16_t slot;                 /*   6  CRO_SLOT_* the op writes (PREFIX, READ, PUSH, REREAD), else 0             */
+    uint64_t bytes;                /*   8  bytes the op moves or folds (PREFIX, READ, PUSH, REREAD), else 0          */
+} cro_p2p_op;                      /*  16 bytes */
+
+typedef struct cro_p2p_finalize_plan {
+    uint32_t n, self, have_push, push_folded;   /*   0  p2p_finalize's arguments (cro_selftest_p2p_finalize)     */
+    uint64_t p2p_bytes;                         /*  16                                                        */
+    uint32_t peer_mask;            /*  24  bit j: the finalize gets peer j's slot array (checks j)                   */
+    uint32_t chase_mask;           /*  28  bit j: the chase walks peer j's table                                     */
+} cro_p2p_finalize_plan;           /*  32 bytes; all 0 for a device without a finalize */
+
+typedef struct cro_p2p_plan {
+    uint64_t p2p_bytes;            /*    0  P (0 without the NVLink phase)                                          */
+    uint32_t n_rounds;             /*    8                                                                         */
+    uint32_t n_ops;                /*   12                                                                         */
+    uint8_t  n_pairs[CRO_P2P_PLAN_ROUNDS];                    /*  16  pairs of round r                         */
+    uint8_t  pair[CRO_P2P_PLAN_ROUNDS][CRO_MAX_DEVICES];      /*  32  round r's pair k: (pair[r][2k], [2k+1])   */
+    cro_p2p_finalize_plan fin[CRO_MAX_DEVICES];               /* 288                                        */
+    cro_p2p_op op[CRO_P2P_PLAN_OPS];                          /* 800  in the order the host enqueues them   */
+} cro_p2p_plan;                    /* 66336 bytes */
+
+/* The plan of cro_probe_all on n devices (0 .. CRO_MAX_DEVICES): sweep_bytes[n] each device's S after any degradation,
+ * access[8 * i + j] device i's p2p_access[j], flags the call's cro_opts.flags (CRO_F_SKIP_P2P, CRO_F_SKIP_P2P_WRITE;
+ * the rest are ignored), unidir the CRO_P2P_UNIDIR knob and write_variant CRO_P2P_WRITE_VARIANT (CRO_COPY_TMA_FUSED
+ * folds the push).  CRO_ERR_INVALID_ARG for a NULL pointer or n out of range. */
+int  cro_selftest_p2p_plan(uint32_t n, const uint64_t *sweep_bytes, uint64_t p2p_bytes, const uint8_t *access,
+                           uint32_t flags, uint32_t unidir, uint32_t write_variant, cro_p2p_plan *out);
 
 /* Kernels cro_selftest_sweep runs (cro_selftest_sweep_opts.kernel). */
 #define CRO_SELFTEST_SWEEP_FILL         1   /* the pattern of seed, or its complement (invert), over the other one   */
