@@ -1515,18 +1515,9 @@ def selftest_xlane_classify(legs: int, iterations: int, seed: int, sm_count: int
     (sm_count XlaneCta, sm_count * XLANE_THREADS XlaneThread, sm_count * XLANE_THREADS * XLANE_THREAD_RECORDS
     XlaneFault), for each leg of `legs` in order, every leg the same number of rounds.  Returns (result, SM entries,
     faults); the result's status may be OK, ERR_CHECKSUM or ERR_UNSUPPORTED.  cap defaults to XLANE_RECORDS."""
-    n_rounds = len(rounds[0]) if rounds else 0
-    assert all(len(r) == n_rounds for r in rounds)
-    flat = [rnd for leg in rounds for rnd in leg]
-    ctas = (XlaneCta * max(1, sm_count * len(flat)))(*[x for rnd in flat for x in rnd[0]])
-    thr = (XlaneThread * max(1, sm_count * XLANE_THREADS * len(flat)))(*[x for rnd in flat for x in rnd[1]])
-    recs = (XlaneFault * max(1, sm_count * XLANE_THREADS * XLANE_THREAD_RECORDS * len(flat)))(*[x for rnd in flat for x in rnd[2]])
-    cap = XLANE_RECORDS if cap is None else cap
-    rc, out = _per_sm(lib.cro_selftest_xlane_classify, (legs, iterations, seed, sm_count, call, n_rounds, ctas, thr, recs),
-                      XlaneResult, XlaneSm, XLANE_MAX_SMS, XlaneFault, cap)
-    if rc not in (OK, ERR_CHECKSUM, ERR_UNSUPPORTED):
-        raise ProbeError(rc, "cro_selftest_xlane_classify")
-    return out
+    return _lane_classify("cro_selftest_xlane_classify", (legs, iterations, seed, sm_count, call), sm_count, rounds,
+                          XLANE_RECORDS if cap is None else cap, XlaneCta, XlaneThread, XlaneFault, XLANE_THREADS,
+                          XLANE_THREAD_RECORDS, XlaneResult, XlaneSm, XLANE_MAX_SMS)
 
 
 def emit_alu_annotations_json(r: AluResult) -> str:
@@ -1547,18 +1538,9 @@ def alu_expected(leg: int, seed: int, warp: int) -> List[AluRecord]:
 def selftest_alu_classify(legs: int, iterations: int, seed: int, sm_count: int, call: int, rounds, cap: Optional[int] = None):
     """cro_selftest_alu_classify: the ALU probe's classification of call `call`, as selftest_xlane_classify with
     AluCta, AluThread and AluFault.  Returns (result, SM entries, faults)."""
-    n_rounds = len(rounds[0]) if rounds else 0
-    assert all(len(r) == n_rounds for r in rounds)
-    flat = [rnd for leg in rounds for rnd in leg]
-    ctas = (AluCta * max(1, sm_count * len(flat)))(*[x for rnd in flat for x in rnd[0]])
-    thr = (AluThread * max(1, sm_count * ALU_THREADS * len(flat)))(*[x for rnd in flat for x in rnd[1]])
-    recs = (AluFault * max(1, sm_count * ALU_THREADS * ALU_THREAD_RECORDS * len(flat)))(*[x for rnd in flat for x in rnd[2]])
-    cap = ALU_RECORDS if cap is None else cap
-    rc, out = _per_sm(lib.cro_selftest_alu_classify, (legs, iterations, seed, sm_count, call, n_rounds, ctas, thr, recs),
-                      AluResult, AluSm, ALU_MAX_SMS, AluFault, cap)
-    if rc not in (OK, ERR_CHECKSUM, ERR_UNSUPPORTED):
-        raise ProbeError(rc, "cro_selftest_alu_classify")
-    return out
+    return _lane_classify("cro_selftest_alu_classify", (legs, iterations, seed, sm_count, call), sm_count, rounds,
+                          ALU_RECORDS if cap is None else cap, AluCta, AluThread, AluFault, ALU_THREADS, ALU_THREAD_RECORDS,
+                          AluResult, AluSm, ALU_MAX_SMS)
 
 
 def emit_barrier_annotations_json(r: BarrierResult) -> str:
@@ -1581,18 +1563,9 @@ def selftest_barrier_classify(legs: int, iterations: int, seed: int, cluster: in
                               cap: Optional[int] = None):
     """cro_selftest_barrier_classify: the barrier probe's classification of call `call`, as selftest_xlane_classify
     with BarrierCta, BarrierThread and BarrierFault.  Returns (result, SM entries, faults)."""
-    n_rounds = len(rounds[0]) if rounds else 0
-    assert all(len(r) == n_rounds for r in rounds)
-    flat = [rnd for leg in rounds for rnd in leg]
-    ctas = (BarrierCta * max(1, sm_count * len(flat)))(*[x for rnd in flat for x in rnd[0]])
-    thr = (BarrierThread * max(1, sm_count * BARRIER_THREADS * len(flat)))(*[x for rnd in flat for x in rnd[1]])
-    recs = (BarrierFault * max(1, sm_count * BARRIER_THREADS * BARRIER_THREAD_RECORDS * len(flat)))(*[x for rnd in flat for x in rnd[2]])
-    cap = BARRIER_RECORDS if cap is None else cap
-    rc, out = _per_sm(lib.cro_selftest_barrier_classify, (legs, iterations, seed, cluster, sm_count, call, n_rounds, ctas, thr, recs),
-                      BarrierResult, BarrierSm, BARRIER_MAX_SMS, BarrierFault, cap)
-    if rc not in (OK, ERR_CHECKSUM, ERR_UNSUPPORTED):
-        raise ProbeError(rc, "cro_selftest_barrier_classify")
-    return out
+    return _lane_classify("cro_selftest_barrier_classify", (legs, iterations, seed, cluster, sm_count, call), sm_count, rounds,
+                          BARRIER_RECORDS if cap is None else cap, BarrierCta, BarrierThread, BarrierFault, BARRIER_THREADS,
+                          BARRIER_THREAD_RECORDS, BarrierResult, BarrierSm, BARRIER_MAX_SMS)
 
 
 def read_sram_health(uuid: str) -> SramHealth:
@@ -1921,6 +1894,24 @@ def _per_sm(fn, head: tuple, result, sm, max_sms: int, fault, cap: int, tail: tu
     n_sms, n = ctypes.c_int(), ctypes.c_int()
     rc = fn(*head, ctypes.byref(r), sms, max_sms, ctypes.byref(n_sms), arr, cap, ctypes.byref(n), *tail)
     return rc, (r, [sms[i] for i in range(n_sms.value)], [arr[i] for i in range(n.value)])
+
+
+def _lane_classify(name: str, head: tuple, sm_count: int, rounds, cap: int, cta, thread, fault, threads: int,
+                   thread_records: int, result, sm, max_sms: int):
+    """One cro_selftest_<probe>_classify call of a lane probe (cross-lane, ALU, barrier): lib.<name>(*head, the round
+    count, the CTA entries, thread entries and records of `rounds`, ...).  rounds[leg index][round] = (sm_count CTA
+    entries, sm_count * threads thread entries, sm_count * threads * thread_records records), every leg the same number
+    of rounds.  Returns (result, SM entries, faults); the result's status may be OK, ERR_CHECKSUM or ERR_UNSUPPORTED."""
+    n_rounds = len(rounds[0]) if rounds else 0
+    assert all(len(r) == n_rounds for r in rounds)
+    flat = [rnd for leg in rounds for rnd in leg]
+    ctas = (cta * max(1, sm_count * len(flat)))(*[x for rnd in flat for x in rnd[0]])
+    thr = (thread * max(1, sm_count * threads * len(flat)))(*[x for rnd in flat for x in rnd[1]])
+    recs = (fault * max(1, sm_count * threads * thread_records * len(flat)))(*[x for rnd in flat for x in rnd[2]])
+    rc, out = _per_sm(getattr(lib, name), head + (n_rounds, ctas, thr, recs), result, sm, max_sms, fault, cap)
+    if rc not in (OK, ERR_CHECKSUM, ERR_UNSUPPORTED):
+        raise ProbeError(rc, name)
+    return out
 
 
 def _link_opts(bytes: int, hops: int, ctas: int, inject: Optional[Tuple[int, int, int]]) -> LinkOpts:

@@ -593,48 +593,9 @@ void table(unsigned leg, u64 seed, unsigned w, cro_alu_record* out) {
 }  // namespace alu
 
 namespace {
-// Iterations per CTA and leg, and launches per leg, when the caller gives none.  On an H100 80GB HBM3 at a 700 W limit
-// (profiles/h100_700w_alu_rate.jsonl) one iteration of the five legs takes about 0.4 ms of launches, one launch per
-// leg covering all 132 SMs, so 12 iterations (4.9 ms) cost about the SRAM, register-file and cross-lane probes' 5 ms.
-// The host table build (about 40 ms there) is on top of that, in table_ns.
-constexpr uint32_t kAluDefaultIterations = 12;
-constexpr uint32_t kAluDefaultRounds = 4;
-constexpr size_t kThreadRecs = CRO_ALU_THREAD_RECORDS;
-
-// The ALU probe's types and constants for the shared report path (lane_report.hpp).
-struct AluReport {
-    using Result = cro_alu_result;
-    using Sm = cro_alu_sm;
-    using Fault = cro_alu_fault;
-    using Thread = cro_alu_thread;
-    using Cta = cro_alu_cta;
-    static constexpr unsigned kLegs = CRO_ALU_LEGS, kThreads = CRO_ALU_THREADS, kThreadRecs = CRO_ALU_THREAD_RECORDS,
-                              kRecords = CRO_ALU_RECORDS, kMaxSms = CRO_ALU_MAX_SMS, kPersistent = CRO_ALU_PERSISTENT,
-                              kIntermittent = CRO_ALU_INTERMITTENT, kNone = CRO_ALU_NONE, kSm = CRO_ALU_SM, kAll = CRO_ALU_ALL;
-    static constexpr const char* kName = "ALU probe";
-    static unsigned ops(unsigned leg) { return alu::kOps[leg]; }
-};
-
-uint32_t legs_of(const cro_alu_opts& o) { return o.legs ? o.legs : CRO_ALU_ALL_LEGS; }
-
-void blank_result(cro_alu_result* r, const cro_alu_result& from, std::vector<cro_alu_sm>* sms, std::vector<cro_alu_fault>* faults) {
-    const cro_alu_result keep = from;
-    memset(r, 0, sizeof *r);
-    r->seed = keep.seed;
-    r->call = keep.call;
-    r->sm_count = keep.sm_count;
-    r->legs = keep.legs;
-    r->iterations = keep.iterations;
-    r->cuda_error = keep.cuda_error;
-    r->table_ns = keep.table_ns;
-    sms->clear();
-    faults->clear();
-}
-
 // The legs' tables, by leg then op, warp, lane (the kernels' op * CRO_ALU_THREADS + thread), and the closed form of
 // every CTA's fold.
 void build(uint64_t seed, uint32_t legs, std::vector<cro_alu_record> tabs[CRO_ALU_LEGS], cro_alu_result* r) {
-    const uint64_t t0 = now_ns();
     for (unsigned leg = 0; leg < CRO_ALU_LEGS; ++leg) {
         if (!(legs >> leg & 1u)) continue;
         const unsigned n = alu::kOps[leg];
@@ -657,31 +618,72 @@ void build(uint64_t seed, uint32_t legs, std::vector<cro_alu_record> tabs[CRO_AL
         r->expect[leg][1] = s;
         r->expect[leg][2] = f;
     }
-    r->table_ns = now_ns() - t0;
 }
 
-void open_alu_call(cro_alu_result* r, uint64_t seed, uint64_t k, uint32_t sm_count, uint32_t legs, uint32_t iters,
-                   std::vector<cro_alu_record> tabs[CRO_ALU_LEGS]) {
-    r->seed = seed;
-    r->call = k;
-    r->sm_count = sm_count;
-    r->legs = legs;
-    r->iterations = iters;
-    build(seed, legs, tabs, r);
-}
+// What the lane probes' host driver (lane_report.hpp) needs of the ALU probe: one table per leg, built on the host.
+struct AluProbe {
+    using Opts = cro_alu_opts;
+    using Result = cro_alu_result;
+    using Sm = cro_alu_sm;
+    using Fault = cro_alu_fault;
+    using Thread = cro_alu_thread;
+    using Cta = cro_alu_cta;
+    using Args = AluArgs;
+    struct Tables {
+        std::vector<cro_alu_record> tabs[CRO_ALU_LEGS];
+    };
+    static constexpr unsigned kLegs = CRO_ALU_LEGS, kAllLegs = CRO_ALU_ALL_LEGS, kThreads = CRO_ALU_THREADS,
+                              kThreadRecs = CRO_ALU_THREAD_RECORDS, kRecords = CRO_ALU_RECORDS, kMaxSms = CRO_ALU_MAX_SMS,
+                              kMaxIterations = CRO_ALU_MAX_ITERATIONS, kMaxRounds = CRO_ALU_MAX_ROUNDS,
+                              kPersistent = CRO_ALU_PERSISTENT, kIntermittent = CRO_ALU_INTERMITTENT, kNone = CRO_ALU_NONE,
+                              kSm = CRO_ALU_SM, kAll = CRO_ALU_ALL;
+    static constexpr const char* kName = "ALU";
+    static constexpr const char* kId = "alu";
+    static constexpr const cro_wire& kWire = cro_wire_alu;
+    static constexpr uint64_t Device::*kCalls = &Device::alu_calls;
+    static constexpr SeedSpace kSeeds = kSeedAlu;
+    // Iterations per CTA and leg, and launches per leg, when the caller gives none.  On an H100 80GB HBM3 at a 700 W
+    // limit (profiles/h100_700w_alu_rate.jsonl) one iteration of the five legs takes about 0.4 ms of launches, one
+    // launch per leg covering all 132 SMs, so 12 iterations (4.9 ms) cost about the SRAM, register-file and cross-lane
+    // probes' 5 ms.  The host table build (about 40 ms there) is on top of that, in table_ns.
+    static constexpr uint32_t kDefaultIterations = 12, kDefaultRounds = 4;
+    static constexpr unsigned kBlobs = 1;
+
+    static unsigned ops(unsigned leg) { return alu::kOps[leg]; }
+    static std::string opts_error(const cro_alu_opts& o) { return alu_opts_error(o); }
+    static cudaError_t plan(int device, unsigned leg) { return alu_plan(device, leg); }
+    static int grids(cro_ctx*, const cro_alu_opts&, uint32_t, int sm_count, int (&grid)[kLegs]) {
+        std::fill(grid, grid + kLegs, sm_count);
+        return CRO_OK;
+    }
+    static cudaError_t launch(const cro_alu_opts&, unsigned leg, const AluArgs& a, int grid, cudaStream_t st) {
+        return launch_alu(leg, a, grid, st);
+    }
+    static void open(const cro_alu_opts&, cro_alu_result* r, Tables& tb, bool timed) {
+        const uint64_t t0 = now_ns();
+        build(r->seed, r->legs, tb.tabs, r);
+        if (timed) r->table_ns = now_ns() - t0;
+    }
+    static std::array<LaneBlob, kBlobs> blobs(const Tables& tb, unsigned leg) {
+        return {LaneBlob{tb.tabs[leg].data(), tb.tabs[leg].size() * sizeof(cro_alu_record)}};
+    }
+    static void args(const cro_alu_opts& o, const cro_alu_result&, unsigned, const std::array<const void*, kBlobs>& on_dev,
+                     AluArgs* a) {
+        a->table = static_cast<const cro_alu_record*>(on_dev[0]);
+        a->inj_operand = o.test_inject_operand;
+    }
+    static bool no_new_sm_ends(unsigned) { return false; }
+    static int close(cro_alu_result* r, LaneTally<AluProbe>& t, std::vector<cro_alu_sm>* sms, std::vector<cro_alu_fault>* faults) {
+        return close_lane_call<AluProbe>(r, t, sms, faults);
+    }
+    static void keep(cro_alu_result* r, const cro_alu_result& from) { r->table_ns = from.table_ns; }
+};
 }  // namespace
 
 void alu_expected(unsigned leg, uint64_t seed, unsigned warp, cro_alu_record* out) { alu::table(leg, seed, warp, out); }
 
 std::string alu_opts_error(const cro_alu_opts& o) {
-    const uint32_t iters = o.iterations ? o.iterations : kAluDefaultIterations;
-    const int leg = o.test_inject_leg;
-    const bool inj_ok = !o.test_inject_mask ||
-                        (leg >= 0 && leg < CRO_ALU_LEGS && (legs_of(o) >> leg & 1u) && o.test_inject_sm >= -1 &&
-                         o.test_inject_sm < CRO_ALU_MAX_SMS && o.test_inject_warp >= -1 && o.test_inject_warp < CRO_ALU_WARPS &&
-                         o.test_inject_lane >= -1 && o.test_inject_lane < 32 && o.test_inject_op < alu::kOps[leg] &&
-                         o.test_inject_iteration < iters && o.test_inject_operand < 4);
-    if (iters > CRO_ALU_MAX_ITERATIONS || o.legs > CRO_ALU_ALL_LEGS || o.max_rounds > CRO_ALU_MAX_ROUNDS || o.deadline_ms < 0 || !inj_ok)
+    if (!lane_opts_ok<AluProbe>(o) || (o.test_inject_mask && o.test_inject_operand >= 4))
         return "ALU probe: iterations at most " + std::to_string(CRO_ALU_MAX_ITERATIONS) + ", legs at most 0x1F, max_rounds at most " +
                std::to_string(CRO_ALU_MAX_ROUNDS) + ", deadline_ms not negative, and an injection must name a leg the call runs, an SM "
                "id below " + std::to_string(CRO_ALU_MAX_SMS) + ", a warp below 8 and a lane below 32 (each or -1), an op of the "
@@ -691,134 +693,21 @@ std::string alu_opts_error(const cro_alu_opts& o) {
 
 int ctx_probe_alu(cro_ctx* c, int idx, const cro_alu_opts& o, cro_alu_result* r, std::vector<cro_alu_sm>* sms,
                   std::vector<cro_alu_fault>* faults) {
-    const uint64_t t_call = now_ns();
-    blank_result(r, cro_alu_result{}, sms, faults);
-    Device* d = dev_at(c, idx);
-    if (!d) return r->status = unknown_device(c, idx, "a GPU attached after init is probed through the helper process, cro_probe_alu_uuid");
-    const uint32_t iters = o.iterations ? o.iterations : kAluDefaultIterations;
-    const uint32_t max_rounds = o.max_rounds ? o.max_rounds : kAluDefaultRounds;
-    const uint32_t legs = legs_of(o);
-    const std::string why = alu_opts_error(o);
-    if (!why.empty()) {
-        c->set_error(why);
-        return r->status = CRO_ERR_INVALID_ARG;
-    }
-    DeviceGuard g = enter_device(c, idx);
-    if (g.rc) return r->status = g.rc;
-    Range nv(c, "cro.probe_alu");
-    LaneTally<AluReport> t;
-    cudaEvent_t ev[2] = {nullptr, nullptr};                  // the call's own, destroyed on every way out
-    int rc = [&]() -> int {
-        const int sm_count = d->plan.sm_count;
-        for (unsigned leg = 0; leg < CRO_ALU_LEGS; ++leg)
-            if (legs >> leg & 1u) CU_TRY(c, alu_plan(d->ordinal, leg));
-        const uint64_t k = d->alu_calls++;
-        std::vector<cro_alu_record> tabs[CRO_ALU_LEGS];
-        open_alu_call(r, space_seed(d, kSeedAlu, k), k, (uint32_t)sm_count, legs, iters, tabs);
-
-        // [CTA entries][thread entries] (armed together every round), then [records], then [tables], allocated per call
-        const size_t n_thr = (size_t)sm_count * CRO_ALU_THREADS;
-        const size_t cta_bytes = (size_t)sm_count * sizeof(cro_alu_cta), thr_bytes = n_thr * sizeof(cro_alu_thread);
-        const size_t rec_off = (cta_bytes + thr_bytes + 255) & ~(size_t)255, rec_bytes = n_thr * kThreadRecs * sizeof(cro_alu_fault);
-        size_t tab_off[CRO_ALU_LEGS], end = (rec_off + rec_bytes + 255) & ~(size_t)255;
-        for (unsigned leg = 0; leg < CRO_ALU_LEGS; ++leg) {
-            tab_off[leg] = end;
-            end += tabs[leg].size() * sizeof(cro_alu_record);
-        }
-        DeviceMem<unsigned char> b;
-        CU_TRY(c, cudaMalloc(&b.p, end));
-        for (unsigned leg = 0; leg < CRO_ALU_LEGS; ++leg)
-            if (!tabs[leg].empty())
-                CU_TRY(c, cudaMemcpyAsync(b.p + tab_off[leg], tabs[leg].data(), tabs[leg].size() * sizeof(cro_alu_record),
-                                          cudaMemcpyHostToDevice, d->stream));
-        for (cudaEvent_t& x : ev) CU_TRY(c, cudaEventCreate(&x));
-        cudaStream_t st = d->stream;
-        AluArgs a{};
-        a.cta = reinterpret_cast<cro_alu_cta*>(b.p);
-        a.thr = reinterpret_cast<cro_alu_thread*>(b.p + cta_bytes);
-        a.rec = reinterpret_cast<cro_alu_fault*>(b.p + rec_off);
-        a.stamp = k;
-        a.iterations = iters;
-        a.inj_sm = o.test_inject_sm;
-        a.inj_warp = o.test_inject_warp;
-        a.inj_lane = o.test_inject_lane;
-        a.inj_op = o.test_inject_op;
-        a.inj_iter = o.test_inject_iteration;
-        a.inj_operand = o.test_inject_operand;
-        std::vector<unsigned char> head(cta_bytes + thr_bytes);
-        std::vector<cro_alu_fault> hr(n_thr * kThreadRecs);
-        const auto* hc = reinterpret_cast<const cro_alu_cta*>(head.data());
-        const auto* ht = reinterpret_cast<const cro_alu_thread*>(head.data() + cta_bytes);
-        for (unsigned leg = 0; leg < CRO_ALU_LEGS; ++leg) {
-            if (!(legs >> leg & 1u)) continue;
-            a.table = reinterpret_cast<const cro_alu_record*>(b.p + tab_off[leg]);
-            a.inj_mask = o.test_inject_mask && o.test_inject_leg == (int)leg ? o.test_inject_mask : 0ull;
-            auto launch = [&] { return launch_alu(leg, a, sm_count, st); };
-            auto fetch = [&] { return cudaMemcpyAsync(head.data(), b.p, head.size(), cudaMemcpyDeviceToHost, st); };
-            auto take = [&](uint32_t* covered) -> int {
-                if (lane_any_failed<AluReport>(ht, sm_count, k)) CU_TRY(c, cudaMemcpy(hr.data(), a.rec, rec_bytes, cudaMemcpyDeviceToHost));
-                return take_lane_round<AluReport>(c, leg, hc, ht, hr.data(), sm_count, k, r, t, covered);
-            };
-            uint32_t rounds = 0;
-            const int e = coverage_rounds(c, d, ev, b.p, head.size(), (uint32_t)sm_count, max_rounds, &rounds, &r->leg_ns[leg], launch,
-                                          fetch, take);
-            r->rounds += rounds;
-            r->ns += r->leg_ns[leg];
-            if (e) return e;
-        }
-        return CRO_OK;
-    }();
-    for (cudaEvent_t x : ev)
-        if (x) cudaEventDestroy(x);
-    if (rc == CRO_ERR_CUDA) r->cuda_error = (int32_t)cudaGetLastError();
-    if (rc) {
-        blank_result(r, *r, sms, faults);
-        r->wall_ns = now_ns() - t_call;
-        return r->status = rc;
-    }
-    const int status = close_lane_call<AluReport>(r, t, sms, faults);
-    r->wall_ns = now_ns() - t_call;
-    return status;
+    return probe_lane_legs<AluProbe>(c, idx, o, r, sms, faults);
 }
 
 int classify_alu(uint32_t legs, uint32_t iterations, uint64_t seed, uint32_t sm_count, uint64_t k, uint32_t rounds,
                  const cro_alu_cta* ctas, const cro_alu_thread* threads, const cro_alu_fault* records, cro_alu_result* r,
                  std::vector<cro_alu_sm>* sms, std::vector<cro_alu_fault>* faults) {
-    blank_result(r, cro_alu_result{}, sms, faults);
-    std::vector<cro_alu_record> tabs[CRO_ALU_LEGS];
-    open_alu_call(r, seed, k, sm_count, legs, iterations, tabs);
-    r->table_ns = 0;
-    LaneTally<AluReport> t;
-    const size_t n_thr = (size_t)sm_count * CRO_ALU_THREADS;
-    for (unsigned leg = 0; leg < CRO_ALU_LEGS; ++leg) {
-        if (!(legs >> leg & 1u)) continue;
-        for (uint32_t j = 0; j < rounds; ++j, ctas += sm_count, threads += n_thr, records += n_thr * kThreadRecs) {
-            ++r->rounds;
-            uint32_t covered = 0;
-            const int e = take_lane_round<AluReport>(nullptr, leg, ctas, threads, records, (int)sm_count, k, r, t, &covered);
-            if (e) {
-                blank_result(r, *r, sms, faults);
-                return r->status = e;
-            }
-        }
-    }
-    return close_lane_call<AluReport>(r, t, sms, faults);
+    cro_alu_opts o{};
+    o.legs = legs;
+    o.iterations = iterations;
+    return classify_lane_legs<AluProbe>(o, seed, sm_count, k, rounds, ctas, threads, records, r, sms, faults);
 }
 
 int ctx_probe_alu_uuid(cro_ctx* c, const char* uuid, const cro_alu_opts& o, cro_alu_result* r, std::vector<cro_alu_sm>* sms,
                        std::vector<cro_alu_fault>* faults, int cap) {
-    blank_result(r, cro_alu_result{}, sms, faults);
-    if (!uuid) return r->status = CRO_ERR_INVALID_ARG;
-    const std::string why = alu_opts_error(o);
-    if (!why.empty()) {
-        set_call_error(c, why);
-        return r->status = CRO_ERR_INVALID_ARG;
-    }
-    uint64_t helper_ns = 0;
-    if (run_check_helper(c, cro_wire_alu, uuid, "ALU helper", "cro.probe_alu.helper", &o, cap, o.deadline_ms, &helper_ns, r, faults,
-                         sms) == CRO_OK)
-        r->helper_ns = helper_ns;
-    return r->status;
+    return probe_lane_legs_uuid<AluProbe>(c, uuid, o, r, sms, faults, cap);
 }
 
 }  // namespace cro

@@ -215,98 +215,116 @@ void folded(unsigned leg, const cro_barrier_row& R, const u64* w, unsigned t, F 
 }  // namespace barrier
 
 namespace {
-// Iterations per CTA and leg when the caller gives none, and launches per leg.  On an H100 80GB HBM3 at a 700 W limit
-// (profiles/h100_700w_barrier_rate.jsonl) one iteration of the three legs takes about 0.28 ms of launches (BAR 244 us,
-// MBAR 10 us, CLUSTER 27 us), so 16 iterations cost about the 5 ms the SRAM, register-file, cross-lane and ALU probes take.
-constexpr uint32_t kBarrierDefaultIterations = 16;
-constexpr uint32_t kBarrierDefaultRounds = 4;
 constexpr uint32_t kBarrierDefaultCluster = 2;
-constexpr size_t kThreadRecs = CRO_BARRIER_THREAD_RECORDS;
 
-// The barrier probe's types and constants for the shared report path (lane_report.hpp).
-struct BarrierReport {
+uint32_t cluster_of(const cro_barrier_opts& o) { return o.cluster ? o.cluster : kBarrierDefaultCluster; }
+
+// What the lane probes' host driver (lane_report.hpp) needs of the barrier probe: per leg a table of rows and words
+// built on the host, and a CLUSTER leg that launches clusters of o.cluster CTAs.
+struct BarrierProbe {
+    using Opts = cro_barrier_opts;
     using Result = cro_barrier_result;
     using Sm = cro_barrier_sm;
     using Fault = cro_barrier_fault;
     using Thread = cro_barrier_thread;
     using Cta = cro_barrier_cta;
-    static constexpr unsigned kLegs = CRO_BARRIER_LEGS, kThreads = CRO_BARRIER_THREADS, kThreadRecs = CRO_BARRIER_THREAD_RECORDS,
-                              kRecords = CRO_BARRIER_RECORDS, kMaxSms = CRO_BARRIER_MAX_SMS, kPersistent = CRO_BARRIER_PERSISTENT,
-                              kIntermittent = CRO_BARRIER_INTERMITTENT, kNone = CRO_BARRIER_NONE, kSm = CRO_BARRIER_SM,
-                              kAll = CRO_BARRIER_ALL;
-    static constexpr const char* kName = "barrier probe";
+    using Args = BarrierArgs;
+    struct Tables {
+        std::vector<cro_barrier_row> rows[CRO_BARRIER_LEGS];
+        std::vector<uint64_t> words[CRO_BARRIER_LEGS];
+    };
+    static constexpr unsigned kLegs = CRO_BARRIER_LEGS, kAllLegs = CRO_BARRIER_ALL_LEGS, kThreads = CRO_BARRIER_THREADS,
+                              kThreadRecs = CRO_BARRIER_THREAD_RECORDS, kRecords = CRO_BARRIER_RECORDS, kMaxSms = CRO_BARRIER_MAX_SMS,
+                              kMaxIterations = CRO_BARRIER_MAX_ITERATIONS, kMaxRounds = CRO_BARRIER_MAX_ROUNDS,
+                              kPersistent = CRO_BARRIER_PERSISTENT, kIntermittent = CRO_BARRIER_INTERMITTENT, kNone = CRO_BARRIER_NONE,
+                              kSm = CRO_BARRIER_SM, kAll = CRO_BARRIER_ALL;
+    static constexpr const char* kName = "barrier";
+    static constexpr const char* kId = "barrier";
+    static constexpr const cro_wire& kWire = cro_wire_barrier;
+    static constexpr uint64_t Device::*kCalls = &Device::barrier_calls;
+    static constexpr SeedSpace kSeeds = kSeedBarrier;
+    // Iterations per CTA and leg when the caller gives none, and launches per leg.  On an H100 80GB HBM3 at a 700 W
+    // limit (profiles/h100_700w_barrier_rate.jsonl) one iteration of the three legs takes about 0.28 ms of launches
+    // (BAR 244 us, MBAR 10 us, CLUSTER 27 us), so 16 iterations cost about the 5 ms the SRAM, register-file, cross-lane
+    // and ALU probes take.
+    static constexpr uint32_t kDefaultIterations = 16, kDefaultRounds = 4;
+    static constexpr unsigned kBlobs = 2;       // rows, words
+
     static unsigned ops(unsigned leg) { return barrier::kOps[leg]; }
-};
-
-uint32_t legs_of(const cro_barrier_opts& o) { return o.legs ? o.legs : CRO_BARRIER_ALL_LEGS; }
-uint32_t cluster_of(const cro_barrier_opts& o) { return o.cluster ? o.cluster : kBarrierDefaultCluster; }
-
-void blank_result(cro_barrier_result* r, const cro_barrier_result& from, std::vector<cro_barrier_sm>* sms,
-                  std::vector<cro_barrier_fault>* faults) {
-    const cro_barrier_result keep = from;
-    memset(r, 0, sizeof *r);
-    r->seed = keep.seed;
-    r->call = keep.call;
-    r->sm_count = keep.sm_count;
-    r->legs = keep.legs;
-    r->iterations = keep.iterations;
-    r->cluster = keep.cluster;
-    r->cuda_error = keep.cuda_error;
-    r->table_ns = keep.table_ns;
-    sms->clear();
-    faults->clear();
-}
-
-struct Tables {
-    std::vector<cro_barrier_row> rows[CRO_BARRIER_LEGS];
-    std::vector<uint64_t> words[CRO_BARRIER_LEGS];
-};
-
-// The legs' tables and the closed form of every CTA's fold.
-void open_barrier_call(cro_barrier_result* r, uint64_t seed, uint64_t k, uint32_t sm_count, uint32_t legs, uint32_t iters,
-                       uint32_t cluster, Tables& tb) {
-    const uint64_t t0 = now_ns();
-    r->seed = seed;
-    r->call = k;
-    r->sm_count = sm_count;
-    r->legs = legs;
-    r->iterations = iters;
-    r->cluster = cluster;
-    for (unsigned leg = 0; leg < CRO_BARRIER_LEGS; ++leg) {
-        if (!(legs >> leg & 1u)) continue;
-        const unsigned n = barrier::kOps[leg];
-        tb.rows[leg].resize(n);
-        tb.words[leg].resize((size_t)n * CRO_BARRIER_THREADS * 2);
-        barrier::table(leg, seed, cluster, tb.rows[leg].data(), tb.words[leg].data());
-        uint64_t x = 0, s = 0, f = 0;
-        for (uint64_t op = 0; op < n; ++op)
-            for (unsigned t = 0; t < CRO_BARRIER_THREADS; ++t)
-                barrier::folded(leg, tb.rows[leg][op], tb.words[leg].data() + op * CRO_BARRIER_THREADS * 2, t, [&](uint64_t v) {
-                    x ^= v;
-                    s += v;
-                    f += v * (2 * op + 1);
-                });
-        r->expect[leg][0] = x;
-        r->expect[leg][1] = s;
-        r->expect[leg][2] = f;
+    static std::string opts_error(const cro_barrier_opts& o) { return barrier_opts_error(o); }
+    static cudaError_t plan(int device, unsigned leg) { return barrier_plan(device, leg); }
+    // BAR and MBAR: one CTA per SM; CLUSTER: as many clusters as the device holds at once.
+    static int grids(cro_ctx* c, const cro_barrier_opts& o, uint32_t legs, int sm_count, int (&grid)[kLegs]) {
+        std::fill(grid, grid + kLegs, sm_count);
+        if (!(legs >> CRO_BARRIER_LEG_CLUSTER & 1u)) return CRO_OK;
+        const uint32_t cluster = cluster_of(o);
+        CU_TRY(c, barrier_cluster_grid(cluster, &grid[CRO_BARRIER_LEG_CLUSTER]));
+        if (grid[CRO_BARRIER_LEG_CLUSTER] < (int)cluster) {
+            c->set_error("barrier probe: the device cannot place one cluster of " + std::to_string(cluster) + " CTAs");
+            return CRO_ERR_UNSUPPORTED;
+        }
+        return CRO_OK;
     }
-    r->table_ns = now_ns() - t0;
-}
+    static cudaError_t launch(const cro_barrier_opts& o, unsigned leg, const BarrierArgs& a, int grid, cudaStream_t st) {
+        return launch_barrier(leg, a, grid, cluster_of(o), st);
+    }
+    // The legs' tables and the closed form of every CTA's fold.
+    static void open(const cro_barrier_opts& o, cro_barrier_result* r, Tables& tb, bool timed) {
+        const uint64_t t0 = now_ns();
+        r->cluster = cluster_of(o);
+        for (unsigned leg = 0; leg < CRO_BARRIER_LEGS; ++leg) {
+            if (!(r->legs >> leg & 1u)) continue;
+            const unsigned n = barrier::kOps[leg];
+            tb.rows[leg].resize(n);
+            tb.words[leg].resize((size_t)n * CRO_BARRIER_THREADS * 2);
+            barrier::table(leg, r->seed, r->cluster, tb.rows[leg].data(), tb.words[leg].data());
+            uint64_t x = 0, s = 0, f = 0;
+            for (uint64_t op = 0; op < n; ++op)
+                for (unsigned t = 0; t < CRO_BARRIER_THREADS; ++t)
+                    barrier::folded(leg, tb.rows[leg][op], tb.words[leg].data() + op * CRO_BARRIER_THREADS * 2, t, [&](uint64_t v) {
+                        x ^= v;
+                        s += v;
+                        f += v * (2 * op + 1);
+                    });
+            r->expect[leg][0] = x;
+            r->expect[leg][1] = s;
+            r->expect[leg][2] = f;
+        }
+        if (timed) r->table_ns = now_ns() - t0;
+    }
+    static std::array<LaneBlob, kBlobs> blobs(const Tables& tb, unsigned leg) {
+        return {LaneBlob{tb.rows[leg].data(), tb.rows[leg].size() * sizeof(cro_barrier_row)},
+                LaneBlob{tb.words[leg].data(), tb.words[leg].size() * sizeof(uint64_t)}};
+    }
+    static void args(const cro_barrier_opts&, const cro_barrier_result&, unsigned, const std::array<const void*, kBlobs>& on_dev,
+                     BarrierArgs* a) {
+        a->rows = static_cast<const cro_barrier_row*>(on_dev[0]);
+        a->words = static_cast<const unsigned long long*>(on_dev[1]);
+    }
+    // A CLUSTER round that reached no new SM ends the leg: the SMs left cannot host a whole cluster.
+    static bool no_new_sm_ends(unsigned leg) { return leg == CRO_BARRIER_LEG_CLUSTER; }
+    static int close(cro_barrier_result* r, LaneTally<BarrierProbe>& t, std::vector<cro_barrier_sm>* sms,
+                     std::vector<cro_barrier_fault>* faults);
+    static void keep(cro_barrier_result* r, const cro_barrier_result& from) {
+        r->cluster = from.cluster;
+        r->table_ns = from.table_ns;
+    }
+};
 
 // The report path's verdict, then the barrier probe's own: the kept timeout records, the coverage, the (SM, peer SM)
 // pairs of every kept CLUSTER record (taken before the records are sorted and capped, so BAR and MBAR records cannot
 // crowd them out), and LINK when only CLUSTER checks failed on a strict subset of the SMs.  A cluster cannot use an SM
 // whose GPC has no room for the whole cluster, so the call's coverage is the CTA-local legs' when one ran, and the
 // CLUSTER leg's own is cluster_sms.
-int close_barrier_call(cro_barrier_result* r, LaneTally<BarrierReport>& t, std::vector<cro_barrier_sm>* sms,
-                       std::vector<cro_barrier_fault>* faults) {
+int BarrierProbe::close(cro_barrier_result* r, LaneTally<BarrierProbe>& t, std::vector<cro_barrier_sm>* sms,
+                        std::vector<cro_barrier_fault>* faults) {
     std::set<std::pair<uint32_t, uint32_t>> pairs;
     for (const cro_barrier_fault& f : t.recs) {
         r->timeouts += f.kind == CRO_BARRIER_KIND_TIMEOUT ? 1 : 0;
         if (f.leg == CRO_BARRIER_LEG_CLUSTER) pairs.insert({f.smid, f.peer_smid});
     }
     r->cluster_sms = (uint32_t)t.seen[CRO_BARRIER_LEG_CLUSTER].size();
-    const int status = close_lane_call<BarrierReport>(r, t, sms, faults);
+    const int status = close_lane_call<BarrierProbe>(r, t, sms, faults);
     if (r->legs & ~(1u << CRO_BARRIER_LEG_CLUSTER)) {
         uint32_t covered = ~0u;
         for (unsigned leg = 0; leg < CRO_BARRIER_LEG_CLUSTER; ++leg)
@@ -331,15 +349,8 @@ void barrier_expected(unsigned leg, uint64_t seed, uint32_t cluster, cro_barrier
 }
 
 std::string barrier_opts_error(const cro_barrier_opts& o) {
-    const uint32_t iters = o.iterations ? o.iterations : kBarrierDefaultIterations, cluster = cluster_of(o);
-    const int leg = o.test_inject_leg;
-    const bool inj_ok = !o.test_inject_mask ||
-                        (leg >= 0 && leg < CRO_BARRIER_LEGS && (legs_of(o) >> leg & 1u) && o.test_inject_sm >= -1 &&
-                         o.test_inject_sm < CRO_BARRIER_MAX_SMS && o.test_inject_warp >= -1 && o.test_inject_warp < CRO_BARRIER_WARPS &&
-                         o.test_inject_lane >= -1 && o.test_inject_lane < 32 && o.test_inject_op < barrier::kOps[leg] &&
-                         o.test_inject_iteration < iters);
-    if (iters > CRO_BARRIER_MAX_ITERATIONS || o.legs > CRO_BARRIER_ALL_LEGS || o.max_rounds > CRO_BARRIER_MAX_ROUNDS || o.deadline_ms < 0 ||
-        (cluster != 2 && cluster != 4 && cluster != 8) || !inj_ok)
+    const uint32_t cluster = cluster_of(o);
+    if (!lane_opts_ok<BarrierProbe>(o) || (cluster != 2 && cluster != 4 && cluster != 8))
         return "barrier probe: iterations at most " + std::to_string(CRO_BARRIER_MAX_ITERATIONS) + ", legs at most 0x7, max_rounds at most " +
                std::to_string(CRO_BARRIER_MAX_ROUNDS) + ", deadline_ms not negative, cluster 2, 4 or 8, and an injection must name a "
                "leg the call runs, an SM id below " + std::to_string(CRO_BARRIER_MAX_SMS) + ", a warp below 8 and a lane below 32 "
@@ -349,159 +360,22 @@ std::string barrier_opts_error(const cro_barrier_opts& o) {
 
 int ctx_probe_barrier(cro_ctx* c, int idx, const cro_barrier_opts& o, cro_barrier_result* r, std::vector<cro_barrier_sm>* sms,
                       std::vector<cro_barrier_fault>* faults) {
-    const uint64_t t_call = now_ns();
-    blank_result(r, cro_barrier_result{}, sms, faults);
-    Device* d = dev_at(c, idx);
-    if (!d)
-        return r->status = unknown_device(c, idx, "a GPU attached after init is probed through the helper process, cro_probe_barrier_uuid");
-    const uint32_t iters = o.iterations ? o.iterations : kBarrierDefaultIterations;
-    const uint32_t max_rounds = o.max_rounds ? o.max_rounds : kBarrierDefaultRounds;
-    const uint32_t legs = legs_of(o), cluster = cluster_of(o);
-    const std::string why = barrier_opts_error(o);
-    if (!why.empty()) {
-        c->set_error(why);
-        return r->status = CRO_ERR_INVALID_ARG;
-    }
-    DeviceGuard g = enter_device(c, idx);
-    if (g.rc) return r->status = g.rc;
-    Range nv(c, "cro.probe_barrier");
-    LaneTally<BarrierReport> t;
-    cudaEvent_t ev[2] = {nullptr, nullptr};                  // the call's own, destroyed on every way out
-    int rc = [&]() -> int {
-        const int sm_count = d->plan.sm_count;
-        for (unsigned leg = 0; leg < CRO_BARRIER_LEGS; ++leg)
-            if (legs >> leg & 1u) CU_TRY(c, barrier_plan(d->ordinal, leg));
-        int net_grid = 0;
-        if (legs >> CRO_BARRIER_LEG_CLUSTER & 1u) {
-            CU_TRY(c, barrier_cluster_grid(cluster, &net_grid));
-            if (net_grid < (int)cluster) {
-                c->set_error("barrier probe: the device cannot place one cluster of " + std::to_string(cluster) + " CTAs");
-                return CRO_ERR_UNSUPPORTED;
-            }
-        }
-        const int max_grid = std::max(sm_count, net_grid);
-        const uint64_t k = d->barrier_calls++;
-        Tables tb;
-        open_barrier_call(r, space_seed(d, kSeedBarrier, k), k, (uint32_t)sm_count, legs, iters, cluster, tb);
-
-        // [CTA entries][thread entries] (armed together every round), then [records], then [rows][words] per leg
-        const size_t n_thr = (size_t)max_grid * CRO_BARRIER_THREADS;
-        const size_t cta_bytes = (size_t)max_grid * sizeof(cro_barrier_cta), thr_bytes = n_thr * sizeof(cro_barrier_thread);
-        const size_t rec_off = (cta_bytes + thr_bytes + 255) & ~(size_t)255, rec_bytes = n_thr * kThreadRecs * sizeof(cro_barrier_fault);
-        size_t row_off[CRO_BARRIER_LEGS], word_off[CRO_BARRIER_LEGS], end = (rec_off + rec_bytes + 255) & ~(size_t)255;
-        for (unsigned leg = 0; leg < CRO_BARRIER_LEGS; ++leg) {
-            row_off[leg] = end;
-            end = (end + tb.rows[leg].size() * sizeof(cro_barrier_row) + 255) & ~(size_t)255;
-            word_off[leg] = end;
-            end += tb.words[leg].size() * sizeof(uint64_t);
-        }
-        DeviceMem<unsigned char> b;
-        CU_TRY(c, cudaMalloc(&b.p, end));
-        for (unsigned leg = 0; leg < CRO_BARRIER_LEGS; ++leg)
-            if (!tb.rows[leg].empty()) {
-                CU_TRY(c, cudaMemcpyAsync(b.p + row_off[leg], tb.rows[leg].data(), tb.rows[leg].size() * sizeof(cro_barrier_row),
-                                          cudaMemcpyHostToDevice, d->stream));
-                CU_TRY(c, cudaMemcpyAsync(b.p + word_off[leg], tb.words[leg].data(), tb.words[leg].size() * sizeof(uint64_t),
-                                          cudaMemcpyHostToDevice, d->stream));
-            }
-        for (cudaEvent_t& x : ev) CU_TRY(c, cudaEventCreate(&x));
-        cudaStream_t st = d->stream;
-        BarrierArgs a{};
-        a.cta = reinterpret_cast<cro_barrier_cta*>(b.p);
-        a.thr = reinterpret_cast<cro_barrier_thread*>(b.p + cta_bytes);
-        a.rec = reinterpret_cast<cro_barrier_fault*>(b.p + rec_off);
-        a.stamp = k;
-        a.iterations = iters;
-        a.inj_sm = o.test_inject_sm;
-        a.inj_warp = o.test_inject_warp;
-        a.inj_lane = o.test_inject_lane;
-        a.inj_op = o.test_inject_op;
-        a.inj_iter = o.test_inject_iteration;
-        std::vector<unsigned char> head(cta_bytes + thr_bytes);
-        std::vector<cro_barrier_fault> hr(n_thr * kThreadRecs);
-        for (unsigned leg = 0; leg < CRO_BARRIER_LEGS; ++leg) {
-            if (!(legs >> leg & 1u)) continue;
-            const int grid = leg == CRO_BARRIER_LEG_CLUSTER ? net_grid : sm_count;
-            // The round's entries sit where the grid's CTA and thread entries end: CTA entries first, then threads.
-            const size_t cb = (size_t)grid * sizeof(cro_barrier_cta), tbytes = (size_t)grid * CRO_BARRIER_THREADS * sizeof(cro_barrier_thread);
-            a.thr = reinterpret_cast<cro_barrier_thread*>(b.p + cb);
-            const auto* hc = reinterpret_cast<const cro_barrier_cta*>(head.data());
-            const auto* ht = reinterpret_cast<const cro_barrier_thread*>(head.data() + cb);
-            a.rows = reinterpret_cast<const cro_barrier_row*>(b.p + row_off[leg]);
-            a.words = reinterpret_cast<const unsigned long long*>(b.p + word_off[leg]);
-            a.inj_mask = o.test_inject_mask && o.test_inject_leg == (int)leg ? o.test_inject_mask : 0ull;
-            auto launch = [&] { return launch_barrier(leg, a, grid, cluster, st); };
-            auto fetch = [&] { return cudaMemcpyAsync(head.data(), b.p, cb + tbytes, cudaMemcpyDeviceToHost, st); };
-            auto take = [&](uint32_t* covered) -> int {
-                if (lane_any_failed<BarrierReport>(ht, grid, k))
-                    CU_TRY(c, cudaMemcpy(hr.data(), a.rec, (size_t)grid * CRO_BARRIER_THREADS * kThreadRecs * sizeof(cro_barrier_fault),
-                                         cudaMemcpyDeviceToHost));
-                const uint32_t before = (uint32_t)t.seen[leg].size();
-                const int e = take_lane_round<BarrierReport>(c, leg, hc, ht, hr.data(), grid, k, r, t, covered);
-                // A CLUSTER round that reached no new SM ends the leg: the SMs left cannot host a whole cluster.
-                if (leg == CRO_BARRIER_LEG_CLUSTER && t.seen[leg].size() == before) *covered = (uint32_t)sm_count;
-                return e;
-            };
-            uint32_t rounds = 0;
-            const int e = coverage_rounds(c, d, ev, b.p, cb + tbytes, (uint32_t)sm_count, max_rounds, &rounds, &r->leg_ns[leg], launch,
-                                          fetch, take);
-            r->rounds += rounds;
-            r->ns += r->leg_ns[leg];
-            if (e) return e;
-        }
-        return CRO_OK;
-    }();
-    for (cudaEvent_t x : ev)
-        if (x) cudaEventDestroy(x);
-    if (rc == CRO_ERR_CUDA) r->cuda_error = (int32_t)cudaGetLastError();
-    if (rc) {
-        blank_result(r, *r, sms, faults);
-        r->wall_ns = now_ns() - t_call;
-        return r->status = rc;
-    }
-    const int status = close_barrier_call(r, t, sms, faults);
-    r->wall_ns = now_ns() - t_call;
-    return status;
+    return probe_lane_legs<BarrierProbe>(c, idx, o, r, sms, faults);
 }
 
 int classify_barrier(uint32_t legs, uint32_t iterations, uint64_t seed, uint32_t cluster, uint32_t sm_count, uint64_t k, uint32_t rounds,
                      const cro_barrier_cta* ctas, const cro_barrier_thread* threads, const cro_barrier_fault* records,
                      cro_barrier_result* r, std::vector<cro_barrier_sm>* sms, std::vector<cro_barrier_fault>* faults) {
-    blank_result(r, cro_barrier_result{}, sms, faults);
-    Tables tb;
-    open_barrier_call(r, seed, k, sm_count, legs, iterations, cluster, tb);
-    r->table_ns = 0;
-    LaneTally<BarrierReport> t;
-    const size_t n_thr = (size_t)sm_count * CRO_BARRIER_THREADS;
-    for (unsigned leg = 0; leg < CRO_BARRIER_LEGS; ++leg) {
-        if (!(legs >> leg & 1u)) continue;
-        for (uint32_t j = 0; j < rounds; ++j, ctas += sm_count, threads += n_thr, records += n_thr * kThreadRecs) {
-            ++r->rounds;
-            uint32_t covered = 0;
-            const int e = take_lane_round<BarrierReport>(nullptr, leg, ctas, threads, records, (int)sm_count, k, r, t, &covered);
-            if (e) {
-                blank_result(r, *r, sms, faults);
-                return r->status = e;
-            }
-        }
-    }
-    return close_barrier_call(r, t, sms, faults);
+    cro_barrier_opts o{};
+    o.legs = legs;
+    o.iterations = iterations;
+    o.cluster = cluster;
+    return classify_lane_legs<BarrierProbe>(o, seed, sm_count, k, rounds, ctas, threads, records, r, sms, faults);
 }
 
 int ctx_probe_barrier_uuid(cro_ctx* c, const char* uuid, const cro_barrier_opts& o, cro_barrier_result* r,
                            std::vector<cro_barrier_sm>* sms, std::vector<cro_barrier_fault>* faults, int cap) {
-    blank_result(r, cro_barrier_result{}, sms, faults);
-    if (!uuid) return r->status = CRO_ERR_INVALID_ARG;
-    const std::string why = barrier_opts_error(o);
-    if (!why.empty()) {
-        set_call_error(c, why);
-        return r->status = CRO_ERR_INVALID_ARG;
-    }
-    uint64_t helper_ns = 0;
-    if (run_check_helper(c, cro_wire_barrier, uuid, "barrier helper", "cro.probe_barrier.helper", &o, cap, o.deadline_ms, &helper_ns, r,
-                         faults, sms) == CRO_OK)
-        r->helper_ns = helper_ns;
-    return r->status;
+    return probe_lane_legs_uuid<BarrierProbe>(c, uuid, o, r, sms, faults, cap);
 }
 
 }  // namespace cro
