@@ -60,7 +60,7 @@ class Opts(ctypes.Structure):
         ("read_variant", ctypes.c_uint32), ("copy_variant", ctypes.c_uint32), ("deadline_ms", ctypes.c_int32),
         ("n_devices", ctypes.c_int32), ("devices", ctypes.c_int32 * MAX_DEVICES),
         ("rank_base", ctypes.c_uint32), ("world_override", ctypes.c_uint32),
-        ("test_inject_after", ctypes.c_uint32), ("reserved0", ctypes.c_uint32),
+        ("test_inject_after", ctypes.c_uint32), ("test_inject_count", ctypes.c_uint32),
         ("test_inject_word", ctypes.c_uint64), ("test_inject_mask", ctypes.c_uint64),
     ]
 
@@ -925,7 +925,7 @@ class SramRecord(ctypes.Structure):
  SELFTEST_SWEEP_READ_TMA, SELFTEST_SWEEP_READ_LDG256, SELFTEST_SWEEP_LOCATE, SELFTEST_SWEEP_FORCE_WORDS,
  SELFTEST_SWEEP_LINK_READ, SELFTEST_SWEEP_LINK_WRITE) = range(1, 12)
 SELFTEST_LAYOUT_SRC_DST, SELFTEST_LAYOUT_DST_SRC, SELFTEST_LAYOUT_APART = 1, 2, 3
-SELFTEST_GUARD_BYTES, SELFTEST_F_INTERIORS = 2 << 20, 1
+SELFTEST_GUARD_BYTES, SELFTEST_F_INTERIORS, SELFTEST_F_XOR = 2 << 20, 1, 2
 
 
 class SelftestSweepOpts(ctypes.Structure):
@@ -1054,9 +1054,15 @@ class LocateRecord(ctypes.Structure):
 
 
 class SweepSlot(ctypes.Structure):
-    """cro_sweep_slot: one sweep's result slot as the kernels write it."""
+    """cro_sweep_slot: one sweep's result slot as the kernels write it.  Its last word is the header's union of
+    `mismatches` and `pad`: kept as `pad` here, read as `mismatches`."""
     _fields_ = [("x", ctypes.c_uint64), ("s", ctypes.c_uint64), ("w", ctypes.c_uint64), ("t0", ctypes.c_uint64),
                 ("t1", ctypes.c_uint64), ("stamp", ctypes.c_uint64), ("n_words", ctypes.c_uint64), ("pad", ctypes.c_uint64)]
+
+    @property
+    def mismatches(self) -> int:
+        """A comparing read's count of words that differ from the pattern (0 from a read that only folds)."""
+        return self.pad
 
 
 LINK_SLOTS = LINK_WORD_CHECKS + 5             # [k] check k's fold, two write roles, the closed forms of P1, P2, P3
@@ -2244,7 +2250,7 @@ class ProbeContext:
                  read_sweeps: int = 0, copy_sweeps: int = 0, read_variant: int = READ_AUTO,
                  copy_variant: int = COPY_AUTO, p2p_bytes: int = 0, latency_hops: int = 0,
                  deadline_ms: int = 0, seed_base: int = 0, rank_base: int = 0, world: int = 0,
-                 inject: Optional[Tuple[int, int, int]] = None) -> None:
+                 inject: Optional[Tuple[int, ...]] = None) -> None:
         o = Opts()
         o.abi_version = ABI_VERSION
         o.flags = flags
@@ -2256,9 +2262,10 @@ class ProbeContext:
         o.read_variant, o.copy_variant = read_variant, copy_variant
         o.deadline_ms = deadline_ms
         o.rank_base, o.world_override = rank_base, world
-        if inject is not None:            # (after sweep number, word index, xor mask): fault injection inside the probe
+        if inject is not None:            # (after sweep number, word index, xor mask[, words]): fault injection inside the probe
             o.flags |= F_TEST_INJECT
-            o.test_inject_after, o.test_inject_word, o.test_inject_mask = inject
+            o.test_inject_after, o.test_inject_word, o.test_inject_mask = inject[:3]
+            o.test_inject_count = inject[3] if len(inject) > 3 else 0
         if devices:
             o.n_devices = len(devices)
             for i, d in enumerate(devices):
@@ -2640,17 +2647,18 @@ class ProbeContext:
 
     def selftest_sweep(self, dev: int, kernel: int, bytes: int, offset: int = 0, layout: int = 0, seed: int = 0,
                        canary: int = 0, invert: int = 0, word0: int = 0, force: List[Tuple[int, int, int, int]] = (),
-                       interiors: bool = False, alloc=bytearray, cap: int = 16):
+                       interiors: bool = False, alloc=bytearray, cap: int = 16, xor: bool = False):
         """One SELFTEST_SWEEP_* kernel on a buffer of the hook's own: guards holding canary words (word j of guard g:
         pattern_word(canary, g * 2^32 + j)) around the interior(s), a copy's in the SELFTEST_LAYOUT_* given.  force: up
-        to two (first, count, and_mask, or_mask) interior ranges.  Returns (SelftestSweepOut, the buffer as alloc(buf_bytes) made it, with the guards and,
+        to two (first, count, and_mask, or_mask) interior ranges; with xor, each word of a range is XORed with or_mask
+        (and_mask all ones).  Returns (SelftestSweepOut, the buffer as alloc(buf_bytes) made it, with the guards and,
         if interiors, the interiors at their offsets, and up to `cap` of the kernel's records by word)."""
         o = SelftestSweepOpts()
         o.kernel, o.layout, o.offset, o.bytes, o.seed, o.canary = kernel, layout, offset, bytes, seed, canary
         o.invert, o.word0 = invert, word0
         for r, (first, count, and_mask, or_mask) in enumerate(force):
             o.force_first[r], o.force_count[r], o.force_and[r], o.force_or[r] = first, count, and_mask, or_mask
-        o.flags = SELFTEST_F_INTERIORS if interiors else 0
+        o.flags = (SELFTEST_F_INTERIORS if interiors else 0) | (SELFTEST_F_XOR if xor else 0)
         out = SelftestSweepOut()
         arr = (FaultWord * max(1, cap))()
         n = ctypes.c_int()

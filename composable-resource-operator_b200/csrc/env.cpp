@@ -16,7 +16,7 @@ const Knob kKnobs[] = {
     {"CRO_COPY_WAVES", 1, 1024, 128, 0, "CTA waves of the LDG copy kernel"},
     {"CRO_TMA_READ_TILE", 1024, 114688, 32768, 16, "bytes per TMA bulk load of the read ring"},
     {"CRO_TMA_READ_STAGES", 2, 16, 4, 0, "ring depth of the read kernel"},
-    {"CRO_TMA_READ_THREADS", 64, 1024, 160, 32, "1 producer warp + consumer warps"},
+    {"CRO_TMA_READ_THREADS", 64, 1024, 1024, 32, "1 producer warp + consumer warps"},
     {"CRO_TMA_READ_CHUNK", 1, 4096, 1, 0, "tiles claimed per atomic"},
     {"CRO_TMA_READ_HINT", 0, 1, 0, 0, "1 = L2 evict_first on the bulk loads"},
     {"CRO_TMA_READ_DYN", 0, 1, 1, 0, "1 = dynamic tile claims"},

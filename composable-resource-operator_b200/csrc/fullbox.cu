@@ -357,8 +357,10 @@ int ctx_probe_all(cro_ctx* c, cro_probe_result* out, int cap, int* n_out) {
                     break;
                 case CRO_P2P_OP_READ:
                     // TMA bulk copies straight out of the peer's HBM (cp.async.bulk on the peer-mapped address) into this
-                    // GPU's shared memory, checksummed as they land
-                    CU_TRY(c, launch_read(d->plan, rvp, p->region, op.bytes, imm_params(d), d->scratch, &d->d_out[op.slot], d->stream));
+                    // GPU's shared memory, checksummed as they land.  Fold only, as is the re-read below: the words are the
+                    // peer's pattern, and p2p_finalize compares the fold with the peer's own closed form.
+                    CU_TRY(c, launch_read(d->plan, rvp, p->region, op.bytes, imm_params(d), d->scratch, &d->d_out[op.slot], d->stream,
+                                          /*compare=*/false));
                     c->launches++;
                     break;
                 case CRO_P2P_OP_PUSH:
@@ -371,7 +373,7 @@ int ctx_probe_all(cro_ctx* c, cro_probe_result* out, int cap, int* n_out) {
                 case CRO_P2P_OP_REREAD:
                     d->half_known[1] = false;                        // its prefix now holds p's pattern
                     CU_TRY(c, launch_read(d->plan, resolve_read_variant(CRO_READ_AUTO, op.bytes, c->knobs), d->region + d->sweep_bytes,
-                                          op.bytes, imm_params(d), d->scratch, &d->d_out[op.slot], d->stream));
+                                          op.bytes, imm_params(d), d->scratch, &d->d_out[op.slot], d->stream, /*compare=*/false));
                     c->launches++;
                     break;
                 case CRO_P2P_OP_CHASE: {

@@ -236,7 +236,7 @@ int ctx_probe_host_link(cro_ctx* c, int idx, const cro_link_opts& o, cro_link_re
         };
         auto inject_b = [&](int check) -> int {
             if (!inj || o.test_inject_check != check) return CRO_OK;
-            CU_TRY(c, launch_xor_word(B, o.test_inject_word, o.test_inject_mask, st));
+            CU_TRY(c, launch_xor_words(B, o.test_inject_word, 1, o.test_inject_mask, st));
             c->launches++;
             return CRO_OK;
         };

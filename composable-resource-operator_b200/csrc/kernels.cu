@@ -5,7 +5,8 @@
 // slot (SURVEY.md §2b, §8d).  They are HBM-bound integer sweeps:
 //
 //   hbm_fill          S bytes written   w[i] = splitmix64-step(seed + i)
-//   hbm_read_*        S bytes read      (XOR, wrapping sum, position-weighted sum) of all words
+//   hbm_read_*        S bytes read      (XOR, wrapping sum, position-weighted sum) of all words; the probe's
+//                                       reads also compare every word with its closed form and count mismatches
 //   hbm_copy_fused    2S bytes moved    + the same checksum of the source stream, folded out of shared memory
 //   hbm_copy_*        2S bytes moved    (plain variants, kept for comparison)
 //   hbm_expected      0 bytes           the same checksum from the closed form
@@ -208,36 +209,46 @@ __device__ __forceinline__ unsigned long long acc_w(const Acc& A) { return A.w +
 // ---------------------------------------------------------------------------
 // CTA reduction + "last CTA publishes" epilogue shared by read / fused copy /
 // expected.  The last CTA also re-arms the scratch (ticket, timers, dynamic
-// tile counter), so no memset node sits between two sweeps.
+// tile counter), so no memset node sits between two sweeps.  COUNT (the read
+// sweeps): m, the thread's count of mismatching words, is summed in the
+// partials' fourth lane and published as out->mismatches.
 // ---------------------------------------------------------------------------
+template <bool COUNT = false>
 __device__ __forceinline__ void publish(unsigned long long x, unsigned long long s, unsigned long long w,
                                         unsigned long long t_start, const SweepScratch sc,
                                         SweepOut* out, const ProbeParams& imm, const ProbeParams* pp,
-                                        unsigned long long n_words) {
+                                        unsigned long long n_words, unsigned long long m = 0) {
     __shared__ unsigned long long sx[32], ss[32], sw[32];
+    __shared__ unsigned long long sm[COUNT ? 32 : 1];
     __shared__ bool is_last;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         x ^= __shfl_xor_sync(0xffffffffu, x, o);
         s += __shfl_xor_sync(0xffffffffu, s, o);
         w += __shfl_xor_sync(0xffffffffu, w, o);
+        if constexpr (COUNT) m += __shfl_xor_sync(0xffffffffu, m, o);
     }
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nwarps = (blockDim.x + 31) >> 5;
-    if (lane == 0) { sx[warp] = x; ss[warp] = s; sw[warp] = w; }
+    if (lane == 0) {
+        sx[warp] = x; ss[warp] = s; sw[warp] = w;
+        if constexpr (COUNT) sm[warp] = m;
+    }
     __syncthreads();
     if (warp == 0) {
         x = lane < nwarps ? sx[lane] : 0ull;
         s = lane < nwarps ? ss[lane] : 0ull;
         w = lane < nwarps ? sw[lane] : 0ull;
+        if constexpr (COUNT) m = lane < nwarps ? sm[lane] : 0ull;
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
             x ^= __shfl_xor_sync(0xffffffffu, x, o);
             s += __shfl_xor_sync(0xffffffffu, s, o);
             w += __shfl_xor_sync(0xffffffffu, w, o);
+            if constexpr (COUNT) m += __shfl_xor_sync(0xffffffffu, m, o);
         }
         if (lane == 0) {
-            sc.partials[blockIdx.x] = make_ulonglong4(x, s, w, 0ull);
+            sc.partials[blockIdx.x] = make_ulonglong4(x, s, w, COUNT ? m : 0ull);
             atomicMin(sc.tmin, t_start);
             atomicMax(sc.tmax, globaltimer_ns());
             __threadfence();
@@ -249,19 +260,25 @@ __device__ __forceinline__ void publish(unsigned long long x, unsigned long long
     if (!is_last) return;
     __threadfence();
     x = 0; s = 0; w = 0;
+    if constexpr (COUNT) m = 0;
     for (unsigned i = threadIdx.x; i < gridDim.x; i += blockDim.x) {
         const ulonglong2* q = reinterpret_cast<const ulonglong2*>(&sc.partials[i]);
         const ulonglong2 p0 = __ldcg(q), p1 = __ldcg(q + 1);
         x ^= p0.x; s += p0.y; w += p1.x;
+        if constexpr (COUNT) m += p1.y;
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         x ^= __shfl_xor_sync(0xffffffffu, x, o);
         s += __shfl_xor_sync(0xffffffffu, s, o);
         w += __shfl_xor_sync(0xffffffffu, w, o);
+        if constexpr (COUNT) m += __shfl_xor_sync(0xffffffffu, m, o);
     }
     __syncthreads();
-    if (lane == 0) { sx[warp] = x; ss[warp] = s; sw[warp] = w; }
+    if (lane == 0) {
+        sx[warp] = x; ss[warp] = s; sw[warp] = w;
+        if constexpr (COUNT) sm[warp] = m;
+    }
     __syncthreads();
     if (threadIdx.x == 0) {
         x = 0; s = 0; w = 0;
@@ -269,6 +286,11 @@ __device__ __forceinline__ void publish(unsigned long long x, unsigned long long
         out->x = x;
         out->s = s;
         out->w = w;
+        if constexpr (COUNT) {
+            m = 0;
+            for (int k = 0; k < nwarps; ++k) m += sm[k];
+            out->mismatches = m;
+        }
         out->t0 = *((volatile unsigned long long*)sc.tmin);
         out->t1 = *((volatile unsigned long long*)sc.tmax);
         out->stamp = pp ? pp->nonce : imm.nonce;
@@ -347,15 +369,55 @@ hbm_fill_kernel(uint4* __restrict__ base, unsigned long long n_vec, const ProbeP
 }
 
 // ---------------------------------------------------------------------------
+// The word compare of the locator and the comparing read sweeps: vector
+// v0 + j * vstride holds words (a[j], b[j]), which should be pattern words
+// 2v and 2v + 1 (^ invert).  d[2j], d[2j + 1] get the differences; bit k of
+// the result is set when d[k] != 0.
+// ---------------------------------------------------------------------------
+template <int J>
+__device__ __forceinline__ unsigned compare_words(const unsigned long long (&a)[J], const unsigned long long (&b)[J],
+                                                  unsigned long long v0, unsigned long long vstride,
+                                                  unsigned long long seed, unsigned long long invert,
+                                                  unsigned long long (&d)[2 * J]) {
+    unsigned m = 0;
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+        const unsigned long long v = v0 + (unsigned long long)j * vstride;
+        d[2 * j] = a[j] ^ pattern_word(seed, 2 * v) ^ invert;
+        d[2 * j + 1] = b[j] ^ pattern_word(seed, 2 * v + 1) ^ invert;
+        m |= (d[2 * j] != 0 ? 1u : 0u) << (2 * j);
+        m |= (d[2 * j + 1] != 0 ? 1u : 0u) << (2 * j + 1);
+    }
+    return m;
+}
+
+// A comparing read's count of the mismatching words among J vectors (compare_words).  A read keeps no records, so it
+// needs neither the locator's ballot nor its atomics: each thread counts its own words and publish sums the counts.
+template <int J>
+__device__ __forceinline__ unsigned count_mismatches(const unsigned long long (&a)[J], const unsigned long long (&b)[J],
+                                                     unsigned long long v0, unsigned long long vstride,
+                                                     unsigned long long seed) {
+    unsigned long long d[2 * J];
+    return (unsigned)__popc(compare_words<J>(a, b, v0, vstride, seed, 0ull, d));
+}
+
+// ---------------------------------------------------------------------------
 // hbm_read (LDG path): UNROLL independent 128-bit ld.global.nc per thread in
 // flight, read-only path, no L1 allocation.  Also usable on a peer-mapped
-// pointer (NVLink read).
+// pointer (NVLink read).  CMP: every word is also compared with
+// pattern_word(seed, i), i counted from base (count_mismatches); the exact
+// count is published as out->mismatches (0 without CMP).
 // ---------------------------------------------------------------------------
-template <int THREADS, bool WIDE>
-__global__ void __launch_bounds__(THREADS)
+// The 16-byte flavour asks for two CTAs per SM: the compare's regeneration of the pattern is ALU work, and 32 warps
+// per SM hide it behind the loads where the 16 its registers would otherwise allow do not (H100, 4 GiB: 3.07 against
+// 2.42 TB/s).  The 32-byte flavour keeps its registers: held to two CTAs it read at 2.40 TB/s, not 2.84.
+template <int THREADS, bool WIDE, bool CMP>
+__global__ void __launch_bounds__(THREADS, WIDE ? 1 : 2)
 hbm_read_ldg_kernel(const uint4* __restrict__ base, unsigned long long n_vec, const ProbeParams imm,
                     const ProbeParams* __restrict__ pp, SweepScratch sc, SweepOut* out) {
     const unsigned long long t_start = globaltimer_ns();
+    const unsigned long long seed = CMP ? (pp ? pp->seed : imm.seed) : 0ull;
+    unsigned long long mism = 0;
     Acc A, B;
     constexpr unsigned long long tile_vecs = (unsigned long long)THREADS * 8;  // 128 B / thread
     const unsigned long long n_tiles = n_vec / tile_vecs;
@@ -373,6 +435,13 @@ hbm_read_ldg_kernel(const uint4* __restrict__ base, unsigned long long n_vec, co
                 fold2(A, w[4 * j], w[4 * j + 1], 4 * v + 1);
                 fold2(B, w[4 * j + 2], w[4 * j + 3], 4 * (v + 1) + 1);
             }
+            if constexpr (CMP) {
+                // the even and the odd 16-byte vector of each 32-byte one: strides of 2T vectors
+                const unsigned long long a0[4] = {w[0], w[4], w[8], w[12]}, b0[4] = {w[1], w[5], w[9], w[13]};
+                const unsigned long long a1[4] = {w[2], w[6], w[10], w[14]}, b1[4] = {w[3], w[7], w[11], w[15]};
+                mism += count_mismatches<4>(a0, b0, v0, 2ull * THREADS, seed);
+                mism += count_mismatches<4>(a1, b1, v0 + 1, 2ull * THREADS, seed);
+            }
         } else {
             const unsigned long long v0 = tile * tile_vecs + threadIdx.x;
             unsigned long long a[8], b[8];
@@ -382,6 +451,7 @@ hbm_read_ldg_kernel(const uint4* __restrict__ base, unsigned long long n_vec, co
                 fold2(A, a[j], b[j], 4 * (v0 + (unsigned long long)j * THREADS) + 1);
                 fold2(B, a[j + 1], b[j + 1], 4 * (v0 + (unsigned long long)(j + 1) * THREADS) + 1);
             }
+            if constexpr (CMP) mism += count_mismatches<8>(a, b, v0, THREADS, seed);
         }
     }
     for (unsigned long long i = n_tiles * tile_vecs + (unsigned long long)blockIdx.x * THREADS +
@@ -389,8 +459,12 @@ hbm_read_ldg_kernel(const uint4* __restrict__ base, unsigned long long n_vec, co
          i < n_vec; i += (unsigned long long)gridDim.x * THREADS) {
         const uint4 v = ldg_stream(base + i);
         fold2(A, lo64(v), hi64(v), 4 * i + 1);
+        if constexpr (CMP) {
+            const unsigned long long a[1] = {lo64(v)}, b[1] = {hi64(v)};
+            mism += count_mismatches<1>(a, b, i, 0ull, seed);
+        }
     }
-    publish(acc_x(A) ^ acc_x(B), A.s + B.s, acc_w(A) + acc_w(B), t_start, sc, out, imm, pp, 2 * n_vec);
+    publish<true>(acc_x(A) ^ acc_x(B), A.s + B.s, acc_w(A) + acc_w(B), t_start, sc, out, imm, pp, 2 * n_vec, mism);
 }
 
 // ---------------------------------------------------------------------------
@@ -490,15 +564,7 @@ hbm_locate_kernel(const uint4* __restrict__ base, unsigned long long n_vec, unsi
             fold2(B, a[j + 1], b[j + 1], 4 * (v0 + (unsigned long long)(j + 1) * THREADS) + 1);
         }
         unsigned long long d[16];
-        unsigned m = 0;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const unsigned long long v = v0 + (unsigned long long)j * THREADS;
-            d[2 * j] = a[j] ^ pattern_word(seed, 2 * v) ^ invert;
-            d[2 * j + 1] = b[j] ^ pattern_word(seed, 2 * v + 1) ^ invert;
-            m |= (d[2 * j] != 0 ? 1u : 0u) << (2 * j);
-            m |= (d[2 * j + 1] != 0 ? 1u : 0u) << (2 * j + 1);
-        }
+        const unsigned m = compare_words<8>(a, b, v0, THREADS, seed, invert, d);
         if (__ballot_sync(0xffffffffu, m != 0)) locate_record<16>(d, m, v0, THREADS, L);
     }
     // ragged tail: warp-uniform trip count, so the ballot sees the whole warp
@@ -670,8 +736,12 @@ __global__ void force_words_kernel(unsigned long long* base, unsigned long long 
 // Consumer side shared by the TMA read kernel and the checksumming copy: folds
 // one landed tile out of shared memory with conflict-free LDS.128.
 // v_tile = index (in 16-byte vectors, relative to the sweep's base) of the tile's first vector.
+// CMP (the comparing read): every word is also compared with its pattern word of `seed`, and *mism counts the ones
+// that differ.
+template <bool CMP = false>
 __device__ __forceinline__ void fold_tile(Acc& A, Acc& B, const uint4* sp, unsigned nvec, unsigned ctid,
-                                          unsigned n_cons, unsigned long long v_tile) {
+                                          unsigned n_cons, unsigned long long v_tile,
+                                          unsigned long long seed = 0, unsigned long long* mism = nullptr) {
     unsigned i = ctid;
     // 4 independent LDS.128 per trip
     for (; i + 3 * n_cons < nvec; i += 4 * n_cons) {
@@ -681,10 +751,18 @@ __device__ __forceinline__ void fold_tile(Acc& A, Acc& B, const uint4* sp, unsig
         fold2(B, lo64(b), hi64(b), m + step);
         fold2(A, lo64(c), hi64(c), m + 2 * step);
         fold2(B, lo64(d), hi64(d), m + 3 * step);
+        if constexpr (CMP) {
+            const unsigned long long lo[4] = {lo64(a), lo64(b), lo64(c), lo64(d)}, hi[4] = {hi64(a), hi64(b), hi64(c), hi64(d)};
+            *mism += count_mismatches<4>(lo, hi, v_tile + i, n_cons, seed);
+        }
     }
     for (; i < nvec; i += n_cons) {
         const uint4 a = sp[i];
         fold2(A, lo64(a), hi64(a), 4 * (v_tile + i) + 1);
+        if constexpr (CMP) {
+            const unsigned long long lo[1] = {lo64(a)}, hi[1] = {hi64(a)};
+            *mism += count_mismatches<1>(lo, hi, v_tile + i, 0ull, seed);
+        }
     }
 }
 
@@ -692,8 +770,10 @@ __device__ __forceinline__ void fold_tile(Acc& A, Acc& B, const uint4* sp, unsig
 // hbm_read (TMA path): warp 0 / lane 0 is the producer, issuing 1-D bulk
 // copies of `tile_bytes` into a `stages`-deep shared-memory ring; the consumer
 // warps fold each landed tile and hand the slot back through an "empty"
-// mbarrier.  Bytes in flight per SM = stages*tile.
+// mbarrier.  Bytes in flight per SM = stages*tile.  CMP: the consumers also
+// compare every word (fold_tile<true>), as the LDG read does.
 // ---------------------------------------------------------------------------
+template <bool CMP>
 __global__ void __launch_bounds__(1024, 1)
 hbm_read_tma_kernel(const unsigned char* __restrict__ base, unsigned long long bytes,
                     unsigned tile_bytes, unsigned stages, unsigned chunk,
@@ -709,6 +789,8 @@ hbm_read_tma_kernel(const unsigned char* __restrict__ base, unsigned long long b
     const unsigned long long n_tiles = (bytes + tile_bytes - 1) / tile_bytes;
     const unsigned hint = chunk >> 16;   // bit 0: L2 evict_first on the loads
     chunk &= 0xFFFFu;
+    const unsigned long long seed = CMP ? (pp ? pp->seed : imm.seed) : 0ull;
+    unsigned long long mism = 0;
 
     if (threadIdx.x == 0) {
         for (unsigned s = 0; s < stages; ++s) {
@@ -766,13 +848,14 @@ hbm_read_tma_kernel(const unsigned char* __restrict__ base, unsigned long long b
             const unsigned long long off = tile * tile_bytes;
             const unsigned long long left = bytes - off;
             const unsigned nvec = (left < tile_bytes ? (unsigned)left : tile_bytes) >> 4;
-            fold_tile(A, B, reinterpret_cast<const uint4*>(ring + (size_t)stage * tile_bytes), nvec, ctid, n_cons, off >> 4);
+            fold_tile<CMP>(A, B, reinterpret_cast<const uint4*>(ring + (size_t)stage * tile_bytes), nvec, ctid, n_cons, off >> 4,
+                           seed, &mism);
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty_bar[stage]);
             if (++stage == stages) { stage = 0; phase ^= 1u; }
         }
     }
-    publish(acc_x(A) ^ acc_x(B), A.s + B.s, acc_w(A) + acc_w(B), t_start, sc, out, imm, pp, bytes >> 3);
+    publish<true>(acc_x(A) ^ acc_x(B), A.s + B.s, acc_w(A) + acc_w(B), t_start, sc, out, imm, pp, bytes >> 3, mism);
 }
 
 // ---------------------------------------------------------------------------
@@ -895,6 +978,8 @@ hbm_copy_tma_kernel(unsigned char* __restrict__ dst, const unsigned char* __rest
 // The sweep therefore yields the checksum of its SOURCE as actually read at
 // no extra HBM traffic.  The probe runs its copy sweeps ping-pong (A->B, B->A,
 // ...), so the fold of sweep k+1 is the verification of what sweep k WROTE.
+// It compares no word: a multi-word fault the fold cannot see (DESIGN.md §3) is
+// carried into every later copy, and the comparing read of that half finds it.
 //   warp 0 lane 0: producer — claims tiles, issues bulk loads, issues the bulk
 //                  store of a tile as soon as it has landed, refills a slot
 //                  once both its store has read it (bulk-group wait) and the
@@ -1028,9 +1113,11 @@ hbm_expected_kernel(unsigned long long n_words, const ProbeParams imm,
     publish(x, s, w, t_start, sc, out, imm, pp, n_words);
 }
 
-__global__ void xor_word_kernel(unsigned long long* base, unsigned long long idx,
-                                unsigned long long mask) {
-    base[idx] ^= mask;
+__global__ void xor_words_kernel(unsigned long long* base, unsigned long long first, unsigned long long count,
+                                 unsigned long long mask) {
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < count;
+         i += (unsigned long long)gridDim.x * blockDim.x)
+        base[first + i] ^= mask;
 }
 
 // Latency: dependent loads, system scope, one slot per 128-byte line.  Warp j
@@ -1121,14 +1208,15 @@ probe_finalize_kernel(const FinalizeArgs a) {
         else if (!same_fold(s, E)) fail(CRO_FAIL_COPY_SRC, i);
         else if (i > 0) ++verified;            // sweep i-1's destination reproduced the pattern
     }
-    // read sweep 0 reads the last copy's destination
+    // read sweep 0 reads the last copy's destination.  A read also compares every word: its fold can match while words
+    // differ (a multi-word fault that cancels in the fold, carried through every copy), and then its count does not.
     const SweepOut* shown = &sl[kSlotSweep0 + C];
     for (unsigned i = 0; i < R; ++i) {
         const SweepOut& s = sl[kSlotSweep0 + C + i];
         tr[i] = s.t1 - s.t0;
         bool ok = true;
         if (s.stamp != nonce || s.n_words != n_words) { if (status == CRO_OK) shown = &s; fail(CRO_FAIL_STALE, 1 + C + i); ok = false; }
-        else if (!same_fold(s, E)) { if (status == CRO_OK) shown = &s; fail(CRO_FAIL_READ, i); ok = false; }
+        else if (!same_fold(s, E) || s.mismatches != 0) { if (status == CRO_OK) shown = &s; fail(CRO_FAIL_READ, i); ok = false; }
         if (i == 0 && ok && C > 0) ++verified;
     }
     r->checksum_xor = shown->x; r->checksum_sum = shown->s; r->checksum_wsum = shown->w;
@@ -1443,11 +1531,11 @@ cudaError_t plan_kernels(int device, const env::Values& knobs, KernelPlan* plan,
         return e;
     plan->fill = {sms * (occ > 0 ? occ : 1) * (int)knob("CRO_FILL_WAVES"), kFillThreads, 0};
 
-    auto rd = hbm_read_ldg_kernel<kReadThreads, false>;
+    auto rd = hbm_read_ldg_kernel<kReadThreads, false, true>;
     if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, rd, kReadThreads, 0)) != cudaSuccess)
         return e;
     plan->read_ldg = {sms * (occ > 0 ? occ : 1) * (int)knob("CRO_READ_WAVES"), kReadThreads, 0};
-    auto rdw = hbm_read_ldg_kernel<kReadThreads, true>;
+    auto rdw = hbm_read_ldg_kernel<kReadThreads, true, true>;
     if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, rdw, kReadThreads, 0)) != cudaSuccess)
         return e;
     plan->read_ldg256 = {sms * (occ > 0 ? occ : 1) * (int)knob("CRO_READ_WAVES"), kReadThreads, 0};
@@ -1491,7 +1579,9 @@ cudaError_t plan_kernels(int device, const env::Values& knobs, KernelPlan* plan,
         plan->read_dyn = knob("CRO_TMA_READ_DYN");
         const int threads = (int)knob("CRO_TMA_READ_THREADS");
         const size_t smem = (size_t)plan->read_tile * plan->read_stages;
-        if ((e = plan_ring((const void*)hbm_read_tma_kernel, "CRO_TMA_READ_TILE", smem, threads)) != cudaSuccess)
+        // both instances: the comparing one sets the occupancy the grid is planned for
+        if ((e = plan_ring((const void*)hbm_read_tma_kernel<false>, "CRO_TMA_READ_TILE", smem, threads)) != cudaSuccess ||
+            (e = plan_ring((const void*)hbm_read_tma_kernel<true>, "CRO_TMA_READ_TILE", smem, threads)) != cudaSuccess)
             return e;
         plan->read_tma = {sms * occ * (int)knob("CRO_TMA_READ_WAVES"), threads, smem};
     }
@@ -1520,7 +1610,8 @@ cudaError_t plan_kernels(int device, const env::Values& knobs, KernelPlan* plan,
     // whole generator.  The generator and the kernels it may run beside therefore ask for the SAME split, the largest
     // shared memory.  That includes the fill: in cro_probe_all it runs beside the generator of the NVLink prefix.  Not
     // the LDG kernels: they never run beside a generator, and they want the L1 the smallest split would take away.
-    for (const void* fn : {(const void*)hbm_expected_kernel, (const void*)hbm_read_tma_kernel, (const void*)hbm_copy_fused_kernel,
+    for (const void* fn : {(const void*)hbm_expected_kernel, (const void*)hbm_read_tma_kernel<false>,
+                           (const void*)hbm_read_tma_kernel<true>, (const void*)hbm_copy_fused_kernel,
                            (const void*)hbm_copy_tma_kernel, (const void*)probe_finalize_kernel})
         if ((e = cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)) != cudaSuccess)
             return e;
@@ -1586,16 +1677,17 @@ cudaError_t launch_link_stream(const LinkRole& rd, const LinkRole& wr, const Loc
 }
 
 cudaError_t launch_read(const KernelPlan& p, unsigned variant, const void* base, uint64_t bytes,
-                        const Params& pr, const SweepScratch& sc, SweepOut* out, cudaStream_t st) {
+                        const Params& pr, const SweepScratch& sc, SweepOut* out, cudaStream_t st, bool compare) {
     if (variant == READ_TMA) {
-        hbm_read_tma_kernel<<<clamp_grid(p.read_tma.grid, bytes, p.read_tile), p.read_tma.block, p.read_tma.smem, st>>>(
+        auto k = compare ? hbm_read_tma_kernel<true> : hbm_read_tma_kernel<false>;
+        k<<<clamp_grid(p.read_tma.grid, bytes, p.read_tile), p.read_tma.block, p.read_tma.smem, st>>>(
             static_cast<const unsigned char*>(base), bytes, p.read_tile, p.read_stages, p.read_chunk,
             (p.read_dyn && sc.tile_ctr) ? sc.tile_ctr : nullptr, pr.imm, pr.pp, sc, out);
-    } else if (variant == READ_LDG256) {
-        hbm_read_ldg_kernel<kReadThreads, true><<<clamp_grid(p.read_ldg256.grid, bytes, kReadThreads * 128), p.read_ldg256.block, 0, st>>>(
-            static_cast<const uint4*>(base), bytes >> 4, pr.imm, pr.pp, sc, out);
     } else {
-        hbm_read_ldg_kernel<kReadThreads, false><<<clamp_grid(p.read_ldg.grid, bytes, kReadThreads * 128), p.read_ldg.block, 0, st>>>(
+        const bool wide = variant == READ_LDG256;
+        auto k = wide ? (compare ? hbm_read_ldg_kernel<kReadThreads, true, true> : hbm_read_ldg_kernel<kReadThreads, true, false>)
+                      : (compare ? hbm_read_ldg_kernel<kReadThreads, false, true> : hbm_read_ldg_kernel<kReadThreads, false, false>);
+        k<<<clamp_grid((wide ? p.read_ldg256 : p.read_ldg).grid, bytes, kReadThreads * 128), kReadThreads, 0, st>>>(
             static_cast<const uint4*>(base), bytes >> 4, pr.imm, pr.pp, sc, out);
     }
     return cudaGetLastError();
@@ -1635,8 +1727,10 @@ cudaError_t launch_expected(const KernelPlan& p, uint64_t bytes, const Params& p
     return cudaGetLastError();
 }
 
-cudaError_t launch_xor_word(void* base, uint64_t word_index, uint64_t mask, cudaStream_t st) {
-    xor_word_kernel<<<1, 1, 0, st>>>(static_cast<unsigned long long*>(base), word_index, mask);
+cudaError_t launch_xor_words(void* base, uint64_t first, uint64_t count, uint64_t mask, cudaStream_t st) {
+    if (count == 0) return cudaSuccess;
+    const uint64_t blocks = std::min<uint64_t>((count + 255) / 256, 1024);
+    xor_words_kernel<<<(unsigned)blocks, 256, 0, st>>>(static_cast<unsigned long long*>(base), first, count, mask);
     return cudaGetLastError();
 }
 

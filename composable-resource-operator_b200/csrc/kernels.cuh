@@ -29,11 +29,13 @@ struct SweepOut {
     unsigned long long t1;      // max %globaltimer at CTA end   (ns)
     unsigned long long stamp;   // nonce of the probe whose kernel wrote the slot (a stale slot is a failure)
     unsigned long long n_words; // words the sweep covered
-    unsigned long long pad;
+    unsigned long long mismatches;  // a comparing read: words that differ from the pattern (exact); 0 from a read that
+                                    // only folds; not written by the fill, the copies and the closed form
 };
 static_assert(sizeof(SweepOut) == 64 && sizeof(SweepOut) == sizeof(cro_sweep_slot), "SweepOut is one 64-byte slot");
 static_assert(offsetof(SweepOut, t0) == offsetof(cro_sweep_slot, t0) && offsetof(SweepOut, stamp) == offsetof(cro_sweep_slot, stamp) &&
-                  offsetof(SweepOut, n_words) == offsetof(cro_sweep_slot, n_words),
+                  offsetof(SweepOut, n_words) == offsetof(cro_sweep_slot, n_words) &&
+                  offsetof(SweepOut, mismatches) == offsetof(cro_sweep_slot, mismatches),
               "SweepOut is the cro_sweep_slot of include/croprobe.h");
 
 // What a probe's kernels read from device memory instead of taking as launch
@@ -96,8 +98,11 @@ struct Params {
 // invert: write the bitwise complement of the pattern (the fault locator's second retest pass; the probe never does).
 cudaError_t launch_fill(const KernelPlan&, void* base, uint64_t bytes, const Params&,
                         const SweepScratch&, SweepOut* out, cudaStream_t, bool invert = false);
+// compare: every word is also compared with pattern_word(seed, i), i counted from `base`, and out->mismatches gets the
+// exact count of words that differ (the probe's reads: a fold alone misses multi-word faults that cancel in it, see
+// DESIGN.md §3).  Without it the read only folds and writes 0 there (a peer's pattern, the single timed sweeps).
 cudaError_t launch_read(const KernelPlan&, unsigned variant, const void* base, uint64_t bytes,
-                        const Params&, const SweepScratch&, SweepOut* out, cudaStream_t);
+                        const Params&, const SweepScratch&, SweepOut* out, cudaStream_t, bool compare);
 // Every variant publishes *out when out is non-null: the %globaltimer window, the stamp and n_words = bytes / 8.
 // COPY_TMA_FUSED also folds every tile it moves (checksum of the SOURCE stream as read) into it and needs out; the
 // plain variants fold nothing and write a zero checksum, like the fill.
@@ -105,7 +110,8 @@ cudaError_t launch_copy(const KernelPlan&, unsigned variant, void* dst, const vo
                         const Params&, const SweepScratch&, SweepOut* out, cudaStream_t);
 cudaError_t launch_expected(const KernelPlan&, uint64_t bytes, const Params&,
                             const SweepScratch&, SweepOut* out, cudaStream_t);
-cudaError_t launch_xor_word(void* base, uint64_t word_index, uint64_t mask, cudaStream_t);
+// word ^= mask for the words [first, first + count) of base: the test hooks' software faults.
+cudaError_t launch_xor_words(void* base, uint64_t first, uint64_t count, uint64_t mask, cudaStream_t);
 
 // Fault locator (cro_locate_faults).  One compare pass over one half: every word is checked against
 // pattern_word(seed, i) ^ invert (i counted from the half's start, as the probe's copies keep it), the half is folded

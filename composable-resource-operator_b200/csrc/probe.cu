@@ -383,6 +383,7 @@ int probe_enqueue(cro_ctx* c, Device* d, Lane& L) {
     }
     std::vector<cudaEvent_t>& ev = L.evpool;
     const bool overlap = c->knobs.get("CRO_EXPECT_OVERLAP") != 0;
+    const uint64_t inject_count = o.test_inject_count ? o.test_inject_count : 1;
     unsigned char* half[2] = {d->region, d->region + d->sweep_bytes};
     const Params gp = graph_params(L);
 
@@ -395,9 +396,10 @@ int probe_enqueue(cro_ctx* c, Device* d, Lane& L) {
         CU_TRY(c, cudaMemcpyAsync(L.d_params, L.h_params, sizeof(ProbeParams), cudaMemcpyHostToDevice, d->stream));
         CU_TRY(c, cudaEventRecordWithFlags(ev[k++], d->stream, flag));
         uint32_t sweep_no = 0;
-        auto maybe_inject = [&]() -> int {      // CRO_F_TEST_INJECT: corrupt one word behind a chosen sweep
-            if ((o.flags & CRO_F_TEST_INJECT) && o.test_inject_after == sweep_no && o.test_inject_word < 2 * (d->sweep_bytes / 8))
-                CU_TRY(c, launch_xor_word(d->region, o.test_inject_word, o.test_inject_mask, d->stream));
+        auto maybe_inject = [&]() -> int {      // CRO_F_TEST_INJECT: corrupt a run of words behind a chosen sweep
+            if ((o.flags & CRO_F_TEST_INJECT) && o.test_inject_after == sweep_no && o.test_inject_word < 2 * (d->sweep_bytes / 8) &&
+                inject_count <= 2 * (d->sweep_bytes / 8) - o.test_inject_word)
+                CU_TRY(c, launch_xor_words(d->region, o.test_inject_word, inject_count, o.test_inject_mask, d->stream));
             ++sweep_no;
             return CRO_OK;
         };
@@ -421,7 +423,7 @@ int probe_enqueue(cro_ctx* c, Device* d, Lane& L) {
         }
         for (uint32_t i = 0; i < R; ++i) {
             CU_TRY(c, launch_read(d->plan, rv, half[read_half(C, i)], d->sweep_bytes, gp, d->scratch,
-                                  &L.d_out[kSlotSweep0 + C + i], d->stream));
+                                  &L.d_out[kSlotSweep0 + C + i], d->stream, /*compare=*/true));
             CU_TRY(c, cudaEventRecordWithFlags(ev[k++], d->stream, flag));
             if (maybe_inject()) return CRO_ERR_CUDA;
         }
@@ -443,7 +445,8 @@ int probe_enqueue(cro_ctx* c, Device* d, Lane& L) {
     // The graph is tied to the options it was captured with; any capture problem falls back to direct launches.
     const uint64_t graph_key = ((uint64_t)rv << 48) ^ ((uint64_t)cv << 40) ^ ((uint64_t)R << 24) ^ ((uint64_t)C << 8) ^
                                (overlap ? 1u : 0u) ^ (d->sweep_bytes << 1) ^
-                               ((o.flags & CRO_F_TEST_INJECT) ? ((uint64_t)o.test_inject_after << 56) ^ (o.test_inject_word * 0x9E3779B97F4A7C15ull) ^ o.test_inject_mask : 0);
+                               ((o.flags & CRO_F_TEST_INJECT) ? ((uint64_t)o.test_inject_after << 56) ^ (o.test_inject_word * 0x9E3779B97F4A7C15ull) ^
+                                                                    o.test_inject_mask ^ (inject_count * 0xC2B2AE3D27D4EB4Full) : 0);
     if (c->knobs.get("CRO_USE_GRAPH") && !L.graph_failed) {
         if (L.graph_exec && L.graph_key != graph_key) {
             cudaGraphExecDestroy(L.graph_exec);

@@ -58,7 +58,10 @@ int ctx_read(cro_ctx* c, int idx, uint32_t variant, uint32_t iters, bool dst_hal
     int rc = ensure_filled(c, d);
     if (rc) return rc;
     const unsigned char* base = d->region + (dst_half ? d->sweep_bytes : 0);
-    auto read = [&] { return launch_read(d->plan, variant, base, d->sweep_bytes, imm_params(d), d->scratch, &d->d_out[kSlotScratch], d->stream); };
+    auto read = [&] {
+        return launch_read(d->plan, variant, base, d->sweep_bytes, imm_params(d), d->scratch, &d->d_out[kSlotScratch], d->stream,
+                           /*compare=*/false);
+    };
     return timed_sweep(c, d, iters, d->sweep_bytes, variant, read, [] {}, /*fold=*/true, /*deadline=*/true, out);
 }
 
@@ -96,7 +99,7 @@ int ctx_inject(cro_ctx* c, int idx, uint64_t word, uint64_t mask) {
     if (g.rc) return g.rc;
     int rc = ensure_filled(c, d);
     if (rc) return rc;
-    CU_TRY(c, launch_xor_word(d->region, word, mask, d->stream));
+    CU_TRY(c, launch_xor_words(d->region, word, 1, mask, d->stream));
     c->launches++;
     CU_TRY(c, cudaStreamSynchronize(d->stream));
     return CRO_OK;
@@ -226,6 +229,9 @@ uint64_t round_up(uint64_t v, uint64_t a) { return (v + a - 1) / a * a; }
 
 bool is_copy(uint32_t k) { return k >= CRO_SELFTEST_SWEEP_COPY_LDG && k <= CRO_SELFTEST_SWEEP_COPY_FUSED; }
 bool is_link(uint32_t k) { return k == CRO_SELFTEST_SWEEP_LINK_READ || k == CRO_SELFTEST_SWEEP_LINK_WRITE; }
+bool is_read(uint32_t k) { return k >= CRO_SELFTEST_SWEEP_READ_LDG && k <= CRO_SELFTEST_SWEEP_READ_LDG256; }
+// The kernels whose interior may carry force ranges before they run: the word checks, and the checksumming copy's source.
+bool is_forced(uint32_t k) { return k == CRO_SELFTEST_SWEEP_LOCATE || is_read(k) || k == CRO_SELFTEST_SWEEP_COPY_FUSED; }
 
 // The hook's buffer: `total` bytes (a multiple of the guard), interior k at byte at[k].  Every interior starts `offset`
 // past a guard boundary; what the interiors leave of [0, total) is guard, at least kGuard of it on each side.
@@ -282,13 +288,16 @@ const char* hook_refusal(const cro_selftest_sweep_opts& o) {
     if (k == CRO_SELFTEST_SWEEP_LOCATE ? o.word0 > kMaxHookWords - o.bytes / 8 : o.word0 != 0)
         return "word0 is locate's, with word0 + bytes / 8 at most 2^37";
     const uint64_t n = o.bytes / 8;
+    const bool xr = (o.flags & CRO_SELFTEST_F_XOR) != 0;
     for (int r = 0; r < 2; ++r) {
         if (!o.force_count[r]) continue;
         if (o.force_first[r] >= n || o.force_count[r] > n - o.force_first[r]) return "a force range must lie in the interior";
-        if (k != CRO_SELFTEST_SWEEP_LOCATE && !(k == CRO_SELFTEST_SWEEP_FORCE_WORDS && r == 0))
-            return "force ranges are locate's, and force_words' range 0";
+        if (!is_forced(k) && !(k == CRO_SELFTEST_SWEEP_FORCE_WORDS && r == 0))
+            return "force ranges are locate's, the reads', the checksumming copy's, and force_words' range 0";
+        if (xr && o.force_and[r] != ~0ull) return "an XOR range's and mask is all ones";
     }
-    if ((o.flags & ~CRO_SELFTEST_F_INTERIORS) || o.reserved) return "unknown flags";
+    if ((o.flags & ~(CRO_SELFTEST_F_INTERIORS | CRO_SELFTEST_F_XOR)) || o.reserved) return "unknown flags";
+    if (xr && !is_forced(k)) return "XOR is for the ranges prepared before the kernel";
     return nullptr;
 }
 
@@ -368,9 +377,12 @@ int ctx_selftest_sweep(cro_ctx* c, int idx, const cro_selftest_sweep_opts* o, cr
     CU_TRY(c, launch_fill(p, in0, bytes, pat, sc, nullptr, st, (o->invert != 0) != writes));
     if (is_copy(kernel)) CU_TRY(c, launch_fill(p, in1, bytes, pat, sc, nullptr, st, true));
     c->launches += is_copy(kernel) ? 2 : 1;
-    if (kernel == CRO_SELFTEST_SWEEP_LOCATE)
+    if (is_forced(kernel))
         for (int r = 0; r < 2; ++r) {
-            CU_TRY(c, launch_force_words(in0, o->force_first[r], o->force_count[r], o->force_and[r], o->force_or[r], p.sm_count, st));
+            if (o->flags & CRO_SELFTEST_F_XOR)
+                CU_TRY(c, launch_xor_words(in0, o->force_first[r], o->force_count[r], o->force_or[r], st));
+            else
+                CU_TRY(c, launch_force_words(in0, o->force_first[r], o->force_count[r], o->force_and[r], o->force_or[r], p.sm_count, st));
             c->launches += o->force_count[r] ? 1 : 0;
         }
 
@@ -387,10 +399,12 @@ int ctx_selftest_sweep(cro_ctx* c, int idx, const cro_selftest_sweep_opts* o, cr
                 return launch_force_words(in0, o->force_first[0], o->force_count[0], o->force_and[0], o->force_or[0], p.sm_count, st);
             case CRO_SELFTEST_SWEEP_LINK_READ: return launch_link_stream(role, off, dv.check(0), p.link_grid, 0, st);
             case CRO_SELFTEST_SWEEP_LINK_WRITE: return launch_link_stream(off, role, dv.check(0), p.link_grid, 0, st);
-            default: return is_copy(kernel) ? launch_copy(p, cv, in1, in0, bytes, pat, sc, slot, st) : launch_read(p, rv, in0, bytes, pat, sc, slot, st);
+            default:
+                return is_copy(kernel) ? launch_copy(p, cv, in1, in0, bytes, pat, sc, slot, st)
+                                       : launch_read(p, rv, in0, bytes, pat, sc, slot, st, /*compare=*/true);
         }
     };
-    const bool reads = kernel >= CRO_SELFTEST_SWEEP_READ_LDG && kernel <= CRO_SELFTEST_SWEEP_READ_LDG256;
+    const bool reads = is_read(kernel);
     const bool fold = reads || kernel == CRO_SELFTEST_SWEEP_COPY_FUSED || kernel == CRO_SELFTEST_SWEEP_LOCATE ||
                       kernel == CRO_SELFTEST_SWEEP_LINK_READ;
     if ((rc = timed_sweep(c, d, 1, is_copy(kernel) ? 2 * bytes : bytes, reads ? rv : is_copy(kernel) ? cv : 0, run, [] {}, fold,
@@ -398,7 +412,8 @@ int ctx_selftest_sweep(cro_ctx* c, int idx, const cro_selftest_sweep_opts* o, cr
         return rc;
 
     // each interior folded by the LDG read, the counters fetched, the guards (and interiors) copied back
-    for (int k = 0; k < L.interiors; ++k) CU_TRY(c, launch_read(p, READ_LDG, base + L.at[k], bytes, pat, sc, &dv.slots[k], st));
+    for (int k = 0; k < L.interiors; ++k)
+        CU_TRY(c, launch_read(p, READ_LDG, base + L.at[k], bytes, pat, sc, &dv.slots[k], st, /*compare=*/false));
     c->launches += L.interiors;
     if ((rc = mb.fetch(c, st))) return rc;
     std::vector<std::pair<uint64_t, uint64_t>> back = guards;
@@ -419,7 +434,7 @@ int ctx_selftest_sweep(cro_ctx* c, int idx, const cro_selftest_sweep_opts* o, cr
         out->after_sum[k] = s.s;
         out->after_wsum[k] = s.w;
     }
-    out->mismatches = hv.ctr[0].mismatches;
+    out->mismatches = reads ? d->h_out[kSlotScratch].mismatches : hv.ctr[0].mismatches;
     out->claims = hv.ctr[0].claims;
     for (uint64_t w = 0; w < hv.gran_words; ++w)
         for (unsigned long long bits = hv.gran[w]; bits; bits &= bits - 1) {

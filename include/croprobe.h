@@ -59,8 +59,10 @@ extern "C" {
 #define CRO_F_SKIP_P2P_WRITE  0x0080u  /* cro_probe_all: peer reads only, no push leg */
 #define CRO_F_TEST_INJECT     0x0100u  /* fault injection INSIDE the probe (tests of the device-side verdict): after sweep
                                           number test_inject_after (launch order: 0 = the fill, 1.. = copies, then reads)
-                                          XOR test_inject_mask into 64-bit word test_inject_word of the region (half A is
-                                          words [0, S/8), half B [S/8, 2S/8)) */
+                                          XOR test_inject_mask into the 64-bit words [test_inject_word, test_inject_word +
+                                          test_inject_count) of the region (half A is words [0, S/8), half B [S/8, 2S/8);
+                                          count 0 means 1).  A run that does not fit the region injects nothing.  A run
+                                          of several words can place faults the checksum cannot see (DESIGN.md §3) */
 
 /* read-sweep kernel variants */
 #define CRO_READ_AUTO   0u   /* by sweep size: 128-bit LDG up to 128 MiB, the TMA ring above (measured crossover) */
@@ -97,7 +99,7 @@ typedef struct cro_opts {
     uint32_t rank_base;            /* one-process-per-GPU hosts: this process's first rank  */
     uint32_t world_override;       /* ... and the job's world size (0 = devices managed)    */
     uint32_t test_inject_after;    /* CRO_F_TEST_INJECT: see above                          */
-    uint32_t reserved0;
+    uint32_t test_inject_count;    /* CRO_F_TEST_INJECT: words from test_inject_word; 0 = 1 */
     uint64_t test_inject_word;
     uint64_t test_inject_mask;
 } cro_opts;
@@ -195,13 +197,17 @@ typedef struct cro_probe_result {
     uint8_t  copy_variant;         /* 495 */
     uint8_t  read_sweeps;          /* 496 */
     uint8_t  copy_sweeps;          /* 497 */
-    uint8_t  copy_verified;        /* 498  copy sweeps whose destination was re-read and matched the closed form
-                                           (sweep k+1 folds what sweep k wrote; the first read sweep folds the last).
-                                           Counted per passing check, also after an earlier failure: every checksumming
-                                           copy k >= 1 that passed, plus read sweep 0 if it passed and copies ran */
+    uint8_t  copy_verified;        /* 498  copy sweeps whose destination was re-read and whose fold matched the closed
+                                           form (sweep k+1 folds what sweep k wrote; the first read sweep folds the last,
+                                           and also compares every word of it).  Counted per passing check, also after an
+                                           earlier failure: every checksumming copy k >= 1 that passed, plus read sweep 0
+                                           if it passed and copies ran.  A copy's fold cannot see every multi-word fault
+                                           (DESIGN.md §3): one it misses is carried into every later copy and found by
+                                           the first read of a half that holds it, which fails as CRO_FAIL_READ */
     uint8_t  fail_code;            /* 499  CRO_FAIL_*: which check failed first (0 = none), in the order: closed form,
                                            fill stamp, each copy sweep (stamp, then fold when it checksums), each read
-                                           sweep (stamp, then fold); p2p_finalize adds its peer checks after all of them */
+                                           sweep (stamp, then fold and word compare); p2p_finalize adds its peer checks
+                                           after all of them */
     uint8_t  fail_index;           /* 500  CRO_FAIL_STALE: the sweep's number in launch order (0 fill, 1.. copies, then
                                            reads); CRO_FAIL_COPY_SRC / CRO_FAIL_READ: the copy / read sweep's own index;
                                            CRO_FAIL_EXPECT: 0, or the peer whose prefix slot is stale; peer checks: the peer */
@@ -215,7 +221,7 @@ typedef struct cro_probe_result {
 #define CRO_FAIL_NONE        0
 #define CRO_FAIL_EXPECT      1   /* the closed-form slot is stale or short: the generator kernel did not run */
 #define CRO_FAIL_COPY_SRC    2   /* copy sweep fail_index read something else than the pattern */
-#define CRO_FAIL_READ        3   /* read sweep fail_index */
+#define CRO_FAIL_READ        3   /* read sweep fail_index: its fold differs from the closed form, or a word differs */
 #define CRO_FAIL_P2P_READ    4   /* NVLink read of peer fail_index */
 #define CRO_FAIL_P2P_PUSH    5   /* what peer fail_index pushed did not land here intact */
 #define CRO_FAIL_P2P_CHASE   6   /* pointer chase through peer fail_index ended on the wrong slot */
@@ -3147,13 +3153,21 @@ const char *cro_version(void);
  * it finish first, runs one kernel on buffers of its own (never a probe's slots or result struct) and frees them before
  * returning. */
 
-/* One sweep's result slot as the kernels write it into a device's slot array: 64 bytes. */
+/* One sweep's result slot as the kernels write it into a device's slot array: 64 bytes.  The fold is linear modulo 2^64,
+ * so some multi-word faults leave it unchanged (DESIGN.md §3); the probe's read sweeps therefore also compare every word
+ * with the pattern and count the words that differ.  probe_finalize fails a read sweep whose stamp is stale, whose fold
+ * differs from the closed form, or whose mismatches is not 0. */
 typedef struct cro_sweep_slot {
     uint64_t x, s, w;              /* checksum triple of what the sweep folded (zero for the fill and the plain copies) */
     uint64_t t0, t1;               /* %globaltimer window: first CTA start, last CTA end                                */
     uint64_t stamp;                /* nonce of the probe whose kernel wrote the slot                                     */
     uint64_t n_words;              /* 64-bit words the sweep covered                                                     */
-    uint64_t pad;
+    union {
+        uint64_t mismatches;       /* a comparing read (the probe's): words that differ from the pattern, exact; a read  */
+                                   /* that only folds (the NVLink legs, the single sweeps) writes 0; the fill, the      */
+                                   /* copies and the closed form leave it as it was                                     */
+        uint64_t pad;              /* the same word under its earlier name, so callers that name it still compile       */
+    };
 } cro_sweep_slot;
 
 /* Slot map of one device's slot array. */
@@ -3279,6 +3293,7 @@ int  cro_selftest_p2p_plan(uint32_t n, const uint64_t *sweep_bytes, uint64_t p2p
 #define CRO_SELFTEST_LAYOUT_APART       3   /* [guard | src | guard | dst | guard]                                    */
 #define CRO_SELFTEST_GUARD_BYTES  (2u << 20) /* the least a guard holds: more than any ring (tile * stages) a knob takes */
 #define CRO_SELFTEST_F_INTERIORS        1u  /* copy the interiors back too, not only the guards                       */
+#define CRO_SELFTEST_F_XOR              2u  /* the force ranges XOR: word ^= force_or[r] (force_and[r] all ones)      */
 
 typedef struct cro_selftest_sweep_opts {
     uint32_t kernel;               /*   0  CRO_SELFTEST_SWEEP_*                                                  */
@@ -3291,9 +3306,10 @@ typedef struct cro_selftest_sweep_opts {
     uint64_t invert;               /*  40  fill, locate: XOR on the pattern (0 or all ones)                      */
     uint64_t word0;                /*  48  locate: scan index of the interior's first word; word0 + bytes / 8 <= 2^37 */
     uint64_t force_first[2];       /*  56  interior word ranges set to (word & and) | or once the interior is   */
-    uint64_t force_count[2];       /*  72  prepared: locate only, both ranges; force_words: range 0 is the       */
-    uint64_t force_and[2];         /*  88  kernel's own and range 1 stays empty; any other kernel: both empty    */
-    uint64_t force_or[2];          /* 104  (count 0 = no range)                                                 */
+    uint64_t force_count[2];       /*  72  prepared (with CRO_SELFTEST_F_XOR: word ^ or, and all ones): locate,  */
+    uint64_t force_and[2];         /*  88  the reads and the checksumming copy (its source), both ranges;        */
+    uint64_t force_or[2];          /* 104  force_words: range 0 is the kernel's own (no XOR) and range 1 stays   */
+                                   /*      empty; any other kernel: both empty (count 0 = no range)              */
     uint32_t flags;                /* 120  CRO_SELFTEST_F_*                                                      */
     uint32_t reserved;             /* 124  0                                                                     */
 } cro_selftest_sweep_opts;
@@ -3307,7 +3323,7 @@ typedef struct cro_selftest_sweep_out {
     uint64_t after_xor[2];         /*  80  each interior's fold once the kernel is done, by the LDG read sweep   */
     uint64_t after_sum[2];         /*  96                                                                        */
     uint64_t after_wsum[2];        /* 112                                                                        */
-    uint64_t mismatches;           /* 128  locate, link read: the kernel's exact count                          */
+    uint64_t mismatches;           /* 128  locate, link read, the reads (comparing): the kernel's exact count   */
     uint64_t claims;               /* 136  ... and the record slots it claimed                                  */
     uint64_t granules;             /* 144  ... and the granule bits it set (the locator's CRO_LOCATE_GRANULE_BYTES) */
     uint64_t granule_min;          /* 152  lowest and highest granule set (0 when none)                         */

@@ -14,7 +14,7 @@ from __future__ import annotations
 
 from typing import Dict, List, Sequence, Tuple
 
-from oracle import go_marshal_string_map
+from oracle import checksum_np, go_marshal_string_map, pattern_word
 
 PASSES = 3
 RECORDS = 4096
@@ -39,6 +39,57 @@ def deltas(records, index) -> Tuple[int, int, int]:
         ds = (ds + d) & U64
         dw = (dw + d * (2 * index(r["word"]) + 1)) & U64
     return dx, ds, dw
+
+
+# ---- faults in a pattern region, seen by the fold and word by word ----------------------------------------------------
+# A fault is (first, count, and_mask, or_mask, xor_mask): words [first, first + count) of the region become
+# ((w & and_mask) | or_mask) ^ xor_mask.  The probe's test hooks place exactly these: an XOR run (CRO_F_TEST_INJECT,
+# CRO_SELFTEST_F_XOR) and a stuck-at run (the and / or force).
+def xor_run(first: int, mask: int, count: int = 1) -> Tuple[int, int, int, int, int]:
+    return (first, count, U64, 0, mask)
+
+
+def stuck_run(first: int, count: int, bit: int, value: int) -> Tuple[int, int, int, int, int]:
+    """Bit `bit` of every word of the run stuck at `value` (0 or 1)."""
+    return (first, count, U64 ^ (1 << bit), value << bit, 0)
+
+
+def fault_records(seed: int, faults) -> List[Dict]:
+    """The words the faults change in the pattern of `seed` (word i = pattern_word(seed, i)), applied in list order,
+    each to the word as the earlier ones left it: one {"word", "expected", "actual"} per word that ends up differing."""
+    now = {}
+    for first, count, and_mask, or_mask, xor_mask in faults:
+        for i in range(first, first + count):
+            w = now.get(i, pattern_word(seed, i))
+            now[i] = ((w & and_mask) | or_mask) ^ xor_mask
+    recs = [dict(word=i, expected=pattern_word(seed, i), actual=a) for i, a in sorted(now.items())]
+    return [r for r in recs if r["actual"] != r["expected"]]
+
+
+def faulted_fold(seed: int, n_words: int, faults) -> Tuple[int, int, int]:
+    """The fold (xor, sum, weighted sum) of words [0, n_words) of the pattern with the faults applied."""
+    x, s, w = checksum_np(seed, 0, n_words)
+    dx, ds, dw = deltas([r for r in fault_records(seed, faults) if r["word"] < n_words], lambda i: i)
+    return x ^ dx, (s + ds) & U64, (w + dw) & U64
+
+
+def word_mismatches(seed: int, n_words: int, faults) -> int:
+    """What a word-by-word compare of words [0, n_words) counts."""
+    return sum(1 for r in fault_records(seed, faults) if r["word"] < n_words)
+
+
+def flip_direction(seed: int, i: int, bit: int) -> int:
+    """+1 when flipping bit `bit` of pattern word i adds 2^bit to it (the bit is 0), -1 when it subtracts."""
+    return -1 if pattern_word(seed, i) >> bit & 1 else 1
+
+
+def find_directions(seed: int, bit: int, dirs: Sequence[int], start: int = 0, stride: int = 1, limit: int = 1 << 16) -> int:
+    """The first a >= start, below start + limit, at which flipping bit `bit` of words a, a + stride, a + 2 stride, ...
+    goes in the directions dirs (+1 / -1 each).  XOR runs placed there take the fold-blind shapes of DESIGN.md §3."""
+    for a in range(start, start + limit):
+        if all(flip_direction(seed, a + m * stride, bit) == d for m, d in enumerate(dirs)):
+            return a
+    raise ValueError("no run of directions %s for bit %d in [%d, %d)" % (list(dirs), bit, start, start + limit))
 
 
 def explained(slot: Dict, cf: Tuple[int, int, int], d: Tuple[int, int, int]) -> bool:

@@ -3,7 +3,7 @@
 
 Pure Python on integers of any size: every 64-bit field is reduced modulo 2^64 where the rule says so, and nothing
 here imports the product.  Inputs are the same bytes the kernels see: the identity template (512 bytes) and slot
-arrays of SLOT_COUNT 64-byte slots (x, s, w, t0, t1, stamp, n_words, pad, little-endian u64 each).
+arrays of SLOT_COUNT 64-byte slots (x, s, w, t0, t1, stamp, n_words, mismatches, little-endian u64 each).
 """
 from __future__ import annotations
 
@@ -49,7 +49,7 @@ class Slot(NamedTuple):
     t1: int = 0
     stamp: int = 0
     n_words: int = 0
-    pad: int = 0
+    mismatches: int = 0           # a comparing read's count of words that differ from the pattern
 
     def fold(self) -> Tuple[int, int, int]:
         return (self.x, self.s, self.w)
@@ -162,7 +162,7 @@ def probe_finalize(tmpl: bytes, slots: Sequence[Slot], seed: int, nonce: int, sw
         s = slots[SLOT_SWEEP0 + C + i]
         read_times.append((s.t1 - s.t0) & MASK64)
         ok = True
-        if stale(s) or s.fold() != E.fold():
+        if stale(s) or s.fold() != E.fold() or s.mismatches != 0:    # the fold can match while words differ
             if state["status"] == OK:
                 shown = s                 # the struct shows the read that failed first
             fail(FAIL_STALE if stale(s) else FAIL_READ, 1 + C + i if stale(s) else i)

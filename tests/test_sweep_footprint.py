@@ -10,8 +10,8 @@ it should write.  Then:
           the canary, the interior is the plain reference, a copy's source is unchanged, force_words changes exactly its
           range;
   readers (three reads, locate, link read): the fold is the oracle's checksum of exactly the interior (a folded guard
-          word would change it), and the word-checking kernels count no mismatch on a clean interior (every guard word
-          is one) and exactly the forced words on a forced one.
+          word would change it), and the word-checking kernels (the reads compare too) count no mismatch on a clean
+          interior (every guard word is one) and exactly the forced words on a forced one.
 Interiors up to 8 MiB are compared word for word on the host; above that their folds (taken by the LDG read after the
 kernel) are compared with the C oracle's checksum.
 
@@ -119,6 +119,11 @@ class Row:
         if self.out.sweep.checksum != want:
             self.fail("the kernel folded %s, not %s" % (self.out.sweep.checksum, want))
 
+    def compared(self, mismatches):
+        """A comparing read: its exact count (it keeps no records)."""
+        if self.out.mismatches != mismatches:
+            self.fail("counted %d mismatches, not %d" % (self.out.mismatches, mismatches))
+
     def counts(self, mismatches, granules=(0, 0, 0)):
         """The word-checking kernels: exact count, record slots claimed (one per mismatch) and granules set."""
         o = self.out
@@ -169,7 +174,15 @@ def _rows(cro, ctx, want, S, offset):
                           (cro.SELFTEST_SWEEP_READ_LDG256, "ldg256")):
         r = row("read " + kname, kernel)
         r.fold(want)
+        r.compared(0)
         r.interior(0, pat, want)
+        # bit 63 stuck at 1 over the last words: the read folds and counts exactly the words that changed
+        k = min(n, 5)
+        changed = [(i, o, o | 1 << 63) for i, o in ((i, oracle.pattern_word(SEED, i)) for i in range(n - k, n)) if not o >> 63]
+        r = row("read %s, bit 63 stuck at 1 in the last %d words" % (kname, k), kernel,
+                force=[(n - k, k, MASK ^ 1 << 63, 1 << 63)])
+        r.fold(_changed_fold(want, changed))
+        r.compared(len(changed))
     r = row("link read", cro.SELFTEST_SWEEP_LINK_READ)
     r.fold(want)
     r.counts(0)
@@ -284,7 +297,10 @@ def test_invalid_arguments_are_refused(cro):
             (cro.SELFTEST_SWEEP_FILL, 4096, dict(invert=1)),
             (cro.SELFTEST_SWEEP_FILL, 4096, dict(word0=1)),                            # word0 is locate's
             (cro.SELFTEST_SWEEP_LOCATE, 4096, dict(word0=(1 << 37) - 511)),           # granule bitmap past 2^37 words
-            (cro.SELFTEST_SWEEP_READ_LDG, 4096, dict(force=[(0, 1, 0, 0)])),          # force ranges are locate's ...
+            (cro.SELFTEST_SWEEP_FILL, 4096, dict(force=[(0, 1, 0, 0)])),              # force ranges are locate's, the reads' ...
+            (cro.SELFTEST_SWEEP_COPY_TMA, 4096, dict(layout=cro.SELFTEST_LAYOUT_SRC_DST, force=[(0, 1, 0, 0)])),
+            (cro.SELFTEST_SWEEP_READ_TMA, 4096, dict(force=[(0, 1, 0, 1)], xor=True)),     # an XOR range keeps every bit
+            (cro.SELFTEST_SWEEP_FORCE_WORDS, 4096, dict(force=[(0, 1, MASK, 1)], xor=True)),   # ... and is a prepared one
             (cro.SELFTEST_SWEEP_FORCE_WORDS, 4096, dict(force=[(0, 1, 0, 0), (1, 1, 0, 0)])),   # ... force_words' first
             (cro.SELFTEST_SWEEP_LOCATE, 4096, dict(force=[(500, 13, 0, 0)])),        # past the interior's 512 words
         ]:
@@ -326,7 +342,7 @@ def test_ctypes_layout_and_constants_match_the_header(cro, tmp_path):
     consts = ["CRO_SELFTEST_SWEEP_" + k for k in ("FILL", "COPY_LDG", "COPY_TMA", "COPY_FUSED", "READ_LDG", "READ_TMA",
                                                     "READ_LDG256", "LOCATE", "FORCE_WORDS", "LINK_READ", "LINK_WRITE")]
     consts += ["CRO_SELFTEST_LAYOUT_SRC_DST", "CRO_SELFTEST_LAYOUT_DST_SRC", "CRO_SELFTEST_LAYOUT_APART",
-               "CRO_SELFTEST_GUARD_BYTES", "CRO_SELFTEST_F_INTERIORS"]
+               "CRO_SELFTEST_GUARD_BYTES", "CRO_SELFTEST_F_INTERIORS", "CRO_SELFTEST_F_XOR"]
     src = ['#include <stdio.h>', '#include <stddef.h>', '#include "croprobe.h"', "int main(void) {"]
     for cname, (_py, fl) in fields.items():
         src.append('printf("%s sizeof %%zu\\n", sizeof(%s));' % (cname, cname))

@@ -79,6 +79,8 @@ PERTURB = {
     "s": lambda s, st: s._replace(s=(s.s + (1 << 63)) & M),
     "w": lambda s, st: s._replace(w=(s.w + 2) & M),
     "armed": lambda s, st: V.ARMED,                                              # the kernel never ran
+    "mismatches": lambda s, st: s._replace(mismatches=1),                        # the fold matches, a word does not
+    "mismatches 2^32": lambda s, st: s._replace(mismatches=1 << 32),             # the whole 64-bit count is compared
 }
 
 

@@ -109,6 +109,39 @@ def test_the_struct_shows_the_read_that_failed_first():
     assert (r.get("fail_code"), r.get("fail_index"), r.get("checksum_xor")) == (V.FAIL_STALE, 4, E[0])  # launch order: 1 + C + 1
 
 
+@pytest.mark.parametrize("count", [1, 2, 1 << 32, M])
+def test_a_read_whose_fold_matches_but_whose_words_differ_fails_at_its_index(count):
+    """A multi-word fault the fold cannot see: the read's fold equals the closed form, its word count does not."""
+    for C, R in ((2, 3), (0, 2), (3, 1)):
+        for i in range(R):
+            sl = healthy(C, R)
+            sl[V.SLOT_SWEEP0 + C + i] = sl[V.SLOT_SWEEP0 + C + i]._replace(mismatches=count)
+            r = fin(sl, C, R)
+            assert (r.get("status"), r.get("fail_code"), r.get("fail_index")) == (V.ERR_CHECKSUM, V.FAIL_READ, i), (C, R, i)
+            assert (r.get("checksum_xor"), r.get("checksum_sum"), r.get("checksum_wsum")) == E     # the shown fold is that read's
+            # read 0 verifies the last copy only when it passed
+            assert r.get("copy_verified") == (C - 1 if C else 0) + (1 if C and i > 0 else 0), (C, R, i)
+    # a copy's slot carries no count the verdict reads
+    sl = healthy(2, 1)
+    sl[V.SLOT_SWEEP0] = sl[V.SLOT_SWEEP0]._replace(mismatches=count)
+    assert (fin(sl, 2, 1).get("status"), fin(sl, 2, 1).get("copy_verified")) == (0, 2)
+
+
+def test_a_stale_read_is_stale_before_its_count_is_looked_at():
+    sl = healthy(1, 2)
+    sl[V.SLOT_SWEEP0 + 1] = sl[V.SLOT_SWEEP0 + 1]._replace(stamp=NONCE + 1, mismatches=5)
+    r = fin(sl, 1, 2)
+    assert (r.get("fail_code"), r.get("fail_index"), r.get("copy_verified")) == (V.FAIL_STALE, 2, 0)
+    sl = healthy(1, 2)                                             # the first failing read wins: the stale one
+    sl[V.SLOT_SWEEP0 + 1] = sl[V.SLOT_SWEEP0 + 1]._replace(n_words=0)
+    sl[V.SLOT_SWEEP0 + 2] = sl[V.SLOT_SWEEP0 + 2]._replace(mismatches=1)
+    assert (fin(sl, 1, 2).get("fail_code"), fin(sl, 1, 2).get("fail_index")) == (V.FAIL_STALE, 2)
+    sl = healthy(1, 2)                                             # ... or the counting one, when it comes first
+    sl[V.SLOT_SWEEP0 + 1] = sl[V.SLOT_SWEEP0 + 1]._replace(mismatches=1)
+    sl[V.SLOT_SWEEP0 + 2] = sl[V.SLOT_SWEEP0 + 2]._replace(stamp=0)
+    assert (fin(sl, 1, 2).get("fail_code"), fin(sl, 1, 2).get("fail_index")) == (V.FAIL_READ, 0)
+
+
 def test_no_copies():
     r = fin(healthy(0, 1), C=0, R=1)
     t = V.Result(TMPL)

@@ -583,6 +583,9 @@ FIELDS = {
     "cro_locate_counters": ("LocateCounters", ["mismatches", "claims", "bits"]),
     "cro_locate_record": ("LocateRecord", ["word", "expected", "actual"]),
     "cro_sweep_slot": ("SweepSlot", ["x", "s", "w", "t0", "t1", "stamp", "n_words", "pad"]),
+    "cro_opts": ("Opts", ["abi_version", "flags", "sweep_bytes", "p2p_bytes", "seed_base", "read_sweeps", "copy_sweeps",
+                          "latency_hops", "read_variant", "copy_variant", "deadline_ms", "n_devices", "devices", "rank_base",
+                          "world_override", "test_inject_after", "test_inject_count", "test_inject_word", "test_inject_mask"]),
 }
 
 
@@ -607,6 +610,18 @@ def test_ctypes_layout_of_the_mirrors_matches_the_header(cro, tmp_path):
         assert [f for f, _ in cls._fields_] == fields, cname
         for f in fields:
             assert getattr(cls, f).offset == got[(cname, f)], (cname, f)
+
+
+def test_a_slots_mismatch_count_is_the_word_its_pad_was(cro, tmp_path):
+    """cro_sweep_slot.mismatches and .pad name one word, the slot's last; the ctypes mirror reads it as mismatches."""
+    c = tmp_path / "slot.c"
+    c.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "croprobe.h"\nint main(void) {\n'
+                 'cro_sweep_slot s = {0};\ns.pad = 7;\nprintf("%zu %zu %zu %llu\\n", offsetof(cro_sweep_slot, mismatches), '
+                 'offsetof(cro_sweep_slot, pad), sizeof s, (unsigned long long)s.mismatches);\nreturn 0; }\n')
+    exe = tmp_path / "slot"
+    subprocess.check_call(["gcc", "-std=c11", "-I" + os.path.join(ROOT, "include"), str(c), "-o", str(exe)])
+    assert subprocess.check_output([str(exe)], text=True).split() == ["56", "56", "64", "7"]
+    assert cro.SweepSlot(pad=1 << 40).mismatches == 1 << 40 and cro.SweepSlot.pad.offset == 56
 
 
 def test_locate_hook_refuses_bad_arguments(cro):
